@@ -1,6 +1,6 @@
 # Build of libsce.so (the C-ABI engine), the standalone GEMM self-test and the oracle's C pieces.
 NVCC ?= nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v
 CSRC := sparse_coding_b200/csrc
 LIB := sparse_coding_b200/libsce.so

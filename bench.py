@@ -10,18 +10,20 @@ BASELINE config 2: 16 tied SAEs, d_model=512, dict_ratio=8 (n=4096), L1 = logspa
 parameters, lr 1e-3. For N>1 every rank trains its own 16-model shard on the same activation stream (config 4:
 model-axis sharding, no data-path collective) — weak scaling; value = rows consumed by all ranks' shards per second.
 
-Printed JSON (one line, rank 0): the driver contract plus
+Printed JSON (one line, rank 0): the throughput result plus
   value           K steps on device-resident batches between two CUDA events, NOTHING else in the loop (max over ranks)
   e2e             the same through the public API with HOST (pinned) batches: side-stream H2D of the next batch
                   (train_loop.HostBatchPrefetcher) + step + D2H of the losses every step; `e2e.serial` is the same
                   loop with the copy on the compute stream, with its copy / step split measured by CUDA events
   phases_ms       per-phase device time of a step, measured in a SEPARATE short loop (events recorded inside libsce)
   roofline        dominant kernel (weight-gradient GEMM): algorithmic FLOPs / CUDA-event time vs the measured bf16
-                  peak; per-GEMM fractions; DRAM bytes per step from the committed ncu capture
+                  peak; per-GEMM fractions
   cpu_baseline    one step of the oracle port of the reference on this box's host cores at the FULL batch
   stock_torch_gpu the same oracle port (the op sequence the reference launches) on THIS GPU, fp32 and TF32
   cfg4_stream     config 4's data path: fp16 chunks from disk -> pinned -> HBM -> device-side gather -> step, with
                   the end-of-chunk metric gather (also a workload of its own: --workload cfg4_stream)
+
+--dump-outputs DIR writes what the last timed step returned (see dump_outputs) for output-by-output comparisons.
 """
 import argparse
 import json
@@ -177,19 +179,56 @@ class _StdoutGuard:
         os.write(self.real, (json.dumps(obj) + "\n").encode())
 
 
+DUMP_BYTES = 64 << 20    # --dump-outputs writes at most this much: larger outputs are sampled on fixed, seeded rows
+
+
+def dump_outputs(path, enss, results):
+    """The last timed step's results as .npy files, for output-by-output comparisons of two builds (inputs are seeded):
+    per ensemble (prefix g<i>_ when the workload steps several), every loss term [M], the code aux["c"] [M, B, n] and the
+    updated parameters (what the caller's tensors hold after the step's Adam / renormalise). Tensors too large for their
+    share of DUMP_BYTES are sampled on a seeded set of rows of dimension 1 (indices in <name>_rows.npy)."""
+    os.makedirs(path, exist_ok=True)
+    gen = torch.Generator().manual_seed(0)
+    big = sum(1 + len(e.params) for e in enss)         # code + parameter tensors share what the loss vectors leave
+    cap = (DUMP_BYTES - (1 << 20)) // big
+    written = 0
+
+    def save(name, t):
+        nonlocal written
+        a = t.detach().float().cpu().numpy() if torch.is_tensor(t) else t
+        np.save(os.path.join(path, name + ".npy"), a)
+        written += a.nbytes
+
+    def save_sampled(name, t):
+        if t.numel() * 4 <= cap:
+            save(name, t)
+            return
+        per_row = t[:, :1].numel() * 4
+        keep = max(1, min(t.shape[1], cap // per_row))
+        rows = torch.randperm(t.shape[1], generator=gen)[:keep].sort().values
+        save(name + "_rows", rows.numpy().astype(np.float64))
+        save(name, t[:, rows.to(t.device)])
+
+    for gi, (ens, (losses, aux)) in enumerate(zip(enss, results)):
+        pre = f"g{gi}_" if len(enss) > 1 else ""
+        for k, v in losses.items():
+            save(f"{pre}loss_{k}", v)
+        c = aux["c"]
+        save_sampled(f"{pre}code", c.dense() if hasattr(c, "dense") else c)
+        if hasattr(c, "_dense"):
+            c._dense = None                               # the full code is 2 GB at cfg2: do not keep it alive
+        for k, v in ens.params.items():
+            save_sampled(f"{pre}param_{k}", v)
+    assert written <= DUMP_BYTES, written
+
+
 def peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         p = json.load(open(path))
         return {"bf16_tflops": p.get("bf16_tflops_sustained", p.get("bf16_tflops")), "hbm_gbs": p.get("hbm_gbs"),
                 "source": "measured (MEASURED_PEAKS.json, sustained bf16)"}
-    return {"bf16_tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def ncu_traffic():
-    """DRAM bytes per launch of every kernel of a step from the committed `ncu --set full` capture (profiles/)."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    return json.load(open(path)) if os.path.exists(path) else None
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense bf16, HBM3), not measured"}
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -482,6 +521,8 @@ def main():
     ap.add_argument("--stream-timeout", type=float, default=240.0, help="watchdog of the config-4 extras, seconds")
     ap.add_argument("--stream-chunks", type=int, default=3)
     ap.add_argument("--stream-rows", type=int, default=1 << 21, help="rows per streamed chunk (reference: 2^21 at d=512)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (losses, a fixed sample of the code) to DIR/<name>.npy")
     ap.add_argument("--feed", default="per_rank", choices=["per_rank", "broadcast", "both"],
                     help="cfg4_stream: every rank reads/copies its own chunk, or rank 0 reads and NCCL broadcasts")
     args = ap.parse_args()
@@ -518,6 +559,8 @@ def main():
     stream_only = args.workload == "cfg4_stream"
     M, d, n, B, desc = WORKLOADS[args.workload]
     K, W = args.steps, max(args.warmup, 3)
+    if K < 1:
+        raise SystemExit("--steps must be at least 1")
     topk = args.workload in ("cfg3", "cfg3g")
 
     # every rank owns its own shard of the sweep: same shapes, different seeds (model-axis sharding)
@@ -557,14 +600,18 @@ def main():
     t_begin = time.time()
     e0.record()
     for i in range(K):
-        losses, aux = step_all(pool[i % n_pool])
+        results = [e.step_batch(pool[i % n_pool]) for e in enss]
     e1.record()
     barrier()
     windows["value"] = (t_begin, time.time())
     ms = e0.elapsed_time(e1)
+    losses = results[-1][0]
     launches = K * sum(e.gpu_launches_last_call() for e in enss)
     final_loss = losses["loss"].detach().clone()
     arith_resolved = ens.resolved_arith()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, enss, results)
+    del results
 
     # ---------------- per-phase device times: a separate short loop with libsce's events switched on
     for e in enss:
@@ -648,21 +695,21 @@ def main():
     if rank == 0:
         pk = peaks()
         arith = arith_resolved
-        # tensor work issued per fp32-equivalent GEMM, in bf16-pass equivalents: three kind::f16 passes, or one
-        # kind::f16 pass + two kind::f8f6f4 passes at twice the rate
-        full_passes = 3 if arith == "bf16x3" else 2
+        # tensor work issued per fp32-equivalent GEMM, in 16-bit passes: three in both arithmetics (bf16x3: hi*hi,
+        # hi*lo, lo*hi; f16f8: h*h plus the two cross terms on e5m2 planes widened to fp16)
+        full_passes = 3
         bwd_eq = full_passes if args.bwd_passes == 3 else 1
         # f16f8 + fp16-representable activations: x has no residual plane, so the x.l8 * W.h8 term of encode and the
-        # dz.h8 * x.l8 term of the dz^T x half of dW are skipped on the device (one 8-bit pass = 1/2 pass equivalent)
+        # dz.h8 * x.l8 term of the dz^T x half of dW are skipped on the device (one pass each)
         x_skip = arith == "f16f8" and ACT_FP16
-        enc_eq = full_passes - (0.5 if x_skip else 0.0)
-        dw_eq = (bwd_eq - (0.25 if x_skip else 0.0)) if args.bwd_passes == 3 else 1
+        enc_eq = full_passes - (1.0 if x_skip else 0.0)
+        dw_eq = (bwd_eq - (0.5 if x_skip else 0.0)) if args.bwd_passes == 3 else 1
         arith_text = {
             "bf16x3": "fp32 parameters/moments/accumulation; every GEMM operand is an exact-to-2^-17 (hi, lo) bf16 pair "
                       "and every product 3 tensor-core passes (hi*hi + hi*lo + lo*hi)",
             "f16f8": "fp32 parameters/moments/accumulation; every GEMM operand is an fp16 plane plus two e5m2 planes "
-                     "(value, scaled residual); every product = one kind::f16 pass (h*h) + two kind::f8f6f4 passes for "
-                     "the cross terms (2 bf16-pass equivalents), rescaled in the accumulator",
+                     "(value, scaled residual); every product = one fp16 pass (h*h) + two fp16 passes for the cross "
+                     "terms on the e5m2 planes widened to fp16 (3 passes), rescaled in the accumulator",
         }[arith] + "; parity <= 1e-4 rel vs the fp32 reference on x_hat and losses (tests/test_scale_parity_gpu.py at this size)"
         value = world * B * K / (ms * 1e-3)
         e2e_value = world * B * K / (ms_e2e * 1e-3)
@@ -697,7 +744,7 @@ def main():
                                           "ensemble.py:185-189 — an unverified reading, torchopt is not installable here; "
                                           "'standard' is selectable and costs the same)",
                        "l2": "per-step working set (code + code-gradient, 4.3 GB) and the 8-batch input pool "
-                             "(134 MB) both exceed the 126 MB L2; no explicit flush",
+                             "(134 MB) both exceed the 50 MB L2; no explicit flush",
                        "timed_loop": "value: step_batch calls only (no profiling events, no host reads)"},
             "clocks": clocks, "gpu_launches": launches,
             "e2e": {"value": e2e_value, "unit": "activations/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -715,10 +762,9 @@ def main():
                          "peak_source": pk["source"], "alg_flops_per_launch": alg_flops_dw,
                          "ms_per_launch": dw_ms,
                          "issued_tflops": alg_flops_dw * dw_eq / (dw_ms * 1e-3) / 1e12 if dw_ms > 0 else None,
-                         "issued_note": f"{dw_eq} bf16-pass equivalents per fp32 FLOP of this kernel ({arith}"
+                         "issued_note": f"{dw_eq} 16-bit passes per fp32 FLOP of this kernel ({arith}"
                                         + (", x residual term skipped" if x_skip else "") + f"): frac <= 1/{dw_eq} x "
-                                        "(tensor-pipe utilisation = issued_tflops / peak; `peak` is cuBLAS's sustained "
-                                        "bf16 rate under the power cap, which kind::f8f6f4 passes can exceed)",
+                                        "(tensor-pipe utilisation = issued_tflops / peak)",
                          "step_alg_tflops": step_flops / (ms / K * 1e-3) / 1e12,
                          "step_frac": step_flops / (ms / K * 1e-3) / 1e12 / pk["bf16_tflops"],
                          "per_gemm_frac": {k: v["frac"] for k, v in gemms.items()}},
@@ -729,16 +775,6 @@ def main():
             "gemms": gemms,
             "final_loss_mean": float(final_loss.mean()),
         }
-        tr = (ncu_traffic() or {}).get(arith)
-        if tr and args.workload == "cfg2":
-            line["roofline"]["traffic"] = tr["dw_dram_bytes_per_launch"]
-            line["roofline"]["traffic_source"] = tr["source"]
-            # dz and c at 4 B / element (3 B for dz when x's residual term is skipped: its h8 plane is not read) + dW
-            line["roofline"]["alg_bytes_per_launch"] = (8.0 - (1.0 if x_skip else 0.0)) * M * B * n + 4.0 * M * n * d
-            if "dram_bytes_per_step" in tr:
-                line["roofline"]["dram_bytes_per_step"] = tr["dram_bytes_per_step"]
-                line["roofline"]["dram_bytes_per_kernel"] = tr.get("dram_bytes_per_kernel")
-                line["roofline"]["alg_bytes_per_step"] = 4.0 * B * d + 24.0 * M * n * d
         if ms_alt == ms_alt:
             line["alt_precision"] = {"note": "informational only: backward GEMMs on the 16-bit plane alone (bwd_passes=1); "
                                              "forward, losses and x̂ unchanged; FVU/L0 parity of this mode at this size: "

@@ -1,4 +1,4 @@
-/* sce.h — C ABI of the B200-native ensemble sparse-autoencoder training engine (libsce.so).
+/* sce.h — C ABI of the H100-native ensemble sparse-autoencoder training engine (libsce.so).
  *
  * The reference (HoagyC/sparse_coding @ 69c5ae0) has no FFI layer: its boundary for this path is the Python
  * protocol DictSignature / FunctionalEnsemble (autoencoders/ensemble.py:15-22, 68-193). This library sits
@@ -29,7 +29,7 @@ typedef enum sce_status {
   SCE_ERR_INVALID = -1,    /* bad argument / unsupported shape */
   SCE_ERR_CUDA = -2,       /* a CUDA runtime or driver call failed */
   SCE_ERR_WORKSPACE = -3,  /* workspace too small / misaligned */
-  SCE_ERR_NO_DEVICE = -4   /* no sm_100 device / driver entry point missing */
+  SCE_ERR_NO_DEVICE = -4   /* no sm_90 device / driver entry point missing */
 } sce_status;
 
 /* Which reference signature the plan reproduces. */
@@ -47,9 +47,9 @@ typedef enum sce_adam_count {
 
 /* How an fp32 GEMM operand is carried to the tensor cores (DESIGN.md section 2). Both reach the reference's fp32
  * results within the 1e-4 bar; they differ in cost and in the range of values they can hold.
- *   BF16X3: x = hi + lo, two bf16 planes; product = hi*hi + hi*lo + lo*hi, three kind::f16 passes. fp32 range.
- *   F16F8 : x = h + l, h = fp16(x); the dominant h*h runs as one kind::f16 pass, the two cross terms (which need
- *           ~3 significant bits) as kind::f8f6f4 E5M2 passes at twice the rate: 2 pass-equivalents instead of 3.
+ *   BF16X3: x = hi + lo, two bf16 planes; product = hi*hi + hi*lo + lo*hi, three bf16 passes. fp32 range.
+ *   F16F8 : x = h + l, h = fp16(x); the dominant h*h runs as one fp16 pass, the two cross terms (which need
+ *           ~3 significant bits) are carried on E5M2 planes (1 byte each), widened to fp16 for their two passes.
  *           Operand values must fit fp16 (|v| < 65504; magnitudes below ~1e-4 lose relative precision) — true for
  *           language-model activations, which the reference itself stores as fp16 (activation_dataset.py:294-299, 364, 404-412).
  *           Needs d % 16 == 0 and n % 16 == 0.

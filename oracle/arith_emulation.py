@@ -60,7 +60,7 @@ def tied_step_emulated(mm, x, W, bias, alpha, pin_active=None):
 
 # ----------------------------------------------------------------------------------------------------------------
 # Candidate (NOT implemented on the device; DESIGN.md section 9.1): cross terms on block-scaled 4-bit planes
-# (tcgen05 kind::mxf4: E2M1 elements, one E8M0 scale per 32 elements along K, K = 64 per instruction at four times the
+# (block-scaled FP4 MMA, which sm_90 does not have: E2M1 elements, one E8M0 scale per 32 elements along K, K = 64 per instruction at four times the
 # kind::f16 rate): 1 + 2 * 1/4 = 1.5 pass-equivalents and 2 + 0.5 + 0.5 (+ scales) ~= 3.06 bytes per operand element.
 # ----------------------------------------------------------------------------------------------------------------
 _E2M1 = torch.tensor([0.0, 0.5, 1.0, 1.5, 2.0, 3.0, 4.0, 6.0])

@@ -1,4 +1,4 @@
-"""sparse_coding_b200 — B200-native engine for the ensemble sparse-autoencoder sweep of HoagyC/sparse_coding.
+"""sparse_coding_b200 — H100-native engine for the ensemble sparse-autoencoder sweep of HoagyC/sparse_coding.
 
 Public names mirror the reference's ``autoencoders`` package for the hot path only (SURVEY.md §8):
 DictSignature / FunctionalEnsemble (ensemble.py), FunctionalSAE / FunctionalTiedSAE / masked variants

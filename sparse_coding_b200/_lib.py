@@ -2,7 +2,7 @@
 device pointers (``tensor.data_ptr()``).
 
 The library is built in-tree (``make`` / ``__graft_entry__.build()``) next to this file. There is NO fallback:
-if it is missing, or the process has no sm_100 device when a plan is created, the engine raises."""
+if it is missing, or the process has no sm_90 device when a plan is created, the engine raises."""
 from __future__ import annotations
 
 import ctypes as C

@@ -1,4 +1,4 @@
-// sce_engine.cu — libsce.so: the C ABI of include/sce.h on top of the tcgen05 GEMM core and the
+// sce_engine.cu — libsce.so: the C ABI of include/sce.h on top of the wgmma GEMM core and the
 // streaming kernels. One `sce_plan` = one stacked ensemble (FunctionalEnsemble, autoencoders/ensemble.py:68-97).
 //
 // One training step (tied variant; untied and top-k differ as noted; "(hi, lo)" stands for the operand planes of the
@@ -101,12 +101,7 @@ struct sce_plan {
   cudaStream_t cap_stream;  // private stream the step is captured on
   int dcode_passes, dw_passes;  // tensor passes of the two backward GEMMs (default: desc.bwd_passes)
   int use_graph;     // 1: replay the step as a CUDA graph (launch-bound shapes; env SCE_GRAPH overrides)
-  int split_decode;  // 1: separate TMEM accumulators for hi*hi and the cross terms in the decode GEMM (default)
-  int pair_encode, pair_decode, pair_dcode, pair_dw;  // 1: run that GEMM on CTA pairs (cta_group::2, 256-row tiles)
-  int bk_encode, bk_decode, bk_dcode;  // K block (64: 128-byte swizzle, 32: 64-byte swizzle) of the K-major GEMMs
-  int dw_collector;  // NSUB = 2 tiles: A slice kept in the tensor core's collector across the two column halves (SCE_TUNE_DW_COLL)
-  int dec_nsub2;     // experiment: decode with 256 x 512 tiles (SCE_TUNE_DEC_NSUB2)
-  int dw_nsub2;      // f16f8 weight gradient: 256 x 512 tiles sharing one A tile (env SCE_TUNE_DW_NSUB2 = 0 switches it off)
+  int split_decode;  // 1: separate accumulators for hi*hi and the cross terms in the decode GEMM
   int last_launches;
   long long step;  // number of optimiser steps taken
   // optional per-phase device timing (sce_profile_*): events bracket each phase of a step
@@ -196,8 +191,8 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
   const size_t M = d.n_models, B = d.batch_max, n = d.n, dd = d.d;
   const size_t xm = d.x_per_model ? M : 1;
   const size_t tiles_mB = (B + kBM - 1) / kBM;
-  const size_t tiles_nN = (n + 127) / 128;  // upper bound over the BN choices (BN >= 128)
-  const size_t tiles_nD = (dd + 127) / 128;
+  const size_t tiles_nN = (n + kBN - 1) / kBN;
+  const size_t tiles_nD = (dd + kBN - 1) / kBN;
   const bool f8 = resolve_arith(d) == kArithF16F8;
   // the planes of one operand tensor: 16-bit, then (bf16x3) a second 16-bit plane or (f16f8) two 8-bit planes
   auto planes = [&](size_t count, __nv_bfloat16*& hi, __nv_bfloat16*& lo, uint8_t*& x8) {
@@ -315,21 +310,9 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
 // ------------------------------------------------------------------------------------------------
 // tensor maps for one batch size
 // ------------------------------------------------------------------------------------------------
-static int bn_for(int N) { return N > 128 ? 256 : 128; }
-// a CTA pair needs at least two 128-row blocks of output
-static bool use_pair(int flag, int rows) { return flag && rows > kBM; }
-constexpr int kBkDw = 32;  // K block of the MN-major weight-gradient GEMM
-// K block of the GEMMs with K-major operands: 32 (64-byte swizzle, 4 stages of 48 KB at BN = 256) keeps three
-// stages in flight behind the one being multiplied; 64 (128-byte swizzle) only has room for two stages.
-// Chosen per GEMM (plan fields bk_encode / bk_decode / bk_dcode; env SCE_TUNE_BK_{ENCODE,DECODE,DCODE} overrides):
-// measured on B200 (profiles/r01f_bk_tuning.txt) the deeper pipeline wins where the A operand streams from HBM
-// (decode: the code tensor) and loses where both operands are L2-resident (encode, dcode: twice the TMA requests).
-static int tune_bk(const char* env, int dflt) {
-  const char* v = getenv(env);
-  if (!v) return dflt;
-  const int k = atoi(v);
-  return (k == 32 || k == 64) ? k : dflt;
-}
+// K block of every bf16x3 GEMM: 32 (64-byte swizzle for K-major tiles; a stage of the four planes is 32 KB, so three or
+// four stages fit beside the accumulator tile). f16f8 stages carry one 16-bit plane per operand: K block 64 (kBkF8).
+constexpr int kBkBf16 = 32;
 static int tune_flag(const char* env, int dflt) {
   const char* v = getenv(env);
   return v ? (atoi(v) != 0) : dflt;
@@ -338,14 +321,11 @@ static CUtensorMapSwizzle swizzle_for_bk(int bk) {
   return bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
 }
 
-static CUtensorMapSwizzle swizzle8_for_bk(int bk) {  // K-major 8-bit tiles: rows of bk bytes
-  return bk == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B;
-}
 constexpr int kBkF8 = 64;  // K block of every GEMM in the f16f8 arithmetic
 
 // The planes of one operand [models][rows][cols] (cols contiguous, `mpitch` elements between models) as GEMM operand
 // maps. kmajor_bk != 0: K-major tiles [box_rows][kmajor_bk]; else MN-major tiles of `box_rows` k-rows by 64 (16-bit)
-// / 128 (8-bit) contiguous elements.
+// / 128 (8-bit) contiguous elements. 8-bit tiles arrive unswizzled: the GEMM widens them to fp16 (widen_tile).
 static bool operand_maps(int arith, CUtensorMap* hi, CUtensorMap* lo, CUtensorMap* x8, const void* phi, const void* plo,
                          const void* px8, uint64_t models, uint64_t rows, uint64_t cols, uint64_t mpitch,
                          uint32_t box_rows, int kmajor_bk) {
@@ -353,15 +333,15 @@ static bool operand_maps(int arith, CUtensorMap* hi, CUtensorMap* lo, CUtensorMa
   if (kmajor_bk) {
     ok = make_tmap_bf16_box(hi, phi, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
     if (arith == kArithF16F8)
-      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle8_for_bk(kmajor_bk)) &&
-           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle8_for_bk(kmajor_bk));
+      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE) &&
+           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
     else
       ok = ok && make_tmap_bf16_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
   } else {
     ok = make_tmap_bf16(hi, phi, models, rows, cols, cols, mpitch, box_rows);
     if (arith == kArithF16F8)
-      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_128B) &&
-           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_128B);
+      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE) &&
+           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
     else
       ok = ok && make_tmap_bf16(lo, plo, models, rows, cols, cols, mpitch, box_rows);
   }
@@ -383,10 +363,8 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   // visible through the map, so rows >= B read as zero (TMA out-of-bounds fill).
   const int ar = p->arith;
   const bool f8 = ar == kArithF16F8;
-  const int bk_enc = f8 ? kBkF8 : p->bk_encode, bk_dec = f8 ? kBkF8 : p->bk_decode, bk_dco = f8 ? kBkF8 : p->bk_dcode;
-  const int bk_dw = f8 ? kBkF8 : kBkDw;
-  // the f16f8 kernels run narrow outputs (<= 128 columns) on single CTAs: an MN-major 8-bit B tile is 128 wide
-  auto pair_ok = [&](int flag, int rows, int out_cols) { return use_pair(flag, rows) && !(f8 && out_cols <= 128); };
+  const int bk = f8 ? kBkF8 : kBkBf16;
+  const int bk_enc = bk, bk_dec = bk, bk_dco = bk, bk_dw = bk;
   struct Pl { const void *hi, *lo, *x8; };
   const Pl X{p->x_hi, p->x_lo, p->x_x8}, WE{p->wenc_hi, p->wenc_lo, p->wenc_x8}, WD{p->wdec_hi, p->wdec_lo, p->wdec_x8},
       C{p->c_hi, p->c_lo, p->c_x8}, G{p->g_hi, p->g_lo, p->g_x8}, DZ{p->dz_hi, p->dz_lo, p->dz_x8};
@@ -400,14 +378,14 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   auto act_b = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
     return operand_maps(ar, &g.b_hi[set], &g.b_lo[set], &g.b_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk_dw, 0);
   };
-  // dictionary [M][n][d] as the B operand: K-major tiles [box_rows][bk] (box_rows = the B rows ONE CTA loads), or MN-major
+  // dictionary [M][n][d] as the B operand: K-major tiles [box_rows][bk] (box_rows = the tile's B rows), or MN-major
   auto dict_b = [&](GemmMaps& g, const Pl& P, uint32_t box_rows, int kmajor_bk) {
     return operand_maps(ar, &g.b_hi[0], &g.b_lo[0], &g.b_x8[0], P.hi, P.lo, P.x8, M, n, dd, n * dd, box_rows, kmajor_bk);
   };
   bool ok = true;
   // encode: A = x [xm,B,d] K-major, B = Wenc [M,n,d] K-major
   ok &= actk(m->encode, 0, X, xm, dd, bk_enc);
-  ok &= dict_b(m->encode, WE, bn_for(d.n) / (pair_ok(p->pair_encode, B, d.n) ? 2 : 1), bk_enc);
+  ok &= dict_b(m->encode, WE, kBN, bk_enc);
   if (d.centering) {
     // centring: A = (x - trans) planes in the X planes (the encode A maps), B = rot [M,d,d] K-major, output d columns
     for (int t = 0; t < 1; ++t) {
@@ -416,14 +394,14 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
       m->center.a_x8[t] = m->encode.a_x8[t];
     }
     ok &= operand_maps(ar, &m->center.b_hi[0], &m->center.b_lo[0], &m->center.b_x8[0], p->rot_hi, p->rot_lo, p->rot_x8, M, dd, dd,
-                       dd * dd, bn_for(d.d) / (pair_ok(p->pair_encode, B, d.d) ? 2 : 1), bk_enc);
+                       dd * dd, kBN, bk_enc);
   }
   // decode: A = c [M,B,n] K-major, B = Wdec [M,n,d] MN-major (bk k-rows per box)
   ok &= actk(m->decode, 0, C, M, n, bk_dec);
   ok &= dict_b(m->decode, WD, bk_dec, 0);
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
   ok &= actk(m->dcode, 0, G, M, dd, bk_dco);
-  ok &= dict_b(m->dcode, WD, bn_for(d.n) / (pair_ok(p->pair_dcode, B, d.n) ? 2 : 1), bk_dco);
+  ok &= dict_b(m->dcode, WD, kBN, bk_dco);
   // weight gradients: everything MN-major, reduction over the batch rows
   if (d.variant == SCE_UNTIED) {
     ok &= act_a(m->dw_enc, 0, DZ, M, n);
@@ -473,13 +451,14 @@ struct ResFlags {
   const uint32_t* b[kMaxSets] = {nullptr, nullptr};
 };
 
-template <class Epi, int BN, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, bool CTA2 = false,
-          int ARITH = kArithBf16x3, int NSUB = 1>
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC = false, int ARITH = kArithBf16x3>
 static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, const int* a_batched,
                          const int* b_batched, int k_total, int passes, int m_total, int n_total,
                          const typename Epi::Params& epi, cudaStream_t st, const ResFlags& rf = ResFlags()) {
-  using SM = GemmSmem<BN, BK, A_MN, B_MN, STAGES, Epi::kWarpStageBytes, CTA2, ARITH, NSUB>;
-  auto kern = gemm_split_kernel<Epi, BN, BK, A_MN, B_MN, STAGES, SPLIT_ACC, CTA2, ARITH, NSUB>;
+  constexpr int BK = ARITH == kArithF16F8 ? kBkF8 : kBkBf16;
+  constexpr int STAGES = gemm_stages<BK, Epi::kWarpStageBytes, ARITH>();
+  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH>;
+  auto kern = gemm_split_kernel<Epi, BK, A_MN, B_MN, STAGES, SPLIT_ACC, ARITH>;
   // the opt-in to > 48 KB of dynamic shared memory is per device: remember which devices have it
   static bool configured[64] = {};
   if (p->device < 0 || p->device >= 64 || !configured[p->device]) {
@@ -506,70 +485,19 @@ static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, con
   gp.n_models = p->d.n_models;
   gp.m_total = m_total;
   gp.n_total = n_total;
-  constexpr int kTileRows = CTA2 ? 2 * kBM : kBM;   // a CTA pair owns 256-row tiles
-  gp.tiles_m = (m_total + kTileRows - 1) / kTileRows;
-  gp.tiles_n = (n_total + NSUB * BN - 1) / (NSUB * BN);
+  gp.tiles_m = (m_total + kBM - 1) / kBM;
+  gp.tiles_n = (n_total + kBN - 1) / kBN;
   gp.epi = epi;
-  gp.a_collector = p->dw_collector;
-  const int units = CTA2 ? p->sms / 2 : p->sms;     // persistent: one CTA (or CTA pair) per SM (pair)
-  int tiles = gp.n_models * gp.tiles_m * gp.tiles_n;
-  if constexpr (NSUB == 2) {
-    // double-width tiles halve the tile count; where that leaves the last wave mostly empty, its row blocks run as
-    // single-width tiles instead (half the time each): cost in single-width tile times, per CTA (pair)
-    if (gp.tiles_n == 1) {
-      const int rows = gp.n_models * gp.tiles_m, rem = rows % units;
-      const int cost_wide = 2 * ((rows + units - 1) / units);
-      const int cost_mixed = 2 * (rows / units) + (2 * rem + units - 1) / units;
-      if (rem > 0 && cost_mixed < cost_wide) {
-        gp.tail_rows = rem;
-        tiles = (rows - rem) + 2 * rem;
-      }
-    }
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((tiles < units ? tiles : units) * (CTA2 ? 2 : 1));
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = SM::kBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CTA2 ? 2 : 1;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, gp));
+  const int tiles = gp.n_models * gp.tiles_m * gp.tiles_n;   // persistent: at most one CTA per SM
+  kern<<<tiles < p->sms ? tiles : p->sms, kGemmThreads, SM::kBytes, st>>>(gp);
+  CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }
 
-// Dispatch a K-major-A GEMM on (output width -> BN, K block, single CTA or CTA pair). Stage counts fill the
-// 192 KB operand ring: single 256x{64,32} -> 2,4; 128x{64,32} -> 3,6; pair 256x{64,32} -> 3,6; 128x{64,32} -> 4,8.
-// f16f8: K block 64 everywhere, a stage is one 16-bit plane of A and of B (or their four 8-bit planes): pair
-// 256-wide -> 6 stages of 32 KB, single 256-wide -> 4 of 48 KB, single 128-wide -> 6 of 32 KB; narrow outputs
-// never run on pairs (see build_maps).
+// Dispatch a K-major-A GEMM (f16f8 rescales inside one accumulator: never split)
 template <class Epi, bool B_MN, bool SPLIT, int ARITH, class... Args>
-static int launch_k(bool wide, int bk, bool pair, Args&&... a) {
-  if constexpr (ARITH == kArithF16F8) {
-    // epilogues that stage two chunks per bulk store take 8 KB per epilogue warp: one ring stage less
-    constexpr int big = Epi::kWarpStageBytes > 4096 ? 1 : 0;
-    if (wide)
-      return pair ? launch_gemm_t<Epi, 256, kBkF8, false, B_MN, 6 - big, false, true, kArithF16F8>(a...)
-                  : launch_gemm_t<Epi, 256, kBkF8, false, B_MN, 4 - big, false, false, kArithF16F8>(a...);
-    return launch_gemm_t<Epi, 128, kBkF8, false, B_MN, 6 - big, false, false, kArithF16F8>(a...);
-  } else {
-  if (wide) {
-    if (bk == 32)
-      return pair ? launch_gemm_t<Epi, 256, 32, false, B_MN, 6, SPLIT, true>(a...)
-                  : launch_gemm_t<Epi, 256, 32, false, B_MN, 4, SPLIT, false>(a...);
-    return pair ? launch_gemm_t<Epi, 256, 64, false, B_MN, 3, SPLIT, true>(a...)
-                : launch_gemm_t<Epi, 256, 64, false, B_MN, 2, SPLIT, false>(a...);
-  }
-  if (bk == 32)
-    return pair ? launch_gemm_t<Epi, 128, 32, false, B_MN, 8, SPLIT, true>(a...)
-                : launch_gemm_t<Epi, 128, 32, false, B_MN, 6, SPLIT, false>(a...);
-  return pair ? launch_gemm_t<Epi, 128, 64, false, B_MN, 4, SPLIT, true>(a...)
-              : launch_gemm_t<Epi, 128, 64, false, B_MN, 3, SPLIT, false>(a...);
-  }
+static int launch_k(Args&&... a) {
+  return launch_gemm_t<Epi, false, B_MN, SPLIT && ARITH != kArithF16F8, ARITH>(a...);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -653,8 +581,6 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   const int tiles_mB = (B + kBM - 1) / kBM;
 
   prof_mark(p, SCE_PHASE_SPLIT, st);
-  // the f16f8 kernels run narrow outputs on single CTAs (build_maps)
-  auto pair_ok = [&](int flag, int rows, int out_cols) { return use_pair(flag, rows) && !(f8 && out_cols <= 128); };
   if (d.centering) {
     // ---- centring (sae_ensemble.py:126-128): (x - trans[m]) -> planes, GEMM with rot[m] (all split passes), * scale[m]
     // -> the per-model fp32 batch every kernel below reads as `x`
@@ -668,8 +594,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     cp.model_stride = (long long)B * dd;
     cp.ld = dd;
     cp.col_scale = p->b.center_scale;
-    rc = launch_k<EpiCenter, false, false, AR>(dd > 128, p->bk_encode, pair_ok(p->pair_encode, B, dd), p, maps->center, 1, one, one,
-                                              dd, 3, B, dd, cp, st);
+    rc = launch_k<EpiCenter, false, false, AR>(p, maps->center, 1, one, one, dd, 3, B, dd, cp, st);
     if (rc) return rc;
     launches += 2;
     x = p->x_centered;
@@ -717,9 +642,8 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     ep.tiles_m = tiles_mB;
     ep.flag_zero = 1;
     ep.act = act;
-    ep.tiles_n = n > 128 ? (n + 255) / 256 : 1;
-    rc = launch_k<EpiEnc, false, false, AR>(n > 128, p->bk_encode, pair_ok(p->pair_encode, B, n), p, maps->encode, 1, xb, one,
-                                            dd, d.fwd_passes, B, n, ep, st, x_is_a);
+    ep.tiles_n = (n + kBN - 1) / kBN;
+    rc = launch_k<EpiEnc, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
     if (rc) return rc;
     ++launches;
     n_enc_parts = tiles_mB * 8 * ep.tiles_n;
@@ -732,8 +656,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       sp.n_chunks = act.n_chunks;
       sp.cmax_model_stride = (long long)Bm * act.n_chunks;
     }
-    rc = launch_k<EpiScoresTma, false, false, AR>(n > 128, p->bk_encode, pair_ok(p->pair_encode, B, n), p, maps->encode, 1, xb,
-                                                 one, dd, d.fwd_passes, B, n, sp, st, x_is_a);
+    rc = launch_k<EpiScoresTma, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, sp, st, x_is_a);
     if (rc) return rc;
     ++launches;
     static bool cfg[64] = {};
@@ -788,19 +711,11 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   dp.ld = dd;
   dp.tiles_m = tiles_mB;
   dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
-  dp.tiles_n = dd > 128 ? (dd + 255) / 256 : 1;
-  if (f8 && p->dec_nsub2 && dd % 512 == 0 && pair_ok(p->pair_decode, B, dd)) {
-    // experiment (SCE_TUNE_DEC_NSUB2=1): 256 x 512 tiles — the code tile (A) read once for both column halves, kept in the
-    // collector; the accumulators fill all of tensor memory, so the epilogue no longer overlaps the next main loop
-    if constexpr (f8)
-      rc = launch_gemm_t<EpiDec, 256, kBkF8, false, true, 4, false, true, kArithF16F8, 2>(p, maps->decode, 1, one, one, n, d.fwd_passes,
-                                                                                      B, dd, dp, st);
-  } else if (p->split_decode && !f8)
-    rc = launch_k<EpiDec, true, true, AR>(dd > 128, p->bk_decode, pair_ok(p->pair_decode, B, dd), p, maps->decode, 1, one, one,
-                                          n, d.fwd_passes, B, dd, dp, st);
+  dp.tiles_n = (dd + kBN - 1) / kBN;
+  if (p->split_decode && !f8)
+    rc = launch_k<EpiDec, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
   else
-    rc = launch_k<EpiDec, true, false, AR>(dd > 128, p->bk_decode, pair_ok(p->pair_decode, B, dd), p, maps->decode, 1, one, one,
-                                           n, d.fwd_passes, B, dd, dp, st);
+    rc = launch_k<EpiDec, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
   if (rc) return rc;
   ++launches;
   n_dec_parts = tiles_mB * 8 * dp.tiles_n;
@@ -839,8 +754,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
     // (per-model batches carry one flag for all of them, so the same test holds)
     zp.x_res_flag = f8 ? p->res_flags : nullptr;
-    rc = launch_k<EpiDco, false, false, AR>(n > 128, p->bk_dcode, pair_ok(p->pair_dcode, B, n), p, maps->dcode, 1, one, one, dd,
-                                            p->dcode_passes, B, n, zp, st);
+    rc = launch_k<EpiDco, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
     if (rc) return rc;
     ++launches;
     }
@@ -853,21 +767,8 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       sp.model_stride = (long long)n * dd;
       sp.ld = dd;
       sp.scale = grad_out_scale(p, B);
-      const bool pair = pair_ok(p->pair_dw, n, dd);
-      if constexpr (f8) {
-        // d > 256: both 256-column halves of a dictionary row block from one A (dz / c) tile per K block (NSUB = 2)
-        if (dd % 512 == 0 && pair && p->dw_nsub2)
-          return launch_gemm_t<EpiStoreF32, 256, kBkF8, true, true, 4, false, true, kArithF16F8, 2>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
-        if (dd > 128)
-          return pair ? launch_gemm_t<EpiStoreF32, 256, kBkF8, true, true, 6, false, true, kArithF16F8>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf)
-                      : launch_gemm_t<EpiStoreF32, 256, kBkF8, true, true, 4, false, false, kArithF16F8>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
-        return launch_gemm_t<EpiStoreF32, 128, kBkF8, true, true, 6, false, false, kArithF16F8>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
-      }
-      if (dd > 128)
-        return pair ? launch_gemm_t<EpiStoreF32, 256, kBkDw, true, true, 6, true, true>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st)
-                    : launch_gemm_t<EpiStoreF32, 256, kBkDw, true, true, 4, true, false>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st);
-      return pair ? launch_gemm_t<EpiStoreF32, 128, kBkDw, true, true, 8, true, true>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st)
-                  : launch_gemm_t<EpiStoreF32, 128, kBkDw, true, true, 6, true, false>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st);
+      // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one)
+      return launch_gemm_t<EpiStoreF32, true, true, !f8, AR>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
     };
     if (d.variant == SCE_UNTIED) {
       rc = dw(maps->dw_enc, 1, one, xb, p->dw_enc, x_is_b);
@@ -928,7 +829,7 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   CUDA_TRY(cudaGetDevice(&dev));
   CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  if (major != 10) return fail(SCE_ERR_NO_DEVICE, "libsce needs an sm_100 device (found compute capability %d.x)", major);
+  if (major != 9) return fail(SCE_ERR_NO_DEVICE, "libsce needs an sm_90 device (found compute capability %d.x)", major);
   if (!get_encode_fn()) return fail(SCE_ERR_NO_DEVICE, "cuTensorMapEncodeTiled driver entry point not available");
   sce_plan* p = new (std::nothrow) sce_plan;
   if (!p) return fail(SCE_ERR_INVALID, "out of host memory");
@@ -939,16 +840,9 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   p->device = dev;
   p->xm = desc->x_per_model ? desc->n_models : 1;
   p->arith = resolve_arith(*desc);
-  // CTA pairs by default for all four GEMMs (same-box A/B in profiles/r01g_pair_tuning.txt: -10 % encode,
-  // -9 % decode, -3 % dcode, -21 % weight gradient on that box; env SCE_TUNE_PAIR_* = 0 switches one back)
-  p->pair_encode = tune_flag("SCE_TUNE_PAIR_ENCODE", 1);
-  p->pair_decode = tune_flag("SCE_TUNE_PAIR_DECODE", 1);
-  p->pair_dcode = tune_flag("SCE_TUNE_PAIR_DCODE", 1);
-  p->pair_dw = tune_flag("SCE_TUNE_PAIR_DW", 1);
-  // The truncation bias of a single accumulation chain grows with the reduction length (about 3.7e-9 * n on x_hat,
-  // up to ~3.6x that on the loss): harmless at n <= 4096 (1.5e-5 / 3e-5 measured), over the 1e-4 bar near
-  // n = 16384-32768. Splitting costs the decode GEMM its accumulator double-buffering (1.14 -> 1.29 ms at config 2,
-  // profiles/r01i_split_decode_tuning.txt), so it is switched on where it is needed.
+  // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
+  // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
+  // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
   p->split_decode = tune_flag("SCE_TUNE_SPLIT_DECODE", desc->n > 4096 ? 1 : 0);
   p->dcode_passes = desc->bwd_passes;
   p->dw_passes = desc->bwd_passes;
@@ -959,15 +853,6 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
     const double issued = 30.0 * desc->n_models * (double)desc->batch_max * desc->n * desc->d;
     p->use_graph = tune_flag("SCE_GRAPH", issued < 3e11 ? 1 : 0);
   }
-  // 256 x 512 weight-gradient tiles (one A tile for both column halves): DRAM traffic of the launch 5.69 -> 4.25 GB
-  // at config 2, device time unchanged within the run-to-run noise (1.51 / 1.50 / 1.57 ms against 1.51 / 1.50 ms: the
-  // kernel is bound by the power-limited tensor rate either way) — off by default, kept as a knob
-  p->dw_nsub2 = tune_flag("SCE_TUNE_DW_NSUB2", 1);
-  p->dw_collector = tune_flag("SCE_TUNE_DW_COLL", 1);
-  p->dec_nsub2 = tune_flag("SCE_TUNE_DEC_NSUB2", 0);
-  p->bk_encode = tune_bk("SCE_TUNE_BK_ENCODE", 64);
-  p->bk_decode = tune_bk("SCE_TUNE_BK_DECODE", 32);
-  p->bk_dcode = tune_bk("SCE_TUNE_BK_DCODE", 64);
   {
     // k-sparse decode / dcode of the top-k variant: lists known (topk_k_max), bulk-copy alignment of the dictionary
     // half rows (16 bytes in every plane), shared memory of the gather kernel
@@ -980,15 +865,11 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
         p->tk_slices = sl;
     }
     // Worth it where the dictionary is large against k: the dense decode + dcode GEMMs cost ~ n per row, the gather
-    // kernel ~ k (it is bound by the latency chain of a block, not by bytes). Measured on B200, d = 768, 12 models,
-    // k in {16, 32, 64}, one launch per k class (tools/run_r02w.sh): n = 6144 dense 1.40 + 1.50 ms / sparse 2.56 + 0.31 ms —
-    // equal as kernels, but the step with the gather path is 4 % shorter (7.83 against 8.17 ms: the GPU runs these steps
-    // at its power cap and the gather kernel leaves the tensor pipes idle); n = 12288 dense 5.8 ms / sparse 2.9 ms;
-    // n = 3072: config 3 with every group on the gather path 22.26 ms against an estimated 22.15 ms with this rule.
+    // kernel ~ k (it is bound by the latency chain of a block, not by bytes): the gather path is used where n >= 96 k.
     // SCE_TOPK_SPARSE = 1 / 0 forces it on / off.
     const int heuristic = (long long)desc->n >= 96ll * (long long)(kmax ? kmax : 1);
     p->topk_sparse = desc->variant == SCE_TOPK && kmax > 0 && p->tk_slices > 0 && tune_flag("SCE_TOPK_SPARSE", heuristic);
-    // selection from the per-chunk maxima the scores epilogue writes (profiles/r02p_*); 0 = read every row twice as before
+    // selection from the per-chunk maxima the scores epilogue writes; 0 = read every row twice
     p->topk_cmax = desc->variant == SCE_TOPK && tune_flag("SCE_TOPK_CMAX", 1);
   }
   p->maps = new std::map<int, BatchMaps*>();

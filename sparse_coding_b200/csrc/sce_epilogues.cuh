@@ -1,6 +1,6 @@
 // sce_epilogues.cuh — the fused epilogues of the four GEMMs of one ensemble training step.
 // Each functor is constructed per (thread, tile) by gemm_split_kernel, receives the fp32
-// accumulator of its row in 32-column chunks straight from TMEM, and writes what the next GEMM
+// accumulator of its row in 32-column chunks, and writes what the next GEMM
 // needs — as operand planes (fp16 + two E5M2 planes, or a (hi, lo) bf16 pair; 4 bytes per element either way) — so
 // the fp32 code tensor [M,B,n] never exists in HBM.
 //
@@ -13,9 +13,8 @@
 #include "sce_gemm.cuh"
 
 #ifndef SCE_EPI_PAIR
-// f16f8 encode / dcode epilogues: 1 = two adjacent chunks per bulk store (stage_pair_and_store), 0 = one chunk per store.
-// Measured slower (ncu, same box: encode 0.905 vs 0.841 ms, dcode 0.981 vs 0.954 ms; profiles/r02b_epilogue_writeout_experiments.txt):
-// kept as a build option only.
+// f16f8 encode / dcode epilogues: 1 = two adjacent chunks per bulk store (stage_pair_and_store), 0 = one chunk per store
+// (the default; the paired form is kept as a build option only).
 #define SCE_EPI_PAIR 0
 #endif
 
@@ -96,8 +95,7 @@ __device__ __forceinline__ void stage_and_store(uint8_t* stage, int lane, const 
 // f16f8, two adjacent 32-column chunks per bulk store (Epi::kPairChunks): an epilogue warp stages the chunks 2q and 2q+1 of
 // its rows side by side — fp16 tile of 32 rows x 128 B (128-byte swizzle), two 8-bit tiles of 32 rows x 64 B (64-byte
 // swizzle), 8 KB per warp — and hands each tile to the TMA engine ONCE per pair: three bulk stores and one wait for the
-// staging tile per 64 columns instead of per 32 (the write-out of these epilogues is bound by the latency of the store
-// queue x requests in flight, profiles/r02b_epilogue_writeout_experiments.txt), and the fp16 plane goes out in full
+// staging tile per 64 columns instead of per 32, and the fp16 plane goes out in full
 // 128-byte lines. `half` = which chunk of the pair this is; `last` = no further chunk of this pair follows (second half,
 // or the first half at the ragged right edge: the engine clips the columns beyond the tensor).
 // ------------------------------------------------------------------------------------------------
@@ -292,7 +290,7 @@ struct EpiEncodeT {
   __device__ __forceinline__ void finish() {
     if (T.lane == 0) tma_store_wait_read();  // the staging tiles must outlive their bulk stores
     const float a = warp_sum(l1), b = warp_sum(float(nnz));
-    if (T.lane == 0 && T.m_blk * kBM < m_total) {  // (a CTA pair's second half may lie wholly past the batch)
+    if (T.lane == 0 && T.m_blk * kBM < m_total) {
       float* o = P.part +
                  ((((long long)T.model * P.tiles_m + T.m_blk) * 8 + T.grp * 4 + T.warp_q) * P.tiles_n + T.n_blk) * 2;
       o[0] = a;

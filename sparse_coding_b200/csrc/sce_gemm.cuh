@@ -1,32 +1,32 @@
-// sce_gemm.cuh — persistent, warp-specialised, batched split-operand GEMM on tcgen05 / TMEM / TMA.
+// sce_gemm.cuh — persistent, warp-specialised, batched split-operand GEMM on wgmma / TMA / mbarrier (sm_90a).
 //
-//   D[model][i][j] = sum_set sum_k A_set[model][i,k] * B_set[model][j,k]            (fp32 in TMEM)
+//   D[model][i][j] = sum_set sum_k A_set[model][i,k] * B_set[model][j,k]            (fp32 accumulators)
 //
-// This is how the engine reaches the reference's true-FP32 results (SURVEY.md H1) on the low-precision tensor
-// pipes. Every fp32 operand is carried as operand planes and the product formed from partial products:
-//   ARITH = bf16x3: x ~= hi + lo (two bf16 planes); hi*hi + hi*lo + lo*hi, three kind::f16 passes (~2^-16);
-//   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h as one kind::f16 pass, the two cross terms as kind::f8f6f4 passes
-//                   on E5M2 planes at twice the rate, rescaled inside the accumulator (see sce_ptx.cuh) — 2 pass
-//                   equivalents, the default.
+// This is how the engine reaches the reference's true-FP32 results (SURVEY.md H1) on the 16-bit tensor cores.
+// Every fp32 operand is carried as operand planes and the product formed from partial products:
+//   ARITH = bf16x3: x ~= hi + lo (two bf16 planes); hi*hi + hi*lo + lo*hi, three bf16 passes (~2^-16);
+//   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h on the fp16 planes, the two cross terms on E5M2 planes widened to fp16
+//                   in shared memory and rescaled in the accumulator (see sce_ptx.cuh) — the default.
 // `passes == 1` keeps only the 16-bit plane product. Operands may be K-major (reduction index contiguous in HBM) or
 // MN-major (row/column index contiguous), so no transposed copies of activations/codes are ever written.
 //
-// One CTA per SM, 384 threads: warp 0 = TMA producer, warp 1 = MMA issuer, warp 2 = TMEM
-// allocator, warps 4..11 = epilogue (TMEM -> registers -> fused epilogue -> HBM). Accumulators are
-// double-buffered in TMEM so the epilogue of tile t overlaps the main loop of tile t+1.
-// Eight epilogue warps (two per TMEM lane quarter, alternating 32-column chunks) because a single
-// warp per scheduler is latency-bound: the r01a profile showed ~37 issued instructions per element
-// at IPC ~0.25 holding the tensor pipe at 31 % in the encode GEMM.
+// One CTA per SM, 384 threads: warp 0 = TMA producer (one thread), warpgroups 1 and 2 = wgmma consumers (rows 0..63
+// and 64..127 of the 128 x 128 tile), which then run the fused epilogue. The accumulators go through a padded fp32
+// tile in shared memory so that each epilogue thread owns one output row and 32 consecutive columns: eight epilogue
+// warps, warp w handling rows 32 (w % 4) .. +31 and the 32-column chunks with chunk % 2 == w / 4. The producer keeps
+// loading the next tile's stages while the epilogue runs.
 #pragma once
 #include <type_traits>
 #include "sce_ptx.cuh"
 
 namespace sce {
 
-constexpr int kBM = 128;        // rows of the output tile == TMEM lanes
+constexpr int kBM = 128;        // rows of the output tile
+constexpr int kBN = 128;        // columns of the output tile
 constexpr int kGemmThreads = 384;
 constexpr int kEpiWarps = 8;
 constexpr int kMaxSets = 2;
+constexpr int kSmemLimit = 232448;  // 227 KB of shared memory one CTA may use on sm_90
 
 // What the epilogue functor sees for each tile.
 struct TileCoord {
@@ -48,59 +48,53 @@ struct GemmParams {
   // f16f8: optional device flags, one per operand: *flag == 0 says "the residual plane (x8) of this operand is all
   // zeros for this launch" (e.g. activations that are exactly fp16, the reference's chunk format). The cross term that
   // multiplies that plane is then skipped together with the loads of its two planes: 25 % fewer operand bytes and
-  // 8-bit instructions for that operand pair, bit-identical results. nullptr = no such knowledge.
+  // cross-term instructions for that operand pair, bit-identical results. nullptr = no such knowledge.
   const uint32_t* a_res_flag[kMaxSets];
   const uint32_t* b_res_flag[kMaxSets];
   int a_batched[kMaxSets], b_batched[kMaxSets];  // 0: operand shared by all models
   int nsets;      // number of (A,B) operand pairs accumulated into the same tile
   int k_total;    // reduction length of each pair
-  int passes;     // 3: hi*hi + hi*lo + lo*hi (f16f8: fp16 hh + two fp8 cross terms), 1: hi*hi
+  int passes;     // 3: hi*hi + hi*lo + lo*hi (f16f8: fp16 hh + two cross terms), 1: hi*hi
   int n_models, m_total, n_total;
   int tiles_m, tiles_n;
-  // NSUB == 2 only: the last `tail_rows` row blocks (model-major order) are processed as single-width tiles, two per
-  // row block, so that the final wave of the persistent grid is not half empty (requires tiles_n == 1). 0 = none.
-  int tail_rows;
-  // NSUB == 2 only: issue the two MMAs of a K slice as collector::a::fill / ::lastuse (A read from shared memory once)
-  int a_collector;
   EpiParams epi;
 };
 
-template <int BN, int BK, bool A_MN, bool B_MN, int STAGES, int EPI_WARP_BYTES = 0, bool CTA2 = false, int ARITH = 0,
-          int NSUB = 1>
-struct GemmSmem {
-  static constexpr int kATile = kBM * BK * 2;   // bytes, one of hi/lo
-  static constexpr int kBSub = CTA2 ? BN / 2 : BN;   // B rows of ONE sub-tile held by this CTA (a pair splits B)
-  static constexpr int kBRows = NSUB * kBSub;        // NSUB sub-tiles of BN output columns share one A tile
-  static constexpr int kBTile = kBRows * BK * 2;
+constexpr int kArithBf16x3 = 0, kArithF16F8 = 1;
+
+constexpr int align1k(int v) { return (v + 1023) / 1024 * 1024; }
+
+template <int BK, int EPI_WARP_BYTES, int ARITH>
+struct GemmSmemLayout {
+  static constexpr int kATile = kBM * BK * 2;   // bytes of one 16-bit A tile
+  static constexpr int kBTile = kBN * BK * 2;
   // bf16x3: hi and lo planes of A and B. f16f8: either the fp16 planes or the four 8-bit planes (same bytes).
-  static constexpr int kStage = ARITH == 1 ? kATile + kBTile : 2 * kATile + 2 * kBTile;
-  static constexpr int kBarOff = STAGES * kStage;
-  static constexpr int kEpiOff = kBarOff + 1024;  // barriers + tmem ptr live in the 1 KB before (keeps 1 KB alignment)
-  static constexpr int kBytes = kEpiOff + kEpiWarps * EPI_WARP_BYTES + 1024 /*align slack*/;
-  static_assert(kBytes <= 232448, "exceeds the 227 KB of shared memory one CTA may use");
+  static constexpr int kStage = ARITH == kArithBf16x3 ? 2 * kATile + 2 * kBTile : kATile + kBTile;
+  static constexpr int kAccLd = kBN + 1;         // padded row of the fp32 accumulator tile (conflict-free both ways)
+  static constexpr int kAccBytes = kBM * kAccLd * 4;
+  // f16f8: the four 8-bit tiles of a stage widened to fp16 (shares the space of the accumulator tile: never live together)
+  static constexpr int kWideBytes = ARITH == kArithF16F8 ? 2 * kATile + 2 * kBTile : 0;
+  static constexpr int kAccRegion = align1k(kAccBytes > kWideBytes ? kAccBytes : kWideBytes);
+  static constexpr int kFixed = kAccRegion + kEpiWarps * EPI_WARP_BYTES + 1024 /*barriers*/ + 1024 /*align slack*/;
+  static constexpr int kMaxStages = (kSmemLimit - kFixed) / kStage;
 };
 
-// ------------------------------------------------------------------------------------------------
-// The kernel
-// ------------------------------------------------------------------------------------------------
-// SPLIT_ACC: keep the dominant hi*hi products and the small cross terms (hi*lo, lo*hi) in two separate
-// TMEM accumulators (summed in the epilogue). The tensor core's fp32 accumulation truncates, which biases a
-// result by about -2e-8 per accumulated MMA (measured: 1.3e-4 at K = 32768 with all three passes in one
-// chain); the cross terms are 2^-8 of the total, so moving them out shortens the chain that matters 3x.
-// Costs the second accumulator stage (tile epilogue no longer overlaps the next main loop), so it is used
-// where the reduction is long and the epilogue short: the decode GEMM (K = n).
-//
-// CTA2: the tile is 256 x BN and is computed by a CTA pair (cluster of 2, tcgen05 cta_group::2). Each CTA
-// keeps 128 accumulator rows in its own TMEM, loads its own 128 rows of A and HALF of the B tile, so a stage
-// is 1/3 smaller (three K=64 stages fit instead of two) and each SM reads a third less shared memory per
-// MMA. `tiles_m` then counts 256-row tiles; TileCoord::m_blk stays in 128-row units (2*tile_m + cta rank).
-//
-// ARITH = kArithF16F8 (see sce_ptx.cuh, "fp16 + fp8 arithmetic"): a tile makes TWO sweeps over K. Sweep 1 streams the
-// 8-bit planes (a stage holds A.h8, A.l8, B.h8, B.l8 — the same bytes as A.f16 + B.f16) and issues the cross terms
-// as kind::f8f6f4; sweep 2 streams the fp16 planes and issues hh as kind::f16, its first instruction rescaling the
-// accumulator by 2^-kLoShift. One accumulator, so the double-buffered TMEM stages stay, and the chain of dominant
-// products is as short as with SPLIT_ACC.
-constexpr int kArithBf16x3 = 0, kArithF16F8 = 1;
+template <int BK, int STAGES, int EPI_WARP_BYTES, int ARITH>
+struct GemmSmem : GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH> {
+  using L = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH>;
+  static constexpr int kAccOff = STAGES * L::kStage;
+  static constexpr int kEpiOff = kAccOff + L::kAccRegion;
+  static constexpr int kBarOff = kEpiOff + kEpiWarps * EPI_WARP_BYTES;
+  static constexpr int kBytes = kBarOff + 1024 + 1024;
+  static_assert(kBytes <= kSmemLimit, "exceeds the 227 KB of shared memory one CTA may use");
+};
+
+// pipeline depth: as many stages as fit beside the accumulator tile and the epilogue staging (at most 8)
+template <int BK, int EPI_WARP_BYTES, int ARITH>
+constexpr int gemm_stages() {
+  constexpr int s = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH>::kMaxStages;
+  return s > 8 ? 8 : s;
+}
 
 // epilogues may declare `static constexpr bool kPairChunks = true` (see the epilogue loop of gemm_split_kernel)
 template <class Epi, class = void>
@@ -108,70 +102,80 @@ struct epi_pairs_chunks : std::false_type {};
 template <class Epi>
 struct epi_pairs_chunks<Epi, std::void_t<decltype(Epi::kPairChunks)>> : std::bool_constant<Epi::kPairChunks> {};
 
+// f16f8: an 8-bit tile as TMA delivers it without swizzle — K-major [ROWS][BK] or MN-major [BK][ROWS] bytes — widened
+// to the fp16 tile the 16-bit loads of the same operand produce: K-major [ROWS][BK] with the 128-byte swizzle (BK = 64),
+// MN-major [ROWS / 64][BK][64] with the 128-byte swizzle. 256 consumer threads, 16 bytes each per round.
+template <bool MN, int BK, int ROWS>
+__device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int tid) {
+  static_assert(BK == 64, "the widened K-major tile has 128-byte rows");
+  constexpr int kPieces = ROWS * BK / 16;
+#pragma unroll 2
+  for (int q = tid; q < kPieces; q += 256) {
+    const uint4 v = *reinterpret_cast<const uint4*>(src + q * 16);
+    uint4 w0, w1;
+    widen_e5m2x4(v.x, w0.x, w0.y);
+    widen_e5m2x4(v.y, w0.z, w0.w);
+    widen_e5m2x4(v.z, w1.x, w1.y);
+    widen_e5m2x4(v.w, w1.z, w1.w);
+    int o0, o1;
+    if constexpr (!MN) {
+      const int r = q / (BK / 16), j = (q % (BK / 16)) * 2;   // 16-byte chunk of the 128-byte fp16 row
+      o0 = r * 128 + ((j ^ (r & 7)) << 4);
+      o1 = r * 128 + (((j + 1) ^ (r & 7)) << 4);
+    } else {
+      const int k = q / (ROWS / 16), m0 = (q % (ROWS / 16)) * 16;
+      const int base = (m0 >> 6) * (BK * 128) + k * 128, j = (m0 & 63) >> 3;
+      o0 = base + ((j ^ (k & 7)) << 4);
+      o1 = base + (((j + 1) ^ (k & 7)) << 4);
+    }
+    *reinterpret_cast<uint4*>(dst + o0) = w0;
+    *reinterpret_cast<uint4*>(dst + o1) = w1;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The kernel
+// ------------------------------------------------------------------------------------------------
+// SPLIT_ACC: keep the dominant hi*hi products and the small cross terms (hi*lo, lo*hi) in two separate
+// accumulators (summed in the epilogue). The tensor core's fp32 accumulation truncates, which biases a
+// result by a small amount per accumulated MMA; the cross terms are 2^-8 of the total, so moving them out
+// shortens the chain that matters 3x. Used where the reduction is long: the decode GEMM at large n and the
+// weight gradient (K = batch).
 //
-// NSUB = 2 (f16f8 only): the output tile is 256 x (2 * BN): both BN-column halves are accumulated from ONE A tile per
-// K block (two MMAs per K slice, two accumulators filling all 512 TMEM columns, so no accumulator double-buffering —
-// for GEMMs whose epilogue is negligible). Shared memory then takes 96 instead of 128 KB per two tiles' worth of MMAs
-// (the f16f8 main loop otherwise runs exactly at the SM's shared-memory bandwidth), and the A operand is read from
-// L2 / HBM once instead of once per column half.
-template <class Epi, int BN, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, bool CTA2 = false,
-          int ARITH = kArithBf16x3, int NSUB = 1>
+// ARITH = kArithF16F8 (see sce_ptx.cuh, "fp16 + fp8 arithmetic"): a tile makes TWO sweeps over K. Sweep 1 streams the
+// 8-bit planes (a stage holds A.h8, A.l8, B.h8, B.l8 — the same bytes as A.f16 + B.f16), widens them to fp16 and
+// accumulates the cross terms; the accumulator is then scaled by 2^-kLoShift; sweep 2 streams the fp16 planes and adds hh.
+template <class Epi, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, int ARITH = kArithBf16x3>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
-  static_assert(NSUB == 1 || (NSUB == 2 && F8 && BN == 256), "two sub-tiles: f16f8, 256 columns each");
+  constexpr int BN = kBN;
   static_assert(!F8 || !SPLIT_ACC, "f16f8 rescales in the accumulator; no split accumulators");
-  static_assert(!F8 || BK % 32 == 0, "an fp8 instruction covers K = 32");
-  static_assert(BN % 64 == 0 && BN <= 256, "BN must be a multiple of 64, at most 256");
-  static_assert(BK % 16 == 0 && BK <= 64, "BK in {16,32,48,64}");
-  static_assert(A_MN || BK == 64 || BK == 32, "K-major A: one swizzled row per tile row, 128 B (BK=64) or 64 B (BK=32)");
-  static_assert(B_MN || BK == 64 || BK == 32, "K-major B: one swizzled row per tile row, 128 B (BK=64) or 64 B (BK=32)");
-  using SM = GemmSmem<BN, BK, A_MN, B_MN, STAGES, Epi::kWarpStageBytes, CTA2, ARITH, NSUB>;
-  static_assert(!CTA2 || BN % 128 == 0, "a CTA pair splits B in halves of whole 64-column boxes");
-  constexpr int EC = Epi::kCols;  // accumulator columns handed to the epilogue per call (32 or 64)
-  static_assert(EC == 32 || EC == 64, "epilogue chunk is 32 or 64 columns");
-  static_assert(BN % EC == 0, "tile width must be a multiple of the epilogue chunk");
-  constexpr int kAccStages = (SPLIT_ACC || NSUB == 2) ? 1 : 2;
-  constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128
-                                 : (2 * BN <= 256) ? 256 : 512;
+  static_assert(!F8 || BK == 64, "f16f8: K block 64");
+  static_assert(BK == 32 || BK == 64, "BK in {32, 64}: one swizzled row (64 or 128 B) per K-major tile row");
+  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH>;
+  constexpr int EC = Epi::kCols;  // accumulator columns handed to the epilogue per call
+  static_assert(EC == 32, "epilogue chunk is 32 columns");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOff);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int cta_rank = CTA2 ? int(cluster_ctarank()) : 0;
-  const int tile0 = CTA2 ? int(blockIdx.x >> 1) : int(blockIdx.x);       // first tile of this CTA (pair)
-  const int tile_step = CTA2 ? int(gridDim.x >> 1) : int(gridDim.x);
-  const int big_tiles = (p.n_models * p.tiles_m - (NSUB == 2 ? p.tail_rows : 0)) * p.tiles_n;
-  const int num_tiles = big_tiles + (NSUB == 2 ? 2 * p.tail_rows : 0);
-  // tile index -> (model, tile row, first BN-column block, number of BN-column sub-tiles)
-  auto decode_tile = [&](int tile, int& model, int& tile_m, int& n0, int& nsub) {
-    if (NSUB == 2 && tile >= big_tiles) {
-      const int t = tile - big_tiles;
-      const int rb = big_tiles + (t >> 1);   // tiles_n == 1 here: row block index == big tile index
-      model = rb / p.tiles_m;
-      tile_m = rb - model * p.tiles_m;
-      n0 = t & 1;
-      nsub = 1;
-    } else {
-      model = tile / (p.tiles_m * p.tiles_n);
-      const int rem = tile - model * (p.tiles_m * p.tiles_n);
-      tile_m = rem / p.tiles_n;
-      n0 = (rem % p.tiles_n) * NSUB;
-      nsub = NSUB;
-    }
+  const int num_tiles = p.n_models * p.tiles_m * p.tiles_n;
+  auto decode_tile = [&](int tile, int& model, int& tile_m, int& tile_n) {
+    model = tile / (p.tiles_m * p.tiles_n);
+    const int rem = tile - model * (p.tiles_m * p.tiles_n);
+    tile_m = rem / p.tiles_n;
+    tile_n = rem % p.tiles_n;
   };
   const int kblocks = (p.k_total + BK - 1) / BK;
   const bool three = p.passes >= 3;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < p.nsets; ++s) {
       tma_prefetch_desc(&p.a_hi[s]);
       tma_prefetch_desc(&p.b_hi[s]);
@@ -184,32 +188,13 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
         }
       }
     }
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], CTA2 ? 2 * kEpiWarps : kEpiWarps);  // pair: both CTAs' epilogues report to CTA 0
+      mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    if constexpr (CTA2) {
-      tmem_alloc_2cta(tmem_ptr, kTmemCols);
-      tmem_relinquish_2cta();
-    } else {
-      tmem_alloc(tmem_ptr, kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();  // the peer's barriers must be initialised before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   // f16f8: which cross terms each operand pair needs (see GemmParams::a_res_flag); the same for every CTA of the launch
   [[maybe_unused]] bool term_lh[kMaxSets], term_hl[kMaxSets];
   if constexpr (F8) {
@@ -220,26 +205,22 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     }
   }
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ======================= TMA producer =======================
-    if (lane == 0) {
-      const uint32_t stage_bytes_full = (three && !F8) ? uint32_t(SM::kStage) : uint32_t(SM::kATile + SM::kBTile);
-      // one copy: same-CTA barrier, or (pair) the cta_group::2 form that completes on CTA 0's barrier
-      auto load = [&](void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-        if constexpr (CTA2) tma_load_3d_2cta(dst, m, bar, c0, c1, c2);
-        else tma_load_3d(dst, m, bar, c0, c1, c2);
-      };
-      constexpr int kBHalf = SM::kBSub;  // B rows (N index) of one sub-tile this CTA loads
+    if (threadIdx.x == 0) {
+      const uint32_t stage_bytes = (three && !F8) ? uint32_t(SM::kStage) : uint32_t(SM::kATile + SM::kBTile);
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        int model, tile_m, n0, nsub;
-        decode_tile(tile, model, tile_m, n0, nsub);
-        const int m_blk = tile_m * (CTA2 ? 2 : 1) + cta_rank;
-        const int b_row0 = n0 * BN + cta_rank * kBHalf;  // (+ sub * BN for the second sub-tile)
-        [[maybe_unused]] const int n_blk = n0;
-        // bytes of a 16-bit stage of THIS tile (a tail tile of an NSUB = 2 launch loads one sub-tile of B only)
-        const uint32_t stage_bytes = F8 ? uint32_t(SM::kATile + nsub * (SM::kBSub * BK * 2)) : stage_bytes_full;
+      auto next = [&]() {
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      };
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int model, tile_m, tile_n;
+        decode_tile(tile, model, tile_m, tile_n);
+        const int a_row0 = tile_m * kBM, b_row0 = tile_n * BN;
         if constexpr (F8) {
           // sweep 1: the 8-bit planes (skipped for passes == 1); sweep 2: the fp16 planes
           for (int sweep = three ? 0 : 1; sweep < 2; ++sweep)
@@ -253,310 +234,223 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
               for (int kb = 0; kb < kblocks; ++kb) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
                 uint8_t* st = smem + stage * SM::kStage;
-                if (!CTA2 || cta_rank == 0) mbar_expect_tx(&full_bar[stage], CTA2 ? 2 * bytes : bytes);
+                uint64_t* bar = &full_bar[stage];
+                mbar_expect_tx(bar, bytes);
                 const int k0 = kb * BK;
                 if (sweep == 1) {
                   uint8_t* sa = st;
                   uint8_t* sb = st + SM::kATile;
-                  if constexpr (!A_MN) load(sa, &p.a_hi[set], &full_bar[stage], k0, m_blk * kBM, am);
+                  if constexpr (!A_MN) tma_load_3d(sa, &p.a_hi[set], bar, k0, a_row0, am);
                   else {
 #pragma unroll
-                    for (int j = 0; j < kBM / 64; ++j)
-                      load(sa + j * (BK * 128), &p.a_hi[set], &full_bar[stage], m_blk * kBM + j * 64, k0, am);
+                    for (int j = 0; j < kBM / 64; ++j) tma_load_3d(sa + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am);
                   }
-                  for (int sub = 0; sub < nsub; ++sub) {
-                    uint8_t* sbs = sb + sub * (kBHalf * BK * 2);
-                    const int r0 = b_row0 + sub * BN;
-                    if constexpr (!B_MN) load(sbs, &p.b_hi[set], &full_bar[stage], k0, r0, bm);
-                    else {
+                  if constexpr (!B_MN) tma_load_3d(sb, &p.b_hi[set], bar, k0, b_row0, bm);
+                  else {
 #pragma unroll
-                      for (int j = 0; j < kBHalf / 64; ++j)
-                        load(sbs + j * (BK * 128), &p.b_hi[set], &full_bar[stage], r0 + j * 64, k0, bm);
-                    }
+                    for (int j = 0; j < BN / 64; ++j) tma_load_3d(sb + j * (BK * 128), &p.b_hi[set], bar, b_row0 + j * 64, k0, bm);
                   }
                 } else {
+                  // 8-bit tiles, unswizzled: K-major [rows][BK] or MN-major [BK][128] bytes
                   uint8_t* sa_h = st;
                   uint8_t* sa_l = st + SM::kATile / 2;
                   uint8_t* sb_h = st + SM::kATile;
                   uint8_t* sb_l = sb_h + SM::kBTile / 2;
-                  if constexpr (!A_MN) {
-                    if (t_hl) load(sa_h, &p.a_lo[set], &full_bar[stage], k0, m_blk * kBM, am);
-                    if (t_lh) load(sa_l, &p.a_x8[set], &full_bar[stage], k0, m_blk * kBM, am);
-                  } else {
-                    static_assert(!F8 || !A_MN || kBM == 128, "one 128-element box per MN-major 8-bit A tile");
-                    if (t_hl) load(sa_h, &p.a_lo[set], &full_bar[stage], m_blk * kBM, k0, am);
-                    if (t_lh) load(sa_l, &p.a_x8[set], &full_bar[stage], m_blk * kBM, k0, am);
-                  }
-                  for (int sub = 0; sub < nsub; ++sub) {
-                    uint8_t* sbh = sb_h + sub * (kBHalf * BK);
-                    uint8_t* sbl = sb_l + sub * (kBHalf * BK);
-                    const int r0 = b_row0 + sub * BN;
-                    if constexpr (!B_MN) {
-                      if (t_lh) load(sbh, &p.b_lo[set], &full_bar[stage], k0, r0, bm);
-                      if (t_hl) load(sbl, &p.b_x8[set], &full_bar[stage], k0, r0, bm);
-                    } else {
-                      static_assert(!F8 || !B_MN || kBHalf % 128 == 0, "MN-major 8-bit B tiles come in 128-element boxes");
-#pragma unroll
-                      for (int j = 0; j < kBHalf / 128; ++j) {
-                        if (t_lh) load(sbh + j * (BK * 128), &p.b_lo[set], &full_bar[stage], r0 + j * 128, k0, bm);
-                        if (t_hl) load(sbl + j * (BK * 128), &p.b_x8[set], &full_bar[stage], r0 + j * 128, k0, bm);
-                      }
-                    }
-                  }
+                  const int ac0 = A_MN ? a_row0 : k0, ac1 = A_MN ? k0 : a_row0;
+                  const int bc0 = B_MN ? b_row0 : k0, bc1 = B_MN ? k0 : b_row0;
+                  if (t_hl) tma_load_3d(sa_h, &p.a_lo[set], bar, ac0, ac1, am);
+                  if (t_lh) tma_load_3d(sa_l, &p.a_x8[set], bar, ac0, ac1, am);
+                  if (t_lh) tma_load_3d(sb_h, &p.b_lo[set], bar, bc0, bc1, bm);
+                  if (t_hl) tma_load_3d(sb_l, &p.b_x8[set], bar, bc0, bc1, bm);
                 }
-                if (++stage == STAGES) {
-                  stage = 0;
-                  phase ^= 1;
-                }
+                next();
               }
             }
         } else {
-        for (int set = 0; set < p.nsets; ++set) {
-          const int am = p.a_batched[set] ? model : 0;
-          const int bm = p.b_batched[set] ? model : 0;
-          for (int kb = 0; kb < kblocks; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa_hi = smem + stage * SM::kStage;
-            uint8_t* sa_lo = sa_hi + SM::kATile;
-            uint8_t* sb_hi = sa_lo + SM::kATile;
-            uint8_t* sb_lo = sb_hi + SM::kBTile;
-            // pair: CTA 0 announces the bytes of BOTH CTAs; the peer's copies complete on CTA 0's barrier
-            if (!CTA2 || cta_rank == 0) mbar_expect_tx(&full_bar[stage], CTA2 ? 2 * stage_bytes : stage_bytes);
-            const int k0 = kb * BK;
-            if constexpr (!A_MN) {
-              load(sa_hi, &p.a_hi[set], &full_bar[stage], k0, m_blk * kBM, am);
-              if (three) load(sa_lo, &p.a_lo[set], &full_bar[stage], k0, m_blk * kBM, am);
-            } else {
+          for (int set = 0; set < p.nsets; ++set) {
+            const int am = p.a_batched[set] ? model : 0;
+            const int bm = p.b_batched[set] ? model : 0;
+            for (int kb = 0; kb < kblocks; ++kb) {
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              uint8_t* sa_hi = smem + stage * SM::kStage;
+              uint8_t* sa_lo = sa_hi + SM::kATile;
+              uint8_t* sb_hi = sa_lo + SM::kATile;
+              uint8_t* sb_lo = sb_hi + SM::kBTile;
+              uint64_t* bar = &full_bar[stage];
+              mbar_expect_tx(bar, stage_bytes);
+              const int k0 = kb * BK;
+              if constexpr (!A_MN) {
+                tma_load_3d(sa_hi, &p.a_hi[set], bar, k0, a_row0, am);
+                if (three) tma_load_3d(sa_lo, &p.a_lo[set], bar, k0, a_row0, am);
+              } else {
 #pragma unroll
-              for (int j = 0; j < kBM / 64; ++j) {
-                load(sa_hi + j * (BK * 128), &p.a_hi[set], &full_bar[stage], m_blk * kBM + j * 64, k0, am);
-                if (three) load(sa_lo + j * (BK * 128), &p.a_lo[set], &full_bar[stage], m_blk * kBM + j * 64, k0, am);
+                for (int j = 0; j < kBM / 64; ++j) {
+                  tma_load_3d(sa_hi + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am);
+                  if (three) tma_load_3d(sa_lo + j * (BK * 128), &p.a_lo[set], bar, a_row0 + j * 64, k0, am);
+                }
               }
-            }
-            if constexpr (!B_MN) {
-              load(sb_hi, &p.b_hi[set], &full_bar[stage], k0, b_row0, bm);
-              if (three) load(sb_lo, &p.b_lo[set], &full_bar[stage], k0, b_row0, bm);
-            } else {
+              if constexpr (!B_MN) {
+                tma_load_3d(sb_hi, &p.b_hi[set], bar, k0, b_row0, bm);
+                if (three) tma_load_3d(sb_lo, &p.b_lo[set], bar, k0, b_row0, bm);
+              } else {
 #pragma unroll
-              for (int j = 0; j < kBHalf / 64; ++j) {
-                load(sb_hi + j * (BK * 128), &p.b_hi[set], &full_bar[stage], b_row0 + j * 64, k0, bm);
-                if (three) load(sb_lo + j * (BK * 128), &p.b_lo[set], &full_bar[stage], b_row0 + j * 64, k0, bm);
+                for (int j = 0; j < BN / 64; ++j) {
+                  tma_load_3d(sb_hi + j * (BK * 128), &p.b_hi[set], bar, b_row0 + j * 64, k0, bm);
+                  if (three) tma_load_3d(sb_lo + j * (BK * 128), &p.b_lo[set], bar, b_row0 + j * 64, k0, bm);
+                }
               }
-            }
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
+              next();
             }
           }
         }
-        }
       }
     }
-  } else if (warp == 1) {
-    // ======================= MMA issuer =======================
-    if (lane == 0 && cta_rank == 0) {  // in a pair only CTA 0 issues; its MMAs drive both SMs
-      constexpr uint32_t idesc = make_idesc_bf16(CTA2 ? 2 * kBM : kBM, BN, A_MN, B_MN);
-      auto mma = [&](uint32_t d, uint64_t a, uint64_t b, uint32_t acc_flag) {
-        if constexpr (CTA2) umma_bf16_2cta(d, a, b, idesc, acc_flag);
-        else umma_bf16(d, a, b, idesc, acc_flag);
-      };
-      auto mma16 = [&](uint32_t d, uint64_t a, uint64_t b, uint32_t id, uint32_t acc_flag) {
-        if constexpr (CTA2) umma_bf16_2cta(d, a, b, id, acc_flag);
-        else umma_bf16(d, a, b, id, acc_flag);
-      };
-      auto commit = [&](uint64_t* bar) {
-        if constexpr (CTA2) umma_commit_2cta(bar);
-        else umma_commit(bar);
-      };
-      constexpr uint32_t a_lbo = A_MN ? BK * 128 : 16;
-      constexpr uint32_t b_lbo = B_MN ? BK * 128 : 16;
-      constexpr uint32_t a_kstep = A_MN ? 2048 : 32;  // bytes per K=16 slice
-      constexpr uint32_t b_kstep = B_MN ? 2048 : 32;
-      // MN-major tiles always use 128-byte rows; K-major tiles have BK*2-byte rows (128B or 64B swizzle)
-      constexpr uint32_t a_sbo = (A_MN || BK == 64) ? 1024 : 512, a_lt = (A_MN || BK == 64) ? 2 : 4;
-      constexpr uint32_t b_sbo = (B_MN || BK == 64) ? 1024 : 512, b_lt = (B_MN || BK == 64) ? 2 : 4;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        int nsub = NSUB;
-        if constexpr (NSUB == 2) nsub = tile >= big_tiles ? 1 : 2;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + uint32_t(acc * BN);   // (NSUB == 2: one stage, sub-tile s at column s * BN)
-        const uint32_t d_cross = SPLIT_ACC ? tmem_base + uint32_t(BN) : d_tmem;
-        uint32_t accumulate = 0;
-        if constexpr (F8) {
-          constexpr uint32_t i16 = make_idesc_fmt(CTA2 ? 2 * kBM : kBM, BN, A_MN, B_MN, 0, 0);  // f16 x f16
-          constexpr uint32_t i8 = make_idesc_fmt(CTA2 ? 2 * kBM : kBM, BN, A_MN, B_MN, 1, 1);   // e5m2 x e5m2
-          // 8-bit planes: K-major rows are BK bytes (64-byte or 32-byte swizzle); MN-major rows hold 128 elements
-          constexpr uint32_t a8_sbo = A_MN ? 1024 : (BK == 64 ? 512 : 256), a8_lt = A_MN ? 2 : (BK == 64 ? 4 : 6);
-          constexpr uint32_t b8_sbo = B_MN ? 1024 : (BK == 64 ? 512 : 256), b8_lt = B_MN ? 2 : (BK == 64 ? 4 : 6);
-          constexpr uint32_t a8_kstep = A_MN ? 4096 : 32, b8_kstep = B_MN ? 4096 : 32;  // bytes per K = 32 slice
-          const int iters = p.nsets * kblocks;
-          if (three) {
-            for (int set = 0; set < p.nsets; ++set) {
+  } else {
+    // ======================= wgmma consumers + epilogue =======================
+    const int ctid = threadIdx.x - 128;      // 0..255
+    const int wg = ctid >> 7;                // rows 64 wg .. +63 of the tile
+    const int wl = ctid & 127;               // thread within the warpgroup
+    auto consumer_sync = [] { named_sync(1, 256); };
+    // descriptor geometry: K-major rows of BK * 2 bytes (128B swizzle at BK = 64, 64B at BK = 32); MN-major 64-element
+    // rows of 128 B, 64-element blocks BK * 128 B apart
+    constexpr uint32_t a_sw = (A_MN || BK == 64) ? 1 : 2, b_sw = (B_MN || BK == 64) ? 1 : 2;
+    constexpr uint32_t a_lbo = A_MN ? BK * 128 : 16, b_lbo = B_MN ? BK * 128 : 16;
+    constexpr uint32_t a_sbo = (A_MN || BK == 64) ? 1024 : 512, b_sbo = (B_MN || BK == 64) ? 1024 : 512;
+    constexpr uint32_t a_kstep = A_MN ? 2048 : 32, b_kstep = B_MN ? 2048 : 32;   // bytes per K = 16 slice
+    const uint32_t a_wg = A_MN ? uint32_t(wg) * (BK * 128) : uint32_t(wg) * (64 * BK * 2);  // this warpgroup's 64 rows
+    auto adesc = [&](uint32_t tile, int k) { return make_wgmma_desc(tile + a_wg + k * a_kstep, a_lbo, a_sbo, a_sw); };
+    auto bdesc = [&](uint32_t tile, int k) { return make_wgmma_desc(tile + k * b_kstep, b_lbo, b_sbo, b_sw); };
+    constexpr bool F16 = F8;   // f16f8 multiplies fp16 (and widened e5m2) planes; bf16x3 bf16 planes
+
+    float acc[64];
+    float accx[SPLIT_ACC ? 64 : 1];
+    float* acc_stage = reinterpret_cast<float*>(smem + SM::kAccOff);
+    int stage = 0;
+    uint32_t phase = 0;
+    auto next = [&]() {
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    };
+    auto release = [&](int s) {
+      if (wl == 0) mbar_arrive(&empty_bar[s]);
+    };
+
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int model, tile_m, tile_n;
+      decode_tile(tile, model, tile_m, tile_n);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      if constexpr (SPLIT_ACC) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) accx[i] = 0.f;
+      }
+      if constexpr (F8) {
+        uint8_t* wide = smem + SM::kAccOff;   // widened tiles: A.h8, A.l8, B.h8, B.l8 (fp16)
+        const uint32_t wa_h = smem_u32(wide), wa_l = wa_h + SM::kATile, wb_h = wa_l + SM::kATile, wb_l = wb_h + SM::kBTile;
+        if (three) {
+          for (int set = 0; set < p.nsets; ++set) {
             const bool t_lh = term_lh[set], t_hl = term_hl[set];
             if (!t_lh && !t_hl) continue;
             for (int kb = 0; kb < kblocks; ++kb) {
               mbar_wait(&full_bar[stage], phase);
-              tc_fence_after();
-              const uint32_t sa_h = smem_u32(smem + stage * SM::kStage);
-              const uint32_t sa_l = sa_h + SM::kATile / 2;
-              const uint32_t sb_h = sa_h + SM::kATile;
-              const uint32_t sb_l = sb_h + SM::kBTile / 2;
+              consumer_sync();   // both warpgroups are done with the widened tiles (and the previous epilogue)
+              const uint8_t* st = smem + stage * SM::kStage;
+              if (t_hl) widen_tile<A_MN, BK, kBM>(st, wide, ctid);
+              if (t_lh) widen_tile<A_MN, BK, kBM>(st + SM::kATile / 2, wide + SM::kATile, ctid);
+              if (t_lh) widen_tile<B_MN, BK, BN>(st + SM::kATile, wide + 2 * SM::kATile, ctid);
+              if (t_hl) widen_tile<B_MN, BK, BN>(st + SM::kATile + SM::kBTile / 2, wide + 2 * SM::kATile + SM::kBTile, ctid);
+              fence_proxy_async_smem();   // generic-proxy writes -> visible to wgmma
+              consumer_sync();
+              release(stage);
+              next();
+              wgmma_fence();
 #pragma unroll
-              for (int k = 0; k < BK / 32; ++k) {
-                const uint64_t ah = make_sdesc(sa_h + k * a8_kstep, a_lbo, a8_sbo, a8_lt);
-                const uint64_t al = make_sdesc(sa_l + k * a8_kstep, a_lbo, a8_sbo, a8_lt);
-                uint32_t acc_after = accumulate;
-                if constexpr (NSUB == 2 && CTA2) {
-                  if (nsub == 2 && p.a_collector) {
-                    const uint32_t sub8 = uint32_t(SM::kBSub * BK);
-                    const uint64_t bh0 = make_sdesc(sb_h + k * b8_kstep, b_lbo, b8_sbo, b8_lt);
-                    const uint64_t bh1 = make_sdesc(sb_h + sub8 + k * b8_kstep, b_lbo, b8_sbo, b8_lt);
-                    const uint64_t bl0 = make_sdesc(sb_l + k * b8_kstep, b_lbo, b8_sbo, b8_lt);
-                    const uint64_t bl1 = make_sdesc(sb_l + sub8 + k * b8_kstep, b_lbo, b8_sbo, b8_lt);
-                    if (t_lh) {
-                      umma_f8_2cta_coll<1>(d_tmem, al, bh0, i8, accumulate);
-                      umma_f8_2cta_coll<2>(d_tmem + uint32_t(BN), al, bh1, i8, accumulate);
-                    }
-                    if (t_hl) {
-                      const uint32_t a2 = t_lh ? 1u : accumulate;
-                      umma_f8_2cta_coll<1>(d_tmem, ah, bl0, i8, a2);
-                      umma_f8_2cta_coll<2>(d_tmem + uint32_t(BN), ah, bl1, i8, a2);
-                    }
-                    accumulate = 1;
-                    continue;
-                  }
-                }
-                for (int sub = 0; sub < nsub; ++sub) {
-                  const uint32_t sub8 = uint32_t(sub * (SM::kBSub * BK));   // bytes of one sub-tile's 8-bit plane
-                  const uint64_t bh = make_sdesc(sb_h + sub8 + k * b8_kstep, b_lbo, b8_sbo, b8_lt);
-                  const uint64_t bl = make_sdesc(sb_l + sub8 + k * b8_kstep, b_lbo, b8_sbo, b8_lt);
-                  uint32_t acc_s = accumulate;
-                  if (t_lh) {
-                    umma_f8<CTA2>(d_tmem + uint32_t(sub * BN), al, bh, i8, acc_s);
-                    acc_s = 1;
-                  }
-                  if (t_hl) {
-                    umma_f8<CTA2>(d_tmem + uint32_t(sub * BN), ah, bl, i8, acc_s);
-                    acc_s = 1;
-                  }
-                  acc_after = acc_s;
-                }
-                accumulate = acc_after;
+              for (int k = 0; k < BK / 16; ++k) {
+                if (t_lh) wgmma_n128<true, A_MN, B_MN>(acc, adesc(wa_l, k), bdesc(wb_h, k));
+                if (t_hl) wgmma_n128<true, A_MN, B_MN>(acc, adesc(wa_h, k), bdesc(wb_l, k));
               }
-              commit(&empty_bar[stage]);
-              if (++stage == STAGES) {
-                stage = 0;
-                phase ^= 1;
-              }
-            }
+              wgmma_commit();
+              wgmma_wait<0>();
             }
           }
-          bool rescale = accumulate != 0;  // some cross term was accumulated (at 2^kLoShift): rescale with the first hh
-          for (int it = 0; it < iters; ++it) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + stage * SM::kStage);
-            const uint32_t sb = sa + SM::kATile;
+          constexpr float kDown = 1.0f / float(1 << kLoShift);
 #pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t ah = make_sdesc(sa + k * a_kstep, a_lbo, a_sbo, a_lt);
-              if constexpr (NSUB == 2 && CTA2) {
-                if (nsub == 2 && p.a_collector) {
-                  const uint64_t bh0 = make_sdesc(sb + k * b_kstep, b_lbo, b_sbo, b_lt);
-                  const uint64_t bh1 = make_sdesc(sb + uint32_t(SM::kBSub * BK * 2) + k * b_kstep, b_lbo, b_sbo, b_lt);
-                  if (k == 0 && rescale) {
-                    umma_f16_rescale_2cta_coll<1>(d_tmem, ah, bh0, i16);
-                    umma_f16_rescale_2cta_coll<2>(d_tmem + uint32_t(BN), ah, bh1, i16);
-                  } else {
-                    umma_f16_2cta_coll<1>(d_tmem, ah, bh0, i16, accumulate);
-                    umma_f16_2cta_coll<2>(d_tmem + uint32_t(BN), ah, bh1, i16, accumulate);
-                  }
-                  if (k == 0) rescale = false;
-                  accumulate = 1;
-                  continue;
-                }
-              }
-              for (int sub = 0; sub < nsub; ++sub) {
-                const uint64_t bh = make_sdesc(sb + uint32_t(sub * (SM::kBSub * BK * 2)) + k * b_kstep, b_lbo, b_sbo, b_lt);
-                if (k == 0 && rescale) umma_f16_rescale<CTA2>(d_tmem + uint32_t(sub * BN), ah, bh, i16);  // D = ah*bh + D * 2^-kLoShift
-                else mma16(d_tmem + uint32_t(sub * BN), ah, bh, i16, accumulate);
-              }
-              if (k == 0) rescale = false;
-              accumulate = 1;
-            }
-            commit(&empty_bar[stage]);
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
+          for (int i = 0; i < 64; ++i) acc[i] *= kDown;   // exact: the cross terms were accumulated at 2^kLoShift
         }
-        if constexpr (!F8)
         for (int it = 0; it < p.nsets * kblocks; ++it) {
           mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
+          const uint32_t sa = smem_u32(smem + stage * SM::kStage);
+          const uint32_t sb = sa + SM::kATile;
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) wgmma_n128<true, A_MN, B_MN>(acc, adesc(sa, k), bdesc(sb, k));
+          wgmma_commit();
+          wgmma_wait<0>();
+          release(stage);
+          next();
+        }
+      } else {
+        for (int it = 0; it < p.nsets * kblocks; ++it) {
+          mbar_wait(&full_bar[stage], phase);
           const uint32_t sa_hi = smem_u32(smem + stage * SM::kStage);
           const uint32_t sa_lo = sa_hi + SM::kATile;
           const uint32_t sb_hi = sa_lo + SM::kATile;
           const uint32_t sb_lo = sb_hi + SM::kBTile;
+          wgmma_fence();
 #pragma unroll
           for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t ah = make_sdesc(sa_hi + k * a_kstep, a_lbo, a_sbo, a_lt);
-            const uint64_t bh = make_sdesc(sb_hi + k * b_kstep, b_lbo, b_sbo, b_lt);
             if (three) {
-              const uint64_t al = make_sdesc(sa_lo + k * a_kstep, a_lbo, a_sbo, a_lt);
-              const uint64_t bl = make_sdesc(sb_lo + k * b_kstep, b_lbo, b_sbo, b_lt);
               // small cross terms first, then the dominant hi*hi term
-              mma(d_cross, al, bh, accumulate);
-              mma(d_cross, ah, bl, 1);
-              mma(d_tmem, ah, bh, SPLIT_ACC ? accumulate : 1u);
-            } else {
-              mma(d_tmem, ah, bh, accumulate);
+              if constexpr (SPLIT_ACC) {
+                wgmma_n128<F16, A_MN, B_MN>(accx, adesc(sa_lo, k), bdesc(sb_hi, k));
+                wgmma_n128<F16, A_MN, B_MN>(accx, adesc(sa_hi, k), bdesc(sb_lo, k));
+              } else {
+                wgmma_n128<F16, A_MN, B_MN>(acc, adesc(sa_lo, k), bdesc(sb_hi, k));
+                wgmma_n128<F16, A_MN, B_MN>(acc, adesc(sa_hi, k), bdesc(sb_lo, k));
+              }
             }
-            accumulate = 1;
+            wgmma_n128<F16, A_MN, B_MN>(acc, adesc(sa_hi, k), bdesc(sb_hi, k));
           }
-          commit(&empty_bar[stage]);  // smem slot is free (in both CTAs of a pair) once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          release(stage);
+          next();
         }
-        commit(&tfull_bar[acc]);  // accumulator complete -> epilogue (of both CTAs)
-        if (++acc == kAccStages) {
-          acc = 0;
-          acc_phase ^= 1;
+        if constexpr (SPLIT_ACC) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) acc[i] += accx[i];
         }
       }
-    }
-  } else if (warp >= 4) {
-    // ======================= epilogue =======================
-    const int wq = warp & 3;
-    const int grp = (warp - 4) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-      TileCoord tc;
-      int tile_m, n0, nsub;
-      decode_tile(tile, tc.model, tile_m, n0, nsub);
-      tc.m_blk = tile_m * (CTA2 ? 2 : 1) + cta_rank;
-      tc.row = tc.m_blk * kBM + wq * 32 + lane;
-      tc.warp_q = wq;
-      tc.grp = grp;
-      tc.lane = lane;
 
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int sub = 0; sub < nsub; ++sub) {
-      tc.n_blk = n0 + sub;   // in units of BN columns
-      tc.col0 = tc.n_blk * BN;
-      Epi epi(p.epi, tc, p.m_total, p.n_total, smem + SM::kEpiOff + (grp * 4 + wq) * Epi::kWarpStageBytes);
-      const uint32_t taddr = tmem_base + uint32_t((acc * NSUB + sub) * BN) + (uint32_t(wq * 32) << 16);
+      // ---- accumulators -> padded fp32 tile (row-per-thread view for the epilogue)
+      consumer_sync();   // the previous tile's epilogue / the widened tiles are no longer read
+      {
+        const int w = wl >> 5, l = wl & 31;
+        const int r0 = wg * 64 + w * 16 + (l >> 2);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int row = r0 + 8 * ((i >> 1) & 1);
+          const int col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+          acc_stage[row * SM::kAccLd + col] = acc[i];
+        }
+      }
+      consumer_sync();
+
+      // ======================= epilogue =======================
+      const int cw = ctid >> 5;   // epilogue warp 0..7
+      TileCoord tc;
+      tc.model = model;
+      tc.m_blk = tile_m;
+      tc.n_blk = tile_n;
+      tc.col0 = tile_n * BN;
+      tc.warp_q = cw & 3;
+      tc.grp = cw >> 2;
+      tc.lane = lane;
+      tc.row = tc.m_blk * kBM + tc.warp_q * 32 + lane;
+      Epi epi(p.epi, tc, p.m_total, p.n_total, smem + SM::kEpiOff + (tc.grp * 4 + tc.warp_q) * Epi::kWarpStageBytes);
+      const float* my_row = acc_stage + (tc.warp_q * 32 + lane) * SM::kAccLd;
       constexpr int kChunks = BN / EC;
       static_assert(kChunks % 2 == 0, "the two epilogue warp groups alternate chunks");
       // chunk order of an epilogue warp group: alternating chunks (grp, grp + 2, ...) or, for epilogues that stage two
@@ -565,48 +459,14 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       static_assert(!kPairs || (EC == 32 && kChunks % 4 == 0), "paired chunks: 32-column chunks, whole pairs per group");
 #pragma unroll 1
       for (int it = 0; it < kChunks / 2; ++it) {
-        const int c = kPairs ? ((it >> 1) * 4 + 2 * grp + (it & 1)) : (grp + 2 * it);
+        const int c = kPairs ? ((it >> 1) * 4 + 2 * tc.grp + (it & 1)) : (tc.grp + 2 * it);
         uint32_t r[EC];
-        tmem_ld32(taddr + uint32_t(c * EC), *reinterpret_cast<uint32_t(*)[32]>(&r[0]));
-        if constexpr (EC == 64) tmem_ld32(taddr + uint32_t(c * EC + 32), *reinterpret_cast<uint32_t(*)[32]>(&r[32]));
-        if constexpr (SPLIT_ACC) {
-          static_assert(!SPLIT_ACC || EC == 32, "split accumulators are read in 32-column chunks");
-          if (three) {
-            uint32_t x[32];
-            tmem_ld32(taddr + uint32_t(BN + c * EC), x);
-            tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(x[i]));
-          }
-        }
-        tmem_ld_wait();
-        if (it == kChunks / 2 - 1 && sub == nsub - 1) {
-          // all TMEM reads of this accumulator are done: hand it back to the MMA warp early
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (CTA2) mbar_arrive_cta0(&tempty_bar[acc]);
-            else mbar_arrive(&tempty_bar[acc]);
-          }
-        }
+        for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(my_row[c * EC + j]);
         epi.chunk(c * EC, r);
       }
       epi.finish();
-      }
-      if (++acc == kAccStages) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CTA2) cluster_sync_all();  // neither CTA may free TMEM / exit while the pair's MMAs or signals are in flight
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (CTA2) tmem_dealloc_2cta(tmem_base, kTmemCols);
-    else tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 

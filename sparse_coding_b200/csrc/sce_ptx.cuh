@@ -1,8 +1,8 @@
-// sce_ptx.cuh — thin inline-PTX wrappers for the sm_100a features the engine uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the
-// shared-memory + instruction descriptors that tcgen05.mma consumes.
+// sce_ptx.cuh — thin inline-PTX wrappers for the sm_90a features the engine uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared memory, accumulators in
+// registers) and the shared-memory matrix descriptors wgmma consumes.
 //
-// Nothing here is specific to sparse autoencoders; sce_gemm.cuh builds the split-bf16
+// Nothing here is specific to sparse autoencoders; sce_gemm.cuh builds the split-operand
 // batched GEMM on top of it.
 #pragma once
 #include <cstdint>
@@ -21,18 +21,9 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 %%rx;\n\t"
-      ".reg .pred %%px;\n\t"
-      "elect.sync %%rx|%%px, %1;\n\t"
-      "@%%px mov.s32 %0, 1;\n\t"
-      "}\n"
-      : "+r"(pred)
-      : "r"(0xffffffffu));
-  return pred != 0;
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -104,264 +95,80 @@ __device__ __forceinline__ void tma_store_wait_read() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: tensor memory allocation
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------------------------
-// tcgen05.mma (kind::f16: bf16 x bf16 -> fp32 in TMEM), single-CTA
-// ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed.
-// (Implies tcgen05.fence::before_thread_sync.)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulation.
-// Bit layout (PTX ISA "Instruction descriptor", kind::f16): [4,6) D format (1 = f32),
-// [7,10) A format (1 = bf16), [10,13) B format, 15 A major (0 = K, 1 = MN), 16 B major,
-// [17,23) N>>3, [24,29) M>>4.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(a_mn) << 15) | (uint32_t(b_mn) << 16) |
-         (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle. Fields (PTX ISA "Matrix descriptor"):
+// wgmma shared-memory matrix descriptor (sm_90). Fields (PTX ISA "Matrix Descriptor Format"):
 // [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4,
-// [46,48) version (1 on sm_100), [61,64) swizzle mode (2 = 128B).
+// [62,64) swizzle mode (1 = 128B, 2 = 64B, 3 = 32B). Tiles are 1024-byte aligned, so the base offset is 0.
 //
-//  * K-major operand (reduction index contiguous): rows are 128 B (64 bf16) apart, 8-row groups
-//    are SBO = 1024 B apart, LBO unused. A K=16 slice is 32 B inside the 128-B row; advance the
-//    start address by 32 B per slice (the hardware applies the XOR swizzle to the final address).
-//  * MN-major operand (non-reduction index contiguous): one "row" of 128 B holds 64 consecutive
-//    M (or N) elements of ONE k; 8 consecutive k make a 1024-B group; the next 8 k are SBO bytes
-//    further; the next 64 M/N elements are LBO bytes further.
-//
-// K-major operands may also use the 64-byte swizzle (layout type 4): rows are 64 B (32 bf16) apart, 8-row
-// groups SBO = 512 B apart; this halves the K extent of a pipeline stage (BK = 32) so that twice as many
-// stages fit in shared memory.
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                               uint32_t layout_type) {
+//  * K-major operand (reduction index contiguous): rows of 128 B (128B swizzle, 64 16-bit elements) or 64 B
+//    (64B swizzle, 32 elements); 8-row groups are SBO = 1024 / 512 B apart; LBO unused. A K=16 slice is 32 B
+//    inside the row: advance the start address by 32 B per slice (the hardware applies the XOR swizzle).
+//  * MN-major operand (row/column index contiguous, 128B swizzle): one 128-B row holds 64 consecutive M (or N)
+//    elements of ONE k; 8 consecutive k make a 1024-B group, the next 8 k are SBO bytes further; the next 64 M/N
+//    elements are LBO bytes further. A K=16 slice is two groups: 2048 B.
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+                                                    uint32_t swizzle_mode) {
   uint64_t d = 0;
   d |= uint64_t((smem_addr & 0x3FFFFu) >> 4);
   d |= uint64_t((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= uint64_t(1) << 46;
-  d |= uint64_t(layout_type) << 61;
+  d |= uint64_t(swizzle_mode) << 62;
   return d;
 }
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                     uint32_t sbo_bytes) {
-  return make_sdesc(smem_addr, lbo_bytes, sbo_bytes, 2);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05.ld: 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread.
-// Warp w of a CTA may only touch TMEM lanes [32*(w%4), 32*(w%4)+32).
+// wgmma m64n128k16, fp32 accumulators in registers: d += A(64 x 16) * B(16 x 128).
+// F16: operands are fp16 (else bf16). TA / TB: operand is MN-major (transposed) in shared memory.
+// Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[i] is row
+// 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+#define SCE_WGMMA_N128(TYPE)                                                                                         \
+  asm volatile(                                                                                                      \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                                               \
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." TYPE "." TYPE " "                                               \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "   \
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "    \
+      "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "        \
+      "%64, %65, p, 1, 1, %66, %67;\n\t}\n"                                                                          \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),              \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),        \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),      \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),      \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),      \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),      \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),      \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])       \
+      : "l"(adesc), "l"(bdesc), "n"(int(TA)), "n"(int(TB)))
 
-// ----------------------------------------------------------------------------------------------
-// CTA pairs (cta_group::2): two CTAs of a 2-cluster share one 256-row MMA tile. Each loads its own half
-// of A (128 rows) and half of B (N/2 rows); only CTA 0 issues tcgen05.mma; TMA completions of both CTAs
-// land on CTA 0's mbarrier (shared::cluster address with the CTA-rank bit 24 cleared); tcgen05.commit
-// multicasts its arrival to the same barrier offset in both CTAs.
-// ----------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+template <bool F16, bool TA, bool TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (F16) SCE_WGMMA_N128("f16");
+  else SCE_WGMMA_N128("bf16");
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2cta(void* smem_dst, const CUtensorMap* m, uint64_t* bar_cta0,
-                                                 int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes "
-      "[%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar_cta0) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cta0(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(uint16_t(3))
-      : "memory");
-}
+#undef SCE_WGMMA_N128
 
 // ----------------------------------------------------------------------------------------------
 // fp16 + fp8 arithmetic ("f16f8"): x ~= h + l with h = fp16(x) (11 significant bits) and l = x - h, |l| <= 2^-11 |x|.
-// The product a*b = ah*bh + (al*bh + ah*bl) + O(2^-22): the dominant term runs as kind::f16 on the fp16 planes,
-// the two cross terms need only ~3 significant bits and run as kind::f8f6f4 (E5M2 x E5M2, K = 32 per
-// instruction, twice the rate) on 8-bit planes: h8 = e5m2(x) and l8 = e5m2(l * 2^kLoShift). The cross terms are
-// accumulated FIRST (they carry the factor 2^kLoShift) and the first hh instruction of the tile rescales the
-// accumulator with tcgen05.mma's scale-input-d: D = A*B + D * 2^-kLoShift. Cost: 1 + 2 * 1/2 = 2 pass
-// equivalents instead of the 3 of the bf16 split, one accumulator.
+// The product a*b = ah*bh + (al*bh + ah*bl) + O(2^-22): the dominant term is formed on the fp16 planes, the two cross
+// terms need only ~3 significant bits and are carried as 8-bit E5M2 planes: h8 = e5m2(x) and l8 = e5m2(l * 2^kLoShift)
+// (1 byte / element in HBM: 4 bytes per operand element in all). The cross terms are accumulated FIRST (they carry the
+// factor 2^kLoShift), the accumulator is then scaled by 2^-kLoShift (exact) and the hh products are added.
+// An E5M2 byte is the high byte of the fp16 with the same value, so the GEMM widens the 8-bit tiles to fp16 in shared
+// memory (exactly) and forms the cross terms with fp16 wgmma, which, unlike the fp8 form, accepts MN-major operands.
 // ----------------------------------------------------------------------------------------------
 constexpr int kLoShift = 11;  // |l| * 2^11 <= |x|: the scaled residual has the range of x itself (fits E5M2 when x fits fp16)
 
-// Instruction descriptor with explicit operand formats. kind::f16: 0 = f16, 1 = bf16. kind::f8f6f4: 0 = e4m3, 1 = e5m2.
-__host__ __device__ constexpr uint32_t make_idesc_fmt(int M, int N, bool a_mn, bool b_mn, uint32_t afmt, uint32_t bfmt) {
-  return (1u << 4) | (afmt << 7) | (bfmt << 10) | (uint32_t(a_mn) << 15) | (uint32_t(b_mn) << 16) |
-         (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-
-template <bool CTA2>
-__device__ __forceinline__ void umma_f8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (CTA2) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
-  } else {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-                 : "memory");
-  }
-}
-// D = A*B + D * 2^-kLoShift (kind::f16 only; the scale is an immediate)
-template <bool CTA2>
-__device__ __forceinline__ void umma_f16_rescale(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  if constexpr (CTA2) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p, %4;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "n"(kLoShift)
-                 : "memory");
-  } else {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p, %4;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "n"(kLoShift)
-                 : "memory");
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// A-operand collector (tcgen05.mma ... .collector::a::fill / ::lastuse): two consecutive MMAs that multiply the SAME
-// A slice by different B sub-tiles (the 256 x 512 output tiles, NSUB = 2) read A from shared memory once — the first
-// keeps it in the tensor core's collector buffer (SASS: A_KEEP), the second takes it from there (A_REUSE). With 4-byte
-// operand planes the main loop otherwise needs more than the SM's 128 B/clk of shared-memory bandwidth.
-// COLL: 0 = default (discard), 1 = fill, 2 = lastuse. CTA pairs only (the only place NSUB = 2 is used).
-// ----------------------------------------------------------------------------------------------
-template <int COLL>
-__device__ __forceinline__ void umma_f8_2cta_coll(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (COLL == 1) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f8f6f4.collector::a::fill [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-  } else if constexpr (COLL == 2) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f8f6f4.collector::a::lastuse [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-  } else {
-    umma_f8<true>(tmem_d, adesc, bdesc, idesc, accumulate);
-  }
-}
-template <int COLL>
-__device__ __forceinline__ void umma_f16_2cta_coll(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (COLL == 1) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-  } else if constexpr (COLL == 2) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-  } else {
-    umma_bf16_2cta(tmem_d, adesc, bdesc, idesc, accumulate);
-  }
-}
-// D = A*B + D * 2^-kLoShift with the collector qualifier
-template <int COLL>
-__device__ __forceinline__ void umma_f16_rescale_2cta_coll(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc) {
-  if constexpr (COLL == 1) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16.collector::a::fill [%0], %1, %2, %3, p, %4;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "n"(kLoShift) : "memory");
-  } else if constexpr (COLL == 2) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-                 "tcgen05.mma.cta_group::2.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p, %4;\n\t}\n" ::"r"(tmem_d),
-                 "l"(adesc), "l"(bdesc), "r"(idesc), "n"(kLoShift) : "memory");
-  } else {
-    umma_f16_rescale<true>(tmem_d, adesc, bdesc, idesc);
-  }
+// four e5m2 bytes -> four fp16 (two packed words): byte b becomes the fp16 with bits b << 8
+__device__ __forceinline__ void widen_e5m2x4(uint32_t w, uint32_t& lo, uint32_t& hi) {
+  lo = __byte_perm(w, 0u, 0x1404);
+  hi = __byte_perm(w, 0u, 0x3424);
 }
 
 // ----------------------------------------------------------------------------------------------

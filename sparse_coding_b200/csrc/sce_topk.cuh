@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(256) topk_select2_kernel(const float* __restri
   };
   if (ncand <= kTopkCand) {
     // ---- 4. exact ranks by counting: rank = candidates above this one; rank < k <=> selected, and rank is its slot.
-    // The ncand^2 comparisons are the bulk of this kernel's instructions (ncu source view, profiles/r02p_*): one 64-bit
+    // The ncand^2 comparisons are the bulk of this kernel's instructions: one 64-bit
     // broadcast load and compare per pair, and every candidate's count is split over `parts` threads so that all 256
     // threads count (typically ncand = 2-3 k < 256).
     const int parts = ncand >= kTopkCand ? 1 : min(8, (kTopkCand + ncand - 1) / max(ncand, 1));
@@ -456,7 +456,7 @@ __global__ void __launch_bounds__(256) topk_sparse_kernel(TopkLists lists, const
   // dependent global load before the copies are in flight, not two), values and the x row are fetched alongside
   // (warp per entry: ONE column load and one base address per dictionary row, lanes stride its 16-byte pieces — the first
   //  version spread the pieces over all threads and paid an integer division, 64-bit address arithmetic and a dependent
-  //  column load per PIECE: 43 % of the kernel's instructions, ncu source view of profiles/r02f_topk_full)
+  //  column load per PIECE)
   {
     const float* wn_slice = wn + (long long)model * n * d + (long long)slice * ds;
     const int* cols = lists.col + lrow * kmax;

@@ -8,7 +8,7 @@ by Python and are updated in place, so ``unstack``/export/IPC keep working.
 
 What differs is *how* a step is computed. The reference builds ``vmap(grad(sig.loss))`` + ``vmap(torchopt.adam)``
 out of ~70 stock PyTorch launches that stream the fp32 code tensor [M, B, n] through HBM a dozen times. Here
-``step_batch`` is one call into libsce.so (include/sce.h): four tcgen05 split-operand GEMMs with fused epilogues plus a
+``step_batch`` is one call into libsce.so (include/sce.h): four wgmma split-operand GEMMs with fused epilogues plus a
 handful of streaming kernels; the code tensor exists only as operand planes (4 bytes per element) consumed by the next GEMM.
 ``aux["c"]`` is therefore a lazy :class:`CodeProxy` — ``aux["c"].count_nonzero(dim=-1).float().mean(dim=-1)``
 (the only use in the reference loop, big_sweep.py:171) is answered from fused counters, and ``.dense()``
@@ -196,7 +196,7 @@ class FunctionalEnsemble:
             raise NotImplementedError(
                 f"{getattr(self.sig, '__name__', self.sig)} has no engine variant: only the signatures of the sweep hot "
                 "path (FunctionalTiedSAE, FunctionalSAE, the Masked variants, TopKEncoder) are implemented in the "
-                "sm_100a engine, and there is deliberately no generic autograd fallback")
+                "sm_90a engine, and there is deliberately no generic autograd fallback")
         self._variant = variant
         self._plan = None
         self._plan_key = None
@@ -218,7 +218,7 @@ class FunctionalEnsemble:
     def _require_cuda(self):
         dev = torch.device(self.device)
         if dev.type != "cuda":
-            raise RuntimeError(f"FunctionalEnsemble computes in the sm_100a CUDA engine; device is {dev}. "
+            raise RuntimeError(f"FunctionalEnsemble computes in the sm_90a CUDA engine; device is {dev}. "
                                "Move it with to_device('cuda:…') — there is no CPU implementation.")
         return dev
 

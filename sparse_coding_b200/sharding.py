@@ -2,7 +2,7 @@
 
 The reference already parallelises this way (cluster_runs.py:110-130: one OS process per ensemble/GPU, zero
 communication; big_sweep_experiments.py:265-291 builds 8 GPUs x 16 L1 values): models of an ensemble never
-exchange anything, so there is no gradient traffic at all. What this module adds is the launch model the B200 box
+exchange anything, so there is no gradient traffic at all. What this module adds is the launch model a multi-GPU box
 uses (torchrun / torch.distributed, rank = GPU) and the only exchange the path has:
 
   * ``shard_slices`` / ``shard_models``: contiguous, balanced split of M_total models over the ranks;

@@ -35,7 +35,7 @@ def engine_loss(sig, params, buffers, batch):
 
     if not batch.is_cuda:
         raise RuntimeError(
-            f"{sig.__name__}.loss runs in the sm_100a CUDA engine and needs CUDA tensors (got {batch.device}); "
+            f"{sig.__name__}.loss runs in the sm_90a CUDA engine and needs CUDA tensors (got {batch.device}); "
             "there is no CPU implementation in the product path")
     dev = batch.device
     model = ({k: v.detach().to(dev) for k, v in params.items()}, {k: v.detach().to(dev) for k, v in buffers.items()})

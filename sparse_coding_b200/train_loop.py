@@ -6,7 +6,7 @@ Reference behaviour being reproduced (HoagyC/sparse_coding @ 69c5ae0):
   make_hyperparam_name          big_sweep.py:75-83     wandb key format
   chunk loop / checkpoints      big_sweep.py:349-384, basic_l1_sweep.py:85-115
 
-What is B200-native here: the reference gathers every batch on the CPU (``dataset[batch_idxs]``, a 16 MiB fancy-index
+What is GPU-native here: the reference gathers every batch on the CPU (``dataset[batch_idxs]``, a 16 MiB fancy-index
 copy per step at config 2) and ships it through a pageable, synchronous H2D copy (its ``pin_memory()`` call discards
 the result, SURVEY.md Q5). Here the whole chunk (2 GiB as fp16) is made resident in HBM once — staged through pinned
 memory on a side stream while the previous chunk is still training — and each batch is a device-side row gather

@@ -1,7 +1,7 @@
 """Informational comparator (not a test, not the product): the restated reference step — stock PyTorch ops under
-vmap(grad(loss)) + Adam, i.e. what HoagyC/sparse_coding would launch on a GPU — timed ON THE B200 at BASELINE
+vmap(grad(loss)) + Adam, i.e. what HoagyC/sparse_coding would launch on a GPU — timed on the GPU at BASELINE
 config 2, in true fp32 (the reference never enables TF32) and with TF32 allowed. Lives under tests/ because it
-drives the oracle.   python tests/bench_stock_torch.py > profiles/rNN_stock_torch_gpu.json"""
+drives the oracle.   python tests/bench_stock_torch.py"""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -1,6 +1,7 @@
-// gemm_selftest.cu — standalone check of the tcgen05 split-bf16 GEMM core (sce_gemm.cuh) against
-// a double-precision CPU product, for every operand-major / tile / pass configuration the engine
-// instantiates. Build: see Makefile target `selftest`. Runs on one B200; exits non-zero on failure.
+// gemm_selftest.cu — standalone check of the wgmma split-operand GEMM core (sce_gemm.cuh) against
+// a double-precision CPU product, for every operand-major / K-block / pass configuration the engine
+// instantiates. Build: see Makefile target `selftest` (build() makes it). Runs on one H100 and exits non-zero on
+// failure; tests/test_engine_gpu.py::test_gemm_selftest runs the default case list, `--big` / `--f8big` are manual.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -94,7 +95,7 @@ static bool tmaps(const Operand& o, uint32_t box_rows_kmajor, int BK, CUtensorMa
          make_tmap_bf16(lo, o.s.d_lo, o.models, o.K, o.rows, o.rows, (uint64_t)o.rows * o.K, BK);
 }
 
-template <int BN, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT = false, bool CTA2 = false>
+template <int BK, bool A_MN, bool B_MN, bool SPLIT = false>
 static bool run_case(const char* name, int models, int M, int N, int K, int nsets, int passes,
                      bool a_shared, bool b_shared, int reps = 1) {
   Operand A[2], B[2];
@@ -111,7 +112,7 @@ static bool run_case(const char* name, int models, int M, int N, int K, int nset
   memset(&p, 0, sizeof(p));
   for (int s = 0; s < nsets; ++s) {
     if (!tmaps(A[s], kBM, BK, &p.a_hi[s], &p.a_lo[s]) ||
-        !tmaps(B[s], CTA2 ? BN / 2 : BN, BK, &p.b_hi[s], &p.b_lo[s])) {
+        !tmaps(B[s], kBN, BK, &p.b_hi[s], &p.b_lo[s])) {
       printf("[%s] tensor map encode failed\n", name);
       return false;
     }
@@ -124,39 +125,27 @@ static bool run_case(const char* name, int models, int M, int N, int K, int nset
   p.n_models = models;
   p.m_total = M;
   p.n_total = N;
-  const int tile_rows = CTA2 ? 2 * kBM : kBM;
-  p.tiles_m = (M + tile_rows - 1) / tile_rows;
-  p.tiles_n = (N + BN - 1) / BN;
+  p.tiles_m = (M + kBM - 1) / kBM;
+  p.tiles_n = (N + kBN - 1) / kBN;
   p.epi.out = d_out;
   p.epi.model_stride = (long long)M * N;
   p.epi.ld = N;
 
-  using SM = GemmSmem<BN, BK, A_MN, B_MN, STAGES, 0, CTA2>;
-  auto kern = gemm_split_kernel<EpiStoreF32, BN, BK, A_MN, B_MN, STAGES, SPLIT, CTA2>;
+  constexpr int STAGES = gemm_stages<BK, 0, kArithBf16x3>();
+  using SM = GemmSmem<BK, STAGES, 0, kArithBf16x3>;
+  auto kern = gemm_split_kernel<EpiStoreF32, BK, A_MN, B_MN, STAGES, SPLIT>;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes));
   int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   int tiles = models * p.tiles_m * p.tiles_n;
-  const int units = CTA2 ? sms / 2 : sms;
-  int grid = (tiles < units ? tiles : units) * (CTA2 ? 2 : 1);
+  int grid = tiles < sms ? tiles : sms;
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
   for (int rep = 0; rep < reps + (reps > 1 ? 2 : 0); ++rep) {
     if (rep == (reps > 1 ? 2 : 0)) CK(cudaEventRecord(e0));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = SM::kBytes;
-    cfg.stream = 0;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CTA2 ? 2 : 1;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    CK(cudaLaunchKernelEx(&cfg, kern, p));
+    kern<<<grid, kGemmThreads, SM::kBytes>>>(p);
+    CK(cudaGetLastError());
   }
   CK(cudaEventRecord(e1));
   cudaError_t err = cudaDeviceSynchronize();
@@ -279,24 +268,24 @@ static void make_operand_f8(OperandF8& o, int models, int rows, int K, bool mn, 
   CK(cudaMemcpy(o.d_h8, o.h8.data(), n, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(o.d_l8, o.l8.data(), n, cudaMemcpyHostToDevice));
 }
+// 16-bit plane: 128-byte swizzle (K block 64); 8-bit planes unswizzled (the GEMM widens them to fp16)
 static bool tmaps_f8(const OperandF8& o, uint32_t box_rows_kmajor, int BK, CUtensorMap* h, CUtensorMap* h8, CUtensorMap* l8) {
   const uint64_t mp = (uint64_t)(o.mn ? o.K : o.rows) * o.pitch;
+  const CUtensorMapSwizzle sw8 = CU_TENSOR_MAP_SWIZZLE_NONE;
   if (!o.mn) {
-    const CUtensorMapSwizzle sw16 = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-    const CUtensorMapSwizzle sw8 = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-    return make_tmap_bf16_box(h, o.d_h, o.models, o.rows, o.K, o.pitch, mp, BK, box_rows_kmajor, sw16) &&
+    return make_tmap_bf16_box(h, o.d_h, o.models, o.rows, o.K, o.pitch, mp, BK, box_rows_kmajor, CU_TENSOR_MAP_SWIZZLE_128B) &&
            make_tmap_u8_box(h8, o.d_h8, o.models, o.rows, o.K, o.pitch, mp, BK, box_rows_kmajor, sw8) &&
            make_tmap_u8_box(l8, o.d_l8, o.models, o.rows, o.K, o.pitch, mp, BK, box_rows_kmajor, sw8);
   }
   return make_tmap_bf16(h, o.d_h, o.models, o.K, o.rows, o.pitch, mp, BK) &&
-         make_tmap_u8_box(h8, o.d_h8, o.models, o.K, o.rows, o.pitch, mp, 128, BK, CU_TENSOR_MAP_SWIZZLE_128B) &&
-         make_tmap_u8_box(l8, o.d_l8, o.models, o.K, o.rows, o.pitch, mp, 128, BK, CU_TENSOR_MAP_SWIZZLE_128B);
+         make_tmap_u8_box(h8, o.d_h8, o.models, o.K, o.rows, o.pitch, mp, 128, BK, sw8) &&
+         make_tmap_u8_box(l8, o.d_l8, o.models, o.K, o.rows, o.pitch, mp, 128, BK, sw8);
 }
 
-template <int BN, int BK, bool A_MN, bool B_MN, int STAGES, bool CTA2, int NSUB = 1>
+template <bool A_MN, bool B_MN>
 static bool run_case_f8(const char* name, int models, int M, int N, int K, int nsets, int passes, bool a_shared,
-                        bool b_shared, int reps = 1, int exact = 0 /*1: A of set 0, 2: B of set 0 is fp16-exact + flagged*/,
-                        int tail_rows = 0 /*NSUB == 2: trailing row blocks run as single-width tiles*/) {
+                        bool b_shared, int reps = 1, int exact = 0 /*1: A of set 0, 2: B of set 0 is fp16-exact + flagged*/) {
+  constexpr int BK = 64;
   OperandF8 A[2], B[2];
   for (int s = 0; s < nsets; ++s) {
     make_operand_f8(A[s], a_shared ? 1 : models, M, K, A_MN, 3.0f, s == 0 && exact == 1);
@@ -313,41 +302,34 @@ static bool run_case_f8(const char* name, int models, int M, int N, int K, int n
   memset(&p, 0, sizeof(p));
   for (int s = 0; s < nsets; ++s) {
     if (!tmaps_f8(A[s], kBM, BK, &p.a_hi[s], &p.a_lo[s], &p.a_x8[s]) ||
-        !tmaps_f8(B[s], CTA2 ? BN / 2 : BN, BK, &p.b_hi[s], &p.b_lo[s], &p.b_x8[s])) {
+        !tmaps_f8(B[s], kBN, BK, &p.b_hi[s], &p.b_lo[s], &p.b_x8[s])) {
       printf("[%s] tensor map encode failed\n", name);
       return false;
     }
     p.a_batched[s] = a_shared ? 0 : 1;
     p.b_batched[s] = b_shared ? 0 : 1;
   }
-  if (NSUB == 2 && tail_rows > 0) p.tail_rows = tail_rows;   // (requires N <= 2 * BN; see GemmParams::tail_rows)
   if (exact == 1) p.a_res_flag[0] = d_flag;
   if (exact == 2) p.b_res_flag[0] = d_flag;
   p.nsets = nsets; p.k_total = K; p.passes = passes; p.n_models = models; p.m_total = M; p.n_total = N;
-  const int tile_rows = CTA2 ? 2 * kBM : kBM;
-  p.tiles_m = (M + tile_rows - 1) / tile_rows;
-  p.tiles_n = (N + NSUB * BN - 1) / (NSUB * BN);
+  p.tiles_m = (M + kBM - 1) / kBM;
+  p.tiles_n = (N + kBN - 1) / kBN;
   p.epi.out = d_out; p.epi.model_stride = (long long)M * N; p.epi.ld = N;
-  using SM = GemmSmem<BN, BK, A_MN, B_MN, STAGES, 0, CTA2, kArithF16F8, NSUB>;
-  auto kern = gemm_split_kernel<EpiStoreF32, BN, BK, A_MN, B_MN, STAGES, false, CTA2, kArithF16F8, NSUB>;
+  constexpr int STAGES = gemm_stages<BK, 0, kArithF16F8>();
+  using SM = GemmSmem<BK, STAGES, 0, kArithF16F8>;
+  auto kern = gemm_split_kernel<EpiStoreF32, BK, A_MN, B_MN, STAGES, false, kArithF16F8>;
   CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes));
   int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
-  int tiles = models * p.tiles_m * p.tiles_n + p.tail_rows;
-  const int units = CTA2 ? sms / 2 : sms;
-  int grid = (tiles < units ? tiles : units) * (CTA2 ? 2 : 1);
+  int tiles = models * p.tiles_m * p.tiles_n;
+  int grid = tiles < sms ? tiles : sms;
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
   float ms = 0;
   for (int rep = 0; rep < reps + (reps > 1 ? 2 : 0); ++rep) {
     if (rep == (reps > 1 ? 2 : 0)) CK(cudaEventRecord(e0));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = SM::kBytes; cfg.stream = 0;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CTA2 ? 2 : 1; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    CK(cudaLaunchKernelEx(&cfg, kern, p));
+    kern<<<grid, kGemmThreads, SM::kBytes>>>(p);
+    CK(cudaGetLastError());
   }
   CK(cudaEventRecord(e1));
   cudaError_t err = cudaDeviceSynchronize();
@@ -422,53 +404,34 @@ int main(int argc, char** argv) {
          prop.multiProcessorCount);
   bool ok = true;
   if (f8only || f8big || argc == 1) {
-    // ---- f16f8 arithmetic: each operand-major combination the engine uses, single CTA then CTA pairs
+    // ---- f16f8 arithmetic: each operand-major combination the engine uses
     if (!f8big) {
-    ok &= run_case_f8<256, 64, false, false, 4, false>("f8_kk_hh", 1, 128, 256, 64, 1, 1, false, false);
-    ok &= run_case_f8<256, 64, false, false, 4, false>("f8_kk_k64", 1, 128, 256, 64, 1, 3, false, false);
-    ok &= run_case_f8<256, 64, false, false, 4, false>("f8_kk_multi", 3, 384, 512, 512, 1, 3, true, false);
-    ok &= run_case_f8<256, 32, false, false, 6, false>("f8_kk32_multi", 3, 384, 512, 512, 1, 3, true, false);
-    ok &= run_case_f8<256, 64, false, true, 4, false>("f8_kmn_k64", 1, 128, 256, 64, 1, 3, false, false);
-    ok &= run_case_f8<256, 64, false, true, 4, false>("f8_kmn_multi", 2, 256, 512, 512, 1, 3, false, false);
-    ok &= run_case_f8<256, 64, true, true, 4, false>("f8_mnmn_k64", 1, 128, 256, 64, 1, 3, false, false);
-    ok &= run_case_f8<256, 64, true, true, 4, false>("f8_mnmn_2set", 2, 256, 512, 320, 2, 3, false, true);
-    ok &= run_case_f8<256, 64, false, false, 6, true>("f8_pair_kk_multi", 3, 768, 512, 512, 1, 3, true, false);
-    ok &= run_case_f8<256, 64, false, false, 6, true>("f8_pair_kk_ragged", 2, 200, 328, 104, 1, 3, true, false);
-    ok &= run_case_f8<256, 64, false, true, 6, true>("f8_pair_kmn", 2, 512, 512, 512, 1, 3, false, false);
-    ok &= run_case_f8<256, 64, false, true, 6, true>("f8_pair_kmn_ragged", 2, 200, 328, 104, 1, 3, false, false);
-    ok &= run_case_f8<256, 64, true, true, 6, true>("f8_pair_mnmn_2set", 2, 512, 512, 320, 2, 3, false, true);
-    ok &= run_case_f8<256, 64, true, true, 6, true>("f8_pair_mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true);
-    ok &= run_case_f8<256, 32, true, true, 8, true>("f8_pair_mnmn32", 2, 512, 512, 320, 2, 3, false, true);
+    ok &= run_case_f8<false, false>("f8_kk_hh", 1, 128, 256, 64, 1, 1, false, false);
+    ok &= run_case_f8<false, false>("f8_kk_k64", 1, 128, 256, 64, 1, 3, false, false);
+    ok &= run_case_f8<false, false>("f8_kk_multi", 3, 384, 512, 512, 1, 3, true, false);
+    ok &= run_case_f8<false, true>("f8_kmn_k64", 1, 128, 256, 64, 1, 3, false, false);
+    ok &= run_case_f8<false, true>("f8_kmn_multi", 2, 256, 512, 512, 1, 3, false, false);
+    ok &= run_case_f8<true, true>("f8_mnmn_k64", 1, 128, 256, 64, 1, 3, false, false);
+    ok &= run_case_f8<true, true>("f8_mnmn_2set", 2, 256, 512, 320, 2, 3, false, true);
+    ok &= run_case_f8<false, false>("f8_kk_ragged", 2, 200, 328, 104, 1, 3, true, false);
+    ok &= run_case_f8<false, true>("f8_kmn", 2, 512, 512, 512, 1, 3, false, false);
+    ok &= run_case_f8<false, true>("f8_kmn_ragged", 2, 200, 328, 104, 1, 3, false, false);
+    ok &= run_case_f8<true, true>("f8_mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true);
     // fp16-exact operand flagged "no residual plane": the cross term and the loads of its planes are skipped
-    ok &= run_case_f8<256, 64, false, false, 6, true>("f8_pair_kk_exactA", 3, 768, 512, 512, 1, 3, true, false, 1, 1);
-    ok &= run_case_f8<256, 64, false, false, 4, false>("f8_kk_exactA", 2, 200, 328, 104, 1, 3, true, false, 1, 1);
-    ok &= run_case_f8<256, 64, true, true, 6, true>("f8_pair_mnmn_exactB", 2, 512, 512, 320, 2, 3, false, true, 1, 2);
-    ok &= run_case_f8<256, 64, true, true, 4, false>("f8_mnmn_exactB", 2, 200, 328, 104, 2, 3, false, true, 1, 2);
-    // two 256-column sub-tiles per A tile (weight-gradient shape, CTA pairs)
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_mnmn_2set", 2, 512, 512, 320, 2, 3, false, true);
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_mnmn_wide", 2, 768, 1024, 320, 2, 3, false, true);
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true);
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_mnmn_exactB", 2, 512, 512, 320, 2, 3, false, true, 1, 2);
-    ok &= run_case_f8<256, 64, false, false, 4, true, 2>("f8_nsub2_kk", 3, 768, 512, 512, 1, 3, true, false);
-    // ... with the last row blocks as single-width tail tiles (3 models x 3 row blocks = 9 row blocks, 4 of them tail)
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_tail", 3, 768, 512, 320, 2, 3, false, true, 1, 0, 4);
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_tail_ragged", 2, 200, 328, 104, 2, 3, false, true, 1, 2, 1);
-    ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_nsub2_tail_all", 2, 512, 512, 320, 2, 3, false, true, 1, 0, 4);
+    ok &= run_case_f8<false, false>("f8_kk_exactA", 3, 768, 512, 512, 1, 3, true, false, 1, 1);
+    ok &= run_case_f8<true, true>("f8_mnmn_exactB", 2, 512, 512, 320, 2, 3, false, true, 1, 2);
     }
     if (f8big) {
-      // same-box comparison: the bf16x3 kernels the engine uses today (3 passes) at config-2 shapes
-      ok &= run_case<256, 64, false, false, 3, false, true>("bf_big_encode", 4, 8192, 4096, 512, 1, 3, true, false, 10);
-      ok &= run_case<256, 32, false, true, 6, false, true>("bf_big_decode", 4, 8192, 512, 4096, 1, 3, false, false, 10);
-      ok &= run_case<256, 32, true, true, 6, true, true>("bf_big_dw", 4, 4096, 512, 8192, 2, 3, false, true, 10);
-      ok &= run_case_f8<256, 64, false, false, 6, true>("f8_big_encode", 4, 8192, 4096, 512, 1, 3, true, false, 10);
-      ok &= run_case_f8<256, 64, false, true, 6, true>("f8_big_decode", 4, 8192, 512, 4096, 1, 3, false, false, 10);
-      ok &= run_case_f8<256, 64, true, true, 6, true>("f8_big_dw", 4, 4096, 512, 8192, 2, 3, false, true, 10);
-      ok &= run_case_f8<256, 32, true, true, 8, true>("f8_big_dw32", 4, 4096, 512, 8192, 2, 3, false, true, 10);
-      ok &= run_case_f8<256, 64, false, false, 6, true>("f8_big_enc_hh", 4, 8192, 4096, 512, 1, 1, true, false, 10);
-      ok &= run_case_f8<256, 64, false, false, 6, true>("f8_big_encode_exactA", 4, 8192, 4096, 512, 1, 3, true, false, 10, 1);
-      ok &= run_case_f8<256, 64, true, true, 6, true>("f8_big_dw_exactB", 4, 4096, 512, 8192, 2, 3, false, true, 10, 2);
-      ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_big_dw_nsub2", 4, 4096, 512, 8192, 2, 3, false, true, 10);
-      ok &= run_case_f8<256, 64, true, true, 4, true, 2>("f8_big_dw_nsub2_exactB", 4, 4096, 512, 8192, 2, 3, false, true, 10, 2);
+      // same-GPU comparison with the bf16x3 configuration the engine uses (K block 32, 3 passes) at config-2 shapes
+      ok &= run_case<32, false, false>("bf_big_encode", 4, 8192, 4096, 512, 1, 3, true, false, 10);
+      ok &= run_case<32, false, true>("bf_big_decode", 4, 8192, 512, 4096, 1, 3, false, false, 10);
+      ok &= run_case<32, true, true, true>("bf_big_dw", 4, 4096, 512, 8192, 2, 3, false, true, 10);
+      ok &= run_case_f8<false, false>("f8_big_encode", 4, 8192, 4096, 512, 1, 3, true, false, 10);
+      ok &= run_case_f8<false, true>("f8_big_decode", 4, 8192, 512, 4096, 1, 3, false, false, 10);
+      ok &= run_case_f8<true, true>("f8_big_dw", 4, 4096, 512, 8192, 2, 3, false, true, 10);
+      ok &= run_case_f8<false, false>("f8_big_enc_hh", 4, 8192, 4096, 512, 1, 1, true, false, 10);
+      ok &= run_case_f8<false, false>("f8_big_encode_exactA", 4, 8192, 4096, 512, 1, 3, true, false, 10, 1);
+      ok &= run_case_f8<true, true>("f8_big_dw_exactB", 4, 4096, 512, 8192, 2, 3, false, true, 10, 2);
     }
     if (f8only || f8big) {
       printf(ok ? "ALL PASS\n" : "SOME FAILED\n");
@@ -476,52 +439,44 @@ int main(int argc, char** argv) {
     }
   }
   // ---- K-major x K-major (encode / dC shape), increasing complexity
-  ok &= run_case<256, 64, false, false, 2>("kk_k16", 1, 128, 256, 16, 1, 1, false, false);
-  ok &= run_case<256, 64, false, false, 2>("kk_k64", 1, 128, 256, 64, 1, 1, false, false);
-  ok &= run_case<256, 64, false, false, 2>("kk_k256", 1, 128, 256, 256, 1, 1, false, false);
-  ok &= run_case<256, 64, false, false, 2>("kk_3pass", 1, 128, 256, 256, 1, 3, false, false);
-  ok &= run_case<256, 64, false, false, 2>("kk_multi", 3, 384, 512, 512, 1, 3, true, false);
-  ok &= run_case<256, 64, false, false, 2>("kk_ragged", 2, 200, 328, 104, 1, 3, true, false);
-  ok &= run_case<128, 64, false, false, 3>("kk_bn128", 2, 256, 384, 256, 1, 3, true, false);
+  ok &= run_case<64, false, false>("kk_k16", 1, 128, 256, 16, 1, 1, false, false);
+  ok &= run_case<64, false, false>("kk_k64", 1, 128, 256, 64, 1, 1, false, false);
+  ok &= run_case<64, false, false>("kk_k256", 1, 128, 256, 256, 1, 1, false, false);
+  ok &= run_case<64, false, false>("kk_3pass", 1, 128, 256, 256, 1, 3, false, false);
+  ok &= run_case<64, false, false>("kk_multi", 3, 384, 512, 512, 1, 3, true, false);
+  ok &= run_case<64, false, false>("kk_ragged", 2, 200, 328, 104, 1, 3, true, false);
+  ok &= run_case<64, false, false>("kk_bn128", 2, 256, 384, 256, 1, 3, true, false);
   // ---- K-major operands with the 64-byte swizzle (BK = 32, four stages)
-  ok &= run_case<256, 32, false, false, 4>("kk32_k16", 1, 128, 256, 16, 1, 1, false, false);
-  ok &= run_case<256, 32, false, false, 4>("kk32_k64", 1, 128, 256, 64, 1, 1, false, false);
-  ok &= run_case<256, 32, false, false, 4>("kk32_multi", 3, 384, 512, 512, 1, 3, true, false);
-  ok &= run_case<256, 32, false, false, 4>("kk32_ragged", 2, 200, 328, 104, 1, 3, true, false);
-  ok &= run_case<128, 32, false, false, 6>("kk32_bn128", 2, 256, 384, 256, 1, 3, true, false);
-  ok &= run_case<256, 32, false, true, 4>("kmn32_3pass", 2, 256, 512, 512, 1, 3, false, false);
-  ok &= run_case<256, 32, false, true, 4>("kmn32_ragged", 2, 200, 328, 104, 1, 3, false, false);
-  // ---- CTA pairs (cta_group::2, 256-row tiles)
-  ok &= run_case<256, 64, false, false, 3, false, true>("pair_kk_k16", 1, 256, 256, 16, 1, 1, false, false);
-  ok &= run_case<256, 64, false, false, 3, false, true>("pair_kk_k64", 1, 256, 256, 64, 1, 1, false, false);
-  ok &= run_case<256, 64, false, false, 3, false, true>("pair_kk_multi", 3, 768, 512, 512, 1, 3, true, false);
-  ok &= run_case<256, 64, false, false, 3, false, true>("pair_kk_ragged", 2, 200, 328, 104, 1, 3, true, false);
-  ok &= run_case<256, 64, false, false, 3, false, true>("pair_kk_short", 2, 100, 328, 104, 1, 3, true, false);
-  ok &= run_case<128, 64, false, false, 4, false, true>("pair_kk_bn128", 2, 512, 384, 256, 1, 3, true, false);
-  ok &= run_case<256, 32, false, true, 6, true, true>("pair_kmn_split", 2, 512, 512, 512, 1, 3, false, false);
-  ok &= run_case<256, 32, false, true, 6, true, true>("pair_kmn_ragged", 2, 200, 328, 104, 1, 3, false, false);
-  ok &= run_case<256, 32, true, true, 6, true, true>("pair_mnmn_2set", 2, 512, 512, 320, 2, 3, false, true);
-  ok &= run_case<256, 32, true, true, 6, true, true>("pair_mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true);
+  ok &= run_case<32, false, false>("kk32_k16", 1, 128, 256, 16, 1, 1, false, false);
+  ok &= run_case<32, false, false>("kk32_k64", 1, 128, 256, 64, 1, 1, false, false);
+  ok &= run_case<32, false, false>("kk32_multi", 3, 384, 512, 512, 1, 3, true, false);
+  ok &= run_case<32, false, false>("kk32_ragged", 2, 200, 328, 104, 1, 3, true, false);
+  ok &= run_case<32, false, false>("kk32_bn128", 2, 256, 384, 256, 1, 3, true, false);
+  ok &= run_case<32, false, true>("kmn32_3pass", 2, 256, 512, 512, 1, 3, false, false);
+  ok &= run_case<32, false, true>("kmn32_ragged", 2, 200, 328, 104, 1, 3, false, false);
+  // ---- longer row counts, split accumulators
+  ok &= run_case<64, false, false>("kk_short", 2, 100, 328, 104, 1, 3, true, false);
+  ok &= run_case<32, false, true, true>("kmn_split", 2, 512, 512, 512, 1, 3, false, false);
+  ok &= run_case<32, false, true, true>("kmn_ragged", 2, 200, 328, 104, 1, 3, false, false);
+  ok &= run_case<32, true, true, true>("mnmn_2set", 2, 512, 512, 320, 2, 3, false, true);
+  ok &= run_case<32, true, true, true>("mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true);
   // ---- K-major A x MN-major B (decode shape: X^ = C W)
-  ok &= run_case<256, 64, false, true, 2>("kmn_k16", 1, 128, 256, 16, 1, 1, false, false);
-  ok &= run_case<256, 64, false, true, 2>("kmn_k64", 1, 128, 256, 64, 1, 1, false, false);
-  ok &= run_case<256, 64, false, true, 2>("kmn_3pass", 2, 256, 512, 512, 1, 3, false, false);
-  ok &= run_case<256, 64, false, true, 2>("kmn_ragged", 2, 200, 328, 104, 1, 3, false, false);
+  ok &= run_case<64, false, true>("kmn_k16", 1, 128, 256, 16, 1, 1, false, false);
+  ok &= run_case<64, false, true>("kmn_k64", 1, 128, 256, 64, 1, 1, false, false);
+  ok &= run_case<64, false, true>("kmn_3pass", 2, 256, 512, 512, 1, 3, false, false);
   // ---- MN-major x MN-major (weight-gradient shape: dW = dZ^T X + C^T G), two operand sets
-  ok &= run_case<256, 64, true, true, 2>("mnmn_k16", 1, 128, 256, 16, 1, 1, false, false);
-  ok &= run_case<256, 64, true, true, 2>("mnmn_k64", 1, 128, 256, 64, 1, 1, false, false);
-  ok &= run_case<256, 64, true, true, 2>("mnmn_2set", 2, 256, 512, 320, 2, 3, false, true);
-  ok &= run_case<256, 32, true, true, 4>("mnmn_bk32", 2, 256, 512, 320, 2, 3, false, true);
-  ok &= run_case<256, 32, true, true, 4>("mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true);
+  ok &= run_case<64, true, true>("mnmn_k16", 1, 128, 256, 16, 1, 1, false, false);
+  ok &= run_case<64, true, true>("mnmn_k64", 1, 128, 256, 64, 1, 1, false, false);
+  ok &= run_case<32, true, true>("mnmn_bk32", 2, 256, 512, 320, 2, 3, false, true);
   if (big) {
     // config-2 shapes, one model's worth of each GEMM, for a first throughput reading
-    ok &= run_case<256, 64, false, false, 2>("big_encode", 4, 8192, 4096, 512, 1, 3, true, false);
-    ok &= run_case<256, 64, false, true, 2>("big_decode", 4, 8192, 512, 4096, 1, 3, false, false);
-    ok &= run_case<256, 32, true, true, 4>("big_dw", 4, 4096, 512, 8192, 2, 3, false, true);
-    ok &= run_case<256, 64, true, true, 2>("big_dw64", 4, 4096, 512, 8192, 2, 3, false, true);
-    ok &= run_case<256, 64, false, false, 2>("big_enc1p", 4, 8192, 4096, 512, 1, 1, true, false);
-    ok &= run_case<256, 32, false, false, 4>("big_encode32", 4, 8192, 4096, 512, 1, 3, true, false);
-    ok &= run_case<256, 32, false, true, 4>("big_decode32", 4, 8192, 512, 4096, 1, 3, false, false);
+    ok &= run_case<64, false, false>("big_encode", 4, 8192, 4096, 512, 1, 3, true, false);
+    ok &= run_case<64, false, true>("big_decode", 4, 8192, 512, 4096, 1, 3, false, false);
+    ok &= run_case<32, true, true>("big_dw", 4, 4096, 512, 8192, 2, 3, false, true);
+    ok &= run_case<64, true, true>("big_dw64", 4, 4096, 512, 8192, 2, 3, false, true);
+    ok &= run_case<64, false, false>("big_enc1p", 4, 8192, 4096, 512, 1, 1, true, false);
+    ok &= run_case<32, false, false>("big_encode32", 4, 8192, 4096, 512, 1, 3, true, false);
+    ok &= run_case<32, false, true>("big_decode32", 4, 8192, 512, 4096, 1, 3, false, false);
   }
   printf(ok ? "ALL PASS\n" : "SOME FAILED\n");
   return ok ? 0 : 1;

@@ -12,6 +12,8 @@ kink; a pre-activation within the engine's rounding of zero (|z| < kink_window) 
 gradient checks pin the activity pattern of those (measure-zero) coefficients to the engine's side.
 """
 import math
+import os
+import subprocess
 
 import pytest
 import torch
@@ -663,3 +665,16 @@ def test_bitwise_determinism(kind):
         assert torch.equal(runs[0][0][k], runs[1][0][k])
         assert torch.equal(runs[0][1]["nu"][k], runs[1][1]["nu"][k])
     assert all(torch.equal(a, b) for a, b in zip(runs[0][2], runs[1][2]))
+
+
+def test_gemm_selftest(tmp_path):
+    """The standalone check of the GEMM core (tests/csrc/gemm_selftest.cu): every operand-major / K-block / pass
+    configuration in both arithmetics against a double-precision product of the same planes, ragged edges included."""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    exe = os.path.join(root, "build", "gemm_selftest")
+    if not os.path.exists(exe):   # build() makes it; a tree built with `make` alone may not have it
+        exe = str(tmp_path / "gemm_selftest")
+        subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-o", exe,
+                        os.path.join(root, "tests", "csrc", "gemm_selftest.cu")], check=True)
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and "ALL PASS" in r.stdout, r.stdout[-4000:] + r.stderr[-2000:]

@@ -1,6 +1,6 @@
 """CPU emulation A/B of operand arithmetics (oracle/arith_emulation.py): the two the engine implements and the
 block-scaled 4-bit cross-term candidate of DESIGN.md section 9.1, on a tied-SAE step (forward, x_hat, pattern-pinned
-weight gradient) against fp64.   python tools/arith_ab.py > profiles/r02_arith_ab.txt"""
+weight gradient) against fp64.   python tools/arith_ab.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -60,9 +60,5 @@ for name, mm, passes, byt in ARITHS:
         cells.append(f"{rel(z, z64):9.1e} {rel(xh, xh64):9.1e} {rel(dW, dW64):9.1e} ")
     print(f"{name:52s} {passes:>6s} {byt:>6s}  " + "  ".join(cells))
 print("""
-# Reading: MXFP4 cross terms keep x_hat at 4-5e-5 — inside the 1e-4 bar but with 2x instead of today's 5x margin (the
-# device's f16f8 figures at config 2, 1.3-1.9e-5, agree with the emulated 1.9e-5, so the emulation is a fair predictor). The
-# gain would be 2 -> 1.5 pass-equivalents and 4 -> 3.06 operand bytes per element (the main loops are bound by operand
-# bytes, DESIGN section 4). Not built this round: it needs block-scale planes in tensor memory (tcgen05.cp of UE8M0 scale
-# tiles in the instruction's scale layout) for every operand of every GEMM, i.e. new producers for x, W, c, g and dz;
-# the evidence here says it is worth prototyping in the standalone GEMM self-test first, with the scale rounded up.""")
+# Reading: MXFP4 cross terms keep x_hat at 4-5e-5 — inside the 1e-4 bar but with 2x instead of 5x margin. The gain would
+# be fewer operand bytes per element (4 -> 3.06); it needs a GPU with block-scaled FP4 MMA, which sm_90 does not have.""")

@@ -1,5 +1,5 @@
 """Parity report: the engine (through the C ABI) against the golden vectors recorded from the reference's own loss
-functions, one line per fixture and model. Run on a B200:  python tools/parity_report.py > profiles/rNN_parity_report.txt"""
+functions, one line per fixture and model. Run on a GPU:  python tools/parity_report.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -200,6 +200,33 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream);
 /* The arithmetic the plan resolved to: SCE_ARITH_BF16X3 or SCE_ARITH_F16F8. */
 int sce_plan_arith(const sce_plan* plan);
 
+/* Dictionary similarity without a plan (standard_metrics.py:270-303 mmcs / mcs_duplicates / mcs_to_fixed /
+ * representedness, :356-362 capacity_per_feature). For each pair q = (i, j) of `pairs` it forms S = A_i B_j^T on the
+ * split-operand GEMM and keeps only reductions of it — the [na, nb] matrix never reaches memory:
+ *   row_max[q][r] = max over valid atoms c of B_j of S[r, c]   (each atom of A_i: its best match in B_j)
+ *   col_max[q][c] = max over valid atoms r of A_i of S[r, c]   (each atom of B_j: its best match in A_i)
+ *   capacity[i][r] = S[r, r]^2 / sum_c S[r, c]^2             for the self-pairs (i, i); needs b == NULL
+ * Entries of atoms beyond rows[m] are NaN; so is the capacity of a zero row (0 / 0, as in the reference).
+ *   a, b        device fp32 [ma, na, d] / [mb, nb, d] stacks of dictionaries; b == NULL: B = A (mb, nb, b_* ignored)
+ *   *_rows      HOST int32 [ma] / [mb]: valid atoms of each model (masked stacks export encoder[:dict_size]), each in
+ *               [1, n]; NULL = all
+ *   *_normalize 1: rows divided by max(||row||, floor) on the device (floor <= 0: no clamp — TopK), the
+ *               get_learned_dict of the SAE and TopK signatures; 0: the matrix as given (a raw truth matrix)
+ *   pairs       HOST int32 [n_pairs][2]: (model of A, model of B)
+ *   arith       sce_arith. AUTO: BF16X3 (the faster and more accurate of the two on this GEMM; env SCE_ARITH=f16f8 pins
+ *               AUTO to F16F8 where d % 16 == 0). Under F16F8 a raw operand fp16 cannot hold (|v| >= 65520 or NaN) is
+ *               SCE_ERR_INVALID (a pinned AUTO runs it on BF16X3); finding out costs one 4-byte copy and a stream
+ *               synchronise for calls with a raw operand.
+ *   row_max, col_max, capacity  device fp32 outputs, each optional (at least one)
+ *   workspace   >= sce_similarity_workspace_bytes(...), 1024-byte aligned: operand planes (4 B per element) and, with
+ *               capacity, sum-of-squares partials [n_pairs][na][2 ceil(na / 128)] — never O(na nb).
+ * Bitwise repeatable: maxima are exact, sums are reduced in a fixed order. Asynchronous on `stream` otherwise. */
+size_t sce_similarity_workspace_bytes(int ma, int na, int mb /* 0: B = A */, int nb, int d, int n_pairs, int want_capacity);
+int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_norm_floor, int a_normalize,
+                   const float* b, int mb, int nb, const int* b_rows, float b_norm_floor, int b_normalize,
+                   int d, const int* pairs, int n_pairs, int arith, float* row_max, float* col_max, float* capacity,
+                   void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

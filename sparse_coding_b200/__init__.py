@@ -3,7 +3,8 @@
 Public names mirror the reference's ``autoencoders`` package for the hot path only (SURVEY.md §8):
 DictSignature / FunctionalEnsemble (ensemble.py), FunctionalSAE / FunctionalTiedSAE / masked variants
 (sae_ensemble.py), TopKEncoder / TopKLearnedDict (topk_encoder.py), LearnedDict / TiedSAE / UntiedSAE
-(learned_dict.py), plus the driver loop pieces of big_sweep.py (train_loop.py)."""
+(learned_dict.py), plus the driver loop pieces of big_sweep.py (train_loop.py) and on-device metrics (metrics.py)."""
+from . import metrics
 from .ensemble import CodeProxy, FunctionalEnsemble, optim_str_to_func, stack_dict, unstack_dict
 from .learned_dict import LearnedDict, TiedSAE, UntiedSAE
 from .optim import AdamConfig, adam

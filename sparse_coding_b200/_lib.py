@@ -25,6 +25,7 @@ EXPORTS = [
     "sce_step", "sce_step_host", "sce_forward", "sce_read_code", "sce_grads", "sce_gather_rows",
     "sce_last_launch_count", "sce_get_step_count", "sce_set_step_count", "sce_profile_begin", "sce_profile_end",
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
+    "sce_similarity_workspace_bytes", "sce_similarity",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -92,6 +93,10 @@ def load():
     lib.sce_health.argtypes = [vp, vp, vp, vp]
     lib.sce_clear_health.argtypes = [vp, vp]
     lib.sce_active_counts.argtypes = [vp, i, vp, vp]
+    lib.sce_similarity_workspace_bytes.restype = C.c_size_t
+    lib.sce_similarity_workspace_bytes.argtypes = [i, i, i, i, i, i, i]
+    f = C.c_float
+    lib.sce_similarity.argtypes = [vp, i, i, vp, f, i, vp, i, i, vp, f, i, i, vp, i, i, vp, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

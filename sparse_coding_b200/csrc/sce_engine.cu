@@ -795,6 +795,171 @@ static int run_pipeline(sce_plan* p, const float* x, int B, float* x_hat, bool b
 }
 
 // ------------------------------------------------------------------------------------------------
+// dictionary similarity (sce_similarity): cosine maxima and capacity over a list of dictionary pairs
+// ------------------------------------------------------------------------------------------------
+// maxima keys (EpiSimilarity) -> floats, in place; key 0 (no valid entry: an atom beyond rows[m]) becomes NaN
+__global__ void key_to_float_kernel(uint32_t* __restrict__ v, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const uint32_t k = v[i];
+    v[i] = (k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k;
+  }
+}
+
+// capacity_per_feature (standard_metrics.py:356-362) of every self-pair (m, m): diag(S^2) / rowsum(S^2), the row sum
+// taken over the partials of EpiSimilarity in a fixed order. Atoms beyond rows[m] get NaN. A zero row gives 0 / 0 = NaN,
+// as in the reference.
+__global__ void capacity_kernel(const int* __restrict__ pairs, const int* __restrict__ rows, const float* __restrict__ sq_part,
+                                const float* __restrict__ diag, int na, int parts, float* __restrict__ out) {
+  const int q = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int m = pairs[2 * q];
+  if (i >= na || m != pairs[2 * q + 1]) return;
+  float* o = out + (long long)m * na + i;
+  if (i >= rows[m]) {
+    *o = __int_as_float(0x7FFFFFFF);
+    return;
+  }
+  const float* s = sq_part + ((long long)q * na + i) * parts;
+  float sum = 0.f;
+  for (int t = 0; t < parts; ++t) sum += s[t];
+  const float dg = diag[(long long)q * na + i];
+  *o = dg * dg / sum;
+}
+
+struct SimOperand {   // one side of sce_similarity
+  const float* w;
+  int models, rows;
+  int normalize;
+  float floor;
+};
+
+// Workspace of one call: operand planes (4 B per element), the pair list and valid-row counts, the range flags of the
+// f16f8 split, and (capacity) the sum-of-squares partials [P][na][2 tiles_n] and diagonal [P][na]. With base == nullptr
+// only measures; `f8` only changes the order of the planes, not the bytes.
+struct SimCarve {
+  void *a_hi, *a_lo, *a_x8, *b_hi, *b_lo, *b_x8;
+  int *pairs, *a_rows, *b_rows;
+  uint32_t* flags;
+  float *sq_part, *diag;
+};
+static size_t sim_carve(uint8_t* base, bool f8, long long ma, long long na, long long mb, long long nb, long long d,
+                        long long n_pairs, bool capacity, SimCarve* out) {
+  Carve c{base, 0};
+  auto planes = [&](size_t count, void*& hi, void*& lo, void*& x8) {
+    hi = c.take<__nv_bfloat16>(count);
+    if (f8) {
+      lo = c.take<uint8_t>(count);
+      x8 = c.take<uint8_t>(count);
+    } else {
+      lo = c.take<__nv_bfloat16>(count);
+      x8 = nullptr;
+    }
+  };
+  SimCarve s;
+  memset(&s, 0, sizeof(s));
+  planes((size_t)(ma * na * d), s.a_hi, s.a_lo, s.a_x8);
+  if (mb > 0) planes((size_t)(mb * nb * d), s.b_hi, s.b_lo, s.b_x8);
+  s.pairs = c.take<int>((size_t)(2 * n_pairs));
+  s.a_rows = c.take<int>((size_t)ma);
+  s.b_rows = mb > 0 ? c.take<int>((size_t)mb) : s.a_rows;
+  s.flags = c.take<uint32_t>(kFlagWords);
+  if (capacity) {
+    const long long tiles_n = (na + kBN - 1) / kBN;
+    s.sq_part = c.take<float>((size_t)(n_pairs * na * 2 * tiles_n));
+    s.diag = c.take<float>((size_t)(n_pairs * na));
+  }
+  if (out) *out = s;
+  return align_up(c.off, 1024);
+}
+static size_t sim_workspace(long long ma, long long na, long long mb, long long nb, long long d, long long n_pairs, bool capacity) {
+  const size_t a = sim_carve(nullptr, false, ma, na, mb, nb, d, n_pairs, capacity, nullptr);
+  const size_t b = sim_carve(nullptr, true, ma, na, mb, nb, d, n_pairs, capacity, nullptr);
+  return a > b ? a : b;
+}
+
+// fp32 operand -> planes: normalised rows (dict_rows_kernel<MODE_PREPARE>, LearnedDict.get_learned_dict) or the matrix
+// as given (split_rows_kernel; f16f8: sets the range flags when a value does not fit fp16)
+template <int AR>
+static int sim_planes(const SimOperand& o, int d, void* hi, void* lo, void* x8, uint32_t* flags, cudaStream_t st) {
+  const long long rows = (long long)o.models * o.rows;
+  if (o.normalize)
+    return launch_dict_rows_t<MODE_PREPARE, AR>(const_cast<float*>(o.w), nullptr, nullptr, nullptr, hi, lo, x8, nullptr, rows, d,
+                                                 1, o.floor, AdamHyper{}, nullptr, nullptr, st);
+  const long long n4 = rows * d / 4;
+  const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
+  split_rows_kernel<AR><<<blocks, 256, 0, st>>>(o.w, hi, lo, x8, n4, AR == kArithF16F8 ? flags : nullptr);
+  CUDA_TRY(cudaGetLastError());
+  return SCE_OK;
+}
+
+template <int AR>
+static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_a, int d, int n_pairs, const SimCarve& w,
+                            float* row_max, float* col_max, float* capacity, int device, int sms, cudaStream_t st) {
+  constexpr int BK = AR == kArithF16F8 ? kBkF8 : kBkBf16;
+  constexpr int STAGES = gemm_stages<BK, EpiSimilarity::kWarpStageBytes, AR>();
+  using SM = GemmSmem<BK, STAGES, EpiSimilarity::kWarpStageBytes, AR>;
+  auto kern = gemm_split_kernel<EpiSimilarity, BK, false, false, STAGES, false, AR>;
+  int rc = sim_planes<AR>(A, d, w.a_hi, w.a_lo, w.a_x8, w.flags, st);
+  if (rc) return rc;
+  if (!b_is_a) {
+    rc = sim_planes<AR>(B, d, w.b_hi, w.b_lo, w.b_x8, w.flags, st);
+    if (rc) return rc;
+  }
+  const void* const b_hi = b_is_a ? w.a_hi : w.b_hi;
+  const void* const b_lo = b_is_a ? w.a_lo : w.b_lo;
+  const void* const b_x8 = b_is_a ? w.a_x8 : w.b_x8;
+  GemmParams<EpiSimilarity::Params> gp;
+  memset(&gp, 0, sizeof(gp));
+  // both operands are dictionary rows, K-major over d: the encode GEMM's B-operand geometry on both sides
+  bool ok = operand_maps(AR, &gp.a_hi[0], &gp.a_lo[0], &gp.a_x8[0], w.a_hi, w.a_lo, w.a_x8, A.models, A.rows, d,
+                         (uint64_t)A.rows * d, kBM, BK);
+  ok = ok && operand_maps(AR, &gp.b_hi[0], &gp.b_lo[0], &gp.b_x8[0], b_hi, b_lo, b_x8, B.models, B.rows, d,
+                          (uint64_t)B.rows * d, kBN, BK);
+  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (similarity: na=%d, nb=%d, d=%d)", A.rows, B.rows, d);
+  gp.a_batched[0] = gp.b_batched[0] = 1;
+  gp.nsets = 1;
+  gp.k_total = d;
+  gp.passes = 3;
+  gp.n_models = n_pairs;
+  gp.m_total = A.rows;
+  gp.n_total = B.rows;
+  gp.tiles_m = (A.rows + kBM - 1) / kBM;
+  gp.tiles_n = (B.rows + kBN - 1) / kBN;
+  gp.epi.pairs = w.pairs;
+  gp.epi.a_rows = w.a_rows;
+  gp.epi.b_rows = w.b_rows;
+  gp.epi.row_max = reinterpret_cast<uint32_t*>(row_max);
+  gp.epi.col_max = reinterpret_cast<uint32_t*>(col_max);
+  gp.epi.sq_part = capacity ? w.sq_part : nullptr;
+  gp.epi.diag = w.diag;
+  gp.epi.tiles_n = gp.tiles_n;
+  if (row_max) CUDA_TRY(cudaMemsetAsync(row_max, 0, (size_t)n_pairs * A.rows * sizeof(float), st));
+  if (col_max) CUDA_TRY(cudaMemsetAsync(col_max, 0, (size_t)n_pairs * B.rows * sizeof(float), st));
+  static bool configured[64] = {};
+  if (device < 0 || device >= 64 || !configured[device]) {
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes));
+    if (device >= 0 && device < 64) configured[device] = true;
+  }
+  const long long tiles = (long long)n_pairs * gp.tiles_m * gp.tiles_n;   // persistent: at most one CTA per SM
+  kern<<<(unsigned)(tiles < sms ? tiles : sms), kGemmThreads, SM::kBytes, st>>>(gp);
+  CUDA_TRY(cudaGetLastError());
+  auto to_float = [&](float* v, long long n) -> int {
+    const int blocks = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
+    key_to_float_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<uint32_t*>(v), n);
+    CUDA_TRY(cudaGetLastError());
+    return SCE_OK;
+  };
+  if (row_max && (rc = to_float(row_max, (long long)n_pairs * A.rows))) return rc;
+  if (col_max && (rc = to_float(col_max, (long long)n_pairs * B.rows))) return rc;
+  if (capacity) {
+    capacity_kernel<<<dim3((A.rows + 255) / 256, n_pairs), 256, 0, st>>>(w.pairs, w.a_rows, w.sq_part, w.diag, A.rows,
+                                                                       2 * gp.tiles_n, capacity);
+    CUDA_TRY(cudaGetLastError());
+  }
+  return SCE_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
 extern "C" {
@@ -1237,6 +1402,97 @@ int sce_set_step_count(sce_plan* plan, long long steps_taken) {
   if (!plan || steps_taken < 0) return fail(SCE_ERR_INVALID, "bad arguments to sce_set_step_count");
   plan->step = steps_taken;
   return SCE_OK;
+}
+
+size_t sce_similarity_workspace_bytes(int ma, int na, int mb, int nb, int d, int n_pairs, int want_capacity) {
+  if (ma < 1 || na < 1 || mb < 0 || (mb > 0 && nb < 1) || d < 8 || n_pairs < 1) return 0;
+  return sim_workspace(ma, na, mb, mb > 0 ? nb : 0, d, n_pairs, want_capacity != 0);
+}
+
+int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_norm_floor, int a_normalize,
+                   const float* b, int mb, int nb, const int* b_rows, float b_norm_floor, int b_normalize,
+                   int d, const int* pairs, int n_pairs, int arith, float* row_max, float* col_max, float* capacity,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!a) return fail(SCE_ERR_INVALID, "similarity: a is NULL");
+  if (ma < 1 || na < 1) return fail(SCE_ERR_INVALID, "similarity: ma (%d) and na (%d) must be >= 1", ma, na);
+  if (d < 8 || d % 8) return fail(SCE_ERR_INVALID, "similarity: d (%d) must be a positive multiple of 8", d);
+  if (d > 8192) return fail(SCE_ERR_INVALID, "similarity: d = %d > 8192 is not supported by the row kernels", d);
+  if ((a_normalize != 0 && a_normalize != 1) || (b && b_normalize != 0 && b_normalize != 1))
+    return fail(SCE_ERR_INVALID, "similarity: a_normalize / b_normalize must be 0 or 1");
+  const bool b_is_a = b == nullptr;
+  if (!b_is_a && (mb < 1 || nb < 1)) return fail(SCE_ERR_INVALID, "similarity: mb (%d) and nb (%d) must be >= 1", mb, nb);
+  const int Mb = b_is_a ? ma : mb, Nb = b_is_a ? na : nb;
+  if (!pairs || n_pairs < 1) return fail(SCE_ERR_INVALID, "similarity: need at least one pair (pairs NULL or n_pairs = %d)", n_pairs);
+  if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "similarity: unknown arith %d", arith);
+  if (arith == SCE_ARITH_F16F8 && d % 16)
+    return fail(SCE_ERR_INVALID, "similarity: arith = F16F8 needs d (%d) to be a multiple of 16", d);
+  if (!row_max && !col_max && !capacity) return fail(SCE_ERR_INVALID, "similarity: no output requested");
+  if (capacity && !b_is_a) return fail(SCE_ERR_INVALID, "similarity: capacity is defined for self-pairs of one stack (b must be NULL)");
+  const long long tiles = (long long)n_pairs * ((na + kBM - 1) / kBM) * ((Nb + kBN - 1) / kBN);
+  if (tiles > 0x7FFFFFFFll) return fail(SCE_ERR_INVALID, "similarity: %lld tiles exceed the 32-bit tile index", tiles);
+  std::vector<int> pv(pairs, pairs + 2 * (size_t)n_pairs);
+  for (int q = 0; q < n_pairs; ++q)
+    if (pv[2 * q] < 0 || pv[2 * q] >= ma || pv[2 * q + 1] < 0 || pv[2 * q + 1] >= Mb)
+      return fail(SCE_ERR_INVALID, "similarity: pair %d = (%d, %d) outside [0, %d) x [0, %d)", q, pv[2 * q], pv[2 * q + 1], ma, Mb);
+  std::vector<int> rows(ma + (b_is_a ? 0 : mb));
+  for (int m = 0; m < ma; ++m) rows[m] = a_rows ? a_rows[m] : na;
+  for (int m = 0; !b_is_a && m < mb; ++m) rows[ma + m] = b_rows ? b_rows[m] : nb;
+  for (int m = 0; m < (int)rows.size(); ++m) {
+    const int n = m < ma ? na : nb;
+    if (rows[m] < 1 || rows[m] > n)
+      return fail(SCE_ERR_INVALID, "similarity: rows[%d] of %s = %d outside [1, %d]", m < ma ? m : m - ma, m < ma ? "a" : "b", rows[m], n);
+  }
+  const size_t need = sim_workspace(ma, na, b_is_a ? 0 : mb, b_is_a ? 0 : nb, d, n_pairs, capacity != nullptr);
+  if (!workspace || workspace_bytes < need)
+    return fail(SCE_ERR_WORKSPACE, "similarity: workspace too small: have %zu bytes, need %zu", workspace_bytes, need);
+  if (reinterpret_cast<uintptr_t>(workspace) % 1024) return fail(SCE_ERR_WORKSPACE, "similarity: workspace must be 1024-byte aligned");
+
+  // ---- device
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int dev = 0, major = 0, sms = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (major != 9) return fail(SCE_ERR_NO_DEVICE, "libsce needs an sm_90 device (found compute capability %d.x)", major);
+  if (!get_encode_fn()) return fail(SCE_ERR_NO_DEVICE, "cuTensorMapEncodeTiled driver entry point not available");
+  const SimOperand A{a, ma, na, a_normalize, a_norm_floor};
+  const SimOperand B = b_is_a ? A : SimOperand{b, mb, nb, b_normalize, b_norm_floor};
+  // AUTO: bf16x3. Unlike the training GEMMs, whose epilogues write operand planes and which are bound by the SM's data
+  // paths, this GEMM's epilogue is light, and the widening of the E5M2 tiles made f16f8 the slower arithmetic here (H100,
+  // config 2: 30.1 ms against 23.9 ms per pass) as well as the less accurate one (5e-6 against 1.3e-6 from fp64).
+  // SCE_ARITH=f16f8 pins AUTO to f16f8 where d % 16 == 0. f16f8 splits a raw operand first and reads its range flag back
+  // (one 4-byte copy + synchronise): a value fp16 cannot hold (|v| >= 65520 or NaN) moves a pinned AUTO to bf16x3 and
+  // is an error under explicit F16F8.
+  const char* env = getenv("SCE_ARITH");
+  bool f8 = arith == SCE_ARITH_F16F8 || (arith == SCE_ARITH_AUTO && env && !strcmp(env, "f16f8") && d % 16 == 0);
+  const bool raw = !A.normalize || (!b_is_a && !B.normalize);
+  SimCarve w;
+  if (f8 && raw) {
+    sim_carve(static_cast<uint8_t*>(workspace), true, ma, na, b_is_a ? 0 : mb, b_is_a ? 0 : nb, d, n_pairs, capacity != nullptr, &w);
+    CUDA_TRY(cudaMemsetAsync(w.flags, 0, kFlagWords * sizeof(uint32_t), st));
+    int rc = SCE_OK;
+    if (!A.normalize) rc = sim_planes<kArithF16F8>(A, d, w.a_hi, w.a_lo, w.a_x8, w.flags, st);
+    if (!rc && !b_is_a && !B.normalize) rc = sim_planes<kArithF16F8>(B, d, w.b_hi, w.b_lo, w.b_x8, w.flags, st);
+    if (rc) return rc;
+    uint32_t bad = 0;
+    CUDA_TRY(cudaMemcpyAsync(&bad, w.flags + kBadWord, sizeof(bad), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (bad) {
+      if (arith == SCE_ARITH_F16F8)
+        return fail(SCE_ERR_INVALID, "similarity: a raw operand holds a value fp16 cannot (|v| >= 65520 or NaN); use "
+                                     "arith = BF16X3 or AUTO");
+      f8 = false;
+    }
+  }
+  sim_carve(static_cast<uint8_t*>(workspace), f8, ma, na, b_is_a ? 0 : mb, b_is_a ? 0 : nb, d, n_pairs, capacity != nullptr, &w);
+  // the pair list and row counts are host locals: copies from pageable memory are staged before cudaMemcpyAsync returns
+  CUDA_TRY(cudaMemcpyAsync(w.pairs, pv.data(), pv.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(w.a_rows, rows.data(), (size_t)ma * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (!b_is_a) CUDA_TRY(cudaMemcpyAsync(w.b_rows, rows.data() + ma, (size_t)mb * sizeof(int), cudaMemcpyHostToDevice, st));
+  // (a raw operand split above for the range check is split again here: the planes of the arithmetic that runs)
+  return f8 ? run_similarity_t<kArithF16F8>(A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms, st)
+            : run_similarity_t<kArithBf16x3>(A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms, st);
 }
 
 }  // extern "C"

@@ -579,6 +579,87 @@ struct EpiCenter {
   __device__ __forceinline__ void finish() {}
 };
 
+// ------------------------------------------------------------------------------------------------
+// dictionary similarity (standard_metrics.py:270-303, 356-362): acc = <a_i, b_j> for the pair (model_a, model_b) of the
+// tile (kPairTiles). The [na, nb] matrix never reaches HBM; per tile the epilogue leaves
+//   row maxima   max over valid j of acc (each A atom's best match in B)       -> row_max keys [P][na]
+//   column maxima max over valid i of acc (each B atom's best match in A)      -> col_max keys [P][nb]
+//   self-pairs (model_a == model_b, capacity): the row sum of acc^2 of this tile's 64 columns of each group ->
+//   sq_part [P][na][2 tiles_n], and the diagonal element -> diag [P][na]
+// Maxima go through integer atomicMax on order-preserving keys (f2key): exact and independent of the order tiles finish
+// in. The sums of squares are partials reduced in a fixed order afterwards (capacity_kernel), so a result is bitwise
+// repeatable. Atoms at index >= rows[model] (masked stacks, and the zero rows TMA fills in beyond na / nb) enter no
+// maximum and no sum: a zero row has cosine 0 and would win where every real cosine is negative.
+// ------------------------------------------------------------------------------------------------
+struct EpiSimilarity {
+  static constexpr int kCols = 32;
+  static constexpr int kWarpStageBytes = 0;
+  static constexpr bool kPairTiles = true;
+  struct Params {
+    const int* pairs;      // [P][2]: model of A, model of B
+    const int* a_rows;     // [Ma] valid atoms of each A model
+    const int* b_rows;     // [Mb]
+    uint32_t* row_max;     // [P][na] keys, zeroed by the caller; or nullptr
+    uint32_t* col_max;     // [P][nb] keys, zeroed by the caller; or nullptr
+    float* sq_part;        // [P][na][2 tiles_n] or nullptr (no capacity)
+    float* diag;           // [P][na]
+    int tiles_n;
+  };
+  const Params& P;
+  const TileCoord& T;
+  int m_total, n_total;
+  int ra, rb;              // valid atoms of this pair's A and B models
+  bool self;               // capacity partials wanted for this tile (self-pair)
+  uint32_t rkey = 0u;      // this thread's row maximum over its chunks (key 0 is below every float)
+  float sq = 0.f;
+  __device__ EpiSimilarity(const Params& p, const TileCoord& t, int m, int n, uint8_t*) : P(p), T(t), m_total(m), n_total(n) {
+    const int ma = __ldg(P.pairs + 2 * T.model), mb = __ldg(P.pairs + 2 * T.model + 1);
+    ra = __ldg(P.a_rows + ma);
+    rb = __ldg(P.b_rows + mb);
+    self = P.sq_part != nullptr && ma == mb;
+  }
+  static __device__ __forceinline__ uint32_t key(uint32_t u) { return u ^ ((uint32_t)((int32_t)u >> 31) | 0x80000000u); }  // == f2key
+
+  __device__ __forceinline__ void chunk(int c, const uint32_t (&r)[32]) {
+    const int col = T.col0 + c;
+    if (col >= rb) return;   // warp-uniform: no valid column in this chunk
+    const int valid = rb - col;
+    const bool row_ok = T.row < ra;
+    uint32_t ck[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const bool ok = row_ok && (valid >= 32 || j < valid);
+      const uint32_t k = ok ? key(r[j]) : 0u;
+      rkey = max(rkey, k);
+      ck[j] = k;
+      if (self && ok) {
+        const float v = __uint_as_float(r[j]);
+        sq += v * v;
+        if (col + j == T.row) P.diag[(long long)T.model * m_total + T.row] = v;
+      }
+    }
+    if (P.col_max && T.m_blk * kBM + T.warp_q * 32 < ra) {   // warp-uniform: some row of this warp is valid
+      // transpose-reduce: 32 lanes x 32 columns -> lane j holds the maximum of column j over the warp's rows
+#pragma unroll
+      for (int half = 16; half >= 1; half >>= 1) {
+        const bool upper = (T.lane & half) != 0;
+#pragma unroll
+        for (int i = 0; i < half; ++i) {
+          const uint32_t send = upper ? ck[i] : ck[i + half];
+          const uint32_t keep = upper ? ck[i + half] : ck[i];
+          ck[i] = max(keep, __shfl_xor_sync(0xffffffffu, send, half));
+        }
+      }
+      if (T.lane < valid) atomicMax(P.col_max + (long long)T.model * n_total + col + T.lane, ck[0]);
+    }
+  }
+  __device__ __forceinline__ void finish() {
+    if (P.row_max && T.row < ra) atomicMax(P.row_max + (long long)T.model * m_total + T.row, rkey);
+    if (self && T.row < m_total)
+      P.sq_part[((long long)T.model * m_total + T.row) * (2 * P.tiles_n) + 2 * T.n_blk + T.grp] = sq;
+  }
+};
+
 using EpiEncode = EpiEncodeT<kArithBf16x3>;
 using EpiDecode = EpiDecodeT<kArithBf16x3>;
 using EpiDcode = EpiDcodeT<kArithBf16x3>;

@@ -30,7 +30,7 @@ constexpr int kSmemLimit = 232448;  // 227 KB of shared memory one CTA may use o
 
 // What the epilogue functor sees for each tile.
 struct TileCoord {
-  int model;    // ensemble index
+  int model;    // ensemble index (pair index for epilogues with kPairTiles)
   int m_blk;    // tile row index
   int n_blk;    // tile column index
   int row;      // global output row owned by this thread (may be >= m_total: predicate!)
@@ -102,6 +102,14 @@ struct epi_pairs_chunks : std::false_type {};
 template <class Epi>
 struct epi_pairs_chunks<Epi, std::void_t<decltype(Epi::kPairChunks)>> : std::bool_constant<Epi::kPairChunks> {};
 
+// epilogues may declare `static constexpr bool kPairTiles = true`: the tile's `model` index is then a PAIR index, and the
+// operand models of pair q are read from the device list Epi::Params::pairs ([q][2] = model of A, model of B) instead of
+// following a_batched / b_batched. One persistent launch then runs any set of (model_a, model_b) products.
+template <class Epi, class = void>
+struct epi_pair_tiles : std::false_type {};
+template <class Epi>
+struct epi_pair_tiles<Epi, std::void_t<decltype(Epi::kPairTiles)>> : std::bool_constant<Epi::kPairTiles> {};
+
 // f16f8: an 8-bit tile as TMA delivers it without swizzle — K-major [ROWS][BK] or MN-major [BK][ROWS] bytes — widened
 // to the fp16 tile the 16-bit loads of the same operand produce: K-major [ROWS][BK] with the 128-byte swizzle (BK = 64),
 // MN-major [ROWS / 64][BK][64] with the 128-byte swizzle. 256 consumer threads, 16 bytes each per round.
@@ -172,6 +180,16 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     tile_m = rem / p.tiles_n;
     tile_n = rem % p.tiles_n;
   };
+  // operand models of operand pair `set` for the tile's model (or pair) index
+  auto operand_models = [&](int model, int set, int& am, int& bm) {
+    if constexpr (epi_pair_tiles<Epi>::value) {
+      am = __ldg(p.epi.pairs + 2 * model);
+      bm = __ldg(p.epi.pairs + 2 * model + 1);
+    } else {
+      am = p.a_batched[set] ? model : 0;
+      bm = p.b_batched[set] ? model : 0;
+    }
+  };
   const int kblocks = (p.k_total + BK - 1) / BK;
   const bool three = p.passes >= 3;
 
@@ -225,8 +243,8 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
           // sweep 1: the 8-bit planes (skipped for passes == 1); sweep 2: the fp16 planes
           for (int sweep = three ? 0 : 1; sweep < 2; ++sweep)
             for (int set = 0; set < p.nsets; ++set) {
-              const int am = p.a_batched[set] ? model : 0;
-              const int bm = p.b_batched[set] ? model : 0;
+              int am, bm;
+              operand_models(model, set, am, bm);
               // cross terms of this operand pair: t_lh = A.l8 x B.h8 (needs A's residual), t_hl = A.h8 x B.l8
               const bool t_lh = term_lh[set], t_hl = term_hl[set];
               if (sweep == 0 && !t_lh && !t_hl) continue;
@@ -268,8 +286,8 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
             }
         } else {
           for (int set = 0; set < p.nsets; ++set) {
-            const int am = p.a_batched[set] ? model : 0;
-            const int bm = p.b_batched[set] ? model : 0;
+            int am, bm;
+            operand_models(model, set, am, bm);
             for (int kb = 0; kb < kblocks; ++kb) {
               mbar_wait(&empty_bar[stage], phase ^ 1);
               uint8_t* sa_hi = smem + stage * SM::kStage;

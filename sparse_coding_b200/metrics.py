@@ -68,3 +68,229 @@ def evaluate_batches(ensemble, batches: Iterable[torch.Tensor],
     return {"fvu": (sq / total).float(), "mean_l0": (l0 / rows).float(), "feature_counts": counts,
             "feature_frequency": counts.float() / rows, "n_ever_active": n_act,
             "frac_dead": 1.0 - n_act.float() / counts.shape[-1], "rows": rows}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Dictionary similarity (standard_metrics.py:270-303, 356-362): cosine maxima between dictionaries and the capacity of
+# Scherlis et al., on the split-operand GEMM (libsce ``sce_similarity``). Each is an [n1, d] x [n2, d]^T product followed
+# by a row maximum, a column maximum or a row sum; the engine keeps only those reductions, so the [n1, n2] matrix never
+# exists, and one launch runs every pair of a sweep.
+# ---------------------------------------------------------------------------------------------------------------------
+class _Stack:
+    """One side of a similarity call: fp32 [M, n, d] on a CUDA device, per-model valid rows, normalisation."""
+
+    def __init__(self, w, rows, floor):
+        self.w, self.rows, self.floor = w, rows, floor      # floor None: the matrix as given
+
+    @property
+    def models(self):
+        return self.w.shape[0]
+
+
+def _ld_matrix(ld):
+    """(matrix [n, d], norm_floor) whose normalised rows are ``ld.get_learned_dict()``."""
+    from .learned_dict import NORM_FLOOR, TiedSAE, UntiedSAE
+    if isinstance(ld, TiedSAE):
+        return ld.encoder, NORM_FLOOR
+    if isinstance(ld, UntiedSAE):
+        return ld.decoder, NORM_FLOOR
+    return ld.get_learned_dict(), None       # TopKLearnedDict (stored normalised) and any other LearnedDict
+
+
+def _as_stack(x):
+    """FunctionalEnsemble, LearnedDict, list of LearnedDicts, or a tensor [M, n, d] / [n, d] (taken as given)."""
+    from .learned_dict import LearnedDict
+    if hasattr(x, "sig") and hasattr(x, "params"):                           # FunctionalEnsemble
+        w, floor, rows = x.sig.learned_dict_stack(x.params, x.buffers)
+        rows = None if rows is None else [int(r) for r in rows.reshape(-1).tolist()]
+        return _Stack(w, rows, floor)
+    if isinstance(x, LearnedDict):
+        w, floor = _ld_matrix(x)
+        return _Stack(w[None], None, floor)
+    if isinstance(x, (list, tuple)):
+        mats = [_ld_matrix(ld) if isinstance(ld, LearnedDict) else (ld, None) for ld in x]
+        floors = {f for _, f in mats}
+        if len(floors) != 1:                                                 # mixed kinds: normalise in torch first
+            mats = [(ld.get_learned_dict() if isinstance(ld, LearnedDict) else ld, None) for ld in x]
+            floors = {None}
+        ns = [m.shape[0] for m, _ in mats]
+        n, d = max(ns), mats[0][0].shape[1]
+        if len(set(ns)) == 1:
+            w = torch.stack([m for m, _ in mats])
+        else:                                                                # zero-padded to the largest dictionary
+            w = mats[0][0].new_zeros(len(mats), n, d)
+            for i, (m, _) in enumerate(mats):
+                w[i, : m.shape[0]] = m
+        return _Stack(w, None if len(set(ns)) == 1 else ns, floors.pop())
+    if torch.is_tensor(x):
+        return _Stack(x if x.dim() == 3 else x[None], None, None)
+    raise TypeError(f"expected a FunctionalEnsemble, LearnedDict(s) or a tensor, got {type(x).__name__}")
+
+
+def _run_similarity(a: _Stack, b: Optional[_Stack], pairs, row=True, col=True, capacity=False, arith="auto"):
+    """(row_max [P, na], col_max [P, nb], capacity [Ma, na]) on the CUDA device of ``a`` (None where not requested)."""
+    import ctypes as C
+    from . import _lib
+    dev = a.w.device
+    if dev.type != "cuda":
+        if not torch.cuda.is_available():
+            raise RuntimeError("dictionary similarity runs in the sm_90a CUDA engine and needs a CUDA device; there is "
+                               "no CPU implementation in the product path")
+        dev = torch.device("cuda", torch.cuda.current_device())
+    if arith not in _lib.ARITH_CODE:
+        raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
+    prep = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
+    aw = prep(a.w)
+    bw = prep(b.w) if b is not None else None
+    Ma, na, d = aw.shape
+    Mb, nb = (bw.shape[0], bw.shape[1]) if bw is not None else (Ma, na)
+    if bw is not None and bw.shape[2] != d:
+        raise ValueError(f"dictionaries of different widths: {d} and {bw.shape[2]}")
+    pv = torch.as_tensor(pairs, dtype=torch.int32).reshape(-1, 2).contiguous()
+    P = pv.shape[0]
+    lib = _lib.load()
+    need = lib.sce_similarity_workspace_bytes(Ma, na, Mb if bw is not None else 0, nb, d, P, int(capacity))
+    if need == 0:
+        raise ValueError(f"invalid similarity shape: a [{Ma}, {na}, {d}], b [{Mb}, {nb}], {P} pairs")
+    ws = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
+    ws_ptr = (ws.data_ptr() + 1023) // 1024 * 1024
+    row_max = torch.empty(P, na, dtype=torch.float32, device=dev) if row else None
+    col_max = torch.empty(P, nb, dtype=torch.float32, device=dev) if col else None
+    cap = torch.full((Ma, na), float("nan"), dtype=torch.float32, device=dev) if capacity else None
+    ints = lambda v: (C.c_int * len(v))(*v) if v is not None else None
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    side = lambda s: (ints(s.rows), C.c_float(s.floor or 0.0), int(s.floor is not None))
+    a_rows, a_floor, a_norm = side(a)
+    b_rows, b_floor, b_norm = side(b) if b is not None else (None, C.c_float(0.0), 0)
+    with torch.cuda.device(dev):
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        _lib.check(lib.sce_similarity(
+            aw.data_ptr(), Ma, na, a_rows, a_floor, a_norm, ptr(bw), Mb, nb, b_rows, b_floor, b_norm, d,
+            pv.numpy().ctypes.data_as(C.c_void_p), P, _lib.ARITH_CODE[arith], ptr(row_max), ptr(col_max), ptr(cap),
+            ws_ptr, need, stream), "sce_similarity")
+    return row_max, col_max, cap
+
+
+def _pair_list(pairs, Ma, Mb, same):
+    if isinstance(pairs, str):
+        if pairs == "lower":
+            if not same:
+                raise ValueError('pairs="lower" compares the models of one stack with each other: pass b=None')
+            return [(i, j) for i in range(Ma) for j in range(i)]
+        if pairs == "all":
+            return [(i, j) for i in range(Ma) for j in range(Mb)]
+        raise ValueError(f'pairs must be "lower", "all" or a list of (i, j), got {pairs!r}')
+    return [(int(i), int(j)) for i, j in torch.as_tensor(pairs).reshape(-1, 2).tolist()]
+
+
+def _valid_mean(v: torch.Tensor, rows) -> torch.Tensor:
+    """Mean of each row of ``v`` [P, n] over its first ``rows[p]`` entries."""
+    r = torch.as_tensor(rows, device=v.device).reshape(-1, 1)
+    mask = torch.arange(v.shape[1], device=v.device)[None, :] < r
+    return torch.where(mask, v, torch.zeros((), device=v.device)).sum(dim=1) / r.reshape(-1).to(v.dtype)
+
+
+def dictionary_similarity(a, b=None, pairs="lower", arith: str = "auto") -> Dict[str, torch.Tensor]:
+    """Cosine maxima of every chosen pair of dictionaries in one launch (the grids of big_sweep.py:108-138 and of the
+    plotting scripts). ``a`` / ``b``: FunctionalEnsembles, lists of LearnedDicts (dictionaries of different sizes are
+    zero-padded and masked) or tensors [M, n, d] / [n, d] taken as given (a raw truth matrix). ``b=None`` compares
+    ``a`` with itself. ``pairs``: "lower" (i > j, b=None), "all" (every (i, j)) or a list of (i, j).
+
+    Returns, on the device of ``a``:
+      ``pairs``  [P, 2] (int64)
+      ``mcs_ab`` [P, na]: for each atom of a[i] its best cosine in b[j] (``mcs_duplicates(b[j], a[i])``)
+      ``mcs_ba`` [P, nb]: for each atom of b[j] its best cosine in a[i] (``mcs_duplicates(a[i], b[j])``)
+      ``mmcs``   [Ma, Mb]: mmcs[i, j] = mean of mcs_ab over the atoms of a[i]; with b=None also mmcs[j, i] = mean of
+                 mcs_ba for each pair (i, j) whose mirror is not itself a pair. Entries no pair covers are NaN.
+    Entries of atoms beyond a model's dictionary size are NaN."""
+    A = _as_stack(a)
+    B = _as_stack(b) if b is not None else None
+    Mb = B.models if B is not None else A.models
+    plist = _pair_list(pairs, A.models, Mb, B is None)
+    if not plist:
+        raise ValueError("no pairs to compare")
+    row_max, col_max, _ = _run_similarity(A, B, plist, arith=arith)
+    dev = row_max.device
+    pt = torch.tensor(plist, dtype=torch.long)
+    na, nb = row_max.shape[1], col_max.shape[1]
+    ra = A.rows or [na] * A.models
+    rb = (B.rows or [nb] * B.models) if B is not None else ra
+    mean_ab = _valid_mean(row_max, [ra[i] for i, _ in plist])
+    mean_ba = _valid_mean(col_max, [rb[j] for _, j in plist])
+    mm = torch.full((A.models, Mb), float("nan"), dtype=torch.float32, device=dev)
+    ii, jj = pt[:, 0].to(dev), pt[:, 1].to(dev)
+    if B is None:
+        covered = set(plist)
+        mirror = torch.tensor([(j, i) not in covered for i, j in plist], device=dev)
+        mm[jj[mirror], ii[mirror]] = mean_ba[mirror]
+    mm[ii, jj] = mean_ab
+    out_dev = _input_device(a)
+    return {"pairs": pt.to(out_dev), "mcs_ab": row_max.to(out_dev), "mcs_ba": col_max.to(out_dev), "mmcs": mm.to(out_dev)}
+
+
+def capacity(a, arith: str = "auto") -> torch.Tensor:
+    """capacity_per_feature (standard_metrics.py:356-362, Scherlis et al. 2022) of every model of ``a`` (as in
+    :func:`dictionary_similarity`): [M, n], NaN beyond a model's dictionary size and for zero rows (as the reference)."""
+    A = _as_stack(a)
+    _, _, cap = _run_similarity(A, None, [(m, m) for m in range(A.models)], row=False, col=False, capacity=True,
+                                arith=arith)
+    return cap.to(_input_device(a))
+
+
+def _input_device(x):
+    if hasattr(x, "sig") and hasattr(x, "params"):
+        return torch.device(x.device)
+    if torch.is_tensor(x):
+        return x.device
+    if isinstance(x, (list, tuple)):
+        return _input_device(x[0])
+    return _ld_matrix(x)[0].device
+
+
+# drop-ins with the reference's names, argument order and results (standard_metrics.py:270-303, 356-362); ``arith``
+# is the engine's operand arithmetic (sce_arith)
+def mcs_duplicates(ground, model, arith: str = "auto") -> torch.Tensor:
+    """For each atom of ``model``, its largest cosine with an atom of ``ground``: [n_model]."""
+    rm, _, _ = _run_similarity(_as_stack(model), _as_stack(ground), [(0, 0)], col=False, arith=arith)
+    return rm[0].to(_input_device(model))
+
+
+def mmcs(model, model2, arith: str = "auto") -> torch.Tensor:
+    return mcs_duplicates(model, model2, arith=arith).mean()
+
+
+def mcs_to_fixed(model, truth: torch.Tensor, arith: str = "auto") -> torch.Tensor:
+    """For each atom of ``model``, its largest dot product with a row of ``truth`` as given (not normalised)."""
+    rm, _, _ = _run_similarity(_as_stack(model), _Stack(truth[None], None, None), [(0, 0)], col=False, arith=arith)
+    return rm[0].to(_input_device(model))
+
+
+def mmcs_to_fixed(model, truth: torch.Tensor, arith: str = "auto") -> torch.Tensor:
+    return mcs_to_fixed(model, truth, arith=arith).mean()
+
+
+def mmcs_from_list(ld_list, arith: str = "auto") -> torch.Tensor:
+    """[n, n]: 1 on the diagonal, [i, j] = [j, i] = mmcs(ld_list[i], ld_list[j]) for j < i."""
+    n = len(ld_list)
+    dev = _input_device(ld_list)
+    out = torch.eye(n, device=dev)
+    if n < 2:
+        return out
+    res = dictionary_similarity(list(ld_list), None, pairs="lower", arith=arith)
+    sizes = [(ld if torch.is_tensor(ld) else _ld_matrix(ld)[0]).shape[0] for ld in ld_list]
+    # mmcs(ld[i], ld[j]) averages, over the atoms of ld[j], their best match in ld[i]: the column maxima of (i, j)
+    vals = _valid_mean(res["mcs_ba"].to(dev), [sizes[j] for _, j in res["pairs"].tolist()])
+    p = res["pairs"].to(dev)
+    out[p[:, 0], p[:, 1]] = vals
+    out[p[:, 1], p[:, 0]] = vals
+    return out
+
+
+def representedness(features: torch.Tensor, model, arith: str = "auto") -> torch.Tensor:
+    """For each row of ``features`` (as given), its largest dot product with an atom of ``model``: [n_features]."""
+    rm, _, _ = _run_similarity(_Stack(features[None], None, None), _as_stack(model), [(0, 0)], col=False, arith=arith)
+    return rm[0].to(features.device)
+
+
+def capacity_per_feature(model, arith: str = "auto") -> torch.Tensor:
+    return capacity(model, arith=arith)[0]

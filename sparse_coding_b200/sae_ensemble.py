@@ -18,7 +18,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from .learned_dict import TiedSAE, UntiedSAE
+from .learned_dict import NORM_FLOOR, TiedSAE, UntiedSAE
 from .signatures import DictSignature, engine_loss
 
 _REF_MODULE = "autoencoders.sae_ensemble"
@@ -48,6 +48,10 @@ class FunctionalSAE(DictSignature):
     @staticmethod
     def to_learned_dict(params, buffers):
         return UntiedSAE(params["encoder"], params["decoder"], params["encoder_bias"])
+
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["decoder"], NORM_FLOOR, None
 
     @staticmethod
     def encode(params, buffers, batch):
@@ -83,6 +87,10 @@ class FunctionalTiedSAE(DictSignature):
         return TiedSAE(params["encoder"], params["encoder_bias"],
                        centering=(buffers["center_trans"], buffers["center_rot"], buffers["center_scale"]),
                        norm_encoder=True)
+
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["encoder"], NORM_FLOOR, None
 
     @staticmethod
     def center(buffers, batch):
@@ -129,6 +137,10 @@ class FunctionalMaskedTiedSAE(DictSignature):
         return TiedSAE(params["encoder"][:k], params["encoder_bias"][:k], norm_encoder=True)
 
     @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["encoder"], NORM_FLOOR, buffers["dict_size"]
+
+    @staticmethod
     def loss(params, buffers, batch):
         return engine_loss(FunctionalMaskedTiedSAE, params, buffers, batch)
 
@@ -151,6 +163,10 @@ class FunctionalMaskedSAE(DictSignature):
     def to_learned_dict(params, buffers):
         k = buffers["dict_size"].item()
         return UntiedSAE(params["encoder"][:k], params["decoder"][:k], params["encoder_bias"][:k])
+
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["decoder"], NORM_FLOOR, buffers["dict_size"]
 
     @staticmethod
     def loss(params, buffers, batch):

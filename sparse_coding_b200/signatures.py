@@ -24,6 +24,14 @@ class DictSignature:
     def loss(params, buffers, batch):
         pass
 
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        """The stacked learned dictionaries of an ensemble as ``(matrix [M, n, d], norm_floor, rows)``: what
+        ``to_learned_dict(...).get_learned_dict()`` returns per model is ``matrix[m, :rows[m]]`` with every row divided
+        by ``max(||row||, norm_floor)`` (``norm_floor <= 0``: no clamp; ``None``: not normalised); ``rows`` is a [M]
+        tensor, or None when every model uses all ``n`` rows. Read by ``metrics.dictionary_similarity``."""
+        raise NotImplementedError("this signature does not describe its learned dictionary")
+
 
 DictSignature.__module__ = "autoencoders.ensemble"
 

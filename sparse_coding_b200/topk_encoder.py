@@ -75,6 +75,10 @@ class TopKEncoder(DictSignature):
     def to_learned_dict(params, buffers):
         return TopKLearnedDict(_unit_norm_rows(params["dict"]), buffers["sparsity"].item())
 
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["dict"], 0.0, None   # unit rows without a clamp (_unit_norm_rows)
+
 
 for _cls in (TopKEncoder, TopKLearnedDict):
     _cls.__module__ = _REF_MODULE

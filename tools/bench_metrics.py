@@ -1,0 +1,149 @@
+#!/usr/bin/env python
+"""Dictionary-similarity metrics (standard_metrics.py mmcs / mcs_duplicates / capacity_per_feature) on the engine against
+the reference's op sequence on the same GPU. One metric pass = the cosine maxima of every pair in both directions plus
+the capacity of every dictionary.
+
+    python tools/bench_metrics.py --workload mmcs_cfg2 [--steps K --warmup W --arith auto|bf16x3|f16f8]
+
+Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
+computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
+the card name and power limit read in the same call. Writes nothing to disk."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def make_models(sig, M, d, n, seed):
+    """M seeded TiedSAEs with L1 = logspace(-4, -2, M), as bench.py builds config 2."""
+    torch.manual_seed(seed)
+    return [sig.init(d, n, float(a)) for a in (np.logspace(-4, -2, M) if M > 1 else [1e-3])]
+
+
+MMCS_WORKLOADS = {
+    # name: (M, n, d, pairs, description)
+    "mmcs_cfg2": (16, 4096, 512, "lower", "16 seeded config-2 TiedSAE dictionaries (4096 x 512): all 120 lower-triangle "
+                                          "pairs, both directions, plus capacity of all 16"),
+    "mmcs_cfg5": (2, 32768, 2048, [(1, 0)], "two config-5 TiedSAE dictionaries (32768 x 2048): one pair, both "
+                                            "directions, plus capacity of each"),
+}
+
+
+def card_info(index):
+    """(name, power limit in W) of the GPU, read in the same call as the measurement."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        name, limit = [s.strip() for s in r.stdout.strip().split(",")[:2]]
+        return name, float(limit)
+    except Exception:
+        return torch.cuda.get_device_name(index), None
+
+
+def run_mmcs(args):
+    """Dictionary-similarity workloads (standard_metrics.py mmcs / mcs_duplicates / capacity_per_feature): one metric
+    pass = the cosine maxima of every pair in both directions plus the capacity of every dictionary, on the engine and
+    as the reference's op sequence (fp32 einsum + maxima per pair) on the same GPU, fp32 and TF32."""
+    import sparse_coding_b200 as S
+    from oracle import metrics_oracle as O
+    from sparse_coding_b200 import metrics as MT
+
+    if not torch.cuda.is_available():
+        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    M, n, d, pairs, desc = MMCS_WORKLOADS[args.workload]
+    ens = S.FunctionalEnsemble(make_models(S.FunctionalTiedSAE, M, d, n, seed=0), S.FunctionalTiedSAE, S.adam,
+                               {"lr": 1e-3}, device=dev)
+    plist = [(i, j) for i in range(M) for j in range(i)] if pairs == "lower" else pairs
+    K, W = args.steps, max(args.warmup, 1)
+    if K < 1:
+        raise SystemExit("--steps must be at least 1")
+
+    def engine_pass():
+        return MT.dictionary_similarity(ens, pairs=plist, arith=args.arith), MT.capacity(ens, arith=args.arith)
+
+    def timed(fn, k, w):
+        for _ in range(w):
+            r = fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(k):
+            r = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / k, r
+
+    ms, (res, cap) = timed(engine_pass, K, W)
+    L = [ens.sig.to_learned_dict(p, b).get_learned_dict() for p, b in ens.unstack()]   # torch, fp32
+
+    def stock_pass():
+        rows, cols, caps = [], [], []
+        for i, j in plist:
+            s = torch.einsum("md,gd->mg", L[i], L[j])
+            rows.append(s.max(dim=-1).values)
+            cols.append(s.max(dim=0).values)
+        for l in L:
+            s = torch.einsum("md,nd->mn", l, l).pow(2)
+            caps.append(torch.diag(s) / s.sum(dim=-1))
+        return torch.stack(rows), torch.stack(cols), torch.stack(caps)
+
+    k_ref = max(1, min(K, 3))
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    try:
+        torch.backends.cuda.matmul.allow_tf32 = False
+        ms_fp32, ref32 = timed(stock_pass, k_ref, 1)
+        torch.backends.cuda.matmul.allow_tf32 = True
+        ms_tf32, reftf = timed(stock_pass, k_ref, 1)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+
+    # deviation of each from the fp64 result
+    L64 = [l.double() for l in L]
+    exact = [O.pair_maxima(L64[i], L64[j]) for i, j in plist]
+    r64 = torch.stack([e[0] for e in exact])
+    c64 = torch.stack([e[1] for e in exact])
+    cap64 = torch.stack([O.capacity_blocked(l) for l in L64])
+
+    def dev_of(rows, cols, caps):
+        return {"cos_max_abs": float(max((rows.double() - r64).abs().max(), (cols.double() - c64).abs().max())),
+                "capacity_max_rel": float(((caps.double() - cap64).abs() / cap64.abs()).max())}
+
+    flops = 2.0 * n * n * d * (len(plist) + M)      # algorithmic: one [n, d] x [d, n] product per pair and per capacity
+    name, limit = card_info(0)
+    print(json.dumps({
+        "metric": "ms per metric pass (dictionary similarity + capacity)", "workload": args.workload, "desc": desc,
+        "value": ms, "unit": "ms", "pairs": len(plist), "dictionaries": M, "n": n, "d": d,
+        "arith": args.arith, "steps": K, "warmup": W,
+        "tflops_algorithmic": flops / (ms * 1e-3) / 1e12,
+        "deviation_from_fp64": dev_of(res["mcs_ab"], res["mcs_ba"], cap),
+        "stock_torch_gpu": {
+            "fp32": {"ms": ms_fp32, "tflops_algorithmic": flops / (ms_fp32 * 1e-3) / 1e12,
+                     "deviation_from_fp64": dev_of(*ref32)},
+            "tf32": {"ms": ms_tf32, "tflops_algorithmic": flops / (ms_tf32 * 1e-3) / 1e12,
+                     "deviation_from_fp64": dev_of(*reftf)},
+            "passes_timed": k_ref},
+        "speedup_vs_stock_fp32": ms_fp32 / ms, "speedup_vs_stock_tf32": ms_tf32 / ms,
+        "gpu": name, "power_limit_w": limit,
+    }), flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="mmcs_cfg2", choices=sorted(MMCS_WORKLOADS))
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
+    run_mmcs(ap.parse_args())
+
+
+if __name__ == "__main__":
+    main()

@@ -197,6 +197,28 @@ int sce_clear_health(sce_plan* plan, void* stream);
  * epilogue / top-k selection wrote (B/8 bytes per feature chunk): the dense code is never materialised. */
 int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream);
 
+/* Evaluation of a set of activations (standard_metrics.py:305-314 fraction_variance_unexplained /
+ * mean_nonzero_activations, :446-454 batched_calc_feature_n_ever_active, :482-511 calc_moments_streaming): sce_forward,
+ * plus per-feature statistics of the code c [M,B,n], without ever materialising it.
+ *   moment_sums  device fp64 [M,n,4], ACCUMULATED: += sum over the B rows of c, c^2, c^3, c^4 per feature. The encode
+ *                epilogue (SAE variants) or a pass over the top-k scores and activity mask (TOPK) sums 32 rows in fp32 from
+ *                the exact fp32 code; those partials are added over the rows in a fixed order in fp64: bitwise repeatable.
+ *   seg_counts   device int32 [M,n], ACCUMULATED: += number of segments of `seg` rows, ending in this call, in which the
+ *                feature is non-zero on some row. seg = 1: rows, exactly as sce_active_counts.
+ *   seg_phase    rows of the first segment that earlier calls already saw, in [0, seg)
+ *   seg_open     device int32 [M,n] (seg > 1; may be NULL for seg = 1): 1 where the feature fired in the segment that
+ *                is still open; read at the start, written at the end, so a segment may span any number of calls
+ *                (zero it before the first call)
+ *   workspace    >= sce_forward_stats_workspace_bytes(desc, B), 1024-byte aligned: the moment partials,
+ *                M * ceil(B/32) * 4 * n fp32 (config 2, M = 16, n = 4096, B = 8192: 256 MiB; M = 1, n = 32768,
+ *                B = 4096: 64 MiB). sce_forward_stats_workspace_bytes is host-only; it returns 0 for an invalid
+ *                desc or B outside [1, batch_max].
+ * x_hat, out_losses and out_nnz are those of sce_forward (x_hat optional). Asynchronous on `stream`. */
+size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B);
+int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
+                      float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 /* The arithmetic the plan resolved to: SCE_ARITH_BF16X3 or SCE_ARITH_F16F8. */
 int sce_plan_arith(const sce_plan* plan);
 

@@ -5,6 +5,8 @@ DictSignature / FunctionalEnsemble (ensemble.py), FunctionalSAE / FunctionalTied
 (sae_ensemble.py), TopKEncoder / TopKLearnedDict (topk_encoder.py), LearnedDict / TiedSAE / UntiedSAE
 (learned_dict.py), plus the driver loop pieces of big_sweep.py (train_loop.py) and on-device metrics (metrics.py)."""
 from . import metrics
+from .metrics import (batched_calc_feature_n_ever_active, calc_moments_streaming, evaluate_dicts,
+                      fraction_variance_unexplained, mean_nonzero_activations, r_squared)
 from .ensemble import CodeProxy, FunctionalEnsemble, optim_str_to_func, stack_dict, unstack_dict
 from .learned_dict import LearnedDict, TiedSAE, UntiedSAE
 from .optim import AdamConfig, adam
@@ -15,5 +17,7 @@ from .topk_encoder import TopKEncoder, TopKLearnedDict
 __all__ = [
     "AdamConfig", "CodeProxy", "DictSignature", "FunctionalEnsemble", "FunctionalMaskedSAE", "FunctionalMaskedTiedSAE",
     "FunctionalSAE", "FunctionalTiedSAE", "LearnedDict", "TiedSAE", "TopKEncoder", "TopKLearnedDict", "UntiedSAE",
-    "adam", "optim_str_to_func", "stack_dict", "unstack_dict",
+    "adam", "batched_calc_feature_n_ever_active", "calc_moments_streaming", "evaluate_dicts",
+    "fraction_variance_unexplained", "mean_nonzero_activations", "optim_str_to_func", "r_squared", "stack_dict",
+    "unstack_dict",
 ]

@@ -25,7 +25,7 @@ EXPORTS = [
     "sce_step", "sce_step_host", "sce_forward", "sce_read_code", "sce_grads", "sce_gather_rows",
     "sce_last_launch_count", "sce_get_step_count", "sce_set_step_count", "sce_profile_begin", "sce_profile_end",
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
-    "sce_similarity_workspace_bytes", "sce_similarity",
+    "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -97,6 +97,9 @@ def load():
     lib.sce_similarity_workspace_bytes.argtypes = [i, i, i, i, i, i, i]
     f = C.c_float
     lib.sce_similarity.argtypes = [vp, i, i, vp, f, i, vp, i, i, vp, f, i, i, vp, i, i, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_forward_stats_workspace_bytes.restype = C.c_size_t
+    lib.sce_forward_stats_workspace_bytes.argtypes = [C.POINTER(SceDesc), i]
+    lib.sce_forward_stats.argtypes = [vp, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

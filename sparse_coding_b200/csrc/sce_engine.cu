@@ -560,9 +560,10 @@ __global__ void l1_over_b_kernel(const float* __restrict__ alpha, float* __restr
 }
 
 // forward (+ optional backward GEMMs). Leaves dW in p->dw_enc / p->dw_dec when `backward`.
+// `mom_part` (forward only, SAE variants): the encode epilogue also writes the moment partials of EpiEncodeT<AR, true>.
 template <int AR>
 static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool backward, float* out_losses,
-                          float* out_nnz, cudaStream_t st) {
+                          float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
   using EpiEnc = EpiEncodeT<AR>;
   using EpiDec = EpiDecodeT<AR>;
   using EpiDco = EpiDcodeT<AR>;
@@ -632,21 +633,33 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   int n_enc_parts;
   TopkLists tk = {nullptr, nullptr, nullptr, 0, 0};
   if (d.variant != SCE_TOPK) {
-    typename EpiEnc::Params ep;
-    ep.out_hi = maps->st_c_hi;
-    ep.out_lo = maps->st_c_lo;
-    ep.out_x8 = maps->st_c_x8;
-    ep.bias = p->b.encoder_bias;
-    ep.mask = p->b.coef_mask;
-    ep.part = p->part_enc;
-    ep.tiles_m = tiles_mB;
-    ep.flag_zero = 1;
-    ep.act = act;
-    ep.tiles_n = (n + kBN - 1) / kBN;
-    rc = launch_k<EpiEnc, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+    auto fill = [&](auto& ep) {
+      ep.out_hi = maps->st_c_hi;
+      ep.out_lo = maps->st_c_lo;
+      ep.out_x8 = maps->st_c_x8;
+      ep.bias = p->b.encoder_bias;
+      ep.mask = p->b.coef_mask;
+      ep.part = p->part_enc;
+      ep.tiles_m = tiles_mB;
+      ep.flag_zero = 1;
+      ep.act = act;
+      ep.tiles_n = (n + kBN - 1) / kBN;
+    };
+    if (mom_part) {
+      using EpiStats = EpiEncodeT<AR, true>;
+      typename EpiStats::Params ep;
+      fill(ep);
+      ep.mom_part = mom_part;
+      ep.row_blocks = (B + 31) / 32;
+      rc = launch_k<EpiStats, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+    } else {
+      typename EpiEnc::Params ep;
+      fill(ep);
+      rc = launch_k<EpiEnc, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+    }
     if (rc) return rc;
     ++launches;
-    n_enc_parts = tiles_mB * 8 * ep.tiles_n;
+    n_enc_parts = tiles_mB * 8 * ((n + kBN - 1) / kBN);
   } else {
     // scores -> fp32, then per-row selection (code planes, activity mask, k-sparse lists)
     EpiScoresTma::Params sp;
@@ -789,9 +802,109 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
 }
 
 static int run_pipeline(sce_plan* p, const float* x, int B, float* x_hat, bool backward, float* out_losses,
-                        float* out_nnz, cudaStream_t st) {
-  return p->arith == kArithF16F8 ? run_pipeline_t<kArithF16F8>(p, x, B, x_hat, backward, out_losses, out_nnz, st)
-                                 : run_pipeline_t<kArithBf16x3>(p, x, B, x_hat, backward, out_losses, out_nnz, st);
+                        float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
+  return p->arith == kArithF16F8 ? run_pipeline_t<kArithF16F8>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part)
+                                 : run_pipeline_t<kArithBf16x3>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
+}
+
+// ------------------------------------------------------------------------------------------------
+// evaluation statistics (sce_forward_stats): per-feature moments and segment activity counts
+// ------------------------------------------------------------------------------------------------
+// Top-k plans: moment partials from the fp32 scores and the activity mask the selection left in the workspace, in the
+// layout of EncodeMomentParams ([M][row_blocks][4][n]): the code is relu(score) where the mask bit is set, 0 elsewhere.
+// One warp per (32-column chunk, row block): lane j sums column 32 chunk + j over the 32 rows in order.
+__global__ void __launch_bounds__(256) topk_moment_kernel(const float* __restrict__ scores, const uint32_t* __restrict__ pos,
+                                                          int n_chunks, int batch_max, int B, int n, int row_blocks,
+                                                          float* __restrict__ part) {
+  const int chunk = blockIdx.x, model = blockIdx.z, lane = threadIdx.x & 31;
+  const int rb = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (rb >= row_blocks) return;
+  const int col = chunk * 32 + lane;
+  const uint32_t* pw = pos + ((long long)model * n_chunks + chunk) * batch_max;
+  const float* s = scores + (long long)model * batch_max * n;
+  float a1 = 0.f, a2 = 0.f, a3 = 0.f, a4 = 0.f;
+  const int r_end = min(B, rb * 32 + 32);
+  for (int r = rb * 32; r < r_end; ++r) {
+    const uint32_t w = __ldg(pw + r);
+    if (col < n && ((w >> (31 - lane)) & 1u)) {
+      const float c = fmaxf(__ldg(s + (long long)r * n + col), 0.f), c2 = c * c;
+      a1 += c;
+      a2 += c2;
+      a3 += c2 * c;
+      a4 += c2 * c2;
+    }
+  }
+  if (col < n) {
+    float* o = part + ((long long)model * row_blocks + rb) * 4 * n + col;
+    o[0] = a1;
+    o[n] = a2;
+    o[2 * (long long)n] = a3;
+    o[3 * (long long)n] = a4;
+  }
+}
+
+// sums[m][j][p] += sum over the row blocks, in order, of part[m][rb][p][j] (fp64): bitwise repeatable, no atomics
+__global__ void moment_reduce_kernel(const float* __restrict__ part, int row_blocks, int n, double* __restrict__ sums) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x, model = blockIdx.y;
+  if (col >= n) return;
+  double a[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int rb = 0; rb < row_blocks; ++rb) {
+    const float* o = part + ((long long)model * row_blocks + rb) * 4 * n + col;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) a[q] += (double)__ldg(o + (long long)q * n);
+  }
+  double* out = sums + ((long long)model * n + col) * 4;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) out[q] += a[q];
+}
+
+// Segment activity counts (calc_moments_streaming's times_active, standard_metrics.py:482-511): the rows are cut into
+// segments of `seg`; counts[m][j] += number of segments that END in this call in which some row has [c > 0] in column j.
+// `phase` rows of the first segment were seen by earlier calls, whose activity is carried in open[m][j] (0 / 1); the
+// flag of a segment that stays open past this call is written back there. One block per (32-column chunk, model); warp
+// w takes the segments w, w + 8, ...; lanes OR 32 rows' mask words at a time, so lane j ends with column j's flag.
+__global__ void __launch_bounds__(256) segment_count_kernel(const uint32_t* __restrict__ pos, int n_chunks, int batch_max,
+                                                            int B, int n, int seg, int phase, int* __restrict__ counts,
+                                                            int* __restrict__ open) {
+  __shared__ int red[8][32];
+  const int chunk = blockIdx.x, model = blockIdx.y;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t* p = pos + ((long long)model * n_chunks + chunk) * batch_max;
+  const int col = chunk * 32 + lane;
+  const long long oi = (long long)model * n + col;
+  const int carried = col < n ? open[oi] : 0;
+  __syncthreads();   // every read of open[] precedes the write below
+  const long long K = ((long long)B + phase + seg - 1) / seg;   // segments this call touches
+  int mine = 0;
+  for (long long k = warp; k < K; k += 8) {
+    const long long lo = k == 0 ? 0 : k * seg - phase;
+    const long long end = (k + 1) * seg - phase;
+    const long long hi = end < B ? end : B;
+    uint32_t any = 0u;
+    for (long long r = lo + lane; r < hi; r += 32) any |= __ldg(p + r);
+    any = __reduce_or_sync(0xffffffffu, any);
+    int act = (int)((any >> (31 - lane)) & 1u);
+    if (k == 0) act |= carried;
+    if (end <= B) {
+      mine += act;
+      if (k == K - 1 && col < n) open[oi] = 0;
+    } else if (col < n) {
+      open[oi] = act;   // (only the last segment can stay open)
+    }
+  }
+  red[warp][lane] = mine;
+  __syncthreads();
+  if (warp == 0) {
+    int t = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += red[i][lane];
+    if (col < n) counts[oi] += t;
+  }
+}
+
+// moment partials of one forward call: [M][ceil(B / 32)][4][n] fp32
+static size_t stats_workspace(const sce_desc& d, int B) {
+  return align_up((size_t)d.n_models * ((B + 31) / 32) * 4 * d.n * sizeof(float), 1024);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1359,6 +1472,50 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
   const int n_chunks = (plan->d.n + 31) / 32;
   active_count_kernel<<<dim3(n_chunks, plan->d.n_models), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       plan->act_pos, n_chunks, plan->d.batch_max, B, plan->d.n, counts);
+  CUDA_TRY(cudaGetLastError());
+  return SCE_OK;
+}
+
+size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
+  if (validate(desc) || B < 1 || B > desc->batch_max) return 0;
+  return stats_workspace(*desc, B);
+}
+
+int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
+                      float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  if (!p) return fail(SCE_ERR_INVALID, "forward_stats: plan is NULL");
+  if (B < 1 || B > p->d.batch_max) return fail(SCE_ERR_INVALID, "forward_stats: B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (!x) return fail(SCE_ERR_INVALID, "forward_stats: x is NULL");
+  if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
+  if (seg_phase < 0 || seg_phase >= seg)
+    return fail(SCE_ERR_INVALID, "forward_stats: seg_phase = %d outside [0, seg = %d)", seg_phase, seg);
+  if (!out_losses || !out_nnz || !moment_sums || !seg_counts)
+    return fail(SCE_ERR_INVALID, "forward_stats: out_losses, out_nnz, moment_sums and seg_counts are required");
+  if (seg > 1 && !seg_open) return fail(SCE_ERR_INVALID, "forward_stats: seg > 1 needs the seg_open flags");
+  const size_t need = stats_workspace(p->d, B);
+  if (!workspace || workspace_bytes < need)
+    return fail(SCE_ERR_WORKSPACE, "forward_stats: workspace too small: have %zu bytes, need %zu", workspace_bytes, need);
+  if (reinterpret_cast<uintptr_t>(workspace) % 1024) return fail(SCE_ERR_WORKSPACE, "forward_stats: workspace must be 1024-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const sce_desc& d = p->d;
+  const bool topk = d.variant == SCE_TOPK;
+  float* part = static_cast<float*>(workspace);
+  int rc = run_pipeline(p, x, B, x_hat, false, out_losses, out_nnz, st, topk ? nullptr : part);
+  if (rc) return rc;
+  const int n_chunks = (d.n + 31) / 32, row_blocks = (B + 31) / 32;
+  if (topk) {
+    topk_moment_kernel<<<dim3(n_chunks, (row_blocks + 7) / 8, d.n_models), 256, 0, st>>>(p->scores, p->act_pos, n_chunks,
+                                                                                        d.batch_max, B, d.n, row_blocks, part);
+    CUDA_TRY(cudaGetLastError());
+  }
+  moment_reduce_kernel<<<dim3((d.n + 255) / 256, d.n_models), 256, 0, st>>>(part, row_blocks, d.n, moment_sums);
+  CUDA_TRY(cudaGetLastError());
+  if (seg == 1)
+    active_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, seg_counts);
+  else
+    segment_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, seg,
+                                                                     seg_phase, seg_counts, seg_open);
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }

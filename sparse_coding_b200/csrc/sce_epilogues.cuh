@@ -186,17 +186,45 @@ struct ActMask {
   }
 };
 
+// transpose-reduce: 32 lanes x 32 columns -> lane j holds the sum of column j over the warp's rows (31 shuffles)
+__device__ __forceinline__ float warp_column_sum(float (&v)[32], int lane) {
+#pragma unroll
+  for (int half = 16; half >= 1; half >>= 1) {
+    const bool upper = (lane & half) != 0;
+#pragma unroll
+    for (int i = 0; i < half; ++i) {
+      const float send = upper ? v[i] : v[i + half];
+      const float keep = upper ? v[i + half] : v[i];
+      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
+    }
+  }
+  return v[0];
+}
+
+// Per-feature moments of the code (EpiEncodeT<ARITH, true>, evaluation only): each epilogue warp writes the column sums
+// of c, c^2, c^3, c^4 over its 32 rows as fp32 partials [M][row_blocks][4][n], row block = global row / 32; a second
+// kernel (moment_reduce_kernel) adds them up over the row blocks in a fixed order in fp64.
+template <bool STATS>
+struct EncodeMomentParams {};
+template <>
+struct EncodeMomentParams<true> {
+  float* mom_part;   // [M][row_blocks][4][n]
+  int row_blocks;    // ceil(B / 32)
+};
+
 // ------------------------------------------------------------------------------------------------
 // encode:  c = relu(acc + bias) -> (c_hi, c_lo);  per-tile partial sums of |c| and count(c > 0)
 // [c > 0] and [z == 0] (clamp(min=0)'s gradient of 1 at exactly 0, SURVEY.md Q4) go to the activity masks, so the
 // backward pass needs neither z nor the code.
+// STATS (compile-time, evaluation only) adds the moment partials of EncodeMomentParams; the training instantiations
+// (STATS = false) compile to the same code as without the switch.
 // ------------------------------------------------------------------------------------------------
-template <int ARITH>
+template <int ARITH, bool STATS = false>
 struct EpiEncodeT {
   static constexpr int kCols = 32;
   static constexpr bool kPairChunks = ARITH == kArithF16F8 && SCE_EPI_PAIR != 0;
   static constexpr int kWarpStageBytes = kPairChunks ? kPairStageBytes : 4096;
-  struct Params {
+  struct Params : EncodeMomentParams<STATS> {
     CUtensorMap out_hi, out_lo, out_x8;  // store maps of the code planes: [M][B][n], box 32 x 32
     const float* bias;             // [M, n] or nullptr
     const unsigned char* mask;     // [M, n] (1 = coefficient unused) or nullptr
@@ -222,6 +250,7 @@ struct EpiEncodeT {
     const float* bias = P.bias ? P.bias + (long long)T.model * n_total + col : nullptr;
     float ls = 0.f;
     uint32_t pos = 0, zero = 0;   // activity-mask words of this row and chunk: bit (31 - j) is column j
+    float cs[32];                 // STATS: the code of this row's chunk, 0 for rows beyond the batch
     if (col + 32 <= n_total && !P.mask && bias) {
       // fast path: whole chunk in range, no coefficient mask; bias fetched as 8 uniform float4.
       // Lean on purpose (this GEMM is bound by the SM's data paths, not by the tensor pipe): relu as max, the sign
@@ -240,6 +269,10 @@ struct EpiEncodeT {
           const float c0 = fmaxf(z0, 0.f), c1 = fmaxf(z1, 0.f);
           split_pair<ARITH>(c0, c1, (j + u) >> 1, whi, wlo);
           ls += c0 + c1;
+          if constexpr (STATS) {
+            cs[j + u] = row_ok ? c0 : 0.f;
+            cs[j + u + 1] = row_ok ? c1 : 0.f;
+          }
         }
       }
       pos = ~neg;  // no zero among the 32 scores: positive <=> sign bit clear
@@ -267,6 +300,7 @@ struct EpiEncodeT {
           if (cv[u] > 0.f) pos |= 0x80000000u >> (j + u);
           if (P.flag_zero && z == 0.f && !masked) zero |= 0x80000000u >> (j + u);
           ls += cv[u];
+          if constexpr (STATS) cs[j + u] = row_ok ? cv[u] : 0.f;
         }
         split_pair<ARITH>(cv[0], cv[1], j >> 1, whi, wlo);
       }
@@ -285,6 +319,23 @@ struct EpiEncodeT {
     } else {
       stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
                              T.m_blk * kBM + T.warp_q * 32, T.model);
+    }
+    if constexpr (STATS) {
+      if (T.m_blk * kBM + T.warp_q * 32 < m_total) {   // warp-uniform: some row of this warp is in the batch
+        float* o = P.mom_part + ((long long)T.model * P.row_blocks + T.m_blk * 4 + T.warp_q) * 4 * n_total + col + T.lane;
+        const bool col_ok = col + T.lane < n_total;
+#pragma unroll
+        for (int p = 0; p < 4; ++p) {
+          float v[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const float c = cs[j], c2 = c * c;
+            v[j] = p == 0 ? c : p == 1 ? c2 : p == 2 ? c2 * c : c2 * c2;
+          }
+          const float sum = warp_column_sum(v, T.lane);
+          if (col_ok) o[(long long)p * n_total] = sum;
+        }
+      }
     }
   }
   __device__ __forceinline__ void finish() {

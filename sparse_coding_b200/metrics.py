@@ -294,3 +294,305 @@ def representedness(features: torch.Tensor, model, arith: str = "auto") -> torch
 
 def capacity_per_feature(model, arith: str = "auto") -> torch.Tensor:
     return capacity(model, arith=arith)[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Scoring exported dictionaries on a set of activations (standard_metrics.py:305-314, 344-345, 446-454, 482-511): FVU,
+# activation counts and per-feature moments of every dictionary in one pass over the activations (libsce
+# ``sce_forward_stats``). Dictionaries of one kind, padded size, width and centring share one forward-only plan; the
+# code [B, n] exists only as the engine's operand planes, and the moments are summed from it in the encode epilogue.
+# ---------------------------------------------------------------------------------------------------------------------
+_EVAL_ROWS = 8192          # rows per engine call
+
+
+def _eval_kind(ld) -> str:
+    from .learned_dict import LearnedDict, TiedSAE, UntiedSAE
+    from .topk_encoder import TopKLearnedDict
+    if isinstance(ld, TiedSAE):
+        if not getattr(ld, "norm_encoder", True):
+            raise NotImplementedError("TiedSAE(norm_encoder=False) is not implemented in the engine: its encoder rows "
+                                      "are used unnormalised, which no engine variant computes")
+        return "tied"
+    if isinstance(ld, UntiedSAE):
+        return "untied"
+    if isinstance(ld, TopKLearnedDict):
+        return "topk"
+    name = type(ld).__name__ if isinstance(ld, LearnedDict) else repr(type(ld))
+    raise NotImplementedError(f"{name} has no engine variant: dictionary evaluation runs TiedSAE (norm_encoder=True), "
+                              "UntiedSAE and TopKLearnedDict, and has no slow path for other dictionaries")
+
+
+def _is_centred(ld) -> bool:
+    if hasattr(ld, "initialize_missing"):
+        ld.initialize_missing()
+    t, r, s = ld.center_trans, ld.center_rot, ld.center_scale
+    return not (bool((t == 0).all()) and bool((s == 1).all())
+                and bool((r == torch.eye(r.shape[0], device=r.device, dtype=r.dtype)).all()))
+
+
+def _eval_groups(lds, centre: bool, multiple: int):
+    """Input dictionaries -> ordered {(kind, padded n, d, centred): [input index, ...]}. ``multiple``: the padded
+    dictionary size is a multiple of it (8, or 16 for f16f8). Raises for what the engine does not run."""
+    groups = {}
+    for i, ld in enumerate(lds):
+        kind = _eval_kind(ld)
+        n, d = int(ld.n_feats), int(ld.activation_size)
+        if d % 8:
+            raise ValueError(f"dictionary {i}: activation width d = {d} must be a multiple of 8")
+        if kind == "topk" and n % multiple:
+            raise ValueError(f"dictionary {i}: a TopKLearnedDict needs n ({n}) to be a multiple of {multiple}: its rows "
+                             "are normalised without a clamp, so zero padding rows would become NaN")
+        n_pad = -(-n // multiple) * multiple
+        centred = centre and kind == "tied" and _is_centred(ld)
+        groups.setdefault((kind, n_pad, d, centred), []).append(i)
+    return groups
+
+
+class _EvalPlan:
+    """One forward-only plan for a group of dictionaries, with its statistics accumulators."""
+
+    def __init__(self, key, lds, batch_max, arith, dev):
+        import ctypes as C
+        from . import _lib
+        kind, n_pad, d, centred = key
+        M = len(lds)
+        self.kind, self.M, self.n, self.d, self.centred, self.dev = kind, M, n_pad, d, centred, dev
+        f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32)
+
+        def stack(ts):
+            out = torch.zeros((M, n_pad) + tuple(ts[0].shape[1:]), dtype=torch.float32, device=dev)
+            for m, t in enumerate(ts):
+                out[m, : t.shape[0]] = f32(t)
+            return out
+
+        t = {}
+        if kind == "topk":
+            t["enc"] = stack([ld.dict for ld in lds])
+            t["sparsity"] = torch.tensor([int(ld.sparsity) for ld in lds], dtype=torch.int64, device=dev)
+        else:
+            t["enc"] = stack([ld.encoder for ld in lds])
+            t["bias"] = stack([ld.encoder_bias for ld in lds])
+            if kind == "untied":
+                t["dec"] = stack([ld.decoder for ld in lds])
+            sizes = [int(ld.n_feats) for ld in lds]
+            if any(k < n_pad for k in sizes):       # padding rows: the masked variants' coef_mask (1 = unused)
+                t["mask"] = (torch.arange(n_pad, device=dev)[None, :] >= torch.tensor(sizes, device=dev)[:, None]).to(torch.uint8)
+        if centred:
+            self.trans = torch.stack([f32(ld.center_trans) for ld in lds]).contiguous()
+            self.rot = torch.stack([f32(ld.center_rot) for ld in lds]).contiguous()
+            self.scale = torch.stack([f32(ld.center_scale) for ld in lds]).contiguous()
+        # sce_prepare and sce_forward_stats never read the Adam moments; the plan only requires their pointers
+        t["unused"] = torch.zeros(1, dtype=torch.float32, device=dev)
+        self._t = t
+        lib = _lib.load()
+        desc = _lib.SceDesc(
+            variant={"tied": _lib.SCE_TIED, "untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK}[kind], n_models=M, d=d,
+            n=n_pad, batch_max=batch_max, x_per_model=int(centred), lr=0.0, beta1=0.9, beta2=0.999, eps=1e-8,
+            eps_root=0.0, adam_count_mode=_lib.SCE_ADAM_FROZEN_T1, fwd_passes=3, bwd_passes=3,
+            norm_floor=0.0 if kind == "topk" else 1e-8, arith=_lib.ARITH_CODE[arith],
+            topk_k_max=int(t["sparsity"].max()) if kind == "topk" else 0, centering=int(centred))
+        nbytes = lib.sce_workspace_bytes(C.byref(desc))
+        sbytes = lib.sce_forward_stats_workspace_bytes(C.byref(desc), batch_max)
+        if nbytes == 0 or sbytes == 0:
+            _lib.check(-1, "sce_workspace_bytes")
+        self._ws = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
+        self._sws = torch.empty(sbytes + 1024, dtype=torch.uint8, device=dev)
+        self.sws_ptr, self.sws_bytes = (self._sws.data_ptr() + 1023) // 1024 * 1024, sbytes
+        ptr = lambda x: x.data_ptr() if x is not None else None
+        u = ptr(t["unused"])
+        b = _lib.SceBuffers()
+        b.encoder, b.encoder_m, b.encoder_v = ptr(t["enc"]), u, u
+        if kind != "topk":
+            b.encoder_bias, b.bias_m, b.bias_v = ptr(t["bias"]), u, u
+        if kind == "untied":
+            b.decoder, b.decoder_m, b.decoder_v = ptr(t["dec"]), u, u
+        b.coef_mask = ptr(t.get("mask"))
+        b.sparsity = ptr(t.get("sparsity"))
+        if centred:
+            b.center_trans, b.center_rot, b.center_scale = ptr(self.trans), ptr(self.rot), ptr(self.scale)
+        b.workspace, b.workspace_bytes = (self._ws.data_ptr() + 1023) // 1024 * 1024, nbytes
+        self.plan = C.c_void_p()
+        _lib.check(lib.sce_plan_create(C.byref(desc), C.byref(b), C.byref(self.plan)), "sce_plan_create")
+        self.stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        try:
+            _lib.check(lib.sce_prepare(self.plan, self.stream), "sce_prepare")
+        except Exception:
+            self.close()
+            raise
+        z = lambda dt: torch.zeros(M, n_pad, dtype=dt, device=dev)
+        self.sums = torch.zeros(M, n_pad, 4, dtype=torch.float64, device=dev)
+        self.seg_counts, self.seg_open, self.counts = z(torch.int32), z(torch.int32), z(torch.int32)
+        self.sq = torch.zeros(M, dtype=torch.float64, device=dev)
+        self.l0 = torch.zeros(M, dtype=torch.float64, device=dev)
+        self.losses = torch.empty(M, _lib.SCE_LOSS_COLS, dtype=torch.float32, device=dev)
+        self.nnz = torch.empty(M, dtype=torch.float32, device=dev)
+
+    def run(self, x, seg, phase):
+        from . import _lib
+        lib = _lib.load()
+        B, d = x.shape
+        x_hat = torch.empty(self.M, B, d, dtype=torch.float32, device=self.dev) if self.centred else None
+        _lib.check(lib.sce_forward_stats(
+            self.plan, x.data_ptr(), B, seg, phase, x_hat.data_ptr() if x_hat is not None else None,
+            self.losses.data_ptr(), self.nnz.data_ptr(), self.sums.data_ptr(), self.seg_counts.data_ptr(),
+            self.seg_open.data_ptr(), self.sws_ptr, self.sws_bytes, self.stream), "sce_forward_stats")
+        _lib.check(lib.sce_active_counts(self.plan, B, self.counts.data_ptr(), self.stream), "sce_active_counts")
+        if x_hat is None:
+            self.sq += self.losses[:, 1].double() * (B * d)
+        else:       # the reference's residual x - uncenter(x^_c), in the raw space (standard_metrics.py:310-314)
+            r = (x[None] - self.trans[:, None]) - torch.bmm(x_hat / self.scale[:, None], self.rot)
+            self.sq += r.double().pow(2).sum(dim=(1, 2))
+        self.l0 += self.nnz.double() * B
+
+    def bad(self) -> bool:
+        import ctypes as C
+        from . import _lib
+        flag, amax = C.c_int(0), C.c_float(0.0)
+        _lib.check(_lib.load().sce_health(self.plan, C.byref(flag), C.byref(amax), self.stream), "sce_health")
+        return bool(flag.value)
+
+    def close(self):
+        from . import _lib
+        if getattr(self, "plan", None) is not None and self.plan.value:
+            _lib.load().sce_plan_destroy(self.plan)
+        self.plan = None
+
+
+def _eval_rows(activations, dev, cuts):
+    """The row ranges ``cuts`` of ``activations`` as fp32 [B, d] batches on ``dev``: device input sliced in place, host
+    input streamed through HostBatchPrefetcher; fp16 is converted per batch on the device."""
+    if activations.device.type == "cuda":
+        for s, e in cuts:
+            yield activations[s:e].float().contiguous()
+        return
+    from .train_loop import HostBatchPrefetcher
+    for xb in HostBatchPrefetcher((activations[s:e] for s, e in cuts), dev):
+        yield xb.float().contiguous()
+
+
+def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
+    from . import _lib
+    if arith not in _lib.ARITH_CODE:
+        raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
+    if int(segment) < 1:
+        raise ValueError(f"batch_size / segment must be >= 1, got {segment}")
+    segment = int(segment)
+    lds = [ld[0] if isinstance(ld, (tuple, list)) else ld for ld in learned_dicts]
+    if not lds:
+        raise ValueError("no dictionaries to evaluate")
+    if activations.dim() != 2 or activations.shape[0] == 0:
+        raise ValueError(f"activations must be a non-empty [N, d] tensor, got shape {tuple(activations.shape)}")
+    if activations.dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"activations must be fp32 or fp16, got {activations.dtype}")
+    N, d = activations.shape
+    # AUTO runs bf16x3: the fp32 range, so activations fp16 cannot hold give finite results
+    ar = "bf16x3" if arith == "auto" else arith
+    groups = _eval_groups(lds, centre, 16 if ar == "f16f8" else 8)
+    for (kind, n_pad, dd, _), idx in groups.items():
+        if dd != d:
+            raise ValueError(f"dictionary {idx[0]} has width {dd}, the activations {d}")
+    if activations.device.type == "cuda":
+        dev = activations.device
+    elif torch.cuda.is_available():
+        dev = torch.device("cuda", torch.cuda.current_device())
+    else:
+        raise RuntimeError("dictionary evaluation runs in the sm_90a CUDA engine and needs a CUDA device; there is no "
+                           "CPU implementation in the product path")
+    # engine calls: a multiple of the segment where one fits, and a cut where the last segment starts (its sums are
+    # weighted by segment / rows, as the reference's running average does)
+    rows = _EVAL_ROWS // segment * segment if segment <= _EVAL_ROWS else _EVAL_ROWS
+    n_seg = -(-N // segment)
+    last = (n_seg - 1) * segment
+    cuts = [(s, min(s + rows, last)) for s in range(0, last, rows)] + [(s, min(s + rows, N)) for s in range(last, N, rows)]
+    batch_max = max(e - s for s, e in cuts)
+    results = [None] * len(lds)
+    with torch.cuda.device(dev):
+        plans = []
+        try:
+            for key, idx in groups.items():
+                plans.append((_EvalPlan(key, [lds[i] for i in idx], batch_max, ar, dev), idx))
+            s1 = torch.zeros(d, dtype=torch.float64, device=dev)
+            s2 = torch.zeros(d, dtype=torch.float64, device=dev)
+            snap = [torch.zeros_like(p.sums) for p, _ in plans]
+            for (s, e), x in zip(cuts, _eval_rows(activations, dev, cuts)):
+                if s == last and last > 0:
+                    snap = [p.sums.clone() for p, _ in plans]
+                for p, _ in plans:
+                    p.run(x, segment, s % segment)
+                xd = x.double()
+                s1 += xd.sum(0)
+                s2 += xd.pow(2).sum(0)
+            if ar == "f16f8" and any(p.bad() for p, _ in plans):
+                raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
+                                 "NaN): use arith='bf16x3' or 'auto'")
+            total = (s2 - s1 * s1 / N).sum()
+            r_last = N - last
+            for (p, idx), sn in zip(plans, snap):
+                full, tail = sn, p.sums - sn
+                m = (full + (segment / r_last) * tail) / (n_seg * segment)        # [M, n, 4] fp64
+                fvu = (p.sq / total).float()
+                l0 = (p.l0 / N).float()
+                for k, i in enumerate(idx):
+                    n = int(lds[i].n_feats)
+                    counts = p.counts[k, :n].clone()
+                    n_act = (counts > threshold).sum()
+                    mean, m2, m3, m4 = (m[k, :n, q] for q in range(4))
+                    var = m2 - mean * mean
+                    out = {"fvu": fvu[k], "mean_l0": l0[k], "feature_counts": counts,
+                           "feature_frequency": counts.float() / N, "n_ever_active": n_act,
+                           "frac_dead": 1.0 - n_act.float() / n, "rows": N,
+                           # (the last segment is still open after the pass: its flags count as well)
+                           "times_active": (p.seg_counts[k, :n] + p.seg_open[k, :n]).float(), "mean": mean.float(), "m2": m2.float(),
+                           "m3": m3.float(), "m4": m4.float(), "var": var.float(),
+                           "skew": (m3 / var.pow(1.5).clamp(min=1e-8)).float(),
+                           "kurtosis": (m4 / var.pow(2).clamp(min=1e-8)).float()}
+                    results[i] = {k2: (v.to(activations.device) if torch.is_tensor(v) else v) for k2, v in out.items()}
+        finally:
+            for p, _ in plans:
+                p.close()
+    return results
+
+
+def evaluate_dicts(learned_dicts, activations: torch.Tensor, segment: int = 1000,
+                   threshold: int = EVER_ACTIVE_THRESHOLD, arith: str = "auto"):
+    """Scores of exported dictionaries on a set of activations, in one pass for all of them.
+
+    ``learned_dicts``: LearnedDicts or ``(LearnedDict, hparams)`` pairs (what ``torch.load("learned_dicts.pt")``
+    returns): TiedSAE (norm_encoder=True, any centring), UntiedSAE, TopKLearnedDict. ``activations``: [N, d] fp32 or
+    fp16, on the CPU (streamed to the GPU) or a CUDA device. Each dictionary encodes the centred batch, as ``predict``
+    and ``mean_nonzero_activations`` do. ``arith``: the engine's operand arithmetic; "auto" runs bf16x3, which holds
+    the fp32 range.
+
+    Returns one dict per input dictionary, in input order, with tensors on the device of ``activations``:
+      ``fvu``, ``mean_l0``, ``feature_counts``, ``feature_frequency``, ``n_ever_active`` (count > ``threshold``),
+      ``frac_dead``, ``rows`` as :func:`evaluate_batches` (FVU with the residual in the raw space, as the reference's
+      ``fraction_variance_unexplained``), and ``times_active``, ``mean``, ``m2``, ``m3``, ``m4``, ``var``, ``skew``,
+      ``kurtosis`` as ``calc_moments_streaming`` with ``batch_size = segment`` defines them (standard_metrics.py:482-511:
+      ``times_active`` counts segments, the last partial segment is weighted like a full one)."""
+    return _evaluate(learned_dicts, activations, segment, threshold, arith, centre=True)
+
+
+# drop-ins with the reference's names, argument order and results (standard_metrics.py:305-314, 344-345, 446-454,
+# 482-511), on the device of the activations
+def fraction_variance_unexplained(model, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:
+    return _evaluate([model], batch, 1000, EVER_ACTIVE_THRESHOLD, arith, centre=True)[0]["fvu"]
+
+
+def r_squared(model, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:
+    return 1.0 - fraction_variance_unexplained(model, batch, arith=arith)
+
+
+def mean_nonzero_activations(model, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:
+    return _evaluate([model], batch, 1000, EVER_ACTIVE_THRESHOLD, arith, centre=True)[0]["feature_frequency"]
+
+
+def batched_calc_feature_n_ever_active(learned_dict, activations: torch.Tensor, batch_size: int = 1000,
+                                       threshold: int = 10, arith: str = "auto") -> int:
+    """Features non-zero on more than ``threshold`` rows; encodes the raw activations (no ``center``)."""
+    return int(_evaluate([learned_dict], activations, batch_size, threshold, arith, centre=False)[0]["n_ever_active"])
+
+
+def calc_moments_streaming(learned_dict, activations: torch.Tensor, batch_size: int = 1000, arith: str = "auto"):
+    """(times_active, mean, var, skew, kurtosis, m4), each [n] fp32; encodes the raw activations (no ``center``)."""
+    r = _evaluate([learned_dict], activations, batch_size, EVER_ACTIVE_THRESHOLD, arith, centre=False)[0]
+    return r["times_active"], r["mean"], r["var"], r["skew"], r["kurtosis"], r["m4"]

@@ -1,9 +1,11 @@
 #!/usr/bin/env python
-"""Dictionary-similarity metrics (standard_metrics.py mmcs / mcs_duplicates / capacity_per_feature) on the engine against
-the reference's op sequence on the same GPU. One metric pass = the cosine maxima of every pair in both directions plus
-the capacity of every dictionary.
+"""Dictionary metrics on the engine against the reference's op sequence on the same GPU.
+  mmcs_*: dictionary similarity (standard_metrics.py mmcs / mcs_duplicates / capacity_per_feature). One metric pass = the
+          cosine maxima of every pair in both directions plus the capacity of every dictionary.
+  eval_*: scores of exported dictionaries on activations (calc_moments_streaming + fraction_variance_unexplained +
+          mean_nonzero_activations). One pass = metrics.evaluate_dicts of every dictionary over every row.
 
-    python tools/bench_metrics.py --workload mmcs_cfg2 [--steps K --warmup W --arith auto|bf16x3|f16f8]
+    python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5 [--steps K --warmup W --arith ...]
 
 Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
 computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
@@ -136,13 +138,122 @@ def run_mmcs(args):
     }), flush=True)
 
 
+EVAL_WORKLOADS = {
+    # name: (M, n, d, rows, description)
+    "eval_cfg2": (16, 4096, 512, 1 << 20, "16 seeded config-2 TiedSAE dictionaries (4096 x 512) over 2^20 fp16 rows, "
+                                          "segment 1000"),
+    "eval_cfg5": (1, 32768, 2048, 1 << 18, "one 32768 x 2048 TiedSAE dictionary over 2^18 fp16 rows, segment 1000"),
+}
+
+
+def run_eval(args):
+    """Scores of exported dictionaries on a set of activations: the engine's evaluate_dicts pass over all rows and all
+    dictionaries, against the reference's per-dictionary op sequence (calc_moments_streaming, then
+    fraction_variance_unexplained and mean_nonzero_activations, fp32 torch on the same GPU; the last two over 8192-row
+    pieces, since the whole set's dense code would not fit) timed on one dictionary."""
+    import sparse_coding_b200 as S
+    from oracle import eval_oracle as O
+    from sparse_coding_b200 import metrics as MT
+
+    if not torch.cuda.is_available():
+        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    M, n, d, N, desc = EVAL_WORKLOADS[args.workload]
+    K, W = args.steps, max(args.warmup, 1)
+    if K < 1:
+        raise SystemExit("--steps must be at least 1")
+    lds = [S.FunctionalTiedSAE.to_learned_dict(p, b) for p, b in make_models(S.FunctionalTiedSAE, M, d, n, seed=0)]
+    for ld in lds:
+        ld.to_device(dev)
+    gen = torch.Generator(device=dev).manual_seed(1)
+    x = torch.empty(N, d, dtype=torch.float16, device=dev)
+    for i in range(0, N, 1 << 16):                 # sparse mixture + noise, generated in pieces, stored as fp16
+        k = min(1 << 16, N - i)
+        feats = torch.nn.functional.normalize(torch.randn(2048, d, generator=gen, device=dev), dim=-1)
+        code = (torch.rand(k, 2048, generator=gen, device=dev) < 0.01) * torch.rand(k, 2048, generator=gen, device=dev)
+        x[i:i + k] = (code @ feats + 0.05 * torch.randn(k, d, generator=gen, device=dev)).half()
+
+    def timed(fn, k, w):
+        for _ in range(w):
+            r = fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(k):
+            r = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / k, r
+
+    ms, _ = timed(lambda: MT.evaluate_dicts(lds, x, segment=1000, arith=args.arith), K, W)
+
+    def stock(ld, xs):
+        """the reference's op sequence for one dictionary (standard_metrics.py:305-314, 482-511)"""
+        moments = [torch.zeros(ld.n_feats, device=dev) for _ in range(5)]
+        times, mean, m2, m3, m4 = moments
+        seen = 0
+        for i in range(0, xs.shape[0], 1000):
+            c = ld.encode(xs[i:i + 1000].float())
+            bm = c.mean(dim=0)
+            times += (bm != 0).float()
+            mean = (seen * mean + 1000 * bm) / (seen + 1000)
+            m2 = (seen * m2 + 1000 * (c ** 2).mean(dim=0)) / (seen + 1000)
+            m3 = (seen * m3 + 1000 * (c ** 3).mean(dim=0)) / (seen + 1000)
+            m4 = (seen * m4 + 1000 * (c ** 4).mean(dim=0)) / (seen + 1000)
+            seen += 1000
+        sq = torch.zeros((), dtype=torch.float64, device=dev)
+        nz = torch.zeros(ld.n_feats, device=dev)
+        for i in range(0, xs.shape[0], 8192):
+            b = xs[i:i + 8192].float()
+            sq += (b - ld.predict(b)).pow(2).sum().double()
+            nz += (ld.encode(ld.center(b)) != 0).float().sum(dim=0)
+        xf = xs.float()
+        total = (xf - xf.mean(dim=0)).pow(2).sum().double()
+        return (sq / total).float(), mean
+
+    k_ref = 1
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    try:
+        torch.backends.cuda.matmul.allow_tf32 = False
+        ms_fp32, _ = timed(lambda: stock(lds[0], x), k_ref, 1)
+        torch.backends.cuda.matmul.allow_tf32 = True
+        ms_tf32, _ = timed(lambda: stock(lds[0], x), k_ref, 1)
+        sub = x[:16384 + 500]                                       # deviation from fp64 on a subsample, dictionary 0
+        m64 = {"kind": "tied", "encoder": lds[0].encoder.double(), "encoder_bias": lds[0].encoder_bias.double()}
+        f64 = O.fraction_variance_unexplained(m64, sub.double())
+        mean64 = O.calc_moments_streaming(m64, sub.double(), 1000)[1]
+        dev_of = lambda f, mean: {"fvu_rel": float(abs(float(f) - float(f64)) / float(f64)),
+                                  "mean_max_rel": float((mean.double() - mean64).abs().max() / mean64.abs().max())}
+        r = MT.evaluate_dicts(lds[:1], sub, segment=1000, arith=args.arith)[0]
+        dev_engine = dev_of(r["fvu"], r["mean"])
+        dev_tf32 = dev_of(*stock(lds[0], sub))
+        torch.backends.cuda.matmul.allow_tf32 = False
+        dev_fp32 = dev_of(*stock(lds[0], sub))
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+    name, limit = card_info(0)
+    print(json.dumps({
+        "metric": "ms per evaluation pass (evaluate_dicts: FVU, counts, moments of every dictionary)",
+        "workload": args.workload, "desc": desc, "value": ms, "unit": "ms", "dictionaries": M, "n": n, "d": d,
+        "rows": N, "rows_per_s": N / (ms * 1e-3), "arith": args.arith, "steps": K, "warmup": W,
+        "deviation_from_fp64": dev_engine,
+        "stock_torch_gpu_per_dictionary": {"fp32": {"ms": ms_fp32, "deviation_from_fp64": dev_fp32},
+                                           "tf32": {"ms": ms_tf32, "deviation_from_fp64": dev_tf32},
+                                           "passes_timed": k_ref},
+        "speedup_vs_stock_fp32": ms_fp32 * M / ms, "speedup_vs_stock_tf32": ms_tf32 * M / ms,
+        "gpu": name, "power_limit_w": limit,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="mmcs_cfg2", choices=sorted(MMCS_WORKLOADS))
+    ap.add_argument("--workload", default="mmcs_cfg2", choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
-    run_mmcs(ap.parse_args())
+    args = ap.parse_args()
+    (run_eval if args.workload in EVAL_WORKLOADS else run_mmcs)(args)
 
 
 if __name__ == "__main__":

@@ -219,6 +219,39 @@ int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_ph
                       float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/* Record selection for reading what features mean (interpret.py:82-212 make_feature_activation_dataset, :265-321
+ * interpret): sce_forward on B rows cut into B / L fragments of L consecutive rows (fragment frag0 + g is rows
+ * g L .. g L + L - 1 of this call), then, per model m and feature j, two lists that ACCUMULATE over calls:
+ *   top    (fragment maximum max_t c[m, gL + t, j], fragment) over every fragment: the n_top largest by
+ *          (maximum descending, fragment ascending)
+ *   random (priority, fragment) over the ACTIVE fragments (the activity mask has c > 0 on some row): the n_random
+ *          largest by (priority descending, fragment ascending), priority = splitmix64(splitmix64(splitmix64(seed) ^ j)
+ *          ^ fragment) >> 1 — a uniform draw without replacement that depends on nothing but (seed, j, fragment)
+ * The code values are those the engine holds: the joined operand planes (as sce_read_code) for the SAE variants,
+ * relu(score) under the activity mask for TOPK; the maximum is taken over the same values, so top_val equals the
+ * maximum of its top_act row bitwise.
+ *   L            fragment length: a multiple of 32 in [32, 8192], dividing B
+ *   frag0        index of this call's first fragment (>= 0); the fragments of a pass must be distinct
+ *   n_top, n_random  list lengths in [0, 64], not both 0
+ *   top_val      device fp32  [M,n,n_top]  \  the lists, in no particular order within a list: sort each by the order
+ *   top_frag     device int64 [M,n,n_top]   | above after the last call. Initialise every *_frag entry to -1 (an
+ *   rnd_key      device int64 [M,n,n_random]| empty entry, below every other) before the first call; the values and
+ *   rnd_frag     device int64 [M,n,n_random]/ keys of empty entries are never read. NULL when the list length is 0.
+ *   top_act, rnd_act  device fp32 [M,n,n_top,L] / [M,n,n_random,L] or NULL: entry i's L code values, written when a
+ *                fragment enters the list at position i
+ *   n_active     device int32 [M,n], ACCUMULATED: += the active fragments of this call (segment counts of
+ *                sce_forward_stats with seg = L)
+ *   workspace    >= sce_fragments_workspace_bytes(desc, B, L), 1024-byte aligned: fragment maxima and activity flags,
+ *                M (B/L) n (4 + 1) bytes, and M n int32 (config 2, M = 16, n = 4096, B = 8192, L = 64: 40 MiB).
+ *                sce_fragments_workspace_bytes is host-only; it returns 0 for an invalid desc, B outside
+ *                [1, batch_max] or an invalid L.
+ * Deterministic (no atomics) and asynchronous on `stream`. */
+size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L);
+int sce_forward_fragments(sce_plan* plan, const float* x, int B, int L, long long frag0, int n_top, int n_random,
+                          unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
+                          long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
 /* The arithmetic the plan resolved to: SCE_ARITH_BF16X3 or SCE_ARITH_F16F8. */
 int sce_plan_arith(const sce_plan* plan);
 

@@ -6,7 +6,8 @@ DictSignature / FunctionalEnsemble (ensemble.py), FunctionalSAE / FunctionalTied
 (learned_dict.py), plus the driver loop pieces of big_sweep.py (train_loop.py) and on-device metrics (metrics.py)."""
 from . import metrics
 from .metrics import (batched_calc_feature_n_ever_active, calc_moments_streaming, evaluate_dicts,
-                      fraction_variance_unexplained, mean_nonzero_activations, r_squared)
+                      fraction_variance_unexplained, mean_nonzero_activations, r_squared,
+                      top_activating_fragments)
 from .ensemble import CodeProxy, FunctionalEnsemble, optim_str_to_func, stack_dict, unstack_dict
 from .learned_dict import LearnedDict, TiedSAE, UntiedSAE
 from .optim import AdamConfig, adam
@@ -19,5 +20,5 @@ __all__ = [
     "FunctionalSAE", "FunctionalTiedSAE", "LearnedDict", "TiedSAE", "TopKEncoder", "TopKLearnedDict", "UntiedSAE",
     "adam", "batched_calc_feature_n_ever_active", "calc_moments_streaming", "evaluate_dicts",
     "fraction_variance_unexplained", "mean_nonzero_activations", "optim_str_to_func", "r_squared", "stack_dict",
-    "unstack_dict",
+    "top_activating_fragments", "unstack_dict",
 ]

@@ -26,6 +26,7 @@ EXPORTS = [
     "sce_last_launch_count", "sce_get_step_count", "sce_set_step_count", "sce_profile_begin", "sce_profile_end",
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
+    "sce_fragments_workspace_bytes", "sce_forward_fragments",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -100,6 +101,10 @@ def load():
     lib.sce_forward_stats_workspace_bytes.restype = C.c_size_t
     lib.sce_forward_stats_workspace_bytes.argtypes = [C.POINTER(SceDesc), i]
     lib.sce_forward_stats.argtypes = [vp, vp, i, i, i, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_fragments_workspace_bytes.restype = C.c_size_t
+    lib.sce_fragments_workspace_bytes.argtypes = [C.POINTER(SceDesc), i, i]
+    lib.sce_forward_fragments.argtypes = [vp, vp, i, i, ll, i, i, C.c_ulonglong, vp, vp, vp, vp, vp, vp, vp, vp,
+                                          C.c_size_t, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

@@ -908,6 +908,169 @@ static size_t stats_workspace(const sce_desc& d, int B) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// top-activating and random activating fragments (sce_forward_fragments; interpret.py:82-212 record tables,
+// :265-321 record selection): fragment g of a call is rows g L .. g L + L - 1.
+// ------------------------------------------------------------------------------------------------
+struct FragCode {             // the code of the last forward, as the engine holds it
+  const void* hi;             // c_hi plane [M][batch_max][n] (bf16 or fp16)
+  const void* lo;             // bf16x3: c_lo plane
+  const uint8_t* x8;          // f16f8: E5M2 plane of the scaled residuals
+  const float* scores;        // top-k: fp32 scores [M][batch_max][n]
+  const uint32_t* pos;        // activity mask [M][n_chunks][batch_max]
+  int n_chunks, batch_max, n;
+};
+
+// One element c[m, r, j] of the code: SAE variants join the operand planes exactly as join_code_kernel does (-0 -> +0);
+// top-k is relu(score) under the activity mask.
+template <int ARITH, bool TOPK>
+__device__ __forceinline__ float frag_code_value(const FragCode& c, int m, int r, int j) {
+  const long long idx = ((long long)m * c.batch_max + r) * c.n + j;
+  float v;
+  if constexpr (TOPK) {
+    const uint32_t w = __ldg(c.pos + ((long long)m * c.n_chunks + (j >> 5)) * c.batch_max + r);
+    v = ((w >> (31 - (j & 31))) & 1u) ? fmaxf(__ldg(c.scores + idx), 0.f) : 0.f;
+  } else if constexpr (ARITH == kArithF16F8) {
+    constexpr float kInv = 1.f / float(1 << kLoShift);
+    v = __half2float(static_cast<const __half*>(c.hi)[idx]) + e5m2_to_float(c.x8[idx]) * kInv;
+  } else {
+    v = __bfloat162float(static_cast<const __nv_bfloat16*>(c.hi)[idx]) +
+        __bfloat162float(static_cast<const __nv_bfloat16*>(c.lo)[idx]);
+  }
+  return v == 0.f ? 0.f : v;
+}
+
+// fmax[m][g][j] = max over the L rows of fragment g of c[m, r, j]; active[m][g][j] = 1 where the activity mask has
+// c > 0 on some row of it. One block per (32-column chunk, fragment, model): lane j reads column 32 chunk + j, so every
+// row is read coalesced over the features; warp w takes the rows w, w + 8, ... and the 8 warps meet in shared memory.
+template <int ARITH, bool TOPK>
+__global__ void __launch_bounds__(256) fragment_max_kernel(FragCode c, int L, int G, float* __restrict__ fmax,
+                                                           uint8_t* __restrict__ active) {
+  __shared__ float smax[8][32];
+  __shared__ uint32_t sact[8][32];
+  const int chunk = blockIdx.x, g = blockIdx.y, m = blockIdx.z;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int j = chunk * 32 + lane;
+  const uint32_t* pw = c.pos + ((long long)m * c.n_chunks + chunk) * c.batch_max;
+  float mx = 0.f;
+  uint32_t any = 0u;
+  for (int t = warp; t < L; t += 8) {
+    const int r = g * L + t;
+    any |= __ldg(pw + r);
+    if (j < c.n) mx = fmaxf(mx, frag_code_value<ARITH, TOPK>(c, m, r, j));
+  }
+  smax[warp][lane] = mx;
+  sact[warp][lane] = (any >> (31 - lane)) & 1u;
+  __syncthreads();
+  if (warp == 0 && j < c.n) {
+    float v = smax[0][lane];
+    uint32_t a = sact[0][lane];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) {
+      v = fmaxf(v, smax[w][lane]);
+      a |= sact[w][lane];
+    }
+    const long long o = ((long long)m * G + g) * c.n + j;
+    fmax[o] = v;
+    active[o] = (uint8_t)a;
+  }
+}
+
+// splitmix64 (Steele, Lea & Flood 2014): the priority of fragment `frag` for feature `feature` under `seed` is
+// mix(mix(mix(seed) ^ feature) ^ frag) >> 1, a 63-bit key that depends on nothing but these three numbers
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// list order: (key descending, fragment ascending); an entry with fragment < 0 is empty and below every other
+template <class K>
+__device__ __forceinline__ bool frag_above(K k, long long f, K k2, long long f2) {
+  return f2 < 0 || (f >= 0 && (k > k2 || (k == k2 && f < f2)));
+}
+template <class K>
+__device__ __forceinline__ int frag_lowest(const K* key, const long long* frag, int cap) {
+  int w = 0;
+  for (int i = 1; i < cap; ++i)
+    if (frag_above(key[w], frag[w], key[i], frag[i])) w = i;
+  return w;
+}
+
+// One thread per (feature, model) walks the call's fragments in order and keeps two lists of `cap` entries that persist
+// across calls: (fragment maximum, fragment) over all fragments, and (priority, fragment) over the active ones. A
+// candidate replaces the list's lowest entry when it is above it, and then its L code values are copied into that
+// entry's row of top_act / rnd_act. The lists are sets (sorted by the caller after the last call): the result depends
+// on nothing but the fragments seen, with no atomics.
+template <int ARITH, bool TOPK>
+__global__ void __launch_bounds__(128) fragment_merge_kernel(FragCode c, int L, int G, long long frag0,
+                                                             const float* __restrict__ fmax,
+                                                             const uint8_t* __restrict__ active, int n_top, int n_random,
+                                                             unsigned long long seed, float* top_val, long long* top_frag,
+                                                             float* top_act, long long* rnd_key, long long* rnd_frag,
+                                                             float* rnd_act) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+  if (j >= c.n) return;
+  const long long list = (long long)m * c.n + j;
+  float* tv = top_val + list * n_top;
+  long long* tf = top_frag + list * n_top;
+  long long* rk = rnd_key + list * n_random;
+  long long* rf = rnd_frag + list * n_random;
+  const uint64_t h_feat = splitmix64(splitmix64(seed) ^ (uint64_t)j);
+  int tlow = n_top ? frag_lowest(tv, tf, n_top) : 0;
+  int rlow = n_random ? frag_lowest(rk, rf, n_random) : 0;
+  for (int g = 0; g < G; ++g) {
+    const long long o = ((long long)m * G + g) * c.n + j, frag = frag0 + g;
+    if (n_top) {
+      const float v = __ldg(fmax + o);
+      if (frag_above(v, frag, tv[tlow], tf[tlow])) {
+        tv[tlow] = v;
+        tf[tlow] = frag;
+        if (top_act) {
+          float* dst = top_act + (list * n_top + tlow) * L;
+          for (int t = 0; t < L; ++t) dst[t] = frag_code_value<ARITH, TOPK>(c, m, g * L + t, j);
+        }
+        tlow = frag_lowest(tv, tf, n_top);
+      }
+    }
+    if (n_random && __ldg(active + o)) {
+      const long long k = (long long)(splitmix64(h_feat ^ (uint64_t)frag) >> 1);
+      if (frag_above(k, frag, rk[rlow], rf[rlow])) {
+        rk[rlow] = k;
+        rf[rlow] = frag;
+        if (rnd_act) {
+          float* dst = rnd_act + (list * n_random + rlow) * L;
+          for (int t = 0; t < L; ++t) dst[t] = frag_code_value<ARITH, TOPK>(c, m, g * L + t, j);
+        }
+        rlow = frag_lowest(rk, rf, n_random);
+      }
+    }
+  }
+}
+
+constexpr int kFragMaxList = 64;   // largest n_top / n_random
+
+static bool frag_len_ok(int L) { return L >= 32 && L <= 8192 && L % 32 == 0; }
+
+// fragment maxima [M][B/L][n] fp32, activity flags [M][B/L][n] u8, open-segment flags [M][n] int32
+static size_t frag_workspace(const sce_desc& d, int B, int L, size_t* off_active, size_t* off_open) {
+  const size_t cells = (size_t)d.n_models * (B / L) * d.n;
+  const size_t a = align_up(cells * sizeof(float), 1024), o = a + align_up(cells, 1024);
+  if (off_active) *off_active = a;
+  if (off_open) *off_open = o;
+  return o + align_up((size_t)d.n_models * d.n * sizeof(int), 1024);
+}
+
+template <int ARITH, bool TOPK>
+static void launch_fragments(const FragCode& c, int M, int L, int G, long long frag0, float* fmax, uint8_t* active,
+                             int n_top, int n_random, unsigned long long seed, float* top_val, long long* top_frag,
+                             float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act, cudaStream_t st) {
+  fragment_max_kernel<ARITH, TOPK><<<dim3(c.n_chunks, G, M), 256, 0, st>>>(c, L, G, fmax, active);
+  fragment_merge_kernel<ARITH, TOPK><<<dim3((c.n + 127) / 128, M), 128, 0, st>>>(
+      c, L, G, frag0, fmax, active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
+}
+
+// ------------------------------------------------------------------------------------------------
 // dictionary similarity (sce_similarity): cosine maxima and capacity over a list of dictionary pairs
 // ------------------------------------------------------------------------------------------------
 // maxima keys (EpiSimilarity) -> floats, in place; key 0 (no valid entry: an atom beyond rows[m]) becomes NaN
@@ -1516,6 +1679,63 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
   else
     segment_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, seg,
                                                                      seg_phase, seg_counts, seg_open);
+  CUDA_TRY(cudaGetLastError());
+  return SCE_OK;
+}
+
+size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
+  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L) return 0;
+  return frag_workspace(*desc, B, L, nullptr, nullptr);
+}
+
+int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long frag0, int n_top, int n_random,
+                          unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
+                          long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  if (!p) return fail(SCE_ERR_INVALID, "forward_fragments: plan is NULL");
+  if (B < 1 || B > p->d.batch_max)
+    return fail(SCE_ERR_INVALID, "forward_fragments: B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (!x) return fail(SCE_ERR_INVALID, "forward_fragments: x is NULL");
+  if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);
+  if (B % L) return fail(SCE_ERR_INVALID, "forward_fragments: B = %d is not a multiple of L = %d", B, L);
+  if (frag0 < 0) return fail(SCE_ERR_INVALID, "forward_fragments: frag0 = %lld must be >= 0", frag0);
+  if (n_top < 0 || n_top > kFragMaxList || n_random < 0 || n_random > kFragMaxList || n_top + n_random == 0)
+    return fail(SCE_ERR_INVALID, "forward_fragments: n_top = %d and n_random = %d must lie in [0, %d], not both 0", n_top,
+                n_random, kFragMaxList);
+  if (n_top && (!top_val || !top_frag)) return fail(SCE_ERR_INVALID, "forward_fragments: n_top > 0 needs top_val and top_frag");
+  if (n_random && (!rnd_key || !rnd_frag))
+    return fail(SCE_ERR_INVALID, "forward_fragments: n_random > 0 needs rnd_key and rnd_frag");
+  if (!n_active) return fail(SCE_ERR_INVALID, "forward_fragments: n_active is required");
+  size_t off_active, off_open;
+  const size_t need = frag_workspace(p->d, B, L, &off_active, &off_open);
+  if (!workspace || workspace_bytes < need)
+    return fail(SCE_ERR_WORKSPACE, "forward_fragments: workspace too small: have %zu bytes, need %zu", workspace_bytes, need);
+  if (reinterpret_cast<uintptr_t>(workspace) % 1024)
+    return fail(SCE_ERR_WORKSPACE, "forward_fragments: workspace must be 1024-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const sce_desc& d = p->d;
+  int rc = run_pipeline(p, x, B, nullptr, false, nullptr, nullptr, st);
+  if (rc) return rc;
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  float* fmax = reinterpret_cast<float*>(ws);
+  uint8_t* active = ws + off_active;
+  int* open = reinterpret_cast<int*>(ws + off_open);
+  const int n_chunks = (d.n + 31) / 32, G = B / L;
+  const FragCode c{p->c_hi, p->c_lo, p->c_x8, p->scores, p->act_pos, n_chunks, d.batch_max, d.n};
+  if (d.variant == SCE_TOPK)
+    launch_fragments<kArithBf16x3, true>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
+                                         top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
+  else if (p->arith == kArithF16F8)
+    launch_fragments<kArithF16F8, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
+                                         top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
+  else
+    launch_fragments<kArithBf16x3, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
+                                          top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
+  CUDA_TRY(cudaGetLastError());
+  // active fragments: segments of L rows, cut at fragment boundaries (phase 0, no segment stays open)
+  CUDA_TRY(cudaMemsetAsync(open, 0, (size_t)d.n_models * d.n * sizeof(int), st));
+  segment_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, L, 0,
+                                                                   n_active, open);
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }

@@ -349,9 +349,10 @@ def _eval_groups(lds, centre: bool, multiple: int):
 
 
 class _EvalPlan:
-    """One forward-only plan for a group of dictionaries, with its statistics accumulators."""
+    """One forward-only plan for a group of dictionaries, with its statistics accumulators (``stats``; without them
+    the plan serves other forward-only passes, such as :func:`top_activating_fragments`)."""
 
-    def __init__(self, key, lds, batch_max, arith, dev):
+    def __init__(self, key, lds, batch_max, arith, dev, stats=True):
         import ctypes as C
         from . import _lib
         kind, n_pad, d, centred = key
@@ -391,13 +392,15 @@ class _EvalPlan:
             eps_root=0.0, adam_count_mode=_lib.SCE_ADAM_FROZEN_T1, fwd_passes=3, bwd_passes=3,
             norm_floor=0.0 if kind == "topk" else 1e-8, arith=_lib.ARITH_CODE[arith],
             topk_k_max=int(t["sparsity"].max()) if kind == "topk" else 0, centering=int(centred))
+        self.desc = desc
         nbytes = lib.sce_workspace_bytes(C.byref(desc))
-        sbytes = lib.sce_forward_stats_workspace_bytes(C.byref(desc), batch_max)
+        sbytes = lib.sce_forward_stats_workspace_bytes(C.byref(desc), batch_max) if stats else 1
         if nbytes == 0 or sbytes == 0:
             _lib.check(-1, "sce_workspace_bytes")
         self._ws = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-        self._sws = torch.empty(sbytes + 1024, dtype=torch.uint8, device=dev)
-        self.sws_ptr, self.sws_bytes = (self._sws.data_ptr() + 1023) // 1024 * 1024, sbytes
+        if stats:
+            self._sws = torch.empty(sbytes + 1024, dtype=torch.uint8, device=dev)
+            self.sws_ptr, self.sws_bytes = (self._sws.data_ptr() + 1023) // 1024 * 1024, sbytes
         ptr = lambda x: x.data_ptr() if x is not None else None
         u = ptr(t["unused"])
         b = _lib.SceBuffers()
@@ -419,6 +422,8 @@ class _EvalPlan:
         except Exception:
             self.close()
             raise
+        if not stats:
+            return
         z = lambda dt: torch.zeros(M, n_pad, dtype=dt, device=dev)
         self.sums = torch.zeros(M, n_pad, 4, dtype=torch.float64, device=dev)
         self.seg_counts, self.seg_open, self.counts = z(torch.int32), z(torch.int32), z(torch.int32)
@@ -596,3 +601,166 @@ def calc_moments_streaming(learned_dict, activations: torch.Tensor, batch_size: 
     """(times_active, mean, var, skew, kurtosis, m4), each [n] fp32; encodes the raw activations (no ``center``)."""
     r = _evaluate([learned_dict], activations, batch_size, EVER_ACTIVE_THRESHOLD, arith, centre=False)[0]
     return r["times_active"], r["mean"], r["var"], r["skew"], r["kurtosis"], r["m4"]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Record selection for reading what features mean (interpret.py:82-212 make_feature_activation_dataset, :265-321
+# interpret): per feature, the fragments with the largest maximum and a random sample of the fragments in which it fires,
+# with their per-token code values (libsce ``sce_forward_fragments``). The [N, n] code and the reference's F·L·N fp16
+# tables are never formed: per engine call the fragment maxima are reduced from the operand planes, and per-feature
+# lists of at most 64 entries are merged on the device.
+# ---------------------------------------------------------------------------------------------------------------------
+FRAGMENT_MAX_LIST = 64     # largest n_top / n_random
+FRAGMENT_MAX_LEN = 8192    # largest fragment: one engine call
+
+
+def _list_order(key, frag):
+    """Per row, the permutation that sorts (key, frag) by key descending, then fragment ascending; empty entries
+    (fragment -1) go last."""
+    empty = frag < 0
+    f = torch.where(empty, torch.iinfo(torch.int64).max, frag)
+    k = torch.where(empty, torch.full_like(key, -1), key)
+    o1 = torch.sort(f, dim=-1, stable=True).indices
+    o2 = torch.sort(k.gather(-1, o1), dim=-1, descending=True, stable=True).indices
+    return o1.gather(-1, o2)
+
+
+class _FragmentPlan:
+    """A forward-only plan for a group of dictionaries with its fragment lists, which accumulate over engine calls."""
+
+    def __init__(self, key, lds, batch_max, L, n_top, n_random, seed, want_act, arith, dev):
+        import ctypes as C
+        from . import _lib
+        self.ep = _EvalPlan(key, lds, batch_max, arith, dev, stats=False)
+        M, n = self.ep.M, self.ep.n
+        self.L, self.n_top, self.n_random, self.seed = L, n_top, n_random, seed
+        wbytes = _lib.load().sce_fragments_workspace_bytes(C.byref(self.ep.desc), batch_max, L)
+        if wbytes == 0:
+            _lib.check(-1, "sce_fragments_workspace_bytes")
+        self._ws = torch.empty(wbytes + 1024, dtype=torch.uint8, device=dev)
+        self.ws_ptr, self.ws_bytes = (self._ws.data_ptr() + 1023) // 1024 * 1024, wbytes
+        self.top_val = torch.zeros(M, n, n_top, dtype=torch.float32, device=dev)
+        self.top_frag = torch.full((M, n, n_top), -1, dtype=torch.int64, device=dev)     # -1: empty entry
+        self.rnd_key = torch.zeros(M, n, n_random, dtype=torch.int64, device=dev)
+        self.rnd_frag = torch.full((M, n, n_random), -1, dtype=torch.int64, device=dev)
+        act = lambda k: torch.zeros(M, n, k, L, dtype=torch.float32, device=dev) if want_act and k else None
+        self.top_act, self.rnd_act = act(n_top), act(n_random)
+        self.n_active = torch.zeros(M, n, dtype=torch.int32, device=dev)
+
+    def run(self, x, frag0):
+        from . import _lib
+        ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None
+        _lib.check(_lib.load().sce_forward_fragments(
+            self.ep.plan, x.data_ptr(), x.shape[0], self.L, frag0, self.n_top, self.n_random,
+            self.seed & 0xFFFFFFFFFFFFFFFF, ptr(self.top_val), ptr(self.top_frag), ptr(self.top_act), ptr(self.rnd_key),
+            ptr(self.rnd_frag), ptr(self.rnd_act), self.n_active.data_ptr(), self.ws_ptr, self.ws_bytes, self.ep.stream),
+            "sce_forward_fragments")
+
+    def results(self, k, n):
+        """Model k's lists, sorted, for its first n features."""
+        top_o = _list_order(self.top_val[k, :n], self.top_frag[k, :n])
+        rnd_o = _list_order(self.rnd_key[k, :n], self.rnd_frag[k, :n])
+        rows = lambda a, o: None if a is None else a[k, :n].gather(1, o[..., None].expand(-1, -1, self.L))
+        count = self.n_active[k, :n].long()
+        return {"top_values": self.top_val[k, :n].gather(1, top_o), "top_fragments": self.top_frag[k, :n].gather(1, top_o),
+                "top_activations": rows(self.top_act, top_o),
+                "random_fragments": self.rnd_frag[k, :n].gather(1, rnd_o), "random_activations": rows(self.rnd_act, rnd_o),
+                "n_active_fragments": count, "skipped": count < self.n_random}
+
+    def close(self):
+        self.ep.close()
+
+
+def top_activating_fragments(learned_dicts, activations: torch.Tensor, fragment_len: int = 64, n_top: int = 20,
+                             n_random: int = 20, seed: int = 0, return_activations: bool = True, arith: str = "auto"):
+    """Each feature's top-activating and random activating fragments, with their per-token code values: the records
+    ``interpret()`` (interpret.py:265-321) hands to the explainer, for every dictionary in one pass.
+
+    ``learned_dicts``: LearnedDicts or ``(LearnedDict, hparams)`` pairs (TiedSAE with norm_encoder=True, UntiedSAE,
+    TopKLearnedDict), grouped, padded and streamed as :func:`evaluate_dicts` does. ``activations``: [N, d] fp32 or
+    fp16, on the CPU (streamed to the GPU) or a CUDA device, in sequence order: fragment g is rows
+    g·L … g·L+L−1, L = ``fragment_len`` (a multiple of 32 in [32, 8192]; N must be a multiple of it). The raw rows are
+    encoded, with no ``center()``, as make_feature_activation_dataset does. ``arith``: "auto" runs bf16x3; "f16f8"
+    raises on values fp16 cannot hold.
+
+    Per feature f, with c the code and the fragment maximum max_t c[g·L+t, f] (>= 0):
+      top records     the ``n_top`` fragments with the largest maximum, descending, ties broken by the lower fragment
+                      index; zero-maximum fragments fill the list when fewer are positive, as the reference's
+                      ``sort_values(...).head(20)``. The engine's fp32 values are ranked, where the reference sorts its
+                      fp16 table with a quicksort that leaves the order of ties unspecified.
+      random records  up to ``n_random`` ACTIVE fragments (c > 0 on some row, from the engine's activity mask), drawn
+                      uniformly without replacement, in draw order: the fragments sorted by a priority
+                      splitmix64(splitmix64(splitmix64(seed) ^ f) ^ g) >> 1, descending, ties broken by fragment.
+                      This is the distribution of the reference's fresh permutation per feature popped until 20 active
+                      fragments are found, not its draws. The reference tests its fp16 maximum for 0 instead of the
+                      activity, which differs only for maxima below fp16's smallest subnormal (2^-24).
+      skipped         fewer than ``n_random`` active fragments (the reference's ``skip_feature``).
+    The per-token values are the code as the engine holds it (the joined operand planes for the SAE kinds, relu(score)
+    under the activity mask for top-k), and ``top_values[f, i] == top_activations[f, i].max()`` bitwise.
+
+    Returns one dict per input dictionary, in input order, on the device of ``activations``: ``top_values`` [n, n_top]
+    fp32, ``top_fragments`` [n, n_top] int64, ``top_activations`` [n, n_top, L] fp32, ``random_fragments``
+    [n, n_random] int64 (-1 where unfilled, with zero activations), ``random_activations`` [n, n_random, L] fp32,
+    ``n_active_fragments`` [n] int64, ``skipped`` [n] bool and ``fragments`` = N / L. With fewer than ``n_top``
+    fragments in all, the top list ends in entries with fragment -1 and value 0. ``return_activations=False`` leaves
+    the two activation entries None and skips their copies.
+
+    Memory: the per-token records take n·(n_top + n_random)·L·4 bytes per dictionary on the device — 671 MB for
+    config 2's 16 dictionaries of 4096 features at 20 + 20 and L = 64."""
+    from . import _lib
+    if arith not in _lib.ARITH_CODE:
+        raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
+    L, n_top, n_random = int(fragment_len), int(n_top), int(n_random)
+    if L < 32 or L > FRAGMENT_MAX_LEN or L % 32:
+        raise ValueError(f"fragment_len must be a multiple of 32 in [32, {FRAGMENT_MAX_LEN}], got {fragment_len}")
+    for name, v in (("n_top", n_top), ("n_random", n_random)):
+        if v < 0 or v > FRAGMENT_MAX_LIST:
+            raise ValueError(f"{name} must lie in [0, {FRAGMENT_MAX_LIST}], got {v}")
+    if n_top + n_random == 0:
+        raise ValueError("n_top and n_random are both 0: there is nothing to select")
+    lds = [ld[0] if isinstance(ld, (tuple, list)) else ld for ld in learned_dicts]
+    if not lds:
+        raise ValueError("no dictionaries to evaluate")
+    if activations.dim() != 2 or activations.shape[0] == 0:
+        raise ValueError(f"activations must be a non-empty [N, d] tensor, got shape {tuple(activations.shape)}")
+    if activations.dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"activations must be fp32 or fp16, got {activations.dtype}")
+    N, d = activations.shape
+    if N % L:
+        raise ValueError(f"the activations' {N} rows are not a whole number of fragments of {L} rows")
+    ar = "bf16x3" if arith == "auto" else arith
+    groups = _eval_groups(lds, False, 16 if ar == "f16f8" else 8)
+    for (kind, n_pad, dd, _), idx in groups.items():
+        if dd != d:
+            raise ValueError(f"dictionary {idx[0]} has width {dd}, the activations {d}")
+    if activations.device.type == "cuda":
+        dev = activations.device
+    elif torch.cuda.is_available():
+        dev = torch.device("cuda", torch.cuda.current_device())
+    else:
+        raise RuntimeError("fragment selection runs in the sm_90a CUDA engine and needs a CUDA device; there is no CPU "
+                           "implementation in the product path")
+    rows = min(_EVAL_ROWS // L * L, N)          # engine calls are cut at fragment boundaries
+    cuts = [(s, min(s + rows, N)) for s in range(0, N, rows)]
+    results = [None] * len(lds)
+    with torch.cuda.device(dev):
+        plans = []
+        try:
+            for key, idx in groups.items():
+                plans.append((_FragmentPlan(key, [lds[i] for i in idx], rows, L, n_top, n_random, int(seed),
+                                            return_activations, ar, dev), idx))
+            for (s, e), x in zip(cuts, _eval_rows(activations, dev, cuts)):
+                for p, _ in plans:
+                    p.run(x, s // L)
+            if ar == "f16f8" and any(p.ep.bad() for p, _ in plans):
+                raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
+                                 "NaN): use arith='bf16x3' or 'auto'")
+            for p, idx in plans:
+                for k, i in enumerate(idx):
+                    out = p.results(k, int(lds[i].n_feats))
+                    out["fragments"] = N // L
+                    results[i] = {k2: (v.to(activations.device) if torch.is_tensor(v) else v) for k2, v in out.items()}
+        finally:
+            for p, _ in plans:
+                p.close()
+    return results

@@ -4,8 +4,12 @@
           cosine maxima of every pair in both directions plus the capacity of every dictionary.
   eval_*: scores of exported dictionaries on activations (calc_moments_streaming + fraction_variance_unexplained +
           mean_nonzero_activations). One pass = metrics.evaluate_dicts of every dictionary over every row.
+  interp_*: record selection for reading features (interpret.py make_feature_activation_dataset + interpret's choice of
+          top and random records). One pass = metrics.top_activating_fragments of every dictionary over 50 000 fragments
+          of 64 fp16 rows, 20 + 20 records per feature with their per-token values.
 
-    python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5 [--steps K --warmup W --arith ...]
+    python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5|interp_cfg2|interp_cfg5
+                                  [--steps K --warmup W --arith ...]
 
 Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
 computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
@@ -246,14 +250,115 @@ def run_eval(args):
     }), flush=True)
 
 
+INTERP_WORKLOADS = {
+    # name: (M, n, d, fragments, description)
+    "interp_cfg2": (16, 4096, 512, 50000, "16 seeded config-2 TiedSAE dictionaries (4096 x 512) over 50 000 fragments "
+                                          "of 64 fp16 rows, 20 top + 20 random records per feature"),
+    "interp_cfg5": (1, 32768, 2048, 50000, "one 32768 x 2048 TiedSAE dictionary over 50 000 fragments of 64 fp16 rows, "
+                                           "20 top + 20 random records per feature"),
+}
+
+
+def run_interp(args):
+    """Record selection: the engine's top_activating_fragments pass over all fragments and dictionaries, against the
+    reference's op sequence on the same GPU for one dictionary, batched over 128 fragments per call (encode, amax over
+    the tokens, then topk over the fragments per feature; fp32 and TF32), and the reference's literal loop, one
+    fragment per encode with the maxima and per-token values copied to host fp16 tables, on 1 000 fragments."""
+    import sparse_coding_b200 as S
+    from sparse_coding_b200 import metrics as MT
+
+    if not torch.cuda.is_available():
+        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    M, n, d, G, desc = INTERP_WORKLOADS[args.workload]
+    L = 64
+    K, W = args.steps, max(args.warmup, 1)
+    if K < 1:
+        raise SystemExit("--steps must be at least 1")
+    lds = [S.FunctionalTiedSAE.to_learned_dict(p, b) for p, b in make_models(S.FunctionalTiedSAE, M, d, n, seed=0)]
+    for ld in lds:
+        ld.to_device(dev)
+    gen = torch.Generator(device=dev).manual_seed(1)
+    N = G * L
+    x = torch.empty(N, d, dtype=torch.float16, device=dev)
+    for i in range(0, N, 1 << 16):                 # sparse mixture + noise, generated in pieces, stored as fp16
+        k = min(1 << 16, N - i)
+        feats = torch.nn.functional.normalize(torch.randn(2048, d, generator=gen, device=dev), dim=-1)
+        code = (torch.rand(k, 2048, generator=gen, device=dev) < 0.01) * torch.rand(k, 2048, generator=gen, device=dev)
+        x[i:i + k] = (code @ feats + 0.05 * torch.randn(k, d, generator=gen, device=dev)).half()
+
+    def timed(fn, k, w):
+        for _ in range(w):
+            r = fn()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(k):
+            r = fn()
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / k, r
+
+    ms, res = timed(lambda: MT.top_activating_fragments(lds, x, arith=args.arith), K, W)
+    skipped = float(sum(r["skipped"].float().mean() for r in res) / M)
+    del res
+
+    def stock(ld):
+        """fragment maxima of one dictionary, 128 fragments per encode, then the top 20 fragments of each feature"""
+        fmax = torch.empty(G, n, device=dev)
+        for g0 in range(0, G, 128):
+            g1 = min(G, g0 + 128)
+            c = ld.encode(x[g0 * L:g1 * L].float())
+            fmax[g0:g1] = c.reshape(g1 - g0, L, n).amax(1)
+        return torch.topk(fmax, 20, dim=0).indices
+
+    def literal(ld, frags=1000):
+        """the reference's loop: one fragment per encode, maxima and per-token values to host fp16 tables"""
+        maxes = np.zeros((frags, n), dtype=np.float16)
+        table = np.zeros((frags, n * L), dtype=np.float16)
+        for g in range(frags):
+            c = ld.encode(x[g * L:(g + 1) * L].float())
+            maxes[g] = torch.max(c, dim=0)[0].cpu().numpy()
+            table[g] = c.cpu().numpy().flatten()
+        return maxes
+
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    try:
+        torch.backends.cuda.matmul.allow_tf32 = False
+        ms_fp32, _ = timed(lambda: stock(lds[0]), 1, 1)
+        ms_literal, _ = timed(lambda: literal(lds[0]), 1, 0)
+        torch.backends.cuda.matmul.allow_tf32 = True
+        ms_tf32, _ = timed(lambda: stock(lds[0]), 1, 1)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+    name, limit = card_info(0)
+    print(json.dumps({
+        "metric": "ms per record-selection pass (top_activating_fragments of every dictionary)",
+        "workload": args.workload, "desc": desc, "value": ms, "unit": "ms", "dictionaries": M, "n": n, "d": d,
+        "fragments": G, "fragment_len": L, "rows": N, "rows_per_s": N / (ms * 1e-3), "arith": args.arith, "steps": K,
+        "warmup": W, "skipped_fraction": skipped,
+        "stock_torch_gpu_per_dictionary": {"batched_fp32_ms": ms_fp32, "batched_tf32_ms": ms_tf32,
+                                           "literal_loop_ms_per_1000_fragments": ms_literal,
+                                           "what": "maxima + topk only: no per-token records, no random records"},
+        "speedup_vs_batched_fp32": ms_fp32 * M / ms, "speedup_vs_batched_tf32": ms_tf32 * M / ms,
+        "speedup_vs_literal_loop": ms_literal * (G / 1000) * M / ms,
+        "gpu": name, "power_limit_w": limit,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="mmcs_cfg2", choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS))
+    ap.add_argument("--workload", default="mmcs_cfg2",
+                    choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS) + sorted(INTERP_WORKLOADS))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
     args = ap.parse_args()
-    (run_eval if args.workload in EVAL_WORKLOADS else run_mmcs)(args)
+    if args.workload in INTERP_WORKLOADS:
+        run_interp(args)
+    else:
+        (run_eval if args.workload in EVAL_WORKLOADS else run_mmcs)(args)
 
 
 if __name__ == "__main__":

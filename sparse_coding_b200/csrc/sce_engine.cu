@@ -78,6 +78,9 @@ struct sce_plan {
   __nv_bfloat16 *g_hi, *g_lo;     // [M, Bmax, d]
   __nv_bfloat16 *dz_hi, *dz_lo;   // [M, Bmax, n]   (top-k: fp32 scores alias these planes)
   uint8_t *x_x8, *wenc_x8, *wdec_x8, *c_x8, *g_x8, *dz_x8;
+  // f16f8: the decoder's planes transposed, [M, d, n]: the decode GEMM's B operand, K-major (transpose_dict)
+  __nv_bfloat16 *wdt_hi, *wdt_lo;
+  uint8_t* wdt_x8;
   __nv_bfloat16 *rot_hi, *rot_lo;  // centring: operand planes of buffers["center_rot"] [M, d, d]
   uint8_t* rot_x8;
   float* x_centered;              // centring: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
@@ -213,6 +216,9 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
   __nv_bfloat16 *wdh = weh, *wdl = wel;
   uint8_t* wd8 = we8;
   if (d.variant == SCE_UNTIED) planes(M * n * dd, wdh, wdl, wd8);
+  __nv_bfloat16 *wth = nullptr, *wtl = nullptr;
+  uint8_t* wt8 = nullptr;
+  if (f8) planes(M * n * dd, wth, wtl, wt8);
   planes(M * B * n, ch, cl, c8);
   planes(M * B * dd, gh, gl, g8);
   auto dzh = c.take<__nv_bfloat16>(2 * M * B * n);  // all planes contiguous, 4 B / element: the top-k scores alias them
@@ -275,6 +281,9 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
     p->x_x8 = x8;
     p->wenc_x8 = we8;
     p->wdec_x8 = wd8;
+    p->wdt_hi = wth;
+    p->wdt_lo = wtl;
+    p->wdt_x8 = wt8;
     p->c_x8 = c8;
     p->g_x8 = g8;
     p->dw_enc = dwe;
@@ -325,7 +334,8 @@ constexpr int kBkF8 = 64;  // K block of every GEMM in the f16f8 arithmetic
 
 // The planes of one operand [models][rows][cols] (cols contiguous, `mpitch` elements between models) as GEMM operand
 // maps. kmajor_bk != 0: K-major tiles [box_rows][kmajor_bk]; else MN-major tiles of `box_rows` k-rows by 64 (16-bit)
-// / 128 (8-bit) contiguous elements. 8-bit tiles arrive unswizzled: the GEMM widens them to fp16 (widen_tile).
+// / 128 (8-bit) contiguous elements. K-major 8-bit tiles (64-byte rows at kBkF8) carry the 64-byte swizzle E5M2 wgmma
+// reads; MN-major ones arrive unswizzled and the GEMM widens them to fp16 (widen_tile).
 static bool operand_maps(int arith, CUtensorMap* hi, CUtensorMap* lo, CUtensorMap* x8, const void* phi, const void* plo,
                          const void* px8, uint64_t models, uint64_t rows, uint64_t cols, uint64_t mpitch,
                          uint32_t box_rows, int kmajor_bk) {
@@ -333,8 +343,8 @@ static bool operand_maps(int arith, CUtensorMap* hi, CUtensorMap* lo, CUtensorMa
   if (kmajor_bk) {
     ok = make_tmap_bf16_box(hi, phi, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
     if (arith == kArithF16F8)
-      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE) &&
-           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
+      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_64B) &&
+           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
     else
       ok = ok && make_tmap_bf16_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
   } else {
@@ -396,9 +406,13 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
     ok &= operand_maps(ar, &m->center.b_hi[0], &m->center.b_lo[0], &m->center.b_x8[0], p->rot_hi, p->rot_lo, p->rot_x8, M, dd, dd,
                        dd * dd, kBN, bk_enc);
   }
-  // decode: A = c [M,B,n] K-major, B = Wdec [M,n,d] MN-major (bk k-rows per box)
+  // decode: A = c [M,B,n] K-major, B = Wdec [M,n,d] MN-major (bk k-rows per box); f16f8: its transposed copy [M,d,n] K-major
   ok &= actk(m->decode, 0, C, M, n, bk_dec);
-  ok &= dict_b(m->decode, WD, bk_dec, 0);
+  if (f8)
+    ok &= operand_maps(ar, &m->decode.b_hi[0], &m->decode.b_lo[0], &m->decode.b_x8[0], p->wdt_hi, p->wdt_lo, p->wdt_x8, M, dd, n,
+                       dd * n, kBN, bk_dec);
+  else
+    ok &= dict_b(m->decode, WD, bk_dec, 0);
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
   ok &= actk(m->dcode, 0, G, M, dd, bk_dco);
   ok &= dict_b(m->dcode, WD, kBN, bk_dco);
@@ -456,9 +470,12 @@ static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, con
                          const int* b_batched, int k_total, int passes, int m_total, int n_total,
                          const typename Epi::Params& epi, cudaStream_t st, const ResFlags& rf = ResFlags()) {
   constexpr int BK = ARITH == kArithF16F8 ? kBkF8 : kBkBf16;
-  constexpr int STAGES = gemm_stages<BK, Epi::kWarpStageBytes, ARITH>();
-  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH>;
-  auto kern = gemm_split_kernel<Epi, BK, A_MN, B_MN, STAGES, SPLIT_ACC, ARITH>;
+  // f16f8: K-major 8-bit maps carry the swizzle of the native path (operand_maps), MN-major ones are widened
+  static_assert(ARITH != kArithF16F8 || A_MN == B_MN, "f16f8 GEMMs are K-major or MN-major on both sides");
+  constexpr bool NATIVE = ARITH == kArithF16F8 && !A_MN;
+  constexpr int STAGES = gemm_stages<BK, Epi::kWarpStageBytes, ARITH, NATIVE>();
+  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH, NATIVE>;
+  auto kern = gemm_split_kernel<Epi, BK, A_MN, B_MN, STAGES, SPLIT_ACC, ARITH, NATIVE>;
   // the opt-in to > 48 KB of dynamic shared memory is per device: remember which devices have it
   static bool configured[64] = {};
   if (p->device < 0 || p->device >= 64 || !configured[p->device]) {
@@ -546,6 +563,22 @@ static int launch_dict_rows(const sce_plan* p, int which, float* e, const float*
   return p->arith == kArithF16F8
              ? launch_dict_rows_t<MODE, kArithF16F8>(e, dw, m, v, hi, lo, x8, grad_out, rows, d, normalize, floor, h, p->res_flags, wf, st)
              : launch_dict_rows_t<MODE, kArithBf16x3>(e, dw, m, v, hi, lo, x8, grad_out, rows, d, normalize, floor, h, p->res_flags, wf, st);
+}
+
+// f16f8: the decoder's planes -> their transposed copy, which the decode GEMM reads K-major (nothing to do where the
+// decode runs without the GEMM: k-sparse top-k plans). Adds its launches to `launches`.
+static int transpose_dict(const sce_plan* p, cudaStream_t st, int& launches) {
+  if (p->arith != kArithF16F8 || p->topk_sparse) return SCE_OK;
+  const sce_desc& d = p->d;
+  const dim3 grid((d.d + 63) / 64, (d.n + 63) / 64, d.n_models);
+  transpose_kernel<uint16_t><<<grid, 256, 0, st>>>(reinterpret_cast<const uint16_t*>(p->wdec_hi),
+                                                   reinterpret_cast<uint16_t*>(p->wdt_hi), d.n, d.d);
+  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(reinterpret_cast<const uint8_t*>(p->wdec_lo),
+                                                  reinterpret_cast<uint8_t*>(p->wdt_lo), d.n, d.d);
+  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(p->wdec_x8, p->wdt_x8, d.n, d.d);
+  CUDA_TRY(cudaGetLastError());
+  launches += 3;
+  return SCE_OK;
 }
 
 // f16f8 runs the backward pass on the residual r instead of g = 2r/(B d) (EpiDecodeT): weight- and bias-gradient
@@ -725,7 +758,9 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   dp.tiles_m = tiles_mB;
   dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
   dp.tiles_n = (dd + kBN - 1) / kBN;
-  if (p->split_decode && !f8)
+  if constexpr (f8)
+    rc = launch_k<EpiDec, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+  else if (p->split_decode)
     rc = launch_k<EpiDec, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
   else
     rc = launch_k<EpiDec, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
@@ -1172,9 +1207,10 @@ template <int AR>
 static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_a, int d, int n_pairs, const SimCarve& w,
                             float* row_max, float* col_max, float* capacity, int device, int sms, cudaStream_t st) {
   constexpr int BK = AR == kArithF16F8 ? kBkF8 : kBkBf16;
-  constexpr int STAGES = gemm_stages<BK, EpiSimilarity::kWarpStageBytes, AR>();
-  using SM = GemmSmem<BK, STAGES, EpiSimilarity::kWarpStageBytes, AR>;
-  auto kern = gemm_split_kernel<EpiSimilarity, BK, false, false, STAGES, false, AR>;
+  constexpr bool NATIVE = AR == kArithF16F8;
+  constexpr int STAGES = gemm_stages<BK, EpiSimilarity::kWarpStageBytes, AR, NATIVE>();
+  using SM = GemmSmem<BK, STAGES, EpiSimilarity::kWarpStageBytes, AR, NATIVE>;
+  auto kern = gemm_split_kernel<EpiSimilarity, BK, false, false, STAGES, false, AR, NATIVE>;
   int rc = sim_planes<AR>(A, d, w.a_hi, w.a_lo, w.a_x8, w.flags, st);
   if (rc) return rc;
   if (!b_is_a) {
@@ -1397,7 +1433,9 @@ int sce_prepare(sce_plan* p, void* stream) {
   } else {
     rc = launch_dict_rows<MODE_PREPARE>(p, 0, p->b.encoder, nullptr, nullptr, nullptr, nullptr, rows, d.d, 1, d.norm_floor, h, st);
   }
-  return rc;
+  if (rc) return rc;
+  int launches = 0;
+  return transpose_dict(p, st, launches);
 }
 
 int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_losses, float* out_nnz, void* stream) {
@@ -1431,6 +1469,8 @@ static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, 
     if (rc) return rc;
     ++launches;
   }
+  rc = transpose_dict(p, st, launches);
+  if (rc) return rc;
   if (p->b.encoder_bias) {
     const long long tot = (long long)d.n_models * d.n;
     const int n_part = ((B + kBM - 1) / kBM) * 4;

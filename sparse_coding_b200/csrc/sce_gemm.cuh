@@ -5,8 +5,9 @@
 // This is how the engine reaches the reference's true-FP32 results (SURVEY.md H1) on the 16-bit tensor cores.
 // Every fp32 operand is carried as operand planes and the product formed from partial products:
 //   ARITH = bf16x3: x ~= hi + lo (two bf16 planes); hi*hi + hi*lo + lo*hi, three bf16 passes (~2^-16);
-//   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h on the fp16 planes, the two cross terms on E5M2 planes widened to fp16
-//                   in shared memory and rescaled in the accumulator (see sce_ptx.cuh) — the default.
+//   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h on the fp16 planes, the two cross terms on E5M2 planes (E5M2 wgmma
+//                   where both operands are K-major, else widened to fp16 in shared memory), rescaled in the
+//                   accumulator (see sce_ptx.cuh) — the default.
 // `passes == 1` keeps only the 16-bit plane product. Operands may be K-major (reduction index contiguous in HBM) or
 // MN-major (row/column index contiguous), so no transposed copies of activations/codes are ever written.
 //
@@ -64,7 +65,8 @@ constexpr int kArithBf16x3 = 0, kArithF16F8 = 1;
 
 constexpr int align1k(int v) { return (v + 1023) / 1024 * 1024; }
 
-template <int BK, int EPI_WARP_BYTES, int ARITH>
+// F8_NATIVE (f16f8, both operands K-major): the cross terms run on E5M2 wgmma from the stage, nothing is widened.
+template <int BK, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
 struct GemmSmemLayout {
   static constexpr int kATile = kBM * BK * 2;   // bytes of one 16-bit A tile
   static constexpr int kBTile = kBN * BK * 2;
@@ -73,15 +75,15 @@ struct GemmSmemLayout {
   static constexpr int kAccLd = kBN + 1;         // padded row of the fp32 accumulator tile (conflict-free both ways)
   static constexpr int kAccBytes = kBM * kAccLd * 4;
   // f16f8: the four 8-bit tiles of a stage widened to fp16 (shares the space of the accumulator tile: never live together)
-  static constexpr int kWideBytes = ARITH == kArithF16F8 ? 2 * kATile + 2 * kBTile : 0;
+  static constexpr int kWideBytes = ARITH == kArithF16F8 && !F8_NATIVE ? 2 * kATile + 2 * kBTile : 0;
   static constexpr int kAccRegion = align1k(kAccBytes > kWideBytes ? kAccBytes : kWideBytes);
   static constexpr int kFixed = kAccRegion + kEpiWarps * EPI_WARP_BYTES + 1024 /*barriers*/ + 1024 /*align slack*/;
   static constexpr int kMaxStages = (kSmemLimit - kFixed) / kStage;
 };
 
-template <int BK, int STAGES, int EPI_WARP_BYTES, int ARITH>
-struct GemmSmem : GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH> {
-  using L = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH>;
+template <int BK, int STAGES, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
+struct GemmSmem : GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH, F8_NATIVE> {
+  using L = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH, F8_NATIVE>;
   static constexpr int kAccOff = STAGES * L::kStage;
   static constexpr int kEpiOff = kAccOff + L::kAccRegion;
   static constexpr int kBarOff = kEpiOff + kEpiWarps * EPI_WARP_BYTES;
@@ -90,9 +92,9 @@ struct GemmSmem : GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH> {
 };
 
 // pipeline depth: as many stages as fit beside the accumulator tile and the epilogue staging (at most 8)
-template <int BK, int EPI_WARP_BYTES, int ARITH>
+template <int BK, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
 constexpr int gemm_stages() {
-  constexpr int s = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH>::kMaxStages;
+  constexpr int s = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH, F8_NATIVE>::kMaxStages;
   return s > 8 ? 8 : s;
 }
 
@@ -110,7 +112,7 @@ struct epi_pair_tiles : std::false_type {};
 template <class Epi>
 struct epi_pair_tiles<Epi, std::void_t<decltype(Epi::kPairTiles)>> : std::bool_constant<Epi::kPairTiles> {};
 
-// f16f8: an 8-bit tile as TMA delivers it without swizzle — K-major [ROWS][BK] or MN-major [BK][ROWS] bytes — widened
+// f16f8 without F8_NATIVE: an 8-bit tile as TMA delivers it without swizzle — K-major [ROWS][BK] or MN-major [BK][ROWS] bytes — widened
 // to the fp16 tile the 16-bit loads of the same operand produce: K-major [ROWS][BK] with the 128-byte swizzle (BK = 64),
 // MN-major [ROWS / 64][BK][64] with the 128-byte swizzle. 256 consumer threads, 16 bytes each per round.
 template <bool MN, int BK, int ROWS>
@@ -151,17 +153,21 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
 // weight gradient (K = batch).
 //
 // ARITH = kArithF16F8 (see sce_ptx.cuh, "fp16 + fp8 arithmetic"): a tile makes TWO sweeps over K. Sweep 1 streams the
-// 8-bit planes (a stage holds A.h8, A.l8, B.h8, B.l8 — the same bytes as A.f16 + B.f16), widens them to fp16 and
-// accumulates the cross terms; the accumulator is then scaled by 2^-kLoShift; sweep 2 streams the fp16 planes and adds hh.
-template <class Epi, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, int ARITH = kArithBf16x3>
+// 8-bit planes (a stage holds A.h8, A.l8, B.h8, B.l8 — the same bytes as A.f16 + B.f16) and accumulates the cross terms;
+// the accumulator is then scaled by 2^-kLoShift; sweep 2 streams the fp16 planes and adds hh. F8_NATIVE (both operands
+// K-major, 8-bit tiles loaded with the 64-byte swizzle): sweep 1 runs E5M2 wgmma on the stage itself. Otherwise the 8-bit
+// tiles arrive unswizzled and are widened to fp16 in shared memory first.
+template <class Epi, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, int ARITH = kArithBf16x3,
+          bool F8_NATIVE = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
   constexpr int BN = kBN;
   static_assert(!F8 || !SPLIT_ACC, "f16f8 rescales in the accumulator; no split accumulators");
+  static_assert(!F8_NATIVE || (F8 && !A_MN && !B_MN), "E5M2 wgmma reads K-major operands only");
   static_assert(!F8 || BK == 64, "f16f8: K block 64");
   static_assert(BK == 32 || BK == 64, "BK in {32, 64}: one swizzled row (64 or 128 B) per K-major tile row");
-  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH>;
+  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH, F8_NATIVE>;
   constexpr int EC = Epi::kCols;  // accumulator columns handed to the epilogue per call
   static_assert(EC == 32, "epilogue chunk is 32 columns");
 
@@ -341,7 +347,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     constexpr bool F16 = F8;   // f16f8 multiplies fp16 (and widened e5m2) planes; bf16x3 bf16 planes
 
     float acc[64];
-    float accx[SPLIT_ACC ? 64 : 1];
+    float accx[SPLIT_ACC || F8_NATIVE ? 64 : 1];   // split cross-term accumulator / one K block of E5M2 cross terms
     float* acc_stage = reinterpret_cast<float*>(smem + SM::kAccOff);
     int stage = 0;
     uint32_t phase = 0;
@@ -360,25 +366,50 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       decode_tile(tile, model, tile_m, tile_n);
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      if constexpr (SPLIT_ACC) {
+      if constexpr (SPLIT_ACC || F8_NATIVE) {
 #pragma unroll
         for (int i = 0; i < 64; ++i) accx[i] = 0.f;
       }
       if constexpr (F8) {
-        uint8_t* wide = smem + SM::kAccOff;   // widened tiles: A.h8, A.l8, B.h8, B.l8 (fp16)
-        const uint32_t wa_h = smem_u32(wide), wa_l = wa_h + SM::kATile, wb_h = wa_l + SM::kATile, wb_l = wb_h + SM::kBTile;
-        if (three) {
-          for (int set = 0; set < p.nsets; ++set) {
-            const bool t_lh = term_lh[set], t_hl = term_hl[set];
-            if (!t_lh && !t_hl) continue;
-            for (int kb = 0; kb < kblocks; ++kb) {
-              mbar_wait(&full_bar[stage], phase);
+        // sweep 1 over one operand pair with a compile-time choice of cross terms (LH: A.l8 x B.h8, HL: A.h8 x B.l8), so
+        // that no wgmma sits behind a run-time branch between fence and commit
+        auto cross_sweep = [&](auto lh, auto hl) {
+          constexpr bool LH = decltype(lh)::value, HL = decltype(hl)::value;
+          for (int kb = 0; kb < kblocks; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint8_t* st = smem + stage * SM::kStage;
+            if constexpr (F8_NATIVE) {
+              // K-major 8-bit tiles [rows][64 B] with the 64-byte swizzle: the geometry of a bf16 tile at K block 32
+              // (8-row groups 512 B apart, 32 B per k32 slice)
+              const uint32_t sa_h = smem_u32(st) + uint32_t(wg) * (64 * BK), sa_l = sa_h + SM::kATile / 2;
+              const uint32_t sb_h = smem_u32(st + SM::kATile), sb_l = sb_h + SM::kBTile / 2;
+              auto d8 = [](uint32_t tile, int k) { return make_wgmma_desc(tile + k * 32, 16, 512, 2); };
+              wgmma_fence();
+#pragma unroll
+              for (int k = 0; k < BK / 32; ++k) {
+                if constexpr (LH) wgmma_n128_e5m2(accx, d8(sa_l, k), d8(sb_h, k));
+                if constexpr (HL) wgmma_n128_e5m2(accx, d8(sa_h, k), d8(sb_l, k));
+              }
+              wgmma_commit();
+              wgmma_wait<0>();
+              release(stage);
+              next();
+              // FP8 wgmma adds with fewer bits than fp32 and truncates, so its sums drift with their length: each K
+              // block's cross terms are promoted into the fp32 accumulator
+#pragma unroll
+              for (int i = 0; i < 64; ++i) {
+                acc[i] += accx[i];
+                accx[i] = 0.f;
+              }
+            } else {
+              uint8_t* wide = smem + SM::kAccOff;   // widened tiles: A.h8, A.l8, B.h8, B.l8 (fp16)
+              const uint32_t wa_h = smem_u32(wide), wa_l = wa_h + SM::kATile, wb_h = wa_l + SM::kATile,
+                             wb_l = wb_h + SM::kBTile;
               consumer_sync();   // both warpgroups are done with the widened tiles (and the previous epilogue)
-              const uint8_t* st = smem + stage * SM::kStage;
-              if (t_hl) widen_tile<A_MN, BK, kBM>(st, wide, ctid);
-              if (t_lh) widen_tile<A_MN, BK, kBM>(st + SM::kATile / 2, wide + SM::kATile, ctid);
-              if (t_lh) widen_tile<B_MN, BK, BN>(st + SM::kATile, wide + 2 * SM::kATile, ctid);
-              if (t_hl) widen_tile<B_MN, BK, BN>(st + SM::kATile + SM::kBTile / 2, wide + 2 * SM::kATile + SM::kBTile, ctid);
+              if constexpr (HL) widen_tile<A_MN, BK, kBM>(st, wide, ctid);
+              if constexpr (LH) widen_tile<A_MN, BK, kBM>(st + SM::kATile / 2, wide + SM::kATile, ctid);
+              if constexpr (LH) widen_tile<B_MN, BK, BN>(st + SM::kATile, wide + 2 * SM::kATile, ctid);
+              if constexpr (HL) widen_tile<B_MN, BK, BN>(st + SM::kATile + SM::kBTile / 2, wide + 2 * SM::kATile + SM::kBTile, ctid);
               fence_proxy_async_smem();   // generic-proxy writes -> visible to wgmma
               consumer_sync();
               release(stage);
@@ -386,12 +417,19 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
               wgmma_fence();
 #pragma unroll
               for (int k = 0; k < BK / 16; ++k) {
-                if (t_lh) wgmma_n128<true, A_MN, B_MN>(acc, adesc(wa_l, k), bdesc(wb_h, k));
-                if (t_hl) wgmma_n128<true, A_MN, B_MN>(acc, adesc(wa_h, k), bdesc(wb_l, k));
+                if constexpr (LH) wgmma_n128<true, A_MN, B_MN>(acc, adesc(wa_l, k), bdesc(wb_h, k));
+                if constexpr (HL) wgmma_n128<true, A_MN, B_MN>(acc, adesc(wa_h, k), bdesc(wb_l, k));
               }
               wgmma_commit();
               wgmma_wait<0>();
             }
+          }
+        };
+        if (three) {
+          for (int set = 0; set < p.nsets; ++set) {
+            if (term_lh[set] && term_hl[set]) cross_sweep(std::true_type{}, std::true_type{});
+            else if (term_lh[set]) cross_sweep(std::true_type{}, std::false_type{});
+            else if (term_hl[set]) cross_sweep(std::false_type{}, std::true_type{});
           }
           constexpr float kDown = 1.0f / float(1 << kLoShift);
 #pragma unroll

@@ -283,6 +283,23 @@ __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, c
 }
 
 // ------------------------------------------------------------------------------------------------
+// [models][rows][cols] -> [models][cols][rows] through 64 x 64 tiles in shared memory (grid: column tiles, row tiles,
+// models). f16f8 runs it on the decoder's planes after every rewrite, so that the decode GEMM reads the dictionary
+// K-major (its reduction runs over the dictionary rows) and forms its cross terms on E5M2 wgmma.
+// ------------------------------------------------------------------------------------------------
+template <class T>
+__global__ void __launch_bounds__(256) transpose_kernel(const T* __restrict__ src, T* __restrict__ dst, int rows, int cols) {
+  __shared__ T tile[64][65];
+  const long long off = (long long)blockIdx.z * rows * cols;
+  const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64, tx = threadIdx.x & 63, ty = threadIdx.x >> 6;
+  for (int i = ty; i < 64; i += 4)
+    if (r0 + i < rows && c0 + tx < cols) tile[i][tx] = src[off + (long long)(r0 + i) * cols + c0 + tx];
+  __syncthreads();
+  for (int i = ty; i < 64; i += 4)
+    if (c0 + i < cols && r0 + tx < rows) dst[off + (long long)(c0 + i) * rows + r0 + tx] = tile[tx][i];
+}
+
+// ------------------------------------------------------------------------------------------------
 // per-model ||bias||_2  (bias-decay loss term and its gradient; sae_ensemble.py:73, :150)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) bias_norm_kernel(const float* __restrict__ bias, int n,

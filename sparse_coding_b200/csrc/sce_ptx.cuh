@@ -154,14 +154,37 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t adesc, uint6
 }
 #undef SCE_WGMMA_N128
 
+// wgmma m64n128k32 on E5M2 operands, both K-major in shared memory (the fp8 forms have no transpose): d += A(64 x 32) *
+// B(32 x 128). Same accumulator fragment as wgmma_n128.
+__device__ __forceinline__ void wgmma_n128_e5m2(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e5m2.e5m2 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+      "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc));
+}
+
 // ----------------------------------------------------------------------------------------------
 // fp16 + fp8 arithmetic ("f16f8"): x ~= h + l with h = fp16(x) (11 significant bits) and l = x - h, |l| <= 2^-11 |x|.
 // The product a*b = ah*bh + (al*bh + ah*bl) + O(2^-22): the dominant term is formed on the fp16 planes, the two cross
 // terms need only ~3 significant bits and are carried as 8-bit E5M2 planes: h8 = e5m2(x) and l8 = e5m2(l * 2^kLoShift)
 // (1 byte / element in HBM: 4 bytes per operand element in all). The cross terms are accumulated FIRST (they carry the
 // factor 2^kLoShift), the accumulator is then scaled by 2^-kLoShift (exact) and the hh products are added.
-// An E5M2 byte is the high byte of the fp16 with the same value, so the GEMM widens the 8-bit tiles to fp16 in shared
-// memory (exactly) and forms the cross terms with fp16 wgmma, which, unlike the fp8 form, accepts MN-major operands.
+// Where both operands are K-major the cross terms run on E5M2 wgmma straight from the TMA stage. FP8 wgmma cannot read
+// MN-major operands: there the GEMM widens the 8-bit tiles to fp16 in shared memory (exactly: an E5M2 byte is the high
+// byte of the fp16 with the same value) and forms the cross terms with fp16 wgmma. The products are exact either way;
+// only the accumulation of the cross-term sum differs.
 // ----------------------------------------------------------------------------------------------
 constexpr int kLoShift = 11;  // |l| * 2^11 <= |x|: the scaled residual has the range of x itself (fits E5M2 when x fits fp16)
 

@@ -76,8 +76,16 @@ struct sce_plan {
   __nv_bfloat16 *wenc_hi, *wenc_lo, *wdec_hi, *wdec_lo;  // [M, n, d] (tied: dec aliases enc)
   __nv_bfloat16 *c_hi, *c_lo;     // [M, Bmax, n]
   __nv_bfloat16 *g_hi, *g_lo;     // [M, Bmax, d]
-  __nv_bfloat16 *dz_hi, *dz_lo;   // [M, Bmax, n]   (top-k: fp32 scores alias these planes)
+  __nv_bfloat16 *dz_hi, *dz_lo;   // [M, Bmax, n]   (top-k: fp32 scores alias these planes; dw_native: 8-bit planes [M, n, Bp])
   uint8_t *x_x8, *wenc_x8, *wdec_x8, *c_x8, *g_x8, *dz_x8;
+  // dw_native (dense f16f8 plans): batch-major copies of the 8-bit planes of x, c and g, [xm or M, cols, Bp] with Bp =
+  // batch_max rounded up to 16 (TMA pitch): the weight gradient reads them K-major over the batch (E5M2 wgmma).
+  // dz's 8-bit planes are written in that layout in the first place (EpiDcodeT<f16f8, true>).
+  uint8_t *xt_lo, *xt_x8, *ct_lo, *ct_x8, *gt_lo, *gt_x8;
+  int bpad;                        // Bp
+  int code_batch_major;            // 1: the last call was a dw_native backward, which left the code's residual plane
+                                   // only in its batch-major copy (ct_x8): dcode overwrote the row-major one (carve)
+  int dw_native;                   // 1: the weight gradient's cross terms run on E5M2 wgmma (see native_dw_layout)
   // f16f8: the decoder's planes transposed, [M, d, n]: the decode GEMM's B operand, K-major (transpose_dict)
   __nv_bfloat16 *wdt_hi, *wdt_lo;
   uint8_t* wdt_x8;
@@ -188,6 +196,20 @@ static int topk_slices(const sce_desc& d, size_t kmax) {
   return best;
 }
 
+// ~30 M B n d tensor FLOPs are issued per step; below ~3e11 (a fifth of a millisecond) launches dominate
+static bool launch_bound(const sce_desc& d) {
+  return 30.0 * d.n_models * (double)d.batch_max * d.n * d.d < 3e11;
+}
+// Dense f16f8 plans with split backward GEMMs keep batch-major copies of the 8-bit planes of x, c, g and dz, from which the
+// weight gradient forms its cross terms on E5M2 wgmma. Top-k plans do not: their code and (k-sparse) code-gradient planes
+// are written by the selection / scatter kernels, row-major only, so their weight gradient widens the 8-bit tiles. Nor do
+// launch-bound plans: there the weight gradient takes microseconds either way, and the copies would add three launches
+// per step and a third to the workspace.
+static bool native_dw_layout(const sce_desc& d) {
+  return resolve_arith(d) == kArithF16F8 && d.variant != SCE_TOPK && d.bwd_passes >= 3 && !launch_bound(d);
+}
+static size_t batch_pad(const sce_desc& d) { return ((size_t)d.batch_max + 15) / 16 * 16; }
+
 // Carves the workspace; with base == nullptr only measures it.
 static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
   Carve c{base, 0};
@@ -219,9 +241,30 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
   __nv_bfloat16 *wth = nullptr, *wtl = nullptr;
   uint8_t* wt8 = nullptr;
   if (f8) planes(M * n * dd, wth, wtl, wt8);
-  planes(M * B * n, ch, cl, c8);
+  const bool tdw = native_dw_layout(d);
+  const size_t Bp = batch_pad(d);
+  const size_t dz8 = tdw ? M * n * Bp : M * B * n;   // bytes of one 8-bit plane of dz
+  uint8_t *xtl = nullptr, *xtx = nullptr, *ctl = nullptr, *ctx = nullptr, *gtl = nullptr, *gtx = nullptr;
+  if (!tdw) {
+    planes(M * B * n, ch, cl, c8);
+  } else {
+    // the code's row-major 8-bit planes are read by the decode GEMM only, which runs before dcode writes dz: they live in
+    // dz's 8-bit planes (below), and the code's own 8-bit space holds the batch-major copies the weight gradient reads
+    ch = c.take<__nv_bfloat16>(M * B * n);
+    ctl = c.take<uint8_t>(dz8);
+    ctx = c.take<uint8_t>(dz8);
+  }
   planes(M * B * dd, gh, gl, g8);
-  auto dzh = c.take<__nv_bfloat16>(2 * M * B * n);  // all planes contiguous, 4 B / element: the top-k scores alias them
+  // all planes contiguous, 4 B / element (the top-k scores alias them); with tdw the 8-bit ones are [M][n][Bp]
+  auto dzh = c.take<__nv_bfloat16>(M * B * n + dz8);
+  if (tdw) {
+    cl = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<uint8_t*>(dzh) + 2 * M * B * n);
+    c8 = reinterpret_cast<uint8_t*>(dzh) + 2 * M * B * n + dz8;
+    xtl = c.take<uint8_t>(xm * dd * Bp);
+    xtx = c.take<uint8_t>(xm * dd * Bp);
+    gtl = c.take<uint8_t>(M * dd * Bp);
+    gtx = c.take<uint8_t>(M * dd * Bp);
+  }
   auto dwe = c.take<float>(M * n * dd);
   float* dwd = dwe;
   if (d.variant == SCE_UNTIED) dwd = c.take<float>(M * n * dd);
@@ -277,7 +320,14 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
     p->g_lo = gl;
     p->dz_hi = dzh;
     p->dz_lo = dzh + M * B * n;
-    p->dz_x8 = f8 ? reinterpret_cast<uint8_t*>(dzh) + 3 * M * B * n : nullptr;
+    p->dz_x8 = f8 ? reinterpret_cast<uint8_t*>(dzh) + 2 * M * B * n + dz8 : nullptr;
+    p->xt_lo = xtl;
+    p->xt_x8 = xtx;
+    p->ct_lo = ctl;
+    p->ct_x8 = ctx;
+    p->gt_lo = gtl;
+    p->gt_x8 = gtx;
+    p->bpad = (int)Bp;
     p->x_x8 = x8;
     p->wenc_x8 = we8;
     p->wdec_x8 = wd8;
@@ -416,17 +466,29 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
   ok &= actk(m->dcode, 0, G, M, dd, bk_dco);
   ok &= dict_b(m->dcode, WD, kBN, bk_dco);
-  // weight gradients: everything MN-major, reduction over the batch rows
+  // weight gradients: everything MN-major, reduction over the batch rows. dw_native: the 8-bit planes come from the
+  // batch-major copies [models][rows][Bp] instead, K-major tiles [128 rows][64 B] with the 64-byte swizzle; only B
+  // columns are exposed, so the tail of a short batch reads as zero
+  const uint64_t Bp = (uint64_t)p->bpad;
+  struct Pt { const uint8_t *lo, *x8; };
+  const Pt XT{p->xt_lo, p->xt_x8}, CT{p->ct_lo, p->ct_x8}, GT{p->gt_lo, p->gt_x8},
+      DZT{reinterpret_cast<const uint8_t*>(p->dz_lo), p->dz_x8};
+  auto kmaj8 = [&](CUtensorMap* lo, CUtensorMap* x8, const Pt& T, uint64_t models, uint64_t rows) {
+    return make_tmap_u8_box(lo, T.lo, models, rows, (uint64_t)B, Bp, rows * Bp, kBkF8, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
+           make_tmap_u8_box(x8, T.x8, models, rows, (uint64_t)B, Bp, rows * Bp, kBkF8, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+  };
+  auto dw_set = [&](GemmMaps& g, int set, const Pl& A, const Pt& AT, uint64_t am, const Pl& Bo, const Pt& BT, uint64_t bm,
+                    uint64_t bcols) {
+    bool r = act_a(g, set, A, am, n) && act_b(g, set, Bo, bm, bcols);
+    if (p->dw_native) r = r && kmaj8(&g.a_lo[set], &g.a_x8[set], AT, am, n) && kmaj8(&g.b_lo[set], &g.b_x8[set], BT, bm, bcols);
+    return r;
+  };
   if (d.variant == SCE_UNTIED) {
-    ok &= act_a(m->dw_enc, 0, DZ, M, n);
-    ok &= act_b(m->dw_enc, 0, X, xm, dd);
-    ok &= act_a(m->dw_dec, 0, C, M, n);
-    ok &= act_b(m->dw_dec, 0, G, M, dd);
+    ok &= dw_set(m->dw_enc, 0, DZ, DZT, M, X, XT, xm, dd);
+    ok &= dw_set(m->dw_dec, 0, C, CT, M, G, GT, M, dd);
   } else {
-    ok &= act_a(m->dw_enc, 0, DZ, M, n);
-    ok &= act_b(m->dw_enc, 0, X, xm, dd);
-    ok &= act_a(m->dw_enc, 1, C, M, n);
-    ok &= act_b(m->dw_enc, 1, G, M, dd);
+    ok &= dw_set(m->dw_enc, 0, DZ, DZT, M, X, XT, xm, dd);
+    ok &= dw_set(m->dw_enc, 1, C, CT, M, G, GT, M, dd);
   }
   if (f8 && SCE_EPI_PAIR) {
     // two adjacent chunks per bulk store (stage_pair_and_store): boxes of 64 columns x 32 rows, 128-byte rows
@@ -441,7 +503,13 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
       if (SCE_EPI_PAIR) return make_tmap_u8_box(t, base, M, (uint64_t)B, n, n, Bm * n, 64, 32, CU_TENSOR_MAP_SWIZZLE_64B);
       return make_tmap_u8_box(t, base, M, (uint64_t)B, n, n, Bm * n, 32, 32, CU_TENSOR_MAP_SWIZZLE_32B);
     };
-    ok &= st8(&m->st_c_lo, p->c_lo) && st8(&m->st_c_x8, p->c_x8) && st8(&m->st_dz_lo, p->dz_lo) && st8(&m->st_dz_x8, p->dz_x8);
+    // dw_native: dz's 8-bit planes [M][n][Bp], boxes of 32 features x 32 batch bytes (EpiDcodeT<f16f8, true>)
+    auto st8t = [&](CUtensorMap* t, const void* base) {
+      return make_tmap_u8_box(t, base, M, n, (uint64_t)B, Bp, n * Bp, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE);
+    };
+    ok &= st8(&m->st_c_lo, p->c_lo) && st8(&m->st_c_x8, p->c_x8);
+    ok &= p->dw_native ? st8t(&m->st_dz_lo, p->dz_lo) && st8t(&m->st_dz_x8, p->dz_x8)
+                       : st8(&m->st_dz_lo, p->dz_lo) && st8(&m->st_dz_x8, p->dz_x8);
   } else {
     ok &= make_tmap_bf16_store32(&m->st_c_lo, p->c_lo, M, (uint64_t)B, n, Bm * n);
     ok &= make_tmap_bf16_store32(&m->st_dz_lo, p->dz_lo, M, (uint64_t)B, n, Bm * n);
@@ -465,14 +533,17 @@ struct ResFlags {
   const uint32_t* b[kMaxSets] = {nullptr, nullptr};
 };
 
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC = false, int ARITH = kArithBf16x3>
+// NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN then describe the fp16
+// planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps batch-major copies.
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC = false, int ARITH = kArithBf16x3,
+          bool NATIVE = ARITH == kArithF16F8 && !A_MN>
 static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, const int* a_batched,
                          const int* b_batched, int k_total, int passes, int m_total, int n_total,
                          const typename Epi::Params& epi, cudaStream_t st, const ResFlags& rf = ResFlags()) {
   constexpr int BK = ARITH == kArithF16F8 ? kBkF8 : kBkBf16;
   // f16f8: K-major 8-bit maps carry the swizzle of the native path (operand_maps), MN-major ones are widened
   static_assert(ARITH != kArithF16F8 || A_MN == B_MN, "f16f8 GEMMs are K-major or MN-major on both sides");
-  constexpr bool NATIVE = ARITH == kArithF16F8 && !A_MN;
+  static_assert(!NATIVE || ARITH == kArithF16F8, "E5M2 cross terms are an f16f8 path");
   constexpr int STAGES = gemm_stages<BK, Epi::kWarpStageBytes, ARITH, NATIVE>();
   using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH, NATIVE>;
   auto kern = gemm_split_kernel<Epi, BK, A_MN, B_MN, STAGES, SPLIT_ACC, ARITH, NATIVE>;
@@ -592,6 +663,11 @@ __global__ void l1_over_b_kernel(const float* __restrict__ alpha, float* __restr
   if (i < M) out[i] = alpha ? alpha[i] * invB : 0.f;
 }
 
+template <class T>
+struct TypeTag {
+  using type = T;
+};
+
 // forward (+ optional backward GEMMs). Leaves dW in p->dw_enc / p->dw_dec when `backward`.
 // `mom_part` (forward only, SAE variants): the encode epilogue also writes the moment partials of EpiEncodeT<AR, true>.
 template <int AR>
@@ -646,6 +722,17 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     ++launches;
   }
   CUDA_TRY(cudaGetLastError());
+  // dw_native: batch-major copies of the 8-bit planes of x, c and g for the weight gradient (dz's are written so by dcode)
+  const bool tdw = f8 && backward && p->dw_native;
+  auto batch_major = [&](const void* lo, const uint8_t* x8, uint8_t* tlo, uint8_t* tx8, int models, int cols) {
+    const BatchPlanes t{{static_cast<const uint8_t*>(lo), x8}, {tlo, tx8}};
+    transpose_batch_u8_kernel<<<dim3((cols + 127) / 128, (B + 127) / 128, 2 * models), 256, 0, st>>>(t, models, B, cols,
+                                                                                                 Bm * cols, p->bpad);
+    ++launches;
+    return cudaGetLastError();
+  };
+  if (tdw) CUDA_TRY(batch_major(p->x_lo, p->x_x8, p->xt_lo, p->xt_x8, p->xm, dd));
+  p->code_batch_major = tdw ? 1 : 0;
   // alpha / B, or (f16f8, backward on r = g B d / 2) alpha d / 2
   l1_over_b_kernel<<<(M + 127) / 128, 128, 0, st>>>(p->b.l1_alpha, p->l1_over_b, M, f8 ? 0.5f * (float)dd : 1.0f / (float)B);
   ++launches;
@@ -693,6 +780,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     if (rc) return rc;
     ++launches;
     n_enc_parts = tiles_mB * 8 * ((n + kBN - 1) / kBN);
+    if (tdw) CUDA_TRY(batch_major(p->c_lo, p->c_x8, p->ct_lo, p->ct_x8, M, n));
   } else {
     // scores -> fp32, then per-row selection (code planes, activity mask, k-sparse lists)
     EpiScoresTma::Params sp;
@@ -767,6 +855,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   if (rc) return rc;
   ++launches;
   n_dec_parts = tiles_mB * 8 * dp.tiles_n;
+  if (tdw) CUDA_TRY(batch_major(p->g_lo, p->g_x8, p->gt_lo, p->gt_x8, M, dd));
   }
 
   // ---- losses
@@ -790,19 +879,25 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       CUDA_TRY(cudaGetLastError());
     } else {
     // ---- dcode
-    typename EpiDco::Params zp;
-    zp.out_hi = maps->st_dz_hi;
-    zp.out_lo = maps->st_dz_lo;
-    zp.out_x8 = maps->st_dz_x8;
-    zp.act = act;
-    zp.l1_over_b = p->l1_over_b;
-    zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
-    zp.tiles_m = tiles_mB;
-    zp.planes = p->dw_passes >= 3 ? 3 : 0;
-    // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
-    // (per-model batches carry one flag for all of them, so the same test holds)
-    zp.x_res_flag = f8 ? p->res_flags : nullptr;
-    rc = launch_k<EpiDco, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
+    auto dcode = [&](auto tag) {
+      using E = typename decltype(tag)::type;
+      typename E::Params zp;
+      zp.out_hi = maps->st_dz_hi;
+      zp.out_lo = maps->st_dz_lo;
+      zp.out_x8 = maps->st_dz_x8;
+      zp.act = act;
+      zp.l1_over_b = p->l1_over_b;
+      zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
+      zp.tiles_m = tiles_mB;
+      zp.planes = p->dw_passes >= 3 ? 3 : 0;
+      // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
+      // (per-model batches carry one flag for all of them, so the same test holds)
+      zp.x_res_flag = f8 ? p->res_flags : nullptr;
+      return launch_k<E, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
+    };
+    // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
+    if constexpr (f8) rc = p->dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
+    else rc = dcode(TypeTag<EpiDco>{});
     if (rc) return rc;
     ++launches;
     }
@@ -815,7 +910,11 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       sp.model_stride = (long long)n * dd;
       sp.ld = dd;
       sp.scale = grad_out_scale(p, B);
-      // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one)
+      // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one). dw_native: fp16 planes
+      // MN-major, 8-bit planes K-major from their batch-major copies, cross terms on E5M2 wgmma; else widened
+      if constexpr (f8)
+        if (p->dw_native)
+          return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
       return launch_gemm_t<EpiStoreF32, true, true, !f8, AR>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
     };
     if (d.variant == SCE_UNTIED) {
@@ -1325,11 +1424,8 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   p->dw_passes = desc->bwd_passes;
   if (const char* v = getenv("SCE_TUNE_DCODE_PASSES")) p->dcode_passes = atoi(v) == 1 ? 1 : 3;
   if (const char* v = getenv("SCE_TUNE_DW_PASSES")) p->dw_passes = atoi(v) == 1 ? 1 : 3;
-  {
-    // ~30 M B n d tensor FLOPs are issued per step; below ~3e11 (a fifth of a millisecond) launches dominate
-    const double issued = 30.0 * desc->n_models * (double)desc->batch_max * desc->n * desc->d;
-    p->use_graph = tune_flag("SCE_GRAPH", issued < 3e11 ? 1 : 0);
-  }
+  p->dw_native = native_dw_layout(*desc) && p->dw_passes >= 3;
+  p->use_graph = tune_flag("SCE_GRAPH", launch_bound(*desc) ? 1 : 0);
   {
     // k-sparse decode / dcode of the top-k variant: lists known (topk_k_max), bulk-copy alignment of the dictionary
     // half rows (16 bytes in every plane), shared memory of the gather kernel
@@ -1614,6 +1710,13 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
   if (B < 1 || B > p->d.batch_max) return fail(SCE_ERR_INVALID, "B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long per = (long long)B * p->d.n;
+  if (p->code_batch_major) {
+    const long long total = (long long)p->d.n_models * per;
+    join_code_batch_major_kernel<<<(unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096), 256, 0, st>>>(
+        reinterpret_cast<const __half*>(p->c_hi), p->ct_x8, out_code, B, p->d.n, p->d.batch_max, p->bpad, total);
+    CUDA_TRY(cudaGetLastError());
+    return SCE_OK;
+  }
   for (int m = 0; m < p->d.n_models; ++m) {
     const long long src = (long long)m * p->d.batch_max * p->d.n;
     if (p->arith == kArithF16F8)

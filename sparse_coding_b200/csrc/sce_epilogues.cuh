@@ -58,20 +58,31 @@ __device__ __forceinline__ void stage_row32_u8(uint8_t* tile, int lane, const ui
   for (int q = 0; q < 2; ++q)
     *reinterpret_cast<uint4*>(tile + lane * 32 + ((q ^ sw) << 4)) = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
 }
+// 8-bit plane tile TRANSPOSED: 32 columns x 32 rows, 32-byte rows, no swizzle. The lane's row becomes byte `lane` of
+// each of the 32 tile rows (one byte store per column: the 32 lanes fill 32 consecutive bytes, conflict-free).
+__device__ __forceinline__ void stage_col32_u8(uint8_t* tile, int lane, const uint32_t* w /*[8]*/) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) tile[j * 32 + lane] = uint8_t(w[j >> 2] >> (8 * (j & 3)));
+}
 // whole warp: wait until the previous tiles have been read out, write the new ones, launch their stores.
 // bf16x3: whi / wx are the hi / lo planes. f16f8: whi is the fp16 plane, wx[0..7] the value-e5m2 plane and
 // wx[8..15] the residual-e5m2 plane (maps m_lo / m_x8).
 // `planes`: which of the f16f8 8-bit planes a consumer will read (bit 0: value plane, bit 1: residual plane); planes
 // nobody reads are neither staged nor stored (warp-uniform). bf16x3 always writes both of its planes.
-template <int ARITH>
+// T8 (f16f8): the 8-bit planes go to batch-major copies [model][col][row] (maps m_lo / m_x8 of box 32 rows x 32 bytes).
+template <int ARITH, bool T8 = false>
 __device__ __forceinline__ void stage_and_store(uint8_t* stage, int lane, const uint32_t (&whi)[16],
                                                 const uint32_t (&wx)[16], const CUtensorMap* m_hi,
                                                 const CUtensorMap* m_lo, const CUtensorMap* m_x8, int col, int row0,
                                                 int model, int planes = 3) {
+  static_assert(!T8 || ARITH == kArithF16F8, "transposed 8-bit planes are f16f8 only");
   if (lane == 0) tma_store_wait_read();
   __syncwarp();
   stage_row32(stage, lane, whi);
-  if constexpr (ARITH == kArithF16F8) {
+  if constexpr (T8) {
+    if (planes & 1) stage_col32_u8(stage + 2048, lane, &wx[0]);
+    if (planes & 2) stage_col32_u8(stage + 3072, lane, &wx[8]);
+  } else if constexpr (ARITH == kArithF16F8) {
     if (planes & 1) stage_row32_u8(stage + 2048, lane, &wx[0]);
     if (planes & 2) stage_row32_u8(stage + 3072, lane, &wx[8]);
   } else {
@@ -81,7 +92,10 @@ __device__ __forceinline__ void stage_and_store(uint8_t* stage, int lane, const 
   __syncwarp();
   if (lane == 0) {
     tma_store_3d(m_hi, stage, col, row0, model);
-    if constexpr (ARITH == kArithF16F8) {
+    if constexpr (T8) {
+      if (planes & 1) tma_store_3d(m_lo, stage + 2048, row0, col, model);
+      if (planes & 2) tma_store_3d(m_x8, stage + 3072, row0, col, model);
+    } else if constexpr (ARITH == kArithF16F8) {
       if (planes & 1) tma_store_3d(m_lo, stage + 2048, col, row0, model);
       if (planes & 2) tma_store_3d(m_x8, stage + 3072, col, row0, model);
     } else {
@@ -438,17 +452,20 @@ struct EpiDecodeT {
 // ------------------------------------------------------------------------------------------------
 // dcode:  dz = (acc + (alpha/B) [c > 0]) * [z >= 0]  -> (dz_hi, dz_lo);
 //         per-warp column sums of dz (32 rows) -> bias-gradient partials
+// T8 (f16f8): dz's 8-bit planes are written batch-major, [M][n][batch] (out_lo / out_x8 map that layout), which is
+// how the weight gradient's native E5M2 path reads them (K-major over the batch); the fp16 plane stays row-major.
 // ------------------------------------------------------------------------------------------------
-template <int ARITH>
+template <int ARITH, bool T8 = false>
 struct EpiDcodeT {
   static constexpr int kCols = 32;
   static constexpr bool kPairChunks = ARITH == kArithF16F8 && SCE_EPI_PAIR != 0;
+  static_assert(!(T8 && kPairChunks), "SCE_EPI_PAIR=1 has no transposed dz store: build f16f8 without it");
   static constexpr int kWarpStageBytes = kPairChunks ? kPairStageBytes : 4096;
   // column offset of this warp's next chunk after the one at offset c (see the epilogue loop of gemm_split_kernel)
   static __device__ __forceinline__ int next_chunk(int c) { return kPairChunks ? (((c >> 5) & 1) ? c + 96 : c + 32) : c + 64; }
   struct Params {
-    CUtensorMap out_hi, out_lo, out_x8;  // store maps of the dz planes: [M][B][n], box 32 x 32
-    ActMask act;                   // [c > 0] / [z == 0] written by encode (or the top-k selection)
+    CUtensorMap out_hi, out_lo, out_x8;  // store maps of the dz planes: [M][B][n] (T8: 8-bit ones [M][n][B]), box 32 x 32
+    ActMask act;                  // [c > 0] / [z == 0] written by encode (or the top-k selection)
     const float* l1_over_b;        // [M]: alpha_m / B (f16f8: alpha_m d / 2, see EpiDecodeT)
     float* db_part;                // [M][tiles_m*4][n] or nullptr (no bias)
     int tiles_m;
@@ -514,8 +531,8 @@ struct EpiDcodeT {
       stage_pair_and_store(stage, T.lane, half, half == 1 || col + 32 >= n_total, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8,
                            col - 32 * half, T.m_blk * kBM + T.warp_q * 32, T.model, planes);
     } else {
-      stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
-                             T.m_blk * kBM + T.warp_q * 32, T.model, planes);
+      stage_and_store<ARITH, T8>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
+                                 T.m_blk * kBM + T.warp_q * 32, T.model, planes);
     }
     if (P.db_part && T.m_blk * kBM < m_total) {  // warp-uniform
       // transpose-reduce: 32 lanes x 32 columns -> lane j holds the sum of column j (31 shuffles)

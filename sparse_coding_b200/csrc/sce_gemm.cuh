@@ -6,10 +6,12 @@
 // Every fp32 operand is carried as operand planes and the product formed from partial products:
 //   ARITH = bf16x3: x ~= hi + lo (two bf16 planes); hi*hi + hi*lo + lo*hi, three bf16 passes (~2^-16);
 //   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h on the fp16 planes, the two cross terms on E5M2 planes (E5M2 wgmma
-//                   where both operands are K-major, else widened to fp16 in shared memory), rescaled in the
+//                   where the 8-bit planes are K-major, else widened to fp16 in shared memory), rescaled in the
 //                   accumulator (see sce_ptx.cuh) — the default.
 // `passes == 1` keeps only the 16-bit plane product. Operands may be K-major (reduction index contiguous in HBM) or
-// MN-major (row/column index contiguous), so no transposed copies of activations/codes are ever written.
+// MN-major (row/column index contiguous). Under F8_NATIVE the 8-bit planes are always K-major and A_MN / B_MN describe
+// the fp16 planes only, so an MN-major GEMM (the weight gradient) runs natively from batch-major copies of its 8-bit
+// planes.
 //
 // One CTA per SM, 384 threads: warp 0 = TMA producer (one thread), warpgroups 1 and 2 = wgmma consumers (rows 0..63
 // and 64..127 of the 128 x 128 tile), which then run the fused epilogue. The accumulators go through a padded fp32
@@ -65,7 +67,7 @@ constexpr int kArithBf16x3 = 0, kArithF16F8 = 1;
 
 constexpr int align1k(int v) { return (v + 1023) / 1024 * 1024; }
 
-// F8_NATIVE (f16f8, both operands K-major): the cross terms run on E5M2 wgmma from the stage, nothing is widened.
+// F8_NATIVE (f16f8, 8-bit planes K-major): the cross terms run on E5M2 wgmma from the stage, nothing is widened.
 template <int BK, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
 struct GemmSmemLayout {
   static constexpr int kATile = kBM * BK * 2;   // bytes of one 16-bit A tile
@@ -156,7 +158,8 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
 // 8-bit planes (a stage holds A.h8, A.l8, B.h8, B.l8 — the same bytes as A.f16 + B.f16) and accumulates the cross terms;
 // the accumulator is then scaled by 2^-kLoShift; sweep 2 streams the fp16 planes and adds hh. F8_NATIVE (both operands
 // K-major, 8-bit tiles loaded with the 64-byte swizzle): sweep 1 runs E5M2 wgmma on the stage itself. Otherwise the 8-bit
-// tiles arrive unswizzled and are widened to fp16 in shared memory first.
+// tiles arrive unswizzled and are widened to fp16 in shared memory first. Under F8_NATIVE, A_MN / B_MN describe the fp16
+// planes only (sweep 2): the 8-bit tiles are K-major whatever the fp16 planes' layout, because E5M2 wgmma reads no other.
 template <class Epi, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, int ARITH = kArithBf16x3,
           bool F8_NATIVE = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -164,7 +167,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
   constexpr int BN = kBN;
   static_assert(!F8 || !SPLIT_ACC, "f16f8 rescales in the accumulator; no split accumulators");
-  static_assert(!F8_NATIVE || (F8 && !A_MN && !B_MN), "E5M2 wgmma reads K-major operands only");
+  static_assert(!F8_NATIVE || F8, "F8_NATIVE is an f16f8 path");
   static_assert(!F8 || BK == 64, "f16f8: K block 64");
   static_assert(BK == 32 || BK == 64, "BK in {32, 64}: one swizzled row (64 or 128 B) per K-major tile row");
   using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH, F8_NATIVE>;
@@ -275,13 +278,15 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
                     for (int j = 0; j < BN / 64; ++j) tma_load_3d(sb + j * (BK * 128), &p.b_hi[set], bar, b_row0 + j * 64, k0, bm);
                   }
                 } else {
-                  // 8-bit tiles, unswizzled: K-major [rows][BK] or MN-major [BK][128] bytes
+                  // 8-bit tiles: K-major [rows][BK] bytes (F8_NATIVE: always, 64-byte swizzle), else unswizzled K-major
+                  // [rows][BK] or MN-major [BK][128] bytes
                   uint8_t* sa_h = st;
                   uint8_t* sa_l = st + SM::kATile / 2;
                   uint8_t* sb_h = st + SM::kATile;
                   uint8_t* sb_l = sb_h + SM::kBTile / 2;
-                  const int ac0 = A_MN ? a_row0 : k0, ac1 = A_MN ? k0 : a_row0;
-                  const int bc0 = B_MN ? b_row0 : k0, bc1 = B_MN ? k0 : b_row0;
+                  constexpr bool A8_MN = A_MN && !F8_NATIVE, B8_MN = B_MN && !F8_NATIVE;
+                  const int ac0 = A8_MN ? a_row0 : k0, ac1 = A8_MN ? k0 : a_row0;
+                  const int bc0 = B8_MN ? b_row0 : k0, bc1 = B8_MN ? k0 : b_row0;
                   if (t_hl) tma_load_3d(sa_h, &p.a_lo[set], bar, ac0, ac1, am);
                   if (t_lh) tma_load_3d(sa_l, &p.a_x8[set], bar, ac0, ac1, am);
                   if (t_lh) tma_load_3d(sb_h, &p.b_lo[set], bar, bc0, bc1, bm);

@@ -300,7 +300,79 @@ __global__ void __launch_bounds__(256) transpose_kernel(const T* __restrict__ sr
 }
 
 // ------------------------------------------------------------------------------------------------
-// per-model ||bias||_2  (bias-decay loss term and its gradient; sae_ensemble.py:73, :150)
+// f16f8 weight gradient: the two 8-bit planes of a batch operand [models][batch_max][cols] (rows 0 .. rows - 1 valid) ->
+// batch-major copies [models][cols][ld], ld = batch_max rounded up to 16, so that the weight-gradient GEMM reads them
+// K-major over the batch and forms its cross terms on E5M2 wgmma. 128 x 128-byte tiles through shared memory, 16-byte
+// loads and stores (cols and ld are multiples of 16): a thread gathers one 4-byte word of 16 source rows and turns it
+// into 16 bytes of four output rows with 4 x 4 byte transposes in registers. Grid: (cols / 128, rows / 128, 2 models),
+// z = plane * models + model.
+// ------------------------------------------------------------------------------------------------
+struct BatchPlanes {
+  const uint8_t* src[2];
+  uint8_t* dst[2];
+};
+// rows a, b, c, d of four bytes each (byte = column) -> column v of the four rows in o[v]
+__device__ __forceinline__ void transpose4x4_u8(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t (&o)[4]) {
+  const uint32_t t0 = __byte_perm(a, b, 0x5140), t1 = __byte_perm(a, b, 0x7362);   // a0 b0 a1 b1 / a2 b2 a3 b3
+  const uint32_t t2 = __byte_perm(c, d, 0x5140), t3 = __byte_perm(c, d, 0x7362);
+  o[0] = __byte_perm(t0, t2, 0x5410);
+  o[1] = __byte_perm(t0, t2, 0x7632);
+  o[2] = __byte_perm(t1, t3, 0x5410);
+  o[3] = __byte_perm(t1, t3, 0x7632);
+}
+__global__ void __launch_bounds__(256) transpose_batch_u8_kernel(BatchPlanes t, int models, int rows, int cols,
+                                                                 long long src_model_pitch, int ld) {
+  // 128 source rows of 128 bytes; 16-byte piece k of row r is stored at k ^ ((r >> 4) & 7), so that the column reads
+  // below (8 groups of 16 rows x 4 words per warp) hit 32 different banks
+  __shared__ uint4 tile[128][8];
+  const int plane = blockIdx.z / models, m = blockIdx.z - plane * models;
+  const uint8_t* src = (plane ? t.src[1] : t.src[0]) + (long long)m * src_model_pitch;   // (no dynamic index into the
+  uint8_t* dst = (plane ? t.dst[1] : t.dst[0]) + (long long)m * cols * ld;                // parameter struct: no local copy)
+  const int r0 = blockIdx.y * 128, c0 = blockIdx.x * 128;
+#pragma unroll
+  for (int i = threadIdx.x; i < 1024; i += 256) {
+    const int r = i >> 3, k = i & 7;
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (r0 + r < rows && c0 + 16 * k < cols) v = __ldg(reinterpret_cast<const uint4*>(src + (long long)(r0 + r) * cols + c0 + 16 * k));
+    tile[r][k ^ ((r >> 4) & 7)] = v;
+  }
+  __syncthreads();
+  // source rows 16 g .. + 15, source word q (columns 4 q .. + 3) -> output rows c0 + 4 q + v, bytes r0 + 16 g .. + 15
+  const int g = threadIdx.x & 7, q = threadIdx.x >> 3;
+  if (r0 + 16 * g >= rows) return;
+  const uint32_t* tw = reinterpret_cast<const uint32_t*>(&tile[0][0]);
+  uint32_t w[16];
+#pragma unroll
+  for (int u = 0; u < 16; ++u) w[u] = tw[(16 * g + u) * 32 + (((q >> 2) ^ g) << 2) + (q & 3)];
+  uint32_t o[4][4];   // [quad of rows][column v]
+#pragma unroll
+  for (int h = 0; h < 4; ++h) transpose4x4_u8(w[4 * h], w[4 * h + 1], w[4 * h + 2], w[4 * h + 3], o[h]);
+#pragma unroll
+  for (int v = 0; v < 4; ++v) {
+    const int j = c0 + 4 * q + v;
+    if (j < cols)
+      *reinterpret_cast<uint4*>(dst + (long long)j * ld + r0 + 16 * g) = make_uint4(o[0][v], o[1][v], o[2][v], o[3][v]);
+  }
+}
+
+// join_code_kernel<f16f8> for plans whose code residual plane is held batch-major, [M][n][ld] (transpose_batch_u8_kernel):
+// out [M][B][n] fp32 from the row-major fp16 plane [M][batch_max][n] and that copy. Read-back only (strided reads).
+__global__ void __launch_bounds__(256) join_code_batch_major_kernel(const __half* __restrict__ hi, const uint8_t* __restrict__ x8t,
+                                                                    float* __restrict__ out, int B, int n, int batch_max, int ld,
+                                                                    long long total) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const long long m = i / ((long long)B * n), rj = i - m * B * n;
+    const int r = (int)(rj / n), j = (int)(rj - (long long)r * n);
+    constexpr float kInv = 1.f / float(1 << kLoShift);
+    float v = __half2float(hi[(m * batch_max + r) * n + j]) + e5m2_to_float(x8t[(m * n + j) * ld + r]) * kInv;
+    if (v == 0.f) v = 0.f;  // -0 -> +0
+    out[i] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// per-model ||bias||_2 (bias-decay loss term and its gradient; sae_ensemble.py:73, :150)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) bias_norm_kernel(const float* __restrict__ bias, int n,
                                                         float* __restrict__ out) {

@@ -49,7 +49,8 @@ typedef enum sce_adam_count {
  * results within the 1e-4 bar; they differ in cost and in the range of values they can hold.
  *   BF16X3: x = hi + lo, two bf16 planes; product = hi*hi + hi*lo + lo*hi, three bf16 passes. fp32 range.
  *   F16F8 : x = h + l, h = fp16(x); the dominant h*h runs as one fp16 pass, the two cross terms (which need
- *           ~3 significant bits) are carried on E5M2 planes (1 byte each), widened to fp16 for their two passes.
+ *           ~3 significant bits) are carried on E5M2 planes (1 byte each) and run as two E5M2 passes (in the weight
+ *           gradient of top-k and launch-bound plans, widened to fp16 for two fp16 passes).
  *           Operand values must fit fp16 (|v| < 65504; magnitudes below ~1e-4 lose relative precision) — true for
  *           language-model activations, which the reference itself stores as fp16 (activation_dataset.py:294-299, 364, 404-412).
  *           Needs d % 16 == 0 and n % 16 == 0.

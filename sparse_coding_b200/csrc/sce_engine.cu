@@ -369,22 +369,18 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
 // ------------------------------------------------------------------------------------------------
 // tensor maps for one batch size
 // ------------------------------------------------------------------------------------------------
-// K block of every bf16x3 GEMM: 32 (64-byte swizzle for K-major tiles; a stage of the four planes is 32 KB, so three or
-// four stages fit beside the accumulator tile). f16f8 stages carry one 16-bit plane per operand: K block 64 (kBkF8).
-constexpr int kBkBf16 = 32;
 static int tune_flag(const char* env, int dflt) {
   const char* v = getenv(env);
   return v ? (atoi(v) != 0) : dflt;
 }
+// K-major 16-bit tiles [rows][bk], bk = gemm_bk(arith): the swizzle span is one tile row of 2 bk bytes
 static CUtensorMapSwizzle swizzle_for_bk(int bk) {
-  return bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+  return bk * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
 }
-
-constexpr int kBkF8 = 64;  // K block of every GEMM in the f16f8 arithmetic
 
 // The planes of one operand [models][rows][cols] (cols contiguous, `mpitch` elements between models) as GEMM operand
 // maps. kmajor_bk != 0: K-major tiles [box_rows][kmajor_bk]; else MN-major tiles of `box_rows` k-rows by 64 (16-bit)
-// / 128 (8-bit) contiguous elements. K-major 8-bit tiles (64-byte rows at kBkF8) carry the 64-byte swizzle E5M2 wgmma
+// / 128 (8-bit) contiguous elements. K-major 8-bit tiles (64-byte rows in f16f8) carry the 64-byte swizzle E5M2 wgmma
 // reads; MN-major ones arrive unswizzled and the GEMM widens them to fp16 (widen_tile).
 static bool operand_maps(int arith, CUtensorMap* hi, CUtensorMap* lo, CUtensorMap* x8, const void* phi, const void* plo,
                          const void* px8, uint64_t models, uint64_t rows, uint64_t cols, uint64_t mpitch,
@@ -423,20 +419,19 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   // visible through the map, so rows >= B read as zero (TMA out-of-bounds fill).
   const int ar = p->arith;
   const bool f8 = ar == kArithF16F8;
-  const int bk = f8 ? kBkF8 : kBkBf16;
-  const int bk_enc = bk, bk_dec = bk, bk_dco = bk, bk_dw = bk;
+  const int bk = gemm_bk(ar);
   struct Pl { const void *hi, *lo, *x8; };
   const Pl X{p->x_hi, p->x_lo, p->x_x8}, WE{p->wenc_hi, p->wenc_lo, p->wenc_x8}, WD{p->wdec_hi, p->wdec_lo, p->wdec_x8},
       C{p->c_hi, p->c_lo, p->c_x8}, G{p->g_hi, p->g_lo, p->g_x8}, DZ{p->dz_hi, p->dz_lo, p->dz_x8};
-  // activations [models][B of batch_max][cols]: K-major A tiles [128 rows][bk] / MN-major tiles of bk_dw batch rows
-  auto actk = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols, int bk) {
+  // activations [models][B of batch_max][cols]: K-major A tiles [128 rows][bk] / MN-major tiles of bk batch rows
+  auto actk = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
     return operand_maps(ar, &g.a_hi[set], &g.a_lo[set], &g.a_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, kBM, bk);
   };
   auto act_a = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
-    return operand_maps(ar, &g.a_hi[set], &g.a_lo[set], &g.a_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk_dw, 0);
+    return operand_maps(ar, &g.a_hi[set], &g.a_lo[set], &g.a_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk, 0);
   };
   auto act_b = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
-    return operand_maps(ar, &g.b_hi[set], &g.b_lo[set], &g.b_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk_dw, 0);
+    return operand_maps(ar, &g.b_hi[set], &g.b_lo[set], &g.b_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk, 0);
   };
   // dictionary [M][n][d] as the B operand: K-major tiles [box_rows][bk] (box_rows = the tile's B rows), or MN-major
   auto dict_b = [&](GemmMaps& g, const Pl& P, uint32_t box_rows, int kmajor_bk) {
@@ -444,28 +439,26 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   };
   bool ok = true;
   // encode: A = x [xm,B,d] K-major, B = Wenc [M,n,d] K-major
-  ok &= actk(m->encode, 0, X, xm, dd, bk_enc);
-  ok &= dict_b(m->encode, WE, kBN, bk_enc);
+  ok &= actk(m->encode, 0, X, xm, dd);
+  ok &= dict_b(m->encode, WE, kBN, bk);
   if (d.centering) {
     // centring: A = (x - trans) planes in the X planes (the encode A maps), B = rot [M,d,d] K-major, output d columns
-    for (int t = 0; t < 1; ++t) {
-      m->center.a_hi[t] = m->encode.a_hi[t];
-      m->center.a_lo[t] = m->encode.a_lo[t];
-      m->center.a_x8[t] = m->encode.a_x8[t];
-    }
+    m->center.a_hi[0] = m->encode.a_hi[0];
+    m->center.a_lo[0] = m->encode.a_lo[0];
+    m->center.a_x8[0] = m->encode.a_x8[0];
     ok &= operand_maps(ar, &m->center.b_hi[0], &m->center.b_lo[0], &m->center.b_x8[0], p->rot_hi, p->rot_lo, p->rot_x8, M, dd, dd,
-                       dd * dd, kBN, bk_enc);
+                       dd * dd, kBN, bk);
   }
   // decode: A = c [M,B,n] K-major, B = Wdec [M,n,d] MN-major (bk k-rows per box); f16f8: its transposed copy [M,d,n] K-major
-  ok &= actk(m->decode, 0, C, M, n, bk_dec);
+  ok &= actk(m->decode, 0, C, M, n);
   if (f8)
     ok &= operand_maps(ar, &m->decode.b_hi[0], &m->decode.b_lo[0], &m->decode.b_x8[0], p->wdt_hi, p->wdt_lo, p->wdt_x8, M, dd, n,
-                       dd * n, kBN, bk_dec);
+                       dd * n, kBN, bk);
   else
-    ok &= dict_b(m->decode, WD, bk_dec, 0);
+    ok &= dict_b(m->decode, WD, bk, 0);
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
-  ok &= actk(m->dcode, 0, G, M, dd, bk_dco);
-  ok &= dict_b(m->dcode, WD, kBN, bk_dco);
+  ok &= actk(m->dcode, 0, G, M, dd);
+  ok &= dict_b(m->dcode, WD, kBN, bk);
   // weight gradients: everything MN-major, reduction over the batch rows. dw_native: the 8-bit planes come from the
   // batch-major copies [models][rows][Bp] instead, K-major tiles [128 rows][64 B] with the 64-byte swizzle; only B
   // columns are exposed, so the tail of a short batch reads as zero
@@ -474,8 +467,8 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   const Pt XT{p->xt_lo, p->xt_x8}, CT{p->ct_lo, p->ct_x8}, GT{p->gt_lo, p->gt_x8},
       DZT{reinterpret_cast<const uint8_t*>(p->dz_lo), p->dz_x8};
   auto kmaj8 = [&](CUtensorMap* lo, CUtensorMap* x8, const Pt& T, uint64_t models, uint64_t rows) {
-    return make_tmap_u8_box(lo, T.lo, models, rows, (uint64_t)B, Bp, rows * Bp, kBkF8, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
-           make_tmap_u8_box(x8, T.x8, models, rows, (uint64_t)B, Bp, rows * Bp, kBkF8, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+    return make_tmap_u8_box(lo, T.lo, models, rows, (uint64_t)B, Bp, rows * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
+           make_tmap_u8_box(x8, T.x8, models, rows, (uint64_t)B, Bp, rows * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
   };
   auto dw_set = [&](GemmMaps& g, int set, const Pl& A, const Pt& AT, uint64_t am, const Pl& Bo, const Pt& BT, uint64_t bm,
                     uint64_t bcols) {
@@ -490,17 +483,10 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
     ok &= dw_set(m->dw_enc, 0, DZ, DZT, M, X, XT, xm, dd);
     ok &= dw_set(m->dw_enc, 1, C, CT, M, G, GT, M, dd);
   }
-  if (f8 && SCE_EPI_PAIR) {
-    // two adjacent chunks per bulk store (stage_pair_and_store): boxes of 64 columns x 32 rows, 128-byte rows
-    ok &= make_tmap_bf16_box(&m->st_c_hi, p->c_hi, M, (uint64_t)B, n, n, Bm * n, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B);
-    ok &= make_tmap_bf16_box(&m->st_dz_hi, p->dz_hi, M, (uint64_t)B, n, n, Bm * n, 64, 32, CU_TENSOR_MAP_SWIZZLE_128B);
-  } else {
-    ok &= make_tmap_bf16_store32(&m->st_c_hi, p->c_hi, M, (uint64_t)B, n, Bm * n);
-    ok &= make_tmap_bf16_store32(&m->st_dz_hi, p->dz_hi, M, (uint64_t)B, n, Bm * n);
-  }
+  ok &= make_tmap_bf16_store32(&m->st_c_hi, p->c_hi, M, (uint64_t)B, n, Bm * n);
+  ok &= make_tmap_bf16_store32(&m->st_dz_hi, p->dz_hi, M, (uint64_t)B, n, Bm * n);
   if (f8) {
     auto st8 = [&](CUtensorMap* t, const void* base) {
-      if (SCE_EPI_PAIR) return make_tmap_u8_box(t, base, M, (uint64_t)B, n, n, Bm * n, 64, 32, CU_TENSOR_MAP_SWIZZLE_64B);
       return make_tmap_u8_box(t, base, M, (uint64_t)B, n, n, Bm * n, 32, 32, CU_TENSOR_MAP_SWIZZLE_32B);
     };
     // dw_native: dz's 8-bit planes [M][n][Bp], boxes of 32 features x 32 batch bytes (EpiDcodeT<f16f8, true>)
@@ -535,24 +521,10 @@ struct ResFlags {
 
 // NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN then describe the fp16
 // planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps batch-major copies.
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC = false, int ARITH = kArithBf16x3,
-          bool NATIVE = ARITH == kArithF16F8 && !A_MN>
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool NATIVE = ARITH == kArithF16F8 && !A_MN>
 static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, const int* a_batched,
                          const int* b_batched, int k_total, int passes, int m_total, int n_total,
                          const typename Epi::Params& epi, cudaStream_t st, const ResFlags& rf = ResFlags()) {
-  constexpr int BK = ARITH == kArithF16F8 ? kBkF8 : kBkBf16;
-  // f16f8: K-major 8-bit maps carry the swizzle of the native path (operand_maps), MN-major ones are widened
-  static_assert(ARITH != kArithF16F8 || A_MN == B_MN, "f16f8 GEMMs are K-major or MN-major on both sides");
-  static_assert(!NATIVE || ARITH == kArithF16F8, "E5M2 cross terms are an f16f8 path");
-  constexpr int STAGES = gemm_stages<BK, Epi::kWarpStageBytes, ARITH, NATIVE>();
-  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH, NATIVE>;
-  auto kern = gemm_split_kernel<Epi, BK, A_MN, B_MN, STAGES, SPLIT_ACC, ARITH, NATIVE>;
-  // the opt-in to > 48 KB of dynamic shared memory is per device: remember which devices have it
-  static bool configured[64] = {};
-  if (p->device < 0 || p->device >= 64 || !configured[p->device]) {
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes));
-    if (p->device >= 0 && p->device < 64) configured[p->device] = true;
-  }
   GemmParams<typename Epi::Params> gp;
   memset(&gp, 0, sizeof(gp));
   for (int s = 0; s < nsets; ++s) {
@@ -576,16 +548,8 @@ static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, con
   gp.tiles_m = (m_total + kBM - 1) / kBM;
   gp.tiles_n = (n_total + kBN - 1) / kBN;
   gp.epi = epi;
-  const int tiles = gp.n_models * gp.tiles_m * gp.tiles_n;   // persistent: at most one CTA per SM
-  kern<<<tiles < p->sms ? tiles : p->sms, kGemmThreads, SM::kBytes, st>>>(gp);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY((launch_gemm<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, NATIVE>(gp, p->device, p->sms, st)));
   return SCE_OK;
-}
-
-// Dispatch a K-major-A GEMM (f16f8 rescales inside one accumulator: never split)
-template <class Epi, bool B_MN, bool SPLIT, int ARITH, class... Args>
-static int launch_k(Args&&... a) {
-  return launch_gemm_t<Epi, false, B_MN, SPLIT && ARITH != kArithF16F8, ARITH>(a...);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -704,7 +668,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     cp.model_stride = (long long)B * dd;
     cp.ld = dd;
     cp.col_scale = p->b.center_scale;
-    rc = launch_k<EpiCenter, false, false, AR>(p, maps->center, 1, one, one, dd, 3, B, dd, cp, st);
+    rc = launch_gemm_t<EpiCenter, false, false, false, AR>(p, maps->center, 1, one, one, dd, 3, B, dd, cp, st);
     if (rc) return rc;
     launches += 2;
     x = p->x_centered;
@@ -771,11 +735,11 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       fill(ep);
       ep.mom_part = mom_part;
       ep.row_blocks = (B + 31) / 32;
-      rc = launch_k<EpiStats, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+      rc = launch_gemm_t<EpiStats, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
     } else {
       typename EpiEnc::Params ep;
       fill(ep);
-      rc = launch_k<EpiEnc, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+      rc = launch_gemm_t<EpiEnc, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
     }
     if (rc) return rc;
     ++launches;
@@ -790,14 +754,10 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       sp.n_chunks = act.n_chunks;
       sp.cmax_model_stride = (long long)Bm * act.n_chunks;
     }
-    rc = launch_k<EpiScoresTma, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, sp, st, x_is_a);
+    rc = launch_gemm_t<EpiScoresTma, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, sp, st, x_is_a);
     if (rc) return rc;
     ++launches;
-    static bool cfg[64] = {};
-    if (p->device < 0 || p->device >= 64 || !cfg[p->device]) {
-      CUDA_TRY(cudaFuncSetAttribute(topk_sparse_kernel<AR>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
-      if (p->device >= 0 && p->device < 64) cfg[p->device] = true;
-    }
+    CUDA_TRY(opt_in_smem<topk_sparse_kernel<AR>>(112 * 1024, p->device));
     tk.col = p->tk_col;
     tk.val = p->tk_val;
     tk.cnt = p->tk_cnt;
@@ -847,11 +807,11 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
   dp.tiles_n = (dd + kBN - 1) / kBN;
   if constexpr (f8)
-    rc = launch_k<EpiDec, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    rc = launch_gemm_t<EpiDec, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
   else if (p->split_decode)
-    rc = launch_k<EpiDec, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    rc = launch_gemm_t<EpiDec, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
   else
-    rc = launch_k<EpiDec, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    rc = launch_gemm_t<EpiDec, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
   if (rc) return rc;
   ++launches;
   n_dec_parts = tiles_mB * 8 * dp.tiles_n;
@@ -893,7 +853,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
       // (per-model batches carry one flag for all of them, so the same test holds)
       zp.x_res_flag = f8 ? p->res_flags : nullptr;
-      return launch_k<E, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
+      return launch_gemm_t<E, false, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
     };
     // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
     if constexpr (f8) rc = p->dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
@@ -1305,11 +1265,6 @@ static int sim_planes(const SimOperand& o, int d, void* hi, void* lo, void* x8, 
 template <int AR>
 static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_a, int d, int n_pairs, const SimCarve& w,
                             float* row_max, float* col_max, float* capacity, int device, int sms, cudaStream_t st) {
-  constexpr int BK = AR == kArithF16F8 ? kBkF8 : kBkBf16;
-  constexpr bool NATIVE = AR == kArithF16F8;
-  constexpr int STAGES = gemm_stages<BK, EpiSimilarity::kWarpStageBytes, AR, NATIVE>();
-  using SM = GemmSmem<BK, STAGES, EpiSimilarity::kWarpStageBytes, AR, NATIVE>;
-  auto kern = gemm_split_kernel<EpiSimilarity, BK, false, false, STAGES, false, AR, NATIVE>;
   int rc = sim_planes<AR>(A, d, w.a_hi, w.a_lo, w.a_x8, w.flags, st);
   if (rc) return rc;
   if (!b_is_a) {
@@ -1323,9 +1278,9 @@ static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_
   memset(&gp, 0, sizeof(gp));
   // both operands are dictionary rows, K-major over d: the encode GEMM's B-operand geometry on both sides
   bool ok = operand_maps(AR, &gp.a_hi[0], &gp.a_lo[0], &gp.a_x8[0], w.a_hi, w.a_lo, w.a_x8, A.models, A.rows, d,
-                         (uint64_t)A.rows * d, kBM, BK);
+                         (uint64_t)A.rows * d, kBM, gemm_bk(AR));
   ok = ok && operand_maps(AR, &gp.b_hi[0], &gp.b_lo[0], &gp.b_x8[0], b_hi, b_lo, b_x8, B.models, B.rows, d,
-                          (uint64_t)B.rows * d, kBN, BK);
+                          (uint64_t)B.rows * d, kBN, gemm_bk(AR));
   if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (similarity: na=%d, nb=%d, d=%d)", A.rows, B.rows, d);
   gp.a_batched[0] = gp.b_batched[0] = 1;
   gp.nsets = 1;
@@ -1346,14 +1301,7 @@ static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_
   gp.epi.tiles_n = gp.tiles_n;
   if (row_max) CUDA_TRY(cudaMemsetAsync(row_max, 0, (size_t)n_pairs * A.rows * sizeof(float), st));
   if (col_max) CUDA_TRY(cudaMemsetAsync(col_max, 0, (size_t)n_pairs * B.rows * sizeof(float), st));
-  static bool configured[64] = {};
-  if (device < 0 || device >= 64 || !configured[device]) {
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes));
-    if (device >= 0 && device < 64) configured[device] = true;
-  }
-  const long long tiles = (long long)n_pairs * gp.tiles_m * gp.tiles_n;   // persistent: at most one CTA per SM
-  kern<<<(unsigned)(tiles < sms ? tiles : sms), kGemmThreads, SM::kBytes, st>>>(gp);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY((launch_gemm<EpiSimilarity, false, false, false, AR, AR == kArithF16F8>(gp, device, sms, st)));
   auto to_float = [&](float* v, long long n) -> int {
     const int blocks = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
     key_to_float_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<uint32_t*>(v), n);

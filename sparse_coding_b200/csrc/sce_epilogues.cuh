@@ -12,12 +12,6 @@
 #pragma once
 #include "sce_gemm.cuh"
 
-#ifndef SCE_EPI_PAIR
-// f16f8 encode / dcode epilogues: 1 = two adjacent chunks per bulk store (stage_pair_and_store), 0 = one chunk per store
-// (the default; the paired form is kept as a build option only).
-#define SCE_EPI_PAIR 0
-#endif
-
 namespace sce {
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -106,52 +100,6 @@ __device__ __forceinline__ void stage_and_store(uint8_t* stage, int lane, const 
 }
 
 // ------------------------------------------------------------------------------------------------
-// f16f8, two adjacent 32-column chunks per bulk store (Epi::kPairChunks): an epilogue warp stages the chunks 2q and 2q+1 of
-// its rows side by side — fp16 tile of 32 rows x 128 B (128-byte swizzle), two 8-bit tiles of 32 rows x 64 B (64-byte
-// swizzle), 8 KB per warp — and hands each tile to the TMA engine ONCE per pair: three bulk stores and one wait for the
-// staging tile per 64 columns instead of per 32, and the fp16 plane goes out in full
-// 128-byte lines. `half` = which chunk of the pair this is; `last` = no further chunk of this pair follows (second half,
-// or the first half at the ragged right edge: the engine clips the columns beyond the tensor).
-// ------------------------------------------------------------------------------------------------
-constexpr int kPairStageBytes = 8192;
-__device__ __forceinline__ void stage_pair_and_store(uint8_t* stage, int lane, int half, bool last, const uint32_t (&whi)[16],
-                                                     const uint32_t (&wx)[16], const CUtensorMap* m_hi,
-                                                     const CUtensorMap* m_lo, const CUtensorMap* m_x8, int pair_col, int row0,
-                                                     int model, int planes) {
-  if (half == 0) {
-    if (lane == 0) tma_store_wait_read();   // the previous pair's stores have read the staging tiles
-    __syncwarp();
-  }
-  {
-    const int sw = lane & 7;   // 128-byte rows: 16-byte piece index ^= row & 7
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-      *reinterpret_cast<uint4*>(stage + lane * 128 + (((4 * half + q) ^ sw) << 4)) =
-          make_uint4(whi[4 * q], whi[4 * q + 1], whi[4 * q + 2], whi[4 * q + 3]);
-  }
-  {
-    const int sw = (lane >> 1) & 3;   // 64-byte rows: piece index ^= (row >> 1) & 3
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int off = lane * 64 + (((2 * half + q) ^ sw) << 4);
-      if (planes & 1) *reinterpret_cast<uint4*>(stage + 4096 + off) = make_uint4(wx[4 * q], wx[4 * q + 1], wx[4 * q + 2], wx[4 * q + 3]);
-      if (planes & 2)
-        *reinterpret_cast<uint4*>(stage + 6144 + off) = make_uint4(wx[8 + 4 * q], wx[9 + 4 * q], wx[10 + 4 * q], wx[11 + 4 * q]);
-    }
-  }
-  if (last) {
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      tma_store_3d(m_hi, stage, pair_col, row0, model);
-      if (planes & 1) tma_store_3d(m_lo, stage + 4096, pair_col, row0, model);
-      if (planes & 2) tma_store_3d(m_x8, stage + 6144, pair_col, row0, model);
-      tma_store_commit();
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // (hi, lo) split of two fp32 values into packed bf16x2 words: one packed conversion per pair for hi
 // and one for lo (cvt.rn.bf16x2.f32), the residual formed on the fp32 pipe.
 // ------------------------------------------------------------------------------------------------
@@ -236,8 +184,7 @@ struct EncodeMomentParams<true> {
 template <int ARITH, bool STATS = false>
 struct EpiEncodeT {
   static constexpr int kCols = 32;
-  static constexpr bool kPairChunks = ARITH == kArithF16F8 && SCE_EPI_PAIR != 0;
-  static constexpr int kWarpStageBytes = kPairChunks ? kPairStageBytes : 4096;
+  static constexpr int kWarpStageBytes = 4096;
   struct Params : EncodeMomentParams<STATS> {
     CUtensorMap out_hi, out_lo, out_x8;  // store maps of the code planes: [M][B][n], box 32 x 32
     const float* bias;             // [M, n] or nullptr
@@ -326,14 +273,8 @@ struct EpiEncodeT {
       P.act.pos[w] = pos;
       if (P.act.zero) P.act.zero[w] = zero;
     }
-    if constexpr (kPairChunks) {
-      const int half = (c >> 5) & 1;
-      stage_pair_and_store(stage, T.lane, half, half == 1 || col + 32 >= n_total, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8,
-                           col - 32 * half, T.m_blk * kBM + T.warp_q * 32, T.model, 3);
-    } else {
-      stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
-                             T.m_blk * kBM + T.warp_q * 32, T.model);
-    }
+    stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, T.m_blk * kBM + T.warp_q * 32,
+                           T.model);
     if constexpr (STATS) {
       if (T.m_blk * kBM + T.warp_q * 32 < m_total) {   // warp-uniform: some row of this warp is in the batch
         float* o = P.mom_part + ((long long)T.model * P.row_blocks + T.m_blk * 4 + T.warp_q) * 4 * n_total + col + T.lane;
@@ -458,11 +399,7 @@ struct EpiDecodeT {
 template <int ARITH, bool T8 = false>
 struct EpiDcodeT {
   static constexpr int kCols = 32;
-  static constexpr bool kPairChunks = ARITH == kArithF16F8 && SCE_EPI_PAIR != 0;
-  static_assert(!(T8 && kPairChunks), "SCE_EPI_PAIR=1 has no transposed dz store: build f16f8 without it");
-  static constexpr int kWarpStageBytes = kPairChunks ? kPairStageBytes : 4096;
-  // column offset of this warp's next chunk after the one at offset c (see the epilogue loop of gemm_split_kernel)
-  static __device__ __forceinline__ int next_chunk(int c) { return kPairChunks ? (((c >> 5) & 1) ? c + 96 : c + 32) : c + 64; }
+  static constexpr int kWarpStageBytes = 4096;
   struct Params {
     CUtensorMap out_hi, out_lo, out_x8;  // store maps of the dz planes: [M][B][n] (T8: 8-bit ones [M][n][B]), box 32 x 32
     ActMask act;                  // [c > 0] / [z == 0] written by encode (or the top-k selection)
@@ -496,13 +433,13 @@ struct EpiDcodeT {
     aB = __ldg(P.l1_over_b + T.model);
     planes = P.planes;
     if (P.x_res_flag && __ldg(P.x_res_flag) == 0u) planes &= ~1;
-    fetch_mask(kPairChunks ? T.grp * 64 : T.grp * 32);
+    fetch_mask(T.grp * 32);
   }
 
   __device__ __forceinline__ void chunk(int c, const uint32_t (&r)[32]) {
     const int col = T.col0 + c;
     const uint32_t pos = pos_n, zero = zero_n;
-    fetch_mask(next_chunk(c));  // this warp's next chunk
+    fetch_mask(c + 64);  // this warp's next chunk
     if (col >= n_total) return;  // warp-uniform
     float dz[32];
     uint32_t whi[16], wlo[16];
@@ -526,14 +463,8 @@ struct EpiDcodeT {
         split_pair<ARITH>(v0, v1, j >> 1, whi, wlo);
       }
     }
-    if constexpr (kPairChunks) {
-      const int half = (c >> 5) & 1;
-      stage_pair_and_store(stage, T.lane, half, half == 1 || col + 32 >= n_total, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8,
-                           col - 32 * half, T.m_blk * kBM + T.warp_q * 32, T.model, planes);
-    } else {
-      stage_and_store<ARITH, T8>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
-                                 T.m_blk * kBM + T.warp_q * 32, T.model, planes);
-    }
+    stage_and_store<ARITH, T8>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
+                               T.m_blk * kBM + T.warp_q * 32, T.model, planes);
     if (P.db_part && T.m_blk * kBM < m_total) {  // warp-uniform
       // transpose-reduce: 32 lanes x 32 columns -> lane j holds the sum of column j (31 shuffles)
 #pragma unroll

@@ -5,13 +5,13 @@
 // This is how the engine reaches the reference's true-FP32 results (SURVEY.md H1) on the 16-bit tensor cores.
 // Every fp32 operand is carried as operand planes and the product formed from partial products:
 //   ARITH = bf16x3: x ~= hi + lo (two bf16 planes); hi*hi + hi*lo + lo*hi, three bf16 passes (~2^-16);
-//   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h on the fp16 planes, the two cross terms on E5M2 planes (E5M2 wgmma
-//                   where the 8-bit planes are K-major, else widened to fp16 in shared memory), rescaled in the
-//                   accumulator (see sce_ptx.cuh) — the default.
+//   ARITH = f16f8 : x ~= h + l, h = fp16(x); h*h on the fp16 planes, the two cross terms on E5M2 planes, rescaled in
+//                   the accumulator (see sce_ptx.cuh) — the default.
 // `passes == 1` keeps only the 16-bit plane product. Operands may be K-major (reduction index contiguous in HBM) or
-// MN-major (row/column index contiguous). Under F8_NATIVE the 8-bit planes are always K-major and A_MN / B_MN describe
-// the fp16 planes only, so an MN-major GEMM (the weight gradient) runs natively from batch-major copies of its 8-bit
-// planes.
+// MN-major (row/column index contiguous); f16f8 GEMMs are one or the other on both sides. The f16f8 cross terms run on
+// E5M2 wgmma (F8_NATIVE), which reads K-major 8-bit tiles only: A_MN / B_MN then describe the fp16 planes alone, and an
+// MN-major GEMM (the weight gradient) reads batch-major copies of its 8-bit planes. Without those copies (top-k and
+// launch-bound plans) the MN-major weight gradient widens its 8-bit tiles to fp16 in shared memory instead.
 //
 // One CTA per SM, 384 threads: warp 0 = TMA producer (one thread), warpgroups 1 and 2 = wgmma consumers (rows 0..63
 // and 64..127 of the 128 x 128 tile), which then run the fused epilogue. The accumulators go through a padded fp32
@@ -65,13 +65,19 @@ struct GemmParams {
 
 constexpr int kArithBf16x3 = 0, kArithF16F8 = 1;
 
+// K block of every GEMM of an arithmetic; a K-major 16-bit tile row is then one swizzle span (64 or 128 bytes).
+// bf16x3: 32 (a stage of the four bf16 planes is 32 KB, so several stages fit beside the accumulator tile).
+// f16f8: 64 (a stage holds one 16-bit plane per operand, or the four 8-bit planes in the same bytes).
+__host__ __device__ constexpr int gemm_bk(int arith) { return arith == kArithF16F8 ? 64 : 32; }
+
 constexpr int align1k(int v) { return (v + 1023) / 1024 * 1024; }
 
-// F8_NATIVE (f16f8, 8-bit planes K-major): the cross terms run on E5M2 wgmma from the stage, nothing is widened.
-template <int BK, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
-struct GemmSmemLayout {
-  static constexpr int kATile = kBM * BK * 2;   // bytes of one 16-bit A tile
-  static constexpr int kBTile = kBN * BK * 2;
+// Shared memory of one CTA. F8_NATIVE (f16f8): the cross terms run on E5M2 wgmma from the stage, nothing is widened.
+template <int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE>
+struct GemmSmem {
+  static constexpr int kBK = gemm_bk(ARITH);
+  static constexpr int kATile = kBM * kBK * 2;   // bytes of one 16-bit A tile
+  static constexpr int kBTile = kBN * kBK * 2;
   // bf16x3: hi and lo planes of A and B. f16f8: either the fp16 planes or the four 8-bit planes (same bytes).
   static constexpr int kStage = ARITH == kArithBf16x3 ? 2 * kATile + 2 * kBTile : kATile + kBTile;
   static constexpr int kAccLd = kBN + 1;         // padded row of the fp32 accumulator tile (conflict-free both ways)
@@ -80,31 +86,14 @@ struct GemmSmemLayout {
   static constexpr int kWideBytes = ARITH == kArithF16F8 && !F8_NATIVE ? 2 * kATile + 2 * kBTile : 0;
   static constexpr int kAccRegion = align1k(kAccBytes > kWideBytes ? kAccBytes : kWideBytes);
   static constexpr int kFixed = kAccRegion + kEpiWarps * EPI_WARP_BYTES + 1024 /*barriers*/ + 1024 /*align slack*/;
-  static constexpr int kMaxStages = (kSmemLimit - kFixed) / kStage;
-};
-
-template <int BK, int STAGES, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
-struct GemmSmem : GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH, F8_NATIVE> {
-  using L = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH, F8_NATIVE>;
-  static constexpr int kAccOff = STAGES * L::kStage;
-  static constexpr int kEpiOff = kAccOff + L::kAccRegion;
+  // pipeline depth: as many stages as fit beside the accumulator tile and the epilogue staging (at most 8)
+  static constexpr int kStages = (kSmemLimit - kFixed) / kStage > 8 ? 8 : (kSmemLimit - kFixed) / kStage;
+  static constexpr int kAccOff = kStages * kStage;
+  static constexpr int kEpiOff = kAccOff + kAccRegion;
   static constexpr int kBarOff = kEpiOff + kEpiWarps * EPI_WARP_BYTES;
   static constexpr int kBytes = kBarOff + 1024 + 1024;
   static_assert(kBytes <= kSmemLimit, "exceeds the 227 KB of shared memory one CTA may use");
 };
-
-// pipeline depth: as many stages as fit beside the accumulator tile and the epilogue staging (at most 8)
-template <int BK, int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE = false>
-constexpr int gemm_stages() {
-  constexpr int s = GemmSmemLayout<BK, EPI_WARP_BYTES, ARITH, F8_NATIVE>::kMaxStages;
-  return s > 8 ? 8 : s;
-}
-
-// epilogues may declare `static constexpr bool kPairChunks = true` (see the epilogue loop of gemm_split_kernel)
-template <class Epi, class = void>
-struct epi_pairs_chunks : std::false_type {};
-template <class Epi>
-struct epi_pairs_chunks<Epi, std::void_t<decltype(Epi::kPairChunks)>> : std::bool_constant<Epi::kPairChunks> {};
 
 // epilogues may declare `static constexpr bool kPairTiles = true`: the tile's `model` index is then a PAIR index, and the
 // operand models of pair q are read from the device list Epi::Params::pairs ([q][2] = model of A, model of B) instead of
@@ -114,12 +103,12 @@ struct epi_pair_tiles : std::false_type {};
 template <class Epi>
 struct epi_pair_tiles<Epi, std::void_t<decltype(Epi::kPairTiles)>> : std::bool_constant<Epi::kPairTiles> {};
 
-// f16f8 without F8_NATIVE: an 8-bit tile as TMA delivers it without swizzle — K-major [ROWS][BK] or MN-major [BK][ROWS] bytes — widened
-// to the fp16 tile the 16-bit loads of the same operand produce: K-major [ROWS][BK] with the 128-byte swizzle (BK = 64),
-// MN-major [ROWS / 64][BK][64] with the 128-byte swizzle. 256 consumer threads, 16 bytes each per round.
-template <bool MN, int BK, int ROWS>
+// f16f8 without F8_NATIVE (MN-major operands): an MN-major 8-bit tile as TMA delivers it without swizzle, [BK][ROWS]
+// bytes, widened to the fp16 tile the 16-bit loads of the same operand produce, [ROWS / 64][BK][64] with the 128-byte
+// swizzle. 256 consumer threads, 16 bytes each per round.
+template <int ROWS>
 __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int tid) {
-  static_assert(BK == 64, "the widened K-major tile has 128-byte rows");
+  constexpr int BK = gemm_bk(kArithF16F8);
   constexpr int kPieces = ROWS * BK / 16;
 #pragma unroll 2
   for (int q = tid; q < kPieces; q += 256) {
@@ -129,19 +118,10 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
     widen_e5m2x4(v.y, w0.z, w0.w);
     widen_e5m2x4(v.z, w1.x, w1.y);
     widen_e5m2x4(v.w, w1.z, w1.w);
-    int o0, o1;
-    if constexpr (!MN) {
-      const int r = q / (BK / 16), j = (q % (BK / 16)) * 2;   // 16-byte chunk of the 128-byte fp16 row
-      o0 = r * 128 + ((j ^ (r & 7)) << 4);
-      o1 = r * 128 + (((j + 1) ^ (r & 7)) << 4);
-    } else {
-      const int k = q / (ROWS / 16), m0 = (q % (ROWS / 16)) * 16;
-      const int base = (m0 >> 6) * (BK * 128) + k * 128, j = (m0 & 63) >> 3;
-      o0 = base + ((j ^ (k & 7)) << 4);
-      o1 = base + (((j + 1) ^ (k & 7)) << 4);
-    }
-    *reinterpret_cast<uint4*>(dst + o0) = w0;
-    *reinterpret_cast<uint4*>(dst + o1) = w1;
+    const int k = q / (ROWS / 16), m0 = (q % (ROWS / 16)) * 16;
+    const int base = (m0 >> 6) * (BK * 128) + k * 128, j = (m0 & 63) >> 3;
+    *reinterpret_cast<uint4*>(dst + base + ((j ^ (k & 7)) << 4)) = w0;
+    *reinterpret_cast<uint4*>(dst + base + (((j + 1) ^ (k & 7)) << 4)) = w1;
   }
 }
 
@@ -156,21 +136,22 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
 //
 // ARITH = kArithF16F8 (see sce_ptx.cuh, "fp16 + fp8 arithmetic"): a tile makes TWO sweeps over K. Sweep 1 streams the
 // 8-bit planes (a stage holds A.h8, A.l8, B.h8, B.l8 — the same bytes as A.f16 + B.f16) and accumulates the cross terms;
-// the accumulator is then scaled by 2^-kLoShift; sweep 2 streams the fp16 planes and adds hh. F8_NATIVE (both operands
-// K-major, 8-bit tiles loaded with the 64-byte swizzle): sweep 1 runs E5M2 wgmma on the stage itself. Otherwise the 8-bit
-// tiles arrive unswizzled and are widened to fp16 in shared memory first. Under F8_NATIVE, A_MN / B_MN describe the fp16
-// planes only (sweep 2): the 8-bit tiles are K-major whatever the fp16 planes' layout, because E5M2 wgmma reads no other.
-template <class Epi, int BK, bool A_MN, bool B_MN, int STAGES, bool SPLIT_ACC = false, int ARITH = kArithBf16x3,
-          bool F8_NATIVE = false>
+// the accumulator is then scaled by 2^-kLoShift; sweep 2 streams the fp16 planes and adds hh. F8_NATIVE (8-bit tiles
+// K-major, loaded with the 64-byte swizzle): sweep 1 runs E5M2 wgmma on the stage itself; A_MN / B_MN describe the fp16
+// planes only (sweep 2), because E5M2 wgmma reads no layout but K-major. Otherwise (MN-major operands) the 8-bit tiles
+// arrive unswizzled and MN-major, and are widened to fp16 in shared memory first.
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
   constexpr int BN = kBN;
   static_assert(!F8 || !SPLIT_ACC, "f16f8 rescales in the accumulator; no split accumulators");
   static_assert(!F8_NATIVE || F8, "F8_NATIVE is an f16f8 path");
-  static_assert(!F8 || BK == 64, "f16f8: K block 64");
-  static_assert(BK == 32 || BK == 64, "BK in {32, 64}: one swizzled row (64 or 128 B) per K-major tile row");
-  using SM = GemmSmem<BK, STAGES, Epi::kWarpStageBytes, ARITH, F8_NATIVE>;
+  static_assert(!F8 || A_MN == B_MN, "f16f8 GEMMs are K-major or MN-major on both sides");
+  static_assert(!F8 || F8_NATIVE || (A_MN && B_MN), "the widened f16f8 path is MN-major on both sides");
+  using SM = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>;
+  constexpr int BK = SM::kBK;
+  constexpr int STAGES = SM::kStages;
   constexpr int EC = Epi::kCols;  // accumulator columns handed to the epilogue per call
   static_assert(EC == 32, "epilogue chunk is 32 columns");
 
@@ -278,15 +259,14 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
                     for (int j = 0; j < BN / 64; ++j) tma_load_3d(sb + j * (BK * 128), &p.b_hi[set], bar, b_row0 + j * 64, k0, bm);
                   }
                 } else {
-                  // 8-bit tiles: K-major [rows][BK] bytes (F8_NATIVE: always, 64-byte swizzle), else unswizzled K-major
-                  // [rows][BK] or MN-major [BK][128] bytes
+                  // 8-bit tiles: F8_NATIVE K-major [rows][BK] bytes (64-byte swizzle), else MN-major [BK][128] bytes
+                  // (unswizzled)
                   uint8_t* sa_h = st;
                   uint8_t* sa_l = st + SM::kATile / 2;
                   uint8_t* sb_h = st + SM::kATile;
                   uint8_t* sb_l = sb_h + SM::kBTile / 2;
-                  constexpr bool A8_MN = A_MN && !F8_NATIVE, B8_MN = B_MN && !F8_NATIVE;
-                  const int ac0 = A8_MN ? a_row0 : k0, ac1 = A8_MN ? k0 : a_row0;
-                  const int bc0 = B8_MN ? b_row0 : k0, bc1 = B8_MN ? k0 : b_row0;
+                  const int ac0 = F8_NATIVE ? k0 : a_row0, ac1 = F8_NATIVE ? a_row0 : k0;
+                  const int bc0 = F8_NATIVE ? k0 : b_row0, bc1 = F8_NATIVE ? b_row0 : k0;
                   if (t_hl) tma_load_3d(sa_h, &p.a_lo[set], bar, ac0, ac1, am);
                   if (t_lh) tma_load_3d(sa_l, &p.a_x8[set], bar, ac0, ac1, am);
                   if (t_lh) tma_load_3d(sb_h, &p.b_lo[set], bar, bc0, bc1, bm);
@@ -411,10 +391,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
               const uint32_t wa_h = smem_u32(wide), wa_l = wa_h + SM::kATile, wb_h = wa_l + SM::kATile,
                              wb_l = wb_h + SM::kBTile;
               consumer_sync();   // both warpgroups are done with the widened tiles (and the previous epilogue)
-              if constexpr (HL) widen_tile<A_MN, BK, kBM>(st, wide, ctid);
-              if constexpr (LH) widen_tile<A_MN, BK, kBM>(st + SM::kATile / 2, wide + SM::kATile, ctid);
-              if constexpr (LH) widen_tile<B_MN, BK, BN>(st + SM::kATile, wide + 2 * SM::kATile, ctid);
-              if constexpr (HL) widen_tile<B_MN, BK, BN>(st + SM::kATile + SM::kBTile / 2, wide + 2 * SM::kATile + SM::kBTile, ctid);
+              if constexpr (HL) widen_tile<kBM>(st, wide, ctid);
+              if constexpr (LH) widen_tile<kBM>(st + SM::kATile / 2, wide + SM::kATile, ctid);
+              if constexpr (LH) widen_tile<BN>(st + SM::kATile, wide + 2 * SM::kATile, ctid);
+              if constexpr (HL) widen_tile<BN>(st + SM::kATile + SM::kBTile / 2, wide + 2 * SM::kATile + SM::kBTile, ctid);
               fence_proxy_async_smem();   // generic-proxy writes -> visible to wgmma
               consumer_sync();
               release(stage);
@@ -514,13 +494,9 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       const float* my_row = acc_stage + (tc.warp_q * 32 + lane) * SM::kAccLd;
       constexpr int kChunks = BN / EC;
       static_assert(kChunks % 2 == 0, "the two epilogue warp groups alternate chunks");
-      // chunk order of an epilogue warp group: alternating chunks (grp, grp + 2, ...) or, for epilogues that stage two
-      // adjacent chunks per bulk store (Epi::kPairChunks), alternating PAIRS: (2 grp, 2 grp + 1), (2 grp + 4, 2 grp + 5), ...
-      constexpr bool kPairs = epi_pairs_chunks<Epi>::value;
-      static_assert(!kPairs || (EC == 32 && kChunks % 4 == 0), "paired chunks: 32-column chunks, whole pairs per group");
 #pragma unroll 1
       for (int it = 0; it < kChunks / 2; ++it) {
-        const int c = kPairs ? ((it >> 1) * 4 + 2 * tc.grp + (it & 1)) : (tc.grp + 2 * it);
+        const int c = tc.grp + 2 * it;   // epilogue warp group g takes the chunks g, g + 2, ...
         uint32_t r[EC];
 #pragma unroll
         for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(my_row[c * EC + j]);
@@ -529,6 +505,33 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       epi.finish();
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Host side
+// ------------------------------------------------------------------------------------------------
+// Opts the kernel KERN in to `bytes` of dynamic shared memory (above the default 48 KB). The opt-in is per device and
+// per kernel, so each instantiation remembers the devices it has made it on.
+template <auto KERN>
+inline cudaError_t opt_in_smem(int bytes, int device) {
+  static bool configured[64] = {};
+  if (device >= 0 && device < 64 && configured[device]) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess && device >= 0 && device < 64) configured[device] = true;
+  return e;
+}
+
+// Launches gemm_split_kernel on `st` as a persistent grid: one CTA per tile, at most one per SM (`sms` of them on
+// `device`, the current device).
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
+cudaError_t launch_gemm(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st) {
+  constexpr auto kern = gemm_split_kernel<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE>;
+  constexpr int bytes = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>::kBytes;
+  const cudaError_t e = opt_in_smem<kern>(bytes, device);
+  if (e != cudaSuccess) return e;
+  const long long tiles = (long long)p.n_models * p.tiles_m * p.tiles_n;
+  kern<<<(unsigned)(tiles < sms ? tiles : sms), kGemmThreads, bytes, st>>>(p);
+  return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------------

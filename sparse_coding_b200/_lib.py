@@ -8,6 +8,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # SCE_LIB: an alternative build of the same library (kernel A/B experiments, tools/ab_variants.sh)
 LIB_PATH = os.environ.get("SCE_LIB") or os.path.join(_HERE, "libsce.so")
@@ -115,3 +117,31 @@ def check(rc: int, what: str) -> None:
     if rc != 0:
         msg = load().sce_last_error().decode("utf-8", "replace")
         raise SceError(f"{what} failed (status {rc}): {msg}")
+
+
+def arith_code(name: str) -> int:
+    """The sce_arith code of "auto", "bf16x3" or "f16f8"."""
+    if name not in ARITH_CODE:
+        raise ValueError(f"arith must be one of {sorted(ARITH_CODE)}, got {name!r}")
+    return ARITH_CODE[name]
+
+
+def workspace(nbytes: int, device, what: str):
+    """(tensor, address): ``nbytes`` of device memory at the 1024-byte aligned address every libsce workspace needs.
+    ``nbytes`` comes from one of the size queries, which return 0 for arguments they reject (``what`` names it)."""
+    if nbytes == 0:
+        check(-1, what)
+    ws = torch.empty(nbytes + 1024, dtype=torch.uint8, device=device)
+    return ws, (ws.data_ptr() + 1023) // 1024 * 1024
+
+
+def create_plan(desc: SceDesc, bufs: SceBuffers, device):
+    """sce_plan_create with a workspace of the size ``desc`` needs, allocated on ``device`` and set in ``bufs``:
+    (plan, workspace tensor). The tensor must outlive the plan."""
+    lib = load()
+    nbytes = lib.sce_workspace_bytes(C.byref(desc))
+    ws, bufs.workspace = workspace(nbytes, device, "sce_workspace_bytes")
+    bufs.workspace_bytes = nbytes
+    plan = C.c_void_p()
+    check(lib.sce_plan_create(C.byref(desc), C.byref(bufs), C.byref(plan)), "sce_plan_create")
+    return plan, ws

@@ -159,6 +159,41 @@ static int validate(const sce_desc* d) {
   return SCE_OK;
 }
 
+// one call's rows: 1 <= B <= batch_max (`prefix` names the entry point in the message, "" for the training calls)
+static int check_rows(const sce_plan* p, int B, const char* prefix) {
+  if (B < 1 || B > p->d.batch_max)
+    return fail(SCE_ERR_INVALID, "%sB = %d outside [1, batch_max = %d]", prefix, B, p->d.batch_max);
+  return SCE_OK;
+}
+
+// a caller's workspace: at least `need` bytes at a 1024-byte aligned address (the carves align their buffers to it)
+static int check_workspace(const void* ws, size_t have, size_t need, const char* prefix) {
+  if (!ws || have < need)
+    return fail(SCE_ERR_WORKSPACE, "%sworkspace too small: have %zu bytes, need %zu", prefix, have, need);
+  if (reinterpret_cast<uintptr_t>(ws) % 1024) return fail(SCE_ERR_WORKSPACE, "%sworkspace must be 1024-byte aligned", prefix);
+  return SCE_OK;
+}
+
+// the current device and its SM count, if libsce runs on it: sm_90, with the driver's tensor-map encoder
+static int query_device(int* device, int* sm_count) {
+  int dev = 0, major = 0, sms = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (major != 9) return fail(SCE_ERR_NO_DEVICE, "libsce needs an sm_90 device (found compute capability %d.x)", major);
+  if (!get_encode_fn()) return fail(SCE_ERR_NO_DEVICE, "cuTensorMapEncodeTiled driver entry point not available");
+  *device = dev;
+  *sm_count = sms;
+  return SCE_OK;
+}
+
+// fp32 rows -> the operand planes of arithmetic AR: n4 float4s, grid-stride over at most 2048 blocks
+template <int AR>
+static void launch_split_rows(const float* x, void* hi, void* lo, void* x8, long long n4, uint32_t* flags, cudaStream_t st) {
+  const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
+  split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, hi, lo, x8, n4, flags);
+}
+
 // desc.arith -> kArithBf16x3 / kArithF16F8. AUTO: f16f8 where the 8-bit planes can be addressed by TMA
 // (row pitches of 16 bytes), bf16x3 otherwise; the environment may pin AUTO to one of them (A/B runs).
 static int resolve_arith(const sce_desc& d) {
@@ -642,7 +677,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   using EpiDco = EpiDcodeT<AR>;
   constexpr bool f8 = AR == kArithF16F8;
   const sce_desc& d = p->d;
-  if (B < 1 || B > d.batch_max) return fail(SCE_ERR_INVALID, "B = %d outside [1, batch_max = %d]", B, d.batch_max);
+  if (int rc = check_rows(p, B, "")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
   BatchMaps* maps = nullptr;
   int rc = build_maps(p, B, &maps);
@@ -676,13 +711,10 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace
   if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), st));
   for (int m = 0; m < p->xm; ++m) {
-    const long long n4 = (long long)B * dd / 4;
-    const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
     // (bf16x3: the lo plane is 2 B / element; f16f8: lo and x8 are 1 B / element)
-    split_rows_kernel<AR><<<blocks, 256, 0, st>>>(
-        x + (long long)m * B * dd, p->x_hi + m * Bm * dd,
-        f8 ? (void*)(reinterpret_cast<uint8_t*>(p->x_lo) + m * Bm * dd) : (void*)(p->x_lo + m * Bm * dd),
-        f8 ? (void*)(p->x_x8 + m * Bm * dd) : nullptr, n4, f8 ? p->res_flags : nullptr);
+    launch_split_rows<AR>(x + (long long)m * B * dd, p->x_hi + m * Bm * dd,
+                          f8 ? (void*)(reinterpret_cast<uint8_t*>(p->x_lo) + m * Bm * dd) : (void*)(p->x_lo + m * Bm * dd),
+                          f8 ? (void*)(p->x_x8 + m * Bm * dd) : nullptr, (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st);
     ++launches;
   }
   CUDA_TRY(cudaGetLastError());
@@ -1255,9 +1287,7 @@ static int sim_planes(const SimOperand& o, int d, void* hi, void* lo, void* x8, 
   if (o.normalize)
     return launch_dict_rows_t<MODE_PREPARE, AR>(const_cast<float*>(o.w), nullptr, nullptr, nullptr, hi, lo, x8, nullptr, rows, d,
                                                  1, o.floor, AdamHyper{}, nullptr, nullptr, st);
-  const long long n4 = rows * d / 4;
-  const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  split_rows_kernel<AR><<<blocks, 256, 0, st>>>(o.w, hi, lo, x8, n4, AR == kArithF16F8 ? flags : nullptr);
+  launch_split_rows<AR>(o.w, hi, lo, x8, rows * d / 4, AR == kArithF16F8 ? flags : nullptr, st);
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }
@@ -1344,17 +1374,11 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   if (desc->variant != SCE_TOPK && (!b.encoder_bias || !b.bias_m || !b.bias_v))
     return fail(SCE_ERR_INVALID, "encoder_bias / bias_m / bias_v are required for SAE variants");
   if (desc->variant == SCE_TOPK && !b.sparsity) return fail(SCE_ERR_INVALID, "top-k variant needs the sparsity buffer");
-  const size_t need = carve(nullptr, *desc, nullptr);
-  if (!b.workspace || b.workspace_bytes < need)
-    return fail(SCE_ERR_WORKSPACE, "workspace too small: have %zu bytes, need %zu", b.workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(b.workspace) % 1024)
-    return fail(SCE_ERR_WORKSPACE, "workspace must be 1024-byte aligned");
-  int dev = 0, major = 0, sms = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  if (major != 9) return fail(SCE_ERR_NO_DEVICE, "libsce needs an sm_90 device (found compute capability %d.x)", major);
-  if (!get_encode_fn()) return fail(SCE_ERR_NO_DEVICE, "cuTensorMapEncodeTiled driver entry point not available");
+  rc = check_workspace(b.workspace, b.workspace_bytes, carve(nullptr, *desc, nullptr), "");
+  if (rc) return rc;
+  int dev = 0, sms = 0;
+  rc = query_device(&dev, &sms);
+  if (rc) return rc;
   sce_plan* p = new (std::nothrow) sce_plan;
   if (!p) return fail(SCE_ERR_INVALID, "out of host memory");
   memset(p, 0, sizeof(*p));
@@ -1461,11 +1485,10 @@ int sce_prepare(sce_plan* p, void* stream) {
     if (!p->b.center_trans || !p->b.center_rot || !p->b.center_scale)
       return fail(SCE_ERR_INVALID, "centering needs the center_trans / center_rot / center_scale buffers");
     const long long n4 = (long long)d.n_models * d.d * d.d / 4;
-    const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
     if (p->arith == kArithF16F8)
-      split_rows_kernel<kArithF16F8><<<blocks, 256, 0, st>>>(p->b.center_rot, p->rot_hi, p->rot_lo, p->rot_x8, n4, nullptr);
+      launch_split_rows<kArithF16F8>(p->b.center_rot, p->rot_hi, p->rot_lo, p->rot_x8, n4, nullptr, st);
     else
-      split_rows_kernel<kArithBf16x3><<<blocks, 256, 0, st>>>(p->b.center_rot, p->rot_hi, p->rot_lo, nullptr, n4, nullptr);
+      launch_split_rows<kArithBf16x3>(p->b.center_rot, p->rot_hi, p->rot_lo, nullptr, n4, nullptr, st);
     CUDA_TRY(cudaGetLastError());
   }
   AdamHyper h = hyper_for(p, 1);
@@ -1543,7 +1566,7 @@ static bool graph_eligible(const sce_plan* p) {
 int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (B < 1 || B > p->d.batch_max) return fail(SCE_ERR_INVALID, "B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (int rc = check_rows(p, B, "")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
   int rc;
   if (!graph_eligible(p)) {
@@ -1638,7 +1661,7 @@ int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_hos
                   void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
   if (!x_host) return fail(SCE_ERR_INVALID, "x_host is NULL");
-  if (B < 1 || B > p->d.batch_max) return fail(SCE_ERR_INVALID, "B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (int rc = check_rows(p, B, "")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t bytes = (size_t)input_models(p) * B * p->d.d * sizeof(float);
   CUDA_TRY(cudaMemcpyAsync(p->x_stage, x_host, bytes, cudaMemcpyHostToDevice, st));
@@ -1655,7 +1678,7 @@ int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_hos
 
 int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
   if (!p || !out_code) return fail(SCE_ERR_INVALID, "plan / out_code is NULL");
-  if (B < 1 || B > p->d.batch_max) return fail(SCE_ERR_INVALID, "B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (int rc = check_rows(p, B, "")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long per = (long long)B * p->d.n;
   if (p->code_batch_major) {
@@ -1722,7 +1745,7 @@ int sce_clear_health(sce_plan* plan, void* stream) {
 
 int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
   if (!plan || !counts) return fail(SCE_ERR_INVALID, "plan / counts is NULL");
-  if (B < 1 || B > plan->d.batch_max) return fail(SCE_ERR_INVALID, "B = %d outside [1, batch_max = %d]", B, plan->d.batch_max);
+  if (int rc = check_rows(plan, B, "")) return rc;
   const int n_chunks = (plan->d.n + 31) / 32;
   active_count_kernel<<<dim3(n_chunks, plan->d.n_models), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       plan->act_pos, n_chunks, plan->d.batch_max, B, plan->d.n, counts);
@@ -1739,7 +1762,7 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
                       float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
                       size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_stats: plan is NULL");
-  if (B < 1 || B > p->d.batch_max) return fail(SCE_ERR_INVALID, "forward_stats: B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (int rc = check_rows(p, B, "forward_stats: ")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "forward_stats: x is NULL");
   if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
   if (seg_phase < 0 || seg_phase >= seg)
@@ -1747,10 +1770,7 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
   if (!out_losses || !out_nnz || !moment_sums || !seg_counts)
     return fail(SCE_ERR_INVALID, "forward_stats: out_losses, out_nnz, moment_sums and seg_counts are required");
   if (seg > 1 && !seg_open) return fail(SCE_ERR_INVALID, "forward_stats: seg > 1 needs the seg_open flags");
-  const size_t need = stats_workspace(p->d, B);
-  if (!workspace || workspace_bytes < need)
-    return fail(SCE_ERR_WORKSPACE, "forward_stats: workspace too small: have %zu bytes, need %zu", workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(workspace) % 1024) return fail(SCE_ERR_WORKSPACE, "forward_stats: workspace must be 1024-byte aligned");
+  if (int rc = check_workspace(workspace, workspace_bytes, stats_workspace(p->d, B), "forward_stats: ")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sce_desc& d = p->d;
   const bool topk = d.variant == SCE_TOPK;
@@ -1784,8 +1804,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_fragments: plan is NULL");
-  if (B < 1 || B > p->d.batch_max)
-    return fail(SCE_ERR_INVALID, "forward_fragments: B = %d outside [1, batch_max = %d]", B, p->d.batch_max);
+  if (int rc = check_rows(p, B, "forward_fragments: ")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "forward_fragments: x is NULL");
   if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);
   if (B % L) return fail(SCE_ERR_INVALID, "forward_fragments: B = %d is not a multiple of L = %d", B, L);
@@ -1799,10 +1818,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   if (!n_active) return fail(SCE_ERR_INVALID, "forward_fragments: n_active is required");
   size_t off_active, off_open;
   const size_t need = frag_workspace(p->d, B, L, &off_active, &off_open);
-  if (!workspace || workspace_bytes < need)
-    return fail(SCE_ERR_WORKSPACE, "forward_fragments: workspace too small: have %zu bytes, need %zu", workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(workspace) % 1024)
-    return fail(SCE_ERR_WORKSPACE, "forward_fragments: workspace must be 1024-byte aligned");
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_fragments: ")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sce_desc& d = p->d;
   int rc = run_pipeline(p, x, B, nullptr, false, nullptr, nullptr, st);
@@ -1912,18 +1928,12 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
       return fail(SCE_ERR_INVALID, "similarity: rows[%d] of %s = %d outside [1, %d]", m < ma ? m : m - ma, m < ma ? "a" : "b", rows[m], n);
   }
   const size_t need = sim_workspace(ma, na, b_is_a ? 0 : mb, b_is_a ? 0 : nb, d, n_pairs, capacity != nullptr);
-  if (!workspace || workspace_bytes < need)
-    return fail(SCE_ERR_WORKSPACE, "similarity: workspace too small: have %zu bytes, need %zu", workspace_bytes, need);
-  if (reinterpret_cast<uintptr_t>(workspace) % 1024) return fail(SCE_ERR_WORKSPACE, "similarity: workspace must be 1024-byte aligned");
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "similarity: ")) return rc;
 
   // ---- device
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int dev = 0, major = 0, sms = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  if (major != 9) return fail(SCE_ERR_NO_DEVICE, "libsce needs an sm_90 device (found compute capability %d.x)", major);
-  if (!get_encode_fn()) return fail(SCE_ERR_NO_DEVICE, "cuTensorMapEncodeTiled driver entry point not available");
+  int dev = 0, sms = 0;
+  if (int rc = query_device(&dev, &sms)) return rc;
   const SimOperand A{a, ma, na, a_normalize, a_norm_floor};
   const SimOperand B = b_is_a ? A : SimOperand{b, mb, nb, b_normalize, b_norm_floor};
   // AUTO: bf16x3. Unlike the training GEMMs, whose epilogues write operand planes and which are bound by the SM's data

@@ -177,8 +177,7 @@ class FunctionalEnsemble:
         self.optimizer = resolve_optimizer(optimizer_func, optimizer_kwargs)
         self.adam_count_mode = adam_count_mode
         self.fwd_passes, self.bwd_passes = fwd_passes, bwd_passes
-        if arith not in _lib.ARITH_CODE:
-            raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
+        _lib.arith_code(arith)
         self.arith = arith
         self.materialize_code = materialize_code
         self.health_check_every = int(health_check_every)
@@ -258,13 +257,6 @@ class FunctionalEnsemble:
             arith=_lib.ARITH_CODE[getattr(self, "_arith_fallback", None) or getattr(self, "arith", "auto")],
             topk_k_max=int(self.buffers["sparsity"].max()) if self._variant == "topk" else 0,
             centering=centering)
-        nbytes = lib.sce_workspace_bytes(C.byref(desc))
-        if nbytes == 0:
-            _lib.check(-1, "sce_workspace_bytes")
-        with torch.cuda.device(dev):
-            self._ws = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-        ws_ptr = (self._ws.data_ptr() + 1023) // 1024 * 1024
-        M = self.n_models
         eb = {}
 
         def f32vec(name):  # [M] fp32 hyper-parameter buffers
@@ -300,10 +292,8 @@ class FunctionalEnsemble:
                 eb[name] = self.buffers[name].to(device=dev, dtype=torch.float32).contiguous()
             bufs.center_trans, bufs.center_rot, bufs.center_scale = (eb["center_trans"].data_ptr(), eb["center_rot"].data_ptr(),
                                                                      eb["center_scale"].data_ptr())
-        bufs.workspace, bufs.workspace_bytes = ws_ptr, nbytes
-        plan = C.c_void_p()
         with torch.cuda.device(dev):
-            _lib.check(lib.sce_plan_create(C.byref(desc), C.byref(bufs), C.byref(plan)), "sce_plan_create")
+            plan, self._ws = _lib.create_plan(desc, bufs, dev)
             self._plan = plan
             self._engine_buffers = eb
             self._plan_key = (batch_max, bool(x_per_model), int(centering))

@@ -10,9 +10,13 @@ FVU is taken in the space the model reconstructs (the centred space for Function
 centring: an orthogonal rotation leaves it unchanged, a non-uniform ``center_scale`` does not)."""
 from __future__ import annotations
 
+import contextlib
+import ctypes as C
 from typing import Dict, Iterable, Optional
 
 import torch
+
+from . import _lib
 
 EVER_ACTIVE_THRESHOLD = 10   # standard_metrics.py:446: a feature counts as "ever active" above this many rows
 
@@ -127,18 +131,20 @@ def _as_stack(x):
     raise TypeError(f"expected a FunctionalEnsemble, LearnedDict(s) or a tensor, got {type(x).__name__}")
 
 
+def _cuda_device(t: torch.Tensor, what: str) -> torch.device:
+    """Where the engine runs ``what`` on ``t``: its device if that is a CUDA device, else the current one."""
+    if t.device.type == "cuda":
+        return t.device
+    if not torch.cuda.is_available():
+        raise RuntimeError(f"{what} runs in the sm_90a CUDA engine and needs a CUDA device; there is no CPU "
+                           "implementation in the product path")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
 def _run_similarity(a: _Stack, b: Optional[_Stack], pairs, row=True, col=True, capacity=False, arith="auto"):
     """(row_max [P, na], col_max [P, nb], capacity [Ma, na]) on the CUDA device of ``a`` (None where not requested)."""
-    import ctypes as C
-    from . import _lib
-    dev = a.w.device
-    if dev.type != "cuda":
-        if not torch.cuda.is_available():
-            raise RuntimeError("dictionary similarity runs in the sm_90a CUDA engine and needs a CUDA device; there is "
-                               "no CPU implementation in the product path")
-        dev = torch.device("cuda", torch.cuda.current_device())
-    if arith not in _lib.ARITH_CODE:
-        raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
+    dev = _cuda_device(a.w, "dictionary similarity")
+    code = _lib.arith_code(arith)
     prep = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
     aw = prep(a.w)
     bw = prep(b.w) if b is not None else None
@@ -152,8 +158,7 @@ def _run_similarity(a: _Stack, b: Optional[_Stack], pairs, row=True, col=True, c
     need = lib.sce_similarity_workspace_bytes(Ma, na, Mb if bw is not None else 0, nb, d, P, int(capacity))
     if need == 0:
         raise ValueError(f"invalid similarity shape: a [{Ma}, {na}, {d}], b [{Mb}, {nb}], {P} pairs")
-    ws = torch.empty(need + 1024, dtype=torch.uint8, device=dev)
-    ws_ptr = (ws.data_ptr() + 1023) // 1024 * 1024
+    ws, ws_ptr = _lib.workspace(need, dev, "sce_similarity_workspace_bytes")
     row_max = torch.empty(P, na, dtype=torch.float32, device=dev) if row else None
     col_max = torch.empty(P, nb, dtype=torch.float32, device=dev) if col else None
     cap = torch.full((Ma, na), float("nan"), dtype=torch.float32, device=dev) if capacity else None
@@ -166,7 +171,7 @@ def _run_similarity(a: _Stack, b: Optional[_Stack], pairs, row=True, col=True, c
         stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
         _lib.check(lib.sce_similarity(
             aw.data_ptr(), Ma, na, a_rows, a_floor, a_norm, ptr(bw), Mb, nb, b_rows, b_floor, b_norm, d,
-            pv.numpy().ctypes.data_as(C.c_void_p), P, _lib.ARITH_CODE[arith], ptr(row_max), ptr(col_max), ptr(cap),
+            pv.numpy().ctypes.data_as(C.c_void_p), P, code, ptr(row_max), ptr(col_max), ptr(cap),
             ws_ptr, need, stream), "sce_similarity")
     return row_max, col_max, cap
 
@@ -348,13 +353,10 @@ def _eval_groups(lds, centre: bool, multiple: int):
     return groups
 
 
-class _EvalPlan:
-    """One forward-only plan for a group of dictionaries, with its statistics accumulators (``stats``; without them
-    the plan serves other forward-only passes, such as :func:`top_activating_fragments`)."""
+class _DictPlan:
+    """The forward-only plan of one group of dictionaries (a key of :func:`_eval_groups`), prepared on ``dev``."""
 
-    def __init__(self, key, lds, batch_max, arith, dev, stats=True):
-        import ctypes as C
-        from . import _lib
+    def __init__(self, key, lds, batch_max, arith, dev):
         kind, n_pad, d, centred = key
         M = len(lds)
         self.kind, self.M, self.n, self.d, self.centred, self.dev = kind, M, n_pad, d, centred, dev
@@ -382,25 +384,15 @@ class _EvalPlan:
             self.trans = torch.stack([f32(ld.center_trans) for ld in lds]).contiguous()
             self.rot = torch.stack([f32(ld.center_rot) for ld in lds]).contiguous()
             self.scale = torch.stack([f32(ld.center_scale) for ld in lds]).contiguous()
-        # sce_prepare and sce_forward_stats never read the Adam moments; the plan only requires their pointers
+        # sce_prepare and the forward-only passes never read the Adam moments; the plan only requires their pointers
         t["unused"] = torch.zeros(1, dtype=torch.float32, device=dev)
         self._t = t
-        lib = _lib.load()
-        desc = _lib.SceDesc(
+        self.desc = _lib.SceDesc(
             variant={"tied": _lib.SCE_TIED, "untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK}[kind], n_models=M, d=d,
             n=n_pad, batch_max=batch_max, x_per_model=int(centred), lr=0.0, beta1=0.9, beta2=0.999, eps=1e-8,
             eps_root=0.0, adam_count_mode=_lib.SCE_ADAM_FROZEN_T1, fwd_passes=3, bwd_passes=3,
-            norm_floor=0.0 if kind == "topk" else 1e-8, arith=_lib.ARITH_CODE[arith],
+            norm_floor=0.0 if kind == "topk" else 1e-8, arith=_lib.arith_code(arith),
             topk_k_max=int(t["sparsity"].max()) if kind == "topk" else 0, centering=int(centred))
-        self.desc = desc
-        nbytes = lib.sce_workspace_bytes(C.byref(desc))
-        sbytes = lib.sce_forward_stats_workspace_bytes(C.byref(desc), batch_max) if stats else 1
-        if nbytes == 0 or sbytes == 0:
-            _lib.check(-1, "sce_workspace_bytes")
-        self._ws = torch.empty(nbytes + 1024, dtype=torch.uint8, device=dev)
-        if stats:
-            self._sws = torch.empty(sbytes + 1024, dtype=torch.uint8, device=dev)
-            self.sws_ptr, self.sws_bytes = (self._sws.data_ptr() + 1023) // 1024 * 1024, sbytes
         ptr = lambda x: x.data_ptr() if x is not None else None
         u = ptr(t["unused"])
         b = _lib.SceBuffers()
@@ -413,19 +405,35 @@ class _EvalPlan:
         b.sparsity = ptr(t.get("sparsity"))
         if centred:
             b.center_trans, b.center_rot, b.center_scale = ptr(self.trans), ptr(self.rot), ptr(self.scale)
-        b.workspace, b.workspace_bytes = (self._ws.data_ptr() + 1023) // 1024 * 1024, nbytes
-        self.plan = C.c_void_p()
-        _lib.check(lib.sce_plan_create(C.byref(desc), C.byref(b), C.byref(self.plan)), "sce_plan_create")
+        self.plan, self._plan_ws = _lib.create_plan(self.desc, b, dev)
         self.stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
         try:
-            _lib.check(lib.sce_prepare(self.plan, self.stream), "sce_prepare")
+            _lib.check(_lib.load().sce_prepare(self.plan, self.stream), "sce_prepare")
         except Exception:
             self.close()
             raise
-        if not stats:
-            return
-        z = lambda dt: torch.zeros(M, n_pad, dtype=dt, device=dev)
-        self.sums = torch.zeros(M, n_pad, 4, dtype=torch.float64, device=dev)
+
+    def bad(self) -> bool:
+        flag, amax = C.c_int(0), C.c_float(0.0)
+        _lib.check(_lib.load().sce_health(self.plan, C.byref(flag), C.byref(amax), self.stream), "sce_health")
+        return bool(flag.value)
+
+    def close(self):
+        if getattr(self, "plan", None) is not None and self.plan.value:
+            _lib.load().sce_plan_destroy(self.plan)
+        self.plan = None
+
+
+class _StatsPlan(_DictPlan):
+    """A dictionary plan with the statistics accumulators of :func:`evaluate_dicts`."""
+
+    def __init__(self, key, lds, batch_max, arith, dev):
+        super().__init__(key, lds, batch_max, arith, dev)
+        M, n = self.M, self.n
+        self.ws_bytes = _lib.load().sce_forward_stats_workspace_bytes(C.byref(self.desc), batch_max)
+        self._pass_ws, self.ws_ptr = _lib.workspace(self.ws_bytes, dev, "sce_forward_stats_workspace_bytes")
+        z = lambda dt: torch.zeros(M, n, dtype=dt, device=dev)
+        self.sums = torch.zeros(M, n, 4, dtype=torch.float64, device=dev)
         self.seg_counts, self.seg_open, self.counts = z(torch.int32), z(torch.int32), z(torch.int32)
         self.sq = torch.zeros(M, dtype=torch.float64, device=dev)
         self.l0 = torch.zeros(M, dtype=torch.float64, device=dev)
@@ -433,14 +441,13 @@ class _EvalPlan:
         self.nnz = torch.empty(M, dtype=torch.float32, device=dev)
 
     def run(self, x, seg, phase):
-        from . import _lib
         lib = _lib.load()
         B, d = x.shape
         x_hat = torch.empty(self.M, B, d, dtype=torch.float32, device=self.dev) if self.centred else None
         _lib.check(lib.sce_forward_stats(
             self.plan, x.data_ptr(), B, seg, phase, x_hat.data_ptr() if x_hat is not None else None,
             self.losses.data_ptr(), self.nnz.data_ptr(), self.sums.data_ptr(), self.seg_counts.data_ptr(),
-            self.seg_open.data_ptr(), self.sws_ptr, self.sws_bytes, self.stream), "sce_forward_stats")
+            self.seg_open.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream), "sce_forward_stats")
         _lib.check(lib.sce_active_counts(self.plan, B, self.counts.data_ptr(), self.stream), "sce_active_counts")
         if x_hat is None:
             self.sq += self.losses[:, 1].double() * (B * d)
@@ -449,18 +456,53 @@ class _EvalPlan:
             self.sq += r.double().pow(2).sum(dim=(1, 2))
         self.l0 += self.nnz.double() * B
 
-    def bad(self) -> bool:
-        import ctypes as C
-        from . import _lib
-        flag, amax = C.c_int(0), C.c_float(0.0)
-        _lib.check(_lib.load().sce_health(self.plan, C.byref(flag), C.byref(amax), self.stream), "sce_health")
-        return bool(flag.value)
 
-    def close(self):
-        from . import _lib
-        if getattr(self, "plan", None) is not None and self.plan.value:
-            _lib.load().sce_plan_destroy(self.plan)
-        self.plan = None
+def _dict_inputs(learned_dicts, activations, arith, centre):
+    """(LearnedDicts, groups of :func:`_eval_groups`, arithmetic that runs) of a forward-only pass of
+    ``learned_dicts`` (LearnedDicts or ``(LearnedDict, hparams)`` pairs) over ``activations``; raises for what the
+    engine does not run."""
+    _lib.arith_code(arith)
+    lds = [ld[0] if isinstance(ld, (tuple, list)) else ld for ld in learned_dicts]
+    if not lds:
+        raise ValueError("no dictionaries to evaluate")
+    if activations.dim() != 2 or activations.shape[0] == 0:
+        raise ValueError(f"activations must be a non-empty [N, d] tensor, got shape {tuple(activations.shape)}")
+    if activations.dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"activations must be fp32 or fp16, got {activations.dtype}")
+    # AUTO runs bf16x3: the fp32 range, so activations fp16 cannot hold give finite results
+    ar = "bf16x3" if arith == "auto" else arith
+    groups = _eval_groups(lds, centre, 16 if ar == "f16f8" else 8)
+    for (kind, n_pad, dd, _), idx in groups.items():
+        if dd != activations.shape[1]:
+            raise ValueError(f"dictionary {idx[0]} has width {dd}, the activations {activations.shape[1]}")
+    return lds, groups, ar
+
+
+@contextlib.contextmanager
+def _plans(groups, lds, dev, make):
+    """[(plan, input indices)]: ``make(key, dictionaries)`` of every group, under ``dev``. Every plan built is closed on
+    exit, also when building a later one fails."""
+    plans = []
+    with torch.cuda.device(dev):
+        try:
+            for key, idx in groups.items():
+                plans.append((make(key, [lds[i] for i in idx]), idx))
+            yield plans
+        finally:
+            for p, _ in plans:
+                p.close()
+
+
+def _check_f16f8_range(plans, arith):
+    """After a pass: raise if f16f8 met a value outside its fp16 plane's range."""
+    if arith == "f16f8" and any(p.bad() for p, _ in plans):
+        raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
+                         "NaN): use arith='bf16x3' or 'auto'")
+
+
+def _to_device(out, device):
+    """A result dict with its tensors on ``device``."""
+    return {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in out.items()}
 
 
 def _eval_rows(activations, dev, cuts):
@@ -476,33 +518,12 @@ def _eval_rows(activations, dev, cuts):
 
 
 def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
-    from . import _lib
-    if arith not in _lib.ARITH_CODE:
-        raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
     if int(segment) < 1:
         raise ValueError(f"batch_size / segment must be >= 1, got {segment}")
     segment = int(segment)
-    lds = [ld[0] if isinstance(ld, (tuple, list)) else ld for ld in learned_dicts]
-    if not lds:
-        raise ValueError("no dictionaries to evaluate")
-    if activations.dim() != 2 or activations.shape[0] == 0:
-        raise ValueError(f"activations must be a non-empty [N, d] tensor, got shape {tuple(activations.shape)}")
-    if activations.dtype not in (torch.float32, torch.float16):
-        raise ValueError(f"activations must be fp32 or fp16, got {activations.dtype}")
+    lds, groups, ar = _dict_inputs(learned_dicts, activations, arith, centre)
+    dev = _cuda_device(activations, "dictionary evaluation")
     N, d = activations.shape
-    # AUTO runs bf16x3: the fp32 range, so activations fp16 cannot hold give finite results
-    ar = "bf16x3" if arith == "auto" else arith
-    groups = _eval_groups(lds, centre, 16 if ar == "f16f8" else 8)
-    for (kind, n_pad, dd, _), idx in groups.items():
-        if dd != d:
-            raise ValueError(f"dictionary {idx[0]} has width {dd}, the activations {d}")
-    if activations.device.type == "cuda":
-        dev = activations.device
-    elif torch.cuda.is_available():
-        dev = torch.device("cuda", torch.cuda.current_device())
-    else:
-        raise RuntimeError("dictionary evaluation runs in the sm_90a CUDA engine and needs a CUDA device; there is no "
-                           "CPU implementation in the product path")
     # engine calls: a multiple of the segment where one fits, and a cut where the last segment starts (its sums are
     # weighted by segment / rows, as the reference's running average does)
     rows = _EVAL_ROWS // segment * segment if segment <= _EVAL_ROWS else _EVAL_ROWS
@@ -511,50 +532,41 @@ def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
     cuts = [(s, min(s + rows, last)) for s in range(0, last, rows)] + [(s, min(s + rows, N)) for s in range(last, N, rows)]
     batch_max = max(e - s for s, e in cuts)
     results = [None] * len(lds)
-    with torch.cuda.device(dev):
-        plans = []
-        try:
-            for key, idx in groups.items():
-                plans.append((_EvalPlan(key, [lds[i] for i in idx], batch_max, ar, dev), idx))
-            s1 = torch.zeros(d, dtype=torch.float64, device=dev)
-            s2 = torch.zeros(d, dtype=torch.float64, device=dev)
-            snap = [torch.zeros_like(p.sums) for p, _ in plans]
-            for (s, e), x in zip(cuts, _eval_rows(activations, dev, cuts)):
-                if s == last and last > 0:
-                    snap = [p.sums.clone() for p, _ in plans]
-                for p, _ in plans:
-                    p.run(x, segment, s % segment)
-                xd = x.double()
-                s1 += xd.sum(0)
-                s2 += xd.pow(2).sum(0)
-            if ar == "f16f8" and any(p.bad() for p, _ in plans):
-                raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
-                                 "NaN): use arith='bf16x3' or 'auto'")
-            total = (s2 - s1 * s1 / N).sum()
-            r_last = N - last
-            for (p, idx), sn in zip(plans, snap):
-                full, tail = sn, p.sums - sn
-                m = (full + (segment / r_last) * tail) / (n_seg * segment)        # [M, n, 4] fp64
-                fvu = (p.sq / total).float()
-                l0 = (p.l0 / N).float()
-                for k, i in enumerate(idx):
-                    n = int(lds[i].n_feats)
-                    counts = p.counts[k, :n].clone()
-                    n_act = (counts > threshold).sum()
-                    mean, m2, m3, m4 = (m[k, :n, q] for q in range(4))
-                    var = m2 - mean * mean
-                    out = {"fvu": fvu[k], "mean_l0": l0[k], "feature_counts": counts,
-                           "feature_frequency": counts.float() / N, "n_ever_active": n_act,
-                           "frac_dead": 1.0 - n_act.float() / n, "rows": N,
-                           # (the last segment is still open after the pass: its flags count as well)
-                           "times_active": (p.seg_counts[k, :n] + p.seg_open[k, :n]).float(), "mean": mean.float(), "m2": m2.float(),
-                           "m3": m3.float(), "m4": m4.float(), "var": var.float(),
-                           "skew": (m3 / var.pow(1.5).clamp(min=1e-8)).float(),
-                           "kurtosis": (m4 / var.pow(2).clamp(min=1e-8)).float()}
-                    results[i] = {k2: (v.to(activations.device) if torch.is_tensor(v) else v) for k2, v in out.items()}
-        finally:
+    with _plans(groups, lds, dev, lambda key, g: _StatsPlan(key, g, batch_max, ar, dev)) as plans:
+        s1 = torch.zeros(d, dtype=torch.float64, device=dev)
+        s2 = torch.zeros(d, dtype=torch.float64, device=dev)
+        snap = [torch.zeros_like(p.sums) for p, _ in plans]
+        for (s, e), x in zip(cuts, _eval_rows(activations, dev, cuts)):
+            if s == last and last > 0:
+                snap = [p.sums.clone() for p, _ in plans]
             for p, _ in plans:
-                p.close()
+                p.run(x, segment, s % segment)
+            xd = x.double()
+            s1 += xd.sum(0)
+            s2 += xd.pow(2).sum(0)
+        _check_f16f8_range(plans, ar)
+        total = (s2 - s1 * s1 / N).sum()
+        r_last = N - last
+        for (p, idx), sn in zip(plans, snap):
+            full, tail = sn, p.sums - sn
+            m = (full + (segment / r_last) * tail) / (n_seg * segment)        # [M, n, 4] fp64
+            fvu = (p.sq / total).float()
+            l0 = (p.l0 / N).float()
+            for k, i in enumerate(idx):
+                n = int(lds[i].n_feats)
+                counts = p.counts[k, :n].clone()
+                n_act = (counts > threshold).sum()
+                mean, m2, m3, m4 = (m[k, :n, q] for q in range(4))
+                var = m2 - mean * mean
+                out = {"fvu": fvu[k], "mean_l0": l0[k], "feature_counts": counts,
+                       "feature_frequency": counts.float() / N, "n_ever_active": n_act,
+                       "frac_dead": 1.0 - n_act.float() / n, "rows": N,
+                       # (the last segment is still open after the pass: its flags count as well)
+                       "times_active": (p.seg_counts[k, :n] + p.seg_open[k, :n]).float(), "mean": mean.float(), "m2": m2.float(),
+                       "m3": m3.float(), "m4": m4.float(), "var": var.float(),
+                       "skew": (m3 / var.pow(1.5).clamp(min=1e-8)).float(),
+                       "kurtosis": (m4 / var.pow(2).clamp(min=1e-8)).float()}
+                results[i] = _to_device(out, activations.device)
     return results
 
 
@@ -625,20 +637,15 @@ def _list_order(key, frag):
     return o1.gather(-1, o2)
 
 
-class _FragmentPlan:
-    """A forward-only plan for a group of dictionaries with its fragment lists, which accumulate over engine calls."""
+class _FragmentPlan(_DictPlan):
+    """A dictionary plan with its fragment lists, which accumulate over engine calls."""
 
     def __init__(self, key, lds, batch_max, L, n_top, n_random, seed, want_act, arith, dev):
-        import ctypes as C
-        from . import _lib
-        self.ep = _EvalPlan(key, lds, batch_max, arith, dev, stats=False)
-        M, n = self.ep.M, self.ep.n
+        super().__init__(key, lds, batch_max, arith, dev)
+        M, n = self.M, self.n
         self.L, self.n_top, self.n_random, self.seed = L, n_top, n_random, seed
-        wbytes = _lib.load().sce_fragments_workspace_bytes(C.byref(self.ep.desc), batch_max, L)
-        if wbytes == 0:
-            _lib.check(-1, "sce_fragments_workspace_bytes")
-        self._ws = torch.empty(wbytes + 1024, dtype=torch.uint8, device=dev)
-        self.ws_ptr, self.ws_bytes = (self._ws.data_ptr() + 1023) // 1024 * 1024, wbytes
+        self.ws_bytes = _lib.load().sce_fragments_workspace_bytes(C.byref(self.desc), batch_max, L)
+        self._pass_ws, self.ws_ptr = _lib.workspace(self.ws_bytes, dev, "sce_fragments_workspace_bytes")
         self.top_val = torch.zeros(M, n, n_top, dtype=torch.float32, device=dev)
         self.top_frag = torch.full((M, n, n_top), -1, dtype=torch.int64, device=dev)     # -1: empty entry
         self.rnd_key = torch.zeros(M, n, n_random, dtype=torch.int64, device=dev)
@@ -648,12 +655,11 @@ class _FragmentPlan:
         self.n_active = torch.zeros(M, n, dtype=torch.int32, device=dev)
 
     def run(self, x, frag0):
-        from . import _lib
         ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None
         _lib.check(_lib.load().sce_forward_fragments(
-            self.ep.plan, x.data_ptr(), x.shape[0], self.L, frag0, self.n_top, self.n_random,
+            self.plan, x.data_ptr(), x.shape[0], self.L, frag0, self.n_top, self.n_random,
             self.seed & 0xFFFFFFFFFFFFFFFF, ptr(self.top_val), ptr(self.top_frag), ptr(self.top_act), ptr(self.rnd_key),
-            ptr(self.rnd_frag), ptr(self.rnd_act), self.n_active.data_ptr(), self.ws_ptr, self.ws_bytes, self.ep.stream),
+            ptr(self.rnd_frag), ptr(self.rnd_act), self.n_active.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream),
             "sce_forward_fragments")
 
     def results(self, k, n):
@@ -666,9 +672,6 @@ class _FragmentPlan:
                 "top_activations": rows(self.top_act, top_o),
                 "random_fragments": self.rnd_frag[k, :n].gather(1, rnd_o), "random_activations": rows(self.rnd_act, rnd_o),
                 "n_active_fragments": count, "skipped": count < self.n_random}
-
-    def close(self):
-        self.ep.close()
 
 
 def top_activating_fragments(learned_dicts, activations: torch.Tensor, fragment_len: int = 64, n_top: int = 20,
@@ -707,9 +710,6 @@ def top_activating_fragments(learned_dicts, activations: torch.Tensor, fragment_
 
     Memory: the per-token records take n·(n_top + n_random)·L·4 bytes per dictionary on the device — 671 MB for
     config 2's 16 dictionaries of 4096 features at 20 + 20 and L = 64."""
-    from . import _lib
-    if arith not in _lib.ARITH_CODE:
-        raise ValueError(f"arith must be one of {sorted(_lib.ARITH_CODE)}, got {arith!r}")
     L, n_top, n_random = int(fragment_len), int(n_top), int(n_random)
     if L < 32 or L > FRAGMENT_MAX_LEN or L % 32:
         raise ValueError(f"fragment_len must be a multiple of 32 in [32, {FRAGMENT_MAX_LEN}], got {fragment_len}")
@@ -718,49 +718,23 @@ def top_activating_fragments(learned_dicts, activations: torch.Tensor, fragment_
             raise ValueError(f"{name} must lie in [0, {FRAGMENT_MAX_LIST}], got {v}")
     if n_top + n_random == 0:
         raise ValueError("n_top and n_random are both 0: there is nothing to select")
-    lds = [ld[0] if isinstance(ld, (tuple, list)) else ld for ld in learned_dicts]
-    if not lds:
-        raise ValueError("no dictionaries to evaluate")
-    if activations.dim() != 2 or activations.shape[0] == 0:
-        raise ValueError(f"activations must be a non-empty [N, d] tensor, got shape {tuple(activations.shape)}")
-    if activations.dtype not in (torch.float32, torch.float16):
-        raise ValueError(f"activations must be fp32 or fp16, got {activations.dtype}")
-    N, d = activations.shape
+    lds, groups, ar = _dict_inputs(learned_dicts, activations, arith, False)
+    N = activations.shape[0]
     if N % L:
         raise ValueError(f"the activations' {N} rows are not a whole number of fragments of {L} rows")
-    ar = "bf16x3" if arith == "auto" else arith
-    groups = _eval_groups(lds, False, 16 if ar == "f16f8" else 8)
-    for (kind, n_pad, dd, _), idx in groups.items():
-        if dd != d:
-            raise ValueError(f"dictionary {idx[0]} has width {dd}, the activations {d}")
-    if activations.device.type == "cuda":
-        dev = activations.device
-    elif torch.cuda.is_available():
-        dev = torch.device("cuda", torch.cuda.current_device())
-    else:
-        raise RuntimeError("fragment selection runs in the sm_90a CUDA engine and needs a CUDA device; there is no CPU "
-                           "implementation in the product path")
+    dev = _cuda_device(activations, "fragment selection")
     rows = min(_EVAL_ROWS // L * L, N)          # engine calls are cut at fragment boundaries
     cuts = [(s, min(s + rows, N)) for s in range(0, N, rows)]
     results = [None] * len(lds)
-    with torch.cuda.device(dev):
-        plans = []
-        try:
-            for key, idx in groups.items():
-                plans.append((_FragmentPlan(key, [lds[i] for i in idx], rows, L, n_top, n_random, int(seed),
-                                            return_activations, ar, dev), idx))
-            for (s, e), x in zip(cuts, _eval_rows(activations, dev, cuts)):
-                for p, _ in plans:
-                    p.run(x, s // L)
-            if ar == "f16f8" and any(p.ep.bad() for p, _ in plans):
-                raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
-                                 "NaN): use arith='bf16x3' or 'auto'")
-            for p, idx in plans:
-                for k, i in enumerate(idx):
-                    out = p.results(k, int(lds[i].n_feats))
-                    out["fragments"] = N // L
-                    results[i] = {k2: (v.to(activations.device) if torch.is_tensor(v) else v) for k2, v in out.items()}
-        finally:
+    make = lambda key, g: _FragmentPlan(key, g, rows, L, n_top, n_random, int(seed), return_activations, ar, dev)
+    with _plans(groups, lds, dev, make) as plans:
+        for (s, e), x in zip(cuts, _eval_rows(activations, dev, cuts)):
             for p, _ in plans:
-                p.close()
+                p.run(x, s // L)
+        _check_f16f8_range(plans, ar)
+        for p, idx in plans:
+            for k, i in enumerate(idx):
+                out = p.results(k, int(lds[i].n_feats))
+                out["fragments"] = N // L
+                results[i] = _to_device(out, activations.device)
     return results

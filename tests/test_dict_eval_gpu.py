@@ -261,14 +261,14 @@ def test_out_of_fp16_range():
         MT.evaluate_dicts([ld], x, arith="f16f8")
 
 
-def test_abi_error_paths():
+def test_stats_plan_abi_error_paths():
     ld = S.TiedSAE(torch.randn(64, 64, device=DEV), torch.zeros(64, device=DEV))
-    p = MT._EvalPlan(("tied", 64, 64, False), [ld], 64, "bf16x3", DEV)
+    p = MT._StatsPlan(("tied", 64, 64, False), [ld], 64, "bf16x3", DEV)
     lib = _lib.load()
     x = torch.randn(64, 64, device=DEV)
     f = lambda t: t.data_ptr()
 
-    def call(B=64, seg=1, phase=0, losses=f(p.losses), sums=f(p.sums), open_=f(p.seg_open), ws=p.sws_ptr, nb=p.sws_bytes):
+    def call(B=64, seg=1, phase=0, losses=f(p.losses), sums=f(p.sums), open_=f(p.seg_open), ws=p.ws_ptr, nb=p.ws_bytes):
         rc = lib.sce_forward_stats(p.plan, f(x), B, seg, phase, None, losses, f(p.nnz), sums, f(p.seg_counts), open_,
                                    ws, nb, p.stream)
         return rc, lib.sce_last_error().decode()
@@ -281,8 +281,8 @@ def test_abi_error_paths():
         assert call(seg=4, phase=4)[0] == -1 and "seg_phase" in call(seg=4, phase=4)[1]
         assert call(losses=None)[0] == -1 and call(sums=None)[0] == -1
         assert call(seg=2, open_=None)[0] == -1 and "seg_open" in call(seg=2, open_=None)[1]
-        assert call(nb=p.sws_bytes - 1)[0] == -3 and "too small" in call(nb=p.sws_bytes - 1)[1]
-        assert call(ws=p.sws_ptr + 256)[0] == -3 and "aligned" in call(ws=p.sws_ptr + 256)[1]
+        assert call(nb=p.ws_bytes - 1)[0] == -3 and "too small" in call(nb=p.ws_bytes - 1)[1]
+        assert call(ws=p.ws_ptr + 256)[0] == -3 and "aligned" in call(ws=p.ws_ptr + 256)[1]
         torch.cuda.synchronize()
     finally:
         p.close()

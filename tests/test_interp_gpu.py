@@ -234,7 +234,7 @@ def test_f16f8_range_rule():
     MT.top_activating_fragments([ld], x)          # auto runs bf16x3
 
 
-def test_abi_error_paths():
+def test_fragment_plan_abi_error_paths():
     ld = S.TiedSAE(torch.randn(64, 64, device=DEV), torch.zeros(64, device=DEV))
     p = MT._FragmentPlan(("tied", 64, 64, False), [ld], 128, 32, 4, 4, 0, True, "bf16x3", DEV)
     lib = _lib.load()
@@ -243,8 +243,8 @@ def test_abi_error_paths():
 
     def call(B=128, L=32, frag0=0, nt=4, nr=4, tv=f(p.top_val), rk=f(p.rnd_key), na=f(p.n_active), ws=p.ws_ptr,
              nb=p.ws_bytes):
-        rc = lib.sce_forward_fragments(p.ep.plan, f(x), B, L, frag0, nt, nr, 0, tv, f(p.top_frag), f(p.top_act), rk,
-                                       f(p.rnd_frag), f(p.rnd_act), na, ws, nb, p.ep.stream)
+        rc = lib.sce_forward_fragments(p.plan, f(x), B, L, frag0, nt, nr, 0, tv, f(p.top_frag), f(p.top_act), rk,
+                                       f(p.rnd_frag), f(p.rnd_act), na, ws, nb, p.stream)
         return rc, lib.sce_last_error().decode()
 
     try:

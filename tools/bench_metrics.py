@@ -33,6 +33,43 @@ def make_models(sig, M, d, n, seed):
     return [sig.init(d, n, float(a)) for a in (np.logspace(-4, -2, M) if M > 1 else [1e-3])]
 
 
+def setup(args):
+    """(device, steps, warmup): cuda:0, made current, and the checked step counts."""
+    if not torch.cuda.is_available():
+        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
+    if args.steps < 1:
+        raise SystemExit("--steps must be at least 1")
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    return dev, args.steps, max(args.warmup, 1)
+
+
+def timed(fn, k, w):
+    """(CUDA-event ms per call over k calls after w warm-up calls, the last result)."""
+    for _ in range(w):
+        r = fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(k):
+        r = fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / k, r
+
+
+def activations(N, d, dev):
+    """[N, d] fp16 on dev: a sparse mixture of 2048 directions plus noise, seeded, generated in pieces of 2^16 rows."""
+    gen = torch.Generator(device=dev).manual_seed(1)
+    x = torch.empty(N, d, dtype=torch.float16, device=dev)
+    for i in range(0, N, 1 << 16):
+        k = min(1 << 16, N - i)
+        feats = torch.nn.functional.normalize(torch.randn(2048, d, generator=gen, device=dev), dim=-1)
+        code = (torch.rand(k, 2048, generator=gen, device=dev) < 0.01) * torch.rand(k, 2048, generator=gen, device=dev)
+        x[i:i + k] = (code @ feats + 0.05 * torch.randn(k, d, generator=gen, device=dev)).half()
+    return x
+
+
 MMCS_WORKLOADS = {
     # name: (M, n, d, pairs, description)
     "mmcs_cfg2": (16, 4096, 512, "lower", "16 seeded config-2 TiedSAE dictionaries (4096 x 512): all 120 lower-triangle "
@@ -61,32 +98,14 @@ def run_mmcs(args):
     from oracle import metrics_oracle as O
     from sparse_coding_b200 import metrics as MT
 
-    if not torch.cuda.is_available():
-        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
+    dev, K, W = setup(args)
     M, n, d, pairs, desc = MMCS_WORKLOADS[args.workload]
     ens = S.FunctionalEnsemble(make_models(S.FunctionalTiedSAE, M, d, n, seed=0), S.FunctionalTiedSAE, S.adam,
                                {"lr": 1e-3}, device=dev)
     plist = [(i, j) for i in range(M) for j in range(i)] if pairs == "lower" else pairs
-    K, W = args.steps, max(args.warmup, 1)
-    if K < 1:
-        raise SystemExit("--steps must be at least 1")
 
     def engine_pass():
         return MT.dictionary_similarity(ens, pairs=plist, arith=args.arith), MT.capacity(ens, arith=args.arith)
-
-    def timed(fn, k, w):
-        for _ in range(w):
-            r = fn()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(k):
-            r = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / k, r
 
     ms, (res, cap) = timed(engine_pass, K, W)
     L = [ens.sig.to_learned_dict(p, b).get_learned_dict() for p, b in ens.unstack()]   # torch, fp32
@@ -159,36 +178,12 @@ def run_eval(args):
     from oracle import eval_oracle as O
     from sparse_coding_b200 import metrics as MT
 
-    if not torch.cuda.is_available():
-        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
+    dev, K, W = setup(args)
     M, n, d, N, desc = EVAL_WORKLOADS[args.workload]
-    K, W = args.steps, max(args.warmup, 1)
-    if K < 1:
-        raise SystemExit("--steps must be at least 1")
     lds = [S.FunctionalTiedSAE.to_learned_dict(p, b) for p, b in make_models(S.FunctionalTiedSAE, M, d, n, seed=0)]
     for ld in lds:
         ld.to_device(dev)
-    gen = torch.Generator(device=dev).manual_seed(1)
-    x = torch.empty(N, d, dtype=torch.float16, device=dev)
-    for i in range(0, N, 1 << 16):                 # sparse mixture + noise, generated in pieces, stored as fp16
-        k = min(1 << 16, N - i)
-        feats = torch.nn.functional.normalize(torch.randn(2048, d, generator=gen, device=dev), dim=-1)
-        code = (torch.rand(k, 2048, generator=gen, device=dev) < 0.01) * torch.rand(k, 2048, generator=gen, device=dev)
-        x[i:i + k] = (code @ feats + 0.05 * torch.randn(k, d, generator=gen, device=dev)).half()
-
-    def timed(fn, k, w):
-        for _ in range(w):
-            r = fn()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(k):
-            r = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / k, r
+    x = activations(N, d, dev)
 
     ms, _ = timed(lambda: MT.evaluate_dicts(lds, x, segment=1000, arith=args.arith), K, W)
 
@@ -267,38 +262,14 @@ def run_interp(args):
     import sparse_coding_b200 as S
     from sparse_coding_b200 import metrics as MT
 
-    if not torch.cuda.is_available():
-        raise SystemExit("tools/bench_metrics.py needs a CUDA device (the engine has no CPU path)")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
+    dev, K, W = setup(args)
     M, n, d, G, desc = INTERP_WORKLOADS[args.workload]
     L = 64
-    K, W = args.steps, max(args.warmup, 1)
-    if K < 1:
-        raise SystemExit("--steps must be at least 1")
     lds = [S.FunctionalTiedSAE.to_learned_dict(p, b) for p, b in make_models(S.FunctionalTiedSAE, M, d, n, seed=0)]
     for ld in lds:
         ld.to_device(dev)
-    gen = torch.Generator(device=dev).manual_seed(1)
     N = G * L
-    x = torch.empty(N, d, dtype=torch.float16, device=dev)
-    for i in range(0, N, 1 << 16):                 # sparse mixture + noise, generated in pieces, stored as fp16
-        k = min(1 << 16, N - i)
-        feats = torch.nn.functional.normalize(torch.randn(2048, d, generator=gen, device=dev), dim=-1)
-        code = (torch.rand(k, 2048, generator=gen, device=dev) < 0.01) * torch.rand(k, 2048, generator=gen, device=dev)
-        x[i:i + k] = (code @ feats + 0.05 * torch.randn(k, d, generator=gen, device=dev)).half()
-
-    def timed(fn, k, w):
-        for _ in range(w):
-            r = fn()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(k):
-            r = fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / k, r
+    x = activations(N, d, dev)
 
     ms, res = timed(lambda: MT.top_activating_fragments(lds, x, arith=args.arith), K, W)
     skipped = float(sum(r["skipped"].float().mean() for r in res) / M)

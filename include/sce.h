@@ -283,6 +283,36 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
                    int d, const int* pairs, int n_pairs, int arith, float* row_max, float* col_max, float* capacity,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* Synthetic sparse-mixture rows (sc_datasets/random_dataset.py:191-245 generate_correlated_dataset, :160-188
+ * generate_rand_dataset, :145-157 generate_noise_dataset with the identity covariance), without a dense code:
+ *   active(i, j) = u_thresh(i, j) <= probs[i / group_rows][j]                      (a p > 1 is always on)
+ *   coef(i, j)   = u_val(i, j) * u_strength(i, j)          in fp32, for the active j
+ *   zero-row rule (zero_row_rule = 1): a row with no active component gets component z(i) with coef 1.0 * u_strength(i, z(i))
+ *   out[i, :]    = fma(noise_scale, n(i, :), sum over active j, ascending, of coef(i, j) feats[j, :])   fp32 FMAs;
+ *                  stored as fp32 (out_half = 0) or rounded to nearest fp16 (out_half = 1)
+ *   feats        device fp32 [n_gt, d], row-major, 16-byte aligned; d a multiple of 8 in [8, 8192]; n_gt >= 1
+ *   probs        device fp32 [ceil(B / group_rows), n_gt]: local row i belongs to group i / group_rows
+ *   row0         global index of local row 0 (>= 0); every draw of local row i is keyed by the global row row0 + i
+ *   out          device [B, d] fp32 or fp16, 16-byte aligned
+ *   row_nnz      device int32 [B] or NULL: the number of active components of each row (1 for a zero-row fill)
+ *   code_idx, code_val  device int32 / fp32 [B, code_cap] or both NULL: each row's active components in ascending j
+ *                and their coef, the ground-truth code; entries beyond code_cap are dropped (row_nnz still counts them)
+ * Random numbers: Philox4x32-10 with key (seed & 0xffffffff, seed >> 32) and counter (c0, global row & 0xffffffff,
+ * global row >> 32, tag); a word x gives the uniform (x >> 8) 2^-24 in [0, 1).
+ *   tag 0 threshold, 1 value, 2 strength: c0 = j / 4, word j % 4
+ *   tag 3 zero-row component: c0 = 0, z(i) = (word 0 * n_gt) >> 32
+ *   tag 4 noise: c0 = k / 4 for columns k .. k + 3 (k % 4 = 0); Box-Muller on the word pairs (0, 1) -> columns k, k + 1
+ *         and (2, 3) -> k + 2, k + 3: u1 = ((a >> 8) + 1) 2^-24, u2 = (b >> 8) 2^-24, r = sqrt(-2 ln u1),
+ *         n = (r cos 2 pi u2, r sin 2 pi u2)
+ *   tag 5 is left to the caller for per-group Gaussians (with the group index in the row words; see
+ *         sparse_coding_b200/synthetic.py), so that they never share a stream with a row's draws.
+ * The active sets, coefficients, row_nnz and lists are therefore a function of (seed, global row, probs) alone, bitwise:
+ * independent of the launch, of how rows are split over calls, and of the GPU. out is that function up to the rounding
+ * of fp32 FMAs in a fixed order, deterministic run to run. Asynchronous on `stream`. */
+int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,
+                   unsigned long long seed, int zero_row_rule, float noise_scale, void* out, int out_half, int* row_nnz,
+                   int* code_idx, float* code_val, int code_cap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

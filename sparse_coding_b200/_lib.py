@@ -28,7 +28,7 @@ EXPORTS = [
     "sce_last_launch_count", "sce_get_step_count", "sce_set_step_count", "sce_profile_begin", "sce_profile_end",
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
-    "sce_fragments_workspace_bytes", "sce_forward_fragments",
+    "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -107,6 +107,7 @@ def load():
     lib.sce_fragments_workspace_bytes.argtypes = [C.POINTER(SceDesc), i, i]
     lib.sce_forward_fragments.argtypes = [vp, vp, i, i, ll, i, i, C.c_ulonglong, vp, vp, vp, vp, vp, vp, vp, vp,
                                           C.c_size_t, vp]
+    lib.sce_synth_rows.argtypes = [vp, i, i, vp, i, ll, i, C.c_ulonglong, i, f, vp, i, vp, vp, vp, i, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

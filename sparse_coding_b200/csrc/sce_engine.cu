@@ -23,6 +23,7 @@
 #include "sce_epilogues.cuh"
 #include "sce_gemm.cuh"
 #include "sce_kernels.cuh"
+#include "sce_synth.cuh"
 #include "sce_topk.cuh"
 #include "sce_tmap.h"
 
@@ -1971,6 +1972,39 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
   // (a raw operand split above for the range check is split again here: the planes of the arithmetic that runs)
   return f8 ? run_similarity_t<kArithF16F8>(A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms, st)
             : run_similarity_t<kArithBf16x3>(A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms, st);
+}
+
+int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,
+                   unsigned long long seed, int zero_row_rule, float noise_scale, void* out, int out_half, int* row_nnz,
+                   int* code_idx, float* code_val, int code_cap, void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!feats || !probs || !out) return fail(SCE_ERR_INVALID, "synth_rows: feats, probs and out are required");
+  if (n_gt < 1 || B < 1) return fail(SCE_ERR_INVALID, "synth_rows: n_gt (%d) and B (%d) must be >= 1", n_gt, B);
+  if (d < 8 || d % 8) return fail(SCE_ERR_INVALID, "synth_rows: d (%d) must be a positive multiple of 8", d);
+  if (d > 8192) return fail(SCE_ERR_INVALID, "synth_rows: d = %d > 8192 is not supported by the row kernels", d);
+  if (group_rows < 1) return fail(SCE_ERR_INVALID, "synth_rows: group_rows (%d) must be >= 1", group_rows);
+  if (row0 < 0) return fail(SCE_ERR_INVALID, "synth_rows: row0 (%lld) must be >= 0", row0);
+  if ((zero_row_rule != 0 && zero_row_rule != 1) || (out_half != 0 && out_half != 1))
+    return fail(SCE_ERR_INVALID, "synth_rows: zero_row_rule and out_half must be 0 or 1");
+  if (!(noise_scale >= 0.f && noise_scale <= 3.0e38f))
+    return fail(SCE_ERR_INVALID, "synth_rows: noise_scale must be finite and >= 0");
+  if (!code_idx != !code_val) return fail(SCE_ERR_INVALID, "synth_rows: code_idx and code_val go together");
+  if (code_idx && code_cap < 1) return fail(SCE_ERR_INVALID, "synth_rows: code_cap (%d) must be >= 1 with code lists", code_cap);
+  if (reinterpret_cast<uintptr_t>(out) % 16 || reinterpret_cast<uintptr_t>(feats) % 16)
+    return fail(SCE_ERR_INVALID, "synth_rows: out and feats must be 16-byte aligned");
+
+  // ---- device
+  SynthArgs a{feats, probs, n_gt, d, group_rows, B, row0, (uint32_t)seed, (uint32_t)(seed >> 32), zero_row_rule,
+              noise_scale, out, out_half, row_nnz, code_idx, code_val, code_idx ? code_cap : 0};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const unsigned rows8 = (unsigned)((B + 7) / 8);
+  if (d <= 128) synth_rows_kernel<1, false><<<rows8, 256, 0, st>>>(a);
+  else if (d <= 256) synth_rows_kernel<2, false><<<rows8, 256, 0, st>>>(a);
+  else if (d <= 512) synth_rows_kernel<4, false><<<rows8, 256, 0, st>>>(a);
+  else if (d <= 1024) synth_rows_kernel<8, false><<<rows8, 256, 0, st>>>(a);
+  else synth_rows_kernel<8, true><<<(unsigned)B, 32 * ((d + 1023) / 1024), 0, st>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  return SCE_OK;
 }
 
 }  // extern "C"

@@ -429,25 +429,33 @@ class _Counter:
 def train_on_chunks(ensemble, args: dict, dataset_folder: str, output_folder: str, batch_size: int,
                     ensemble_hyperparams: List[str], buffer_hyperparams: List[str], n_repetitions: int = 1,
                     center_activations: bool = False, cfg=None, chunk_order: Optional[List[int]] = None,
-                    save_schedule: str = "sweep", feed: str = "per_rank", on_chunk_end=None):
+                    save_schedule: str = "sweep", feed: str = "per_rank", on_chunk_end=None, chunks=None):
     """The chunk loop of ``sweep`` (big_sweep.py:349-384) / ``basic_l1_sweep`` (basic_l1_sweep.py:85-115) for ONE
     ensemble on ONE GPU, with streamed chunks. Writes ``_{i}/learned_dicts.pt`` (+ ``config.yaml`` when ``cfg`` is
     given) on the reference's schedule: last chunk, or chunk count in {8, 16, …, 512}. ``feed``: see
-    :class:`ChunkStreamer`; ``on_chunk_end(i, chunk_idx, ensemble)`` runs after the last step of every chunk."""
+    :class:`ChunkStreamer`; ``on_chunk_end(i, chunk_idx, ensemble)`` runs after the last step of every chunk.
+    ``chunks``: a sized iterable of ``(chunk_idx, device chunk)`` that replaces the streamer (for example
+    ``synthetic.SyntheticChunks``, which generates each chunk on the GPU); ``dataset_folder``, ``chunk_order``,
+    ``n_repetitions`` and ``feed`` are then unused."""
     import yaml
 
     device = torch.device(args["device"])
-    n_chunks = len([f for f in os.listdir(dataset_folder) if f.endswith(".pt") and f[:-3].isdigit()])
-    if chunk_order is None:
-        chunk_order = list(np.random.permutation(n_chunks))
-        if n_repetitions is not None:
-            chunk_order = list(np.tile(chunk_order, n_repetitions))
+    if chunks is None:
+        n_chunks = len([f for f in os.listdir(dataset_folder) if f.endswith(".pt") and f[:-3].isdigit()])
+        if chunk_order is None:
+            chunk_order = list(np.random.permutation(n_chunks))
+            if n_repetitions is not None:
+                chunk_order = list(np.tile(chunk_order, n_repetitions))
+        chunks = ChunkStreamer(dataset_folder, chunk_order, device, feed=feed)
+        n_total = len(chunk_order)
+    else:
+        n_total = len(chunks)
     os.makedirs(output_folder, exist_ok=True)
     means = None
     cfg = cfg if cfg is not None else type("Cfg", (), {"use_wandb": False})()
     learned_dicts = []
     perm_cache: dict = {}
-    for i, (chunk_idx, chunk) in enumerate(ChunkStreamer(dataset_folder, chunk_order, device, feed=feed)):
+    for i, (chunk_idx, chunk) in enumerate(chunks):
         if center_activations:
             if means is None:
                 means = chunk.float().mean(dim=0)
@@ -465,7 +473,7 @@ def train_on_chunks(ensemble, args: dict, dataset_folder: str, output_folder: st
         check_input_range(ensemble)
         if on_chunk_end is not None:
             on_chunk_end(i, chunk_idx, ensemble)      # e.g. the end-of-chunk metric gather (sharding.gather_metrics)
-        last = i == len(chunk_order) - 1
+        last = i == n_total - 1
         if last or (save_schedule == "sweep" and (i + 1) in [2 ** j for j in range(3, 10)]) or save_schedule == "every":
             # export (a full D2H of the parameters, which also drains the GPU) only when a checkpoint is due
             with nvtx_range("sce.export_learned_dicts"):

@@ -1,12 +1,12 @@
 // sce_engine.cu — libsce.so: the C ABI of include/sce.h on top of the wgmma GEMM core and the
 // streaming kernels. One `sce_plan` = one stacked ensemble (FunctionalEnsemble, autoencoders/ensemble.py:68-97).
 //
-// One training step (tied variant; untied and top-k differ as noted; "(hi, lo)" stands for the operand planes of the
-// plan's arithmetic: fp16 + two E5M2 planes with f16f8, a bf16 pair with bf16x3) is
-//   split_rows      x -> (x_hi, x_lo)  [+ residual-plane flag, input range monitor]
-//   GEMM encode     z = x W^T (+b) -> relu -> (c_hi, c_lo), activity masks, sum|c|, nnz   [M x B x n, K = d]
-//   GEMM decode     x^ = c W -> r = x^ - x, sum r^2, g = 2r/(Bd) -> (g_hi, g_lo)  [M x B x d, K = n]
-//   GEMM dcode      dz = (g W^T + alpha/B [c>0]) [z>=0] -> (dz_hi, dz_lo), db partials
+// One training step (tied variant; untied and top-k differ as noted; "planes" are the operand planes of the plan's
+// arithmetic, see Planes: fp16 + two E5M2 planes with f16f8, a bf16 pair with bf16x3) is
+//   split_rows      x -> x planes  [+ residual-plane flag, input range monitor]
+//   GEMM encode     z = x W^T (+b) -> relu -> c planes, activity masks, sum|c|, nnz   [M x B x n, K = d]
+//   GEMM decode     x^ = c W -> r = x^ - x, sum r^2, g = 2r/(Bd) -> g planes  [M x B x d, K = n]
+//   GEMM dcode      dz = (g W^T + alpha/B [c>0]) [z>=0] -> dz planes, db partials
 //   GEMM dW         dW = dz^T x + c^T g                                            [M x n x d, K = 2B]
 //   bias_norm, finalize (losses), dict_rows<ADAM> (Jacobian + Adam + renormalise + re-split), bias<ADAM>
 // Top-k variant: the encode GEMM stores fp32 scores; topk_select2_kernel keeps k per row; with the k-sparse path
@@ -49,66 +49,88 @@ static int fail(int code, const char* fmt, ...) {
 // ------------------------------------------------------------------------------------------------
 // plan
 // ------------------------------------------------------------------------------------------------
-struct GemmMaps {  // tensor maps of one GEMM for one batch size (x8: third plane of the f16f8 arithmetic)
-  CUtensorMap a_hi[kMaxSets], a_lo[kMaxSets], b_hi[kMaxSets], b_lo[kMaxSets];
-  CUtensorMap a_x8[kMaxSets], b_x8[kMaxSets];
+// The planes of one operand tensor. bf16x3: hi, lo = bf16 planes (2 B / element each), x8 = nullptr. f16f8: hi = fp16
+// plane, lo = E5M2 plane of the values, x8 = E5M2 plane of the scaled residuals (1 B / element each): 4 B / element
+// either way. The batch-major 8-bit copies of native dW are Planes without a 16-bit plane.
+struct Planes {
+  void* hi;
+  void* lo;
+  uint8_t* x8;
+  bool f8;
+  size_t lo_size() const { return f8 ? 1 : 2; }   // bytes per element of lo (and of x8)
+  // the planes from element `e` on (a model's slab)
+  Planes at(size_t e) const {
+    return {hi ? static_cast<uint8_t*>(hi) + 2 * e : nullptr, lo ? static_cast<uint8_t*>(lo) + lo_size() * e : nullptr,
+            x8 ? x8 + e : nullptr, f8};
+  }
+  // zero the first `count` elements of every plane
+  cudaError_t zero(size_t count, cudaStream_t st) const {
+    cudaError_t e = cudaMemsetAsync(hi, 0, 2 * count, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(lo, 0, lo_size() * count, st);
+    if (e == cudaSuccess && x8) e = cudaMemsetAsync(x8, 0, count, st);
+    return e;
+  }
+};
+
+struct OperandMaps {   // tensor maps of one operand's planes
+  CUtensorMap hi, lo, x8;
+};
+struct GemmMaps {      // tensor maps of one GEMM for one batch size
+  OperandMaps a[kMaxSets], b[kMaxSets];
 };
 struct BatchMaps {
   GemmMaps encode, decode, dcode, dw_enc, dw_dec;
   GemmMaps center;             // centring: A = (x - trans) planes [M,B,d], B = rot planes [M,d,d], both K-major
-  CUtensorMap st_c_hi, st_c_lo, st_c_x8, st_dz_hi, st_dz_lo, st_dz_x8;  // epilogue TMA-store maps
-  CUtensorMap st_scores;                                                // top-k: fp32 scores
+  OperandMaps st_c, st_dz;     // epilogue TMA-store maps
+  CUtensorMap st_scores;       // top-k: fp32 scores
   cudaGraphExec_t graph;       // captured step for this batch size (launch-bound shapes), or nullptr
   int graph_launches, eager_steps;
 };
 
-struct sce_plan {
+// The plan's workspace buffers, in carve order (carve)
+struct PlanBuffers {
+  float* x_stage;                 // [xm, Bmax, d] staging for host-fed steps
+  Planes x;                       // [xm, Bmax, d]
+  Planes wenc, wdec;              // [M, n, d] (tied: wdec is a copy of wenc)
+  Planes wdt;                     // f16f8: the decoder's planes transposed, [M, d, n]: the decode GEMM's B operand, K-major (transpose_dict)
+  Planes c;                       // [M, Bmax, n]   (dw_native: the 8-bit planes are dz's, see carve)
+  Planes g;                       // [M, Bmax, d]
+  Planes dz;                      // [M, Bmax, n], one contiguous block of 4 B / element (top-k: fp32 scores alias it);
+                                  // dw_native: the 8-bit planes are [M, n, Bp]
+  // dw_native (dense f16f8 plans): batch-major copies of the 8-bit planes of x, c and g, [xm or M, cols, Bp] with Bp =
+  // batch_max rounded up to 16 (TMA pitch): the weight gradient reads them K-major over the batch (E5M2 wgmma).
+  // dz's 8-bit planes are written in that layout in the first place (EpiDcodeT<f16f8, true>).
+  Planes xt, ct, gt;
+  Planes rot;                     // centring: operand planes of buffers["center_rot"] [M, d, d]
+  float* x_centered;              // centring: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
+  float* scores;                  // top-k: fp32 scores [M, Bmax, n] of the encode GEMM
+  int* tk_models;                 // top-k gather kernel: the models sorted into k classes (device copy of tk_group_models)
+  uint32_t* tk_cmax;              // top-k: largest key per 32-column chunk of the scores [M, Bmax, n_chunks] (EpiScoresTma)
+  int *tk_col, *tk_cnt;           // top-k lists (TopkLists): selected columns [M, Bmax, kmax], entries per row [M, Bmax]
+  float *tk_val, *tk_dots;        // their values [M, Bmax, kmax]; per-slice shares of g . W_j [M, Bmax, kmax, slices]
+  float* wn_f32;                  // top-k: fp32 copy of the normalised dictionary [M, n, d] the gather kernel reads
+  uint32_t *act_pos, *act_zero;   // activity masks [M][ceil(n/32)][Bmax]: bit 31-j of a word = column 32*chunk + j (ActMask)
+  uint32_t* res_flags;            // [0]: the batch has a non-zero residual plane (f16f8; written by the batch split)
+  float *dw_enc, *dw_dec;         // [M, n, d]
+  float *part_enc, *part_dec, *db_part, *bnorm, *l1_over_b, *loss_stage, *nnz_stage;
+};
+
+struct sce_plan : PlanBuffers {
   sce_desc d;
   sce_buffers b;
   int sms;
   int device;  // CUDA device the plan was created on (the caller keeps it current for every call)
   int xm;  // number of distinct input batches (1 shared, or M)
-  // workspace carve-up
-  // Operand planes. bf16x3: hi, lo = bf16 planes (2 B / element each), x8 unused. f16f8: hi = fp16 plane, lo =
-  // e5m2 plane of the values, x8 = e5m2 plane of the scaled residuals (1 B / element each): 4 B / element either way.
-  int arith;                      // kArithBf16x3 or kArithF16F8 (resolved from desc.arith / env SCE_ARITH / the shape)
-  float* x_stage;                 // [xm, Bmax, d] staging for host-fed steps
-  __nv_bfloat16 *x_hi, *x_lo;     // [xm, Bmax, d]
-  __nv_bfloat16 *wenc_hi, *wenc_lo, *wdec_hi, *wdec_lo;  // [M, n, d] (tied: dec aliases enc)
-  __nv_bfloat16 *c_hi, *c_lo;     // [M, Bmax, n]
-  __nv_bfloat16 *g_hi, *g_lo;     // [M, Bmax, d]
-  __nv_bfloat16 *dz_hi, *dz_lo;   // [M, Bmax, n]   (top-k: fp32 scores alias these planes; dw_native: 8-bit planes [M, n, Bp])
-  uint8_t *x_x8, *wenc_x8, *wdec_x8, *c_x8, *g_x8, *dz_x8;
-  // dw_native (dense f16f8 plans): batch-major copies of the 8-bit planes of x, c and g, [xm or M, cols, Bp] with Bp =
-  // batch_max rounded up to 16 (TMA pitch): the weight gradient reads them K-major over the batch (E5M2 wgmma).
-  // dz's 8-bit planes are written in that layout in the first place (EpiDcodeT<f16f8, true>).
-  uint8_t *xt_lo, *xt_x8, *ct_lo, *ct_x8, *gt_lo, *gt_x8;
+  int arith;                       // kArithBf16x3 or kArithF16F8 (resolved from desc.arith / env SCE_ARITH / the shape)
   int bpad;                        // Bp
   int code_batch_major;            // 1: the last call was a dw_native backward, which left the code's residual plane
-                                   // only in its batch-major copy (ct_x8): dcode overwrote the row-major one (carve)
+                                   // only in its batch-major copy (ct.x8): dcode overwrote the row-major one (carve)
   int dw_native;                   // 1: the weight gradient's cross terms run on E5M2 wgmma (see native_dw_layout)
-  // f16f8: the decoder's planes transposed, [M, d, n]: the decode GEMM's B operand, K-major (transpose_dict)
-  __nv_bfloat16 *wdt_hi, *wdt_lo;
-  uint8_t* wdt_x8;
-  __nv_bfloat16 *rot_hi, *rot_lo;  // centring: operand planes of buffers["center_rot"] [M, d, d]
-  uint8_t* rot_x8;
-  float* x_centered;              // centring: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
-  float* scores;                  // top-k: fp32 scores [M, Bmax, n] of the encode GEMM
-  int* tk_models;                 // top-k gather kernel: the models sorted into k classes (device copy of tk_group_models)
   int tk_groups, tk_group_off[5], tk_group_krows[4];   // classes: models [off[g], off[g+1]) need at most krows[g] rows
-  uint32_t* tk_cmax;              // top-k: largest key per 32-column chunk of the scores [M, Bmax, n_chunks] (EpiScoresTma)
   int topk_cmax;                  // 1: the selection works from the chunk maxima (SCE_TOPK_CMAX=0 turns it off)
-  int *tk_col, *tk_cnt;           // top-k lists (TopkLists): selected columns [M, Bmax, kmax], entries per row [M, Bmax]
-  float *tk_val, *tk_dots;        // their values [M, Bmax, kmax]; per-slice shares of g . W_j [M, Bmax, kmax, slices]
-  float* wn_f32;                  // top-k: fp32 copy of the normalised dictionary [M, n, d] the gather kernel reads
   int tk_slices;                  // slices of the activation width topk_sparse_kernel runs per row
   int tk_kmax;                    // list capacity per row (desc.topk_k_max rounded up to 8; 0: no lists)
   int topk_sparse;                // 1: decode / dcode of the top-k variant run as the k-sparse gather kernels
-  uint32_t *act_pos, *act_zero;   // activity masks [M][ceil(n/32)][Bmax]: bit 31-j of a word = column 32*chunk + j (ActMask)
-  uint32_t* res_flags;            // [0]: the batch has a non-zero residual plane (f16f8; written by the batch split)
-  float *dw_enc, *dw_dec;         // [M, n, d]
-  float *part_enc, *part_dec, *db_part, *bnorm, *l1_over_b, *loss_stage, *nnz_stage;
-  int tiles_mB_max;
   std::map<int, BatchMaps*>* maps;
   cudaStream_t cap_stream;  // private stream the step is captured on
   int dcode_passes, dw_passes;  // tensor passes of the two backward GEMMs (default: desc.bwd_passes)
@@ -138,6 +160,17 @@ struct Carve {
     off = align_up(off, 1024);
     T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
     off += count * sizeof(T);
+    return p;
+  }
+  // the planes of `count` elements of one operand tensor: 16-bit, then a second 16-bit plane (bf16x3) or two 8-bit ones
+  Planes planes(size_t count, bool f8) {
+    Planes p{take<uint16_t>(count), nullptr, nullptr, f8};
+    if (f8) {
+      p.lo = take<uint8_t>(count);
+      p.x8 = take<uint8_t>(count);
+    } else {
+      p.lo = take<uint16_t>(count);
+    }
     return p;
   }
 };
@@ -190,9 +223,9 @@ static int query_device(int* device, int* sm_count) {
 
 // fp32 rows -> the operand planes of arithmetic AR: n4 float4s, grid-stride over at most 2048 blocks
 template <int AR>
-static void launch_split_rows(const float* x, void* hi, void* lo, void* x8, long long n4, uint32_t* flags, cudaStream_t st) {
+static void launch_split_rows(const float* x, const Planes& w, long long n4, uint32_t* flags, cudaStream_t st) {
   const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, hi, lo, x8, n4, flags);
+  split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags);
 }
 
 // desc.arith -> kArithBf16x3 / kArithF16F8. AUTO: f16f8 where the 8-bit planes can be addressed by TMA
@@ -246,8 +279,8 @@ static bool native_dw_layout(const sce_desc& d) {
 }
 static size_t batch_pad(const sce_desc& d) { return ((size_t)d.batch_max + 15) / 16 * 16; }
 
-// Carves the workspace; with base == nullptr only measures it.
-static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
+// Carves the workspace into `w` (buffers the plan does not use stay null); with base == nullptr only measures it.
+static size_t carve(PlanBuffers& w, const sce_desc& d, uint8_t* base) {
   Carve c{base, 0};
   const size_t M = d.n_models, B = d.batch_max, n = d.n, dd = d.d;
   const size_t xm = d.x_per_model ? M : 1;
@@ -255,150 +288,69 @@ static size_t carve(sce_plan* p, const sce_desc& d, uint8_t* base) {
   const size_t tiles_nN = (n + kBN - 1) / kBN;
   const size_t tiles_nD = (dd + kBN - 1) / kBN;
   const bool f8 = resolve_arith(d) == kArithF16F8;
-  // the planes of one operand tensor: 16-bit, then (bf16x3) a second 16-bit plane or (f16f8) two 8-bit planes
-  auto planes = [&](size_t count, __nv_bfloat16*& hi, __nv_bfloat16*& lo, uint8_t*& x8) {
-    hi = c.take<__nv_bfloat16>(count);
-    if (f8) {
-      lo = reinterpret_cast<__nv_bfloat16*>(c.take<uint8_t>(count));
-      x8 = c.take<uint8_t>(count);
-    } else {
-      lo = c.take<__nv_bfloat16>(count);
-      x8 = nullptr;
-    }
-  };
-  auto X = c.take<float>(xm * B * dd);
-  __nv_bfloat16 *xh, *xl, *weh, *wel, *ch, *cl, *gh, *gl;
-  uint8_t *x8, *we8, *c8, *g8;
-  planes(xm * B * dd, xh, xl, x8);
-  planes(M * n * dd, weh, wel, we8);
-  __nv_bfloat16 *wdh = weh, *wdl = wel;
-  uint8_t* wd8 = we8;
-  if (d.variant == SCE_UNTIED) planes(M * n * dd, wdh, wdl, wd8);
-  __nv_bfloat16 *wth = nullptr, *wtl = nullptr;
-  uint8_t* wt8 = nullptr;
-  if (f8) planes(M * n * dd, wth, wtl, wt8);
+  w.x_stage = c.take<float>(xm * B * dd);
+  w.x = c.planes(xm * B * dd, f8);
+  w.wenc = c.planes(M * n * dd, f8);
+  w.wdec = d.variant == SCE_UNTIED ? c.planes(M * n * dd, f8) : w.wenc;
+  if (f8) w.wdt = c.planes(M * n * dd, f8);
   const bool tdw = native_dw_layout(d);
   const size_t Bp = batch_pad(d);
   const size_t dz8 = tdw ? M * n * Bp : M * B * n;   // bytes of one 8-bit plane of dz
-  uint8_t *xtl = nullptr, *xtx = nullptr, *ctl = nullptr, *ctx = nullptr, *gtl = nullptr, *gtx = nullptr;
   if (!tdw) {
-    planes(M * B * n, ch, cl, c8);
+    w.c = c.planes(M * B * n, f8);
   } else {
     // the code's row-major 8-bit planes are read by the decode GEMM only, which runs before dcode writes dz: they live in
     // dz's 8-bit planes (below), and the code's own 8-bit space holds the batch-major copies the weight gradient reads
-    ch = c.take<__nv_bfloat16>(M * B * n);
-    ctl = c.take<uint8_t>(dz8);
-    ctx = c.take<uint8_t>(dz8);
+    w.c.hi = c.take<uint16_t>(M * B * n);
+    w.ct.lo = c.take<uint8_t>(dz8);
+    w.ct.x8 = c.take<uint8_t>(dz8);
   }
-  planes(M * B * dd, gh, gl, g8);
+  w.g = c.planes(M * B * dd, f8);
   // all planes contiguous, 4 B / element (the top-k scores alias them); with tdw the 8-bit ones are [M][n][Bp]
-  auto dzh = c.take<__nv_bfloat16>(M * B * n + dz8);
+  uint8_t* dz = c.take<uint8_t>(2 * (M * B * n + dz8));
+  w.dz = Planes{dz, dz + 2 * M * B * n, f8 ? dz + 2 * M * B * n + dz8 : nullptr, f8};
   if (tdw) {
-    cl = reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<uint8_t*>(dzh) + 2 * M * B * n);
-    c8 = reinterpret_cast<uint8_t*>(dzh) + 2 * M * B * n + dz8;
-    xtl = c.take<uint8_t>(xm * dd * Bp);
-    xtx = c.take<uint8_t>(xm * dd * Bp);
-    gtl = c.take<uint8_t>(M * dd * Bp);
-    gtx = c.take<uint8_t>(M * dd * Bp);
+    w.c.lo = w.dz.lo;
+    w.c.x8 = w.dz.x8;
+    w.xt.lo = c.take<uint8_t>(xm * dd * Bp);
+    w.xt.x8 = c.take<uint8_t>(xm * dd * Bp);
+    w.gt.lo = c.take<uint8_t>(M * dd * Bp);
+    w.gt.x8 = c.take<uint8_t>(M * dd * Bp);
+    w.c.f8 = w.ct.f8 = w.xt.f8 = w.gt.f8 = true;
   }
-  auto dwe = c.take<float>(M * n * dd);
-  float* dwd = dwe;
-  if (d.variant == SCE_UNTIED) dwd = c.take<float>(M * n * dd);
+  w.dw_enc = c.take<float>(M * n * dd);
+  w.dw_dec = d.variant == SCE_UNTIED ? c.take<float>(M * n * dd) : w.dw_enc;
   const size_t enc_parts = d.variant == SCE_TOPK ? B : tiles_mB * 8 * tiles_nN;
-  auto pe = c.take<float>(M * enc_parts * 2);
+  w.part_enc = c.take<float>(M * enc_parts * 2);
   const size_t dec_parts = tiles_mB * 8 * tiles_nD;   // top-k: up to kTopkMaxSlices partials per row from the gather kernel
-  auto pd = c.take<float>(M * (d.variant == SCE_TOPK && dec_parts < kTopkMaxSlices * B ? kTopkMaxSlices * B : dec_parts));
-  auto dbp = c.take<float>(M * tiles_mB * 4 * n);
-  auto bn = c.take<float>(M);
-  auto lob = c.take<float>(M);
-  auto ls = c.take<float>(M * 4);
-  auto ns = c.take<float>(M);
+  w.part_dec = c.take<float>(M * (d.variant == SCE_TOPK && dec_parts < kTopkMaxSlices * B ? kTopkMaxSlices * B : dec_parts));
+  w.db_part = c.take<float>(M * tiles_mB * 4 * n);
+  w.bnorm = c.take<float>(M);
+  w.l1_over_b = c.take<float>(M);
+  w.loss_stage = c.take<float>(M * 4);
+  w.nnz_stage = c.take<float>(M);
   const size_t n_chunks = (n + 31) / 32;
-  auto apos = c.take<uint32_t>(M * n_chunks * B);
-  auto azero = c.take<uint32_t>(M * n_chunks * B);
+  w.act_pos = c.take<uint32_t>(M * n_chunks * B);
+  w.act_zero = c.take<uint32_t>(M * n_chunks * B);
   // top-k: scores of their own (the code-gradient planes must keep their scattered zeros) and the k-sparse lists
-  const size_t kmax = topk_kmax(d);
-  float* sc = nullptr;
-  int *tkc = nullptr, *tkn = nullptr, *tkm = nullptr;
-  float *tkv = nullptr, *tkd = nullptr, *wnf = nullptr;
-  uint32_t* tcm = nullptr;
   if (d.variant == SCE_TOPK) {
-    sc = c.take<float>(M * B * n);
-    tcm = c.take<uint32_t>(M * B * n_chunks);
+    const size_t kmax = topk_kmax(d);
+    w.scores = c.take<float>(M * B * n);
+    w.tk_cmax = c.take<uint32_t>(M * B * n_chunks);
     if (kmax) {
-      tkc = c.take<int>(M * B * kmax);
-      tkv = c.take<float>(M * B * kmax);
-      tkn = c.take<int>(M * B);
-      tkm = c.take<int>(M);
-      tkd = c.take<float>(M * B * kmax * kTopkMaxSlices);
-      wnf = c.take<float>(M * n * dd);
+      w.tk_col = c.take<int>(M * B * kmax);
+      w.tk_val = c.take<float>(M * B * kmax);
+      w.tk_cnt = c.take<int>(M * B);
+      w.tk_models = c.take<int>(M);
+      w.tk_dots = c.take<float>(M * B * kmax * kTopkMaxSlices);
+      w.wn_f32 = c.take<float>(M * n * dd);
     }
   }
-  __nv_bfloat16 *roth = nullptr, *rotl = nullptr;
-  uint8_t* rot8 = nullptr;
-  float* xcen = nullptr;
   if (d.centering) {
-    planes(M * dd * dd, roth, rotl, rot8);
-    xcen = c.take<float>(M * B * dd);
+    w.rot = c.planes(M * dd * dd, f8);
+    w.x_centered = c.take<float>(M * B * dd);
   }
-  auto rf = c.take<uint32_t>(kFlagWords);   // [0] residual flag, [kAbsmaxWord] input range monitor, [kBadWord] health (separate 128-byte lines)
-  if (p) {
-    p->x_stage = X;
-    p->x_hi = xh;
-    p->x_lo = xl;
-    p->wenc_hi = weh;
-    p->wenc_lo = wel;
-    p->wdec_hi = wdh;
-    p->wdec_lo = wdl;
-    p->c_hi = ch;
-    p->c_lo = cl;
-    p->g_hi = gh;
-    p->g_lo = gl;
-    p->dz_hi = dzh;
-    p->dz_lo = dzh + M * B * n;
-    p->dz_x8 = f8 ? reinterpret_cast<uint8_t*>(dzh) + 2 * M * B * n + dz8 : nullptr;
-    p->xt_lo = xtl;
-    p->xt_x8 = xtx;
-    p->ct_lo = ctl;
-    p->ct_x8 = ctx;
-    p->gt_lo = gtl;
-    p->gt_x8 = gtx;
-    p->bpad = (int)Bp;
-    p->x_x8 = x8;
-    p->wenc_x8 = we8;
-    p->wdec_x8 = wd8;
-    p->wdt_hi = wth;
-    p->wdt_lo = wtl;
-    p->wdt_x8 = wt8;
-    p->c_x8 = c8;
-    p->g_x8 = g8;
-    p->dw_enc = dwe;
-    p->dw_dec = dwd;
-    p->part_enc = pe;
-    p->part_dec = pd;
-    p->db_part = dbp;
-    p->bnorm = bn;
-    p->l1_over_b = lob;
-    p->loss_stage = ls;
-    p->nnz_stage = ns;
-    p->res_flags = rf;
-    p->rot_hi = roth;
-    p->rot_lo = rotl;
-    p->rot_x8 = rot8;
-    p->x_centered = xcen;
-    p->scores = sc;
-    p->tk_cmax = tcm;
-    p->tk_models = tkm;
-    p->tk_col = tkc;
-    p->tk_val = tkv;
-    p->tk_cnt = tkn;
-    p->tk_dots = tkd;
-    p->wn_f32 = wnf;
-    p->tk_kmax = (int)kmax;
-    p->act_pos = apos;
-    p->act_zero = azero;
-    p->tiles_mB_max = (int)tiles_mB;
-  }
+  w.res_flags = c.take<uint32_t>(kFlagWords);   // [0] residual flag, [kAbsmaxWord] input range monitor, [kBadWord] health (separate 128-byte lines)
   return align_up(c.off, 1024);
 }
 
@@ -418,24 +370,23 @@ static CUtensorMapSwizzle swizzle_for_bk(int bk) {
 // maps. kmajor_bk != 0: K-major tiles [box_rows][kmajor_bk]; else MN-major tiles of `box_rows` k-rows by 64 (16-bit)
 // / 128 (8-bit) contiguous elements. K-major 8-bit tiles (64-byte rows in f16f8) carry the 64-byte swizzle E5M2 wgmma
 // reads; MN-major ones arrive unswizzled and the GEMM widens them to fp16 (widen_tile).
-static bool operand_maps(int arith, CUtensorMap* hi, CUtensorMap* lo, CUtensorMap* x8, const void* phi, const void* plo,
-                         const void* px8, uint64_t models, uint64_t rows, uint64_t cols, uint64_t mpitch,
+static bool operand_maps(OperandMaps& m, const Planes& P, uint64_t models, uint64_t rows, uint64_t cols, uint64_t mpitch,
                          uint32_t box_rows, int kmajor_bk) {
   bool ok;
   if (kmajor_bk) {
-    ok = make_tmap_bf16_box(hi, phi, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
-    if (arith == kArithF16F8)
-      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_64B) &&
-           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
+    ok = make_tmap_bf16_box(&m.hi, P.hi, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
+    if (P.f8)
+      ok = ok && make_tmap_u8_box(&m.lo, P.lo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_64B) &&
+           make_tmap_u8_box(&m.x8, P.x8, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
     else
-      ok = ok && make_tmap_bf16_box(lo, plo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
+      ok = ok && make_tmap_bf16_box(&m.lo, P.lo, models, rows, cols, cols, mpitch, kmajor_bk, box_rows, swizzle_for_bk(kmajor_bk));
   } else {
-    ok = make_tmap_bf16(hi, phi, models, rows, cols, cols, mpitch, box_rows);
-    if (arith == kArithF16F8)
-      ok = ok && make_tmap_u8_box(lo, plo, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE) &&
-           make_tmap_u8_box(x8, px8, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
+    ok = make_tmap_bf16(&m.hi, P.hi, models, rows, cols, cols, mpitch, box_rows);
+    if (P.f8)
+      ok = ok && make_tmap_u8_box(&m.lo, P.lo, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE) &&
+           make_tmap_u8_box(&m.x8, P.x8, models, rows, cols, cols, mpitch, 128, box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
     else
-      ok = ok && make_tmap_bf16(lo, plo, models, rows, cols, cols, mpitch, box_rows);
+      ok = ok && make_tmap_bf16(&m.lo, P.lo, models, rows, cols, cols, mpitch, box_rows);
   }
   return ok;
 }
@@ -453,74 +404,49 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   const uint64_t M = d.n_models, n = d.n, dd = d.d, xm = p->xm, Bm = d.batch_max;
   // NOTE: activations are laid out with the plan's batch_max pitch between models; only `B` rows are
   // visible through the map, so rows >= B read as zero (TMA out-of-bounds fill).
-  const int ar = p->arith;
-  const bool f8 = ar == kArithF16F8;
-  const int bk = gemm_bk(ar);
-  struct Pl { const void *hi, *lo, *x8; };
-  const Pl X{p->x_hi, p->x_lo, p->x_x8}, WE{p->wenc_hi, p->wenc_lo, p->wenc_x8}, WD{p->wdec_hi, p->wdec_lo, p->wdec_x8},
-      C{p->c_hi, p->c_lo, p->c_x8}, G{p->g_hi, p->g_lo, p->g_x8}, DZ{p->dz_hi, p->dz_lo, p->dz_x8};
-  // activations [models][B of batch_max][cols]: K-major A tiles [128 rows][bk] / MN-major tiles of bk batch rows
-  auto actk = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
-    return operand_maps(ar, &g.a_hi[set], &g.a_lo[set], &g.a_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, kBM, bk);
-  };
-  auto act_a = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
-    return operand_maps(ar, &g.a_hi[set], &g.a_lo[set], &g.a_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk, 0);
-  };
-  auto act_b = [&](GemmMaps& g, int set, const Pl& P, uint64_t models, uint64_t cols) {
-    return operand_maps(ar, &g.b_hi[set], &g.b_lo[set], &g.b_x8[set], P.hi, P.lo, P.x8, models, (uint64_t)B, cols, Bm * cols, bk, 0);
+  const bool f8 = p->arith == kArithF16F8;
+  const int bk = gemm_bk(p->arith);
+  // activations [models][B of batch_max][cols] as the A operand: K-major tiles [128 rows][bk]
+  auto act_a = [&](OperandMaps& o, const Planes& P, uint64_t models, uint64_t cols) {
+    return operand_maps(o, P, models, (uint64_t)B, cols, Bm * cols, kBM, bk);
   };
   // dictionary [M][n][d] as the B operand: K-major tiles [box_rows][bk] (box_rows = the tile's B rows), or MN-major
-  auto dict_b = [&](GemmMaps& g, const Pl& P, uint32_t box_rows, int kmajor_bk) {
-    return operand_maps(ar, &g.b_hi[0], &g.b_lo[0], &g.b_x8[0], P.hi, P.lo, P.x8, M, n, dd, n * dd, box_rows, kmajor_bk);
+  auto dict_b = [&](OperandMaps& o, const Planes& P, uint32_t box_rows, int kmajor_bk) {
+    return operand_maps(o, P, M, n, dd, n * dd, box_rows, kmajor_bk);
   };
   bool ok = true;
   // encode: A = x [xm,B,d] K-major, B = Wenc [M,n,d] K-major
-  ok &= actk(m->encode, 0, X, xm, dd);
-  ok &= dict_b(m->encode, WE, kBN, bk);
+  ok &= act_a(m->encode.a[0], p->x, xm, dd);
+  ok &= dict_b(m->encode.b[0], p->wenc, kBN, bk);
   if (d.centering) {
     // centring: A = (x - trans) planes in the X planes (the encode A maps), B = rot [M,d,d] K-major, output d columns
-    m->center.a_hi[0] = m->encode.a_hi[0];
-    m->center.a_lo[0] = m->encode.a_lo[0];
-    m->center.a_x8[0] = m->encode.a_x8[0];
-    ok &= operand_maps(ar, &m->center.b_hi[0], &m->center.b_lo[0], &m->center.b_x8[0], p->rot_hi, p->rot_lo, p->rot_x8, M, dd, dd,
-                       dd * dd, kBN, bk);
+    m->center.a[0] = m->encode.a[0];
+    ok &= operand_maps(m->center.b[0], p->rot, M, dd, dd, dd * dd, kBN, bk);
   }
   // decode: A = c [M,B,n] K-major, B = Wdec [M,n,d] MN-major (bk k-rows per box); f16f8: its transposed copy [M,d,n] K-major
-  ok &= actk(m->decode, 0, C, M, n);
-  if (f8)
-    ok &= operand_maps(ar, &m->decode.b_hi[0], &m->decode.b_lo[0], &m->decode.b_x8[0], p->wdt_hi, p->wdt_lo, p->wdt_x8, M, dd, n,
-                       dd * n, kBN, bk);
-  else
-    ok &= dict_b(m->decode, WD, bk, 0);
+  ok &= act_a(m->decode.a[0], p->c, M, n);
+  ok &= f8 ? operand_maps(m->decode.b[0], p->wdt, M, dd, n, dd * n, kBN, bk) : dict_b(m->decode.b[0], p->wdec, bk, 0);
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
-  ok &= actk(m->dcode, 0, G, M, dd);
-  ok &= dict_b(m->dcode, WD, kBN, bk);
-  // weight gradients: everything MN-major, reduction over the batch rows. dw_native: the 8-bit planes come from the
-  // batch-major copies [models][rows][Bp] instead, K-major tiles [128 rows][64 B] with the 64-byte swizzle; only B
-  // columns are exposed, so the tail of a short batch reads as zero
+  ok &= act_a(m->dcode.a[0], p->g, M, dd);
+  ok &= dict_b(m->dcode.b[0], p->wdec, kBN, bk);
+  // weight gradients: everything MN-major, tiles of bk batch rows, reduction over the batch rows. dw_native: the 8-bit
+  // planes come from the batch-major copies T [models][cols][Bp] instead, K-major tiles [128 rows][64 B] with the 64-byte
+  // swizzle; only B columns are exposed, so the tail of a short batch reads as zero
   const uint64_t Bp = (uint64_t)p->bpad;
-  struct Pt { const uint8_t *lo, *x8; };
-  const Pt XT{p->xt_lo, p->xt_x8}, CT{p->ct_lo, p->ct_x8}, GT{p->gt_lo, p->gt_x8},
-      DZT{reinterpret_cast<const uint8_t*>(p->dz_lo), p->dz_x8};
-  auto kmaj8 = [&](CUtensorMap* lo, CUtensorMap* x8, const Pt& T, uint64_t models, uint64_t rows) {
-    return make_tmap_u8_box(lo, T.lo, models, rows, (uint64_t)B, Bp, rows * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
-           make_tmap_u8_box(x8, T.x8, models, rows, (uint64_t)B, Bp, rows * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+  auto dw_operand = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t models, uint64_t cols) {
+    if (!p->dw_native) return operand_maps(o, P, models, (uint64_t)B, cols, Bm * cols, bk, 0);
+    return make_tmap_bf16(&o.hi, P.hi, models, (uint64_t)B, cols, cols, Bm * cols, bk) &&
+           make_tmap_u8_box(&o.lo, T.lo, models, cols, (uint64_t)B, Bp, cols * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
+           make_tmap_u8_box(&o.x8, T.x8, models, cols, (uint64_t)B, Bp, cols * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
   };
-  auto dw_set = [&](GemmMaps& g, int set, const Pl& A, const Pt& AT, uint64_t am, const Pl& Bo, const Pt& BT, uint64_t bm,
-                    uint64_t bcols) {
-    bool r = act_a(g, set, A, am, n) && act_b(g, set, Bo, bm, bcols);
-    if (p->dw_native) r = r && kmaj8(&g.a_lo[set], &g.a_x8[set], AT, am, n) && kmaj8(&g.b_lo[set], &g.b_x8[set], BT, bm, bcols);
-    return r;
-  };
-  if (d.variant == SCE_UNTIED) {
-    ok &= dw_set(m->dw_enc, 0, DZ, DZT, M, X, XT, xm, dd);
-    ok &= dw_set(m->dw_dec, 0, C, CT, M, G, GT, M, dd);
-  } else {
-    ok &= dw_set(m->dw_enc, 0, DZ, DZT, M, X, XT, xm, dd);
-    ok &= dw_set(m->dw_enc, 1, C, CT, M, G, GT, M, dd);
-  }
-  ok &= make_tmap_bf16_store32(&m->st_c_hi, p->c_hi, M, (uint64_t)B, n, Bm * n);
-  ok &= make_tmap_bf16_store32(&m->st_dz_hi, p->dz_hi, M, (uint64_t)B, n, Bm * n);
+  // dz^T x, then c^T g: a second GEMM of the decoder (untied) or a second operand set of the one dictionary's
+  // (dz's own 8-bit planes are batch-major in dw_native plans)
+  GemmMaps& cg = d.variant == SCE_UNTIED ? m->dw_dec : m->dw_enc;
+  const int cg_set = d.variant == SCE_UNTIED ? 0 : 1;
+  ok &= dw_operand(m->dw_enc.a[0], p->dz, p->dz, M, n) && dw_operand(m->dw_enc.b[0], p->x, p->xt, xm, dd);
+  ok &= dw_operand(cg.a[cg_set], p->c, p->ct, M, n) && dw_operand(cg.b[cg_set], p->g, p->gt, M, dd);
+  ok &= make_tmap_bf16_store32(&m->st_c.hi, p->c.hi, M, (uint64_t)B, n, Bm * n);
+  ok &= make_tmap_bf16_store32(&m->st_dz.hi, p->dz.hi, M, (uint64_t)B, n, Bm * n);
   if (f8) {
     auto st8 = [&](CUtensorMap* t, const void* base) {
       return make_tmap_u8_box(t, base, M, (uint64_t)B, n, n, Bm * n, 32, 32, CU_TENSOR_MAP_SWIZZLE_32B);
@@ -529,12 +455,12 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
     auto st8t = [&](CUtensorMap* t, const void* base) {
       return make_tmap_u8_box(t, base, M, n, (uint64_t)B, Bp, n * Bp, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE);
     };
-    ok &= st8(&m->st_c_lo, p->c_lo) && st8(&m->st_c_x8, p->c_x8);
-    ok &= p->dw_native ? st8t(&m->st_dz_lo, p->dz_lo) && st8t(&m->st_dz_x8, p->dz_x8)
-                       : st8(&m->st_dz_lo, p->dz_lo) && st8(&m->st_dz_x8, p->dz_x8);
+    ok &= st8(&m->st_c.lo, p->c.lo) && st8(&m->st_c.x8, p->c.x8);
+    ok &= p->dw_native ? st8t(&m->st_dz.lo, p->dz.lo) && st8t(&m->st_dz.x8, p->dz.x8)
+                       : st8(&m->st_dz.lo, p->dz.lo) && st8(&m->st_dz.x8, p->dz.x8);
   } else {
-    ok &= make_tmap_bf16_store32(&m->st_c_lo, p->c_lo, M, (uint64_t)B, n, Bm * n);
-    ok &= make_tmap_bf16_store32(&m->st_dz_lo, p->dz_lo, M, (uint64_t)B, n, Bm * n);
+    ok &= make_tmap_bf16_store32(&m->st_c.lo, p->c.lo, M, (uint64_t)B, n, Bm * n);
+    ok &= make_tmap_bf16_store32(&m->st_dz.lo, p->dz.lo, M, (uint64_t)B, n, Bm * n);
   }
   if (d.variant == SCE_TOPK) ok &= make_tmap_f32_store32(&m->st_scores, p->scores, M, (uint64_t)B, n, Bm * n);
   if (!ok) {
@@ -555,6 +481,17 @@ struct ResFlags {
   const uint32_t* b[kMaxSets] = {nullptr, nullptr};
 };
 
+// the tensor maps of operand set `s` into the kernel's parameters
+template <class EpiParams>
+static void set_operand_maps(GemmParams<EpiParams>& gp, int s, const OperandMaps& a, const OperandMaps& b) {
+  gp.a_hi[s] = a.hi;
+  gp.a_lo[s] = a.lo;
+  gp.a_x8[s] = a.x8;
+  gp.b_hi[s] = b.hi;
+  gp.b_lo[s] = b.lo;
+  gp.b_x8[s] = b.x8;
+}
+
 // NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN then describe the fp16
 // planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps batch-major copies.
 template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool NATIVE = ARITH == kArithF16F8 && !A_MN>
@@ -564,12 +501,7 @@ static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, con
   GemmParams<typename Epi::Params> gp;
   memset(&gp, 0, sizeof(gp));
   for (int s = 0; s < nsets; ++s) {
-    gp.a_hi[s] = maps.a_hi[s];
-    gp.a_lo[s] = maps.a_lo[s];
-    gp.b_hi[s] = maps.b_hi[s];
-    gp.b_lo[s] = maps.b_lo[s];
-    gp.a_x8[s] = maps.a_x8[s];
-    gp.b_x8[s] = maps.b_x8[s];
+    set_operand_maps(gp, s, maps.a[s], maps.b[s]);
     gp.a_batched[s] = a_batched[s];
     gp.b_batched[s] = b_batched[s];
     gp.a_res_flag[s] = rf.a[s];
@@ -605,9 +537,10 @@ static AdamHyper hyper_for(const sce_plan* p, long long t) {
 }
 
 template <int MODE, int ARITH>
-static int launch_dict_rows_t(float* e, const float* dw, float* m, float* v, void* hi, void* lo, void* x8,
-                              float* grad_out, long long rows, int d, int normalize, float floor, AdamHyper h,
-                              const uint32_t* health, float* w_f32, cudaStream_t st) {
+static int launch_dict_rows_t(float* e, const float* dw, float* m, float* v, const Planes& w, float* grad_out,
+                              long long rows, int d, int normalize, float floor, AdamHyper h, const uint32_t* health,
+                              float* w_f32, cudaStream_t st) {
+  void *const hi = w.hi, *const lo = w.lo, *const x8 = w.x8;
   const int nv = (d + 511) / 512;
   if (nv == 1)
     dict_rows_kernel<1, MODE, ARITH><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
@@ -622,18 +555,39 @@ static int launch_dict_rows_t(float* e, const float* dw, float* m, float* v, voi
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }
-// `which`: 0 = the encoder's operand planes, 1 = the decoder's
+// One dictionary of the plan: its weights, their gradient, Adam moments, operand planes and row normalisation
+struct DictSide {
+  float *w, *dw, *m, *v;
+  Planes planes;
+  int normalize;
+  float floor;
+};
+// The plan's dictionaries, encoder first: one for tied and top-k plans, which normalise it; two for untied plans, whose
+// decoder alone is normalised. Returns the count.
+static int dict_sides(const sce_plan* p, DictSide out[2]) {
+  const sce_buffers& b = p->b;
+  if (p->d.variant != SCE_UNTIED) {
+    out[0] = {b.encoder, p->dw_enc, b.encoder_m, b.encoder_v, p->wenc, 1, p->d.norm_floor};
+    return 1;
+  }
+  out[0] = {b.encoder, p->dw_enc, b.encoder_m, b.encoder_v, p->wenc, 0, 0.f};
+  out[1] = {b.decoder, p->dw_dec, b.decoder_m, b.decoder_v, p->wdec, 1, p->d.norm_floor};
+  return 2;
+}
+
+// MODE_PREPARE reads the weights and writes the planes; MODE_ADAM also reads dW and updates the moments; MODE_GRAD
+// reads the weights and dW and writes `grad_out` only
 template <int MODE>
-static int launch_dict_rows(const sce_plan* p, int which, float* e, const float* dw, float* m, float* v, float* grad_out,
-                            long long rows, int d, int normalize, float floor, AdamHyper h, cudaStream_t st) {
-  void* hi = which ? (void*)p->wdec_hi : (void*)p->wenc_hi;
-  void* lo = which ? (void*)p->wdec_lo : (void*)p->wenc_lo;
-  void* x8 = which ? (void*)p->wdec_x8 : (void*)p->wenc_x8;
-  if (MODE == MODE_GRAD) hi = lo = x8 = nullptr;
+static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_out, AdamHyper h, cudaStream_t st) {
+  const long long rows = (long long)p->d.n_models * p->d.n;
+  const float* dw = MODE == MODE_PREPARE ? nullptr : s.dw;
+  float* m = MODE == MODE_ADAM ? s.m : nullptr;
+  float* v = MODE == MODE_ADAM ? s.v : nullptr;
+  const Planes w = MODE == MODE_GRAD ? Planes{} : s.planes;
   float* wf = (MODE != MODE_GRAD && p->topk_sparse) ? p->wn_f32 : nullptr;   // (top-k plans have one dictionary)
   return p->arith == kArithF16F8
-             ? launch_dict_rows_t<MODE, kArithF16F8>(e, dw, m, v, hi, lo, x8, grad_out, rows, d, normalize, floor, h, p->res_flags, wf, st)
-             : launch_dict_rows_t<MODE, kArithBf16x3>(e, dw, m, v, hi, lo, x8, grad_out, rows, d, normalize, floor, h, p->res_flags, wf, st);
+             ? launch_dict_rows_t<MODE, kArithF16F8>(s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st)
+             : launch_dict_rows_t<MODE, kArithBf16x3>(s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
 }
 
 // f16f8: the decoder's planes -> their transposed copy, which the decode GEMM reads K-major (nothing to do where the
@@ -642,11 +596,11 @@ static int transpose_dict(const sce_plan* p, cudaStream_t st, int& launches) {
   if (p->arith != kArithF16F8 || p->topk_sparse) return SCE_OK;
   const sce_desc& d = p->d;
   const dim3 grid((d.d + 63) / 64, (d.n + 63) / 64, d.n_models);
-  transpose_kernel<uint16_t><<<grid, 256, 0, st>>>(reinterpret_cast<const uint16_t*>(p->wdec_hi),
-                                                   reinterpret_cast<uint16_t*>(p->wdt_hi), d.n, d.d);
-  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(reinterpret_cast<const uint8_t*>(p->wdec_lo),
-                                                  reinterpret_cast<uint8_t*>(p->wdt_lo), d.n, d.d);
-  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(p->wdec_x8, p->wdt_x8, d.n, d.d);
+  transpose_kernel<uint16_t><<<grid, 256, 0, st>>>(static_cast<const uint16_t*>(p->wdec.hi),
+                                                   static_cast<uint16_t*>(p->wdt.hi), d.n, d.d);
+  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(p->wdec.lo),
+                                                  static_cast<uint8_t*>(p->wdt.lo), d.n, d.d);
+  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(p->wdec.x8, p->wdt.x8, d.n, d.d);
   CUDA_TRY(cudaGetLastError());
   launches += 3;
   return SCE_OK;
@@ -697,7 +651,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     const long long n4 = (long long)B * dd / 4;
     const int blocks = (int)((n4 + 255) / 256 < 1024 ? (n4 + 255) / 256 : 1024);
     center_split_kernel<AR><<<dim3(blocks, M), 256, 0, st>>>(
-        x, d.centering == 2 ? (long long)B * dd : 0, p->b.center_trans, p->x_hi, p->x_lo, p->x_x8, Bm * dd, B, dd);
+        x, d.centering == 2 ? (long long)B * dd : 0, p->b.center_trans, p->x.hi, p->x.lo, p->x.x8, Bm * dd, B, dd);
     CUDA_TRY(cudaGetLastError());
     EpiCenter::Params cp;
     cp.out = p->x_centered;
@@ -712,23 +666,20 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace
   if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), st));
   for (int m = 0; m < p->xm; ++m) {
-    // (bf16x3: the lo plane is 2 B / element; f16f8: lo and x8 are 1 B / element)
-    launch_split_rows<AR>(x + (long long)m * B * dd, p->x_hi + m * Bm * dd,
-                          f8 ? (void*)(reinterpret_cast<uint8_t*>(p->x_lo) + m * Bm * dd) : (void*)(p->x_lo + m * Bm * dd),
-                          f8 ? (void*)(p->x_x8 + m * Bm * dd) : nullptr, (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st);
+    launch_split_rows<AR>(x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st);
     ++launches;
   }
   CUDA_TRY(cudaGetLastError());
   // dw_native: batch-major copies of the 8-bit planes of x, c and g for the weight gradient (dz's are written so by dcode)
   const bool tdw = f8 && backward && p->dw_native;
-  auto batch_major = [&](const void* lo, const uint8_t* x8, uint8_t* tlo, uint8_t* tx8, int models, int cols) {
-    const BatchPlanes t{{static_cast<const uint8_t*>(lo), x8}, {tlo, tx8}};
+  auto batch_major = [&](const Planes& P, const Planes& T, int models, int cols) {
+    const BatchPlanes t{{static_cast<const uint8_t*>(P.lo), P.x8}, {static_cast<uint8_t*>(T.lo), T.x8}};
     transpose_batch_u8_kernel<<<dim3((cols + 127) / 128, (B + 127) / 128, 2 * models), 256, 0, st>>>(t, models, B, cols,
                                                                                                  Bm * cols, p->bpad);
     ++launches;
     return cudaGetLastError();
   };
-  if (tdw) CUDA_TRY(batch_major(p->x_lo, p->x_x8, p->xt_lo, p->xt_x8, p->xm, dd));
+  if (tdw) CUDA_TRY(batch_major(p->x, p->xt, p->xm, dd));
   p->code_batch_major = tdw ? 1 : 0;
   // alpha / B, or (f16f8, backward on r = g B d / 2) alpha d / 2
   l1_over_b_kernel<<<(M + 127) / 128, 128, 0, st>>>(p->b.l1_alpha, p->l1_over_b, M, f8 ? 0.5f * (float)dd : 1.0f / (float)B);
@@ -751,9 +702,9 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   TopkLists tk = {nullptr, nullptr, nullptr, 0, 0};
   if (d.variant != SCE_TOPK) {
     auto fill = [&](auto& ep) {
-      ep.out_hi = maps->st_c_hi;
-      ep.out_lo = maps->st_c_lo;
-      ep.out_x8 = maps->st_c_x8;
+      ep.out_hi = maps->st_c.hi;
+      ep.out_lo = maps->st_c.lo;
+      ep.out_x8 = maps->st_c.x8;
       ep.bias = p->b.encoder_bias;
       ep.mask = p->b.coef_mask;
       ep.part = p->part_enc;
@@ -777,7 +728,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     if (rc) return rc;
     ++launches;
     n_enc_parts = tiles_mB * 8 * ((n + kBN - 1) / kBN);
-    if (tdw) CUDA_TRY(batch_major(p->c_lo, p->c_x8, p->ct_lo, p->ct_x8, M, n));
+    if (tdw) CUDA_TRY(batch_major(p->c, p->ct, M, n));
   } else {
     // scores -> fp32, then per-row selection (code planes, activity mask, k-sparse lists)
     EpiScoresTma::Params sp;
@@ -798,7 +749,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     tk.batch_max = d.batch_max;
     // one block per (row, model); scores / codes of model m start at m * batch_max * n
     topk_select2_kernel<AR><<<dim3(B, M), 256, 0, st>>>(
-        p->scores, p->b.sparsity, p->c_hi, p->c_lo, p->c_x8, p->topk_sparse ? (void*)p->dz_hi : nullptr, p->dz_lo, p->dz_x8,
+        p->scores, p->b.sparsity, p->c.hi, p->c.lo, p->c.x8, p->topk_sparse ? p->dz.hi : nullptr, p->dz.lo, p->dz.x8,
         act, tk, p->part_enc, B, n, Bm * n, p->topk_cmax ? p->tk_cmax : nullptr);
     ++launches;
     CUDA_TRY(cudaGetLastError());
@@ -817,38 +768,38 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       const int cnt = p->tk_group_off[g + 1] - p->tk_group_off[g];
       if (cnt == 0) continue;
       topk_sparse_kernel<AR><<<dim3(B, cnt, p->tk_slices), 256, topk_sparse_smem(d, p->tk_group_krows[g], p->tk_slices), st>>>(
-          tk, p->b.sparsity, p->wn_f32, x, d.x_per_model ? (long long)B * dd : 0, p->g_hi, p->g_lo, p->g_x8, x_hat, p->part_dec,
+          tk, p->b.sparsity, p->wn_f32, x, d.x_per_model ? (long long)B * dd : 0, p->g.hi, p->g.lo, p->g.x8, x_hat, p->part_dec,
           backward ? p->tk_dots : nullptr, B, n, dd, gscale, p->tk_models + p->tk_group_off[g], p->tk_group_krows[g]);
       ++launches;
     }
     CUDA_TRY(cudaGetLastError());
     n_dec_parts = p->tk_slices * B;
   } else {
-  // ---- decode (+ residual, loss partial, g)
-  typename EpiDec::Params dp;
-  dp.x = x;
-  dp.x_model_stride = d.x_per_model ? (long long)B * dd : 0;
-  dp.g_hi = reinterpret_cast<uint16_t*>(p->g_hi);
-  dp.g_lo = reinterpret_cast<uint8_t*>(p->g_lo);
-  dp.g_x8 = p->g_x8;
-  dp.x_hat = x_hat;
-  dp.part = p->part_dec;
-  dp.g_model_stride = Bm * dd;
-  dp.xhat_model_stride = (long long)B * dd;
-  dp.ld = dd;
-  dp.tiles_m = tiles_mB;
-  dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
-  dp.tiles_n = (dd + kBN - 1) / kBN;
-  if constexpr (f8)
-    rc = launch_gemm_t<EpiDec, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-  else if (p->split_decode)
-    rc = launch_gemm_t<EpiDec, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-  else
-    rc = launch_gemm_t<EpiDec, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-  if (rc) return rc;
-  ++launches;
-  n_dec_parts = tiles_mB * 8 * dp.tiles_n;
-  if (tdw) CUDA_TRY(batch_major(p->g_lo, p->g_x8, p->gt_lo, p->gt_x8, M, dd));
+    // ---- decode (+ residual, loss partial, g)
+    typename EpiDec::Params dp;
+    dp.x = x;
+    dp.x_model_stride = d.x_per_model ? (long long)B * dd : 0;
+    dp.g_hi = static_cast<uint16_t*>(p->g.hi);
+    dp.g_lo = static_cast<uint8_t*>(p->g.lo);
+    dp.g_x8 = p->g.x8;
+    dp.x_hat = x_hat;
+    dp.part = p->part_dec;
+    dp.g_model_stride = Bm * dd;
+    dp.xhat_model_stride = (long long)B * dd;
+    dp.ld = dd;
+    dp.tiles_m = tiles_mB;
+    dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
+    dp.tiles_n = (dd + kBN - 1) / kBN;
+    if constexpr (f8)
+      rc = launch_gemm_t<EpiDec, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    else if (p->split_decode)
+      rc = launch_gemm_t<EpiDec, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    else
+      rc = launch_gemm_t<EpiDec, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    if (rc) return rc;
+    ++launches;
+    n_dec_parts = tiles_mB * 8 * dp.tiles_n;
+    if (tdw) CUDA_TRY(batch_major(p->g, p->gt, M, dd));
   }
 
   // ---- losses
@@ -867,32 +818,32 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   if (backward) {
     if (sparse) {
       // ---- code gradient planes: zero the rows, scatter the k entries
-      topk_dz_scatter_kernel<AR><<<dim3(B, M), 64, 0, st>>>(tk, p->tk_dots, p->tk_slices, p->dz_hi, p->dz_lo, p->dz_x8, n);
+      topk_dz_scatter_kernel<AR><<<dim3(B, M), 64, 0, st>>>(tk, p->tk_dots, p->tk_slices, p->dz.hi, p->dz.lo, p->dz.x8, n);
       ++launches;
       CUDA_TRY(cudaGetLastError());
     } else {
-    // ---- dcode
-    auto dcode = [&](auto tag) {
-      using E = typename decltype(tag)::type;
-      typename E::Params zp;
-      zp.out_hi = maps->st_dz_hi;
-      zp.out_lo = maps->st_dz_lo;
-      zp.out_x8 = maps->st_dz_x8;
-      zp.act = act;
-      zp.l1_over_b = p->l1_over_b;
-      zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
-      zp.tiles_m = tiles_mB;
-      zp.planes = p->dw_passes >= 3 ? 3 : 0;
-      // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
-      // (per-model batches carry one flag for all of them, so the same test holds)
-      zp.x_res_flag = f8 ? p->res_flags : nullptr;
-      return launch_gemm_t<E, false, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
-    };
-    // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
-    if constexpr (f8) rc = p->dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
-    else rc = dcode(TypeTag<EpiDco>{});
-    if (rc) return rc;
-    ++launches;
+      // ---- dcode
+      auto dcode = [&](auto tag) {
+        using E = typename decltype(tag)::type;
+        typename E::Params zp;
+        zp.out_hi = maps->st_dz.hi;
+        zp.out_lo = maps->st_dz.lo;
+        zp.out_x8 = maps->st_dz.x8;
+        zp.act = act;
+        zp.l1_over_b = p->l1_over_b;
+        zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
+        zp.tiles_m = tiles_mB;
+        zp.planes = p->dw_passes >= 3 ? 3 : 0;
+        // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
+        // (per-model batches carry one flag for all of them, so the same test holds)
+        zp.x_res_flag = f8 ? p->res_flags : nullptr;
+        return launch_gemm_t<E, false, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
+      };
+      // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
+      if constexpr (f8) rc = p->dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
+      else rc = dcode(TypeTag<EpiDco>{});
+      if (rc) return rc;
+      ++launches;
     }
 
     // ---- weight gradients
@@ -1039,8 +990,8 @@ static size_t stats_workspace(const sce_desc& d, int B) {
 // :265-321 record selection): fragment g of a call is rows g L .. g L + L - 1.
 // ------------------------------------------------------------------------------------------------
 struct FragCode {             // the code of the last forward, as the engine holds it
-  const void* hi;             // c_hi plane [M][batch_max][n] (bf16 or fp16)
-  const void* lo;             // bf16x3: c_lo plane
+  const void* hi;             // the code's 16-bit plane [M][batch_max][n] (bf16 or fp16)
+  const void* lo;             // bf16x3: its second bf16 plane
   const uint8_t* x8;          // f16f8: E5M2 plane of the scaled residuals
   const float* scores;        // top-k: fp32 scores [M][batch_max][n]
   const uint32_t* pos;        // activity mask [M][n_chunks][batch_max]
@@ -1240,7 +1191,7 @@ struct SimOperand {   // one side of sce_similarity
 // f16f8 split, and (capacity) the sum-of-squares partials [P][na][2 tiles_n] and diagonal [P][na]. With base == nullptr
 // only measures; `f8` only changes the order of the planes, not the bytes.
 struct SimCarve {
-  void *a_hi, *a_lo, *a_x8, *b_hi, *b_lo, *b_x8;
+  Planes a, b;
   int *pairs, *a_rows, *b_rows;
   uint32_t* flags;
   float *sq_part, *diag;
@@ -1248,20 +1199,9 @@ struct SimCarve {
 static size_t sim_carve(uint8_t* base, bool f8, long long ma, long long na, long long mb, long long nb, long long d,
                         long long n_pairs, bool capacity, SimCarve* out) {
   Carve c{base, 0};
-  auto planes = [&](size_t count, void*& hi, void*& lo, void*& x8) {
-    hi = c.take<__nv_bfloat16>(count);
-    if (f8) {
-      lo = c.take<uint8_t>(count);
-      x8 = c.take<uint8_t>(count);
-    } else {
-      lo = c.take<__nv_bfloat16>(count);
-      x8 = nullptr;
-    }
-  };
-  SimCarve s;
-  memset(&s, 0, sizeof(s));
-  planes((size_t)(ma * na * d), s.a_hi, s.a_lo, s.a_x8);
-  if (mb > 0) planes((size_t)(mb * nb * d), s.b_hi, s.b_lo, s.b_x8);
+  SimCarve s{};
+  s.a = c.planes((size_t)(ma * na * d), f8);
+  if (mb > 0) s.b = c.planes((size_t)(mb * nb * d), f8);
   s.pairs = c.take<int>((size_t)(2 * n_pairs));
   s.a_rows = c.take<int>((size_t)ma);
   s.b_rows = mb > 0 ? c.take<int>((size_t)mb) : s.a_rows;
@@ -1283,12 +1223,12 @@ static size_t sim_workspace(long long ma, long long na, long long mb, long long 
 // fp32 operand -> planes: normalised rows (dict_rows_kernel<MODE_PREPARE>, LearnedDict.get_learned_dict) or the matrix
 // as given (split_rows_kernel; f16f8: sets the range flags when a value does not fit fp16)
 template <int AR>
-static int sim_planes(const SimOperand& o, int d, void* hi, void* lo, void* x8, uint32_t* flags, cudaStream_t st) {
+static int sim_planes(const SimOperand& o, int d, const Planes& w, uint32_t* flags, cudaStream_t st) {
   const long long rows = (long long)o.models * o.rows;
   if (o.normalize)
-    return launch_dict_rows_t<MODE_PREPARE, AR>(const_cast<float*>(o.w), nullptr, nullptr, nullptr, hi, lo, x8, nullptr, rows, d,
-                                                 1, o.floor, AdamHyper{}, nullptr, nullptr, st);
-  launch_split_rows<AR>(o.w, hi, lo, x8, rows * d / 4, AR == kArithF16F8 ? flags : nullptr, st);
+    return launch_dict_rows_t<MODE_PREPARE, AR>(const_cast<float*>(o.w), nullptr, nullptr, nullptr, w, nullptr, rows, d, 1,
+                                                 o.floor, AdamHyper{}, nullptr, nullptr, st);
+  launch_split_rows<AR>(o.w, w, rows * d / 4, AR == kArithF16F8 ? flags : nullptr, st);
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }
@@ -1296,23 +1236,20 @@ static int sim_planes(const SimOperand& o, int d, void* hi, void* lo, void* x8, 
 template <int AR>
 static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_a, int d, int n_pairs, const SimCarve& w,
                             float* row_max, float* col_max, float* capacity, int device, int sms, cudaStream_t st) {
-  int rc = sim_planes<AR>(A, d, w.a_hi, w.a_lo, w.a_x8, w.flags, st);
+  int rc = sim_planes<AR>(A, d, w.a, w.flags, st);
   if (rc) return rc;
   if (!b_is_a) {
-    rc = sim_planes<AR>(B, d, w.b_hi, w.b_lo, w.b_x8, w.flags, st);
+    rc = sim_planes<AR>(B, d, w.b, w.flags, st);
     if (rc) return rc;
   }
-  const void* const b_hi = b_is_a ? w.a_hi : w.b_hi;
-  const void* const b_lo = b_is_a ? w.a_lo : w.b_lo;
-  const void* const b_x8 = b_is_a ? w.a_x8 : w.b_x8;
   GemmParams<EpiSimilarity::Params> gp;
   memset(&gp, 0, sizeof(gp));
   // both operands are dictionary rows, K-major over d: the encode GEMM's B-operand geometry on both sides
-  bool ok = operand_maps(AR, &gp.a_hi[0], &gp.a_lo[0], &gp.a_x8[0], w.a_hi, w.a_lo, w.a_x8, A.models, A.rows, d,
-                         (uint64_t)A.rows * d, kBM, gemm_bk(AR));
-  ok = ok && operand_maps(AR, &gp.b_hi[0], &gp.b_lo[0], &gp.b_x8[0], b_hi, b_lo, b_x8, B.models, B.rows, d,
-                          (uint64_t)B.rows * d, kBN, gemm_bk(AR));
+  OperandMaps am{}, bm{};
+  bool ok = operand_maps(am, w.a, A.models, A.rows, d, (uint64_t)A.rows * d, kBM, gemm_bk(AR));
+  ok = ok && operand_maps(bm, b_is_a ? w.a : w.b, B.models, B.rows, d, (uint64_t)B.rows * d, kBN, gemm_bk(AR));
   if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (similarity: na=%d, nb=%d, d=%d)", A.rows, B.rows, d);
+  set_operand_maps(gp, 0, am, bm);
   gp.a_batched[0] = gp.b_batched[0] = 1;
   gp.nsets = 1;
   gp.k_total = d;
@@ -1357,9 +1294,14 @@ extern "C" {
 int sce_version(void) { return SCE_VERSION; }
 const char* sce_last_error(void) { return g_err; }
 
+static size_t plan_workspace(const sce_desc& d) {
+  PlanBuffers w{};
+  return carve(w, d, nullptr);
+}
+
 size_t sce_workspace_bytes(const sce_desc* desc) {
   if (validate(desc)) return 0;
-  return carve(nullptr, *desc, nullptr);
+  return plan_workspace(*desc);
 }
 
 int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan** out_plan) {
@@ -1375,7 +1317,7 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   if (desc->variant != SCE_TOPK && (!b.encoder_bias || !b.bias_m || !b.bias_v))
     return fail(SCE_ERR_INVALID, "encoder_bias / bias_m / bias_v are required for SAE variants");
   if (desc->variant == SCE_TOPK && !b.sparsity) return fail(SCE_ERR_INVALID, "top-k variant needs the sparsity buffer");
-  rc = check_workspace(b.workspace, b.workspace_bytes, carve(nullptr, *desc, nullptr), "");
+  rc = check_workspace(b.workspace, b.workspace_bytes, plan_workspace(*desc), "");
   if (rc) return rc;
   int dev = 0, sms = 0;
   rc = query_device(&dev, &sms);
@@ -1389,6 +1331,8 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   p->device = dev;
   p->xm = desc->x_per_model ? desc->n_models : 1;
   p->arith = resolve_arith(*desc);
+  p->bpad = (int)batch_pad(*desc);
+  p->tk_kmax = (int)topk_kmax(*desc);
   // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
   // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
   // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
@@ -1402,7 +1346,7 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   {
     // k-sparse decode / dcode of the top-k variant: lists known (topk_k_max), bulk-copy alignment of the dictionary
     // half rows (16 bytes in every plane), shared memory of the gather kernel
-    const size_t kmax = topk_kmax(*desc);
+    const size_t kmax = p->tk_kmax;
     p->tk_slices = kmax ? topk_slices(*desc, kmax) : 0;
     if (const char* v = getenv("SCE_TOPK_SLICES")) {
       const int sl = atoi(v);
@@ -1419,7 +1363,7 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
     p->topk_cmax = desc->variant == SCE_TOPK && tune_flag("SCE_TOPK_CMAX", 1);
   }
   p->maps = new std::map<int, BatchMaps*>();
-  carve(p, *desc, static_cast<uint8_t*>(b.workspace));
+  carve(*p, *desc, static_cast<uint8_t*>(b.workspace));
   *out_plan = p;
   return SCE_OK;
 }
@@ -1445,16 +1389,12 @@ int sce_prepare(sce_plan* p, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, kFlagWords * sizeof(uint32_t), st));   // residual flag, input range monitor, health
   const sce_desc& d = p->d;
-  const long long rows = (long long)d.n_models * d.n;
   if (d.variant == SCE_TOPK && p->tk_kmax) {
     // the top-k selection keeps the code planes (and, in k-sparse plans, the code-gradient planes) all-zero except for
     // the entries its lists record: start them zeroed, with empty lists
     const size_t el = (size_t)d.n_models * d.batch_max * d.n;
-    const bool f8 = p->arith == kArithF16F8;
-    CUDA_TRY(cudaMemsetAsync(p->c_hi, 0, el * 2, st));
-    CUDA_TRY(cudaMemsetAsync(p->c_lo, 0, el * (f8 ? 1 : 2), st));
-    if (f8) CUDA_TRY(cudaMemsetAsync(p->c_x8, 0, el, st));
-    CUDA_TRY(cudaMemsetAsync(p->dz_hi, 0, el * 4, st));   // (the code-gradient planes are one contiguous block, 4 B / element)
+    CUDA_TRY(p->c.zero(el, st));
+    CUDA_TRY(cudaMemsetAsync(p->dz.hi, 0, el * 4, st));   // (the code-gradient planes are one contiguous block, 4 B / element)
     CUDA_TRY(cudaMemsetAsync(p->act_pos, 0, (size_t)d.n_models * ((d.n + 31) / 32) * d.batch_max * sizeof(uint32_t), st));
     CUDA_TRY(cudaMemsetAsync(p->tk_cnt, 0, (size_t)d.n_models * d.batch_max * sizeof(int), st));
     // k classes for the gather kernel: rows of shared memory in {8, 16, 32, 64, ...} capped at the list capacity
@@ -1487,21 +1427,14 @@ int sce_prepare(sce_plan* p, void* stream) {
       return fail(SCE_ERR_INVALID, "centering needs the center_trans / center_rot / center_scale buffers");
     const long long n4 = (long long)d.n_models * d.d * d.d / 4;
     if (p->arith == kArithF16F8)
-      launch_split_rows<kArithF16F8>(p->b.center_rot, p->rot_hi, p->rot_lo, p->rot_x8, n4, nullptr, st);
+      launch_split_rows<kArithF16F8>(p->b.center_rot, p->rot, n4, nullptr, st);
     else
-      launch_split_rows<kArithBf16x3>(p->b.center_rot, p->rot_hi, p->rot_lo, nullptr, n4, nullptr, st);
+      launch_split_rows<kArithBf16x3>(p->b.center_rot, p->rot, n4, nullptr, st);
     CUDA_TRY(cudaGetLastError());
   }
-  AdamHyper h = hyper_for(p, 1);
-  int rc;
-  if (d.variant == SCE_UNTIED) {
-    rc = launch_dict_rows<MODE_PREPARE>(p, 0, p->b.encoder, nullptr, nullptr, nullptr, nullptr, rows, d.d, 0, 0.f, h, st);
-    if (rc) return rc;
-    rc = launch_dict_rows<MODE_PREPARE>(p, 1, p->b.decoder, nullptr, nullptr, nullptr, nullptr, rows, d.d, 1, d.norm_floor, h, st);
-  } else {
-    rc = launch_dict_rows<MODE_PREPARE>(p, 0, p->b.encoder, nullptr, nullptr, nullptr, nullptr, rows, d.d, 1, d.norm_floor, h, st);
-  }
-  if (rc) return rc;
+  DictSide sides[2];
+  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
+    if (int rc = launch_dict_rows<MODE_PREPARE>(p, sides[s], nullptr, hyper_for(p, 1), st)) return rc;
   int launches = 0;
   return transpose_dict(p, st, launches);
 }
@@ -1520,23 +1453,11 @@ static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, 
   int rc = run_pipeline(p, x, B, nullptr, true, out_losses, out_nnz, st);
   if (rc) return rc;
   const sce_desc& d = p->d;
-  const long long rows = (long long)d.n_models * d.n;
   const AdamHyper h = hyper_for(p, t);
   int launches = p->last_launches;
-  if (d.variant == SCE_UNTIED) {
-    rc = launch_dict_rows<MODE_ADAM>(p, 0, p->b.encoder, p->dw_enc, p->b.encoder_m, p->b.encoder_v, nullptr, rows, d.d, 0,
-                                     0.f, h, st);
-    if (rc) return rc;
-    rc = launch_dict_rows<MODE_ADAM>(p, 1, p->b.decoder, p->dw_dec, p->b.decoder_m, p->b.decoder_v, nullptr, rows, d.d, 1,
-                                     d.norm_floor, h, st);
-    if (rc) return rc;
-    launches += 2;
-  } else {
-    rc = launch_dict_rows<MODE_ADAM>(p, 0, p->b.encoder, p->dw_enc, p->b.encoder_m, p->b.encoder_v, nullptr, rows, d.d, 1,
-                                     d.norm_floor, h, st);
-    if (rc) return rc;
-    ++launches;
-  }
+  DictSide sides[2];
+  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s, ++launches)
+    if ((rc = launch_dict_rows<MODE_ADAM>(p, sides[s], nullptr, h, st))) return rc;
   rc = transpose_dict(p, st, launches);
   if (rc) return rc;
   if (p->b.encoder_bias) {
@@ -1630,23 +1551,11 @@ int sce_grads(sce_plan* p, const float* x, int B, float* d_encoder, float* d_bia
   int rc = run_pipeline(p, x, B, nullptr, true, out_losses, out_nnz, st);
   if (rc) return rc;
   const sce_desc& d = p->d;
-  const long long rows = (long long)d.n_models * d.n;
   const AdamHyper h = hyper_for(p, 1);
-  if (d.variant == SCE_UNTIED) {
-    if (d_encoder) {
-      rc = launch_dict_rows<MODE_GRAD>(p, 0, p->b.encoder, p->dw_enc, nullptr, nullptr, d_encoder, rows, d.d, 0, 0.f, h, st);
-      if (rc) return rc;
-    }
-    if (d_decoder) {
-      rc = launch_dict_rows<MODE_GRAD>(p, 1, p->b.decoder, p->dw_dec, nullptr, nullptr, d_decoder, rows, d.d, 1, d.norm_floor,
-                                       h, st);
-      if (rc) return rc;
-    }
-  } else if (d_encoder) {
-    rc = launch_dict_rows<MODE_GRAD>(p, 0, p->b.encoder, p->dw_enc, nullptr, nullptr, d_encoder, rows, d.d, 1, d.norm_floor, h,
-                                     st);
-    if (rc) return rc;
-  }
+  DictSide sides[2];
+  float* const grad_out[2] = {d_encoder, d_decoder};
+  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
+    if (grad_out[s] && (rc = launch_dict_rows<MODE_GRAD>(p, sides[s], grad_out[s], h, st))) return rc;
   if (p->b.encoder_bias && d_bias) {
     const long long tot = (long long)d.n_models * d.n;
     const int n_part = ((B + kBM - 1) / kBM) * 4;
@@ -1685,16 +1594,16 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
   if (p->code_batch_major) {
     const long long total = (long long)p->d.n_models * per;
     join_code_batch_major_kernel<<<(unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096), 256, 0, st>>>(
-        reinterpret_cast<const __half*>(p->c_hi), p->ct_x8, out_code, B, p->d.n, p->d.batch_max, p->bpad, total);
+        static_cast<const __half*>(p->c.hi), p->ct.x8, out_code, B, p->d.n, p->d.batch_max, p->bpad, total);
     CUDA_TRY(cudaGetLastError());
     return SCE_OK;
   }
   for (int m = 0; m < p->d.n_models; ++m) {
-    const long long src = (long long)m * p->d.batch_max * p->d.n;
+    const Planes c = p->c.at((size_t)m * p->d.batch_max * p->d.n);
     if (p->arith == kArithF16F8)
-      join_code_kernel<kArithF16F8><<<1024, 256, 0, st>>>(p->c_hi + src, nullptr, p->c_x8 + src, out_code + (long long)m * per, per / 2);
+      join_code_kernel<kArithF16F8><<<1024, 256, 0, st>>>(c.hi, nullptr, c.x8, out_code + (long long)m * per, per / 2);
     else
-      join_code_kernel<kArithBf16x3><<<1024, 256, 0, st>>>(p->c_hi + src, p->c_lo + src, nullptr, out_code + (long long)m * per, per / 2);
+      join_code_kernel<kArithBf16x3><<<1024, 256, 0, st>>>(c.hi, c.lo, nullptr, out_code + (long long)m * per, per / 2);
   }
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
@@ -1829,7 +1738,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   uint8_t* active = ws + off_active;
   int* open = reinterpret_cast<int*>(ws + off_open);
   const int n_chunks = (d.n + 31) / 32, G = B / L;
-  const FragCode c{p->c_hi, p->c_lo, p->c_x8, p->scores, p->act_pos, n_chunks, d.batch_max, d.n};
+  const FragCode c{p->c.hi, p->c.lo, p->c.x8, p->scores, p->act_pos, n_chunks, d.batch_max, d.n};
   if (d.variant == SCE_TOPK)
     launch_fragments<kArithBf16x3, true>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
                                          top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
@@ -1951,8 +1860,8 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
     sim_carve(static_cast<uint8_t*>(workspace), true, ma, na, b_is_a ? 0 : mb, b_is_a ? 0 : nb, d, n_pairs, capacity != nullptr, &w);
     CUDA_TRY(cudaMemsetAsync(w.flags, 0, kFlagWords * sizeof(uint32_t), st));
     int rc = SCE_OK;
-    if (!A.normalize) rc = sim_planes<kArithF16F8>(A, d, w.a_hi, w.a_lo, w.a_x8, w.flags, st);
-    if (!rc && !b_is_a && !B.normalize) rc = sim_planes<kArithF16F8>(B, d, w.b_hi, w.b_lo, w.b_x8, w.flags, st);
+    if (!A.normalize) rc = sim_planes<kArithF16F8>(A, d, w.a, w.flags, st);
+    if (!rc && !b_is_a && !B.normalize) rc = sim_planes<kArithF16F8>(B, d, w.b, w.flags, st);
     if (rc) return rc;
     uint32_t bad = 0;
     CUDA_TRY(cudaMemcpyAsync(&bad, w.flags + kBadWord, sizeof(bad), cudaMemcpyDeviceToHost, st));

@@ -11,7 +11,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# SCE_LIB: an alternative build of the same library (kernel A/B experiments, tools/ab_variants.sh)
+# SCE_LIB: an alternative build of the same library (kernel A/B experiments)
 LIB_PATH = os.environ.get("SCE_LIB") or os.path.join(_HERE, "libsce.so")
 
 SCE_TIED, SCE_UNTIED, SCE_TOPK = 0, 1, 2

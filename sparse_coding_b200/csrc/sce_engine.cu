@@ -115,27 +115,30 @@ struct PlanBuffers {
   float *part_enc, *part_dec, *db_part, *bnorm, *l1_over_b, *loss_stage, *nnz_stage;
 };
 
+// What a plan decides from its descriptor, once (plan_config): the workspace carve and every launch follow from it
+struct PlanConfig {
+  int arith;           // kArithBf16x3 or kArithF16F8
+  int xm;              // number of distinct input batches (1 shared, or M)
+  int bpad;            // Bp: batch_max rounded up to 16 (TMA pitch of the batch-major 8-bit planes)
+  int tk_kmax;         // top-k list capacity per row (desc.topk_k_max rounded up to 8; 0: no lists)
+  int tk_slices;       // slices of the activation width topk_sparse_kernel runs per row (0: none fits)
+  bool topk_sparse;    // decode / dcode of the top-k variant run as the k-sparse gather kernels
+  bool dw_native;      // the weight gradient's cross terms run on E5M2 wgmma from batch-major copies (carve)
+  bool split_decode;   // separate accumulators for hi*hi and the cross terms in the decode GEMM (bf16x3)
+  bool use_graph;      // replay the step as a CUDA graph
+};
+
 struct sce_plan : PlanBuffers {
   sce_desc d;
   sce_buffers b;
+  PlanConfig cfg;
   int sms;
   int device;  // CUDA device the plan was created on (the caller keeps it current for every call)
-  int xm;  // number of distinct input batches (1 shared, or M)
-  int arith;                       // kArithBf16x3 or kArithF16F8 (resolved from desc.arith / env SCE_ARITH / the shape)
-  int bpad;                        // Bp
   int code_batch_major;            // 1: the last call was a dw_native backward, which left the code's residual plane
                                    // only in its batch-major copy (ct.x8): dcode overwrote the row-major one (carve)
-  int dw_native;                   // 1: the weight gradient's cross terms run on E5M2 wgmma (see native_dw_layout)
   int tk_groups, tk_group_off[5], tk_group_krows[4];   // classes: models [off[g], off[g+1]) need at most krows[g] rows
-  int topk_cmax;                  // 1: the selection works from the chunk maxima (SCE_TOPK_CMAX=0 turns it off)
-  int tk_slices;                  // slices of the activation width topk_sparse_kernel runs per row
-  int tk_kmax;                    // list capacity per row (desc.topk_k_max rounded up to 8; 0: no lists)
-  int topk_sparse;                // 1: decode / dcode of the top-k variant run as the k-sparse gather kernels
   std::map<int, BatchMaps*>* maps;
   cudaStream_t cap_stream;  // private stream the step is captured on
-  int dcode_passes, dw_passes;  // tensor passes of the two backward GEMMs (default: desc.bwd_passes)
-  int use_graph;     // 1: replay the step as a CUDA graph (launch-bound shapes; env SCE_GRAPH overrides)
-  int split_decode;  // 1: separate accumulators for hi*hi and the cross terms in the decode GEMM
   int last_launches;
   long long step;  // number of optimiser steps taken
   // optional per-phase device timing (sce_profile_*): events bracket each phase of a step
@@ -228,25 +231,21 @@ static void launch_split_rows(const float* x, const Planes& w, long long n4, uin
   split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags);
 }
 
-// desc.arith -> kArithBf16x3 / kArithF16F8. AUTO: f16f8 where the 8-bit planes can be addressed by TMA
-// (row pitches of 16 bytes), bf16x3 otherwise; the environment may pin AUTO to one of them (A/B runs).
-static int resolve_arith(const sce_desc& d) {
-  if (d.arith == SCE_ARITH_BF16X3) return kArithBf16x3;
-  if (d.arith == SCE_ARITH_F16F8) return kArithF16F8;
-  const bool shape_ok = d.d % 16 == 0 && d.n % 16 == 0;
-  if (const char* v = getenv("SCE_ARITH")) {
-    if (!strcmp(v, "bf16x3")) return kArithBf16x3;
-    if (!strcmp(v, "f16f8") && shape_ok) return kArithF16F8;
-  }
-  return shape_ok ? kArithF16F8 : kArithBf16x3;
+// SCE_ARITH=bf16x3|f16f8: the arithmetic the environment pins arith = AUTO to (include/sce.h), else SCE_ARITH_AUTO
+static int env_arith() {
+  const char* v = getenv("SCE_ARITH");
+  if (v && !strcmp(v, "bf16x3")) return SCE_ARITH_BF16X3;
+  if (v && !strcmp(v, "f16f8")) return SCE_ARITH_F16F8;
+  return SCE_ARITH_AUTO;
 }
 
-// capacity per row of the top-k lists: the largest k of the ensemble (desc.topk_k_max, supplied by the host mirror, which
-// knows buffers["sparsity"]) rounded up to 8; 0 = unknown or too large for the gather kernel -> dense path, no lists
-static size_t topk_kmax(const sce_desc& d) {
-  if (d.variant != SCE_TOPK || d.topk_k_max < 1 || d.topk_k_max > 256) return 0;
-  return (size_t)(d.topk_k_max + 7) / 8 * 8;
+// desc.arith -> kArithBf16x3 / kArithF16F8. AUTO (unless pinned to bf16x3): f16f8 where the 8-bit planes can be
+// addressed by TMA (row pitches of 16 bytes), bf16x3 otherwise; validate holds an explicit F16F8 to such shapes.
+static int resolve_arith(const sce_desc& d) {
+  if ((d.arith == SCE_ARITH_AUTO ? env_arith() : d.arith) == SCE_ARITH_BF16X3) return kArithBf16x3;
+  return d.d % 16 == 0 && d.n % 16 == 0 ? kArithF16F8 : kArithBf16x3;
 }
+
 // topk_sparse_kernel: dynamic shared memory for `slices` slices of the activation width (see there), and the slice
 // count a plan uses: the smallest of 2, 4, 8 whose slice fits (two blocks per SM); 0 when none does (the plan then runs
 // the dense GEMMs)
@@ -258,43 +257,61 @@ static size_t topk_sparse_smem(const sce_desc& d, size_t krows, int slices) {
 static int topk_slices(const sce_desc& d, size_t kmax) {
   int best = 0;
   for (int s = 2; s <= kTopkMaxSlices; s *= 2) {
-    if (d.d % (4 * s) || d.d / s > 512) continue;
+    if (d.d % (4 * s) || d.d / s > 512) continue;   // (16-byte aligned slices for the bulk copies)
     const size_t b = topk_sparse_smem(d, kmax, s);
     if (b <= 112 * 1024) return s;   // fewest slices that fit: the kernel's time goes with the number of blocks
   }
   return best;
 }
 
-// ~30 M B n d tensor FLOPs are issued per step; below ~3e11 (a fifth of a millisecond) launches dominate
-static bool launch_bound(const sce_desc& d) {
-  return 30.0 * d.n_models * (double)d.batch_max * d.n * d.d < 3e11;
+// The configuration of a plan for a validated descriptor
+static PlanConfig plan_config(const sce_desc& d) {
+  PlanConfig c{};
+  c.arith = resolve_arith(d);
+  c.xm = d.x_per_model ? d.n_models : 1;
+  c.bpad = (d.batch_max + 15) / 16 * 16;
+  // top-k lists hold the largest k of the ensemble (desc.topk_k_max, supplied by the host mirror, which knows
+  // buffers["sparsity"]) rounded up to 8; none when it is unknown or too large for the gather kernel (dense path)
+  if (d.variant == SCE_TOPK && d.topk_k_max >= 1 && d.topk_k_max <= 256) {
+    c.tk_kmax = (d.topk_k_max + 7) / 8 * 8;
+    c.tk_slices = topk_slices(d, c.tk_kmax);
+    // Worth it where the dictionary is large against k: the dense decode + dcode GEMMs cost ~ n per row, the gather
+    // kernel ~ k (it is bound by the latency chain of a block, not by bytes): the gather path is used where n >= 96 k.
+    c.topk_sparse = c.tk_slices > 0 && d.n >= 96 * c.tk_kmax;
+  }
+  // ~30 M B n d tensor FLOPs are issued per step; below ~3e11 (a fifth of a millisecond) launches dominate, and the
+  // step is replayed as a CUDA graph (sce_step)
+  const bool launch_bound = 30.0 * d.n_models * (double)d.batch_max * d.n * d.d < 3e11;
+  c.use_graph = launch_bound;
+  // Dense f16f8 plans with split backward GEMMs keep batch-major copies of the 8-bit planes of x, c, g and dz, from
+  // which the weight gradient forms its cross terms on E5M2 wgmma. Top-k plans do not: their code and (k-sparse)
+  // code-gradient planes are written by the selection / scatter kernels, row-major only, so their weight gradient widens
+  // the 8-bit tiles. Nor do launch-bound plans: there the weight gradient takes microseconds either way, and the copies
+  // would add three launches per step and a third to the workspace.
+  c.dw_native = c.arith == kArithF16F8 && d.variant != SCE_TOPK && d.bwd_passes >= 3 && !launch_bound;
+  // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
+  // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
+  // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
+  c.split_decode = d.n > 4096;
+  return c;
 }
-// Dense f16f8 plans with split backward GEMMs keep batch-major copies of the 8-bit planes of x, c, g and dz, from which the
-// weight gradient forms its cross terms on E5M2 wgmma. Top-k plans do not: their code and (k-sparse) code-gradient planes
-// are written by the selection / scatter kernels, row-major only, so their weight gradient widens the 8-bit tiles. Nor do
-// launch-bound plans: there the weight gradient takes microseconds either way, and the copies would add three launches
-// per step and a third to the workspace.
-static bool native_dw_layout(const sce_desc& d) {
-  return resolve_arith(d) == kArithF16F8 && d.variant != SCE_TOPK && d.bwd_passes >= 3 && !launch_bound(d);
-}
-static size_t batch_pad(const sce_desc& d) { return ((size_t)d.batch_max + 15) / 16 * 16; }
 
 // Carves the workspace into `w` (buffers the plan does not use stay null); with base == nullptr only measures it.
-static size_t carve(PlanBuffers& w, const sce_desc& d, uint8_t* base) {
+static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, uint8_t* base) {
   Carve c{base, 0};
   const size_t M = d.n_models, B = d.batch_max, n = d.n, dd = d.d;
-  const size_t xm = d.x_per_model ? M : 1;
+  const size_t xm = cfg.xm;
   const size_t tiles_mB = (B + kBM - 1) / kBM;
   const size_t tiles_nN = (n + kBN - 1) / kBN;
   const size_t tiles_nD = (dd + kBN - 1) / kBN;
-  const bool f8 = resolve_arith(d) == kArithF16F8;
+  const bool f8 = cfg.arith == kArithF16F8;
   w.x_stage = c.take<float>(xm * B * dd);
   w.x = c.planes(xm * B * dd, f8);
   w.wenc = c.planes(M * n * dd, f8);
   w.wdec = d.variant == SCE_UNTIED ? c.planes(M * n * dd, f8) : w.wenc;
   if (f8) w.wdt = c.planes(M * n * dd, f8);
-  const bool tdw = native_dw_layout(d);
-  const size_t Bp = batch_pad(d);
+  const bool tdw = cfg.dw_native;
+  const size_t Bp = cfg.bpad;
   const size_t dz8 = tdw ? M * n * Bp : M * B * n;   // bytes of one 8-bit plane of dz
   if (!tdw) {
     w.c = c.planes(M * B * n, f8);
@@ -334,7 +351,7 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, uint8_t* base) {
   w.act_zero = c.take<uint32_t>(M * n_chunks * B);
   // top-k: scores of their own (the code-gradient planes must keep their scattered zeros) and the k-sparse lists
   if (d.variant == SCE_TOPK) {
-    const size_t kmax = topk_kmax(d);
+    const size_t kmax = cfg.tk_kmax;
     w.scores = c.take<float>(M * B * n);
     w.tk_cmax = c.take<uint32_t>(M * B * n_chunks);
     if (kmax) {
@@ -357,10 +374,6 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, uint8_t* base) {
 // ------------------------------------------------------------------------------------------------
 // tensor maps for one batch size
 // ------------------------------------------------------------------------------------------------
-static int tune_flag(const char* env, int dflt) {
-  const char* v = getenv(env);
-  return v ? (atoi(v) != 0) : dflt;
-}
 // K-major 16-bit tiles [rows][bk], bk = gemm_bk(arith): the swizzle span is one tile row of 2 bk bytes
 static CUtensorMapSwizzle swizzle_for_bk(int bk) {
   return bk * 2 == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
@@ -401,11 +414,12 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   if (!m) return fail(SCE_ERR_INVALID, "out of host memory");
   memset(m, 0, sizeof(*m));
   const sce_desc& d = p->d;
-  const uint64_t M = d.n_models, n = d.n, dd = d.d, xm = p->xm, Bm = d.batch_max;
+  const PlanConfig& cfg = p->cfg;
+  const uint64_t M = d.n_models, n = d.n, dd = d.d, xm = cfg.xm, Bm = d.batch_max;
   // NOTE: activations are laid out with the plan's batch_max pitch between models; only `B` rows are
   // visible through the map, so rows >= B read as zero (TMA out-of-bounds fill).
-  const bool f8 = p->arith == kArithF16F8;
-  const int bk = gemm_bk(p->arith);
+  const bool f8 = cfg.arith == kArithF16F8;
+  const int bk = gemm_bk(cfg.arith);
   // activations [models][B of batch_max][cols] as the A operand: K-major tiles [128 rows][bk]
   auto act_a = [&](OperandMaps& o, const Planes& P, uint64_t models, uint64_t cols) {
     return operand_maps(o, P, models, (uint64_t)B, cols, Bm * cols, kBM, bk);
@@ -432,9 +446,9 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   // weight gradients: everything MN-major, tiles of bk batch rows, reduction over the batch rows. dw_native: the 8-bit
   // planes come from the batch-major copies T [models][cols][Bp] instead, K-major tiles [128 rows][64 B] with the 64-byte
   // swizzle; only B columns are exposed, so the tail of a short batch reads as zero
-  const uint64_t Bp = (uint64_t)p->bpad;
+  const uint64_t Bp = (uint64_t)cfg.bpad;
   auto dw_operand = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t models, uint64_t cols) {
-    if (!p->dw_native) return operand_maps(o, P, models, (uint64_t)B, cols, Bm * cols, bk, 0);
+    if (!cfg.dw_native) return operand_maps(o, P, models, (uint64_t)B, cols, Bm * cols, bk, 0);
     return make_tmap_bf16(&o.hi, P.hi, models, (uint64_t)B, cols, cols, Bm * cols, bk) &&
            make_tmap_u8_box(&o.lo, T.lo, models, cols, (uint64_t)B, Bp, cols * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
            make_tmap_u8_box(&o.x8, T.x8, models, cols, (uint64_t)B, Bp, cols * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
@@ -456,8 +470,8 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
       return make_tmap_u8_box(t, base, M, n, (uint64_t)B, Bp, n * Bp, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE);
     };
     ok &= st8(&m->st_c.lo, p->c.lo) && st8(&m->st_c.x8, p->c.x8);
-    ok &= p->dw_native ? st8t(&m->st_dz.lo, p->dz.lo) && st8t(&m->st_dz.x8, p->dz.x8)
-                       : st8(&m->st_dz.lo, p->dz.lo) && st8(&m->st_dz.x8, p->dz.x8);
+    ok &= cfg.dw_native ? st8t(&m->st_dz.lo, p->dz.lo) && st8t(&m->st_dz.x8, p->dz.x8)
+                        : st8(&m->st_dz.lo, p->dz.lo) && st8(&m->st_dz.x8, p->dz.x8);
   } else {
     ok &= make_tmap_bf16_store32(&m->st_c.lo, p->c.lo, M, (uint64_t)B, n, Bm * n);
     ok &= make_tmap_bf16_store32(&m->st_dz.lo, p->dz.lo, M, (uint64_t)B, n, Bm * n);
@@ -584,8 +598,8 @@ static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_ou
   float* m = MODE == MODE_ADAM ? s.m : nullptr;
   float* v = MODE == MODE_ADAM ? s.v : nullptr;
   const Planes w = MODE == MODE_GRAD ? Planes{} : s.planes;
-  float* wf = (MODE != MODE_GRAD && p->topk_sparse) ? p->wn_f32 : nullptr;   // (top-k plans have one dictionary)
-  return p->arith == kArithF16F8
+  float* wf = (MODE != MODE_GRAD && p->cfg.topk_sparse) ? p->wn_f32 : nullptr;   // (top-k plans have one dictionary)
+  return p->cfg.arith == kArithF16F8
              ? launch_dict_rows_t<MODE, kArithF16F8>(s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st)
              : launch_dict_rows_t<MODE, kArithBf16x3>(s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
 }
@@ -593,7 +607,7 @@ static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_ou
 // f16f8: the decoder's planes -> their transposed copy, which the decode GEMM reads K-major (nothing to do where the
 // decode runs without the GEMM: k-sparse top-k plans). Adds its launches to `launches`.
 static int transpose_dict(const sce_plan* p, cudaStream_t st, int& launches) {
-  if (p->arith != kArithF16F8 || p->topk_sparse) return SCE_OK;
+  if (p->cfg.arith != kArithF16F8 || p->cfg.topk_sparse) return SCE_OK;
   const sce_desc& d = p->d;
   const dim3 grid((d.d + 63) / 64, (d.n + 63) / 64, d.n_models);
   transpose_kernel<uint16_t><<<grid, 256, 0, st>>>(static_cast<const uint16_t*>(p->wdec.hi),
@@ -609,7 +623,7 @@ static int transpose_dict(const sce_plan* p, cudaStream_t st, int& launches) {
 // f16f8 runs the backward pass on the residual r instead of g = 2r/(B d) (EpiDecodeT): weight- and bias-gradient
 // outputs are multiplied by 2/(B d) on the way out, the sparsity term enters dcode as alpha d / 2.
 static float grad_out_scale(const sce_plan* p, int B) {
-  return p->arith == kArithF16F8 ? 2.0f / ((float)B * (float)p->d.d) : 1.0f;
+  return p->cfg.arith == kArithF16F8 ? 2.0f / ((float)B * (float)p->d.d) : 1.0f;
 }
 
 __global__ void l1_over_b_kernel(const float* __restrict__ alpha, float* __restrict__ out, int M, float invB) {
@@ -632,6 +646,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   using EpiDco = EpiDcodeT<AR>;
   constexpr bool f8 = AR == kArithF16F8;
   const sce_desc& d = p->d;
+  const PlanConfig& cfg = p->cfg;
   if (int rc = check_rows(p, B, "")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
   BatchMaps* maps = nullptr;
@@ -665,21 +680,21 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   }
   // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace
   if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), st));
-  for (int m = 0; m < p->xm; ++m) {
+  for (int m = 0; m < cfg.xm; ++m) {
     launch_split_rows<AR>(x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st);
     ++launches;
   }
   CUDA_TRY(cudaGetLastError());
   // dw_native: batch-major copies of the 8-bit planes of x, c and g for the weight gradient (dz's are written so by dcode)
-  const bool tdw = f8 && backward && p->dw_native;
+  const bool tdw = f8 && backward && cfg.dw_native;
   auto batch_major = [&](const Planes& P, const Planes& T, int models, int cols) {
     const BatchPlanes t{{static_cast<const uint8_t*>(P.lo), P.x8}, {static_cast<uint8_t*>(T.lo), T.x8}};
     transpose_batch_u8_kernel<<<dim3((cols + 127) / 128, (B + 127) / 128, 2 * models), 256, 0, st>>>(t, models, B, cols,
-                                                                                                 Bm * cols, p->bpad);
+                                                                                                 Bm * cols, cfg.bpad);
     ++launches;
     return cudaGetLastError();
   };
-  if (tdw) CUDA_TRY(batch_major(p->x, p->xt, p->xm, dd));
+  if (tdw) CUDA_TRY(batch_major(p->x, p->xt, cfg.xm, dd));
   p->code_batch_major = tdw ? 1 : 0;
   // alpha / B, or (f16f8, backward on r = g B d / 2) alpha d / 2
   l1_over_b_kernel<<<(M + 127) / 128, 128, 0, st>>>(p->b.l1_alpha, p->l1_over_b, M, f8 ? 0.5f * (float)dd : 1.0f / (float)B);
@@ -730,14 +745,13 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     n_enc_parts = tiles_mB * 8 * ((n + kBN - 1) / kBN);
     if (tdw) CUDA_TRY(batch_major(p->c, p->ct, M, n));
   } else {
-    // scores -> fp32, then per-row selection (code planes, activity mask, k-sparse lists)
+    // scores -> fp32 and the chunk maxima of every row, then per-row selection (code planes, activity mask, k-sparse
+    // lists) from the chunk maxima (the kernel reads whole rows where they cannot bound the k-th largest score)
     EpiScoresTma::Params sp;
     sp.out = maps->st_scores;
-    if (p->topk_cmax) {
-      sp.cmax = p->tk_cmax;
-      sp.n_chunks = act.n_chunks;
-      sp.cmax_model_stride = (long long)Bm * act.n_chunks;
-    }
+    sp.cmax = p->tk_cmax;
+    sp.n_chunks = act.n_chunks;
+    sp.cmax_model_stride = (long long)Bm * act.n_chunks;
     rc = launch_gemm_t<EpiScoresTma, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, sp, st, x_is_a);
     if (rc) return rc;
     ++launches;
@@ -745,18 +759,18 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     tk.col = p->tk_col;
     tk.val = p->tk_val;
     tk.cnt = p->tk_cnt;
-    tk.kmax = p->tk_kmax;
+    tk.kmax = cfg.tk_kmax;
     tk.batch_max = d.batch_max;
     // one block per (row, model); scores / codes of model m start at m * batch_max * n
     topk_select2_kernel<AR><<<dim3(B, M), 256, 0, st>>>(
-        p->scores, p->b.sparsity, p->c.hi, p->c.lo, p->c.x8, p->topk_sparse ? p->dz.hi : nullptr, p->dz.lo, p->dz.x8,
-        act, tk, p->part_enc, B, n, Bm * n, p->topk_cmax ? p->tk_cmax : nullptr);
+        p->scores, p->b.sparsity, p->c.hi, p->c.lo, p->c.x8, cfg.topk_sparse ? p->dz.hi : nullptr, p->dz.lo, p->dz.x8,
+        act, tk, p->part_enc, B, n, Bm * n, p->tk_cmax);
     ++launches;
     CUDA_TRY(cudaGetLastError());
     n_enc_parts = B;
   }
 
-  const bool sparse = d.variant == SCE_TOPK && p->topk_sparse;
+  const bool sparse = cfg.topk_sparse;
   int n_dec_parts;
   prof_mark(p, SCE_PHASE_DECODE, st);
   if (sparse) {
@@ -767,13 +781,13 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     for (int g = 0; g < p->tk_groups; ++g) {
       const int cnt = p->tk_group_off[g + 1] - p->tk_group_off[g];
       if (cnt == 0) continue;
-      topk_sparse_kernel<AR><<<dim3(B, cnt, p->tk_slices), 256, topk_sparse_smem(d, p->tk_group_krows[g], p->tk_slices), st>>>(
+      topk_sparse_kernel<AR><<<dim3(B, cnt, cfg.tk_slices), 256, topk_sparse_smem(d, p->tk_group_krows[g], cfg.tk_slices), st>>>(
           tk, p->b.sparsity, p->wn_f32, x, d.x_per_model ? (long long)B * dd : 0, p->g.hi, p->g.lo, p->g.x8, x_hat, p->part_dec,
           backward ? p->tk_dots : nullptr, B, n, dd, gscale, p->tk_models + p->tk_group_off[g], p->tk_group_krows[g]);
       ++launches;
     }
     CUDA_TRY(cudaGetLastError());
-    n_dec_parts = p->tk_slices * B;
+    n_dec_parts = cfg.tk_slices * B;
   } else {
     // ---- decode (+ residual, loss partial, g)
     typename EpiDec::Params dp;
@@ -792,7 +806,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     dp.tiles_n = (dd + kBN - 1) / kBN;
     if constexpr (f8)
       rc = launch_gemm_t<EpiDec, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-    else if (p->split_decode)
+    else if (cfg.split_decode)
       rc = launch_gemm_t<EpiDec, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
     else
       rc = launch_gemm_t<EpiDec, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
@@ -818,7 +832,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   if (backward) {
     if (sparse) {
       // ---- code gradient planes: zero the rows, scatter the k entries
-      topk_dz_scatter_kernel<AR><<<dim3(B, M), 64, 0, st>>>(tk, p->tk_dots, p->tk_slices, p->dz.hi, p->dz.lo, p->dz.x8, n);
+      topk_dz_scatter_kernel<AR><<<dim3(B, M), 64, 0, st>>>(tk, p->tk_dots, cfg.tk_slices, p->dz.hi, p->dz.lo, p->dz.x8, n);
       ++launches;
       CUDA_TRY(cudaGetLastError());
     } else {
@@ -833,14 +847,14 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
         zp.l1_over_b = p->l1_over_b;
         zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
         zp.tiles_m = tiles_mB;
-        zp.planes = p->dw_passes >= 3 ? 3 : 0;
+        zp.planes = d.bwd_passes >= 3 ? 3 : 0;
         // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
         // (per-model batches carry one flag for all of them, so the same test holds)
         zp.x_res_flag = f8 ? p->res_flags : nullptr;
-        return launch_gemm_t<E, false, false, false, AR>(p, maps->dcode, 1, one, one, dd, p->dcode_passes, B, n, zp, st);
+        return launch_gemm_t<E, false, false, false, AR>(p, maps->dcode, 1, one, one, dd, d.bwd_passes, B, n, zp, st);
       };
       // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
-      if constexpr (f8) rc = p->dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
+      if constexpr (f8) rc = cfg.dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
       else rc = dcode(TypeTag<EpiDco>{});
       if (rc) return rc;
       ++launches;
@@ -857,9 +871,9 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one). dw_native: fp16 planes
       // MN-major, 8-bit planes K-major from their batch-major copies, cross terms on E5M2 wgmma; else widened
       if constexpr (f8)
-        if (p->dw_native)
-          return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
-      return launch_gemm_t<EpiStoreF32, true, true, !f8, AR>(p, gm, nsets, ab, bb, B, p->dw_passes, n, dd, sp, st, rf);
+        if (cfg.dw_native)
+          return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(p, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, st, rf);
+      return launch_gemm_t<EpiStoreF32, true, true, !f8, AR>(p, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, st, rf);
     };
     if (d.variant == SCE_UNTIED) {
       rc = dw(maps->dw_enc, 1, one, xb, p->dw_enc, x_is_b);
@@ -881,8 +895,9 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
 
 static int run_pipeline(sce_plan* p, const float* x, int B, float* x_hat, bool backward, float* out_losses,
                         float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
-  return p->arith == kArithF16F8 ? run_pipeline_t<kArithF16F8>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part)
-                                 : run_pipeline_t<kArithBf16x3>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
+  return p->cfg.arith == kArithF16F8
+             ? run_pipeline_t<kArithF16F8>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part)
+             : run_pipeline_t<kArithBf16x3>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1294,14 +1309,14 @@ extern "C" {
 int sce_version(void) { return SCE_VERSION; }
 const char* sce_last_error(void) { return g_err; }
 
-static size_t plan_workspace(const sce_desc& d) {
+static size_t plan_workspace(const sce_desc& d, const PlanConfig& cfg) {
   PlanBuffers w{};
-  return carve(w, d, nullptr);
+  return carve(w, d, cfg, nullptr);
 }
 
 size_t sce_workspace_bytes(const sce_desc* desc) {
   if (validate(desc)) return 0;
-  return plan_workspace(*desc);
+  return plan_workspace(*desc, plan_config(*desc));
 }
 
 int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan** out_plan) {
@@ -1317,7 +1332,8 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   if (desc->variant != SCE_TOPK && (!b.encoder_bias || !b.bias_m || !b.bias_v))
     return fail(SCE_ERR_INVALID, "encoder_bias / bias_m / bias_v are required for SAE variants");
   if (desc->variant == SCE_TOPK && !b.sparsity) return fail(SCE_ERR_INVALID, "top-k variant needs the sparsity buffer");
-  rc = check_workspace(b.workspace, b.workspace_bytes, plan_workspace(*desc), "");
+  const PlanConfig cfg = plan_config(*desc);
+  rc = check_workspace(b.workspace, b.workspace_bytes, plan_workspace(*desc, cfg), "");
   if (rc) return rc;
   int dev = 0, sms = 0;
   rc = query_device(&dev, &sms);
@@ -1327,43 +1343,11 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   memset(p, 0, sizeof(*p));
   p->d = *desc;
   p->b = b;
+  p->cfg = cfg;
   p->sms = sms;
   p->device = dev;
-  p->xm = desc->x_per_model ? desc->n_models : 1;
-  p->arith = resolve_arith(*desc);
-  p->bpad = (int)batch_pad(*desc);
-  p->tk_kmax = (int)topk_kmax(*desc);
-  // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
-  // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
-  // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
-  p->split_decode = tune_flag("SCE_TUNE_SPLIT_DECODE", desc->n > 4096 ? 1 : 0);
-  p->dcode_passes = desc->bwd_passes;
-  p->dw_passes = desc->bwd_passes;
-  if (const char* v = getenv("SCE_TUNE_DCODE_PASSES")) p->dcode_passes = atoi(v) == 1 ? 1 : 3;
-  if (const char* v = getenv("SCE_TUNE_DW_PASSES")) p->dw_passes = atoi(v) == 1 ? 1 : 3;
-  p->dw_native = native_dw_layout(*desc) && p->dw_passes >= 3;
-  p->use_graph = tune_flag("SCE_GRAPH", launch_bound(*desc) ? 1 : 0);
-  {
-    // k-sparse decode / dcode of the top-k variant: lists known (topk_k_max), bulk-copy alignment of the dictionary
-    // half rows (16 bytes in every plane), shared memory of the gather kernel
-    const size_t kmax = p->tk_kmax;
-    p->tk_slices = kmax ? topk_slices(*desc, kmax) : 0;
-    if (const char* v = getenv("SCE_TOPK_SLICES")) {
-      const int sl = atoi(v);
-      if (kmax && (sl == 2 || sl == 4 || sl == 8) && desc->d % (4 * sl) == 0 && desc->d / sl <= 512 &&
-          topk_sparse_smem(*desc, kmax, sl) <= 112 * 1024)
-        p->tk_slices = sl;
-    }
-    // Worth it where the dictionary is large against k: the dense decode + dcode GEMMs cost ~ n per row, the gather
-    // kernel ~ k (it is bound by the latency chain of a block, not by bytes): the gather path is used where n >= 96 k.
-    // SCE_TOPK_SPARSE = 1 / 0 forces it on / off.
-    const int heuristic = (long long)desc->n >= 96ll * (long long)(kmax ? kmax : 1);
-    p->topk_sparse = desc->variant == SCE_TOPK && kmax > 0 && p->tk_slices > 0 && tune_flag("SCE_TOPK_SPARSE", heuristic);
-    // selection from the per-chunk maxima the scores epilogue writes; 0 = read every row twice
-    p->topk_cmax = desc->variant == SCE_TOPK && tune_flag("SCE_TOPK_CMAX", 1);
-  }
   p->maps = new std::map<int, BatchMaps*>();
-  carve(*p, *desc, static_cast<uint8_t*>(b.workspace));
+  carve(*p, *desc, cfg, static_cast<uint8_t*>(b.workspace));
   *out_plan = p;
   return SCE_OK;
 }
@@ -1389,7 +1373,8 @@ int sce_prepare(sce_plan* p, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, kFlagWords * sizeof(uint32_t), st));   // residual flag, input range monitor, health
   const sce_desc& d = p->d;
-  if (d.variant == SCE_TOPK && p->tk_kmax) {
+  const int kmax = p->cfg.tk_kmax;   // (top-k plans only)
+  if (kmax) {
     // the top-k selection keeps the code planes (and, in k-sparse plans, the code-gradient planes) all-zero except for
     // the entries its lists record: start them zeroed, with empty lists
     const size_t el = (size_t)d.n_models * d.batch_max * d.n;
@@ -1401,22 +1386,22 @@ int sce_prepare(sce_plan* p, void* stream) {
     std::vector<long long> ks(d.n_models);
     CUDA_TRY(cudaMemcpyAsync(ks.data(), p->b.sparsity, ks.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    const int caps[4] = {16, 32, 64, p->tk_kmax};
+    const int caps[4] = {16, 32, 64, kmax};
     std::vector<int> order;
     p->tk_groups = 0;
     p->tk_group_off[0] = 0;
     int lo = 0;
     for (int g = 0; g < 4; ++g) {
-      const int cap = caps[g] < p->tk_kmax ? caps[g] : p->tk_kmax;
+      const int cap = caps[g] < kmax ? caps[g] : kmax;
       if (g > 0 && cap <= lo) continue;
       for (int m = 0; m < d.n_models; ++m) {
-        const long long k = ks[m] < 1 ? 1 : (ks[m] > p->tk_kmax ? (long long)p->tk_kmax : ks[m]);   // (kernels clip k the same way)
+        const long long k = ks[m] < 1 ? 1 : (ks[m] > kmax ? (long long)kmax : ks[m]);   // (kernels clip k the same way)
         if (k > lo && k <= cap) order.push_back(m);
       }
       p->tk_group_krows[p->tk_groups] = cap;
       p->tk_group_off[++p->tk_groups] = (int)order.size();
       lo = cap;
-      if (cap == p->tk_kmax) break;
+      if (cap == kmax) break;
     }
     if ((int)order.size() != d.n_models) return fail(SCE_ERR_INVALID, "top-k classes: %d of %d models placed", (int)order.size(), d.n_models);
     CUDA_TRY(cudaMemcpyAsync(p->tk_models, order.data(), order.size() * sizeof(int), cudaMemcpyHostToDevice, st));
@@ -1426,7 +1411,7 @@ int sce_prepare(sce_plan* p, void* stream) {
     if (!p->b.center_trans || !p->b.center_rot || !p->b.center_scale)
       return fail(SCE_ERR_INVALID, "centering needs the center_trans / center_rot / center_scale buffers");
     const long long n4 = (long long)d.n_models * d.d * d.d / 4;
-    if (p->arith == kArithF16F8)
+    if (p->cfg.arith == kArithF16F8)
       launch_split_rows<kArithF16F8>(p->b.center_rot, p->rot, n4, nullptr, st);
     else
       launch_split_rows<kArithBf16x3>(p->b.center_rot, p->rot, n4, nullptr, st);
@@ -1445,7 +1430,7 @@ int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_los
 }
 
 // models' worth of rows in the caller's batch: 1 when it is shared ([B,d]; also with centering = 1), else M
-static int input_models(const sce_plan* p) { return p->d.centering == 1 ? 1 : p->xm; }
+static int input_models(const sce_plan* p) { return p->d.centering == 1 ? 1 : p->cfg.xm; }
 
 // every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph)
 static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
@@ -1482,7 +1467,7 @@ static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, 
 static bool graph_eligible(const sce_plan* p) {
   if (p->prof_on) return false;                                   // per-phase events are recorded eagerly
   if (p->d.adam_count_mode != SCE_ADAM_FROZEN_T1) return false;   // bias correction is a kernel argument that moves
-  return p->use_graph != 0;
+  return p->cfg.use_graph;
 }
 
 int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, void* stream) {
@@ -1594,13 +1579,13 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
   if (p->code_batch_major) {
     const long long total = (long long)p->d.n_models * per;
     join_code_batch_major_kernel<<<(unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096), 256, 0, st>>>(
-        static_cast<const __half*>(p->c.hi), p->ct.x8, out_code, B, p->d.n, p->d.batch_max, p->bpad, total);
+        static_cast<const __half*>(p->c.hi), p->ct.x8, out_code, B, p->d.n, p->d.batch_max, p->cfg.bpad, total);
     CUDA_TRY(cudaGetLastError());
     return SCE_OK;
   }
   for (int m = 0; m < p->d.n_models; ++m) {
     const Planes c = p->c.at((size_t)m * p->d.batch_max * p->d.n);
-    if (p->arith == kArithF16F8)
+    if (p->cfg.arith == kArithF16F8)
       join_code_kernel<kArithF16F8><<<1024, 256, 0, st>>>(c.hi, nullptr, c.x8, out_code + (long long)m * per, per / 2);
     else
       join_code_kernel<kArithBf16x3><<<1024, 256, 0, st>>>(c.hi, c.lo, nullptr, out_code + (long long)m * per, per / 2);
@@ -1626,7 +1611,7 @@ int sce_last_launch_count(const sce_plan* plan) { return plan ? plan->last_launc
 int sce_input_absmax(sce_plan* plan, float* out_host, void* stream) {
   if (!plan || !out_host) return fail(SCE_ERR_INVALID, "plan / out_host is NULL");
   *out_host = 0.f;
-  if (plan->arith != kArithF16F8) return SCE_OK;
+  if (plan->cfg.arith != kArithF16F8) return SCE_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint32_t bits = 0;
   CUDA_TRY(cudaMemcpyAsync(&bits, plan->res_flags + kAbsmaxWord, sizeof(bits), cudaMemcpyDeviceToHost, st));
@@ -1643,7 +1628,7 @@ int sce_health(sce_plan* plan, int* bad_out, float* absmax_out, void* stream) {
   if (bad_out) *bad_out = words[kBadWord] != 0u;
   if (absmax_out) {
     *absmax_out = 0.f;
-    if (plan->arith == kArithF16F8) memcpy(absmax_out, &words[kAbsmaxWord], sizeof(float));
+    if (plan->cfg.arith == kArithF16F8) memcpy(absmax_out, &words[kAbsmaxWord], sizeof(float));
   }
   return SCE_OK;
 }
@@ -1742,7 +1727,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   if (d.variant == SCE_TOPK)
     launch_fragments<kArithBf16x3, true>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
                                          top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
-  else if (p->arith == kArithF16F8)
+  else if (p->cfg.arith == kArithF16F8)
     launch_fragments<kArithF16F8, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
                                          top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
   else
@@ -1758,7 +1743,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
 }
 
 int sce_plan_arith(const sce_plan* plan) {
-  return !plan ? 0 : plan->arith == kArithF16F8 ? SCE_ARITH_F16F8 : SCE_ARITH_BF16X3;
+  return !plan ? 0 : plan->cfg.arith == kArithF16F8 ? SCE_ARITH_F16F8 : SCE_ARITH_BF16X3;
 }
 
 int sce_profile_begin(sce_plan* p) {
@@ -1852,8 +1837,7 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
   // SCE_ARITH=f16f8 pins AUTO to f16f8 where d % 16 == 0. f16f8 splits a raw operand first and reads its range flag back
   // (one 4-byte copy + synchronise): a value fp16 cannot hold (|v| >= 65520 or NaN) moves a pinned AUTO to bf16x3 and
   // is an error under explicit F16F8.
-  const char* env = getenv("SCE_ARITH");
-  bool f8 = arith == SCE_ARITH_F16F8 || (arith == SCE_ARITH_AUTO && env && !strcmp(env, "f16f8") && d % 16 == 0);
+  bool f8 = arith == SCE_ARITH_F16F8 || (arith == SCE_ARITH_AUTO && env_arith() == SCE_ARITH_F16F8 && d % 16 == 0);
   const bool raw = !A.normalize || (!b_is_a && !B.normalize);
   SimCarve w;
   if (f8 && raw) {

@@ -118,7 +118,9 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
 int sce_plan_destroy(sce_plan* plan);
 
 /* (Re)derive the normalised operand planes of the dictionaries from the fp32 parameters. Must be
- * called once before the first step and again whenever the caller modified the parameters itself. */
+ * called once before the first step and again whenever the caller modified the parameters itself.
+ * SCE_TOPK: also reads the sparsity buffer and returns SCE_ERR_INVALID when some k lies outside [1, n] or, with
+ * topk_k_max in 1..256, above topk_k_max (a larger k needs a new plan). */
 int sce_prepare(sce_plan* plan, void* stream);
 
 /* One optimisation step for all M models on one batch == FunctionalEnsemble.step_batch (ensemble.py:175-193):

@@ -1374,6 +1374,21 @@ int sce_prepare(sce_plan* p, void* stream) {
   CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, kFlagWords * sizeof(uint32_t), st));   // residual flag, input range monitor, health
   const sce_desc& d = p->d;
   const int kmax = p->cfg.tk_kmax;   // (top-k plans only)
+  std::vector<long long> ks;
+  if (d.variant == SCE_TOPK) {
+    // the selection scatters k entries into the code planes but records (and clears on the next call) at most the list
+    // capacity of them, and a k below 1 leaves its bound undefined: hold every k to [1, n] and, with lists, to topk_k_max
+    ks.resize(d.n_models);
+    CUDA_TRY(cudaMemcpyAsync(ks.data(), p->b.sparsity, ks.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    for (int m = 0; m < d.n_models; ++m) {
+      if (ks[m] < 1 || ks[m] > d.n)
+        return fail(SCE_ERR_INVALID, "sparsity of model %d = %lld outside [1, n = %d]", m, ks[m], d.n);
+      if (kmax && ks[m] > d.topk_k_max)
+        return fail(SCE_ERR_INVALID, "sparsity of model %d = %lld exceeds desc.topk_k_max = %d, the top-k list capacity the "
+                    "plan was created with", m, ks[m], d.topk_k_max);
+    }
+  }
   if (kmax) {
     // the top-k selection keeps the code planes (and, in k-sparse plans, the code-gradient planes) all-zero except for
     // the entries its lists record: start them zeroed, with empty lists
@@ -1383,9 +1398,6 @@ int sce_prepare(sce_plan* p, void* stream) {
     CUDA_TRY(cudaMemsetAsync(p->act_pos, 0, (size_t)d.n_models * ((d.n + 31) / 32) * d.batch_max * sizeof(uint32_t), st));
     CUDA_TRY(cudaMemsetAsync(p->tk_cnt, 0, (size_t)d.n_models * d.batch_max * sizeof(int), st));
     // k classes for the gather kernel: rows of shared memory in {8, 16, 32, 64, ...} capped at the list capacity
-    std::vector<long long> ks(d.n_models);
-    CUDA_TRY(cudaMemcpyAsync(ks.data(), p->b.sparsity, ks.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
     const int caps[4] = {16, 32, 64, kmax};
     std::vector<int> order;
     p->tk_groups = 0;
@@ -1395,8 +1407,7 @@ int sce_prepare(sce_plan* p, void* stream) {
       const int cap = caps[g] < kmax ? caps[g] : kmax;
       if (g > 0 && cap <= lo) continue;
       for (int m = 0; m < d.n_models; ++m) {
-        const long long k = ks[m] < 1 ? 1 : (ks[m] > kmax ? (long long)kmax : ks[m]);   // (kernels clip k the same way)
-        if (k > lo && k <= cap) order.push_back(m);
+        if (ks[m] > lo && ks[m] <= cap) order.push_back(m);   // (1 <= k <= topk_k_max <= kmax: checked above)
       }
       p->tk_group_krows[p->tk_groups] = cap;
       p->tk_group_off[++p->tk_groups] = (int)order.size();

@@ -237,8 +237,17 @@ class FunctionalEnsemble:
         return not (bool((b["center_rot"] == eye).all()) and bool((b["center_trans"] == 0).all())
                     and bool((b["center_scale"] == 1).all()))
 
+    def _check_sparsity(self):
+        """Top-k: every model's k must lie in [1, n], as ``TopKEncoder.init`` requires (the engine rejects it too)."""
+        if self._variant != "topk":
+            return
+        for k in self.buffers["sparsity"].reshape(-1).tolist():
+            if not 0 < int(k) <= self._n:
+                raise ValueError(f"sparsity must be in [1, {self._n}], got {k}")
+
     def _build_plan(self, batch_max: int, x_per_model: bool, centering: int = 0):
         dev = self._require_cuda()
+        self._check_sparsity()
         lib = _lib.load()
         for k, v in self.params.items():
             if v.dtype != torch.float32:
@@ -297,6 +306,7 @@ class FunctionalEnsemble:
             self._plan = plan
             self._engine_buffers = eb
             self._plan_key = (batch_max, bool(x_per_model), int(centering))
+            self._plan_k_max = desc.topk_k_max
             _lib.check(lib.sce_set_step_count(plan, self._steps), "sce_set_step_count")
             _lib.check(lib.sce_prepare(plan, self._stream()), "sce_prepare")
         self._plan_steps = 0
@@ -477,9 +487,20 @@ class FunctionalEnsemble:
 
     def refresh(self):
         """Call after modifying ``params`` / ``buffers`` from outside the engine (re-derives the operand
-        copies and the cached centring check)."""
+        copies and the cached centring check; a top-k ensemble whose largest sparsity changed is planned anew)."""
         self._centering = None
         if self._plan is not None:
+            try:
+                self._check_sparsity()
+            except ValueError:
+                # the plan reads the sparsity buffer in place: drop it, so that no call runs the rejected k (the next
+                # call plans anew and raises again until the buffer is valid)
+                self._destroy_plan()
+                raise
+            if self._variant == "topk" and int(self.buffers["sparsity"].max()) != self._plan_k_max:
+                # the largest k sets the plan's top-k list capacity and its decode path (gather or dense): plan anew
+                self._build_plan(*self._plan_key)
+                return
             # engine-side copies of the buffers (dtype-converted hyper-parameter vectors, uint8 coef_mask, int64
             # sparsity) keep their addresses — the plan holds the pointers — and are refilled in place
             for name, t in (self._engine_buffers or {}).items():

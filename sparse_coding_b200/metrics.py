@@ -344,6 +344,8 @@ def _eval_groups(lds, centre: bool, multiple: int):
         n, d = int(ld.n_feats), int(ld.activation_size)
         if d % 8:
             raise ValueError(f"dictionary {i}: activation width d = {d} must be a multiple of 8")
+        if kind == "topk" and not 0 < int(ld.sparsity) <= n:
+            raise ValueError(f"dictionary {i}: sparsity must be in [1, {n}], got {ld.sparsity}")
         if kind == "topk" and n % multiple:
             raise ValueError(f"dictionary {i}: a TopKLearnedDict needs n ({n}) to be a multiple of {multiple}: its rows "
                              "are normalised without a clamp, so zero padding rows would become NaN")

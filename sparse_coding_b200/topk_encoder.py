@@ -6,8 +6,9 @@ normal on the CPU and carries a per-model integer ``sparsity`` buffer (:10-17); 
 with fewer than ``k`` non-zeros (:19-27); the loss is the plain MSE of the reconstruction, without bias or L1 term
 (:29-40); export wraps the normalised dictionary together with ``k`` (:43-62).
 
-Training-time ``loss`` runs in the CUDA engine: scores on the tensor cores, a per-row radix select
-(``topk_select_kernel``), then the same decode / backward / Adam pipeline as the tied SAE. Unlike the reference,
+Training-time ``loss`` runs in the CUDA engine: scores on the tensor cores, a per-row selection that bounds the k-th
+largest score and ranks the few candidates above it (``topk_select2_kernel``), then a gather decode over the k selected
+rows or the tied SAE's dense decode, and the same backward / Adam pipeline. Unlike the reference,
 which has to fall back to a Python loop over models because ``torch.topk`` with a data-dependent ``k`` cannot be
 vmapped (``no_stacking=True``), models with different ``k`` are batched in one launch sequence.
 """

@@ -310,3 +310,25 @@ def test_c_abi_error_paths_on_device():
     bufs.workspace_bytes = need
     assert lib.sce_plan_create(C.byref(desc), C.byref(bufs), C.byref(plan)) == 0
     assert lib.sce_plan_destroy(plan) == 0
+    # top-k: sce_prepare reads the sparsities; k outside [1, n], or above topk_k_max where the plan keeps lists (1..256),
+    # is rejected before any selection could write past its lists. The valid ones (positive controls) prepare.
+    d, n = 32, 256
+    dct = torch.randn(1, n, d, device="cuda")
+    mom = torch.zeros_like(dct)
+    for k, k_max, want in ((20, 16, b"topk_k_max"), (0, 16, b"outside [1, n"), (n + 1, 0, b"outside [1, n"),
+                           (300, 300, b"outside [1, n"), (16, 16, None), (9, 16, None), (20, 0, None), (n, 300, None)):
+        desc = _lib.SceDesc(variant=_lib.SCE_TOPK, n_models=1, d=d, n=n, batch_max=16, x_per_model=0, lr=0.0, beta1=0.9,
+                            beta2=0.999, eps=1e-8, eps_root=0.0, adam_count_mode=0, fwd_passes=3, bwd_passes=3,
+                            norm_floor=0.0, arith=0, topk_k_max=k_max, centering=0)
+        sp = torch.tensor([k], dtype=torch.int64, device="cuda")
+        bufs = _lib.SceBuffers(encoder=dct.data_ptr(), encoder_m=mom.data_ptr(), encoder_v=mom.data_ptr(),
+                               sparsity=sp.data_ptr())
+        plan, ws = _lib.create_plan(desc, bufs, torch.device("cuda"))
+        try:
+            if want is None:
+                assert lib.sce_prepare(plan, stream) == 0, (k, k_max, lib.sce_last_error())
+            else:
+                assert lib.sce_prepare(plan, stream) == -1, (k, k_max)
+                assert want in lib.sce_last_error(), (k, k_max, lib.sce_last_error())
+        finally:
+            lib.sce_plan_destroy(plan)

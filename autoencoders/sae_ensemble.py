@@ -1,2 +1,2 @@
 from sparse_coding_b200.sae_ensemble import (FunctionalMaskedSAE, FunctionalMaskedTiedSAE, FunctionalSAE,  # noqa: F401
-                                             FunctionalTiedSAE)
+                                             FunctionalTiedCenteredSAE, FunctionalTiedSAE)

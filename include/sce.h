@@ -22,6 +22,9 @@
 extern "C" {
 #endif
 
+/* 201 also covers the additive extension for FunctionalTiedCenteredSAE: the enum value SCE_TIED_LEARNED_CENTER, the
+ * center / center_m / center_v fields appended to sce_buffers, and sce_read_center_grad. Nothing earlier moved, so a
+ * caller built against the earlier 201 header keeps working unchanged. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -36,7 +39,11 @@ typedef enum sce_status {
 typedef enum sce_variant {
   SCE_TIED = 0,   /* FunctionalTiedSAE.loss   (sae_ensemble.py:135-162); + coef_mask = FunctionalMaskedTiedSAE (:347-373) */
   SCE_UNTIED = 1, /* FunctionalSAE.loss       (sae_ensemble.py:53-78);   + coef_mask = FunctionalMaskedSAE     (:418-444) */
-  SCE_TOPK = 2    /* TopKEncoder.loss         (topk_encoder.py:29-40) */
+  SCE_TOPK = 2,   /* TopKEncoder.loss         (topk_encoder.py:29-40) */
+  SCE_TIED_LEARNED_CENTER = 3 /* FunctionalTiedCenteredSAE.loss, sae_ensemble.py:204-230: tied, on x - center[m] with the
+                                 centre a trained parameter (sce_buffers.center). x_per_model only says how the caller's
+                                 batch is laid out: the plan always holds M centred batches. No bias decay; needs
+                                 desc.centering = 0. */
 } sce_variant;
 
 /* How the Adam step counter behaves (SURVEY.md Q2). */
@@ -99,6 +106,10 @@ typedef struct sce_buffers {
   const float* center_trans;      /* [M,d]   buffers["center_trans"]  (desc.centering != 0; else NULL) */
   const float* center_rot;        /* [M,d,d] buffers["center_rot"]    */
   const float* center_scale;      /* [M,d]   buffers["center_scale"]  */
+  float* center;                  /* [M,d]   params["center"] (SCE_TIED_LEARNED_CENTER; else NULL), updated in place by
+                                             sce_step like the other parameters */
+  float* center_m;                /* its Adam moments, same shape */
+  float* center_v;
 } sce_buffers;
 
 typedef struct sce_plan sce_plan;
@@ -137,7 +148,8 @@ int sce_step_host(sce_plan* plan, const float* x_host, int B, float* out_losses_
                   void* stream);
 
 /* Forward only (evaluation; LearnedDict.predict semantics on already-centred inputs): writes x_hat
- * [M,B,d] fp32 if non-NULL and the same losses / nnz as sce_step, without touching parameters. */
+ * [M,B,d] fp32 if non-NULL and the same losses / nnz as sce_step, without touching parameters. SCE_TIED_LEARNED_CENTER:
+ * x_hat is in the centred space (x_hat + center[m] is the reconstruction of x). */
 int sce_forward(sce_plan* plan, const float* x, int B, float* x_hat, float* out_losses, float* out_nnz,
                 void* stream);
 
@@ -148,6 +160,11 @@ int sce_read_code(sce_plan* plan, int B, float* out_code, void* stream);
 /* Materialise the fp32 parameter gradients of the most recent sce_grads call (parity tests). */
 int sce_grads(sce_plan* plan, const float* x, int B, float* d_encoder, float* d_bias, float* d_decoder,
               float* out_losses, float* out_nnz, void* stream);
+
+/* SCE_TIED_LEARNED_CENTER: copy the gradient of params["center"] that the most recent sce_grads or sce_step computed,
+ * d_center = sum_b g_b - db W (g = dL/dx_hat, db the bias gradient, W the normalised dictionary), to the device fp32
+ * array d_center [M,d]. Asynchronous on `stream`. SCE_ERR_INVALID for the other variants. */
+int sce_read_center_grad(sce_plan* plan, float* d_center, void* stream);
 
 /* Split a row-gathered, optionally mean-centred batch out of a resident activation chunk:
  *   out[r,:] = float(chunk[idx[r],:]) - sub[:]      chunk fp16 or fp32 [N,d]; idx int64 [B] or NULL (identity)
@@ -216,6 +233,8 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream);
  *                M * ceil(B/32) * 4 * n fp32 (config 2, M = 16, n = 4096, B = 8192: 256 MiB; M = 1, n = 32768,
  *                B = 4096: 64 MiB). sce_forward_stats_workspace_bytes is host-only; it returns 0 for an invalid
  *                desc or B outside [1, batch_max].
+ * Not available for SCE_TIED_LEARNED_CENTER (the size query returns 0, the call SCE_ERR_INVALID): evaluate its exported
+ * dictionaries, which are TiedSAE objects with the centre as their translation.
  * x_hat, out_losses and out_nnz are those of sce_forward (x_hat optional). Asynchronous on `stream`. */
 size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B);
 int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
@@ -248,6 +267,7 @@ int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_ph
  *                M (B/L) n (4 + 1) bytes, and M n int32 (config 2, M = 16, n = 4096, B = 8192, L = 64: 40 MiB).
  *                sce_fragments_workspace_bytes is host-only; it returns 0 for an invalid desc, B outside
  *                [1, batch_max] or an invalid L.
+ * Not available for SCE_TIED_LEARNED_CENTER, as sce_forward_stats.
  * Deterministic (no atomics) and asynchronous on `stream`. */
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L);
 int sce_forward_fragments(sce_plan* plan, const float* x, int B, int L, long long frag0, int n_top, int n_random,

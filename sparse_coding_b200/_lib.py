@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # SCE_LIB: an alternative build of the same library (kernel A/B experiments)
 LIB_PATH = os.environ.get("SCE_LIB") or os.path.join(_HERE, "libsce.so")
 
-SCE_TIED, SCE_UNTIED, SCE_TOPK = 0, 1, 2
+SCE_TIED, SCE_UNTIED, SCE_TOPK, SCE_TIED_LEARNED_CENTER = 0, 1, 2, 3
 SCE_ADAM_FROZEN_T1, SCE_ADAM_STANDARD = 0, 1
 SCE_LOSS_COLS = 4
 SCE_ARITH_AUTO, SCE_ARITH_BF16X3, SCE_ARITH_F16F8 = 0, 1, 2
@@ -28,7 +28,7 @@ EXPORTS = [
     "sce_last_launch_count", "sce_get_step_count", "sce_set_step_count", "sce_profile_begin", "sce_profile_end",
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
-    "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows",
+    "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows", "sce_read_center_grad",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -51,6 +51,7 @@ class SceBuffers(C.Structure):
         ("l1_alpha", C.c_void_p), ("bias_decay", C.c_void_p), ("coef_mask", C.c_void_p), ("sparsity", C.c_void_p),
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
         ("center_trans", C.c_void_p), ("center_rot", C.c_void_p), ("center_scale", C.c_void_p),
+        ("center", C.c_void_p), ("center_m", C.c_void_p), ("center_v", C.c_void_p),
     ]
 
 
@@ -84,6 +85,7 @@ def load():
     lib.sce_forward.argtypes = [vp, vp, i, vp, vp, vp, vp]
     lib.sce_read_code.argtypes = [vp, i, vp, vp]
     lib.sce_grads.argtypes = [vp, vp, i, vp, vp, vp, vp, vp, vp]
+    lib.sce_read_center_grad.argtypes = [vp, vp, vp]
     lib.sce_gather_rows.argtypes = [vp, i, ll, i, vp, i, vp, vp, vp]
     lib.sce_last_launch_count.argtypes = [vp]
     lib.sce_get_step_count.argtypes = [vp]

@@ -11,6 +11,9 @@
 //   bias_norm, finalize (losses), dict_rows<ADAM> (Jacobian + Adam + renormalise + re-split), bias<ADAM>
 // Top-k variant: the encode GEMM stores fp32 scores; topk_select2_kernel keeps k per row; with the k-sparse path
 // (sce_topk.cuh) decode and dcode are a gather kernel over the k selected dictionary rows instead of two dense GEMMs.
+// Learned-centre variant (tied in every other respect): center_sub_kernel forms x - center[m] first, the decode epilogue
+// also writes column sums of g, and before the Adam update three kernels form the centre gradient sum_b g - db W
+// (center_coef / center_gemv / center_grad) and update the centre.
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -102,7 +105,10 @@ struct PlanBuffers {
   // dz's 8-bit planes are written in that layout in the first place (EpiDcodeT<f16f8, true>).
   Planes xt, ct, gt;
   Planes rot;                     // centring: operand planes of buffers["center_rot"] [M, d, d]
-  float* x_centered;              // centring: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
+  float* x_centered;              // centring, learned centre: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
+  // learned centre: column sums of g [M, tiles_m*4, d] (EpiDecodeT<AR, true>), db / ||E_n|| [M, n], the GEMV partials
+  // [M, ceil(n / kCenterChunkRows), d] and the centre gradient [M, d] (sce_read_center_grad)
+  float *g_part, *center_coef, *center_part, *center_grad;
   float* scores;                  // top-k: fp32 scores [M, Bmax, n] of the encode GEMM
   int* tk_models;                 // top-k gather kernel: the models sorted into k classes (device copy of tk_group_models)
   uint32_t* tk_cmax;              // top-k: largest key per 32-column chunk of the scores [M, Bmax, n_chunks] (EpiScoresTma)
@@ -180,7 +186,7 @@ struct Carve {
 
 static int validate(const sce_desc* d) {
   if (!d) return fail(SCE_ERR_INVALID, "desc is NULL");
-  if (d->variant < SCE_TIED || d->variant > SCE_TOPK) return fail(SCE_ERR_INVALID, "unknown variant %d", d->variant);
+  if (d->variant < SCE_TIED || d->variant > SCE_TIED_LEARNED_CENTER) return fail(SCE_ERR_INVALID, "unknown variant %d", d->variant);
   if (d->n_models < 1 || d->batch_max < 1) return fail(SCE_ERR_INVALID, "n_models and batch_max must be >= 1");
   if (d->d < 8 || d->d % 8 || d->n < 8 || d->n % 8)
     return fail(SCE_ERR_INVALID, "d (%d) and n (%d) must be positive multiples of 8", d->d, d->n);
@@ -189,6 +195,8 @@ static int validate(const sce_desc* d) {
     return fail(SCE_ERR_INVALID, "fwd_passes / bwd_passes must be 1 or 3");
   if (d->centering < 0 || d->centering > 2) return fail(SCE_ERR_INVALID, "centering must be 0, 1 or 2");
   if (d->centering && !d->x_per_model) return fail(SCE_ERR_INVALID, "centering needs x_per_model = 1 (the centred batch differs per model)");
+  if (d->centering && d->variant == SCE_TIED_LEARNED_CENTER)
+    return fail(SCE_ERR_INVALID, "the learned-centre variant centres the batch itself: desc.centering must be 0");
   if (d->arith < SCE_ARITH_AUTO || d->arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "unknown arith %d", d->arith);
   if (d->arith == SCE_ARITH_F16F8 && (d->d % 16 || d->n % 16))
     return fail(SCE_ERR_INVALID, "arith = F16F8 needs d (%d) and n (%d) to be multiples of 16 (TMA pitch of the 8-bit planes)",
@@ -268,7 +276,8 @@ static int topk_slices(const sce_desc& d, size_t kmax) {
 static PlanConfig plan_config(const sce_desc& d) {
   PlanConfig c{};
   c.arith = resolve_arith(d);
-  c.xm = d.x_per_model ? d.n_models : 1;
+  // (the learned-centre variant always holds M centred batches, whatever the caller's layout)
+  c.xm = d.x_per_model || d.variant == SCE_TIED_LEARNED_CENTER ? d.n_models : 1;
   c.bpad = (d.batch_max + 15) / 16 * 16;
   // top-k lists hold the largest k of the ensemble (desc.topk_k_max, supplied by the host mirror, which knows
   // buffers["sparsity"]) rounded up to 8; none when it is unknown or too large for the gather kernel (dense path)
@@ -366,6 +375,13 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
   if (d.centering) {
     w.rot = c.planes(M * dd * dd, f8);
     w.x_centered = c.take<float>(M * B * dd);
+  }
+  if (d.variant == SCE_TIED_LEARNED_CENTER) {
+    w.x_centered = c.take<float>(M * B * dd);
+    w.g_part = c.take<float>(M * tiles_mB * 4 * dd);
+    w.center_coef = c.take<float>(M * n);
+    w.center_part = c.take<float>(M * ((n + kCenterChunkRows - 1) / kCenterChunkRows) * dd);
+    w.center_grad = c.take<float>(M * dd);
   }
   w.res_flags = c.take<uint32_t>(kFlagWords);   // [0] residual flag, [kAbsmaxWord] input range monitor, [kBadWord] health (separate 128-byte lines)
   return align_up(c.off, 1024);
@@ -643,6 +659,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
                           float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
   using EpiEnc = EpiEncodeT<AR>;
   using EpiDec = EpiDecodeT<AR>;
+  using EpiDecG = EpiDecodeT<AR, true>;
   using EpiDco = EpiDcodeT<AR>;
   constexpr bool f8 = AR == kArithF16F8;
   const sce_desc& d = p->d;
@@ -656,7 +673,9 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   const int M = d.n_models, n = d.n, dd = d.d;
   const long long Bm = d.batch_max;
   const int one[2] = {1, 1};
-  const int xb[2] = {d.x_per_model ? 1 : 0, 1};
+  const bool learned = d.variant == SCE_TIED_LEARNED_CENTER;
+  const bool x_models = d.x_per_model || learned;   // the batch the kernels below read holds one slab per model
+  const int xb[2] = {x_models ? 1 : 0, 1};
   const int tiles_mB = (B + kBM - 1) / kBM;
 
   prof_mark(p, SCE_PHASE_SPLIT, st);
@@ -676,6 +695,15 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     rc = launch_gemm_t<EpiCenter, false, false, false, AR>(p, maps->center, 1, one, one, dd, 3, B, dd, cp, st);
     if (rc) return rc;
     launches += 2;
+    x = p->x_centered;
+  } else if (learned) {
+    // ---- learned centre (sae_ensemble.py:198-200): x - center[m] -> the per-model fp32 batch every kernel below reads
+    const long long n4 = (long long)B * dd / 4;
+    const int blocks = (int)((n4 + 255) / 256 < 1024 ? (n4 + 255) / 256 : 1024);
+    center_sub_kernel<<<dim3(blocks, M), 256, 0, st>>>(x, d.x_per_model ? (long long)B * dd : 0, p->b.center,
+                                                       p->x_centered, B, dd);
+    CUDA_TRY(cudaGetLastError());
+    ++launches;
     x = p->x_centered;
   }
   // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace
@@ -789,30 +817,35 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     CUDA_TRY(cudaGetLastError());
     n_dec_parts = cfg.tk_slices * B;
   } else {
-    // ---- decode (+ residual, loss partial, g)
-    typename EpiDec::Params dp;
-    dp.x = x;
-    dp.x_model_stride = d.x_per_model ? (long long)B * dd : 0;
-    dp.g_hi = static_cast<uint16_t*>(p->g.hi);
-    dp.g_lo = static_cast<uint8_t*>(p->g.lo);
-    dp.g_x8 = p->g.x8;
-    dp.x_hat = x_hat;
-    dp.part = p->part_dec;
-    dp.g_model_stride = Bm * dd;
-    dp.xhat_model_stride = (long long)B * dd;
-    dp.ld = dd;
-    dp.tiles_m = tiles_mB;
-    dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
-    dp.tiles_n = (dd + kBN - 1) / kBN;
-    if constexpr (f8)
-      rc = launch_gemm_t<EpiDec, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-    else if (cfg.split_decode)
-      rc = launch_gemm_t<EpiDec, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-    else
-      rc = launch_gemm_t<EpiDec, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    // ---- decode (+ residual, loss partial, g; learned centre: + column sums of g)
+    auto decode = [&](auto tag) {
+      using E = typename decltype(tag)::type;
+      typename E::Params dp;
+      dp.x = x;
+      dp.x_model_stride = x_models ? (long long)B * dd : 0;
+      dp.g_hi = static_cast<uint16_t*>(p->g.hi);
+      dp.g_lo = static_cast<uint8_t*>(p->g.lo);
+      dp.g_x8 = p->g.x8;
+      dp.x_hat = x_hat;
+      dp.part = p->part_dec;
+      dp.g_model_stride = Bm * dd;
+      dp.xhat_model_stride = (long long)B * dd;
+      dp.ld = dd;
+      dp.tiles_m = tiles_mB;
+      dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
+      dp.tiles_n = (dd + kBN - 1) / kBN;
+      if constexpr (!std::is_same<E, EpiDec>::value) dp.g_part = p->g_part;
+      if constexpr (f8)
+        return launch_gemm_t<E, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+      else if (cfg.split_decode)
+        return launch_gemm_t<E, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+      else
+        return launch_gemm_t<E, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+    };
+    rc = learned ? decode(TypeTag<EpiDecG>{}) : decode(TypeTag<EpiDec>{});
     if (rc) return rc;
     ++launches;
-    n_dec_parts = tiles_mB * 8 * dp.tiles_n;
+    n_dec_parts = tiles_mB * 8 * ((dd + kBN - 1) / kBN);
     if (tdw) CUDA_TRY(batch_major(p->g, p->gt, M, dd));
   }
 
@@ -899,6 +932,30 @@ static int run_pipeline(sce_plan* p, const float* x, int B, float* x_hat, bool b
              ? run_pipeline_t<kArithF16F8>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part)
              : run_pipeline_t<kArithBf16x3>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
 }
+
+// Learned-centre plans: the centre gradient of the last backward pass into p->center_grad (sum_b g - db W, with db and
+// W those of this step: it runs before dict_rows_kernel<MODE_ADAM> rewrites the encoder), and with MODE_ADAM the Adam
+// update of the centre. Adds its launches to `launches`.
+template <int MODE>
+static int center_grad_launches(sce_plan* p, int B, const AdamHyper& h, cudaStream_t st, int& launches) {
+  const sce_desc& d = p->d;
+  const int M = d.n_models, n = d.n, dd = d.d;
+  const int n_part = ((B + kBM - 1) / kBM) * 4;
+  const int chunks = (n + kCenterChunkRows - 1) / kCenterChunkRows;
+  const float scale = grad_out_scale(p, B);
+  center_coef_kernel<<<dim3((n + kCenterCoefRows - 1) / kCenterCoefRows, M), 256, 0, st>>>(
+      p->b.encoder, p->db_part, n_part, n, dd, d.norm_floor, scale, p->center_coef);
+  center_gemv_kernel<<<dim3((dd + 511) / 512, chunks, M), 128, 0, st>>>(p->b.encoder, p->center_coef, n, dd, p->center_part);
+  const long long tot = (long long)M * dd;
+  center_grad_kernel<MODE><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
+      p->g_part, n_part, scale, p->center_part, chunks, M, dd, p->center_grad, MODE == MODE_ADAM ? p->b.center : nullptr,
+      MODE == MODE_ADAM ? p->b.center_m : nullptr, MODE == MODE_ADAM ? p->b.center_v : nullptr, h,
+      MODE == MODE_ADAM ? p->res_flags : nullptr);
+  CUDA_TRY(cudaGetLastError());
+  launches += 3;
+  return SCE_OK;
+}
+
 
 // ------------------------------------------------------------------------------------------------
 // evaluation statistics (sce_forward_stats): per-feature moments and segment activity counts
@@ -1332,6 +1389,8 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   if (desc->variant != SCE_TOPK && (!b.encoder_bias || !b.bias_m || !b.bias_v))
     return fail(SCE_ERR_INVALID, "encoder_bias / bias_m / bias_v are required for SAE variants");
   if (desc->variant == SCE_TOPK && !b.sparsity) return fail(SCE_ERR_INVALID, "top-k variant needs the sparsity buffer");
+  if (desc->variant == SCE_TIED_LEARNED_CENTER && (!b.center || !b.center_m || !b.center_v))
+    return fail(SCE_ERR_INVALID, "the learned-centre variant needs center / center_m / center_v");
   const PlanConfig cfg = plan_config(*desc);
   rc = check_workspace(b.workspace, b.workspace_bytes, plan_workspace(*desc, cfg), "");
   if (rc) return rc;
@@ -1441,7 +1500,10 @@ int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_los
 }
 
 // models' worth of rows in the caller's batch: 1 when it is shared ([B,d]; also with centering = 1), else M
-static int input_models(const sce_plan* p) { return p->d.centering == 1 ? 1 : p->cfg.xm; }
+static int input_models(const sce_plan* p) {
+  if (p->d.variant == SCE_TIED_LEARNED_CENTER) return p->d.x_per_model ? p->d.n_models : 1;
+  return p->d.centering == 1 ? 1 : p->cfg.xm;
+}
 
 // every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph)
 static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
@@ -1451,6 +1513,7 @@ static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, 
   const sce_desc& d = p->d;
   const AdamHyper h = hyper_for(p, t);
   int launches = p->last_launches;
+  if (d.variant == SCE_TIED_LEARNED_CENTER && (rc = center_grad_launches<MODE_ADAM>(p, B, h, st, launches))) return rc;
   DictSide sides[2];
   for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s, ++launches)
     if ((rc = launch_dict_rows<MODE_ADAM>(p, sides[s], nullptr, h, st))) return rc;
@@ -1548,6 +1611,8 @@ int sce_grads(sce_plan* p, const float* x, int B, float* d_encoder, float* d_bia
   if (rc) return rc;
   const sce_desc& d = p->d;
   const AdamHyper h = hyper_for(p, 1);
+  int launches = 0;
+  if (d.variant == SCE_TIED_LEARNED_CENTER && (rc = center_grad_launches<MODE_GRAD>(p, B, h, st, launches))) return rc;
   DictSide sides[2];
   float* const grad_out[2] = {d_encoder, d_decoder};
   for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
@@ -1602,6 +1667,14 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
       join_code_kernel<kArithBf16x3><<<1024, 256, 0, st>>>(c.hi, c.lo, nullptr, out_code + (long long)m * per, per / 2);
   }
   CUDA_TRY(cudaGetLastError());
+  return SCE_OK;
+}
+
+int sce_read_center_grad(sce_plan* p, float* d_center, void* stream) {
+  if (!p || !d_center) return fail(SCE_ERR_INVALID, "plan / d_center is NULL");
+  if (p->d.variant != SCE_TIED_LEARNED_CENTER) return fail(SCE_ERR_INVALID, "read_center_grad: the plan has no learned centre");
+  CUDA_TRY(cudaMemcpyAsync(d_center, p->center_grad, (size_t)p->d.n_models * p->d.d * sizeof(float),
+                           cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return SCE_OK;
 }
 
@@ -1660,7 +1733,7 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
 }
 
 size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
-  if (validate(desc) || B < 1 || B > desc->batch_max) return 0;
+  if (validate(desc) || B < 1 || B > desc->batch_max || desc->variant == SCE_TIED_LEARNED_CENTER) return 0;
   return stats_workspace(*desc, B);
 }
 
@@ -1668,6 +1741,9 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
                       float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
                       size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_stats: plan is NULL");
+  if (p->d.variant == SCE_TIED_LEARNED_CENTER)
+    return fail(SCE_ERR_INVALID, "forward_stats: not available for the learned-centre variant; evaluate its exported "
+                                 "dictionaries (TiedSAE)");
   if (int rc = check_rows(p, B, "forward_stats: ")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "forward_stats: x is NULL");
   if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
@@ -1701,7 +1777,8 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
 }
 
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L) return 0;
+  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || desc->variant == SCE_TIED_LEARNED_CENTER)
+    return 0;
   return frag_workspace(*desc, B, L, nullptr, nullptr);
 }
 
@@ -1710,6 +1787,9 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_fragments: plan is NULL");
+  if (p->d.variant == SCE_TIED_LEARNED_CENTER)
+    return fail(SCE_ERR_INVALID, "forward_fragments: not available for the learned-centre variant; evaluate its exported "
+                                 "dictionaries (TiedSAE)");
   if (int rc = check_rows(p, B, "forward_fragments: ")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "forward_fragments: x is NULL");
   if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);

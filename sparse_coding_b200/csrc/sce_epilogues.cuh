@@ -163,6 +163,24 @@ __device__ __forceinline__ float warp_column_sum(float (&v)[32], int lane) {
   return v[0];
 }
 
+// the same for W < 32 columns: lanes j, j + W, j + 2W, ... all end with the sum of column j over the warp's rows
+template <int W>
+__device__ __forceinline__ float warp_column_sum_part(float (&v)[W], int lane) {
+#pragma unroll
+  for (int half = W / 2; half >= 1; half >>= 1) {
+    const bool upper = (lane & half) != 0;
+#pragma unroll
+    for (int i = 0; i < half; ++i) {
+      const float send = upper ? v[i] : v[i + half];
+      const float keep = upper ? v[i + half] : v[i];
+      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
+    }
+  }
+#pragma unroll
+  for (int o = W; o < 32; o <<= 1) v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
+  return v[0];
+}
+
 // Per-feature moments of the code (EpiEncodeT<ARITH, true>, evaluation only): each epilogue warp writes the column sums
 // of c, c^2, c^3, c^4 over its 32 rows as fp32 partials [M][row_blocks][4][n], row block = global row / 32; a second
 // kernel (moment_reduce_kernel) adds them up over the row blocks in a fixed order in fp64.
@@ -305,17 +323,29 @@ struct EpiEncodeT {
   }
 };
 
+// Column sums of g (EpiDecodeT<ARITH, true>, learned-centre variant only): each epilogue warp writes the sums of its 32
+// rows of g = r * gscale per column as fp32 partials [M][tiles_m*4][d], laid out like the bias-gradient partials of
+// EpiDcodeT; center_grad_kernel adds them up over the row blocks in a fixed order (sum_b g_b of the centre gradient).
+template <bool GSUM>
+struct DecodeGsumParams {};
+template <>
+struct DecodeGsumParams<true> {
+  float* g_part;   // [M][tiles_m*4][d]
+};
+
 // ------------------------------------------------------------------------------------------------
 // decode:  r = acc - x;  partial sum r^2;  g = r * gscale -> planes of g;  optional x^ store
 // bf16x3: gscale = 2/(B d) (g is the loss gradient). f16f8: gscale = 1 — the fp16 plane could not hold 2r/(Bd)
 // (~1e-7), so the backward pass runs on the residual itself and its consumers carry the factor (dcode adds
 // alpha d/2 instead of alpha/B; the weight- and bias-gradient outputs are multiplied by 2/(B d)).
+// GSUM (compile-time) adds the column sums of DecodeGsumParams; there rows beyond the batch stay in the warp (as zeros)
+// for the transpose-reduce. The instantiations without it compile to the same code as without the switch.
 // ------------------------------------------------------------------------------------------------
-template <int ARITH>
+template <int ARITH, bool GSUM = false>
 struct EpiDecodeT {
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 0;
-  struct Params {
+  struct Params : DecodeGsumParams<GSUM> {
     const float* x;                // [B, d] (x_model_stride = 0) or [M, B, d]
     long long x_model_stride;
     uint16_t* g_hi;                // [M, B, d] 16-bit plane
@@ -354,33 +384,58 @@ struct EpiDecodeT {
 #pragma unroll
     for (int j = 0; j < 8; ++j) xc[j] = xn[j];
     fetch_x(c + 64);  // this warp's next chunk (harmless past the tile: predicated on n_total, unused)
-    if (col >= n_total || T.row >= m_total) return;
+    if constexpr (GSUM) {
+      if (col >= n_total) return;  // warp-uniform
+    } else {
+      if (col >= n_total || T.row >= m_total) return;
+    }
+    const bool row_ok = !GSUM || T.row < m_total;
     const long long off = (long long)T.model * P.g_model_stride + (long long)T.row * P.ld + col;
     uint32_t whi[16], wlo[16];
+    // GSUM: every row block of a tile in the batch writes its column sums (as EpiDcodeT's db_part); warp-uniform. They are
+    // reduced 8 columns at a time as the loop goes, so that few values are live beside the split decode's accumulators
+    const bool gsum = GSUM && T.m_blk * kBM < m_total;
+    float gv[8], gs = 0.f;
 #pragma unroll
     for (int j = 0; j < 32; j += 4) {
       const float4 xv = xc[j >> 2];
-      const bool ok = col + j < n_total;  // d % 4 == 0
+      const bool ok = row_ok && col + j < n_total;  // d % 4 == 0
       const float r0 = ok ? __uint_as_float(r[j]) - xv.x : 0.f, r1 = ok ? __uint_as_float(r[j + 1]) - xv.y : 0.f;
       const float r2 = ok ? __uint_as_float(r[j + 2]) - xv.z : 0.f, r3 = ok ? __uint_as_float(r[j + 3]) - xv.w : 0.f;
       sq += r0 * r0 + r1 * r1 + r2 * r2 + r3 * r3;
       split_pair<ARITH>(r0 * P.gscale, r1 * P.gscale, j >> 1, whi, wlo);
       split_pair<ARITH>(r2 * P.gscale, r3 * P.gscale, (j >> 1) + 1, whi, wlo);
+      if constexpr (GSUM) {
+        gv[j & 7] = r0 * P.gscale;   // this row's g as split, 0 outside the batch and the matrix
+        gv[(j & 7) + 1] = r1 * P.gscale;
+        gv[(j & 7) + 2] = r2 * P.gscale;
+        gv[(j & 7) + 3] = r3 * P.gscale;
+        if ((j & 7) == 4 && gsum) {   // columns j - 4 .. j + 3 -> lanes j - 4 .. j + 3 (and their copies)
+          const float t = warp_column_sum_part<8>(gv, T.lane);
+          if ((T.lane >> 3) == (j >> 3)) gs = t;
+        }
+      }
       if (P.x_hat && ok)
         *reinterpret_cast<float4*>(P.x_hat + (long long)T.model * P.xhat_model_stride + (long long)T.row * P.ld + col + j) =
             make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]),
                         __uint_as_float(r[j + 3]));
     }
-    store_bf16x32(reinterpret_cast<__nv_bfloat16*>(P.g_hi) + off, whi, n_total - col);
-    if constexpr (ARITH == kArithF16F8) {
+    if (row_ok) {
+      store_bf16x32(reinterpret_cast<__nv_bfloat16*>(P.g_hi) + off, whi, n_total - col);
+      if constexpr (ARITH == kArithF16F8) {
 #pragma unroll
-      for (int q = 0; q < 2; ++q)
-        if (q * 16 < n_total - col) {  // d % 16 == 0 in this arithmetic
-          *reinterpret_cast<uint4*>(P.g_lo + off + q * 16) = make_uint4(wlo[4 * q], wlo[4 * q + 1], wlo[4 * q + 2], wlo[4 * q + 3]);
-          *reinterpret_cast<uint4*>(P.g_x8 + off + q * 16) = make_uint4(wlo[8 + 4 * q], wlo[9 + 4 * q], wlo[10 + 4 * q], wlo[11 + 4 * q]);
-        }
-    } else {
-      store_bf16x32(reinterpret_cast<__nv_bfloat16*>(P.g_lo) + off, wlo, n_total - col);
+        for (int q = 0; q < 2; ++q)
+          if (q * 16 < n_total - col) {  // d % 16 == 0 in this arithmetic
+            *reinterpret_cast<uint4*>(P.g_lo + off + q * 16) = make_uint4(wlo[4 * q], wlo[4 * q + 1], wlo[4 * q + 2], wlo[4 * q + 3]);
+            *reinterpret_cast<uint4*>(P.g_x8 + off + q * 16) = make_uint4(wlo[8 + 4 * q], wlo[9 + 4 * q], wlo[10 + 4 * q], wlo[11 + 4 * q]);
+          }
+      } else {
+        store_bf16x32(reinterpret_cast<__nv_bfloat16*>(P.g_lo) + off, wlo, n_total - col);
+      }
+    }
+    if constexpr (GSUM) {
+      if (gsum && col + T.lane < n_total)
+        P.g_part[(((long long)T.model * P.tiles_m + T.m_blk) * 4 + T.warp_q) * n_total + col + T.lane] = gs;
     }
   }
   __device__ __forceinline__ void finish() {

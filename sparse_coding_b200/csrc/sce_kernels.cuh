@@ -106,6 +106,25 @@ __global__ void center_split_kernel(const float* __restrict__ x, long long x_mod
 }
 
 // ------------------------------------------------------------------------------------------------
+// learned centre (FunctionalTiedCenteredSAE.center, sae_ensemble.py:198-200): out[m] = x[m] - center[m], fp32 [M][B][d];
+// x is [B][d] shared by the models (x_model_stride = 0) or [M][B][d]. grid.y = model.
+// ------------------------------------------------------------------------------------------------
+__global__ void center_sub_kernel(const float* __restrict__ x, long long x_model_stride, const float* __restrict__ center,
+                                  float* __restrict__ out, int B, int d) {
+  const int model = blockIdx.y;
+  const int d4 = d >> 2;
+  const long long n4 = (long long)B * d4;
+  const float4* xs = reinterpret_cast<const float4*>(x + (long long)model * x_model_stride);
+  const float4* cs = reinterpret_cast<const float4*>(center + (long long)model * d);
+  float4* o = reinterpret_cast<float4*>(out + (long long)model * B * d);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const float4 v = xs[i];
+    const float4 c = __ldg(cs + (int)(i % d4));
+    o[i] = make_float4(v.x - c.x, v.y - c.y, v.z - c.z, v.w - c.w);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // chunk row gather (+ fp16 -> fp32, + mean-centring): out[r,:] = float(chunk[idx[r],:]) - sub
 // one warp per row; big_sweep.py:168 and :359-364
 // ------------------------------------------------------------------------------------------------
@@ -419,6 +438,97 @@ __global__ void bias_kernel(float* __restrict__ bias, float* __restrict__ m, flo
   } else {
     float mm = m[i], vv = v[i];
     bias[i] = adam_apply(b, g, mm, vv, h);
+    m[i] = mm;
+    v[i] = vv;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Gradient of the learned centre: d_center = sum_b g_b - db W, W = E / max(||E_n||, floor) (the dictionary the step
+// used: these kernels run before dict_rows_kernel<MODE_ADAM> rewrites E). Three passes, no atomics: bitwise repeatable.
+// ------------------------------------------------------------------------------------------------
+constexpr int kCenterCoefRows = 32;    // dictionary rows per block of center_coef_kernel
+constexpr int kCenterChunkRows = 64;   // dictionary rows per partial of center_gemv_kernel
+
+// coef[m][n] = db[m][n] / max(||E[m][n]||, floor), db summed from the dcode epilogue's partials in the order bias_kernel
+// uses (the same fp32 value) times part_scale. Grid (ceil(n / 32), M), 256 threads: thread t < 32 sums row t's db,
+// warp w takes the norms of rows w, w + 8, ...
+__global__ void __launch_bounds__(256) center_coef_kernel(const float* __restrict__ e, const float* __restrict__ db_part,
+                                                          int n_part, int n, int d, float floor, float part_scale,
+                                                          float* __restrict__ coef) {
+  __shared__ float sdb[kCenterCoefRows], snorm[kCenterCoefRows];
+  const int model = blockIdx.y, j0 = blockIdx.x * kCenterCoefRows;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x < kCenterCoefRows && j0 + threadIdx.x < n) {
+    const float* p = db_part + (long long)model * n_part * n + j0 + threadIdx.x;
+    float g = 0.f;
+    for (int k = 0; k < n_part; ++k) g += p[(long long)k * n];
+    sdb[threadIdx.x] = g * part_scale;
+  }
+  for (int r = warp; r < kCenterCoefRows; r += 8) {
+    if (j0 + r >= n) break;   // warp-uniform
+    const float* row = e + ((long long)model * n + j0 + r) * d;
+    float ss = 0.f;
+    for (int c = lane * 4; c < d; c += 128) {
+      const float4 v = *reinterpret_cast<const float4*>(row + c);
+      ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+    }
+    ss = warp_sum(ss);
+    if (lane == 0) {
+      const float nrm = sqrtf(ss);
+      snorm[r] = floor > 0.f && nrm < floor ? floor : nrm;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < kCenterCoefRows && j0 + threadIdx.x < n)
+    coef[(long long)model * n + j0 + threadIdx.x] = sdb[threadIdx.x] / snorm[threadIdx.x];
+}
+
+// part[m][chunk][c] = sum over the chunk's rows, in order, of coef[m][j] E[m][j][c]. Grid (ceil(d / 512), chunks, M),
+// 128 threads of four columns each.
+__global__ void __launch_bounds__(128) center_gemv_kernel(const float* __restrict__ e, const float* __restrict__ coef, int n,
+                                                          int d, float* __restrict__ part) {
+  const int model = blockIdx.z, chunk = blockIdx.y;
+  const int c = (blockIdx.x * 128 + threadIdx.x) * 4;
+  if (c >= d) return;
+  const int j0 = chunk * kCenterChunkRows, j1 = min(n, j0 + kCenterChunkRows);
+  const float* kp = coef + (long long)model * n;
+  const float* ep = e + (long long)model * n * d + c;
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 4
+  for (int j = j0; j < j1; ++j) {
+    const float k = __ldg(kp + j);
+    const float4 v = __ldg(reinterpret_cast<const float4*>(ep + (long long)j * d));
+    acc.x += k * v.x;
+    acc.y += k * v.y;
+    acc.z += k * v.z;
+    acc.w += k * v.w;
+  }
+  *reinterpret_cast<float4*>(part + ((long long)model * gridDim.y + chunk) * d + c) = acc;
+}
+
+// grad[m][c] = g_scale * sum_k g_part[m][k][c] - sum_chunk part[m][chunk][c] (both in index order); MODE_ADAM then
+// applies Adam to center / center_m / center_v, unless the step is bad (kBadWord, as bias_kernel).
+template <int MODE>
+__global__ void center_grad_kernel(const float* __restrict__ g_part, int n_gpart, float g_scale,
+                                   const float* __restrict__ part, int n_chunks, int M, int d, float* __restrict__ grad,
+                                   float* __restrict__ center, float* __restrict__ m, float* __restrict__ v, AdamHyper h,
+                                   const uint32_t* __restrict__ health) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)M * d) return;
+  const int model = int(i / d), c = int(i - (long long)model * d);
+  const float* gp = g_part + (long long)model * n_gpart * d + c;
+  float gs = 0.f;
+  for (int k = 0; k < n_gpart; ++k) gs += gp[(long long)k * d];
+  const float* pp = part + (long long)model * n_chunks * d + c;
+  float dw = 0.f;
+  for (int k = 0; k < n_chunks; ++k) dw += pp[(long long)k * d];
+  const float g = gs * g_scale - dw;
+  grad[i] = g;
+  if (MODE == MODE_ADAM) {
+    if (step_is_bad(health)) return;
+    float mm = m[i], vv = v[i];
+    center[i] = adam_apply(center[i], g, mm, vv, h);
     m[i] = mm;
     v[i] = vv;
   }

@@ -40,13 +40,15 @@ from .tracing import nvtx_range
 Tensor = torch.Tensor
 
 _VARIANT_CODE = {"tied": _lib.SCE_TIED, "masked_tied": _lib.SCE_TIED, "untied": _lib.SCE_UNTIED,
-                 "masked_untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK}
+                 "masked_untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK,
+                 "tied_learned_center": _lib.SCE_TIED_LEARNED_CENTER}
 _LOSS_KEYS = {
     "tied": ("loss", "l_reconstruction", "l_l1"),
     "masked_tied": ("loss", "l_reconstruction", "l_l1"),
     "masked_untied": ("loss", "l_reconstruction", "l_l1"),
     "untied": ("loss", "l_reconstruction", "l_l1", "l_bias_decay"),
     "topk": ("loss",),
+    "tied_learned_center": ("loss", "l_reconstruction", "l_l1"),
 }
 
 
@@ -194,7 +196,8 @@ class FunctionalEnsemble:
         if variant not in _VARIANT_CODE:
             raise NotImplementedError(
                 f"{getattr(self.sig, '__name__', self.sig)} has no engine variant: only the signatures of the sweep hot "
-                "path (FunctionalTiedSAE, FunctionalSAE, the Masked variants, TopKEncoder) are implemented in the "
+                "path (FunctionalTiedSAE, FunctionalTiedCenteredSAE, FunctionalSAE, the Masked variants, TopKEncoder) "
+                "are implemented in the "
                 "sm_90a engine, and there is deliberately no generic autograd fallback")
         self._variant = variant
         self._plan = None
@@ -289,6 +292,10 @@ class FunctionalEnsemble:
         if self._variant in ("untied", "masked_untied"):
             bufs.decoder = ptr(self.params["decoder"])
             bufs.decoder_m, bufs.decoder_v = ptr(mu["decoder"]), ptr(nu["decoder"])
+        if self._variant == "tied_learned_center":
+            # FunctionalTiedCenteredSAE: the centre is a parameter, trained by the engine with its Adam moments
+            bufs.center = ptr(self.params["center"])
+            bufs.center_m, bufs.center_v = ptr(mu["center"]), ptr(nu["center"])
         if self._variant in ("masked_tied", "masked_untied"):
             eb["coef_mask"] = self.buffers["coef_mask"].to(device=dev, dtype=torch.uint8).contiguous()
             bufs.coef_mask = eb["coef_mask"].data_ptr()
@@ -473,6 +480,9 @@ class FunctionalEnsemble:
                 _lib.check(_lib.load().sce_grads(self._plan, x.data_ptr(), B, ptr(self._main), ptr("encoder_bias"),
                                                  ptr("decoder"), self._out_losses.data_ptr(),
                                                  self._out_nnz.data_ptr(), self._stream()), "sce_grads")
+                if "center" in g:
+                    _lib.check(_lib.load().sce_read_center_grad(self._plan, g["center"].data_ptr(), self._stream()),
+                               "sce_read_center_grad")
             return g, self._results(B)
 
     def calc_grads(self, params, buffers, minibatches):

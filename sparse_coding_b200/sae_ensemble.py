@@ -2,6 +2,7 @@
 
     FunctionalSAE            untied encoder/decoder        sae_ensemble.py:13-78
     FunctionalTiedSAE        tied, optional centring       sae_ensemble.py:81-162
+    FunctionalTiedCenteredSAE tied, learned centre         sae_ensemble.py:164-230
     FunctionalMaskedTiedSAE  tied, per-model dict size     sae_ensemble.py:309-373
     FunctionalMaskedSAE      untied, per-model dict size   sae_ensemble.py:377-444
 
@@ -105,6 +106,45 @@ class FunctionalTiedSAE(DictSignature):
         return engine_loss(FunctionalTiedSAE, params, buffers, batch)
 
 
+class FunctionalTiedCenteredSAE(DictSignature):
+    """A tied SAE on ``x - center``, the centre a trained parameter (a learned pre-encoder bias): loss
+    ``mean((x̂_c - x_c)^2) + l1_alpha * mean_b sum_n |c|`` with ``x_c = x - center``, no bias decay. The engine computes
+    the centre's gradient ``sum_b g_b - db W`` and updates it with Adam like the other parameters."""
+    variant = "tied_learned_center"
+
+    @staticmethod
+    def init(activation_size, n_dict_components, l1_alpha, center=None, device=None, dtype=None):
+        params = {}
+        buffers = {}
+        # the reference's order (zero centre, then the xavier encoder, then the zero bias): seeded init is bitwise its own
+        params["center"] = torch.zeros(activation_size, device=device, dtype=dtype) if center is None else center
+        params["encoder"] = _xavier(n_dict_components, activation_size, device, dtype)
+        params["encoder_bias"] = torch.zeros((n_dict_components,), device=device, dtype=dtype)
+        buffers["l1_alpha"] = torch.tensor(l1_alpha, device=device, dtype=dtype)
+        return params, buffers
+
+    @staticmethod
+    def to_learned_dict(params, buffers):
+        return TiedSAE(params["encoder"], params["encoder_bias"], centering=(params["center"], None, None),
+                       norm_encoder=True)
+
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["encoder"], NORM_FLOOR, None
+
+    @staticmethod
+    def center(params, batch):
+        return batch - params["center"][None, :]
+
+    @staticmethod
+    def uncenter(params, batch):
+        return batch + params["center"][None, :]
+
+    @staticmethod
+    def loss(params, buffers, batch):
+        return engine_loss(FunctionalTiedCenteredSAE, params, buffers, batch)
+
+
 def _mask_buffers(n_dict_components, n_components_stack, l1_alpha, bias_decay, device, dtype):
     mask = torch.ones(n_components_stack, device=device, dtype=torch.bool)
     mask[:n_dict_components] = False
@@ -173,5 +213,5 @@ class FunctionalMaskedSAE(DictSignature):
         return engine_loss(FunctionalMaskedSAE, params, buffers, batch)
 
 
-for _cls in (FunctionalSAE, FunctionalTiedSAE, FunctionalMaskedTiedSAE, FunctionalMaskedSAE):
+for _cls in (FunctionalSAE, FunctionalTiedSAE, FunctionalTiedCenteredSAE, FunctionalMaskedTiedSAE, FunctionalMaskedSAE):
     _cls.__module__ = _REF_MODULE

@@ -24,7 +24,12 @@ extern "C" {
 
 /* 201 also covers the additive extension for FunctionalTiedCenteredSAE: the enum value SCE_TIED_LEARNED_CENTER, the
  * center / center_m / center_v fields appended to sce_buffers, and sce_read_center_grad. Nothing earlier moved, so a
- * caller built against the earlier 201 header keeps working unchanged. */
+ * caller built against the earlier 201 header keeps working unchanged.
+ * 201 also covers the additive extension for FunctionalPositiveTiedSAE: encoder_nonneg and input_shift appended to the
+ * descriptor struct; the signature is SCE_TIED plus these two fields, as the masked variants are SCE_TIED plus coef_mask.
+ * Zero in both is the earlier behaviour. Unlike the extension above, this one lengthens the descriptor, and the library
+ * reads both fields: a caller compiled against the earlier 201 header passes a shorter struct and must be rebuilt (with
+ * the two fields zeroed) before it uses this library. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -37,7 +42,8 @@ typedef enum sce_status {
 
 /* Which reference signature the plan reproduces. */
 typedef enum sce_variant {
-  SCE_TIED = 0,   /* FunctionalTiedSAE.loss   (sae_ensemble.py:135-162); + coef_mask = FunctionalMaskedTiedSAE (:347-373) */
+  SCE_TIED = 0,   /* FunctionalTiedSAE.loss   (sae_ensemble.py:135-162); + coef_mask = FunctionalMaskedTiedSAE (:347-373);
+                     + desc.encoder_nonneg = 1, input_shift = 0.18 = FunctionalPositiveTiedSAE (mlp_tests.py:68-125) */
   SCE_UNTIED = 1, /* FunctionalSAE.loss       (sae_ensemble.py:53-78);   + coef_mask = FunctionalMaskedSAE     (:418-444) */
   SCE_TOPK = 2,   /* TopKEncoder.loss         (topk_encoder.py:29-40) */
   SCE_TIED_LEARNED_CENTER = 3 /* FunctionalTiedCenteredSAE.loss, sae_ensemble.py:204-230: tied, on x - center[m] with the
@@ -84,6 +90,16 @@ typedef struct sce_desc {
                            x_c[m] = (rot[m] (x - trans[m])) * scale[m]. 0 = off (identity centring); 1 = the batch is one
                            [B,d] array shared by all models; 2 = [M,B,d]. Needs x_per_model = 1 (the centred batch differs per
                            model) and the three center_* buffers. */
+  int encoder_nonneg;   /* SCE_TIED only, 0 or 1. 1: the dictionary is built from the encoder clamped at 0,
+                           W = max(E, 0) / max(||max(E, 0)||, norm_floor) (mlp_tests.py:100-102). The encoder gradient is
+                           the one with respect to max(E, 0), applied to E without an [E >= 0] mask (straight-through, as
+                           the reference's loss gives it); Adam updates the raw E, so negative entries keep moving. */
+  float input_shift;    /* SCE_TIED only; not with centering. Non-zero: the plan encodes and reconstructs x + input_shift
+                           (fp32 add, once per step on the batch as the caller laid it out; mlp_tests.py:104, :110), so
+                           the f16f8 range checks judge the shifted values and sce_forward's x_hat is in the shifted
+                           space (x_hat - input_shift reconstructs x). Neither field is allowed with coef_mask, nor in
+                           sce_forward_stats / sce_forward_fragments (exports of such dictionaries are plain TiedSAE
+                           objects of the raw encoder, evaluated as such). */
 } sce_desc;
 
 /* Device pointers owned by the caller; all fp32 unless noted. Unused ones are NULL. */
@@ -149,7 +165,8 @@ int sce_step_host(sce_plan* plan, const float* x_host, int B, float* out_losses_
 
 /* Forward only (evaluation; LearnedDict.predict semantics on already-centred inputs): writes x_hat
  * [M,B,d] fp32 if non-NULL and the same losses / nnz as sce_step, without touching parameters. SCE_TIED_LEARNED_CENTER:
- * x_hat is in the centred space (x_hat + center[m] is the reconstruction of x). */
+ * x_hat is in the centred space (x_hat + center[m] is the reconstruction of x). desc.input_shift != 0: x_hat is in the
+ * shifted space (x_hat - input_shift is the reconstruction of x). */
 int sce_forward(sce_plan* plan, const float* x, int B, float* x_hat, float* out_losses, float* out_nnz,
                 void* stream);
 
@@ -234,7 +251,8 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream);
  *                B = 4096: 64 MiB). sce_forward_stats_workspace_bytes is host-only; it returns 0 for an invalid
  *                desc or B outside [1, batch_max].
  * Not available for SCE_TIED_LEARNED_CENTER (the size query returns 0, the call SCE_ERR_INVALID): evaluate its exported
- * dictionaries, which are TiedSAE objects with the centre as their translation.
+ * dictionaries, which are TiedSAE objects with the centre as their translation. Nor with desc.encoder_nonneg or
+ * desc.input_shift set (likewise): evaluate the exported TiedSAE of the raw encoder.
  * x_hat, out_losses and out_nnz are those of sce_forward (x_hat optional). Asynchronous on `stream`. */
 size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B);
 int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
@@ -267,7 +285,7 @@ int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_ph
  *                M (B/L) n (4 + 1) bytes, and M n int32 (config 2, M = 16, n = 4096, B = 8192, L = 64: 40 MiB).
  *                sce_fragments_workspace_bytes is host-only; it returns 0 for an invalid desc, B outside
  *                [1, batch_max] or an invalid L.
- * Not available for SCE_TIED_LEARNED_CENTER, as sce_forward_stats.
+ * Not available for SCE_TIED_LEARNED_CENTER, nor with desc.encoder_nonneg or desc.input_shift, as sce_forward_stats.
  * Deterministic (no atomics) and asynchronous on `stream`. */
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L);
 int sce_forward_fragments(sce_plan* plan, const float* x, int B, int L, long long frag0, int n_top, int n_random,

@@ -40,6 +40,7 @@ class SceDesc(C.Structure):
         ("lr", C.c_float), ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("eps_root", C.c_float),
         ("adam_count_mode", C.c_int), ("fwd_passes", C.c_int), ("bwd_passes", C.c_int), ("norm_floor", C.c_float),
         ("arith", C.c_int), ("topk_k_max", C.c_int), ("centering", C.c_int),
+        ("encoder_nonneg", C.c_int), ("input_shift", C.c_float),
     ]
 
 

@@ -14,6 +14,9 @@
 // Learned-centre variant (tied in every other respect): center_sub_kernel forms x - center[m] first, the decode epilogue
 // also writes column sums of g, and before the Adam update three kernels form the centre gradient sum_b g - db W
 // (center_coef / center_gemv / center_grad) and update the centre.
+// Non-negative tied plans (desc.encoder_nonneg, desc.input_shift; FunctionalPositiveTiedSAE) are tied plans whose batch
+// split also forms x + input_shift, and whose dict_rows kernels build the dictionary from max(E, 0).
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -109,6 +112,7 @@ struct PlanBuffers {
   // learned centre: column sums of g [M, tiles_m*4, d] (EpiDecodeT<AR, true>), db / ||E_n|| [M, n], the GEMV partials
   // [M, ceil(n / kCenterChunkRows), d] and the centre gradient [M, d] (sce_read_center_grad)
   float *g_part, *center_coef, *center_part, *center_grad;
+  float* x_shifted;               // input_shift: x + input_shift [xm, B, d], written by the batch split
   float* scores;                  // top-k: fp32 scores [M, Bmax, n] of the encode GEMM
   int* tk_models;                 // top-k gather kernel: the models sorted into k classes (device copy of tk_group_models)
   uint32_t* tk_cmax;              // top-k: largest key per 32-column chunk of the scores [M, Bmax, n_chunks] (EpiScoresTma)
@@ -132,6 +136,8 @@ struct PlanConfig {
   bool dw_native;      // the weight gradient's cross terms run on E5M2 wgmma from batch-major copies (carve)
   bool split_decode;   // separate accumulators for hi*hi and the cross terms in the decode GEMM (bf16x3)
   bool use_graph;      // replay the step as a CUDA graph
+  bool nonneg;         // desc.encoder_nonneg: the dictionary rows are built from max(E, 0) (dict_rows_kernel<..., true>)
+  bool shift;          // desc.input_shift != 0: the batch split also writes x + input_shift, which the step reads
 };
 
 struct sce_plan : PlanBuffers {
@@ -197,6 +203,12 @@ static int validate(const sce_desc* d) {
   if (d->centering && !d->x_per_model) return fail(SCE_ERR_INVALID, "centering needs x_per_model = 1 (the centred batch differs per model)");
   if (d->centering && d->variant == SCE_TIED_LEARNED_CENTER)
     return fail(SCE_ERR_INVALID, "the learned-centre variant centres the batch itself: desc.centering must be 0");
+  if (d->encoder_nonneg != 0 && d->encoder_nonneg != 1) return fail(SCE_ERR_INVALID, "encoder_nonneg must be 0 or 1");
+  if (!std::isfinite(d->input_shift)) return fail(SCE_ERR_INVALID, "input_shift must be finite");
+  if ((d->encoder_nonneg || d->input_shift != 0.f) && d->variant != SCE_TIED)
+    return fail(SCE_ERR_INVALID, "encoder_nonneg / input_shift are defined for SCE_TIED only (variant %d)", d->variant);
+  if (d->input_shift != 0.f && d->centering)
+    return fail(SCE_ERR_INVALID, "input_shift cannot be combined with centering");
   if (d->arith < SCE_ARITH_AUTO || d->arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "unknown arith %d", d->arith);
   if (d->arith == SCE_ARITH_F16F8 && (d->d % 16 || d->n % 16))
     return fail(SCE_ERR_INVALID, "arith = F16F8 needs d (%d) and n (%d) to be multiples of 16 (TMA pitch of the 8-bit planes)",
@@ -232,11 +244,16 @@ static int query_device(int* device, int* sm_count) {
   return SCE_OK;
 }
 
-// fp32 rows -> the operand planes of arithmetic AR: n4 float4s, grid-stride over at most 2048 blocks
+// fp32 rows -> the operand planes of arithmetic AR: n4 float4s, grid-stride over at most 2048 blocks. With `xs`, the
+// rows are shifted by `shift` first and the shifted fp32 rows are written to `xs` as well (input_shift plans).
 template <int AR>
-static void launch_split_rows(const float* x, const Planes& w, long long n4, uint32_t* flags, cudaStream_t st) {
+static void launch_split_rows(const float* x, const Planes& w, long long n4, uint32_t* flags, cudaStream_t st,
+                              float shift = 0.f, float* xs = nullptr) {
   const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags);
+  if (xs)
+    split_rows_kernel<AR, true><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags, shift, xs);
+  else
+    split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags, 0.f, nullptr);
 }
 
 // SCE_ARITH=bf16x3|f16f8: the arithmetic the environment pins arith = AUTO to (include/sce.h), else SCE_ARITH_AUTO
@@ -302,6 +319,8 @@ static PlanConfig plan_config(const sce_desc& d) {
   // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
   // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
   c.split_decode = d.n > 4096;
+  c.nonneg = d.encoder_nonneg != 0;
+  c.shift = d.input_shift != 0.f;
   return c;
 }
 
@@ -383,6 +402,7 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
     w.center_part = c.take<float>(M * ((n + kCenterChunkRows - 1) / kCenterChunkRows) * dd);
     w.center_grad = c.take<float>(M * dd);
   }
+  if (cfg.shift) w.x_shifted = c.take<float>(xm * B * dd);
   w.res_flags = c.take<uint32_t>(kFlagWords);   // [0] residual flag, [kAbsmaxWord] input range monitor, [kBadWord] health (separate 128-byte lines)
   return align_up(c.off, 1024);
 }
@@ -566,22 +586,22 @@ static AdamHyper hyper_for(const sce_plan* p, long long t) {
   return h;
 }
 
-template <int MODE, int ARITH>
+template <int MODE, int ARITH, bool NONNEG = false>
 static int launch_dict_rows_t(float* e, const float* dw, float* m, float* v, const Planes& w, float* grad_out,
                               long long rows, int d, int normalize, float floor, AdamHyper h, const uint32_t* health,
                               float* w_f32, cudaStream_t st) {
   void *const hi = w.hi, *const lo = w.lo, *const x8 = w.x8;
   const int nv = (d + 511) / 512;
   if (nv == 1)
-    dict_rows_kernel<1, MODE, ARITH><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
+    dict_rows_kernel<1, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
   else if (nv == 2)
-    dict_rows_kernel<2, MODE, ARITH><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
+    dict_rows_kernel<2, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
   else if (nv <= 4)
-    dict_rows_kernel<4, MODE, ARITH><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
+    dict_rows_kernel<4, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
   else if (nv <= 8)    // d <= 4096 (Pythia-6.9b residual width)
-    dict_rows_kernel<8, MODE, ARITH><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
+    dict_rows_kernel<8, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
   else                 // d <= 8192
-    dict_rows_kernel<16, MODE, ARITH><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
+    dict_rows_kernel<16, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }
@@ -615,9 +635,15 @@ static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_ou
   float* v = MODE == MODE_ADAM ? s.v : nullptr;
   const Planes w = MODE == MODE_GRAD ? Planes{} : s.planes;
   float* wf = (MODE != MODE_GRAD && p->cfg.topk_sparse) ? p->wn_f32 : nullptr;   // (top-k plans have one dictionary)
-  return p->cfg.arith == kArithF16F8
-             ? launch_dict_rows_t<MODE, kArithF16F8>(s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st)
-             : launch_dict_rows_t<MODE, kArithBf16x3>(s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
+  auto run = [&](auto arith, auto nonneg) {
+    return launch_dict_rows_t<MODE, decltype(arith)::value, decltype(nonneg)::value>(
+        s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
+  };
+  using F8 = std::integral_constant<int, kArithF16F8>;
+  using B3 = std::integral_constant<int, kArithBf16x3>;
+  if (p->cfg.nonneg)   // (tied plans only: one dictionary, normalised)
+    return p->cfg.arith == kArithF16F8 ? run(F8{}, std::true_type{}) : run(B3{}, std::true_type{});
+  return p->cfg.arith == kArithF16F8 ? run(F8{}, std::false_type{}) : run(B3{}, std::false_type{});
 }
 
 // f16f8: the decoder's planes -> their transposed copy, which the decode GEMM reads K-major (nothing to do where the
@@ -706,13 +732,16 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     ++launches;
     x = p->x_centered;
   }
-  // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace
+  // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace. input_shift (mlp_tests.py:104): the split
+  // forms x + shift once, as the caller laid the batch out, and every kernel below reads that shifted batch
   if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), st));
   for (int m = 0; m < cfg.xm; ++m) {
-    launch_split_rows<AR>(x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st);
+    launch_split_rows<AR>(x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st,
+                          d.input_shift, cfg.shift ? p->x_shifted + (long long)m * B * dd : nullptr);
     ++launches;
   }
   CUDA_TRY(cudaGetLastError());
+  if (cfg.shift) x = p->x_shifted;
   // dw_native: batch-major copies of the 8-bit planes of x, c and g for the weight gradient (dz's are written so by dcode)
   const bool tdw = f8 && backward && cfg.dw_native;
   auto batch_major = [&](const Planes& P, const Planes& T, int models, int cols) {
@@ -1391,6 +1420,8 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   if (desc->variant == SCE_TOPK && !b.sparsity) return fail(SCE_ERR_INVALID, "top-k variant needs the sparsity buffer");
   if (desc->variant == SCE_TIED_LEARNED_CENTER && (!b.center || !b.center_m || !b.center_v))
     return fail(SCE_ERR_INVALID, "the learned-centre variant needs center / center_m / center_v");
+  if (b.coef_mask && (desc->encoder_nonneg || desc->input_shift != 0.f))
+    return fail(SCE_ERR_INVALID, "encoder_nonneg / input_shift cannot be combined with coef_mask");
   const PlanConfig cfg = plan_config(*desc);
   rc = check_workspace(b.workspace, b.workspace_bytes, plan_workspace(*desc, cfg), "");
   if (rc) return rc;
@@ -1732,8 +1763,14 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
   return SCE_OK;
 }
 
+// Plans whose training forward differs from the export it evaluates as (sce_forward_stats / sce_forward_fragments): the
+// learned centre, and the non-negative tied plans, whose exports are TiedSAE objects of the raw encoder
+static bool training_only(const sce_desc& d) {
+  return d.variant == SCE_TIED_LEARNED_CENTER || d.encoder_nonneg || d.input_shift != 0.f;
+}
+
 size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || desc->variant == SCE_TIED_LEARNED_CENTER) return 0;
+  if (validate(desc) || B < 1 || B > desc->batch_max || training_only(*desc)) return 0;
   return stats_workspace(*desc, B);
 }
 
@@ -1741,9 +1778,9 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
                       float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
                       size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_stats: plan is NULL");
-  if (p->d.variant == SCE_TIED_LEARNED_CENTER)
-    return fail(SCE_ERR_INVALID, "forward_stats: not available for the learned-centre variant; evaluate its exported "
-                                 "dictionaries (TiedSAE)");
+  if (training_only(p->d))
+    return fail(SCE_ERR_INVALID, "forward_stats: not available for the learned-centre variant or with encoder_nonneg / "
+                                 "input_shift; evaluate the exported dictionaries (TiedSAE)");
   if (int rc = check_rows(p, B, "forward_stats: ")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "forward_stats: x is NULL");
   if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
@@ -1777,8 +1814,7 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
 }
 
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || desc->variant == SCE_TIED_LEARNED_CENTER)
-    return 0;
+  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || training_only(*desc)) return 0;
   return frag_workspace(*desc, B, L, nullptr, nullptr);
 }
 
@@ -1787,9 +1823,9 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_fragments: plan is NULL");
-  if (p->d.variant == SCE_TIED_LEARNED_CENTER)
-    return fail(SCE_ERR_INVALID, "forward_fragments: not available for the learned-centre variant; evaluate its exported "
-                                 "dictionaries (TiedSAE)");
+  if (training_only(p->d))
+    return fail(SCE_ERR_INVALID, "forward_fragments: not available for the learned-centre variant or with encoder_nonneg / "
+                                 "input_shift; evaluate the exported dictionaries (TiedSAE)");
   if (int rc = check_rows(p, B, "forward_fragments: ")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "forward_fragments: x is NULL");
   if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);

@@ -47,14 +47,21 @@ constexpr int kFlagWords = 128;
 __device__ __forceinline__ bool step_is_bad(const uint32_t* __restrict__ flags) {
   return flags != nullptr && *reinterpret_cast<const volatile uint32_t*>(flags + kBadWord) != 0u;
 }
-template <int ARITH>
+// SHIFT (input_shift plans): the planes are those of x + shift (fp32 add), and the shifted fp32 values are also written
+// to `xs`, the batch every later kernel of the step reads; the flags above judge the shifted values.
+template <int ARITH, bool SHIFT = false>
 __global__ void split_rows_kernel(const float* __restrict__ x, void* __restrict__ hi, void* __restrict__ lo,
-                                  void* __restrict__ x8, long long n4, uint32_t* __restrict__ res_flag) {
+                                  void* __restrict__ x8, long long n4, uint32_t* __restrict__ res_flag, float shift,
+                                  float* __restrict__ xs) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   uint32_t any = 0;
   float amax = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    const float4 v = reinterpret_cast<const float4*>(x)[i];
+    float4 v = reinterpret_cast<const float4*>(x)[i];
+    if constexpr (SHIFT) {
+      v = make_float4(v.x + shift, v.y + shift, v.z + shift, v.w + shift);
+      reinterpret_cast<float4*>(xs)[i] = v;
+    }
     const float vv[4] = {v.x, v.y, v.z, v.w};
     if constexpr (ARITH == kArithF16F8) {
       amax = fmaxf(fmaxf(amax, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
@@ -208,11 +215,25 @@ __device__ __forceinline__ float adam_apply(float p, float g, float& m, float& v
 //   MODE_GRAD    : de = J(dw) -> grad_out                                         (sce_grads)
 // J is the Jacobian of the row normalisation, de = (dw - w <w, dw>) / s (sae_ensemble.py:136-137
 // differentiated); with `normalize == 0` (untied encoder) J = I and the split is of e itself.
+// NONNEG (desc.encoder_nonneg, mlp_tests.py:100-102): the norm, w, J and the emitted planes use e+ = max(e, 0), formed
+// in place from the raw row as it is read; de = J(dw) is the gradient with respect to e+, which MODE_GRAD returns and
+// MODE_ADAM applies to the raw e, read again for the update (straight-through: no [e >= 0] mask, as the reference's
+// gradient).
 // NV = ceil(d / 512) float4 per thread.
 // ------------------------------------------------------------------------------------------------
 enum { MODE_PREPARE = 0, MODE_ADAM = 1, MODE_GRAD = 2 };
 
-template <int NV, int MODE, int ARITH>
+__device__ __forceinline__ float4 nonneg4(const float4& e) {
+  return make_float4(fmaxf(e.x, 0.f), fmaxf(e.y, 0.f), fmaxf(e.z, 0.f), fmaxf(e.w, 0.f));
+}
+// NONNEG rows: the sum of squares in explicitly rounded steps, so that the norm MODE_ADAM re-splits the updated row with
+// and the one MODE_PREPARE derives from the same row are bitwise equal (a resumed run prepares its planes afresh), which
+// free contraction of the two loops does not guarantee
+__device__ __forceinline__ float sumsq4_rn(const float4& v) {
+  return __fmaf_rn(v.w, v.w, __fmaf_rn(v.z, v.z, __fmaf_rn(v.y, v.y, __fmul_rn(v.x, v.x))));
+}
+
+template <int NV, int MODE, int ARITH, bool NONNEG = false>
 __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, const float* __restrict__ dw,
                                                         float* __restrict__ m, float* __restrict__ v,
                                                         void* __restrict__ w_hi, void* __restrict__ w_lo,
@@ -234,8 +255,10 @@ __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, c
     if (c < d) {
       ev[i] = *reinterpret_cast<const float4*>(e + base + c);
       if (MODE != MODE_PREPARE) gv[i] = *reinterpret_cast<const float4*>(dw + base + c);
+      if constexpr (NONNEG) ev[i] = nonneg4(ev[i]);
     }
-    ss += ev[i].x * ev[i].x + ev[i].y * ev[i].y + ev[i].z * ev[i].z + ev[i].w * ev[i].w;
+    if constexpr (NONNEG) ss = __fadd_rn(ss, sumsq4_rn(ev[i]));
+    else ss += ev[i].x * ev[i].x + ev[i].y * ev[i].y + ev[i].z * ev[i].z + ev[i].w * ev[i].w;
     dot += ev[i].x * gv[i].x + ev[i].y * gv[i].y + ev[i].z * gv[i].z + ev[i].w * gv[i].w;
   }
   float s = 1.f;
@@ -273,6 +296,7 @@ __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, c
       if (c < d) {
         float4 mv = *reinterpret_cast<const float4*>(m + base + c);
         float4 vv = *reinterpret_cast<const float4*>(v + base + c);
+        if constexpr (NONNEG) ev[i] = *reinterpret_cast<const float4*>(e + base + c);   // Adam moves the raw entries
         ev[i].x = adam_apply(ev[i].x, gv[i].x, mv.x, vv.x, h);
         ev[i].y = adam_apply(ev[i].y, gv[i].y, mv.y, vv.y, h);
         ev[i].z = adam_apply(ev[i].z, gv[i].z, mv.z, vv.z, h);
@@ -280,7 +304,12 @@ __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, c
         *reinterpret_cast<float4*>(m + base + c) = mv;
         *reinterpret_cast<float4*>(v + base + c) = vv;
         *reinterpret_cast<float4*>(e + base + c) = ev[i];
-        ss2 += ev[i].x * ev[i].x + ev[i].y * ev[i].y + ev[i].z * ev[i].z + ev[i].w * ev[i].w;
+        if constexpr (NONNEG) {
+          ev[i] = nonneg4(ev[i]);
+          ss2 = __fadd_rn(ss2, sumsq4_rn(ev[i]));
+        } else {
+          ss2 += ev[i].x * ev[i].x + ev[i].y * ev[i].y + ev[i].z * ev[i].z + ev[i].w * ev[i].w;
+        }
       }
     }
     if (normalize) {

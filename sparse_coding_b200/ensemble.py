@@ -41,7 +41,9 @@ Tensor = torch.Tensor
 
 _VARIANT_CODE = {"tied": _lib.SCE_TIED, "masked_tied": _lib.SCE_TIED, "untied": _lib.SCE_UNTIED,
                  "masked_untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK,
-                 "tied_learned_center": _lib.SCE_TIED_LEARNED_CENTER}
+                 "tied_learned_center": _lib.SCE_TIED_LEARNED_CENTER, "positive_tied": _lib.SCE_TIED}
+# FunctionalPositiveTiedSAE encodes and reconstructs x + 0.18 (autoencoders/mlp_tests.py:104, :110)
+_POSITIVE_TIED_SHIFT = 0.18
 _LOSS_KEYS = {
     "tied": ("loss", "l_reconstruction", "l_l1"),
     "masked_tied": ("loss", "l_reconstruction", "l_l1"),
@@ -49,6 +51,7 @@ _LOSS_KEYS = {
     "untied": ("loss", "l_reconstruction", "l_l1", "l_bias_decay"),
     "topk": ("loss",),
     "tied_learned_center": ("loss", "l_reconstruction", "l_l1"),
+    "positive_tied": ("loss", "l_reconstruction", "l_l1", "l_bias_decay"),
 }
 
 
@@ -196,8 +199,8 @@ class FunctionalEnsemble:
         if variant not in _VARIANT_CODE:
             raise NotImplementedError(
                 f"{getattr(self.sig, '__name__', self.sig)} has no engine variant: only the signatures of the sweep hot "
-                "path (FunctionalTiedSAE, FunctionalTiedCenteredSAE, FunctionalSAE, the Masked variants, TopKEncoder) "
-                "are implemented in the "
+                "path (FunctionalTiedSAE, FunctionalTiedCenteredSAE, FunctionalPositiveTiedSAE, FunctionalSAE, the "
+                "Masked variants, TopKEncoder) are implemented in the "
                 "sm_90a engine, and there is deliberately no generic autograd fallback")
         self._variant = variant
         self._plan = None
@@ -259,6 +262,7 @@ class FunctionalEnsemble:
                 self.params[k] = v.contiguous()
         self._destroy_plan()
         cfg: AdamConfig = self.optimizer
+        positive = self._variant == "positive_tied"   # tied on max(E, 0) and x + 0.18 (sce_desc.encoder_nonneg / input_shift)
         desc = _lib.SceDesc(
             variant=_VARIANT_CODE[self._variant], n_models=self.n_models, d=self._d, n=self._n,
             batch_max=batch_max, x_per_model=int(x_per_model), lr=cfg.lr, beta1=cfg.b1, beta2=cfg.b2, eps=cfg.eps,
@@ -268,7 +272,8 @@ class FunctionalEnsemble:
             norm_floor=0.0 if self._variant == "topk" else 1e-8,
             arith=_lib.ARITH_CODE[getattr(self, "_arith_fallback", None) or getattr(self, "arith", "auto")],
             topk_k_max=int(self.buffers["sparsity"].max()) if self._variant == "topk" else 0,
-            centering=centering)
+            centering=centering, encoder_nonneg=int(positive),
+            input_shift=_POSITIVE_TIED_SHIFT if positive else 0.0)
         eb = {}
 
         def f32vec(name):  # [M] fp32 hyper-parameter buffers
@@ -287,7 +292,7 @@ class FunctionalEnsemble:
             bufs.encoder_bias = ptr(self.params["encoder_bias"])
             bufs.bias_m, bufs.bias_v = ptr(mu["encoder_bias"]), ptr(nu["encoder_bias"])
             bufs.l1_alpha = f32vec("l1_alpha")
-            if self._variant in ("tied", "untied"):
+            if self._variant in ("tied", "untied", "positive_tied"):
                 bufs.bias_decay = f32vec("bias_decay")
         if self._variant in ("untied", "masked_untied"):
             bufs.decoder = ptr(self.params["decoder"])
@@ -458,7 +463,9 @@ class FunctionalEnsemble:
             self._health_action(rerun=None)
 
     def forward_batch(self, minibatches, expand_dims=True, return_x_hat=False):
-        """Forward only: losses and code statistics (and optionally x̂ [M,B,d]) without touching parameters."""
+        """Forward only: losses and code statistics (and optionally x̂ [M,B,d]) without touching parameters.
+        x̂ is in the space the signature reconstructs: FunctionalTiedCenteredSAE's centred space (x̂ + center[m]
+        reconstructs x) and FunctionalPositiveTiedSAE's shifted space (x̂ - 0.18 reconstructs x)."""
         with torch.no_grad():
             x, B = self._prep_batch(minibatches, expand_dims)
             x_hat = torch.empty(self.n_models, B, self._d, dtype=torch.float32, device=x.device) if return_x_hat else None

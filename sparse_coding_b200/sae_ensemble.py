@@ -3,6 +3,7 @@
     FunctionalSAE            untied encoder/decoder        sae_ensemble.py:13-78
     FunctionalTiedSAE        tied, optional centring       sae_ensemble.py:81-162
     FunctionalTiedCenteredSAE tied, learned centre         sae_ensemble.py:164-230
+    FunctionalPositiveTiedSAE tied, clamped encoder        mlp_tests.py:68-125
     FunctionalMaskedTiedSAE  tied, per-model dict size     sae_ensemble.py:309-373
     FunctionalMaskedSAE      untied, per-model dict size   sae_ensemble.py:377-444
 
@@ -145,6 +146,38 @@ class FunctionalTiedCenteredSAE(DictSignature):
         return engine_loss(FunctionalTiedCenteredSAE, params, buffers, batch)
 
 
+class FunctionalPositiveTiedSAE(DictSignature):
+    """A tied SAE on non-negative dictionary rows (reference: autoencoders/mlp_tests.py:68-125): the loss reads the
+    encoder clamped at 0, ``W = max(E, 0) / max(||max(E, 0)||, 1e-8)``, encodes and reconstructs ``x + 0.18``, and adds
+    bias decay: ``mean((x̂ - 0.18 - x)^2) + l1_alpha * mean_b sum_n |c| + bias_decay * ||b||``. As in the reference,
+    the encoder's gradient is taken with respect to the clamped encoder and applied to the raw one (straight-through),
+    so entries that went negative keep moving. The export is the reference's: a plain ``TiedSAE`` of the raw encoder,
+    with neither the clamp nor the shift, so an exported dictionary's FVU is not the training loss."""
+    variant = "positive_tied"
+
+    @staticmethod
+    def init(activation_size, n_dict_components, l1_alpha, bias_decay=0.0, device=None, dtype=None):
+        params = {}
+        buffers = {}
+        params["encoder"] = _xavier(n_dict_components, activation_size, device, dtype).abs()
+        params["encoder_bias"] = torch.full((n_dict_components,), -1.0, device=device, dtype=dtype)
+        buffers["l1_alpha"] = torch.tensor(l1_alpha, device=device, dtype=dtype)
+        buffers["bias_decay"] = torch.tensor(bias_decay, device=device, dtype=dtype)
+        return params, buffers
+
+    @staticmethod
+    def to_learned_dict(params, buffers):
+        return TiedSAE(params["encoder"], params["encoder_bias"], norm_encoder=True)
+
+    @staticmethod
+    def learned_dict_stack(params, buffers):
+        return params["encoder"], NORM_FLOOR, None
+
+    @staticmethod
+    def loss(params, buffers, batch):
+        return engine_loss(FunctionalPositiveTiedSAE, params, buffers, batch)
+
+
 def _mask_buffers(n_dict_components, n_components_stack, l1_alpha, bias_decay, device, dtype):
     mask = torch.ones(n_components_stack, device=device, dtype=torch.bool)
     mask[:n_dict_components] = False
@@ -215,3 +248,4 @@ class FunctionalMaskedSAE(DictSignature):
 
 for _cls in (FunctionalSAE, FunctionalTiedSAE, FunctionalTiedCenteredSAE, FunctionalMaskedTiedSAE, FunctionalMaskedSAE):
     _cls.__module__ = _REF_MODULE
+FunctionalPositiveTiedSAE.__module__ = "autoencoders.mlp_tests"

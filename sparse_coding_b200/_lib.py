@@ -7,8 +7,11 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from dataclasses import dataclass
 
 import torch
+
+from .optim import AdamConfig
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # SCE_LIB: an alternative build of the same library (kernel A/B experiments)
@@ -54,6 +57,82 @@ class SceBuffers(C.Structure):
         ("center_trans", C.c_void_p), ("center_rot", C.c_void_p), ("center_scale", C.c_void_p),
         ("center", C.c_void_p), ("center_m", C.c_void_p), ("center_v", C.c_void_p),
     ]
+
+
+@dataclass(frozen=True)
+class EngineSignature:
+    """What one engine-backed signature (``DictSignature.variant``) puts into ``SceDesc`` / ``SceBuffers``."""
+    variant: int                 # sce_variant
+    main: str                    # the parameter the engine trains as its (first) dictionary
+    loss_keys: tuple             # the loss columns it reports (of "loss", "l_reconstruction", "l_l1", "l_bias_decay")
+    decoder: bool = False        # a separate decoder (untied)
+    bias_decay: bool = False     # the engine adds buffers["bias_decay"] to the loss
+    learned_center: bool = False   # params["center"], trained with its Adam moments
+    centering: bool = False      # FunctionalTiedSAE's centring buffers (center_trans / center_rot / center_scale)
+    encoder_nonneg: bool = False   # the dictionary is max(E, 0)
+    input_shift: float = 0.0     # encode and reconstruct x + input_shift
+    norm_floor: float = 1e-8     # clamp of the dictionary's row norms (0: none)
+    topk: bool = False           # buffers["sparsity"] holds each model's k; no bias, no sparsity penalty
+
+
+_SAE_LOSSES = ("loss", "l_reconstruction", "l_l1")
+SIGNATURES = {
+    "tied": EngineSignature(SCE_TIED, "encoder", _SAE_LOSSES, bias_decay=True, centering=True),
+    "masked_tied": EngineSignature(SCE_TIED, "encoder", _SAE_LOSSES),
+    "untied": EngineSignature(SCE_UNTIED, "encoder", _SAE_LOSSES + ("l_bias_decay",), decoder=True, bias_decay=True),
+    "masked_untied": EngineSignature(SCE_UNTIED, "encoder", _SAE_LOSSES, decoder=True),
+    "topk": EngineSignature(SCE_TOPK, "dict", ("loss",), norm_floor=0.0, topk=True),
+    "tied_learned_center": EngineSignature(SCE_TIED_LEARNED_CENTER, "encoder", _SAE_LOSSES, learned_center=True),
+    # FunctionalPositiveTiedSAE encodes and reconstructs x + 0.18 (autoencoders/mlp_tests.py:104, :110)
+    "positive_tied": EngineSignature(SCE_TIED, "encoder", _SAE_LOSSES + ("l_bias_decay",), bias_decay=True,
+                                     encoder_nonneg=True, input_shift=0.18),
+}
+
+
+def plan_structs(sig: EngineSignature, params, buffers, mu, nu, *, batch_max: int, x_per_model: bool, centering: int,
+                 adam: AdamConfig, adam_count_mode: str, fwd_passes: int, bwd_passes: int, arith: str):
+    """``(SceDesc, SceBuffers, keep)`` of a plan of ``sig`` over the stacked ``params`` / ``buffers`` and the Adam moments
+    ``mu`` / ``nu`` (keyed like ``params``); a ``coef_mask`` in ``buffers`` is applied whatever the signature (padding
+    rows). ``keep`` holds the buffers as the engine reads them, by name; it and the tensors passed must outlive the plan.
+    Reads only ``data_ptr()``: no CUDA call."""
+    keep = {}
+
+    def converted(name, dtype):
+        if name not in buffers:
+            return None
+        keep[name] = buffers[name].to(dtype=dtype).contiguous()
+        return keep[name].data_ptr()
+
+    def param(name):   # a parameter and its Adam moments
+        return params[name].data_ptr(), mu[name].data_ptr(), nu[name].data_ptr()
+
+    main = params[sig.main]
+    desc = SceDesc(
+        variant=sig.variant, n_models=main.shape[0], d=main.shape[2], n=main.shape[1], batch_max=batch_max,
+        x_per_model=int(x_per_model), lr=adam.lr, beta1=adam.b1, beta2=adam.b2, eps=adam.eps, eps_root=adam.eps_root,
+        adam_count_mode=SCE_ADAM_FROZEN_T1 if adam_count_mode == "frozen_t1" else SCE_ADAM_STANDARD,
+        fwd_passes=fwd_passes, bwd_passes=bwd_passes, norm_floor=sig.norm_floor, arith=arith_code(arith),
+        centering=centering, encoder_nonneg=int(sig.encoder_nonneg), input_shift=sig.input_shift)
+    bufs = SceBuffers()
+    bufs.encoder, bufs.encoder_m, bufs.encoder_v = param(sig.main)
+    if sig.topk:
+        bufs.sparsity = converted("sparsity", torch.int64)
+        desc.topk_k_max = int(keep["sparsity"].max())
+    else:
+        bufs.encoder_bias, bufs.bias_m, bufs.bias_v = param("encoder_bias")
+        bufs.l1_alpha = converted("l1_alpha", torch.float32)
+        if sig.bias_decay:
+            bufs.bias_decay = converted("bias_decay", torch.float32)
+    if sig.decoder:
+        bufs.decoder, bufs.decoder_m, bufs.decoder_v = param("decoder")
+    if sig.learned_center:
+        bufs.center, bufs.center_m, bufs.center_v = param("center")
+    bufs.coef_mask = converted("coef_mask", torch.uint8)
+    if centering:
+        # FunctionalTiedSAE.center (sae_ensemble.py:126-128) runs on the device: (x - trans) planes, GEMM with rot, * scale
+        bufs.center_trans, bufs.center_rot, bufs.center_scale = (converted(k, torch.float32) for k in
+                                                                 ("center_trans", "center_rot", "center_scale"))
+    return desc, bufs, keep
 
 
 class SceError(RuntimeError):

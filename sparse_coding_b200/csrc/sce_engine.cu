@@ -128,7 +128,13 @@ struct PlanBuffers {
 // What a plan decides from its descriptor, once (plan_config): the workspace carve and every launch follow from it
 struct PlanConfig {
   int arith;           // kArithBf16x3 or kArithF16F8
+  bool untied;         // SCE_UNTIED: a decoder of its own, a second dictionary side
+  bool topk;           // SCE_TOPK
+  bool learned;        // SCE_TIED_LEARNED_CENTER: the step centres the batch on params["center"] and trains the centre
+  bool x_models;       // the batch the kernels read holds one slab per model (x_per_model, or always with a learned centre)
   int xm;              // number of distinct input batches (1 shared, or M)
+  int input_models;    // models' worth of rows in the caller's batch: 1 when it is shared ([B,d]; also centering = 1), else M
+  bool evaluable;      // the forward-only passes may run it: not plans whose export (a TiedSAE) differs from their forward
   int bpad;            // Bp: batch_max rounded up to 16 (TMA pitch of the batch-major 8-bit planes)
   int tk_kmax;         // top-k list capacity per row (desc.topk_k_max rounded up to 8; 0: no lists)
   int tk_slices;       // slices of the activation width topk_sparse_kernel runs per row (0: none fits)
@@ -137,7 +143,7 @@ struct PlanConfig {
   bool split_decode;   // separate accumulators for hi*hi and the cross terms in the decode GEMM (bf16x3)
   bool use_graph;      // replay the step as a CUDA graph
   bool nonneg;         // desc.encoder_nonneg: the dictionary rows are built from max(E, 0) (dict_rows_kernel<..., true>)
-  bool shift;          // desc.input_shift != 0: the batch split also writes x + input_shift, which the step reads
+  float shift;         // desc.input_shift; non-zero: the batch split also writes x + shift, which the step reads
 };
 
 struct sce_plan : PlanBuffers {
@@ -293,12 +299,20 @@ static int topk_slices(const sce_desc& d, size_t kmax) {
 static PlanConfig plan_config(const sce_desc& d) {
   PlanConfig c{};
   c.arith = resolve_arith(d);
+  c.untied = d.variant == SCE_UNTIED;
+  c.topk = d.variant == SCE_TOPK;
+  c.learned = d.variant == SCE_TIED_LEARNED_CENTER;
   // (the learned-centre variant always holds M centred batches, whatever the caller's layout)
-  c.xm = d.x_per_model || d.variant == SCE_TIED_LEARNED_CENTER ? d.n_models : 1;
+  c.x_models = d.x_per_model || c.learned;
+  c.xm = c.x_models ? d.n_models : 1;
+  c.input_models = c.learned ? (d.x_per_model ? d.n_models : 1) : d.centering == 1 ? 1 : c.xm;
+  c.nonneg = d.encoder_nonneg != 0;
+  c.shift = d.input_shift;
+  c.evaluable = !c.learned && !c.nonneg && c.shift == 0.f;
   c.bpad = (d.batch_max + 15) / 16 * 16;
   // top-k lists hold the largest k of the ensemble (desc.topk_k_max, supplied by the host mirror, which knows
   // buffers["sparsity"]) rounded up to 8; none when it is unknown or too large for the gather kernel (dense path)
-  if (d.variant == SCE_TOPK && d.topk_k_max >= 1 && d.topk_k_max <= 256) {
+  if (c.topk && d.topk_k_max >= 1 && d.topk_k_max <= 256) {
     c.tk_kmax = (d.topk_k_max + 7) / 8 * 8;
     c.tk_slices = topk_slices(d, c.tk_kmax);
     // Worth it where the dictionary is large against k: the dense decode + dcode GEMMs cost ~ n per row, the gather
@@ -314,13 +328,11 @@ static PlanConfig plan_config(const sce_desc& d) {
   // code-gradient planes are written by the selection / scatter kernels, row-major only, so their weight gradient widens
   // the 8-bit tiles. Nor do launch-bound plans: there the weight gradient takes microseconds either way, and the copies
   // would add three launches per step and a third to the workspace.
-  c.dw_native = c.arith == kArithF16F8 && d.variant != SCE_TOPK && d.bwd_passes >= 3 && !launch_bound;
+  c.dw_native = c.arith == kArithF16F8 && !c.topk && d.bwd_passes >= 3 && !launch_bound;
   // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
   // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
   // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
   c.split_decode = d.n > 4096;
-  c.nonneg = d.encoder_nonneg != 0;
-  c.shift = d.input_shift != 0.f;
   return c;
 }
 
@@ -336,7 +348,7 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
   w.x_stage = c.take<float>(xm * B * dd);
   w.x = c.planes(xm * B * dd, f8);
   w.wenc = c.planes(M * n * dd, f8);
-  w.wdec = d.variant == SCE_UNTIED ? c.planes(M * n * dd, f8) : w.wenc;
+  w.wdec = cfg.untied ? c.planes(M * n * dd, f8) : w.wenc;
   if (f8) w.wdt = c.planes(M * n * dd, f8);
   const bool tdw = cfg.dw_native;
   const size_t Bp = cfg.bpad;
@@ -364,11 +376,11 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
     w.c.f8 = w.ct.f8 = w.xt.f8 = w.gt.f8 = true;
   }
   w.dw_enc = c.take<float>(M * n * dd);
-  w.dw_dec = d.variant == SCE_UNTIED ? c.take<float>(M * n * dd) : w.dw_enc;
-  const size_t enc_parts = d.variant == SCE_TOPK ? B : tiles_mB * 8 * tiles_nN;
+  w.dw_dec = cfg.untied ? c.take<float>(M * n * dd) : w.dw_enc;
+  const size_t enc_parts = cfg.topk ? B : tiles_mB * 8 * tiles_nN;
   w.part_enc = c.take<float>(M * enc_parts * 2);
   const size_t dec_parts = tiles_mB * 8 * tiles_nD;   // top-k: up to kTopkMaxSlices partials per row from the gather kernel
-  w.part_dec = c.take<float>(M * (d.variant == SCE_TOPK && dec_parts < kTopkMaxSlices * B ? kTopkMaxSlices * B : dec_parts));
+  w.part_dec = c.take<float>(M * (cfg.topk && dec_parts < kTopkMaxSlices * B ? kTopkMaxSlices * B : dec_parts));
   w.db_part = c.take<float>(M * tiles_mB * 4 * n);
   w.bnorm = c.take<float>(M);
   w.l1_over_b = c.take<float>(M);
@@ -378,7 +390,7 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
   w.act_pos = c.take<uint32_t>(M * n_chunks * B);
   w.act_zero = c.take<uint32_t>(M * n_chunks * B);
   // top-k: scores of their own (the code-gradient planes must keep their scattered zeros) and the k-sparse lists
-  if (d.variant == SCE_TOPK) {
+  if (cfg.topk) {
     const size_t kmax = cfg.tk_kmax;
     w.scores = c.take<float>(M * B * n);
     w.tk_cmax = c.take<uint32_t>(M * B * n_chunks);
@@ -395,14 +407,14 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
     w.rot = c.planes(M * dd * dd, f8);
     w.x_centered = c.take<float>(M * B * dd);
   }
-  if (d.variant == SCE_TIED_LEARNED_CENTER) {
+  if (cfg.learned) {
     w.x_centered = c.take<float>(M * B * dd);
     w.g_part = c.take<float>(M * tiles_mB * 4 * dd);
     w.center_coef = c.take<float>(M * n);
     w.center_part = c.take<float>(M * ((n + kCenterChunkRows - 1) / kCenterChunkRows) * dd);
     w.center_grad = c.take<float>(M * dd);
   }
-  if (cfg.shift) w.x_shifted = c.take<float>(xm * B * dd);
+  if (cfg.shift != 0.f) w.x_shifted = c.take<float>(xm * B * dd);
   w.res_flags = c.take<uint32_t>(kFlagWords);   // [0] residual flag, [kAbsmaxWord] input range monitor, [kBadWord] health (separate 128-byte lines)
   return align_up(c.off, 1024);
 }
@@ -491,8 +503,8 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   };
   // dz^T x, then c^T g: a second GEMM of the decoder (untied) or a second operand set of the one dictionary's
   // (dz's own 8-bit planes are batch-major in dw_native plans)
-  GemmMaps& cg = d.variant == SCE_UNTIED ? m->dw_dec : m->dw_enc;
-  const int cg_set = d.variant == SCE_UNTIED ? 0 : 1;
+  GemmMaps& cg = cfg.untied ? m->dw_dec : m->dw_enc;
+  const int cg_set = cfg.untied ? 0 : 1;
   ok &= dw_operand(m->dw_enc.a[0], p->dz, p->dz, M, n) && dw_operand(m->dw_enc.b[0], p->x, p->xt, xm, dd);
   ok &= dw_operand(cg.a[cg_set], p->c, p->ct, M, n) && dw_operand(cg.b[cg_set], p->g, p->gt, M, dd);
   ok &= make_tmap_bf16_store32(&m->st_c.hi, p->c.hi, M, (uint64_t)B, n, Bm * n);
@@ -512,7 +524,7 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
     ok &= make_tmap_bf16_store32(&m->st_c.lo, p->c.lo, M, (uint64_t)B, n, Bm * n);
     ok &= make_tmap_bf16_store32(&m->st_dz.lo, p->dz.lo, M, (uint64_t)B, n, Bm * n);
   }
-  if (d.variant == SCE_TOPK) ok &= make_tmap_f32_store32(&m->st_scores, p->scores, M, (uint64_t)B, n, Bm * n);
+  if (cfg.topk) ok &= make_tmap_f32_store32(&m->st_scores, p->scores, M, (uint64_t)B, n, Bm * n);
   if (!ok) {
     delete m;
     return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (B=%d, M=%d, n=%d, d=%d)", B, d.n_models, d.n, d.d);
@@ -616,13 +628,19 @@ struct DictSide {
 // decoder alone is normalised. Returns the count.
 static int dict_sides(const sce_plan* p, DictSide out[2]) {
   const sce_buffers& b = p->b;
-  if (p->d.variant != SCE_UNTIED) {
+  if (!p->cfg.untied) {
     out[0] = {b.encoder, p->dw_enc, b.encoder_m, b.encoder_v, p->wenc, 1, p->d.norm_floor};
     return 1;
   }
   out[0] = {b.encoder, p->dw_enc, b.encoder_m, b.encoder_v, p->wenc, 0, 0.f};
   out[1] = {b.decoder, p->dw_dec, b.decoder_m, b.decoder_v, p->wdec, 1, p->d.norm_floor};
   return 2;
+}
+
+// Calls f(arith) with the plan's arithmetic as a compile-time constant (std::integral_constant<int, AR>)
+template <class F>
+static auto with_arith(int arith, F&& f) {
+  return arith == kArithF16F8 ? f(std::integral_constant<int, kArithF16F8>{}) : f(std::integral_constant<int, kArithBf16x3>{});
 }
 
 // MODE_PREPARE reads the weights and writes the planes; MODE_ADAM also reads dW and updates the moments; MODE_GRAD
@@ -635,15 +653,13 @@ static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_ou
   float* v = MODE == MODE_ADAM ? s.v : nullptr;
   const Planes w = MODE == MODE_GRAD ? Planes{} : s.planes;
   float* wf = (MODE != MODE_GRAD && p->cfg.topk_sparse) ? p->wn_f32 : nullptr;   // (top-k plans have one dictionary)
-  auto run = [&](auto arith, auto nonneg) {
-    return launch_dict_rows_t<MODE, decltype(arith)::value, decltype(nonneg)::value>(
-        s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
-  };
-  using F8 = std::integral_constant<int, kArithF16F8>;
-  using B3 = std::integral_constant<int, kArithBf16x3>;
-  if (p->cfg.nonneg)   // (tied plans only: one dictionary, normalised)
-    return p->cfg.arith == kArithF16F8 ? run(F8{}, std::true_type{}) : run(B3{}, std::true_type{});
-  return p->cfg.arith == kArithF16F8 ? run(F8{}, std::false_type{}) : run(B3{}, std::false_type{});
+  return with_arith(p->cfg.arith, [&](auto arith) {
+    auto run = [&](auto nonneg) {
+      return launch_dict_rows_t<MODE, decltype(arith)::value, decltype(nonneg)::value>(
+          s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
+    };
+    return p->cfg.nonneg ? run(std::true_type{}) : run(std::false_type{});   // (nonneg: tied plans only, one side)
+  });
 }
 
 // f16f8: the decoder's planes -> their transposed copy, which the decode GEMM reads K-major (nothing to do where the
@@ -699,9 +715,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   const int M = d.n_models, n = d.n, dd = d.d;
   const long long Bm = d.batch_max;
   const int one[2] = {1, 1};
-  const bool learned = d.variant == SCE_TIED_LEARNED_CENTER;
-  const bool x_models = d.x_per_model || learned;   // the batch the kernels below read holds one slab per model
-  const int xb[2] = {x_models ? 1 : 0, 1};
+  const int xb[2] = {cfg.x_models ? 1 : 0, 1};
   const int tiles_mB = (B + kBM - 1) / kBM;
 
   prof_mark(p, SCE_PHASE_SPLIT, st);
@@ -722,7 +736,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
     if (rc) return rc;
     launches += 2;
     x = p->x_centered;
-  } else if (learned) {
+  } else if (cfg.learned) {
     // ---- learned centre (sae_ensemble.py:198-200): x - center[m] -> the per-model fp32 batch every kernel below reads
     const long long n4 = (long long)B * dd / 4;
     const int blocks = (int)((n4 + 255) / 256 < 1024 ? (n4 + 255) / 256 : 1024);
@@ -737,11 +751,11 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), st));
   for (int m = 0; m < cfg.xm; ++m) {
     launch_split_rows<AR>(x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st,
-                          d.input_shift, cfg.shift ? p->x_shifted + (long long)m * B * dd : nullptr);
+                          cfg.shift, cfg.shift != 0.f ? p->x_shifted + (long long)m * B * dd : nullptr);
     ++launches;
   }
   CUDA_TRY(cudaGetLastError());
-  if (cfg.shift) x = p->x_shifted;
+  if (cfg.shift != 0.f) x = p->x_shifted;
   // dw_native: batch-major copies of the 8-bit planes of x, c and g for the weight gradient (dz's are written so by dcode)
   const bool tdw = f8 && backward && cfg.dw_native;
   auto batch_major = [&](const Planes& P, const Planes& T, int models, int cols) {
@@ -767,12 +781,12 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
   act.zero = p->act_zero;
   act.n_chunks = (n + 31) / 32;
   act.batch_max = d.batch_max;
-  if (d.variant == SCE_TOPK) act.zero = nullptr;   // relu semantics: no gradient at exactly 0
+  if (cfg.topk) act.zero = nullptr;   // relu semantics: no gradient at exactly 0
   // ---- encode
   prof_mark(p, SCE_PHASE_ENCODE, st);
   int n_enc_parts;
   TopkLists tk = {nullptr, nullptr, nullptr, 0, 0};
-  if (d.variant != SCE_TOPK) {
+  if (!cfg.topk) {
     auto fill = [&](auto& ep) {
       ep.out_hi = maps->st_c.hi;
       ep.out_lo = maps->st_c.lo;
@@ -851,7 +865,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       using E = typename decltype(tag)::type;
       typename E::Params dp;
       dp.x = x;
-      dp.x_model_stride = x_models ? (long long)B * dd : 0;
+      dp.x_model_stride = cfg.x_models ? (long long)B * dd : 0;
       dp.g_hi = static_cast<uint16_t*>(p->g.hi);
       dp.g_lo = static_cast<uint8_t*>(p->g.lo);
       dp.g_x8 = p->g.x8;
@@ -871,7 +885,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       else
         return launch_gemm_t<E, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
     };
-    rc = learned ? decode(TypeTag<EpiDecG>{}) : decode(TypeTag<EpiDec>{});
+    rc = cfg.learned ? decode(TypeTag<EpiDecG>{}) : decode(TypeTag<EpiDec>{});
     if (rc) return rc;
     ++launches;
     n_dec_parts = tiles_mB * 8 * ((dd + kBN - 1) / kBN);
@@ -937,7 +951,7 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
           return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(p, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, st, rf);
       return launch_gemm_t<EpiStoreF32, true, true, !f8, AR>(p, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, st, rf);
     };
-    if (d.variant == SCE_UNTIED) {
+    if (cfg.untied) {
       rc = dw(maps->dw_enc, 1, one, xb, p->dw_enc, x_is_b);
       if (rc) return rc;
       rc = dw(maps->dw_dec, 1, one, one, p->dw_dec, ResFlags());
@@ -957,9 +971,9 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
 
 static int run_pipeline(sce_plan* p, const float* x, int B, float* x_hat, bool backward, float* out_losses,
                         float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
-  return p->cfg.arith == kArithF16F8
-             ? run_pipeline_t<kArithF16F8>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part)
-             : run_pipeline_t<kArithBf16x3>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
+  return with_arith(p->cfg.arith, [&](auto arith) {
+    return run_pipeline_t<decltype(arith)::value>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
+  });
 }
 
 // Learned-centre plans: the centre gradient of the last backward pass into p->center_grad (sum_b g - db W, with db and
@@ -982,6 +996,36 @@ static int center_grad_launches(sce_plan* p, int B, const AdamHyper& h, cudaStre
       MODE == MODE_ADAM ? p->res_flags : nullptr);
   CUDA_TRY(cudaGetLastError());
   launches += 3;
+  return SCE_OK;
+}
+
+// What follows the backward pass, in order: the centre gradient (learned centre), dict_rows per dictionary side, the
+// decoder's transposed planes (MODE_ADAM) and the bias kernel. MODE_ADAM updates the parameters; MODE_GRAD writes the
+// gradients to grad_out[side] and d_bias, skipping a launch whose output is null. Adds its launches to `launches`.
+template <int MODE>
+static int train_tail(sce_plan* p, int B, const AdamHyper& h, float* const* grad_out, float* d_bias, cudaStream_t st,
+                      int& launches) {
+  constexpr bool adam = MODE == MODE_ADAM;
+  int rc;
+  if (p->cfg.learned && (rc = center_grad_launches<MODE>(p, B, h, st, launches))) return rc;
+  DictSide sides[2];
+  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s) {
+    if (!adam && !grad_out[s]) continue;
+    if ((rc = launch_dict_rows<MODE>(p, sides[s], adam ? nullptr : grad_out[s], h, st))) return rc;
+    ++launches;
+  }
+  if (adam && (rc = transpose_dict(p, st, launches))) return rc;
+  if (p->b.encoder_bias && (adam || d_bias)) {
+    const sce_desc& d = p->d;
+    const long long tot = (long long)d.n_models * d.n;
+    const int n_part = ((B + kBM - 1) / kBM) * 4;
+    bias_kernel<MODE><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
+        p->b.encoder_bias, adam ? p->b.bias_m : nullptr, adam ? p->b.bias_v : nullptr, p->db_part, n_part, d.n,
+        d.n_models, p->b.bias_decay, p->bnorm, adam ? nullptr : d_bias, h, grad_out_scale(p, B),
+        adam ? p->res_flags : nullptr);
+    CUDA_TRY(cudaGetLastError());
+    ++launches;
+  }
   return SCE_OK;
 }
 
@@ -1465,7 +1509,7 @@ int sce_prepare(sce_plan* p, void* stream) {
   const sce_desc& d = p->d;
   const int kmax = p->cfg.tk_kmax;   // (top-k plans only)
   std::vector<long long> ks;
-  if (d.variant == SCE_TOPK) {
+  if (p->cfg.topk) {
     // the selection scatters k entries into the code planes but records (and clears on the next call) at most the list
     // capacity of them, and a k below 1 leaves its bound undefined: hold every k to [1, n] and, with lists, to topk_k_max
     ks.resize(d.n_models);
@@ -1512,10 +1556,8 @@ int sce_prepare(sce_plan* p, void* stream) {
     if (!p->b.center_trans || !p->b.center_rot || !p->b.center_scale)
       return fail(SCE_ERR_INVALID, "centering needs the center_trans / center_rot / center_scale buffers");
     const long long n4 = (long long)d.n_models * d.d * d.d / 4;
-    if (p->cfg.arith == kArithF16F8)
-      launch_split_rows<kArithF16F8>(p->b.center_rot, p->rot, n4, nullptr, st);
-    else
-      launch_split_rows<kArithBf16x3>(p->b.center_rot, p->rot, n4, nullptr, st);
+    with_arith(p->cfg.arith,
+               [&](auto arith) { launch_split_rows<decltype(arith)::value>(p->b.center_rot, p->rot, n4, nullptr, st); });
     CUDA_TRY(cudaGetLastError());
   }
   DictSide sides[2];
@@ -1530,35 +1572,13 @@ int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_los
   return run_pipeline(p, x, B, x_hat, false, out_losses, out_nnz, static_cast<cudaStream_t>(stream));
 }
 
-// models' worth of rows in the caller's batch: 1 when it is shared ([B,d]; also with centering = 1), else M
-static int input_models(const sce_plan* p) {
-  if (p->d.variant == SCE_TIED_LEARNED_CENTER) return p->d.x_per_model ? p->d.n_models : 1;
-  return p->d.centering == 1 ? 1 : p->cfg.xm;
-}
-
 // every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph)
 static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
                          cudaStream_t st) {
   int rc = run_pipeline(p, x, B, nullptr, true, out_losses, out_nnz, st);
   if (rc) return rc;
-  const sce_desc& d = p->d;
-  const AdamHyper h = hyper_for(p, t);
   int launches = p->last_launches;
-  if (d.variant == SCE_TIED_LEARNED_CENTER && (rc = center_grad_launches<MODE_ADAM>(p, B, h, st, launches))) return rc;
-  DictSide sides[2];
-  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s, ++launches)
-    if ((rc = launch_dict_rows<MODE_ADAM>(p, sides[s], nullptr, h, st))) return rc;
-  rc = transpose_dict(p, st, launches);
-  if (rc) return rc;
-  if (p->b.encoder_bias) {
-    const long long tot = (long long)d.n_models * d.n;
-    const int n_part = ((B + kBM - 1) / kBM) * 4;
-    bias_kernel<MODE_ADAM><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
-        p->b.encoder_bias, p->b.bias_m, p->b.bias_v, p->db_part, n_part, d.n, d.n_models, p->b.bias_decay, p->bnorm,
-        nullptr, h, grad_out_scale(p, B), p->res_flags);
-    CUDA_TRY(cudaGetLastError());
-    ++launches;
-  }
+  if ((rc = train_tail<MODE_ADAM>(p, B, hyper_for(p, t), nullptr, nullptr, st, launches))) return rc;
   prof_mark(p, SCE_PHASE_COUNT, st);
   p->last_launches = launches;
   return SCE_OK;
@@ -1587,7 +1607,7 @@ int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_n
     BatchMaps* maps = nullptr;
     rc = build_maps(p, B, &maps);
     if (rc) return rc;
-    const size_t bytes = (size_t)input_models(p) * B * p->d.d * sizeof(float);
+    const size_t bytes = (size_t)p->cfg.input_models * B * p->d.d * sizeof(float);
     if (x != p->x_stage) CUDA_TRY(cudaMemcpyAsync(p->x_stage, x, bytes, cudaMemcpyDeviceToDevice, st));
     // the captured kernels write the plan's own staging outputs (stable addresses: callers may pass fresh tensors
     // every step, as the reference returns them); the results are copied out below
@@ -1640,23 +1660,9 @@ int sce_grads(sce_plan* p, const float* x, int B, float* d_encoder, float* d_bia
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int rc = run_pipeline(p, x, B, nullptr, true, out_losses, out_nnz, st);
   if (rc) return rc;
-  const sce_desc& d = p->d;
-  const AdamHyper h = hyper_for(p, 1);
-  int launches = 0;
-  if (d.variant == SCE_TIED_LEARNED_CENTER && (rc = center_grad_launches<MODE_GRAD>(p, B, h, st, launches))) return rc;
-  DictSide sides[2];
+  int launches = 0;   // (not counted: last_launches stays the pipeline's)
   float* const grad_out[2] = {d_encoder, d_decoder};
-  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
-    if (grad_out[s] && (rc = launch_dict_rows<MODE_GRAD>(p, sides[s], grad_out[s], h, st))) return rc;
-  if (p->b.encoder_bias && d_bias) {
-    const long long tot = (long long)d.n_models * d.n;
-    const int n_part = ((B + kBM - 1) / kBM) * 4;
-    bias_kernel<MODE_GRAD><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
-        p->b.encoder_bias, nullptr, nullptr, p->db_part, n_part, d.n, d.n_models, p->b.bias_decay, p->bnorm, d_bias, h,
-        grad_out_scale(p, B), nullptr);
-    CUDA_TRY(cudaGetLastError());
-  }
-  return SCE_OK;
+  return train_tail<MODE_GRAD>(p, B, hyper_for(p, 1), grad_out, d_bias, st, launches);
 }
 
 int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_host, float* out_nnz_host,
@@ -1665,7 +1671,7 @@ int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_hos
   if (!x_host) return fail(SCE_ERR_INVALID, "x_host is NULL");
   if (int rc = check_rows(p, B, "")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t bytes = (size_t)input_models(p) * B * p->d.d * sizeof(float);
+  const size_t bytes = (size_t)p->cfg.input_models * B * p->d.d * sizeof(float);
   CUDA_TRY(cudaMemcpyAsync(p->x_stage, x_host, bytes, cudaMemcpyHostToDevice, st));
   int rc = sce_step(p, p->x_stage, B, p->loss_stage, p->nnz_stage, st);
   if (rc) return rc;
@@ -1692,10 +1698,9 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
   }
   for (int m = 0; m < p->d.n_models; ++m) {
     const Planes c = p->c.at((size_t)m * p->d.batch_max * p->d.n);
-    if (p->cfg.arith == kArithF16F8)
-      join_code_kernel<kArithF16F8><<<1024, 256, 0, st>>>(c.hi, nullptr, c.x8, out_code + (long long)m * per, per / 2);
-    else
-      join_code_kernel<kArithBf16x3><<<1024, 256, 0, st>>>(c.hi, c.lo, nullptr, out_code + (long long)m * per, per / 2);
+    with_arith(p->cfg.arith, [&](auto arith) {   // (each arithmetic reads its own planes)
+      join_code_kernel<decltype(arith)::value><<<1024, 256, 0, st>>>(c.hi, c.lo, c.x8, out_code + (long long)m * per, per / 2);
+    });
   }
   CUDA_TRY(cudaGetLastError());
   return SCE_OK;
@@ -1703,7 +1708,7 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
 
 int sce_read_center_grad(sce_plan* p, float* d_center, void* stream) {
   if (!p || !d_center) return fail(SCE_ERR_INVALID, "plan / d_center is NULL");
-  if (p->d.variant != SCE_TIED_LEARNED_CENTER) return fail(SCE_ERR_INVALID, "read_center_grad: the plan has no learned centre");
+  if (!p->cfg.learned) return fail(SCE_ERR_INVALID, "read_center_grad: the plan has no learned centre");
   CUDA_TRY(cudaMemcpyAsync(d_center, p->center_grad, (size_t)p->d.n_models * p->d.d * sizeof(float),
                            cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return SCE_OK;
@@ -1763,14 +1768,8 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
   return SCE_OK;
 }
 
-// Plans whose training forward differs from the export it evaluates as (sce_forward_stats / sce_forward_fragments): the
-// learned centre, and the non-negative tied plans, whose exports are TiedSAE objects of the raw encoder
-static bool training_only(const sce_desc& d) {
-  return d.variant == SCE_TIED_LEARNED_CENTER || d.encoder_nonneg || d.input_shift != 0.f;
-}
-
 size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || training_only(*desc)) return 0;
+  if (validate(desc) || B < 1 || B > desc->batch_max || !plan_config(*desc).evaluable) return 0;
   return stats_workspace(*desc, B);
 }
 
@@ -1778,7 +1777,7 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
                       float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
                       size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_stats: plan is NULL");
-  if (training_only(p->d))
+  if (!p->cfg.evaluable)
     return fail(SCE_ERR_INVALID, "forward_stats: not available for the learned-centre variant or with encoder_nonneg / "
                                  "input_shift; evaluate the exported dictionaries (TiedSAE)");
   if (int rc = check_rows(p, B, "forward_stats: ")) return rc;
@@ -1792,12 +1791,11 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
   if (int rc = check_workspace(workspace, workspace_bytes, stats_workspace(p->d, B), "forward_stats: ")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sce_desc& d = p->d;
-  const bool topk = d.variant == SCE_TOPK;
   float* part = static_cast<float*>(workspace);
-  int rc = run_pipeline(p, x, B, x_hat, false, out_losses, out_nnz, st, topk ? nullptr : part);
+  int rc = run_pipeline(p, x, B, x_hat, false, out_losses, out_nnz, st, p->cfg.topk ? nullptr : part);
   if (rc) return rc;
   const int n_chunks = (d.n + 31) / 32, row_blocks = (B + 31) / 32;
-  if (topk) {
+  if (p->cfg.topk) {
     topk_moment_kernel<<<dim3(n_chunks, (row_blocks + 7) / 8, d.n_models), 256, 0, st>>>(p->scores, p->act_pos, n_chunks,
                                                                                         d.batch_max, B, d.n, row_blocks, part);
     CUDA_TRY(cudaGetLastError());
@@ -1814,7 +1812,7 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
 }
 
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || training_only(*desc)) return 0;
+  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || !plan_config(*desc).evaluable) return 0;
   return frag_workspace(*desc, B, L, nullptr, nullptr);
 }
 
@@ -1823,7 +1821,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "forward_fragments: plan is NULL");
-  if (training_only(p->d))
+  if (!p->cfg.evaluable)
     return fail(SCE_ERR_INVALID, "forward_fragments: not available for the learned-centre variant or with encoder_nonneg / "
                                  "input_shift; evaluate the exported dictionaries (TiedSAE)");
   if (int rc = check_rows(p, B, "forward_fragments: ")) return rc;
@@ -1851,15 +1849,14 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   int* open = reinterpret_cast<int*>(ws + off_open);
   const int n_chunks = (d.n + 31) / 32, G = B / L;
   const FragCode c{p->c.hi, p->c.lo, p->c.x8, p->scores, p->act_pos, n_chunks, d.batch_max, d.n};
-  if (d.variant == SCE_TOPK)
+  if (p->cfg.topk)
     launch_fragments<kArithBf16x3, true>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
                                          top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
-  else if (p->cfg.arith == kArithF16F8)
-    launch_fragments<kArithF16F8, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
-                                         top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
   else
-    launch_fragments<kArithBf16x3, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
-                                          top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
+    with_arith(p->cfg.arith, [&](auto ar) {
+      launch_fragments<decltype(ar)::value, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed,
+                                                   top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
+    });
   CUDA_TRY(cudaGetLastError());
   // active fragments: segments of L rows, cut at fragment boundaries (phase 0, no segment stays open)
   CUDA_TRY(cudaMemsetAsync(open, 0, (size_t)d.n_models * d.n * sizeof(int), st));

@@ -33,27 +33,11 @@ from typing import Dict, List, Optional
 import torch
 
 from . import _lib
-from .optim import AdamConfig, adam, resolve_optimizer
+from .optim import adam, resolve_optimizer
 from .signatures import DictSignature
 from .tracing import nvtx_range
 
 Tensor = torch.Tensor
-
-_VARIANT_CODE = {"tied": _lib.SCE_TIED, "masked_tied": _lib.SCE_TIED, "untied": _lib.SCE_UNTIED,
-                 "masked_untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK,
-                 "tied_learned_center": _lib.SCE_TIED_LEARNED_CENTER, "positive_tied": _lib.SCE_TIED}
-# FunctionalPositiveTiedSAE encodes and reconstructs x + 0.18 (autoencoders/mlp_tests.py:104, :110)
-_POSITIVE_TIED_SHIFT = 0.18
-_LOSS_KEYS = {
-    "tied": ("loss", "l_reconstruction", "l_l1"),
-    "masked_tied": ("loss", "l_reconstruction", "l_l1"),
-    "masked_untied": ("loss", "l_reconstruction", "l_l1"),
-    "untied": ("loss", "l_reconstruction", "l_l1", "l_bias_decay"),
-    "topk": ("loss",),
-    "tied_learned_center": ("loss", "l_reconstruction", "l_l1"),
-    "positive_tied": ("loss", "l_reconstruction", "l_l1", "l_bias_decay"),
-}
-
 
 def optim_str_to_func(optim_str):
     """ensemble.py:25-31."""
@@ -195,23 +179,21 @@ class FunctionalEnsemble:
 
     # ------------------------------------------------------------------------------------------------------
     def init_functions(self):
-        variant = getattr(self.sig, "variant", None)
-        if variant not in _VARIANT_CODE:
+        engine_sig = _lib.SIGNATURES.get(getattr(self.sig, "variant", None))
+        if engine_sig is None:
             raise NotImplementedError(
                 f"{getattr(self.sig, '__name__', self.sig)} has no engine variant: only the signatures of the sweep hot "
                 "path (FunctionalTiedSAE, FunctionalTiedCenteredSAE, FunctionalPositiveTiedSAE, FunctionalSAE, the "
                 "Masked variants, TopKEncoder) are implemented in the "
                 "sm_90a engine, and there is deliberately no generic autograd fallback")
-        self._variant = variant
+        self._engine_sig = engine_sig
         self._plan = None
         self._plan_key = None
         self._ws = None
         self._centering = None
         self._serial = 0
         self._steps = 0
-        main = "dict" if variant == "topk" else "encoder"
-        self._main = main
-        self._n, self._d = self.params[main].shape[1], self.params[main].shape[2]
+        self._n, self._d = self.params[engine_sig.main].shape[1:]
         self._engine_buffers = None
         self._arith_fallback = None       # "bf16x3" once an auto plan left the fp16 range (sticky for this object)
         self._since_health = 0            # steps since the health flag was last read
@@ -230,10 +212,8 @@ class FunctionalEnsemble:
     def _needs_centering(self) -> bool:
         """Whether the tied signature's centring is non-trivial. Evaluated once (it costs three device
         reductions and a host sync) and cached until ``refresh()`` / ``to_device()``."""
-        if self._variant != "tied":
-            return False
         if self._centering is None:
-            self._centering = self._centering_is_nontrivial()
+            self._centering = self._engine_sig.centering and self._centering_is_nontrivial()
         return self._centering
 
     def _centering_is_nontrivial(self) -> bool:
@@ -245,7 +225,7 @@ class FunctionalEnsemble:
 
     def _check_sparsity(self):
         """Top-k: every model's k must lie in [1, n], as ``TopKEncoder.init`` requires (the engine rejects it too)."""
-        if self._variant != "topk":
+        if not self._engine_sig.topk:
             return
         for k in self.buffers["sparsity"].reshape(-1).tolist():
             if not 0 < int(k) <= self._n:
@@ -261,58 +241,11 @@ class FunctionalEnsemble:
             if not v.is_contiguous():
                 self.params[k] = v.contiguous()
         self._destroy_plan()
-        cfg: AdamConfig = self.optimizer
-        positive = self._variant == "positive_tied"   # tied on max(E, 0) and x + 0.18 (sce_desc.encoder_nonneg / input_shift)
-        desc = _lib.SceDesc(
-            variant=_VARIANT_CODE[self._variant], n_models=self.n_models, d=self._d, n=self._n,
-            batch_max=batch_max, x_per_model=int(x_per_model), lr=cfg.lr, beta1=cfg.b1, beta2=cfg.b2, eps=cfg.eps,
-            eps_root=cfg.eps_root,
-            adam_count_mode=_lib.SCE_ADAM_FROZEN_T1 if self.adam_count_mode == "frozen_t1" else _lib.SCE_ADAM_STANDARD,
-            fwd_passes=self.fwd_passes, bwd_passes=self.bwd_passes,
-            norm_floor=0.0 if self._variant == "topk" else 1e-8,
-            arith=_lib.ARITH_CODE[getattr(self, "_arith_fallback", None) or getattr(self, "arith", "auto")],
-            topk_k_max=int(self.buffers["sparsity"].max()) if self._variant == "topk" else 0,
-            centering=centering, encoder_nonneg=int(positive),
-            input_shift=_POSITIVE_TIED_SHIFT if positive else 0.0)
-        eb = {}
-
-        def f32vec(name):  # [M] fp32 hyper-parameter buffers
-            t = self.buffers.get(name)
-            if t is None:
-                return None
-            eb[name] = t.to(device=dev, dtype=torch.float32).contiguous()
-            return eb[name].data_ptr()
-
-        ptr = lambda t: t.data_ptr() if t is not None else None
-        mu, nu = self.optim_states["mu"], self.optim_states["nu"]
-        bufs = _lib.SceBuffers()
-        bufs.encoder = ptr(self.params[self._main])
-        bufs.encoder_m, bufs.encoder_v = ptr(mu[self._main]), ptr(nu[self._main])
-        if self._variant != "topk":
-            bufs.encoder_bias = ptr(self.params["encoder_bias"])
-            bufs.bias_m, bufs.bias_v = ptr(mu["encoder_bias"]), ptr(nu["encoder_bias"])
-            bufs.l1_alpha = f32vec("l1_alpha")
-            if self._variant in ("tied", "untied", "positive_tied"):
-                bufs.bias_decay = f32vec("bias_decay")
-        if self._variant in ("untied", "masked_untied"):
-            bufs.decoder = ptr(self.params["decoder"])
-            bufs.decoder_m, bufs.decoder_v = ptr(mu["decoder"]), ptr(nu["decoder"])
-        if self._variant == "tied_learned_center":
-            # FunctionalTiedCenteredSAE: the centre is a parameter, trained by the engine with its Adam moments
-            bufs.center = ptr(self.params["center"])
-            bufs.center_m, bufs.center_v = ptr(mu["center"]), ptr(nu["center"])
-        if self._variant in ("masked_tied", "masked_untied"):
-            eb["coef_mask"] = self.buffers["coef_mask"].to(device=dev, dtype=torch.uint8).contiguous()
-            bufs.coef_mask = eb["coef_mask"].data_ptr()
-        if self._variant == "topk":
-            eb["sparsity"] = self.buffers["sparsity"].to(device=dev, dtype=torch.int64).contiguous()
-            bufs.sparsity = eb["sparsity"].data_ptr()
-        if centering:
-            # FunctionalTiedSAE.center (sae_ensemble.py:126-128) runs on the device: (x - trans) planes, GEMM with rot, * scale
-            for name in ("center_trans", "center_rot", "center_scale"):
-                eb[name] = self.buffers[name].to(device=dev, dtype=torch.float32).contiguous()
-            bufs.center_trans, bufs.center_rot, bufs.center_scale = (eb["center_trans"].data_ptr(), eb["center_rot"].data_ptr(),
-                                                                     eb["center_scale"].data_ptr())
+        desc, bufs, eb = _lib.plan_structs(
+            self._engine_sig, self.params, self.buffers, self.optim_states["mu"], self.optim_states["nu"],
+            batch_max=batch_max, x_per_model=x_per_model, centering=centering, adam=self.optimizer,
+            adam_count_mode=self.adam_count_mode, fwd_passes=self.fwd_passes, bwd_passes=self.bwd_passes,
+            arith=getattr(self, "_arith_fallback", None) or getattr(self, "arith", "auto"))
         with torch.cuda.device(dev):
             plan, self._ws = _lib.create_plan(desc, bufs, dev)
             self._plan = plan
@@ -370,7 +303,7 @@ class FunctionalEnsemble:
     def _losses_dict(self) -> Dict[str, Tensor]:
         cols = self._out_losses
         return {k: cols[:, i] for i, k in enumerate(("loss", "l_reconstruction", "l_l1", "l_bias_decay"))
-                if k in _LOSS_KEYS[self._variant]}
+                if k in self._engine_sig.loss_keys}
 
     def _aux(self, B):
         self._serial += 1
@@ -484,8 +417,8 @@ class FunctionalEnsemble:
             g = {k: torch.empty_like(v) for k, v in self.params.items()}
             ptr = lambda k: g[k].data_ptr() if k in g else None
             with torch.cuda.device(x.device):
-                _lib.check(_lib.load().sce_grads(self._plan, x.data_ptr(), B, ptr(self._main), ptr("encoder_bias"),
-                                                 ptr("decoder"), self._out_losses.data_ptr(),
+                _lib.check(_lib.load().sce_grads(self._plan, x.data_ptr(), B, ptr(self._engine_sig.main),
+                                                 ptr("encoder_bias"), ptr("decoder"), self._out_losses.data_ptr(),
                                                  self._out_nnz.data_ptr(), self._stream()), "sce_grads")
                 if "center" in g:
                     _lib.check(_lib.load().sce_read_center_grad(self._plan, g["center"].data_ptr(), self._stream()),
@@ -514,7 +447,7 @@ class FunctionalEnsemble:
                 # call plans anew and raises again until the buffer is valid)
                 self._destroy_plan()
                 raise
-            if self._variant == "topk" and int(self.buffers["sparsity"].max()) != self._plan_k_max:
+            if self._engine_sig.topk and int(self.buffers["sparsity"].max()) != self._plan_k_max:
                 # the largest k sets the plan's top-k list capacity and its decode path (gather or dense): plan anew
                 self._build_plan(*self._plan_key)
                 return

@@ -17,6 +17,7 @@ from typing import Dict, Iterable, Optional
 import torch
 
 from . import _lib
+from .optim import AdamConfig
 
 EVER_ACTIVE_THRESHOLD = 10   # standard_metrics.py:446: a feature counts as "ever active" above this many rows
 
@@ -344,13 +345,14 @@ def _eval_groups(lds, centre: bool, multiple: int):
         n, d = int(ld.n_feats), int(ld.activation_size)
         if d % 8:
             raise ValueError(f"dictionary {i}: activation width d = {d} must be a multiple of 8")
-        if kind == "topk" and not 0 < int(ld.sparsity) <= n:
+        topk = _lib.SIGNATURES[kind].topk
+        if topk and not 0 < int(ld.sparsity) <= n:
             raise ValueError(f"dictionary {i}: sparsity must be in [1, {n}], got {ld.sparsity}")
-        if kind == "topk" and n % multiple:
+        if topk and n % multiple:
             raise ValueError(f"dictionary {i}: a TopKLearnedDict needs n ({n}) to be a multiple of {multiple}: its rows "
                              "are normalised without a clamp, so zero padding rows would become NaN")
         n_pad = -(-n // multiple) * multiple
-        centred = centre and kind == "tied" and _is_centred(ld)
+        centred = centre and _lib.SIGNATURES[kind].centering and _is_centred(ld)
         groups.setdefault((kind, n_pad, d, centred), []).append(i)
     return groups
 
@@ -370,43 +372,29 @@ class _DictPlan:
                 out[m, : t.shape[0]] = f32(t)
             return out
 
-        t = {}
-        if kind == "topk":
-            t["enc"] = stack([ld.dict for ld in lds])
-            t["sparsity"] = torch.tensor([int(ld.sparsity) for ld in lds], dtype=torch.int64, device=dev)
+        sig = _lib.SIGNATURES[kind]
+        params, buffers = {}, {}
+        if sig.topk:
+            params["dict"] = stack([ld.dict for ld in lds])
+            buffers["sparsity"] = torch.tensor([int(ld.sparsity) for ld in lds], dtype=torch.int64, device=dev)
         else:
-            t["enc"] = stack([ld.encoder for ld in lds])
-            t["bias"] = stack([ld.encoder_bias for ld in lds])
-            if kind == "untied":
-                t["dec"] = stack([ld.decoder for ld in lds])
+            params["encoder"] = stack([ld.encoder for ld in lds])
+            params["encoder_bias"] = stack([ld.encoder_bias for ld in lds])
+            if sig.decoder:
+                params["decoder"] = stack([ld.decoder for ld in lds])
             sizes = [int(ld.n_feats) for ld in lds]
             if any(k < n_pad for k in sizes):       # padding rows: the masked variants' coef_mask (1 = unused)
-                t["mask"] = (torch.arange(n_pad, device=dev)[None, :] >= torch.tensor(sizes, device=dev)[:, None]).to(torch.uint8)
+                buffers["coef_mask"] = (torch.arange(n_pad, device=dev)[None, :] >= torch.tensor(sizes, device=dev)[:, None]).to(torch.uint8)
         if centred:
-            self.trans = torch.stack([f32(ld.center_trans) for ld in lds]).contiguous()
-            self.rot = torch.stack([f32(ld.center_rot) for ld in lds]).contiguous()
-            self.scale = torch.stack([f32(ld.center_scale) for ld in lds]).contiguous()
+            self.trans = buffers["center_trans"] = torch.stack([f32(ld.center_trans) for ld in lds]).contiguous()
+            self.rot = buffers["center_rot"] = torch.stack([f32(ld.center_rot) for ld in lds]).contiguous()
+            self.scale = buffers["center_scale"] = torch.stack([f32(ld.center_scale) for ld in lds]).contiguous()
         # sce_prepare and the forward-only passes never read the Adam moments; the plan only requires their pointers
-        t["unused"] = torch.zeros(1, dtype=torch.float32, device=dev)
-        self._t = t
-        self.desc = _lib.SceDesc(
-            variant={"tied": _lib.SCE_TIED, "untied": _lib.SCE_UNTIED, "topk": _lib.SCE_TOPK}[kind], n_models=M, d=d,
-            n=n_pad, batch_max=batch_max, x_per_model=int(centred), lr=0.0, beta1=0.9, beta2=0.999, eps=1e-8,
-            eps_root=0.0, adam_count_mode=_lib.SCE_ADAM_FROZEN_T1, fwd_passes=3, bwd_passes=3,
-            norm_floor=0.0 if kind == "topk" else 1e-8, arith=_lib.arith_code(arith),
-            topk_k_max=int(t["sparsity"].max()) if kind == "topk" else 0, centering=int(centred))
-        ptr = lambda x: x.data_ptr() if x is not None else None
-        u = ptr(t["unused"])
-        b = _lib.SceBuffers()
-        b.encoder, b.encoder_m, b.encoder_v = ptr(t["enc"]), u, u
-        if kind != "topk":
-            b.encoder_bias, b.bias_m, b.bias_v = ptr(t["bias"]), u, u
-        if kind == "untied":
-            b.decoder, b.decoder_m, b.decoder_v = ptr(t["dec"]), u, u
-        b.coef_mask = ptr(t.get("mask"))
-        b.sparsity = ptr(t.get("sparsity"))
-        if centred:
-            b.center_trans, b.center_rot, b.center_scale = ptr(self.trans), ptr(self.rot), ptr(self.scale)
+        moments = dict.fromkeys(params, torch.zeros(1, dtype=torch.float32, device=dev))
+        self.desc, b, keep = _lib.plan_structs(sig, params, buffers, moments, moments, batch_max=batch_max,
+                                               x_per_model=centred, centering=int(centred), adam=AdamConfig(lr=0.0),
+                                               adam_count_mode="frozen_t1", fwd_passes=3, bwd_passes=3, arith=arith)
+        self._keep_alive = (params, buffers, moments, keep)
         self.plan, self._plan_ws = _lib.create_plan(self.desc, b, dev)
         self.stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
         try:

@@ -14,7 +14,8 @@ import torch
 
 
 class DictSignature:
-    variant = None  # "tied" | "untied" | "masked_tied" | "masked_untied" | "topk" for engine-backed signatures
+    variant = None  # engine-backed signatures: a key of _lib.SIGNATURES ("tied", "masked_tied", "untied", "masked_untied",
+                    # "topk", "tied_learned_center", "positive_tied")
 
     @staticmethod
     def to_learned_dict(params, buffers):

@@ -168,7 +168,7 @@ def test_export_declared_and_exported(lib):
     assert lib.sce_read_center_grad(None, None, None) == -1
 
 
-def test_ensemble_maps_the_signature():
-    from sparse_coding_b200 import ensemble as E
-    assert E._VARIANT_CODE["tied_learned_center"] == _lib.SCE_TIED_LEARNED_CENTER
-    assert E._LOSS_KEYS["tied_learned_center"] == ("loss", "l_reconstruction", "l_l1")
+def test_signature_table_maps_the_signature():
+    sig = _lib.SIGNATURES["tied_learned_center"]
+    assert sig.variant == _lib.SCE_TIED_LEARNED_CENTER
+    assert sig.loss_keys == ("loss", "l_reconstruction", "l_l1")

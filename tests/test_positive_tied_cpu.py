@@ -169,17 +169,17 @@ def test_learned_dict_export(cases, name):
         assert rel(ld.predict(fx["batch"]), ex["predict"]) <= 1e-6
 
 
-def test_public_names():
+def test_public_names_and_engine_record():
     import autoencoders.mlp_tests as MT
     import sparse_coding_b200 as S
-    from sparse_coding_b200 import ensemble as E
     assert MT.FunctionalPositiveTiedSAE is S.FunctionalPositiveTiedSAE
     assert "FunctionalPositiveTiedSAE" in S.__all__
     assert S.FunctionalPositiveTiedSAE.__module__ == "autoencoders.mlp_tests"
     assert S.FunctionalPositiveTiedSAE.variant == "positive_tied"
-    assert E._VARIANT_CODE["positive_tied"] == _lib.SCE_TIED
-    assert E._LOSS_KEYS["positive_tied"] == LOSS_KEYS
-    assert E._POSITIVE_TIED_SHIFT == PT.SHIFT == 0.18
+    sig = _lib.SIGNATURES["positive_tied"]
+    assert sig.variant == _lib.SCE_TIED
+    assert sig.loss_keys == LOSS_KEYS
+    assert sig.input_shift == PT.SHIFT == 0.18
 
 
 def test_unsupported_signature_error_names_it():

@@ -24,6 +24,7 @@
 #include <map>
 #include <vector>
 #include <new>
+#include <utility>
 
 #include "../../include/sce.h"
 #include "sce_epilogues.cuh"
@@ -51,6 +52,25 @@ static int fail(int code, const char* fmt, ...) {
     cudaError_t e_ = (x);                                                                      \
     if (e_ != cudaSuccess) return fail(SCE_ERR_CUDA, "%s failed: %s", #x, cudaGetErrorString(e_)); \
   } while (0)
+// returns the SCE_ERR_* code of a failed call
+#define TRY(x)                       \
+  do {                               \
+    if (int rc_ = (x)) return rc_;   \
+  } while (0)
+
+// The kernel launches of one call on one stream. Every launch goes through launch() (or launch_gemm_t), which checks
+// it and counts it; the entry points that report their launches (sce_last_launch_count) read `count`.
+struct Launcher {
+  cudaStream_t st;
+  int count = 0;
+  template <class... P, class... A>
+  int launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A&&... args) {
+    kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    CUDA_TRY(cudaGetLastError());
+    ++count;
+    return SCE_OK;
+  }
+};
 
 // ------------------------------------------------------------------------------------------------
 // plan
@@ -166,10 +186,6 @@ struct sce_plan : PlanBuffers {
 };
 
 constexpr int kProfMaxSteps = 64;
-static inline void prof_mark(sce_plan* p, int idx, cudaStream_t st) {
-  if (p->prof_on && p->prof_steps < kProfMaxSteps)
-    cudaEventRecord(p->prof_ev[p->prof_steps * (SCE_PHASE_COUNT + 1) + idx], st);
-}
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -253,13 +269,11 @@ static int query_device(int* device, int* sm_count) {
 // fp32 rows -> the operand planes of arithmetic AR: n4 float4s, grid-stride over at most 2048 blocks. With `xs`, the
 // rows are shifted by `shift` first and the shifted fp32 rows are written to `xs` as well (input_shift plans).
 template <int AR>
-static void launch_split_rows(const float* x, const Planes& w, long long n4, uint32_t* flags, cudaStream_t st,
-                              float shift = 0.f, float* xs = nullptr) {
+static int launch_split_rows(Launcher& L, const float* x, const Planes& w, long long n4, uint32_t* flags,
+                             float shift = 0.f, float* xs = nullptr) {
   const int blocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  if (xs)
-    split_rows_kernel<AR, true><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags, shift, xs);
-  else
-    split_rows_kernel<AR><<<blocks, 256, 0, st>>>(x, w.hi, w.lo, w.x8, n4, flags, 0.f, nullptr);
+  if (xs) return L.launch(split_rows_kernel<AR, true>, blocks, 256, 0, x, w.hi, w.lo, w.x8, n4, flags, shift, xs);
+  return L.launch(split_rows_kernel<AR>, blocks, 256, 0, x, w.hi, w.lo, w.x8, n4, flags, 0.f, nullptr);
 }
 
 // SCE_ARITH=bf16x3|f16f8: the arithmetic the environment pins arith = AUTO to (include/sce.h), else SCE_ARITH_AUTO
@@ -554,12 +568,14 @@ static void set_operand_maps(GemmParams<EpiParams>& gp, int s, const OperandMaps
   gp.b_x8[s] = b.x8;
 }
 
-// NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN then describe the fp16
-// planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps batch-major copies.
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool NATIVE = ARITH == kArithF16F8 && !A_MN>
-static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, const int* a_batched,
-                         const int* b_batched, int k_total, int passes, int m_total, int n_total,
-                         const typename Epi::Params& epi, cudaStream_t st, const ResFlags& rf = ResFlags()) {
+// a_batched / b_batched of the operand sets that hold one slab per model
+static const int kOnes[2] = {1, 1};
+
+// One GEMM over `n_models` models on `device` (with `sms` SMs), launched and counted by L
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool NATIVE>
+static int launch_gemm_t(Launcher& L, int n_models, int device, int sms, const GemmMaps& maps, int nsets,
+                         const int* a_batched, const int* b_batched, int k_total, int passes, int m_total, int n_total,
+                         const typename Epi::Params& epi, const ResFlags& rf = ResFlags()) {
   GemmParams<typename Epi::Params> gp;
   memset(&gp, 0, sizeof(gp));
   for (int s = 0; s < nsets; ++s) {
@@ -572,15 +588,35 @@ static int launch_gemm_t(const sce_plan* p, const GemmMaps& maps, int nsets, con
   gp.nsets = nsets;
   gp.k_total = k_total;
   gp.passes = passes;
-  gp.n_models = p->d.n_models;
+  gp.n_models = n_models;
   gp.m_total = m_total;
   gp.n_total = n_total;
   gp.tiles_m = (m_total + kBM - 1) / kBM;
   gp.tiles_n = (n_total + kBN - 1) / kBN;
   gp.epi = epi;
-  CUDA_TRY((launch_gemm<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, NATIVE>(gp, p->device, p->sms, st)));
+  CUDA_TRY((launch_gemm<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, NATIVE>(gp, device, sms, L.st)));
+  ++L.count;
   return SCE_OK;
 }
+
+// One call of a plan: its launches, and the batch of B rows and its tensor maps (run_pipeline opens it)
+struct PlanCall : Launcher {
+  sce_plan* p;
+  BatchMaps* maps;
+  int B;
+  // one GEMM of the plan. NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN
+  // then describe the fp16 planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps
+  // batch-major copies.
+  template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int AR, bool NATIVE = AR == kArithF16F8 && !A_MN, class... A>
+  int gemm(const A&... args) {
+    return launch_gemm_t<Epi, A_MN, B_MN, SPLIT_ACC, AR, NATIVE>(*this, p->d.n_models, p->device, p->sms, args...);
+  }
+  // with sce_profile_begin: the event at the start of phase `idx` of this step (SCE_PHASE_COUNT: the step's end)
+  void mark(int idx) {
+    if (p->prof_on && p->prof_steps < kProfMaxSteps)
+      cudaEventRecord(p->prof_ev[p->prof_steps * (SCE_PHASE_COUNT + 1) + idx], st);
+  }
+};
 
 // ------------------------------------------------------------------------------------------------
 // helpers shared by step / forward / grads
@@ -598,24 +634,32 @@ static AdamHyper hyper_for(const sce_plan* p, long long t) {
   return h;
 }
 
-template <int MODE, int ARITH, bool NONNEG = false>
-static int launch_dict_rows_t(float* e, const float* dw, float* m, float* v, const Planes& w, float* grad_out,
-                              long long rows, int d, int normalize, float floor, AdamHyper h, const uint32_t* health,
-                              float* w_f32, cudaStream_t st) {
-  void *const hi = w.hi, *const lo = w.lo, *const x8 = w.x8;
+// Calls f(arith) with the plan's arithmetic as a compile-time constant (std::integral_constant<int, AR>)
+template <class F>
+static auto with_arith(int arith, F&& f) {
+  return arith == kArithF16F8 ? f(std::integral_constant<int, kArithF16F8>{}) : f(std::integral_constant<int, kArithBf16x3>{});
+}
+
+// Calls f(nv) with the float4s per thread that dict_rows_kernel needs for rows of d values, ceil(d / 512) rounded up
+// to 1, 2, 4, 8 or 16, as a compile-time constant
+template <class F>
+static auto with_row_vectors(int d, F&& f) {
   const int nv = (d + 511) / 512;
-  if (nv == 1)
-    dict_rows_kernel<1, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
-  else if (nv == 2)
-    dict_rows_kernel<2, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
-  else if (nv <= 4)
-    dict_rows_kernel<4, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
-  else if (nv <= 8)    // d <= 4096 (Pythia-6.9b residual width)
-    dict_rows_kernel<8, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
-  else                 // d <= 8192
-    dict_rows_kernel<16, MODE, ARITH, NONNEG><<<(unsigned)rows, 128, 0, st>>>(e, dw, m, v, hi, lo, x8, grad_out, d, normalize, floor, h, health, w_f32);
-  CUDA_TRY(cudaGetLastError());
-  return SCE_OK;
+  if (nv == 1) return f(std::integral_constant<int, 1>{});
+  if (nv == 2) return f(std::integral_constant<int, 2>{});
+  if (nv <= 4) return f(std::integral_constant<int, 4>{});
+  if (nv <= 8) return f(std::integral_constant<int, 8>{});   // d <= 4096 (Pythia-6.9b residual width)
+  return f(std::integral_constant<int, 16>{});                // d <= 8192
+}
+
+template <int MODE, int ARITH, bool NONNEG = false>
+static int launch_dict_rows_t(Launcher& L, float* e, const float* dw, float* m, float* v, const Planes& w,
+                              float* grad_out, long long rows, int d, int normalize, float floor, AdamHyper h,
+                              const uint32_t* health, float* w_f32) {
+  return with_row_vectors(d, [&](auto nv) {
+    return L.launch(dict_rows_kernel<decltype(nv)::value, MODE, ARITH, NONNEG>, (unsigned)rows, 128, 0, e, dw, m, v,
+                    w.hi, w.lo, w.x8, grad_out, d, normalize, floor, h, health, w_f32);
+  });
 }
 // One dictionary of the plan: its weights, their gradient, Adam moments, operand planes and row normalisation
 struct DictSide {
@@ -637,16 +681,10 @@ static int dict_sides(const sce_plan* p, DictSide out[2]) {
   return 2;
 }
 
-// Calls f(arith) with the plan's arithmetic as a compile-time constant (std::integral_constant<int, AR>)
-template <class F>
-static auto with_arith(int arith, F&& f) {
-  return arith == kArithF16F8 ? f(std::integral_constant<int, kArithF16F8>{}) : f(std::integral_constant<int, kArithBf16x3>{});
-}
-
 // MODE_PREPARE reads the weights and writes the planes; MODE_ADAM also reads dW and updates the moments; MODE_GRAD
 // reads the weights and dW and writes `grad_out` only
 template <int MODE>
-static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_out, AdamHyper h, cudaStream_t st) {
+static int launch_dict_rows(Launcher& L, const sce_plan* p, const DictSide& s, float* grad_out, AdamHyper h) {
   const long long rows = (long long)p->d.n_models * p->d.n;
   const float* dw = MODE == MODE_PREPARE ? nullptr : s.dw;
   float* m = MODE == MODE_ADAM ? s.m : nullptr;
@@ -656,26 +694,23 @@ static int launch_dict_rows(const sce_plan* p, const DictSide& s, float* grad_ou
   return with_arith(p->cfg.arith, [&](auto arith) {
     auto run = [&](auto nonneg) {
       return launch_dict_rows_t<MODE, decltype(arith)::value, decltype(nonneg)::value>(
-          s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf, st);
+          L, s.w, dw, m, v, w, grad_out, rows, p->d.d, s.normalize, s.floor, h, p->res_flags, wf);
     };
     return p->cfg.nonneg ? run(std::true_type{}) : run(std::false_type{});   // (nonneg: tied plans only, one side)
   });
 }
 
 // f16f8: the decoder's planes -> their transposed copy, which the decode GEMM reads K-major (nothing to do where the
-// decode runs without the GEMM: k-sparse top-k plans). Adds its launches to `launches`.
-static int transpose_dict(const sce_plan* p, cudaStream_t st, int& launches) {
+// decode runs without the GEMM: k-sparse top-k plans)
+static int transpose_dict(Launcher& L, const sce_plan* p) {
   if (p->cfg.arith != kArithF16F8 || p->cfg.topk_sparse) return SCE_OK;
   const sce_desc& d = p->d;
   const dim3 grid((d.d + 63) / 64, (d.n + 63) / 64, d.n_models);
-  transpose_kernel<uint16_t><<<grid, 256, 0, st>>>(static_cast<const uint16_t*>(p->wdec.hi),
-                                                   static_cast<uint16_t*>(p->wdt.hi), d.n, d.d);
-  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(p->wdec.lo),
-                                                  static_cast<uint8_t*>(p->wdt.lo), d.n, d.d);
-  transpose_kernel<uint8_t><<<grid, 256, 0, st>>>(p->wdec.x8, p->wdt.x8, d.n, d.d);
-  CUDA_TRY(cudaGetLastError());
-  launches += 3;
-  return SCE_OK;
+  TRY(L.launch(transpose_kernel<uint16_t>, grid, 256, 0, static_cast<const uint16_t*>(p->wdec.hi),
+               static_cast<uint16_t*>(p->wdt.hi), d.n, d.d));
+  TRY(L.launch(transpose_kernel<uint8_t>, grid, 256, 0, static_cast<const uint8_t*>(p->wdec.lo),
+               static_cast<uint8_t*>(p->wdt.lo), d.n, d.d));
+  return L.launch(transpose_kernel<uint8_t>, grid, 256, 0, p->wdec.x8, p->wdt.x8, d.n, d.d);
 }
 
 // f16f8 runs the backward pass on the residual r instead of g = 2r/(B d) (EpiDecodeT): weight- and bias-gradient
@@ -694,107 +729,95 @@ struct TypeTag {
   using type = T;
 };
 
-// forward (+ optional backward GEMMs). Leaves dW in p->dw_enc / p->dw_dec when `backward`.
-// `mom_part` (forward only, SAE variants): the encode epilogue also writes the moment partials of EpiEncodeT<AR, true>.
+// ------------------------------------------------------------------------------------------------
+// the pipeline: the phases of a forward pass and its backward GEMMs, in launch order (run_pipeline_t)
+// ------------------------------------------------------------------------------------------------
+// the activity masks [c > 0] / [z == 0] that encode (or the top-k selection) writes and the code gradient reads
+// (top-k: relu semantics, no gradient at exactly 0, no [z == 0] mask)
+static ActMask act_mask(const sce_plan* p) {
+  return {p->act_pos, p->cfg.topk ? nullptr : p->act_zero, (p->d.n + 31) / 32, p->d.batch_max};
+}
+
+// top-k: the k-sparse lists the selection writes and the gather and scatter kernels read
+static TopkLists topk_lists(const sce_plan* p) {
+  return {p->tk_col, p->tk_val, p->tk_cnt, p->cfg.tk_kmax, p->d.batch_max};
+}
+
+// dw_native: the batch-major copy T [models][cols][Bp] of the 8-bit planes of P [models][B of batch_max][cols], which
+// the weight gradient reads (dz's are written so by dcode)
+static int batch_major(PlanCall& c, const Planes& P, const Planes& T, int models, int cols) {
+  const BatchPlanes t{{static_cast<const uint8_t*>(P.lo), P.x8}, {static_cast<uint8_t*>(T.lo), T.x8}};
+  const long long Bm = c.p->d.batch_max;
+  return c.launch(transpose_batch_u8_kernel, dim3((cols + 127) / 128, (c.B + 127) / 128, 2 * models), 256, 0, t, models,
+                  c.B, cols, Bm * cols, c.p->cfg.bpad);
+}
+
+// Input: centring or the learned centre's subtraction, the batch split (with the input shift), the batch-major copy of
+// x (`tdw`: a native weight gradient follows) and alpha / B. Points `x` at the fp32 batch the later phases read.
 template <int AR>
-static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool backward, float* out_losses,
-                          float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
-  using EpiEnc = EpiEncodeT<AR>;
-  using EpiDec = EpiDecodeT<AR>;
-  using EpiDecG = EpiDecodeT<AR, true>;
-  using EpiDco = EpiDcodeT<AR>;
+static int input_phase(PlanCall& c, const float*& x, bool tdw) {
   constexpr bool f8 = AR == kArithF16F8;
+  sce_plan* const p = c.p;
   const sce_desc& d = p->d;
   const PlanConfig& cfg = p->cfg;
-  if (int rc = check_rows(p, B, "")) return rc;
-  if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
-  BatchMaps* maps = nullptr;
-  int rc = build_maps(p, B, &maps);
-  if (rc) return rc;
-  int launches = 0;
-  const int M = d.n_models, n = d.n, dd = d.d;
+  const int B = c.B, M = d.n_models, dd = d.d;
   const long long Bm = d.batch_max;
-  const int one[2] = {1, 1};
-  const int xb[2] = {cfg.x_models ? 1 : 0, 1};
-  const int tiles_mB = (B + kBM - 1) / kBM;
-
-  prof_mark(p, SCE_PHASE_SPLIT, st);
+  const long long n4 = (long long)B * dd / 4;   // (the centring kernels: float4s of one model's batch, <= 1024 blocks)
+  const int blocks = (int)((n4 + 255) / 256 < 1024 ? (n4 + 255) / 256 : 1024);
   if (d.centering) {
     // ---- centring (sae_ensemble.py:126-128): (x - trans[m]) -> planes, GEMM with rot[m] (all split passes), * scale[m]
     // -> the per-model fp32 batch every kernel below reads as `x`
-    const long long n4 = (long long)B * dd / 4;
-    const int blocks = (int)((n4 + 255) / 256 < 1024 ? (n4 + 255) / 256 : 1024);
-    center_split_kernel<AR><<<dim3(blocks, M), 256, 0, st>>>(
-        x, d.centering == 2 ? (long long)B * dd : 0, p->b.center_trans, p->x.hi, p->x.lo, p->x.x8, Bm * dd, B, dd);
-    CUDA_TRY(cudaGetLastError());
+    TRY(c.launch(center_split_kernel<AR>, dim3(blocks, M), 256, 0, x, d.centering == 2 ? (long long)B * dd : 0,
+                 p->b.center_trans, p->x.hi, p->x.lo, p->x.x8, Bm * dd, B, dd));
     EpiCenter::Params cp;
     cp.out = p->x_centered;
     cp.model_stride = (long long)B * dd;
     cp.ld = dd;
     cp.col_scale = p->b.center_scale;
-    rc = launch_gemm_t<EpiCenter, false, false, false, AR>(p, maps->center, 1, one, one, dd, 3, B, dd, cp, st);
-    if (rc) return rc;
-    launches += 2;
+    TRY((c.gemm<EpiCenter, false, false, false, AR>(c.maps->center, 1, kOnes, kOnes, dd, 3, B, dd, cp)));
     x = p->x_centered;
   } else if (cfg.learned) {
     // ---- learned centre (sae_ensemble.py:198-200): x - center[m] -> the per-model fp32 batch every kernel below reads
-    const long long n4 = (long long)B * dd / 4;
-    const int blocks = (int)((n4 + 255) / 256 < 1024 ? (n4 + 255) / 256 : 1024);
-    center_sub_kernel<<<dim3(blocks, M), 256, 0, st>>>(x, d.x_per_model ? (long long)B * dd : 0, p->b.center,
-                                                       p->x_centered, B, dd);
-    CUDA_TRY(cudaGetLastError());
-    ++launches;
+    TRY(c.launch(center_sub_kernel, dim3(blocks, M), 256, 0, x, d.x_per_model ? (long long)B * dd : 0, p->b.center,
+                 p->x_centered, B, dd));
     x = p->x_centered;
   }
   // ---- x -> (hi, lo): per model slabs are batch_max apart in the workspace. input_shift (mlp_tests.py:104): the split
   // forms x + shift once, as the caller laid the batch out, and every kernel below reads that shifted batch
-  if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), st));
-  for (int m = 0; m < cfg.xm; ++m) {
-    launch_split_rows<AR>(x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4, f8 ? p->res_flags : nullptr, st,
-                          cfg.shift, cfg.shift != 0.f ? p->x_shifted + (long long)m * B * dd : nullptr);
-    ++launches;
-  }
-  CUDA_TRY(cudaGetLastError());
+  if constexpr (f8) CUDA_TRY(cudaMemsetAsync(p->res_flags, 0, sizeof(uint32_t), c.st));
+  for (int m = 0; m < cfg.xm; ++m)
+    TRY(launch_split_rows<AR>(c, x + (long long)m * B * dd, p->x.at(m * Bm * dd), (long long)B * dd / 4,
+                              f8 ? p->res_flags : nullptr, cfg.shift,
+                              cfg.shift != 0.f ? p->x_shifted + (long long)m * B * dd : nullptr));
   if (cfg.shift != 0.f) x = p->x_shifted;
-  // dw_native: batch-major copies of the 8-bit planes of x, c and g for the weight gradient (dz's are written so by dcode)
-  const bool tdw = f8 && backward && cfg.dw_native;
-  auto batch_major = [&](const Planes& P, const Planes& T, int models, int cols) {
-    const BatchPlanes t{{static_cast<const uint8_t*>(P.lo), P.x8}, {static_cast<uint8_t*>(T.lo), T.x8}};
-    transpose_batch_u8_kernel<<<dim3((cols + 127) / 128, (B + 127) / 128, 2 * models), 256, 0, st>>>(t, models, B, cols,
-                                                                                                 Bm * cols, cfg.bpad);
-    ++launches;
-    return cudaGetLastError();
-  };
-  if (tdw) CUDA_TRY(batch_major(p->x, p->xt, cfg.xm, dd));
+  if (tdw) TRY(batch_major(c, p->x, p->xt, cfg.xm, dd));
   p->code_batch_major = tdw ? 1 : 0;
   // alpha / B, or (f16f8, backward on r = g B d / 2) alpha d / 2
-  l1_over_b_kernel<<<(M + 127) / 128, 128, 0, st>>>(p->b.l1_alpha, p->l1_over_b, M, f8 ? 0.5f * (float)dd : 1.0f / (float)B);
-  ++launches;
-  // the batch's residual-plane flag, for the GEMMs that read x as their A (encode) or B (weight gradient, set 0) operand
-  ResFlags x_is_a, x_is_b;
-  if constexpr (f8) {
-    x_is_a.a[0] = p->res_flags;
-    x_is_b.b[0] = p->res_flags;
-  }
-  ActMask act;
-  act.pos = p->act_pos;
-  act.zero = p->act_zero;
-  act.n_chunks = (n + 31) / 32;
-  act.batch_max = d.batch_max;
-  if (cfg.topk) act.zero = nullptr;   // relu semantics: no gradient at exactly 0
-  // ---- encode
-  prof_mark(p, SCE_PHASE_ENCODE, st);
-  int n_enc_parts;
-  TopkLists tk = {nullptr, nullptr, nullptr, 0, 0};
+  return c.launch(l1_over_b_kernel, (M + 127) / 128, 128, 0, p->b.l1_alpha, p->l1_over_b, M,
+                  f8 ? 0.5f * (float)dd : 1.0f / (float)B);
+}
+
+// Encode: z = x W^T (+b) -> relu -> code planes, activity masks and loss partials in the epilogue (with `mom_part`,
+// also the moment partials of EpiEncodeT<AR, true>); top-k: the scores, then the per-row selection
+template <int AR>
+static int encode_phase(PlanCall& c, bool tdw, float* mom_part) {
+  sce_plan* const p = c.p;
+  const sce_desc& d = p->d;
+  const PlanConfig& cfg = p->cfg;
+  const int B = c.B, M = d.n_models, n = d.n;
+  const int xb[2] = {cfg.x_models ? 1 : 0, 1};
+  const ActMask act = act_mask(p);
+  ResFlags x_is_a;   // the batch's residual-plane flag, for the GEMM that reads x as its A operand
+  if constexpr (AR == kArithF16F8) x_is_a.a[0] = p->res_flags;
   if (!cfg.topk) {
     auto fill = [&](auto& ep) {
-      ep.out_hi = maps->st_c.hi;
-      ep.out_lo = maps->st_c.lo;
-      ep.out_x8 = maps->st_c.x8;
+      ep.out_hi = c.maps->st_c.hi;
+      ep.out_lo = c.maps->st_c.lo;
+      ep.out_x8 = c.maps->st_c.x8;
       ep.bias = p->b.encoder_bias;
       ep.mask = p->b.coef_mask;
       ep.part = p->part_enc;
-      ep.tiles_m = tiles_mB;
+      ep.tiles_m = (B + kBM - 1) / kBM;
       ep.flag_zero = 1;
       ep.act = act;
       ep.tiles_n = (n + kBN - 1) / kBN;
@@ -805,230 +828,233 @@ static int run_pipeline_t(sce_plan* p, const float* x, int B, float* x_hat, bool
       fill(ep);
       ep.mom_part = mom_part;
       ep.row_blocks = (B + 31) / 32;
-      rc = launch_gemm_t<EpiStats, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+      TRY((c.gemm<EpiStats, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep, x_is_a)));
     } else {
-      typename EpiEnc::Params ep;
+      typename EpiEncodeT<AR>::Params ep;
       fill(ep);
-      rc = launch_gemm_t<EpiEnc, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, ep, st, x_is_a);
+      TRY((c.gemm<EpiEncodeT<AR>, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep,
+                                                           x_is_a)));
     }
-    if (rc) return rc;
-    ++launches;
-    n_enc_parts = tiles_mB * 8 * ((n + kBN - 1) / kBN);
-    if (tdw) CUDA_TRY(batch_major(p->c, p->ct, M, n));
-  } else {
-    // scores -> fp32 and the chunk maxima of every row, then per-row selection (code planes, activity mask, k-sparse
-    // lists) from the chunk maxima (the kernel reads whole rows where they cannot bound the k-th largest score)
-    EpiScoresTma::Params sp;
-    sp.out = maps->st_scores;
-    sp.cmax = p->tk_cmax;
-    sp.n_chunks = act.n_chunks;
-    sp.cmax_model_stride = (long long)Bm * act.n_chunks;
-    rc = launch_gemm_t<EpiScoresTma, false, false, false, AR>(p, maps->encode, 1, xb, one, dd, d.fwd_passes, B, n, sp, st, x_is_a);
-    if (rc) return rc;
-    ++launches;
-    CUDA_TRY(opt_in_smem<topk_sparse_kernel<AR>>(112 * 1024, p->device));
-    tk.col = p->tk_col;
-    tk.val = p->tk_val;
-    tk.cnt = p->tk_cnt;
-    tk.kmax = cfg.tk_kmax;
-    tk.batch_max = d.batch_max;
-    // one block per (row, model); scores / codes of model m start at m * batch_max * n
-    topk_select2_kernel<AR><<<dim3(B, M), 256, 0, st>>>(
-        p->scores, p->b.sparsity, p->c.hi, p->c.lo, p->c.x8, cfg.topk_sparse ? p->dz.hi : nullptr, p->dz.lo, p->dz.x8,
-        act, tk, p->part_enc, B, n, Bm * n, p->tk_cmax);
-    ++launches;
-    CUDA_TRY(cudaGetLastError());
-    n_enc_parts = B;
+    return tdw ? batch_major(c, p->c, p->ct, M, n) : SCE_OK;
   }
+  // scores -> fp32 and the chunk maxima of every row, then per-row selection (code planes, activity mask, k-sparse
+  // lists) from the chunk maxima (the kernel reads whole rows where they cannot bound the k-th largest score)
+  EpiScoresTma::Params sp;
+  sp.out = c.maps->st_scores;
+  sp.cmax = p->tk_cmax;
+  sp.n_chunks = act.n_chunks;
+  sp.cmax_model_stride = (long long)d.batch_max * act.n_chunks;
+  TRY((c.gemm<EpiScoresTma, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, sp, x_is_a)));
+  // one block per (row, model); scores / codes of model m start at m * batch_max * n
+  return c.launch(topk_select2_kernel<AR>, dim3(B, M), 256, 0, p->scores, p->b.sparsity, p->c.hi, p->c.lo, p->c.x8,
+                  cfg.topk_sparse ? p->dz.hi : nullptr, p->dz.lo, p->dz.x8, act, topk_lists(p), p->part_enc, B, n,
+                  (long long)d.batch_max * n, p->tk_cmax);
+}
 
-  const bool sparse = cfg.topk_sparse;
-  int n_dec_parts;
-  prof_mark(p, SCE_PHASE_DECODE, st);
-  if (sparse) {
-    // ---- k-sparse decode + residual + loss partial + g planes + the code gradient at the selected entries
-    const float gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
+// Decode: x^ = c W -> r = x^ - x, loss partials and the g planes (learned centre: + column sums of g), as the dense GEMM
+// or, in k-sparse top-k plans, as the gather kernel per k class (which also forms the code gradient's shares, `backward`)
+template <int AR>
+static int decode_phase(PlanCall& c, const float* x, float* x_hat, bool backward, bool tdw) {
+  constexpr bool f8 = AR == kArithF16F8;
+  sce_plan* const p = c.p;
+  const sce_desc& d = p->d;
+  const PlanConfig& cfg = p->cfg;
+  const int B = c.B, M = d.n_models, n = d.n, dd = d.d;
+  const float gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
+  if (cfg.topk_sparse) {
+    CUDA_TRY(opt_in_smem<topk_sparse_kernel<AR>>(112 * 1024, p->device));
     // one launch per k class (sce_prepare sorted the models): a block's shared memory goes with ITS models' k, so the
     // k = 16 and k = 32 models of a mixed ensemble run at 5 and 3 blocks per SM instead of the 2 that k_max = 64 allows
     for (int g = 0; g < p->tk_groups; ++g) {
       const int cnt = p->tk_group_off[g + 1] - p->tk_group_off[g];
       if (cnt == 0) continue;
-      topk_sparse_kernel<AR><<<dim3(B, cnt, cfg.tk_slices), 256, topk_sparse_smem(d, p->tk_group_krows[g], cfg.tk_slices), st>>>(
-          tk, p->b.sparsity, p->wn_f32, x, d.x_per_model ? (long long)B * dd : 0, p->g.hi, p->g.lo, p->g.x8, x_hat, p->part_dec,
-          backward ? p->tk_dots : nullptr, B, n, dd, gscale, p->tk_models + p->tk_group_off[g], p->tk_group_krows[g]);
-      ++launches;
+      TRY(c.launch(topk_sparse_kernel<AR>, dim3(B, cnt, cfg.tk_slices), 256,
+                   topk_sparse_smem(d, p->tk_group_krows[g], cfg.tk_slices), topk_lists(p), p->b.sparsity, p->wn_f32, x,
+                   d.x_per_model ? (long long)B * dd : 0, p->g.hi, p->g.lo, p->g.x8, x_hat, p->part_dec,
+                   backward ? p->tk_dots : nullptr, B, n, dd, gscale, p->tk_models + p->tk_group_off[g],
+                   p->tk_group_krows[g]));
     }
-    CUDA_TRY(cudaGetLastError());
-    n_dec_parts = cfg.tk_slices * B;
+    return SCE_OK;
+  }
+  auto decode = [&](auto tag) {
+    using E = typename decltype(tag)::type;
+    typename E::Params dp;
+    dp.x = x;
+    dp.x_model_stride = cfg.x_models ? (long long)B * dd : 0;
+    dp.g_hi = static_cast<uint16_t*>(p->g.hi);
+    dp.g_lo = static_cast<uint8_t*>(p->g.lo);
+    dp.g_x8 = p->g.x8;
+    dp.x_hat = x_hat;
+    dp.part = p->part_dec;
+    dp.g_model_stride = (long long)d.batch_max * dd;
+    dp.xhat_model_stride = (long long)B * dd;
+    dp.ld = dd;
+    dp.tiles_m = (B + kBM - 1) / kBM;
+    dp.gscale = gscale;
+    dp.tiles_n = (dd + kBN - 1) / kBN;
+    if constexpr (!std::is_same<E, EpiDecodeT<AR>>::value) dp.g_part = p->g_part;
+    if constexpr (f8)
+      return c.gemm<E, false, false, false, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
+    else if (cfg.split_decode)
+      return c.gemm<E, false, true, true, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
+    else
+      return c.gemm<E, false, true, false, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
+  };
+  TRY(cfg.learned ? decode(TypeTag<EpiDecodeT<AR, true>>{}) : decode(TypeTag<EpiDecodeT<AR>>{}));
+  return tdw ? batch_major(c, p->g, p->gt, M, dd) : SCE_OK;
+}
+
+// Losses: the bias norm (bias decay), then the loss columns and nnz from the partials of encode and decode
+static int losses_phase(PlanCall& c, float* out_losses, float* out_nnz) {
+  sce_plan* const p = c.p;
+  const sce_desc& d = p->d;
+  const int B = c.B, M = d.n_models, tiles_mB = (B + kBM - 1) / kBM;
+  const int n_enc_parts = p->cfg.topk ? B : tiles_mB * 8 * ((d.n + kBN - 1) / kBN);
+  const int n_dec_parts = p->cfg.topk_sparse ? p->cfg.tk_slices * B : tiles_mB * 8 * ((d.d + kBN - 1) / kBN);
+  if (p->b.encoder_bias && p->b.bias_decay) TRY(c.launch(bias_norm_kernel, M, 256, 0, p->b.encoder_bias, d.n, p->bnorm));
+  return c.launch(finalize_kernel, M, 256, 0, p->part_enc, n_enc_parts, p->part_dec, n_dec_parts, p->b.l1_alpha,
+                  p->b.encoder_bias ? p->b.bias_decay : nullptr, p->bnorm, B, d.d, out_losses, out_nnz, p->res_flags);
+}
+
+// Backward: the code gradient (dcode GEMM, or the k-sparse scatter), then the weight gradients into p->dw_enc /
+// p->dw_dec
+template <int AR>
+static int backward_phase(PlanCall& c) {
+  constexpr bool f8 = AR == kArithF16F8;
+  sce_plan* const p = c.p;
+  const sce_desc& d = p->d;
+  const PlanConfig& cfg = p->cfg;
+  const int B = c.B, M = d.n_models, n = d.n, dd = d.d;
+  const int xb[2] = {cfg.x_models ? 1 : 0, 1};
+  if (cfg.topk_sparse) {
+    // ---- code gradient planes: zero the rows, scatter the k entries
+    TRY(c.launch(topk_dz_scatter_kernel<AR>, dim3(B, M), 64, 0, topk_lists(p), p->tk_dots, cfg.tk_slices, p->dz.hi,
+                 p->dz.lo, p->dz.x8, n));
   } else {
-    // ---- decode (+ residual, loss partial, g; learned centre: + column sums of g)
-    auto decode = [&](auto tag) {
+    // ---- dcode
+    auto dcode = [&](auto tag) {
       using E = typename decltype(tag)::type;
-      typename E::Params dp;
-      dp.x = x;
-      dp.x_model_stride = cfg.x_models ? (long long)B * dd : 0;
-      dp.g_hi = static_cast<uint16_t*>(p->g.hi);
-      dp.g_lo = static_cast<uint8_t*>(p->g.lo);
-      dp.g_x8 = p->g.x8;
-      dp.x_hat = x_hat;
-      dp.part = p->part_dec;
-      dp.g_model_stride = Bm * dd;
-      dp.xhat_model_stride = (long long)B * dd;
-      dp.ld = dd;
-      dp.tiles_m = tiles_mB;
-      dp.gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
-      dp.tiles_n = (dd + kBN - 1) / kBN;
-      if constexpr (!std::is_same<E, EpiDec>::value) dp.g_part = p->g_part;
-      if constexpr (f8)
-        return launch_gemm_t<E, false, false, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-      else if (cfg.split_decode)
-        return launch_gemm_t<E, false, true, true, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
-      else
-        return launch_gemm_t<E, false, true, false, AR>(p, maps->decode, 1, one, one, n, d.fwd_passes, B, dd, dp, st);
+      typename E::Params zp;
+      zp.out_hi = c.maps->st_dz.hi;
+      zp.out_lo = c.maps->st_dz.lo;
+      zp.out_x8 = c.maps->st_dz.x8;
+      zp.act = act_mask(p);
+      zp.l1_over_b = p->l1_over_b;
+      zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
+      zp.tiles_m = (B + kBM - 1) / kBM;
+      zp.planes = d.bwd_passes >= 3 ? 3 : 0;
+      // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
+      // (per-model batches carry one flag for all of them, so the same test holds)
+      zp.x_res_flag = f8 ? p->res_flags : nullptr;
+      return c.gemm<E, false, false, false, AR>(c.maps->dcode, 1, kOnes, kOnes, dd, d.bwd_passes, B, n, zp);
     };
-    rc = cfg.learned ? decode(TypeTag<EpiDecG>{}) : decode(TypeTag<EpiDec>{});
-    if (rc) return rc;
-    ++launches;
-    n_dec_parts = tiles_mB * 8 * ((dd + kBN - 1) / kBN);
-    if (tdw) CUDA_TRY(batch_major(p->g, p->gt, M, dd));
+    // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
+    if constexpr (f8) TRY(cfg.dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDcodeT<AR>>{}));
+    else TRY(dcode(TypeTag<EpiDcodeT<AR>>{}));
   }
 
-  // ---- losses
-  prof_mark(p, SCE_PHASE_LOSSES, st);
-  if (p->b.encoder_bias && p->b.bias_decay) {
-    bias_norm_kernel<<<M, 256, 0, st>>>(p->b.encoder_bias, n, p->bnorm);
-    ++launches;
+  // ---- weight gradients
+  c.mark(SCE_PHASE_DW);
+  auto dw = [&](const GemmMaps& gm, int nsets, const int* ab, const int* bb, float* out, const ResFlags& rf) -> int {
+    EpiStoreF32::Params sp;
+    sp.out = out;
+    sp.model_stride = (long long)n * dd;
+    sp.ld = dd;
+    sp.scale = grad_out_scale(p, B);
+    // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one). dw_native: fp16 planes
+    // MN-major, 8-bit planes K-major from their batch-major copies, cross terms on E5M2 wgmma; else widened
+    if constexpr (f8)
+      if (cfg.dw_native)
+        return c.gemm<EpiStoreF32, true, true, false, AR, true>(gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
+    return c.gemm<EpiStoreF32, true, true, !f8, AR>(gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
+  };
+  ResFlags x_is_b;   // the batch's residual-plane flag, for the GEMM that reads x as its B operand (set 0)
+  if constexpr (f8) x_is_b.b[0] = p->res_flags;
+  if (!cfg.untied) {
+    const int bb[2] = {xb[0], 1};
+    return dw(c.maps->dw_enc, 2, kOnes, bb, p->dw_enc, x_is_b);
   }
-  finalize_kernel<<<M, 256, 0, st>>>(p->part_enc, n_enc_parts, p->part_dec, n_dec_parts, p->b.l1_alpha,
-                                     p->b.encoder_bias ? p->b.bias_decay : nullptr, p->bnorm, B, dd, out_losses, out_nnz,
-                                     p->res_flags);
-  ++launches;
-  CUDA_TRY(cudaGetLastError());
+  TRY(dw(c.maps->dw_enc, 1, kOnes, xb, p->dw_enc, x_is_b));
+  return dw(c.maps->dw_dec, 1, kOnes, kOnes, p->dw_dec, ResFlags());
+}
 
-  prof_mark(p, SCE_PHASE_DCODE, st);
-  if (backward) {
-    if (sparse) {
-      // ---- code gradient planes: zero the rows, scatter the k entries
-      topk_dz_scatter_kernel<AR><<<dim3(B, M), 64, 0, st>>>(tk, p->tk_dots, cfg.tk_slices, p->dz.hi, p->dz.lo, p->dz.x8, n);
-      ++launches;
-      CUDA_TRY(cudaGetLastError());
-    } else {
-      // ---- dcode
-      auto dcode = [&](auto tag) {
-        using E = typename decltype(tag)::type;
-        typename E::Params zp;
-        zp.out_hi = maps->st_dz.hi;
-        zp.out_lo = maps->st_dz.lo;
-        zp.out_x8 = maps->st_dz.x8;
-        zp.act = act;
-        zp.l1_over_b = p->l1_over_b;
-        zp.db_part = p->b.encoder_bias ? p->db_part : nullptr;
-        zp.tiles_m = tiles_mB;
-        zp.planes = d.bwd_passes >= 3 ? 3 : 0;
-        // the only reader of dz's value plane is the dz^T x term of the weight gradient, against x's residual plane
-        // (per-model batches carry one flag for all of them, so the same test holds)
-        zp.x_res_flag = f8 ? p->res_flags : nullptr;
-        return launch_gemm_t<E, false, false, false, AR>(p, maps->dcode, 1, one, one, dd, d.bwd_passes, B, n, zp, st);
-      };
-      // dw_native: dz's 8-bit planes are written batch-major, as the native weight gradient reads them
-      if constexpr (f8) rc = cfg.dw_native ? dcode(TypeTag<EpiDcodeT<AR, true>>{}) : dcode(TypeTag<EpiDco>{});
-      else rc = dcode(TypeTag<EpiDco>{});
-      if (rc) return rc;
-      ++launches;
-    }
-
-    // ---- weight gradients
-    prof_mark(p, SCE_PHASE_DW, st);
-    auto dw = [&](const GemmMaps& gm, int nsets, const int* ab, const int* bb, float* out, const ResFlags& rf) -> int {
-      EpiStoreF32::Params sp;
-      sp.out = out;
-      sp.model_stride = (long long)n * dd;
-      sp.ld = dd;
-      sp.scale = grad_out_scale(p, B);
-      // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one). dw_native: fp16 planes
-      // MN-major, 8-bit planes K-major from their batch-major copies, cross terms on E5M2 wgmma; else widened
-      if constexpr (f8)
-        if (cfg.dw_native)
-          return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(p, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, st, rf);
-      return launch_gemm_t<EpiStoreF32, true, true, !f8, AR>(p, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, st, rf);
-    };
-    if (cfg.untied) {
-      rc = dw(maps->dw_enc, 1, one, xb, p->dw_enc, x_is_b);
-      if (rc) return rc;
-      rc = dw(maps->dw_dec, 1, one, one, p->dw_dec, ResFlags());
-      if (rc) return rc;
-      launches += 2;
-    } else {
-      const int bb[2] = {xb[0], 1};
-      rc = dw(maps->dw_enc, 2, one, bb, p->dw_enc, x_is_b);
-      if (rc) return rc;
-      ++launches;
-    }
-  }
-  prof_mark(p, SCE_PHASE_ADAM, st);
-  p->last_launches = launches;
+// The forward pass on the rows of `x` (+ the backward GEMMs, which leave dW in p->dw_enc / p->dw_dec, when `backward`),
+// with the profile marks at its phase boundaries. `mom_part` (forward only, SAE variants): the encode epilogue also
+// writes the moment partials of EpiEncodeT<AR, true>.
+template <int AR>
+static int run_pipeline_t(PlanCall& c, const float* x, float* x_hat, bool backward, float* out_losses, float* out_nnz,
+                          float* mom_part) {
+  const bool tdw = AR == kArithF16F8 && backward && c.p->cfg.dw_native;
+  c.mark(SCE_PHASE_SPLIT);
+  TRY(input_phase<AR>(c, x, tdw));
+  c.mark(SCE_PHASE_ENCODE);
+  TRY(encode_phase<AR>(c, tdw, mom_part));
+  c.mark(SCE_PHASE_DECODE);
+  TRY(decode_phase<AR>(c, x, x_hat, backward, tdw));
+  c.mark(SCE_PHASE_LOSSES);
+  TRY(losses_phase(c, out_losses, out_nnz));
+  c.mark(SCE_PHASE_DCODE);
+  if (backward) TRY(backward_phase<AR>(c));
+  c.mark(SCE_PHASE_ADAM);
   return SCE_OK;
 }
 
-static int run_pipeline(sce_plan* p, const float* x, int B, float* x_hat, bool backward, float* out_losses,
-                        float* out_nnz, cudaStream_t st, float* mom_part = nullptr) {
+// Opens call `c` of plan `p` on `st` for the B rows of `x` (checks them, finds or builds the batch's tensor maps) and
+// runs the pipeline in it
+static int run_pipeline(PlanCall& c, sce_plan* p, const float* x, int B, cudaStream_t st, float* x_hat, bool backward,
+                        float* out_losses, float* out_nnz, float* mom_part = nullptr) {
+  TRY(check_rows(p, B, ""));
+  if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
+  c = PlanCall{{st}, p, nullptr, B};
+  TRY(build_maps(p, B, &c.maps));
   return with_arith(p->cfg.arith, [&](auto arith) {
-    return run_pipeline_t<decltype(arith)::value>(p, x, B, x_hat, backward, out_losses, out_nnz, st, mom_part);
+    return run_pipeline_t<decltype(arith)::value>(c, x, x_hat, backward, out_losses, out_nnz, mom_part);
   });
 }
 
 // Learned-centre plans: the centre gradient of the last backward pass into p->center_grad (sum_b g - db W, with db and
 // W those of this step: it runs before dict_rows_kernel<MODE_ADAM> rewrites the encoder), and with MODE_ADAM the Adam
-// update of the centre. Adds its launches to `launches`.
+// update of the centre
 template <int MODE>
-static int center_grad_launches(sce_plan* p, int B, const AdamHyper& h, cudaStream_t st, int& launches) {
+static int center_grad_launches(PlanCall& c, const AdamHyper& h) {
+  sce_plan* const p = c.p;
   const sce_desc& d = p->d;
   const int M = d.n_models, n = d.n, dd = d.d;
-  const int n_part = ((B + kBM - 1) / kBM) * 4;
+  const int n_part = ((c.B + kBM - 1) / kBM) * 4;
   const int chunks = (n + kCenterChunkRows - 1) / kCenterChunkRows;
-  const float scale = grad_out_scale(p, B);
-  center_coef_kernel<<<dim3((n + kCenterCoefRows - 1) / kCenterCoefRows, M), 256, 0, st>>>(
-      p->b.encoder, p->db_part, n_part, n, dd, d.norm_floor, scale, p->center_coef);
-  center_gemv_kernel<<<dim3((dd + 511) / 512, chunks, M), 128, 0, st>>>(p->b.encoder, p->center_coef, n, dd, p->center_part);
+  const float scale = grad_out_scale(p, c.B);
+  TRY(c.launch(center_coef_kernel, dim3((n + kCenterCoefRows - 1) / kCenterCoefRows, M), 256, 0, p->b.encoder, p->db_part,
+               n_part, n, dd, d.norm_floor, scale, p->center_coef));
+  TRY(c.launch(center_gemv_kernel, dim3((dd + 511) / 512, chunks, M), 128, 0, p->b.encoder, p->center_coef, n, dd,
+               p->center_part));
   const long long tot = (long long)M * dd;
-  center_grad_kernel<MODE><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
-      p->g_part, n_part, scale, p->center_part, chunks, M, dd, p->center_grad, MODE == MODE_ADAM ? p->b.center : nullptr,
-      MODE == MODE_ADAM ? p->b.center_m : nullptr, MODE == MODE_ADAM ? p->b.center_v : nullptr, h,
-      MODE == MODE_ADAM ? p->res_flags : nullptr);
-  CUDA_TRY(cudaGetLastError());
-  launches += 3;
-  return SCE_OK;
+  return c.launch(center_grad_kernel<MODE>, (unsigned)((tot + 255) / 256), 256, 0, p->g_part, n_part, scale,
+                  p->center_part, chunks, M, dd, p->center_grad, MODE == MODE_ADAM ? p->b.center : nullptr,
+                  MODE == MODE_ADAM ? p->b.center_m : nullptr, MODE == MODE_ADAM ? p->b.center_v : nullptr, h,
+                  MODE == MODE_ADAM ? p->res_flags : nullptr);
 }
 
 // What follows the backward pass, in order: the centre gradient (learned centre), dict_rows per dictionary side, the
 // decoder's transposed planes (MODE_ADAM) and the bias kernel. MODE_ADAM updates the parameters; MODE_GRAD writes the
-// gradients to grad_out[side] and d_bias, skipping a launch whose output is null. Adds its launches to `launches`.
+// gradients to grad_out[side] and d_bias, skipping a launch whose output is null.
 template <int MODE>
-static int train_tail(sce_plan* p, int B, const AdamHyper& h, float* const* grad_out, float* d_bias, cudaStream_t st,
-                      int& launches) {
+static int train_tail(PlanCall& c, const AdamHyper& h, float* const* grad_out, float* d_bias) {
   constexpr bool adam = MODE == MODE_ADAM;
-  int rc;
-  if (p->cfg.learned && (rc = center_grad_launches<MODE>(p, B, h, st, launches))) return rc;
+  sce_plan* const p = c.p;
+  if (p->cfg.learned) TRY(center_grad_launches<MODE>(c, h));
   DictSide sides[2];
-  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s) {
-    if (!adam && !grad_out[s]) continue;
-    if ((rc = launch_dict_rows<MODE>(p, sides[s], adam ? nullptr : grad_out[s], h, st))) return rc;
-    ++launches;
-  }
-  if (adam && (rc = transpose_dict(p, st, launches))) return rc;
-  if (p->b.encoder_bias && (adam || d_bias)) {
-    const sce_desc& d = p->d;
-    const long long tot = (long long)d.n_models * d.n;
-    const int n_part = ((B + kBM - 1) / kBM) * 4;
-    bias_kernel<MODE><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(
-        p->b.encoder_bias, adam ? p->b.bias_m : nullptr, adam ? p->b.bias_v : nullptr, p->db_part, n_part, d.n,
-        d.n_models, p->b.bias_decay, p->bnorm, adam ? nullptr : d_bias, h, grad_out_scale(p, B),
-        adam ? p->res_flags : nullptr);
-    CUDA_TRY(cudaGetLastError());
-    ++launches;
-  }
-  return SCE_OK;
+  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
+    if (adam || grad_out[s]) TRY(launch_dict_rows<MODE>(c, p, sides[s], adam ? nullptr : grad_out[s], h));
+  if (adam) TRY(transpose_dict(c, p));
+  if (!p->b.encoder_bias || !(adam || d_bias)) return SCE_OK;
+  const sce_desc& d = p->d;
+  const long long tot = (long long)d.n_models * d.n;
+  const int n_part = ((c.B + kBM - 1) / kBM) * 4;
+  return c.launch(bias_kernel<MODE>, (unsigned)((tot + 255) / 256), 256, 0, p->b.encoder_bias,
+                  adam ? p->b.bias_m : nullptr, adam ? p->b.bias_v : nullptr, p->db_part, n_part, d.n, d.n_models,
+                  p->b.bias_decay, p->bnorm, adam ? nullptr : d_bias, h, grad_out_scale(p, c.B),
+                  adam ? p->res_flags : nullptr);
 }
-
 
 // ------------------------------------------------------------------------------------------------
 // evaluation statistics (sce_forward_stats): per-feature moments and segment activity counts
@@ -1285,12 +1311,12 @@ static size_t frag_workspace(const sce_desc& d, int B, int L, size_t* off_active
 }
 
 template <int ARITH, bool TOPK>
-static void launch_fragments(const FragCode& c, int M, int L, int G, long long frag0, float* fmax, uint8_t* active,
-                             int n_top, int n_random, unsigned long long seed, float* top_val, long long* top_frag,
-                             float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act, cudaStream_t st) {
-  fragment_max_kernel<ARITH, TOPK><<<dim3(c.n_chunks, G, M), 256, 0, st>>>(c, L, G, fmax, active);
-  fragment_merge_kernel<ARITH, TOPK><<<dim3((c.n + 127) / 128, M), 128, 0, st>>>(
-      c, L, G, frag0, fmax, active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
+static int launch_fragments(Launcher& launcher, const FragCode& c, int M, int L, int G, long long frag0, float* fmax,
+                            uint8_t* active, int n_top, int n_random, unsigned long long seed, float* top_val,
+                            long long* top_frag, float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act) {
+  TRY(launcher.launch(fragment_max_kernel<ARITH, TOPK>, dim3(c.n_chunks, G, M), 256, 0, c, L, G, fmax, active));
+  return launcher.launch(fragment_merge_kernel<ARITH, TOPK>, dim3((c.n + 127) / 128, M), 128, 0, c, L, G, frag0, fmax,
+                         active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1368,67 +1394,40 @@ static size_t sim_workspace(long long ma, long long na, long long mb, long long 
 // fp32 operand -> planes: normalised rows (dict_rows_kernel<MODE_PREPARE>, LearnedDict.get_learned_dict) or the matrix
 // as given (split_rows_kernel; f16f8: sets the range flags when a value does not fit fp16)
 template <int AR>
-static int sim_planes(const SimOperand& o, int d, const Planes& w, uint32_t* flags, cudaStream_t st) {
+static int sim_planes(Launcher& L, const SimOperand& o, int d, const Planes& w, uint32_t* flags) {
   const long long rows = (long long)o.models * o.rows;
   if (o.normalize)
-    return launch_dict_rows_t<MODE_PREPARE, AR>(const_cast<float*>(o.w), nullptr, nullptr, nullptr, w, nullptr, rows, d, 1,
-                                                 o.floor, AdamHyper{}, nullptr, nullptr, st);
-  launch_split_rows<AR>(o.w, w, rows * d / 4, AR == kArithF16F8 ? flags : nullptr, st);
-  CUDA_TRY(cudaGetLastError());
-  return SCE_OK;
+    return launch_dict_rows_t<MODE_PREPARE, AR>(L, const_cast<float*>(o.w), nullptr, nullptr, nullptr, w, nullptr, rows, d,
+                                                 1, o.floor, AdamHyper{}, nullptr, nullptr);
+  return launch_split_rows<AR>(L, o.w, w, rows * d / 4, AR == kArithF16F8 ? flags : nullptr);
 }
 
 template <int AR>
-static int run_similarity_t(const SimOperand& A, const SimOperand& B, bool b_is_a, int d, int n_pairs, const SimCarve& w,
-                            float* row_max, float* col_max, float* capacity, int device, int sms, cudaStream_t st) {
-  int rc = sim_planes<AR>(A, d, w.a, w.flags, st);
-  if (rc) return rc;
-  if (!b_is_a) {
-    rc = sim_planes<AR>(B, d, w.b, w.flags, st);
-    if (rc) return rc;
-  }
-  GemmParams<EpiSimilarity::Params> gp;
-  memset(&gp, 0, sizeof(gp));
+static int run_similarity_t(Launcher& L, const SimOperand& A, const SimOperand& B, bool b_is_a, int d, int n_pairs,
+                            const SimCarve& w, float* row_max, float* col_max, float* capacity, int device, int sms) {
+  TRY(sim_planes<AR>(L, A, d, w.a, w.flags));
+  if (!b_is_a) TRY(sim_planes<AR>(L, B, d, w.b, w.flags));
   // both operands are dictionary rows, K-major over d: the encode GEMM's B-operand geometry on both sides
-  OperandMaps am{}, bm{};
-  bool ok = operand_maps(am, w.a, A.models, A.rows, d, (uint64_t)A.rows * d, kBM, gemm_bk(AR));
-  ok = ok && operand_maps(bm, b_is_a ? w.a : w.b, B.models, B.rows, d, (uint64_t)B.rows * d, kBN, gemm_bk(AR));
+  GemmMaps maps{};
+  bool ok = operand_maps(maps.a[0], w.a, A.models, A.rows, d, (uint64_t)A.rows * d, kBM, gemm_bk(AR));
+  ok = ok && operand_maps(maps.b[0], b_is_a ? w.a : w.b, B.models, B.rows, d, (uint64_t)B.rows * d, kBN, gemm_bk(AR));
   if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (similarity: na=%d, nb=%d, d=%d)", A.rows, B.rows, d);
-  set_operand_maps(gp, 0, am, bm);
-  gp.a_batched[0] = gp.b_batched[0] = 1;
-  gp.nsets = 1;
-  gp.k_total = d;
-  gp.passes = 3;
-  gp.n_models = n_pairs;
-  gp.m_total = A.rows;
-  gp.n_total = B.rows;
-  gp.tiles_m = (A.rows + kBM - 1) / kBM;
-  gp.tiles_n = (B.rows + kBN - 1) / kBN;
-  gp.epi.pairs = w.pairs;
-  gp.epi.a_rows = w.a_rows;
-  gp.epi.b_rows = w.b_rows;
-  gp.epi.row_max = reinterpret_cast<uint32_t*>(row_max);
-  gp.epi.col_max = reinterpret_cast<uint32_t*>(col_max);
-  gp.epi.sq_part = capacity ? w.sq_part : nullptr;
-  gp.epi.diag = w.diag;
-  gp.epi.tiles_n = gp.tiles_n;
-  if (row_max) CUDA_TRY(cudaMemsetAsync(row_max, 0, (size_t)n_pairs * A.rows * sizeof(float), st));
-  if (col_max) CUDA_TRY(cudaMemsetAsync(col_max, 0, (size_t)n_pairs * B.rows * sizeof(float), st));
-  CUDA_TRY((launch_gemm<EpiSimilarity, false, false, false, AR, AR == kArithF16F8>(gp, device, sms, st)));
-  auto to_float = [&](float* v, long long n) -> int {
+  const int tiles_n = (B.rows + kBN - 1) / kBN;
+  const EpiSimilarity::Params ep{w.pairs, w.a_rows, w.b_rows, reinterpret_cast<uint32_t*>(row_max),
+                                 reinterpret_cast<uint32_t*>(col_max), capacity ? w.sq_part : nullptr, w.diag, tiles_n};
+  if (row_max) CUDA_TRY(cudaMemsetAsync(row_max, 0, (size_t)n_pairs * A.rows * sizeof(float), L.st));
+  if (col_max) CUDA_TRY(cudaMemsetAsync(col_max, 0, (size_t)n_pairs * B.rows * sizeof(float), L.st));
+  TRY((launch_gemm_t<EpiSimilarity, false, false, false, AR, AR == kArithF16F8>(L, n_pairs, device, sms, maps, 1, kOnes,
+                                                                                  kOnes, d, 3, A.rows, B.rows, ep)));
+  auto to_float = [&](float* v, long long n) {
     const int blocks = (int)((n + 255) / 256 < 1024 ? (n + 255) / 256 : 1024);
-    key_to_float_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<uint32_t*>(v), n);
-    CUDA_TRY(cudaGetLastError());
-    return SCE_OK;
+    return L.launch(key_to_float_kernel, blocks, 256, 0, reinterpret_cast<uint32_t*>(v), n);
   };
-  if (row_max && (rc = to_float(row_max, (long long)n_pairs * A.rows))) return rc;
-  if (col_max && (rc = to_float(col_max, (long long)n_pairs * B.rows))) return rc;
-  if (capacity) {
-    capacity_kernel<<<dim3((A.rows + 255) / 256, n_pairs), 256, 0, st>>>(w.pairs, w.a_rows, w.sq_part, w.diag, A.rows,
-                                                                       2 * gp.tiles_n, capacity);
-    CUDA_TRY(cudaGetLastError());
-  }
-  return SCE_OK;
+  if (row_max) TRY(to_float(row_max, (long long)n_pairs * A.rows));
+  if (col_max) TRY(to_float(col_max, (long long)n_pairs * B.rows));
+  if (!capacity) return SCE_OK;
+  return L.launch(capacity_kernel, dim3((A.rows + 255) / 256, n_pairs), 256, 0, w.pairs, w.a_rows, w.sq_part, w.diag,
+                  A.rows, 2 * tiles_n, capacity);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1552,35 +1551,35 @@ int sce_prepare(sce_plan* p, void* stream) {
     CUDA_TRY(cudaMemcpyAsync(p->tk_models, order.data(), order.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));   // (`order` is a local)
   }
+  Launcher L{st};
   if (d.centering) {
     if (!p->b.center_trans || !p->b.center_rot || !p->b.center_scale)
       return fail(SCE_ERR_INVALID, "centering needs the center_trans / center_rot / center_scale buffers");
     const long long n4 = (long long)d.n_models * d.d * d.d / 4;
-    with_arith(p->cfg.arith,
-               [&](auto arith) { launch_split_rows<decltype(arith)::value>(p->b.center_rot, p->rot, n4, nullptr, st); });
-    CUDA_TRY(cudaGetLastError());
+    TRY(with_arith(p->cfg.arith, [&](auto arith) {
+      return launch_split_rows<decltype(arith)::value>(L, p->b.center_rot, p->rot, n4, nullptr);
+    }));
   }
   DictSide sides[2];
   for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
-    if (int rc = launch_dict_rows<MODE_PREPARE>(p, sides[s], nullptr, hyper_for(p, 1), st)) return rc;
-  int launches = 0;
-  return transpose_dict(p, st, launches);
+    TRY(launch_dict_rows<MODE_PREPARE>(L, p, sides[s], nullptr, hyper_for(p, 1)));
+  return transpose_dict(L, p);
 }
 
 int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_losses, float* out_nnz, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
-  return run_pipeline(p, x, B, x_hat, false, out_losses, out_nnz, static_cast<cudaStream_t>(stream));
+  PlanCall c;
+  TRY(run_pipeline(c, p, x, B, static_cast<cudaStream_t>(stream), x_hat, false, out_losses, out_nnz));
+  p->last_launches = c.count;
+  return SCE_OK;
 }
 
-// every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph)
-static int step_launches(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
+// every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph), counted in `c`
+static int step_launches(PlanCall& c, sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
                          cudaStream_t st) {
-  int rc = run_pipeline(p, x, B, nullptr, true, out_losses, out_nnz, st);
-  if (rc) return rc;
-  int launches = p->last_launches;
-  if ((rc = train_tail<MODE_ADAM>(p, B, hyper_for(p, t), nullptr, nullptr, st, launches))) return rc;
-  prof_mark(p, SCE_PHASE_COUNT, st);
-  p->last_launches = launches;
+  TRY(run_pipeline(c, p, x, B, st, nullptr, true, out_losses, out_nnz));
+  TRY(train_tail<MODE_ADAM>(c, hyper_for(p, t), nullptr, nullptr));
+  c.mark(SCE_PHASE_COUNT);
   return SCE_OK;
 }
 
@@ -1600,9 +1599,10 @@ int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_n
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = check_rows(p, B, "")) return rc;
   if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
+  PlanCall c;
   int rc;
   if (!graph_eligible(p)) {
-    rc = step_launches(p, x, B, out_losses, out_nnz, p->step + 1, st);
+    rc = step_launches(c, p, x, B, out_losses, out_nnz, p->step + 1, st);
   } else {
     BatchMaps* maps = nullptr;
     rc = build_maps(p, B, &maps);
@@ -1615,18 +1615,17 @@ int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_n
     float* const cap_nnz = p->nnz_stage;
     if (maps->graph) {
       CUDA_TRY(cudaGraphLaunch(maps->graph, st));
-      p->last_launches = maps->graph_launches;
-      rc = SCE_OK;
+      c.count = maps->graph_launches;
     } else if (maps->eager_steps == 0) {
       maps->eager_steps = 1;
-      rc = step_launches(p, p->x_stage, B, cap_losses, cap_nnz, 1, st);
+      rc = step_launches(c, p, p->x_stage, B, cap_losses, cap_nnz, 1, st);
     } else {
       // capture on a private stream (the caller's may be the legacy default stream, which cannot be captured);
       // capturing records the launches without running them, the instantiated graph is launched on `st`
       cudaGraph_t g = nullptr;
       if (!p->cap_stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->cap_stream, cudaStreamNonBlocking));
       CUDA_TRY(cudaStreamBeginCapture(p->cap_stream, cudaStreamCaptureModeThreadLocal));
-      rc = step_launches(p, p->x_stage, B, cap_losses, cap_nnz, 1, p->cap_stream);
+      rc = step_launches(c, p, p->x_stage, B, cap_losses, cap_nnz, 1, p->cap_stream);
       cudaError_t ce = cudaStreamEndCapture(p->cap_stream, &g);
       if (rc == SCE_OK && ce == cudaSuccess && g) {
         cudaGraphExec_t ge = nullptr;
@@ -1634,7 +1633,7 @@ int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_n
         cudaGraphDestroy(g);
         if (ce != cudaSuccess) return fail(SCE_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
         maps->graph = ge;
-        maps->graph_launches = p->last_launches;
+        maps->graph_launches = c.count;
         CUDA_TRY(cudaGraphLaunch(maps->graph, st));
       } else {
         if (g) cudaGraphDestroy(g);
@@ -1649,6 +1648,7 @@ int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_n
       CUDA_TRY(cudaMemcpyAsync(out_nnz, cap_nnz, (size_t)p->d.n_models * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   if (rc) return rc;
+  p->last_launches = c.count;   // every launch of the step, eager or replayed
   p->step += 1;
   if (p->prof_on && p->prof_steps < kProfMaxSteps) p->prof_steps += 1;
   return SCE_OK;
@@ -1657,12 +1657,11 @@ int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_n
 int sce_grads(sce_plan* p, const float* x, int B, float* d_encoder, float* d_bias, float* d_decoder,
               float* out_losses, float* out_nnz, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = run_pipeline(p, x, B, nullptr, true, out_losses, out_nnz, st);
-  if (rc) return rc;
-  int launches = 0;   // (not counted: last_launches stays the pipeline's)
+  PlanCall c;
+  TRY(run_pipeline(c, p, x, B, static_cast<cudaStream_t>(stream), nullptr, true, out_losses, out_nnz));
+  p->last_launches = c.count;   // the pipeline's: the gradient kernels below are not counted
   float* const grad_out[2] = {d_encoder, d_decoder};
-  return train_tail<MODE_GRAD>(p, B, hyper_for(p, 1), grad_out, d_bias, st, launches);
+  return train_tail<MODE_GRAD>(c, hyper_for(p, 1), grad_out, d_bias);
 }
 
 int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_host, float* out_nnz_host,
@@ -1687,22 +1686,21 @@ int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_hos
 int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
   if (!p || !out_code) return fail(SCE_ERR_INVALID, "plan / out_code is NULL");
   if (int rc = check_rows(p, B, "")) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Launcher L{static_cast<cudaStream_t>(stream)};
   const long long per = (long long)B * p->d.n;
   if (p->code_batch_major) {
     const long long total = (long long)p->d.n_models * per;
-    join_code_batch_major_kernel<<<(unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096), 256, 0, st>>>(
-        static_cast<const __half*>(p->c.hi), p->ct.x8, out_code, B, p->d.n, p->d.batch_max, p->cfg.bpad, total);
-    CUDA_TRY(cudaGetLastError());
-    return SCE_OK;
+    return L.launch(join_code_batch_major_kernel, (unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096), 256,
+                    0, static_cast<const __half*>(p->c.hi), p->ct.x8, out_code, B, p->d.n, p->d.batch_max, p->cfg.bpad,
+                    total);
   }
   for (int m = 0; m < p->d.n_models; ++m) {
     const Planes c = p->c.at((size_t)m * p->d.batch_max * p->d.n);
-    with_arith(p->cfg.arith, [&](auto arith) {   // (each arithmetic reads its own planes)
-      join_code_kernel<decltype(arith)::value><<<1024, 256, 0, st>>>(c.hi, c.lo, c.x8, out_code + (long long)m * per, per / 2);
-    });
+    TRY(with_arith(p->cfg.arith, [&](auto arith) {   // (each arithmetic reads its own planes)
+      return L.launch(join_code_kernel<decltype(arith)::value>, 1024, 256, 0, c.hi, c.lo, c.x8, out_code + (long long)m * per,
+                      per / 2);
+    }));
   }
-  CUDA_TRY(cudaGetLastError());
   return SCE_OK;
 }
 
@@ -1717,14 +1715,12 @@ int sce_read_center_grad(sce_plan* p, float* d_center, void* stream) {
 int sce_gather_rows(const void* chunk, int chunk_is_half, long long n_rows, int d, const long long* idx, int B,
                     const float* sub, float* out, void* stream) {
   if (!chunk || !out || B < 1 || d < 4 || d % 4) return fail(SCE_ERR_INVALID, "bad arguments to sce_gather_rows");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Launcher L{static_cast<cudaStream_t>(stream)};
   const int blocks = (B + 7) / 8;
   if (chunk_is_half)
-    gather_rows_kernel<__half><<<blocks, 256, 0, st>>>(static_cast<const __half*>(chunk), n_rows, d, idx, B, sub, out);
-  else
-    gather_rows_kernel<float><<<blocks, 256, 0, st>>>(static_cast<const float*>(chunk), n_rows, d, idx, B, sub, out);
-  CUDA_TRY(cudaGetLastError());
-  return SCE_OK;
+    return L.launch(gather_rows_kernel<__half>, blocks, 256, 0, static_cast<const __half*>(chunk), n_rows, d, idx, B, sub,
+                    out);
+  return L.launch(gather_rows_kernel<float>, blocks, 256, 0, static_cast<const float*>(chunk), n_rows, d, idx, B, sub, out);
 }
 
 int sce_last_launch_count(const sce_plan* plan) { return plan ? plan->last_launches : 0; }
@@ -1762,9 +1758,19 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
   if (!plan || !counts) return fail(SCE_ERR_INVALID, "plan / counts is NULL");
   if (int rc = check_rows(plan, B, "")) return rc;
   const int n_chunks = (plan->d.n + 31) / 32;
-  active_count_kernel<<<dim3(n_chunks, plan->d.n_models), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      plan->act_pos, n_chunks, plan->d.batch_max, B, plan->d.n, counts);
-  CUDA_TRY(cudaGetLastError());
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  return L.launch(active_count_kernel, dim3(n_chunks, plan->d.n_models), 256, 0, plan->act_pos, n_chunks,
+                  plan->d.batch_max, B, plan->d.n, counts);
+}
+
+// The checks that open sce_forward_stats and sce_forward_fragments; `prefix` names the entry point in the messages
+static int check_forward_only(const sce_plan* p, const float* x, int B, const char* prefix) {
+  if (!p) return fail(SCE_ERR_INVALID, "%splan is NULL", prefix);
+  if (!p->cfg.evaluable)
+    return fail(SCE_ERR_INVALID, "%snot available for the learned-centre variant or with encoder_nonneg / input_shift; "
+                                 "evaluate the exported dictionaries (TiedSAE)", prefix);
+  TRY(check_rows(p, B, prefix));
+  if (!x) return fail(SCE_ERR_INVALID, "%sx is NULL", prefix);
   return SCE_OK;
 }
 
@@ -1776,12 +1782,7 @@ size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
 int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
                       float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
                       size_t workspace_bytes, void* stream) {
-  if (!p) return fail(SCE_ERR_INVALID, "forward_stats: plan is NULL");
-  if (!p->cfg.evaluable)
-    return fail(SCE_ERR_INVALID, "forward_stats: not available for the learned-centre variant or with encoder_nonneg / "
-                                 "input_shift; evaluate the exported dictionaries (TiedSAE)");
-  if (int rc = check_rows(p, B, "forward_stats: ")) return rc;
-  if (!x) return fail(SCE_ERR_INVALID, "forward_stats: x is NULL");
+  TRY(check_forward_only(p, x, B, "forward_stats: "));
   if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
   if (seg_phase < 0 || seg_phase >= seg)
     return fail(SCE_ERR_INVALID, "forward_stats: seg_phase = %d outside [0, seg = %d)", seg_phase, seg);
@@ -1789,26 +1790,22 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
     return fail(SCE_ERR_INVALID, "forward_stats: out_losses, out_nnz, moment_sums and seg_counts are required");
   if (seg > 1 && !seg_open) return fail(SCE_ERR_INVALID, "forward_stats: seg > 1 needs the seg_open flags");
   if (int rc = check_workspace(workspace, workspace_bytes, stats_workspace(p->d, B), "forward_stats: ")) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sce_desc& d = p->d;
   float* part = static_cast<float*>(workspace);
-  int rc = run_pipeline(p, x, B, x_hat, false, out_losses, out_nnz, st, p->cfg.topk ? nullptr : part);
-  if (rc) return rc;
+  PlanCall c;
+  TRY(run_pipeline(c, p, x, B, static_cast<cudaStream_t>(stream), x_hat, false, out_losses, out_nnz,
+                   p->cfg.topk ? nullptr : part));
+  p->last_launches = c.count;   // the pipeline's: the statistics kernels below are not counted
   const int n_chunks = (d.n + 31) / 32, row_blocks = (B + 31) / 32;
-  if (p->cfg.topk) {
-    topk_moment_kernel<<<dim3(n_chunks, (row_blocks + 7) / 8, d.n_models), 256, 0, st>>>(p->scores, p->act_pos, n_chunks,
-                                                                                        d.batch_max, B, d.n, row_blocks, part);
-    CUDA_TRY(cudaGetLastError());
-  }
-  moment_reduce_kernel<<<dim3((d.n + 255) / 256, d.n_models), 256, 0, st>>>(part, row_blocks, d.n, moment_sums);
-  CUDA_TRY(cudaGetLastError());
+  if (p->cfg.topk)
+    TRY(c.launch(topk_moment_kernel, dim3(n_chunks, (row_blocks + 7) / 8, d.n_models), 256, 0, p->scores, p->act_pos,
+                 n_chunks, d.batch_max, B, d.n, row_blocks, part));
+  TRY(c.launch(moment_reduce_kernel, dim3((d.n + 255) / 256, d.n_models), 256, 0, part, row_blocks, d.n, moment_sums));
   if (seg == 1)
-    active_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, seg_counts);
-  else
-    segment_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, seg,
-                                                                     seg_phase, seg_counts, seg_open);
-  CUDA_TRY(cudaGetLastError());
-  return SCE_OK;
+    return c.launch(active_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
+                    seg_counts);
+  return c.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n, seg,
+                  seg_phase, seg_counts, seg_open);
 }
 
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
@@ -1820,12 +1817,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
                           unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream) {
-  if (!p) return fail(SCE_ERR_INVALID, "forward_fragments: plan is NULL");
-  if (!p->cfg.evaluable)
-    return fail(SCE_ERR_INVALID, "forward_fragments: not available for the learned-centre variant or with encoder_nonneg / "
-                                 "input_shift; evaluate the exported dictionaries (TiedSAE)");
-  if (int rc = check_rows(p, B, "forward_fragments: ")) return rc;
-  if (!x) return fail(SCE_ERR_INVALID, "forward_fragments: x is NULL");
+  TRY(check_forward_only(p, x, B, "forward_fragments: "));
   if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);
   if (B % L) return fail(SCE_ERR_INVALID, "forward_fragments: B = %d is not a multiple of L = %d", B, L);
   if (frag0 < 0) return fail(SCE_ERR_INVALID, "forward_fragments: frag0 = %lld must be >= 0", frag0);
@@ -1839,10 +1831,10 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   size_t off_active, off_open;
   const size_t need = frag_workspace(p->d, B, L, &off_active, &off_open);
   if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_fragments: ")) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sce_desc& d = p->d;
-  int rc = run_pipeline(p, x, B, nullptr, false, nullptr, nullptr, st);
-  if (rc) return rc;
+  PlanCall call;
+  TRY(run_pipeline(call, p, x, B, static_cast<cudaStream_t>(stream), nullptr, false, nullptr, nullptr));
+  p->last_launches = call.count;   // the pipeline's: the fragment kernels below are not counted
   uint8_t* ws = static_cast<uint8_t*>(workspace);
   float* fmax = reinterpret_cast<float*>(ws);
   uint8_t* active = ws + off_active;
@@ -1850,20 +1842,17 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   const int n_chunks = (d.n + 31) / 32, G = B / L;
   const FragCode c{p->c.hi, p->c.lo, p->c.x8, p->scores, p->act_pos, n_chunks, d.batch_max, d.n};
   if (p->cfg.topk)
-    launch_fragments<kArithBf16x3, true>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed, top_val,
-                                         top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
+    TRY((launch_fragments<kArithBf16x3, true>(call, c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed,
+                                              top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act)));
   else
-    with_arith(p->cfg.arith, [&](auto ar) {
-      launch_fragments<decltype(ar)::value, false>(c, d.n_models, L, G, frag0, fmax, active, n_top, n_random, seed,
-                                                   top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act, st);
-    });
-  CUDA_TRY(cudaGetLastError());
+    TRY(with_arith(p->cfg.arith, [&](auto ar) {
+      return launch_fragments<decltype(ar)::value, false>(call, c, d.n_models, L, G, frag0, fmax, active, n_top, n_random,
+                                                          seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
+    }));
   // active fragments: segments of L rows, cut at fragment boundaries (phase 0, no segment stays open)
-  CUDA_TRY(cudaMemsetAsync(open, 0, (size_t)d.n_models * d.n * sizeof(int), st));
-  segment_count_kernel<<<dim3(n_chunks, d.n_models), 256, 0, st>>>(p->act_pos, n_chunks, d.batch_max, B, d.n, L, 0,
-                                                                   n_active, open);
-  CUDA_TRY(cudaGetLastError());
-  return SCE_OK;
+  CUDA_TRY(cudaMemsetAsync(open, 0, (size_t)d.n_models * d.n * sizeof(int), call.st));
+  return call.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
+                     L, 0, n_active, open);
 }
 
 int sce_plan_arith(const sce_plan* plan) {
@@ -1951,6 +1940,7 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
 
   // ---- device
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Launcher L{st};
   int dev = 0, sms = 0;
   if (int rc = query_device(&dev, &sms)) return rc;
   const SimOperand A{a, ma, na, a_normalize, a_norm_floor};
@@ -1968,8 +1958,8 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
     sim_carve(static_cast<uint8_t*>(workspace), true, ma, na, b_is_a ? 0 : mb, b_is_a ? 0 : nb, d, n_pairs, capacity != nullptr, &w);
     CUDA_TRY(cudaMemsetAsync(w.flags, 0, kFlagWords * sizeof(uint32_t), st));
     int rc = SCE_OK;
-    if (!A.normalize) rc = sim_planes<kArithF16F8>(A, d, w.a, w.flags, st);
-    if (!rc && !b_is_a && !B.normalize) rc = sim_planes<kArithF16F8>(B, d, w.b, w.flags, st);
+    if (!A.normalize) rc = sim_planes<kArithF16F8>(L, A, d, w.a, w.flags);
+    if (!rc && !b_is_a && !B.normalize) rc = sim_planes<kArithF16F8>(L, B, d, w.b, w.flags);
     if (rc) return rc;
     uint32_t bad = 0;
     CUDA_TRY(cudaMemcpyAsync(&bad, w.flags + kBadWord, sizeof(bad), cudaMemcpyDeviceToHost, st));
@@ -1987,8 +1977,8 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
   CUDA_TRY(cudaMemcpyAsync(w.a_rows, rows.data(), (size_t)ma * sizeof(int), cudaMemcpyHostToDevice, st));
   if (!b_is_a) CUDA_TRY(cudaMemcpyAsync(w.b_rows, rows.data() + ma, (size_t)mb * sizeof(int), cudaMemcpyHostToDevice, st));
   // (a raw operand split above for the range check is split again here: the planes of the arithmetic that runs)
-  return f8 ? run_similarity_t<kArithF16F8>(A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms, st)
-            : run_similarity_t<kArithBf16x3>(A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms, st);
+  return f8 ? run_similarity_t<kArithF16F8>(L, A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms)
+            : run_similarity_t<kArithBf16x3>(L, A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms);
 }
 
 int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,
@@ -2013,15 +2003,13 @@ int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int 
   // ---- device
   SynthArgs a{feats, probs, n_gt, d, group_rows, B, row0, (uint32_t)seed, (uint32_t)(seed >> 32), zero_row_rule,
               noise_scale, out, out_half, row_nnz, code_idx, code_val, code_idx ? code_cap : 0};
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  Launcher L{static_cast<cudaStream_t>(stream)};
   const unsigned rows8 = (unsigned)((B + 7) / 8);
-  if (d <= 128) synth_rows_kernel<1, false><<<rows8, 256, 0, st>>>(a);
-  else if (d <= 256) synth_rows_kernel<2, false><<<rows8, 256, 0, st>>>(a);
-  else if (d <= 512) synth_rows_kernel<4, false><<<rows8, 256, 0, st>>>(a);
-  else if (d <= 1024) synth_rows_kernel<8, false><<<rows8, 256, 0, st>>>(a);
-  else synth_rows_kernel<8, true><<<(unsigned)B, 32 * ((d + 1023) / 1024), 0, st>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  return SCE_OK;
+  if (d <= 128) return L.launch(synth_rows_kernel<1, false>, rows8, 256, 0, a);
+  if (d <= 256) return L.launch(synth_rows_kernel<2, false>, rows8, 256, 0, a);
+  if (d <= 512) return L.launch(synth_rows_kernel<4, false>, rows8, 256, 0, a);
+  if (d <= 1024) return L.launch(synth_rows_kernel<8, false>, rows8, 256, 0, a);
+  return L.launch(synth_rows_kernel<8, true>, (unsigned)B, 32 * ((d + 1023) / 1024), 0, a);
 }
 
 }  // extern "C"

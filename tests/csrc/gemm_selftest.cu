@@ -3,7 +3,9 @@
 //   bf16x3 (K block 32): K x K; K x MN; K x MN and MN x MN with split accumulators;
 //   f16f8 (K block 64): K x K and MN x MN with the cross terms on E5M2 wgmma (MN x MN: 8-bit planes from batch-major
 //   copies), and MN x MN with the 8-bit tiles widened to fp16.
-// The default run prints one PASS / FAIL line per case and exits non-zero when one fails
+// Each configuration has one `_persist` case with more than twice as many output tiles as an H100 has SMs and ragged M,
+// N and K, so that every persistent CTA runs a second tile (ring phase carried over, accumulator reset, epilogue staging
+// reused) and some a partial one. The default run prints one PASS / FAIL line per case and exits non-zero when one fails
 // (tests/test_engine_gpu.py::test_gemm_selftest). `--big` runs each configuration at config-2 shapes instead, for a
 // kernel-level throughput reading. Build: Makefile target `selftest`.
 #include <cmath>
@@ -253,8 +255,17 @@ static void make_case(const Case& c, int arith, Operand* A, Operand* B) {
   }
 }
 
+// Every index of [0, n) up to 512, else every step-th one, and always the last one (the partial tile's edge).
+static std::vector<int> sample_indices(int n, int step) {
+  std::vector<int> v;
+  for (int i = 0; i < n; i += n > 512 ? step : 1) v.push_back(i);
+  if (v.back() != n - 1) v.push_back(n - 1);
+  return v;
+}
+
 // Checks a case's output against plane_exact at 1e-3 sqrt(K sets) (bf16x3) or 1e-4 sqrt(K sets) (f16f8); rows and
-// columns are sampled beyond 512. Prints the PASS / FAIL line and, on failure, a map of the failing 4 x 16 blocks.
+// columns are sampled beyond 512, the last row and column always. Prints the PASS / FAIL line with the number of output
+// tiles (beyond the SM count, persistent CTAs run more than one) and, on failure, a map of the failing 4 x 16 blocks.
 static bool check_case(const Case& c, const char* path, const Operand* A, const Operand* B, const std::vector<float>& out,
                        float ms) {
   const int arith = A[0].arith, M = c.M, N = c.N;
@@ -262,10 +273,11 @@ static bool check_case(const Case& c, const char* path, const Operand* A, const 
   double max_err = 0, max_ref = 0, se_full = 0, s_full = 0;
   long long bad = 0;
   int fb[3] = {-1, -1, -1};
-  const int rstep = M > 512 ? 37 : 1, cstep = N > 512 ? 29 : 1;
+  const int tiles = c.models * ((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN);
+  const std::vector<int> rows = sample_indices(M, 37), cols = sample_indices(N, 29);
   for (int m = 0; m < c.models; ++m)
-    for (int i = 0; i < M; i += rstep)
-      for (int j = 0; j < N; j += cstep) {
+    for (int i : rows)
+      for (int j : cols) {
         const double ex = plane_exact(A, B, c.nsets, m, i, j, c.passes), got = out[((size_t)m * M + i) * N + j];
         double fu = 0;   // the fp32 operands' product
         for (int s = 0; s < c.nsets; ++s)
@@ -280,10 +292,11 @@ static bool check_case(const Case& c, const char* path, const Operand* A, const 
       }
   const bool ok = bad == 0;
   const double flops = 2.0 * c.models * M * N * (double)c.K * c.nsets * (arith == kBf && c.passes >= 3 ? 3 : 1);
-  printf("[%s%s%s] %s  models=%d M=%d N=%d K=%d sets=%d passes=%d  max|err| vs plane-exact %.3e (bound %.3e, max|ref| "
-         "%.2f), rel. rms vs fp32 product %.2e  %.3f ms  %.1f TF(%s)\n",
-         c.name, *path ? "/" : "", path, ok ? "PASS" : "FAIL", c.models, M, N, c.K, c.nsets, c.passes, max_err, bound,
-         max_ref, sqrt(se_full / (s_full + 1e-300)), ms, flops / ms * 1e-9, arith == kBf ? "bf16 passes" : "algorithmic");
+  printf("[%s%s%s] %s  models=%d M=%d N=%d K=%d sets=%d passes=%d tiles=%d  max|err| vs plane-exact %.3e (bound %.3e, "
+         "max|ref| %.2f), rel. rms vs fp32 product %.2e  %.3f ms  %.1f TF(%s)\n",
+         c.name, *path ? "/" : "", path, ok ? "PASS" : "FAIL", c.models, M, N, c.K, c.nsets, c.passes, tiles, max_err,
+         bound, max_ref, sqrt(se_full / (s_full + 1e-300)), ms, flops / ms * 1e-9,
+         arith == kBf ? "bf16 passes" : "algorithmic");
   if (!ok) {
     printf("    %lld bad samples; first at model %d row %d col %d: got %.6f\n", bad, fb[0], fb[1], fb[2],
            out[((size_t)fb[0] * M + fb[1]) * N + fb[2]]);
@@ -432,20 +445,24 @@ int main(int argc, char** argv) {
     const Case kk[] = {{"kk_k16", 1, 128, 256, 16, 1, 1},          {"kk_k64", 1, 128, 256, 64, 1, 1},
                        {"kk_k256", 1, 128, 256, 256, 1, 1},        {"kk_3pass", 1, 128, 256, 256, 1, 3},
                        {"kk_multi", 3, 384, 512, 512, 1, 3, true}, {"kk_ragged", 2, 200, 328, 104, 1, 3, true},
-                       {"kk_bn128", 2, 256, 384, 256, 1, 3, true}, {"kk_short", 2, 100, 328, 104, 1, 3, true}};
+                       {"kk_bn128", 2, 256, 384, 256, 1, 3, true}, {"kk_short", 2, 100, 328, 104, 1, 3, true},
+                       {"kk_persist", 4, 1000, 1040, 400, 1, 3, true}};
     for (const Case& c : kk) ok &= run_case<false, false, false, kBf, false>(c);
     // ---- bf16x3, K x MN (decode: X^ = C W), without and with split accumulators
     const Case kmn[] = {{"kmn_k16", 1, 128, 256, 16, 1, 1}, {"kmn_k64", 1, 128, 256, 64, 1, 1},
-                        {"kmn_3pass", 2, 256, 512, 512, 1, 3}, {"kmn_ragged", 2, 200, 328, 104, 1, 3}};
+                        {"kmn_3pass", 2, 256, 512, 512, 1, 3}, {"kmn_ragged", 2, 200, 328, 104, 1, 3},
+                        {"kmn_persist", 4, 1000, 1040, 400, 1, 3}};
     for (const Case& c : kmn) ok &= run_case<false, true, false, kBf, false>(c);
-    const Case kmn_split[] = {{"kmn_split", 2, 512, 512, 512, 1, 3}, {"kmn_split_ragged", 2, 200, 328, 104, 1, 3}};
+    const Case kmn_split[] = {{"kmn_split", 2, 512, 512, 512, 1, 3}, {"kmn_split_ragged", 2, 200, 328, 104, 1, 3},
+                              {"kmn_split_persist", 4, 1000, 1040, 400, 1, 3}};
     for (const Case& c : kmn_split) ok &= run_case<false, true, true, kBf, false>(c);
     // ---- bf16x3, MN x MN with split accumulators (weight gradient: dW = dZ^T X + C^T G), up to two operand sets
     const Case mnmn[] = {{"mnmn_k16", 1, 128, 256, 16, 1, 1},
                          {"mnmn_k64", 1, 128, 256, 64, 1, 1},
                          {"mnmn_2set", 2, 512, 512, 320, 2, 3, false, true},
                          {"mnmn_2set_m256", 2, 256, 512, 320, 2, 3, false, true},
-                         {"mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true}};
+                         {"mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true},
+                         {"mnmn_persist", 4, 1000, 1040, 400, 2, 3, false, true}};
     for (const Case& c : mnmn) ok &= run_case<true, true, true, kBf, false>(c);
     // ---- f16f8 native K x K (the f8_kmn cases: decode, which reads the transposed dictionary K-major)
     const Case f8_kk[] = {{"f8_kk_hh", 1, 128, 256, 64, 1, 1},
@@ -456,13 +473,15 @@ int main(int argc, char** argv) {
                           {"f8_kmn_k64", 1, 128, 256, 64, 1, 3},
                           {"f8_kmn_multi", 2, 256, 512, 512, 1, 3},
                           {"f8_kmn", 2, 512, 512, 512, 1, 3},
-                          {"f8_kmn_ragged", 2, 200, 328, 104, 1, 3}};
+                          {"f8_kmn_ragged", 2, 200, 328, 104, 1, 3},
+                          {"f8_kk_persist", 4, 1000, 1040, 400, 1, 3, true}};
     for (const Case& c : f8_kk) ok &= run_case<false, false, false, kF8, true>(c);
     // ---- f16f8 MN x MN (weight gradient), native and widened
     const Case f8_mnmn[] = {{"f8_mnmn_k64", 1, 128, 256, 64, 1, 3},
                             {"f8_mnmn_2set", 2, 256, 512, 320, 2, 3, false, true},
                             {"f8_mnmn_ragged", 2, 200, 328, 104, 2, 3, false, true},
-                            {"f8_mnmn_exactB", 2, 512, 512, 320, 2, 3, false, true, 2}};
+                            {"f8_mnmn_exactB", 2, 512, 512, 320, 2, 3, false, true, 2},
+                            {"f8_mnmn_persist", 4, 1000, 1040, 400, 2, 3, false, true}};
     for (const Case& c : f8_mnmn) ok &= run_case_f8_mnmn(c);
     ok &= cross_terms();
     ok &= mixed_dw();

@@ -671,7 +671,9 @@ def test_gemm_selftest(tmp_path):
     """The standalone check of the GEMM core (tests/csrc/gemm_selftest.cu): the seven configurations libsce launches
     against a double-precision product of the same planes, ragged edges included; the accuracy of the f16f8 cross-term
     accumulation (native and widened) at reduction lengths up to 16384; and the f16f8 weight gradient with mixed
-    operand layouts, native against widened."""
+    operand layouts, native against widened. Each configuration's `_persist` case (f16f8 MN x MN both native and
+    widened) has more than two output tiles per SM, so persistent CTAs run second and partial tiles."""
+    import re
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     exe = os.path.join(root, "build", "gemm_selftest")
     if not os.path.exists(exe):   # build() makes it; a tree built with `make` alone may not have it
@@ -681,3 +683,6 @@ def test_gemm_selftest(tmp_path):
     r = subprocess.run([exe], capture_output=True, text=True, timeout=1800)
     print(r.stdout)
     assert r.returncode == 0 and "ALL PASS" in r.stdout, r.stdout[-4000:] + r.stderr[-2000:]
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    persist = re.findall(r"\[(\w+_persist(?:/\w+)?)\] PASS .* tiles=(\d+)", r.stdout)
+    assert len(persist) == 7 and all(int(t) > 2 * sms for _, t in persist), (sms, persist)

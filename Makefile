@@ -15,5 +15,10 @@ build/gemm_selftest: tests/csrc/gemm_selftest.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.
 	mkdir -p build
 	$(NVCC) $(NVFLAGS) -o $@ tests/csrc/gemm_selftest.cu
 
+probe: build/gemm_overlap_probe
+build/gemm_overlap_probe: tools/gemm_overlap_probe.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
+	mkdir -p build
+	$(NVCC) $(NVFLAGS) -o $@ tools/gemm_overlap_probe.cu
+
 clean:
-	rm -f $(LIB) build/gemm_selftest
+	rm -f $(LIB) build/gemm_selftest build/gemm_overlap_probe

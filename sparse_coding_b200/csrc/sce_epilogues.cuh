@@ -203,6 +203,7 @@ template <int ARITH, bool STATS = false>
 struct EpiEncodeT {
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 4096;
+  static constexpr bool kInline = STATS;   // the moment sums do not fit the epilogue warpgroup's registers (sce_gemm.cuh)
   struct Params : EncodeMomentParams<STATS> {
     CUtensorMap out_hi, out_lo, out_x8;  // store maps of the code planes: [M][B][n], box 32 x 32
     const float* bias;             // [M, n] or nullptr
@@ -345,6 +346,7 @@ template <int ARITH, bool GSUM = false>
 struct EpiDecodeT {
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 0;
+  static constexpr bool kInline = true;   // a few percent of a tile beside a K = n main loop (sce_gemm.cuh)
   struct Params : DecodeGsumParams<GSUM> {
     const float* x;                // [B, d] (x_model_stride = 0) or [M, B, d]
     long long x_model_stride;

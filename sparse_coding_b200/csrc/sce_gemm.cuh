@@ -13,11 +13,16 @@
 // MN-major GEMM (the weight gradient) reads batch-major copies of its 8-bit planes. Without those copies (top-k and
 // launch-bound plans) the MN-major weight gradient widens its 8-bit tiles to fp16 in shared memory instead.
 //
-// One CTA per SM, 384 threads: warp 0 = TMA producer (one thread), warpgroups 1 and 2 = wgmma consumers (rows 0..63
-// and 64..127 of the 128 x 128 tile), which then run the fused epilogue. The accumulators go through a padded fp32
-// tile in shared memory so that each epilogue thread owns one output row and 32 consecutive columns: eight epilogue
-// warps, warp w handling rows 32 (w % 4) .. +31 and the 32-column chunks with chunk % 2 == w / 4. The producer keeps
-// loading the next tile's stages while the epilogue runs.
+// One CTA per SM, 512 threads in four warpgroups, each setting its registers with setmaxnreg: warpgroup 0 = TMA
+// producer (one thread), warpgroups 1 and 2 = wgmma consumers (rows 0..63 and 64..127 of the 128 x 128 tile),
+// warpgroup 3 = the fused epilogue. The consumers write the accumulators into a padded fp32 tile in shared memory
+// (acc_stage) and arrive on the mbarrier acc_full; the epilogue warpgroup reads the tile, arrives on acc_empty, and
+// runs the epilogue while the consumers run the next tile's main loop (they wait on acc_empty only before writing
+// acc_stage again). Each epilogue thread owns one output row and 32 consecutive columns. A tile's epilogue has eight
+// shares (q, g): rows 32 q .. +31 and the 32-column chunks with chunk % 2 == g; epilogue warp q runs (q, 0), then
+// (q, 1). Where the epilogue does not overlap (gemm_overlap: kInline epilogues, the widened path) the kernel runs 384
+// threads without the epilogue warpgroup, and the eight consumer warps run it in line after the main loop, warp w
+// taking share (w % 4, w / 4). The outputs are the same either way.
 #pragma once
 #include <type_traits>
 #include "sce_ptx.cuh"
@@ -26,8 +31,12 @@ namespace sce {
 
 constexpr int kBM = 128;        // rows of the output tile
 constexpr int kBN = 128;        // columns of the output tile
-constexpr int kGemmThreads = 384;
-constexpr int kEpiWarps = 8;
+constexpr int kEpiWarps = 8;    // epilogue shares of a tile (warp quarter x column group), each with its own staging
+// Launches that overlap the epilogue run 512 threads, and each warpgroup sets its per-thread registers with setmaxnreg:
+// producer, each of the two consumers, epilogue. They add up to the 65536 registers of the SM over 128 threads each
+// (the launch count of 128 per thread at 512 threads). In-line launches run 384 threads without setmaxnreg.
+constexpr int kProducerRegs = 40, kConsumerRegs = 168, kEpilogueRegs = 136;
+static_assert(kProducerRegs + 2 * kConsumerRegs + kEpilogueRegs == 65536 / 128, "register split of the four warpgroups");
 constexpr int kMaxSets = 2;
 constexpr int kSmemLimit = 232448;  // 227 KB of shared memory one CTA may use on sm_90
 
@@ -103,6 +112,29 @@ struct epi_pair_tiles : std::false_type {};
 template <class Epi>
 struct epi_pair_tiles<Epi, std::void_t<decltype(Epi::kPairTiles)>> : std::bool_constant<Epi::kPairTiles> {};
 
+// epilogues may declare `static constexpr bool kInline = true`: the consumers then run them in line after each tile's
+// main loop, in the 384-thread kernel without an epilogue warpgroup. For epilogues whose state needs more than the
+// epilogue warpgroup's kEpilogueRegs registers, and for light ones beside a long main loop, where the overlap has
+// nothing to win and its epilogue traffic during the main loop measured slower (decode, the fp32 store of dW).
+template <class Epi, class = void>
+struct epi_inline : std::false_type {};
+template <class Epi>
+struct epi_inline<Epi, std::void_t<decltype(Epi::kInline)>> : std::bool_constant<Epi::kInline> {};
+
+// Whether the epilogue warpgroup runs a tile's epilogue while the consumers run the next tile's main loop. Not for
+// kInline epilogues, nor on the widened f16f8 path (MN-major 8-bit tiles without F8_NATIVE), which widens into the space
+// of the accumulator tile, so that tile cannot be held for the epilogue during the main loop there. A region of its own
+// would cost two of its five ring stages, and the plans on that path (top-k, launch-bound shapes) run it for the weight
+// gradient only, whose fp32 store epilogue is in line anyway.
+template <class Epi, int ARITH, bool F8_NATIVE>
+__host__ __device__ constexpr bool gemm_overlap() {
+  return (ARITH != kArithF16F8 || F8_NATIVE) && !epi_inline<Epi>::value;
+}
+template <class Epi, int ARITH, bool F8_NATIVE>
+__host__ __device__ constexpr int gemm_threads() {
+  return gemm_overlap<Epi, ARITH, F8_NATIVE>() ? 512 : 384;
+}
+
 // f16f8 without F8_NATIVE (MN-major operands): an MN-major 8-bit tile as TMA delivers it without swizzle, [BK][ROWS]
 // bytes, widened to the fp16 tile the 16-bit loads of the same operand produce, [ROWS / 64][BK][64] with the 128-byte
 // swizzle. 256 consumer threads, 16 bytes each per round.
@@ -141,7 +173,7 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
 // planes only (sweep 2), because E5M2 wgmma reads no layout but K-major. Otherwise (MN-major operands) the 8-bit tiles
 // arrive unswizzled and MN-major, and are widened to fp16 in shared memory first.
 template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(gemm_threads<Epi, ARITH, F8_NATIVE>(), 1)
 gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
   constexpr int BN = kBN;
@@ -154,12 +186,16 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr int STAGES = SM::kStages;
   constexpr int EC = Epi::kCols;  // accumulator columns handed to the epilogue per call
   static_assert(EC == 32, "epilogue chunk is 32 columns");
+  constexpr bool OVERLAP = gemm_overlap<Epi, ARITH, F8_NATIVE>();
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOff);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* acc_full = empty_bar + STAGES;   // OVERLAP: acc_stage holds a tile for the epilogue warpgroup
+  uint64_t* acc_empty = acc_full + 1;        // OVERLAP: the epilogue warpgroup has read acc_stage
+  float* acc_stage = reinterpret_cast<float*>(smem + SM::kAccOff);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -200,6 +236,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
     }
+    if constexpr (OVERLAP) {
+      mbar_init(acc_full, 256);      // every consumer thread, after its accumulators are in acc_stage
+      mbar_init(acc_empty, 128);     // every epilogue thread, after its last read of acc_stage
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -213,8 +253,37 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     }
   }
 
+  // One epilogue warp's share of the tile in acc_stage: rows 32 warp_q .. +31 and the 32-column chunks grp, grp + 2.
+  // `read_done` runs once the warp has read the last accumulators of its share.
+  auto epilogue_share = [&](int model, int tile_m, int tile_n, int warp_q, int grp, auto read_done) {
+    TileCoord tc;
+    tc.model = model;
+    tc.m_blk = tile_m;
+    tc.n_blk = tile_n;
+    tc.col0 = tile_n * BN;
+    tc.warp_q = warp_q;
+    tc.grp = grp;
+    tc.lane = lane;
+    tc.row = tc.m_blk * kBM + tc.warp_q * 32 + lane;
+    Epi epi(p.epi, tc, p.m_total, p.n_total, smem + SM::kEpiOff + (tc.grp * 4 + tc.warp_q) * Epi::kWarpStageBytes);
+    const float* my_row = acc_stage + (tc.warp_q * 32 + lane) * SM::kAccLd;
+    constexpr int kChunks = BN / EC;
+    static_assert(kChunks % 2 == 0, "the two column groups alternate chunks");
+#pragma unroll 1
+    for (int it = 0; it < kChunks / 2; ++it) {
+      const int c = tc.grp + 2 * it;   // column group g takes the chunks g, g + 2, ...
+      uint32_t r[EC];
+#pragma unroll
+      for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(my_row[c * EC + j]);
+      if (it == kChunks / 2 - 1) read_done();
+      epi.chunk(c * EC, r);
+    }
+    epi.finish();
+  };
+
   if (warp < 4) {
     // ======================= TMA producer =======================
+    if constexpr (OVERLAP) reg_dealloc<kProducerRegs>();
     if (threadIdx.x == 0) {
       const uint32_t stage_bytes = (three && !F8) ? uint32_t(SM::kStage) : uint32_t(SM::kATile + SM::kBTile);
       int stage = 0;
@@ -314,8 +383,9 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
         }
       }
     }
-  } else {
-    // ======================= wgmma consumers + epilogue =======================
+  } else if (!OVERLAP || warp < 12) {
+    // ======================= wgmma consumers (+ the epilogue where !OVERLAP) =======================
+    if constexpr (OVERLAP) reg_alloc<kConsumerRegs>();
     const int ctid = threadIdx.x - 128;      // 0..255
     const int wg = ctid >> 7;                // rows 64 wg .. +63 of the tile
     const int wl = ctid & 127;               // thread within the warpgroup
@@ -333,9 +403,9 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
 
     float acc[64];
     float accx[SPLIT_ACC || F8_NATIVE ? 64 : 1];   // split cross-term accumulator / one K block of E5M2 cross terms
-    float* acc_stage = reinterpret_cast<float*>(smem + SM::kAccOff);
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t acc_phase = 0;   // OVERLAP: parity of the tiles handed to the epilogue warpgroup
     auto next = [&]() {
       if (++stage == STAGES) {
         stage = 0;
@@ -466,7 +536,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       }
 
       // ---- accumulators -> padded fp32 tile (row-per-thread view for the epilogue)
-      consumer_sync();   // the previous tile's epilogue / the widened tiles are no longer read
+      // OVERLAP: the epilogue warpgroup has read the previous tile (it ran under this tile's main loop). Otherwise both
+      // consumer warpgroups are past their previous epilogue and the widened tiles.
+      if constexpr (OVERLAP) mbar_wait(acc_empty, acc_phase ^ 1);
+      else consumer_sync();
       {
         const int w = wl >> 5, l = wl & 31;
         const int r0 = wg * 64 + w * 16 + (l >> 2);
@@ -477,32 +550,30 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
           acc_stage[row * SM::kAccLd + col] = acc[i];
         }
       }
-      consumer_sync();
-
-      // ======================= epilogue =======================
-      const int cw = ctid >> 5;   // epilogue warp 0..7
-      TileCoord tc;
-      tc.model = model;
-      tc.m_blk = tile_m;
-      tc.n_blk = tile_n;
-      tc.col0 = tile_n * BN;
-      tc.warp_q = cw & 3;
-      tc.grp = cw >> 2;
-      tc.lane = lane;
-      tc.row = tc.m_blk * kBM + tc.warp_q * 32 + lane;
-      Epi epi(p.epi, tc, p.m_total, p.n_total, smem + SM::kEpiOff + (tc.grp * 4 + tc.warp_q) * Epi::kWarpStageBytes);
-      const float* my_row = acc_stage + (tc.warp_q * 32 + lane) * SM::kAccLd;
-      constexpr int kChunks = BN / EC;
-      static_assert(kChunks % 2 == 0, "the two epilogue warp groups alternate chunks");
-#pragma unroll 1
-      for (int it = 0; it < kChunks / 2; ++it) {
-        const int c = tc.grp + 2 * it;   // epilogue warp group g takes the chunks g, g + 2, ...
-        uint32_t r[EC];
-#pragma unroll
-        for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(my_row[c * EC + j]);
-        epi.chunk(c * EC, r);
+      if constexpr (OVERLAP) {
+        mbar_arrive(acc_full);
+        acc_phase ^= 1;
+      } else {
+        // ======================= epilogue in line: eight warps, warp w plays (w % 4, w / 4) =======================
+        consumer_sync();
+        const int cw = ctid >> 5;
+        epilogue_share(model, tile_m, tile_n, cw & 3, cw >> 2, [] {});
       }
-      epi.finish();
+    }
+  } else if constexpr (OVERLAP) {
+    // ======================= epilogue warpgroup =======================
+    // Warp q plays both of the in-line epilogue's warps (q, 0) and (q, 1) in turn: each share's sums, partial-sum slots
+    // and staging are those of the in-line mapping, so the outputs do not depend on which warps run them.
+    reg_alloc<kEpilogueRegs>();
+    const int warp_q = warp - 12;
+    uint32_t acc_phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      int model, tile_m, tile_n;
+      decode_tile(tile, model, tile_m, tile_n);
+      mbar_wait(acc_full, acc_phase);
+      acc_phase ^= 1;
+      epilogue_share(model, tile_m, tile_n, warp_q, 0, [] {});
+      epilogue_share(model, tile_m, tile_n, warp_q, 1, [&] { mbar_arrive(acc_empty); });
     }
   }
 }
@@ -530,7 +601,7 @@ cudaError_t launch_gemm(const GemmParams<typename Epi::Params>& p, int device, i
   const cudaError_t e = opt_in_smem<kern>(bytes, device);
   if (e != cudaSuccess) return e;
   const long long tiles = (long long)p.n_models * p.tiles_m * p.tiles_n;
-  kern<<<(unsigned)(tiles < sms ? tiles : sms), kGemmThreads, bytes, st>>>(p);
+  kern<<<(unsigned)(tiles < sms ? tiles : sms), gemm_threads<Epi, ARITH, F8_NATIVE>(), bytes, st>>>(p);
   return cudaGetLastError();
 }
 
@@ -540,6 +611,7 @@ cudaError_t launch_gemm(const GemmParams<typename Epi::Params>& p, int device, i
 struct EpiStoreF32 {
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 0;
+  static constexpr bool kInline = true;   // a few percent of a weight-gradient tile (K = batch)
   struct Params {
     float* out;
     long long model_stride;  // elements

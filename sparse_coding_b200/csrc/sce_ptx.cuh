@@ -26,6 +26,18 @@ __device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// setmaxnreg: sets the per-thread register count of the executing warpgroup to N (a multiple of 8 in 24..256). Every
+// thread of the warpgroup executes it. `dec` hands registers back to the CTA's pool; `inc` waits until the pool has
+// them. The kernel's launch register count (from __launch_bounds__) times its threads is the pool.
+template <uint32_t N>
+__device__ __forceinline__ void reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ----------------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------------

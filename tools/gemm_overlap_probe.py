@@ -1,0 +1,142 @@
+"""How much of each split-operand GEMM of a config-2 training step is its epilogue.
+
+Config 2: 16 tied SAEs, d = 512, n = 4096, batch 8192, f16f8 arithmetic, fp16-exact activations (bench.py's cfg2).
+For each of the step's four GEMMs (encode, decode, dcode, weight gradient) it reports
+  (a) engine_ms: the mean time of the engine's gemm_split_kernel launch inside step_batch, from torch.profiler with CUDA
+      activities, in a run of its own;
+  (b) main_loop_ms: the same kernel configuration at the same shapes with an epilogue that only reads the accumulators
+      (build/gemm_overlap_probe, Makefile target `probe`), declaring the engine epilogue's staging bytes so that the
+      stage ring is as deep;
+  (c) the card's name, power limit and SM clock, read in the same run after each measurement.
+(a) and (b) are taken in alternated rounds and their medians reported with the range. (a) - (b) is the time the
+epilogue adds to the kernel; the two run on different operands (the engine's training data, hashed finite values),
+which alone can move (b) against (a). Prints a table and one JSON line; --out DIR
+also writes it there.
+
+    python tools/gemm_overlap_probe.py [--steps 20] [--reps 20] [--rounds 5] [--out DIR]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+# epilogue functor in the kernel's name -> GEMM of the step
+EPILOGUES = (("EpiEncodeT", "encode"), ("EpiDecodeT", "decode"), ("EpiDcodeT", "dcode"), ("EpiStoreF32", "dw"))
+
+
+def card():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    out = subprocess.run(["nvidia-smi", "-i", "0", f"--query-gpu={q}", "--format=csv,noheader"],
+                         capture_output=True, text=True, check=True).stdout.strip()
+    return dict(zip(q.split(","), (v.strip() for v in out.split(","))))
+
+
+class EngineRun:
+    """A config-2 ensemble, warmed up; `times()` profiles `steps` training steps and returns the mean device time of
+    each GEMM launch of a step by epilogue (None where no launch of that epilogue was seen) and its launches per step."""
+
+    def __init__(self, steps):
+        import bench
+        import sparse_coding_b200 as S
+
+        M, d, n, B, _ = bench.WORKLOADS["cfg2"]
+        dev = torch.device("cuda", 0)
+        sig = S.FunctionalTiedSAE
+        self.ens = S.FunctionalEnsemble(bench.make_models(sig, M, d, n, seed=0), sig, S.adam, {"lr": 1e-3}, device=dev)
+        self.pool = [x.to(dev) for x in bench.synth_batches(4, B, d, seed=1000)]
+        self.steps = steps
+        for i in range(5):
+            self.ens.step_batch(self.pool[i % len(self.pool)])
+        torch.cuda.synchronize()
+
+    def times(self):
+        from torch.profiler import ProfilerActivity, profile
+
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for i in range(self.steps):
+                self.ens.step_batch(self.pool[i % len(self.pool)])
+            torch.cuda.synchronize()
+        sums = {g: [0.0, 0] for _, g in EPILOGUES}
+        for ev in prof.events():
+            if "gemm_split_kernel" not in ev.name:
+                continue
+            for tag, g in EPILOGUES:
+                if tag in ev.name:
+                    sums[g][0] += ev.device_time / 1e3   # us -> ms
+                    sums[g][1] += 1
+                    break
+        return {g: (t / c if c else None, c / self.steps) for g, (t, c) in sums.items()}
+
+
+def main_loop_times(reps):
+    exe = os.path.join(ROOT, "build", "gemm_overlap_probe")
+    if not os.path.exists(exe):
+        raise SystemExit(f"{exe} is missing: run `make probe` first")
+    out = subprocess.run([exe, str(reps)], capture_output=True, text=True, check=True).stdout
+    return {r["gemm"]: r for r in (json.loads(l) for l in out.splitlines() if l.startswith("{"))}
+
+
+def fmt(v, width):
+    return f"{v:{width}.3f}" if v is not None else f"{'-':>{width}s}"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20, help="profiled training steps per round")
+    ap.add_argument("--reps", type=int, default=20, help="timed launches of each main-loop-only GEMM per round")
+    ap.add_argument("--rounds", type=int, default=5, help="alternated rounds of (a) and (b); medians are reported")
+    ap.add_argument("--out", default=None, help="directory for gemm_overlap_probe.json")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("the probe times kernels on cuda:0 and needs a GPU")
+    info = card()
+    run = EngineRun(args.steps)
+    rounds = []
+    for _ in range(args.rounds):
+        eng = run.times()
+        clock_a = card()["clocks.sm"]
+        ml = main_loop_times(args.reps)
+        clock_b = card()["clocks.sm"]
+        rounds.append({"engine": eng, "main_loop": ml, "clock_after_engine": clock_a, "clock_after_main_loop": clock_b})
+
+    def med(v):
+        v = sorted(x for x in v if x is not None)
+        return v[len(v) // 2] if v else None
+
+    print(f"{info['name']}, power limit {info['power.limit']}, max SM clock {info['clocks.max.sm']}; SM clock read "
+          f"after each round's (a) and (b): " + ", ".join(f"{r['clock_after_engine']} / {r['clock_after_main_loop']}"
+                                                           for r in rounds))
+    print(f"medians of {args.rounds} rounds (min-max in brackets)")
+    print(f"{'gemm':8s} {'launches/step':>13s} {'engine ms':>10s} {'':15s} {'main loop ms':>13s} {'':15s} "
+          f"{'epilogue ms':>12s}")
+    rows = []
+    for _, g in EPILOGUES:
+        a = [r["engine"][g][0] for r in rounds]
+        b = [r["main_loop"][g]["main_loop_ms"] for r in rounds]
+        per_step = rounds[0]["engine"][g][1]
+        ma, mb = med(a), med(b)
+        av = [x for x in a if x is not None]
+        rows.append({"gemm": g, "launches_per_step": per_step, "engine_ms": ma, "main_loop_ms": mb,
+                     "engine_ms_rounds": a, "main_loop_ms_rounds": b,
+                     "epilogue_ms": None if ma is None else ma - mb, "stages": rounds[0]["main_loop"][g]["stages"],
+                     "tiles": rounds[0]["main_loop"][g]["tiles"]})
+        ra = f"[{min(av):.3f}-{max(av):.3f}]" if av else ""
+        print(f"{g:8s} {per_step:13.1f} {fmt(ma, 10)} {ra:15s} {mb:13.3f} {f'[{min(b):.3f}-{max(b):.3f}]':15s} "
+              f"{fmt(None if ma is None else ma - mb, 12)}")
+    res = {"card": info, "rounds": [{k: v for k, v in r.items() if k.startswith("clock")} for r in rounds], "gemms": rows}
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        os.makedirs(args.out, exist_ok=True)
+        with open(os.path.join(args.out, "gemm_overlap_probe.json"), "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()

@@ -1,1 +1,1 @@
-from sparse_coding_b200.learned_dict import LearnedDict, TiedSAE, UntiedSAE  # noqa: F401
+from sparse_coding_b200.learned_dict import LearnedDict, Rotation, TiedSAE, UntiedSAE  # noqa: F401

@@ -29,7 +29,9 @@ extern "C" {
  * descriptor struct; the signature is SCE_TIED plus these two fields, as the masked variants are SCE_TIED plus coef_mask.
  * Zero in both is the earlier behaviour. Unlike the extension above, this one lengthens the descriptor, and the library
  * reads both fields: a caller compiled against the earlier 201 header passes a shorter struct and must be rebuilt (with
- * the two fields zeroed) before it uses this library. */
+ * the two fields zeroed) before it uses this library.
+ * 201 also covers the additive entry points sce_second_moments_workspace_bytes / sce_second_moments (BatchedPCA). They
+ * are plan-less and change nothing above. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -352,6 +354,29 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
 int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,
                    unsigned long long seed, int zero_row_rule, float noise_scale, void* out, int out_half, int* row_nnz,
                    int* code_idx, float* code_val, int code_cap, void* stream);
+
+/* Streaming second moments of shifted rows without a plan (autoencoders/pca.py:54-64 BatchedPCA.train_batch, as one Gram
+ * matrix instead of a [B, d, d] outer-product tensor): for the B rows x_b of x and v_b = x_b - shift (fp32),
+ *   col_sum[j]    += sum_b v_b[j]
+ *   gram[i * d + j] += sum_b v_b[i] v_b[j]
+ *   x            device [B, d] row-major, fp16 (x_is_half = 1, read as it is) or fp32; 16-byte aligned
+ *   shift        device fp32 [d], 16-byte aligned (BatchedPCA: the first batch's column mean, so that the sums stay small
+ *                against the offset of the data and the covariance needs no large cancellation)
+ *   col_sum, gram  device fp64 [d] / [d, d] (gram 16-byte aligned), ACCUMULATED
+ *   arith        sce_arith. AUTO: BF16X3 (the fp32 range, no range check), as sce_similarity. F16F8 needs d % 16 == 0.
+ *   range_flag   device uint32 or NULL: F16F8 sets it to 1 when some v does not fit the fp16 plane (|v| >= 65520 or
+ *                NaN); the sums are then not meaningful. The caller zeroes it.
+ *   d            a multiple of 8 in [8, 8192];  B in [1, 2^21]
+ *   workspace    >= sce_second_moments_workspace_bytes(d, B), 1024-byte aligned: the operand planes of the rows (6 B per
+ *                element), the fp32 Gram partials of the row slices, S d^2 4 B, and the column-sum partials. Host-only;
+ *                0 for invalid arguments. Never decreases with B, so a workspace sized for the longest call serves
+ *                every shorter one.
+ * The Gram matrix runs on the weight gradient's GEMM. The rows are cut into S slices of at most 2048 rows (S chosen from d
+ * and B only), each slice's product is summed in fp32 on the tensor cores, and the slices are added in fp64 in slice order;
+ * the column sums are fp64 from fp32 v. No atomics: results are bitwise repeatable. Asynchronous on `stream`. */
+size_t sce_second_moments_workspace_bytes(int d, int B);
+int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* shift, int arith, double* col_sum,
+                       double* gram, unsigned int* range_flag, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -32,6 +32,7 @@ EXPORTS = [
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
     "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows", "sce_read_center_grad",
+    "sce_second_moments_workspace_bytes", "sce_second_moments",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -190,6 +191,9 @@ def load():
     lib.sce_forward_fragments.argtypes = [vp, vp, i, i, ll, i, i, C.c_ulonglong, vp, vp, vp, vp, vp, vp, vp, vp,
                                           C.c_size_t, vp]
     lib.sce_synth_rows.argtypes = [vp, i, i, vp, i, ll, i, C.c_ulonglong, i, f, vp, i, vp, vp, vp, i, vp]
+    lib.sce_second_moments_workspace_bytes.restype = C.c_size_t
+    lib.sce_second_moments_workspace_bytes.argtypes = [i, i]
+    lib.sce_second_moments.argtypes = [vp, i, i, i, vp, i, vp, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

@@ -20,6 +20,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <vector>
@@ -1431,6 +1432,208 @@ static int run_similarity_t(Launcher& L, const SimOperand& A, const SimOperand& 
 }
 
 // ------------------------------------------------------------------------------------------------
+// second moments (sce_second_moments): column sums and the Gram matrix of shifted rows, for BatchedPCA
+// ------------------------------------------------------------------------------------------------
+// The Gram matrix X^T X reduces over the rows: it is the weight gradient's GEMM (MN-major 16-bit planes, K = rows; f16f8
+// cross terms on E5M2 wgmma from batch-major copies of the 8-bit planes, EpiStoreF32). The rows are cut into S slices of
+// R rows, run as the GEMM's models, so that a d x d output of few tiles still fills the SMs; each slice leaves an fp32
+// partial, and the partials are added in slice order in fp64.
+// Rows one slice accumulates in fp32. The tensor cores' fp32 accumulation truncates, and the Gram diagonal is a sum of
+// squares, so its bias grows with K: 8192-row slices (the training weight gradient's K) left config 5's width 1.1e-5
+// (bf16x3) and 1.7e-5 (f16f8) from fp64 in Frobenius norm, against a 2e-5 bar. 2048 rows leave a quarter of that, for
+// a few more fp32 partials.
+constexpr int kMomRowsMax = 2048;
+constexpr int kMomTargetTiles = 528;   // output tiles a launch aims for (4 waves of 132 SMs; fixed, so results do not
+                                       // depend on the device)
+constexpr int kMomSliceMin = 256;      // no slice shorter than this, unless the call is
+constexpr int kMomBlockRows = 64;      // rows per block of the split kernel (one column-sum partial each)
+constexpr int kMomCallRowsMax = 1 << 21;
+
+// S slices of R rows (R a multiple of 64, the f16f8 K block, and at most kMomRowsMax) for a call of B rows of width d
+static void mom_slices(int d, int B, int* S_out, int* R_out) {
+  const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
+  const int s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
+  int s = (kMomTargetTiles + tiles - 1) / tiles;
+  const int s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
+  if (s > s_short) s = s_short;
+  if (s < s_rows) s = s_rows;
+  const int R = ((B + s - 1) / s + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows;
+  *R_out = R;
+  *S_out = (B + R - 1) / R;
+}
+
+struct MomCarve {
+  Planes x;          // [S * R][d]: the shifted rows, zero beyond B
+  Planes xt;         // f16f8: batch-major copies of the 8-bit planes, [S][d][R]
+  float* part;       // [S][d][d] fp32 Gram partials
+  double* col_part;  // [S * R / kMomBlockRows][d] column-sum partials
+};
+// Carves S slices of `rows` (= S R) padded rows. The workspace query carves upper bounds of both instead, which never
+// decrease with B: the exact S is not monotone in B (at d = 512, B = 64000 takes 33 slices of 1984 rows, B = 65536 32
+// of 2048), and a caller sizes one workspace for its longest call.
+static size_t mom_carve_rows(uint8_t* base, bool f8, int d, size_t S, size_t rows, MomCarve* out) {
+  const size_t dd = (size_t)d;
+  Carve c{base, 0};
+  MomCarve w{};
+  w.x = c.planes(rows * dd, f8);
+  if (f8) {
+    w.xt.lo = c.take<uint8_t>(rows * dd);
+    w.xt.x8 = c.take<uint8_t>(rows * dd);
+    w.xt.f8 = true;
+  }
+  w.part = c.take<float>(S * dd * dd);
+  w.col_part = c.take<double>(rows / kMomBlockRows * dd);
+  if (out) *out = w;
+  return align_up(c.off, 1024);
+}
+static size_t mom_carve(uint8_t* base, bool f8, int d, int B, MomCarve* out) {
+  int S, R;
+  mom_slices(d, B, &S, &R);
+  return mom_carve_rows(base, f8, d, (size_t)S, (size_t)S * R, out);
+}
+// Bounds of mom_slices, non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts
+// from), and S R < B + R <= B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
+static size_t mom_workspace(bool f8, int d, int B) {
+  const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
+  const size_t s_target = (kMomTargetTiles + tiles - 1) / tiles, s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
+  const size_t s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
+  const size_t S = std::max(std::min(s_target, s_short), s_rows);
+  const size_t rows = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax,
+                               S * kMomRowsMax);
+  return mom_carve_rows(nullptr, f8, d, S, rows, nullptr);
+}
+
+// rows r0 .. r0 + 63 of the call (grid.y), four columns per thread (grid.x covers d / 4 threads):
+//   v = x - shift (fp32) -> operand planes; rows >= B are stored as zero in every plane, so that the padded tail of the
+//   last slice adds nothing to the Gram matrix (0 - shift would add shift shift^T per row)
+//   col_part[blockIdx.y][c] = sum of v over the block's rows, in row order in fp64
+//   f16f8: range_flag = 1 when some |v| >= 65520 or v is NaN (the fp16 plane cannot hold it)
+template <int ARITH, class InT>
+__global__ void __launch_bounds__(128) moment_split_kernel(const InT* __restrict__ x, int B, int d,
+                                                           const float* __restrict__ shift, void* __restrict__ hi,
+                                                           void* __restrict__ lo, void* __restrict__ x8,
+                                                           double* __restrict__ col_part, uint32_t* __restrict__ range_flag) {
+  const int c = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (c >= d) return;
+  const float4 sh = __ldg(reinterpret_cast<const float4*>(shift + c));
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+  bool bad = false;
+  const int r0 = blockIdx.y * kMomBlockRows;
+#pragma unroll 4
+  for (int i = 0; i < kMomBlockRows; ++i) {
+    const int r = r0 + i;
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (r < B) {
+      const long long e = (long long)r * d + c;
+      if constexpr (sizeof(InT) == 2) {
+        const uint2 raw = __ldg(reinterpret_cast<const uint2*>(x + e));
+        const __half2 a = *reinterpret_cast<const __half2*>(&raw.x);
+        const __half2 b = *reinterpret_cast<const __half2*>(&raw.y);
+        v[0] = __low2float(a) - sh.x;
+        v[1] = __high2float(a) - sh.y;
+        v[2] = __low2float(b) - sh.z;
+        v[3] = __high2float(b) - sh.w;
+      } else {
+        const float4 f = __ldg(reinterpret_cast<const float4*>(x + e));
+        v[0] = f.x - sh.x;
+        v[1] = f.y - sh.y;
+        v[2] = f.z - sh.z;
+        v[3] = f.w - sh.w;
+      }
+      s0 += v[0];
+      s1 += v[1];
+      s2 += v[2];
+      s3 += v[3];
+      if constexpr (ARITH == kArithF16F8)
+        bad |= !(fabsf(v[0]) < 65520.f && fabsf(v[1]) < 65520.f && fabsf(v[2]) < 65520.f && fabsf(v[3]) < 65520.f);
+    }
+    store_planes4<ARITH>(v, hi, lo, x8, ((long long)r * d + c) / 4);
+  }
+  double* o = col_part + (long long)blockIdx.y * d + c;
+  o[0] = s0;
+  o[1] = s1;
+  o[2] = s2;
+  o[3] = s3;
+  if (bad && range_flag) *range_flag = 1u;   // benign race: all write 1
+}
+
+// gram[i] += sum over the slices s, in order, of part[s][i]; col_sum[j] += sum over the row blocks b, in order, of
+// col_part[b][j]. fp64 throughout; four Gram entries per thread.
+__global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restrict__ part, int S, long long n4,
+                                                            double* __restrict__ gram, const double* __restrict__ col_part,
+                                                            int blocks, int d, double* __restrict__ col_sum) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    for (int s = 0; s < S; ++s) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(part) + (long long)s * n4 + i);
+      a0 += v.x;
+      a1 += v.y;
+      a2 += v.z;
+      a3 += v.w;
+    }
+    double2* g = reinterpret_cast<double2*>(gram) + 2 * i;
+    const double2 g0 = g[0], g1 = g[1];
+    g[0] = make_double2(g0.x + a0, g0.y + a1);
+    g[1] = make_double2(g1.x + a2, g1.y + a3);
+    if (i < d) {
+      double t = 0.0;
+      for (int b = 0; b < blocks; ++b) t += col_part[(long long)b * d + i];
+      col_sum[i] += t;
+    }
+  }
+}
+
+template <int AR>
+static int run_moments_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const MomCarve& w,
+                         double* col_sum, double* gram, uint32_t* range_flag, int device, int sms) {
+  int S, R;
+  mom_slices(d, B, &S, &R);
+  const int blocks = S * R / kMomBlockRows;
+  const dim3 grid((d / 4 + 127) / 128, blocks);
+  uint32_t* flag = AR == kArithF16F8 ? range_flag : nullptr;
+  if (half)
+    TRY(L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi, w.x.lo,
+                 w.x.x8, w.col_part, flag));
+  else
+    TRY(L.launch(moment_split_kernel<AR, float>, grid, 128, 0, static_cast<const float*>(x), B, d, shift, w.x.hi, w.x.lo,
+                 w.x.x8, w.col_part, flag));
+  // the weight gradient's operand geometry (build_maps, dw_operand): 16-bit planes MN-major in tiles of bk rows; f16f8:
+  // 8-bit planes K-major from the batch-major copies
+  const uint64_t S64 = S, R64 = R, d64 = d;
+  const int bk = gemm_bk(AR);
+  GemmMaps maps{};
+  bool ok;
+  if constexpr (AR == kArithF16F8) {
+    const BatchPlanes t{{static_cast<const uint8_t*>(w.x.lo), w.x.x8}, {static_cast<uint8_t*>(w.xt.lo), w.xt.x8}};
+    TRY(L.launch(transpose_batch_u8_kernel, dim3((d + 127) / 128, (R + 127) / 128, 2 * S), 256, 0, t, S, R, d,
+                 (long long)R * d, R));
+    OperandMaps& o = maps.a[0];
+    ok = make_tmap_bf16(&o.hi, w.x.hi, S64, R64, d64, d64, R64 * d64, bk) &&
+         make_tmap_u8_box(&o.lo, w.xt.lo, S64, d64, R64, R64, d64 * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
+         make_tmap_u8_box(&o.x8, w.xt.x8, S64, d64, R64, R64, d64 * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+  } else {
+    ok = operand_maps(maps.a[0], w.x, S64, R64, d64, R64 * d64, bk, 0);
+  }
+  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (second moments: d=%d, %d slices of %d rows)", d, S, R);
+  maps.b[0] = maps.a[0];
+  EpiStoreF32::Params sp;
+  sp.out = w.part;
+  sp.model_stride = (long long)d * d;
+  sp.ld = d;
+  sp.scale = 1.f;
+  // bf16x3 with split accumulators, f16f8 native: the two weight-gradient instantiations
+  if constexpr (AR == kArithF16F8)
+    TRY((launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, S, device, sms, maps, 1, kOnes, kOnes, R, 3, d, d, sp)));
+  else
+    TRY((launch_gemm_t<EpiStoreF32, true, true, true, AR, false>(L, S, device, sms, maps, 1, kOnes, kOnes, R, 3, d, d, sp)));
+  const long long n4 = (long long)d * d / 4;
+  const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
+  return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, gram, w.col_part, (B + kMomBlockRows - 1) / kMomBlockRows,
+                  d, col_sum);
+}
+
+// ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
 extern "C" {
@@ -1979,6 +2182,42 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
   // (a raw operand split above for the range check is split again here: the planes of the arithmetic that runs)
   return f8 ? run_similarity_t<kArithF16F8>(L, A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms)
             : run_similarity_t<kArithBf16x3>(L, A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms);
+}
+
+size_t sce_second_moments_workspace_bytes(int d, int B) {
+  if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
+  return std::max(mom_workspace(false, d, B), mom_workspace(true, d, B));
+}
+
+int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* shift, int arith, double* col_sum,
+                       double* gram, unsigned int* range_flag, void* workspace, size_t workspace_bytes, void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!x || !shift || !col_sum || !gram)
+    return fail(SCE_ERR_INVALID, "second_moments: x, shift, col_sum and gram are required");
+  if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "second_moments: x_is_half must be 0 or 1");
+  if (B < 1 || B > kMomCallRowsMax)
+    return fail(SCE_ERR_INVALID, "second_moments: B = %d outside [1, %d]", B, kMomCallRowsMax);
+  if (d < 8 || d % 8) return fail(SCE_ERR_INVALID, "second_moments: d (%d) must be a positive multiple of 8", d);
+  if (d > 8192) return fail(SCE_ERR_INVALID, "second_moments: d = %d > 8192 is not supported by the row kernels", d);
+  if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "second_moments: unknown arith %d", arith);
+  if (arith == SCE_ARITH_F16F8 && d % 16)
+    return fail(SCE_ERR_INVALID, "second_moments: arith = F16F8 needs d (%d) to be a multiple of 16", d);
+  if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(shift) % 16 ||
+      reinterpret_cast<uintptr_t>(gram) % 16)
+    return fail(SCE_ERR_INVALID, "second_moments: x, shift and gram must be 16-byte aligned");
+  if (int rc = check_workspace(workspace, workspace_bytes, sce_second_moments_workspace_bytes(d, B), "second_moments: "))
+    return rc;
+
+  // ---- device
+  int dev = 0, sms = 0;
+  if (int rc = query_device(&dev, &sms)) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  // AUTO: bf16x3, as sce_similarity: the fp32 range, no range check
+  const bool f8 = arith == SCE_ARITH_F16F8;
+  MomCarve w;
+  mom_carve(static_cast<uint8_t*>(workspace), f8, d, B, &w);
+  return f8 ? run_moments_t<kArithF16F8>(L, x, x_is_half, B, d, shift, w, col_sum, gram, range_flag, dev, sms)
+            : run_moments_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, w, col_sum, gram, range_flag, dev, sms);
 }
 
 int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,

@@ -123,5 +123,26 @@ class TiedSAE(LearnedDict):
         return (batch @ enc.T + self.encoder_bias).clamp(min=0.0)
 
 
-for _cls in (LearnedDict, UntiedSAE, TiedSAE):
+class Rotation(LearnedDict):
+    """learned_dict.py:277-293: a fixed matrix whose rows are the dictionary; the code is linear, ``batch @ matrix^T``.
+    ``activation_size`` is the matrix's row count, as in the reference. The matrix is moved to ``device`` (the CPU by
+    default) on construction."""
+
+    def __init__(self, matrix, device=None):
+        self.device = "cpu" if device is None else device
+        self.matrix = matrix.to(self.device)
+        self.activation_size = matrix.shape[0]
+
+    def get_learned_dict(self):
+        return self.matrix
+
+    def to_device(self, device):
+        self.device = device
+        self.matrix = self.matrix.to(device)
+
+    def encode(self, batch):
+        return batch @ self.matrix.T
+
+
+for _cls in (LearnedDict, UntiedSAE, TiedSAE, Rotation):
     _cls.__module__ = _REF_MODULE

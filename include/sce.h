@@ -31,7 +31,8 @@ extern "C" {
  * reads both fields: a caller compiled against the earlier 201 header passes a shorter struct and must be rebuilt (with
  * the two fields zeroed) before it uses this library.
  * 201 also covers the additive entry points sce_second_moments_workspace_bytes / sce_second_moments (BatchedPCA). They
- * are plan-less and change nothing above. */
+ * are plan-less and change nothing above. So are sce_ica_pass_workspace_bytes / sce_ica_pass (ICAEncoder), added
+ * under 201 as well. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -377,6 +378,32 @@ int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int 
 size_t sce_second_moments_workspace_bytes(int d, int B);
 int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* shift, int arith, double* col_sum,
                        double* gram, unsigned int* range_flag, void* workspace, size_t workspace_bytes, void* stream);
+
+/* One data pass of FastICA's parallel update with the logcosh nonlinearity, without a plan (autoencoders/ica.py's
+ * FastICA().fit, one iteration's two GEMMs): for the B rows x_b of x, v_b = x_b - shift and t_b = tanh(alpha unmix v_b),
+ *   g_sum[i]        += sum_b alpha (1 - t_b[i]^2)
+ *   gx[i * d + j]   += sum_b t_b[i] v_b[j]
+ *   x            device [B, d] row-major, fp16 (x_is_half = 1) or fp32; 16-byte aligned
+ *   shift        device fp32 [d], 16-byte aligned (ICAEncoder: the fp32 column mean)
+ *   unmix        device fp32 [n, d] row-major, 16-byte aligned. ICAEncoder folds the whitening into it, unmix = W Kw, so
+ *                that no whitened copy of the rows is written; gx Kw^T then is the whitened rows' G X1^T.
+ *   alpha        in [1, 2] (sklearn's fun_args alpha)
+ *   g_sum, gx    device fp64 [n] / [n, d] (gx 16-byte aligned), ACCUMULATED
+ *   arith        sce_arith. AUTO: BF16X3 (the fp32 range, no range check). F16F8 needs d % 16 == 0 and n % 16 == 0.
+ *   range_flag   device uint32 or NULL: F16F8 sets it to 1 when some v or some unmix entry does not fit the fp16 plane
+ *                (|v| >= 65520 or NaN); the sums are then not meaningful. The caller zeroes it.
+ *   d            a multiple of 8 in [8, 8192];  n a multiple of 8 in [8, d];  B in [1, 2^21]
+ *   workspace    >= sce_ica_pass_workspace_bytes(d, n, B), 1024-byte aligned: the planes of v, of t and of unmix, the
+ *                fp32 gx partials of the row slices (S n d 4 B) and the g' partials. Host-only; 0 for invalid arguments.
+ *                Never decreases with B.
+ * The rows are sliced as in sce_second_moments. U = V unmix^T runs on the encode GEMM, whose epilogue writes the planes
+ * of t = tanhf(alpha U) (the accurate tanh) and fp32 partials of g' per 32 rows; gx runs on the weight gradient's GEMM per
+ * slice. Partials are added in fp64 in a fixed order. No atomics: results are bitwise repeatable. Asynchronous on
+ * `stream`. */
+size_t sce_ica_pass_workspace_bytes(int d, int n, int B);
+int sce_ica_pass(const void* x, int x_is_half, int B, int d, const float* shift, const float* unmix, int n, float alpha,
+                 int arith, double* g_sum, double* gx, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
+                 void* stream);
 
 #ifdef __cplusplus
 }

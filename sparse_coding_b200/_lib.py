@@ -32,7 +32,7 @@ EXPORTS = [
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
     "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows", "sce_read_center_grad",
-    "sce_second_moments_workspace_bytes", "sce_second_moments",
+    "sce_second_moments_workspace_bytes", "sce_second_moments", "sce_ica_pass_workspace_bytes", "sce_ica_pass",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -194,6 +194,9 @@ def load():
     lib.sce_second_moments_workspace_bytes.restype = C.c_size_t
     lib.sce_second_moments_workspace_bytes.argtypes = [i, i]
     lib.sce_second_moments.argtypes = [vp, i, i, i, vp, i, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_ica_pass_workspace_bytes.restype = C.c_size_t
+    lib.sce_ica_pass_workspace_bytes.argtypes = [i, i, i]
+    lib.sce_ica_pass.argtypes = [vp, i, i, i, vp, vp, i, f, i, vp, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

@@ -1493,13 +1493,17 @@ static size_t mom_carve(uint8_t* base, bool f8, int d, int B, MomCarve* out) {
 }
 // Bounds of mom_slices, non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts
 // from), and S R < B + R <= B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
-static size_t mom_workspace(bool f8, int d, int B) {
+static void mom_bounds(int d, int B, size_t* S_out, size_t* rows_out) {
   const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
   const size_t s_target = (kMomTargetTiles + tiles - 1) / tiles, s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
   const size_t s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
   const size_t S = std::max(std::min(s_target, s_short), s_rows);
-  const size_t rows = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax,
-                               S * kMomRowsMax);
+  *S_out = S;
+  *rows_out = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax, S * kMomRowsMax);
+}
+static size_t mom_workspace(bool f8, int d, int B) {
+  size_t S, rows;
+  mom_bounds(d, B, &S, &rows);
   return mom_carve_rows(nullptr, f8, d, S, rows, nullptr);
 }
 
@@ -1557,11 +1561,15 @@ __global__ void __launch_bounds__(128) moment_split_kernel(const InT* __restrict
   if (bad && range_flag) *range_flag = 1u;   // benign race: all write 1
 }
 
-// gram[i] += sum over the slices s, in order, of part[s][i]; col_sum[j] += sum over the row blocks b, in order, of
-// col_part[b][j]. fp64 throughout; four Gram entries per thread.
+// gram[i] += sum over the slices s, in order, of part[s][i] (an n x d output: n4 = n d / 4, n d >= 4 d); and with
+// col_part, col_sum[j] += sum over the row blocks b, in order, of col_part[b][j] (j < d); with vec_part (sce_ica_pass's
+// g' sums, fp32 per 32 rows), vec_sum[j] += the same over its vec_blocks row blocks (j < n). fp64 throughout; four Gram
+// entries per thread.
 __global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restrict__ part, int S, long long n4,
                                                             double* __restrict__ gram, const double* __restrict__ col_part,
-                                                            int blocks, int d, double* __restrict__ col_sum) {
+                                                            int blocks, int d, double* __restrict__ col_sum,
+                                                            const float* __restrict__ vec_part, int vec_blocks, int n,
+                                                            double* __restrict__ vec_sum) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
     double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
@@ -1576,10 +1584,15 @@ __global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restric
     const double2 g0 = g[0], g1 = g[1];
     g[0] = make_double2(g0.x + a0, g0.y + a1);
     g[1] = make_double2(g1.x + a2, g1.y + a3);
-    if (i < d) {
+    if (col_part && i < d) {
       double t = 0.0;
       for (int b = 0; b < blocks; ++b) t += col_part[(long long)b * d + i];
       col_sum[i] += t;
+    }
+    if (vec_part && i < n) {
+      double t = 0.0;
+      for (int b = 0; b < vec_blocks; ++b) t += vec_part[(long long)b * n + i];
+      vec_sum[i] += t;
     }
   }
 }
@@ -1630,7 +1643,139 @@ static int run_moments_t(Launcher& L, const void* x, bool half, int B, int d, co
   const long long n4 = (long long)d * d / 4;
   const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
   return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, gram, w.col_part, (B + kMomBlockRows - 1) / kMomBlockRows,
-                  d, col_sum);
+                  d, col_sum, nullptr, 0, 0, nullptr);
+}
+
+// ------------------------------------------------------------------------------------------------
+// FastICA pass (sce_ica_pass): one iteration's data pass of sklearn's parallel FastICA with logcosh, for ICAEncoder
+// ------------------------------------------------------------------------------------------------
+// For v = x - shift and t = tanh(alpha unmix v): g_sum += sum_b alpha (1 - t_b^2), gx += sum_b t_b v_b^T. The rows are
+// split and sliced as sce_second_moments splits them (moment_split_kernel, mom_slices: zero padding rows, the range
+// flag). GEMM 1, U = V unmix^T, is the encode geometry (both operands K-major over d) as one model of S R rows, with
+// EpiIcaT writing the planes of t and the g' partials; GEMM 2, gx = T^T V per slice, is the weight gradient's, as
+// run_moments_t launches it with T in place of the first V. Slice partials are added in fp64 in slice order.
+struct IcaCarve {
+  Planes x, xt;      // the shifted rows [S * R][d] (zero beyond B); f16f8: batch-major 8-bit copies [S][d][R]
+  Planes t, tt;      // t [S * R][n]; f16f8: batch-major 8-bit copies [S][n][R]
+  Planes w;          // unmix [n][d]
+  float* part;       // [S][n][d] fp32 gx partials
+  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (unused here)
+  float* g_part;     // [S * R / 32][n] g' partials
+  uint32_t* flags;   // kFlagWords: the f16f8 range check of unmix
+};
+static size_t ica_carve_rows(uint8_t* base, bool f8, int d, int n, size_t S, size_t rows, IcaCarve* out) {
+  const size_t dd = (size_t)d, nn = (size_t)n;
+  Carve c{base, 0};
+  IcaCarve w{};
+  auto copies = [&](Planes& p, size_t count) {
+    p.lo = c.take<uint8_t>(count);
+    p.x8 = c.take<uint8_t>(count);
+    p.f8 = true;
+  };
+  w.x = c.planes(rows * dd, f8);
+  w.t = c.planes(rows * nn, f8);
+  if (f8) {
+    copies(w.xt, rows * dd);
+    copies(w.tt, rows * nn);
+  }
+  w.w = c.planes(nn * dd, f8);
+  w.part = c.take<float>(S * nn * dd);
+  w.col_part = c.take<double>(rows / kMomBlockRows * dd);
+  w.g_part = c.take<float>(rows / 32 * nn);
+  w.flags = c.take<uint32_t>(kFlagWords);
+  if (out) *out = w;
+  return align_up(c.off, 1024);
+}
+static size_t ica_carve(uint8_t* base, bool f8, int d, int n, int B, IcaCarve* out) {
+  int S, R;
+  mom_slices(d, B, &S, &R);
+  return ica_carve_rows(base, f8, d, n, (size_t)S, (size_t)S * R, out);
+}
+// the same upper bounds as mom_workspace, non-decreasing in B
+static size_t ica_workspace(bool f8, int d, int n, int B) {
+  size_t S, rows;
+  mom_bounds(d, B, &S, &rows);
+  return ica_carve_rows(nullptr, f8, d, n, S, rows, nullptr);
+}
+
+__global__ void set_flag_if_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
+  if (*src) *dst = 1u;
+}
+
+template <int AR>
+static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* unmix, int n,
+                     float alpha, const IcaCarve& w, double* g_sum, double* gx, uint32_t* range_flag, int device, int sms) {
+  constexpr bool f8 = AR == kArithF16F8;
+  int S, R;
+  mom_slices(d, B, &S, &R);
+  const int rows = S * R;
+  const dim3 grid((d / 4 + 127) / 128, rows / kMomBlockRows);
+  uint32_t* flag = f8 ? range_flag : nullptr;
+  if (half)
+    TRY(L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi, w.x.lo,
+                 w.x.x8, w.col_part, flag));
+  else
+    TRY(L.launch(moment_split_kernel<AR, float>, grid, 128, 0, static_cast<const float*>(x), B, d, shift, w.x.hi, w.x.lo,
+                 w.x.x8, w.col_part, flag));
+  // unmix -> planes (sce_similarity's raw split); f16f8: its range check joins the rows' in range_flag
+  if (f8 && range_flag) {
+    CUDA_TRY(cudaMemsetAsync(w.flags, 0, kFlagWords * sizeof(uint32_t), L.st));
+    TRY(launch_split_rows<AR>(L, unmix, w.w, (long long)n * d / 4, w.flags));
+    TRY(L.launch(set_flag_if_kernel, 1, 1, 0, w.flags + kBadWord, range_flag));
+  } else {
+    TRY(launch_split_rows<AR>(L, unmix, w.w, (long long)n * d / 4, nullptr));
+  }
+  const uint64_t S64 = S, R64 = R, rows64 = rows, d64 = d, n64 = n;
+  const int bk = gemm_bk(AR);
+  // ---- GEMM 1: U = V unmix^T, t = tanh(alpha U) -> planes of t, g' partials
+  GemmMaps m1{};
+  typename EpiIcaT<AR>::Params ep;
+  bool ok = operand_maps(m1.a[0], w.x, 1, rows64, d64, rows64 * d64, kBM, bk) &&
+            operand_maps(m1.b[0], w.w, 1, n64, d64, n64 * d64, kBN, bk) &&
+            make_tmap_bf16_store32(&ep.out_hi, w.t.hi, 1, rows64, n64, rows64 * n64);
+  if constexpr (f8)
+    ok = ok && make_tmap_u8_box(&ep.out_lo, w.t.lo, 1, rows64, n64, n64, rows64 * n64, 32, 32, CU_TENSOR_MAP_SWIZZLE_32B) &&
+         make_tmap_u8_box(&ep.out_x8, w.t.x8, 1, rows64, n64, n64, rows64 * n64, 32, 32, CU_TENSOR_MAP_SWIZZLE_32B);
+  else
+    ok = ok && make_tmap_bf16_store32(&ep.out_lo, w.t.lo, 1, rows64, n64, rows64 * n64);
+  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (ica pass: d=%d, n=%d, %d rows)", d, n, rows);
+  ep.g_part = w.g_part;
+  ep.alpha = alpha;
+  ep.rows_valid = B;
+  TRY((launch_gemm_t<EpiIcaT<AR>, false, false, false, AR, f8>(L, 1, device, sms, m1, 1, kOnes, kOnes, d, 3, rows, n, ep)));
+  // ---- GEMM 2: gx partials [S][n][d] = T^T V per slice, the weight gradient's operand geometry
+  GemmMaps m2{};
+  if constexpr (f8) {
+    const BatchPlanes tt{{static_cast<const uint8_t*>(w.t.lo), w.t.x8}, {static_cast<uint8_t*>(w.tt.lo), w.tt.x8}};
+    const BatchPlanes xt{{static_cast<const uint8_t*>(w.x.lo), w.x.x8}, {static_cast<uint8_t*>(w.xt.lo), w.xt.x8}};
+    TRY(L.launch(transpose_batch_u8_kernel, dim3((n + 127) / 128, (R + 127) / 128, 2 * S), 256, 0, tt, S, R, n,
+                 (long long)R * n, R));
+    TRY(L.launch(transpose_batch_u8_kernel, dim3((d + 127) / 128, (R + 127) / 128, 2 * S), 256, 0, xt, S, R, d,
+                 (long long)R * d, R));
+    auto native = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t cols) {
+      return make_tmap_bf16(&o.hi, P.hi, S64, R64, cols, cols, R64 * cols, bk) &&
+             make_tmap_u8_box(&o.lo, T.lo, S64, cols, R64, R64, cols * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
+             make_tmap_u8_box(&o.x8, T.x8, S64, cols, R64, R64, cols * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+    };
+    ok = native(m2.a[0], w.t, w.tt, n64) && native(m2.b[0], w.x, w.xt, d64);
+  } else {
+    ok = operand_maps(m2.a[0], w.t, S64, R64, n64, R64 * n64, bk, 0) &&
+         operand_maps(m2.b[0], w.x, S64, R64, d64, R64 * d64, bk, 0);
+  }
+  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (ica pass: d=%d, n=%d, %d slices of %d rows)", d, n, S, R);
+  EpiStoreF32::Params sp;
+  sp.out = w.part;
+  sp.model_stride = (long long)n * d;
+  sp.ld = d;
+  sp.scale = 1.f;
+  if constexpr (f8)
+    TRY((launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, S, device, sms, m2, 1, kOnes, kOnes, R, 3, n, d, sp)));
+  else
+    TRY((launch_gemm_t<EpiStoreF32, true, true, true, AR, false>(L, S, device, sms, m2, 1, kOnes, kOnes, R, 3, n, d, sp)));
+  const long long n4 = (long long)n * d / 4;
+  const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
+  return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, gx, nullptr, 0, d, nullptr, w.g_part, (B + 31) / 32,
+                  n, g_sum);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2218,6 +2363,43 @@ int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* 
   mom_carve(static_cast<uint8_t*>(workspace), f8, d, B, &w);
   return f8 ? run_moments_t<kArithF16F8>(L, x, x_is_half, B, d, shift, w, col_sum, gram, range_flag, dev, sms)
             : run_moments_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, w, col_sum, gram, range_flag, dev, sms);
+}
+
+size_t sce_ica_pass_workspace_bytes(int d, int n, int B) {
+  if (d < 8 || d % 8 || d > 8192 || n < 8 || n % 8 || n > d || B < 1 || B > kMomCallRowsMax) return 0;
+  return std::max(ica_workspace(false, d, n, B), ica_workspace(true, d, n, B));
+}
+
+int sce_ica_pass(const void* x, int x_is_half, int B, int d, const float* shift, const float* unmix, int n, float alpha,
+                 int arith, double* g_sum, double* gx, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
+                 void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!x || !shift || !unmix || !g_sum || !gx)
+    return fail(SCE_ERR_INVALID, "ica_pass: x, shift, unmix, g_sum and gx are required");
+  if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "ica_pass: x_is_half must be 0 or 1");
+  if (B < 1 || B > kMomCallRowsMax) return fail(SCE_ERR_INVALID, "ica_pass: B = %d outside [1, %d]", B, kMomCallRowsMax);
+  if (d < 8 || d % 8 || d > 8192) return fail(SCE_ERR_INVALID, "ica_pass: d (%d) must be a multiple of 8 in [8, 8192]", d);
+  if (n < 8 || n % 8 || n > d) return fail(SCE_ERR_INVALID, "ica_pass: n (%d) must be a multiple of 8 in [8, d = %d]", n, d);
+  if (!(alpha >= 1.f && alpha <= 2.f)) return fail(SCE_ERR_INVALID, "ica_pass: alpha (%g) must be in [1, 2]", (double)alpha);
+  if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "ica_pass: unknown arith %d", arith);
+  if (arith == SCE_ARITH_F16F8 && (d % 16 || n % 16))
+    return fail(SCE_ERR_INVALID, "ica_pass: arith = F16F8 needs d (%d) and n (%d) to be multiples of 16", d, n);
+  if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(shift) % 16 ||
+      reinterpret_cast<uintptr_t>(unmix) % 16 || reinterpret_cast<uintptr_t>(gx) % 16 ||
+      reinterpret_cast<uintptr_t>(g_sum) % 8)
+    return fail(SCE_ERR_INVALID, "ica_pass: x, shift, unmix and gx must be 16-byte aligned, g_sum 8-byte aligned");
+  if (int rc = check_workspace(workspace, workspace_bytes, sce_ica_pass_workspace_bytes(d, n, B), "ica_pass: ")) return rc;
+
+  // ---- device
+  int dev = 0, sms = 0;
+  if (int rc = query_device(&dev, &sms)) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  // AUTO: bf16x3, as sce_second_moments
+  const bool f8 = arith == SCE_ARITH_F16F8;
+  IcaCarve w;
+  ica_carve(static_cast<uint8_t*>(workspace), f8, d, n, B, &w);
+  return f8 ? run_ica_t<kArithF16F8>(L, x, x_is_half, B, d, shift, unmix, n, alpha, w, g_sum, gx, range_flag, dev, sms)
+            : run_ica_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, unmix, n, alpha, w, g_sum, gx, range_flag, dev, sms);
 }
 
 int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,

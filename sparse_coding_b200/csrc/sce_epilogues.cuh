@@ -716,6 +716,56 @@ struct EpiSimilarity {
   }
 };
 
+// ------------------------------------------------------------------------------------------------
+// FastICA pass (sce_ica_pass, sklearn's logcosh nonlinearity): acc = u = unmix v of one row;
+//   t = tanh(alpha u) -> (t_hi, t_lo), [rows][n], as EpiEncodeT writes the code
+//   per warp of 32 rows, the column sums of g' = alpha (1 - t^2) over the rows < rows_valid -> g_part [row_block][n]
+//   (row block = global row / 32; a second kernel adds them over the row blocks in a fixed order in fp64)
+// The accurate tanhf, not tanh.approx.f32: its 2^-11 error would reach gx = sum t v unreduced. The padding rows of the
+// last slice are zero (u = 0, t = 0 adds nothing to gx), but g' = alpha there: they are kept out of the sums.
+// ------------------------------------------------------------------------------------------------
+template <int ARITH>
+struct EpiIcaT {
+  static constexpr int kCols = 32;
+  static constexpr int kWarpStageBytes = 4096;
+  struct Params {
+    CUtensorMap out_hi, out_lo, out_x8;  // store maps of the t planes: [1][rows][n], box 32 x 32
+    float* g_part;                       // [ceil(rows_valid / 32)][n]
+    float alpha;
+    int rows_valid;                      // B: rows at or beyond it are padding
+  };
+  const Params& P;
+  const TileCoord& T;
+  int m_total, n_total;
+  uint8_t* stage;
+  __device__ EpiIcaT(const Params& p, const TileCoord& t, int m, int n, uint8_t* st)
+      : P(p), T(t), m_total(m), n_total(n), stage(st) {}
+
+  __device__ __forceinline__ void chunk(int c, const uint32_t (&r)[32]) {
+    const int col = T.col0 + c;
+    if (col >= n_total) return;  // warp-uniform
+    const bool row_ok = T.row < P.rows_valid;
+    uint32_t whi[16], wlo[16];
+    float g[32];
+#pragma unroll
+    for (int j = 0; j < 32; j += 2) {
+      const float t0 = tanhf(P.alpha * __uint_as_float(r[j])), t1 = tanhf(P.alpha * __uint_as_float(r[j + 1]));
+      split_pair<ARITH>(t0, t1, j >> 1, whi, wlo);
+      g[j] = row_ok ? P.alpha * (1.f - t0 * t0) : 0.f;
+      g[j + 1] = row_ok ? P.alpha * (1.f - t1 * t1) : 0.f;
+    }
+    const int row0 = T.m_blk * kBM + T.warp_q * 32;
+    stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, row0, T.model);
+    if (row0 < P.rows_valid) {   // warp-uniform: some row of this warp is in the batch
+      const float s = warp_column_sum(g, T.lane);
+      if (col + T.lane < n_total) P.g_part[(long long)(row0 >> 5) * n_total + col + T.lane] = s;
+    }
+  }
+  __device__ __forceinline__ void finish() {
+    if (T.lane == 0) tma_store_wait_read();  // the staging tiles must outlive their bulk stores
+  }
+};
+
 using EpiEncode = EpiEncodeT<kArithBf16x3>;
 using EpiDecode = EpiDecodeT<kArithBf16x3>;
 using EpiDcode = EpiDcodeT<kArithBf16x3>;

@@ -211,6 +211,8 @@ struct Carve {
     }
     return p;
   }
+  // the batch-major copies of the two 8-bit planes of `count` elements (f16f8), which have no 16-bit plane
+  Planes copies(size_t count) { return {nullptr, take<uint8_t>(count), take<uint8_t>(count), true}; }
 };
 
 static int validate(const sce_desc* d) {
@@ -374,8 +376,7 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
     // the code's row-major 8-bit planes are read by the decode GEMM only, which runs before dcode writes dz: they live in
     // dz's 8-bit planes (below), and the code's own 8-bit space holds the batch-major copies the weight gradient reads
     w.c.hi = c.take<uint16_t>(M * B * n);
-    w.ct.lo = c.take<uint8_t>(dz8);
-    w.ct.x8 = c.take<uint8_t>(dz8);
+    w.ct = c.copies(dz8);
   }
   w.g = c.planes(M * B * dd, f8);
   // all planes contiguous, 4 B / element (the top-k scores alias them); with tdw the 8-bit ones are [M][n][Bp]
@@ -384,11 +385,9 @@ static size_t carve(PlanBuffers& w, const sce_desc& d, const PlanConfig& cfg, ui
   if (tdw) {
     w.c.lo = w.dz.lo;
     w.c.x8 = w.dz.x8;
-    w.xt.lo = c.take<uint8_t>(xm * dd * Bp);
-    w.xt.x8 = c.take<uint8_t>(xm * dd * Bp);
-    w.gt.lo = c.take<uint8_t>(M * dd * Bp);
-    w.gt.x8 = c.take<uint8_t>(M * dd * Bp);
-    w.c.f8 = w.ct.f8 = w.xt.f8 = w.gt.f8 = true;
+    w.xt = c.copies(xm * dd * Bp);
+    w.gt = c.copies(M * dd * Bp);
+    w.c.f8 = true;
   }
   w.dw_enc = c.take<float>(M * n * dd);
   w.dw_dec = cfg.untied ? c.take<float>(M * n * dd) : w.dw_enc;
@@ -467,6 +466,18 @@ static bool operand_maps(OperandMaps& m, const Planes& P, uint64_t models, uint6
   return ok;
 }
 
+// The weight gradient's operand P [models][k_rows][cols] (`mpitch` elements between models), reduced over its k_rows:
+// MN-major tiles of bk rows. With T, the 8-bit planes come from P's batch-major copies T [models][cols][t_pitch] instead
+// (batch_major), K-major tiles [128 rows][64 B] with the 64-byte swizzle E5M2 wgmma reads; only k_rows columns of T are
+// exposed, so the tail of a short batch reads as zero.
+static bool dw_operand_maps(OperandMaps& m, const Planes& P, const Planes* T, uint64_t models, uint64_t k_rows,
+                            uint64_t cols, uint64_t mpitch, uint64_t t_pitch, int bk) {
+  if (!T) return operand_maps(m, P, models, k_rows, cols, mpitch, bk, 0);
+  return make_tmap_bf16(&m.hi, P.hi, models, k_rows, cols, cols, mpitch, bk) &&
+         make_tmap_u8_box(&m.lo, T->lo, models, cols, k_rows, t_pitch, cols * t_pitch, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
+         make_tmap_u8_box(&m.x8, T->x8, models, cols, k_rows, t_pitch, cols * t_pitch, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
 static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   auto it = p->maps->find(B);
   if (it != p->maps->end()) {
@@ -506,15 +517,10 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
   ok &= act_a(m->dcode.a[0], p->g, M, dd);
   ok &= dict_b(m->dcode.b[0], p->wdec, kBN, bk);
-  // weight gradients: everything MN-major, tiles of bk batch rows, reduction over the batch rows. dw_native: the 8-bit
-  // planes come from the batch-major copies T [models][cols][Bp] instead, K-major tiles [128 rows][64 B] with the 64-byte
-  // swizzle; only B columns are exposed, so the tail of a short batch reads as zero
+  // weight gradients: reduction over the batch rows; dw_native: the 8-bit planes from the batch-major copies [models][cols][Bp]
   const uint64_t Bp = (uint64_t)cfg.bpad;
   auto dw_operand = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t models, uint64_t cols) {
-    if (!cfg.dw_native) return operand_maps(o, P, models, (uint64_t)B, cols, Bm * cols, bk, 0);
-    return make_tmap_bf16(&o.hi, P.hi, models, (uint64_t)B, cols, cols, Bm * cols, bk) &&
-           make_tmap_u8_box(&o.lo, T.lo, models, cols, (uint64_t)B, Bp, cols * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
-           make_tmap_u8_box(&o.x8, T.x8, models, cols, (uint64_t)B, Bp, cols * Bp, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+    return dw_operand_maps(o, P, cfg.dw_native ? &T : nullptr, models, (uint64_t)B, cols, Bm * cols, Bp, bk);
   };
   // dz^T x, then c^T g: a second GEMM of the decoder (untied) or a second operand set of the one dictionary's
   // (dz's own 8-bit planes are batch-major in dw_native plans)
@@ -598,6 +604,17 @@ static int launch_gemm_t(Launcher& L, int n_models, int device, int sms, const G
   CUDA_TRY((launch_gemm<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, NATIVE>(gp, device, sms, L.st)));
   ++L.count;
   return SCE_OK;
+}
+
+// The weight gradient's GEMM (launch_gemm_t's arguments after L): a reduction over rows, both operands as
+// dw_operand_maps builds them, fp32 out. bf16x3 keeps split accumulators (f16f8 rescales inside one). `native` (f16f8,
+// 8-bit planes from batch-major copies): the cross terms run on E5M2 wgmma; else the 8-bit tiles are widened to fp16.
+template <int AR, class... A>
+static int launch_dw_t(Launcher& L, bool native, const A&... args) {
+  constexpr bool f8 = AR == kArithF16F8;
+  if constexpr (f8)
+    if (native) return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, args...);
+  return launch_gemm_t<EpiStoreF32, true, true, !f8, AR, false>(L, args...);
 }
 
 // One call of a plan: its launches, and the batch of B rows and its tensor maps (run_pipeline opens it)
@@ -744,13 +761,13 @@ static TopkLists topk_lists(const sce_plan* p) {
   return {p->tk_col, p->tk_val, p->tk_cnt, p->cfg.tk_kmax, p->d.batch_max};
 }
 
-// dw_native: the batch-major copy T [models][cols][Bp] of the 8-bit planes of P [models][B of batch_max][cols], which
-// the weight gradient reads (dz's are written so by dcode)
-static int batch_major(PlanCall& c, const Planes& P, const Planes& T, int models, int cols) {
+// The batch-major copy T [models][cols][ld] of the 8-bit planes of P [models][rows][cols] (`src_pitch` elements between
+// models), from which the native weight gradient reads them (dw_operand_maps; dz's are written so by dcode)
+static int batch_major(Launcher& L, const Planes& P, const Planes& T, int models, int rows, int cols, long long src_pitch,
+                       int ld) {
   const BatchPlanes t{{static_cast<const uint8_t*>(P.lo), P.x8}, {static_cast<uint8_t*>(T.lo), T.x8}};
-  const long long Bm = c.p->d.batch_max;
-  return c.launch(transpose_batch_u8_kernel, dim3((cols + 127) / 128, (c.B + 127) / 128, 2 * models), 256, 0, t, models,
-                  c.B, cols, Bm * cols, c.p->cfg.bpad);
+  return L.launch(transpose_batch_u8_kernel, dim3((cols + 127) / 128, (rows + 127) / 128, 2 * models), 256, 0, t, models,
+                  rows, cols, src_pitch, ld);
 }
 
 // Input: centring or the learned centre's subtraction, the batch split (with the input shift), the batch-major copy of
@@ -791,7 +808,7 @@ static int input_phase(PlanCall& c, const float*& x, bool tdw) {
                               f8 ? p->res_flags : nullptr, cfg.shift,
                               cfg.shift != 0.f ? p->x_shifted + (long long)m * B * dd : nullptr));
   if (cfg.shift != 0.f) x = p->x_shifted;
-  if (tdw) TRY(batch_major(c, p->x, p->xt, cfg.xm, dd));
+  if (tdw) TRY(batch_major(c, p->x, p->xt, cfg.xm, B, dd, Bm * dd, cfg.bpad));
   p->code_batch_major = tdw ? 1 : 0;
   // alpha / B, or (f16f8, backward on r = g B d / 2) alpha d / 2
   return c.launch(l1_over_b_kernel, (M + 127) / 128, 128, 0, p->b.l1_alpha, p->l1_over_b, M,
@@ -836,7 +853,7 @@ static int encode_phase(PlanCall& c, bool tdw, float* mom_part) {
       TRY((c.gemm<EpiEncodeT<AR>, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep,
                                                            x_is_a)));
     }
-    return tdw ? batch_major(c, p->c, p->ct, M, n) : SCE_OK;
+    return tdw ? batch_major(c, p->c, p->ct, M, B, n, (long long)d.batch_max * n, cfg.bpad) : SCE_OK;
   }
   // scores -> fp32 and the chunk maxima of every row, then per-row selection (code planes, activity mask, k-sparse
   // lists) from the chunk maxima (the kernel reads whole rows where they cannot bound the k-th largest score)
@@ -902,7 +919,7 @@ static int decode_phase(PlanCall& c, const float* x, float* x_hat, bool backward
       return c.gemm<E, false, true, false, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
   };
   TRY(cfg.learned ? decode(TypeTag<EpiDecodeT<AR, true>>{}) : decode(TypeTag<EpiDecodeT<AR>>{}));
-  return tdw ? batch_major(c, p->g, p->gt, M, dd) : SCE_OK;
+  return tdw ? batch_major(c, p->g, p->gt, M, B, dd, (long long)d.batch_max * dd, cfg.bpad) : SCE_OK;
 }
 
 // Losses: the bias norm (bias decay), then the loss columns and nnz from the partials of encode and decode
@@ -962,12 +979,7 @@ static int backward_phase(PlanCall& c) {
     sp.model_stride = (long long)n * dd;
     sp.ld = dd;
     sp.scale = grad_out_scale(p, B);
-    // reduction over the batch: split accumulators for bf16x3 (f16f8 rescales inside one). dw_native: fp16 planes
-    // MN-major, 8-bit planes K-major from their batch-major copies, cross terms on E5M2 wgmma; else widened
-    if constexpr (f8)
-      if (cfg.dw_native)
-        return c.gemm<EpiStoreF32, true, true, false, AR, true>(gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
-    return c.gemm<EpiStoreF32, true, true, !f8, AR>(gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
+    return launch_dw_t<AR>(c, cfg.dw_native, M, p->device, p->sms, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
   };
   ResFlags x_is_b;   // the batch's residual-plane flag, for the GEMM that reads x as its B operand (set 0)
   if constexpr (f8) x_is_b.b[0] = p->res_flags;
@@ -1432,12 +1444,13 @@ static int run_similarity_t(Launcher& L, const SimOperand& A, const SimOperand& 
 }
 
 // ------------------------------------------------------------------------------------------------
-// second moments (sce_second_moments): column sums and the Gram matrix of shifted rows, for BatchedPCA
+// sliced row passes: second moments (sce_second_moments, for BatchedPCA) and the FastICA pass (sce_ica_pass)
 // ------------------------------------------------------------------------------------------------
-// The Gram matrix X^T X reduces over the rows: it is the weight gradient's GEMM (MN-major 16-bit planes, K = rows; f16f8
-// cross terms on E5M2 wgmma from batch-major copies of the 8-bit planes, EpiStoreF32). The rows are cut into S slices of
-// R rows, run as the GEMM's models, so that a d x d output of few tiles still fills the SMs; each slice leaves an fp32
-// partial, and the partials are added in slice order in fp64.
+// Both end in a reduction over the rows, A^T V for the shifted rows V: the Gram matrix V^T V, or FastICA's T^T V. It is
+// the weight gradient's GEMM (MN-major 16-bit planes, K = rows; f16f8 cross terms on E5M2 wgmma from batch-major copies
+// of the 8-bit planes, EpiStoreF32). The rows are cut into S slices of R rows, run as the GEMM's models, so that an
+// output of few tiles still fills the SMs; each slice leaves an fp32 partial, and the partials are added in slice order
+// in fp64.
 // Rows one slice accumulates in fp32. The tensor cores' fp32 accumulation truncates, and the Gram diagonal is a sum of
 // squares, so its bias grows with K: 8192-row slices (the training weight gradient's K) left config 5's width 1.1e-5
 // (bf16x3) and 1.7e-5 (f16f8) from fp64 in Frobenius norm, against a 2e-5 bar. 2048 rows leave a quarter of that, for
@@ -1449,8 +1462,11 @@ constexpr int kMomSliceMin = 256;      // no slice shorter than this, unless the
 constexpr int kMomBlockRows = 64;      // rows per block of the split kernel (one column-sum partial each)
 constexpr int kMomCallRowsMax = 1 << 21;
 
-// S slices of R rows (R a multiple of 64, the f16f8 K block, and at most kMomRowsMax) for a call of B rows of width d
-static void mom_slices(int d, int B, int* S_out, int* R_out) {
+struct Slices {   // a call's rows as S slices of R rows (R a multiple of 64, the f16f8 K block, and at most kMomRowsMax)
+  int S, R;
+};
+// the slices of a call of B rows of width d
+static Slices mom_slices(int d, int B) {
   const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
   const int s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
   int s = (kMomTargetTiles + tiles - 1) / tiles;
@@ -1458,53 +1474,54 @@ static void mom_slices(int d, int B, int* S_out, int* R_out) {
   if (s > s_short) s = s_short;
   if (s < s_rows) s = s_rows;
   const int R = ((B + s - 1) / s + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows;
-  *R_out = R;
-  *S_out = (B + R - 1) / R;
+  return {(B + R - 1) / R, R};
 }
 
-struct MomCarve {
-  Planes x;          // [S * R][d]: the shifted rows, zero beyond B
-  Planes xt;         // f16f8: batch-major copies of the 8-bit planes, [S][d][R]
-  float* part;       // [S][d][d] fp32 Gram partials
-  double* col_part;  // [S * R / kMomBlockRows][d] column-sum partials
+// The buffers of a row pass of width d: the second moments' (n = 0), or the FastICA pass's with n components, which
+// alone take t, its copies, the unmix planes, the g' partials and the flag words
+struct RowCarve {
+  Planes x, xt;      // the shifted rows [S * R][d] (zero beyond B); f16f8: batch-major 8-bit copies [S][d][R]
+  Planes t, tt;      // ICA: t [S * R][n]; f16f8: batch-major 8-bit copies [S][n][R]
+  Planes w;          // ICA: unmix [n][d]
+  float* part;       // [S][n, or d][d] fp32 slice partials
+  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (unused by ICA)
+  float* g_part;     // ICA: [S * R / 32][n] g' partials
+  uint32_t* flags;   // ICA: kFlagWords, the f16f8 range check of unmix
 };
 // Carves S slices of `rows` (= S R) padded rows. The workspace query carves upper bounds of both instead, which never
 // decrease with B: the exact S is not monotone in B (at d = 512, B = 64000 takes 33 slices of 1984 rows, B = 65536 32
 // of 2048), and a caller sizes one workspace for its longest call.
-static size_t mom_carve_rows(uint8_t* base, bool f8, int d, size_t S, size_t rows, MomCarve* out) {
-  const size_t dd = (size_t)d;
+static size_t row_carve(uint8_t* base, bool f8, int d, int n, size_t S, size_t rows, RowCarve* out) {
+  const size_t dd = (size_t)d, nn = (size_t)n;
   Carve c{base, 0};
-  MomCarve w{};
+  RowCarve w{};
   w.x = c.planes(rows * dd, f8);
+  if (n) w.t = c.planes(rows * nn, f8);
   if (f8) {
-    w.xt.lo = c.take<uint8_t>(rows * dd);
-    w.xt.x8 = c.take<uint8_t>(rows * dd);
-    w.xt.f8 = true;
+    w.xt = c.copies(rows * dd);
+    if (n) w.tt = c.copies(rows * nn);
   }
-  w.part = c.take<float>(S * dd * dd);
+  if (n) w.w = c.planes(nn * dd, f8);
+  w.part = c.take<float>(S * (n ? nn : dd) * dd);
   w.col_part = c.take<double>(rows / kMomBlockRows * dd);
+  if (n) {
+    w.g_part = c.take<float>(rows / 32 * nn);
+    w.flags = c.take<uint32_t>(kFlagWords);
+  }
   if (out) *out = w;
   return align_up(c.off, 1024);
 }
-static size_t mom_carve(uint8_t* base, bool f8, int d, int B, MomCarve* out) {
-  int S, R;
-  mom_slices(d, B, &S, &R);
-  return mom_carve_rows(base, f8, d, (size_t)S, (size_t)S * R, out);
-}
-// Bounds of mom_slices, non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts
-// from), and S R < B + R <= B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
-static void mom_bounds(int d, int B, size_t* S_out, size_t* rows_out) {
+// The workspace of a row pass, for both arithmetics; 0 when d or B is out of range. It carves the bounds of mom_slices,
+// non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts from), and S R < B + R <=
+// B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
+static size_t row_pass_workspace(int d, int n, int B) {
+  if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
   const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
   const size_t s_target = (kMomTargetTiles + tiles - 1) / tiles, s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
   const size_t s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
   const size_t S = std::max(std::min(s_target, s_short), s_rows);
-  *S_out = S;
-  *rows_out = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax, S * kMomRowsMax);
-}
-static size_t mom_workspace(bool f8, int d, int B) {
-  size_t S, rows;
-  mom_bounds(d, B, &S, &rows);
-  return mom_carve_rows(nullptr, f8, d, S, rows, nullptr);
+  const size_t rows = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax, S * kMomRowsMax);
+  return std::max(row_carve(nullptr, false, d, n, S, rows, nullptr), row_carve(nullptr, true, d, n, S, rows, nullptr));
 }
 
 // rows r0 .. r0 + 63 of the call (grid.y), four columns per thread (grid.x covers d / 4 threads):
@@ -1597,126 +1614,82 @@ __global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restric
   }
 }
 
+// moment_split_kernel over the S R rows of a call: the shifted rows into the planes of w.x, the column-sum partials and,
+// with f16f8, the range flag
 template <int AR>
-static int run_moments_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const MomCarve& w,
-                         double* col_sum, double* gram, uint32_t* range_flag, int device, int sms) {
-  int S, R;
-  mom_slices(d, B, &S, &R);
-  const int blocks = S * R / kMomBlockRows;
-  const dim3 grid((d / 4 + 127) / 128, blocks);
+static int launch_row_split(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const Slices& sl,
+                            const RowCarve& w, uint32_t* range_flag) {
+  const dim3 grid((d / 4 + 127) / 128, sl.S * sl.R / kMomBlockRows);
   uint32_t* flag = AR == kArithF16F8 ? range_flag : nullptr;
   if (half)
-    TRY(L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi, w.x.lo,
-                 w.x.x8, w.col_part, flag));
-  else
-    TRY(L.launch(moment_split_kernel<AR, float>, grid, 128, 0, static_cast<const float*>(x), B, d, shift, w.x.hi, w.x.lo,
-                 w.x.x8, w.col_part, flag));
-  // the weight gradient's operand geometry (build_maps, dw_operand): 16-bit planes MN-major in tiles of bk rows; f16f8:
-  // 8-bit planes K-major from the batch-major copies
-  const uint64_t S64 = S, R64 = R, d64 = d;
+    return L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi,
+                    w.x.lo, w.x.x8, w.col_part, flag);
+  return L.launch(moment_split_kernel<AR, float>, grid, 128, 0, static_cast<const float*>(x), B, d, shift, w.x.hi, w.x.lo,
+                  w.x.x8, w.col_part, flag);
+}
+
+// part[s] = A_s^T V_s (fp32 [S][m][d]) for the slices s of R rows of A [S R][m] and V [S R][d]: the weight gradient's
+// GEMM, one slice per model. f16f8: first the batch-major copies At and Vt of their 8-bit planes (one when A is V).
+template <int AR>
+static int sliced_gemm_t(Launcher& L, const Slices& sl, const Planes& A, const Planes& At, int m, const Planes& V,
+                         const Planes& Vt, int d, float* part, int device, int sms) {
+  constexpr bool f8 = AR == kArithF16F8;
+  const bool a_is_v = A.hi == V.hi;
+  const int S = sl.S, R = sl.R;
+  if constexpr (f8) {
+    TRY(batch_major(L, A, At, S, R, m, (long long)R * m, R));
+    if (!a_is_v) TRY(batch_major(L, V, Vt, S, R, d, (long long)R * d, R));
+  }
   const int bk = gemm_bk(AR);
   GemmMaps maps{};
-  bool ok;
-  if constexpr (AR == kArithF16F8) {
-    const BatchPlanes t{{static_cast<const uint8_t*>(w.x.lo), w.x.x8}, {static_cast<uint8_t*>(w.xt.lo), w.xt.x8}};
-    TRY(L.launch(transpose_batch_u8_kernel, dim3((d + 127) / 128, (R + 127) / 128, 2 * S), 256, 0, t, S, R, d,
-                 (long long)R * d, R));
-    OperandMaps& o = maps.a[0];
-    ok = make_tmap_bf16(&o.hi, w.x.hi, S64, R64, d64, d64, R64 * d64, bk) &&
-         make_tmap_u8_box(&o.lo, w.xt.lo, S64, d64, R64, R64, d64 * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
-         make_tmap_u8_box(&o.x8, w.xt.x8, S64, d64, R64, R64, d64 * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
-  } else {
-    ok = operand_maps(maps.a[0], w.x, S64, R64, d64, R64 * d64, bk, 0);
-  }
-  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (second moments: d=%d, %d slices of %d rows)", d, S, R);
-  maps.b[0] = maps.a[0];
+  bool ok = dw_operand_maps(maps.a[0], A, f8 ? &At : nullptr, S, R, m, (uint64_t)R * m, R, bk);
+  if (a_is_v) maps.b[0] = maps.a[0];
+  else ok = ok && dw_operand_maps(maps.b[0], V, f8 ? &Vt : nullptr, S, R, d, (uint64_t)R * d, R, bk);
+  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (row pass: %d x %d, %d slices of %d rows)", m, d, S, R);
   EpiStoreF32::Params sp;
-  sp.out = w.part;
-  sp.model_stride = (long long)d * d;
+  sp.out = part;
+  sp.model_stride = (long long)m * d;
   sp.ld = d;
   sp.scale = 1.f;
-  // bf16x3 with split accumulators, f16f8 native: the two weight-gradient instantiations
-  if constexpr (AR == kArithF16F8)
-    TRY((launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, S, device, sms, maps, 1, kOnes, kOnes, R, 3, d, d, sp)));
-  else
-    TRY((launch_gemm_t<EpiStoreF32, true, true, true, AR, false>(L, S, device, sms, maps, 1, kOnes, kOnes, R, 3, d, d, sp)));
-  const long long n4 = (long long)d * d / 4;
+  return launch_dw_t<AR>(L, f8, S, device, sms, maps, 1, kOnes, kOnes, R, 3, m, d, sp);
+}
+
+// out [n, or d][d] += the slice partials of a row pass of B rows; second moments (n = 0): col_sum += the split's
+// column sums; ICA: g_sum += the g' partials
+static int reduce_rows(Launcher& L, const RowCarve& w, int B, int S, int n, int d, double* out, double* col_sum,
+                       double* g_sum) {
+  const long long n4 = (long long)(n ? n : d) * d / 4;
   const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, gram, w.col_part, (B + kMomBlockRows - 1) / kMomBlockRows,
-                  d, col_sum, nullptr, 0, 0, nullptr);
+  return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, out, n ? nullptr : w.col_part,
+                  (B + kMomBlockRows - 1) / kMomBlockRows, d, col_sum, w.g_part, (B + 31) / 32, n, g_sum);
+}
+
+template <int AR>
+static int run_moments_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const Slices& sl,
+                         const RowCarve& w, double* col_sum, double* gram, uint32_t* range_flag, int device, int sms) {
+  TRY(launch_row_split<AR>(L, x, half, B, d, shift, sl, w, range_flag));
+  TRY(sliced_gemm_t<AR>(L, sl, w.x, w.xt, d, w.x, w.xt, d, w.part, device, sms));
+  return reduce_rows(L, w, B, sl.S, 0, d, gram, col_sum, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------
 // FastICA pass (sce_ica_pass): one iteration's data pass of sklearn's parallel FastICA with logcosh, for ICAEncoder
 // ------------------------------------------------------------------------------------------------
 // For v = x - shift and t = tanh(alpha unmix v): g_sum += sum_b alpha (1 - t_b^2), gx += sum_b t_b v_b^T. The rows are
-// split and sliced as sce_second_moments splits them (moment_split_kernel, mom_slices: zero padding rows, the range
-// flag). GEMM 1, U = V unmix^T, is the encode geometry (both operands K-major over d) as one model of S R rows, with
-// EpiIcaT writing the planes of t and the g' partials; GEMM 2, gx = T^T V per slice, is the weight gradient's, as
-// run_moments_t launches it with T in place of the first V. Slice partials are added in fp64 in slice order.
-struct IcaCarve {
-  Planes x, xt;      // the shifted rows [S * R][d] (zero beyond B); f16f8: batch-major 8-bit copies [S][d][R]
-  Planes t, tt;      // t [S * R][n]; f16f8: batch-major 8-bit copies [S][n][R]
-  Planes w;          // unmix [n][d]
-  float* part;       // [S][n][d] fp32 gx partials
-  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (unused here)
-  float* g_part;     // [S * R / 32][n] g' partials
-  uint32_t* flags;   // kFlagWords: the f16f8 range check of unmix
-};
-static size_t ica_carve_rows(uint8_t* base, bool f8, int d, int n, size_t S, size_t rows, IcaCarve* out) {
-  const size_t dd = (size_t)d, nn = (size_t)n;
-  Carve c{base, 0};
-  IcaCarve w{};
-  auto copies = [&](Planes& p, size_t count) {
-    p.lo = c.take<uint8_t>(count);
-    p.x8 = c.take<uint8_t>(count);
-    p.f8 = true;
-  };
-  w.x = c.planes(rows * dd, f8);
-  w.t = c.planes(rows * nn, f8);
-  if (f8) {
-    copies(w.xt, rows * dd);
-    copies(w.tt, rows * nn);
-  }
-  w.w = c.planes(nn * dd, f8);
-  w.part = c.take<float>(S * nn * dd);
-  w.col_part = c.take<double>(rows / kMomBlockRows * dd);
-  w.g_part = c.take<float>(rows / 32 * nn);
-  w.flags = c.take<uint32_t>(kFlagWords);
-  if (out) *out = w;
-  return align_up(c.off, 1024);
-}
-static size_t ica_carve(uint8_t* base, bool f8, int d, int n, int B, IcaCarve* out) {
-  int S, R;
-  mom_slices(d, B, &S, &R);
-  return ica_carve_rows(base, f8, d, n, (size_t)S, (size_t)S * R, out);
-}
-// the same upper bounds as mom_workspace, non-decreasing in B
-static size_t ica_workspace(bool f8, int d, int n, int B) {
-  size_t S, rows;
-  mom_bounds(d, B, &S, &rows);
-  return ica_carve_rows(nullptr, f8, d, n, S, rows, nullptr);
-}
-
+// split and sliced as for the second moments (launch_row_split: zero padding rows, the range flag). GEMM 1, U = V
+// unmix^T, is the encode geometry (both operands K-major over d) as one model of S R rows, with EpiIcaT writing the
+// planes of t and the g' partials; GEMM 2, gx = T^T V per slice, is sliced_gemm_t with T in place of the first V.
 __global__ void set_flag_if_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
   if (*src) *dst = 1u;
 }
 
 template <int AR>
 static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* unmix, int n,
-                     float alpha, const IcaCarve& w, double* g_sum, double* gx, uint32_t* range_flag, int device, int sms) {
+                     float alpha, const Slices& sl, const RowCarve& w, double* g_sum, double* gx, uint32_t* range_flag,
+                     int device, int sms) {
   constexpr bool f8 = AR == kArithF16F8;
-  int S, R;
-  mom_slices(d, B, &S, &R);
-  const int rows = S * R;
-  const dim3 grid((d / 4 + 127) / 128, rows / kMomBlockRows);
-  uint32_t* flag = f8 ? range_flag : nullptr;
-  if (half)
-    TRY(L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi, w.x.lo,
-                 w.x.x8, w.col_part, flag));
-  else
-    TRY(L.launch(moment_split_kernel<AR, float>, grid, 128, 0, static_cast<const float*>(x), B, d, shift, w.x.hi, w.x.lo,
-                 w.x.x8, w.col_part, flag));
+  const int rows = sl.S * sl.R;
+  TRY(launch_row_split<AR>(L, x, half, B, d, shift, sl, w, range_flag));
   // unmix -> planes (sce_similarity's raw split); f16f8: its range check joins the rows' in range_flag
   if (f8 && range_flag) {
     CUDA_TRY(cudaMemsetAsync(w.flags, 0, kFlagWords * sizeof(uint32_t), L.st));
@@ -1725,7 +1698,7 @@ static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const 
   } else {
     TRY(launch_split_rows<AR>(L, unmix, w.w, (long long)n * d / 4, nullptr));
   }
-  const uint64_t S64 = S, R64 = R, rows64 = rows, d64 = d, n64 = n;
+  const uint64_t rows64 = rows, d64 = d, n64 = n;
   const int bk = gemm_bk(AR);
   // ---- GEMM 1: U = V unmix^T, t = tanh(alpha U) -> planes of t, g' partials
   GemmMaps m1{};
@@ -1743,39 +1716,26 @@ static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const 
   ep.alpha = alpha;
   ep.rows_valid = B;
   TRY((launch_gemm_t<EpiIcaT<AR>, false, false, false, AR, f8>(L, 1, device, sms, m1, 1, kOnes, kOnes, d, 3, rows, n, ep)));
-  // ---- GEMM 2: gx partials [S][n][d] = T^T V per slice, the weight gradient's operand geometry
-  GemmMaps m2{};
-  if constexpr (f8) {
-    const BatchPlanes tt{{static_cast<const uint8_t*>(w.t.lo), w.t.x8}, {static_cast<uint8_t*>(w.tt.lo), w.tt.x8}};
-    const BatchPlanes xt{{static_cast<const uint8_t*>(w.x.lo), w.x.x8}, {static_cast<uint8_t*>(w.xt.lo), w.xt.x8}};
-    TRY(L.launch(transpose_batch_u8_kernel, dim3((n + 127) / 128, (R + 127) / 128, 2 * S), 256, 0, tt, S, R, n,
-                 (long long)R * n, R));
-    TRY(L.launch(transpose_batch_u8_kernel, dim3((d + 127) / 128, (R + 127) / 128, 2 * S), 256, 0, xt, S, R, d,
-                 (long long)R * d, R));
-    auto native = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t cols) {
-      return make_tmap_bf16(&o.hi, P.hi, S64, R64, cols, cols, R64 * cols, bk) &&
-             make_tmap_u8_box(&o.lo, T.lo, S64, cols, R64, R64, cols * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
-             make_tmap_u8_box(&o.x8, T.x8, S64, cols, R64, R64, cols * R64, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
-    };
-    ok = native(m2.a[0], w.t, w.tt, n64) && native(m2.b[0], w.x, w.xt, d64);
-  } else {
-    ok = operand_maps(m2.a[0], w.t, S64, R64, n64, R64 * n64, bk, 0) &&
-         operand_maps(m2.b[0], w.x, S64, R64, d64, R64 * d64, bk, 0);
-  }
-  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (ica pass: d=%d, n=%d, %d slices of %d rows)", d, n, S, R);
-  EpiStoreF32::Params sp;
-  sp.out = w.part;
-  sp.model_stride = (long long)n * d;
-  sp.ld = d;
-  sp.scale = 1.f;
-  if constexpr (f8)
-    TRY((launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, S, device, sms, m2, 1, kOnes, kOnes, R, 3, n, d, sp)));
-  else
-    TRY((launch_gemm_t<EpiStoreF32, true, true, true, AR, false>(L, S, device, sms, m2, 1, kOnes, kOnes, R, 3, n, d, sp)));
-  const long long n4 = (long long)n * d / 4;
-  const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, gx, nullptr, 0, d, nullptr, w.g_part, (B + 31) / 32,
-                  n, g_sum);
+  // ---- GEMM 2: gx partials [S][n][d] = T^T V per slice
+  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, n, w.x, w.xt, d, w.part, device, sms));
+  return reduce_rows(L, w, B, sl.S, n, d, gx, nullptr, g_sum);
+}
+
+// The checks sce_second_moments and sce_ica_pass share, made before any CUDA call (`n`: ICA's, or 0): the rows x [B][d],
+// fp16 or fp32, and shift [d], 16-byte aligned; the arithmetic
+static int check_row_pass(const char* prefix, const void* x, int x_is_half, int B, int d, const float* shift, int n,
+                          int arith) {
+  if (!x || !shift) return fail(SCE_ERR_INVALID, "%sx and shift are required", prefix);
+  if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "%sx_is_half must be 0 or 1", prefix);
+  if (B < 1 || B > kMomCallRowsMax) return fail(SCE_ERR_INVALID, "%sB = %d outside [1, %d]", prefix, B, kMomCallRowsMax);
+  if (d < 8 || d % 8 || d > 8192) return fail(SCE_ERR_INVALID, "%sd (%d) must be a multiple of 8 in [8, 8192]", prefix, d);
+  if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "%sunknown arith %d", prefix, arith);
+  if (arith == SCE_ARITH_F16F8 && (d % 16 || n % 16))
+    return n ? fail(SCE_ERR_INVALID, "%sarith = F16F8 needs d (%d) and n (%d) to be multiples of 16", prefix, d, n)
+             : fail(SCE_ERR_INVALID, "%sarith = F16F8 needs d (%d) to be a multiple of 16", prefix, d);
+  if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(shift) % 16)
+    return fail(SCE_ERR_INVALID, "%sx and shift must be 16-byte aligned", prefix);
+  return SCE_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2329,29 +2289,15 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
             : run_similarity_t<kArithBf16x3>(L, A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms);
 }
 
-size_t sce_second_moments_workspace_bytes(int d, int B) {
-  if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
-  return std::max(mom_workspace(false, d, B), mom_workspace(true, d, B));
-}
+size_t sce_second_moments_workspace_bytes(int d, int B) { return row_pass_workspace(d, 0, B); }
 
 int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* shift, int arith, double* col_sum,
                        double* gram, unsigned int* range_flag, void* workspace, size_t workspace_bytes, void* stream) {
   // ---- arguments (all checked before any CUDA call)
-  if (!x || !shift || !col_sum || !gram)
-    return fail(SCE_ERR_INVALID, "second_moments: x, shift, col_sum and gram are required");
-  if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "second_moments: x_is_half must be 0 or 1");
-  if (B < 1 || B > kMomCallRowsMax)
-    return fail(SCE_ERR_INVALID, "second_moments: B = %d outside [1, %d]", B, kMomCallRowsMax);
-  if (d < 8 || d % 8) return fail(SCE_ERR_INVALID, "second_moments: d (%d) must be a positive multiple of 8", d);
-  if (d > 8192) return fail(SCE_ERR_INVALID, "second_moments: d = %d > 8192 is not supported by the row kernels", d);
-  if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "second_moments: unknown arith %d", arith);
-  if (arith == SCE_ARITH_F16F8 && d % 16)
-    return fail(SCE_ERR_INVALID, "second_moments: arith = F16F8 needs d (%d) to be a multiple of 16", d);
-  if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(shift) % 16 ||
-      reinterpret_cast<uintptr_t>(gram) % 16)
-    return fail(SCE_ERR_INVALID, "second_moments: x, shift and gram must be 16-byte aligned");
-  if (int rc = check_workspace(workspace, workspace_bytes, sce_second_moments_workspace_bytes(d, B), "second_moments: "))
-    return rc;
+  if (!col_sum || !gram) return fail(SCE_ERR_INVALID, "second_moments: col_sum and gram are required");
+  TRY(check_row_pass("second_moments: ", x, x_is_half, B, d, shift, 0, arith));
+  if (reinterpret_cast<uintptr_t>(gram) % 16) return fail(SCE_ERR_INVALID, "second_moments: gram must be 16-byte aligned");
+  TRY(check_workspace(workspace, workspace_bytes, sce_second_moments_workspace_bytes(d, B), "second_moments: "));
 
   // ---- device
   int dev = 0, sms = 0;
@@ -2359,36 +2305,29 @@ int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* 
   Launcher L{static_cast<cudaStream_t>(stream)};
   // AUTO: bf16x3, as sce_similarity: the fp32 range, no range check
   const bool f8 = arith == SCE_ARITH_F16F8;
-  MomCarve w;
-  mom_carve(static_cast<uint8_t*>(workspace), f8, d, B, &w);
-  return f8 ? run_moments_t<kArithF16F8>(L, x, x_is_half, B, d, shift, w, col_sum, gram, range_flag, dev, sms)
-            : run_moments_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, w, col_sum, gram, range_flag, dev, sms);
+  const Slices sl = mom_slices(d, B);
+  RowCarve w;
+  row_carve(static_cast<uint8_t*>(workspace), f8, d, 0, sl.S, (size_t)sl.S * sl.R, &w);
+  return f8 ? run_moments_t<kArithF16F8>(L, x, x_is_half, B, d, shift, sl, w, col_sum, gram, range_flag, dev, sms)
+            : run_moments_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, sl, w, col_sum, gram, range_flag, dev, sms);
 }
 
 size_t sce_ica_pass_workspace_bytes(int d, int n, int B) {
-  if (d < 8 || d % 8 || d > 8192 || n < 8 || n % 8 || n > d || B < 1 || B > kMomCallRowsMax) return 0;
-  return std::max(ica_workspace(false, d, n, B), ica_workspace(true, d, n, B));
+  return n < 8 || n % 8 || n > d ? 0 : row_pass_workspace(d, n, B);
 }
 
 int sce_ica_pass(const void* x, int x_is_half, int B, int d, const float* shift, const float* unmix, int n, float alpha,
                  int arith, double* g_sum, double* gx, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
                  void* stream) {
   // ---- arguments (all checked before any CUDA call)
-  if (!x || !shift || !unmix || !g_sum || !gx)
-    return fail(SCE_ERR_INVALID, "ica_pass: x, shift, unmix, g_sum and gx are required");
-  if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "ica_pass: x_is_half must be 0 or 1");
-  if (B < 1 || B > kMomCallRowsMax) return fail(SCE_ERR_INVALID, "ica_pass: B = %d outside [1, %d]", B, kMomCallRowsMax);
-  if (d < 8 || d % 8 || d > 8192) return fail(SCE_ERR_INVALID, "ica_pass: d (%d) must be a multiple of 8 in [8, 8192]", d);
+  if (!unmix || !g_sum || !gx) return fail(SCE_ERR_INVALID, "ica_pass: unmix, g_sum and gx are required");
+  TRY(check_row_pass("ica_pass: ", x, x_is_half, B, d, shift, n, arith));
   if (n < 8 || n % 8 || n > d) return fail(SCE_ERR_INVALID, "ica_pass: n (%d) must be a multiple of 8 in [8, d = %d]", n, d);
   if (!(alpha >= 1.f && alpha <= 2.f)) return fail(SCE_ERR_INVALID, "ica_pass: alpha (%g) must be in [1, 2]", (double)alpha);
-  if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "ica_pass: unknown arith %d", arith);
-  if (arith == SCE_ARITH_F16F8 && (d % 16 || n % 16))
-    return fail(SCE_ERR_INVALID, "ica_pass: arith = F16F8 needs d (%d) and n (%d) to be multiples of 16", d, n);
-  if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(shift) % 16 ||
-      reinterpret_cast<uintptr_t>(unmix) % 16 || reinterpret_cast<uintptr_t>(gx) % 16 ||
+  if (reinterpret_cast<uintptr_t>(unmix) % 16 || reinterpret_cast<uintptr_t>(gx) % 16 ||
       reinterpret_cast<uintptr_t>(g_sum) % 8)
-    return fail(SCE_ERR_INVALID, "ica_pass: x, shift, unmix and gx must be 16-byte aligned, g_sum 8-byte aligned");
-  if (int rc = check_workspace(workspace, workspace_bytes, sce_ica_pass_workspace_bytes(d, n, B), "ica_pass: ")) return rc;
+    return fail(SCE_ERR_INVALID, "ica_pass: unmix and gx must be 16-byte aligned, g_sum 8-byte aligned");
+  TRY(check_workspace(workspace, workspace_bytes, sce_ica_pass_workspace_bytes(d, n, B), "ica_pass: "));
 
   // ---- device
   int dev = 0, sms = 0;
@@ -2396,10 +2335,11 @@ int sce_ica_pass(const void* x, int x_is_half, int B, int d, const float* shift,
   Launcher L{static_cast<cudaStream_t>(stream)};
   // AUTO: bf16x3, as sce_second_moments
   const bool f8 = arith == SCE_ARITH_F16F8;
-  IcaCarve w;
-  ica_carve(static_cast<uint8_t*>(workspace), f8, d, n, B, &w);
-  return f8 ? run_ica_t<kArithF16F8>(L, x, x_is_half, B, d, shift, unmix, n, alpha, w, g_sum, gx, range_flag, dev, sms)
-            : run_ica_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, unmix, n, alpha, w, g_sum, gx, range_flag, dev, sms);
+  const Slices sl = mom_slices(d, B);
+  RowCarve w;
+  row_carve(static_cast<uint8_t*>(workspace), f8, d, n, sl.S, (size_t)sl.S * sl.R, &w);
+  return f8 ? run_ica_t<kArithF16F8>(L, x, x_is_half, B, d, shift, unmix, n, alpha, sl, w, g_sum, gx, range_flag, dev, sms)
+            : run_ica_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, unmix, n, alpha, sl, w, g_sum, gx, range_flag, dev, sms);
 }
 
 int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,

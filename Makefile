@@ -10,10 +10,14 @@ all: $(LIB)
 $(LIB): $(CSRC)/sce_engine.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h include/sce.h
 	$(NVCC) $(NVFLAGS) -shared -o $@ $(CSRC)/sce_engine.cu
 
-selftest: build/gemm_selftest
+selftest: build/gemm_selftest build/gemm_cluster_selftest
 build/gemm_selftest: tests/csrc/gemm_selftest.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
 	mkdir -p build
 	$(NVCC) $(NVFLAGS) -o $@ tests/csrc/gemm_selftest.cu
+
+build/gemm_cluster_selftest: tests/csrc/gemm_cluster_selftest.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
+	mkdir -p build
+	$(NVCC) $(NVFLAGS) -o $@ tests/csrc/gemm_cluster_selftest.cu
 
 probe: build/gemm_overlap_probe
 build/gemm_overlap_probe: tools/gemm_overlap_probe.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
@@ -21,4 +25,4 @@ build/gemm_overlap_probe: tools/gemm_overlap_probe.cu $(CSRC)/*.cuh $(CSRC)/sce_
 	$(NVCC) $(NVFLAGS) -o $@ tools/gemm_overlap_probe.cu
 
 clean:
-	rm -f $(LIB) build/gemm_selftest build/gemm_overlap_probe
+	rm -f $(LIB) build/gemm_selftest build/gemm_cluster_selftest build/gemm_overlap_probe

@@ -23,6 +23,13 @@
 // (q, 1). Where the epilogue does not overlap (gemm_overlap: kInline epilogues, the widened path) the kernel runs 384
 // threads without the epilogue warpgroup, and the eight consumer warps run it in line after the main loop, warp w
 // taking share (w % 4, w / 4). The outputs are the same either way.
+//
+// Where a model's column-tile count is even and the K loop long, the CTAs run in clusters of two along N (launch_gemm,
+// gemm_cluster_size): the pair works on the two columns of one tile row at a time, so both need the same A tile at
+// every K block, and one of them loads it for both with a TMA multicast. That cuts the operand bytes read from L2 per
+// MMA by a quarter (A and B tiles are the same size). Each stage then holds bytes written by both CTAs, so it is free
+// only once the consumers of both have released it. Nothing about the arithmetic, its order or the epilogues depends on
+// the cluster size.
 #pragma once
 #include <type_traits>
 #include "sce_ptx.cuh"
@@ -172,7 +179,10 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
 // K-major, loaded with the 64-byte swizzle): sweep 1 runs E5M2 wgmma on the stage itself; A_MN / B_MN describe the fp16
 // planes only (sweep 2), because E5M2 wgmma reads no layout but K-major. Otherwise (MN-major operands) the 8-bit tiles
 // arrive unswizzled and MN-major, and are widened to fp16 in shared memory first.
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
+//
+// CLUSTER (1 or 2): the CTAs of the launch run in clusters of that many along N, sharing each A tile (see the top of the
+// file). A compile-time value, so that a launch in clusters of one runs the kernel without any of the pairing.
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int CLUSTER>
 __global__ void __launch_bounds__(gemm_threads<Epi, ARITH, F8_NATIVE>(), 1)
 gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
@@ -181,6 +191,8 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   static_assert(!F8_NATIVE || F8, "F8_NATIVE is an f16f8 path");
   static_assert(!F8 || A_MN == B_MN, "f16f8 GEMMs are K-major or MN-major on both sides");
   static_assert(!F8 || F8_NATIVE || (A_MN && B_MN), "the widened f16f8 path is MN-major on both sides");
+  static_assert(CLUSTER == 1 || CLUSTER == 2, "clusters of one or two CTAs");
+  static_assert(CLUSTER == 1 || !F8 || F8_NATIVE, "the widened f16f8 path runs in clusters of one");
   using SM = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>;
   constexpr int BK = SM::kBK;
   constexpr int STAGES = SM::kStages;
@@ -199,6 +211,11 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  // Tile schedule: CTA b runs tiles b, b + gridDim.x, ... The launch groups the CTAs in clusters of CLUSTER consecutive
+  // CTAs, and takes CLUSTER = 2 only where tiles_n is even (launch_gemm_clusters). The two CTAs of a cluster then run
+  // tiles 2 u and 2 u + 1 at every step: the two columns of one model and tile row, with the same operand sets and K
+  // loop, and the same A tile (for kPairTiles epilogues too: the A model is the tile's pair).
+  [[maybe_unused]] const int cta_rank = CLUSTER == 2 ? int(cluster_ctarank()) : 0;
   const int num_tiles = p.n_models * p.tiles_m * p.tiles_n;
   auto decode_tile = [&](int tile, int& model, int& tile_m, int& tile_n) {
     model = tile / (p.tiles_m * p.tiles_n);
@@ -234,7 +251,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[s], 2 * CLUSTER);   // one arrival per consumer warpgroup of each CTA of the cluster
     }
     if constexpr (OVERLAP) {
       mbar_init(acc_full, 256);      // every consumer thread, after its accumulators are in acc_stage
@@ -242,7 +259,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  // in a pair, the barriers of both CTAs are initialised before either multicasts into the other or arrives on its
+  // barriers
+  if constexpr (CLUSTER == 2) cluster_sync();
+  else __syncthreads();
   // f16f8: which cross terms each operand pair needs (see GemmParams::a_res_flag); the same for every CTA of the launch
   [[maybe_unused]] bool term_lh[kMaxSets], term_hl[kMaxSets];
   if constexpr (F8) {
@@ -294,6 +314,13 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
           phase ^= 1;
         }
       };
+      // A tiles. In a cluster of two both CTAs need the same A tile at every K block: the CTA of rank kb % 2 loads it
+      // for both (multicast), so each A tile crosses from L2 once per cluster. B tiles are loaded by each CTA for itself.
+      // Every CTA's full barrier still expects the whole stage.
+      auto load_a = [&](void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int kb) {
+        if constexpr (CLUSTER == 1) tma_load_3d(dst, m, bar, c0, c1, c2);
+        else if ((kb & 1) == cta_rank) tma_load_3d_multicast(dst, m, bar, c0, c1, c2, uint16_t(0x3));
+      };
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int model, tile_m, tile_n;
         decode_tile(tile, model, tile_m, tile_n);
@@ -317,10 +344,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
                 if (sweep == 1) {
                   uint8_t* sa = st;
                   uint8_t* sb = st + SM::kATile;
-                  if constexpr (!A_MN) tma_load_3d(sa, &p.a_hi[set], bar, k0, a_row0, am);
+                  if constexpr (!A_MN) load_a(sa, &p.a_hi[set], bar, k0, a_row0, am, kb);
                   else {
 #pragma unroll
-                    for (int j = 0; j < kBM / 64; ++j) tma_load_3d(sa + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am);
+                    for (int j = 0; j < kBM / 64; ++j) load_a(sa + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am, kb);
                   }
                   if constexpr (!B_MN) tma_load_3d(sb, &p.b_hi[set], bar, k0, b_row0, bm);
                   else {
@@ -336,8 +363,8 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
                   uint8_t* sb_l = sb_h + SM::kBTile / 2;
                   const int ac0 = F8_NATIVE ? k0 : a_row0, ac1 = F8_NATIVE ? a_row0 : k0;
                   const int bc0 = F8_NATIVE ? k0 : b_row0, bc1 = F8_NATIVE ? b_row0 : k0;
-                  if (t_hl) tma_load_3d(sa_h, &p.a_lo[set], bar, ac0, ac1, am);
-                  if (t_lh) tma_load_3d(sa_l, &p.a_x8[set], bar, ac0, ac1, am);
+                  if (t_hl) load_a(sa_h, &p.a_lo[set], bar, ac0, ac1, am, kb);
+                  if (t_lh) load_a(sa_l, &p.a_x8[set], bar, ac0, ac1, am, kb);
                   if (t_lh) tma_load_3d(sb_h, &p.b_lo[set], bar, bc0, bc1, bm);
                   if (t_hl) tma_load_3d(sb_l, &p.b_x8[set], bar, bc0, bc1, bm);
                 }
@@ -358,13 +385,13 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
               mbar_expect_tx(bar, stage_bytes);
               const int k0 = kb * BK;
               if constexpr (!A_MN) {
-                tma_load_3d(sa_hi, &p.a_hi[set], bar, k0, a_row0, am);
-                if (three) tma_load_3d(sa_lo, &p.a_lo[set], bar, k0, a_row0, am);
+                load_a(sa_hi, &p.a_hi[set], bar, k0, a_row0, am, kb);
+                if (three) load_a(sa_lo, &p.a_lo[set], bar, k0, a_row0, am, kb);
               } else {
 #pragma unroll
                 for (int j = 0; j < kBM / 64; ++j) {
-                  tma_load_3d(sa_hi + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am);
-                  if (three) tma_load_3d(sa_lo + j * (BK * 128), &p.a_lo[set], bar, a_row0 + j * 64, k0, am);
+                  load_a(sa_hi + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am, kb);
+                  if (three) load_a(sa_lo + j * (BK * 128), &p.a_lo[set], bar, a_row0 + j * 64, k0, am, kb);
                 }
               }
               if constexpr (!B_MN) {
@@ -412,8 +439,13 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
         phase ^= 1;
       }
     };
+    // A stage is free once the consumers of every CTA of the cluster are done with it: the peer's multicast writes this
+    // CTA's stage as well as its own
     auto release = [&](int s) {
-      if (wl == 0) mbar_arrive(&empty_bar[s]);
+      if (wl == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if constexpr (CLUSTER == 2) mbar_arrive_cluster(&empty_bar[s], uint32_t(cta_rank ^ 1));
+      }
     };
 
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -576,6 +608,8 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       epilogue_share(model, tile_m, tile_n, warp_q, 1, [&] { mbar_arrive(acc_empty); });
     }
   }
+  // no CTA of a pair leaves while its peer may still arrive on its barriers
+  if constexpr (CLUSTER == 2) cluster_sync();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -592,17 +626,98 @@ inline cudaError_t opt_in_smem(int bytes, int device) {
   return e;
 }
 
-// Launches gemm_split_kernel on `st` as a persistent grid: one CTA per tile, at most one per SM (`sms` of them on
-// `device`, the current device).
+// The most clusters of `cluster` CTAs of the kernel KERN that can be resident on `device` at once (0: none), queried
+// once per device and cluster size.
+template <auto KERN>
+inline int max_active_clusters(int cluster, int threads, int bytes, int device) {
+  static int known[64][2] = {};   // [device][cluster - 1]: the count + 1 once queried
+  if (device >= 0 && device < 64 && known[device][cluster - 1]) return known[device][cluster - 1] - 1;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = cluster;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.gridDim = dim3(cluster);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = bytes;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, KERN, &cfg) != cudaSuccess) n = 0;
+  if (device >= 0 && device < 64) known[device][cluster - 1] = n + 1;
+  return n;
+}
+
+// Cluster size of a launch: two CTAs along N, which share each A tile, where a model's column-tile count is even (a
+// column pair never straddles two tile rows) and each tile's K loop runs at least kClusterMinKBlocks K blocks over its
+// operand sets; one otherwise, and on the widened f16f8 path. The pair reads a quarter fewer operand bytes from L2 but
+// runs in lockstep, each stage waiting for both CTAs' consumers. On an H100 at 700 W the main loop alone (config 2
+// shapes) got 13-21 % shorter in pairs at 64 K blocks (decode) and 2 x 64 (the weight gradient), and no shorter at 8
+// (encode, dcode). Only those lengths were measured: where between 8 and 64 blocks pairs start to pay is not known, and
+// 64 is the shortest loop they were seen to pay on.
+constexpr int kClusterMinKBlocks = 64;
+inline int gemm_cluster_size(int tiles_n, int k_blocks, bool widened) {
+  return tiles_n % 2 == 0 && k_blocks >= kClusterMinKBlocks && !widened ? 2 : 1;
+}
+
+// Launches gemm_split_kernel<..., CLUSTER> on `st` as a persistent grid of clusters of CLUSTER CTAs (2 only where
+// p.tiles_n is even): one cluster per column group of CLUSTER tiles, at most as many as are resident at once, and at
+// most one CTA per SM (`sms` of them on `device`, the current device).
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int CLUSTER>
+cudaError_t launch_gemm_cluster_t(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st) {
+  constexpr auto kern = gemm_split_kernel<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, CLUSTER>;
+  constexpr int bytes = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>::kBytes;
+  constexpr int threads = gemm_threads<Epi, ARITH, F8_NATIVE>();
+  if (p.tiles_n % CLUSTER != 0) return cudaErrorInvalidValue;
+  cudaError_t e = opt_in_smem<kern>(bytes, device);
+  if (e != cudaSuccess) return e;
+  long long slots = sms / CLUSTER;
+  if constexpr (CLUSTER > 1) {
+    const int resident = max_active_clusters<kern>(CLUSTER, threads, bytes, device);
+    if (resident <= 0) return cudaErrorInvalidConfiguration;
+    if (resident < slots) slots = resident;
+  }
+  const long long units = (long long)p.n_models * p.tiles_m * (p.tiles_n / CLUSTER);
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = CLUSTER;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.gridDim = dim3((unsigned)(CLUSTER * (units < slots ? units : slots)));
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = bytes;
+  cfg.stream = st;
+  cfg.attrs = &attr;
+  cfg.numAttrs = CLUSTER > 1 ? 1 : 0;
+  e = cudaLaunchKernelEx(&cfg, kern, p);
+  return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+// The same with the cluster size given at run time (1 or 2; always 1 on the widened f16f8 path).
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
+cudaError_t launch_gemm_clusters(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st,
+                                 int cluster) {
+  if (cluster == 1) return launch_gemm_cluster_t<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, 1>(p, device, sms, st);
+  if constexpr (ARITH != kArithF16F8 || F8_NATIVE) {
+    if (cluster == 2) return launch_gemm_cluster_t<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, 2>(p, device, sms, st);
+  }
+  return cudaErrorInvalidValue;
+}
+
+// The cluster size launch_gemm takes for p's shape on this path (gemm_cluster_size).
+template <int ARITH, bool F8_NATIVE, class EpiParams>
+inline int gemm_launch_cluster(const GemmParams<EpiParams>& p) {
+  const int k_blocks = p.nsets * ((p.k_total + gemm_bk(ARITH) - 1) / gemm_bk(ARITH));
+  return gemm_cluster_size(p.tiles_n, k_blocks, ARITH == kArithF16F8 && !F8_NATIVE);
+}
+
+// Launches gemm_split_kernel in the cluster size that p's shape and path take.
 template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
 cudaError_t launch_gemm(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st) {
-  constexpr auto kern = gemm_split_kernel<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE>;
-  constexpr int bytes = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>::kBytes;
-  const cudaError_t e = opt_in_smem<kern>(bytes, device);
-  if (e != cudaSuccess) return e;
-  const long long tiles = (long long)p.n_models * p.tiles_m * p.tiles_n;
-  kern<<<(unsigned)(tiles < sms ? tiles : sms), gemm_threads<Epi, ARITH, F8_NATIVE>(), bytes, st>>>(p);
-  return cudaGetLastError();
+  return launch_gemm_clusters<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE>(p, device, sms, st,
+                                                                            gemm_launch_cluster<ARITH, F8_NATIVE>(p));
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,6 +1,6 @@
 // sce_ptx.cuh — thin inline-PTX wrappers for the sm_90a features the engine uses:
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared memory, accumulators in
-// registers) and the shared-memory matrix descriptors wgmma consumes.
+// mbarrier, thread block clusters, TMA (cp.async.bulk.tensor, multicast included), wgmma (warpgroup MMA from shared
+// memory, accumulators in registers) and the shared-memory matrix descriptors wgmma consumes.
 //
 // Nothing here is specific to sparse autoencoders; sce_gemm.cuh builds the split-operand
 // batched GEMM on top of it.
@@ -77,6 +77,31 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ----------------------------------------------------------------------------------------------
+// thread block clusters
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+  uint32_t n;
+  asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+  return n;
+}
+// Every thread of every CTA of the cluster arrives, then waits for all of them; release / acquire order the shared
+// memory and mbarrier operations before it against those after it, across the cluster. Also a barrier of the CTA.
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// Arrives on the mbarrier at the same shared-memory offset as `bar` in CTA `cta` of the cluster.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
 // TMA: 3-D tiled tensor map load, global -> shared, completion on an mbarrier
 // ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -89,6 +114,18 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "[%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+
+// The same load multicast to the CTAs of the cluster in `cta_mask`: the box lands at the same shared-memory offset in
+// each of them and completes its bytes on the mbarrier at the same offset in each.
+__device__ __forceinline__ void tma_load_3d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
+                                                      int c0, int c1, int c2, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
+      "[%0], [%1, {%3, %4, %5}], [%2], %6;"
+      ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
       : "memory");
 }
 

@@ -4,8 +4,14 @@
 // Each GEMM runs in the configuration libsce launches it in (layouts, operand sets, passes, skipped cross terms,
 // persistent grid), but with an epilogue that does nothing with the accumulators beyond reading them from the staging
 // tile. It declares the staging bytes of the engine's epilogue, so the stage ring is as deep. The time per launch is
-// the main loop alone: the engine's kernel time for the same GEMM minus this one is what its epilogue adds.
-// tools/gemm_overlap_probe.py reads one JSON line per GEMM from stdout. Build: Makefile target `probe`.
+// the main loop alone: the engine's kernel time for the same GEMM minus this one is what its epilogue adds. Each GEMM
+// runs in clusters of each size given on the command line, in that order: 1 (every CTA loads its own A tiles), 2 (two
+// CTAs along N share each A tile by multicast) or 0 (the size launch_gemm takes, as libsce launches it: 2 for decode and
+// the weight gradient, 1 for encode and dcode). Without sizes, 0. Each JSON line names the size run ("cluster") and the
+// size launch_gemm takes ("engine_cluster"). tools/gemm_overlap_probe.py reads them from stdout. Build: Makefile target
+// `probe`.
+//
+//   build/gemm_overlap_probe [reps] [cluster sizes ...]
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -96,7 +102,8 @@ struct Shape {
 };
 
 template <int STAGE_BYTES, bool INLINE, bool MN, bool NATIVE>
-static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32_t* sink, int reps) {
+static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32_t* sink, int reps,
+                const std::vector<int>& clusters) {
   using Epi = EpiNoop<STAGE_BYTES, INLINE>;
   GemmParams<typename Epi::Params> p;
   memset(&p, 0, sizeof(p));
@@ -121,17 +128,26 @@ static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
-  for (int rep = 0; rep < 3; ++rep) CK((launch_gemm<Epi, MN, MN, false, kArithF16F8, NATIVE>(p, 0, sms, 0)));
-  CK(cudaEventRecord(e0));
-  for (int rep = 0; rep < reps; ++rep) CK((launch_gemm<Epi, MN, MN, false, kArithF16F8, NATIVE>(p, 0, sms, 0)));
-  CK(cudaEventRecord(e1));
-  CK(cudaDeviceSynchronize());
-  float ms = 0;
-  CK(cudaEventElapsedTime(&ms, e0, e1));
-  const double flops = 2.0 * models * s.M * s.N * (double)s.K * s.nsets;
-  printf("{\"gemm\": \"%s\", \"main_loop_ms\": %.4f, \"tiles\": %d, \"stages\": %d, \"reps\": %d, \"tflops\": %.1f}\n",
-         s.name, ms / reps, models * p.tiles_m * p.tiles_n,
-         GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE>::kStages, reps, flops / (ms / reps) * 1e-9);
+  const int engine_cluster = gemm_launch_cluster<kArithF16F8, NATIVE>(p);
+  for (int asked : clusters) {
+    const int cluster = asked == 0 ? engine_cluster : asked;
+    auto launch = [&] { return launch_gemm_clusters<Epi, MN, MN, false, kArithF16F8, NATIVE>(p, 0, sms, 0, cluster); };
+    for (int rep = 0; rep < 3; ++rep) CK(launch());
+    CK(cudaEventRecord(e0));
+    for (int rep = 0; rep < reps; ++rep) CK(launch());
+    CK(cudaEventRecord(e1));
+    CK(cudaDeviceSynchronize());
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, e0, e1));
+    const double flops = 2.0 * models * s.M * s.N * (double)s.K * s.nsets;
+    constexpr auto kern2 = gemm_split_kernel<Epi, MN, MN, false, kArithF16F8, NATIVE, 2>;
+    const int resident = cluster == 1 ? sms : max_active_clusters<kern2>(2, gemm_threads<Epi, kArithF16F8, NATIVE>(),
+                                                                         GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE>::kBytes, 0);
+    printf("{\"gemm\": \"%s\", \"cluster\": %d, \"engine_cluster\": %d, \"resident_clusters\": %d, \"main_loop_ms\": "
+           "%.4f, \"tiles\": %d, \"stages\": %d, \"reps\": %d, \"tflops\": %.1f}\n",
+           s.name, cluster, engine_cluster, resident, ms / reps, models * p.tiles_m * p.tiles_n, GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE>::kStages,
+           reps, flops / (ms / reps) * 1e-9);
+  }
   CK(cudaEventDestroy(e0));
   CK(cudaEventDestroy(e1));
   for (void* d : g_dev) cudaFree(d);
@@ -140,6 +156,9 @@ static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32
 
 int main(int argc, char** argv) {
   const int reps = argc > 1 ? atoi(argv[1]) : 20;
+  std::vector<int> clusters;
+  for (int i = 2; i < argc; ++i) clusters.push_back(atoi(argv[i]));
+  if (clusters.empty()) clusters.push_back(0);
   setvbuf(stdout, nullptr, _IOLBF, 0);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, 0));
@@ -149,14 +168,14 @@ int main(int argc, char** argv) {
   CK(cudaMalloc(&sink, 4));
   const int M = 16, d = 512, n = 4096, B = 8192, sms = prop.multiProcessorCount;
   // encode: z = x W_enc^T, x shared and fp16-exact (its cross term skipped); EpiEncodeT stages 4 KB per warp
-  run<4096, false, false, true>({"encode", 1, M, B, n, d, 1, false, true}, M, sms, zero_flag, sink, reps);
+  run<4096, false, false, true>({"encode", 1, M, B, n, d, 1, false, true}, M, sms, zero_flag, sink, reps, clusters);
   // decode: x^ = c W_dec, both operands per model; EpiDecodeT stages nothing and runs in line
-  run<0, true, false, true>({"decode", M, M, B, d, n, 1, false, false}, M, sms, zero_flag, sink, reps);
+  run<0, true, false, true>({"decode", M, M, B, d, n, 1, false, false}, M, sms, zero_flag, sink, reps, clusters);
   // dcode: g W_dec^T; EpiDcodeT stages 4 KB per warp
-  run<4096, false, false, true>({"dcode", M, M, B, n, d, 1, false, false}, M, sms, zero_flag, sink, reps);
+  run<4096, false, false, true>({"dcode", M, M, B, n, d, 1, false, false}, M, sms, zero_flag, sink, reps, clusters);
   // weight gradient: dz^T x + c^T g, reduction over the batch, fp16 planes MN-major, 8-bit ones from batch-major copies;
   // x (set 0's B) fp16-exact; EpiStoreF32 runs in line
-  run<0, true, true, true>({"dw", M, 1, n, d, B, 2, true, false}, M, sms, zero_flag, sink, reps);
+  run<0, true, true, true>({"dw", M, 1, n, d, B, 2, true, false}, M, sms, zero_flag, sink, reps, clusters);
   cudaFree(zero_flag);
   cudaFree(sink);
   return 0;

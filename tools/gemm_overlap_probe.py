@@ -1,4 +1,4 @@
-"""How much of each split-operand GEMM of a config-2 training step is its epilogue.
+"""How much of each split-operand GEMM of a config-2 training step is its epilogue, and what sharing A tiles saves.
 
 Config 2: 16 tied SAEs, d = 512, n = 4096, batch 8192, f16f8 arithmetic, fp16-exact activations (bench.py's cfg2).
 For each of the step's four GEMMs (encode, decode, dcode, weight gradient) it reports
@@ -6,11 +6,14 @@ For each of the step's four GEMMs (encode, decode, dcode, weight gradient) it re
       activities, in a run of its own;
   (b) main_loop_ms: the same kernel configuration at the same shapes with an epilogue that only reads the accumulators
       (build/gemm_overlap_probe, Makefile target `probe`), declaring the engine epilogue's staging bytes so that the
-      stage ring is as deep;
+      stage ring is as deep; once in clusters of one CTA (each loads its own A tiles) and once in clusters of two along
+      N (the pair shares each A tile by TMA multicast, as the engine launches decode and dW), in alternating order;
   (c) the card's name, power limit and SM clock, read in the same run after each measurement.
-(a) and (b) are taken in alternated rounds and their medians reported with the range. (a) - (b) is the time the
-epilogue adds to the kernel; the two run on different operands (the engine's training data, hashed finite values),
-which alone can move (b) against (a). Prints a table and one JSON line; --out DIR
+(a) and (b) are taken in alternated rounds and their medians reported with the range. (a) minus (b) at the cluster
+size the engine launches the GEMM in (2 for decode and dW, 1 for encode and dcode; the probe reports it) is the time
+the epilogue adds; (b) at cluster 2 over (b) at cluster 1 is what a 25 % cut of the main loop's L2 operand reads buys.
+(a) and (b) run on different operands (the engine's training data, hashed finite values), which alone can move (b)
+against (a). Prints a table and one JSON line; --out DIR
 also writes it there.
 
     python tools/gemm_overlap_probe.py [--steps 20] [--reps 20] [--rounds 5] [--out DIR]
@@ -74,12 +77,16 @@ class EngineRun:
         return {g: (t / c if c else None, c / self.steps) for g, (t, c) in sums.items()}
 
 
-def main_loop_times(reps):
+CLUSTERS = (1, 2)
+
+
+def main_loop_times(reps, clusters):
     exe = os.path.join(ROOT, "build", "gemm_overlap_probe")
     if not os.path.exists(exe):
         raise SystemExit(f"{exe} is missing: run `make probe` first")
-    out = subprocess.run([exe, str(reps)], capture_output=True, text=True, check=True).stdout
-    return {r["gemm"]: r for r in (json.loads(l) for l in out.splitlines() if l.startswith("{"))}
+    out = subprocess.run([exe, str(reps)] + [str(c) for c in clusters], capture_output=True, text=True,
+                         check=True).stdout
+    return {(r["gemm"], r["cluster"]): r for r in (json.loads(l) for l in out.splitlines() if l.startswith("{"))}
 
 
 def fmt(v, width):
@@ -98,10 +105,10 @@ def main():
     info = card()
     run = EngineRun(args.steps)
     rounds = []
-    for _ in range(args.rounds):
+    for i in range(args.rounds):
         eng = run.times()
         clock_a = card()["clocks.sm"]
-        ml = main_loop_times(args.reps)
+        ml = main_loop_times(args.reps, CLUSTERS if i % 2 == 0 else CLUSTERS[::-1])
         clock_b = card()["clocks.sm"]
         rounds.append({"engine": eng, "main_loop": ml, "clock_after_engine": clock_a, "clock_after_main_loop": clock_b})
 
@@ -113,22 +120,27 @@ def main():
           f"after each round's (a) and (b): " + ", ".join(f"{r['clock_after_engine']} / {r['clock_after_main_loop']}"
                                                            for r in rounds))
     print(f"medians of {args.rounds} rounds (min-max in brackets)")
-    print(f"{'gemm':8s} {'launches/step':>13s} {'engine ms':>10s} {'':15s} {'main loop ms':>13s} {'':15s} "
-          f"{'epilogue ms':>12s}")
+    print(f"{'gemm':8s} {'launches/step':>13s} {'engine ms':>10s} {'':15s} {'main loop ms, cluster 1':>24s} {'':15s} "
+          f"{'cluster 2':>10s} {'':15s} {'c2 / c1':>8s} {'epilogue ms':>12s}  (against the main loop at the engine's cluster size)")
     rows = []
     for _, g in EPILOGUES:
         a = [r["engine"][g][0] for r in rounds]
-        b = [r["main_loop"][g]["main_loop_ms"] for r in rounds]
+        b = {c: [r["main_loop"][(g, c)]["main_loop_ms"] for r in rounds] for c in CLUSTERS}
         per_step = rounds[0]["engine"][g][1]
-        ma, mb = med(a), med(b)
+        ma, mb1, mb2 = med(a), med(b[1]), med(b[2])
+        ec = rounds[0]["main_loop"][(g, 1)]["engine_cluster"]   # the cluster size the engine launches this GEMM in
+        mbe = mb2 if ec == 2 else mb1
         av = [x for x in a if x is not None]
-        rows.append({"gemm": g, "launches_per_step": per_step, "engine_ms": ma, "main_loop_ms": mb,
-                     "engine_ms_rounds": a, "main_loop_ms_rounds": b,
-                     "epilogue_ms": None if ma is None else ma - mb, "stages": rounds[0]["main_loop"][g]["stages"],
-                     "tiles": rounds[0]["main_loop"][g]["tiles"]})
+        rows.append({"gemm": g, "launches_per_step": per_step, "engine_cluster": ec, "engine_ms": ma,
+                     "main_loop_ms": mbe, "main_loop_ms_rounds": b[ec], "main_loop_ms_cluster1": mb1,
+                     "main_loop_ms_cluster2": mb2, "main_loop_ms_cluster1_rounds": b[1],
+                     "main_loop_ms_cluster2_rounds": b[2], "engine_ms_rounds": a,
+                     "epilogue_ms": None if ma is None else ma - mbe,
+                     "stages": rounds[0]["main_loop"][(g, 1)]["stages"], "tiles": rounds[0]["main_loop"][(g, 1)]["tiles"]})
         ra = f"[{min(av):.3f}-{max(av):.3f}]" if av else ""
-        print(f"{g:8s} {per_step:13.1f} {fmt(ma, 10)} {ra:15s} {mb:13.3f} {f'[{min(b):.3f}-{max(b):.3f}]':15s} "
-              f"{fmt(None if ma is None else ma - mb, 12)}")
+        r1, r2 = f"[{min(b[1]):.3f}-{max(b[1]):.3f}]", f"[{min(b[2]):.3f}-{max(b[2]):.3f}]"
+        print(f"{g:8s} {per_step:13.1f} {fmt(ma, 10)} {ra:15s} {mb1:24.3f} {r1:15s} {mb2:10.3f} {r2:15s} "
+              f"{mb2 / mb1:8.3f} {fmt(None if ma is None else ma - mbe, 12)}")
     res = {"card": info, "rounds": [{k: v for k, v in r.items() if k.startswith("clock")} for r in rounds], "gemms": rows}
     line = json.dumps(res)
     print(line)

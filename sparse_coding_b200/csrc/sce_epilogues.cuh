@@ -53,25 +53,40 @@ __device__ __forceinline__ void stage_row32_u8(uint8_t* tile, int lane, const ui
     *reinterpret_cast<uint4*>(tile + lane * 32 + ((q ^ sw) << 4)) = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
 }
 // 8-bit plane tile TRANSPOSED: 32 columns x 32 rows, 32-byte rows, no swizzle. The lane's row becomes byte `lane` of
-// each of the 32 tile rows (one byte store per column: the 32 lanes fill 32 consecutive bytes, conflict-free).
+// each of the 32 tile rows. A lane holds one row of each 4 x 4 byte block (4 columns of the 4 rows of its lane quad), so
+// the blocks are transposed across the quad in two exchanges: lanes 2 apart swap byte pairs, then lanes 1 apart single
+// bytes, the halves of two words per shuffle. Lane 4 a + s then holds bytes 4 a .. + 3 of the tile rows 4 w + s and
+// writes them as words; the 32 lanes of each store hit 32 different banks.
 __device__ __forceinline__ void stage_col32_u8(uint8_t* tile, int lane, const uint32_t* w /*[8]*/) {
+  const bool h = lane & 2, l = lane & 1;
+  // PRMT selectors of this lane's place in its quad: what it sends, and how it joins what it keeps with what it receives
+  const uint32_t s1_send = h ? 0x5410 : 0x7632, s1_lo = h ? 0x3254 : 0x5410, s1_hi = h ? 0x3276 : 0x7610;
+  const uint32_t s2_send = l ? 0x6420 : 0x7531, s2_lo = l ? 0x3514 : 0x5240, s2_hi = l ? 0x3716 : 0x7260;
+  uint32_t* out = reinterpret_cast<uint32_t*>(tile) + (lane & 3) * 8 + (lane >> 2);
 #pragma unroll
-  for (int j = 0; j < 32; ++j) tile[j * 32 + lane] = uint8_t(w[j >> 2] >> (8 * (j & 3)));
+  for (int q = 0; q < 4; ++q) {   // words 2 q and 2 q + 1: tile rows 8 q + s and 8 q + 4 + s
+    const uint32_t x0 = w[2 * q], x1 = w[2 * q + 1];
+    uint32_t t = __shfl_xor_sync(0xffffffffu, __byte_perm(x0, x1, s1_send), 2);
+    const uint32_t z0 = __byte_perm(x0, t, s1_lo), z1 = __byte_perm(x1, t, s1_hi);
+    t = __shfl_xor_sync(0xffffffffu, __byte_perm(z0, z1, s2_send), 1);
+    out[(2 * q) * 32] = __byte_perm(z0, t, s2_lo);
+    out[(2 * q + 1) * 32] = __byte_perm(z1, t, s2_hi);
+  }
 }
-// whole warp: wait until the previous tiles have been read out, write the new ones, launch their stores.
+// whole warp: wait until the share's staging tiles may be written (staging_wait), write them, launch their stores.
 // bf16x3: whi / wx are the hi / lo planes. f16f8: whi is the fp16 plane, wx[0..7] the value-e5m2 plane and
 // wx[8..15] the residual-e5m2 plane (maps m_lo / m_x8).
 // `planes`: which of the f16f8 8-bit planes a consumer will read (bit 0: value plane, bit 1: residual plane); planes
 // nobody reads are neither staged nor stored (warp-uniform). bf16x3 always writes both of its planes.
 // T8 (f16f8): the 8-bit planes go to batch-major copies [model][col][row] (maps m_lo / m_x8 of box 32 rows x 32 bytes).
 template <int ARITH, bool T8 = false>
-__device__ __forceinline__ void stage_and_store(uint8_t* stage, int lane, const uint32_t (&whi)[16],
+__device__ __forceinline__ void stage_and_store(uint8_t* stage, const TileCoord& t, const uint32_t (&whi)[16],
                                                 const uint32_t (&wx)[16], const CUtensorMap* m_hi,
                                                 const CUtensorMap* m_lo, const CUtensorMap* m_x8, int col, int row0,
                                                 int model, int planes = 3) {
   static_assert(!T8 || ARITH == kArithF16F8, "transposed 8-bit planes are f16f8 only");
-  if (lane == 0) tma_store_wait_read();
-  __syncwarp();
+  const int lane = t.lane;
+  staging_wait(t);
   stage_row32(stage, lane, whi);
   if constexpr (T8) {
     if (planes & 1) stage_col32_u8(stage + 2048, lane, &wx[0]);
@@ -148,19 +163,27 @@ struct ActMask {
   }
 };
 
-// transpose-reduce: 32 lanes x 32 columns -> lane j holds the sum of column j over the warp's rows (31 shuffles)
-__device__ __forceinline__ float warp_column_sum(float (&v)[32], int lane) {
+// transpose-reduce: 32 lanes x 32 columns -> lane j holds op over the warp's rows of column j (31 shuffles). The inner
+// loop runs a fixed 16 steps and skips those at or beyond `half`: with a trip count of `half` it is not unrolled before
+// the outer loop, and v, indexed at run time, would live in local memory.
+template <class T, class Op>
+__device__ __forceinline__ T warp_column_reduce(T (&v)[32], int lane, Op op) {
 #pragma unroll
   for (int half = 16; half >= 1; half >>= 1) {
     const bool upper = (lane & half) != 0;
 #pragma unroll
-    for (int i = 0; i < half; ++i) {
-      const float send = upper ? v[i] : v[i + half];
-      const float keep = upper ? v[i + half] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
+    for (int i = 0; i < 16; ++i) {
+      if (i < half) {
+        const T send = upper ? v[i] : v[i + half];
+        const T keep = upper ? v[i + half] : v[i];
+        v[i] = op(keep, __shfl_xor_sync(0xffffffffu, send, half));
+      }
     }
   }
   return v[0];
+}
+__device__ __forceinline__ float warp_column_sum(float (&v)[32], int lane) {
+  return warp_column_reduce(v, lane, [](float a, float b) { return a + b; });
 }
 
 // the same for W < 32 columns: lanes j, j + W, j + 2W, ... all end with the sum of column j over the warp's rows
@@ -292,7 +315,7 @@ struct EpiEncodeT {
       P.act.pos[w] = pos;
       if (P.act.zero) P.act.zero[w] = zero;
     }
-    stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, T.m_blk * kBM + T.warp_q * 32,
+    stage_and_store<ARITH>(stage, T, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, T.m_blk * kBM + T.warp_q * 32,
                            T.model);
     if constexpr (STATS) {
       if (T.m_blk * kBM + T.warp_q * 32 < m_total) {   // warp-uniform: some row of this warp is in the batch
@@ -520,22 +543,12 @@ struct EpiDcodeT {
         split_pair<ARITH>(v0, v1, j >> 1, whi, wlo);
       }
     }
-    stage_and_store<ARITH, T8>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
+    stage_and_store<ARITH, T8>(stage, T, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col,
                                T.m_blk * kBM + T.warp_q * 32, T.model, planes);
     if (P.db_part && T.m_blk * kBM < m_total) {  // warp-uniform
-      // transpose-reduce: 32 lanes x 32 columns -> lane j holds the sum of column j (31 shuffles)
-#pragma unroll
-      for (int half = 16; half >= 1; half >>= 1) {
-        const bool upper = (T.lane & half) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-          const float send = upper ? dz[i] : dz[i + half];
-          const float keep = upper ? dz[i + half] : dz[i];
-          dz[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-        }
-      }
+      const float s = warp_column_sum(dz, T.lane);   // lane j: the sum of column j over the warp's rows
       if (col + T.lane < n_total)
-        P.db_part[(((long long)T.model * P.tiles_m + T.m_blk) * 4 + T.warp_q) * n_total + col + T.lane] = dz[0];
+        P.db_part[(((long long)T.model * P.tiles_m + T.m_blk) * 4 + T.warp_q) * n_total + col + T.lane] = s;
     }
   }
   __device__ __forceinline__ void finish() {
@@ -570,8 +583,7 @@ struct EpiScoresTma {
   __device__ __forceinline__ void chunk(int c, const uint32_t (&r)[32]) {
     const int col = T.col0 + c;
     if (col >= n_total) return;   // warp-uniform
-    if (T.lane == 0) tma_store_wait_read();
-    __syncwarp();
+    staging_wait(T);
     const int sw = T.lane & 7;
 #pragma unroll
     for (int q = 0; q < 8; ++q)
@@ -695,18 +707,9 @@ struct EpiSimilarity {
       }
     }
     if (P.col_max && T.m_blk * kBM + T.warp_q * 32 < ra) {   // warp-uniform: some row of this warp is valid
-      // transpose-reduce: 32 lanes x 32 columns -> lane j holds the maximum of column j over the warp's rows
-#pragma unroll
-      for (int half = 16; half >= 1; half >>= 1) {
-        const bool upper = (T.lane & half) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-          const uint32_t send = upper ? ck[i] : ck[i + half];
-          const uint32_t keep = upper ? ck[i + half] : ck[i];
-          ck[i] = max(keep, __shfl_xor_sync(0xffffffffu, send, half));
-        }
-      }
-      if (T.lane < valid) atomicMax(P.col_max + (long long)T.model * n_total + col + T.lane, ck[0]);
+      // lane j: the maximum of column j over the warp's rows
+      const uint32_t m = warp_column_reduce(ck, T.lane, [](uint32_t a, uint32_t b) { return max(a, b); });
+      if (T.lane < valid) atomicMax(P.col_max + (long long)T.model * n_total + col + T.lane, m);
     }
   }
   __device__ __forceinline__ void finish() {
@@ -755,7 +758,7 @@ struct EpiIcaT {
       g[j + 1] = row_ok ? P.alpha * (1.f - t1 * t1) : 0.f;
     }
     const int row0 = T.m_blk * kBM + T.warp_q * 32;
-    stage_and_store<ARITH>(stage, T.lane, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, row0, T.model);
+    stage_and_store<ARITH>(stage, T, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, row0, T.model);
     if (row0 < P.rows_valid) {   // warp-uniform: some row of this warp is in the batch
       const float s = warp_column_sum(g, T.lane);
       if (col + T.lane < n_total) P.g_part[(long long)(row0 >> 5) * n_total + col + T.lane] = s;

@@ -19,10 +19,10 @@
 // (acc_stage) and arrive on the mbarrier acc_full; the epilogue warpgroup reads the tile, arrives on acc_empty, and
 // runs the epilogue while the consumers run the next tile's main loop (they wait on acc_empty only before writing
 // acc_stage again). Each epilogue thread owns one output row and 32 consecutive columns. A tile's epilogue has eight
-// shares (q, g): rows 32 q .. +31 and the 32-column chunks with chunk % 2 == g; epilogue warp q runs (q, 0), then
-// (q, 1). Where the epilogue does not overlap (gemm_overlap: kInline epilogues, the widened path) the kernel runs 384
-// threads without the epilogue warpgroup, and the eight consumer warps run it in line after the main loop, warp w
-// taking share (w % 4, w / 4). The outputs are the same either way.
+// shares (q, g): rows 32 q .. +31 and the 32-column chunks with chunk % 2 == g; epilogue warp q runs (q, 0) and (q, 1)
+// chunk by chunk, alternating between their staging tiles. Where the epilogue does not overlap (gemm_overlap: kInline
+// epilogues, the widened path) the kernel runs 384 threads without the epilogue warpgroup, and the eight consumer warps
+// run it in line after the main loop, warp w taking share (w % 4, w / 4). The outputs are the same either way.
 //
 // Where a model's column-tile count is even and the K loop long, the CTAs run in clusters of two along N (launch_gemm,
 // gemm_cluster_size): the pair works on the two columns of one tile row at a time, so both need the same A tile at
@@ -57,7 +57,22 @@ struct TileCoord {
   int warp_q;   // epilogue warp quarter 0..3 (rows 32*warp_q .. +31 of the tile)
   int grp;      // epilogue warp group 0..1 (handles the 32-column chunks with chunk % 2 == grp)
   int lane;
+  // The warp runs this share chunk by chunk alternately with its other share (the epilogue warpgroup), so the bulk
+  // store issued just before a chunk read the other share's staging tile, not this one's.
+  bool alternate;
 };
+
+// Whole warp, before a chunk writes its share's staging tile: wait until the bulk stores that read that tile are done
+// with it. Where the warp alternates between two shares' tiles, the most recent store may still be reading the other.
+// Each share's last chunk is followed by its epilogue's finish(), which waits for every store (the staging tiles must
+// outlive them), so the next tile's first chunk never meets a store of this tile.
+__device__ __forceinline__ void staging_wait(const TileCoord& t) {
+  if (t.lane == 0) {
+    if (t.alternate) tma_store_wait_read<1>();
+    else tma_store_wait_read<0>();
+  }
+  __syncwarp();
+}
 
 template <class EpiParams>
 struct GemmParams {
@@ -200,9 +215,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   static_assert(EC == 32, "epilogue chunk is 32 columns");
   constexpr bool OVERLAP = gemm_overlap<Epi, ARITH, F8_NATIVE>();
 
+  // Aligned by an offset from smem_raw, not by a round trip through an integer: a pointer derived from smem_raw stays
+  // in the shared address space, so every access through it compiles to LDS / STS, not to generic LD / ST.
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + SM::kBarOff);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* acc_full = empty_bar + STAGES;   // OVERLAP: acc_stage holds a tile for the epilogue warpgroup
@@ -263,19 +279,20 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   // barriers
   if constexpr (CLUSTER == 2) cluster_sync();
   else __syncthreads();
-  // f16f8: which cross terms each operand pair needs (see GemmParams::a_res_flag); the same for every CTA of the launch
-  [[maybe_unused]] bool term_lh[kMaxSets], term_hl[kMaxSets];
+  // f16f8: which cross terms each operand pair needs (see GemmParams::a_res_flag), bit s for operand pair s; the same
+  // for every CTA of the launch. Bit masks, not arrays: an array indexed by the run-time pair would live in local memory.
+  [[maybe_unused]] uint32_t term_lh = 0u, term_hl = 0u;
   if constexpr (F8) {
 #pragma unroll
     for (int s = 0; s < kMaxSets; ++s) {
-      term_lh[s] = s < p.nsets && (p.a_res_flag[s] == nullptr || __ldg(p.a_res_flag[s]) != 0u);
-      term_hl[s] = s < p.nsets && (p.b_res_flag[s] == nullptr || __ldg(p.b_res_flag[s]) != 0u);
+      term_lh |= uint32_t(s < p.nsets && (p.a_res_flag[s] == nullptr || __ldg(p.a_res_flag[s]) != 0u)) << s;
+      term_hl |= uint32_t(s < p.nsets && (p.b_res_flag[s] == nullptr || __ldg(p.b_res_flag[s]) != 0u)) << s;
     }
   }
 
-  // One epilogue warp's share of the tile in acc_stage: rows 32 warp_q .. +31 and the 32-column chunks grp, grp + 2.
-  // `read_done` runs once the warp has read the last accumulators of its share.
-  auto epilogue_share = [&](int model, int tile_m, int tile_n, int warp_q, int grp, auto read_done) {
+  // One epilogue share (warp_q, grp) of the tile in acc_stage: rows 32 warp_q .. +31 and the 32-column chunks grp,
+  // grp + 2, ... (column group g takes the chunks g, g + 2, ...), with its own epilogue object and staging tile.
+  auto share_coord = [&](int model, int tile_m, int tile_n, int warp_q, int grp, bool alternate) {
     TileCoord tc;
     tc.model = model;
     tc.m_blk = tile_m;
@@ -285,20 +302,17 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     tc.grp = grp;
     tc.lane = lane;
     tc.row = tc.m_blk * kBM + tc.warp_q * 32 + lane;
-    Epi epi(p.epi, tc, p.m_total, p.n_total, smem + SM::kEpiOff + (tc.grp * 4 + tc.warp_q) * Epi::kWarpStageBytes);
-    const float* my_row = acc_stage + (tc.warp_q * 32 + lane) * SM::kAccLd;
-    constexpr int kChunks = BN / EC;
-    static_assert(kChunks % 2 == 0, "the two column groups alternate chunks");
-#pragma unroll 1
-    for (int it = 0; it < kChunks / 2; ++it) {
-      const int c = tc.grp + 2 * it;   // column group g takes the chunks g, g + 2, ...
-      uint32_t r[EC];
+    tc.alternate = alternate;
+    return tc;
+  };
+  auto share_staging = [&](int warp_q, int grp) { return smem + SM::kEpiOff + (grp * 4 + warp_q) * Epi::kWarpStageBytes; };
+  constexpr int kChunks = BN / EC;
+  static_assert(kChunks % 2 == 0, "the two column groups alternate chunks");
+  // chunk c of this thread's row of acc_stage
+  auto read_chunk = [&](int warp_q, int c, uint32_t (&r)[EC]) {
+    const float* src = acc_stage + (warp_q * 32 + lane) * SM::kAccLd + c * EC;
 #pragma unroll
-      for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(my_row[c * EC + j]);
-      if (it == kChunks / 2 - 1) read_done();
-      epi.chunk(c * EC, r);
-    }
-    epi.finish();
+    for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(src[j]);
   };
 
   if (warp < 4) {
@@ -332,7 +346,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
               int am, bm;
               operand_models(model, set, am, bm);
               // cross terms of this operand pair: t_lh = A.l8 x B.h8 (needs A's residual), t_hl = A.h8 x B.l8
-              const bool t_lh = term_lh[set], t_hl = term_hl[set];
+              const bool t_lh = (term_lh >> set) & 1u, t_hl = (term_hl >> set) & 1u;
               if (sweep == 0 && !t_lh && !t_hl) continue;
               const uint32_t bytes = sweep == 1 ? stage_bytes : (uint32_t(t_lh) + uint32_t(t_hl)) * (stage_bytes / 2);
               for (int kb = 0; kb < kblocks; ++kb) {
@@ -514,9 +528,10 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
         };
         if (three) {
           for (int set = 0; set < p.nsets; ++set) {
-            if (term_lh[set] && term_hl[set]) cross_sweep(std::true_type{}, std::true_type{});
-            else if (term_lh[set]) cross_sweep(std::true_type{}, std::false_type{});
-            else if (term_hl[set]) cross_sweep(std::false_type{}, std::true_type{});
+            const bool t_lh = (term_lh >> set) & 1u, t_hl = (term_hl >> set) & 1u;
+            if (t_lh && t_hl) cross_sweep(std::true_type{}, std::true_type{});
+            else if (t_lh) cross_sweep(std::true_type{}, std::false_type{});
+            else if (t_hl) cross_sweep(std::false_type{}, std::true_type{});
           }
           constexpr float kDown = 1.0f / float(1 << kLoShift);
 #pragma unroll
@@ -588,14 +603,24 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       } else {
         // ======================= epilogue in line: eight warps, warp w plays (w % 4, w / 4) =======================
         consumer_sync();
-        const int cw = ctid >> 5;
-        epilogue_share(model, tile_m, tile_n, cw & 3, cw >> 2, [] {});
+        const int cw = ctid >> 5, warp_q = cw & 3, grp = cw >> 2;
+        const TileCoord tc = share_coord(model, tile_m, tile_n, warp_q, grp, false);
+        Epi epi(p.epi, tc, p.m_total, p.n_total, share_staging(warp_q, grp));
+#pragma unroll 1
+        for (int c = grp; c < kChunks; c += 2) {
+          uint32_t r[EC];
+          read_chunk(warp_q, c, r);
+          epi.chunk(c * EC, r);
+        }
+        epi.finish();
       }
     }
   } else if constexpr (OVERLAP) {
     // ======================= epilogue warpgroup =======================
-    // Warp q plays both of the in-line epilogue's warps (q, 0) and (q, 1) in turn: each share's sums, partial-sum slots
-    // and staging are those of the in-line mapping, so the outputs do not depend on which warps run them.
+    // Warp q plays both of the in-line epilogue's warps (q, 0) and (q, 1), chunk by chunk: chunks 0, 2, ... go to share
+    // (q, 0) and chunks 1, 3, ... to share (q, 1). Each share's sums, partial-sum slots, staging and chunk order are
+    // those of the in-line mapping, so the outputs do not depend on which warps run them. Consecutive chunks write
+    // different staging tiles, so a chunk does not wait for the bulk store issued just before it (staging_wait).
     reg_alloc<kEpilogueRegs>();
     const int warp_q = warp - 12;
     uint32_t acc_phase = 0;
@@ -604,8 +629,21 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       decode_tile(tile, model, tile_m, tile_n);
       mbar_wait(acc_full, acc_phase);
       acc_phase ^= 1;
-      epilogue_share(model, tile_m, tile_n, warp_q, 0, [] {});
-      epilogue_share(model, tile_m, tile_n, warp_q, 1, [&] { mbar_arrive(acc_empty); });
+      const TileCoord tc0 = share_coord(model, tile_m, tile_n, warp_q, 0, true);
+      const TileCoord tc1 = share_coord(model, tile_m, tile_n, warp_q, 1, true);
+      Epi epi0(p.epi, tc0, p.m_total, p.n_total, share_staging(warp_q, 0));
+      Epi epi1(p.epi, tc1, p.m_total, p.n_total, share_staging(warp_q, 1));
+#pragma unroll 1
+      for (int c = 0; c < kChunks; c += 2) {
+        uint32_t r[EC];
+        read_chunk(warp_q, c, r);
+        epi0.chunk(c * EC, r);
+        read_chunk(warp_q, c + 1, r);
+        if (c + 2 == kChunks) mbar_arrive(acc_empty);   // the warp's last read of acc_stage for this tile
+        epi1.chunk((c + 1) * EC, r);
+      }
+      epi0.finish();
+      epi1.finish();
     }
   }
   // no CTA of a pair leaves while its peer may still arrive on its barriers

@@ -138,9 +138,11 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* s
                : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all committed bulk stores of this thread have finished READING shared memory (it may be rewritten)
+// all committed bulk stores of this thread but the N most recent have finished READING shared memory (it may be
+// rewritten)
+template <int N = 0>
 __device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------

@@ -8,13 +8,15 @@ For each of the step's four GEMMs (encode, decode, dcode, weight gradient) it re
       (build/gemm_overlap_probe, Makefile target `probe`), declaring the engine epilogue's staging bytes so that the
       stage ring is as deep; once in clusters of one CTA (each loads its own A tiles) and once in clusters of two along
       N (the pair shares each A tile by TMA multicast, as the engine launches decode and dW), in alternating order;
-  (c) the card's name, power limit and SM clock, read in the same run after each measurement.
-(a) and (b) are taken in alternated rounds and their medians reported with the range. (a) minus (b) at the cluster
-size the engine launches the GEMM in (2 for decode and dW, 1 for encode and dcode; the probe reports it) is the time
-the epilogue adds; (b) at cluster 2 over (b) at cluster 1 is what a 25 % cut of the main loop's L2 operand reads buys.
-(a) and (b) run on different operands (the engine's training data, hashed finite values), which alone can move (b)
-against (a). Prints a table and one JSON line; --out DIR
-also writes it there.
+  (c) epilogue_bound_ms, encode and dcode only: the engine's kernel time for the same GEMM, measured as (a), at the same
+      M, n and B but d = 64. Their K loop is then a single K block, so the time is bounded by the epilogue's per-tile
+      throughput: where (c) is below (b), the epilogue keeps pace with the main loop at d = 512;
+and the card's name, power limit and SM clock, read in the same run after each measurement.
+(a), (b) and (c) are taken in alternated rounds and their medians reported with the range. (a) minus (b) at the
+cluster size the engine launches the GEMM in (2 for decode and dW, 1 for encode and dcode; the probe reports it) is the
+time the epilogue adds; (b) at cluster 2 over (b) at cluster 1 is what a 25 % cut of the main loop's L2 operand reads
+buys. (a) and (b) run on different operands (the engine's training data, hashed finite values), which alone can move
+(b) against (a). Prints a table and one JSON line; --out DIR also writes it there.
 
     python tools/gemm_overlap_probe.py [--steps 20] [--reps 20] [--rounds 5] [--out DIR]
 """
@@ -41,14 +43,16 @@ def card():
 
 
 class EngineRun:
-    """A config-2 ensemble, warmed up; `times()` profiles `steps` training steps and returns the mean device time of
-    each GEMM launch of a step by epilogue (None where no launch of that epilogue was seen) and its launches per step."""
+    """A config-2 ensemble (at input dimension `d`, config 2's 512 by default), warmed up; `times()` profiles `steps`
+    training steps and returns the mean device time of each GEMM launch of a step by epilogue (None where no launch of
+    that epilogue was seen) and its launches per step."""
 
-    def __init__(self, steps):
+    def __init__(self, steps, d=None):
         import bench
         import sparse_coding_b200 as S
 
-        M, d, n, B, _ = bench.WORKLOADS["cfg2"]
+        M, d512, n, B, _ = bench.WORKLOADS["cfg2"]
+        d = d or d512
         dev = torch.device("cuda", 0)
         sig = S.FunctionalTiedSAE
         self.ens = S.FunctionalEnsemble(bench.make_models(sig, M, d, n, seed=0), sig, S.adam, {"lr": 1e-3}, device=dev)
@@ -57,6 +61,7 @@ class EngineRun:
         for i in range(5):
             self.ens.step_batch(self.pool[i % len(self.pool)])
         torch.cuda.synchronize()
+        self.arith = self.ens.resolved_arith()
 
     def times(self):
         from torch.profiler import ProfilerActivity, profile
@@ -78,6 +83,8 @@ class EngineRun:
 
 
 CLUSTERS = (1, 2)
+EPILOGUE_BOUND_D = 64                 # input dimension of (c): one K block of the encode and dcode GEMMs
+EPILOGUE_BOUND = ("encode", "dcode")  # the GEMMs (c) is reported for
 
 
 def main_loop_times(reps, clusters):
@@ -104,24 +111,32 @@ def main():
         raise SystemExit("the probe times kernels on cuda:0 and needs a GPU")
     info = card()
     run = EngineRun(args.steps)
+    run_c = EngineRun(args.steps, d=EPILOGUE_BOUND_D)
+    if run_c.arith != run.arith:
+        raise SystemExit(f"d = {EPILOGUE_BOUND_D} runs {run_c.arith}, d = 512 {run.arith}: (c) would time another kernel")
     rounds = []
     for i in range(args.rounds):
         eng = run.times()
         clock_a = card()["clocks.sm"]
         ml = main_loop_times(args.reps, CLUSTERS if i % 2 == 0 else CLUSTERS[::-1])
         clock_b = card()["clocks.sm"]
-        rounds.append({"engine": eng, "main_loop": ml, "clock_after_engine": clock_a, "clock_after_main_loop": clock_b})
+        eb = run_c.times()
+        clock_c = card()["clocks.sm"]
+        rounds.append({"engine": eng, "main_loop": ml, "epilogue_bound": eb, "clock_after_engine": clock_a,
+                       "clock_after_main_loop": clock_b, "clock_after_epilogue_bound": clock_c})
 
     def med(v):
         v = sorted(x for x in v if x is not None)
         return v[len(v) // 2] if v else None
 
     print(f"{info['name']}, power limit {info['power.limit']}, max SM clock {info['clocks.max.sm']}; SM clock read "
-          f"after each round's (a) and (b): " + ", ".join(f"{r['clock_after_engine']} / {r['clock_after_main_loop']}"
-                                                           for r in rounds))
+          f"after each round's (a), (b) and (c): "
+          + ", ".join(f"{r['clock_after_engine']} / {r['clock_after_main_loop']} / {r['clock_after_epilogue_bound']}"
+                      for r in rounds))
     print(f"medians of {args.rounds} rounds (min-max in brackets)")
     print(f"{'gemm':8s} {'launches/step':>13s} {'engine ms':>10s} {'':15s} {'main loop ms, cluster 1':>24s} {'':15s} "
-          f"{'cluster 2':>10s} {'':15s} {'c2 / c1':>8s} {'epilogue ms':>12s}  (against the main loop at the engine's cluster size)")
+          f"{'cluster 2':>10s} {'':15s} {'c2 / c1':>8s} {'epilogue ms':>12s} {'d=64 ms':>8s} {'':15s}"
+          f"  (epilogue: (a) against the main loop at the engine's cluster size; d=64: (c))")
     rows = []
     for _, g in EPILOGUES:
         a = [r["engine"][g][0] for r in rounds]
@@ -131,7 +146,9 @@ def main():
         ec = rounds[0]["main_loop"][(g, 1)]["engine_cluster"]   # the cluster size the engine launches this GEMM in
         mbe = mb2 if ec == 2 else mb1
         av = [x for x in a if x is not None]
-        rows.append({"gemm": g, "launches_per_step": per_step, "engine_cluster": ec, "engine_ms": ma,
+        cv = [r["epilogue_bound"][g][0] for r in rounds] if g in EPILOGUE_BOUND else []
+        mc = med(cv)
+        rows.append({"epilogue_bound_ms": mc, "epilogue_bound_ms_rounds": cv, "gemm": g, "launches_per_step": per_step, "engine_cluster": ec, "engine_ms": ma,
                      "main_loop_ms": mbe, "main_loop_ms_rounds": b[ec], "main_loop_ms_cluster1": mb1,
                      "main_loop_ms_cluster2": mb2, "main_loop_ms_cluster1_rounds": b[1],
                      "main_loop_ms_cluster2_rounds": b[2], "engine_ms_rounds": a,
@@ -139,9 +156,11 @@ def main():
                      "stages": rounds[0]["main_loop"][(g, 1)]["stages"], "tiles": rounds[0]["main_loop"][(g, 1)]["tiles"]})
         ra = f"[{min(av):.3f}-{max(av):.3f}]" if av else ""
         r1, r2 = f"[{min(b[1]):.3f}-{max(b[1]):.3f}]", f"[{min(b[2]):.3f}-{max(b[2]):.3f}]"
+        cvv = [x for x in cv if x is not None]
+        rc = f"[{min(cvv):.3f}-{max(cvv):.3f}]" if cvv else ""
         print(f"{g:8s} {per_step:13.1f} {fmt(ma, 10)} {ra:15s} {mb1:24.3f} {r1:15s} {mb2:10.3f} {r2:15s} "
-              f"{mb2 / mb1:8.3f} {fmt(None if ma is None else ma - mbe, 12)}")
-    res = {"card": info, "rounds": [{k: v for k, v in r.items() if k.startswith("clock")} for r in rounds], "gemms": rows}
+              f"{mb2 / mb1:8.3f} {fmt(None if ma is None else ma - mbe, 12)} {fmt(mc, 8)} {rc:15s}")
+    res = {"card": info, "arith": run.arith, "epilogue_bound_d": EPILOGUE_BOUND_D, "rounds": [{k: v for k, v in r.items() if k.startswith("clock")} for r in rounds], "gemms": rows}
     line = json.dumps(res)
     print(line)
     if args.out:

@@ -32,7 +32,8 @@ extern "C" {
  * the two fields zeroed) before it uses this library.
  * 201 also covers the additive entry points sce_second_moments_workspace_bytes / sce_second_moments (BatchedPCA). They
  * are plan-less and change nothing above. So are sce_ica_pass_workspace_bytes / sce_ica_pass (ICAEncoder), added
- * under 201 as well. */
+ * under 201 as well, and the NMF entry points sce_nmf_project, sce_nmf_grams, sce_nmf_residual and sce_nmf_cd_sweep
+ * with their *_workspace_bytes queries (NMFEncoder). */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -404,6 +405,69 @@ size_t sce_ica_pass_workspace_bytes(int d, int n, int B);
 int sce_ica_pass(const void* x, int x_is_half, int B, int d, const float* shift, const float* unmix, int n, float alpha,
                  int arith, double* g_sum, double* gx, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
                  void* stream);
+
+/* NMF with sklearn's coordinate-descent solver (autoencoders/nmf.py's NMF().fit and transform), without a plan. For the B
+ * rows x_b of x, v_b = max(x_b - shift, 0) (fp32; NaN stays NaN):
+ *
+ * sce_nmf_project: p[b * k + j] = sum_i m[j * d + i] v_b[i], fp32 [B, k] (transform's X H^T with m = H, or NNDSVD's
+ * X V^T with m = the right singular vectors), and with norms (device fp64 [2][k], ACCUMULATED, or NULL)
+ *   norms[j]     += sum_b max(p_bj, 0)^2,   norms[k + j] += sum_b min(p_bj, 0)^2
+ * It runs on the encode GEMM; its epilogue stores p and fp32 partials of the norms per 32 rows, added in fp64 in row-block
+ * order.
+ *
+ * sce_nmf_grams: for w [B, k] fp32 (rows of the codes W),
+ *   wtw[i * k + j] += sum_b w_bi w_bj,   wtv[i * d + j] += sum_b w_bi v_b[j]     (device fp64, 16-byte aligned)
+ * The rows are sliced as in sce_second_moments; both products run on the weight gradient's GEMM per slice, and the
+ * slices are added in fp64 in slice order.
+ *
+ * For both:
+ *   x            device [B, d] row-major, fp16 (x_is_half = 1, read as it is) or fp32; 16-byte aligned
+ *   shift        device fp32 [d], 16-byte aligned
+ *   m / w        device fp32, 16-byte aligned; p device fp32 [B, k], 16-byte aligned
+ *   arith        sce_arith. AUTO: BF16X3. F16F8 needs d % 16 == 0 and k % 16 == 0.
+ *   range_flag   device uint32 or NULL: F16F8 sets it to 1 when some v, m or w entry does not fit the fp16 plane
+ *                (|v| >= 65520 or NaN); the results are then not meaningful. The caller zeroes it.
+ *   d            a multiple of 8 in [8, 8192];  k a multiple of 8 in [8, d];  B in [1, 2^21]
+ *   workspace    >= the matching *_workspace_bytes(d, k, B), 1024-byte aligned: the planes of the operands and the
+ *                fp32 partials. Host-only; 0 for invalid arguments. Never decreases with B.
+ *
+ * sce_nmf_cd_sweep: coordinate-descent sweeps of sklearn's _update_cdnmf_fast (no regularisation, coordinates in order
+ * 0 .. k-1) over the R rows of w [R, k] (in/out), with g [k, k] (HH^T or W^T W) and l [R, k] (XH^T or X^T W) fixed:
+ *   for t in 0 .. k-1, per row i:  grad = sum_r g[t][r] w[i][r] - l[i][t];  pg = w[i][t] == 0 ? min(grad, 0) : grad;
+ *   violation += |pg|;  if g[t][t] != 0: w[i][t] = max(w[i][t] - grad / g[t][t], 0)
+ *   g            must be symmetric (H H^T and W^T W are in exact arithmetic; NMFEncoder symmetrises both): the kernel
+ *                keeps the gradient as sum_r w[i][r] g[r][t] and so reads row t of g where the loop above names its
+ *                column t
+ *   w_is_f64     0: w, g and l are fp32 (NMFEncoder's W-update and transform), 1: fp64 (its H-update)
+ *   k            in [1, 2048];  R >= 1
+ *   n_iter NULL  one sweep (max_sweeps = 1): violation[0] (device fp64) += its violation
+ *   n_iter       device int: transform's loop. violation[0..1] and n_iter are zeroed, then up to max_sweeps sweeps are
+ *                queued; sweep s is a no-op once the stop rule held after sweep s - 1 (violation[0] == 0, or
+ *                violation[1] / violation[0] <= tol), so n_iter ends as sklearn's iteration count, violation[0] as the
+ *                first sweep's violation and violation[1] as the last one's. No host read.
+ *   workspace    >= sce_nmf_cd_sweep_workspace_bytes(k, R), 1024-byte aligned: one fp64 partial per 8 rows.
+ * One warp sweeps one row, with the row and its gradient in registers and rows of g staged in shared memory; a coordinate
+ * whose step is zero costs no gradient update. Violations are fp64, added in a fixed order.
+ * No atomics anywhere: results are bitwise repeatable. All three are asynchronous on `stream`. */
+size_t sce_nmf_project_workspace_bytes(int d, int k, int B);
+int sce_nmf_project(const void* x, int x_is_half, int B, int d, const float* shift, const float* m, int k, int arith,
+                    float* p, double* norms, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
+                    void* stream);
+size_t sce_nmf_grams_workspace_bytes(int d, int k, int B);
+int sce_nmf_grams(const void* x, int x_is_half, int B, int d, const float* shift, const float* w, int k, int arith,
+                  double* wtw, double* wtv, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
+                  void* stream);
+/* sce_nmf_residual: sum[0] += sum_b ||v_b - w_b h||^2 (device fp64, ACCUMULATED) for w [B, k] and h [k, d], both fp32
+ * and 16-byte aligned, with v_b as above (the fit's reconstruction_err_). A plain fp32 product on the CUDA cores, not the
+ * split-operand GEMM: at a good fit the residual is a small fraction of the rows, which products good to 2^-16 would
+ * not resolve. d, k and B as for sce_nmf_project; workspace >= sce_nmf_residual_workspace_bytes(d, B) (one fp64
+ * partial per 64 x 64 tile), 1024-byte aligned. Squares are fp64, added in a fixed order. */
+size_t sce_nmf_residual_workspace_bytes(int d, int B);
+int sce_nmf_residual(const void* x, int x_is_half, int B, int d, const float* shift, const float* w, int k,
+                     const float* h, double* sum, void* workspace, size_t workspace_bytes, void* stream);
+size_t sce_nmf_cd_sweep_workspace_bytes(int k, int R);
+int sce_nmf_cd_sweep(void* w, int w_is_f64, int R, int k, const void* g, const void* l, int max_sweeps, double tol,
+                     double* violation, int* n_iter, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -33,6 +33,8 @@ EXPORTS = [
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
     "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows", "sce_read_center_grad",
     "sce_second_moments_workspace_bytes", "sce_second_moments", "sce_ica_pass_workspace_bytes", "sce_ica_pass",
+    "sce_nmf_project_workspace_bytes", "sce_nmf_project", "sce_nmf_grams_workspace_bytes", "sce_nmf_grams",
+    "sce_nmf_cd_sweep_workspace_bytes", "sce_nmf_cd_sweep", "sce_nmf_residual_workspace_bytes", "sce_nmf_residual",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -197,6 +199,18 @@ def load():
     lib.sce_ica_pass_workspace_bytes.restype = C.c_size_t
     lib.sce_ica_pass_workspace_bytes.argtypes = [i, i, i]
     lib.sce_ica_pass.argtypes = [vp, i, i, i, vp, vp, i, f, i, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_nmf_project_workspace_bytes.restype = C.c_size_t
+    lib.sce_nmf_project_workspace_bytes.argtypes = [i, i, i]
+    lib.sce_nmf_project.argtypes = [vp, i, i, i, vp, vp, i, i, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_nmf_grams_workspace_bytes.restype = C.c_size_t
+    lib.sce_nmf_grams_workspace_bytes.argtypes = [i, i, i]
+    lib.sce_nmf_grams.argtypes = [vp, i, i, i, vp, vp, i, i, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_nmf_residual_workspace_bytes.restype = C.c_size_t
+    lib.sce_nmf_residual_workspace_bytes.argtypes = [i, i]
+    lib.sce_nmf_residual.argtypes = [vp, i, i, i, vp, vp, i, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_nmf_cd_sweep_workspace_bytes.restype = C.c_size_t
+    lib.sce_nmf_cd_sweep_workspace_bytes.argtypes = [i, i]
+    lib.sce_nmf_cd_sweep.argtypes = [vp, i, i, i, vp, vp, i, C.c_double, vp, vp, vp, C.c_size_t, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

@@ -1477,21 +1477,23 @@ static Slices mom_slices(int d, int B) {
   return {(B + R - 1) / R, R};
 }
 
-// The buffers of a row pass of width d: the second moments' (n = 0), or the FastICA pass's with n components, which
-// alone take t, its copies, the unmix planes, the g' partials and the flag words
+// The buffers of a row pass of width d: the second moments' (n = 0), the FastICA pass's with n components, which
+// alone take t, its copies, the unmix planes, the g' partials and the flag words, or (nmf) sce_nmf_grams' with k = n
+// codes, which takes W's planes and copies in t / tt, the W^T W partials and the flag words, but no column sums
 struct RowCarve {
   Planes x, xt;      // the shifted rows [S * R][d] (zero beyond B); f16f8: batch-major 8-bit copies [S][d][R]
-  Planes t, tt;      // ICA: t [S * R][n]; f16f8: batch-major 8-bit copies [S][n][R]
+  Planes t, tt;      // ICA: t [S * R][n] (NMF: W); f16f8: batch-major 8-bit copies [S][n][R]
   Planes w;          // ICA: unmix [n][d]
   float* part;       // [S][n, or d][d] fp32 slice partials
-  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (unused by ICA)
+  float* part_g;     // NMF: [S][n][n] fp32 slice partials of W^T W
+  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (unused by ICA, not carved for NMF)
   float* g_part;     // ICA: [S * R / 32][n] g' partials
   uint32_t* flags;   // ICA: kFlagWords, the f16f8 range check of unmix
 };
 // Carves S slices of `rows` (= S R) padded rows. The workspace query carves upper bounds of both instead, which never
 // decrease with B: the exact S is not monotone in B (at d = 512, B = 64000 takes 33 slices of 1984 rows, B = 65536 32
 // of 2048), and a caller sizes one workspace for its longest call.
-static size_t row_carve(uint8_t* base, bool f8, int d, int n, size_t S, size_t rows, RowCarve* out) {
+static size_t row_carve(uint8_t* base, bool f8, int d, int n, size_t S, size_t rows, RowCarve* out, bool nmf = false) {
   const size_t dd = (size_t)d, nn = (size_t)n;
   Carve c{base, 0};
   RowCarve w{};
@@ -1500,6 +1502,13 @@ static size_t row_carve(uint8_t* base, bool f8, int d, int n, size_t S, size_t r
   if (f8) {
     w.xt = c.copies(rows * dd);
     if (n) w.tt = c.copies(rows * nn);
+  }
+  if (nmf) {
+    w.part = c.take<float>(S * nn * dd);
+    w.part_g = c.take<float>(S * nn * nn);
+    w.flags = c.take<uint32_t>(kFlagWords);
+    if (out) *out = w;
+    return align_up(c.off, 1024);
   }
   if (n) w.w = c.planes(nn * dd, f8);
   w.part = c.take<float>(S * (n ? nn : dd) * dd);
@@ -1514,14 +1523,14 @@ static size_t row_carve(uint8_t* base, bool f8, int d, int n, size_t S, size_t r
 // The workspace of a row pass, for both arithmetics; 0 when d or B is out of range. It carves the bounds of mom_slices,
 // non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts from), and S R < B + R <=
 // B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
-static size_t row_pass_workspace(int d, int n, int B) {
+static size_t row_pass_workspace(int d, int n, int B, bool nmf = false) {
   if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
   const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
   const size_t s_target = (kMomTargetTiles + tiles - 1) / tiles, s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
   const size_t s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
   const size_t S = std::max(std::min(s_target, s_short), s_rows);
   const size_t rows = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax, S * kMomRowsMax);
-  return std::max(row_carve(nullptr, false, d, n, S, rows, nullptr), row_carve(nullptr, true, d, n, S, rows, nullptr));
+  return std::max(row_carve(nullptr, false, d, n, S, rows, nullptr, nmf), row_carve(nullptr, true, d, n, S, rows, nullptr, nmf));
 }
 
 // rows r0 .. r0 + 63 of the call (grid.y), four columns per thread (grid.x covers d / 4 threads):
@@ -1529,7 +1538,8 @@ static size_t row_pass_workspace(int d, int n, int B) {
 //   last slice adds nothing to the Gram matrix (0 - shift would add shift shift^T per row)
 //   col_part[blockIdx.y][c] = sum of v over the block's rows, in row order in fp64
 //   f16f8: range_flag = 1 when some |v| >= 65520 or v is NaN (the fp16 plane cannot hold it)
-template <int ARITH, class InT>
+// CLAMP (the NMF passes): v = max(x - shift, 0) instead (NaN stays NaN), and no column sums (col_part is not read)
+template <int ARITH, class InT, bool CLAMP = false>
 __global__ void __launch_bounds__(128) moment_split_kernel(const InT* __restrict__ x, int B, int d,
                                                            const float* __restrict__ shift, void* __restrict__ hi,
                                                            void* __restrict__ lo, void* __restrict__ x8,
@@ -1561,6 +1571,10 @@ __global__ void __launch_bounds__(128) moment_split_kernel(const InT* __restrict
         v[2] = f.z - sh.z;
         v[3] = f.w - sh.w;
       }
+      if constexpr (CLAMP) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) v[q] = v[q] < 0.f ? 0.f : v[q];
+      }
       s0 += v[0];
       s1 += v[1];
       s2 += v[2];
@@ -1570,11 +1584,13 @@ __global__ void __launch_bounds__(128) moment_split_kernel(const InT* __restrict
     }
     store_planes4<ARITH>(v, hi, lo, x8, ((long long)r * d + c) / 4);
   }
-  double* o = col_part + (long long)blockIdx.y * d + c;
-  o[0] = s0;
-  o[1] = s1;
-  o[2] = s2;
-  o[3] = s3;
+  if constexpr (!CLAMP) {
+    double* o = col_part + (long long)blockIdx.y * d + c;
+    o[0] = s0;
+    o[1] = s1;
+    o[2] = s2;
+    o[3] = s3;
+  }
   if (bad && range_flag) *range_flag = 1u;   // benign race: all write 1
 }
 
@@ -1616,11 +1632,18 @@ __global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restric
 
 // moment_split_kernel over the S R rows of a call: the shifted rows into the planes of w.x, the column-sum partials and,
 // with f16f8, the range flag
-template <int AR>
+template <int AR, bool CLAMP = false>
 static int launch_row_split(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const Slices& sl,
                             const RowCarve& w, uint32_t* range_flag) {
   const dim3 grid((d / 4 + 127) / 128, sl.S * sl.R / kMomBlockRows);
   uint32_t* flag = AR == kArithF16F8 ? range_flag : nullptr;
+  if constexpr (CLAMP) {
+    if (half)
+      return L.launch(moment_split_kernel<AR, __half, true>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift,
+                      w.x.hi, w.x.lo, w.x.x8, nullptr, flag);
+    return L.launch(moment_split_kernel<AR, float, true>, grid, 128, 0, static_cast<const float*>(x), B, d, shift,
+                    w.x.hi, w.x.lo, w.x.x8, nullptr, flag);
+  }
   if (half)
     return L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi,
                     w.x.lo, w.x.x8, w.col_part, flag);
@@ -1629,15 +1652,16 @@ static int launch_row_split(Launcher& L, const void* x, bool half, int B, int d,
 }
 
 // part[s] = A_s^T V_s (fp32 [S][m][d]) for the slices s of R rows of A [S R][m] and V [S R][d]: the weight gradient's
-// GEMM, one slice per model. f16f8: first the batch-major copies At and Vt of their 8-bit planes (one when A is V).
+// GEMM, one slice per model. f16f8: first the batch-major copies At and Vt of their 8-bit planes (one when A is V; none
+// of A with a_copied, when an earlier call of the same rows made At).
 template <int AR>
 static int sliced_gemm_t(Launcher& L, const Slices& sl, const Planes& A, const Planes& At, int m, const Planes& V,
-                         const Planes& Vt, int d, float* part, int device, int sms) {
+                         const Planes& Vt, int d, float* part, int device, int sms, bool a_copied = false) {
   constexpr bool f8 = AR == kArithF16F8;
   const bool a_is_v = A.hi == V.hi;
   const int S = sl.S, R = sl.R;
   if constexpr (f8) {
-    TRY(batch_major(L, A, At, S, R, m, (long long)R * m, R));
+    if (!a_copied) TRY(batch_major(L, A, At, S, R, m, (long long)R * m, R));
     if (!a_is_v) TRY(batch_major(L, V, Vt, S, R, d, (long long)R * d, R));
   }
   const int bk = gemm_bk(AR);
@@ -1721,10 +1745,11 @@ static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const 
   return reduce_rows(L, w, B, sl.S, n, d, gx, nullptr, g_sum);
 }
 
-// The checks sce_second_moments and sce_ica_pass share, made before any CUDA call (`n`: ICA's, or 0): the rows x [B][d],
-// fp16 or fp32, and shift [d], 16-byte aligned; the arithmetic
+// The checks the row passes share, made before any CUDA call (`n`: ICA's or NMF's, or 0): the rows x [B][d], fp16 or
+// fp32, and shift [d], 16-byte aligned; the arithmetic. With `mat_name` (the NMF passes), also the fp32 matrix `mat` of
+// n rows (M [n][d] or W [B][n]): present and 16-byte aligned, n a multiple of 8 in [8, d].
 static int check_row_pass(const char* prefix, const void* x, int x_is_half, int B, int d, const float* shift, int n,
-                          int arith) {
+                          int arith, const float* mat = nullptr, const char* mat_name = nullptr) {
   if (!x || !shift) return fail(SCE_ERR_INVALID, "%sx and shift are required", prefix);
   if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "%sx_is_half must be 0 or 1", prefix);
   if (B < 1 || B > kMomCallRowsMax) return fail(SCE_ERR_INVALID, "%sB = %d outside [1, %d]", prefix, B, kMomCallRowsMax);
@@ -1735,7 +1760,388 @@ static int check_row_pass(const char* prefix, const void* x, int x_is_half, int 
              : fail(SCE_ERR_INVALID, "%sarith = F16F8 needs d (%d) to be a multiple of 16", prefix, d);
   if (reinterpret_cast<uintptr_t>(x) % 16 || reinterpret_cast<uintptr_t>(shift) % 16)
     return fail(SCE_ERR_INVALID, "%sx and shift must be 16-byte aligned", prefix);
+  if (mat_name) {
+    if (!mat) return fail(SCE_ERR_INVALID, "%s%s is required", prefix, mat_name);
+    if (n < 8 || n % 8 || n > d) return fail(SCE_ERR_INVALID, "%sk (%d) must be a multiple of 8 in [8, d = %d]", prefix, n, d);
+    if (reinterpret_cast<uintptr_t>(mat) % 16) return fail(SCE_ERR_INVALID, "%s%s must be 16-byte aligned", prefix, mat_name);
+  }
   return SCE_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// NMF (sce_nmf_project, sce_nmf_grams, sce_nmf_cd_sweep): sklearn's NMF() with the coordinate-descent solver, for
+// NMFEncoder
+// ------------------------------------------------------------------------------------------------
+// Projection: for v = max(x - shift, 0) and an fp32 M [k][d], P = v M^T, fp32 [B][k]. The rows are split as for the row
+// passes (CLAMP) into one model of B rows padded to kMomBlockRows; the GEMM is the encode geometry (both operands K-major
+// over d), its epilogue EpiNmfProject stores P and, optionally, the per-32-row partials of the squared positive and
+// negative parts of each column, which nmf_col_reduce_kernel adds up over the row blocks in order in fp64.
+struct NmfProjectCarve {
+  Planes x, m;       // v [rows][d], M [k][d]
+  float* part;       // [ceil(B / 32)][2][k]
+  uint32_t* flags;   // kFlagWords: the f16f8 range check of M
+};
+static size_t nmf_project_carve(uint8_t* base, bool f8, int d, int k, int B, NmfProjectCarve* out) {
+  const size_t rows = ((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows;
+  Carve c{base, 0};
+  NmfProjectCarve w{};
+  w.x = c.planes(rows * d, f8);
+  w.m = c.planes((size_t)k * d, f8);
+  w.part = c.take<float>(((size_t)B + 31) / 32 * 2 * k);
+  w.flags = c.take<uint32_t>(kFlagWords);
+  if (out) *out = w;
+  return align_up(c.off, 1024);
+}
+
+// sums[j] += sum over the row blocks b, in order, of part[b][j], j < n (fp64)
+__global__ void nmf_col_reduce_kernel(const float* __restrict__ part, int blocks, int n, double* __restrict__ sums) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  double a = 0.0;
+  for (int b = 0; b < blocks; ++b) a += (double)__ldg(part + (long long)b * n + j);
+  sums[j] += a;
+}
+
+// fp32 M [k][d] -> planes; f16f8: its range check joins the rows' in range_flag
+template <int AR>
+static int split_matrix(Launcher& L, const float* m, const Planes& planes, long long count, uint32_t* flags,
+                        uint32_t* range_flag) {
+  if (AR == kArithF16F8 && range_flag) {
+    CUDA_TRY(cudaMemsetAsync(flags, 0, kFlagWords * sizeof(uint32_t), L.st));
+    TRY(launch_split_rows<AR>(L, m, planes, count / 4, flags));
+    return L.launch(set_flag_if_kernel, 1, 1, 0, flags + kBadWord, range_flag);
+  }
+  return launch_split_rows<AR>(L, m, planes, count / 4, nullptr);
+}
+
+template <int AR>
+static int run_nmf_project_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* m,
+                             int k, float* p, double* norms, const NmfProjectCarve& w, uint32_t* range_flag, int device,
+                             int sms) {
+  constexpr bool f8 = AR == kArithF16F8;
+  const int rows = (B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows;
+  RowCarve rc{};
+  rc.x = w.x;
+  TRY((launch_row_split<AR, true>(L, x, half, B, d, shift, Slices{1, rows}, rc, range_flag)));
+  TRY(split_matrix<AR>(L, m, w.m, (long long)k * d, w.flags, range_flag));
+  const int bk = gemm_bk(AR);
+  GemmMaps maps{};
+  EpiNmfProject::Params ep;
+  bool ok = operand_maps(maps.a[0], w.x, 1, (uint64_t)B, (uint64_t)d, (uint64_t)B * d, kBM, bk) &&
+            operand_maps(maps.b[0], w.m, 1, (uint64_t)k, (uint64_t)d, (uint64_t)k * d, kBN, bk) &&
+            make_tmap_f32_store32(&ep.out, p, 1, (uint64_t)B, (uint64_t)k, (uint64_t)B * k);
+  if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (nmf project: d=%d, k=%d, B=%d)", d, k, B);
+  ep.part = norms ? w.part : nullptr;
+  TRY((launch_gemm_t<EpiNmfProject, false, false, false, AR, f8>(L, 1, device, sms, maps, 1, kOnes, kOnes, d, 3, B, k, ep)));
+  if (!norms) return SCE_OK;
+  return L.launch(nmf_col_reduce_kernel, (2 * k + 255) / 256, 256, 0, w.part, (B + 31) / 32, 2 * k, norms);
+}
+
+// Gram matrices: for v as above and an fp32 W [B][k], wtw += W^T W and wtv += W^T v (fp64). The sliced row reduction of
+// the second moments: v and W are split into the planes of S slices of R rows (padding rows zero), each slice's two
+// products run on the weight gradient's GEMM (sliced_gemm_t: W^T W with A = V = W, then W^T v), and gram_reduce_kernel
+// adds the slice partials in slice order in fp64.
+static int reduce_slices(Launcher& L, const float* part, int S, long long n4, double* out) {
+  const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
+  return L.launch(gram_reduce_kernel, rblocks, 256, 0, part, S, n4, out, nullptr, 0, 0, nullptr, nullptr, 0, 0, nullptr);
+}
+
+template <int AR>
+static int run_nmf_grams_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* wm,
+                           int k, const Slices& sl, const RowCarve& w, double* wtw, double* wtv, uint32_t* range_flag,
+                           int device, int sms) {
+  const long long rows = (long long)sl.S * sl.R;
+  TRY((launch_row_split<AR, true>(L, x, half, B, d, shift, sl, w, range_flag)));
+  TRY(split_matrix<AR>(L, wm, w.t, (long long)B * k, w.flags, range_flag));
+  if (rows > B) CUDA_TRY(w.t.at((size_t)B * k).zero((size_t)(rows - B) * k, L.st));
+  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, k, w.t, w.tt, k, w.part_g, device, sms));
+  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, k, w.x, w.xt, d, w.part, device, sms, true));   // W's copies: made above
+  TRY(reduce_slices(L, w.part_g, sl.S, (long long)k * k / 4, wtw));
+  return reduce_slices(L, w.part, sl.S, (long long)k * d / 4, wtv);
+}
+
+// One coordinate-descent sweep (sklearn's _update_cdnmf_fast, coordinates in order, no regularisation) over the rows
+// of W [R][k], with G [k][k] and L [R][k] fixed: for t = 0 .. k-1, per row i,
+//   grad = sum_r G[t][r] W[i][r] - L[i][t];  pg = W[i][t] == 0 ? min(grad, 0) : grad;  violation += |pg|
+//   G[t][t] != 0: W[i][t] = max(W[i][t] - grad / G[t][t], 0)
+// The rows are independent, so each is swept by one warp, which keeps the row and its gradient g = W G - L in
+// registers: lane l holds the columns VW l + 32 VW q + e (q < KPL / VW, e < VW; VW = min(KPL, 4) consecutive columns,
+// so that a lane reads its share of a row of G as one 16-byte load). Per coordinate, the owning lane takes the step and
+// broadcasts the change delta with one shuffle; only when delta != 0 (a code entry that stays at 0 changes nothing) do
+// the lanes add delta G[t][:] to g. g starts as -L plus W[r] G[r][:] for the non-zero W[r] (skipped for a block whose
+// rows are all zero, as transform's first sweep). The blocks' kCdWarps warps share rows of G, staged in shared memory
+// `tb` rows at a time. T is the arithmetic of W, G, L and g; the violation is fp64. No atomics: each lane sums its
+// coordinates in order, the warp and the block add in a fixed order, and nmf_violation_kernel adds the block partials
+// in block order.
+// With n_iter (transform's loop), a sweep is a no-op once the stop rule held after the previous one.
+constexpr int kCdWarps = 8;
+constexpr int kCdMaxK = 2048;
+
+__device__ __forceinline__ bool nmf_stopped(const double* viol, const int* n_iter, double tol) {
+  if (!n_iter || *n_iter < 1) return false;
+  return viol[0] == 0.0 || viol[1] / viol[0] <= tol;
+}
+
+template <class T, int VW>
+__device__ __forceinline__ void load_vec(const T* p, T (&v)[VW]) {
+  if constexpr (VW == 4 && sizeof(T) == 4) {
+    const float4 a = *reinterpret_cast<const float4*>(p);
+    v[0] = a.x, v[1] = a.y, v[2] = a.z, v[3] = a.w;
+  } else if constexpr (VW >= 2 && VW % 2 == 0 && sizeof(T) == 8) {
+#pragma unroll
+    for (int e = 0; e < VW; e += 2) {
+      const double2 a = *reinterpret_cast<const double2*>(p + e);
+      v[e] = a.x, v[e + 1] = a.y;
+    }
+  } else {
+#pragma unroll
+    for (int e = 0; e < VW; ++e) v[e] = p[e];
+  }
+}
+
+// g += a row[:] over the lane's columns (row: a staged row of G, 32 KPL entries)
+template <class T, int KPL>
+__device__ __forceinline__ void cd_axpy(T (&g)[KPL], T a, const T* row, int lane) {
+  constexpr int VW = KPL < 4 ? KPL : 4;
+#pragma unroll
+  for (int q = 0; q < KPL / VW; ++q) {
+    T v[VW];
+    load_vec<T, VW>(row + 32 * VW * q + VW * lane, v);
+#pragma unroll
+    for (int e = 0; e < VW; ++e) g[q * VW + e] = fma(a, v[e], g[q * VW + e]);
+  }
+}
+
+template <class T, int KPL>
+__global__ void __launch_bounds__(kCdWarps * 32) nmf_cd_sweep_kernel(T* __restrict__ w, int R, int k,
+                                                                    const T* __restrict__ G, const T* __restrict__ Lm,
+                                                                    int tb, double* __restrict__ part,
+                                                                    const double* __restrict__ viol,
+                                                                    const int* __restrict__ n_iter, double tol) {
+  if (nmf_stopped(viol, n_iter, tol)) return;   // (block-uniform)
+  constexpr int VW = KPL < 4 ? KPL : 4, KP = 32 * KPL;
+  extern __shared__ __align__(16) unsigned char cd_smem[];
+  T* gs = reinterpret_cast<T*>(cd_smem);   // [tb][KP]: rows t0 .. t0 + tb - 1 of G, zero beyond k
+  __shared__ double wsum[kCdWarps];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long row = (long long)blockIdx.x * kCdWarps + warp;
+  const bool live = row < R;
+  T wr[KPL], g[KPL];
+  bool nonzero = false;
+#pragma unroll
+  for (int q = 0; q < KPL / VW; ++q)
+#pragma unroll
+    for (int e = 0; e < VW; ++e) {
+      const int j = 32 * VW * q + VW * lane + e;
+      const bool ok = live && j < k;
+      wr[q * VW + e] = ok ? w[row * k + j] : T(0);
+      g[q * VW + e] = ok ? -Lm[row * k + j] : T(0);
+      nonzero |= wr[q * VW + e] != T(0);
+    }
+  auto stage = [&](int t0) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < tb * KP; i += blockDim.x) {
+      const int t = t0 + i / KP, c = i % KP;
+      gs[i] = t < k && c < k ? G[(long long)t * k + c] : T(0);
+    }
+    __syncthreads();
+  };
+  const int sb = tb / VW;   // lane groups per staged block (tb is a multiple of VW and divides 32 VW)
+  // ---- g = W G - L
+  if (__syncthreads_or(nonzero)) {
+#pragma unroll
+    for (int q = 0; q < KPL / VW; ++q) {
+      for (int s0 = 0; s0 < 32 && 32 * VW * q + VW * s0 < k; s0 += sb) {
+        const int t0 = 32 * VW * q + VW * s0;
+        stage(t0);
+        for (int s = s0; s < s0 + sb; ++s) {
+#pragma unroll
+          for (int e = 0; e < VW; ++e) {
+            const T a = __shfl_sync(0xffffffffu, wr[q * VW + e], s);
+            if (a != T(0)) cd_axpy<T, KPL>(g, a, gs + (VW * (s - s0) + e) * KP, lane);
+          }
+        }
+      }
+    }
+  }
+  // ---- the sweep
+  double v = 0.0;
+#pragma unroll
+  for (int q = 0; q < KPL / VW; ++q) {
+    for (int s0 = 0; s0 < 32 && 32 * VW * q + VW * s0 < k; s0 += sb) {
+      const int t0 = 32 * VW * q + VW * s0;
+      stage(t0);
+      for (int s = s0; s < s0 + sb; ++s) {
+#pragma unroll
+        for (int e = 0; e < VW; ++e) {
+          const T* grow = gs + (VW * (s - s0) + e) * KP;
+          const int t = t0 + VW * (s - s0) + e;
+          const T hess = grow[t];   // G[t][t] (t < KP)
+          T delta = T(0);
+          if (lane == s) {
+            const T gt = g[q * VW + e], wt = wr[q * VW + e];
+            const T pg = wt == T(0) ? (gt < T(0) ? gt : T(0)) : gt;
+            v += fabs((double)pg);
+            if (hess != T(0)) {
+              const T u = wt - gt / hess;
+              const T wn = u > T(0) ? u : T(0);
+              delta = wn - wt;
+              wr[q * VW + e] = wn;
+            }
+          }
+          delta = __shfl_sync(0xffffffffu, delta, s);
+          if (delta != T(0)) cd_axpy<T, KPL>(g, delta, grow, lane);
+        }
+      }
+    }
+  }
+  if (live) {
+#pragma unroll
+    for (int q = 0; q < KPL / VW; ++q)
+#pragma unroll
+      for (int e = 0; e < VW; ++e) {
+        const int j = 32 * VW * q + VW * lane + e;
+        if (j < k) w[row * k + j] = wr[q * VW + e];
+      }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if (lane == 0) wsum[warp] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double b = 0.0;
+#pragma unroll
+    for (int i = 0; i < kCdWarps; ++i) b += wsum[i];
+    part[blockIdx.x] = b;
+  }
+}
+
+// The sweep's violation: the block partials added in block order. Without n_iter, violation[0] += it. With n_iter
+// (transform's loop): unless the stop rule already held, ++n_iter, violation[1] = it and, on the first sweep,
+// violation[0] = it.
+__global__ void __launch_bounds__(256) nmf_violation_kernel(const double* __restrict__ part, int blocks, double* viol,
+                                                            int* n_iter, double tol) {
+  if (nmf_stopped(viol, n_iter, tol)) return;
+  __shared__ double s[256];
+  double a = 0.0;
+  for (int i = threadIdx.x; i < blocks; i += 256) a += part[i];
+  s[threadIdx.x] = a;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (threadIdx.x < h) s[threadIdx.x] += s[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x) return;
+  if (!n_iter) {
+    viol[0] += s[0];
+    return;
+  }
+  const int it = *n_iter + 1;
+  *n_iter = it;
+  if (it == 1) viol[0] = s[0];
+  viol[1] = s[0];
+}
+
+// Residual (sce_nmf_residual): sum over the rows of ||max(x - shift, 0) - w h||^2 for W [B][k] and H [k][d] fp32, the fit's
+// reconstruction_err_. A plain fp32 SIMT product, not the split-operand GEMM: at a good fit the residual is ~1e-3 of
+// the rows, and products good to 2^-16 (bf16x3) would leave its square with no correct digit. Block tile 64 rows x 64
+// columns, 4 x 4 per thread, k in steps of 16 through shared memory; squares in fp64, one partial per block (added in
+// block order by nmf_violation_kernel).
+constexpr int kResTile = 64, kResK = 16;
+template <class InT>
+__global__ void __launch_bounds__(256) nmf_residual_kernel(const InT* __restrict__ x, int B, int d,
+                                                           const float* __restrict__ shift, const float* __restrict__ w,
+                                                           int k, const float* __restrict__ h, double* __restrict__ part) {
+  __shared__ float ws[kResK][kResTile + 4];
+  __shared__ float hs[kResK][kResTile];
+  __shared__ double red[8];
+  const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
+  const long long r0 = (long long)blockIdx.y * kResTile;
+  const int c0 = blockIdx.x * kResTile;
+  float acc[4][4] = {};
+  for (int k0 = 0; k0 < k; k0 += kResK) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int i = threadIdx.x + 256 * q;
+      const int wr = i / kResK, wk = i % kResK, hk = i / kResTile, hc = i % kResTile;
+      const long long r = r0 + wr;
+      ws[wk][wr] = r < B && k0 + wk < k ? w[r * k + k0 + wk] : 0.f;
+      hs[hk][hc] = k0 + hk < k && c0 + hc < d ? h[(long long)(k0 + hk) * d + c0 + hc] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kResK; ++kk) {
+      float a[4], b[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = ws[kk][ty * 4 + i], b[i] = hs[kk][tx * 4 + i];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+  double s = 0.0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const long long r = r0 + ty * 4 + i;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + tx * 4 + j;
+      if (r < B && c < d) {
+        float v = (float)x[r * d + c] - shift[c];
+        v = v < 0.f ? 0.f : v;
+        const double e = (double)v - (double)acc[i][j];
+        s += e * e;
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += red[i];
+    part[(long long)blockIdx.y * gridDim.x + blockIdx.x] = t;
+  }
+}
+
+// the shared-memory rows of G per staged block: a power of two, a multiple of VW, at most 32 VW, within 48 KB where VW
+// rows fit
+static int cd_stage_rows(int kpl, size_t elem) {
+  const int vw = kpl < 4 ? kpl : 4;
+  const size_t row = (size_t)32 * kpl * elem;
+  int tb = vw;
+  while (tb * 2 <= 32 * vw && (size_t)tb * 2 * row <= 48 * 1024) tb *= 2;
+  return tb;
+}
+
+template <class T, int KPL>
+static int launch_cd_t(Launcher& L, T* w, int R, int k, const T* G, const T* Lm, double* part, double* viol, int* n_iter,
+                       double tol) {
+  const int tb = cd_stage_rows(KPL, sizeof(T));
+  const size_t smem = (size_t)tb * 32 * KPL * sizeof(T);
+  if (smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute(nmf_cd_sweep_kernel<T, KPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int blocks = (R + kCdWarps - 1) / kCdWarps;
+  TRY(L.launch(nmf_cd_sweep_kernel<T, KPL>, blocks, kCdWarps * 32, smem, w, R, k, G, Lm, tb, part, viol, n_iter, tol));
+  return L.launch(nmf_violation_kernel, 1, 256, 0, part, blocks, viol, n_iter, tol);
+}
+
+// columns per lane: ceil(k / 32) rounded up to a power of two
+template <class T>
+static int launch_cd(Launcher& L, T* w, int R, int k, const T* G, const T* Lm, double* part, double* viol, int* n_iter,
+                     double tol) {
+  const int c = (k + 31) / 32;
+  if (c <= 1) return launch_cd_t<T, 1>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
+  if (c <= 2) return launch_cd_t<T, 2>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
+  if (c <= 4) return launch_cd_t<T, 4>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
+  if (c <= 8) return launch_cd_t<T, 8>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
+  if (c <= 16) return launch_cd_t<T, 16>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
+  if (c <= 32) return launch_cd_t<T, 32>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
+  return launch_cd_t<T, 64>(L, w, R, k, G, Lm, part, viol, n_iter, tol);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2371,6 +2777,126 @@ int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int 
   if (d <= 512) return L.launch(synth_rows_kernel<4, false>, rows8, 256, 0, a);
   if (d <= 1024) return L.launch(synth_rows_kernel<8, false>, rows8, 256, 0, a);
   return L.launch(synth_rows_kernel<8, true>, (unsigned)B, 32 * ((d + 1023) / 1024), 0, a);
+}
+
+
+size_t sce_nmf_project_workspace_bytes(int d, int k, int B) {
+  if (d < 8 || d % 8 || d > 8192 || k < 8 || k % 8 || k > d || B < 1 || B > kMomCallRowsMax) return 0;
+  return std::max(nmf_project_carve(nullptr, false, d, k, B, nullptr), nmf_project_carve(nullptr, true, d, k, B, nullptr));
+}
+
+int sce_nmf_project(const void* x, int x_is_half, int B, int d, const float* shift, const float* m, int k, int arith,
+                    float* p, double* norms, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
+                    void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!p) return fail(SCE_ERR_INVALID, "nmf_project: p is required");
+  TRY(check_row_pass("nmf_project: ", x, x_is_half, B, d, shift, k, arith, m, "m"));
+  if (reinterpret_cast<uintptr_t>(p) % 16 || reinterpret_cast<uintptr_t>(norms) % 8)
+    return fail(SCE_ERR_INVALID, "nmf_project: p must be 16-byte aligned, norms 8-byte aligned");
+  TRY(check_workspace(workspace, workspace_bytes, sce_nmf_project_workspace_bytes(d, k, B), "nmf_project: "));
+
+  // ---- device
+  int dev = 0, sms = 0;
+  if (int rc = query_device(&dev, &sms)) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  // AUTO: bf16x3, as the row passes
+  const bool f8 = arith == SCE_ARITH_F16F8;
+  NmfProjectCarve w;
+  nmf_project_carve(static_cast<uint8_t*>(workspace), f8, d, k, B, &w);
+  return f8 ? run_nmf_project_t<kArithF16F8>(L, x, x_is_half, B, d, shift, m, k, p, norms, w, range_flag, dev, sms)
+            : run_nmf_project_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, m, k, p, norms, w, range_flag, dev, sms);
+}
+
+size_t sce_nmf_grams_workspace_bytes(int d, int k, int B) {
+  return k < 8 || k % 8 || k > d ? 0 : row_pass_workspace(d, k, B, true);
+}
+
+int sce_nmf_grams(const void* x, int x_is_half, int B, int d, const float* shift, const float* w, int k, int arith,
+                  double* wtw, double* wtv, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
+                  void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!wtw || !wtv) return fail(SCE_ERR_INVALID, "nmf_grams: wtw and wtv are required");
+  TRY(check_row_pass("nmf_grams: ", x, x_is_half, B, d, shift, k, arith, w, "w"));
+  if (reinterpret_cast<uintptr_t>(wtw) % 16 || reinterpret_cast<uintptr_t>(wtv) % 16)
+    return fail(SCE_ERR_INVALID, "nmf_grams: wtw and wtv must be 16-byte aligned");
+  TRY(check_workspace(workspace, workspace_bytes, sce_nmf_grams_workspace_bytes(d, k, B), "nmf_grams: "));
+
+  // ---- device
+  int dev = 0, sms = 0;
+  if (int rc = query_device(&dev, &sms)) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  const bool f8 = arith == SCE_ARITH_F16F8;
+  const Slices sl = mom_slices(d, B);
+  RowCarve rc;
+  row_carve(static_cast<uint8_t*>(workspace), f8, d, k, sl.S, (size_t)sl.S * sl.R, &rc, true);
+  return f8 ? run_nmf_grams_t<kArithF16F8>(L, x, x_is_half, B, d, shift, w, k, sl, rc, wtw, wtv, range_flag, dev, sms)
+            : run_nmf_grams_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, w, k, sl, rc, wtw, wtv, range_flag, dev, sms);
+}
+
+size_t sce_nmf_cd_sweep_workspace_bytes(int k, int R) {
+  if (k < 1 || k > kCdMaxK || R < 1) return 0;
+  return align_up((size_t)((R + kCdWarps - 1) / kCdWarps) * sizeof(double), 1024);
+}
+
+int sce_nmf_cd_sweep(void* w, int w_is_f64, int R, int k, const void* g, const void* l, int max_sweeps, double tol,
+                     double* violation, int* n_iter, void* workspace, size_t workspace_bytes, void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!w || !g || !l || !violation) return fail(SCE_ERR_INVALID, "nmf_cd_sweep: w, g, l and violation are required");
+  if (w_is_f64 != 0 && w_is_f64 != 1) return fail(SCE_ERR_INVALID, "nmf_cd_sweep: w_is_f64 must be 0 or 1");
+  if (R < 1) return fail(SCE_ERR_INVALID, "nmf_cd_sweep: R (%d) must be >= 1", R);
+  if (k < 1 || k > kCdMaxK) return fail(SCE_ERR_INVALID, "nmf_cd_sweep: k (%d) must be in [1, %d]", k, kCdMaxK);
+  if (max_sweeps < 1 || (!n_iter && max_sweeps != 1))
+    return fail(SCE_ERR_INVALID, "nmf_cd_sweep: max_sweeps (%d) must be 1 without n_iter, >= 1 with it", max_sweeps);
+  if (!(tol >= 0.0 && tol <= 1e300)) return fail(SCE_ERR_INVALID, "nmf_cd_sweep: tol must be finite and >= 0");
+  const size_t elem = w_is_f64 ? 8 : 4;
+  if (reinterpret_cast<uintptr_t>(w) % elem || reinterpret_cast<uintptr_t>(g) % elem ||
+      reinterpret_cast<uintptr_t>(l) % elem || reinterpret_cast<uintptr_t>(violation) % 8 ||
+      reinterpret_cast<uintptr_t>(n_iter) % 4)
+    return fail(SCE_ERR_INVALID, "nmf_cd_sweep: w, g, l, violation and n_iter must be aligned to their elements");
+  TRY(check_workspace(workspace, workspace_bytes, sce_nmf_cd_sweep_workspace_bytes(k, R), "nmf_cd_sweep: "));
+
+  // ---- device
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  double* part = static_cast<double*>(workspace);
+  if (n_iter) {
+    CUDA_TRY(cudaMemsetAsync(violation, 0, 2 * sizeof(double), L.st));
+    CUDA_TRY(cudaMemsetAsync(n_iter, 0, sizeof(int), L.st));
+  }
+  for (int s = 0; s < max_sweeps; ++s) {
+    if (w_is_f64)
+      TRY(launch_cd(L, static_cast<double*>(w), R, k, static_cast<const double*>(g), static_cast<const double*>(l), part,
+                    violation, n_iter, tol));
+    else
+      TRY(launch_cd(L, static_cast<float*>(w), R, k, static_cast<const float*>(g), static_cast<const float*>(l), part,
+                    violation, n_iter, tol));
+  }
+  return SCE_OK;
+}
+
+
+size_t sce_nmf_residual_workspace_bytes(int d, int B) {
+  if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
+  return align_up((size_t)((d + kResTile - 1) / kResTile) * ((B + kResTile - 1) / kResTile) * sizeof(double), 1024);
+}
+
+int sce_nmf_residual(const void* x, int x_is_half, int B, int d, const float* shift, const float* w, int k,
+                     const float* h, double* sum, void* workspace, size_t workspace_bytes, void* stream) {
+  // ---- arguments (all checked before any CUDA call)
+  if (!h || !sum) return fail(SCE_ERR_INVALID, "nmf_residual: h and sum are required");
+  TRY(check_row_pass("nmf_residual: ", x, x_is_half, B, d, shift, k, SCE_ARITH_AUTO, w, "w"));
+  if (reinterpret_cast<uintptr_t>(h) % 16 || reinterpret_cast<uintptr_t>(sum) % 8)
+    return fail(SCE_ERR_INVALID, "nmf_residual: h must be 16-byte aligned, sum 8-byte aligned");
+  TRY(check_workspace(workspace, workspace_bytes, sce_nmf_residual_workspace_bytes(d, B), "nmf_residual: "));
+
+  // ---- device
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  double* part = static_cast<double*>(workspace);
+  const dim3 grid((d + kResTile - 1) / kResTile, (B + kResTile - 1) / kResTile);
+  if (x_is_half)
+    TRY(L.launch(nmf_residual_kernel<__half>, grid, 256, 0, static_cast<const __half*>(x), B, d, shift, w, k, h, part));
+  else
+    TRY(L.launch(nmf_residual_kernel<float>, grid, 256, 0, static_cast<const float*>(x), B, d, shift, w, k, h, part));
+  return L.launch(nmf_violation_kernel, 1, 256, 0, part, (int)(grid.x * grid.y), sum, nullptr, 0.0);
 }
 
 }  // extern "C"

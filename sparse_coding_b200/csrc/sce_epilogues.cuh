@@ -769,6 +769,67 @@ struct EpiIcaT {
   }
 };
 
+// ------------------------------------------------------------------------------------------------
+// NMF projection (sce_nmf_project): acc = p = M v of one row -> fp32 [rows][k] through EpiScoresTma's staging and bulk
+// stores; with `part`, per warp of 32 rows the column sums of max(p, 0)^2 and min(p, 0)^2 over the rows < m_total ->
+// part [row_block][2][k] (fp32; a second kernel adds them over the row blocks in a fixed order in fp64). NNDSVD reads
+// the norms of the positive and negative parts of X v_j from them.
+// ------------------------------------------------------------------------------------------------
+struct EpiNmfProject {
+  static constexpr int kCols = 32;
+  static constexpr int kWarpStageBytes = 4096;
+  struct Params {
+    CUtensorMap out;   // [1][rows][k] fp32, box 32 x 32
+    float* part;       // [ceil(rows / 32)][2][k], or nullptr
+  };
+  const Params& P;
+  const TileCoord& T;
+  int m_total, n_total;
+  uint8_t* stage;
+  __device__ EpiNmfProject(const Params& p, const TileCoord& t, int m, int n, uint8_t* st)
+      : P(p), T(t), m_total(m), n_total(n), stage(st) {}
+  __device__ __forceinline__ void chunk(int c, const uint32_t (&r)[32]) {
+    const int col = T.col0 + c;
+    if (col >= n_total) return;   // warp-uniform
+    const int row0 = T.m_blk * kBM + T.warp_q * 32;
+    staging_wait(T);
+    const int sw = T.lane & 7;
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      *reinterpret_cast<uint4*>(stage + T.lane * 128 + ((q ^ sw) << 4)) = make_uint4(r[4 * q], r[4 * q + 1], r[4 * q + 2], r[4 * q + 3]);
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (T.lane == 0) {
+      tma_store_3d(&P.out, stage, col, row0, T.model);
+      tma_store_commit();
+    }
+    if (P.part && row0 < m_total) {   // (warp-uniform) some row of this warp is in the batch
+      const bool row_ok = T.row < m_total;
+      float* o = P.part + (long long)(row0 >> 5) * 2 * n_total + col + T.lane;
+      float s[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const float v = row_ok ? __uint_as_float(r[j]) : 0.f;
+        s[j] = v > 0.f ? v * v : 0.f;
+      }
+      const float sp = warp_column_sum(s, T.lane);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        const float v = row_ok ? __uint_as_float(r[j]) : 0.f;
+        s[j] = v < 0.f ? v * v : 0.f;
+      }
+      const float sn = warp_column_sum(s, T.lane);
+      if (col + T.lane < n_total) {
+        o[0] = sp;
+        o[n_total] = sn;
+      }
+    }
+  }
+  __device__ __forceinline__ void finish() {
+    if (T.lane == 0) tma_store_wait_read();
+  }
+};
+
 using EpiEncode = EpiEncodeT<kArithBf16x3>;
 using EpiDecode = EpiDecodeT<kArithBf16x3>;
 using EpiDcode = EpiDcodeT<kArithBf16x3>;

@@ -1444,9 +1444,12 @@ static int run_similarity_t(Launcher& L, const SimOperand& A, const SimOperand& 
 }
 
 // ------------------------------------------------------------------------------------------------
-// sliced row passes: second moments (sce_second_moments, for BatchedPCA) and the FastICA pass (sce_ica_pass)
+// sliced row passes: second moments (sce_second_moments, for BatchedPCA), the FastICA pass (sce_ica_pass) and the NMF
+// projection and Grams (sce_nmf_project, sce_nmf_grams, for NMFEncoder)
 // ------------------------------------------------------------------------------------------------
-// Both end in a reduction over the rows, A^T V for the shifted rows V: the Gram matrix V^T V, or FastICA's T^T V. It is
+// Each splits the rows x, shifted by a vector (clamped at 0 for NMF), into operand planes (moment_split_kernel). All
+// but the projection end in a reduction over the rows, A^T V for the shifted rows V: the Gram matrix V^T V, FastICA's
+// T^T V, or NMF's W^T W and W^T V. It is
 // the weight gradient's GEMM (MN-major 16-bit planes, K = rows; f16f8 cross terms on E5M2 wgmma from batch-major copies
 // of the 8-bit planes, EpiStoreF32). The rows are cut into S slices of R rows, run as the GEMM's models, so that an
 // output of few tiles still fills the SMs; each slice leaves an fp32 partial, and the partials are added in slice order
@@ -1477,60 +1480,85 @@ static Slices mom_slices(int d, int B) {
   return {(B + R - 1) / R, R};
 }
 
-// The buffers of a row pass of width d: the second moments' (n = 0), the FastICA pass's with n components, which
-// alone take t, its copies, the unmix planes, the g' partials and the flag words, or (nmf) sce_nmf_grams' with k = n
-// codes, which takes W's planes and copies in t / tt, the W^T W partials and the flag words, but no column sums
+// the (d, B) of a row pass: rows of width d, a multiple of 8 in [8, 8192], and 1 <= B <= kMomCallRowsMax rows per call
+static bool row_shape_ok(int d, int B) { return d >= 8 && d % 8 == 0 && d <= 8192 && B >= 1 && B <= kMomCallRowsMax; }
+// the component count n of a pass over rows of width d (ICA's n, NMF's k): a multiple of 8 in [8, d]
+static bool components_ok(int n, int d) { return n >= 8 && n % 8 == 0 && n <= d; }
+
+// The rows a pass reads and where it runs: x [B][d] (fp16 when half, else fp32), shift [d], the f16f8 range flag (set
+// when a shifted row, or a matrix split beside them, holds a value the fp16 plane cannot), the device and its SMs
+struct RowArgs {
+  const void* x;
+  bool half;
+  int B, d;
+  const float* shift;
+  uint32_t* range_flag;
+  int device, sms;
+};
+
+enum RowPass { kPassMoments, kPassIca, kPassNmfProject, kPassNmfGrams };
+
+// The buffers of the row passes; each pass takes its own (row_carve). The projection runs one model of B rows padded
+// to kMomBlockRows (S = 1) and takes no batch-major copies.
 struct RowCarve {
   Planes x, xt;      // the shifted rows [S * R][d] (zero beyond B); f16f8: batch-major 8-bit copies [S][d][R]
-  Planes t, tt;      // ICA: t [S * R][n] (NMF: W); f16f8: batch-major 8-bit copies [S][n][R]
-  Planes w;          // ICA: unmix [n][d]
-  float* part;       // [S][n, or d][d] fp32 slice partials
-  float* part_g;     // NMF: [S][n][n] fp32 slice partials of W^T W
-  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (unused by ICA, not carved for NMF)
+  Planes t, tt;      // ICA: t [S * R][n]; NMF Grams: W [S * R][k]; f16f8: batch-major 8-bit copies [S][n][R]
+  Planes mat;        // ICA: unmix [n][d]; NMF projection: M [k][d]
+  float* part;       // [S][n, or d][d] fp32 slice partials; NMF projection: [ceil(B / 32)][2][k] column-norm partials
+  float* part_g;     // NMF Grams: [S][k][k] fp32 slice partials of W^T W
+  double* col_part;  // [S * R / kMomBlockRows][d]: the split kernel's column sums (second moments; ICA leaves them unread)
   float* g_part;     // ICA: [S * R / 32][n] g' partials
-  uint32_t* flags;   // ICA: kFlagWords, the f16f8 range check of unmix
+  uint32_t* flags;   // ICA, NMF: kFlagWords, the f16f8 range check of the matrix
 };
-// Carves S slices of `rows` (= S R) padded rows. The workspace query carves upper bounds of both instead, which never
-// decrease with B: the exact S is not monotone in B (at d = 512, B = 64000 takes 33 slices of 1984 rows, B = 65536 32
-// of 2048), and a caller sizes one workspace for its longest call.
-static size_t row_carve(uint8_t* base, bool f8, int d, int n, size_t S, size_t rows, RowCarve* out, bool nmf = false) {
-  const size_t dd = (size_t)d, nn = (size_t)n;
+// Carves the buffers `pass` takes, for S slices of `rows` (= S R) padded rows of a call of B rows with n components,
+// in the order of RowCarve; a buffer a pass does not take has no elements and carves nothing. The workspace query
+// carves upper bounds of S and rows instead, which never decrease with B: the exact S is not monotone in B (at d = 512,
+// B = 64000 takes 33 slices of 1984 rows, B = 65536 32 of 2048), and a caller sizes one workspace for its longest call.
+static size_t row_carve(uint8_t* base, RowPass pass, bool f8, int d, int n, int B, size_t S, size_t rows, RowCarve* out) {
+  const size_t dd = (size_t)d, nn = (size_t)n, col = rows / kMomBlockRows * dd;
+  struct {
+    size_t t, mat, part, part_g, col_part, g_part, flags;
+    bool copies;
+  } z{};
+  switch (pass) {   // t, mat, part, part_g, col_part, g_part, flags, copies
+    case kPassMoments: z = {0, 0, S * dd * dd, 0, col, 0, 0, true}; break;
+    case kPassIca: z = {rows * nn, nn * dd, S * nn * dd, 0, col, rows / 32 * nn, kFlagWords, true}; break;
+    case kPassNmfProject: z = {0, nn * dd, ((size_t)B + 31) / 32 * 2 * nn, 0, 0, 0, kFlagWords, false}; break;
+    case kPassNmfGrams: z = {rows * nn, 0, S * nn * dd, S * nn * nn, 0, 0, kFlagWords, true}; break;
+  }
   Carve c{base, 0};
   RowCarve w{};
   w.x = c.planes(rows * dd, f8);
-  if (n) w.t = c.planes(rows * nn, f8);
-  if (f8) {
+  w.t = c.planes(z.t, f8);
+  if (f8 && z.copies) {
     w.xt = c.copies(rows * dd);
-    if (n) w.tt = c.copies(rows * nn);
+    w.tt = c.copies(z.t);
   }
-  if (nmf) {
-    w.part = c.take<float>(S * nn * dd);
-    w.part_g = c.take<float>(S * nn * nn);
-    w.flags = c.take<uint32_t>(kFlagWords);
-    if (out) *out = w;
-    return align_up(c.off, 1024);
-  }
-  if (n) w.w = c.planes(nn * dd, f8);
-  w.part = c.take<float>(S * (n ? nn : dd) * dd);
-  w.col_part = c.take<double>(rows / kMomBlockRows * dd);
-  if (n) {
-    w.g_part = c.take<float>(rows / 32 * nn);
-    w.flags = c.take<uint32_t>(kFlagWords);
-  }
+  w.mat = c.planes(z.mat, f8);
+  w.part = c.take<float>(z.part);
+  w.part_g = c.take<float>(z.part_g);
+  w.col_part = c.take<double>(z.col_part);
+  w.g_part = c.take<float>(z.g_part);
+  w.flags = c.take<uint32_t>(z.flags);
   if (out) *out = w;
   return align_up(c.off, 1024);
 }
-// The workspace of a row pass, for both arithmetics; 0 when d or B is out of range. It carves the bounds of mom_slices,
-// non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts from), and S R < B + R <=
-// B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
-static size_t row_pass_workspace(int d, int n, int B, bool nmf = false) {
-  if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
-  const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
-  const size_t s_target = (kMomTargetTiles + tiles - 1) / tiles, s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
-  const size_t s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
-  const size_t S = std::max(std::min(s_target, s_short), s_rows);
-  const size_t rows = std::min(((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows + kMomRowsMax, S * kMomRowsMax);
-  return std::max(row_carve(nullptr, false, d, n, S, rows, nullptr, nmf), row_carve(nullptr, true, d, n, S, rows, nullptr, nmf));
+static size_t padded_rows(int B) { return ((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows; }
+// The workspace of a row pass, for both arithmetics; 0 when d, B or n is out of range. The sliced passes carve the
+// bounds of mom_slices, non-decreasing in B: S <= max(min(target, ceil(B / 256)), ceil(B / 2048)) (the s it starts
+// from), and S R < B + R <= B + 2048 with S R <= S kMomRowsMax; rows are a multiple of kMomBlockRows.
+static size_t row_pass_workspace(RowPass pass, int d, int n, int B) {
+  if (!row_shape_ok(d, B) || (pass != kPassMoments && !components_ok(n, d))) return 0;
+  size_t S = 1, rows = padded_rows(B);
+  if (pass != kPassNmfProject) {
+    const int tiles = ((d + kBM - 1) / kBM) * ((d + kBN - 1) / kBN);
+    const size_t s_target = (kMomTargetTiles + tiles - 1) / tiles, s_short = (B + kMomSliceMin - 1) / kMomSliceMin;
+    const size_t s_rows = (B + kMomRowsMax - 1) / kMomRowsMax;
+    S = std::max(std::min(s_target, s_short), s_rows);
+    rows = std::min(rows + kMomRowsMax, S * kMomRowsMax);
+  }
+  return std::max(row_carve(nullptr, pass, false, d, n, B, S, rows, nullptr),
+                  row_carve(nullptr, pass, true, d, n, B, S, rows, nullptr));
 }
 
 // rows r0 .. r0 + 63 of the call (grid.y), four columns per thread (grid.x covers d / 4 threads):
@@ -1594,29 +1622,31 @@ __global__ void __launch_bounds__(128) moment_split_kernel(const InT* __restrict
   if (bad && range_flag) *range_flag = 1u;   // benign race: all write 1
 }
 
-// gram[i] += sum over the slices s, in order, of part[s][i] (an n x d output: n4 = n d / 4, n d >= 4 d); and with
-// col_part, col_sum[j] += sum over the row blocks b, in order, of col_part[b][j] (j < d); with vec_part (sce_ica_pass's
-// g' sums, fp32 per 32 rows), vec_sum[j] += the same over its vec_blocks row blocks (j < n). fp64 throughout; four Gram
-// entries per thread.
+// gram[i] += sum over the slices s, in order, of part[s][i] (an n x d output: n4 = n d / 4, n d >= 4 d; none with
+// n4 = 0); with col_part, col_sum[j] += sum over the row blocks b, in order, of col_part[b][j] (j < d); with vec_part
+// (fp32 row-block partials: sce_ica_pass's g' sums per 32 rows, sce_nmf_project's column norms), vec_sum[j] += the
+// same over its vec_blocks row blocks (j < n). fp64 throughout; four Gram entries per thread.
 __global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restrict__ part, int S, long long n4,
                                                             double* __restrict__ gram, const double* __restrict__ col_part,
                                                             int blocks, int d, double* __restrict__ col_sum,
                                                             const float* __restrict__ vec_part, int vec_blocks, int n,
                                                             double* __restrict__ vec_sum) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
-    for (int s = 0; s < S; ++s) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(part) + (long long)s * n4 + i);
-      a0 += v.x;
-      a1 += v.y;
-      a2 += v.z;
-      a3 += v.w;
+  const long long stride = (long long)gridDim.x * blockDim.x, end = n4 > n ? n4 : n;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+    if (i < n4) {
+      double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+      for (int s = 0; s < S; ++s) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(part) + (long long)s * n4 + i);
+        a0 += v.x;
+        a1 += v.y;
+        a2 += v.z;
+        a3 += v.w;
+      }
+      double2* g = reinterpret_cast<double2*>(gram) + 2 * i;
+      const double2 g0 = g[0], g1 = g[1];
+      g[0] = make_double2(g0.x + a0, g0.y + a1);
+      g[1] = make_double2(g1.x + a2, g1.y + a3);
     }
-    double2* g = reinterpret_cast<double2*>(gram) + 2 * i;
-    const double2 g0 = g[0], g1 = g[1];
-    g[0] = make_double2(g0.x + a0, g0.y + a1);
-    g[1] = make_double2(g1.x + a2, g1.y + a3);
     if (col_part && i < d) {
       double t = 0.0;
       for (int b = 0; b < blocks; ++b) t += col_part[(long long)b * d + i];
@@ -1630,25 +1660,44 @@ __global__ void __launch_bounds__(256) gram_reduce_kernel(const float* __restric
   }
 }
 
-// moment_split_kernel over the S R rows of a call: the shifted rows into the planes of w.x, the column-sum partials and,
-// with f16f8, the range flag
+// gram_reduce_kernel: out += the S slice partials `part` of n4 float4s, col_sum [d] += the column sums col_part of
+// `blocks` row blocks, vec_sum [n] += the vec_blocks row-block partials vec_part (each only where given)
+static int reduce_partials(Launcher& L, const float* part, int S, long long n4, double* out,
+                           const double* col_part = nullptr, int blocks = 0, int d = 0, double* col_sum = nullptr,
+                           const float* vec_part = nullptr, int vec_blocks = 0, int n = 0, double* vec_sum = nullptr) {
+  const long long items = n4 > n ? n4 : n;
+  const int rblocks = (int)((items + 255) / 256 < 2048 ? (items + 255) / 256 : 2048);
+  return L.launch(gram_reduce_kernel, rblocks, 256, 0, part, S, n4, out, col_part, blocks, d, col_sum, vec_part,
+                  vec_blocks, n, vec_sum);
+}
+
+// moment_split_kernel over the S R rows of a call: the shifted rows into the planes of w.x, the column-sum partials
+// (not with CLAMP) and, with f16f8, the range flag
 template <int AR, bool CLAMP = false>
-static int launch_row_split(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const Slices& sl,
-                            const RowCarve& w, uint32_t* range_flag) {
-  const dim3 grid((d / 4 + 127) / 128, sl.S * sl.R / kMomBlockRows);
-  uint32_t* flag = AR == kArithF16F8 ? range_flag : nullptr;
-  if constexpr (CLAMP) {
-    if (half)
-      return L.launch(moment_split_kernel<AR, __half, true>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift,
-                      w.x.hi, w.x.lo, w.x.x8, nullptr, flag);
-    return L.launch(moment_split_kernel<AR, float, true>, grid, 128, 0, static_cast<const float*>(x), B, d, shift,
-                    w.x.hi, w.x.lo, w.x.x8, nullptr, flag);
+static int launch_row_split(Launcher& L, const RowArgs& a, const Slices& sl, const RowCarve& w) {
+  const dim3 grid((a.d / 4 + 127) / 128, sl.S * sl.R / kMomBlockRows);
+  uint32_t* flag = AR == kArithF16F8 ? a.range_flag : nullptr;
+  auto split = [&](auto* x) {
+    return L.launch(moment_split_kernel<AR, std::decay_t<decltype(*x)>, CLAMP>, grid, 128, 0, x, a.B, a.d, a.shift,
+                    w.x.hi, w.x.lo, w.x.x8, CLAMP ? nullptr : w.col_part, flag);
+  };
+  return a.half ? split(static_cast<const __half*>(a.x)) : split(static_cast<const float*>(a.x));
+}
+
+__global__ void set_flag_if_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
+  if (*src) *dst = 1u;
+}
+
+// fp32 matrix [count / its width] -> planes; f16f8: its range check joins the rows' in range_flag
+template <int AR>
+static int split_matrix(Launcher& L, const float* m, const Planes& planes, long long count, uint32_t* flags,
+                        uint32_t* range_flag) {
+  if (AR == kArithF16F8 && range_flag) {
+    CUDA_TRY(cudaMemsetAsync(flags, 0, kFlagWords * sizeof(uint32_t), L.st));
+    TRY(launch_split_rows<AR>(L, m, planes, count / 4, flags));
+    return L.launch(set_flag_if_kernel, 1, 1, 0, flags + kBadWord, range_flag);
   }
-  if (half)
-    return L.launch(moment_split_kernel<AR, __half>, grid, 128, 0, static_cast<const __half*>(x), B, d, shift, w.x.hi,
-                    w.x.lo, w.x.x8, w.col_part, flag);
-  return L.launch(moment_split_kernel<AR, float>, grid, 128, 0, static_cast<const float*>(x), B, d, shift, w.x.hi, w.x.lo,
-                  w.x.x8, w.col_part, flag);
+  return launch_split_rows<AR>(L, m, planes, count / 4, nullptr);
 }
 
 // part[s] = A_s^T V_s (fp32 [S][m][d]) for the slices s of R rows of A [S R][m] and V [S R][d]: the weight gradient's
@@ -1678,22 +1727,13 @@ static int sliced_gemm_t(Launcher& L, const Slices& sl, const Planes& A, const P
   return launch_dw_t<AR>(L, f8, S, device, sms, maps, 1, kOnes, kOnes, R, 3, m, d, sp);
 }
 
-// out [n, or d][d] += the slice partials of a row pass of B rows; second moments (n = 0): col_sum += the split's
-// column sums; ICA: g_sum += the g' partials
-static int reduce_rows(Launcher& L, const RowCarve& w, int B, int S, int n, int d, double* out, double* col_sum,
-                       double* g_sum) {
-  const long long n4 = (long long)(n ? n : d) * d / 4;
-  const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  return L.launch(gram_reduce_kernel, rblocks, 256, 0, w.part, S, n4, out, n ? nullptr : w.col_part,
-                  (B + kMomBlockRows - 1) / kMomBlockRows, d, col_sum, w.g_part, (B + 31) / 32, n, g_sum);
-}
-
 template <int AR>
-static int run_moments_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const Slices& sl,
-                         const RowCarve& w, double* col_sum, double* gram, uint32_t* range_flag, int device, int sms) {
-  TRY(launch_row_split<AR>(L, x, half, B, d, shift, sl, w, range_flag));
-  TRY(sliced_gemm_t<AR>(L, sl, w.x, w.xt, d, w.x, w.xt, d, w.part, device, sms));
-  return reduce_rows(L, w, B, sl.S, 0, d, gram, col_sum, nullptr);
+static int run_moments_t(Launcher& L, const RowArgs& a, const Slices& sl, const RowCarve& w, double* col_sum,
+                         double* gram) {
+  TRY(launch_row_split<AR>(L, a, sl, w));
+  TRY(sliced_gemm_t<AR>(L, sl, w.x, w.xt, a.d, w.x, w.xt, a.d, w.part, a.device, a.sms));
+  return reduce_partials(L, w.part, sl.S, (long long)a.d * a.d / 4, gram, w.col_part,
+                         (a.B + kMomBlockRows - 1) / kMomBlockRows, a.d, col_sum);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1703,32 +1743,20 @@ static int run_moments_t(Launcher& L, const void* x, bool half, int B, int d, co
 // split and sliced as for the second moments (launch_row_split: zero padding rows, the range flag). GEMM 1, U = V
 // unmix^T, is the encode geometry (both operands K-major over d) as one model of S R rows, with EpiIcaT writing the
 // planes of t and the g' partials; GEMM 2, gx = T^T V per slice, is sliced_gemm_t with T in place of the first V.
-__global__ void set_flag_if_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
-  if (*src) *dst = 1u;
-}
-
 template <int AR>
-static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* unmix, int n,
-                     float alpha, const Slices& sl, const RowCarve& w, double* g_sum, double* gx, uint32_t* range_flag,
-                     int device, int sms) {
+static int run_ica_t(Launcher& L, const RowArgs& a, const Slices& sl, const RowCarve& w, const float* unmix, int n,
+                     float alpha, double* g_sum, double* gx) {
   constexpr bool f8 = AR == kArithF16F8;
-  const int rows = sl.S * sl.R;
-  TRY(launch_row_split<AR>(L, x, half, B, d, shift, sl, w, range_flag));
-  // unmix -> planes (sce_similarity's raw split); f16f8: its range check joins the rows' in range_flag
-  if (f8 && range_flag) {
-    CUDA_TRY(cudaMemsetAsync(w.flags, 0, kFlagWords * sizeof(uint32_t), L.st));
-    TRY(launch_split_rows<AR>(L, unmix, w.w, (long long)n * d / 4, w.flags));
-    TRY(L.launch(set_flag_if_kernel, 1, 1, 0, w.flags + kBadWord, range_flag));
-  } else {
-    TRY(launch_split_rows<AR>(L, unmix, w.w, (long long)n * d / 4, nullptr));
-  }
+  const int rows = sl.S * sl.R, d = a.d;
+  TRY(launch_row_split<AR>(L, a, sl, w));
+  TRY(split_matrix<AR>(L, unmix, w.mat, (long long)n * d, w.flags, a.range_flag));   // sce_similarity's raw split
   const uint64_t rows64 = rows, d64 = d, n64 = n;
   const int bk = gemm_bk(AR);
   // ---- GEMM 1: U = V unmix^T, t = tanh(alpha U) -> planes of t, g' partials
   GemmMaps m1{};
   typename EpiIcaT<AR>::Params ep;
   bool ok = operand_maps(m1.a[0], w.x, 1, rows64, d64, rows64 * d64, kBM, bk) &&
-            operand_maps(m1.b[0], w.w, 1, n64, d64, n64 * d64, kBN, bk) &&
+            operand_maps(m1.b[0], w.mat, 1, n64, d64, n64 * d64, kBN, bk) &&
             make_tmap_bf16_store32(&ep.out_hi, w.t.hi, 1, rows64, n64, rows64 * n64);
   if constexpr (f8)
     ok = ok && make_tmap_u8_box(&ep.out_lo, w.t.lo, 1, rows64, n64, n64, rows64 * n64, 32, 32, CU_TENSOR_MAP_SWIZZLE_32B) &&
@@ -1738,22 +1766,27 @@ static int run_ica_t(Launcher& L, const void* x, bool half, int B, int d, const 
   if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (ica pass: d=%d, n=%d, %d rows)", d, n, rows);
   ep.g_part = w.g_part;
   ep.alpha = alpha;
-  ep.rows_valid = B;
-  TRY((launch_gemm_t<EpiIcaT<AR>, false, false, false, AR, f8>(L, 1, device, sms, m1, 1, kOnes, kOnes, d, 3, rows, n, ep)));
+  ep.rows_valid = a.B;
+  TRY((launch_gemm_t<EpiIcaT<AR>, false, false, false, AR, f8>(L, 1, a.device, a.sms, m1, 1, kOnes, kOnes, d, 3, rows, n,
+                                                                 ep)));
   // ---- GEMM 2: gx partials [S][n][d] = T^T V per slice
-  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, n, w.x, w.xt, d, w.part, device, sms));
-  return reduce_rows(L, w, B, sl.S, n, d, gx, nullptr, g_sum);
+  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, n, w.x, w.xt, d, w.part, a.device, a.sms));
+  return reduce_partials(L, w.part, sl.S, (long long)n * d / 4, gx, nullptr, 0, 0, nullptr, w.g_part, (a.B + 31) / 32, n,
+                         g_sum);
 }
 
-// The checks the row passes share, made before any CUDA call (`n`: ICA's or NMF's, or 0): the rows x [B][d], fp16 or
-// fp32, and shift [d], 16-byte aligned; the arithmetic. With `mat_name` (the NMF passes), also the fp32 matrix `mat` of
-// n rows (M [n][d] or W [B][n]): present and 16-byte aligned, n a multiple of 8 in [8, d].
-static int check_row_pass(const char* prefix, const void* x, int x_is_half, int B, int d, const float* shift, int n,
-                          int arith, const float* mat = nullptr, const char* mat_name = nullptr) {
+// The checks the row passes share, made before any CUDA call: the rows x [B][d], fp16 or fp32, and shift [d], 16-byte
+// aligned; the arithmetic (with n components, 0 for the second moments). With `mat_name`, also the fp32 matrix `mat`
+// with n rows or columns (ICA's unmix [n][d], NMF's M [k][d] or W [B][k]): present and 16-byte aligned, and n (named
+// `n_name`) a multiple of 8 in [8, d].
+static int check_row_pass(const char* prefix, const void* x, int x_is_half, int B, int d, const float* shift, int arith,
+                          int n = 0, const char* n_name = nullptr, const float* mat = nullptr,
+                          const char* mat_name = nullptr) {
   if (!x || !shift) return fail(SCE_ERR_INVALID, "%sx and shift are required", prefix);
   if (x_is_half != 0 && x_is_half != 1) return fail(SCE_ERR_INVALID, "%sx_is_half must be 0 or 1", prefix);
-  if (B < 1 || B > kMomCallRowsMax) return fail(SCE_ERR_INVALID, "%sB = %d outside [1, %d]", prefix, B, kMomCallRowsMax);
-  if (d < 8 || d % 8 || d > 8192) return fail(SCE_ERR_INVALID, "%sd (%d) must be a multiple of 8 in [8, 8192]", prefix, d);
+  if (!row_shape_ok(d, B))
+    return row_shape_ok(8, B) ? fail(SCE_ERR_INVALID, "%sd (%d) must be a multiple of 8 in [8, 8192]", prefix, d)
+                              : fail(SCE_ERR_INVALID, "%sB = %d outside [1, %d]", prefix, B, kMomCallRowsMax);
   if (arith < SCE_ARITH_AUTO || arith > SCE_ARITH_F16F8) return fail(SCE_ERR_INVALID, "%sunknown arith %d", prefix, arith);
   if (arith == SCE_ARITH_F16F8 && (d % 16 || n % 16))
     return n ? fail(SCE_ERR_INVALID, "%sarith = F16F8 needs d (%d) and n (%d) to be multiples of 16", prefix, d, n)
@@ -1762,10 +1795,25 @@ static int check_row_pass(const char* prefix, const void* x, int x_is_half, int 
     return fail(SCE_ERR_INVALID, "%sx and shift must be 16-byte aligned", prefix);
   if (mat_name) {
     if (!mat) return fail(SCE_ERR_INVALID, "%s%s is required", prefix, mat_name);
-    if (n < 8 || n % 8 || n > d) return fail(SCE_ERR_INVALID, "%sk (%d) must be a multiple of 8 in [8, d = %d]", prefix, n, d);
+    if (!components_ok(n, d))
+      return fail(SCE_ERR_INVALID, "%s%s (%d) must be a multiple of 8 in [8, d = %d]", prefix, n_name, n, d);
     if (reinterpret_cast<uintptr_t>(mat) % 16) return fail(SCE_ERR_INVALID, "%s%s must be 16-byte aligned", prefix, mat_name);
   }
   return SCE_OK;
+}
+
+// The prologue every row pass runs after its argument checks: the device, the arithmetic (AUTO: bf16x3, the fp32 range
+// and no range check, as sce_similarity), the slices (the projection: one of B rows padded to kMomBlockRows) and the
+// carve of the workspace. Then body(AR, L, a, sl, w), with the arithmetic as a compile-time constant.
+template <class F>
+static int row_pass(RowPass pass, RowArgs a, int n, int arith, void* workspace, void* stream, F&& body) {
+  TRY(query_device(&a.device, &a.sms));
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  const bool f8 = arith == SCE_ARITH_F16F8;
+  const Slices sl = pass == kPassNmfProject ? Slices{1, (int)padded_rows(a.B)} : mom_slices(a.d, a.B);
+  RowCarve w;
+  row_carve(static_cast<uint8_t*>(workspace), pass, f8, a.d, n, a.B, sl.S, (size_t)sl.S * sl.R, &w);
+  return with_arith(f8 ? kArithF16F8 : kArithBf16x3, [&](auto ar) { return body(ar, L, a, sl, w); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1775,90 +1823,45 @@ static int check_row_pass(const char* prefix, const void* x, int x_is_half, int 
 // Projection: for v = max(x - shift, 0) and an fp32 M [k][d], P = v M^T, fp32 [B][k]. The rows are split as for the row
 // passes (CLAMP) into one model of B rows padded to kMomBlockRows; the GEMM is the encode geometry (both operands K-major
 // over d), its epilogue EpiNmfProject stores P and, optionally, the per-32-row partials of the squared positive and
-// negative parts of each column, which nmf_col_reduce_kernel adds up over the row blocks in order in fp64.
-struct NmfProjectCarve {
-  Planes x, m;       // v [rows][d], M [k][d]
-  float* part;       // [ceil(B / 32)][2][k]
-  uint32_t* flags;   // kFlagWords: the f16f8 range check of M
-};
-static size_t nmf_project_carve(uint8_t* base, bool f8, int d, int k, int B, NmfProjectCarve* out) {
-  const size_t rows = ((size_t)B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows;
-  Carve c{base, 0};
-  NmfProjectCarve w{};
-  w.x = c.planes(rows * d, f8);
-  w.m = c.planes((size_t)k * d, f8);
-  w.part = c.take<float>(((size_t)B + 31) / 32 * 2 * k);
-  w.flags = c.take<uint32_t>(kFlagWords);
-  if (out) *out = w;
-  return align_up(c.off, 1024);
-}
-
-// sums[j] += sum over the row blocks b, in order, of part[b][j], j < n (fp64)
-__global__ void nmf_col_reduce_kernel(const float* __restrict__ part, int blocks, int n, double* __restrict__ sums) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  double a = 0.0;
-  for (int b = 0; b < blocks; ++b) a += (double)__ldg(part + (long long)b * n + j);
-  sums[j] += a;
-}
-
-// fp32 M [k][d] -> planes; f16f8: its range check joins the rows' in range_flag
+// negative parts of each column, which gram_reduce_kernel adds up over the row blocks in order in fp64.
 template <int AR>
-static int split_matrix(Launcher& L, const float* m, const Planes& planes, long long count, uint32_t* flags,
-                        uint32_t* range_flag) {
-  if (AR == kArithF16F8 && range_flag) {
-    CUDA_TRY(cudaMemsetAsync(flags, 0, kFlagWords * sizeof(uint32_t), L.st));
-    TRY(launch_split_rows<AR>(L, m, planes, count / 4, flags));
-    return L.launch(set_flag_if_kernel, 1, 1, 0, flags + kBadWord, range_flag);
-  }
-  return launch_split_rows<AR>(L, m, planes, count / 4, nullptr);
-}
-
-template <int AR>
-static int run_nmf_project_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* m,
-                             int k, float* p, double* norms, const NmfProjectCarve& w, uint32_t* range_flag, int device,
-                             int sms) {
+static int run_nmf_project_t(Launcher& L, const RowArgs& a, const Slices& sl, const RowCarve& w, const float* m, int k,
+                             float* p, double* norms) {
   constexpr bool f8 = AR == kArithF16F8;
-  const int rows = (B + kMomBlockRows - 1) / kMomBlockRows * kMomBlockRows;
-  RowCarve rc{};
-  rc.x = w.x;
-  TRY((launch_row_split<AR, true>(L, x, half, B, d, shift, Slices{1, rows}, rc, range_flag)));
-  TRY(split_matrix<AR>(L, m, w.m, (long long)k * d, w.flags, range_flag));
+  const int B = a.B, d = a.d;
+  TRY((launch_row_split<AR, true>(L, a, sl, w)));
+  TRY(split_matrix<AR>(L, m, w.mat, (long long)k * d, w.flags, a.range_flag));
   const int bk = gemm_bk(AR);
   GemmMaps maps{};
   EpiNmfProject::Params ep;
   bool ok = operand_maps(maps.a[0], w.x, 1, (uint64_t)B, (uint64_t)d, (uint64_t)B * d, kBM, bk) &&
-            operand_maps(maps.b[0], w.m, 1, (uint64_t)k, (uint64_t)d, (uint64_t)k * d, kBN, bk) &&
+            operand_maps(maps.b[0], w.mat, 1, (uint64_t)k, (uint64_t)d, (uint64_t)k * d, kBN, bk) &&
             make_tmap_f32_store32(&ep.out, p, 1, (uint64_t)B, (uint64_t)k, (uint64_t)B * k);
   if (!ok) return fail(SCE_ERR_CUDA, "cuTensorMapEncodeTiled failed (nmf project: d=%d, k=%d, B=%d)", d, k, B);
   ep.part = norms ? w.part : nullptr;
-  TRY((launch_gemm_t<EpiNmfProject, false, false, false, AR, f8>(L, 1, device, sms, maps, 1, kOnes, kOnes, d, 3, B, k, ep)));
+  TRY((launch_gemm_t<EpiNmfProject, false, false, false, AR, f8>(L, 1, a.device, a.sms, maps, 1, kOnes, kOnes, d, 3, B,
+                                                                   k, ep)));
   if (!norms) return SCE_OK;
-  return L.launch(nmf_col_reduce_kernel, (2 * k + 255) / 256, 256, 0, w.part, (B + 31) / 32, 2 * k, norms);
+  return reduce_partials(L, nullptr, 0, 0, nullptr, nullptr, 0, 0, nullptr, w.part, (B + 31) / 32, 2 * k, norms);
 }
 
 // Gram matrices: for v as above and an fp32 W [B][k], wtw += W^T W and wtv += W^T v (fp64). The sliced row reduction of
 // the second moments: v and W are split into the planes of S slices of R rows (padding rows zero), each slice's two
 // products run on the weight gradient's GEMM (sliced_gemm_t: W^T W with A = V = W, then W^T v), and gram_reduce_kernel
 // adds the slice partials in slice order in fp64.
-static int reduce_slices(Launcher& L, const float* part, int S, long long n4, double* out) {
-  const int rblocks = (int)((n4 + 255) / 256 < 2048 ? (n4 + 255) / 256 : 2048);
-  return L.launch(gram_reduce_kernel, rblocks, 256, 0, part, S, n4, out, nullptr, 0, 0, nullptr, nullptr, 0, 0, nullptr);
+template <int AR>
+static int run_nmf_grams_t(Launcher& L, const RowArgs& a, const Slices& sl, const RowCarve& w, const float* wm, int k,
+                           double* wtw, double* wtv) {
+  const long long rows = (long long)sl.S * sl.R;
+  TRY((launch_row_split<AR, true>(L, a, sl, w)));
+  TRY(split_matrix<AR>(L, wm, w.t, (long long)a.B * k, w.flags, a.range_flag));
+  if (rows > a.B) CUDA_TRY(w.t.at((size_t)a.B * k).zero((size_t)(rows - a.B) * k, L.st));
+  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, k, w.t, w.tt, k, w.part_g, a.device, a.sms));
+  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, k, w.x, w.xt, a.d, w.part, a.device, a.sms, true));   // W's copies: made above
+  TRY(reduce_partials(L, w.part_g, sl.S, (long long)k * k / 4, wtw));
+  return reduce_partials(L, w.part, sl.S, (long long)k * a.d / 4, wtv);
 }
 
-template <int AR>
-static int run_nmf_grams_t(Launcher& L, const void* x, bool half, int B, int d, const float* shift, const float* wm,
-                           int k, const Slices& sl, const RowCarve& w, double* wtw, double* wtv, uint32_t* range_flag,
-                           int device, int sms) {
-  const long long rows = (long long)sl.S * sl.R;
-  TRY((launch_row_split<AR, true>(L, x, half, B, d, shift, sl, w, range_flag)));
-  TRY(split_matrix<AR>(L, wm, w.t, (long long)B * k, w.flags, range_flag));
-  if (rows > B) CUDA_TRY(w.t.at((size_t)B * k).zero((size_t)(rows - B) * k, L.st));
-  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, k, w.t, w.tt, k, w.part_g, device, sms));
-  TRY(sliced_gemm_t<AR>(L, sl, w.t, w.tt, k, w.x, w.xt, d, w.part, device, sms, true));   // W's copies: made above
-  TRY(reduce_slices(L, w.part_g, sl.S, (long long)k * k / 4, wtw));
-  return reduce_slices(L, w.part, sl.S, (long long)k * d / 4, wtv);
-}
 
 // One coordinate-descent sweep (sklearn's _update_cdnmf_fast, coordinates in order, no regularisation) over the rows
 // of W [R][k], with G [k][k] and L [R][k] fixed: for t = 0 .. k-1, per row i,
@@ -2695,57 +2698,33 @@ int sce_similarity(const float* a, int ma, int na, const int* a_rows, float a_no
             : run_similarity_t<kArithBf16x3>(L, A, B, b_is_a, d, n_pairs, w, row_max, col_max, capacity, dev, sms);
 }
 
-size_t sce_second_moments_workspace_bytes(int d, int B) { return row_pass_workspace(d, 0, B); }
+size_t sce_second_moments_workspace_bytes(int d, int B) { return row_pass_workspace(kPassMoments, d, 0, B); }
 
 int sce_second_moments(const void* x, int x_is_half, int B, int d, const float* shift, int arith, double* col_sum,
                        double* gram, unsigned int* range_flag, void* workspace, size_t workspace_bytes, void* stream) {
   // ---- arguments (all checked before any CUDA call)
   if (!col_sum || !gram) return fail(SCE_ERR_INVALID, "second_moments: col_sum and gram are required");
-  TRY(check_row_pass("second_moments: ", x, x_is_half, B, d, shift, 0, arith));
+  TRY(check_row_pass("second_moments: ", x, x_is_half, B, d, shift, arith));
   if (reinterpret_cast<uintptr_t>(gram) % 16) return fail(SCE_ERR_INVALID, "second_moments: gram must be 16-byte aligned");
   TRY(check_workspace(workspace, workspace_bytes, sce_second_moments_workspace_bytes(d, B), "second_moments: "));
-
-  // ---- device
-  int dev = 0, sms = 0;
-  if (int rc = query_device(&dev, &sms)) return rc;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  // AUTO: bf16x3, as sce_similarity: the fp32 range, no range check
-  const bool f8 = arith == SCE_ARITH_F16F8;
-  const Slices sl = mom_slices(d, B);
-  RowCarve w;
-  row_carve(static_cast<uint8_t*>(workspace), f8, d, 0, sl.S, (size_t)sl.S * sl.R, &w);
-  return f8 ? run_moments_t<kArithF16F8>(L, x, x_is_half, B, d, shift, sl, w, col_sum, gram, range_flag, dev, sms)
-            : run_moments_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, sl, w, col_sum, gram, range_flag, dev, sms);
+  return row_pass(kPassMoments, {x, x_is_half == 1, B, d, shift, range_flag}, 0, arith, workspace, stream,
+                  [&](auto ar, auto&... r) { return run_moments_t<decltype(ar)::value>(r..., col_sum, gram); });
 }
 
-size_t sce_ica_pass_workspace_bytes(int d, int n, int B) {
-  return n < 8 || n % 8 || n > d ? 0 : row_pass_workspace(d, n, B);
-}
+size_t sce_ica_pass_workspace_bytes(int d, int n, int B) { return row_pass_workspace(kPassIca, d, n, B); }
 
 int sce_ica_pass(const void* x, int x_is_half, int B, int d, const float* shift, const float* unmix, int n, float alpha,
                  int arith, double* g_sum, double* gx, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
                  void* stream) {
   // ---- arguments (all checked before any CUDA call)
-  if (!unmix || !g_sum || !gx) return fail(SCE_ERR_INVALID, "ica_pass: unmix, g_sum and gx are required");
-  TRY(check_row_pass("ica_pass: ", x, x_is_half, B, d, shift, n, arith));
-  if (n < 8 || n % 8 || n > d) return fail(SCE_ERR_INVALID, "ica_pass: n (%d) must be a multiple of 8 in [8, d = %d]", n, d);
+  if (!g_sum || !gx) return fail(SCE_ERR_INVALID, "ica_pass: g_sum and gx are required");
+  TRY(check_row_pass("ica_pass: ", x, x_is_half, B, d, shift, arith, n, "n", unmix, "unmix"));
   if (!(alpha >= 1.f && alpha <= 2.f)) return fail(SCE_ERR_INVALID, "ica_pass: alpha (%g) must be in [1, 2]", (double)alpha);
-  if (reinterpret_cast<uintptr_t>(unmix) % 16 || reinterpret_cast<uintptr_t>(gx) % 16 ||
-      reinterpret_cast<uintptr_t>(g_sum) % 8)
-    return fail(SCE_ERR_INVALID, "ica_pass: unmix and gx must be 16-byte aligned, g_sum 8-byte aligned");
+  if (reinterpret_cast<uintptr_t>(gx) % 16 || reinterpret_cast<uintptr_t>(g_sum) % 8)
+    return fail(SCE_ERR_INVALID, "ica_pass: gx must be 16-byte aligned, g_sum 8-byte aligned");
   TRY(check_workspace(workspace, workspace_bytes, sce_ica_pass_workspace_bytes(d, n, B), "ica_pass: "));
-
-  // ---- device
-  int dev = 0, sms = 0;
-  if (int rc = query_device(&dev, &sms)) return rc;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  // AUTO: bf16x3, as sce_second_moments
-  const bool f8 = arith == SCE_ARITH_F16F8;
-  const Slices sl = mom_slices(d, B);
-  RowCarve w;
-  row_carve(static_cast<uint8_t*>(workspace), f8, d, n, sl.S, (size_t)sl.S * sl.R, &w);
-  return f8 ? run_ica_t<kArithF16F8>(L, x, x_is_half, B, d, shift, unmix, n, alpha, sl, w, g_sum, gx, range_flag, dev, sms)
-            : run_ica_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, unmix, n, alpha, sl, w, g_sum, gx, range_flag, dev, sms);
+  return row_pass(kPassIca, {x, x_is_half == 1, B, d, shift, range_flag}, n, arith, workspace, stream,
+                  [&](auto ar, auto&... r) { return run_ica_t<decltype(ar)::value>(r..., unmix, n, alpha, g_sum, gx); });
 }
 
 int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int group_rows, long long row0, int B,
@@ -2780,57 +2759,34 @@ int sce_synth_rows(const float* feats, int n_gt, int d, const float* probs, int 
 }
 
 
-size_t sce_nmf_project_workspace_bytes(int d, int k, int B) {
-  if (d < 8 || d % 8 || d > 8192 || k < 8 || k % 8 || k > d || B < 1 || B > kMomCallRowsMax) return 0;
-  return std::max(nmf_project_carve(nullptr, false, d, k, B, nullptr), nmf_project_carve(nullptr, true, d, k, B, nullptr));
-}
+size_t sce_nmf_project_workspace_bytes(int d, int k, int B) { return row_pass_workspace(kPassNmfProject, d, k, B); }
 
 int sce_nmf_project(const void* x, int x_is_half, int B, int d, const float* shift, const float* m, int k, int arith,
                     float* p, double* norms, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
                     void* stream) {
   // ---- arguments (all checked before any CUDA call)
   if (!p) return fail(SCE_ERR_INVALID, "nmf_project: p is required");
-  TRY(check_row_pass("nmf_project: ", x, x_is_half, B, d, shift, k, arith, m, "m"));
+  TRY(check_row_pass("nmf_project: ", x, x_is_half, B, d, shift, arith, k, "k", m, "m"));
   if (reinterpret_cast<uintptr_t>(p) % 16 || reinterpret_cast<uintptr_t>(norms) % 8)
     return fail(SCE_ERR_INVALID, "nmf_project: p must be 16-byte aligned, norms 8-byte aligned");
   TRY(check_workspace(workspace, workspace_bytes, sce_nmf_project_workspace_bytes(d, k, B), "nmf_project: "));
-
-  // ---- device
-  int dev = 0, sms = 0;
-  if (int rc = query_device(&dev, &sms)) return rc;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  // AUTO: bf16x3, as the row passes
-  const bool f8 = arith == SCE_ARITH_F16F8;
-  NmfProjectCarve w;
-  nmf_project_carve(static_cast<uint8_t*>(workspace), f8, d, k, B, &w);
-  return f8 ? run_nmf_project_t<kArithF16F8>(L, x, x_is_half, B, d, shift, m, k, p, norms, w, range_flag, dev, sms)
-            : run_nmf_project_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, m, k, p, norms, w, range_flag, dev, sms);
+  return row_pass(kPassNmfProject, {x, x_is_half == 1, B, d, shift, range_flag}, k, arith, workspace, stream,
+                  [&](auto ar, auto&... r) { return run_nmf_project_t<decltype(ar)::value>(r..., m, k, p, norms); });
 }
 
-size_t sce_nmf_grams_workspace_bytes(int d, int k, int B) {
-  return k < 8 || k % 8 || k > d ? 0 : row_pass_workspace(d, k, B, true);
-}
+size_t sce_nmf_grams_workspace_bytes(int d, int k, int B) { return row_pass_workspace(kPassNmfGrams, d, k, B); }
 
 int sce_nmf_grams(const void* x, int x_is_half, int B, int d, const float* shift, const float* w, int k, int arith,
                   double* wtw, double* wtv, unsigned int* range_flag, void* workspace, size_t workspace_bytes,
                   void* stream) {
   // ---- arguments (all checked before any CUDA call)
   if (!wtw || !wtv) return fail(SCE_ERR_INVALID, "nmf_grams: wtw and wtv are required");
-  TRY(check_row_pass("nmf_grams: ", x, x_is_half, B, d, shift, k, arith, w, "w"));
+  TRY(check_row_pass("nmf_grams: ", x, x_is_half, B, d, shift, arith, k, "k", w, "w"));
   if (reinterpret_cast<uintptr_t>(wtw) % 16 || reinterpret_cast<uintptr_t>(wtv) % 16)
     return fail(SCE_ERR_INVALID, "nmf_grams: wtw and wtv must be 16-byte aligned");
   TRY(check_workspace(workspace, workspace_bytes, sce_nmf_grams_workspace_bytes(d, k, B), "nmf_grams: "));
-
-  // ---- device
-  int dev = 0, sms = 0;
-  if (int rc = query_device(&dev, &sms)) return rc;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  const bool f8 = arith == SCE_ARITH_F16F8;
-  const Slices sl = mom_slices(d, B);
-  RowCarve rc;
-  row_carve(static_cast<uint8_t*>(workspace), f8, d, k, sl.S, (size_t)sl.S * sl.R, &rc, true);
-  return f8 ? run_nmf_grams_t<kArithF16F8>(L, x, x_is_half, B, d, shift, w, k, sl, rc, wtw, wtv, range_flag, dev, sms)
-            : run_nmf_grams_t<kArithBf16x3>(L, x, x_is_half, B, d, shift, w, k, sl, rc, wtw, wtv, range_flag, dev, sms);
+  return row_pass(kPassNmfGrams, {x, x_is_half == 1, B, d, shift, range_flag}, k, arith, workspace, stream,
+                  [&](auto ar, auto&... r) { return run_nmf_grams_t<decltype(ar)::value>(r..., w, k, wtw, wtv); });
 }
 
 size_t sce_nmf_cd_sweep_workspace_bytes(int k, int R) {
@@ -2875,7 +2831,7 @@ int sce_nmf_cd_sweep(void* w, int w_is_f64, int R, int k, const void* g, const v
 
 
 size_t sce_nmf_residual_workspace_bytes(int d, int B) {
-  if (d < 8 || d % 8 || d > 8192 || B < 1 || B > kMomCallRowsMax) return 0;
+  if (!row_shape_ok(d, B)) return 0;
   return align_up((size_t)((d + kResTile - 1) / kResTile) * ((B + kResTile - 1) / kResTile) * sizeof(double), 1024);
 }
 
@@ -2883,7 +2839,7 @@ int sce_nmf_residual(const void* x, int x_is_half, int B, int d, const float* sh
                      const float* h, double* sum, void* workspace, size_t workspace_bytes, void* stream) {
   // ---- arguments (all checked before any CUDA call)
   if (!h || !sum) return fail(SCE_ERR_INVALID, "nmf_residual: h and sum are required");
-  TRY(check_row_pass("nmf_residual: ", x, x_is_half, B, d, shift, k, SCE_ARITH_AUTO, w, "w"));
+  TRY(check_row_pass("nmf_residual: ", x, x_is_half, B, d, shift, SCE_ARITH_AUTO, k, "k", w, "w"));
   if (reinterpret_cast<uintptr_t>(h) % 16 || reinterpret_cast<uintptr_t>(sum) % 8)
     return fail(SCE_ERR_INVALID, "nmf_residual: h must be 16-byte aligned, sum 8-byte aligned");
   TRY(check_workspace(workspace, workspace_bytes, sce_nmf_residual_workspace_bytes(d, B), "nmf_residual: "));

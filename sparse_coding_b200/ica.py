@@ -24,23 +24,17 @@ unit-norm torch rows (the reference passes raw numpy components_, which its own 
 ``to_nneg_dict`` is not mirrored (see there); rank-deficient data raises instead of dividing by ~0."""
 from __future__ import annotations
 
-import ctypes as C
 import warnings
 
 import numpy as np
 import torch
 
-from . import _lib
+from ._rowpass import RowPasses, check_width, convergence_warning, device_rows, fit_device
 from .learned_dict import LearnedDict
-from .pca import BatchedPCA, _call_rows, _pca_device
+from .pca import BatchedPCA
 from .topk_encoder import TopKLearnedDict
 
 _REF_MODULE = "autoencoders.ica"
-
-try:
-    from sklearn.exceptions import ConvergenceWarning
-except ImportError:   # the warning category sklearn would use; a UserWarning where sklearn is not installed
-    ConvergenceWarning = UserWarning
 
 
 class FittedScaler:
@@ -87,28 +81,23 @@ class ICAEncoder(LearnedDict):
         pass
 
     # ---- fitting
-    def _rows(self, dataset):
-        """The rows on the fit's device, once, in their own dtype (fp16 / fp32; others, fp64 included, become fp32)."""
-        x = torch.as_tensor(dataset)
-        if x.dim() != 2 or x.shape[1] != self.activation_size:
-            raise ValueError(f"dataset must be [N, {self.activation_size}], got {tuple(x.shape)}")
-        if x.shape[0] < 2:
-            raise ValueError("ICA needs at least two rows")
-        dev = _pca_device(self.device if self.device is not None else "cuda")
-        if x.dtype not in (torch.float16, torch.float32):
-            x = x.to(dev, torch.float32)   # fp64 rows are rounded to fp32 here
-        return x.to(dev).contiguous(), dev
+    def _device(self):
+        return fit_device(self.device if self.device is not None else "cuda")
 
     def fit(self, dataset):
         """Fits the scaler and FastICA to the rows of ``dataset`` [N, d] and returns ``self``; ``train`` also returns the
         sources."""
         d = int(self.activation_size)
-        code = _lib.arith_code(self.arith)
-        if d < 8 or d % 8 or d > 8192 or (code == _lib.SCE_ARITH_F16F8 and d % 16):
-            raise ValueError(f"the engine fits d in multiples of 8 (16 for f16f8) up to 8192, got {d}")
+        check_width(d, self.arith)
         if not 1.0 <= self.alpha <= 2.0:
             raise ValueError(f"alpha must be in [1, 2], got {self.alpha}")
-        x, dev = self._rows(dataset)
+        x = torch.as_tensor(dataset)
+        if x.dim() != 2 or x.shape[1] != d:
+            raise ValueError(f"dataset must be [N, {d}], got {tuple(x.shape)}")
+        if x.shape[0] < 2:
+            raise ValueError("ICA needs at least two rows")
+        dev = self._device()
+        x = device_rows(x, dev)
         N = x.shape[0]
         w_init = np.random.normal(size=(d, d)) if self.w_init is None else np.asarray(self.w_init, dtype=np.float64)
         if w_init.shape != (d, d):
@@ -134,40 +123,27 @@ class ICAEncoder(LearnedDict):
         K = (u / (N * lam).sqrt()).T
         Kw = (u / lam.sqrt()).T / scale
         # ---- iterations
-        lib = _lib.load()
-        step = _call_rows(d)
-        cuts = [(s, min(s + step, N)) for s in range(0, N, step)]
-        ws, ws_ptr = _lib.workspace(lib.sce_ica_pass_workspace_bytes(d, d, cuts[0][1]), dev, "sce_ica_pass_workspace_bytes")
-        ws_bytes = ws.numel() - 1024
+        passes = RowPasses(d, dev, self.arith)
         g_sum = torch.empty(d, dtype=torch.float64, device=dev)
         gx = torch.empty(d, d, dtype=torch.float64, device=dev)
-        flag = torch.zeros(1, dtype=torch.int32, device=dev)
         W = _sym_decorrelation(torch.as_tensor(w_init, dtype=torch.float64).to(dev))
         n_iter, lim = 0, float("inf")
         with torch.cuda.device(dev):
-            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             for n_iter in range(1, self.max_iter + 1):
                 unmix = (W @ Kw).float().contiguous()
                 g_sum.zero_()
                 gx.zero_()
-                for s, e in cuts:
-                    xb = x[s:e]
-                    _lib.check(lib.sce_ica_pass(xb.data_ptr(), int(x.dtype == torch.float16), e - s, d,
-                                                pca.shift.data_ptr(), unmix.data_ptr(), d, C.c_float(self.alpha), code,
-                                                g_sum.data_ptr(), gx.data_ptr(), flag.data_ptr(), ws_ptr, ws_bytes,
-                                                stream), "sce_ica_pass")
+                passes.ica_pass(x, pca.shift, unmix, self.alpha, g_sum, gx)
                 W1 = _sym_decorrelation(gx @ Kw.T / N - (g_sum / N)[:, None] * W)
                 lim_t = ((W1 * W).sum(dim=1).abs() - 1).abs().max()
                 W = W1
                 lim = float(lim_t)
                 if lim < self.tol:
                     break
-        if int(flag.item()):
-            raise ValueError("the rows or the unmixing matrix hold a value the f16f8 arithmetic's fp16 plane cannot "
-                             "(|v| >= 65520 or NaN): use arith='bf16x3' or 'auto'")
+        passes.check_flag("the rows or the unmixing matrix")
         if not lim < self.tol:
             warnings.warn("FastICA did not converge. Consider increasing tolerance or the maximum number of "
-                          "iterations.", ConvergenceWarning)
+                          "iterations.", convergence_warning())
         # ---- unit variance and the read-out
         W = W / ((W * W).sum(dim=1, keepdim=True) / N).sqrt()
         comp = W @ K
@@ -182,7 +158,7 @@ class ICAEncoder(LearnedDict):
         self.fit(dataset)
         x = torch.as_tensor(dataset)
         out = torch.empty(x.shape, dtype=torch.float64, device=x.device)
-        dev = _pca_device(self.device if self.device is not None else "cuda")
+        dev = self._device()
         step = max(1, (1 << 27) // max(1, x.shape[1]))
         for s in range(0, x.shape[0], step):
             out[s:s + step] = self._encode64(x[s:s + step].to(dev)).to(x.device)

@@ -47,18 +47,14 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._rowpass import RowPasses, call_rows, check_width, convergence_warning, device_rows, fit_device
 from .learned_dict import LearnedDict
-from .pca import _call_rows, _pca_device
 from .topk_encoder import TopKLearnedDict
 
 _REF_MODULE = "autoencoders.nmf"
 _EPS_INIT = 1e-6      # sklearn's _initialize_nmf eps
 _MAX_K = 2048         # sce_nmf_cd_sweep's widest row
-
-try:
-    from sklearn.exceptions import ConvergenceWarning
-except ImportError:   # the warning category sklearn would use; a UserWarning where sklearn is not installed
-    ConvergenceWarning = UserWarning
+_FLAG_WHAT = "the rows or the factors"
 
 
 class FittedNMF:
@@ -79,8 +75,12 @@ def _gram(H):
     return 0.5 * (G + G.T)
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+def _cd_sweep(w, w_is_f64, k, g, l, ws, viol, max_sweeps=1, tol=0.0, n_iter=None):
+    """sce_nmf_cd_sweep over the rows of w [R, k] on the current stream; ``ws``: (tensor, address) of its workspace."""
+    lib, stream = _lib.load(), C.c_void_p(torch.cuda.current_stream(w.device).cuda_stream)
+    _lib.check(lib.sce_nmf_cd_sweep(w.data_ptr(), w_is_f64, w.shape[0], k, g.data_ptr(), l.data_ptr(), max_sweeps,
+                                    C.c_double(tol), viol.data_ptr(), None if n_iter is None else n_iter.data_ptr(),
+                                    ws[1], ws[0].numel() - 1024, stream), "sce_nmf_cd_sweep")
 
 
 class NMFEncoder(LearnedDict):
@@ -113,33 +113,7 @@ class NMFEncoder(LearnedDict):
         dev = getattr(self, "device", None)
         if dev is None:
             dev = fallback if fallback is not None and torch.device(fallback).type == "cuda" else "cuda"
-        return _pca_device(dev)
-
-    def _code(self):
-        return _lib.arith_code(getattr(self, "arith", "auto"))
-
-    @staticmethod
-    def _rows(x, dev):
-        if x.dtype not in (torch.float16, torch.float32):
-            x = x.to(dev, torch.float32)   # fp64 rows are rounded to fp32 here
-        return x.to(dev).contiguous()
-
-    @staticmethod
-    def _check_flag(flag):
-        if int(flag.item()):
-            raise ValueError("the rows or the factors hold a value the f16f8 arithmetic's fp16 plane cannot "
-                             "(|v| >= 65520 or NaN): use arith='bf16x3' or 'auto'")
-
-    def _project(self, lib, x, cuts, shift_vec, m, out, norms, flag, ws):
-        """out[s:e] = max(x[s:e] - shift, 0) m^T per call (fp32), adding the part norms to ``norms`` if given."""
-        d, k = x.shape[1], m.shape[0]
-        ws_ptr, ws_bytes = ws
-        stream = _stream(x.device)
-        for s, e in cuts:
-            _lib.check(lib.sce_nmf_project(x[s:e].data_ptr(), int(x.dtype == torch.float16), e - s, d,
-                                           shift_vec.data_ptr(), m.data_ptr(), k, self._code(), out[s:e].data_ptr(),
-                                           None if norms is None else norms.data_ptr(), flag.data_ptr(), ws_ptr,
-                                           ws_bytes, stream), "sce_nmf_project")
+        return fit_device(dev)
 
     # ---- fitting
     def fit(self, dataset):
@@ -154,9 +128,8 @@ class NMFEncoder(LearnedDict):
     def _fit(self, dataset):
         """(W, the violation of each iteration): the fit behind ``fit`` and ``fit_transform``."""
         d = int(self.activation_size)
-        code = self._code()
-        if d < 8 or d % 8 or d > _MAX_K or (code == _lib.SCE_ARITH_F16F8 and d % 16):
-            raise ValueError(f"the engine fits d in multiples of 8 (16 for f16f8) up to {_MAX_K}, got {d}")
+        arith = getattr(self, "arith", "auto")
+        check_width(d, arith, _MAX_K)
         x_in = torch.as_tensor(dataset)
         if x_in.dim() != 2 or x_in.shape[1] != d:
             raise ValueError(f"dataset must be [N, {d}], got {tuple(x_in.shape)}")
@@ -168,30 +141,18 @@ class NMFEncoder(LearnedDict):
         if lo < self.shift:
             self.shift = lo
         dev = self._device(x_in.device)
-        x = self._rows(x_in, dev)
-        lib = _lib.load()
-        step = _call_rows(d)
-        cuts = [(s, min(s + step, N)) for s in range(0, N, step)]
-        B0 = cuts[0][1]
-        ws_need = max(lib.sce_second_moments_workspace_bytes(d, B0), lib.sce_nmf_project_workspace_bytes(d, d, B0),
-                      lib.sce_nmf_grams_workspace_bytes(d, d, B0))
-        ws, ws_ptr = _lib.workspace(ws_need, dev, "sce_nmf_*_workspace_bytes")
-        ws = (ws, ws_ptr, ws.numel() - 1024)
-        cd_need = max(lib.sce_nmf_cd_sweep_workspace_bytes(d, B0), lib.sce_nmf_cd_sweep_workspace_bytes(d, d))
-        cd_ws, cd_ptr = _lib.workspace(cd_need, dev, "sce_nmf_cd_sweep_workspace_bytes")
+        x = device_rows(x_in, dev)
+        passes = RowPasses(d, dev, arith)
+        B0 = min(call_rows(d), N)
+        cd_ws = _lib.workspace(max(_lib.load().sce_nmf_cd_sweep_workspace_bytes(d, R) for R in (B0, d)), dev,
+                               "sce_nmf_cd_sweep_workspace_bytes")
         f64 = dict(dtype=torch.float64, device=dev)
-        flag = torch.zeros(1, dtype=torch.int32, device=dev)
         shift_vec = torch.full((d,), float(self.shift), dtype=torch.float32, device=dev)
-        half = int(x.dtype == torch.float16)
         with torch.cuda.device(dev):
-            stream = _stream(dev)
             # ---- NNDSVDA
             col_sum, gram = torch.zeros(d, **f64), torch.zeros(d, d, **f64)
-            for s, e in cuts:
-                _lib.check(lib.sce_second_moments(x[s:e].data_ptr(), half, e - s, d, shift_vec.data_ptr(), code,
-                                                  col_sum.data_ptr(), gram.data_ptr(), flag.data_ptr(), ws[1], ws[2],
-                                                  stream), "sce_second_moments")
-            self._check_flag(flag)
+            passes.second_moments(x, shift_vec, col_sum, gram)
+            passes.check_flag(_FLAG_WHAT)
             if not bool(torch.isfinite(gram).all()):
                 raise ValueError("the rows hold a non-finite value")
             avg = float(col_sum.sum()) / (N * d)
@@ -204,7 +165,7 @@ class NMFEncoder(LearnedDict):
             Vr = vec.T.contiguous()                      # rows: the right singular vectors
             W = torch.empty(N, d, dtype=torch.float32, device=dev)
             norms = torch.zeros(2 * d, **f64)
-            self._project(lib, x, cuts, shift_vec, Vr.float().contiguous(), W, norms, flag, ws[1:])
+            passes.nmf_project(x, shift_vec, Vr.float().contiguous(), W, norms)
             pos, neg = norms[:d], norms[d:]
             yp, yn = Vr.clamp(min=0), (-Vr).clamp(min=0)
             ypn, ynn = yp.norm(dim=1), yn.norm(dim=1)
@@ -221,8 +182,7 @@ class NMFEncoder(LearnedDict):
             w_scale = torch.nan_to_num(torch.where(zero, 0.0, w_scale), nan=0.0, posinf=0.0).float()
             w_sign = w_sign.float()
             H = torch.nan_to_num(torch.where(zero[:, None], 0.0, H), nan=0.0)
-            for s, e in cuts:
-                blk = W[s:e]
+            for blk in W.split(call_rows(d)):
                 blk[:, 0].abs_()
                 blk.mul_(w_sign).clamp_(min=0).mul_(w_scale)
                 blk.masked_fill_(blk < _EPS_INIT, avg)
@@ -231,7 +191,6 @@ class NMFEncoder(LearnedDict):
             L = torch.empty(B0, d, dtype=torch.float32, device=dev)
             wtw, wtv = torch.zeros(d, d, **f64), torch.zeros(d, d, **f64)
             viol = torch.zeros(1, **f64)
-            cd_bytes = cd_ws.numel() - 1024
             v0, n_iter, violations = None, 0, []
             for n_iter in range(1, self.max_iter + 1):
                 Hf = H.float().contiguous()
@@ -239,20 +198,14 @@ class NMFEncoder(LearnedDict):
                 viol.zero_()
                 wtw.zero_()
                 wtv.zero_()
-                for s, e in cuts:
-                    self._project(lib, x[s:e], [(0, e - s)], shift_vec, Hf, L, None, flag, ws[1:])
-                    _lib.check(lib.sce_nmf_cd_sweep(W[s:e].data_ptr(), 0, e - s, d, G.data_ptr(), L.data_ptr(), 1,
-                                                    C.c_double(0.0), viol.data_ptr(), None, cd_ptr, cd_bytes, stream),
-                               "sce_nmf_cd_sweep")
-                    _lib.check(lib.sce_nmf_grams(x[s:e].data_ptr(), half, e - s, d, shift_vec.data_ptr(),
-                                                 W[s:e].data_ptr(), d, code, wtw.data_ptr(), wtv.data_ptr(),
-                                                 flag.data_ptr(), ws[1], ws[2], stream), "sce_nmf_grams")
+                for xb, wb in zip(x.split(B0), W.split(B0)):
+                    passes.nmf_project(xb, shift_vec, Hf, L)
+                    _cd_sweep(wb, 0, d, G, L, cd_ws, viol)
+                    passes.nmf_grams(xb, shift_vec, wb, wtw, wtv)
                 Ht = H.T.contiguous()
                 Lh = wtv.T.contiguous()
                 wtw_s = (0.5 * (wtw + wtw.T)).contiguous()   # the sweep reads G[t][:] as its column t too
-                _lib.check(lib.sce_nmf_cd_sweep(Ht.data_ptr(), 1, d, d, wtw_s.data_ptr(), Lh.data_ptr(), 1,
-                                                C.c_double(0.0), viol.data_ptr(), None, cd_ptr, cd_bytes, stream),
-                           "sce_nmf_cd_sweep")
+                _cd_sweep(Ht, 1, d, wtw_s, Lh, cd_ws, viol)
                 H = Ht.T.contiguous()
                 v = float(viol)
                 violations.append(v)
@@ -263,16 +216,11 @@ class NMFEncoder(LearnedDict):
             # ---- reconstruction_err_: one fp32 residual pass over the rows
             Hf = H.float().contiguous()
             res = torch.zeros(1, **f64)
-            rs, rs_ptr = _lib.workspace(lib.sce_nmf_residual_workspace_bytes(d, B0), dev,
-                                        "sce_nmf_residual_workspace_bytes")
-            for s, e in cuts:
-                _lib.check(lib.sce_nmf_residual(x[s:e].data_ptr(), half, e - s, d, shift_vec.data_ptr(),
-                                                W[s:e].data_ptr(), d, Hf.data_ptr(), res.data_ptr(), rs_ptr,
-                                                rs.numel() - 1024, stream), "sce_nmf_residual")
-        self._check_flag(flag)
+            passes.nmf_residual(x, shift_vec, W, Hf, res)
+        passes.check_flag(_FLAG_WHAT)
         if n_iter == self.max_iter and self.tol > 0:
             warnings.warn(f"Maximum number of iterations {self.max_iter} reached. Increase it to improve convergence.",
-                          ConvergenceWarning)
+                          convergence_warning())
         self.nmf = FittedNMF(H.cpu().numpy().astype(np.float64), n_iter, float(res.sqrt()), self.tol, self.max_iter)
         self._cache = None
         return W, violations
@@ -301,28 +249,21 @@ class NMFEncoder(LearnedDict):
         if k % 8 or k > _MAX_K:
             raise ValueError(f"the engine encodes k in multiples of 8 up to {_MAX_K} components, got {k}")
         dev = self._device(x.device)
-        xs = self._rows(x, dev)
+        xs = device_rows(x, dev)
         B = xs.shape[0]
-        lib = _lib.load()
-        step = _call_rows(d)
-        cuts = [(s, min(s + step, B)) for s in range(0, B, step)]
-        ws, ws_ptr = _lib.workspace(lib.sce_nmf_project_workspace_bytes(d, k, cuts[0][1]), dev,
-                                    "sce_nmf_project_workspace_bytes")
-        cd_ws, cd_ptr = _lib.workspace(lib.sce_nmf_cd_sweep_workspace_bytes(k, B), dev,
-                                       "sce_nmf_cd_sweep_workspace_bytes")
-        flag = torch.zeros(1, dtype=torch.int32, device=dev)
+        passes = RowPasses(d, dev, getattr(self, "arith", "auto"))
+        cd_ws = _lib.workspace(_lib.load().sce_nmf_cd_sweep_workspace_bytes(k, B), dev,
+                               "sce_nmf_cd_sweep_workspace_bytes")
         with torch.cuda.device(dev):
             Hf, G = self._factors(dev)
             shift_vec = torch.full((d,), float(self.shift), dtype=torch.float32, device=dev)
             P = torch.empty(B, k, dtype=torch.float32, device=dev)
-            self._project(lib, xs, cuts, shift_vec, Hf, P, None, flag, (ws_ptr, ws.numel() - 1024))
+            passes.nmf_project(xs, shift_vec, Hf, P)
             W = torch.zeros(B, k, dtype=torch.float32, device=dev)
             viol = torch.empty(2, dtype=torch.float64, device=dev)
             n_it = torch.empty(1, dtype=torch.int32, device=dev)
-            _lib.check(lib.sce_nmf_cd_sweep(W.data_ptr(), 0, B, k, G.data_ptr(), P.data_ptr(), int(self.nmf.max_iter),
-                                            C.c_double(float(self.nmf.tol)), viol.data_ptr(), n_it.data_ptr(), cd_ptr,
-                                            cd_ws.numel() - 1024, _stream(dev)), "sce_nmf_cd_sweep")
-        self._check_flag(flag)
+            _cd_sweep(W, 0, k, G, P, cd_ws, viol, int(self.nmf.max_iter), float(self.nmf.tol), n_it)
+        passes.check_flag(_FLAG_WHAT)
         return W, int(n_it.item())
 
     def encode(self, x):

@@ -36,32 +36,13 @@ on the CPU beside device rows.
 ``BatchedMean`` / ``calc_mean`` are not mirrored: no caller uses them (SURVEY, quirks)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
-from . import _lib
+from ._rowpass import RowPasses, check_width, cuts, fit_device
 from .learned_dict import LearnedDict, Rotation, TiedSAE
 from .topk_encoder import TopKLearnedDict
 
 _REF_MODULE = "autoencoders.pca"
-_MAX_PLANE_ELEMS = 1 << 27       # rows per engine call x d: the planes of one call stay under ~0.8 GB
-_MAX_CALL_ROWS = 1 << 16
-
-
-def _call_rows(d: int) -> int:
-    """Rows per engine call at width d."""
-    return max(64, min(_MAX_CALL_ROWS, _MAX_PLANE_ELEMS // d))
-
-
-def _pca_device(device) -> torch.device:
-    dev = torch.device(device)
-    if dev.type != "cuda" or not torch.cuda.is_available():
-        raise RuntimeError(f"BatchedPCA fits in the sm_90a CUDA engine and needs a CUDA device (got {device!r}, CUDA "
-                           f"available: {torch.cuda.is_available()}); there is no CPU implementation in the product path")
-    if dev.index is None:
-        dev = torch.device("cuda", torch.cuda.current_device())
-    return dev
 
 
 class BatchedPCA:
@@ -70,21 +51,15 @@ class BatchedPCA:
 
     def __init__(self, n_dims, device, arith: str = "auto"):
         self.n_dims = int(n_dims)
-        self.device = _pca_device(device)
+        self.device = fit_device(device)
         self.arith = arith
-        code = _lib.arith_code(arith)
+        check_width(self.n_dims, arith)
         d = self.n_dims
-        if d < 8 or d % 8 or d > 8192:
-            raise ValueError(f"n_dims must be a multiple of 8 in [8, 8192], got {n_dims}")
-        if code == _lib.SCE_ARITH_F16F8 and d % 16:
-            raise ValueError(f"arith='f16f8' needs n_dims to be a multiple of 16, got {n_dims}")
-        self._code = code
         self.n_samples = 0
         self.shift = None
         self.col_sum = torch.zeros(d, dtype=torch.float64, device=self.device)
         self.gram = torch.zeros(d, d, dtype=torch.float64, device=self.device)
-        self._flag = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self._ws, self._ws_bytes = None, 0
+        self._passes = RowPasses(d, self.device, arith)
         self._eig = None
 
     # ---- fitting
@@ -104,16 +79,6 @@ class BatchedPCA:
         from .train_loop import HostBatchPrefetcher
         yield from HostBatchPrefetcher((activations[s:e].contiguous() for s, e in cuts), self.device)
 
-    def _workspace(self, cuts):
-        """(address, bytes) of a workspace that serves every call of ``cuts``: grown to the largest need, kept after."""
-        lib = _lib.load()
-        need = max(lib.sce_second_moments_workspace_bytes(self.n_dims, e - s) for s, e in cuts)
-        if need > self._ws_bytes:
-            self._ws = None
-            self._ws, self._ws_ptr = _lib.workspace(need, self.device, "sce_second_moments_workspace_bytes")
-            self._ws_bytes = need
-        return self._ws_ptr, self._ws_bytes
-
     def train_batch(self, activations):
         """Adds the rows of ``activations`` [B, d] (fp16 or fp32, on a CUDA device or the CPU, B >= 1).
 
@@ -125,23 +90,16 @@ class BatchedPCA:
         B = activations.shape[0]
         if B == 0:
             return
-        step = _call_rows(self.n_dims)
-        cuts = [(s, min(s + step, B)) for s in range(0, B, step)]
-        lib = _lib.load()
+        calls = cuts(B, self.n_dims)
         col_sum = lambda xb: xb.sum(dim=0, dtype=torch.float64)
         with torch.cuda.device(self.device):
-            if self.shift is None and len(cuts) > 1:
-                total = sum(col_sum(xb) for xb in self._batches(activations, cuts))
+            if self.shift is None and len(calls) > 1:
+                total = sum(col_sum(xb) for xb in self._batches(activations, calls))
                 self.shift = (total / B).float().contiguous()
-            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-            ws_ptr, ws_bytes = self._workspace(cuts)
-            for xb in self._batches(activations, cuts):
+            for xb in self._batches(activations, calls):
                 if self.shift is None:
                     self.shift = (col_sum(xb) / B).float().contiguous()
-                _lib.check(lib.sce_second_moments(
-                    xb.data_ptr(), int(xb.dtype == torch.float16), xb.shape[0], self.n_dims, self.shift.data_ptr(),
-                    self._code, self.col_sum.data_ptr(), self.gram.data_ptr(), self._flag.data_ptr(), ws_ptr, ws_bytes,
-                    stream), "sce_second_moments")
+                self._passes.second_moments(xb, self.shift, self.col_sum, self.gram)
         self.n_samples += B
         self._eig = None
 
@@ -149,9 +107,7 @@ class BatchedPCA:
     def _ready(self):
         if self.n_samples == 0:
             raise ValueError("BatchedPCA has seen no rows")
-        if self._code == _lib.SCE_ARITH_F16F8 and int(self._flag.item()):
-            raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
-                             "NaN): use arith='bf16x3' or 'auto'")
+        self._passes.check_flag("the activations")
 
     def _mean64(self):
         return self.shift.double() + self.col_sum / self.n_samples

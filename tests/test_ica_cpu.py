@@ -102,10 +102,10 @@ def test_workspace_query_rejects_invalid_arguments():
 
 
 def test_workspace_need_never_decreases_with_rows():
-    from sparse_coding_b200.pca import _call_rows
+    from sparse_coding_b200._rowpass import call_rows
     lib = _lib.load()
     for d, n in ((8, 8), (512, 512), (512, 256), (2048, 2048)):
-        top = _call_rows(d)
+        top = call_rows(d)
         needs = [lib.sce_ica_pass_workspace_bytes(d, n, B) for B in range(1, top + 1, 7)] + \
                 [lib.sce_ica_pass_workspace_bytes(d, n, top)]
         assert all(v > 0 for v in needs)

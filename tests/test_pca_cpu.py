@@ -66,10 +66,10 @@ def test_workspace_query_rejects_invalid_arguments():
 def test_workspace_need_never_decreases_with_rows():
     """A workspace sized for the longest call serves every shorter one, although the slice count of a call is not
     monotone in its rows (at d = 512, 64000 rows take 33 slices of 1984 rows and 65536 rows 32 of 2048)."""
-    from sparse_coding_b200.pca import _call_rows
+    from sparse_coding_b200._rowpass import call_rows
     lib = _lib.load()
     for d in (8, 512, 2048):
-        top = _call_rows(d)
+        top = call_rows(d)
         needs = [lib.sce_second_moments_workspace_bytes(d, B) for B in range(1, top + 1)]
         assert all(n > 0 for n in needs)
         assert all(a <= b for a, b in zip(needs, needs[1:])), d

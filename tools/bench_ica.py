@@ -72,7 +72,7 @@ def main():
     dev, K, W = setup(args)
     from sparse_coding_b200 import _lib
     from sparse_coding_b200.ica import ICAEncoder, _sym_decorrelation
-    from sparse_coding_b200.pca import _call_rows
+    from sparse_coding_b200._rowpass import call_rows
     d, N = WORKLOADS[args.workload], N_ROWS
     x = chunk_rows(N, d, dev)
     flops = 4.0 * N * d * d
@@ -84,7 +84,7 @@ def main():
     unmix = (torch.from_numpy(rs.normal(size=(d, d))).float().to(dev) / d ** 0.5).contiguous()
     ref64 = op_pass(x, shift, unmix, torch.float64)
     lib = _lib.load()
-    step = _call_rows(d)
+    step = call_rows(d)
     ws, ptr = _lib.workspace(lib.sce_ica_pass_workspace_bytes(d, d, step), dev, "sce_ica_pass_workspace_bytes")
     stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     warnings.simplefilter("ignore")

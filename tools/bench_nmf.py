@@ -24,7 +24,7 @@ import torch
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 from sparse_coding_b200 import _lib  # noqa: E402
 from sparse_coding_b200.nmf import NMFEncoder, _gram  # noqa: E402
-from sparse_coding_b200.pca import _call_rows  # noqa: E402
+from sparse_coding_b200._rowpass import call_rows  # noqa: E402
 
 
 def card():
@@ -55,7 +55,7 @@ def main():
         enc = NMFEncoder(d, max_iter=1)
         W = enc.fit_transform(x)
         H = torch.as_tensor(enc.nmf.components_, device=dev)
-        step = _call_rows(d)
+        step = call_rows(d)
         cuts = [(s, min(s + step, N)) for s in range(0, N, step)]
         ws, ws_ptr = _lib.workspace(max(lib.sce_nmf_project_workspace_bytes(d, d, step),
                                         lib.sce_nmf_grams_workspace_bytes(d, d, step)), dev, "ws")

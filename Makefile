@@ -4,11 +4,17 @@ ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v
 CSRC := sparse_coding_b200/csrc
 LIB := sparse_coding_b200/libsce.so
+# one object per family of entry points (make -j compiles them side by side)
+LIB_OBJS := $(patsubst %,build/%.o,sce_abi sce_plan sce_similarity sce_rowpass)
 
 all: $(LIB)
 
-$(LIB): $(CSRC)/sce_engine.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h include/sce.h
-	$(NVCC) $(NVFLAGS) -shared -o $@ $(CSRC)/sce_engine.cu
+$(LIB): $(LIB_OBJS)
+	$(NVCC) $(ARCH) -shared -o $@ $(LIB_OBJS)
+
+build/sce_%.o: $(CSRC)/sce_%.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h include/sce.h
+	mkdir -p build
+	$(NVCC) $(NVFLAGS) -c -o $@ $<
 
 selftest: build/gemm_selftest build/gemm_cluster_selftest
 build/gemm_selftest: tests/csrc/gemm_selftest.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
@@ -25,4 +31,4 @@ build/gemm_overlap_probe: tools/gemm_overlap_probe.cu $(CSRC)/*.cuh $(CSRC)/sce_
 	$(NVCC) $(NVFLAGS) -o $@ tools/gemm_overlap_probe.cu
 
 clean:
-	rm -f $(LIB) build/gemm_selftest build/gemm_cluster_selftest build/gemm_overlap_probe
+	rm -f $(LIB) $(LIB_OBJS) build/gemm_selftest build/gemm_cluster_selftest build/gemm_overlap_probe

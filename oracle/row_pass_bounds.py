@@ -104,7 +104,7 @@ def reference(kind: str, x: Tensor, shift: Tensor, mat: Tensor = None, alpha: fl
     return nmf_project(V, mat) if kind == "project" else nmf_grams(V, mat)
 
 
-# ---- the engine's slicing and cluster rules, restated (sce_engine.cu mom_slices, sce_gemm.cuh gemm_cluster_size)
+# ---- the engine's slicing and cluster rules, restated (sce_rowpass.cu mom_slices, sce_gemm.cuh gemm_cluster_size)
 ROWS_MAX, TARGET_TILES, SLICE_MIN, BLOCK_ROWS = 2048, 528, 256, 64
 
 

@@ -1,8 +1,11 @@
 // sce_kernels.cuh — the HBM-bound streaming kernels around the GEMMs of one training step:
 // batch split, dictionary normalise+split, row-norm Jacobian + Adam + re-split, bias Adam,
-// loss finalisation, top-k selection, code materialisation, chunk row gather.
+// top-k selection, code materialisation, chunk row gather.
 // Each is a single pass over its data with 16-byte accesses; algorithmic bytes per element are
 // listed in DESIGN.md.
+// Every translation unit of libsce.so includes this header, so every kernel here is a template: a kernel that is not
+// one is defined in the one .cu that owns it (the loss finalisation, centre gradient, activity counts and batch-major
+// transpose of the training step: sce_plan.cu), or each includer would define it again.
 #pragma once
 #include "sce_epilogues.cuh"
 
@@ -109,25 +112,6 @@ __global__ void center_split_kernel(const float* __restrict__ x, long long x_mod
     const float4 t = __ldg(ts + (int)(i % d4));
     const float vv[4] = {v.x - t.x, v.y - t.y, v.z - t.z, v.w - t.w};
     store_planes4<ARITH>(vv, hi, lo, x8, p4 + i);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// learned centre (FunctionalTiedCenteredSAE.center, sae_ensemble.py:198-200): out[m] = x[m] - center[m], fp32 [M][B][d];
-// x is [B][d] shared by the models (x_model_stride = 0) or [M][B][d]. grid.y = model.
-// ------------------------------------------------------------------------------------------------
-__global__ void center_sub_kernel(const float* __restrict__ x, long long x_model_stride, const float* __restrict__ center,
-                                  float* __restrict__ out, int B, int d) {
-  const int model = blockIdx.y;
-  const int d4 = d >> 2;
-  const long long n4 = (long long)B * d4;
-  const float4* xs = reinterpret_cast<const float4*>(x + (long long)model * x_model_stride);
-  const float4* cs = reinterpret_cast<const float4*>(center + (long long)model * d);
-  float4* o = reinterpret_cast<float4*>(out + (long long)model * B * d);
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
-    const float4 v = xs[i];
-    const float4 c = __ldg(cs + (int)(i % d4));
-    o[i] = make_float4(v.x - c.x, v.y - c.y, v.z - c.z, v.w - c.w);
   }
 }
 
@@ -348,98 +332,6 @@ __global__ void __launch_bounds__(256) transpose_kernel(const T* __restrict__ sr
 }
 
 // ------------------------------------------------------------------------------------------------
-// f16f8 weight gradient: the two 8-bit planes of a batch operand [models][batch_max][cols] (rows 0 .. rows - 1 valid) ->
-// batch-major copies [models][cols][ld], ld = batch_max rounded up to 16, so that the weight-gradient GEMM reads them
-// K-major over the batch and forms its cross terms on E5M2 wgmma. 128 x 128-byte tiles through shared memory, 16-byte
-// loads and stores (cols and ld are multiples of 16): a thread gathers one 4-byte word of 16 source rows and turns it
-// into 16 bytes of four output rows with 4 x 4 byte transposes in registers. Grid: (cols / 128, rows / 128, 2 models),
-// z = plane * models + model.
-// ------------------------------------------------------------------------------------------------
-struct BatchPlanes {
-  const uint8_t* src[2];
-  uint8_t* dst[2];
-};
-// rows a, b, c, d of four bytes each (byte = column) -> column v of the four rows in o[v]
-__device__ __forceinline__ void transpose4x4_u8(uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t (&o)[4]) {
-  const uint32_t t0 = __byte_perm(a, b, 0x5140), t1 = __byte_perm(a, b, 0x7362);   // a0 b0 a1 b1 / a2 b2 a3 b3
-  const uint32_t t2 = __byte_perm(c, d, 0x5140), t3 = __byte_perm(c, d, 0x7362);
-  o[0] = __byte_perm(t0, t2, 0x5410);
-  o[1] = __byte_perm(t0, t2, 0x7632);
-  o[2] = __byte_perm(t1, t3, 0x5410);
-  o[3] = __byte_perm(t1, t3, 0x7632);
-}
-__global__ void __launch_bounds__(256) transpose_batch_u8_kernel(BatchPlanes t, int models, int rows, int cols,
-                                                                 long long src_model_pitch, int ld) {
-  // 128 source rows of 128 bytes; 16-byte piece k of row r is stored at k ^ ((r >> 4) & 7), so that the column reads
-  // below (8 groups of 16 rows x 4 words per warp) hit 32 different banks
-  __shared__ uint4 tile[128][8];
-  const int plane = blockIdx.z / models, m = blockIdx.z - plane * models;
-  const uint8_t* src = (plane ? t.src[1] : t.src[0]) + (long long)m * src_model_pitch;   // (no dynamic index into the
-  uint8_t* dst = (plane ? t.dst[1] : t.dst[0]) + (long long)m * cols * ld;                // parameter struct: no local copy)
-  const int r0 = blockIdx.y * 128, c0 = blockIdx.x * 128;
-#pragma unroll
-  for (int i = threadIdx.x; i < 1024; i += 256) {
-    const int r = i >> 3, k = i & 7;
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (r0 + r < rows && c0 + 16 * k < cols) v = __ldg(reinterpret_cast<const uint4*>(src + (long long)(r0 + r) * cols + c0 + 16 * k));
-    tile[r][k ^ ((r >> 4) & 7)] = v;
-  }
-  __syncthreads();
-  // source rows 16 g .. + 15, source word q (columns 4 q .. + 3) -> output rows c0 + 4 q + v, bytes r0 + 16 g .. + 15
-  const int g = threadIdx.x & 7, q = threadIdx.x >> 3;
-  if (r0 + 16 * g >= rows) return;
-  const uint32_t* tw = reinterpret_cast<const uint32_t*>(&tile[0][0]);
-  uint32_t w[16];
-#pragma unroll
-  for (int u = 0; u < 16; ++u) w[u] = tw[(16 * g + u) * 32 + (((q >> 2) ^ g) << 2) + (q & 3)];
-  uint32_t o[4][4];   // [quad of rows][column v]
-#pragma unroll
-  for (int h = 0; h < 4; ++h) transpose4x4_u8(w[4 * h], w[4 * h + 1], w[4 * h + 2], w[4 * h + 3], o[h]);
-#pragma unroll
-  for (int v = 0; v < 4; ++v) {
-    const int j = c0 + 4 * q + v;
-    if (j < cols)
-      *reinterpret_cast<uint4*>(dst + (long long)j * ld + r0 + 16 * g) = make_uint4(o[0][v], o[1][v], o[2][v], o[3][v]);
-  }
-}
-
-// join_code_kernel<f16f8> for plans whose code residual plane is held batch-major, [M][n][ld] (transpose_batch_u8_kernel):
-// out [M][B][n] fp32 from the row-major fp16 plane [M][batch_max][n] and that copy. Read-back only (strided reads).
-__global__ void __launch_bounds__(256) join_code_batch_major_kernel(const __half* __restrict__ hi, const uint8_t* __restrict__ x8t,
-                                                                    float* __restrict__ out, int B, int n, int batch_max, int ld,
-                                                                    long long total) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const long long m = i / ((long long)B * n), rj = i - m * B * n;
-    const int r = (int)(rj / n), j = (int)(rj - (long long)r * n);
-    constexpr float kInv = 1.f / float(1 << kLoShift);
-    float v = __half2float(hi[(m * batch_max + r) * n + j]) + e5m2_to_float(x8t[(m * n + j) * ld + r]) * kInv;
-    if (v == 0.f) v = 0.f;  // -0 -> +0
-    out[i] = v;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// per-model ||bias||_2 (bias-decay loss term and its gradient; sae_ensemble.py:73, :150)
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) bias_norm_kernel(const float* __restrict__ bias, int n,
-                                                        float* __restrict__ out) {
-  __shared__ double red[8];
-  const float* b = bias + (long long)blockIdx.x * n;
-  double acc = 0.0;
-  for (int i = threadIdx.x; i < n; i += 256) acc += (double)b[i] * (double)b[i];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0;
-    for (int i = 0; i < 8; ++i) t += red[i];
-    out[blockIdx.x] = (float)sqrt(t);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // bias gradient = sum of the per-warp column partials (+ bias decay), then Adam or plain output
 // ------------------------------------------------------------------------------------------------
 template <int MODE>
@@ -469,188 +361,6 @@ __global__ void bias_kernel(float* __restrict__ bias, float* __restrict__ m, flo
     bias[i] = adam_apply(b, g, mm, vv, h);
     m[i] = mm;
     v[i] = vv;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Gradient of the learned centre: d_center = sum_b g_b - db W, W = E / max(||E_n||, floor) (the dictionary the step
-// used: these kernels run before dict_rows_kernel<MODE_ADAM> rewrites E). Three passes, no atomics: bitwise repeatable.
-// ------------------------------------------------------------------------------------------------
-constexpr int kCenterCoefRows = 32;    // dictionary rows per block of center_coef_kernel
-constexpr int kCenterChunkRows = 64;   // dictionary rows per partial of center_gemv_kernel
-
-// coef[m][n] = db[m][n] / max(||E[m][n]||, floor), db summed from the dcode epilogue's partials in the order bias_kernel
-// uses (the same fp32 value) times part_scale. Grid (ceil(n / 32), M), 256 threads: thread t < 32 sums row t's db,
-// warp w takes the norms of rows w, w + 8, ...
-__global__ void __launch_bounds__(256) center_coef_kernel(const float* __restrict__ e, const float* __restrict__ db_part,
-                                                          int n_part, int n, int d, float floor, float part_scale,
-                                                          float* __restrict__ coef) {
-  __shared__ float sdb[kCenterCoefRows], snorm[kCenterCoefRows];
-  const int model = blockIdx.y, j0 = blockIdx.x * kCenterCoefRows;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x < kCenterCoefRows && j0 + threadIdx.x < n) {
-    const float* p = db_part + (long long)model * n_part * n + j0 + threadIdx.x;
-    float g = 0.f;
-    for (int k = 0; k < n_part; ++k) g += p[(long long)k * n];
-    sdb[threadIdx.x] = g * part_scale;
-  }
-  for (int r = warp; r < kCenterCoefRows; r += 8) {
-    if (j0 + r >= n) break;   // warp-uniform
-    const float* row = e + ((long long)model * n + j0 + r) * d;
-    float ss = 0.f;
-    for (int c = lane * 4; c < d; c += 128) {
-      const float4 v = *reinterpret_cast<const float4*>(row + c);
-      ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-    }
-    ss = warp_sum(ss);
-    if (lane == 0) {
-      const float nrm = sqrtf(ss);
-      snorm[r] = floor > 0.f && nrm < floor ? floor : nrm;
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x < kCenterCoefRows && j0 + threadIdx.x < n)
-    coef[(long long)model * n + j0 + threadIdx.x] = sdb[threadIdx.x] / snorm[threadIdx.x];
-}
-
-// part[m][chunk][c] = sum over the chunk's rows, in order, of coef[m][j] E[m][j][c]. Grid (ceil(d / 512), chunks, M),
-// 128 threads of four columns each.
-__global__ void __launch_bounds__(128) center_gemv_kernel(const float* __restrict__ e, const float* __restrict__ coef, int n,
-                                                          int d, float* __restrict__ part) {
-  const int model = blockIdx.z, chunk = blockIdx.y;
-  const int c = (blockIdx.x * 128 + threadIdx.x) * 4;
-  if (c >= d) return;
-  const int j0 = chunk * kCenterChunkRows, j1 = min(n, j0 + kCenterChunkRows);
-  const float* kp = coef + (long long)model * n;
-  const float* ep = e + (long long)model * n * d + c;
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 4
-  for (int j = j0; j < j1; ++j) {
-    const float k = __ldg(kp + j);
-    const float4 v = __ldg(reinterpret_cast<const float4*>(ep + (long long)j * d));
-    acc.x += k * v.x;
-    acc.y += k * v.y;
-    acc.z += k * v.z;
-    acc.w += k * v.w;
-  }
-  *reinterpret_cast<float4*>(part + ((long long)model * gridDim.y + chunk) * d + c) = acc;
-}
-
-// grad[m][c] = g_scale * sum_k g_part[m][k][c] - sum_chunk part[m][chunk][c] (both in index order); MODE_ADAM then
-// applies Adam to center / center_m / center_v, unless the step is bad (kBadWord, as bias_kernel).
-template <int MODE>
-__global__ void center_grad_kernel(const float* __restrict__ g_part, int n_gpart, float g_scale,
-                                   const float* __restrict__ part, int n_chunks, int M, int d, float* __restrict__ grad,
-                                   float* __restrict__ center, float* __restrict__ m, float* __restrict__ v, AdamHyper h,
-                                   const uint32_t* __restrict__ health) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)M * d) return;
-  const int model = int(i / d), c = int(i - (long long)model * d);
-  const float* gp = g_part + (long long)model * n_gpart * d + c;
-  float gs = 0.f;
-  for (int k = 0; k < n_gpart; ++k) gs += gp[(long long)k * d];
-  const float* pp = part + (long long)model * n_chunks * d + c;
-  float dw = 0.f;
-  for (int k = 0; k < n_chunks; ++k) dw += pp[(long long)k * d];
-  const float g = gs * g_scale - dw;
-  grad[i] = g;
-  if (MODE == MODE_ADAM) {
-    if (step_is_bad(health)) return;
-    float mm = m[i], vv = v[i];
-    center[i] = adam_apply(center[i], g, mm, vv, h);
-    m[i] = mm;
-    v[i] = vv;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// losses: deterministic reduction of the GEMM epilogues' per-warp partials
-//   out[m] = {loss, l_reconstruction, l_l1, l_bias_decay}, nnz[m] = mean_b count_nonzero(c)
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) finalize_kernel(const float* __restrict__ enc_part, int n_enc,
-                                                       const float* __restrict__ dec_part, int n_dec,
-                                                       const float* __restrict__ l1_alpha,
-                                                       const float* __restrict__ bias_decay,
-                                                       const float* __restrict__ bnorm, int B, int d,
-                                                       float* __restrict__ out, float* __restrict__ nnz,
-                                                       uint32_t* __restrict__ health) {
-  __shared__ double red[3][8];
-  const int model = blockIdx.x;
-  double l1 = 0, cnt = 0, sq = 0;
-  if (enc_part) {
-    const float* e = enc_part + (long long)model * n_enc * 2;
-    for (int i = threadIdx.x; i < n_enc; i += 256) {
-      l1 += e[2 * i];
-      cnt += e[2 * i + 1];
-    }
-  }
-  const float* dp = dec_part + (long long)model * n_dec;
-  for (int i = threadIdx.x; i < n_dec; i += 256) sq += dp[i];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    l1 += __shfl_xor_sync(0xffffffffu, l1, o);
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    red[0][threadIdx.x >> 5] = l1;
-    red[1][threadIdx.x >> 5] = cnt;
-    red[2][threadIdx.x >> 5] = sq;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double a = 0, b = 0, c = 0;
-    for (int i = 0; i < 8; ++i) {
-      a += red[0][i];
-      b += red[1][i];
-      c += red[2][i];
-    }
-    const float l_rec = (float)(c / ((double)B * d));
-    const float l_l1 = l1_alpha ? (float)(l1_alpha[model] * (a / B)) : 0.f;
-    const float l_bd = (bias_decay && bnorm) ? bias_decay[model] * bnorm[model] : 0.f;
-    if (health && !isfinite(l_rec + l_l1 + l_bd)) health[kBadWord] = 1u;   // the Adam kernels of this step skip
-    if (out) {
-      out[model * 4 + 0] = l_rec + l_l1 + l_bd;
-      out[model * 4 + 1] = l_rec;
-      out[model * 4 + 2] = l_l1;
-      out[model * 4 + 3] = l_bd;
-    }
-    if (nnz) nnz[model] = (float)(b / B);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// per-feature activation counts (standard_metrics.py:305-308 `(c != 0).float().mean(0)` and :441-454
-// `n_active_count += (c != 0).sum(0)`; "ever active" = count > threshold): column sums of the [c > 0] activity-mask
-// plane over the batch rows. One block per (32-column chunk, model): every lane holds the mask word of one row, a
-// ballot per bit position counts 32 rows at once. counts[model][32 chunk + j] += sum_r bit(31 - j) of
-// pos[model][chunk][r], accumulated across calls so a held-out set can be streamed through in batches. Reads B words
-// per block, coalesced (the plane is chunk-major); the dense code is never touched.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) active_count_kernel(const uint32_t* __restrict__ pos, int n_chunks, int batch_max,
-                                                           int B, int n, int* __restrict__ counts) {
-  __shared__ int red[8][32];
-  const int chunk = blockIdx.x, model = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t* p = pos + ((long long)model * n_chunks + chunk) * batch_max;
-  int mine = 0;   // lane j accumulates the count of column j of the chunk
-  for (int r0 = warp * 32; r0 < B; r0 += 256) {
-    const int r = r0 + lane;
-    const uint32_t w = r < B ? __ldg(p + r) : 0u;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int c = __popc(__ballot_sync(0xffffffffu, (w >> (31 - j)) & 1u));
-      if (lane == j) mine += c;
-    }
-  }
-  red[warp][lane] = mine;
-  __syncthreads();
-  if (warp == 0) {
-    int t = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += red[i][lane];
-    const int col = chunk * 32 + lane;
-    if (col < n) counts[(long long)model * n + col] += t;
   }
 }
 

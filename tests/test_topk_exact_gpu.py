@@ -89,7 +89,7 @@ def assert_exact_inputs(Sc, code, x_hat):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# the engine's path, as plan_config (sce_engine.cu) decides it
+# the engine's path, as plan_config (sce_plan.cu) decides it
 # ----------------------------------------------------------------------------------------------------------------
 def gather_classes(d, n, ks):
     """Gather launches per call: non-empty k classes where the plan takes the gather path, else 0."""

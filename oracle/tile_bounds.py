@@ -122,3 +122,98 @@ def tile_ratios(got: Tensor, want: Tensor, scale: Tensor, tile: Tuple[int, int] 
     Tr, Tc = ratio.shape[1:]
     where = (flat // (Tr * Tc), (flat // Tc) % Tr, flat % Tc)
     return {"ratio": ratio, "peak": peak, "worst": (float(ratio.max()), where), "elem": float(peak.max())}
+
+
+def kink_window(Z: Tensor) -> float:
+    """Width of the band around a kink of the step (a ReLU's 0, a top-k's k-th score) inside which an engine and the
+    fp64 oracle may decide differently: 1e-4 of the RMS pre-activation, at least 1e-5."""
+    return max(1e-5, 1e-4 * float(Z.double().pow(2).mean().sqrt()))
+
+
+class Worst:
+    """The worst tile and element of each output over the models of one check."""
+
+    def __init__(self):
+        self.tile, self.elem, self.minimum = {}, {}, {}
+
+    def add(self, name, m, r):
+        ratio, (_, tr, tc) = r["worst"]
+        if ratio >= self.tile.get(name, (-1.0,))[0]:
+            self.tile[name] = (ratio, (m, tr, tc))
+        self.elem[name] = max(self.elem.get(name, 0.0), r["elem"])
+        lo = float(r["ratio"].min()), float(r["peak"].min())
+        old = self.minimum.get(name, (float("inf"), float("inf")))
+        self.minimum[name] = (min(old[0], lo[0]), min(old[1], lo[1]))
+
+    def add_scalar(self, name, m, v):
+        if v >= self.tile.get(name, (-1.0,))[0]:
+            self.tile[name] = (v, (m,))
+        self.elem[name] = max(self.elem.get(name, 0.0), v)
+        self.minimum[name] = (min(self.minimum.get(name, (float("inf"),))[0], v),) * 2
+
+
+def engine_activity(code, counts, near, Z):
+    """[c > 0] as the engine gates the backward pass. The dense code is read back from the operand planes, where an f16f8
+    code below about 4e-9 (under the fp16 plane's subnormals and the scaled residual's) reads as 0 although the engine's
+    activity mask, the sign of its fp32 z, has it active: then the feature's mask count (``active_counts``) exceeds its
+    count of non-zero codes. Those coefficients lie inside the kink window with a zero code; each such feature gets as
+    many of them, the largest z first, back on the active side. A wrong pick could only fail the gradient check."""
+    pos = code > 0
+    missing = counts.long() - pos.sum(0)
+    assert int(missing.min()) >= 0, int(missing.min())
+    for j in torch.nonzero(missing).flatten().tolist():
+        cand = near[:, j] & ~pos[:, j]
+        k = int(missing[j])
+        assert int(cand.sum()) >= k, (j, k, int(cand.sum()))
+        zc = torch.where(cand, Z[:, j], torch.full_like(Z[:, j], -float("inf")))
+        pos[torch.topk(zc, k).indices, j] = True
+    return pos
+
+
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# top-k (TopKEncoder): code c = relu(z) on the selected support, x_hat = c W, dict gradient through the row norm
+# ----------------------------------------------------------------------------------------------------------------------
+def topk_scales(X: Tensor, W: Tensor, s: Tensor, C: Tensor, G: Tensor, support: Tensor) -> Dict[str, Tensor]:
+    """Scales of TopKEncoder's outputs for scores z = x W^T against the unit rows W (norms s) on ``support`` (bool
+    [B, n], selected and positive), from the formulas above with no bias and no L1 term: the code's scale on the support
+    (0 elsewhere, where code and oracle are both 0), x_hat's as that scale times |W|, and the dict gradient's from
+    S_dz = |g| |W|^T on the support, through the row-norm Jacobian."""
+    on = support.to(X.dtype)
+    S_code = code_scale(X, W, torch.zeros(W.shape[0], dtype=X.dtype, device=X.device)) * on
+    S_dz = pre_activation_grad_scale(G, W, 0.0, support)
+    return {"code": S_code, "x_hat": S_code @ W.abs(),
+            "dict": row_norm_jacobian_scale(W, s, weight_grad_scale(S_dz, X, C, G))}
+
+
+def topk_support_check(Z: Tensor, support: Tensor, k: int, window: float) -> Dict[str, int]:
+    """Whether ``support`` (bool [B, n]) is, row by row, the positive part of a top-k of the fp64 scores ``Z`` up to
+    ``window``. Returns counts (rows, or entries for ``outside``):
+      over_k     rows keeping more than k
+      misranked  rows that keep a score below -window, or drop one above (k-th kept score, or 0 where fewer than k are
+                 kept) + window
+      differ     rows whose support is not Z's own (its k largest scores, the positive ones)
+      outside    entries where the two differ farther than window from the row's boundary, max(k-th score, 0)"""
+    inf = torch.full_like(Z, float("inf"))
+    kept = support.sum(-1)
+    kept_min = torch.where(support, Z, inf).amin(-1)
+    dropped_max = torch.where(support, -inf, Z).amax(-1)
+    thr = torch.where(kept >= k, kept_min, torch.zeros_like(kept_min))
+    misranked = (kept_min < -window) | (dropped_max > thr + window)
+    top = torch.topk(Z, k, dim=-1)
+    own = torch.zeros_like(support).scatter_(-1, top.indices, True) & (Z > 0)
+    diff = own != support
+    boundary = top.values[:, -1:].clamp(min=0.0)
+    return {"over_k": int((kept > k).sum()), "misranked": int(misranked.sum()), "differ": int(diff.any(-1).sum()),
+            "outside": int((diff & ((Z - boundary).abs() > window)).sum())}
+
+
+# (tile ratio bar, element bar) of TopKEncoder's outputs per arithmetic ("loss": one relative error per model), and the
+# outputs whose bar separates 3-pass from 1-pass tiles: set from measurement in tests/test_topk_tile_bounds_gpu.py (see
+# its docstring); tests/test_tile_bounds_cpu.py shows that they reject planted top-k defects
+TOPK_BARS = {
+    "bf16x3": {"code": (4.3e-6, 7.8e-6), "x_hat": (6.6e-7, 5.1e-6), "dict": (8.7e-7, 4.2e-5), "loss": (6.1e-6, 6.1e-6)},
+    "f16f8": {"code": (1.6e-5, 3.2e-5), "x_hat": (2.8e-6, 1.9e-5), "dict": (3.9e-6, 2.1e-4), "loss": (2.6e-6, 2.6e-6)},
+}
+TOPK_SEPARATED = {"bf16x3": ("code", "x_hat", "dict"), "f16f8": ("x_hat",)}

@@ -111,3 +111,96 @@ def test_one_tile_at_single_pass_accuracy_passes_the_norm_bar_and_fails_the_tile
     assert rel <= 1e-4, rel
     assert r["worst"][1] == (0, 63, 3)
     assert r["worst"][0] > 10 * float(r["ratio"][0].flatten()[:-1].max()), r["worst"]
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# top-k: planted defects against the bars of tests/test_topk_tile_bounds_gpu.py (oracle/tile_bounds.py: TOPK_BARS)
+# ----------------------------------------------------------------------------------------------------------------------
+def _topk(D, X, k):
+    """fp64 TopKEncoder outputs and their scales on the oracle's own support."""
+    f = O.topk_grads(D, X, k)
+    support = f["sel"] & (f["Z"] > 0)
+    return f, support, T.topk_scales(X, f["W"], f["s"], f["c"], f["G"], support)
+
+
+def _topk_case(k=12, seed=3):
+    """Ragged tiles in every output: B = 160, d = 200, n = 320; a previous batch X0 for the stale-state defects."""
+    g = torch.Generator().manual_seed(seed)
+    B, d, n = 160, 200, 320
+    D = torch.randn(n, d, generator=g, dtype=torch.float64)
+    X, X0 = (torch.randn(B, d, generator=g, dtype=torch.float64) for _ in range(2))
+    return D, X, X0, k
+
+
+def _dict_grad(f, X, dZ):
+    return O._row_norm_jacobian(f["W"], f["s"], dZ.T @ X + f["c"].T @ f["G"])
+
+
+def _verdict(name, got, want, S):
+    """Per arithmetic: does the check fail (tile ratio or element maximum above its bar)?"""
+    r = T.tile_ratios(got, want, S)
+    return {a: r["worst"][0] > T.TOPK_BARS[a][name][0] or r["elem"] > T.TOPK_BARS[a][name][1] for a in T.TOPK_BARS}
+
+
+def _plane_residual(v, arith):
+    """What the residual planes hold of v: v minus its leading bf16 (bf16x3) or fp16 (f16f8) plane."""
+    return v - v.to(torch.bfloat16 if arith == "bf16x3" else torch.float16).double()
+
+
+def test_topk_bars_accept_the_exact_result_rounded_to_fp32():
+    D, X, _, k = _topk_case()
+    f, _, S = _topk(D, X, k)
+    for name, want in (("code", f["c"]), ("x_hat", f["x_hat"]), ("dict", f["grads"]["dict"])):
+        assert not any(_verdict(name, want.float(), want, S[name]).values()), name
+
+
+def test_topk_bars_reject_a_stale_code_gradient_residual():
+    """Code-gradient residual-plane entries left from the previous call, at columns that call selected and this one does
+    not: stray lo x terms in the weight gradient. The entries a selection failed to clear are rejected under both
+    arithmetics; so is a single one under bf16x3 (a bf16 residual, up to 2^-9 of its entry). A single f16f8 residual
+    (up to 2^-12 of its entry) measures 3e-6 of its element's scale here, under the element bar of 2.1e-4."""
+    D, X, X0, k = _topk_case()
+    f, support, S = _topk(D, X, k)
+    f0, support0, _ = _topk(D, X0, k)
+    stale = support0 & ~support
+    for arith in T.TOPK_BARS:
+        resid = _plane_residual(f0["dZ"], arith) * stale.to(X.dtype)
+        got = _dict_grad(f, X, f["dZ"] + resid)
+        assert _verdict("dict", got, f["grads"]["dict"], S["dict"])[arith], arith
+    r, j = (int(i) for i in torch.nonzero(stale)[0])
+    one = f["dZ"].clone()
+    one[r, j] += _plane_residual(f0["dZ"], "bf16x3")[r, j]
+    assert _verdict("dict", _dict_grad(f, X, one), f["grads"]["dict"], S["dict"])["bf16x3"]
+
+
+def test_topk_bars_reject_x_hat_from_the_dictionary_before_the_last_step():
+    """x_hat gathered from the normalised dictionary as it was before the last Adam step (a stale fp32 copy): the
+    scores see the new rows, the decode the old ones (an Adam step moves every entry by about lr = 1e-3)."""
+    D, X, _, k = _topk_case()
+    f, _, S = _topk(D, X, k)
+    old, _ = O.unit_rows(D + 1e-3 * torch.sign(f["grads"]["dict"]), floor=None)
+    assert all(_verdict("x_hat", f["c"] @ old, f["x_hat"], S["x_hat"]).values())
+
+
+def test_topk_bars_reject_a_gather_sum_missing_one_entry():
+    """x_hat of one row without one selected entry's contribution to one slice (the first half) of its columns."""
+    D, X, _, k = _topk_case()
+    f, support, S = _topk(D, X, k)
+    r, j = (int(i) for i in torch.nonzero(support)[len(torch.nonzero(support)) // 2])
+    got = f["x_hat"].clone()
+    h = X.shape[1] // 2
+    got[r, :h] -= f["c"][r, j] * f["W"][j, :h]
+    assert all(_verdict("x_hat", got, f["x_hat"], S["x_hat"]).values())
+
+
+def test_topk_bars_reject_a_gradient_through_a_nonpositive_selected_score():
+    """k = 200 of n = 320 keeps non-positive scores in every row; one of them passes g w^T to the weight gradient,
+    which the ReLU stops."""
+    D, X, _, k = _topk_case(k=200)
+    f, support, S = _topk(D, X, k)
+    cand = f["sel"] & (f["Z"] < 0)
+    dz = (f["G"] @ f["W"].T)[cand]
+    at = torch.nonzero(cand)[int(dz.abs().argsort()[len(dz) // 2])]          # the median |g w^T| of them
+    dZ = f["dZ"].clone()
+    dZ[at[0], at[1]] = (f["G"][at[0]] @ f["W"][at[1]])
+    assert all(_verdict("dict", _dict_grad(f, X, dZ), f["grads"]["dict"], S["dict"]).values())

@@ -15,8 +15,9 @@ Signatures: tied, tied with FunctionalTiedSAE's centring, untied, masked tied an
 multiples of 128), learned centre, positive tied; both arithmetics; a batch shared by the models and per-model batches;
 fp16-exact inputs (the f16f8 residual-flag skip) and arbitrary fp32 ones. The ragged shape M = 4, d = 400, n = 1040,
 B = 4001 gives every GEMM of the step more than 132 tiles (the H100's SM count) and a partial last tile in each output
-dimension and in K; config 2 runs at full size with all 16 models, config 5's width tied and untied. Each case is
-checked at initialisation and again after 3 steps on the engine's own fp32 parameters as read back (which covers the
+dimension and in K, and replays the step as a CUDA graph; at B = 8001, above the launch-bound rule, tied and untied
+run the step eagerly and, under f16f8, the native E5M2 weight gradient (dw_native) with those partial tiles; config 2
+runs at full size with all 16 models, config 5's width tied and untied. Each case is checked at initialisation and again after 3 steps on the engine's own fp32 parameters as read back (which covers the
 planes the dictionary-row kernel re-splits). Adam is not compared element by element. Gradients keep the kink rule of
 the other parity tests: coefficients with |z| < kink_window are pinned to the engine's side, none outside it may be on
 the other side, and their number is bounded.
@@ -70,12 +71,14 @@ from oracle import learned_center_oracle as LC
 from oracle import positive_tied_oracle as PT
 from oracle import sae_oracle as O
 from oracle import tile_bounds as T
+from oracle.plan_paths import launch_bound
 
 pytestmark = pytest.mark.gpu
 
 ARITHS = ["bf16x3", "f16f8"]
 VARIANTS = ["tied", "tied_centering", "untied", "masked_tied", "masked_untied", "learned_center", "positive_tied"]
 RAGGED = (4, 400, 1040, 4001)        # M, d, n, B
+RAGGED_EAGER = (4, 400, 1040, 8001)  # the same, above the launch-bound rule (oracle/plan_paths.py)
 REL, GRAD_REL = 1e-4, 2e-4           # the per-model norm-relative bars of the other parity tests
 NEAR_FRAC = 5e-4                     # bound on the share of coefficients inside the kink window
 EXACT_ZERO_FLOOR = 3e-5              # bias-gradient error / scale above which an exact-zero pre-activation is looked for
@@ -109,10 +112,6 @@ SEPARATED = {"bf16x3": {"signed": ("code", "x_hat", "decoder", "encoder_bias", "
 
 def sign(variant):
     return "nonneg" if variant == "positive_tied" else "signed"
-
-
-def kink_window(Z):
-    return max(1e-5, 1e-4 * float(Z.double().pow(2).mean().sqrt()))
 
 
 def relnorm(a, b):
@@ -227,46 +226,6 @@ def scales(variant, f, b):
     return out
 
 
-class Worst:
-    """The worst tile and element of each output over the models of one check."""
-
-    def __init__(self):
-        self.tile, self.elem, self.minimum = {}, {}, {}
-
-    def add(self, name, m, r):
-        ratio, (_, tr, tc) = r["worst"]
-        if ratio >= self.tile.get(name, (-1.0,))[0]:
-            self.tile[name] = (ratio, (m, tr, tc))
-        self.elem[name] = max(self.elem.get(name, 0.0), r["elem"])
-        lo = float(r["ratio"].min()), float(r["peak"].min())
-        old = self.minimum.get(name, (float("inf"), float("inf")))
-        self.minimum[name] = (min(old[0], lo[0]), min(old[1], lo[1]))
-
-    def add_scalar(self, name, m, v):
-        if v >= self.tile.get(name, (-1.0,))[0]:
-            self.tile[name] = (v, (m,))
-        self.elem[name] = max(self.elem.get(name, 0.0), v)
-        self.minimum[name] = (min(self.minimum.get(name, (float("inf"),))[0], v),) * 2
-
-
-def engine_activity(code, counts, near, Z):
-    """[c > 0] as the engine gates the backward pass. The dense code is read back from the operand planes, where an f16f8
-    code below about 4e-9 (under the fp16 plane's subnormals and the scaled residual's) reads as 0 although the engine's
-    activity mask, the sign of its fp32 z, has it active: then the feature's mask count (``active_counts``) exceeds its
-    count of non-zero codes. Those coefficients lie inside the kink window with a zero code; each such feature gets as
-    many of them, the largest z first, back on the active side. A wrong pick could only fail the gradient check."""
-    pos = code > 0
-    missing = counts.long() - pos.sum(0)
-    assert int(missing.min()) >= 0, int(missing.min())
-    for j in torch.nonzero(missing).flatten().tolist():
-        cand = near[:, j] & ~pos[:, j]
-        k = int(missing[j])
-        assert int(cand.sum()) >= k, (j, k, int(cand.sum()))
-        zc = torch.where(cand, Z[:, j], torch.full_like(Z[:, j], -float("inf")))
-        pos[torch.topk(zc, k).indices, j] = True
-    return pos
-
-
 def regate_exact_zeros(variant, f, db_engine, candidates):
     """A pre-activation the engine computes as exactly 0 is inactive in its code and mask but passes the reconstruction
     gradient, without the L1 term (clamp's gradient at 0); the API does not read that bit back, and the pinned oracle has
@@ -300,20 +259,20 @@ def regate_exact_zeros(variant, f, db_engine, candidates):
 
 def measure(variant, ens, X, per_model):
     """Engine outputs of one grads_batch / forward_batch on X against the fp64 oracle, every model, every tile.
-    Returns (Worst, kink counts per model)."""
+    Returns (T.Worst, kink counts per model)."""
     grads, (loss, aux) = ens.grads_batch(X, expand_dims=not per_model)
     code = aux["c"].dense()
     counts = ens.active_counts(X.shape[-2])
     _, _, x_hat = ens.forward_batch(X, expand_dims=not per_model, return_x_hat=True)
-    w, kinks = Worst(), []
+    w, kinks = T.Worst(), []
     for m in range(ens.n_models):
         P = {k: v[m].double() for k, v in ens.params.items()}
         buf = {k: v[m] for k, v in ens.buffers.items()}
         Xm = (X[m] if per_model else X).double()
         f0 = oracle(variant, P, buf, Xm)
         Z = f0["Z"]
-        near = Z.abs() < kink_window(Z)
-        eng_pos = engine_activity(code[m], counts[m], near, Z)
+        near = Z.abs() < T.kink_window(Z)
+        eng_pos = T.engine_activity(code[m], counts[m], near, Z)
         across = eng_pos != (f0["c"] > 0)                      # (a masked coefficient is 0 on both sides)
         kinks.append((int(near.sum()), int((across & near).sum()), int((across & ~near).sum()), Z.numel()))
         del across
@@ -391,6 +350,21 @@ def test_ragged_shape_every_tile(variant, arith, per_model, inputs):
     run_case(tag, variant, models, sig, arith, RAGGED, per_model, inputs == "fp16")
 
 
+@pytest.mark.parametrize("inputs", ["fp16", "fp32"])
+@pytest.mark.parametrize("arith", ARITHS)
+@pytest.mark.parametrize("variant", ["tied", "untied"])
+def test_ragged_eager_shape_every_tile(variant, arith, inputs):
+    """M = 4, d = 400, n = 1040, B = 8001: ragged like the shape above but not launch-bound, so the step runs eagerly
+    and, under f16f8, the weight gradient takes the native E5M2 path (dw_native) with a partial tile in n, in d and in
+    K = B (Bp = 8016)."""
+    M, d, n, B = RAGGED_EAGER
+    assert not launch_bound(M, B, n, d)
+    models, sig = make_models(variant, M, d, n, 0)
+    tag = f"ragged eager {variant} {inputs}"
+    print(f"{tag}: step eager, dw_native {'yes' if arith == 'f16f8' else 'no'}")
+    run_case(tag, variant, models, sig, arith, RAGGED_EAGER, False, inputs == "fp16", seed=200)
+
+
 @pytest.mark.parametrize("arith", ARITHS)
 def test_config2_all_models_every_tile(arith):
     """BASELINE config 2 at full size (d = 512, n = 4096, B = 8192) with all 16 models across its L1 grid."""
@@ -463,8 +437,8 @@ def test_negative_control_single_pass_tile(arith):
     P = {k: v[m].double() for k, v in full.params.items()}
     buf = {k: v[m] for k, v in full.buffers.items()}
     f0 = oracle("tied", P, buf, X.double())
-    near = f0["Z"].abs() < kink_window(f0["Z"])
-    active = torch.where(near, engine_activity(code[m], counts[m], near, f0["Z"]), f0["Z"] > 0)
+    near = f0["Z"].abs() < T.kink_window(f0["Z"])
+    active = torch.where(near, T.engine_activity(code[m], counts[m], near, f0["Z"]), f0["Z"] > 0)
     f = oracle("tied", P, buf, X.double(), active)
     regate_exact_zeros("tied", f, grads["encoder_bias"][m], near & ~active & (code[m] == 0))
     S_x = T.x_hat_scale(f["Xabs"], f["W"], P["encoder_bias"], f["W"])

@@ -29,6 +29,7 @@ import torch
 import sparse_coding_b200 as S
 from oracle import interp_oracle as IO
 from oracle import sae_oracle as O
+from oracle.plan_paths import gather_classes, launch_bound, launches
 from sparse_coding_b200 import metrics as MT
 
 pytestmark = pytest.mark.gpu
@@ -86,49 +87,6 @@ def assert_exact_inputs(Sc, code, x_hat):
     assert sig_bits_at_most(Sc, 11) and sig_bits_at_most(code, 11)
     q = x_hat * 16
     assert bool((q == torch.round(q)).all()) and bool((x_hat.abs() < 2.0 ** 18).all())
-
-
-# ----------------------------------------------------------------------------------------------------------------
-# the engine's path, as plan_config (sce_plan.cu) decides it
-# ----------------------------------------------------------------------------------------------------------------
-def gather_classes(d, n, ks):
-    """Gather launches per call: non-empty k classes where the plan takes the gather path, else 0."""
-    kmax = max(ks)
-    if kmax > 256:
-        return 0
-    kr = (kmax + 7) // 8 * 8
-    slices = 0
-    for s in (2, 4, 8):
-        ds = d // s
-        if d % (4 * s) or ds > 512:
-            continue
-        if kr * ds * 4 + 9 * ds * 4 + kr * 8 + 128 <= 112 * 1024:
-            slices = s
-            break
-    if not slices or n < 96 * kr:
-        return 0
-    caps, lo, used = [16, 32, 64, kr], 0, 0
-    for g, cap in enumerate(caps):
-        cap = min(cap, kr)
-        if g > 0 and cap <= lo:
-            continue
-        used += any(lo < k <= cap for k in ks)
-        lo = cap
-        if cap == kr:
-            break
-    return used
-
-
-def launches(kind, classes, xm, arith):
-    """Kernel launches of one call: split of x per batch, l1/B, scores GEMM, selection, decode (gather classes or one
-    GEMM), finalize; backward adds the code-gradient scatter or GEMM and the weight-gradient GEMM; a step adds the
-    dictionary-row Adam kernel and, on the dense f16f8 path, the three transposes of the decoder planes."""
-    fwd = xm + 4 + (classes or 1)
-    if kind == "forward":
-        return fwd
-    if kind == "grads":
-        return fwd + 2
-    return fwd + 3 + (3 if arith == "f16f8" and not classes else 0)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -268,11 +226,6 @@ SEQUENCES = {
     # gather decode, not launch-bound: every step runs its launches eagerly
     "gather-eager": (1024, 6144, [16, 64], 1024),
 }
-
-
-def launch_bound(M, batch_max, n, d):
-    """plan_config's rule for replaying the step as a CUDA graph: ~30 M B n d tensor FLOPs below 3e11."""
-    return 30.0 * M * batch_max * n * d < 3e11
 
 
 @pytest.mark.parametrize("arith", ["bf16x3", "f16f8"])

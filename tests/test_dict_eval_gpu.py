@@ -2,21 +2,26 @@
 (golden fixture) under both arithmetics, evaluate_dicts at config-2 / config-5 / config-3 scale against the fp64 oracle
 on the device, bitwise agreement with evaluate_batches, repeatability, the fp16 range rule and the ABI's error paths.
 
-Tolerances, from the arithmetic's error model. Both arithmetics give each pre-activation z with an error below
-~1e-6 |x| |w| (bf16x3: 2^-16 per split product; f16f8: 2^-14 on the cross terms), i.e. ~1e-6 relative on each c,
-~4e-6 on c^4. The moments add these fp32 values in 32-row fp32 partials (relative error <= 32 * 2^-24 = 2e-6) and then
-in fp64. So sums of powers carry <= ~1e-5 relative error; the bar is 1e-4 (of the largest value of the vector, so that
-near-dead features are not judged on a relative scale). FVU is a ratio of two such sums: 1e-4 relative. Counts are
-exact outside the kink window (DESIGN §5, |z| < max(1e-5, 1e-4 rms(z))): any difference is bounded by the number of
-coefficients inside it. A top-k score inside the window around its row's k-th largest may be selected on the other
-side and move its feature's sums by a whole value: at scale that value is added to the feature's bar. skew / kurtosis divide by var^1.5 / var^2 and are compared where var >= 1e-3 max(var)."""
+Tolerances, per feature. Counts are exact outside the kink window (DESIGN §5, |z| < max(1e-5, 1e-4 rms(z))): feature
+j's row count may differ by at most its own coefficients inside the window (kink_j), and its times_active by at most
+its segments holding one. The moments (mean, var, m4, as the streaming average weights each row: 1 / (n_seg seg), the
+last partial segment's rows seg / r_last times that) are held to oracle/eval_bounds.py's bound of the sums under the
+same weights: e sum_b w_b p (c_b + e S_b)^(p-1) S_b + K sum_b w_b c_b^p, with e the code's element bar and S_b its
+absolute-product scale, plus (SAE variants) sum over feature j's kink coefficients of w_b window^p, and the final fp32
+rounding. A top-k score inside the window around its row's k-th largest may be selected on the other side and move its
+feature's sums by a whole value: that value (selection_slack) is added to the feature's bound. The drop-ins' golden
+results, which the reference computed in fp32, are held to the same per-feature bounds against the fp64 oracle on the
+same activations, and to 1e-4 of the largest value against the golden values themselves. FVU is a ratio of two sums:
+1e-4 relative. skew / kurtosis divide by var^1.5 / var^2 and are compared where var >= 1e-3 max(var)."""
 import ctypes as C
 
 import pytest
 import torch
 
 import sparse_coding_b200 as S
+from oracle import eval_bounds as EB
 from oracle import eval_oracle as O
+from oracle import tile_bounds as T
 from sparse_coding_b200 import _lib
 from sparse_coding_b200 import metrics as MT
 
@@ -43,6 +48,52 @@ def kink_coefficients(m, x, centred, rows=8192):
 
 def n_kink(m, x, centred):
     return int(kink_coefficients(m, x, centred).sum())
+
+
+def feature_bounds(m, x, centred, segment, arith="bf16x3", rows=8192):
+    """Per feature of dictionary ``m`` on the fp64 activations ``x`` for a pass at ``segment`` (module docstring):
+    ``kink`` [n] its coefficients inside the kink window, ``seg_kink`` [n] its segments holding one, and ``moments``
+    [n, 4] the bound on its streaming means of c, c^2, c^3, c^4."""
+    xs = O.center(m, x) if centred else x
+    N, topk = x.shape[0], m["kind"] == "topk"
+    near = kink_coefficients(m, x, centred, rows)
+    z2 = sum(float(O.pre_activations(m, xs[i:i + rows]).pow(2).sum()) for i in range(0, N, rows))
+    window = max(1e-5, 1e-4 * (z2 / (N * near.shape[1])) ** 0.5)
+    n_seg = -(-N // segment)
+    last = (n_seg - 1) * segment
+    weight = torch.full((N,), 1.0 / (n_seg * segment), dtype=torch.float64, device=x.device)
+    weight[last:] *= segment / (N - last)
+    pad = torch.zeros(n_seg * segment - N, near.shape[1], dtype=torch.bool, device=x.device)
+    seg_kink = torch.cat([near, pad]).reshape(n_seg, segment, -1).any(1).sum(0)
+    if topk:
+        e, K = T.TOPK_BARS[arith]["code"][1], EB.K_RUNNING
+        W = torch.nn.functional.normalize(m["dict"], dim=-1)
+    else:
+        e, K = T.BARS[arith]["signed"]["code"][1], EB.K_TREE
+        W = O.learned(m) if m["kind"] == "tied" else m["encoder"]
+    bound = torch.zeros(near.shape[1], 4, dtype=torch.float64, device=x.device)
+    for i in range(0, N, rows):
+        xr, sr = x[i:i + rows], xs[i:i + rows]
+        c = O.encode(m, sr)
+        if topk:
+            S_c = (sr.abs() @ W.abs().T) * (c != 0)
+        else:
+            cen = centred and "center_trans" in m
+            Xabs = T.centered_input_scale(xr, m["center_trans"], m["center_rot"], m["center_scale"]) if cen else sr.abs()
+            S_c = T.code_scale(Xabs, W, m["encoder_bias"])
+        bound += EB.moment_bound(c, S_c, e, K, weight[i:i + rows])
+        del c, S_c
+    if not topk:
+        wk = (weight[:, None] * near).sum(0)
+        bound += torch.stack([wk * window ** p for p in (1, 2, 3, 4)], dim=-1)
+    return {"kink": near.sum(0), "seg_kink": seg_kink, "moments": bound}
+
+
+def check_counts(got, want, kink, what):
+    """Per feature: |got_j - want_j| <= kink_j."""
+    diff = (got.double().to(want.device) - want.double()).abs()
+    bad = diff > kink.double().to(want.device)
+    assert not bool(bad.any()), (what, int(bad.sum()), float((diff - kink.double().to(want.device)).max()))
 
 
 def selection_slack(m, x, centred, segment, rows=8192):
@@ -89,26 +140,38 @@ def close(got, want, what, rtol=RTOL):
     assert err <= rtol * max(scale, 1e-30) + 1e-12, (what, err, scale)
 
 
-def check_moments(got, want, kink, what, slack=None):
-    """``slack``: selection_slack (top-k), added per feature to the bars of mean, var and m4; skew and kurtosis are
-    then compared on the features without any."""
+def check_moments(got, want, fb, what, slack=None):
+    """Per feature against the fp64 ``want`` (oracle.eval_oracle.calc_moments_streaming): times_active within its
+    kink-holding segments, mean / var / m4 within feature_bounds' moment bound (``fb``), plus ``slack``
+    (selection_slack, top-k) per feature; skew and kurtosis are then compared on the features without any."""
+    times, mean, var, skew, kurt, m4 = (t.double().to(want[0].device) for t in got)
+    wt, wm, wv, ws, wk, w4 = (t.double() for t in want)
+    check_counts(times, wt, fb["seg_kink"], (what, "times_active"))
+    b1, b2, _, b4 = fb["moments"].unbind(-1)
+    if slack is not None:
+        s1, s2, _, s4 = slack
+        b1, b2, b4 = b1 + s1, b2 + s2, b4 + s4
+    bv = b2 + 2 * wm.abs() * b1 + b1 * b1 + 2.0 ** -50 * (wv.abs() + 2 * wm * wm)
+    for a, b, bd, k in ((mean, wm, b1, "mean"), (var, wv, bv, "var"), (m4, w4, b4, "m4")):
+        err = (a - b).abs()
+        lim = bd + 2.0 ** -23 * (b.abs() + bd)            # (+ the result's rounding to fp32)
+        assert bool((err <= lim).all()), (what, k, int((err > lim).sum()), float((err / lim).max()))
+    ok = wv >= 1e-3 * wv.max()
+    if slack is not None:
+        ok &= slack[0] == 0
+    for a, b, k in ((skew, ws, "skew"), (kurt, wk, "kurtosis")):
+        a, b = a[ok], b[ok]
+        assert ((a - b).abs() <= 1e-3 * b.abs() + 1e-6).all(), (what, k, ((a - b).abs() / b.abs()).max())
+
+
+def check_moments_golden(got, want, kink, what):
+    """Against the reference's own fp32 results: mean, var and m4 within 1e-4 of the vector's largest value, and
+    times_active within the kink coefficients in total."""
     times, mean, var, skew, kurt, m4 = got
     wt, wm, wv, ws, wk, w4 = want
     assert float((times.double().cpu() - wt.double().cpu()).abs().sum()) <= kink, (what, "times_active")
-    if slack is None:
-        for a, b, k in ((mean, wm, "mean"), (var, wv, "var"), (m4, w4, "m4")):
-            close(a, b, (what, k))
-        ok = wv >= 1e-3 * wv.max()
-    else:
-        s1, s2, _, s4 = slack
-        sv = s2 + 2 * wm.abs() * s1 + s1 * s1
-        for a, b, sl, k in ((mean, wm, s1, "mean"), (var, wv, sv, "var"), (m4, w4, s4, "m4")):
-            err = (a.double().to(b.device) - b).abs()
-            assert (err <= RTOL * b.abs().max() + sl + 1e-12).all(), (what, k, float((err - sl).max()))
-        ok = (wv >= 1e-3 * wv.max()) & (s1 == 0)
-    for a, b, k in ((skew, ws, "skew"), (kurt, wk, "kurtosis")):
-        a, b = a.double().to(b.device)[ok], b[ok]
-        assert ((a - b).abs() <= 1e-3 * b.abs() + 1e-6).all(), (what, k, ((a - b).abs() / b.abs()).max())
+    for a, b, k in ((mean, wm, "mean"), (var, wv, "var"), (m4, w4, "m4")):
+        close(a, b, (what, k))
 
 
 @pytest.mark.parametrize("arith", ["bf16x3", "f16f8"])
@@ -126,10 +189,16 @@ def test_drop_ins_match_reference_golden(golden, arith):
             assert isinstance(got, int) and abs(got - want) <= kink, (what, got, want, kink)
         elif c["fn"] == "mean_nonzero_activations":
             assert got.device == x.device and got.shape == want.shape
-            assert float((got.double().cpu() - want.double()).abs().sum()) * x.shape[0] <= kink + 1e-6, what
+            # both are counts / N rounded to fp32: back to whole counts, then per feature within its kink coefficients
+            n_got, n_want = got.double() * x.shape[0], want.double().to(DEV) * x.shape[0]
+            assert float((n_got - n_got.round()).abs().max()) < 1e-3 and float((n_want - n_want.round()).abs().max()) < 1e-3
+            check_counts(n_got.round(), n_want.round(), kink_coefficients(m, x.double(), centred=True).sum(0), what)
         elif c["fn"] == "calc_moments_streaming":
             assert len(got) == 6 and all(t.device == x.device and t.dtype == torch.float32 for t in got)
-            check_moments(got, tuple(w.to(DEV) for w in want), kink, what)
+            check_moments_golden(got, tuple(w.to(DEV) for w in want), kink, what)
+            bs = c["kwargs"].get("batch_size", 1000)
+            check_moments(got, O.calc_moments_streaming(m, x.double(), bs), feature_bounds(m, x.double(), False, bs, arith),
+                          what, slack=selection_slack(m, x.double(), False, bs))
         else:
             assert got.device == x.device and got.dim() == 0
             close(got, want.to(DEV), what)
@@ -140,13 +209,14 @@ def score_against_oracle(lds, x, segment=1000, threshold=10, arith="auto"):
     xd = x.double()
     for i, (ld, r) in enumerate(zip(lds, res)):
         m = from_ld(ld)
-        kink = n_kink(m, xd, centred=True)
+        fb = feature_bounds(m, xd, True, segment, "bf16x3" if arith == "auto" else arith)
+        kink = int(fb["kink"].sum())
         close(r["fvu"], O.fraction_variance_unexplained(m, xd), (i, "fvu"))
         counts = O.feature_counts(m, xd, centred=True)
-        assert int((r["feature_counts"].long() - counts).abs().sum()) <= kink, (i, "counts", kink)
+        check_counts(r["feature_counts"], counts, fb["kink"], (i, "feature_counts"))
         assert int((r["n_ever_active"] - (counts > threshold).sum()).abs()) <= kink
         want = O.calc_moments_streaming(m, xd, segment, centred=True)
-        check_moments([r[k] for k in ("times_active", "mean", "var", "skew", "kurtosis", "m4")], want, kink, i,
+        check_moments([r[k] for k in ("times_active", "mean", "var", "skew", "kurtosis", "m4")], want, fb, i,
                       slack=selection_slack(m, xd, True, segment))
         print(f"dict {i}: fvu {float(r['fvu']):.5f} mean_l0 {float(r['mean_l0']):.2f} kink {kink}")
     return res
@@ -205,15 +275,13 @@ def test_segment_longer_than_an_engine_call():
     ld = S.TiedSAE(torch.randn(1024, 256, device=DEV), torch.randn(1024, device=DEV) * 0.1 - 0.45)
     x = synth(50000, 256, 9)
     m, xd = from_ld(ld), x.double()
-    kink = n_kink(m, xd, centred=False)
     for bs in (20000, 8193, 1000, 1):
         got = MT.calc_moments_streaming(ld, x, batch_size=bs)
-        want = O.calc_moments_streaming(m, xd, bs) if bs > 1 else None
-        if want is None:                                              # every row its own segment: row counts
-            assert torch.equal(got[0].long(), O.feature_counts(m, xd)) or \
-                float((got[0].double() - O.feature_counts(m, xd).double()).abs().sum()) <= kink
+        fb = feature_bounds(m, xd, False, bs)
+        if bs == 1:                                                   # every row its own segment: row counts
+            check_counts(got[0], O.feature_counts(m, xd), fb["kink"], (bs, "times_active"))
         else:
-            check_moments(got, want, kink, bs)
+            check_moments(got, O.calc_moments_streaming(m, xd, bs), fb, bs)
 
 
 @pytest.mark.parametrize("sig", ["tied", "untied", "masked"])

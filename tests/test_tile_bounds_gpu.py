@@ -84,30 +84,7 @@ NEAR_FRAC = 5e-4                     # bound on the share of coefficients inside
 EXACT_ZERO_FLOOR = 3e-5              # bias-gradient error / scale above which an exact-zero pre-activation is looked for
 TILE_OUTPUTS = ("code", "x_hat", "encoder", "decoder", "encoder_bias", "center")
 
-# (tile ratio bar, element bar) per arithmetic, dictionary sign and output; "loss" is one relative error per loss term.
-# FunctionalPositiveTiedSAE ("nonneg") has its own: every product of its encode and decode has one sign, so the fp32
-# accumulation of the tensor cores, not the operand split, sets its 3-pass error.
-BARS = {
-    "bf16x3": {
-        "signed": {"code": (6.5e-7, 6.3e-6), "x_hat": (5.8e-8, 3.2e-7), "loss": (6.3e-5, 6.3e-5),
-                   "encoder": (1.1e-5, 1.9e-4), "decoder": (6.5e-6, 2.6e-5), "encoder_bias": (5.3e-6, 5.6e-5),
-                   "center": (7.6e-8, 2.1e-7)},
-        "nonneg": {"code": (3.6e-6, 1.2e-5), "x_hat": (5.5e-6, 8.2e-6), "loss": (2.3e-5, 2.3e-5),
-                   "encoder": (2.7e-5, 9.2e-5), "encoder_bias": (1.5e-5, 1.6e-5)},
-    },
-    "f16f8": {
-        "signed": {"code": (2.8e-6, 2.5e-5), "x_hat": (1.6e-7, 8.8e-7), "loss": (1.7e-4, 1.7e-4),
-                   "encoder": (1.4e-5, 3.8e-4), "decoder": (7.0e-5, 2.5e-4), "encoder_bias": (1.6e-5, 1.1e-4),
-                   "center": (1.2e-7, 3.7e-7)},
-        "nonneg": {"code": (1.7e-5, 5.2e-5), "x_hat": (1.7e-5, 2.5e-5), "loss": (6.9e-5, 6.9e-5),
-                   "encoder": (5.4e-5, 1.7e-4), "encoder_bias": (3.9e-5, 4.3e-5)},
-    },
-}
-# outputs whose tile bar sits at most half the smallest 1-pass tile ratio: the single-pass runs must clear it, and only
-# these get a negative-control claim (the others are listed in the module docstring)
-SEPARATED = {"bf16x3": {"signed": ("code", "x_hat", "decoder", "encoder_bias", "center"),
-                        "nonneg": ("code", "x_hat", "encoder_bias")},
-             "f16f8": {"signed": ("code", "x_hat"), "nonneg": ()}}
+BARS, SEPARATED = T.BARS, T.SEPARATED   # (tile ratio bar, element bar) and the separated outputs: see the docstring
 
 
 def sign(variant):

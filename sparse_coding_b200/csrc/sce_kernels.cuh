@@ -210,9 +210,14 @@ enum { MODE_PREPARE = 0, MODE_ADAM = 1, MODE_GRAD = 2 };
 __device__ __forceinline__ float4 nonneg4(const float4& e) {
   return make_float4(fmaxf(e.x, 0.f), fmaxf(e.y, 0.f), fmaxf(e.z, 0.f), fmaxf(e.w, 0.f));
 }
-// NONNEG rows: the sum of squares in explicitly rounded steps, so that the norm MODE_ADAM re-splits the updated row with
-// and the one MODE_PREPARE derives from the same row are bitwise equal (a resumed run prepares its planes afresh), which
-// free contraction of the two loops does not guarantee
+// The row sums and the Jacobian in explicitly rounded steps: every instantiation then rounds them alike, which free
+// contraction does not guarantee (MODE_GRAD and MODE_ADAM of one width had fused different products). So the gradient
+// MODE_ADAM applies is bitwise the one MODE_GRAD returns (sce_grads). dot4_rn is the order the step's kernels were
+// compiled to. NONNEG rows take the sum of squares as sumsq4_rn, so that the norm MODE_ADAM re-splits the updated row
+// with and the one MODE_PREPARE derives from the same row are bitwise equal (a resumed run prepares its planes afresh).
+__device__ __forceinline__ float dot4_rn(const float4& a, const float4& b) {
+  return __fmaf_rn(a.w, b.w, __fmaf_rn(a.z, b.z, __fmaf_rn(a.x, b.x, __fmul_rn(a.y, b.y))));
+}
 __device__ __forceinline__ float sumsq4_rn(const float4& v) {
   return __fmaf_rn(v.w, v.w, __fmaf_rn(v.z, v.z, __fmaf_rn(v.y, v.y, __fmul_rn(v.x, v.x))));
 }
@@ -242,8 +247,8 @@ __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, c
       if constexpr (NONNEG) ev[i] = nonneg4(ev[i]);
     }
     if constexpr (NONNEG) ss = __fadd_rn(ss, sumsq4_rn(ev[i]));
-    else ss += ev[i].x * ev[i].x + ev[i].y * ev[i].y + ev[i].z * ev[i].z + ev[i].w * ev[i].w;
-    dot += ev[i].x * gv[i].x + ev[i].y * gv[i].y + ev[i].z * gv[i].z + ev[i].w * gv[i].w;
+    else ss = __fadd_rn(ss, dot4_rn(ev[i], ev[i]));
+    dot = __fadd_rn(dot, dot4_rn(ev[i], gv[i]));
   }
   float s = 1.f;
   if (normalize) {
@@ -257,10 +262,10 @@ __global__ void __launch_bounds__(128) dict_rows_kernel(float* __restrict__ e, c
       const float k = clamped ? 0.f : dot * inv * inv * inv;  // clamp active: d s / d e = 0
 #pragma unroll
       for (int i = 0; i < NV; ++i) {
-        gv[i].x = gv[i].x * inv - ev[i].x * k;
-        gv[i].y = gv[i].y * inv - ev[i].y * k;
-        gv[i].z = gv[i].z * inv - ev[i].z * k;
-        gv[i].w = gv[i].w * inv - ev[i].w * k;
+        gv[i].x = __fmaf_rn(gv[i].x, inv, -__fmul_rn(ev[i].x, k));
+        gv[i].y = __fmaf_rn(gv[i].y, inv, -__fmul_rn(ev[i].y, k));
+        gv[i].z = __fmaf_rn(gv[i].z, inv, -__fmul_rn(ev[i].z, k));
+        gv[i].w = __fmaf_rn(gv[i].w, inv, -__fmul_rn(ev[i].w, k));
       }
     }
   }
@@ -348,7 +353,8 @@ __global__ void bias_kernel(float* __restrict__ bias, float* __restrict__ m, flo
   const float* p = db_part + (long long)model * n_part * n + j;
   float g = 0.f;
   for (int k = 0; k < n_part; ++k) g += p[(long long)k * n];
-  g *= part_scale;  // f16f8: the partials are sums of dz * B d / 2 (see EpiDecodeT)
+  g = __fmul_rn(g, part_scale);  // f16f8: the partials are sums of dz * B d / 2 (see EpiDecodeT); not fused with the
+                                 // decay term, so that MODE_GRAD and MODE_ADAM round it alike
   const float b = bias[i];
   if (bias_decay) {
     const float bd = bias_decay[model], nb = bnorm[model];

@@ -209,7 +209,7 @@ __global__ void center_grad_kernel(const float* __restrict__ g_part, int n_gpart
   const float* pp = part + (long long)model * n_chunks * d + c;
   float dw = 0.f;
   for (int k = 0; k < n_chunks; ++k) dw += pp[(long long)k * d];
-  const float g = gs * g_scale - dw;
+  const float g = __fmaf_rn(gs, g_scale, -dw);   // (explicit: MODE_GRAD and MODE_ADAM round it alike)
   grad[i] = g;
   if (MODE == MODE_ADAM) {
     if (step_is_bad(health)) return;

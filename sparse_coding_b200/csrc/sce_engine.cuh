@@ -300,7 +300,8 @@ __global__ void __launch_bounds__(256) transpose_batch_u8_kernel(BatchPlanes t, 
 }  // namespace sce
 
 // The batch-major copy T [models][cols][ld] of the 8-bit planes of P [models][rows][cols] (`src_pitch` elements between
-// models), from which the native weight gradient reads them (dw_operand_maps; dz's are written so by dcode)
+// models), from which the native weight gradient reads them (dw_operand_maps; the code's, g's and dz's are written so
+// by the encode, decode and dcode epilogues)
 static int batch_major(Launcher& L, const Planes& P, const Planes& T, int models, int rows, int cols, long long src_pitch,
                        int ld) {
   const BatchPlanes t{{static_cast<const uint8_t*>(P.lo), P.x8}, {static_cast<uint8_t*>(T.lo), T.x8}};

@@ -73,6 +73,29 @@ __device__ __forceinline__ void stage_col32_u8(uint8_t* tile, int lane, const ui
     out[(2 * q + 1) * 32] = __byte_perm(z1, t, s2_hi);
   }
 }
+// The same transpose stored straight to global memory, without staging: tile row j (a column of the 32-row block) goes
+// to dst + j * ld, each store instruction writing four whole 32-byte segments. Only tile rows below `cols` (a multiple
+// of 16, as f16f8 shapes are) and words whose first byte lies below `rows` are written; a word that crosses `rows` writes
+// up to three bytes beyond it, which stay inside the row pitch ld (a multiple of 16 at least `rows`) and which no reader
+// of the copy looks at. (Its own copy of the exchange: sharing one with stage_col32_u8 moved the dcode kernel's
+// instruction schedule.)
+__device__ __forceinline__ void store_col32_u8(uint8_t* dst, int ld, int lane, const uint32_t* w /*[8]*/, int rows,
+                                               int cols) {
+  const bool h = lane & 2, l = lane & 1;
+  const uint32_t s1_send = h ? 0x5410 : 0x7632, s1_lo = h ? 0x3254 : 0x5410, s1_hi = h ? 0x3276 : 0x7610;
+  const uint32_t s2_send = l ? 0x6420 : 0x7531, s2_lo = l ? 0x3514 : 0x5240, s2_hi = l ? 0x3716 : 0x7260;
+  const bool lo_ok = 4 * (lane >> 2) < rows, hi_ok = lo_ok && cols > 16;   // tile rows 0 .. 15, 16 .. 31
+  uint8_t* out = dst + (lane & 3) * ld + 4 * (lane >> 2);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const uint32_t x0 = w[2 * q], x1 = w[2 * q + 1];
+    uint32_t t = __shfl_xor_sync(0xffffffffu, __byte_perm(x0, x1, s1_send), 2);
+    const uint32_t z0 = __byte_perm(x0, t, s1_lo), z1 = __byte_perm(x1, t, s1_hi);
+    t = __shfl_xor_sync(0xffffffffu, __byte_perm(z0, z1, s2_send), 1);
+    st_global_u32_if(out + 8 * q * ld, __byte_perm(z0, t, s2_lo), q < 2 ? lo_ok : hi_ok);
+    st_global_u32_if(out + (8 * q + 4) * ld, __byte_perm(z1, t, s2_hi), q < 2 ? lo_ok : hi_ok);
+  }
+}
 // whole warp: wait until the share's staging tiles may be written (staging_wait), write them, launch their stores.
 // bf16x3: whi / wx are the hi / lo planes. f16f8: whi is the fp16 plane, wx[0..7] the value-e5m2 plane and
 // wx[8..15] the residual-e5m2 plane (maps m_lo / m_x8).
@@ -215,19 +238,42 @@ struct EncodeMomentParams<true> {
   int row_blocks;    // ceil(B / 32)
 };
 
+// Batch-major copies of an epilogue's two 8-bit planes (T8 of EpiEncodeT and EpiDecodeT, f16f8 plans whose weight
+// gradient runs native): [M][cols][ld], ld = batch_max rounded up to 16, as the weight gradient reads them (K-major over
+// the batch). Written besides the row-major planes, straight from the epilogue's registers (store_col32_u8).
+template <bool T8>
+struct BatchMajorParams {};
+template <>
+struct BatchMajorParams<true> {
+  uint8_t* t_lo;   // value-e5m2 plane
+  uint8_t* t_x8;   // residual-e5m2 plane
+  int t_ld;
+};
+
+// the batch-major copies of the 8-bit planes wx of the warp's 32 rows from row0 and 32 columns from col (T8)
+__device__ __forceinline__ void store_batch_major(const BatchMajorParams<true>& P, const TileCoord& t, const uint32_t (&wx)[16],
+                                                  int col, int row0, int m_total, int n_total) {
+  const long long off = ((long long)t.model * n_total + col) * P.t_ld + row0;
+  store_col32_u8(P.t_lo + off, P.t_ld, t.lane, &wx[0], m_total - row0, n_total - col);
+  store_col32_u8(P.t_x8 + off, P.t_ld, t.lane, &wx[8], m_total - row0, n_total - col);
+}
+
 // ------------------------------------------------------------------------------------------------
 // encode:  c = relu(acc + bias) -> (c_hi, c_lo);  per-tile partial sums of |c| and count(c > 0)
 // [c > 0] and [z == 0] (clamp(min=0)'s gradient of 1 at exactly 0, SURVEY.md Q4) go to the activity masks, so the
 // backward pass needs neither z nor the code.
 // STATS (compile-time, evaluation only) adds the moment partials of EncodeMomentParams; the training instantiations
 // (STATS = false) compile to the same code as without the switch.
+// T8 (f16f8 training steps with a native weight gradient) also writes the batch-major copies of BatchMajorParams; the
+// row-major planes are stored as without it (the decode GEMM reads the 8-bit ones).
 // ------------------------------------------------------------------------------------------------
-template <int ARITH, bool STATS = false>
+template <int ARITH, bool STATS = false, bool T8 = false>
 struct EpiEncodeT {
+  static_assert(!T8 || (ARITH == kArithF16F8 && !STATS), "batch-major copies: f16f8 training steps only");
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 4096;
   static constexpr bool kInline = STATS;   // the moment sums do not fit the epilogue warpgroup's registers (sce_gemm.cuh)
-  struct Params : EncodeMomentParams<STATS> {
+  struct Params : EncodeMomentParams<STATS>, BatchMajorParams<T8> {
     CUtensorMap out_hi, out_lo, out_x8;  // store maps of the code planes: [M][B][n], box 32 x 32
     const float* bias;             // [M, n] or nullptr
     const unsigned char* mask;     // [M, n] (1 = coefficient unused) or nullptr
@@ -317,6 +363,7 @@ struct EpiEncodeT {
     }
     stage_and_store<ARITH>(stage, T, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, T.m_blk * kBM + T.warp_q * 32,
                            T.model);
+    if constexpr (T8) store_batch_major(P, T, wlo, col, T.m_blk * kBM + T.warp_q * 32, m_total, n_total);
     if constexpr (STATS) {
       if (T.m_blk * kBM + T.warp_q * 32 < m_total) {   // warp-uniform: some row of this warp is in the batch
         float* o = P.mom_part + ((long long)T.model * P.row_blocks + T.m_blk * 4 + T.warp_q) * 4 * n_total + col + T.lane;
@@ -363,14 +410,18 @@ struct DecodeGsumParams<true> {
 // (~1e-7), so the backward pass runs on the residual itself and its consumers carry the factor (dcode adds
 // alpha d/2 instead of alpha/B; the weight- and bias-gradient outputs are multiplied by 2/(B d)).
 // GSUM (compile-time) adds the column sums of DecodeGsumParams; there rows beyond the batch stay in the warp (as zeros)
-// for the transpose-reduce. The instantiations without it compile to the same code as without the switch.
+// for the transpose-reduce. T8 (f16f8 training steps with a native weight gradient) also writes the batch-major copies
+// of g's 8-bit planes (BatchMajorParams), through a lane-quad transpose for which the rows beyond the batch stay in the
+// warp as well. The instantiations without the switches compile to the same code as without them.
 // ------------------------------------------------------------------------------------------------
-template <int ARITH, bool GSUM = false>
+template <int ARITH, bool GSUM = false, bool T8 = false>
 struct EpiDecodeT {
+  static_assert(!T8 || ARITH == kArithF16F8, "batch-major copies: f16f8 only");
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 0;
   static constexpr bool kInline = true;   // a few percent of a tile beside a K = n main loop (sce_gemm.cuh)
-  struct Params : DecodeGsumParams<GSUM> {
+  static constexpr bool kWarpRows = GSUM || T8;   // rows beyond the batch run the chunk with the warp (as zeros)
+  struct Params : DecodeGsumParams<GSUM>, BatchMajorParams<T8> {
     const float* x;                // [B, d] (x_model_stride = 0) or [M, B, d]
     long long x_model_stride;
     uint16_t* g_hi;                // [M, B, d] 16-bit plane
@@ -409,12 +460,12 @@ struct EpiDecodeT {
 #pragma unroll
     for (int j = 0; j < 8; ++j) xc[j] = xn[j];
     fetch_x(c + 64);  // this warp's next chunk (harmless past the tile: predicated on n_total, unused)
-    if constexpr (GSUM) {
+    if constexpr (kWarpRows) {
       if (col >= n_total) return;  // warp-uniform
     } else {
       if (col >= n_total || T.row >= m_total) return;
     }
-    const bool row_ok = !GSUM || T.row < m_total;
+    const bool row_ok = !kWarpRows || T.row < m_total;
     const long long off = (long long)T.model * P.g_model_stride + (long long)T.row * P.ld + col;
     uint32_t whi[16], wlo[16];
     // GSUM: every row block of a tile in the batch writes its column sums (as EpiDcodeT's db_part); warp-uniform. They are
@@ -458,6 +509,7 @@ struct EpiDecodeT {
         store_bf16x32(reinterpret_cast<__nv_bfloat16*>(P.g_lo) + off, wlo, n_total - col);
       }
     }
+    if constexpr (T8) store_batch_major(P, T, wlo, col, T.m_blk * kBM + T.warp_q * 32, m_total, n_total);
     if constexpr (GSUM) {
       if (gsum && col + T.lane < n_total)
         P.g_part[(((long long)T.model * P.tiles_m + T.m_blk) * 4 + T.warp_q) * n_total + col + T.lane] = gs;

@@ -337,7 +337,8 @@ struct PlanBuffers {
                                   // dw_native: the 8-bit planes are [M, n, Bp]
   // dw_native (dense f16f8 plans): batch-major copies of the 8-bit planes of x, c and g, [xm or M, cols, Bp] with Bp =
   // batch_max rounded up to 16 (TMA pitch): the weight gradient reads them K-major over the batch (E5M2 wgmma).
-  // dz's 8-bit planes are written in that layout in the first place (EpiDcodeT<f16f8, true>).
+  // x's are made by a transpose pass (batch_major); the epilogues that produce c and g write their copies besides the
+  // row-major planes (EpiEncodeT / EpiDecodeT with T8), and dz's 8-bit planes exist only in that layout (EpiDcodeT<f16f8, true>).
   Planes xt, ct, gt;
   Planes rot;                     // centring: operand planes of buffers["center_rot"] [M, d, d]
   float* x_centered;              // centring, learned centre: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
@@ -489,7 +490,7 @@ static PlanConfig plan_config(const sce_desc& d) {
   // which the weight gradient forms its cross terms on E5M2 wgmma. Top-k plans do not: their code and (k-sparse)
   // code-gradient planes are written by the selection / scatter kernels, row-major only, so their weight gradient widens
   // the 8-bit tiles. Nor do launch-bound plans: there the weight gradient takes microseconds either way, and the copies
-  // would add three launches per step and a third to the workspace.
+  // would add a launch per step (x's transpose pass) and a third to the workspace.
   c.dw_native = c.arith == kArithF16F8 && !c.topk && d.bwd_passes >= 3 && !launch_bound;
   // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
   // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
@@ -851,14 +852,23 @@ static int encode_phase(PlanCall& c, bool tdw, float* mom_part) {
       fill(ep);
       ep.mom_part = mom_part;
       ep.row_blocks = (B + 31) / 32;
-      TRY((c.gemm<EpiStats, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep, x_is_a)));
-    } else {
-      typename EpiEncodeT<AR>::Params ep;
-      fill(ep);
-      TRY((c.gemm<EpiEncodeT<AR>, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep,
-                                                           x_is_a)));
+      return c.gemm<EpiStats, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep, x_is_a);
     }
-    return tdw ? batch_major(c, p->c, p->ct, M, B, n, (long long)d.batch_max * n, cfg.bpad) : SCE_OK;
+    if constexpr (AR == kArithF16F8) {
+      if (tdw) {   // the epilogue also writes the batch-major copies of the code's 8-bit planes the weight gradient reads
+        using EpiT8 = EpiEncodeT<AR, false, true>;
+        typename EpiT8::Params ep;
+        fill(ep);
+        ep.t_lo = static_cast<uint8_t*>(p->ct.lo);
+        ep.t_x8 = p->ct.x8;
+        ep.t_ld = cfg.bpad;
+        return c.gemm<EpiT8, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep, x_is_a);
+      }
+    }
+    typename EpiEncodeT<AR>::Params ep;
+    fill(ep);
+    return c.gemm<EpiEncodeT<AR>, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep,
+                                                          x_is_a);
   }
   // scores -> fp32 and the chunk maxima of every row, then per-row selection (code planes, activity mask, k-sparse
   // lists) from the chunk maxima (the kernel reads whole rows where they cannot bound the k-th largest score)
@@ -882,7 +892,7 @@ static int decode_phase(PlanCall& c, const float* x, float* x_hat, bool backward
   sce_plan* const p = c.p;
   const sce_desc& d = p->d;
   const PlanConfig& cfg = p->cfg;
-  const int B = c.B, M = d.n_models, n = d.n, dd = d.d;
+  const int B = c.B, n = d.n, dd = d.d;
   const float gscale = f8 ? 1.0f : 2.0f / ((float)B * (float)dd);
   if (cfg.topk_sparse) {
     CUDA_TRY(opt_in_smem<topk_sparse_kernel<AR>>(112 * 1024, p->device));
@@ -915,7 +925,12 @@ static int decode_phase(PlanCall& c, const float* x, float* x_hat, bool backward
     dp.tiles_m = (B + kBM - 1) / kBM;
     dp.gscale = gscale;
     dp.tiles_n = (dd + kBN - 1) / kBN;
-    if constexpr (!std::is_same<E, EpiDecodeT<AR>>::value) dp.g_part = p->g_part;
+    if constexpr (std::is_base_of<DecodeGsumParams<true>, typename E::Params>::value) dp.g_part = p->g_part;
+    if constexpr (std::is_base_of<BatchMajorParams<true>, typename E::Params>::value) {
+      dp.t_lo = static_cast<uint8_t*>(p->gt.lo);
+      dp.t_x8 = p->gt.x8;
+      dp.t_ld = cfg.bpad;
+    }
     if constexpr (f8)
       return c.gemm<E, false, false, false, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
     else if (cfg.split_decode)
@@ -923,8 +938,10 @@ static int decode_phase(PlanCall& c, const float* x, float* x_hat, bool backward
     else
       return c.gemm<E, false, true, false, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
   };
-  TRY(cfg.learned ? decode(TypeTag<EpiDecodeT<AR, true>>{}) : decode(TypeTag<EpiDecodeT<AR>>{}));
-  return tdw ? batch_major(c, p->g, p->gt, M, B, dd, (long long)d.batch_max * dd, cfg.bpad) : SCE_OK;
+  // tdw: the epilogue also writes the batch-major copies of g's 8-bit planes the weight gradient reads
+  if constexpr (f8)
+    if (tdw) return cfg.learned ? decode(TypeTag<EpiDecodeT<AR, true, true>>{}) : decode(TypeTag<EpiDecodeT<AR, false, true>>{});
+  return cfg.learned ? decode(TypeTag<EpiDecodeT<AR, true>>{}) : decode(TypeTag<EpiDecodeT<AR>>{});
 }
 
 // Losses: the bias norm (bias decay), then the loss columns and nnz from the partials of encode and decode

@@ -145,6 +145,15 @@ __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
+// A 4-byte global store made only where `ok`, as one predicated instruction. Where an epilogue writes words under
+// conditions that differ per word (store_col32_u8), a C++ `if` around each store costs branches and registers: the encode
+// kernel spilled at its 128-register launch bound with them, and does not with this.
+__device__ __forceinline__ void st_global_u32_if(void* p, uint32_t v, bool ok) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.b32 [%0], %1;\n\t}" ::"l"(p), "r"(v),
+               "r"((uint32_t)ok)
+               : "memory");
+}
+
 // ----------------------------------------------------------------------------------------------
 // wgmma shared-memory matrix descriptor (sm_90). Fields (PTX ISA "Matrix Descriptor Format"):
 // [0,14) start address >> 4, [16,30) leading byte offset >> 4, [32,46) stride byte offset >> 4,

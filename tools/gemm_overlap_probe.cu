@@ -169,6 +169,8 @@ int main(int argc, char** argv) {
   const int M = 16, d = 512, n = 4096, B = 8192, sms = prop.multiProcessorCount;
   // encode: z = x W_enc^T, x shared and fp16-exact (its cross term skipped); EpiEncodeT stages 4 KB per warp
   run<4096, false, false, true>({"encode", 1, M, B, n, d, 1, false, true}, M, sms, zero_flag, sink, reps, clusters);
+  // the same with 6 KB per warp, what staging the code's batch-major copies as well would take: one ring stage fewer
+  run<6144, false, false, true>({"encode_6k", 1, M, B, n, d, 1, false, true}, M, sms, zero_flag, sink, reps, clusters);
   // decode: x^ = c W_dec, both operands per model; EpiDecodeT stages nothing and runs in line
   run<0, true, false, true>({"decode", M, M, B, d, n, 1, false, false}, M, sms, zero_flag, sink, reps, clusters);
   // dcode: g W_dec^T; EpiDcodeT stages 4 KB per warp

@@ -11,7 +11,10 @@ For each of the step's four GEMMs (encode, decode, dcode, weight gradient) it re
   (c) epilogue_bound_ms, encode and dcode only: the engine's kernel time for the same GEMM, measured as (a), at the same
       M, n and B but d = 64. Their K loop is then a single K block, so the time is bounded by the epilogue's per-tile
       throughput: where (c) is below (b), the epilogue keeps pace with the main loop at d = 512;
-and the card's name, power limit and SM clock, read in the same run after each measurement.
+and the card's name, power limit and SM clock, read in the same run after each measurement. Beside them: (b) of encode
+with 6 KB of epilogue staging per warp instead of 4 KB (one ring stage fewer, what staging the code's batch-major copies
+through shared memory would cost), and the time and launches per step of transpose_batch_u8_kernel, the pass that makes
+the batch-major copies of the 8-bit planes the epilogues do not write.
 (a), (b) and (c) are taken in alternated rounds and their medians reported with the range. (a) minus (b) at the
 cluster size the engine launches the GEMM in (2 for decode and dW, 1 for encode and dcode; the probe reports it) is the
 time the epilogue adds; (b) at cluster 2 over (b) at cluster 1 is what a 25 % cut of the main loop's L2 operand reads
@@ -71,7 +74,11 @@ class EngineRun:
                 self.ens.step_batch(self.pool[i % len(self.pool)])
             torch.cuda.synchronize()
         sums = {g: [0.0, 0] for _, g in EPILOGUES}
+        sums[TRANSPOSE] = [0.0, 0]
         for ev in prof.events():
+            if TRANSPOSE in ev.name:
+                sums[TRANSPOSE][0] += ev.device_time / 1e3
+                sums[TRANSPOSE][1] += 1
             if "gemm_split_kernel" not in ev.name:
                 continue
             for tag, g in EPILOGUES:
@@ -79,9 +86,12 @@ class EngineRun:
                     sums[g][0] += ev.device_time / 1e3   # us -> ms
                     sums[g][1] += 1
                     break
-        return {g: (t / c if c else None, c / self.steps) for g, (t, c) in sums.items()}
+        out = {g: (t / c if c else None, c / self.steps) for g, (t, c) in sums.items()}
+        out[TRANSPOSE] = (sums[TRANSPOSE][0] / self.steps, sums[TRANSPOSE][1] / self.steps)   # per step, not per launch
+        return out
 
 
+TRANSPOSE = "transpose_batch_u8_kernel"
 CLUSTERS = (1, 2)
 EPILOGUE_BOUND_D = 64                 # input dimension of (c): one K block of the encode and dcode GEMMs
 EPILOGUE_BOUND = ("encode", "dcode")  # the GEMMs (c) is reported for
@@ -160,7 +170,16 @@ def main():
         rc = f"[{min(cvv):.3f}-{max(cvv):.3f}]" if cvv else ""
         print(f"{g:8s} {per_step:13.1f} {fmt(ma, 10)} {ra:15s} {mb1:24.3f} {r1:15s} {mb2:10.3f} {r2:15s} "
               f"{mb2 / mb1:8.3f} {fmt(None if ma is None else ma - mbe, 12)} {fmt(mc, 8)} {rc:15s}")
-    res = {"card": info, "arith": run.arith, "epilogue_bound_d": EPILOGUE_BOUND_D, "rounds": [{k: v for k, v in r.items() if k.startswith("clock")} for r in rounds], "gemms": rows}
+    tr = [r["engine"][TRANSPOSE][0] for r in rounds]
+    tr_launches = rounds[0]["engine"][TRANSPOSE][1]
+    e6 = [r["main_loop"][("encode_6k", 1)]["main_loop_ms"] for r in rounds]
+    e6_stages = rounds[0]["main_loop"][("encode_6k", 1)]["stages"]
+    print(f"encode main loop with 6 KB staging per warp ({e6_stages} stages), cluster 1: {med(e6):.3f} "
+          f"[{min(e6):.3f}-{max(e6):.3f}] ms")
+    print(f"{TRANSPOSE}: {med(tr):.3f} [{min(tr):.3f}-{max(tr):.3f}] ms per step, {tr_launches:.1f} launches per step")
+    res = {"card": info, "encode_6k_main_loop_ms": med(e6), "encode_6k_main_loop_ms_rounds": e6,
+           "encode_6k_stages": e6_stages, "transpose_ms_per_step": med(tr), "transpose_ms_per_step_rounds": tr,
+           "transpose_launches_per_step": tr_launches, "arith": run.arith, "epilogue_bound_d": EPILOGUE_BOUND_D, "rounds": [{k: v for k, v in r.items() if k.startswith("clock")} for r in rounds], "gemms": rows}
     line = json.dumps(res)
     print(line)
     if args.out:

@@ -33,7 +33,10 @@ extern "C" {
  * 201 also covers the additive entry points sce_second_moments_workspace_bytes / sce_second_moments (BatchedPCA). They
  * are plan-less and change nothing above. So are sce_ica_pass_workspace_bytes / sce_ica_pass (ICAEncoder), added
  * under 201 as well, and the NMF entry points sce_nmf_project, sce_nmf_grams, sce_nmf_residual and sce_nmf_cd_sweep
- * with their *_workspace_bytes queries (NMFEncoder). */
+ * with their *_workspace_bytes queries (NMFEncoder).
+ * 201 also covers the additive dead-feature tracking entry points sce_track_workspace_bytes, sce_step_tracked and
+ * sce_resample with the struct sce_track they take. sce_step and every other entry point are unchanged, and a plan that
+ * never sees sce_step_tracked launches exactly the kernels it did before. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -296,6 +299,57 @@ int sce_forward_fragments(sce_plan* plan, const float* x, int B, int L, long lon
                           unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream);
+
+/* Dead-feature resampling (experiments/huge_batch_size.py:120-146 WorstIndices, :189-250 process_reinit), per model m,
+ * over a WINDOW of tracked steps (the sce_step_tracked calls since the caller emptied the lists, or since sce_resample):
+ *   e_r        mean over d of (x_hat - x)^2 for row r, in the space the plan reconstructs (centred, x - center[m],
+ *              x + input_shift), from the same fp32 residuals whose sum is l_reconstruction
+ *   list       the N rows of the window with the largest e, by (e descending, window serial ascending); an entry holds e,
+ *              the row's serial (row number within the window) and a bitwise copy of the row of `x` as the caller passed
+ *              it (x[m] when x_per_model, the shared row otherwise)
+ *   counts     per feature, the rows of the window whose code is non-zero (as sce_active_counts)
+ * A step whose update was skipped (the health word is set, see sce_health) enters nothing and counts nothing.
+ * sce_track: caller-owned device arrays, kept between calls (start a window with filled and counts zeroed and
+ * next_serial = 0):
+ *   err [M,N] fp32, serial [M,N] int64, rows [M,N,d] fp32 (16-byte aligned): the lists, entries 0 .. filled[m] - 1
+ *              valid, in no particular order
+ *   filled [M] int32, counts [M,n] int32
+ *   next_serial  window serial of this call's first row (the caller adds B after each call); next_serial + B must stay
+ *              below 2^32 - 1
+ *   n_worst    N, in [1, n]
+ *   workspace  >= sce_track_workspace_bytes(desc, N), 1024-byte aligned: scratch of one call (nothing in it is kept).
+ *              Host-only; 0 for an invalid desc or N. Config 2 (M = 16, B = 8192, d = 512, n = N = 4096): 7 MiB.
+ * sce_step_tracked: sce_step, then one merge kernel (row errors from the decode epilogue's per-row partials or the top-k
+ *   gather kernel's, the list merge as a radix select over 64-bit keys (e bits, inverted serial), the window's counts)
+ *   and one kernel copying the entering rows. No host synchronisation, no atomics whose order matters: bitwise
+ *   repeatable. The step itself computes exactly what sce_step computes; launch-bound plans run it without their CUDA
+ *   graph.
+ * sce_resample: for the dead features j_1 < j_2 < ... (count 0 over the window; masked padding, coef_mask = 1, is never
+ *   dead) and the list sorted as above, v_1, v_2, ...: for i <= min(#dead, filled), row j_i of the dictionary parameter
+ *   (encoder; dict for SCE_TOPK) becomes v_i * (ratio / mu), mu the mean L2 norm of the model's valid rows before the
+ *   replacement (fp64, fixed order), and the Adam moments of that row of the encoder, of the decoder (untied) and of its
+ *   bias entry become 0. Bias values, decoder rows, the centre, the step count, the health and range words and every
+ *   other row stay as they are. The operand planes of the dictionary are re-derived as sce_prepare does. Writes
+ *   n_dead[m], n_replaced[m] (device int32 [M]) and replaced (device uint8 [M,n], 1 = row replaced), then restarts the
+ *   window on the device (filled and counts zeroed; the caller sets next_serial = 0).
+ * Argument errors (NULL pointers, N outside [1, n], a small or misaligned workspace, misaligned rows) are reported
+ * before any device call. Asynchronous on `stream`. */
+typedef struct sce_track {
+  float* err;
+  long long* serial;
+  float* rows;
+  int* filled;
+  int* counts;
+  long long next_serial;
+  int n_worst;
+  void* workspace;
+  size_t workspace_bytes;
+} sce_track;
+size_t sce_track_workspace_bytes(const sce_desc* desc, int n_worst);
+int sce_step_tracked(sce_plan* plan, const float* x, int B, float* out_losses, float* out_nnz, const sce_track* track,
+                     void* stream);
+int sce_resample(sce_plan* plan, const sce_track* track, float ratio, int* n_dead, int* n_replaced,
+                 unsigned char* replaced, void* stream);
 
 /* The arithmetic the plan resolved to: SCE_ARITH_BF16X3 or SCE_ARITH_F16F8. */
 int sce_plan_arith(const sce_plan* plan);

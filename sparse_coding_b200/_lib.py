@@ -35,6 +35,7 @@ EXPORTS = [
     "sce_second_moments_workspace_bytes", "sce_second_moments", "sce_ica_pass_workspace_bytes", "sce_ica_pass",
     "sce_nmf_project_workspace_bytes", "sce_nmf_project", "sce_nmf_grams_workspace_bytes", "sce_nmf_grams",
     "sce_nmf_cd_sweep_workspace_bytes", "sce_nmf_cd_sweep", "sce_nmf_residual_workspace_bytes", "sce_nmf_residual",
+    "sce_track_workspace_bytes", "sce_step_tracked", "sce_resample",
 ]
 PHASES = ["split", "encode", "decode", "losses", "dcode", "dw", "adam"]
 
@@ -59,6 +60,14 @@ class SceBuffers(C.Structure):
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
         ("center_trans", C.c_void_p), ("center_rot", C.c_void_p), ("center_scale", C.c_void_p),
         ("center", C.c_void_p), ("center_m", C.c_void_p), ("center_v", C.c_void_p),
+    ]
+
+
+class SceTrack(C.Structure):
+    _fields_ = [
+        ("err", C.c_void_p), ("serial", C.c_void_p), ("rows", C.c_void_p), ("filled", C.c_void_p),
+        ("counts", C.c_void_p), ("next_serial", C.c_longlong), ("n_worst", C.c_int),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
     ]
 
 
@@ -211,6 +220,10 @@ def load():
     lib.sce_nmf_cd_sweep_workspace_bytes.restype = C.c_size_t
     lib.sce_nmf_cd_sweep_workspace_bytes.argtypes = [i, i]
     lib.sce_nmf_cd_sweep.argtypes = [vp, i, i, i, vp, vp, i, C.c_double, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_track_workspace_bytes.restype = C.c_size_t
+    lib.sce_track_workspace_bytes.argtypes = [C.POINTER(SceDesc), i]
+    lib.sce_step_tracked.argtypes = [vp, vp, i, vp, vp, C.POINTER(SceTrack), vp]
+    lib.sce_resample.argtypes = [vp, C.POINTER(SceTrack), f, vp, vp, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)  # AttributeError here means header and library disagree
     _lib = lib

@@ -404,6 +404,16 @@ struct DecodeGsumParams<true> {
   float* g_part;   // [M][tiles_m*4][d]
 };
 
+// Per-row squared residuals (EpiDecodeT<ARITH, GSUM, T8, true>, tracked training steps): each thread stores the sum of
+// r^2 over its 64 columns of the tile before the warp reduction, [M][B][2 tiles_n] (index 2 n_blk + grp), so that
+// sum_p row_part[m][r][p] / d is row r's error e_r, made of the same fp32 residuals whose sum is l_reconstruction.
+template <bool ROWERR>
+struct DecodeRowErrParams {};
+template <>
+struct DecodeRowErrParams<true> {
+  float* row_part;   // [M][B][2 tiles_n]
+};
+
 // ------------------------------------------------------------------------------------------------
 // decode:  r = acc - x;  partial sum r^2;  g = r * gscale -> planes of g;  optional x^ store
 // bf16x3: gscale = 2/(B d) (g is the loss gradient). f16f8: gscale = 1 — the fp16 plane could not hold 2r/(Bd)
@@ -412,16 +422,17 @@ struct DecodeGsumParams<true> {
 // GSUM (compile-time) adds the column sums of DecodeGsumParams; there rows beyond the batch stay in the warp (as zeros)
 // for the transpose-reduce. T8 (f16f8 training steps with a native weight gradient) also writes the batch-major copies
 // of g's 8-bit planes (BatchMajorParams), through a lane-quad transpose for which the rows beyond the batch stay in the
-// warp as well. The instantiations without the switches compile to the same code as without them.
+// warp as well. ROWERR also stores each thread's partial sum of r^2 per row (DecodeRowErrParams). The instantiations
+// without the switches compile to the same code as without them.
 // ------------------------------------------------------------------------------------------------
-template <int ARITH, bool GSUM = false, bool T8 = false>
+template <int ARITH, bool GSUM = false, bool T8 = false, bool ROWERR = false>
 struct EpiDecodeT {
   static_assert(!T8 || ARITH == kArithF16F8, "batch-major copies: f16f8 only");
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 0;
   static constexpr bool kInline = true;   // a few percent of a tile beside a K = n main loop (sce_gemm.cuh)
   static constexpr bool kWarpRows = GSUM || T8;   // rows beyond the batch run the chunk with the warp (as zeros)
-  struct Params : DecodeGsumParams<GSUM>, BatchMajorParams<T8> {
+  struct Params : DecodeGsumParams<GSUM>, BatchMajorParams<T8>, DecodeRowErrParams<ROWERR> {
     const float* x;                // [B, d] (x_model_stride = 0) or [M, B, d]
     long long x_model_stride;
     uint16_t* g_hi;                // [M, B, d] 16-bit plane
@@ -516,6 +527,9 @@ struct EpiDecodeT {
     }
   }
   __device__ __forceinline__ void finish() {
+    if constexpr (ROWERR) {
+      if (T.row < m_total) P.row_part[((long long)T.model * m_total + T.row) * (2 * P.tiles_n) + 2 * T.n_blk + T.grp] = sq;
+    }
     const float a = warp_sum(sq);
     if (T.lane == 0 && T.m_blk * kBM < m_total)
       P.part[(((long long)T.model * P.tiles_m + T.m_blk) * 8 + T.grp * 4 + T.warp_q) * P.tiles_n + T.n_blk] = a;

@@ -198,6 +198,7 @@ class FunctionalEnsemble:
         self._arith_fallback = None       # "bf16x3" once an auto plan left the fp16 range (sticky for this object)
         self._since_health = 0            # steps since the health flag was last read
         self._plan_steps = 0              # steps taken on the current plan
+        self._track = None                # the open dead-feature window (track_dead_features), or None
 
     # ------------------------------------------------------------------------------------------------------
     # engine plumbing
@@ -252,6 +253,7 @@ class FunctionalEnsemble:
             self._engine_buffers = eb
             self._plan_key = (batch_max, bool(x_per_model), int(centering))
             self._plan_k_max = desc.topk_k_max
+            self._plan_desc = desc
             _lib.check(lib.sce_set_step_count(plan, self._steps), "sce_set_step_count")
             _lib.check(lib.sce_prepare(plan, self._stream()), "sce_prepare")
         self._plan_steps = 0
@@ -342,6 +344,8 @@ class FunctionalEnsemble:
                 if self._health_action(rerun=True) != "rerun":
                     break
                 # the plan was rebuilt on bf16x3 (the update of this batch was skipped on the device): take the step again
+            if self._track is not None:
+                self._track["next_serial"] += B
             self._steps += 1
             if self.adam_count_mode != "frozen_t1":
                 for t in self.optim_states["count"].values():
@@ -350,8 +354,92 @@ class FunctionalEnsemble:
 
     def _launch_step(self, x, B):
         with torch.cuda.device(x.device):
-            _lib.check(_lib.load().sce_step(self._plan, x.data_ptr(), B, self._out_losses.data_ptr(),
-                                            self._out_nnz.data_ptr(), self._stream()), "sce_step")
+            if self._track is None:
+                _lib.check(_lib.load().sce_step(self._plan, x.data_ptr(), B, self._out_losses.data_ptr(),
+                                                self._out_nnz.data_ptr(), self._stream()), "sce_step")
+            else:
+                _lib.check(_lib.load().sce_step_tracked(self._plan, x.data_ptr(), B, self._out_losses.data_ptr(),
+                                                        self._out_nnz.data_ptr(), C.byref(self._track_struct()),
+                                                        self._stream()), "sce_step_tracked")
+
+    # ------------------------------------------------------------------------------------------------------
+    # dead-feature resampling (experiments/huge_batch_size.py:120-146, :189-250; include/sce.h, sce_track)
+    # ------------------------------------------------------------------------------------------------------
+    def track_dead_features(self, n_worst: Optional[int] = None) -> None:
+        """Open (or restart) a window: from now on every ``step_batch`` also keeps, per model, the ``n_worst`` rows
+        with the largest reconstruction error e_r = mean over d of (x_hat - x)^2 (default n, as the reference's
+        ``WorstIndices(n_features)``) with a copy of each row as it was fed, and counts each feature's active rows.
+        Both live on the GPU; nothing is read back until ``resample_dead_features`` or ``worst_rows``. The window
+        survives plan rebuilds. It is not part of ``state_dict()``: a resumed run starts a new window."""
+        dev = self._require_cuda()
+        n_worst = self._n if n_worst is None else int(n_worst)
+        if not 1 <= n_worst <= self._n:
+            raise ValueError(f"n_worst must lie in [1, n = {self._n}], got {n_worst}")
+        M, d = self.n_models, self._d
+        self._track = {
+            "err": torch.zeros(M, n_worst, dtype=torch.float32, device=dev),
+            "serial": torch.zeros(M, n_worst, dtype=torch.int64, device=dev),
+            "rows": torch.zeros(M, n_worst, d, dtype=torch.float32, device=dev),
+            "filled": torch.zeros(M, dtype=torch.int32, device=dev),
+            "counts": torch.zeros(M, self._n, dtype=torch.int32, device=dev),
+            "n_worst": n_worst, "next_serial": 0, "ws": None, "ws_addr": 0, "ws_bytes": 0,
+        }
+
+    def stop_tracking(self) -> None:
+        """Close the window: steps go back to plain ``sce_step``."""
+        self._track = None
+
+    def _track_struct(self):
+        """The open window as an ``SceTrack``, with a scratch workspace sized for the current plan."""
+        t = self._track
+        need = _lib.load().sce_track_workspace_bytes(C.byref(self._plan_desc), t["n_worst"])
+        if need > t["ws_bytes"]:
+            t["ws"], t["ws_addr"] = _lib.workspace(need, torch.device(self.device), "sce_track_workspace_bytes")
+            t["ws_bytes"] = need
+        return _lib.SceTrack(err=t["err"].data_ptr(), serial=t["serial"].data_ptr(), rows=t["rows"].data_ptr(),
+                             filled=t["filled"].data_ptr(), counts=t["counts"].data_ptr(),
+                             next_serial=t["next_serial"], n_worst=t["n_worst"], workspace=t["ws_addr"],
+                             workspace_bytes=t["ws_bytes"])
+
+    def resample_dead_features(self, ratio: float = 0.2) -> Dict[str, Tensor]:
+        """Reinitialise, per model, the features that fired on no row of the window (masked padding excluded): the
+        i-th dead feature (ascending index) gets the i-th worst row of the window scaled by ``ratio / mu``, mu the mean
+        row norm of the model's valid features before the change (the reference's ``encoder_norm_ratio /
+        av_encoder_norms``, huge_batch_size.py:236-240; SURVEY.md Q11), and the Adam moments of its encoder (``dict``
+        for TopK), decoder and bias entries are zeroed. Dead features beyond the listed rows stay as they are. Runs on
+        the GPU, including the operand planes; the window then restarts. Returns ``{"n_dead": [M], "n_replaced": [M],
+        "replaced": [M, n] bool}`` as device tensors."""
+        if self._track is None:
+            raise RuntimeError("resample_dead_features needs an open window: call track_dead_features() and train on "
+                               "it first")
+        self._require_cuda()
+        if self._plan is None:
+            raise RuntimeError("resample_dead_features needs a built plan: run step_batch first")
+        dev = torch.device(self.device)
+        n_dead = torch.empty(self.n_models, dtype=torch.int32, device=dev)
+        n_replaced = torch.empty(self.n_models, dtype=torch.int32, device=dev)
+        replaced = torch.empty(self.n_models, self._n, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().sce_resample(self._plan, C.byref(self._track_struct()), float(ratio),
+                                                n_dead.data_ptr(), n_replaced.data_ptr(), replaced.data_ptr(),
+                                                self._stream()), "sce_resample")
+        self._track["next_serial"] = 0
+        return {"n_dead": n_dead, "n_replaced": n_replaced, "replaced": replaced.bool()}
+
+    def worst_rows(self) -> List[Dict[str, Tensor]]:
+        """The window's lists, per model sorted by (error descending, window row number ascending): ``{"err": [k],
+        "serial": [k], "rows": [k, d]}`` with k the rows listed so far, plus ``"counts"``: the features' active rows."""
+        if self._track is None:
+            raise RuntimeError("worst_rows needs an open window: call track_dead_features() first")
+        t = self._track
+        out = []
+        for m, k in enumerate(t["filled"].tolist()):
+            err, ser = t["err"][m, :k], t["serial"][m, :k]
+            order = torch.sort(ser, stable=True).indices
+            order = order[torch.sort(err[order], descending=True, stable=True).indices]
+            out.append({"err": err[order].clone(), "serial": ser[order].clone(), "rows": t["rows"][m, order].clone(),
+                        "counts": t["counts"][m].clone()})
+        return out
 
     # ------------------------------------------------------------------------------------------------------
     # health (range contract of the f16f8 arithmetic, non-finite losses)
@@ -557,6 +645,7 @@ class FunctionalEnsemble:
 
     def to_device(self, device):
         self._destroy_plan()
+        self._track = None
         self._plan_key = None
         self._centering = None
         self.device = device

@@ -429,14 +429,20 @@ class _Counter:
 def train_on_chunks(ensemble, args: dict, dataset_folder: str, output_folder: str, batch_size: int,
                     ensemble_hyperparams: List[str], buffer_hyperparams: List[str], n_repetitions: int = 1,
                     center_activations: bool = False, cfg=None, chunk_order: Optional[List[int]] = None,
-                    save_schedule: str = "sweep", feed: str = "per_rank", on_chunk_end=None, chunks=None):
+                    save_schedule: str = "sweep", feed: str = "per_rank", on_chunk_end=None, chunks=None,
+                    resample_every: int = 0, resample_ratio: float = 0.2, on_resample=None):
     """The chunk loop of ``sweep`` (big_sweep.py:349-384) / ``basic_l1_sweep`` (basic_l1_sweep.py:85-115) for ONE
     ensemble on ONE GPU, with streamed chunks. Writes ``_{i}/learned_dicts.pt`` (+ ``config.yaml`` when ``cfg`` is
     given) on the reference's schedule: last chunk, or chunk count in {8, 16, …, 512}. ``feed``: see
     :class:`ChunkStreamer`; ``on_chunk_end(i, chunk_idx, ensemble)`` runs after the last step of every chunk.
     ``chunks``: a sized iterable of ``(chunk_idx, device chunk)`` that replaces the streamer (for example
     ``synthetic.SyntheticChunks``, which generates each chunk on the GPU); ``dataset_folder``, ``chunk_order``,
-    ``n_repetitions`` and ``feed`` are then unused."""
+    ``n_repetitions`` and ``feed`` are then unused.
+    ``resample_every`` > 0: dead-feature resampling as the reference's ``process_reinit`` does it
+    (experiments/huge_batch_size.py:189-250): every chunk is one window (``track_dead_features``), and after the chunk
+    at loop position i with ``i % resample_every == 0`` (the reference's ``chunk_idx % 10 == 0`` over
+    ``range(n)``, so the first chunk included) ``resample_dead_features(resample_ratio)`` runs and
+    ``on_resample(i, chunk_idx, ensemble, result)`` is called; the window is closed when the loop ends."""
     import yaml
 
     device = torch.device(args["device"])
@@ -466,6 +472,8 @@ def train_on_chunks(ensemble, args: dict, dataset_folder: str, output_folder: st
         torch.set_grad_enabled(False)
         torch.manual_seed(0)
         np.random.seed(0)
+        if resample_every > 0:
+            ensemble.track_dead_features()
         with nvtx_range(f"sce.chunk {chunk_idx}"):
             for j, idx in enumerate(_batch_index_lists(sampler, device, perm_cache)):
                 batch = gather_rows(chunk, idx, sub=means)
@@ -473,6 +481,10 @@ def train_on_chunks(ensemble, args: dict, dataset_folder: str, output_folder: st
         check_input_range(ensemble)
         if on_chunk_end is not None:
             on_chunk_end(i, chunk_idx, ensemble)      # e.g. the end-of-chunk metric gather (sharding.gather_metrics)
+        if resample_every > 0 and i % resample_every == 0:
+            result = ensemble.resample_dead_features(resample_ratio)
+            if on_resample is not None:
+                on_resample(i, chunk_idx, ensemble, result)
         last = i == n_total - 1
         if last or (save_schedule == "sweep" and (i + 1) in [2 ** j for j in range(3, 10)]) or save_schedule == "every":
             # export (a full D2H of the parameters, which also drains the GPU) only when a checkpoint is due
@@ -488,6 +500,8 @@ def train_on_chunks(ensemble, args: dict, dataset_folder: str, output_folder: st
                                    if isinstance(v, (int, float, str, bool, list, type(None)))}, f)
                 except Exception:
                     pass
+    if resample_every > 0:
+        ensemble.stop_tracking()
     return learned_dicts
 
 

@@ -1,0 +1,465 @@
+// sce_eval.cu — the entry points that read a plan's call back: the dense code (sce_read_code), activation counts
+// (sce_active_counts), the evaluation statistics of a forward pass (sce_forward_stats) and its top-activating and
+// random activating fragments (sce_forward_fragments).
+#include "sce_plan.cuh"
+
+namespace sce {
+__global__ void __launch_bounds__(256) active_count_kernel(const uint32_t* __restrict__ pos, int n_chunks, int batch_max,
+                                                           int B, int n, int* __restrict__ counts) {
+  active_count_block(pos, n_chunks, batch_max, B, n, counts, blockIdx.x, blockIdx.y);
+}
+}  // namespace sce
+
+// ------------------------------------------------------------------------------------------------
+// evaluation statistics (sce_forward_stats): per-feature moments and segment activity counts
+// ------------------------------------------------------------------------------------------------
+// Top-k plans: moment partials from the fp32 scores and the activity mask the selection left in the workspace, in the
+// layout of EncodeMomentParams ([M][row_blocks][4][n]): the code is relu(score) where the mask bit is set, 0 elsewhere.
+// One warp per (32-column chunk, row block): lane j sums column 32 chunk + j over the 32 rows in order.
+__global__ void __launch_bounds__(256) topk_moment_kernel(const float* __restrict__ scores, const uint32_t* __restrict__ pos,
+                                                          int n_chunks, int batch_max, int B, int n, int row_blocks,
+                                                          float* __restrict__ part) {
+  const int chunk = blockIdx.x, model = blockIdx.z, lane = threadIdx.x & 31;
+  const int rb = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (rb >= row_blocks) return;
+  const int col = chunk * 32 + lane;
+  const uint32_t* pw = pos + ((long long)model * n_chunks + chunk) * batch_max;
+  const float* s = scores + (long long)model * batch_max * n;
+  float a1 = 0.f, a2 = 0.f, a3 = 0.f, a4 = 0.f;
+  const int r_end = min(B, rb * 32 + 32);
+  for (int r = rb * 32; r < r_end; ++r) {
+    const uint32_t w = __ldg(pw + r);
+    if (col < n && ((w >> (31 - lane)) & 1u)) {
+      const float c = fmaxf(__ldg(s + (long long)r * n + col), 0.f), c2 = c * c;
+      a1 += c;
+      a2 += c2;
+      a3 += c2 * c;
+      a4 += c2 * c2;
+    }
+  }
+  if (col < n) {
+    float* o = part + ((long long)model * row_blocks + rb) * 4 * n + col;
+    o[0] = a1;
+    o[n] = a2;
+    o[2 * (long long)n] = a3;
+    o[3 * (long long)n] = a4;
+  }
+}
+
+// sums[m][j][p] += sum over the row blocks, in order, of part[m][rb][p][j] (fp64): bitwise repeatable, no atomics
+__global__ void moment_reduce_kernel(const float* __restrict__ part, int row_blocks, int n, double* __restrict__ sums) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x, model = blockIdx.y;
+  if (col >= n) return;
+  double a[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int rb = 0; rb < row_blocks; ++rb) {
+    const float* o = part + ((long long)model * row_blocks + rb) * 4 * n + col;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) a[q] += (double)__ldg(o + (long long)q * n);
+  }
+  double* out = sums + ((long long)model * n + col) * 4;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) out[q] += a[q];
+}
+
+// Segment activity counts (calc_moments_streaming's times_active, standard_metrics.py:482-511): the rows are cut into
+// segments of `seg`; counts[m][j] += number of segments that END in this call in which some row has [c > 0] in column j.
+// `phase` rows of the first segment were seen by earlier calls, whose activity is carried in open[m][j] (0 / 1); the
+// flag of a segment that stays open past this call is written back there. One block per (32-column chunk, model); warp
+// w takes the segments w, w + 8, ...; lanes OR 32 rows' mask words at a time, so lane j ends with column j's flag.
+__global__ void __launch_bounds__(256) segment_count_kernel(const uint32_t* __restrict__ pos, int n_chunks, int batch_max,
+                                                            int B, int n, int seg, int phase, int* __restrict__ counts,
+                                                            int* __restrict__ open) {
+  __shared__ int red[8][32];
+  const int chunk = blockIdx.x, model = blockIdx.y;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t* p = pos + ((long long)model * n_chunks + chunk) * batch_max;
+  const int col = chunk * 32 + lane;
+  const long long oi = (long long)model * n + col;
+  const int carried = col < n ? open[oi] : 0;
+  __syncthreads();   // every read of open[] precedes the write below
+  const long long K = ((long long)B + phase + seg - 1) / seg;   // segments this call touches
+  int mine = 0;
+  for (long long k = warp; k < K; k += 8) {
+    const long long lo = k == 0 ? 0 : k * seg - phase;
+    const long long end = (k + 1) * seg - phase;
+    const long long hi = end < B ? end : B;
+    uint32_t any = 0u;
+    for (long long r = lo + lane; r < hi; r += 32) any |= __ldg(p + r);
+    any = __reduce_or_sync(0xffffffffu, any);
+    int act = (int)((any >> (31 - lane)) & 1u);
+    if (k == 0) act |= carried;
+    if (end <= B) {
+      mine += act;
+      if (k == K - 1 && col < n) open[oi] = 0;
+    } else if (col < n) {
+      open[oi] = act;   // (only the last segment can stay open)
+    }
+  }
+  red[warp][lane] = mine;
+  __syncthreads();
+  if (warp == 0) {
+    int t = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += red[i][lane];
+    if (col < n) counts[oi] += t;
+  }
+}
+
+// The workspace of one forward-stats call: the moment partials [M][ceil(B / 32)][4][n] fp32. With base == nullptr only
+// measures it.
+static size_t stats_carve(uint8_t* base, const sce_desc& d, int B, float** part) {
+  Carve c{base, 0};
+  float* mp = c.take<float>((size_t)d.n_models * ((B + 31) / 32) * 4 * d.n);
+  if (part) *part = mp;
+  return align_up(c.off, 1024);
+}
+
+// ------------------------------------------------------------------------------------------------
+// the code of the plan's last call, as the engine holds it (sce_read_code, sce_forward_fragments)
+// ------------------------------------------------------------------------------------------------
+// Where a CodeView reads the code from. The row-major operand planes are numbered by their arithmetic (with_arith).
+enum CodeSource {
+  kCodeBf16x3 = kArithBf16x3,   // the bf16 pair hi + lo
+  kCodeF16F8 = kArithF16F8,     // the fp16 plane hi + the E5M2 plane of the residuals x8, scaled by 2^-kLoShift
+  kCodeBatchMajor,              // f16f8 after a dw_native backward (sce_plan::code_batch_major): hi + x8 as above, with x8
+                                // the residuals' batch-major copy [M][n][ld], since dcode overwrote the row-major plane
+  kCodeScores,                  // top-k: relu(score) where the activity mask has the bit, else 0
+};
+
+// W adjacent elements of a plane, loaded as one
+template <class T, int W>
+struct alignas(W * sizeof(T)) Adjacent {
+  T e[W];
+};
+template <class T, int W>
+__device__ __forceinline__ Adjacent<T, W> adjacent(const void* plane, long long idx) {
+  return *reinterpret_cast<const Adjacent<T, W>*>(static_cast<const T*>(plane) + idx);
+}
+
+// The code c[m, r, j] read from source SRC, the one decoder of the planes' format: -0 (the [z == 0] flag) reads as +0.
+template <int SRC>
+struct CodeView {
+  const void* hi;             // the code's 16-bit plane [M][batch_max][n] (bf16 or fp16)
+  const void* lo;             // bf16x3: its second bf16 plane
+  const uint8_t* x8;          // f16f8: E5M2 plane of the scaled residuals, [M][batch_max][n] or (kCodeBatchMajor) [M][n][ld]
+  const float* scores;        // top-k: fp32 scores [M][batch_max][n]
+  const uint32_t* pos;        // activity mask [M][n_chunks][batch_max]
+  int n_chunks, batch_max, n, ld;
+
+  // c[m, r, j + u] for u < W; with W = 2 (j even) one load reads both values of a row-major plane
+  template <int W>
+  __device__ __forceinline__ void get(int m, int r, int j, float (&v)[W]) const {
+    const long long idx = ((long long)m * batch_max + r) * n + j;
+    if constexpr (SRC == kCodeScores) {
+      const uint32_t w = __ldg(pos + ((long long)m * n_chunks + (j >> 5)) * batch_max + r);
+#pragma unroll
+      for (int u = 0; u < W; ++u) v[u] = ((w >> (31 - ((j + u) & 31))) & 1u) ? fmaxf(__ldg(scores + idx + u), 0.f) : 0.f;
+    } else if constexpr (SRC == kCodeBf16x3) {
+      const Adjacent<__nv_bfloat16, W> h = adjacent<__nv_bfloat16, W>(hi, idx), l = adjacent<__nv_bfloat16, W>(lo, idx);
+#pragma unroll
+      for (int u = 0; u < W; ++u) v[u] = __bfloat162float(h.e[u]) + __bfloat162float(l.e[u]);
+    } else {
+      constexpr float kInv = 1.f / float(1 << kLoShift);
+      const Adjacent<__half, W> h = adjacent<__half, W>(hi, idx);
+      Adjacent<uint8_t, W> res;
+      if constexpr (SRC == kCodeF16F8) {
+        res = adjacent<uint8_t, W>(x8, idx);
+      } else {
+#pragma unroll
+        for (int u = 0; u < W; ++u) res.e[u] = x8[((long long)m * n + j + u) * ld + r];
+      }
+#pragma unroll
+      for (int u = 0; u < W; ++u) v[u] = __half2float(h.e[u]) + e5m2_to_float(res.e[u]) * kInv;
+    }
+#pragma unroll
+    for (int u = 0; u < W; ++u) v[u] = v[u] == 0.f ? 0.f : v[u];
+  }
+  __device__ __forceinline__ float at(int m, int r, int j) const {
+    float v[1];
+    get(m, r, j, v);
+    return v[0];
+  }
+};
+
+// The view of the code of p's last call from source SRC
+template <int SRC>
+static CodeView<SRC> code_view(const sce_plan* p) {
+  return {p->c.hi, p->c.lo, SRC == kCodeBatchMajor ? p->ct.x8 : p->c.x8, p->scores, p->act_pos, (p->d.n + 31) / 32,
+          p->d.batch_max, p->d.n, p->cfg.bpad};
+}
+
+// out [M][B][n] fp32 = the code of the B rows of the last call. Grid (<= 1024, M), two adjacent columns per thread.
+template <int SRC>
+__global__ void __launch_bounds__(256) read_code_kernel(CodeView<SRC> c, int B, float* __restrict__ out) {
+  const int m = blockIdx.y, row_pairs = c.n / 2;
+  const long long pairs = (long long)B * row_pairs;
+  float2* o = reinterpret_cast<float2*>(out + (long long)m * B * c.n);
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < pairs; i += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / row_pairs);
+    float v[2];
+    c.get(m, r, 2 * (int)(i - (long long)r * row_pairs), v);
+    o[i] = make_float2(v[0], v[1]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// top-activating and random activating fragments (sce_forward_fragments; interpret.py:82-212 record tables,
+// :265-321 record selection): fragment g of a call is rows g L .. g L + L - 1.
+// ------------------------------------------------------------------------------------------------
+// fmax[m][g][j] = max over the L rows of fragment g of c[m, r, j]; active[m][g][j] = 1 where the activity mask has
+// c > 0 on some row of it. One block per (32-column chunk, fragment, model): lane j reads column 32 chunk + j, so every
+// row is read coalesced over the features; warp w takes the rows w, w + 8, ... and the 8 warps meet in shared memory.
+template <int SRC>
+__global__ void __launch_bounds__(256) fragment_max_kernel(CodeView<SRC> c, int L, int G, float* __restrict__ fmax,
+                                                           uint8_t* __restrict__ active) {
+  __shared__ float smax[8][32];
+  __shared__ uint32_t sact[8][32];
+  const int chunk = blockIdx.x, g = blockIdx.y, m = blockIdx.z;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int j = chunk * 32 + lane;
+  const uint32_t* pw = c.pos + ((long long)m * c.n_chunks + chunk) * c.batch_max;
+  float mx = 0.f;
+  uint32_t any = 0u;
+  for (int t = warp; t < L; t += 8) {
+    const int r = g * L + t;
+    any |= __ldg(pw + r);
+    if (j < c.n) mx = fmaxf(mx, c.at(m, r, j));
+  }
+  smax[warp][lane] = mx;
+  sact[warp][lane] = (any >> (31 - lane)) & 1u;
+  __syncthreads();
+  if (warp == 0 && j < c.n) {
+    float v = smax[0][lane];
+    uint32_t a = sact[0][lane];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) {
+      v = fmaxf(v, smax[w][lane]);
+      a |= sact[w][lane];
+    }
+    const long long o = ((long long)m * G + g) * c.n + j;
+    fmax[o] = v;
+    active[o] = (uint8_t)a;
+  }
+}
+
+// splitmix64 (Steele, Lea & Flood 2014): the priority of fragment `frag` for feature `feature` under `seed` is
+// mix(mix(mix(seed) ^ feature) ^ frag) >> 1, a 63-bit key that depends on nothing but these three numbers
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// list order: (key descending, fragment ascending); an entry with fragment < 0 is empty and below every other
+template <class K>
+__device__ __forceinline__ bool frag_above(K k, long long f, K k2, long long f2) {
+  return f2 < 0 || (f >= 0 && (k > k2 || (k == k2 && f < f2)));
+}
+template <class K>
+__device__ __forceinline__ int frag_lowest(const K* key, const long long* frag, int cap) {
+  int w = 0;
+  for (int i = 1; i < cap; ++i)
+    if (frag_above(key[w], frag[w], key[i], frag[i])) w = i;
+  return w;
+}
+
+// One thread per (feature, model) walks the call's fragments in order and keeps two lists of `cap` entries that persist
+// across calls: (fragment maximum, fragment) over all fragments, and (priority, fragment) over the active ones. A
+// candidate replaces the list's lowest entry when it is above it, and then its L code values are copied into that
+// entry's row of top_act / rnd_act. The lists are sets (sorted by the caller after the last call): the result depends
+// on nothing but the fragments seen, with no atomics.
+template <int SRC>
+__global__ void __launch_bounds__(128) fragment_merge_kernel(CodeView<SRC> c, int L, int G, long long frag0,
+                                                             const float* __restrict__ fmax,
+                                                             const uint8_t* __restrict__ active, int n_top, int n_random,
+                                                             unsigned long long seed, float* top_val, long long* top_frag,
+                                                             float* top_act, long long* rnd_key, long long* rnd_frag,
+                                                             float* rnd_act) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+  if (j >= c.n) return;
+  const long long list = (long long)m * c.n + j;
+  float* tv = top_val + list * n_top;
+  long long* tf = top_frag + list * n_top;
+  long long* rk = rnd_key + list * n_random;
+  long long* rf = rnd_frag + list * n_random;
+  const uint64_t h_feat = splitmix64(splitmix64(seed) ^ (uint64_t)j);
+  int tlow = n_top ? frag_lowest(tv, tf, n_top) : 0;
+  int rlow = n_random ? frag_lowest(rk, rf, n_random) : 0;
+  for (int g = 0; g < G; ++g) {
+    const long long o = ((long long)m * G + g) * c.n + j, frag = frag0 + g;
+    if (n_top) {
+      const float v = __ldg(fmax + o);
+      if (frag_above(v, frag, tv[tlow], tf[tlow])) {
+        tv[tlow] = v;
+        tf[tlow] = frag;
+        if (top_act) {
+          float* dst = top_act + (list * n_top + tlow) * L;
+          for (int t = 0; t < L; ++t) dst[t] = c.at(m, g * L + t, j);
+        }
+        tlow = frag_lowest(tv, tf, n_top);
+      }
+    }
+    if (n_random && __ldg(active + o)) {
+      const long long k = (long long)(splitmix64(h_feat ^ (uint64_t)frag) >> 1);
+      if (frag_above(k, frag, rk[rlow], rf[rlow])) {
+        rk[rlow] = k;
+        rf[rlow] = frag;
+        if (rnd_act) {
+          float* dst = rnd_act + (list * n_random + rlow) * L;
+          for (int t = 0; t < L; ++t) dst[t] = c.at(m, g * L + t, j);
+        }
+        rlow = frag_lowest(rk, rf, n_random);
+      }
+    }
+  }
+}
+
+constexpr int kFragMaxList = 64;   // largest n_top / n_random
+
+static bool frag_len_ok(int L) { return L >= 32 && L <= 8192 && L % 32 == 0; }
+
+// The workspace of one fragments call: fragment maxima [M][B/L][n] fp32, activity flags [M][B/L][n] u8, open-segment
+// flags [M][n] int32. With base == nullptr only measures it.
+struct FragCarve {
+  float* fmax;
+  uint8_t* active;
+  int* open;
+};
+static size_t frag_carve(uint8_t* base, const sce_desc& d, int B, int L, FragCarve* out) {
+  const size_t cells = (size_t)d.n_models * (B / L) * d.n;
+  Carve c{base, 0};
+  FragCarve w;
+  w.fmax = c.take<float>(cells);
+  w.active = c.take<uint8_t>(cells);
+  w.open = c.take<int>((size_t)d.n_models * d.n);
+  if (out) *out = w;
+  return align_up(c.off, 1024);
+}
+
+template <int SRC>
+static int launch_fragments(Launcher& launcher, const CodeView<SRC>& c, int M, int L, int G, long long frag0, float* fmax,
+                            uint8_t* active, int n_top, int n_random, unsigned long long seed, float* top_val,
+                            long long* top_frag, float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act) {
+  TRY(launcher.launch(fragment_max_kernel<SRC>, dim3(c.n_chunks, G, M), 256, 0, c, L, G, fmax, active));
+  return launcher.launch(fragment_merge_kernel<SRC>, dim3((c.n + 127) / 128, M), 128, 0, c, L, G, frag0, fmax,
+                         active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
+}
+
+// ------------------------------------------------------------------------------------------------
+// C ABI
+// ------------------------------------------------------------------------------------------------
+extern "C" {
+
+int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
+  if (!p || !out_code) return fail(SCE_ERR_INVALID, "plan / out_code is NULL");
+  if (int rc = check_rows(p, B, "")) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  const long long blocks = ((long long)B * p->d.n / 2 + 255) / 256;   // per model
+  auto read = [&](auto src) {
+    constexpr int SRC = decltype(src)::value;
+    return L.launch(read_code_kernel<SRC>, dim3((unsigned)(blocks < 1024 ? blocks : 1024), p->d.n_models), 256, 0,
+                    code_view<SRC>(p), B, out_code);
+  };
+  // (top-k plans too: the selection writes their code planes)
+  if (p->code_batch_major) return read(std::integral_constant<int, kCodeBatchMajor>{});
+  return with_arith(p->cfg.arith, read);
+}
+
+int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
+  if (!plan || !counts) return fail(SCE_ERR_INVALID, "plan / counts is NULL");
+  if (int rc = check_rows(plan, B, "")) return rc;
+  const int n_chunks = (plan->d.n + 31) / 32;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  return L.launch(active_count_kernel, dim3(n_chunks, plan->d.n_models), 256, 0, plan->act_pos, n_chunks,
+                  plan->d.batch_max, B, plan->d.n, counts);
+}
+
+// The checks that open sce_forward_stats and sce_forward_fragments; `prefix` names the entry point in the messages
+static int check_forward_only(const sce_plan* p, const float* x, int B, const char* prefix) {
+  if (!p) return fail(SCE_ERR_INVALID, "%splan is NULL", prefix);
+  if (!p->cfg.evaluable)
+    return fail(SCE_ERR_INVALID, "%snot available for the learned-centre variant or with encoder_nonneg / input_shift; "
+                                 "evaluate the exported dictionaries (TiedSAE)", prefix);
+  TRY(check_rows(p, B, prefix));
+  if (!x) return fail(SCE_ERR_INVALID, "%sx is NULL", prefix);
+  return SCE_OK;
+}
+
+size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
+  if (validate(desc) || B < 1 || B > desc->batch_max || !plan_config(*desc).evaluable) return 0;
+  return stats_carve(nullptr, *desc, B, nullptr);
+}
+
+int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
+                      float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  TRY(check_forward_only(p, x, B, "forward_stats: "));
+  if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
+  if (seg_phase < 0 || seg_phase >= seg)
+    return fail(SCE_ERR_INVALID, "forward_stats: seg_phase = %d outside [0, seg = %d)", seg_phase, seg);
+  if (!out_losses || !out_nnz || !moment_sums || !seg_counts)
+    return fail(SCE_ERR_INVALID, "forward_stats: out_losses, out_nnz, moment_sums and seg_counts are required");
+  if (seg > 1 && !seg_open) return fail(SCE_ERR_INVALID, "forward_stats: seg > 1 needs the seg_open flags");
+  float* part;
+  const size_t need = stats_carve(static_cast<uint8_t*>(workspace), p->d, B, &part);
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_stats: ")) return rc;
+  const sce_desc& d = p->d;
+  PlanCall c;
+  TRY(run_pipeline(c, p, x, B, static_cast<cudaStream_t>(stream), x_hat, false, out_losses, out_nnz,
+                   p->cfg.topk ? nullptr : part));
+  p->last_launches = c.count;   // the pipeline's: the statistics kernels below are not counted
+  const int n_chunks = (d.n + 31) / 32, row_blocks = (B + 31) / 32;
+  if (p->cfg.topk)
+    TRY(c.launch(topk_moment_kernel, dim3(n_chunks, (row_blocks + 7) / 8, d.n_models), 256, 0, p->scores, p->act_pos,
+                 n_chunks, d.batch_max, B, d.n, row_blocks, part));
+  TRY(c.launch(moment_reduce_kernel, dim3((d.n + 255) / 256, d.n_models), 256, 0, part, row_blocks, d.n, moment_sums));
+  if (seg == 1)
+    return c.launch(active_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
+                    seg_counts);
+  return c.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n, seg,
+                  seg_phase, seg_counts, seg_open);
+}
+
+size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
+  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || !plan_config(*desc).evaluable) return 0;
+  return frag_carve(nullptr, *desc, B, L, nullptr);
+}
+
+int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long frag0, int n_top, int n_random,
+                          unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
+                          long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  TRY(check_forward_only(p, x, B, "forward_fragments: "));
+  if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);
+  if (B % L) return fail(SCE_ERR_INVALID, "forward_fragments: B = %d is not a multiple of L = %d", B, L);
+  if (frag0 < 0) return fail(SCE_ERR_INVALID, "forward_fragments: frag0 = %lld must be >= 0", frag0);
+  if (n_top < 0 || n_top > kFragMaxList || n_random < 0 || n_random > kFragMaxList || n_top + n_random == 0)
+    return fail(SCE_ERR_INVALID, "forward_fragments: n_top = %d and n_random = %d must lie in [0, %d], not both 0", n_top,
+                n_random, kFragMaxList);
+  if (n_top && (!top_val || !top_frag)) return fail(SCE_ERR_INVALID, "forward_fragments: n_top > 0 needs top_val and top_frag");
+  if (n_random && (!rnd_key || !rnd_frag))
+    return fail(SCE_ERR_INVALID, "forward_fragments: n_random > 0 needs rnd_key and rnd_frag");
+  if (!n_active) return fail(SCE_ERR_INVALID, "forward_fragments: n_active is required");
+  FragCarve w;
+  const size_t need = frag_carve(static_cast<uint8_t*>(workspace), p->d, B, L, &w);
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_fragments: ")) return rc;
+  const sce_desc& d = p->d;
+  PlanCall call;
+  TRY(run_pipeline(call, p, x, B, static_cast<cudaStream_t>(stream), nullptr, false, nullptr, nullptr));
+  p->last_launches = call.count;   // the pipeline's: the fragment kernels below are not counted
+  const int n_chunks = (d.n + 31) / 32, G = B / L;
+  auto fragments = [&](auto src) {
+    constexpr int SRC = decltype(src)::value;
+    return launch_fragments<SRC>(call, code_view<SRC>(p), d.n_models, L, G, frag0, w.fmax, w.active, n_top, n_random,
+                                 seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
+  };
+  // (a forward pass leaves the code planes row-major)
+  TRY(p->cfg.topk ? fragments(std::integral_constant<int, kCodeScores>{}) : with_arith(p->cfg.arith, fragments));
+  // active fragments: segments of L rows, cut at fragment boundaries (phase 0, no segment stays open)
+  CUDA_TRY(cudaMemsetAsync(w.open, 0, (size_t)d.n_models * d.n * sizeof(int), call.st));
+  return call.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
+                     L, 0, n_active, w.open);
+}
+
+}  // extern "C"

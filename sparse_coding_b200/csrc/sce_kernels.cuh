@@ -1,11 +1,11 @@
 // sce_kernels.cuh — the HBM-bound streaming kernels around the GEMMs of one training step:
 // batch split, dictionary normalise+split, row-norm Jacobian + Adam + re-split, bias Adam,
-// top-k selection, code materialisation, chunk row gather.
+// top-k selection, chunk row gather.
 // Each is a single pass over its data with 16-byte accesses; algorithmic bytes per element are
 // listed in DESIGN.md.
 // Every translation unit of libsce.so includes this header, so every kernel here is a template: a kernel that is not
-// one is defined in the one .cu that owns it (the loss finalisation, centre gradient, activity counts and batch-major
-// transpose of the training step: sce_plan.cu), or each includer would define it again.
+// one is defined in the one .cu that owns it (the loss finalisation, centre gradient and batch-major transpose of the
+// training step: sce_plan.cu; the activity counts: sce_eval.cu), or each includer would define it again.
 #pragma once
 #include "sce_epilogues.cuh"
 
@@ -367,33 +367,6 @@ __global__ void bias_kernel(float* __restrict__ bias, float* __restrict__ m, flo
     bias[i] = adam_apply(b, g, mm, vv, h);
     m[i] = mm;
     v[i] = vv;
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// dense fp32 code from its (hi, lo) pair (the -0.0 "z == 0" flag decodes to +0)
-// ------------------------------------------------------------------------------------------------
-template <int ARITH>
-__global__ void join_code_kernel(const void* __restrict__ hi, const void* __restrict__ lo, const void* __restrict__ x8,
-                                 float* __restrict__ out, long long n2) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += stride) {
-    float2 o;
-    if constexpr (ARITH == kArithF16F8) {
-      const float2 h = __half22float2(reinterpret_cast<const __half2*>(hi)[i]);
-      const uint32_t l = reinterpret_cast<const uint16_t*>(x8)[i];
-      constexpr float kInv = 1.f / float(1 << kLoShift);
-      o.x = h.x + e5m2_to_float(l & 0xFFu) * kInv;
-      o.y = h.y + e5m2_to_float(l >> 8) * kInv;
-    } else {
-      const __nv_bfloat162 h = reinterpret_cast<const __nv_bfloat162*>(hi)[i];
-      const __nv_bfloat162 l = reinterpret_cast<const __nv_bfloat162*>(lo)[i];
-      o.x = __low2float(h) + __low2float(l);
-      o.y = __high2float(h) + __high2float(l);
-    }
-    if (o.x == 0.f) o.x = 0.f;  // -0 -> +0
-    if (o.y == 0.f) o.y = 0.f;
-    reinterpret_cast<float2*>(out)[i] = o;
   }
 }
 

@@ -1,5 +1,7 @@
-// sce_plan.cu — the entry points of include/sce.h that take an sce_plan, on top of the wgmma GEMM core and the
-// streaming kernels. One `sce_plan` = one stacked ensemble (FunctionalEnsemble, autoencoders/ensemble.py:68-97).
+// sce_plan.cu — the plan and its training step: the entry points of include/sce.h that create, prepare, step and
+// inspect an sce_plan, on top of the wgmma GEMM core and the streaming kernels. One `sce_plan` = one stacked ensemble
+// (FunctionalEnsemble, autoencoders/ensemble.py:68-97). The entry points that read a call's code back are in
+// sce_eval.cu, dead-feature tracking is in sce_track.cu, and what the three files share is in sce_plan.cuh.
 //
 // One training step (tied variant; untied and top-k differ as noted; "planes" are the operand planes of the plan's
 // arithmetic, see Planes: fp16 + two E5M2 planes with f16f8, a bf16 pair with bf16x3) is
@@ -17,11 +19,10 @@
 // Non-negative tied plans (desc.encoder_nonneg, desc.input_shift; FunctionalPositiveTiedSAE) are tied plans whose batch
 // split also forms x + input_shift, and whose dict_rows kernels build the dictionary from max(E, 0).
 #include <cmath>
-#include <map>
 #include <new>
 #include <vector>
 
-#include "sce_engine.cuh"
+#include "sce_plan.cuh"
 #include "sce_topk.cuh"
 
 // The training step's kernels that are not templates (see sce_kernels.cuh)
@@ -93,21 +94,6 @@ __global__ void __launch_bounds__(256) transpose_batch_u8_kernel(BatchPlanes t, 
   }
 }
 
-// join_code_kernel<f16f8> for plans whose code residual plane is held batch-major, [M][n][ld] (transpose_batch_u8_kernel):
-// out [M][B][n] fp32 from the row-major fp16 plane [M][batch_max][n] and that copy. Read-back only (strided reads).
-__global__ void __launch_bounds__(256) join_code_batch_major_kernel(const __half* __restrict__ hi, const uint8_t* __restrict__ x8t,
-                                                                    float* __restrict__ out, int B, int n, int batch_max, int ld,
-                                                                    long long total) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
-    const long long m = i / ((long long)B * n), rj = i - m * B * n;
-    const int r = (int)(rj / n), j = (int)(rj - (long long)r * n);
-    constexpr float kInv = 1.f / float(1 << kLoShift);
-    float v = __half2float(hi[(m * batch_max + r) * n + j]) + e5m2_to_float(x8t[(m * n + j) * ld + r]) * kInv;
-    if (v == 0.f) v = 0.f;  // -0 -> +0
-    out[i] = v;
-  }
-}
 
 // ------------------------------------------------------------------------------------------------
 // per-model ||bias||_2 (bias-decay loss term and its gradient; sae_ensemble.py:73, :150)
@@ -276,451 +262,9 @@ __global__ void __launch_bounds__(256) finalize_kernel(const float* __restrict__
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// per-feature activation counts (standard_metrics.py:305-308 `(c != 0).float().mean(0)` and :441-454
-// `n_active_count += (c != 0).sum(0)`; "ever active" = count > threshold): column sums of the [c > 0] activity-mask
-// plane over the batch rows. One block per (32-column chunk, model): every lane holds the mask word of one row, a
-// ballot per bit position counts 32 rows at once. counts[model][32 chunk + j] += sum_r bit(31 - j) of
-// pos[model][chunk][r], accumulated across calls so a held-out set can be streamed through in batches. Reads B words
-// per block, coalesced (the plane is chunk-major); the dense code is never touched.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void active_count_block(const uint32_t* __restrict__ pos, int n_chunks, int batch_max, int B,
-                                                   int n, int* __restrict__ counts, int chunk, int model) {
-  __shared__ int red[8][32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t* p = pos + ((long long)model * n_chunks + chunk) * batch_max;
-  int mine = 0;   // lane j accumulates the count of column j of the chunk
-  for (int r0 = warp * 32; r0 < B; r0 += 256) {
-    const int r = r0 + lane;
-    const uint32_t w = r < B ? __ldg(p + r) : 0u;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int c = __popc(__ballot_sync(0xffffffffu, (w >> (31 - j)) & 1u));
-      if (lane == j) mine += c;
-    }
-  }
-  red[warp][lane] = mine;
-  __syncthreads();
-  if (warp == 0) {
-    int t = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += red[i][lane];
-    const int col = chunk * 32 + lane;
-    if (col < n) counts[(long long)model * n + col] += t;
-  }
-}
-__global__ void __launch_bounds__(256) active_count_kernel(const uint32_t* __restrict__ pos, int n_chunks, int batch_max,
-                                                           int B, int n, int* __restrict__ counts) {
-  active_count_block(pos, n_chunks, batch_max, B, n, counts, blockIdx.x, blockIdx.y);
-}
-
-// ------------------------------------------------------------------------------------------------
-// dead-feature tracking (sce_step_tracked, sce_resample; experiments/huge_batch_size.py:120-146 WorstIndices, :189-250)
-// ------------------------------------------------------------------------------------------------
-constexpr int kTrackThreads = 256;   // every tracking kernel; active_count_block needs 8 warps
-
-// The list order as one 64-bit key, larger = earlier in the list: the bits of e (>= 0, so they order as the values do)
-// above the inverted window serial (e descending, serial ascending). Every real key is >= 1 (serial < 2^32 - 1).
-__device__ __forceinline__ unsigned long long track_key(float e, long long serial) {
-  return ((unsigned long long)__float_as_uint(e) << 32) | (unsigned long long)(0xFFFFFFFFu - (uint32_t)serial);
-}
-
-// Exclusive prefix count of `flag` over the block's threads in thread order, and the block's total. Every thread calls.
-__device__ __forceinline__ int block_prefix(bool flag, int* total) {
-  __shared__ int warp_cnt[kTrackThreads / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t bal = __ballot_sync(0xffffffffu, flag);
-  if (lane == 0) warp_cnt[warp] = __popc(bal);
-  __syncthreads();
-  int before = 0, all = 0;
-#pragma unroll
-  for (int w = 0; w < kTrackThreads / 32; ++w) {
-    before += w < warp ? warp_cnt[w] : 0;
-    all += warp_cnt[w];
-  }
-  __syncthreads();   // (warp_cnt is reused by the next call)
-  *total = all;
-  return before + __popc(bal & ((1u << lane) - 1u));
-}
-
-__device__ __forceinline__ unsigned long long block_min_u64(unsigned long long v) {
-  __shared__ unsigned long long red[kTrackThreads / 32];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = min(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  unsigned long long r = red[0];
-#pragma unroll
-  for (int w = 1; w < kTrackThreads / 32; ++w) r = min(r, red[w]);
-  __syncthreads();
-  return r;
-}
-
-// One tracked step's view of the caller's lists and of its scratch (TrackCarve)
-struct TrackArgs {
-  float* err;                  // [M][N]
-  long long* serial;           // [M][N]
-  float* rows;                 // [M][N][d]
-  int* filled;                 // [M]
-  int* counts;                 // [M][n]
-  long long next_serial;
-  int N;
-  const float* part;           // [M][B][n_part] partial sums of r^2 per row
-  int n_part;
-  unsigned long long* keys;    // [M][N + batch_max]: the list's keys (slots), then the rows' (0: not a candidate)
-  int *enter_row, *enter_slot; // [M][cap]: the rows entering the list, in row order, and the slots they take
-  int* enter_cnt;              // [M]
-  int cap;                     // min(N, batch_max)
-  const float* x;              // the caller's batch; model m's rows start at x + m x_model_stride
-  long long x_model_stride;
-};
-
-// The key of rank `want` (1 = largest) among the non-zero keys of keys[0, n_list) and keys[N, N + B): a most-significant-
-// digit radix select, 8 bits per pass, with a 256-bin histogram in shared memory (integer counts: any order of the adds
-// gives the same result). Keys are distinct, so exactly one key equals the result.
-__device__ unsigned long long track_select(const unsigned long long* keys, int n_list, int N, int B, int want) {
-  __shared__ int hist[256];
-  __shared__ unsigned long long s_prefix;
-  __shared__ int s_want;
-  unsigned long long prefix = 0ull, mask = 0ull;
-  for (int shift = 56; shift >= 0; shift -= 8) {
-    for (int i = threadIdx.x; i < 256; i += kTrackThreads) hist[i] = 0;
-    __syncthreads();
-    for (int i = threadIdx.x; i < n_list + B; i += kTrackThreads) {
-      const unsigned long long k = keys[i < n_list ? i : N + (i - n_list)];
-      if (k != 0ull && (k & mask) == prefix) atomicAdd(&hist[(int)((k >> shift) & 255ull)], 1);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int b = 255;
-      for (; b > 0; --b) {
-        if (want <= hist[b]) break;
-        want -= hist[b];
-      }
-      s_prefix = prefix | ((unsigned long long)b << shift);
-      s_want = want;
-    }
-    __syncthreads();
-    prefix = s_prefix;
-    want = s_want;
-    mask |= 255ull << shift;
-    __syncthreads();
-  }
-  return prefix;
-}
-
-// Merge of one tracked step. Block (0, m): model m's list; blocks (1 + chunk, m): the window's activity counts of a
-// 32-feature chunk (active_count_block). Nothing happens when the step's update was skipped (kBadWord).
-// List merge: e_r = (sum of row r's partials, in order) / d; rows whose key is not above the N-th key of a full list
-// drop out; the cut K is the N-th largest key of list and candidates (track_select, only when they overflow N); list
-// entries below K leave, candidates at or above K enter: the i-th entering row (row order) takes the i-th free slot
-// (slot order: vacated slots and slots past filled), and track_copy_kernel copies its d values.
-__global__ void __launch_bounds__(kTrackThreads) track_merge_kernel(TrackArgs t, const uint32_t* __restrict__ pos,
-                                                                    int n_chunks, int batch_max, int B, int n, int d,
-                                                                    const uint32_t* __restrict__ health) {
-  const int m = blockIdx.y;
-  if (step_is_bad(health)) {
-    if (blockIdx.x == 0 && threadIdx.x == 0) t.enter_cnt[m] = 0;
-    return;
-  }
-  if (blockIdx.x > 0) {
-    active_count_block(pos, n_chunks, batch_max, B, n, t.counts, blockIdx.x - 1, m);
-    return;
-  }
-  const int N = t.N;
-  float* err = t.err + (long long)m * N;
-  long long* ser = t.serial + (long long)m * N;
-  unsigned long long* keys = t.keys + (long long)m * (N + batch_max);
-  int* enter_row = t.enter_row + (long long)m * t.cap;
-  int* enter_slot = t.enter_slot + (long long)m * t.cap;
-  const int filled = t.filled[m];
-  unsigned long long lo = ~0ull;
-  for (int s = threadIdx.x; s < filled; s += kTrackThreads) {
-    const unsigned long long k = track_key(err[s], ser[s]);
-    keys[s] = k;
-    lo = min(lo, k);
-  }
-  lo = block_min_u64(lo);
-  const unsigned long long thr = filled == N ? lo : 0ull;
-  const float* part = t.part + (long long)m * B * t.n_part;
-  int mine = 0;
-  for (int r = threadIdx.x; r < B; r += kTrackThreads) {
-    float sq = 0.f;
-    for (int q = 0; q < t.n_part; ++q) sq += part[(long long)r * t.n_part + q];
-    unsigned long long k = track_key(sq / (float)d, t.next_serial + r);
-    if (k <= thr) k = 0ull;
-    else ++mine;
-    keys[N + r] = k;
-  }
-  int cand;
-  block_prefix(mine > 0, &cand);   // (only whether some thread has one)
-  __syncthreads();                 // keys[] complete for every thread
-  if (cand == 0) {
-    if (threadIdx.x == 0) t.enter_cnt[m] = 0;
-    return;
-  }
-  // candidates in total (an integer sum: order-independent)
-  __shared__ int s_total;
-  if (threadIdx.x == 0) s_total = 0;
-  __syncthreads();
-  if (mine) atomicAdd(&s_total, mine);
-  __syncthreads();
-  const int C = s_total;
-  const unsigned long long cut = filled + C > N ? track_select(keys, filled, N, B, N) : 1ull;
-  const int new_filled = filled + C < N ? filled + C : N;
-  int n_in = 0, n_free = 0;
-  for (int r0 = 0; r0 < B; r0 += kTrackThreads) {
-    const int r = r0 + threadIdx.x;
-    const bool in = r < B && keys[N + r] >= cut;
-    int tot;
-    const int at = block_prefix(in, &tot);
-    if (in) enter_row[n_in + at] = r;
-    n_in += tot;
-  }
-  for (int s0 = 0; s0 < new_filled; s0 += kTrackThreads) {
-    const int s = s0 + threadIdx.x;
-    const bool fr = s < new_filled && (s >= filled || keys[s] < cut);
-    int tot;
-    const int at = block_prefix(fr, &tot);
-    if (fr) enter_slot[n_free + at] = s;
-    n_free += tot;
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < n_in; i += kTrackThreads) {
-    const int r = enter_row[i], s = enter_slot[i];
-    err[s] = __uint_as_float((uint32_t)(keys[N + r] >> 32));
-    ser[s] = t.next_serial + r;
-  }
-  if (threadIdx.x == 0) {
-    t.enter_cnt[m] = n_in;   // (== n_free)
-    t.filled[m] = new_filled;
-  }
-}
-
-// The d values of each row that entered model blockIdx.y's list, from the caller's batch into its slot
-__global__ void __launch_bounds__(kTrackThreads) track_copy_kernel(TrackArgs t, int d) {
-  const int m = blockIdx.y, cnt = t.enter_cnt[m], d4 = d >> 2;
-  for (int i = blockIdx.x; i < cnt; i += gridDim.x) {
-    const int r = t.enter_row[(long long)m * t.cap + i], s = t.enter_slot[(long long)m * t.cap + i];
-    const float4* src = reinterpret_cast<const float4*>(t.x + m * t.x_model_stride + (long long)r * d);
-    float4* dst = reinterpret_cast<float4*>(t.rows + ((long long)m * t.N + s) * d);
-    for (int c = threadIdx.x; c < d4; c += kTrackThreads) dst[c] = src[c];
-  }
-}
-
-// norms[m][j] = ||W[m][j]|| in fp64 (squares summed per lane in column order, then across the warp in a fixed tree).
-// One warp per row, grid (ceil(n / 8), M).
-__global__ void __launch_bounds__(kTrackThreads) track_norm_kernel(const float* __restrict__ w, int n, int d,
-                                                                   double* __restrict__ norms) {
-  const int m = blockIdx.y, j = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (j >= n) return;
-  const float* row = w + ((long long)m * n + j) * d;
-  double ss = 0.0;
-  for (int c = lane; c < d; c += 32) ss += (double)row[c] * (double)row[c];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  if (lane == 0) norms[(long long)m * n + j] = sqrt(ss);
-}
-
-// order[m][rank] = slot: the rank of each filled entry in the list order, by counting the entries above it (keys are
-// distinct). Grid (ceil(N / 256), M).
-__global__ void __launch_bounds__(kTrackThreads) track_rank_kernel(const float* __restrict__ err,
-                                                                   const long long* __restrict__ serial,
-                                                                   const int* __restrict__ filled, int N,
-                                                                   int* __restrict__ order) {
-  __shared__ unsigned long long tile[kTrackThreads];
-  const int m = blockIdx.y, f = filled[m], s = blockIdx.x * kTrackThreads + threadIdx.x;
-  const float* e = err + (long long)m * N;
-  const long long* sr = serial + (long long)m * N;
-  const unsigned long long k = s < f ? track_key(e[s], sr[s]) : 0ull;
-  int rank = 0;
-  for (int u0 = 0; u0 < f; u0 += kTrackThreads) {
-    const int u = u0 + threadIdx.x;
-    tile[threadIdx.x] = u < f ? track_key(e[u], sr[u]) : 0ull;
-    __syncthreads();
-    const int lim = f - u0 < kTrackThreads ? f - u0 : kTrackThreads;
-    for (int q = 0; q < lim; ++q) rank += tile[q] > k;
-    __syncthreads();
-  }
-  if (s < f) order[(long long)m * N + rank] = s;
-}
-
-// Per model (one block): the dead set j_1 < j_2 < ... in dead[m] (count 0, not masked), mu = mean of the valid rows'
-// norms (fp64, each thread's columns in order, then the threads in order), scale[m] = ratio / mu, the outputs n_dead,
-// n_replaced = min(n_dead, filled) and replaced; then the window restarts (filled and counts zeroed).
-__global__ void __launch_bounds__(kTrackThreads) track_dead_kernel(int* __restrict__ counts, int* __restrict__ filled,
-                                                                   const unsigned char* __restrict__ mask,
-                                                                   const double* __restrict__ norms, int n, float ratio,
-                                                                   int* __restrict__ dead, int* __restrict__ n_rep,
-                                                                   float* __restrict__ scale, int* __restrict__ n_dead_out,
-                                                                   int* __restrict__ n_rep_out,
-                                                                   unsigned char* __restrict__ replaced) {
-  __shared__ double red[kTrackThreads];
-  __shared__ int red_valid[kTrackThreads];
-  const int m = blockIdx.x;
-  int* cnt = counts + (long long)m * n;
-  const unsigned char* mk = mask ? mask + (long long)m * n : nullptr;
-  int n_dead = 0;
-  for (int j0 = 0; j0 < n; j0 += kTrackThreads) {
-    const int j = j0 + threadIdx.x;
-    const bool dd = j < n && cnt[j] == 0 && !(mk && mk[j]);
-    int tot;
-    const int at = block_prefix(dd, &tot);
-    if (dd) dead[(long long)m * n + n_dead + at] = j;
-    n_dead += tot;
-  }
-  double acc = 0.0;
-  int valid = 0;
-  for (int j = threadIdx.x; j < n; j += kTrackThreads)
-    if (!(mk && mk[j])) {
-      acc += norms[(long long)m * n + j];
-      ++valid;
-    }
-  red[threadIdx.x] = acc;
-  red_valid[threadIdx.x] = valid;
-  __syncthreads();
-  const int f = filled[m];
-  const int nr = n_dead < f ? n_dead : f;
-  for (int j = threadIdx.x; j < n; j += kTrackThreads) replaced[(long long)m * n + j] = 0;
-  __syncthreads();
-  for (int i = threadIdx.x; i < nr; i += kTrackThreads) replaced[(long long)m * n + dead[(long long)m * n + i]] = 1;
-  for (int j = threadIdx.x; j < n; j += kTrackThreads) cnt[j] = 0;
-  if (threadIdx.x == 0) {
-    double sum = 0.0;
-    int nv = 0;
-    for (int i = 0; i < kTrackThreads; ++i) {
-      sum += red[i];
-      nv += red_valid[i];
-    }
-    scale[m] = (float)((double)ratio / (sum / nv));
-    n_rep[m] = nr;
-    n_dead_out[m] = n_dead;
-    n_rep_out[m] = nr;
-    filled[m] = 0;
-  }
-}
-
-// Row dead[m][i] of the dictionary parameter <- rows[m][order[m][i]] * scale[m] for i < n_rep[m]; the Adam moments of that
-// row (encoder, decoder) and of its bias entry <- 0. Grid (<= n, M).
-__global__ void __launch_bounds__(kTrackThreads) track_write_kernel(const float* __restrict__ rows,
-                                                                    const int* __restrict__ order,
-                                                                    const int* __restrict__ dead,
-                                                                    const int* __restrict__ n_rep,
-                                                                    const float* __restrict__ scale, int N, int n, int d,
-                                                                    float* w, float* w_m, float* w_v, float* dec_m,
-                                                                    float* dec_v, float* b_m, float* b_v) {
-  const int m = blockIdx.y, cnt = n_rep[m];
-  const float sc = scale[m];
-  for (int i = blockIdx.x; i < cnt; i += gridDim.x) {
-    const int j = dead[(long long)m * n + i], s = order[(long long)m * N + i];
-    const float* src = rows + ((long long)m * N + s) * d;
-    const long long o = ((long long)m * n + j) * d;
-    for (int c = threadIdx.x; c < d; c += kTrackThreads) {
-      w[o + c] = src[c] * sc;
-      w_m[o + c] = 0.f;
-      w_v[o + c] = 0.f;
-      if (dec_m) {
-        dec_m[o + c] = 0.f;
-        dec_v[o + c] = 0.f;
-      }
-    }
-    if (threadIdx.x == 0 && b_m) {
-      b_m[(long long)m * n + j] = 0.f;
-      b_v[(long long)m * n + j] = 0.f;
-    }
-  }
-}
-
 }  // namespace sce
 
-// ------------------------------------------------------------------------------------------------
-// plan
-// ------------------------------------------------------------------------------------------------
-struct BatchMaps {
-  GemmMaps encode, decode, dcode, dw_enc, dw_dec;
-  GemmMaps center;             // centring: A = (x - trans) planes [M,B,d], B = rot planes [M,d,d], both K-major
-  OperandMaps st_c, st_dz;     // epilogue TMA-store maps
-  CUtensorMap st_scores;       // top-k: fp32 scores
-  cudaGraphExec_t graph;       // captured step for this batch size (launch-bound shapes), or nullptr
-  int graph_launches, eager_steps;
-};
-
-// The plan's workspace buffers, in carve order (carve)
-struct PlanBuffers {
-  float* x_stage;                 // [xm, Bmax, d] staging for host-fed steps
-  Planes x;                       // [xm, Bmax, d]
-  Planes wenc, wdec;              // [M, n, d] (tied: wdec is a copy of wenc)
-  Planes wdt;                     // f16f8: the decoder's planes transposed, [M, d, n]: the decode GEMM's B operand, K-major (transpose_dict)
-  Planes c;                       // [M, Bmax, n]   (dw_native: the 8-bit planes are dz's, see carve)
-  Planes g;                       // [M, Bmax, d]
-  Planes dz;                      // [M, Bmax, n], one contiguous block of 4 B / element (top-k: fp32 scores alias it);
-                                  // dw_native: the 8-bit planes are [M, n, Bp]
-  // dw_native (dense f16f8 plans): batch-major copies of the 8-bit planes of x, c and g, [xm or M, cols, Bp] with Bp =
-  // batch_max rounded up to 16 (TMA pitch): the weight gradient reads them K-major over the batch (E5M2 wgmma).
-  // x's are made by a transpose pass (batch_major); the epilogues that produce c and g write their copies besides the
-  // row-major planes (EpiEncodeT / EpiDecodeT with T8), and dz's 8-bit planes exist only in that layout (EpiDcodeT<f16f8, true>).
-  Planes xt, ct, gt;
-  Planes rot;                     // centring: operand planes of buffers["center_rot"] [M, d, d]
-  float* x_centered;              // centring, learned centre: the centred batch [M, B, d] (B, not Bmax, rows per model: what a caller's [M,B,d] looks like)
-  // learned centre: column sums of g [M, tiles_m*4, d] (EpiDecodeT<AR, true>), db / ||E_n|| [M, n], the GEMV partials
-  // [M, ceil(n / kCenterChunkRows), d] and the centre gradient [M, d] (sce_read_center_grad)
-  float *g_part, *center_coef, *center_part, *center_grad;
-  float* x_shifted;               // input_shift: x + input_shift [xm, B, d], written by the batch split
-  float* scores;                  // top-k: fp32 scores [M, Bmax, n] of the encode GEMM
-  int* tk_models;                 // top-k gather kernel: the models sorted into k classes (device copy of tk_group_models)
-  uint32_t* tk_cmax;              // top-k: largest key per 32-column chunk of the scores [M, Bmax, n_chunks] (EpiScoresTma)
-  int *tk_col, *tk_cnt;           // top-k lists (TopkLists): selected columns [M, Bmax, kmax], entries per row [M, Bmax]
-  float *tk_val, *tk_dots;        // their values [M, Bmax, kmax]; per-slice shares of g . W_j [M, Bmax, kmax, slices]
-  float* wn_f32;                  // top-k: fp32 copy of the normalised dictionary [M, n, d] the gather kernel reads
-  uint32_t *act_pos, *act_zero;   // activity masks [M][ceil(n/32)][Bmax]: bit 31-j of a word = column 32*chunk + j (ActMask)
-  uint32_t* res_flags;            // [0]: the batch has a non-zero residual plane (f16f8; written by the batch split)
-  float *dw_enc, *dw_dec;         // [M, n, d]
-  float *part_enc, *part_dec, *db_part, *bnorm, *l1_over_b, *loss_stage, *nnz_stage;
-};
-
-// What a plan decides from its descriptor, once (plan_config): the workspace carve and every launch follow from it
-struct PlanConfig {
-  int arith;           // kArithBf16x3 or kArithF16F8
-  bool untied;         // SCE_UNTIED: a decoder of its own, a second dictionary side
-  bool topk;           // SCE_TOPK
-  bool learned;        // SCE_TIED_LEARNED_CENTER: the step centres the batch on params["center"] and trains the centre
-  bool x_models;       // the batch the kernels read holds one slab per model (x_per_model, or always with a learned centre)
-  int xm;              // number of distinct input batches (1 shared, or M)
-  int input_models;    // models' worth of rows in the caller's batch: 1 when it is shared ([B,d]; also centering = 1), else M
-  bool evaluable;      // the forward-only passes may run it: not plans whose export (a TiedSAE) differs from their forward
-  int bpad;            // Bp: batch_max rounded up to 16 (TMA pitch of the batch-major 8-bit planes)
-  int tk_kmax;         // top-k list capacity per row (desc.topk_k_max rounded up to 8; 0: no lists)
-  int tk_slices;       // slices of the activation width topk_sparse_kernel runs per row (0: none fits)
-  bool topk_sparse;    // decode / dcode of the top-k variant run as the k-sparse gather kernels
-  bool dw_native;      // the weight gradient's cross terms run on E5M2 wgmma from batch-major copies (carve)
-  bool split_decode;   // separate accumulators for hi*hi and the cross terms in the decode GEMM (bf16x3)
-  bool use_graph;      // replay the step as a CUDA graph
-  bool nonneg;         // desc.encoder_nonneg: the dictionary rows are built from max(E, 0) (dict_rows_kernel<..., true>)
-  float shift;         // desc.input_shift; non-zero: the batch split also writes x + shift, which the step reads
-};
-
-struct sce_plan : PlanBuffers {
-  sce_desc d;
-  sce_buffers b;
-  PlanConfig cfg;
-  int sms;
-  int device;  // CUDA device the plan was created on (the caller keeps it current for every call)
-  int code_batch_major;            // 1: the last call was a dw_native backward, which left the code's residual plane
-                                   // only in its batch-major copy (ct.x8): dcode overwrote the row-major one (carve)
-  int tk_groups, tk_group_off[5], tk_group_krows[4];   // classes: models [off[g], off[g+1]) need at most krows[g] rows
-  std::map<int, BatchMaps*>* maps;
-  cudaStream_t cap_stream;  // private stream the step is captured on
-  int last_launches;
-  long long step;  // number of optimiser steps taken
-  // optional per-phase device timing (sce_profile_*): events bracket each phase of a step
-  bool prof_on;
-  int prof_steps;                          // steps recorded since sce_profile_begin
-  cudaEvent_t* prof_ev;                    // [kProfMaxSteps][SCE_PHASE_COUNT + 1]
-};
-
-constexpr int kProfMaxSteps = 64;
-
-static int validate(const sce_desc* d) {
+int validate(const sce_desc* d) {
   if (!d) return fail(SCE_ERR_INVALID, "desc is NULL");
   if (d->variant < SCE_TIED || d->variant > SCE_TIED_LEARNED_CENTER) return fail(SCE_ERR_INVALID, "unknown variant %d", d->variant);
   if (d->n_models < 1 || d->batch_max < 1) return fail(SCE_ERR_INVALID, "n_models and batch_max must be >= 1");
@@ -747,7 +291,7 @@ static int validate(const sce_desc* d) {
 }
 
 // one call's rows: 1 <= B <= batch_max (`prefix` names the entry point in the message, "" for the training calls)
-static int check_rows(const sce_plan* p, int B, const char* prefix) {
+int check_rows(const sce_plan* p, int B, const char* prefix) {
   if (B < 1 || B > p->d.batch_max)
     return fail(SCE_ERR_INVALID, "%sB = %d outside [1, batch_max = %d]", prefix, B, p->d.batch_max);
   return SCE_OK;
@@ -779,7 +323,7 @@ static int topk_slices(const sce_desc& d, size_t kmax) {
 }
 
 // The configuration of a plan for a validated descriptor
-static PlanConfig plan_config(const sce_desc& d) {
+PlanConfig plan_config(const sce_desc& d) {
   PlanConfig c{};
   c.arith = resolve_arith(d);
   c.untied = d.variant == SCE_UNTIED;
@@ -979,25 +523,6 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
   return SCE_OK;
 }
 
-// One call of a plan: its launches, and the batch of B rows and its tensor maps (run_pipeline opens it)
-struct PlanCall : Launcher {
-  sce_plan* p;
-  BatchMaps* maps;
-  int B;
-  float* row_part = nullptr;   // tracked steps: the decode epilogue's per-row partials of r^2 (EpiDecodeT<..., true>)
-  // one GEMM of the plan. NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN
-  // then describe the fp16 planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps
-  // batch-major copies.
-  template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int AR, bool NATIVE = AR == kArithF16F8 && !A_MN, class... A>
-  int gemm(const A&... args) {
-    return launch_gemm_t<Epi, A_MN, B_MN, SPLIT_ACC, AR, NATIVE>(*this, p->d.n_models, p->device, p->sms, args...);
-  }
-  // with sce_profile_begin: the event at the start of phase `idx` of this step (SCE_PHASE_COUNT: the step's end)
-  void mark(int idx) {
-    if (p->prof_on && p->prof_steps < kProfMaxSteps)
-      cudaEventRecord(p->prof_ev[p->prof_steps * (SCE_PHASE_COUNT + 1) + idx], st);
-  }
-};
 
 // ------------------------------------------------------------------------------------------------
 // helpers shared by step / forward / grads
@@ -1068,7 +593,7 @@ static int transpose_dict(Launcher& L, const sce_plan* p) {
 }
 
 // The normalised operand planes of every dictionary side from the fp32 parameters (sce_prepare, sce_resample)
-static int prepare_dict(Launcher& L, const sce_plan* p) {
+int prepare_dict(Launcher& L, const sce_plan* p) {
   DictSide sides[2];
   for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
     TRY(launch_dict_rows<MODE_PREPARE>(L, p, sides[s], nullptr, hyper_for(p, 1)));
@@ -1372,8 +897,8 @@ static int run_pipeline_t(PlanCall& c, const float* x, float* x_hat, bool backwa
 
 // Opens call `c` of plan `p` on `st` for the B rows of `x` (checks them, finds or builds the batch's tensor maps) and
 // runs the pipeline in it
-static int run_pipeline(PlanCall& c, sce_plan* p, const float* x, int B, cudaStream_t st, float* x_hat, bool backward,
-                        float* out_losses, float* out_nnz, float* mom_part = nullptr, float* row_part = nullptr) {
+int run_pipeline(PlanCall& c, sce_plan* p, const float* x, int B, cudaStream_t st, float* x_hat, bool backward,
+                 float* out_losses, float* out_nnz, float* mom_part, float* row_part) {
   TRY(check_rows(p, B, ""));
   if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
   c = PlanCall{{st}, p, nullptr, B, row_part};
@@ -1427,325 +952,83 @@ static int train_tail(PlanCall& c, const AdamHyper& h, float* const* grad_out, f
                   adam ? p->res_flags : nullptr);
 }
 
-// ------------------------------------------------------------------------------------------------
-// evaluation statistics (sce_forward_stats): per-feature moments and segment activity counts
-// ------------------------------------------------------------------------------------------------
-// Top-k plans: moment partials from the fp32 scores and the activity mask the selection left in the workspace, in the
-// layout of EncodeMomentParams ([M][row_blocks][4][n]): the code is relu(score) where the mask bit is set, 0 elsewhere.
-// One warp per (32-column chunk, row block): lane j sums column 32 chunk + j over the 32 rows in order.
-__global__ void __launch_bounds__(256) topk_moment_kernel(const float* __restrict__ scores, const uint32_t* __restrict__ pos,
-                                                          int n_chunks, int batch_max, int B, int n, int row_blocks,
-                                                          float* __restrict__ part) {
-  const int chunk = blockIdx.x, model = blockIdx.z, lane = threadIdx.x & 31;
-  const int rb = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (rb >= row_blocks) return;
-  const int col = chunk * 32 + lane;
-  const uint32_t* pw = pos + ((long long)model * n_chunks + chunk) * batch_max;
-  const float* s = scores + (long long)model * batch_max * n;
-  float a1 = 0.f, a2 = 0.f, a3 = 0.f, a4 = 0.f;
-  const int r_end = min(B, rb * 32 + 32);
-  for (int r = rb * 32; r < r_end; ++r) {
-    const uint32_t w = __ldg(pw + r);
-    if (col < n && ((w >> (31 - lane)) & 1u)) {
-      const float c = fmaxf(__ldg(s + (long long)r * n + col), 0.f), c2 = c * c;
-      a1 += c;
-      a2 += c2;
-      a3 += c2 * c;
-      a4 += c2 * c2;
-    }
-  }
-  if (col < n) {
-    float* o = part + ((long long)model * row_blocks + rb) * 4 * n + col;
-    o[0] = a1;
-    o[n] = a2;
-    o[2 * (long long)n] = a3;
-    o[3 * (long long)n] = a4;
-  }
+// every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph), counted in `c`
+static int step_launches(PlanCall& c, sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
+                         cudaStream_t st, float* row_part = nullptr) {
+  TRY(run_pipeline(c, p, x, B, st, nullptr, true, out_losses, out_nnz, nullptr, row_part));
+  TRY(train_tail<MODE_ADAM>(c, hyper_for(p, t), nullptr, nullptr));
+  c.mark(SCE_PHASE_COUNT);
+  return SCE_OK;
 }
 
-// sums[m][j][p] += sum over the row blocks, in order, of part[m][rb][p][j] (fp64): bitwise repeatable, no atomics
-__global__ void moment_reduce_kernel(const float* __restrict__ part, int row_blocks, int n, double* __restrict__ sums) {
-  const int col = blockIdx.x * blockDim.x + threadIdx.x, model = blockIdx.y;
-  if (col >= n) return;
-  double a[4] = {0.0, 0.0, 0.0, 0.0};
-  for (int rb = 0; rb < row_blocks; ++rb) {
-    const float* o = part + ((long long)model * row_blocks + rb) * 4 * n + col;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) a[q] += (double)__ldg(o + (long long)q * n);
-  }
-  double* out = sums + ((long long)model * n + col) * 4;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) out[q] += a[q];
+// Launch-bound shapes (a step of ~10 kernels that each run a few microseconds, e.g. BASELINE config 1) replay the
+// step as one CUDA graph: the batch is first copied into the plan's staging buffer so that every kernel argument is
+// stable, the graph is captured on the second step at a given batch size (the first one runs eagerly and performs
+// the one-off cudaFuncSetAttribute calls); the captured kernels write the plan's staging outputs, which are copied to
+// the caller's buffers after the launch.
+static bool graph_eligible(const sce_plan* p) {
+  if (p->prof_on) return false;                                   // per-phase events are recorded eagerly
+  if (p->d.adam_count_mode != SCE_ADAM_FROZEN_T1) return false;   // bias correction is a kernel argument that moves
+  return p->cfg.use_graph;
 }
 
-// Segment activity counts (calc_moments_streaming's times_active, standard_metrics.py:482-511): the rows are cut into
-// segments of `seg`; counts[m][j] += number of segments that END in this call in which some row has [c > 0] in column j.
-// `phase` rows of the first segment were seen by earlier calls, whose activity is carried in open[m][j] (0 / 1); the
-// flag of a segment that stays open past this call is written back there. One block per (32-column chunk, model); warp
-// w takes the segments w, w + 8, ...; lanes OR 32 rows' mask words at a time, so lane j ends with column j's flag.
-__global__ void __launch_bounds__(256) segment_count_kernel(const uint32_t* __restrict__ pos, int n_chunks, int batch_max,
-                                                            int B, int n, int seg, int phase, int* __restrict__ counts,
-                                                            int* __restrict__ open) {
-  __shared__ int red[8][32];
-  const int chunk = blockIdx.x, model = blockIdx.y;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t* p = pos + ((long long)model * n_chunks + chunk) * batch_max;
-  const int col = chunk * 32 + lane;
-  const long long oi = (long long)model * n + col;
-  const int carried = col < n ? open[oi] : 0;
-  __syncthreads();   // every read of open[] precedes the write below
-  const long long K = ((long long)B + phase + seg - 1) / seg;   // segments this call touches
-  int mine = 0;
-  for (long long k = warp; k < K; k += 8) {
-    const long long lo = k == 0 ? 0 : k * seg - phase;
-    const long long end = (k + 1) * seg - phase;
-    const long long hi = end < B ? end : B;
-    uint32_t any = 0u;
-    for (long long r = lo + lane; r < hi; r += 32) any |= __ldg(p + r);
-    any = __reduce_or_sync(0xffffffffu, any);
-    int act = (int)((any >> (31 - lane)) & 1u);
-    if (k == 0) act |= carried;
-    if (end <= B) {
-      mine += act;
-      if (k == K - 1 && col < n) open[oi] = 0;
-    } else if (col < n) {
-      open[oi] = act;   // (only the last segment can stay open)
-    }
-  }
-  red[warp][lane] = mine;
-  __syncthreads();
-  if (warp == 0) {
-    int t = 0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += red[i][lane];
-    if (col < n) counts[oi] += t;
-  }
-}
-
-// The workspace of one forward-stats call: the moment partials [M][ceil(B / 32)][4][n] fp32. With base == nullptr only
-// measures it.
-static size_t stats_carve(uint8_t* base, const sce_desc& d, int B, float** part) {
-  Carve c{base, 0};
-  float* mp = c.take<float>((size_t)d.n_models * ((B + 31) / 32) * 4 * d.n);
-  if (part) *part = mp;
-  return align_up(c.off, 1024);
-}
-
-// ------------------------------------------------------------------------------------------------
-// top-activating and random activating fragments (sce_forward_fragments; interpret.py:82-212 record tables,
-// :265-321 record selection): fragment g of a call is rows g L .. g L + L - 1.
-// ------------------------------------------------------------------------------------------------
-struct FragCode {             // the code of the last forward, as the engine holds it
-  const void* hi;             // the code's 16-bit plane [M][batch_max][n] (bf16 or fp16)
-  const void* lo;             // bf16x3: its second bf16 plane
-  const uint8_t* x8;          // f16f8: E5M2 plane of the scaled residuals
-  const float* scores;        // top-k: fp32 scores [M][batch_max][n]
-  const uint32_t* pos;        // activity mask [M][n_chunks][batch_max]
-  int n_chunks, batch_max, n;
-};
-
-// One element c[m, r, j] of the code: SAE variants join the operand planes exactly as join_code_kernel does (-0 -> +0);
-// top-k is relu(score) under the activity mask.
-template <int ARITH, bool TOPK>
-__device__ __forceinline__ float frag_code_value(const FragCode& c, int m, int r, int j) {
-  const long long idx = ((long long)m * c.batch_max + r) * c.n + j;
-  float v;
-  if constexpr (TOPK) {
-    const uint32_t w = __ldg(c.pos + ((long long)m * c.n_chunks + (j >> 5)) * c.batch_max + r);
-    v = ((w >> (31 - (j & 31))) & 1u) ? fmaxf(__ldg(c.scores + idx), 0.f) : 0.f;
-  } else if constexpr (ARITH == kArithF16F8) {
-    constexpr float kInv = 1.f / float(1 << kLoShift);
-    v = __half2float(static_cast<const __half*>(c.hi)[idx]) + e5m2_to_float(c.x8[idx]) * kInv;
+// sce_step; with row_part (sce_step_tracked) the step also leaves its per-row partials there, and runs eagerly
+int step_impl(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, cudaStream_t st, float* row_part) {
+  if (int rc = check_rows(p, B, "")) return rc;
+  if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
+  PlanCall c;
+  int rc;
+  if (row_part || !graph_eligible(p)) {
+    rc = step_launches(c, p, x, B, out_losses, out_nnz, p->step + 1, st, row_part);
   } else {
-    v = __bfloat162float(static_cast<const __nv_bfloat16*>(c.hi)[idx]) +
-        __bfloat162float(static_cast<const __nv_bfloat16*>(c.lo)[idx]);
-  }
-  return v == 0.f ? 0.f : v;
-}
-
-// fmax[m][g][j] = max over the L rows of fragment g of c[m, r, j]; active[m][g][j] = 1 where the activity mask has
-// c > 0 on some row of it. One block per (32-column chunk, fragment, model): lane j reads column 32 chunk + j, so every
-// row is read coalesced over the features; warp w takes the rows w, w + 8, ... and the 8 warps meet in shared memory.
-template <int ARITH, bool TOPK>
-__global__ void __launch_bounds__(256) fragment_max_kernel(FragCode c, int L, int G, float* __restrict__ fmax,
-                                                           uint8_t* __restrict__ active) {
-  __shared__ float smax[8][32];
-  __shared__ uint32_t sact[8][32];
-  const int chunk = blockIdx.x, g = blockIdx.y, m = blockIdx.z;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int j = chunk * 32 + lane;
-  const uint32_t* pw = c.pos + ((long long)m * c.n_chunks + chunk) * c.batch_max;
-  float mx = 0.f;
-  uint32_t any = 0u;
-  for (int t = warp; t < L; t += 8) {
-    const int r = g * L + t;
-    any |= __ldg(pw + r);
-    if (j < c.n) mx = fmaxf(mx, frag_code_value<ARITH, TOPK>(c, m, r, j));
-  }
-  smax[warp][lane] = mx;
-  sact[warp][lane] = (any >> (31 - lane)) & 1u;
-  __syncthreads();
-  if (warp == 0 && j < c.n) {
-    float v = smax[0][lane];
-    uint32_t a = sact[0][lane];
-#pragma unroll
-    for (int w = 1; w < 8; ++w) {
-      v = fmaxf(v, smax[w][lane]);
-      a |= sact[w][lane];
-    }
-    const long long o = ((long long)m * G + g) * c.n + j;
-    fmax[o] = v;
-    active[o] = (uint8_t)a;
-  }
-}
-
-// splitmix64 (Steele, Lea & Flood 2014): the priority of fragment `frag` for feature `feature` under `seed` is
-// mix(mix(mix(seed) ^ feature) ^ frag) >> 1, a 63-bit key that depends on nothing but these three numbers
-__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
-  z += 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-// list order: (key descending, fragment ascending); an entry with fragment < 0 is empty and below every other
-template <class K>
-__device__ __forceinline__ bool frag_above(K k, long long f, K k2, long long f2) {
-  return f2 < 0 || (f >= 0 && (k > k2 || (k == k2 && f < f2)));
-}
-template <class K>
-__device__ __forceinline__ int frag_lowest(const K* key, const long long* frag, int cap) {
-  int w = 0;
-  for (int i = 1; i < cap; ++i)
-    if (frag_above(key[w], frag[w], key[i], frag[i])) w = i;
-  return w;
-}
-
-// One thread per (feature, model) walks the call's fragments in order and keeps two lists of `cap` entries that persist
-// across calls: (fragment maximum, fragment) over all fragments, and (priority, fragment) over the active ones. A
-// candidate replaces the list's lowest entry when it is above it, and then its L code values are copied into that
-// entry's row of top_act / rnd_act. The lists are sets (sorted by the caller after the last call): the result depends
-// on nothing but the fragments seen, with no atomics.
-template <int ARITH, bool TOPK>
-__global__ void __launch_bounds__(128) fragment_merge_kernel(FragCode c, int L, int G, long long frag0,
-                                                             const float* __restrict__ fmax,
-                                                             const uint8_t* __restrict__ active, int n_top, int n_random,
-                                                             unsigned long long seed, float* top_val, long long* top_frag,
-                                                             float* top_act, long long* rnd_key, long long* rnd_frag,
-                                                             float* rnd_act) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
-  if (j >= c.n) return;
-  const long long list = (long long)m * c.n + j;
-  float* tv = top_val + list * n_top;
-  long long* tf = top_frag + list * n_top;
-  long long* rk = rnd_key + list * n_random;
-  long long* rf = rnd_frag + list * n_random;
-  const uint64_t h_feat = splitmix64(splitmix64(seed) ^ (uint64_t)j);
-  int tlow = n_top ? frag_lowest(tv, tf, n_top) : 0;
-  int rlow = n_random ? frag_lowest(rk, rf, n_random) : 0;
-  for (int g = 0; g < G; ++g) {
-    const long long o = ((long long)m * G + g) * c.n + j, frag = frag0 + g;
-    if (n_top) {
-      const float v = __ldg(fmax + o);
-      if (frag_above(v, frag, tv[tlow], tf[tlow])) {
-        tv[tlow] = v;
-        tf[tlow] = frag;
-        if (top_act) {
-          float* dst = top_act + (list * n_top + tlow) * L;
-          for (int t = 0; t < L; ++t) dst[t] = frag_code_value<ARITH, TOPK>(c, m, g * L + t, j);
-        }
-        tlow = frag_lowest(tv, tf, n_top);
+    BatchMaps* maps = nullptr;
+    rc = build_maps(p, B, &maps);
+    if (rc) return rc;
+    const size_t bytes = (size_t)p->cfg.input_models * B * p->d.d * sizeof(float);
+    if (x != p->x_stage) CUDA_TRY(cudaMemcpyAsync(p->x_stage, x, bytes, cudaMemcpyDeviceToDevice, st));
+    // the captured kernels write the plan's own staging outputs (stable addresses: callers may pass fresh tensors
+    // every step, as the reference returns them); the results are copied out below
+    float* const cap_losses = p->loss_stage;
+    float* const cap_nnz = p->nnz_stage;
+    if (maps->graph) {
+      CUDA_TRY(cudaGraphLaunch(maps->graph, st));
+      c.count = maps->graph_launches;
+    } else if (maps->eager_steps == 0) {
+      maps->eager_steps = 1;
+      rc = step_launches(c, p, p->x_stage, B, cap_losses, cap_nnz, 1, st);
+    } else {
+      // capture on a private stream (the caller's may be the legacy default stream, which cannot be captured);
+      // capturing records the launches without running them, the instantiated graph is launched on `st`
+      cudaGraph_t g = nullptr;
+      if (!p->cap_stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->cap_stream, cudaStreamNonBlocking));
+      CUDA_TRY(cudaStreamBeginCapture(p->cap_stream, cudaStreamCaptureModeThreadLocal));
+      rc = step_launches(c, p, p->x_stage, B, cap_losses, cap_nnz, 1, p->cap_stream);
+      cudaError_t ce = cudaStreamEndCapture(p->cap_stream, &g);
+      if (rc == SCE_OK && ce == cudaSuccess && g) {
+        cudaGraphExec_t ge = nullptr;
+        ce = cudaGraphInstantiate(&ge, g, 0);
+        cudaGraphDestroy(g);
+        if (ce != cudaSuccess) return fail(SCE_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
+        maps->graph = ge;
+        maps->graph_launches = c.count;
+        CUDA_TRY(cudaGraphLaunch(maps->graph, st));
+      } else {
+        if (g) cudaGraphDestroy(g);
+        cudaGetLastError();
+        if (rc == SCE_OK) return fail(SCE_ERR_CUDA, "stream capture of the step failed: %s", cudaGetErrorString(ce));
       }
     }
-    if (n_random && __ldg(active + o)) {
-      const long long k = (long long)(splitmix64(h_feat ^ (uint64_t)frag) >> 1);
-      if (frag_above(k, frag, rk[rlow], rf[rlow])) {
-        rk[rlow] = k;
-        rf[rlow] = frag;
-        if (rnd_act) {
-          float* dst = rnd_act + (list * n_random + rlow) * L;
-          for (int t = 0; t < L; ++t) dst[t] = frag_code_value<ARITH, TOPK>(c, m, g * L + t, j);
-        }
-        rlow = frag_lowest(rk, rf, n_random);
-      }
-    }
+    if (rc == SCE_OK && out_losses && out_losses != cap_losses)
+      CUDA_TRY(cudaMemcpyAsync(out_losses, cap_losses, (size_t)p->d.n_models * SCE_LOSS_COLS * sizeof(float),
+                               cudaMemcpyDeviceToDevice, st));
+    if (rc == SCE_OK && out_nnz && out_nnz != cap_nnz)
+      CUDA_TRY(cudaMemcpyAsync(out_nnz, cap_nnz, (size_t)p->d.n_models * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
-}
-
-constexpr int kFragMaxList = 64;   // largest n_top / n_random
-
-static bool frag_len_ok(int L) { return L >= 32 && L <= 8192 && L % 32 == 0; }
-
-// The workspace of one fragments call: fragment maxima [M][B/L][n] fp32, activity flags [M][B/L][n] u8, open-segment
-// flags [M][n] int32. With base == nullptr only measures it.
-struct FragCarve {
-  float* fmax;
-  uint8_t* active;
-  int* open;
-};
-static size_t frag_carve(uint8_t* base, const sce_desc& d, int B, int L, FragCarve* out) {
-  const size_t cells = (size_t)d.n_models * (B / L) * d.n;
-  Carve c{base, 0};
-  FragCarve w;
-  w.fmax = c.take<float>(cells);
-  w.active = c.take<uint8_t>(cells);
-  w.open = c.take<int>((size_t)d.n_models * d.n);
-  if (out) *out = w;
-  return align_up(c.off, 1024);
-}
-
-template <int ARITH, bool TOPK>
-static int launch_fragments(Launcher& launcher, const FragCode& c, int M, int L, int G, long long frag0, float* fmax,
-                            uint8_t* active, int n_top, int n_random, unsigned long long seed, float* top_val,
-                            long long* top_frag, float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act) {
-  TRY(launcher.launch(fragment_max_kernel<ARITH, TOPK>, dim3(c.n_chunks, G, M), 256, 0, c, L, G, fmax, active));
-  return launcher.launch(fragment_merge_kernel<ARITH, TOPK>, dim3((c.n + 127) / 128, M), 128, 0, c, L, G, frag0, fmax,
-                         active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
-}
-
-// The scratch of one tracked step or resample (sce_track.workspace). With base == nullptr only measures it.
-struct TrackCarve {
-  float* row_part;              // [M][batch_max][2 tiles_n] decode epilogue partials (unused by k-sparse top-k plans)
-  unsigned long long* keys;     // [M][N + batch_max]
-  int *enter_row, *enter_slot;  // [M][cap]
-  int* enter_cnt;               // [M]
-  int cap;                      // min(N, batch_max)
-  double* norms;                // [M][n]
-  int *order, *dead;            // [M][N], [M][n]
-  int* n_rep;                   // [M]
-  float* scale;                 // [M]
-};
-static size_t track_carve(uint8_t* base, const sce_desc& d, int N, TrackCarve* out) {
-  const size_t M = d.n_models, Bm = d.batch_max, n = d.n;
-  Carve c{base, 0};
-  TrackCarve w;
-  w.cap = N < d.batch_max ? N : d.batch_max;
-  w.row_part = c.take<float>(M * Bm * 2 * ((d.d + kBN - 1) / kBN));
-  w.keys = c.take<unsigned long long>(M * (N + Bm));
-  w.enter_row = c.take<int>(M * w.cap);
-  w.enter_slot = c.take<int>(M * w.cap);
-  w.enter_cnt = c.take<int>(M);
-  w.norms = c.take<double>(M * n);
-  w.order = c.take<int>(M * N);
-  w.dead = c.take<int>(M * n);
-  w.n_rep = c.take<int>(M);
-  w.scale = c.take<float>(M);
-  if (out) *out = w;
-  return align_up(c.off, 1024);
-}
-
-// The checks of sce_step_tracked / sce_resample that come before any device call. Those on the track alone come first,
-// then the plan and what depends on it; carves the workspace into `w`.
-static int check_track(const sce_plan* p, const sce_track* t, const char* prefix, TrackCarve* w) {
-  if (!t) return fail(SCE_ERR_INVALID, "%strack is NULL", prefix);
-  if (!t->err || !t->serial || !t->rows || !t->filled || !t->counts)
-    return fail(SCE_ERR_INVALID, "%strack: err, serial, rows, filled and counts are required", prefix);
-  if (reinterpret_cast<uintptr_t>(t->rows) % 16) return fail(SCE_ERR_INVALID, "%strack: rows must be 16-byte aligned", prefix);
-  if (t->n_worst < 1) return fail(SCE_ERR_INVALID, "%strack: n_worst = %d must be >= 1", prefix, t->n_worst);
-  if (!p) return fail(SCE_ERR_INVALID, "%splan is NULL", prefix);
-  if (t->n_worst > p->d.n) return fail(SCE_ERR_INVALID, "%strack: n_worst = %d outside [1, n = %d]", prefix, t->n_worst, p->d.n);
-  const size_t need = track_carve(static_cast<uint8_t*>(t->workspace), p->d, t->n_worst, w);
-  return check_workspace(t->workspace, t->workspace_bytes, need, prefix);
+  if (rc) return rc;
+  p->last_launches = c.count;   // every launch of the step, eager or replayed
+  p->step += 1;
+  if (p->prof_on && p->prof_steps < kProfMaxSteps) p->prof_steps += 1;
+  return SCE_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1886,86 +1169,6 @@ int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_los
   return SCE_OK;
 }
 
-// every launch of one optimisation step, in order, on `st` (also what gets captured into a CUDA graph), counted in `c`
-static int step_launches(PlanCall& c, sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, long long t,
-                         cudaStream_t st, float* row_part = nullptr) {
-  TRY(run_pipeline(c, p, x, B, st, nullptr, true, out_losses, out_nnz, nullptr, row_part));
-  TRY(train_tail<MODE_ADAM>(c, hyper_for(p, t), nullptr, nullptr));
-  c.mark(SCE_PHASE_COUNT);
-  return SCE_OK;
-}
-
-// Launch-bound shapes (a step of ~10 kernels that each run a few microseconds, e.g. BASELINE config 1) replay the
-// step as one CUDA graph: the batch is first copied into the plan's staging buffer so that every kernel argument is
-// stable, the graph is captured on the second step at a given batch size (the first one runs eagerly and performs
-// the one-off cudaFuncSetAttribute calls); the captured kernels write the plan's staging outputs, which are copied to
-// the caller's buffers after the launch.
-static bool graph_eligible(const sce_plan* p) {
-  if (p->prof_on) return false;                                   // per-phase events are recorded eagerly
-  if (p->d.adam_count_mode != SCE_ADAM_FROZEN_T1) return false;   // bias correction is a kernel argument that moves
-  return p->cfg.use_graph;
-}
-
-// sce_step; with row_part (sce_step_tracked) the step also leaves its per-row partials there, and runs eagerly
-static int step_impl(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, cudaStream_t st,
-                     float* row_part) {
-  if (int rc = check_rows(p, B, "")) return rc;
-  if (!x) return fail(SCE_ERR_INVALID, "x is NULL");
-  PlanCall c;
-  int rc;
-  if (row_part || !graph_eligible(p)) {
-    rc = step_launches(c, p, x, B, out_losses, out_nnz, p->step + 1, st, row_part);
-  } else {
-    BatchMaps* maps = nullptr;
-    rc = build_maps(p, B, &maps);
-    if (rc) return rc;
-    const size_t bytes = (size_t)p->cfg.input_models * B * p->d.d * sizeof(float);
-    if (x != p->x_stage) CUDA_TRY(cudaMemcpyAsync(p->x_stage, x, bytes, cudaMemcpyDeviceToDevice, st));
-    // the captured kernels write the plan's own staging outputs (stable addresses: callers may pass fresh tensors
-    // every step, as the reference returns them); the results are copied out below
-    float* const cap_losses = p->loss_stage;
-    float* const cap_nnz = p->nnz_stage;
-    if (maps->graph) {
-      CUDA_TRY(cudaGraphLaunch(maps->graph, st));
-      c.count = maps->graph_launches;
-    } else if (maps->eager_steps == 0) {
-      maps->eager_steps = 1;
-      rc = step_launches(c, p, p->x_stage, B, cap_losses, cap_nnz, 1, st);
-    } else {
-      // capture on a private stream (the caller's may be the legacy default stream, which cannot be captured);
-      // capturing records the launches without running them, the instantiated graph is launched on `st`
-      cudaGraph_t g = nullptr;
-      if (!p->cap_stream) CUDA_TRY(cudaStreamCreateWithFlags(&p->cap_stream, cudaStreamNonBlocking));
-      CUDA_TRY(cudaStreamBeginCapture(p->cap_stream, cudaStreamCaptureModeThreadLocal));
-      rc = step_launches(c, p, p->x_stage, B, cap_losses, cap_nnz, 1, p->cap_stream);
-      cudaError_t ce = cudaStreamEndCapture(p->cap_stream, &g);
-      if (rc == SCE_OK && ce == cudaSuccess && g) {
-        cudaGraphExec_t ge = nullptr;
-        ce = cudaGraphInstantiate(&ge, g, 0);
-        cudaGraphDestroy(g);
-        if (ce != cudaSuccess) return fail(SCE_ERR_CUDA, "cudaGraphInstantiate failed: %s", cudaGetErrorString(ce));
-        maps->graph = ge;
-        maps->graph_launches = c.count;
-        CUDA_TRY(cudaGraphLaunch(maps->graph, st));
-      } else {
-        if (g) cudaGraphDestroy(g);
-        cudaGetLastError();
-        if (rc == SCE_OK) return fail(SCE_ERR_CUDA, "stream capture of the step failed: %s", cudaGetErrorString(ce));
-      }
-    }
-    if (rc == SCE_OK && out_losses && out_losses != cap_losses)
-      CUDA_TRY(cudaMemcpyAsync(out_losses, cap_losses, (size_t)p->d.n_models * SCE_LOSS_COLS * sizeof(float),
-                               cudaMemcpyDeviceToDevice, st));
-    if (rc == SCE_OK && out_nnz && out_nnz != cap_nnz)
-      CUDA_TRY(cudaMemcpyAsync(out_nnz, cap_nnz, (size_t)p->d.n_models * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  }
-  if (rc) return rc;
-  p->last_launches = c.count;   // every launch of the step, eager or replayed
-  p->step += 1;
-  if (p->prof_on && p->prof_steps < kProfMaxSteps) p->prof_steps += 1;
-  return SCE_OK;
-}
-
 int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
   return step_impl(p, x, B, out_losses, out_nnz, static_cast<cudaStream_t>(stream), nullptr);
@@ -1997,27 +1200,6 @@ int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_hos
   if (out_nnz_host)
     CUDA_TRY(cudaMemcpyAsync(out_nnz_host, p->nnz_stage, (size_t)p->d.n_models * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  return SCE_OK;
-}
-
-int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
-  if (!p || !out_code) return fail(SCE_ERR_INVALID, "plan / out_code is NULL");
-  if (int rc = check_rows(p, B, "")) return rc;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  const long long per = (long long)B * p->d.n;
-  if (p->code_batch_major) {
-    const long long total = (long long)p->d.n_models * per;
-    return L.launch(join_code_batch_major_kernel, (unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096), 256,
-                    0, static_cast<const __half*>(p->c.hi), p->ct.x8, out_code, B, p->d.n, p->d.batch_max, p->cfg.bpad,
-                    total);
-  }
-  for (int m = 0; m < p->d.n_models; ++m) {
-    const Planes c = p->c.at((size_t)m * p->d.batch_max * p->d.n);
-    TRY(with_arith(p->cfg.arith, [&](auto arith) {   // (each arithmetic reads its own planes)
-      return L.launch(join_code_kernel<decltype(arith)::value>, 1024, 256, 0, c.hi, c.lo, c.x8, out_code + (long long)m * per,
-                      per / 2);
-    }));
-  }
   return SCE_OK;
 }
 
@@ -2059,157 +1241,6 @@ int sce_clear_health(sce_plan* plan, void* stream) {
   if (!plan) return fail(SCE_ERR_INVALID, "plan is NULL");
   CUDA_TRY(cudaMemsetAsync(plan->res_flags + kBadWord, 0, sizeof(uint32_t), static_cast<cudaStream_t>(stream)));
   return SCE_OK;
-}
-
-int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
-  if (!plan || !counts) return fail(SCE_ERR_INVALID, "plan / counts is NULL");
-  if (int rc = check_rows(plan, B, "")) return rc;
-  const int n_chunks = (plan->d.n + 31) / 32;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  return L.launch(active_count_kernel, dim3(n_chunks, plan->d.n_models), 256, 0, plan->act_pos, n_chunks,
-                  plan->d.batch_max, B, plan->d.n, counts);
-}
-
-// The checks that open sce_forward_stats and sce_forward_fragments; `prefix` names the entry point in the messages
-static int check_forward_only(const sce_plan* p, const float* x, int B, const char* prefix) {
-  if (!p) return fail(SCE_ERR_INVALID, "%splan is NULL", prefix);
-  if (!p->cfg.evaluable)
-    return fail(SCE_ERR_INVALID, "%snot available for the learned-centre variant or with encoder_nonneg / input_shift; "
-                                 "evaluate the exported dictionaries (TiedSAE)", prefix);
-  TRY(check_rows(p, B, prefix));
-  if (!x) return fail(SCE_ERR_INVALID, "%sx is NULL", prefix);
-  return SCE_OK;
-}
-
-size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !plan_config(*desc).evaluable) return 0;
-  return stats_carve(nullptr, *desc, B, nullptr);
-}
-
-int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase, float* x_hat, float* out_losses,
-                      float* out_nnz, double* moment_sums, int* seg_counts, int* seg_open, void* workspace,
-                      size_t workspace_bytes, void* stream) {
-  TRY(check_forward_only(p, x, B, "forward_stats: "));
-  if (seg < 1) return fail(SCE_ERR_INVALID, "forward_stats: seg = %d must be >= 1", seg);
-  if (seg_phase < 0 || seg_phase >= seg)
-    return fail(SCE_ERR_INVALID, "forward_stats: seg_phase = %d outside [0, seg = %d)", seg_phase, seg);
-  if (!out_losses || !out_nnz || !moment_sums || !seg_counts)
-    return fail(SCE_ERR_INVALID, "forward_stats: out_losses, out_nnz, moment_sums and seg_counts are required");
-  if (seg > 1 && !seg_open) return fail(SCE_ERR_INVALID, "forward_stats: seg > 1 needs the seg_open flags");
-  float* part;
-  const size_t need = stats_carve(static_cast<uint8_t*>(workspace), p->d, B, &part);
-  if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_stats: ")) return rc;
-  const sce_desc& d = p->d;
-  PlanCall c;
-  TRY(run_pipeline(c, p, x, B, static_cast<cudaStream_t>(stream), x_hat, false, out_losses, out_nnz,
-                   p->cfg.topk ? nullptr : part));
-  p->last_launches = c.count;   // the pipeline's: the statistics kernels below are not counted
-  const int n_chunks = (d.n + 31) / 32, row_blocks = (B + 31) / 32;
-  if (p->cfg.topk)
-    TRY(c.launch(topk_moment_kernel, dim3(n_chunks, (row_blocks + 7) / 8, d.n_models), 256, 0, p->scores, p->act_pos,
-                 n_chunks, d.batch_max, B, d.n, row_blocks, part));
-  TRY(c.launch(moment_reduce_kernel, dim3((d.n + 255) / 256, d.n_models), 256, 0, part, row_blocks, d.n, moment_sums));
-  if (seg == 1)
-    return c.launch(active_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
-                    seg_counts);
-  return c.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n, seg,
-                  seg_phase, seg_counts, seg_open);
-}
-
-size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || !plan_config(*desc).evaluable) return 0;
-  return frag_carve(nullptr, *desc, B, L, nullptr);
-}
-
-int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long frag0, int n_top, int n_random,
-                          unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
-                          long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
-                          size_t workspace_bytes, void* stream) {
-  TRY(check_forward_only(p, x, B, "forward_fragments: "));
-  if (!frag_len_ok(L)) return fail(SCE_ERR_INVALID, "forward_fragments: L = %d must be a multiple of 32 in [32, 8192]", L);
-  if (B % L) return fail(SCE_ERR_INVALID, "forward_fragments: B = %d is not a multiple of L = %d", B, L);
-  if (frag0 < 0) return fail(SCE_ERR_INVALID, "forward_fragments: frag0 = %lld must be >= 0", frag0);
-  if (n_top < 0 || n_top > kFragMaxList || n_random < 0 || n_random > kFragMaxList || n_top + n_random == 0)
-    return fail(SCE_ERR_INVALID, "forward_fragments: n_top = %d and n_random = %d must lie in [0, %d], not both 0", n_top,
-                n_random, kFragMaxList);
-  if (n_top && (!top_val || !top_frag)) return fail(SCE_ERR_INVALID, "forward_fragments: n_top > 0 needs top_val and top_frag");
-  if (n_random && (!rnd_key || !rnd_frag))
-    return fail(SCE_ERR_INVALID, "forward_fragments: n_random > 0 needs rnd_key and rnd_frag");
-  if (!n_active) return fail(SCE_ERR_INVALID, "forward_fragments: n_active is required");
-  FragCarve w;
-  const size_t need = frag_carve(static_cast<uint8_t*>(workspace), p->d, B, L, &w);
-  if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_fragments: ")) return rc;
-  const sce_desc& d = p->d;
-  PlanCall call;
-  TRY(run_pipeline(call, p, x, B, static_cast<cudaStream_t>(stream), nullptr, false, nullptr, nullptr));
-  p->last_launches = call.count;   // the pipeline's: the fragment kernels below are not counted
-  const int n_chunks = (d.n + 31) / 32, G = B / L;
-  const FragCode c{p->c.hi, p->c.lo, p->c.x8, p->scores, p->act_pos, n_chunks, d.batch_max, d.n};
-  if (p->cfg.topk)
-    TRY((launch_fragments<kArithBf16x3, true>(call, c, d.n_models, L, G, frag0, w.fmax, w.active, n_top, n_random,
-                                              seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act)));
-  else
-    TRY(with_arith(p->cfg.arith, [&](auto ar) {
-      return launch_fragments<decltype(ar)::value, false>(call, c, d.n_models, L, G, frag0, w.fmax, w.active, n_top,
-                                                          n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag,
-                                                          rnd_act);
-    }));
-  // active fragments: segments of L rows, cut at fragment boundaries (phase 0, no segment stays open)
-  CUDA_TRY(cudaMemsetAsync(w.open, 0, (size_t)d.n_models * d.n * sizeof(int), call.st));
-  return call.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
-                     L, 0, n_active, w.open);
-}
-
-size_t sce_track_workspace_bytes(const sce_desc* desc, int n_worst) {
-  if (validate(desc)) return 0;
-  if (n_worst < 1 || n_worst > desc->n) {
-    fail(SCE_ERR_INVALID, "track: n_worst = %d outside [1, n = %d]", n_worst, desc->n);
-    return 0;
-  }
-  return track_carve(nullptr, *desc, n_worst, nullptr);
-}
-
-int sce_step_tracked(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, const sce_track* track,
-                     void* stream) {
-  TrackCarve w;
-  TRY(check_track(p, track, "step_tracked: ", &w));
-  TRY(check_rows(p, B, "step_tracked: "));
-  if (track->next_serial < 0 || track->next_serial + B >= 0xFFFFFFFFll)
-    return fail(SCE_ERR_INVALID, "step_tracked: next_serial = %lld with B = %d leaves [0, 2^32 - 1)", track->next_serial, B);
-  const sce_desc& d = p->d;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  TRY(step_impl(p, x, B, out_losses, out_nnz, st, p->cfg.topk_sparse ? nullptr : w.row_part));
-  sce::TrackArgs t{track->err, track->serial, track->rows, track->filled, track->counts, track->next_serial,
-                   track->n_worst, p->cfg.topk_sparse ? p->part_dec : w.row_part,
-                   p->cfg.topk_sparse ? p->cfg.tk_slices : 2 * ((d.d + kBN - 1) / kBN), w.keys, w.enter_row, w.enter_slot,
-                   w.enter_cnt, w.cap, x, p->cfg.input_models == 1 ? 0 : (long long)B * d.d};
-  Launcher L{st};
-  const int n_chunks = (d.n + 31) / 32;
-  TRY(L.launch(track_merge_kernel, dim3(1 + n_chunks, d.n_models), kTrackThreads, 0, t, p->act_pos, n_chunks,
-               d.batch_max, B, d.n, d.d, p->res_flags));
-  return L.launch(track_copy_kernel, dim3(w.cap < 1024 ? w.cap : 1024, d.n_models), kTrackThreads, 0, t, d.d);
-}
-
-int sce_resample(sce_plan* p, const sce_track* track, float ratio, int* n_dead, int* n_replaced, unsigned char* replaced,
-                 void* stream) {
-  TrackCarve w;
-  TRY(check_track(p, track, "resample: ", &w));
-  if (!(ratio > 0.f) || !std::isfinite(ratio)) return fail(SCE_ERR_INVALID, "resample: ratio must be positive and finite");
-  if (!n_dead || !n_replaced || !replaced) return fail(SCE_ERR_INVALID, "resample: n_dead, n_replaced and replaced are required");
-  const sce_desc& d = p->d;
-  const sce_buffers& b = p->b;
-  const int M = d.n_models, n = d.n, N = track->n_worst;
-  Launcher L{static_cast<cudaStream_t>(stream)};
-  TRY(L.launch(track_norm_kernel, dim3((n + 7) / 8, M), kTrackThreads, 0, b.encoder, n, d.d, w.norms));
-  TRY(L.launch(track_rank_kernel, dim3((N + kTrackThreads - 1) / kTrackThreads, M), kTrackThreads, 0, track->err,
-               track->serial, track->filled, N, w.order));
-  TRY(L.launch(track_dead_kernel, M, kTrackThreads, 0, track->counts, track->filled, b.coef_mask, w.norms, n, ratio,
-               w.dead, w.n_rep, w.scale, n_dead, n_replaced, replaced));
-  const int cap = N < n ? N : n;
-  TRY(L.launch(track_write_kernel, dim3(cap < 1024 ? cap : 1024, M), kTrackThreads, 0, track->rows, w.order, w.dead, w.n_rep,
-               w.scale, N, n, d.d, b.encoder, b.encoder_m, b.encoder_v, p->cfg.untied ? b.decoder_m : nullptr,
-               p->cfg.untied ? b.decoder_v : nullptr, b.bias_m, b.bias_v));
-  return prepare_dict(L, p);
 }
 
 int sce_plan_arith(const sce_plan* plan) {

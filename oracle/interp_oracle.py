@@ -85,3 +85,96 @@ def fragment_values(code: torch.Tensor, frags: torch.Tensor, L: int) -> torch.Te
     r = (frags.clamp(min=0)[..., None] * L + t).reshape(n, -1)                  # [n, k L] rows
     v = torch.gather(code.T, 1, r).reshape(n, k, L)
     return torch.where(frags[..., None] >= 0, v, torch.zeros((), dtype=v.dtype, device=v.device))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# one engine call (sce_forward_fragments' fragment_merge_kernel) and the per-element bounds of its values
+# ----------------------------------------------------------------------------------------------------------------------
+def list_order(key: torch.Tensor, frag: torch.Tensor) -> torch.Tensor:
+    """[n, k] -> [n, k] per row, the permutation that sorts (key descending, fragment ascending) with the empty entries
+    (fragment < 0) last. The key of an empty entry is never compared: it may be anything, NaN included."""
+    empty = frag < 0
+    key = torch.where(empty, torch.zeros_like(key), key)
+    o = torch.sort(torch.where(empty, torch.iinfo(torch.int64).max, frag), dim=-1, stable=True).indices
+    o = o.gather(-1, torch.sort(key.gather(-1, o), dim=-1, descending=True, stable=True).indices)
+    return o.gather(-1, torch.sort(empty.gather(-1, o).to(torch.int8), dim=-1, stable=True).indices)
+
+
+def _keep(key, frag, rows, cand_key, cand_frag, frag0, code, L, cap):
+    """The ``cap`` highest of a list (key, frag, rows: [n, cap], [n, cap], [n, cap, L] or None) and the candidates
+    (cand_key, cand_frag: [n, G], fragment -1 where not a candidate; their rows are those of ``code``), in list order."""
+    if cap == 0:
+        return key, frag, rows
+    allk, allf = torch.cat([key, cand_key.to(key.dtype)], 1), torch.cat([frag, cand_frag], 1)
+    idx = list_order(allk, allf)[:, :cap]
+    f = allf.gather(1, idx)
+    empty = f < 0
+    k = torch.where(empty, torch.zeros_like(allk[:, :cap]), allk.gather(1, idx))
+    f = torch.where(empty, torch.full_like(f, -1), f)
+    r = None
+    if rows is not None:
+        old = idx < cap
+        kept = rows.gather(1, idx.clamp(max=cap - 1)[..., None].expand(-1, -1, L))
+        new = fragment_values(code, torch.where(old | empty, torch.full_like(f, -1), f - frag0), L).to(rows.dtype)
+        r = torch.where(empty[..., None], torch.zeros_like(kept), torch.where(old[..., None], kept, new))
+    return k, f, r
+
+
+def merge_call(top, rnd, fmax: torch.Tensor, active: torch.Tensor, frag0: int, seed: int, code: torch.Tensor = None,
+               L: int = None):
+    """One sce_forward_fragments call on the caller's lists: what fragment_merge_kernel leaves in them.
+
+    ``top`` = (values [n, n_top], fragments [n, n_top], rows [n, n_top, L] or None) and ``rnd`` = (keys [n, n_random],
+    fragments, rows) as the caller holds them, an entry with fragment < 0 empty whatever its key and rows; ``fmax`` /
+    ``active`` [G, n]: the call's fragment maxima and activity (fragment_tables), its fragment g being frag0 + g; ``code``
+    [G L, n]: the call's code, where rows are wanted. Returns (top, rnd) in the same form, as sets: each list in list
+    order, its empty entries last with key 0, fragment -1 and zero rows. A list of length 0 passes through.
+
+    The top list keeps the n_top highest (maximum, fragment) over its entries and every fragment of the call; the random
+    list the n_random highest (priority, fragment) over its entries and the call's active fragments."""
+    G, n = fmax.shape
+    frags = frag0 + torch.arange(G, device=fmax.device)
+    cand = frags[:, None].expand(G, n).T                                         # [n, G]
+    out_top = _keep(*top, fmax.T, cand, frag0, code, L, top[1].shape[1])
+    p = priority(seed, torch.arange(n, device=fmax.device), frags).T
+    out_rnd = _keep(*rnd, p, torch.where(active.T, cand, torch.full_like(cand, -1)), frag0, code, L, rnd[1].shape[1])
+    return out_top, out_rnd
+
+
+def empty_lists(n: int, k: int, L: int = None, key_dtype=torch.float64, row_dtype=torch.float64, device=None):
+    """n lists of length k with every entry empty, as merge_call takes them (rows only when L is given)."""
+    rows = torch.zeros(n, k, L, dtype=row_dtype, device=device) if L else None
+    return (torch.zeros(n, k, dtype=key_dtype, device=device), torch.full((n, k), -1, dtype=torch.int64, device=device),
+            rows)
+
+
+def value_bounds(S: torch.Tensor, e: float, L: int):
+    """Per-element bounds of the engine's code values and fragment maxima from the code's element bar ``e``
+    (tile_bounds.BARS / TOPK_BARS) and its scale S [N, n] (tile_bounds.code_scale; top-k: on the pinned support). The
+    engine's code is relu of its fp32 pre-activation, and relu is 1-Lipschitz, so |c' - c| <= e S per element (the
+    argument of oracle/eval_bounds.py); a maximum moves by at most the largest bound of its fragment's elements:
+    |max_t c'_t - max_t c_t| <= max_t e S_t. Returns (code bound [N, n], fragment-maximum bound [G, n])."""
+    b = e * S.double().abs()
+    return b, b.reshape(S.shape[0] // L, L, -1).amax(1)
+
+
+def top_ratios(values: torch.Tensor, frags: torch.Tensor, fmax: torch.Tensor, fbound: torch.Tensor):
+    """The engine's top lists ([n, n_top] values and fragments, numbered as the rows of ``fmax``; -1 empty) against the
+    fp64 fragment maxima ``fmax`` [G, n] and their bounds ``fbound`` (value_bounds). Returns per entry, [n, n_top]:
+      value   |value - fmax[frag]| / fbound[frag]
+      set     for a fragment the fp64 top list does not hold: (m_k - fmax[frag]) / (fbound[frag] + fbound[k-th]), m_k
+              the fp64 n_top-th maximum, so it may stand in for the k-th only within both bounds (0 otherwise)
+    Ratios above 1 fail; a NaN value is an infinite ratio."""
+    n_top = frags.shape[1]
+    ref = select_top(fmax, n_top)
+    on = frags >= 0
+    f = frags.clamp(min=0)
+    want, fb = fmax.T.gather(1, f), fbound.T.gather(1, f)
+    err = (values.double() - want).abs()
+    err = torch.where(torch.isnan(err), torch.full_like(err, float("inf")), err)
+    value = torch.where(on & (err > 0), err / fb, torch.zeros_like(err))
+    kth = ref[:, -1:].clamp(min=0)
+    m_k, fb_k = fmax.T.gather(1, kth), fbound.T.gather(1, kth)
+    extra = on & ~(frags[..., None] == ref[:, None, :]).any(-1)
+    gap = (m_k - want).clamp(min=0.0)
+    return {"value": value, "set": torch.where(extra & (gap > 0), gap / (fb + fb_k), torch.zeros_like(gap))}

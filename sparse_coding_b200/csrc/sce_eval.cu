@@ -209,36 +209,41 @@ __global__ void __launch_bounds__(256) read_code_kernel(CodeView<SRC> c, int B, 
 // fmax[m][g][j] = max over the L rows of fragment g of c[m, r, j]; active[m][g][j] = 1 where the activity mask has
 // c > 0 on some row of it. One block per (32-column chunk, fragment, model): lane j reads column 32 chunk + j, so every
 // row is read coalesced over the features; warp w takes the rows w, w + 8, ... and the 8 warps meet in shared memory.
+// grid.y is capped at kMaxGridY: a block takes the fragments blockIdx.y, blockIdx.y + gridDim.y, ... (one when G fits).
+constexpr int kMaxGridY = 65535;
 template <int SRC>
 __global__ void __launch_bounds__(256) fragment_max_kernel(CodeView<SRC> c, int L, int G, float* __restrict__ fmax,
                                                            uint8_t* __restrict__ active) {
   __shared__ float smax[8][32];
   __shared__ uint32_t sact[8][32];
-  const int chunk = blockIdx.x, g = blockIdx.y, m = blockIdx.z;
+  const int chunk = blockIdx.x, m = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int j = chunk * 32 + lane;
   const uint32_t* pw = c.pos + ((long long)m * c.n_chunks + chunk) * c.batch_max;
-  float mx = 0.f;
-  uint32_t any = 0u;
-  for (int t = warp; t < L; t += 8) {
-    const int r = g * L + t;
-    any |= __ldg(pw + r);
-    if (j < c.n) mx = fmaxf(mx, c.at(m, r, j));
-  }
-  smax[warp][lane] = mx;
-  sact[warp][lane] = (any >> (31 - lane)) & 1u;
-  __syncthreads();
-  if (warp == 0 && j < c.n) {
-    float v = smax[0][lane];
-    uint32_t a = sact[0][lane];
-#pragma unroll
-    for (int w = 1; w < 8; ++w) {
-      v = fmaxf(v, smax[w][lane]);
-      a |= sact[w][lane];
+  for (int g = blockIdx.y; g < G; g += gridDim.y) {
+    float mx = 0.f;
+    uint32_t any = 0u;
+    for (int t = warp; t < L; t += 8) {
+      const int r = g * L + t;
+      any |= __ldg(pw + r);
+      if (j < c.n) mx = fmaxf(mx, c.at(m, r, j));
     }
-    const long long o = ((long long)m * G + g) * c.n + j;
-    fmax[o] = v;
-    active[o] = (uint8_t)a;
+    smax[warp][lane] = mx;
+    sact[warp][lane] = (any >> (31 - lane)) & 1u;
+    __syncthreads();
+    if (warp == 0 && j < c.n) {
+      float v = smax[0][lane];
+      uint32_t a = sact[0][lane];
+#pragma unroll
+      for (int w = 1; w < 8; ++w) {
+        v = fmaxf(v, smax[w][lane]);
+        a |= sact[w][lane];
+      }
+      const long long o = ((long long)m * G + g) * c.n + j;
+      fmax[o] = v;
+      active[o] = (uint8_t)a;
+    }
+    __syncthreads();   // warp 0 has read smax / sact before the next fragment overwrites them
   }
 }
 
@@ -341,7 +346,8 @@ template <int SRC>
 static int launch_fragments(Launcher& launcher, const CodeView<SRC>& c, int M, int L, int G, long long frag0, float* fmax,
                             uint8_t* active, int n_top, int n_random, unsigned long long seed, float* top_val,
                             long long* top_frag, float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act) {
-  TRY(launcher.launch(fragment_max_kernel<SRC>, dim3(c.n_chunks, G, M), 256, 0, c, L, G, fmax, active));
+  TRY(launcher.launch(fragment_max_kernel<SRC>, dim3(c.n_chunks, G < kMaxGridY ? G : kMaxGridY, M), 256, 0, c, L, G,
+                      fmax, active));
   return launcher.launch(fragment_merge_kernel<SRC>, dim3((c.n + 127) / 128, M), 128, 0, c, L, G, frag0, fmax,
                          active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
 }

@@ -44,6 +44,23 @@ from oracle import tile_bounds as T
 
 Tensor = torch.Tensor
 
+ALPHA = 1.5        # the FastICA pass's tanh gain in the tests
+# the outputs a row pass adds to instead of overwriting
+ACCUMULATED = ("gram", "col_sum", "gx", "g_sum", "norms", "wtw", "wtv")
+# (tile ratio, element maximum) per pass, output and arithmetic: max(twice the worst value measured, 2^-24) rounded up,
+# set from measurement in tests/test_row_pass_tiles_gpu.py (see its docstring); "residual" is one relative error per call
+BARS = {
+    "moments": {"gram": {"bf16x3": (9.2e-6, 4.0e-5), "f16f8": (4.5e-5, 2.6e-4)},
+                "col_sum": {"bf16x3": (6.0e-8, 1.1e-7), "f16f8": (6.0e-8, 1.1e-7)}},
+    "ica": {"gx": {"bf16x3": (9.3e-7, 3.9e-6), "f16f8": (3.4e-6, 1.6e-5)},
+            "g_sum": {"bf16x3": (4.3e-7, 2.8e-6), "f16f8": (1.5e-6, 7.7e-6)}},
+    "project": {"p": {"bf16x3": (1.9e-6, 1.1e-5), "f16f8": (8.4e-6, 4.7e-5)},
+                "norms": {"bf16x3": (3.4e-7, 1.5e-6), "f16f8": (1.7e-6, 6.4e-6)}},
+    "grams": {"wtw": {"bf16x3": (5.4e-6, 2.7e-5), "f16f8": (4.2e-5, 1.9e-4)},
+              "wtv": {"bf16x3": (6.5e-6, 2.8e-5), "f16f8": (4.1e-5, 1.9e-4)}},
+    "residual": 6.0e-8,
+}
+
 
 def shifted(x: Tensor, shift: Tensor, clamp: bool = False) -> Tensor:
     """V = x - shift in fp64 (clamp: max(x - shift, 0), the NMF passes)."""

@@ -42,26 +42,19 @@ the row-norm Jacobian into FMAs differently in the instantiation for d <= 512 (o
 applied a gradient a rounding away from the one grads_batch returned. Those sums, and the centre and bias gradients,
 are now rounded explicitly, in the order the step's kernel was compiled to.
 """
-import importlib.util
-import os
-
 import pytest
 import torch
 
+import engine_cases as EC
 from oracle import adam_bounds as A
 from oracle.plan_paths import gather_classes, launch_bound, launches
 
 pytestmark = pytest.mark.gpu
 
-_spec = importlib.util.spec_from_file_location(
-    "tile_bounds_checks", os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_tile_bounds_gpu.py"))
-TB = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(TB)
-
-ARITHS = ["bf16x3", "f16f8"]
-RAGGED, RAGGED_EAGER = TB.RAGGED, TB.RAGGED_EAGER
+ARITHS = EC.ARITHS
+RAGGED, RAGGED_EAGER = EC.RAGGED, EC.RAGGED_EAGER
 TOPK = {"topk_gather": (1, (3, 8, 5, 8)), "topk_dense": (0, (16, 33, 17, 40))}   # gather launches, k per model
-SIGNATURES = TB.VARIANTS + list(TOPK)
+SIGNATURES = EC.VARIANTS + list(TOPK)
 OTHER_HYPER = {"lr": 3e-3, "betas": (0.8, 0.99), "eps": 1e-6}
 WORST = {}   # (arith, output) -> worst ratio over the passing cases
 
@@ -94,7 +87,7 @@ def make(variant, arith, shape, seed=0, optim=None, **kw):
         models = [S.TopKEncoder.init(d, n, k) for k in TOPK[variant][1]]
         return S.FunctionalEnsemble(models, S.TopKEncoder, S.adam, optim, device="cuda", arith=arith,
                                     no_stacking=True, **kw)
-    models, sig = TB.make_models(variant, M, d, n, seed)
+    models, sig = EC.make_models(variant, M, d, n, seed)
     return S.FunctionalEnsemble(models, sig, S.adam, optim, device="cuda", arith=arith, **kw)
 
 
@@ -179,7 +172,7 @@ def walk(ens, batches, per_model, tag, steps=0, launches_expected=None):
 
 def batches(shape, per_model, seed, count, fp16_values=True):
     M, d, _, B = shape
-    return [TB.batch(M, B, d, seed + s, per_model, fp16_values) for s in range(count)]
+    return [EC.batch(M, B, d, seed + s, per_model, fp16_values) for s in range(count)]
 
 
 def topk_launches(variant, shape, per_model, arith):

@@ -12,42 +12,30 @@ Tied plans run every B in {1210, 1037, 33, 5} with fp16-exact and fp32 inputs; t
 (untied: c^T g is a GEMM of its own; masked; learned centre: the decode epilogue with column sums of g; non-negative
 tied: a shifted batch) run one ragged B each.
 """
-import importlib.util
-import os
-
 import pytest
-import torch
 
+import engine_cases as EC
 from oracle.plan_paths import launch_bound
 
 pytestmark = pytest.mark.gpu
 
-_spec = importlib.util.spec_from_file_location(
-    "tile_bounds_checks", os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_tile_bounds_gpu.py"))
-TB = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(TB)
-
 M, D, N, BMAX = 4, 512, 4096, 1210
-
-
-def raw(t):
-    return t.detach().contiguous().cpu().view(torch.int32).numpy().tobytes()
 
 
 def run(variant, B, fp16_values, seed):
     assert not launch_bound(M, BMAX, N, D)
-    models, sig = TB.make_models(variant, M, D, N, seed)
-    ens = TB.ensemble(models, sig, "f16f8")
-    ens.forward_batch(TB.batch(M, BMAX, D, seed + 1, False, fp16_values))   # batch_max = BMAX; stale rows behind B
+    models, sig = EC.make_models(variant, M, D, N, seed)
+    ens = EC.ensemble(models, sig, "f16f8")
+    ens.forward_batch(EC.batch(M, BMAX, D, seed + 1, False, fp16_values))   # batch_max = BMAX; stale rows behind B
     assert ens.resolved_arith() == "f16f8"
-    X = TB.batch(M, B, D, seed + 2, False, fp16_values)
+    X = EC.batch(M, B, D, seed + 2, False, fp16_values)
     _, (_, aux) = ens.grads_batch(X)
     code_bwd = aux["c"].dense().clone()
     _, aux = ens.forward_batch(X)
     code_fwd = aux["c"].dense().clone()
     assert code_bwd.shape == (M, B, N)
-    assert raw(code_bwd) == raw(code_fwd), (variant, B, "code from the batch-major copy differs from the row-major one")
-    TB.check(f"batch-major {variant} B={B} {'fp16' if fp16_values else 'fp32'}", variant, ens, X, False, "f16f8")
+    assert EC.raw(code_bwd) == EC.raw(code_fwd), (variant, B, "code from the batch-major copy differs from the row-major one")
+    EC.check(f"batch-major {variant} B={B} {'fp16' if fp16_values else 'fp32'}", variant, ens, X, False, "f16f8")
 
 
 @pytest.mark.parametrize("inputs", ["fp16", "fp32"])

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 import sparse_coding_b200 as S
+from engine_cases import desc
 from oracle import eval_oracle as O
 from sparse_coding_b200 import _lib
 from sparse_coding_b200 import metrics as MT
@@ -97,15 +98,9 @@ def test_errors_name_the_constraint():
         MT.evaluate_dicts([_tied(64, 64)], x, segment=0)
 
 
-def _desc(M, n, d, B, variant=_lib.SCE_TIED):
-    return _lib.SceDesc(variant=variant, n_models=M, d=d, n=n, batch_max=B, x_per_model=0, lr=0.0, beta1=0.9,
-                        beta2=0.999, eps=1e-8, eps_root=0.0, adam_count_mode=0, fwd_passes=3, bwd_passes=3,
-                        norm_floor=1e-8, arith=0, topk_k_max=0, centering=0)
-
-
 def test_stats_workspace_bound():
     lib = _lib.load()
-    ws = lambda M, n, d, B, Bmax=None: lib.sce_forward_stats_workspace_bytes(C.byref(_desc(M, n, d, Bmax or B)), B)
+    ws = lambda M, n, d, B, Bmax=None: lib.sce_forward_stats_workspace_bytes(C.byref(desc(M, n, d, Bmax or B, lr=0.0)), B)
     assert ws(16, 4096, 512, 8192) == 16 * 256 * 4 * 4096 * 4 == 256 << 20          # config 2
     assert ws(1, 32768, 2048, 4096) == 128 * 4 * 32768 * 4 == 64 << 20             # config 5's width
     assert ws(2, 40, 64, 33) == 1024 * -(-(2 * 2 * 4 * 40 * 4) // 1024)

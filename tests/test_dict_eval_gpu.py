@@ -19,6 +19,7 @@ import pytest
 import torch
 
 import sparse_coding_b200 as S
+from engine_cases import DEV, as_oracle, synth
 from oracle import eval_bounds as EB
 from oracle import eval_oracle as O
 from oracle import tile_bounds as T
@@ -26,12 +27,7 @@ from sparse_coding_b200 import _lib
 from sparse_coding_b200 import metrics as MT
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
 RTOL = 1e-4
-
-
-def kink_window(z):
-    return max(1e-5, 1e-4 * float(z.double().pow(2).mean().sqrt()))
 
 
 def kink_coefficients(m, x, centred, rows=8192):
@@ -39,7 +35,7 @@ def kink_coefficients(m, x, centred, rows=8192):
     the k-th largest, where the selection may take the other side)."""
     xs = O.center(m, x) if centred else x
     z = torch.cat([O.pre_activations(m, xs[i:i + rows]) for i in range(0, x.shape[0], rows)])
-    w = kink_window(z)
+    w = T.kink_window(z)
     near = z.abs() < w
     if m["kind"] == "topk":
         near |= (z - torch.topk(z, int(m["sparsity"]), dim=-1).values[:, -1:]).abs() < w
@@ -105,7 +101,7 @@ def selection_slack(m, x, centred, segment, rows=8192):
         return None
     xs = O.center(m, x) if centred else x
     z = torch.cat([O.pre_activations(m, xs[i:i + rows]) for i in range(0, x.shape[0], rows)])
-    near = (z - torch.topk(z, int(m["sparsity"]), dim=-1).values[:, -1:]).abs() < kink_window(z)
+    near = (z - torch.topk(z, int(m["sparsity"]), dim=-1).values[:, -1:]).abs() < T.kink_window(z)
     N = x.shape[0]
     r_last = N - (-(-N // segment) - 1) * segment
     w = max(1.0, segment / r_last) / N
@@ -121,16 +117,6 @@ def to_ld(m):
     if m["kind"] == "untied":
         return S.UntiedSAE(f(m["encoder"]), f(m["decoder"]), f(m["encoder_bias"]))
     return S.TopKLearnedDict(f(m["dict"]), int(m["sparsity"]))
-
-
-def from_ld(ld):
-    g = lambda t: t.double().to(DEV)
-    if isinstance(ld, S.TopKLearnedDict):
-        return {"kind": "topk", "dict": g(ld.dict), "sparsity": int(ld.sparsity)}
-    if isinstance(ld, S.UntiedSAE):
-        return {"kind": "untied", "encoder": g(ld.encoder), "encoder_bias": g(ld.encoder_bias), "decoder": g(ld.decoder)}
-    return {"kind": "tied", "encoder": g(ld.encoder), "encoder_bias": g(ld.encoder_bias), "center_trans": g(ld.center_trans),
-            "center_rot": g(ld.center_rot), "center_scale": g(ld.center_scale)}
 
 
 def close(got, want, what, rtol=RTOL):
@@ -208,7 +194,7 @@ def score_against_oracle(lds, x, segment=1000, threshold=10, arith="auto"):
     res = MT.evaluate_dicts(lds, x, segment=segment, threshold=threshold, arith=arith)
     xd = x.double()
     for i, (ld, r) in enumerate(zip(lds, res)):
-        m = from_ld(ld)
+        m = as_oracle(ld)
         fb = feature_bounds(m, xd, True, segment, "bf16x3" if arith == "auto" else arith)
         kink = int(fb["kink"].sum())
         close(r["fvu"], O.fraction_variance_unexplained(m, xd), (i, "fvu"))
@@ -222,20 +208,11 @@ def score_against_oracle(lds, x, segment=1000, threshold=10, arith="auto"):
     return res
 
 
-def synth(N, d, seed, half=True):
-    gen = torch.Generator(device=DEV).manual_seed(seed)
-    feats = torch.randn(2048, d, generator=gen, device=DEV)
-    feats /= feats.norm(dim=-1, keepdim=True)
-    code = (torch.rand(N, 2048, generator=gen, device=DEV) < 0.01) * torch.rand(N, 2048, generator=gen, device=DEV)
-    x = code @ feats + 0.05 * torch.randn(N, d, generator=gen, device=DEV)
-    return x.half() if half else x
-
-
 def test_config2_fresh_and_trained():
     torch.manual_seed(0)
     models = [S.FunctionalTiedSAE.init(512, 4096, a) for a in torch.logspace(-4, -2, 16).tolist()]
     ens = S.FunctionalEnsemble(models, S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device=DEV)
-    x = synth(65536 + 500, 512, 1)                                   # fp16 chunk format, partial last segment
+    x = synth(65536 + 500, 512, 1).half()                            # fp16 chunk format, partial last segment
     for steps in (0, 30):
         for s in range(steps):
             ens.step_batch(x[s * 2048:(s + 1) * 2048].float())
@@ -246,7 +223,7 @@ def test_config2_fresh_and_trained():
 def test_config5_width():
     torch.manual_seed(2)
     ld = S.TiedSAE(torch.randn(32768, 2048, device=DEV), torch.randn(32768, device=DEV) * 0.1 - 0.3)
-    score_against_oracle([ld], synth(10000, 2048, 3))
+    score_against_oracle([ld], synth(10000, 2048, 3).half())
 
 
 def test_config3_topk_shapes():
@@ -254,7 +231,7 @@ def test_config3_topk_shapes():
     lds = [S.TopKEncoder.to_learned_dict(*S.TopKEncoder.init(768, n, k)) for n in (3072, 6144, 12288) for k in (16, 32, 64)]
     for ld in lds:
         ld.to_device(DEV)
-    score_against_oracle(lds, synth(8192 + 300, 768, 5))
+    score_against_oracle(lds, synth(8192 + 300, 768, 5).half())
 
 
 def test_centred_tied_with_nonuniform_scale_and_host_input():
@@ -263,7 +240,7 @@ def test_centred_tied_with_nonuniform_scale_and_host_input():
     cen = (torch.randn(d, device=DEV) * 0.1, torch.eye(d, device=DEV) + 0.05 * torch.randn(d, d, device=DEV) / d ** 0.5,
            torch.rand(d, device=DEV) * 1.5 + 0.5)
     ld = S.TiedSAE(torch.randn(2048, d, device=DEV), torch.randn(2048, device=DEV) * 0.05 - 0.1, centering=cen)
-    x = synth(20000, d, 7, half=False).cpu()                          # host input: streamed
+    x = synth(20000, d, 7, False).cpu()                               # host input: streamed
     res = score_against_oracle([ld, S.TiedSAE(ld.encoder, ld.encoder_bias)], x.to(DEV))
     host = MT.evaluate_dicts([ld], x)
     assert host[0]["fvu"].device.type == "cpu"
@@ -273,8 +250,8 @@ def test_centred_tied_with_nonuniform_scale_and_host_input():
 def test_segment_longer_than_an_engine_call():
     torch.manual_seed(8)
     ld = S.TiedSAE(torch.randn(1024, 256, device=DEV), torch.randn(1024, device=DEV) * 0.1 - 0.45)
-    x = synth(50000, 256, 9)
-    m, xd = from_ld(ld), x.double()
+    x = synth(50000, 256, 9).half()
+    m, xd = as_oracle(ld), x.double()
     for bs in (20000, 8193, 1000, 1):
         got = MT.calc_moments_streaming(ld, x, batch_size=bs)
         fb = feature_bounds(m, xd, False, bs)
@@ -294,7 +271,7 @@ def test_exported_dicts_agree_bitwise_with_evaluate_batches(sig):
     else:
         S_, models = S.FunctionalMaskedSAE, [S.FunctionalMaskedSAE.init(256, k, 1024, 1e-3) for k in (1024, 300, 777)]
     ens = S.FunctionalEnsemble(models, S_, S.adam, {"lr": 1e-3}, device=DEV, arith="bf16x3")
-    x = synth(24000, 256, 11, half=False)
+    x = synth(24000, 256, 11, False)
     for s in range(10):
         ens.step_batch(x[s * 2000:(s + 1) * 2000])
     batches = [x[i:i + 8000] for i in range(0, 24000, 8000)]
@@ -310,7 +287,7 @@ def test_repeated_calls_are_bitwise_equal():
     torch.manual_seed(12)
     lds = [S.TiedSAE(torch.randn(1000, 256, device=DEV), torch.zeros(1000, device=DEV)),
            S.TopKLearnedDict(torch.nn.functional.normalize(torch.randn(512, 256, device=DEV), dim=-1), 16)]
-    x = synth(30000, 256, 13)
+    x = synth(30000, 256, 13).half()
     a, b = MT.evaluate_dicts(lds, x), MT.evaluate_dicts(lds, x)
     for ra, rb in zip(a, b):
         for k, v in ra.items():
@@ -324,7 +301,7 @@ def test_out_of_fp16_range():
     assert x.abs().max() > 65504
     r = MT.evaluate_dicts([ld], x)[0]
     assert all(torch.isfinite(r[k]).all() for k in ("fvu", "mean", "m2", "m4"))
-    close(r["fvu"], O.fraction_variance_unexplained(from_ld(ld), x.double()), "fvu")
+    close(r["fvu"], O.fraction_variance_unexplained(as_oracle(ld), x.double()), "fvu")
     with pytest.raises(ValueError, match="fp16"):
         MT.evaluate_dicts([ld], x, arith="f16f8")
 

@@ -18,18 +18,14 @@ import subprocess
 import pytest
 import torch
 
+from engine_cases import clone_models, relnorm
 from oracle import sae_oracle as O
+from oracle.tile_bounds import kink_window
 
 pytestmark = pytest.mark.gpu
 
 REL = 1e-4
 ARITHS = ["bf16x3", "f16f8"]
-
-
-def kink_window(Z):
-    """|z| below which the engine and the fp64 oracle may disagree about [z > 0]: ~5 sigma of the engine's error on z
-    (2e-5 relative to rms(z) in the f16f8 arithmetic, 4e-6 in bf16x3), never below the 1e-5 the suite always used."""
-    return max(1e-5, 1e-4 * float(Z.double().pow(2).mean().sqrt()))
 
 
 def tied_grads_engine_kinks(p, b, X, code, mask=None):
@@ -43,11 +39,6 @@ def tied_grads_engine_kinks(p, b, X, code, mask=None):
     f0 = O.tied_forward(pd["encoder"], pd["encoder_bias"], Xd, float(b["l1_alpha"]), bd, mask)
     active = torch.where(f0["Z"].abs() < kink_window(f0["Z"]), code.cpu() > 0, f0["Z"] > 0)
     return O.tied_grads(pd["encoder"], pd["encoder_bias"], Xd, float(b["l1_alpha"]), bd, mask, active=active), f0
-
-
-def relnorm(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
 
 
 def _sigs():
@@ -149,8 +140,7 @@ def test_device_side_centring(arith, per_model):
                                         rotation=q.contiguous(), scaling=0.5 + torch.rand(d, generator=gen))
         p["encoder_bias"] = 0.05 * torch.randn(n, generator=gen)
         models.append((p, b))
-    clone = lambda ms: [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-    ens = S.FunctionalEnsemble(clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith=arith)
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith=arith)
     X = torch.randn(M, B, d, generator=gen) if per_model else torch.randn(B, d, generator=gen)
     kw = dict(expand_dims=not per_model)
     grads, (loss, aux) = ens.grads_batch(X.cuda(), **kw)
@@ -163,7 +153,7 @@ def test_device_side_centring(arith, per_model):
         assert abs(float(loss["loss"][i]) - float(f0["loss"])) <= REL * float(f0["loss"])
         for k in ("encoder", "encoder_bias"):
             assert relnorm(grads[k][i], f["grads"][k]) <= 2e-4, (i, k, relnorm(grads[k][i], f["grads"][k]))
-    ref = O.RefPortEnsemble(clone(models), O.SIG_LOSSES["tied"], lr=1e-3)
+    ref = O.RefPortEnsemble(clone_models(models), O.SIG_LOSSES["tied"], lr=1e-3)
     for _ in range(3):
         le, _ = ens.step_batch(X.cuda(), **kw)
         lr_, _ = ref.step_batch(X, **kw)
@@ -320,10 +310,9 @@ def test_training_trajectory_matches_oracle(kind, mode, arith):
     for a in (1e-4, 1e-3, 1e-2):
         p, b = sig.init(d, n, a) if kind == "tied" else sig.init(d, n, a, bias_decay=0.01)
         models.append((p, b))
-    clone = lambda ms: [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-    ens = S.FunctionalEnsemble(clone(models), sig, S.adam, {"lr": 1e-3}, device="cuda", adam_count_mode=mode,
+    ens = S.FunctionalEnsemble(clone_models(models), sig, S.adam, {"lr": 1e-3}, device="cuda", adam_count_mode=mode,
                                arith=arith)
-    ref = O.RefPortEnsemble(clone(models), O.SIG_LOSSES[kind], lr=1e-3, count_mode=mode)
+    ref = O.RefPortEnsemble(clone_models(models), O.SIG_LOSSES[kind], lr=1e-3, count_mode=mode)
     gen = torch.Generator().manual_seed(2)
     feats = torch.randn(512, d, generator=gen)
     feats /= feats.norm(dim=-1, keepdim=True)
@@ -346,9 +335,8 @@ def test_topk_trajectory_matches_oracle():
     torch.manual_seed(3)
     d, n, B = 64, 256, 128
     models = [S.TopKEncoder.init(d, n, k) for k in (4, 8, 16)]
-    clone = lambda ms: [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-    ens = S.FunctionalEnsemble(clone(models), S.TopKEncoder, S.adam, {"lr": 1e-3}, device="cuda", no_stacking=True)
-    ref = O.RefPortEnsemble(clone(models), O.SIG_LOSSES["topk"], lr=1e-3, no_stacking=True)
+    ens = S.FunctionalEnsemble(clone_models(models), S.TopKEncoder, S.adam, {"lr": 1e-3}, device="cuda", no_stacking=True)
+    ref = O.RefPortEnsemble(clone_models(models), O.SIG_LOSSES["topk"], lr=1e-3, no_stacking=True)
     gen = torch.Generator().manual_seed(4)
     for step in range(10):
         X = torch.randn(B, d, generator=gen)
@@ -470,8 +458,7 @@ def test_wide_activation_widths_backward(kind, d, n, B):
         sig = S.FunctionalSAE
     for p, _b in models:
         p["encoder_bias"] = 0.05 * torch.randn(n, generator=gen)
-    clone = lambda ms: [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-    ens = S.FunctionalEnsemble(clone(models), sig, S.adam, {"lr": 1e-3}, device="cuda")
+    ens = S.FunctionalEnsemble(clone_models(models), sig, S.adam, {"lr": 1e-3}, device="cuda")
     X = torch.randn(B, d, generator=gen)
     grads, (loss, aux) = ens.grads_batch(X.cuda())
     code = aux["c"].dense().cpu()
@@ -489,7 +476,7 @@ def test_wide_activation_widths_backward(kind, d, n, B):
     assert abs(float(loss["loss"][0]) - float(f0["loss"])) <= REL * float(f0["loss"])
     for k, g in f["grads"].items():
         assert relnorm(grads[k][0], g) <= 2e-4, (kind, k, relnorm(grads[k][0], g))
-    ref = O.RefPortEnsemble(clone(models), O.SIG_LOSSES[kind], lr=1e-3)
+    ref = O.RefPortEnsemble(clone_models(models), O.SIG_LOSSES[kind], lr=1e-3)
     for _ in range(3):
         le, _ = ens.step_batch(X.cuda())
         lr_, _ = ref.step_batch(X)
@@ -509,10 +496,9 @@ def test_fvu_and_l0_match_reference_after_training(bwd_passes):
     torch.manual_seed(0)
     d, n, B = 64, 256, 512
     models = [S.FunctionalTiedSAE.init(d, n, a) for a in (3e-4, 1e-3, 3e-3)]
-    clone = lambda ms: [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-    ens = S.FunctionalEnsemble(clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda",
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda",
                                bwd_passes=bwd_passes)
-    ref = O.RefPortEnsemble(clone(models), O.SIG_LOSSES["tied"], lr=1e-3)
+    ref = O.RefPortEnsemble(clone_models(models), O.SIG_LOSSES["tied"], lr=1e-3)
     gen = torch.Generator().manual_seed(1)
     feats = torch.randn(384, d, generator=gen)
     feats /= feats.norm(dim=-1, keepdim=True)
@@ -655,10 +641,9 @@ def test_bitwise_determinism(kind):
         models, sig = [S.TopKEncoder.init(d, n, k) for k in (8, 24)], S.TopKEncoder
     gen = torch.Generator().manual_seed(1)
     batches = [torch.randn(B, d, generator=gen).cuda() for _ in range(6)]
-    clone = lambda ms: [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
     runs = []
     for _ in range(2):
-        ens = S.FunctionalEnsemble(clone(models), sig, S.adam, {"lr": 1e-3}, device="cuda")
+        ens = S.FunctionalEnsemble(clone_models(models), sig, S.adam, {"lr": 1e-3}, device="cuda")
         losses = [ens.step_batch(x)[0]["loss"].clone() for x in batches]
         runs.append((ens.params, ens.optim_states, losses))
     for k in runs[0][0]:

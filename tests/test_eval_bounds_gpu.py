@@ -68,7 +68,7 @@ import ctypes as C
 import pytest
 import torch
 
-import sparse_coding_b200 as S
+from engine_cases import ARITHS, DEV, as_oracle, one_key, synth, tied, topk, untied
 from oracle import eval_bounds as EB
 from oracle import eval_oracle as EO
 from oracle import tile_bounds as T
@@ -77,8 +77,6 @@ from sparse_coding_b200 import _lib
 from sparse_coding_b200 import metrics as MT
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-ARITHS = ["bf16x3", "f16f8"]
 GUARD = 256                           # sentinel entries past the end of every output
 SIZES = (4001, 33, 1, 31, 129, 2048)  # the call sequence
 # (tile, element) bars of x_hat where this file's cases leave the regime the training-step bars were measured in (see
@@ -89,53 +87,6 @@ CENTRED_X_HAT_ELEM = {"bf16x3": 3.2e-7, "f16f8": 1.9e-6}
 # which a single f16f8 pass stays under once summed over many rows, so there the moment check is no evidence against a
 # single-pass encode; only the per-tile code check (tile_bounds.SEPARATED) is
 MOMENTS_SEPARATED = ("bf16x3",)
-
-
-def synth(B, d, seed, fp16_values=True, n_feats=2048):
-    """Sparse-mixture activations, generated on the device (as tests/test_tile_bounds_gpu.py)."""
-    gen = torch.Generator(device=DEV).manual_seed(seed)
-    feats = torch.randn(n_feats, d, generator=gen, device=DEV)
-    feats /= feats.norm(dim=-1, keepdim=True)
-    codes = (torch.rand(B, n_feats, generator=gen, device=DEV) < 0.01).float() * \
-        torch.rand(B, n_feats, generator=gen, device=DEV)
-    x = codes @ feats + 0.05 * torch.randn(B, d, generator=gen, device=DEV)
-    return x.half().float() if fp16_values else x
-
-
-def tied(n, d, seed, centering=(None, None, None)):
-    """A TiedSAE whose biases leave some features active on most rows, most on few, some positive on an all-zero row."""
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    return S.TiedSAE(torch.randn(n, d, generator=g, device=DEV), 0.05 * torch.randn(n, generator=g, device=DEV) - 0.03,
-                     centering=centering)
-
-
-def untied(n, d, seed):
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    enc = torch.randn(n, d, generator=g, device=DEV) / d ** 0.5
-    return S.UntiedSAE(enc, torch.randn(n, d, generator=g, device=DEV), 0.05 * torch.randn(n, generator=g, device=DEV) - 0.03)
-
-
-def topk(n, d, k, seed):
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    return S.TopKLearnedDict(torch.nn.functional.normalize(torch.randn(n, d, generator=g, device=DEV), dim=-1), k)
-
-
-def one_key(lds, arith, centre=False):
-    """The key evaluate_dicts groups ``lds`` under (the dictionaries must share one)."""
-    groups = MT._eval_groups(lds, centre, 16 if arith == "f16f8" else 8)
-    assert len(groups) == 1, groups
-    return next(iter(groups))
-
-
-def as_oracle(ld):
-    """A dictionary of oracle/eval_oracle.py (fp64) from a LearnedDict."""
-    g = lambda t: t.double().to(DEV)
-    if isinstance(ld, S.TopKLearnedDict):
-        return {"kind": "topk", "dict": g(ld.dict), "sparsity": int(ld.sparsity)}
-    if isinstance(ld, S.UntiedSAE):
-        return {"kind": "untied", "encoder": g(ld.encoder), "encoder_bias": g(ld.encoder_bias), "decoder": g(ld.decoder)}
-    return {"kind": "tied", "encoder": g(ld.encoder), "encoder_bias": g(ld.encoder_bias),
-            "center_trans": g(ld.center_trans), "center_rot": g(ld.center_rot), "center_scale": g(ld.center_scale)}
 
 
 class Harness:

@@ -6,20 +6,12 @@ import warnings
 import pytest
 import torch
 
+from engine_cases import clone_models, relnorm
 from oracle import sae_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 REL = 1e-4
-
-
-def relnorm(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
-
-
-def _clone(ms):
-    return [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
 
 
 def _tied(M, d, n, seed=0):
@@ -33,7 +25,7 @@ def test_out_of_range_batch_never_poisons_the_parameters():
     device — parameters, Adam moments bit-identical to before — and step_batch raises at its health check."""
     import sparse_coding_b200 as S
     models = _tied(2, 64, 128)
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith="f16f8",
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith="f16f8",
                                health_check_every=4)
     gen = torch.Generator().manual_seed(1)
     good = torch.randn(96, 64, generator=gen)
@@ -63,8 +55,8 @@ def test_auto_plan_falls_back_to_bf16x3_and_retakes_the_step():
     gen = torch.Generator().manual_seed(2)
     X = 300.0 * torch.randn(128, 64, generator=gen)
     X[5, 9] = 9.0e4
-    auto = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
-    ref = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith="bf16x3")
+    auto = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ref = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith="bf16x3")
     with warnings.catch_warnings(record=True) as w:
         warnings.simplefilter("always")
         la, _ = auto.step_batch(X.cuda())
@@ -82,7 +74,7 @@ def test_auto_plan_falls_back_to_bf16x3_and_retakes_the_step():
 def test_nonfinite_loss_is_caught_in_bf16x3_too():
     import sparse_coding_b200 as S
     models = _tied(1, 32, 64)
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith="bf16x3")
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda", arith="bf16x3")
     X = torch.randn(64, 32)
     X[0, 0] = float("nan")
     snap = ens.params["encoder"].clone()
@@ -107,7 +99,7 @@ def test_lm_residual_outlier_dimensions(d, n):
     X[:, d - 5] *= 100.0
     X[:, 200] += 40.0                              # a dimension with a large mean, as massive activations have
     X = X.half().float()
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
     assert_arith = ens.resolved_arith()
     grads, (loss, aux) = ens.grads_batch(X.cuda())
     code = aux["c"].dense()
@@ -205,8 +197,8 @@ def test_host_batch_prefetcher_feeds_identical_steps():
     models = _tied(2, 64, 128, seed=5)
     gen = torch.Generator().manual_seed(6)
     host = [torch.randn(200 if i != 4 else 77, 64, generator=gen).pin_memory() for i in range(7)]
-    a = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
-    b = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    a = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    b = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
     la = [a.step_batch(x.cuda())[0]["loss"].cpu() for x in host]
     lb = [b.step_batch(x)[0]["loss"].cpu() for x in HostBatchPrefetcher(host, "cuda")]
     assert len(lb) == 7 and all(torch.equal(p, q) for p, q in zip(la, lb))

@@ -64,7 +64,7 @@ case; the 2^16-fragment one needs the strided grid. The file runs in about 17 s.
 import pytest
 import torch
 
-import test_eval_bounds_gpu as EV
+import engine_cases as EC
 from oracle import eval_bounds as EB
 from oracle import eval_oracle as EO
 from oracle import interp_oracle as IO
@@ -74,8 +74,8 @@ from sparse_coding_b200 import _lib
 from sparse_coding_b200 import metrics as MT
 
 pytestmark = pytest.mark.gpu
-DEV = EV.DEV
-ARITHS = EV.ARITHS
+DEV = EC.DEV
+ARITHS = EC.ARITHS
 GUARD = 256
 SENTINEL = -7.25
 SEED = (1 << 63) + 977
@@ -109,7 +109,7 @@ class Harness:
         self.nact0 = self.view("n_active").clone()
         self.sizes = [int(ld.n_feats) for ld in lds]
         self.pad = torch.arange(n, device=DEV)[None, :] >= torch.tensor(self.sizes, device=DEV)[:, None]
-        self.oracles = [EV.as_oracle(ld) for ld in lds]
+        self.oracles = [EC.as_oracle(ld) for ld in lds]
         f32 = lambda k, L_=None: IO.empty_lists(n, k, L_, key_dtype=torch.float32, row_dtype=torch.float32, device=DEV)
         i64 = lambda k, L_=None: IO.empty_lists(n, k, L_, key_dtype=torch.int64, row_dtype=torch.float32, device=DEV)
         self.ref_top = [f32(n_top, L) for _ in range(M)]
@@ -301,12 +301,12 @@ LISTS = {"64x64": (64, 64), "20x20": (20, 20), "1x0": (1, 0), "0x64": (0, 64)}
 @pytest.mark.parametrize("lists", list(LISTS))
 def test_call_sequence_on_one_plan(lists, arith, inputs):
     d, L = 400, 96
-    lds = [EV.tied(1000, d, s) for s in range(3)]
-    key = EV.one_key(lds, arith)
+    lds = [EC.tied(1000, d, s) for s in range(3)]
+    key = EC.one_key(lds, arith)
     assert key[1] == (1008 if arith == "f16f8" else 1000)
     frags = (1, 43, 2, 5, 3)
     frag0s = (0, 1, 44, 60, (1 << 32) + 11)
-    xs = [EV.synth(k * L, d, 10 + i, inputs == "fp16") for i, k in enumerate(frags)]
+    xs = [EC.synth(k * L, d, 10 + i, inputs == "fp16") for i, k in enumerate(frags)]
     h = Harness(key, lds, max(frags) * L, L, *LISTS[lists], arith)
     try:
         run(h, xs, frag0s, f"sequence {lists} {inputs}")
@@ -317,10 +317,10 @@ def test_call_sequence_on_one_plan(lists, arith, inputs):
 @pytest.mark.parametrize("arith", ARITHS)
 def test_untied(arith):
     d, L = 256, 64
-    lds = [EV.untied(512, d, s) for s in (1, 2)]
-    h = Harness(EV.one_key(lds, arith), lds, 40 * L, L, 20, 20, arith)
+    lds = [EC.untied(512, d, s) for s in (1, 2)]
+    h = Harness(EC.one_key(lds, arith), lds, 40 * L, L, 20, 20, arith)
     try:
-        run(h, [EV.synth(40 * L, d, 20, False), EV.synth(7 * L, d, 21, False)], (0, 40), "untied")
+        run(h, [EC.synth(40 * L, d, 20, False), EC.synth(7 * L, d, 21, False)], (0, 40), "untied")
     finally:
         h.close()
 
@@ -328,10 +328,10 @@ def test_untied(arith):
 @pytest.mark.parametrize("arith", ARITHS)
 def test_masked_padding(arith):
     d, L = 256, 64
-    lds = [EV.tied(k, d, k) for k in (1000, 777, 1024)]
+    lds = [EC.tied(k, d, k) for k in (1000, 777, 1024)]
     h = Harness(("tied", 1024, d, False), lds, 30 * L, L, 20, 20, arith)
     try:
-        run(h, [EV.synth(30 * L, d, 22, False), EV.synth(3 * L, d, 23, False)], (0, 30), "masked")
+        run(h, [EC.synth(30 * L, d, 22, False), EC.synth(3 * L, d, 23, False)], (0, 30), "masked")
     finally:
         h.close()
 
@@ -347,11 +347,11 @@ def test_topk(path, arith, inputs):
     classes = gather_classes(d, n, ks)
     assert (classes > 0) == (path == "gather")
     L = 64
-    lds = [EV.topk(n, d, k, 40 + k) for k in ks]
-    h = Harness(EV.one_key(lds, arith), lds, 40 * L, L, 20, 20, arith)
+    lds = [EC.topk(n, d, k, 40 + k) for k in ks]
+    h = Harness(EC.one_key(lds, arith), lds, 40 * L, L, 20, 20, arith)
     try:
         for i, (k, f0) in enumerate(((40, 0), (3, 40))):
-            h.call(EV.synth(k * L, d, 41 + i, inputs == "fp16"), f0, zero_ws_too=(i == 0), tag=f"topk {path} call {i}")
+            h.call(EC.synth(k * L, d, 41 + i, inputs == "fp16"), f0, zero_ws_too=(i == 0), tag=f"topk {path} call {i}")
             assert h.launches == launches("forward", classes, 1, arith), (h.launches, classes)
         h.finish(f"topk {path} {inputs}")
     finally:
@@ -362,11 +362,11 @@ def test_topk(path, arith, inputs):
 @pytest.mark.parametrize("L", [32, 8192])
 def test_fragment_lengths(L, arith):
     d = 256
-    lds = [EV.tied(512, d, 80 + s) for s in range(2)]
+    lds = [EC.tied(512, d, 80 + s) for s in range(2)]
     G = 50 if L == 32 else 2
-    h = Harness(EV.one_key(lds, arith), lds, G * L, L, 3 if L == 8192 else 20, 3 if L == 8192 else 20, arith)
+    h = Harness(EC.one_key(lds, arith), lds, G * L, L, 3 if L == 8192 else 20, 3 if L == 8192 else 20, arith)
     try:
-        run(h, [EV.synth(G * L, d, 81, False), EV.synth(G * L, d, 82, False)], (0, G), f"L {L}")
+        run(h, [EC.synth(G * L, d, 81, False), EC.synth(G * L, d, 82, False)], (0, G), f"L {L}")
     finally:
         h.close()
 
@@ -376,14 +376,14 @@ def test_planted_ties_and_dead_features(arith):
     """Fragments copied bitwise (rows aligned to the GEMM's 128-row tiles): within call 0, 5 <- 1 and 7 <- 3; across
     calls, fragment 0 of call 1 (id 12) <- 2. Features 0, 9 and 500 are dead (bias -100)."""
     d, L = 256, 128
-    lds = [EV.tied(512, d, 90 + s) for s in range(2)]
+    lds = [EC.tied(512, d, 90 + s) for s in range(2)]
     dead = (0, 9, 500)
     for ld in lds:
         ld.encoder_bias[list(dead)] = -100.0
-    x0, x1 = EV.synth(12 * L, d, 91, False), EV.synth(4 * L, d, 92, False)
+    x0, x1 = EC.synth(12 * L, d, 91, False), EC.synth(4 * L, d, 92, False)
     x0[5 * L:6 * L], x0[7 * L:8 * L], x1[:L] = x0[L:2 * L], x0[3 * L:4 * L], x0[2 * L:3 * L]
     ties = ((1, 5), (3, 7), (2, 12))
-    h = Harness(EV.one_key(lds, arith), lds, 12 * L, L, 4, 4, arith)
+    h = Harness(EC.one_key(lds, arith), lds, 12 * L, L, 4, 4, arith)
     try:
         h.call(x0, 0, zero_ws_too=True, tag="ties call 0")
         c0 = torch.empty(h.M, 12 * L, h.n, device=DEV)
@@ -404,30 +404,30 @@ def test_planted_ties_and_dead_features(arith):
 @pytest.mark.parametrize("arith", ARITHS)
 def test_config2(arith):
     d, L = 512, 64
-    lds = [EV.tied(4096, d, 50 + m) for m in range(16)]
-    h = Harness(EV.one_key(lds, arith), lds, 8192, L, 20, 20, arith)
+    lds = [EC.tied(4096, d, 50 + m) for m in range(16)]
+    h = Harness(EC.one_key(lds, arith), lds, 8192, L, 20, 20, arith)
     try:
-        run(h, [EV.synth(8192, d, 51)], (0,), "cfg2")
+        run(h, [EC.synth(8192, d, 51)], (0,), "cfg2")
     finally:
         h.close()
 
 
 def test_config5_width():
     d, L = 2048, 64
-    lds = [EV.tied(32768, d, 60)]
-    h = Harness(EV.one_key(lds, "f16f8"), lds, 4096, L, 8, 8, "f16f8")
+    lds = [EC.tied(32768, d, 60)]
+    h = Harness(EC.one_key(lds, "f16f8"), lds, 4096, L, 8, 8, "f16f8")
     try:
-        run(h, [EV.synth(4096, d, 61, n_feats=4096)], (0,), "cfg5")
+        run(h, [EC.synth(4096, d, 61, n_feats=4096)], (0,), "cfg5")
     finally:
         h.close()
 
 
 def test_config3_topk_shape():
     d, L = 768, 64
-    lds = [EV.topk(3072, d, 16, 70)]
-    h = Harness(EV.one_key(lds, "bf16x3"), lds, 4096, L, 20, 20, "bf16x3")
+    lds = [EC.topk(3072, d, 16, 70)]
+    h = Harness(EC.one_key(lds, "bf16x3"), lds, 4096, L, 20, 20, "bf16x3")
     try:
-        run(h, [EV.synth(4096, d, 71, False)], (0,), "cfg3 topk")
+        run(h, [EC.synth(4096, d, 71, False)], (0,), "cfg3 topk")
     finally:
         h.close()
 
@@ -438,9 +438,9 @@ def test_more_fragments_than_grid_y_holds():
     measured on the training-step shapes, and at 2^27 code elements of a 64-term dot product its tail does not hold
     (one row value at 1.02 of its bound on fp32 inputs, 1.07 on fp16-exact inputs)."""
     d, L, B = 64, 32, 1 << 21
-    lds = [EV.tied(64, d, 99)]
-    h = Harness(EV.one_key(lds, "bf16x3"), lds, B, L, 64, 64, "bf16x3", fp64_bars=False)
+    lds = [EC.tied(64, d, 99)]
+    h = Harness(EC.one_key(lds, "bf16x3"), lds, B, L, 64, 64, "bf16x3", fp64_bars=False)
     try:
-        run(h, [EV.synth(B, d, 98, False, n_feats=256)], (0,), "G 65536")
+        run(h, [EC.synth(B, d, 98, False, n_feats=256)], (0,), "G 65536")
     finally:
         h.close()

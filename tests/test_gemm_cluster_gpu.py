@@ -16,19 +16,14 @@ both are done with it; none of that may change a value. These tests check it:
   odd    M = 2, d = 128, n = 640,  B = 2048   one column tile of d: singles throughout
   mixed  M = 3, d = 256, n = 640,  B = 2049   decode singles (K = 640), weight gradient pairs (2 x 2049)
 """
-import importlib.util
 import os
 import subprocess
 
 import pytest
-import torch
+
+import engine_cases as EC
 
 pytestmark = pytest.mark.gpu
-
-_spec = importlib.util.spec_from_file_location(
-    "tile_bounds_checks", os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_tile_bounds_gpu.py"))
-TB = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(TB)
 
 SHAPES = {"even": (2, 256, 4096, 2048), "odd": (2, 128, 640, 2048), "mixed": (3, 256, 640, 2049)}
 
@@ -61,41 +56,19 @@ def test_gemm_cluster_selftest(tmp_path):
     assert r.stdout.count("cluster sizes 1, 1, 2, 2") >= 20 and r.stdout.count("cluster sizes 1, 1 ") >= 12
 
 
-@pytest.mark.parametrize("arith", TB.ARITHS)
+@pytest.mark.parametrize("arith", EC.ARITHS)
 @pytest.mark.parametrize("case", sorted(SHAPES))
 def test_every_tile_against_fp64(case, arith):
     shp = SHAPES[case]
     M, d, n, _ = shp
-    models, sig = TB.make_models("tied", M, d, n, 21)
-    TB.run_case(f"cluster {case}", "tied", models, sig, arith, shp, False, True, steps=1, seed=710)
+    models, sig = EC.make_models("tied", M, d, n, 21)
+    EC.run_case(f"cluster {case}", "tied", models, sig, arith, shp, False, True, steps=1, seed=710)
 
 
-def raw(t):
-    t = t.detach().cpu()
-    return (t.view(torch.int16) if t.dtype == torch.bfloat16 else t).numpy().tobytes()
-
-
-def _run(models, sig, arith, shp, steps):
-    M, d, _, B = shp
-    ens = TB.ensemble(models, sig, arith)
-    out = []
-    for s in range(steps):
-        loss, aux = ens.step_batch(TB.batch(M, B, d, 910 + s, False, True))
-        out += [v.clone() for _, v in sorted(loss.items())] + [aux["c"].dense().clone()]
-    grads, _ = ens.grads_batch(TB.batch(M, B, d, 995, False, True))
-    out += [v.clone() for _, v in sorted(grads.items())] + [v.clone() for _, v in sorted(ens.params.items())]
-    return out
-
-
-@pytest.mark.parametrize("arith", TB.ARITHS)
+@pytest.mark.parametrize("arith", EC.ARITHS)
 @pytest.mark.parametrize("case", sorted(SHAPES))
 def test_two_runs_bitwise_equal(case, arith):
     shp = SHAPES[case]
     M, d, n, _ = shp
-    models, sig = TB.make_models("tied", M, d, n, 22)
-    a = _run(models, sig, arith, shp, 2)
-    b = _run(models, sig, arith, shp, 2)
-    assert len(a) == len(b)
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert x.shape == y.shape and x.dtype == y.dtype, i
-        assert raw(x) == raw(y), (case, arith, i)
+    models, sig = EC.make_models("tied", M, d, n, 22)
+    EC.bitwise_reruns(models, sig, arith, shp, (910, 995))

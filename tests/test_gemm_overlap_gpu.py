@@ -17,18 +17,12 @@ Each is checked against fp64 per (model, 128 x 128 tile) with the bars of tests/
 (oracle/tile_bounds.py), at initialisation and after a step, in both arithmetics; and two runs of the same steps on
 fresh ensembles must return bitwise equal tensors, since the hand-off changes when an epilogue runs, never what it sums.
 """
-import importlib.util
-import os
-
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+import engine_cases as EC
 
-_spec = importlib.util.spec_from_file_location(
-    "tile_bounds_checks", os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_tile_bounds_gpu.py"))
-TB = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(TB)
+pytestmark = pytest.mark.gpu
 
 D = 256
 CASES = ["fewer", "one_each", "one_more", "many"]
@@ -59,42 +53,20 @@ def test_tile_counts_around_the_sm_count():
     assert tiles["many"] > 4 * sms, tiles
 
 
-@pytest.mark.parametrize("arith", TB.ARITHS)
+@pytest.mark.parametrize("arith", EC.ARITHS)
 @pytest.mark.parametrize("case", CASES)
 def test_every_tile_against_fp64(case, arith):
     shp = shape(case)
     M, d, n, _ = shp
-    models, sig = TB.make_models("tied", M, d, n, 11)
-    TB.run_case(f"overlap {case}", "tied", models, sig, arith, shp, False, True, steps=1, seed=700)
+    models, sig = EC.make_models("tied", M, d, n, 11)
+    EC.run_case(f"overlap {case}", "tied", models, sig, arith, shp, False, True, steps=1, seed=700)
 
 
-def raw(t):
-    t = t.detach().cpu()
-    return (t.view(torch.int16) if t.dtype == torch.bfloat16 else t).numpy().tobytes()
-
-
-def _run(models, sig, arith, shp, steps):
-    M, d, _, B = shp
-    ens = TB.ensemble(models, sig, arith)
-    out = []
-    for s in range(steps):
-        loss, aux = ens.step_batch(TB.batch(M, B, d, 900 + s, False, True))
-        out += [v.clone() for _, v in sorted(loss.items())] + [aux["c"].dense().clone()]
-    grads, (loss, aux) = ens.grads_batch(TB.batch(M, B, d, 990, False, True))
-    out += [v.clone() for _, v in sorted(grads.items())] + [v.clone() for _, v in sorted(ens.params.items())]
-    return out, ens.gpu_launches_last_call()
-
-
-@pytest.mark.parametrize("arith", TB.ARITHS)
+@pytest.mark.parametrize("arith", EC.ARITHS)
 @pytest.mark.parametrize("case", CASES)
 def test_two_runs_bitwise_equal(case, arith):
     shp = shape(case)
     M, d, n, _ = shp
-    models, sig = TB.make_models("tied", M, d, n, 12)
-    a, la = _run(models, sig, arith, shp, 2)
-    b, lb = _run(models, sig, arith, shp, 2)
+    models, sig = EC.make_models("tied", M, d, n, 12)
+    la, lb = EC.bitwise_reruns(models, sig, arith, shp, (900, 990))
     assert la == lb
-    assert len(a) == len(b)
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert x.shape == y.shape and x.dtype == y.dtype, i
-        assert raw(x) == raw(y), (case, arith, i)

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import sparse_coding_b200 as S
+from engine_cases import desc
 from oracle import interp_oracle as IO
 from sparse_coding_b200 import _lib
 from sparse_coding_b200 import metrics as MT
@@ -130,15 +131,9 @@ def test_errors_name_the_constraint():
         MT.top_activating_fragments([(Other(), {})], x)
 
 
-def _desc(M, n, d, B, variant=_lib.SCE_TIED):
-    return _lib.SceDesc(variant=variant, n_models=M, d=d, n=n, batch_max=B, x_per_model=0, lr=0.0, beta1=0.9,
-                        beta2=0.999, eps=1e-8, eps_root=0.0, adam_count_mode=0, fwd_passes=3, bwd_passes=3,
-                        norm_floor=1e-8, arith=0, topk_k_max=0, centering=0)
-
-
 def test_fragments_workspace_bound():
     lib = _lib.load()
-    ws = lambda M, n, d, B, L, Bmax=None: lib.sce_fragments_workspace_bytes(C.byref(_desc(M, n, d, Bmax or B)), B, L)
+    ws = lambda M, n, d, B, L, Bmax=None: lib.sce_fragments_workspace_bytes(C.byref(desc(M, n, d, Bmax or B, lr=0.0)), B, L)
     # config 2: 16 x 4096 features, 8192-row calls of 128 fragments: maxima + flags + open flags = 40 MiB + 256 KiB
     assert ws(16, 4096, 512, 8192, 64) == 16 * 128 * 4096 * 5 + 16 * 4096 * 4 == (40 << 20) + (256 << 10)
     assert ws(16, 4096, 512, 8192, 32) == 16 * 256 * 4096 * 5 + 16 * 4096 * 4

@@ -1,11 +1,13 @@
 """FunctionalTiedCenteredSAE (a tied SAE on x - center with the centre trained) without a GPU: the oracle against the
 reference's recorded results, seeded init, the exported dictionary and the C ABI's host-side checks."""
 import ctypes as C
+import functools
 import os
 
 import pytest
 import torch
 
+from engine_cases import desc
 from oracle import learned_center_oracle as LC
 from oracle import sae_oracle as O
 from sparse_coding_b200 import _lib
@@ -107,10 +109,8 @@ def test_learned_dict_export(cases):
         assert w is fx["params"]["encoder"] and floor == 1e-8 and rows is None
 
 
-def _desc(M=2, n=128, d=64, B=100, xpm=0, cen=0, variant=_lib.SCE_TIED_LEARNED_CENTER):
-    return _lib.SceDesc(variant=variant, n_models=M, d=d, n=n, batch_max=B, x_per_model=xpm, lr=1e-3, beta1=0.9,
-                        beta2=0.999, eps=1e-8, eps_root=0.0, adam_count_mode=0, fwd_passes=3, bwd_passes=3,
-                        norm_floor=1e-8, arith=0, topk_k_max=0, centering=cen)
+# two learned-centre models, n = 128, d = 64, batch_max = 100
+learned_desc = functools.partial(desc, 2, 128, 64, 100, variant=_lib.SCE_TIED_LEARNED_CENTER)
 
 
 @pytest.fixture
@@ -121,16 +121,17 @@ def lib(monkeypatch):
 
 def test_workspace_sizes(lib):
     for xpm in (0, 1):
-        learned = lib.sce_workspace_bytes(C.byref(_desc(xpm=xpm)))
-        tied_per_model = lib.sce_workspace_bytes(C.byref(_desc(xpm=1, variant=_lib.SCE_TIED)))
+        learned = lib.sce_workspace_bytes(C.byref(learned_desc(x_per_model=xpm)))
+        tied_per_model = lib.sce_workspace_bytes(C.byref(learned_desc(x_per_model=1, variant=_lib.SCE_TIED)))
         assert learned > tied_per_model > 0   # M centred batches plus the centre-gradient buffers
-    assert lib.sce_workspace_bytes(C.byref(_desc(xpm=0))) == lib.sce_workspace_bytes(C.byref(_desc(xpm=1)))
-    assert lib.sce_workspace_bytes(C.byref(_desc(xpm=1, cen=1))) == 0
-    assert lib.sce_workspace_bytes(C.byref(_desc(variant=4))) == 0
-    assert lib.sce_forward_stats_workspace_bytes(C.byref(_desc()), 64) == 0
-    assert lib.sce_fragments_workspace_bytes(C.byref(_desc()), 64, 32) == 0
-    assert lib.sce_forward_stats_workspace_bytes(C.byref(_desc(variant=_lib.SCE_TIED)), 64) > 0
-    assert lib.sce_fragments_workspace_bytes(C.byref(_desc(variant=_lib.SCE_TIED)), 64, 32) > 0
+    assert lib.sce_workspace_bytes(C.byref(learned_desc(x_per_model=0))) == \
+        lib.sce_workspace_bytes(C.byref(learned_desc(x_per_model=1)))
+    assert lib.sce_workspace_bytes(C.byref(learned_desc(x_per_model=1, centering=1))) == 0
+    assert lib.sce_workspace_bytes(C.byref(learned_desc(variant=4))) == 0
+    assert lib.sce_forward_stats_workspace_bytes(C.byref(learned_desc()), 64) == 0
+    assert lib.sce_fragments_workspace_bytes(C.byref(learned_desc()), 64, 32) == 0
+    assert lib.sce_forward_stats_workspace_bytes(C.byref(learned_desc(variant=_lib.SCE_TIED)), 64) > 0
+    assert lib.sce_fragments_workspace_bytes(C.byref(learned_desc(variant=_lib.SCE_TIED)), 64, 32) > 0
 
 
 def _create(lib, desc, with_center=True):
@@ -148,12 +149,12 @@ def _create(lib, desc, with_center=True):
 
 
 def test_plan_create_rejections(lib):
-    rc, msg = _create(lib, _desc(), with_center=False)
+    rc, msg = _create(lib, learned_desc(), with_center=False)
     assert rc == -1 and "center" in msg
-    rc, msg = _create(lib, _desc(xpm=1, cen=2))
+    rc, msg = _create(lib, learned_desc(x_per_model=1, centering=2))
     assert rc == -1 and "centering" in msg
     # positive control: with the centre buffers the checks pass, and creation stops at the device query (no GPU here)
-    rc, msg = _create(lib, _desc())
+    rc, msg = _create(lib, learned_desc())
     assert rc != -1 or "center" not in msg
 
 

@@ -11,27 +11,16 @@ import math
 import pytest
 import torch
 
+from engine_cases import clone_models, relnorm, synth
 from oracle import learned_center_oracle as LC
 from oracle import sae_oracle as O
+from oracle.tile_bounds import kink_window
 
 pytestmark = pytest.mark.gpu
 
 REL = 1e-4
 ARITHS = ["bf16x3", "f16f8"]
 CASES = ["three_models", "mean_offset", "f64", "zero_center"]
-
-
-def kink_window(Z):
-    return max(1e-5, 1e-4 * float(Z.double().pow(2).mean().sqrt()))
-
-
-def relnorm(a, b):
-    a, b = a.double(), b.double().to(a.device)
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
-
-
-def clone(ms):
-    return [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
 
 
 def sig():
@@ -42,7 +31,7 @@ def sig():
 def ensemble(models, **kw):
     import sparse_coding_b200 as S
     kw.setdefault("device", "cuda")
-    return S.FunctionalEnsemble(clone(models), sig(), S.adam, {"lr": 1e-3}, **kw)
+    return S.FunctionalEnsemble(clone_models(models), sig(), S.adam, {"lr": 1e-3}, **kw)
 
 
 def fixture_models(fx):
@@ -137,7 +126,7 @@ def test_trajectory_matches_ref_port(arith, mode):
     M, d, n, B = 3, 64, 256, 256
     models = _trajectory_models(M, d, n, 5)
     ens = ensemble(models, adam_count_mode=mode, arith=arith)
-    ref = O.RefPortEnsemble(clone(models), LC.sig_loss_tied_learned_center, lr=1e-3, count_mode=mode)
+    ref = O.RefPortEnsemble(clone_models(models), LC.sig_loss_tied_learned_center, lr=1e-3, count_mode=mode)
     gen = torch.Generator().manual_seed(6)
     offset = 0.5 * torch.randn(d, generator=gen)
     for step in range(30):
@@ -179,12 +168,7 @@ def test_launch_count_and_graph_replay():
 
 def _offset_data(B, d, seed, offset_scale=4.0):
     """fp16-representable sparse-mixture activations whose column mean lies several spreads from the origin."""
-    gen = torch.Generator(device="cuda").manual_seed(seed)
-    feats = torch.randn(2048, d, generator=gen, device="cuda")
-    feats /= feats.norm(dim=-1, keepdim=True)
-    codes = (torch.rand(B, 2048, generator=gen, device="cuda") < 0.01).float() * \
-        torch.rand(B, 2048, generator=gen, device="cuda")
-    x = codes @ feats + 0.05 * torch.randn(B, d, generator=gen, device="cuda")
+    x = synth(B, d, seed, fp16_values=False)
     mu = torch.randn(d, generator=torch.Generator().manual_seed(seed)).cuda()
     x = x + offset_scale * float(x.std()) * mu / float(mu.abs().mean())
     return x.half().float()
@@ -217,7 +201,7 @@ def test_quality_against_ref_port():
     models = [sig().init(d, n, a) for a in (3e-4, 1e-3)]
     ens = ensemble(models)
     ref = O.RefPortEnsemble([({k: v.cuda() for k, v in p.items()}, {k: v.cuda() for k, v in b.items()})
-                             for p, b in clone(models)], LC.sig_loss_tied_learned_center, lr=1e-3)
+                             for p, b in clone_models(models)], LC.sig_loss_tied_learned_center, lr=1e-3)
     for s in range(300):
         X = _offset_data(B, d, 1000 + s)
         ens.step_batch(X)

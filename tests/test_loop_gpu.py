@@ -7,14 +7,10 @@ import numpy as np
 import pytest
 import torch
 
+from engine_cases import clone_models, relnorm
 from oracle import sae_oracle as O
 
 pytestmark = pytest.mark.gpu
-
-
-def relnorm(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.float32])
@@ -32,10 +28,6 @@ def test_gather_rows_bit_exact(dtype):
     assert gather_rows(dev, idx[:1].cuda()).shape == (1, 192)
 
 
-def _clone(ms):
-    return [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-
-
 def test_ensemble_train_loop_matches_reference_loop():
     """big_sweep.py:159-199 semantics on one chunk: same seeds, same sampler, same batches (incl. the short last
     one) as the restated reference loop; final parameters agree with the oracle trained on the same batches."""
@@ -45,8 +37,8 @@ def test_ensemble_train_loop_matches_reference_loop():
     d, n, N, B = 64, 128, 1000, 256
     models = [S.FunctionalTiedSAE.init(d, n, a) for a in (1e-3, 1e-2)]
     chunk = torch.randn(N, d, generator=torch.Generator().manual_seed(5)).half()      # chunks are fp16 on disk
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
-    ref = O.RefPortEnsemble(_clone(models), O.SIG_LOSSES["tied"], lr=1e-3)
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ref = O.RefPortEnsemble(clone_models(models), O.SIG_LOSSES["tied"], lr=1e-3)
 
     class Cfg:
         use_wandb = False
@@ -112,7 +104,7 @@ def test_chunk_streaming_checkpoints_and_resume(tmp_path):
     torch.manual_seed(1)
     models = [S.FunctionalTiedSAE.init(64, 128, a) for a in (1e-3, 1e-2)]
     args = {"device": "cuda", "dict_size": 128, "batch_size": 256}
-    mk = lambda: S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda",
+    mk = lambda: S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda",
                                       adam_count_mode="standard")
     ens = mk()
     dicts = train_on_chunks(ens, args, str(data), str(out), 256, ["dict_size"], ["l1_alpha"], chunk_order=[0, 1, 2],
@@ -143,7 +135,7 @@ def test_per_model_batches_expand_dims_false():
     torch.manual_seed(0)
     d, n, B = 64, 128, 96
     models = [S.FunctionalSAE.init(d, n, a) for a in (1e-3, 1e-2, 3e-2)]
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalSAE, S.adam, {"lr": 1e-3}, device="cuda")
     X = torch.randn(3, B, d)
     grads, (loss, aux) = ens.grads_batch(X.cuda(), expand_dims=False)
     for i, (p, b) in enumerate(models):
@@ -160,7 +152,7 @@ def test_calc_grads_reference_shape():
     import sparse_coding_b200 as S
     torch.manual_seed(0)
     models = [S.FunctionalTiedSAE.init(32, 64, a) for a in (1e-3, 1e-2)]
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
     X = torch.randn(48, 32).cuda()
     g1, (l1, _) = ens.calc_grads(ens.params, ens.buffers, X.expand(2, 48, 32))
     g2, (l2, _) = ens.grads_batch(X)
@@ -176,8 +168,8 @@ def test_host_fed_step_through_c_abi():
     torch.manual_seed(0)
     d, n, B = 64, 128, 200
     models = [S.FunctionalTiedSAE.init(d, n, a) for a in (1e-3, 1e-2)]
-    ens_a = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
-    ens_b = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ens_a = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
+    ens_b = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda")
     X = torch.randn(B, d).pin_memory()
     la, _ = ens_a.step_batch(X.cuda())
     ens_b.forward_batch(X.cuda())                       # builds the plan
@@ -235,8 +227,8 @@ def test_spawned_worker_trains_parent_memory_in_place():
     torch.manual_seed(0)
     d, n, B = 64, 128, 256
     models = [S.FunctionalTiedSAE.init(d, n, a) for a in (1e-3, 1e-2)]
-    ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda:0")
-    twin = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda:0")
+    ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda:0")
+    twin = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device="cuda:0")
     gen = torch.Generator().manual_seed(1)
     batches = [torch.randn(B, d, generator=gen) for _ in range(3)]
     before = ens.params["encoder"].clone()
@@ -266,7 +258,7 @@ def test_two_devices_in_one_process():
     X = torch.randn(256, 64)
     outs = []
     for dev in ("cuda:0", "cuda:1"):
-        ens = S.FunctionalEnsemble(_clone(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device=dev)
+        ens = S.FunctionalEnsemble(clone_models(models), S.FunctionalTiedSAE, S.adam, {"lr": 1e-3}, device=dev)
         loss, _ = ens.step_batch(X.to(dev))
         outs.append((loss["loss"].cpu(), ens.params["encoder"].cpu()))
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])

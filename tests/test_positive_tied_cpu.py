@@ -2,11 +2,13 @@
 against the reference's recorded results, including its straight-through encoder gradient, seeded init, the exported
 dictionary and the C ABI's host-side checks."""
 import ctypes as C
+import functools
 import pickle
 
 import pytest
 import torch
 
+from engine_cases import desc
 from oracle import positive_tied_oracle as PT
 from sparse_coding_b200 import _lib
 
@@ -192,11 +194,8 @@ def test_unsupported_signature_error_names_it():
         S.FunctionalEnsemble([({"encoder": torch.zeros(8, 8)}, {})], Other, S.adam, {"lr": 1e-3})
 
 
-def _desc(M=2, n=128, d=64, B=100, xpm=0, cen=0, variant=_lib.SCE_TIED, nonneg=1, shift=0.18):
-    return _lib.SceDesc(variant=variant, n_models=M, d=d, n=n, batch_max=B, x_per_model=xpm, lr=1e-3, beta1=0.9,
-                        beta2=0.999, eps=1e-8, eps_root=0.0, adam_count_mode=0, fwd_passes=3, bwd_passes=3,
-                        norm_floor=1e-8, arith=0, topk_k_max=0, centering=cen, encoder_nonneg=nonneg,
-                        input_shift=shift)
+# two non-negative tied models on x + 0.18, n = 128, d = 64, batch_max = 100
+positive_desc = functools.partial(desc, 2, 128, 64, 100, encoder_nonneg=1, input_shift=0.18)
 
 
 @pytest.fixture
@@ -211,39 +210,41 @@ def test_desc_fields_appended():
 
 
 def test_workspace_sizes(lib):
-    ws = lambda **kw: lib.sce_workspace_bytes(C.byref(_desc(**kw)))
+    ws = lambda **kw: lib.sce_workspace_bytes(C.byref(positive_desc(**kw)))
     for xpm in (0, 1):
         xm = 2 if xpm else 1
-        tied = ws(xpm=xpm, nonneg=0, shift=0.0)
+        tied = ws(x_per_model=xpm, encoder_nonneg=0, input_shift=0.0)
         assert tied > 0
-        assert ws(xpm=xpm, shift=0.0) == tied                            # the clamp needs no workspace
+        assert ws(x_per_model=xpm, input_shift=0.0) == tied              # the clamp needs no workspace
         shifted = (xm * 100 * 64 * 4 + 1023) // 1024 * 1024             # x + shift, [xm, batch_max, d] fp32
-        assert ws(xpm=xpm) == tied + shifted
-        assert ws(xpm=xpm, nonneg=0) == tied + shifted
+        assert ws(x_per_model=xpm) == tied + shifted
+        assert ws(x_per_model=xpm, encoder_nonneg=0) == tied + shifted
 
 
 @pytest.mark.parametrize("variant", [_lib.SCE_UNTIED, _lib.SCE_TOPK, _lib.SCE_TIED_LEARNED_CENTER])
 @pytest.mark.parametrize("fields", [(1, 0.0), (0, 0.18), (1, 0.18)])
 def test_fields_rejected_on_other_variants(lib, variant, fields):
     nonneg, shift = fields
-    assert lib.sce_workspace_bytes(C.byref(_desc(variant=variant, nonneg=0, shift=0.0, xpm=1))) > 0   # positive control
-    assert lib.sce_workspace_bytes(C.byref(_desc(variant=variant, nonneg=nonneg, shift=shift, xpm=1))) == 0
+    ws = lambda **kw: lib.sce_workspace_bytes(C.byref(positive_desc(variant=variant, x_per_model=1, **kw)))
+    assert ws(encoder_nonneg=0, input_shift=0.0) > 0   # positive control
+    assert ws(encoder_nonneg=nonneg, input_shift=shift) == 0
 
 
 def test_validate_rejections(lib):
-    ws = lambda **kw: lib.sce_workspace_bytes(C.byref(_desc(**kw)))
-    assert ws(xpm=1, cen=2, shift=0.0) > 0                    # centring with the clamp alone is allowed
-    assert ws(xpm=1, cen=2) == 0 and ws(xpm=1, cen=1) == 0    # the shift is not combined with centring
-    assert ws(nonneg=2) == 0
-    assert ws(shift=float("inf")) == 0 and ws(shift=float("nan")) == 0
+    ws = lambda **kw: lib.sce_workspace_bytes(C.byref(positive_desc(**kw)))
+    assert ws(x_per_model=1, centering=2, input_shift=0.0) > 0     # centring with the clamp alone is allowed
+    # the shift is not combined with centring
+    assert ws(x_per_model=1, centering=2) == 0 and ws(x_per_model=1, centering=1) == 0
+    assert ws(encoder_nonneg=2) == 0
+    assert ws(input_shift=float("inf")) == 0 and ws(input_shift=float("nan")) == 0
 
 
 def test_forward_only_passes_refused(lib):
     for nonneg, shift in ((1, 0.0), (0, 0.18), (1, 0.18)):
-        d = _desc(nonneg=nonneg, shift=shift)
+        d = positive_desc(encoder_nonneg=nonneg, input_shift=shift)
         assert lib.sce_forward_stats_workspace_bytes(C.byref(d), 64) == 0
         assert lib.sce_fragments_workspace_bytes(C.byref(d), 64, 32) == 0
-    plain = _desc(nonneg=0, shift=0.0)
+    plain = positive_desc(encoder_nonneg=0, input_shift=0.0)
     assert lib.sce_forward_stats_workspace_bytes(C.byref(plain), 64) > 0
     assert lib.sce_fragments_workspace_bytes(C.byref(plain), 64, 32) > 0
 
@@ -269,10 +270,10 @@ def _create(lib, desc, coef_mask=False):
 
 def test_plan_create_rejects_the_fields_with_coef_mask(lib):
     for nonneg, shift in ((1, 0.0), (0, 0.18), (1, 0.18)):
-        rc, msg = _create(lib, _desc(nonneg=nonneg, shift=shift), coef_mask=True)
+        rc, msg = _create(lib, positive_desc(encoder_nonneg=nonneg, input_shift=shift), coef_mask=True)
         assert rc == -1 and "coef_mask" in msg, msg
     # positive controls: the masked tied plan alone, and the fields without a mask, pass these checks: creation goes on
     # to the device query, which fails without an sm_90 device (SCE_ERR_NO_DEVICE) and succeeds with one (SCE_OK)
-    for desc, mask in ((_desc(nonneg=0, shift=0.0), True), (_desc(), False)):
+    for desc, mask in ((positive_desc(encoder_nonneg=0, input_shift=0.0), True), (positive_desc(), False)):
         rc, msg = _create(lib, desc, coef_mask=mask)
         assert rc != -1, (rc, msg)

@@ -13,8 +13,10 @@ import numpy as np
 import pytest
 import torch
 
+from engine_cases import clone_models, relnorm
 from oracle import positive_tied_oracle as PT
 from oracle import sae_oracle as O
+from oracle.tile_bounds import kink_window
 
 pytestmark = pytest.mark.gpu
 
@@ -27,19 +29,6 @@ CAT_D = CAT_N = CAT_B = 2048
 CAT_L1 = [0.0] + np.logspace(-5, -3.5, 8).tolist()
 
 
-def kink_window(Z):
-    return max(1e-5, 1e-4 * float(Z.double().pow(2).mean().sqrt()))
-
-
-def relnorm(a, b):
-    a, b = a.double(), b.double().to(a.device)
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
-
-
-def clone(ms):
-    return [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
-
-
 def sig():
     import sparse_coding_b200 as S
     return S.FunctionalPositiveTiedSAE
@@ -48,7 +37,7 @@ def sig():
 def ensemble(models, lr=1e-3, **kw):
     import sparse_coding_b200 as S
     kw.setdefault("device", "cuda")
-    return S.FunctionalEnsemble(clone(models), sig(), S.adam, {"lr": lr}, **kw)
+    return S.FunctionalEnsemble(clone_models(models), sig(), S.adam, {"lr": lr}, **kw)
 
 
 def fixture_models(fx):
@@ -155,7 +144,7 @@ def test_trajectory_matches_ref_port(arith, mode):
     lr = 3e-3
     models = _trajectory_models(M, d, n, 5)
     ens = ensemble(models, lr=lr, adam_count_mode=mode, arith=arith)
-    ref = O.RefPortEnsemble(clone(models), PT.sig_loss_positive_tied, lr=lr, count_mode=mode)
+    ref = O.RefPortEnsemble(clone_models(models), PT.sig_loss_positive_tied, lr=lr, count_mode=mode)
     for step in range(30):
         X = mlp_data(B if step % 10 != 9 else 37, d, 100 + step).cpu()
         loss, _ = ens.step_batch(X.cuda())
@@ -258,7 +247,7 @@ def test_quality_against_ref_port():
     models = catalogue_models(1)
     ens = ensemble(models)
     ref = O.RefPortEnsemble([({k: v.cuda() for k, v in p.items()}, {k: v.cuda() for k, v in b.items()})
-                             for p, b in clone(models)], PT.sig_loss_positive_tied, lr=1e-3)
+                             for p, b in clone_models(models)], PT.sig_loss_positive_tied, lr=1e-3)
     for s in range(300):
         X = mlp_data(CAT_B, CAT_D, 1000 + s)
         ens.step_batch(X)

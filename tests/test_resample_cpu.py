@@ -8,6 +8,7 @@ import os
 import pytest
 import torch
 
+import engine_cases
 import sparse_coding_b200 as S
 from oracle import resample_oracle as RO
 from sparse_coding_b200 import _lib, train_loop
@@ -65,16 +66,9 @@ def test_oracle_leaves_extra_dead_features_and_skips_masked_padding():
     assert torch.allclose(out["W"][2], rows[1].double() * 0.2 / mu)
 
 
-def _desc(**kw):
-    d = dict(variant=0, n_models=2, d=64, n=128, batch_max=256, x_per_model=0, lr=1e-3, beta1=0.9, beta2=0.999,
-             eps=1e-8, eps_root=0.0, adam_count_mode=0, fwd_passes=3, bwd_passes=3, norm_floor=1e-8)
-    d.update(kw)
-    return _lib.SceDesc(**d)
-
-
 def test_track_workspace_bytes():
     lib = _lib.load()
-    desc = _desc()
+    desc = engine_cases.desc(2, 128, 64, 256)
     need = lib.sce_track_workspace_bytes(C.byref(desc), 128)
     assert need > 0 and need % 1024 == 0
     assert lib.sce_track_workspace_bytes(C.byref(desc), 16) < need
@@ -85,7 +79,7 @@ def test_track_workspace_bytes():
         assert b"n_worst" in lib.sce_last_error()
     desc.d = 63
     assert lib.sce_track_workspace_bytes(C.byref(desc), 16) == 0
-    cfg2 = _desc(n_models=16, d=512, n=4096, batch_max=8192)
+    cfg2 = engine_cases.desc(16, 4096, 512, 8192)
     assert lib.sce_track_workspace_bytes(C.byref(cfg2), 4096) < 16 * 2**20
 
 

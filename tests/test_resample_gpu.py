@@ -6,21 +6,15 @@ Row errors e_r are held per row to a bound derived from the per-element x_hat ba
 |x_hat - x_hat*| <= bar S (S the absolute-product scale of x_hat), |e_r - e_r*| <= mean_d bar S (2 |x_hat* - x| + bar S),
 doubled, plus the fp32 rounding of the row sum. Lists must hold the oracle's top N by fp64 error except rows within
 that bound of the N-th value; rows, serials and counts are exact."""
-import importlib.util
-import os
-
 import pytest
 import torch
 
+import engine_cases as EC
 from oracle import resample_oracle as RO
+from oracle import sae_oracle as O
 from oracle import tile_bounds as T
 
 pytestmark = pytest.mark.gpu
-
-_spec = importlib.util.spec_from_file_location(
-    "tile_bounds_checks", os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_tile_bounds_gpu.py"))
-TB = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(TB)
 
 SHAPE = (4, 400, 1040, 1000)          # M, d, n, B (B <= n: one step from an empty window lists every row)
 VARIANTS = ["tied", "untied", "masked_tied", "masked_untied", "learned_center", "positive_tied", "topk_gather",
@@ -43,8 +37,8 @@ def build(variant, arith, shape=SHAPE, seed=3):
         ks = TOPK_K[variant][:M] if M <= 4 else [32] * M
         models, sig = [S.TopKEncoder.init(d, n, k) for k in ks], S.TopKEncoder
     else:
-        models, sig = TB.make_models(variant, M, d, n, seed)
-    return TB.ensemble(models, sig, arith), models
+        models, sig = EC.make_models(variant, M, d, n, seed)
+    return EC.ensemble(models, sig, arith), models
 
 
 def main_key(ens):
@@ -62,15 +56,15 @@ def xhat_bound(variant, arith, P, buf, X):
     code, e = RO.forward64(name, P, buf, X)
     p = {k: v.double() for k, v in P.items()}
     if name == "topk":
-        W, _ = TB.O.unit_rows(p["dict"], floor=None)
+        W, _ = O.unit_rows(p["dict"], floor=None)
         S_ = (X.double().abs() @ W.abs().T) * (code > 0) @ W.abs()
         bar = T.TOPK_BARS[arith]["x_hat"][1]
         xin = X.double()
     else:
-        f = TB.oracle(variant, p, {k: v.double() if v.is_floating_point() else v for k, v in buf.items()}, X.double())
+        f = EC.oracle(variant, p, {k: v.double() if v.is_floating_point() else v for k, v in buf.items()}, X.double())
         W_dec = f["W"]
         S_ = T.x_hat_scale(f["Xabs"], f["W_enc"], p["encoder_bias"], W_dec)
-        bar = T.BARS[arith][TB.sign(variant)]["x_hat"][1]
+        bar = T.BARS[arith][EC.sign(variant)]["x_hat"][1]
         xin = f["Xin"]
         code = f["c"]
     xh = code @ (W if name == "topk" else f["W"])
@@ -87,7 +81,7 @@ def per_model(ens, m):
 
 def data(shape, seed, scale=1.0):
     M, d, n, B = shape
-    return TB.synth(B, d, seed) * scale
+    return EC.synth(B, d, seed) * scale
 
 
 @pytest.mark.parametrize("arith", ["bf16x3", "f16f8"])
@@ -141,7 +135,7 @@ def _window(ens, shape, seeds, ragged=None):
     batches, pres = [], []
     for i, s in enumerate(seeds):
         rows = ragged if (ragged and i == len(seeds) - 1) else B
-        X = TB.synth(rows, d, s)
+        X = EC.synth(rows, d, s)
         pres.append(snapshot(ens)[0])
         ens.step_batch(X)
         batches.append(X)
@@ -164,7 +158,7 @@ def test_window_lists_counts_and_resample(variant, arith):
     counts = torch.zeros(M, n, dtype=torch.int32, device="cuda")
     batches, pres = [], []
     for i, s in enumerate([21, 22, 23]):
-        X = TB.synth(B if i < 2 else 333, d, s)
+        X = EC.synth(B if i < 2 else 333, d, s)
         pres.append(snapshot(ens)[0])
         ens.step_batch(X)
         ens.active_counts(X.shape[0], counts)
@@ -244,7 +238,7 @@ def test_window_lists_counts_and_resample(variant, arith):
     clone = lambda tree: {k: (clone(v) if isinstance(v, dict) else v.clone()) for k, v in tree.items()}
     fresh = S.FunctionalEnsemble.from_state(dict(sd, params=clone(sd["params"]), buffers=clone(sd["buffers"]),
                                                  optim_states=clone(sd["optim_states"])))
-    X = TB.synth(B, d, 77)
+    X = EC.synth(B, d, 77)
     la, _ = ens.step_batch(X)
     lb, _ = fresh.step_batch(X)
     for k in la:
@@ -260,8 +254,8 @@ def test_repeatable_and_survives_rebuild_and_fallback():
     for _ in range(2):
         ens, _ = build("tied", "auto", shape, seed=9)
         ens.track_dead_features(200)
-        ens.step_batch(TB.synth(500, 400, 1))
-        ens.step_batch(TB.synth(900, 400, 2))                  # a larger batch: the plan is rebuilt, the window stays
+        ens.step_batch(EC.synth(500, 400, 1))
+        ens.step_batch(EC.synth(900, 400, 2))                  # a larger batch: the plan is rebuilt, the window stays
         assert ens._plan_key[0] == 900
         runs.append([{k: v.clone() for k, v in l.items()} for l in ens.worst_rows()])
         assert ens._track["next_serial"] == 1400
@@ -272,8 +266,8 @@ def test_repeatable_and_survives_rebuild_and_fallback():
     # arith="auto": an out-of-range batch is skipped on f16f8 and re-run on bf16x3; it enters the window once
     ens, _ = build("tied", "auto", shape, seed=9)
     ens.track_dead_features(200)
-    ens.step_batch(TB.synth(500, 400, 1))
-    X = TB.synth(500, 400, 3)
+    ens.step_batch(EC.synth(500, 400, 1))
+    X = EC.synth(500, 400, 3)
     X[7, 3] = 1e5
     with pytest.warns(RuntimeWarning):
         ens.health_check_every = 1
@@ -295,7 +289,7 @@ def test_config_shapes_agree_with_the_oracle(shape):
     ens.track_dead_features()
     pres, batches = [], []
     for s in (31, 32):
-        X = TB.synth(B, d, s)
+        X = EC.synth(B, d, s)
         pres.append(snapshot(ens)[0])
         ens.step_batch(X)
         batches.append(X)

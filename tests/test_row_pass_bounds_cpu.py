@@ -1,25 +1,18 @@
 """oracle/row_pass_bounds.py on the CPU: the absolute-product scales bound what they scale, the slicing restatement keeps
-its invariants, and the per-tile check with the bars of tests/test_row_pass_tiles_gpu.py rejects each planted defect of
-a row pass (one tile off by 4 bars, the last slice's padding rows added as 0 - shift, the last partial slice dropped,
+its invariants, and the per-tile check with its bars (measured in tests/test_row_pass_tiles_gpu.py) rejects each
+planted defect of a row pass (one tile off by 4 bars, the last slice's padding rows added as 0 - shift, the last partial slice dropped,
 g' counted over padding rows, an output stored instead of accumulated) while it accepts the exact result rounded to
 fp32."""
-import importlib.util
-import os
-
 import pytest
 import torch
 
+from engine_cases import ARITHS
 from oracle import row_pass_bounds as RB
 from oracle import tile_bounds as T
 
-_spec = importlib.util.spec_from_file_location(
-    "row_pass_tiles", os.path.join(os.path.dirname(os.path.abspath(__file__)), "test_row_pass_tiles_gpu.py"))
-G = importlib.util.module_from_spec(_spec)
-_spec.loader.exec_module(G)
-
 KINDS = ("moments", "ica", "project", "grams")
 D, N, B = 200, 136, 700            # 2 x 2 tiles, the last ragged; 3 slices of 256 rows, 68 of them padding
-ALPHA = G.ALPHA
+ALPHA = RB.ALPHA
 
 
 def data(kind, positive, seed=0):
@@ -45,7 +38,7 @@ def worst(kind, name, got, want, scale):
 
 
 def bar(kind, name, arith):
-    return G.BARS[kind][name][arith][0]
+    return RB.BARS[kind][name][arith][0]
 
 
 def test_slicing_restatement():
@@ -64,7 +57,7 @@ def test_scales_bound_their_outputs(kind):
         assert bool((scale > 0).all()), name
 
 
-@pytest.mark.parametrize("arith", G.ARITHS)
+@pytest.mark.parametrize("arith", ARITHS)
 @pytest.mark.parametrize("kind", KINDS)
 def test_bars_accept_the_exact_result_rounded_to_fp32(kind, arith):
     for positive in (False, True):
@@ -73,10 +66,10 @@ def test_bars_accept_the_exact_result_rounded_to_fp32(kind, arith):
             r = worst(kind, name, want.float().double(), want, scale)
             assert r <= bar(kind, name, arith), (name, r, bar(kind, name, arith))
     want, scale = RB.nmf_residual(RB.shifted(x, shift, clamp=True), torch.rand(B, 8), torch.rand(8, D))
-    assert abs(float(torch.tensor(want).float()) - want) / scale <= G.BARS["residual"]
+    assert abs(float(torch.tensor(want).float()) - want) / scale <= RB.BARS["residual"]
 
 
-@pytest.mark.parametrize("arith", G.ARITHS)
+@pytest.mark.parametrize("arith", ARITHS)
 @pytest.mark.parametrize("kind", KINDS)
 def test_one_tile_off_by_four_bars_fails(kind, arith):
     x, shift, mat = data(kind, True)
@@ -101,7 +94,7 @@ def padded(x, mat, kind):
     return x, mat
 
 
-@pytest.mark.parametrize("arith", G.ARITHS)
+@pytest.mark.parametrize("arith", ARITHS)
 @pytest.mark.parametrize("kind", ("moments", "ica"))
 def test_padding_rows_as_minus_shift_fail(kind, arith):
     x, shift, mat = data(kind, False)
@@ -111,7 +104,7 @@ def test_padding_rows_as_minus_shift_fail(kind, arith):
     assert worst(kind, name, bad[name][0], *ref[name]) > bar(kind, name, arith)
 
 
-@pytest.mark.parametrize("arith", G.ARITHS)
+@pytest.mark.parametrize("arith", ARITHS)
 @pytest.mark.parametrize("kind", ("moments", "ica", "grams"))
 def test_last_partial_slice_dropped_fails(kind, arith):
     x, shift, mat = data(kind, False)
@@ -123,7 +116,7 @@ def test_last_partial_slice_dropped_fails(kind, arith):
         assert worst(kind, name, bad[name][0], *ref[name]) > bar(kind, name, arith), name
 
 
-@pytest.mark.parametrize("arith", G.ARITHS)
+@pytest.mark.parametrize("arith", ARITHS)
 def test_g_prime_over_padding_rows_fails(arith):
     """g' = alpha (1 - 0) on the rows of the last 32-row block past B (u = 0 on a zero padding row)."""
     x, shift, mat = data("ica", False)
@@ -132,13 +125,13 @@ def test_g_prime_over_padding_rows_fails(arith):
     assert worst("ica", "g_sum", got, want, scale) > bar("ica", "g_sum", arith)
 
 
-@pytest.mark.parametrize("arith", G.ARITHS)
+@pytest.mark.parametrize("arith", ARITHS)
 @pytest.mark.parametrize("kind", KINDS)
 def test_stored_instead_of_accumulated_fails(kind, arith):
     """out - initial, where the pass wrote its result over the initial values instead of adding to them."""
     x, shift, mat = data(kind, False)
     for name, (want, scale) in RB.reference(kind, x, shift, mat, ALPHA).items():
-        if name not in G.ACCUMULATED:
+        if name not in RB.ACCUMULATED:
             continue
         init = (float(scale.abs().mean()) + 1.0) * (torch.rand(want.shape, generator=torch.Generator().manual_seed(3),
                                                                dtype=torch.float64) + 0.5)

@@ -22,7 +22,9 @@ import os
 import pytest
 import torch
 
+from engine_cases import clone_models, relnorm, synth
 from oracle import sae_oracle as O
+from oracle.tile_bounds import kink_window
 
 pytestmark = pytest.mark.gpu
 
@@ -34,32 +36,8 @@ def report(line: str) -> None:
     print(line)
 
 
-def relnorm(a, b):
-    a, b = a.double(), b.double().to(a.device)
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
-
-
 def relabs(a, b):
     return abs(float(a) - float(b)) / max(abs(float(b)), 1e-30)
-
-
-def kink_window(Z):
-    return max(1e-5, 1e-4 * float(Z.double().pow(2).mean().sqrt()))
-
-
-def synth(B, d, seed, device="cuda", n_feats=2048, density=0.01, noise=0.05, fp16_values=True):
-    """Sparse-mixture activations (sc_datasets/random_dataset.py:76-142 semantics), generated on the device."""
-    gen = torch.Generator(device=device).manual_seed(seed)
-    feats = torch.randn(n_feats, d, generator=gen, device=device)
-    feats /= feats.norm(dim=-1, keepdim=True)
-    codes = (torch.rand(B, n_feats, generator=gen, device=device) < density).float() * \
-        torch.rand(B, n_feats, generator=gen, device=device)
-    x = codes @ feats + noise * torch.randn(B, d, generator=gen, device=device)
-    return x.half().float() if fp16_values else x
-
-
-def clone_models(ms):
-    return [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in ms]
 
 
 def sae_case(kind, M, d, n, seed, alphas, bias_std=0.02):

@@ -62,256 +62,21 @@ the pre-activation gradient's scale is as small as the 3-pass error of the featu
 inactive), the non-negative dictionary in f16f8 (its one-signed sums accumulate fp32 rounding in the tensor cores as
 large as a single pass's operand rounding), and the bf16x3 encoder gradient. For those outputs the bar still bounds
 every tile and element at twice the worst value measured, but a tile at 1-pass accuracy is not guaranteed to fail it.
-The whole file runs in about 30 s on an H100.
+The whole file runs in about 30 s on an H100. The harness it runs is tests/engine_cases.py, shared with the other
+step tests.
 """
 import pytest
 import torch
 
-from oracle import learned_center_oracle as LC
-from oracle import positive_tied_oracle as PT
-from oracle import sae_oracle as O
+from engine_cases import (ARITHS, RAGGED, RAGGED_EAGER, VARIANTS, batch, ensemble, make_models, measure, oracle,
+                          regate_exact_zeros, relnorm, report, run_case, scales, sign)
 from oracle import tile_bounds as T
 from oracle.plan_paths import launch_bound
 
 pytestmark = pytest.mark.gpu
 
-ARITHS = ["bf16x3", "f16f8"]
-VARIANTS = ["tied", "tied_centering", "untied", "masked_tied", "masked_untied", "learned_center", "positive_tied"]
-RAGGED = (4, 400, 1040, 4001)        # M, d, n, B
-RAGGED_EAGER = (4, 400, 1040, 8001)  # the same, above the launch-bound rule (oracle/plan_paths.py)
 REL, GRAD_REL = 1e-4, 2e-4           # the per-model norm-relative bars of the other parity tests
-NEAR_FRAC = 5e-4                     # bound on the share of coefficients inside the kink window
-EXACT_ZERO_FLOOR = 3e-5              # bias-gradient error / scale above which an exact-zero pre-activation is looked for
-TILE_OUTPUTS = ("code", "x_hat", "encoder", "decoder", "encoder_bias", "center")
-
 BARS, SEPARATED = T.BARS, T.SEPARATED   # (tile ratio bar, element bar) and the separated outputs: see the docstring
-
-
-def sign(variant):
-    return "nonneg" if variant == "positive_tied" else "signed"
-
-
-def relnorm(a, b):
-    a, b = a.double(), b.double().to(a.device)
-    return float((a - b).norm() / b.norm().clamp(min=1e-30))
-
-
-def synth(B, d, seed, fp16_values=True, n_feats=2048):
-    """Sparse-mixture activations, generated on the device (as tests/test_scale_parity_gpu.py)."""
-    gen = torch.Generator(device="cuda").manual_seed(seed)
-    feats = torch.randn(n_feats, d, generator=gen, device="cuda")
-    feats /= feats.norm(dim=-1, keepdim=True)
-    codes = (torch.rand(B, n_feats, generator=gen, device="cuda") < 0.01).float() * \
-        torch.rand(B, n_feats, generator=gen, device="cuda")
-    x = codes @ feats + 0.05 * torch.randn(B, d, generator=gen, device="cuda")
-    return x.half().float() if fp16_values else x
-
-
-def batch(M, B, d, seed, per_model, fp16_values, n_feats=2048):
-    if per_model:
-        return torch.stack([synth(B, d, seed + 7919 * m, fp16_values, n_feats) for m in range(M)])
-    return synth(B, d, seed, fp16_values, n_feats)
-
-
-def make_models(variant, M, d, n, seed):
-    import sparse_coding_b200 as S
-    torch.manual_seed(seed)
-    gen = torch.Generator().manual_seed(seed + 1)
-    models = []
-    for m, a in enumerate(torch.logspace(-4, -2, M).tolist()):
-        size = [n, n - 57, n // 2 + 3, n // 5 + 1][m % 4]     # masked dictionary sizes, not multiples of 128
-        if variant == "tied":
-            sig = S.FunctionalTiedSAE
-            p, b = sig.init(d, n, a)
-        elif variant == "tied_centering":
-            sig = S.FunctionalTiedSAE
-            q, _ = torch.linalg.qr(torch.randn(d, d, generator=gen))
-            p, b = sig.init(d, n, a, translation=0.3 * torch.randn(d, generator=gen), rotation=q.contiguous(),
-                            scaling=0.5 + torch.rand(d, generator=gen))
-        elif variant == "untied":
-            sig = S.FunctionalSAE
-            p, b = sig.init(d, n, a, bias_decay=0.01)
-        elif variant == "masked_tied":
-            sig = S.FunctionalMaskedTiedSAE
-            p, b = sig.init(d, size, n, a)
-        elif variant == "masked_untied":
-            sig = S.FunctionalMaskedSAE
-            p, b = sig.init(d, size, n, a)
-        elif variant == "learned_center":
-            sig = S.FunctionalTiedCenteredSAE
-            p, b = sig.init(d, n, a, center=0.1 * torch.randn(d, generator=gen))
-        else:
-            sig = S.FunctionalPositiveTiedSAE
-            p, b = sig.init(d, n, a, 0.01)
-        if variant != "positive_tied":
-            p["encoder_bias"] = 0.02 * torch.randn(n, generator=gen)
-        models.append((p, b))
-    return models, sig
-
-
-def ensemble(models, sig, arith, **kw):
-    import sparse_coding_b200 as S
-    clone = [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in models]
-    return S.FunctionalEnsemble(clone, sig, S.adam, {"lr": 1e-3}, device="cuda", arith=arith, **kw)
-
-
-def oracle(variant, P, buf, X, active=None):
-    """fp64 forward of one model (and, given the activity pattern ``active``, its gradients), with the batch the loss
-    sees (``Xin``: centred or shifted) and the encoder matrix the code is computed from (``W_enc``)."""
-    alpha = float(buf["l1_alpha"])
-    bd = float(buf["bias_decay"]) if "bias_decay" in buf and not variant.startswith("masked") else 0.0
-    mask = buf["coef_mask"].bool() if variant.startswith("masked") else None
-    E, b = P["encoder"], P["encoder_bias"]
-    if variant in ("untied", "masked_untied"):
-        Xin, W_enc = X, E
-        f = (O.untied_forward(E, b, P["decoder"], X, alpha, bd, mask) if active is None else
-             O.untied_grads(E, b, P["decoder"], X, alpha, bd, mask, active))
-    elif variant == "learned_center":
-        Xin = X - P["center"][None, :]
-        f = O.tied_forward(E, b, Xin, alpha) if active is None else \
-            LC.tied_center_grads(E, b, P["center"], X, alpha, active)
-    elif variant == "positive_tied":
-        Xin = X + PT.SHIFT
-        f = O.tied_forward(E.clamp(min=0.0), b, Xin, alpha, bd) if active is None else \
-            PT.positive_tied_grads(E, b, X, alpha, bd, active)
-    else:
-        Xin = X if variant != "tied_centering" else \
-            O.center(X, buf["center_trans"].double(), buf["center_rot"].double(), buf["center_scale"].double())
-        f = O.tied_forward(E, b, Xin, alpha, bd, mask) if active is None else \
-            O.tied_grads(E, b, Xin, alpha, bd, mask, active)
-    if variant not in ("untied", "masked_untied"):
-        W_enc = f["W"]
-    Xabs = Xin.abs() if variant != "tied_centering" else \
-        T.centered_input_scale(X, buf["center_trans"].double(), buf["center_rot"].double(), buf["center_scale"].double())
-    f.update(Xin=Xin, Xabs=Xabs, W_enc=W_enc, bd=bd, alpha_over_B=alpha / X.shape[0])
-    if active is not None:
-        f["gate"] = (active | (f["Z"] == 0)) & (~mask if mask is not None else True)
-    return f
-
-
-def scales(variant, f, b):
-    """Absolute-product scale of every gradient the signature has (oracle/tile_bounds.py)."""
-    S_dz = T.pre_activation_grad_scale(f["G"], f["W"], f["alpha_over_B"], f["gate"])
-    out = {"encoder_bias": T.bias_grad_scale(S_dz, O._bias_decay_grad(b, f["bd"]))}
-    if variant not in ("untied", "masked_untied"):
-        out["encoder"] = T.row_norm_jacobian_scale(f["W"], f["s"], T.weight_grad_scale(S_dz, f["Xabs"], f["c"], f["G"]))
-    else:
-        out["encoder"] = T.weight_grad_scale(S_dz, f["Xabs"])
-        out["decoder"] = T.row_norm_jacobian_scale(f["W"], f["s"], T.weight_grad_scale(None, None, f["c"], f["G"]))
-    if variant == "learned_center":
-        out["center"] = T.center_grad_scale(f["G"], out["encoder_bias"], f["W"])
-    return out
-
-
-def regate_exact_zeros(variant, f, db_engine, candidates):
-    """A pre-activation the engine computes as exactly 0 is inactive in its code and mask but passes the reconstruction
-    gradient, without the L1 term (clamp's gradient at 0); the API does not read that bit back, and the pinned oracle has
-    the coefficient closed. A feature whose bias-gradient error is explained to 90 % by one candidate (inside the kink
-    window, zero code) gets that coefficient opened in ``f``: dz = g w^T there, added to the bias, encoder (and centre)
-    gradients. Only an error above EXACT_ZERO_FLOOR of the bias gradient's scale qualifies, so at most one coefficient's
-    worth of error per feature is explained away, and the caller bounds how many are. Returns the coefficients opened."""
-    G, W, X = f["G"], f["W"], f["Xin"]
-    err = db_engine.double() - f["grads"]["encoder_bias"]
-    floor = EXACT_ZERO_FLOOR * T.bias_grad_scale(T.pre_activation_grad_scale(G, W, f["alpha_over_B"], f["gate"]))
-    opened = []
-    for j in torch.nonzero(candidates.any(0) & (err.abs() > floor)).flatten().tolist():
-        rows = torch.nonzero(candidates[:, j]).flatten()
-        v = G[rows] @ W[j]
-        k = int((err[j] - v).abs().argmin())
-        if not float((err[j] - v[k]).abs()) <= 0.1 * abs(float(err[j])):
-            continue
-        r, dz = int(rows[k]), float(v[k])
-        dw = dz * X[r]
-        f["grads"]["encoder_bias"][j] += dz
-        if variant in ("untied", "masked_untied"):
-            f["grads"]["encoder"][j] += dw
-        else:
-            f["grads"]["encoder"][j] += (dw - W[j] * (W[j] @ dw)) / f["s"][j]
-        if "center" in f["grads"]:
-            f["grads"]["center"] -= dz * W[j]
-        f["gate"][r, j] = True
-        opened.append((r, j))
-    return opened
-
-
-def measure(variant, ens, X, per_model):
-    """Engine outputs of one grads_batch / forward_batch on X against the fp64 oracle, every model, every tile.
-    Returns (T.Worst, kink counts per model)."""
-    grads, (loss, aux) = ens.grads_batch(X, expand_dims=not per_model)
-    code = aux["c"].dense()
-    counts = ens.active_counts(X.shape[-2])
-    _, _, x_hat = ens.forward_batch(X, expand_dims=not per_model, return_x_hat=True)
-    w, kinks = T.Worst(), []
-    for m in range(ens.n_models):
-        P = {k: v[m].double() for k, v in ens.params.items()}
-        buf = {k: v[m] for k, v in ens.buffers.items()}
-        Xm = (X[m] if per_model else X).double()
-        f0 = oracle(variant, P, buf, Xm)
-        Z = f0["Z"]
-        near = Z.abs() < T.kink_window(Z)
-        eng_pos = T.engine_activity(code[m], counts[m], near, Z)
-        across = eng_pos != (f0["c"] > 0)                      # (a masked coefficient is 0 on both sides)
-        kinks.append((int(near.sum()), int((across & near).sum()), int((across & ~near).sum()), Z.numel()))
-        del across
-        S_code = T.code_scale(f0["Xabs"], f0["W_enc"], P["encoder_bias"])
-        w.add("code", m, T.tile_ratios(code[m], f0["c"], S_code))
-        w.add("x_hat", m, T.tile_ratios(x_hat[m], f0["x_hat"], S_code @ f0["W"].abs()))
-        del S_code
-        want = {"l_reconstruction": f0["l_reconstruction"], "l_l1": f0["l_l1"], "l_bias_decay": f0["l_bias_decay"],
-                "loss": f0["l_reconstruction"] + f0["l_l1"] + f0["l_bias_decay"]}
-        for k in loss:
-            v = float(want[k])
-            w.add_scalar("loss", m, abs(float(loss[k][m]) - v) / abs(v) if v != 0 else abs(float(loss[k][m])))
-        active = torch.where(near, eng_pos, Z > 0)
-        f = oracle(variant, P, buf, Xm, active)
-        closed = near & ~eng_pos & (code[m] == 0)
-        if "coef_mask" in buf:
-            closed &= ~buf["coef_mask"].bool()
-        opened = regate_exact_zeros(variant, f, grads["encoder_bias"][m], closed)
-        kinks[-1] += (len(opened),)
-        del f0, Z, near, eng_pos
-        for k, S in scales(variant, f, P["encoder_bias"]).items():
-            w.add(k, m, T.tile_ratios(grads[k][m], f["grads"][k], S))
-        del f, active
-    return w, kinks
-
-
-def report(tag, arith, variant, w, kinks=None):
-    for name in w.tile:
-        ratio, where = w.tile[name]
-        tb, eb = BARS[arith][sign(variant)][name]
-        at = f"model {where[0]}" + (f" tile ({where[1]}, {where[2]})" if len(where) == 3 else "")
-        print(f"{tag:44s} {arith:6s} {name:12s} worst tile {ratio:.2e} at {at:24s} element max {w.elem[name]:.2e} | "
-              f"bars {tb:.1e} {eb:.1e} | smallest tile {w.minimum[name][0]:.2e} element {w.minimum[name][1]:.2e}")
-    if kinks:
-        print(f"{tag:44s} {arith:6s} kink window per model (inside, engine across inside, across outside, of, opened "
-              f"at an exact zero): {kinks}")
-
-
-def check(tag, variant, ens, X, per_model, arith):
-    w, kinks = measure(variant, ens, X, per_model)
-    report(tag, arith, variant, w, kinks)
-    for name, (ratio, where) in w.tile.items():
-        tb, eb = BARS[arith][sign(variant)][name]
-        assert ratio <= tb, (tag, name, "tile", ratio, where, tb)
-        assert w.elem[name] <= eb, (tag, name, "element", w.elem[name], eb)
-    for m, (inside, across_in, across_out, total, opened) in enumerate(kinks):
-        assert across_out == 0, (tag, m, "flipped outside the kink window", across_out)
-        assert inside <= NEAR_FRAC * total, (tag, m, inside, total)
-        assert opened <= 2 + 1e-7 * total, (tag, m, "coefficients at an exact zero", opened)
-    return w
-
-
-def run_case(tag, variant, models, sig, arith, shape, per_model, fp16_values, steps=3, seed=100, n_feats=2048):
-    M, d, n, B = shape
-    ens = ensemble(models, sig, arith)
-    X = batch(M, B, d, seed, per_model, fp16_values, n_feats)
-    check(f"{tag} init", variant, ens, X, per_model, arith)
-    assert ens.resolved_arith() == arith
-    for s in range(steps):
-        ens.step_batch(batch(M, B, d, seed + 1 + s, per_model, fp16_values, n_feats), expand_dims=not per_model)
-    check(f"{tag} step{steps}", variant, ens, batch(M, B, d, seed + 50, per_model, fp16_values, n_feats), per_model,
-          arith)
 
 
 @pytest.mark.parametrize("inputs", ["fp16", "fp32"])

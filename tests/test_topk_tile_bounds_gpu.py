@@ -55,6 +55,7 @@ decode's own rounding adds little. The whole file runs in about 30 s on an H100.
 import pytest
 import torch
 
+from engine_cases import batch, clone_models, synth
 from oracle import sae_oracle as O
 from oracle import tile_bounds as T
 from oracle.plan_paths import gather_classes, gather_slices, launch_bound, launches
@@ -83,23 +84,6 @@ CASES = {
 }
 
 
-def synth(B, d, seed, fp16_values=True, n_feats=2048):
-    """Sparse-mixture activations, generated on the device (as tests/test_tile_bounds_gpu.py)."""
-    gen = torch.Generator(device="cuda").manual_seed(seed)
-    feats = torch.randn(n_feats, d, generator=gen, device="cuda")
-    feats /= feats.norm(dim=-1, keepdim=True)
-    codes = (torch.rand(B, n_feats, generator=gen, device="cuda") < 0.01).float() * \
-        torch.rand(B, n_feats, generator=gen, device="cuda")
-    x = codes @ feats + 0.05 * torch.randn(B, d, generator=gen, device="cuda")
-    return x.half().float() if fp16_values else x
-
-
-def batch(M, B, d, seed, per_model, fp16_values):
-    if per_model:
-        return torch.stack([synth(B, d, seed + 7919 * m, fp16_values) for m in range(M)])
-    return synth(B, d, seed, fp16_values)
-
-
 def make_models(d, n, ks, seed):
     import sparse_coding_b200 as S
     torch.manual_seed(seed)
@@ -108,8 +92,7 @@ def make_models(d, n, ks, seed):
 
 def ensemble(models, arith, **kw):
     import sparse_coding_b200 as S
-    clone = [({k: v.clone() for k, v in p.items()}, {k: v.clone() for k, v in b.items()}) for p, b in models]
-    return S.FunctionalEnsemble(clone, S.TopKEncoder, S.adam, {"lr": 1e-3}, device="cuda", arith=arith,
+    return S.FunctionalEnsemble(clone_models(models), S.TopKEncoder, S.adam, {"lr": 1e-3}, device="cuda", arith=arith,
                                 no_stacking=True, **kw)
 
 

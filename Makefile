@@ -16,7 +16,7 @@ build/sce_%.o: $(CSRC)/sce_%.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h include/sce.h
 	mkdir -p build
 	$(NVCC) $(NVFLAGS) -c -o $@ $<
 
-selftest: build/gemm_selftest build/gemm_cluster_selftest
+selftest: build/gemm_selftest build/gemm_cluster_selftest build/gemm_tall_selftest
 build/gemm_selftest: tests/csrc/gemm_selftest.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
 	mkdir -p build
 	$(NVCC) $(NVFLAGS) -o $@ tests/csrc/gemm_selftest.cu
@@ -25,10 +25,14 @@ build/gemm_cluster_selftest: tests/csrc/gemm_cluster_selftest.cu $(CSRC)/*.cuh $
 	mkdir -p build
 	$(NVCC) $(NVFLAGS) -o $@ tests/csrc/gemm_cluster_selftest.cu
 
+build/gemm_tall_selftest: tests/csrc/gemm_tall_selftest.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
+	mkdir -p build
+	$(NVCC) $(NVFLAGS) -o $@ tests/csrc/gemm_tall_selftest.cu
+
 probe: build/gemm_overlap_probe
 build/gemm_overlap_probe: tools/gemm_overlap_probe.cu $(CSRC)/*.cuh $(CSRC)/sce_tmap.h
 	mkdir -p build
 	$(NVCC) $(NVFLAGS) -o $@ tools/gemm_overlap_probe.cu
 
 clean:
-	rm -f $(LIB) $(LIB_OBJS) build/gemm_selftest build/gemm_cluster_selftest build/gemm_overlap_probe
+	rm -f $(LIB) $(LIB_OBJS) build/gemm_selftest build/gemm_cluster_selftest build/gemm_tall_selftest build/gemm_overlap_probe

@@ -179,14 +179,15 @@ static bool operand_maps(OperandMaps& m, const Planes& P, uint64_t models, uint6
 
 // The weight gradient's operand P [models][k_rows][cols] (`mpitch` elements between models), reduced over its k_rows:
 // MN-major tiles of bk rows. With T, the 8-bit planes come from P's batch-major copies T [models][cols][t_pitch] instead
-// (batch_major), K-major tiles [128 rows][64 B] with the 64-byte swizzle E5M2 wgmma reads; only k_rows columns of T are
-// exposed, so the tail of a short batch reads as zero.
+// (batch_major), K-major tiles [t_rows][64 B] with the 64-byte swizzle E5M2 wgmma reads (t_rows: the tile's rows on
+// this side, kBN for B, the launch's BM for A); only k_rows columns of T are exposed, so the tail of a short batch reads
+// as zero.
 static bool dw_operand_maps(OperandMaps& m, const Planes& P, const Planes* T, uint64_t models, uint64_t k_rows,
-                            uint64_t cols, uint64_t mpitch, uint64_t t_pitch, int bk) {
+                            uint64_t cols, uint64_t mpitch, uint64_t t_pitch, int bk, uint32_t t_rows = kBM) {
   if (!T) return operand_maps(m, P, models, k_rows, cols, mpitch, bk, 0);
   return make_tmap_bf16(&m.hi, P.hi, models, k_rows, cols, cols, mpitch, bk) &&
-         make_tmap_u8_box(&m.lo, T->lo, models, cols, k_rows, t_pitch, cols * t_pitch, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B) &&
-         make_tmap_u8_box(&m.x8, T->x8, models, cols, k_rows, t_pitch, cols * t_pitch, bk, kBM, CU_TENSOR_MAP_SWIZZLE_64B);
+         make_tmap_u8_box(&m.lo, T->lo, models, cols, k_rows, t_pitch, cols * t_pitch, bk, t_rows, CU_TENSOR_MAP_SWIZZLE_64B) &&
+         make_tmap_u8_box(&m.x8, T->x8, models, cols, k_rows, t_pitch, cols * t_pitch, bk, t_rows, CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
 // device flags "this operand's residual plane is all zeros" (f16f8; GemmParams::a_res_flag), nullptr = unknown
@@ -209,8 +210,9 @@ static void set_operand_maps(GemmParams<EpiParams>& gp, int s, const OperandMaps
 // a_batched / b_batched of the operand sets that hold one slab per model
 static const int kOnes[2] = {1, 1};
 
-// One GEMM over `n_models` models on `device` (with `sms` SMs), launched and counted by L
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool NATIVE>
+// One GEMM over `n_models` models on `device` (with `sms` SMs) on output tiles of BM rows (kBMTall: the maps' A boxes
+// must be that tall), launched and counted by L
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool NATIVE, int BM = kBM>
 static int launch_gemm_t(Launcher& L, int n_models, int device, int sms, const GemmMaps& maps, int nsets,
                          const int* a_batched, const int* b_batched, int k_total, int passes, int m_total, int n_total,
                          const typename Epi::Params& epi, const ResFlags& rf = ResFlags()) {
@@ -229,10 +231,10 @@ static int launch_gemm_t(Launcher& L, int n_models, int device, int sms, const G
   gp.n_models = n_models;
   gp.m_total = m_total;
   gp.n_total = n_total;
-  gp.tiles_m = (m_total + kBM - 1) / kBM;
+  gp.tiles_m = gemm_tiles_m<BM>(m_total);
   gp.tiles_n = (n_total + kBN - 1) / kBN;
   gp.epi = epi;
-  CUDA_TRY((launch_gemm<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, NATIVE>(gp, device, sms, L.st)));
+  CUDA_TRY((launch_gemm<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, NATIVE, BM>(gp, device, sms, L.st)));
   ++L.count;
   return SCE_OK;
 }
@@ -240,11 +242,15 @@ static int launch_gemm_t(Launcher& L, int n_models, int device, int sms, const G
 // The weight gradient's GEMM (launch_gemm_t's arguments after L): a reduction over rows, both operands as
 // dw_operand_maps builds them, fp32 out. bf16x3 keeps split accumulators (f16f8 rescales inside one). `native` (f16f8,
 // 8-bit planes from batch-major copies): the cross terms run on E5M2 wgmma; else the 8-bit tiles are widened to fp16.
+// `tall` (native only): on kBMTall-row tiles, from maps whose A-side 8-bit boxes are that tall.
 template <int AR, class... A>
-static int launch_dw_t(Launcher& L, bool native, const A&... args) {
+static int launch_dw_t(Launcher& L, bool native, bool tall, const A&... args) {
   constexpr bool f8 = AR == kArithF16F8;
   if constexpr (f8)
-    if (native) return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, args...);
+    if (native) {
+      if (tall) return launch_gemm_t<EpiStoreF32, true, true, false, AR, true, kBMTall>(L, args...);
+      return launch_gemm_t<EpiStoreF32, true, true, false, AR, true>(L, args...);
+    }
   return launch_gemm_t<EpiStoreF32, true, true, !f8, AR, false>(L, args...);
 }
 

@@ -44,6 +44,12 @@ constexpr int kEpiWarps = 8;    // epilogue shares of a tile (warp quarter x col
 // (the launch count of 128 per thread at 512 threads). In-line launches run 384 threads without setmaxnreg.
 constexpr int kProducerRegs = 40, kConsumerRegs = 168, kEpilogueRegs = 136;
 static_assert(kProducerRegs + 2 * kConsumerRegs + kEpilogueRegs == 65536 / 128, "register split of the four warpgroups");
+// Tall tiles (BM = kBMTall, see gemm_split_kernel): 512 threads, a producer warpgroup and three consumer warpgroups. A
+// native f16f8 consumer holds acc[64] and accx[64] and compiles to about 153 registers, so a fourth consumer warpgroup
+// (256 rows) would leave it 122 and spill; three fit at 160.
+constexpr int kBMTall = 192;
+constexpr int kTallProducerRegs = 32, kTallConsumerRegs = 160;
+static_assert(kTallProducerRegs + 3 * kTallConsumerRegs <= 65536 / 128, "register split of the tall-tile warpgroups");
 constexpr int kMaxSets = 2;
 constexpr int kSmemLimit = 232448;  // 227 KB of shared memory one CTA may use on sm_90
 
@@ -104,10 +110,12 @@ __host__ __device__ constexpr int gemm_bk(int arith) { return arith == kArithF16
 constexpr int align1k(int v) { return (v + 1023) / 1024 * 1024; }
 
 // Shared memory of one CTA. F8_NATIVE (f16f8): the cross terms run on E5M2 wgmma from the stage, nothing is widened.
-template <int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE>
+// BM: rows of the output tile. The accumulator tile holds kBM rows either way (a tall tile's epilogue runs in two
+// rounds through it), so at BM = kBMTall four 40 KB stages fill the 227 KB exactly.
+template <int EPI_WARP_BYTES, int ARITH, bool F8_NATIVE, int BM = kBM>
 struct GemmSmem {
   static constexpr int kBK = gemm_bk(ARITH);
-  static constexpr int kATile = kBM * kBK * 2;   // bytes of one 16-bit A tile
+  static constexpr int kATile = BM * kBK * 2;   // bytes of one 16-bit A tile
   static constexpr int kBTile = kBN * kBK * 2;
   // bf16x3: hi and lo planes of A and B. f16f8: either the fp16 planes or the four 8-bit planes (same bytes).
   static constexpr int kStage = ARITH == kArithBf16x3 ? 2 * kATile + 2 * kBTile : kATile + kBTile;
@@ -152,9 +160,16 @@ template <class Epi, int ARITH, bool F8_NATIVE>
 __host__ __device__ constexpr bool gemm_overlap() {
   return (ARITH != kArithF16F8 || F8_NATIVE) && !epi_inline<Epi>::value;
 }
-template <class Epi, int ARITH, bool F8_NATIVE>
+template <class Epi, int ARITH, bool F8_NATIVE, int BM = kBM>
 __host__ __device__ constexpr int gemm_threads() {
-  return gemm_overlap<Epi, ARITH, F8_NATIVE>() ? 512 : 384;
+  return gemm_overlap<Epi, ARITH, F8_NATIVE>() || BM == kBMTall ? 512 : 384;
+}
+
+// Output-tile rows of the GEMM's launch over m_total rows. Tall tiles cover at least the rows of the kBM tiling, so that
+// every epilogue share of that tiling (whose slots the epilogues fill, rows beyond m_total included) is run.
+template <int BM>
+__host__ __device__ constexpr int gemm_tiles_m(int m_total) {
+  return ((m_total + kBM - 1) / kBM * kBM + BM - 1) / BM;
 }
 
 // f16f8 without F8_NATIVE (MN-major operands): an MN-major 8-bit tile as TMA delivers it without swizzle, [BK][ROWS]
@@ -197,8 +212,17 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
 //
 // CLUSTER (1 or 2): the CTAs of the launch run in clusters of that many along N, sharing each A tile (see the top of the
 // file). A compile-time value, so that a launch in clusters of one runs the kernel without any of the pairing.
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int CLUSTER>
-__global__ void __launch_bounds__(gemm_threads<Epi, ARITH, F8_NATIVE>(), 1)
+//
+// BM (kBM or kBMTall): rows of the output tile. Tall tiles (192 rows) read (96 + 128) operand elements per k for 192 x
+// 128 outputs in pairs, against (64 + 128) for 128 x 128: 22 % fewer L2 bytes per MMA, for GEMMs whose main loop is
+// fed from L2 rather than bound by the tensor pipe (decode and the weight gradient). Only for in-line epilogues on the
+// native f16f8 path: 512 threads, the producer warpgroup and three consumer warpgroups of 64 rows each (setmaxnreg
+// kTallProducerRegs / kTallConsumerRegs). The epilogue runs in two rounds through the kBM-row acc_stage: rows 0..127
+// from consumers 0 and 1, then rows 128..191 from consumer 2 (while 0 and 1 start the next tile). Every share keeps the
+// TileCoord of the kBM tiling (m_blk = row / kBM, warp_q = row % kBM / 32), and each output's accumulation order
+// depends on the K sweep only, so the outputs are bitwise those of BM = kBM.
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int CLUSTER, int BM = kBM>
+__global__ void __launch_bounds__(gemm_threads<Epi, ARITH, F8_NATIVE, BM>(), 1)
 gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   constexpr bool F8 = ARITH == kArithF16F8;
   constexpr int BN = kBN;
@@ -208,7 +232,12 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   static_assert(!F8 || F8_NATIVE || (A_MN && B_MN), "the widened f16f8 path is MN-major on both sides");
   static_assert(CLUSTER == 1 || CLUSTER == 2, "clusters of one or two CTAs");
   static_assert(CLUSTER == 1 || !F8 || F8_NATIVE, "the widened f16f8 path runs in clusters of one");
-  using SM = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>;
+  constexpr bool TALL = BM == kBMTall;
+  static_assert(BM == kBM || TALL, "tiles of 128 or 192 rows");
+  static_assert(!TALL || (F8_NATIVE && epi_inline<Epi>::value && Epi::kWarpStageBytes == 0),
+                "tall tiles: native f16f8, in-line epilogues without staging");
+  constexpr int kWGs = BM / 64;   // consumer warpgroups
+  using SM = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE, BM>;
   constexpr int BK = SM::kBK;
   constexpr int STAGES = SM::kStages;
   constexpr int EC = Epi::kCols;  // accumulator columns handed to the epilogue per call
@@ -267,7 +296,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2 * CLUSTER);   // one arrival per consumer warpgroup of each CTA of the cluster
+      mbar_init(&empty_bar[s], kWGs * CLUSTER);   // one arrival per consumer warpgroup of each CTA of the cluster
     }
     if constexpr (OVERLAP) {
       mbar_init(acc_full, 256);      // every consumer thread, after its accumulators are in acc_stage
@@ -305,12 +334,17 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
     tc.alternate = alternate;
     return tc;
   };
+  // Tall tiles: the share of the tile's rows 32 q .. +31 (q = 0..5) under the kBM tiling's coordinates
+  [[maybe_unused]] auto tall_share_coord = [&](int model, int tile_m, int tile_n, int q, int grp) {
+    const int quarter = tile_m * (BM / 32) + q;   // 32-row quarter of the output rows
+    return share_coord(model, quarter >> 2, tile_n, quarter & 3, grp, false);
+  };
   auto share_staging = [&](int warp_q, int grp) { return smem + SM::kEpiOff + (grp * 4 + warp_q) * Epi::kWarpStageBytes; };
   constexpr int kChunks = BN / EC;
   static_assert(kChunks % 2 == 0, "the two column groups alternate chunks");
-  // chunk c of this thread's row of acc_stage
-  auto read_chunk = [&](int warp_q, int c, uint32_t (&r)[EC]) {
-    const float* src = acc_stage + (warp_q * 32 + lane) * SM::kAccLd + c * EC;
+  // chunk c of this thread's row of acc_stage, in its rows 32 q .. +31
+  auto read_chunk = [&](int q, int c, uint32_t (&r)[EC]) {
+    const float* src = acc_stage + (q * 32 + lane) * SM::kAccLd + c * EC;
 #pragma unroll
     for (int j = 0; j < EC; ++j) r[j] = __float_as_uint(src[j]);
   };
@@ -318,6 +352,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   if (warp < 4) {
     // ======================= TMA producer =======================
     if constexpr (OVERLAP) reg_dealloc<kProducerRegs>();
+    if constexpr (TALL) reg_dealloc<kTallProducerRegs>();
     if (threadIdx.x == 0) {
       const uint32_t stage_bytes = (three && !F8) ? uint32_t(SM::kStage) : uint32_t(SM::kATile + SM::kBTile);
       int stage = 0;
@@ -338,7 +373,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int model, tile_m, tile_n;
         decode_tile(tile, model, tile_m, tile_n);
-        const int a_row0 = tile_m * kBM, b_row0 = tile_n * BN;
+        const int a_row0 = tile_m * BM, b_row0 = tile_n * BN;
         if constexpr (F8) {
           // sweep 1: the 8-bit planes (skipped for passes == 1); sweep 2: the fp16 planes
           for (int sweep = three ? 0 : 1; sweep < 2; ++sweep)
@@ -361,7 +396,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
                   if constexpr (!A_MN) load_a(sa, &p.a_hi[set], bar, k0, a_row0, am, kb);
                   else {
 #pragma unroll
-                    for (int j = 0; j < kBM / 64; ++j) load_a(sa + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am, kb);
+                    for (int j = 0; j < BM / 64; ++j) load_a(sa + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am, kb);
                   }
                   if constexpr (!B_MN) tma_load_3d(sb, &p.b_hi[set], bar, k0, b_row0, bm);
                   else {
@@ -403,7 +438,7 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
                 if (three) load_a(sa_lo, &p.a_lo[set], bar, k0, a_row0, am, kb);
               } else {
 #pragma unroll
-                for (int j = 0; j < kBM / 64; ++j) {
+                for (int j = 0; j < BM / 64; ++j) {
                   load_a(sa_hi + j * (BK * 128), &p.a_hi[set], bar, a_row0 + j * 64, k0, am, kb);
                   if (three) load_a(sa_lo + j * (BK * 128), &p.a_lo[set], bar, a_row0 + j * 64, k0, am, kb);
                 }
@@ -427,7 +462,8 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
   } else if (!OVERLAP || warp < 12) {
     // ======================= wgmma consumers (+ the epilogue where !OVERLAP) =======================
     if constexpr (OVERLAP) reg_alloc<kConsumerRegs>();
-    const int ctid = threadIdx.x - 128;      // 0..255
+    if constexpr (TALL) reg_alloc<kTallConsumerRegs>();
+    const int ctid = threadIdx.x - 128;      // 0..255 (tall tiles: 0..383)
     const int wg = ctid >> 7;                // rows 64 wg .. +63 of the tile
     const int wl = ctid & 127;               // thread within the warpgroup
     auto consumer_sync = [] { named_sync(1, 256); };
@@ -582,6 +618,44 @@ gemm_split_kernel(const __grid_constant__ GemmParams<typename Epi::Params> p) {
         }
       }
 
+      if constexpr (TALL) {
+        // ---- epilogue in two rounds through acc_stage: rows 0..127 of the tile from consumers 0 and 1 (eight warps, warp w
+        // plays quarter w % 4, group w / 4, as in line below), then rows 128..191 from consumer 2 (warp w: quarter 4 + w % 2,
+        // group w / 2) in acc_stage rows 0..63. Named barriers: kBarRound1Read (0, 1 -> 2: round 1 read, acc_stage free
+        // for round 2), kBarRound2Read (2 -> 0, 1: round 2 read, free for the next tile's round 1; 0 and 1 run the next
+        // main loop meanwhile), kBarRound1Full / kBarRound2Full (written -> read, within each round).
+        constexpr uint32_t kBarRound1Full = 2, kBarRound2Full = 3, kBarRound1Read = 4, kBarRound2Read = 5;
+        const bool round2 = wg == 2;
+        if (round2) named_sync(kBarRound1Read, 384);
+        else if (tile != int(blockIdx.x)) named_sync(kBarRound2Read, 384);
+        {
+          const int w = wl >> 5, l = wl & 31;
+          const int r0 = (wg & 1) * 64 + w * 16 + (l >> 2);
+#pragma unroll
+          for (int i = 0; i < 64; ++i) {
+            const int row = r0 + 8 * ((i >> 1) & 1);
+            const int col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+            acc_stage[row * SM::kAccLd + col] = acc[i];
+          }
+        }
+        if (round2) named_sync(kBarRound2Full, 128);
+        else named_sync(kBarRound1Full, 256);
+        const int cw = (ctid >> 5) & 7;
+        const int sq = round2 ? cw & 1 : cw & 3;        // quarter of acc_stage
+        const int grp = round2 ? cw >> 1 : cw >> 2;
+        const TileCoord tc = tall_share_coord(model, tile_m, tile_n, round2 ? 4 + sq : sq, grp);
+        Epi epi(p.epi, tc, p.m_total, p.n_total, nullptr);
+#pragma unroll 1
+        for (int c = grp; c < kChunks; c += 2) {
+          uint32_t r[EC];
+          read_chunk(sq, c, r);
+          epi.chunk(c * EC, r);
+        }
+        epi.finish();
+        if (!round2) named_arrive(kBarRound1Read, 384);
+        else if (tile + int(gridDim.x) < num_tiles) named_arrive(kBarRound2Read, 384);
+        continue;
+      }
       // ---- accumulators -> padded fp32 tile (row-per-thread view for the epilogue)
       // OVERLAP: the epilogue warpgroup has read the previous tile (it ran under this tile's main loop). Otherwise both
       // consumer warpgroups are past their previous epilogue and the widened tiles.
@@ -701,13 +775,15 @@ inline int gemm_cluster_size(int tiles_n, int k_blocks, bool widened) {
 
 // Launches gemm_split_kernel<..., CLUSTER> on `st` as a persistent grid of clusters of CLUSTER CTAs (2 only where
 // p.tiles_n is even): one cluster per column group of CLUSTER tiles, at most as many as are resident at once, and at
-// most one CTA per SM (`sms` of them on `device`, the current device).
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int CLUSTER>
+// most one CTA per SM (`sms` of them on `device`, the current device). BM: rows of the output tile; p.tiles_m must be
+// gemm_tiles_m<BM>(p.m_total).
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int CLUSTER, int BM = kBM>
 cudaError_t launch_gemm_cluster_t(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st) {
-  constexpr auto kern = gemm_split_kernel<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, CLUSTER>;
-  constexpr int bytes = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE>::kBytes;
-  constexpr int threads = gemm_threads<Epi, ARITH, F8_NATIVE>();
+  constexpr auto kern = gemm_split_kernel<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, CLUSTER, BM>;
+  constexpr int bytes = GemmSmem<Epi::kWarpStageBytes, ARITH, F8_NATIVE, BM>::kBytes;
+  constexpr int threads = gemm_threads<Epi, ARITH, F8_NATIVE, BM>();
   if (p.tiles_n % CLUSTER != 0) return cudaErrorInvalidValue;
+  if (BM != kBM && p.tiles_m != gemm_tiles_m<BM>(p.m_total)) return cudaErrorInvalidValue;
   cudaError_t e = opt_in_smem<kern>(bytes, device);
   if (e != cudaSuccess) return e;
   long long slots = sms / CLUSTER;
@@ -734,12 +810,12 @@ cudaError_t launch_gemm_cluster_t(const GemmParams<typename Epi::Params>& p, int
 }
 
 // The same with the cluster size given at run time (1 or 2; always 1 on the widened f16f8 path).
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int BM = kBM>
 cudaError_t launch_gemm_clusters(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st,
                                  int cluster) {
-  if (cluster == 1) return launch_gemm_cluster_t<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, 1>(p, device, sms, st);
+  if (cluster == 1) return launch_gemm_cluster_t<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, 1, BM>(p, device, sms, st);
   if constexpr (ARITH != kArithF16F8 || F8_NATIVE) {
-    if (cluster == 2) return launch_gemm_cluster_t<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, 2>(p, device, sms, st);
+    if (cluster == 2) return launch_gemm_cluster_t<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, 2, BM>(p, device, sms, st);
   }
   return cudaErrorInvalidValue;
 }
@@ -752,10 +828,10 @@ inline int gemm_launch_cluster(const GemmParams<EpiParams>& p) {
 }
 
 // Launches gemm_split_kernel in the cluster size that p's shape and path take.
-template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE>
+template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int ARITH, bool F8_NATIVE, int BM = kBM>
 cudaError_t launch_gemm(const GemmParams<typename Epi::Params>& p, int device, int sms, cudaStream_t st) {
-  return launch_gemm_clusters<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE>(p, device, sms, st,
-                                                                            gemm_launch_cluster<ARITH, F8_NATIVE>(p));
+  return launch_gemm_clusters<Epi, A_MN, B_MN, SPLIT_ACC, ARITH, F8_NATIVE, BM>(p, device, sms, st,
+                                                                                gemm_launch_cluster<ARITH, F8_NATIVE>(p));
 }
 
 // ------------------------------------------------------------------------------------------------

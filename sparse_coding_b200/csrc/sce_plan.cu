@@ -356,6 +356,11 @@ PlanConfig plan_config(const sce_desc& d) {
   // the 8-bit tiles. Nor do launch-bound plans: there the weight gradient takes microseconds either way, and the copies
   // would add a launch per step (x's transpose pass) and a third to the workspace.
   c.dw_native = c.arith == kArithF16F8 && !c.topk && d.bwd_passes >= 3 && !launch_bound;
+  // The same plans run decode and the native weight gradient on 192-row tiles (kBMTall, sce_gemm.cuh): both have long
+  // K loops fed from L2, and a taller tile reads 22 % fewer operand bytes per MMA. Encode and dcode overlap their
+  // epilogue, which leaves no registers for a third consumer warpgroup; the widened weight gradient, bf16x3, top-k and
+  // launch-bound plans keep 128-row tiles.
+  c.tall_tiles = c.dw_native;
   // The truncation bias of a single accumulation chain grows with the reduction length; n > 4096 splits the decode
   // GEMM's cross terms into their own accumulator (config 5's width, n = 32768, needs it for the 1e-4 bar; the parity
   // tests cover both sides). Splitting doubles the decode GEMM's accumulator registers, so it is used where needed.
@@ -480,22 +485,25 @@ static int build_maps(sce_plan* p, int B, BatchMaps** out) {
     ok &= operand_maps(m->center.b[0], p->rot, M, dd, dd, dd * dd, kBN, bk);
   }
   // decode: A = c [M,B,n] K-major, B = Wdec [M,n,d] MN-major (bk k-rows per box); f16f8: its transposed copy [M,d,n] K-major
-  ok &= act_a(m->decode.a[0], p->c, M, n);
+  ok &= cfg.tall_tiles ? operand_maps(m->decode.a[0], p->c, M, (uint64_t)B, n, Bm * n, kBMTall, bk)
+                        : act_a(m->decode.a[0], p->c, M, n);
   ok &= f8 ? operand_maps(m->decode.b[0], p->wdt, M, dd, n, dd * n, kBN, bk) : dict_b(m->decode.b[0], p->wdec, bk, 0);
   // dcode: A = g [M,B,d] K-major, B = Wdec K-major
   ok &= act_a(m->dcode.a[0], p->g, M, dd);
   ok &= dict_b(m->dcode.b[0], p->wdec, kBN, bk);
   // weight gradients: reduction over the batch rows; dw_native: the 8-bit planes from the batch-major copies [models][cols][Bp]
   const uint64_t Bp = (uint64_t)cfg.bpad;
-  auto dw_operand = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t models, uint64_t cols) {
-    return dw_operand_maps(o, P, cfg.dw_native ? &T : nullptr, models, (uint64_t)B, cols, Bm * cols, Bp, bk);
+  // (t_rows: the tile's rows on this side, the launch's BM for A)
+  auto dw_operand = [&](OperandMaps& o, const Planes& P, const Planes& T, uint64_t models, uint64_t cols, uint32_t t_rows) {
+    return dw_operand_maps(o, P, cfg.dw_native ? &T : nullptr, models, (uint64_t)B, cols, Bm * cols, Bp, bk, t_rows);
   };
+  const uint32_t dw_bm = cfg.tall_tiles ? kBMTall : kBM;
   // dz^T x, then c^T g: a second GEMM of the decoder (untied) or a second operand set of the one dictionary's
   // (dz's own 8-bit planes are batch-major in dw_native plans)
   GemmMaps& cg = cfg.untied ? m->dw_dec : m->dw_enc;
   const int cg_set = cfg.untied ? 0 : 1;
-  ok &= dw_operand(m->dw_enc.a[0], p->dz, p->dz, M, n) && dw_operand(m->dw_enc.b[0], p->x, p->xt, xm, dd);
-  ok &= dw_operand(cg.a[cg_set], p->c, p->ct, M, n) && dw_operand(cg.b[cg_set], p->g, p->gt, M, dd);
+  ok &= dw_operand(m->dw_enc.a[0], p->dz, p->dz, M, n, dw_bm) && dw_operand(m->dw_enc.b[0], p->x, p->xt, xm, dd, kBN);
+  ok &= dw_operand(cg.a[cg_set], p->c, p->ct, M, n, dw_bm) && dw_operand(cg.b[cg_set], p->g, p->gt, M, dd, kBN);
   ok &= make_tmap_bf16_store32(&m->st_c.hi, p->c.hi, M, (uint64_t)B, n, Bm * n);
   ok &= make_tmap_bf16_store32(&m->st_dz.hi, p->dz.hi, M, (uint64_t)B, n, Bm * n);
   if (f8) {
@@ -786,8 +794,11 @@ static int decode_phase(PlanCall& c, const float* x, float* x_hat, bool backward
       dp.t_x8 = p->gt.x8;
       dp.t_ld = cfg.bpad;
     }
-    if constexpr (f8)
+    if constexpr (f8) {
+      if (cfg.tall_tiles)
+        return c.gemm<E, false, false, false, AR, true, kBMTall>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
       return c.gemm<E, false, false, false, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
+    }
     else if (cfg.split_decode)
       return c.gemm<E, false, true, true, AR>(c.maps->decode, 1, kOnes, kOnes, n, d.fwd_passes, B, dd, dp);
     else
@@ -862,7 +873,7 @@ static int backward_phase(PlanCall& c) {
     sp.model_stride = (long long)n * dd;
     sp.ld = dd;
     sp.scale = grad_out_scale(p, B);
-    return launch_dw_t<AR>(c, cfg.dw_native, M, p->device, p->sms, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
+    return launch_dw_t<AR>(c, cfg.dw_native, cfg.tall_tiles, M, p->device, p->sms, gm, nsets, ab, bb, B, d.bwd_passes, n, dd, sp, rf);
   };
   ResFlags x_is_b;   // the batch's residual-plane flag, for the GEMM that reads x as its B operand (set 0)
   if constexpr (f8) x_is_b.b[0] = p->res_flags;

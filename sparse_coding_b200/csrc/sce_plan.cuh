@@ -104,6 +104,7 @@ struct PlanConfig {
   int tk_slices;       // slices of the activation width topk_sparse_kernel runs per row (0: none fits)
   bool topk_sparse;    // decode / dcode of the top-k variant run as the k-sparse gather kernels
   bool dw_native;      // the weight gradient's cross terms run on E5M2 wgmma from batch-major copies (carve)
+  bool tall_tiles;     // decode and the native weight gradient run on kBMTall-row output tiles (f16f8, see plan_config)
   bool split_decode;   // separate accumulators for hi*hi and the cross terms in the decode GEMM (bf16x3)
   bool use_graph;      // replay the step as a CUDA graph
   bool nonneg;         // desc.encoder_nonneg: the dictionary rows are built from max(E, 0) (dict_rows_kernel<..., true>)
@@ -140,9 +141,11 @@ struct PlanCall : Launcher {
   // one GEMM of the plan. NATIVE (f16f8): the cross terms run on E5M2 wgmma, which needs K-major 8-bit maps (A_MN / B_MN
   // then describe the fp16 planes alone); K-major GEMMs always have them, the weight gradient where the plan keeps
   // batch-major copies.
-  template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int AR, bool NATIVE = AR == kArithF16F8 && !A_MN, class... A>
+  // BM: rows of the output tile (kBMTall where the plan takes tall tiles and the maps are built for them).
+  template <class Epi, bool A_MN, bool B_MN, bool SPLIT_ACC, int AR, bool NATIVE = AR == kArithF16F8 && !A_MN, int BM = kBM,
+            class... A>
   int gemm(const A&... args) {
-    return launch_gemm_t<Epi, A_MN, B_MN, SPLIT_ACC, AR, NATIVE>(*this, p->d.n_models, p->device, p->sms, args...);
+    return launch_gemm_t<Epi, A_MN, B_MN, SPLIT_ACC, AR, NATIVE, BM>(*this, p->d.n_models, p->device, p->sms, args...);
   }
   // with sce_profile_begin: the event at the start of phase `idx` of this step (SCE_PHASE_COUNT: the step's end)
   void mark(int idx) {

@@ -25,6 +25,11 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// arrives on named barrier `id` without waiting: the threads that named_sync on it (count in all) go on once the
+// arrivals are in, and see this thread's memory accesses from before the arrival
+__device__ __forceinline__ void named_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // setmaxnreg: sets the per-thread register count of the executing warpgroup to N (a multiple of 8 in 24..256). Every
 // thread of the warpgroup executes it. `dec` hands registers back to the CTA's pool; `inc` waits until the pool has

@@ -285,7 +285,7 @@ static int sliced_gemm_t(Launcher& L, const Slices& sl, const Planes& A, const P
   sp.model_stride = (long long)m * d;
   sp.ld = d;
   sp.scale = 1.f;
-  return launch_dw_t<AR>(L, f8, S, device, sms, maps, 1, kOnes, kOnes, R, 3, m, d, sp);
+  return launch_dw_t<AR>(L, f8, false, S, device, sms, maps, 1, kOnes, kOnes, R, 3, m, d, sp);
 }
 
 template <int AR>

@@ -9,7 +9,8 @@
 // CTAs along N share each A tile by multicast) or 0 (the size launch_gemm takes, as libsce launches it: 2 for decode and
 // the weight gradient, 1 for encode and dcode). Without sizes, 0. Each JSON line names the size run ("cluster") and the
 // size launch_gemm takes ("engine_cluster"). tools/gemm_overlap_probe.py reads them from stdout. Build: Makefile target
-// `probe`.
+// `probe`. Decode and the weight gradient also run on tall tiles (192 rows, BM = kBMTall) at each size, right after the
+// 128-row tiles; each JSON line names its tile height ("bm").
 //
 //   build/gemm_overlap_probe [reps] [cluster sizes ...]
 #include <cstdio>
@@ -76,18 +77,26 @@ static void* plane(size_t bytes, int elem) {
   return d;
 }
 
+// The planes of one operand [models][rows][K]: fp16, value-e5m2 and residual-e5m2, filled with hashed values
+struct Planes3 {
+  void *hi, *lo, *x8;
+};
+static Planes3 planes(int models, int rows, int K) {
+  const size_t n = (size_t)models * rows * K;
+  return {plane(2 * n, 2), plane(n, 1), plane(n, 1)};
+}
+
 // The maps of one operand [models][rows][K]: the fp16 plane K-major (box rows x 64, 128-byte swizzle) or MN-major
 // ([models][K][rows], boxes 64 x 64); the two 8-bit planes always K-major (64-byte swizzle), as the native cross terms
 // read them (the weight gradient's are the batch-major copies).
-static void operand(int models, int rows, int K, bool mn, uint32_t box_rows, CUtensorMap* hi, CUtensorMap* lo,
-                    CUtensorMap* x8) {
+static void operand(const Planes3& P, int models, int rows, int K, bool mn, uint32_t box_rows, CUtensorMap* hi,
+                    CUtensorMap* lo, CUtensorMap* x8) {
   constexpr int BK = gemm_bk(kArithF16F8);
-  const size_t n = (size_t)models * rows * K;
-  bool ok = mn ? make_tmap_bf16(hi, plane(2 * n, 2), models, K, rows, rows, (uint64_t)K * rows, BK)
-               : make_tmap_bf16_box(hi, plane(2 * n, 2), models, rows, K, K, (uint64_t)rows * K, BK, box_rows,
+  bool ok = mn ? make_tmap_bf16(hi, P.hi, models, K, rows, rows, (uint64_t)K * rows, BK)
+               : make_tmap_bf16_box(hi, P.hi, models, rows, K, K, (uint64_t)rows * K, BK, box_rows,
                                     CU_TENSOR_MAP_SWIZZLE_128B);
-  ok &= make_tmap_u8_box(lo, plane(n, 1), models, rows, K, K, (uint64_t)rows * K, BK, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
-  ok &= make_tmap_u8_box(x8, plane(n, 1), models, rows, K, K, (uint64_t)rows * K, BK, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
+  ok &= make_tmap_u8_box(lo, P.lo, models, rows, K, K, (uint64_t)rows * K, BK, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
+  ok &= make_tmap_u8_box(x8, P.x8, models, rows, K, K, (uint64_t)rows * K, BK, box_rows, CU_TENSOR_MAP_SWIZZLE_64B);
   if (!ok) {
     printf("tensor map encode failed\n");
     exit(2);
@@ -101,16 +110,16 @@ struct Shape {
   bool a0_exact;   // set 0's A operand (x) is fp16-exact
 };
 
-template <int STAGE_BYTES, bool INLINE, bool MN, bool NATIVE>
-static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32_t* sink, int reps,
-                const std::vector<int>& clusters) {
-  using Epi = EpiNoop<STAGE_BYTES, INLINE>;
+// The GEMM's parameters for output tiles of BM rows, on operand planes pa / pb per set
+template <class Epi, int BM>
+static GemmParams<typename Epi::Params> params(const Shape& s, int models, bool mn, const Planes3* pa, const Planes3* pb,
+                                               uint32_t* zero_flag, uint32_t* sink) {
   GemmParams<typename Epi::Params> p;
   memset(&p, 0, sizeof(p));
   for (int set = 0; set < s.nsets; ++set) {
     const int bm = set == 0 ? s.b_models : models;   // the weight gradient's second set (c^T g) is per model on both sides
-    operand(s.a_models, s.M, s.K, MN, kBM, &p.a_hi[set], &p.a_lo[set], &p.a_x8[set]);
-    operand(bm, s.N, s.K, MN, kBN, &p.b_hi[set], &p.b_lo[set], &p.b_x8[set]);
+    operand(pa[set], s.a_models, s.M, s.K, mn, BM, &p.a_hi[set], &p.a_lo[set], &p.a_x8[set]);
+    operand(pb[set], bm, s.N, s.K, mn, kBN, &p.b_hi[set], &p.b_lo[set], &p.b_x8[set]);
     p.a_batched[set] = s.a_models > 1;
     p.b_batched[set] = bm > 1;
   }
@@ -122,16 +131,31 @@ static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32
   p.n_models = models;
   p.m_total = s.M;
   p.n_total = s.N;
-  p.tiles_m = (s.M + kBM - 1) / kBM;
+  p.tiles_m = gemm_tiles_m<BM>(s.M);
   p.tiles_n = (s.N + kBN - 1) / kBN;
   p.epi.sink = sink;
+  return p;
+}
+
+// Times the GEMM at each asked cluster size; TALL: at each, also with tall tiles (BM = kBMTall) right after the kBM
+// tiles, on the same operands, so that the two alternate in the session
+template <int STAGE_BYTES, bool INLINE, bool MN, bool NATIVE, bool TALL = false>
+static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32_t* sink, int reps,
+                const std::vector<int>& clusters) {
+  using Epi = EpiNoop<STAGE_BYTES, INLINE>;
+  Planes3 pa[kMaxSets], pb[kMaxSets];
+  for (int set = 0; set < s.nsets; ++set) {
+    pa[set] = planes(s.a_models, s.M, s.K);
+    pb[set] = planes(set == 0 ? s.b_models : models, s.N, s.K);
+  }
+  const auto p = params<Epi, kBM>(s, models, MN, pa, pb, zero_flag, sink);
+  const auto pt = params<Epi, kBMTall>(s, models, MN, pa, pb, zero_flag, sink);
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
   const int engine_cluster = gemm_launch_cluster<kArithF16F8, NATIVE>(p);
-  for (int asked : clusters) {
-    const int cluster = asked == 0 ? engine_cluster : asked;
-    auto launch = [&] { return launch_gemm_clusters<Epi, MN, MN, false, kArithF16F8, NATIVE>(p, 0, sms, 0, cluster); };
+  // resident(): the clusters resident at once, asked after the launches have opted the kernel in to its shared memory
+  auto time = [&](int bm, int cluster, auto launch, int tiles, int stages, auto resident) {
     for (int rep = 0; rep < 3; ++rep) CK(launch());
     CK(cudaEventRecord(e0));
     for (int rep = 0; rep < reps; ++rep) CK(launch());
@@ -140,13 +164,32 @@ static void run(const Shape& s, int models, int sms, uint32_t* zero_flag, uint32
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, e0, e1));
     const double flops = 2.0 * models * s.M * s.N * (double)s.K * s.nsets;
-    constexpr auto kern2 = gemm_split_kernel<Epi, MN, MN, false, kArithF16F8, NATIVE, 2>;
-    const int resident = cluster == 1 ? sms : max_active_clusters<kern2>(2, gemm_threads<Epi, kArithF16F8, NATIVE>(),
-                                                                         GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE>::kBytes, 0);
-    printf("{\"gemm\": \"%s\", \"cluster\": %d, \"engine_cluster\": %d, \"resident_clusters\": %d, \"main_loop_ms\": "
-           "%.4f, \"tiles\": %d, \"stages\": %d, \"reps\": %d, \"tflops\": %.1f}\n",
-           s.name, cluster, engine_cluster, resident, ms / reps, models * p.tiles_m * p.tiles_n, GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE>::kStages,
-           reps, flops / (ms / reps) * 1e-9);
+    printf("{\"gemm\": \"%s\", \"bm\": %d, \"cluster\": %d, \"engine_cluster\": %d, \"resident_clusters\": %d, "
+           "\"main_loop_ms\": %.4f, \"tiles\": %d, \"stages\": %d, \"reps\": %d, \"tflops\": %.1f}\n",
+           s.name, bm, cluster, engine_cluster, resident(), ms / reps, tiles, stages, reps, flops / (ms / reps) * 1e-9);
+  };
+  for (int asked : clusters) {
+    const int cluster = asked == 0 ? engine_cluster : asked;
+    {
+      using SM = GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE>;
+      constexpr auto kern2 = gemm_split_kernel<Epi, MN, MN, false, kArithF16F8, NATIVE, 2>;
+      auto resident = [&] {
+        return cluster == 1 ? sms : max_active_clusters<kern2>(2, gemm_threads<Epi, kArithF16F8, NATIVE>(), SM::kBytes, 0);
+      };
+      time(kBM, cluster, [&] { return launch_gemm_clusters<Epi, MN, MN, false, kArithF16F8, NATIVE>(p, 0, sms, 0, cluster); },
+           models * p.tiles_m * p.tiles_n, SM::kStages, resident);
+    }
+    if constexpr (TALL) {
+      using SM = GemmSmem<STAGE_BYTES, kArithF16F8, NATIVE, kBMTall>;
+      constexpr auto kern2 = gemm_split_kernel<Epi, MN, MN, false, kArithF16F8, NATIVE, 2, kBMTall>;
+      auto resident = [&] {
+        return cluster == 1 ? sms
+                            : max_active_clusters<kern2>(2, gemm_threads<Epi, kArithF16F8, NATIVE, kBMTall>(), SM::kBytes, 0);
+      };
+      time(kBMTall, cluster,
+           [&] { return launch_gemm_clusters<Epi, MN, MN, false, kArithF16F8, NATIVE, kBMTall>(pt, 0, sms, 0, cluster); },
+           models * pt.tiles_m * pt.tiles_n, SM::kStages, resident);
+    }
   }
   CK(cudaEventDestroy(e0));
   CK(cudaEventDestroy(e1));
@@ -172,12 +215,12 @@ int main(int argc, char** argv) {
   // the same with 6 KB per warp, what staging the code's batch-major copies as well would take: one ring stage fewer
   run<6144, false, false, true>({"encode_6k", 1, M, B, n, d, 1, false, true}, M, sms, zero_flag, sink, reps, clusters);
   // decode: x^ = c W_dec, both operands per model; EpiDecodeT stages nothing and runs in line
-  run<0, true, false, true>({"decode", M, M, B, d, n, 1, false, false}, M, sms, zero_flag, sink, reps, clusters);
+  run<0, true, false, true, true>({"decode", M, M, B, d, n, 1, false, false}, M, sms, zero_flag, sink, reps, clusters);
   // dcode: g W_dec^T; EpiDcodeT stages 4 KB per warp
   run<4096, false, false, true>({"dcode", M, M, B, n, d, 1, false, false}, M, sms, zero_flag, sink, reps, clusters);
   // weight gradient: dz^T x + c^T g, reduction over the batch, fp16 planes MN-major, 8-bit ones from batch-major copies;
   // x (set 0's B) fp16-exact; EpiStoreF32 runs in line
-  run<0, true, true, true>({"dw", M, 1, n, d, B, 2, true, false}, M, sms, zero_flag, sink, reps, clusters);
+  run<0, true, true, true, true>({"dw", M, 1, n, d, B, 2, true, false}, M, sms, zero_flag, sink, reps, clusters);
   cudaFree(zero_flag);
   cudaFree(sink);
   return 0;

@@ -11,6 +11,8 @@ For each of the step's four GEMMs (encode, decode, dcode, weight gradient) it re
   (c) epilogue_bound_ms, encode and dcode only: the engine's kernel time for the same GEMM, measured as (a), at the same
       M, n and B but d = 64. Their K loop is then a single K block, so the time is bounded by the epilogue's per-tile
       throughput: where (c) is below (b), the epilogue keeps pace with the main loop at d = 512;
+(d) tall_main_loop_ms, decode and the weight gradient only: (b) on 192-row output tiles (BM = kBMTall in
+    sce_gemm.cuh), each launch right after the same one on 128-row tiles;
 and the card's name, power limit and SM clock, read in the same run after each measurement. Beside them: (b) of encode
 with 6 KB of epilogue staging per warp instead of 4 KB (one ring stage fewer, what staging the code's batch-major copies
 through shared memory would cost), and the time and launches per step of transpose_batch_u8_kernel, the pass that makes
@@ -95,6 +97,7 @@ TRANSPOSE = "transpose_batch_u8_kernel"
 CLUSTERS = (1, 2)
 EPILOGUE_BOUND_D = 64                 # input dimension of (c): one K block of the encode and dcode GEMMs
 EPILOGUE_BOUND = ("encode", "dcode")  # the GEMMs (c) is reported for
+TALL = ("decode", "dw")               # the GEMMs (d) is reported for
 
 
 def main_loop_times(reps, clusters):
@@ -103,7 +106,7 @@ def main_loop_times(reps, clusters):
         raise SystemExit(f"{exe} is missing: run `make probe` first")
     out = subprocess.run([exe, str(reps)] + [str(c) for c in clusters], capture_output=True, text=True,
                          check=True).stdout
-    return {(r["gemm"], r["cluster"]): r for r in (json.loads(l) for l in out.splitlines() if l.startswith("{"))}
+    return {(r["gemm"], r["cluster"], r["bm"]): r for r in (json.loads(l) for l in out.splitlines() if l.startswith("{"))}
 
 
 def fmt(v, width):
@@ -150,10 +153,11 @@ def main():
     rows = []
     for _, g in EPILOGUES:
         a = [r["engine"][g][0] for r in rounds]
-        b = {c: [r["main_loop"][(g, c)]["main_loop_ms"] for r in rounds] for c in CLUSTERS}
+        b = {c: [r["main_loop"][(g, c, 128)]["main_loop_ms"] for r in rounds] for c in CLUSTERS}
+        tall = {c: [r["main_loop"][(g, c, 192)]["main_loop_ms"] for r in rounds] for c in CLUSTERS} if g in TALL else None
         per_step = rounds[0]["engine"][g][1]
         ma, mb1, mb2 = med(a), med(b[1]), med(b[2])
-        ec = rounds[0]["main_loop"][(g, 1)]["engine_cluster"]   # the cluster size the engine launches this GEMM in
+        ec = rounds[0]["main_loop"][(g, 1, 128)]["engine_cluster"]   # the cluster size the engine launches this GEMM in
         mbe = mb2 if ec == 2 else mb1
         av = [x for x in a if x is not None]
         cv = [r["epilogue_bound"][g][0] for r in rounds] if g in EPILOGUE_BOUND else []
@@ -163,7 +167,12 @@ def main():
                      "main_loop_ms_cluster2": mb2, "main_loop_ms_cluster1_rounds": b[1],
                      "main_loop_ms_cluster2_rounds": b[2], "engine_ms_rounds": a,
                      "epilogue_ms": None if ma is None else ma - mbe,
-                     "stages": rounds[0]["main_loop"][(g, 1)]["stages"], "tiles": rounds[0]["main_loop"][(g, 1)]["tiles"]})
+                     "stages": rounds[0]["main_loop"][(g, 1, 128)]["stages"], "tiles": rounds[0]["main_loop"][(g, 1, 128)]["tiles"]})
+        if tall:
+            rows[-1].update({"tall_main_loop_ms_cluster1": med(tall[1]), "tall_main_loop_ms_cluster2": med(tall[2]),
+                             "tall_main_loop_ms_cluster1_rounds": tall[1], "tall_main_loop_ms_cluster2_rounds": tall[2],
+                             "tall_stages": rounds[0]["main_loop"][(g, 1, 192)]["stages"],
+                             "tall_tiles": rounds[0]["main_loop"][(g, 1, 192)]["tiles"]})
         ra = f"[{min(av):.3f}-{max(av):.3f}]" if av else ""
         r1, r2 = f"[{min(b[1]):.3f}-{max(b[1]):.3f}]", f"[{min(b[2]):.3f}-{max(b[2]):.3f}]"
         cvv = [x for x in cv if x is not None]
@@ -172,10 +181,17 @@ def main():
               f"{mb2 / mb1:8.3f} {fmt(None if ma is None else ma - mbe, 12)} {fmt(mc, 8)} {rc:15s}")
     tr = [r["engine"][TRANSPOSE][0] for r in rounds]
     tr_launches = rounds[0]["engine"][TRANSPOSE][1]
-    e6 = [r["main_loop"][("encode_6k", 1)]["main_loop_ms"] for r in rounds]
-    e6_stages = rounds[0]["main_loop"][("encode_6k", 1)]["stages"]
+    e6 = [r["main_loop"][("encode_6k", 1, 128)]["main_loop_ms"] for r in rounds]
+    e6_stages = rounds[0]["main_loop"][("encode_6k", 1, 128)]["stages"]
     print(f"encode main loop with 6 KB staging per warp ({e6_stages} stages), cluster 1: {med(e6):.3f} "
           f"[{min(e6):.3f}-{max(e6):.3f}] ms")
+    for row in rows:
+        if "tall_main_loop_ms_cluster1" not in row:
+            continue
+        for c in CLUSTERS:
+            t, t128 = row[f"tall_main_loop_ms_cluster{c}_rounds"], row[f"main_loop_ms_cluster{c}_rounds"]
+            print(f"{row['gemm']} main loop, 192-row tiles ({row['tall_stages']} stages, {row['tall_tiles']} tiles), cluster {c}: "
+                  f"{med(t):.3f} [{min(t):.3f}-{max(t):.3f}] ms, {med(t) / med(t128):.3f} x the 128-row tiles")
     print(f"{TRANSPOSE}: {med(tr):.3f} [{min(tr):.3f}-{max(tr):.3f}] ms per step, {tr_launches:.1f} launches per step")
     res = {"card": info, "encode_6k_main_loop_ms": med(e6), "encode_6k_main_loop_ms_rounds": e6,
            "encode_6k_stages": e6_stages, "transpose_ms_per_step": med(tr), "transpose_ms_per_step_rounds": tr,

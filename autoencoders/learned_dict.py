@@ -1,1 +1,1 @@
-from sparse_coding_b200.learned_dict import LearnedDict, Rotation, TiedSAE, UntiedSAE  # noqa: F401
+from sparse_coding_b200.learned_dict import IdentityReLU, LearnedDict, RandomDict, Rotation, TiedSAE, UntiedSAE  # noqa: F401

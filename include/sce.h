@@ -36,7 +36,10 @@ extern "C" {
  * with their *_workspace_bytes queries (NMFEncoder).
  * 201 also covers the additive dead-feature tracking entry points sce_track_workspace_bytes, sce_step_tracked and
  * sce_resample with the struct sce_track they take. sce_step and every other entry point are unchanged, and a plan that
- * never sees sce_step_tracked launches exactly the kernels it did before. */
+ * never sees sce_step_tracked launches exactly the kernels it did before.
+ * 201 also covers the forward-only modifiers SCE_CODE_LINEAR and SCE_DECODER_RAW, or'ed into desc.variant of an SCE_UNTIED
+ * plan (ICAEncoder, RandomDict). They live in bits the variant word never used, so the descriptor keeps its layout and a
+ * caller built against the earlier 201 header keeps working unchanged. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -59,6 +62,21 @@ typedef enum sce_variant {
                                  desc.centering = 0. */
 } sce_variant;
 
+/* Forward-only modifiers of SCE_UNTIED, or'ed into desc.variant (desc.variant & 0xff is the variant). A plan with either is
+ * a scoring plan for a baseline dictionary, not a training plan: sce_step, sce_step_host, sce_grads, sce_step_tracked and
+ * sce_resample return SCE_ERR_INVALID before any device call; sce_forward, sce_forward_stats, sce_forward_fragments,
+ * sce_read_code and sce_active_counts run. Any other bit, or either bit with another variant, is SCE_ERR_INVALID.
+ *   SCE_CODE_LINEAR  the code is c = x E^T + b with no clamp (ICAEncoder's signed code; autoencoders/ica.py). Masked and
+ *                    padding columns are 0. The activity mask is [c != 0] (no [z == 0] plane is written), so out_nnz is
+ *                    the mean count of c != 0 per row, sce_active_counts and the segment counts count rows / segments on
+ *                    which c != 0, and the moment sums of sce_forward_stats are those of the signed c. l_l1 is 0 (give
+ *                    l1_alpha = NULL). sce_forward_fragments takes each fragment's maximum of the signed code, which may be
+ *                    negative, and calls a fragment active where c != 0 on some row of it.
+ *   SCE_DECODER_RAW  the decoder's operand planes are split from sce_buffers.decoder as given, without row normalisation
+ *                    (RandomDict decodes with its raw rows; learned_dict.py:107-127). Under F16F8 a decoder entry fp16 cannot
+ *                    hold sets the health word, as an out-of-range batch does, and counts in sce_input_absmax. */
+enum { SCE_CODE_LINEAR = 1 << 8, SCE_DECODER_RAW = 1 << 9 };
+
 /* How the Adam step counter behaves (SURVEY.md Q2). */
 typedef enum sce_adam_count {
   SCE_ADAM_FROZEN_T1 = 0, /* the reference: step_batch drops torchopt's incremented count (ensemble.py:185-189) */
@@ -79,7 +97,7 @@ typedef enum sce_arith { SCE_ARITH_AUTO = 0, SCE_ARITH_BF16X3 = 1, SCE_ARITH_F16
 
 /* Static description of one stacked ensemble (FunctionalEnsemble.__init__, ensemble.py:69-97). */
 typedef struct sce_desc {
-  int variant;          /* sce_variant */
+  int variant;          /* sce_variant, with SCE_UNTIED optionally or'ed with SCE_CODE_LINEAR / SCE_DECODER_RAW */
   int n_models;         /* M: models stacked on dim 0 */
   int d;                /* activation width, multiple of 8 */
   int n;                /* dictionary rows (stack size for masked variants), multiple of 8 */
@@ -271,7 +289,8 @@ int sce_forward_stats(sce_plan* plan, const float* x, int B, int seg, int seg_ph
  * g L .. g L + L - 1 of this call), then, per model m and feature j, two lists that ACCUMULATE over calls:
  *   top    (fragment maximum max_t c[m, gL + t, j], fragment) over every fragment: the n_top largest by
  *          (maximum descending, fragment ascending)
- *   random (priority, fragment) over the ACTIVE fragments (the activity mask has c > 0 on some row): the n_random
+ *   random (priority, fragment) over the ACTIVE fragments (the activity mask has c > 0 on some row; c != 0 with
+ *          SCE_CODE_LINEAR, whose maxima start at -inf and may be negative): the n_random
  *          largest by (priority descending, fragment ascending), priority = splitmix64(splitmix64(splitmix64(seed) ^ j)
  *          ^ fragment) >> 1 — a uniform draw without replacement that depends on nothing but (seed, j, fragment)
  * The code values are those the engine holds: the joined operand planes (as sce_read_code) for the SAE variants,

@@ -18,6 +18,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SCE_LIB") or os.path.join(_HERE, "libsce.so")
 
 SCE_TIED, SCE_UNTIED, SCE_TOPK, SCE_TIED_LEARNED_CENTER = 0, 1, 2, 3
+SCE_CODE_LINEAR, SCE_DECODER_RAW = 1 << 8, 1 << 9     # forward-only modifiers of SCE_UNTIED, or'ed into desc.variant
 SCE_ADAM_FROZEN_T1, SCE_ADAM_STANDARD = 0, 1
 SCE_LOSS_COLS = 4
 SCE_ARITH_AUTO, SCE_ARITH_BF16X3, SCE_ARITH_F16F8 = 0, 1, 2
@@ -85,6 +86,8 @@ class EngineSignature:
     input_shift: float = 0.0     # encode and reconstruct x + input_shift
     norm_floor: float = 1e-8     # clamp of the dictionary's row norms (0: none)
     topk: bool = False           # buffers["sparsity"] holds each model's k; no bias, no sparsity penalty
+    code_linear: bool = False    # forward-only: the code is x E^T + b, no clamp (SCE_CODE_LINEAR)
+    decoder_raw: bool = False    # forward-only: the decoder's rows as given, not normalised (SCE_DECODER_RAW)
 
 
 _SAE_LOSSES = ("loss", "l_reconstruction", "l_l1")
@@ -98,6 +101,10 @@ SIGNATURES = {
     # FunctionalPositiveTiedSAE encodes and reconstructs x + 0.18 (autoencoders/mlp_tests.py:104, :110)
     "positive_tied": EngineSignature(SCE_TIED, "encoder", _SAE_LOSSES + ("l_bias_decay",), bias_decay=True,
                                      encoder_nonneg=True, input_shift=0.18),
+    # forward-only kinds of metrics.evaluate_dicts / top_activating_fragments (no DictSignature trains them):
+    # RandomDict decodes with its raw rows, ICAEncoder's code is signed and linear
+    "random": EngineSignature(SCE_UNTIED, "encoder", _SAE_LOSSES, decoder=True, decoder_raw=True),
+    "ica": EngineSignature(SCE_UNTIED, "encoder", _SAE_LOSSES, decoder=True, code_linear=True),
 }
 
 
@@ -119,8 +126,9 @@ def plan_structs(sig: EngineSignature, params, buffers, mu, nu, *, batch_max: in
         return params[name].data_ptr(), mu[name].data_ptr(), nu[name].data_ptr()
 
     main = params[sig.main]
+    modifiers = (SCE_CODE_LINEAR if sig.code_linear else 0) | (SCE_DECODER_RAW if sig.decoder_raw else 0)
     desc = SceDesc(
-        variant=sig.variant, n_models=main.shape[0], d=main.shape[2], n=main.shape[1], batch_max=batch_max,
+        variant=sig.variant | modifiers, n_models=main.shape[0], d=main.shape[2], n=main.shape[1], batch_max=batch_max,
         x_per_model=int(x_per_model), lr=adam.lr, beta1=adam.b1, beta2=adam.b2, eps=adam.eps, eps_root=adam.eps_root,
         adam_count_mode=SCE_ADAM_FROZEN_T1 if adam_count_mode == "frozen_t1" else SCE_ADAM_STANDARD,
         fwd_passes=fwd_passes, bwd_passes=bwd_passes, norm_floor=sig.norm_floor, arith=arith_code(arith),

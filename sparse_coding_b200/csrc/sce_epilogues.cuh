@@ -266,10 +266,14 @@ __device__ __forceinline__ void store_batch_major(const BatchMajorParams<true>& 
 // (STATS = false) compile to the same code as without the switch.
 // T8 (f16f8 training steps with a native weight gradient) also writes the batch-major copies of BatchMajorParams; the
 // row-major planes are stored as without it (the decode GEMM reads the 8-bit ones).
+// LINEAR (compile-time, forward-only SCE_CODE_LINEAR plans) keeps the signed c = z: the activity word is [c != 0] (the
+// zmin tracker finds the exact zeros), no [z == 0] word is written, nnz counts c != 0 and no |c| sum is kept (l_l1 = 0).
+// Instantiated for forward passes only; the instantiations without it compile to the same code as without the switch.
 // ------------------------------------------------------------------------------------------------
-template <int ARITH, bool STATS = false, bool T8 = false>
+template <int ARITH, bool STATS = false, bool T8 = false, bool LINEAR = false>
 struct EpiEncodeT {
   static_assert(!T8 || (ARITH == kArithF16F8 && !STATS), "batch-major copies: f16f8 training steps only");
+  static_assert(!(T8 && LINEAR), "a linear code is forward-only");
   static constexpr int kCols = 32;
   static constexpr int kWarpStageBytes = 4096;
   static constexpr bool kInline = STATS;   // the moment sums do not fit the epilogue warpgroup's registers (sce_gemm.cuh)
@@ -315,23 +319,23 @@ struct EpiEncodeT {
           const float z0 = __uint_as_float(r[j + u]) + bb[u], z1 = __uint_as_float(r[j + u + 1]) + bb[u + 1];
           zmin = fminf(zmin, fminf(fabsf(z0), fabsf(z1)));
           neg = __funnelshift_l(__float_as_uint(z1), __funnelshift_l(__float_as_uint(z0), neg, 1), 1);
-          const float c0 = fmaxf(z0, 0.f), c1 = fmaxf(z1, 0.f);
+          const float c0 = LINEAR ? z0 : fmaxf(z0, 0.f), c1 = LINEAR ? z1 : fmaxf(z1, 0.f);
           split_pair<ARITH>(c0, c1, (j + u) >> 1, whi, wlo);
-          ls += c0 + c1;
+          if constexpr (!LINEAR) ls += c0 + c1;
           if constexpr (STATS) {
             cs[j + u] = row_ok ? c0 : 0.f;
             cs[j + u + 1] = row_ok ? c1 : 0.f;
           }
         }
       }
-      pos = ~neg;  // no zero among the 32 scores: positive <=> sign bit clear
+      pos = LINEAR ? ~0u : ~neg;  // no zero among the 32 scores: positive <=> sign bit clear (LINEAR: every c != 0)
       if (zmin == 0.f) {  // some score is exactly +-0: not positive; recorded for the clamp semantics
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
           const float z = __uint_as_float(r[j]) + __ldg(bias + j);
           if (z == 0.f) {
             pos &= ~(0x80000000u >> j);
-            if (P.flag_zero) zero |= 0x80000000u >> j;
+            if (!LINEAR && P.flag_zero) zero |= 0x80000000u >> j;
           }
         }
       }
@@ -345,10 +349,15 @@ struct EpiEncodeT {
           const bool col_ok = col + j + u < n_total;
           const float z = __uint_as_float(r[j + u]) + ((bias && col_ok) ? __ldg(bias + j + u) : 0.f);
           const bool masked = !col_ok || (mask && __ldg(mask + j + u));
-          cv[u] = (z > 0.f && !masked) ? z : 0.f;
-          if (cv[u] > 0.f) pos |= 0x80000000u >> (j + u);
-          if (P.flag_zero && z == 0.f && !masked) zero |= 0x80000000u >> (j + u);
-          ls += cv[u];
+          if constexpr (LINEAR) {
+            cv[u] = masked ? 0.f : z;
+            if (cv[u] != 0.f) pos |= 0x80000000u >> (j + u);
+          } else {
+            cv[u] = (z > 0.f && !masked) ? z : 0.f;
+            if (cv[u] > 0.f) pos |= 0x80000000u >> (j + u);
+            if (P.flag_zero && z == 0.f && !masked) zero |= 0x80000000u >> (j + u);
+            ls += cv[u];
+          }
           if constexpr (STATS) cs[j + u] = row_ok ? cv[u] : 0.f;
         }
         split_pair<ARITH>(cv[0], cv[1], j >> 1, whi, wlo);
@@ -359,7 +368,7 @@ struct EpiEncodeT {
       nnz += __popc(pos);
       const long long w = P.act.at(T.model, col >> 5, T.row);   // 32 lanes = 32 consecutive rows: coalesced
       P.act.pos[w] = pos;
-      if (P.act.zero) P.act.zero[w] = zero;
+      if (!LINEAR && P.act.zero) P.act.zero[w] = zero;
     }
     stage_and_store<ARITH>(stage, T, whi, wlo, &P.out_hi, &P.out_lo, &P.out_x8, col, T.m_blk * kBM + T.warp_q * 32,
                            T.model);

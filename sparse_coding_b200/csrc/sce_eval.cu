@@ -62,7 +62,9 @@ __global__ void moment_reduce_kernel(const float* __restrict__ part, int row_blo
 }
 
 // Segment activity counts (calc_moments_streaming's times_active, standard_metrics.py:482-511): the rows are cut into
-// segments of `seg`; counts[m][j] += number of segments that END in this call in which some row has [c > 0] in column j.
+// segments of `seg`; counts[m][j] += number of segments that END in this call in which some row has [c > 0] in column j
+// ([c != 0] for SCE_CODE_LINEAR plans, whose activity mask holds that; the reference tests the segment's mean of c for
+// != 0, standard_metrics.py:498, which differs only where a segment's non-zero values cancel exactly).
 // `phase` rows of the first segment were seen by earlier calls, whose activity is carried in open[m][j] (0 / 1); the
 // flag of a segment that stays open past this call is written back there. One block per (32-column chunk, model); warp
 // w takes the segments w, w + 8, ...; lanes OR 32 rows' mask words at a time, so lane j ends with column j's flag.
@@ -210,8 +212,12 @@ __global__ void __launch_bounds__(256) read_code_kernel(CodeView<SRC> c, int B, 
 // c > 0 on some row of it. One block per (32-column chunk, fragment, model): lane j reads column 32 chunk + j, so every
 // row is read coalesced over the features; warp w takes the rows w, w + 8, ... and the 8 warps meet in shared memory.
 // grid.y is capped at kMaxGridY: a block takes the fragments blockIdx.y, blockIdx.y + gridDim.y, ... (one when G fits).
+// SIGNED (SCE_CODE_LINEAR plans): the maximum starts at -inf, not 0, so a fragment whose code is negative on every row
+// keeps its negative maximum; "active" stays the OR of the activity mask, there c != 0 on some row. (The reference's
+// interpret.py:309 tests the maximum for 0 instead: the two differ for a fragment whose maximum is exactly 0 while some
+// row is negative.)
 constexpr int kMaxGridY = 65535;
-template <int SRC>
+template <int SRC, bool SIGNED = false>
 __global__ void __launch_bounds__(256) fragment_max_kernel(CodeView<SRC> c, int L, int G, float* __restrict__ fmax,
                                                            uint8_t* __restrict__ active) {
   __shared__ float smax[8][32];
@@ -221,7 +227,7 @@ __global__ void __launch_bounds__(256) fragment_max_kernel(CodeView<SRC> c, int 
   const int j = chunk * 32 + lane;
   const uint32_t* pw = c.pos + ((long long)m * c.n_chunks + chunk) * c.batch_max;
   for (int g = blockIdx.y; g < G; g += gridDim.y) {
-    float mx = 0.f;
+    float mx = SIGNED ? -INFINITY : 0.f;
     uint32_t any = 0u;
     for (int t = warp; t < L; t += 8) {
       const int r = g * L + t;
@@ -343,11 +349,17 @@ static size_t frag_carve(uint8_t* base, const sce_desc& d, int B, int L, FragCar
 }
 
 template <int SRC>
-static int launch_fragments(Launcher& launcher, const CodeView<SRC>& c, int M, int L, int G, long long frag0, float* fmax,
-                            uint8_t* active, int n_top, int n_random, unsigned long long seed, float* top_val,
+static int launch_fragments(Launcher& launcher, const CodeView<SRC>& c, bool linear, int M, int L, int G, long long frag0,
+                            float* fmax, uint8_t* active, int n_top, int n_random, unsigned long long seed, float* top_val,
                             long long* top_frag, float* top_act, long long* rnd_key, long long* rnd_frag, float* rnd_act) {
-  TRY(launcher.launch(fragment_max_kernel<SRC>, dim3(c.n_chunks, G < kMaxGridY ? G : kMaxGridY, M), 256, 0, c, L, G,
-                      fmax, active));
+  const dim3 grid(c.n_chunks, G < kMaxGridY ? G : kMaxGridY, M);
+  bool signed_max = false;
+  if constexpr (SRC != kCodeScores) signed_max = linear;   // (top-k plans have no linear code)
+  if (signed_max) {
+    if constexpr (SRC != kCodeScores) TRY(launcher.launch(fragment_max_kernel<SRC, true>, grid, 256, 0, c, L, G, fmax, active));
+  } else {
+    TRY(launcher.launch(fragment_max_kernel<SRC>, grid, 256, 0, c, L, G, fmax, active));
+  }
   return launcher.launch(fragment_merge_kernel<SRC>, dim3((c.n + 127) / 128, M), 128, 0, c, L, G, frag0, fmax,
                          active, n_top, n_random, seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
 }
@@ -457,7 +469,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   const int n_chunks = (d.n + 31) / 32, G = B / L;
   auto fragments = [&](auto src) {
     constexpr int SRC = decltype(src)::value;
-    return launch_fragments<SRC>(call, code_view<SRC>(p), d.n_models, L, G, frag0, w.fmax, w.active, n_top, n_random,
+    return launch_fragments<SRC>(call, code_view<SRC>(p), p->cfg.linear, d.n_models, L, G, frag0, w.fmax, w.active, n_top, n_random,
                                  seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
   };
   // (a forward pass leaves the code planes row-major)

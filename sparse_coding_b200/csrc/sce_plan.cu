@@ -264,9 +264,15 @@ __global__ void __launch_bounds__(256) finalize_kernel(const float* __restrict__
 
 }  // namespace sce
 
+// desc.variant without its forward-only modifiers
+static int base_variant(const sce_desc& d) { return d.variant & ~(SCE_CODE_LINEAR | SCE_DECODER_RAW); }
+
 int validate(const sce_desc* d) {
   if (!d) return fail(SCE_ERR_INVALID, "desc is NULL");
-  if (d->variant < SCE_TIED || d->variant > SCE_TIED_LEARNED_CENTER) return fail(SCE_ERR_INVALID, "unknown variant %d", d->variant);
+  const int variant = base_variant(*d);
+  if (variant < SCE_TIED || variant > SCE_TIED_LEARNED_CENTER) return fail(SCE_ERR_INVALID, "unknown variant %d", d->variant);
+  if (variant != SCE_UNTIED && variant != d->variant)
+    return fail(SCE_ERR_INVALID, "SCE_CODE_LINEAR / SCE_DECODER_RAW are defined for SCE_UNTIED only (variant %d)", d->variant);
   if (d->n_models < 1 || d->batch_max < 1) return fail(SCE_ERR_INVALID, "n_models and batch_max must be >= 1");
   if (d->d < 8 || d->d % 8 || d->n < 8 || d->n % 8)
     return fail(SCE_ERR_INVALID, "d (%d) and n (%d) must be positive multiples of 8", d->d, d->n);
@@ -294,6 +300,13 @@ int validate(const sce_desc* d) {
 int check_rows(const sce_plan* p, int B, const char* prefix) {
   if (B < 1 || B > p->d.batch_max)
     return fail(SCE_ERR_INVALID, "%sB = %d outside [1, batch_max = %d]", prefix, B, p->d.batch_max);
+  return SCE_OK;
+}
+
+// the training entry points (sce_step, sce_step_host, sce_grads, sce_step_tracked, sce_resample), before any device call
+int check_trainable(const sce_plan* p, const char* prefix) {
+  if (p->cfg.forward_only)
+    return fail(SCE_ERR_INVALID, "%sa plan with SCE_CODE_LINEAR or SCE_DECODER_RAW is forward-only: it cannot train", prefix);
   return SCE_OK;
 }
 
@@ -326,9 +339,12 @@ static int topk_slices(const sce_desc& d, size_t kmax) {
 PlanConfig plan_config(const sce_desc& d) {
   PlanConfig c{};
   c.arith = resolve_arith(d);
-  c.untied = d.variant == SCE_UNTIED;
+  c.untied = base_variant(d) == SCE_UNTIED;
   c.topk = d.variant == SCE_TOPK;
   c.learned = d.variant == SCE_TIED_LEARNED_CENTER;
+  c.linear = (d.variant & SCE_CODE_LINEAR) != 0;
+  c.raw_decoder = (d.variant & SCE_DECODER_RAW) != 0;
+  c.forward_only = c.linear || c.raw_decoder;
   // (the learned-centre variant always holds M centred batches, whatever the caller's layout)
   c.x_models = d.x_per_model || c.learned;
   c.xm = c.x_models ? d.n_models : 1;
@@ -603,8 +619,18 @@ static int transpose_dict(Launcher& L, const sce_plan* p) {
 // The normalised operand planes of every dictionary side from the fp32 parameters (sce_prepare, sce_resample)
 int prepare_dict(Launcher& L, const sce_plan* p) {
   DictSide sides[2];
-  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s)
+  for (int s = 0, ns = dict_sides(p, sides); s < ns; ++s) {
+    if (s == 1 && p->cfg.raw_decoder) {
+      // SCE_DECODER_RAW: sce_similarity's split of a raw operand; f16f8 judges its range with the batch split's flags
+      const long long n4 = (long long)p->d.n_models * p->d.n * p->d.d / 4;
+      TRY(with_arith(p->cfg.arith, [&](auto arith) {
+        constexpr int AR = decltype(arith)::value;
+        return launch_split_rows<AR>(L, sides[s].w, sides[s].planes, n4, AR == kArithF16F8 ? p->res_flags : nullptr);
+      }));
+      continue;
+    }
     TRY(launch_dict_rows<MODE_PREPARE>(L, p, sides[s], nullptr, hyper_for(p, 1)));
+  }
   return transpose_dict(L, p);
 }
 
@@ -708,14 +734,23 @@ static int encode_phase(PlanCall& c, bool tdw, float* mom_part) {
       ep.act = act;
       ep.tiles_n = (n + kBN - 1) / kBN;
     };
-    if (mom_part) {
-      using EpiStats = EpiEncodeT<AR, true>;
+    // (forward-only plans: a forward pass, with or without the moment partials)
+    auto stats = [&](auto linear) {
+      using EpiStats = EpiEncodeT<AR, true, false, decltype(linear)::value>;
       typename EpiStats::Params ep;
       fill(ep);
       ep.mom_part = mom_part;
       ep.row_blocks = (B + 31) / 32;
       return c.gemm<EpiStats, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep, x_is_a);
+    };
+    if (cfg.linear) {
+      if (mom_part) return stats(std::true_type{});
+      using EpiLinear = EpiEncodeT<AR, false, false, true>;
+      typename EpiLinear::Params ep;
+      fill(ep);
+      return c.gemm<EpiLinear, false, false, false, AR>(c.maps->encode, 1, xb, kOnes, d.d, d.fwd_passes, B, n, ep, x_is_a);
     }
+    if (mom_part) return stats(std::false_type{});
     if constexpr (AR == kArithF16F8) {
       if (tdw) {   // the epilogue also writes the batch-major copies of the code's 8-bit planes the weight gradient reads
         using EpiT8 = EpiEncodeT<AR, false, true>;
@@ -1065,7 +1100,7 @@ int sce_plan_create(const sce_desc* desc, const sce_buffers* buffers, sce_plan**
   if (!buffers) return fail(SCE_ERR_INVALID, "buffers is NULL");
   const sce_buffers& b = *buffers;
   if (!b.encoder || !b.encoder_m || !b.encoder_v) return fail(SCE_ERR_INVALID, "encoder / encoder_m / encoder_v are required");
-  if (desc->variant == SCE_UNTIED && (!b.decoder || !b.decoder_m || !b.decoder_v))
+  if (base_variant(*desc) == SCE_UNTIED && (!b.decoder || !b.decoder_m || !b.decoder_v))
     return fail(SCE_ERR_INVALID, "untied variant needs decoder / decoder_m / decoder_v");
   if (desc->variant != SCE_TOPK && (!b.encoder_bias || !b.bias_m || !b.bias_v))
     return fail(SCE_ERR_INVALID, "encoder_bias / bias_m / bias_v are required for SAE variants");
@@ -1182,12 +1217,14 @@ int sce_forward(sce_plan* p, const float* x, int B, float* x_hat, float* out_los
 
 int sce_step(sce_plan* p, const float* x, int B, float* out_losses, float* out_nnz, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
+  TRY(check_trainable(p, ""));
   return step_impl(p, x, B, out_losses, out_nnz, static_cast<cudaStream_t>(stream), nullptr);
 }
 
 int sce_grads(sce_plan* p, const float* x, int B, float* d_encoder, float* d_bias, float* d_decoder,
               float* out_losses, float* out_nnz, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
+  TRY(check_trainable(p, ""));
   PlanCall c;
   TRY(run_pipeline(c, p, x, B, static_cast<cudaStream_t>(stream), nullptr, true, out_losses, out_nnz));
   p->last_launches = c.count;   // the pipeline's: the gradient kernels below are not counted
@@ -1198,6 +1235,7 @@ int sce_grads(sce_plan* p, const float* x, int B, float* d_encoder, float* d_bia
 int sce_step_host(sce_plan* p, const float* x_host, int B, float* out_losses_host, float* out_nnz_host,
                   void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "plan is NULL");
+  TRY(check_trainable(p, ""));
   if (!x_host) return fail(SCE_ERR_INVALID, "x_host is NULL");
   if (int rc = check_rows(p, B, "")) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -109,6 +109,9 @@ struct PlanConfig {
   bool use_graph;      // replay the step as a CUDA graph
   bool nonneg;         // desc.encoder_nonneg: the dictionary rows are built from max(E, 0) (dict_rows_kernel<..., true>)
   float shift;         // desc.input_shift; non-zero: the batch split also writes x + shift, which the step reads
+  bool linear;         // SCE_CODE_LINEAR: the encode epilogue keeps the signed code (EpiEncodeT<..., LINEAR = true>)
+  bool raw_decoder;    // SCE_DECODER_RAW: the decoder's planes are split from it as given (prepare_dict)
+  bool forward_only;   // either modifier: the training entry points refuse the plan
 };
 
 struct sce_plan : PlanBuffers {
@@ -158,6 +161,7 @@ struct PlanCall : Launcher {
 __attribute__((visibility("hidden"))) int validate(const sce_desc* d);
 __attribute__((visibility("hidden"))) PlanConfig plan_config(const sce_desc& d);
 __attribute__((visibility("hidden"))) int check_rows(const sce_plan* p, int B, const char* prefix);
+__attribute__((visibility("hidden"))) int check_trainable(const sce_plan* p, const char* prefix);
 __attribute__((visibility("hidden"))) int run_pipeline(PlanCall& c, sce_plan* p, const float* x, int B, cudaStream_t st,
                                                        float* x_hat, bool backward, float* out_losses, float* out_nnz,
                                                        float* mom_part = nullptr, float* row_part = nullptr);

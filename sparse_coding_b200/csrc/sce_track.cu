@@ -363,6 +363,7 @@ static int check_track(const sce_plan* p, const sce_track* t, const char* prefix
   if (reinterpret_cast<uintptr_t>(t->rows) % 16) return fail(SCE_ERR_INVALID, "%strack: rows must be 16-byte aligned", prefix);
   if (t->n_worst < 1) return fail(SCE_ERR_INVALID, "%strack: n_worst = %d must be >= 1", prefix, t->n_worst);
   if (!p) return fail(SCE_ERR_INVALID, "%splan is NULL", prefix);
+  TRY(check_trainable(p, prefix));
   if (t->n_worst > p->d.n) return fail(SCE_ERR_INVALID, "%strack: n_worst = %d outside [1, n = %d]", prefix, t->n_worst, p->d.n);
   const size_t need = track_carve(static_cast<uint8_t*>(t->workspace), p->d, t->n_worst, w);
   return check_workspace(t->workspace, t->workspace_bytes, need, prefix);

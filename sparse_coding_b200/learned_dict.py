@@ -123,6 +123,55 @@ class TiedSAE(LearnedDict):
         return (batch @ enc.T + self.encoder_bias).clamp(min=0.0)
 
 
+class IdentityReLU(LearnedDict):
+    """learned_dict.py:86-104: the activations themselves as the code, ``relu(x + bias)``, with the identity as the
+    dictionary. Keeps the reference's quirks: ``if bias:`` raises for a bias of more than one element (so only the
+    default zero bias can be given), and ``get_learned_dict`` returns a CPU identity."""
+
+    def __init__(self, activation_size, bias=None):
+        self.n_feats = activation_size
+        self.activation_size = activation_size
+        if bias:
+            self.bias = bias
+        else:
+            self.bias = torch.zeros(activation_size)
+        assert self.bias.shape == (activation_size,)
+
+    def get_learned_dict(self):
+        return torch.eye(self.n_feats)
+
+    def encode(self, batch):
+        return torch.clamp(batch + self.bias, min=0.0)
+
+    def to_device(self, device):
+        self.bias = self.bias.to(device)
+
+
+class RandomDict(LearnedDict):
+    """learned_dict.py:107-127: a Gaussian matrix drawn with ``torch.randn`` from the global RNG at construction, used
+    as the encoder, ``relu(x E^T + b)``, and as the dictionary, with its rows as drawn (not normalised)."""
+
+    def __init__(self, activation_size, n_feats=None):
+        if not n_feats:
+            n_feats = activation_size
+        self.n_feats = n_feats
+        self.activation_size = activation_size
+        self.encoder = torch.randn(n_feats, activation_size)
+        self.encoder_bias = torch.zeros(n_feats)
+
+    def get_learned_dict(self):
+        return self.encoder
+
+    def encode(self, batch):
+        c = torch.einsum("nd,bd->bn", self.encoder, batch)
+        c = c + self.encoder_bias
+        return torch.clamp(c, min=0.0)
+
+    def to_device(self, device):
+        self.encoder = self.encoder.to(device)
+        self.encoder_bias = self.encoder_bias.to(device)
+
+
 class Rotation(LearnedDict):
     """learned_dict.py:277-293: a fixed matrix whose rows are the dictionary; the code is linear, ``batch @ matrix^T``.
     ``activation_size`` is the matrix's row count, as in the reference. The matrix is moved to ``device`` (the CPU by
@@ -144,5 +193,5 @@ class Rotation(LearnedDict):
         return batch @ self.matrix.T
 
 
-for _cls in (LearnedDict, UntiedSAE, TiedSAE, Rotation):
+for _cls in (LearnedDict, UntiedSAE, TiedSAE, IdentityReLU, RandomDict, Rotation):
     _cls.__module__ = _REF_MODULE

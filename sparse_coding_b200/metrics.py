@@ -14,6 +14,7 @@ import contextlib
 import ctypes as C
 from typing import Dict, Iterable, Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -312,20 +313,51 @@ _EVAL_ROWS = 8192          # rows per engine call
 
 
 def _eval_kind(ld) -> str:
-    from .learned_dict import LearnedDict, TiedSAE, UntiedSAE
+    from .ica import ICAEncoder
+    from .learned_dict import IdentityReLU, LearnedDict, RandomDict, TiedSAE, UntiedSAE
     from .topk_encoder import TopKLearnedDict
     if isinstance(ld, TiedSAE):
         if not getattr(ld, "norm_encoder", True):
             raise NotImplementedError("TiedSAE(norm_encoder=False) is not implemented in the engine: its encoder rows "
                                       "are used unnormalised, which no engine variant computes")
         return "tied"
-    if isinstance(ld, UntiedSAE):
+    if isinstance(ld, (UntiedSAE, IdentityReLU)):
         return "untied"
     if isinstance(ld, TopKLearnedDict):
         return "topk"
+    if isinstance(ld, RandomDict):
+        return "random"
+    if isinstance(ld, ICAEncoder):
+        return "ica"
     name = type(ld).__name__ if isinstance(ld, LearnedDict) else repr(type(ld))
     raise NotImplementedError(f"{name} has no engine variant: dictionary evaluation runs TiedSAE (norm_encoder=True), "
-                              "UntiedSAE and TopKLearnedDict, and has no slow path for other dictionaries")
+                              "UntiedSAE, TopKLearnedDict, ICAEncoder, RandomDict and IdentityReLU, and has no slow path "
+                              "for other dictionaries")
+
+
+def _sae_inputs(ld):
+    """(encoder [n, d], bias [n], decoder [n, d] or None, translation [d] or None) of the forward-only plan that computes
+    the SAE-kind dictionary ``ld``: code = flags(x - t) E^T + b), reconstruction code D. The plan's kind supplies the
+    flags (``_lib.SIGNATURES``); the translation belongs to ``encode``, so the raw-batch passes apply it as well."""
+    from .ica import ICAEncoder
+    from .learned_dict import IdentityReLU, RandomDict, TiedSAE
+    if isinstance(ld, TiedSAE):
+        return ld.encoder, ld.encoder_bias, None, None
+    if isinstance(ld, IdentityReLU):
+        eye = torch.eye(ld.n_feats, device=ld.bias.device)
+        return eye, ld.bias, eye, None
+    if isinstance(ld, RandomDict):
+        return ld.encoder, ld.encoder_bias, ld.encoder, None
+    if isinstance(ld, ICAEncoder):
+        # encode = ((x - mean) / scale - ica.mean) C^T = (x - t) (C / scale)^T with t = mean + scale * ica.mean; t is
+        # subtracted from the batch, not folded into the bias: x E^T - E t would cancel on columns whose mean is far
+        # larger than their spread
+        f64 = lambda a: torch.as_tensor(np.asarray(a, dtype=np.float64))
+        comp, mean, scale = f64(ld.ica.components_), f64(ld.scaler.mean_), f64(ld.scaler.scale_)
+        enc = (comp / scale[None, :]).float()
+        t = (mean + scale * f64(ld.ica.mean_)).float()
+        return enc, torch.zeros(enc.shape[0]), ld.get_learned_dict(), t
+    return ld.encoder, ld.encoder_bias, ld.decoder, None          # UntiedSAE
 
 
 def _is_centred(ld) -> bool:
@@ -351,6 +383,10 @@ def _eval_groups(lds, centre: bool, multiple: int):
         if topk and n % multiple:
             raise ValueError(f"dictionary {i}: a TopKLearnedDict needs n ({n}) to be a multiple of {multiple}: its rows "
                              "are normalised without a clamp, so zero padding rows would become NaN")
+        if kind == "ica" and (ld.ica is None or n != ld.ica.components_.shape[0]):
+            raise ValueError(f"dictionary {i}: an ICAEncoder is evaluated with n_feats equal to its fitted components' "
+                             f"count, got n_feats = {n}" + ("" if ld.ica is None else
+                                                             f" and {ld.ica.components_.shape[0]} components"))
         n_pad = -(-n // multiple) * multiple
         centred = centre and _lib.SIGNATURES[kind].centering and _is_centred(ld)
         groups.setdefault((kind, n_pad, d, centred), []).append(i)
@@ -374,14 +410,18 @@ class _DictPlan:
 
         sig = _lib.SIGNATURES[kind]
         params, buffers = {}, {}
+        self.shift = None        # [M, d]: the translation each model's encode subtracts from the batch (ICAEncoder)
         if sig.topk:
             params["dict"] = stack([ld.dict for ld in lds])
             buffers["sparsity"] = torch.tensor([int(ld.sparsity) for ld in lds], dtype=torch.int64, device=dev)
         else:
-            params["encoder"] = stack([ld.encoder for ld in lds])
-            params["encoder_bias"] = stack([ld.encoder_bias for ld in lds])
+            enc, bias, dec, shift = zip(*(_sae_inputs(ld) for ld in lds))
+            params["encoder"] = stack(enc)
+            params["encoder_bias"] = stack(bias)
             if sig.decoder:
-                params["decoder"] = stack([ld.decoder for ld in lds])
+                params["decoder"] = stack(dec)
+            if shift[0] is not None:
+                self.shift = torch.stack([f32(t) for t in shift]).contiguous()
             sizes = [int(ld.n_feats) for ld in lds]
             if any(k < n_pad for k in sizes):       # padding rows: the masked variants' coef_mask (1 = unused)
                 buffers["coef_mask"] = (torch.arange(n_pad, device=dev)[None, :] >= torch.tensor(sizes, device=dev)[:, None]).to(torch.uint8)
@@ -392,7 +432,7 @@ class _DictPlan:
         # sce_prepare and the forward-only passes never read the Adam moments; the plan only requires their pointers
         moments = dict.fromkeys(params, torch.zeros(1, dtype=torch.float32, device=dev))
         self.desc, b, keep = _lib.plan_structs(sig, params, buffers, moments, moments, batch_max=batch_max,
-                                               x_per_model=centred, centering=int(centred), adam=AdamConfig(lr=0.0),
+                                               x_per_model=centred or self.shift is not None, centering=int(centred), adam=AdamConfig(lr=0.0),
                                                adam_count_mode="frozen_t1", fwd_passes=3, bwd_passes=3, arith=arith)
         self._keep_alive = (params, buffers, moments, keep)
         self.plan, self._plan_ws = _lib.create_plan(self.desc, b, dev)
@@ -402,6 +442,10 @@ class _DictPlan:
         except Exception:
             self.close()
             raise
+
+    def batch(self, x):
+        """The batch the plan reads for the rows ``x`` [B, d]: ``x`` itself, or [M, B, d] rows x - shift[m]."""
+        return x if self.shift is None else (x[None] - self.shift[:, None]).contiguous()
 
     def bad(self) -> bool:
         flag, amax = C.c_int(0), C.c_float(0.0)
@@ -435,7 +479,7 @@ class _StatsPlan(_DictPlan):
         B, d = x.shape
         x_hat = torch.empty(self.M, B, d, dtype=torch.float32, device=self.dev) if self.centred else None
         _lib.check(lib.sce_forward_stats(
-            self.plan, x.data_ptr(), B, seg, phase, x_hat.data_ptr() if x_hat is not None else None,
+            self.plan, self.batch(x).data_ptr(), B, seg, phase, x_hat.data_ptr() if x_hat is not None else None,
             self.losses.data_ptr(), self.nnz.data_ptr(), self.sums.data_ptr(), self.seg_counts.data_ptr(),
             self.seg_open.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream), "sce_forward_stats")
         _lib.check(lib.sce_active_counts(self.plan, B, self.counts.data_ptr(), self.stream), "sce_active_counts")
@@ -486,8 +530,10 @@ def _plans(groups, lds, dev, make):
 def _check_f16f8_range(plans, arith):
     """After a pass: raise if f16f8 met a value outside its fp16 plane's range."""
     if arith == "f16f8" and any(p.bad() for p, _ in plans):
-        raise ValueError("the activations hold a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or "
-                         "NaN): use arith='bf16x3' or 'auto'")
+        raw = [p for p, _ in plans if p.bad() and _lib.SIGNATURES[p.kind].decoder_raw]
+        where = "the activations or a RandomDict's raw decoder rows hold" if raw else "the activations hold"
+        raise ValueError(f"{where} a value the f16f8 arithmetic's fp16 plane cannot (|v| >= 65520 or NaN): use "
+                         "arith='bf16x3' or 'auto'")
 
 
 def _to_device(out, device):
@@ -540,7 +586,8 @@ def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
         for (p, idx), sn in zip(plans, snap):
             full, tail = sn, p.sums - sn
             m = (full + (segment / r_last) * tail) / (n_seg * segment)        # [M, n, 4] fp64
-            fvu = (p.sq / total).float()
+            # ICAEncoder: the reference's decode of its fp64 code by the fp32 dictionary raises, so no FVU is defined
+            fvu = (p.sq / total).float() if p.kind != "ica" else torch.full_like(p.sq, float("nan"), dtype=torch.float32)
             l0 = (p.l0 / N).float()
             for k, i in enumerate(idx):
                 n = int(lds[i].n_feats)
@@ -565,7 +612,9 @@ def evaluate_dicts(learned_dicts, activations: torch.Tensor, segment: int = 1000
     """Scores of exported dictionaries on a set of activations, in one pass for all of them.
 
     ``learned_dicts``: LearnedDicts or ``(LearnedDict, hparams)`` pairs (what ``torch.load("learned_dicts.pt")``
-    returns): TiedSAE (norm_encoder=True, any centring), UntiedSAE, TopKLearnedDict. ``activations``: [N, d] fp32 or
+    returns): TiedSAE (norm_encoder=True, any centring), UntiedSAE, TopKLearnedDict, and the baselines ICAEncoder (its
+    signed code, translation included), RandomDict (raw decoder rows) and IdentityReLU. ICAEncoder's ``fvu`` is NaN:
+    the reference's decode of its fp64 code raises (SURVEY Q12). ``activations``: [N, d] fp32 or
     fp16, on the CPU (streamed to the GPU) or a CUDA device. Each dictionary encodes the centred batch, as ``predict``
     and ``mean_nonzero_activations`` do. ``arith``: the engine's operand arithmetic; "auto" runs bf16x3, which holds
     the fp32 range.
@@ -618,10 +667,11 @@ FRAGMENT_MAX_LEN = 8192    # largest fragment: one engine call
 
 def _list_order(key, frag):
     """Per row, the permutation that sorts (key, frag) by key descending, then fragment ascending; empty entries
-    (fragment -1) go last."""
+    (fragment -1) go last: float keys, which may be negative (ICAEncoder's maxima), rank them at -inf, integer keys
+    (priorities, >= 0) at -1."""
     empty = frag < 0
     f = torch.where(empty, torch.iinfo(torch.int64).max, frag)
-    k = torch.where(empty, torch.full_like(key, -1), key)
+    k = torch.where(empty, torch.full_like(key, float("-inf") if key.is_floating_point() else -1), key)
     o1 = torch.sort(f, dim=-1, stable=True).indices
     o2 = torch.sort(k.gather(-1, o1), dim=-1, descending=True, stable=True).indices
     return o1.gather(-1, o2)
@@ -647,7 +697,7 @@ class _FragmentPlan(_DictPlan):
     def run(self, x, frag0):
         ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None
         _lib.check(_lib.load().sce_forward_fragments(
-            self.plan, x.data_ptr(), x.shape[0], self.L, frag0, self.n_top, self.n_random,
+            self.plan, self.batch(x).data_ptr(), x.shape[0], self.L, frag0, self.n_top, self.n_random,
             self.seed & 0xFFFFFFFFFFFFFFFF, ptr(self.top_val), ptr(self.top_frag), ptr(self.top_act), ptr(self.rnd_key),
             ptr(self.rnd_frag), ptr(self.rnd_act), self.n_active.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream),
             "sce_forward_fragments")
@@ -670,13 +720,14 @@ def top_activating_fragments(learned_dicts, activations: torch.Tensor, fragment_
     ``interpret()`` (interpret.py:265-321) hands to the explainer, for every dictionary in one pass.
 
     ``learned_dicts``: LearnedDicts or ``(LearnedDict, hparams)`` pairs (TiedSAE with norm_encoder=True, UntiedSAE,
-    TopKLearnedDict), grouped, padded and streamed as :func:`evaluate_dicts` does. ``activations``: [N, d] fp32 or
+    TopKLearnedDict, ICAEncoder, RandomDict, IdentityReLU), grouped, padded and streamed as :func:`evaluate_dicts` does. ``activations``: [N, d] fp32 or
     fp16, on the CPU (streamed to the GPU) or a CUDA device, in sequence order: fragment g is rows
     g·L … g·L+L−1, L = ``fragment_len`` (a multiple of 32 in [32, 8192]; N must be a multiple of it). The raw rows are
     encoded, with no ``center()``, as make_feature_activation_dataset does. ``arith``: "auto" runs bf16x3; "f16f8"
     raises on values fp16 cannot hold.
 
-    Per feature f, with c the code and the fragment maximum max_t c[g·L+t, f] (>= 0):
+    Per feature f, with c the code and the fragment maximum max_t c[g·L+t, f] (>= 0; ICAEncoder's signed code may give
+    negative maxima, and "active" below means c != 0 on some row, where the reference tests the maximum for 0):
       top records     the ``n_top`` fragments with the largest maximum, descending, ties broken by the lower fragment
                       index; zero-maximum fragments fill the list when fewer are positive, as the reference's
                       ``sort_values(...).head(20)``. The engine's fp32 values are ranked, where the reference sorts its

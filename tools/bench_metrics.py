@@ -7,9 +7,11 @@
   interp_*: record selection for reading features (interpret.py make_feature_activation_dataset + interpret's choice of
           top and random records). One pass = metrics.top_activating_fragments of every dictionary over 50 000 fragments
           of 64 fp16 rows, 20 + 20 records per feature with their per-token values.
+  *_baselines: the same two passes on the baselines of sweep_baselines.py: one ICAEncoder, RandomDict(512) and
+          IdentityReLU(512) at d = 512, in one pass (2^20 rows / 50 000 fragments of 64 rows).
 
-    python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5|interp_cfg2|interp_cfg5
-                                  [--steps K --warmup W --arith ...]
+    python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5|interp_cfg2|interp_cfg5|
+                                             eval_baselines|interp_baselines [--steps K --warmup W --arith ...]
 
 Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
 computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
@@ -318,15 +320,150 @@ def run_interp(args):
     }), flush=True)
 
 
+BASELINE_WORKLOADS = {
+    # name: (d, rows or fragments, description)
+    "eval_baselines": (512, 1 << 20, "ICAEncoder (fitted by the engine), RandomDict(512) and IdentityReLU(512) over 2^20 "
+                                     "fp16 rows in one evaluate_dicts pass, segment 1000"),
+    "interp_baselines": (512, 50000, "ICAEncoder, RandomDict(512) and IdentityReLU(512): top_activating_fragments over "
+                                     "50 000 fragments of 64 fp16 rows, 20 top + 20 random records per feature"),
+}
+SKLEARN_ROWS = 1 << 16     # host subsample the reference's ICA encode is timed on, scaled to the workload's rows
+
+
+def baseline_dicts(d, x, dev):
+    """[ICAEncoder fitted by the engine on the first 2^18 rows (at most 50 iterations), RandomDict, IdentityReLU]."""
+    import warnings
+
+    import sparse_coding_b200 as S  # noqa: F401  (the engine's library)
+    from sparse_coding_b200.ica import ICAEncoder
+    from sparse_coding_b200.learned_dict import IdentityReLU, RandomDict
+    np.random.seed(0)
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        ica = ICAEncoder(d, device=dev, max_iter=50).fit(x[: 1 << 18])
+    torch.manual_seed(0)
+    rd, ir = RandomDict(d), IdentityReLU(d)
+    rd.to_device(dev)
+    ir.to_device(dev)
+    return [ica, rd, ir]
+
+
+def sklearn_ica_encode_ms(x, rows):
+    """ms of the reference's ICA encode (ica.py:30-34: the rows to host fp64, StandardScaler.transform,
+    FastICA.transform, the code back to the device) over ``rows`` rows, timed on SKLEARN_ROWS rows and scaled; sklearn's
+    objects are fitted on a small subsample (their values do not change the cost). None without sklearn."""
+    import time
+    import warnings
+    try:
+        from sklearn.decomposition import FastICA
+        from sklearn.preprocessing import StandardScaler
+    except ImportError:
+        return None
+    sub = x[:SKLEARN_ROWS]
+    scaler = StandardScaler()
+    fit = scaler.fit_transform(sub[:8192].float().cpu().numpy().astype(np.float64))
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        ica = FastICA(max_iter=5).fit(fit)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    c = ica.transform(scaler.transform(sub.float().cpu().numpy().astype(np.float64)))
+    torch.tensor(c, device=x.device)
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3 * rows / sub.shape[0]
+
+
+def run_baselines(args):
+    """The baselines of sweep_baselines.py in one engine pass, against the reference's op sequences on the same GPU:
+    RandomDict and IdentityReLU as fp32 / TF32 torch (evaluation: calc_moments_streaming's loop over segments of 1000
+    rows, then FVU and mean_nonzero_activations over 8192-row pieces; record selection: 128 fragments per encode, amax
+    over the tokens, topk over the fragments), ICA as the reference's sklearn encode on the host, scaled from a
+    subsample (its moment and top-k arithmetic, on the GPU, is not added)."""
+    from sparse_coding_b200 import metrics as MT
+
+    dev, K, W = setup(args)
+    d, size, desc = BASELINE_WORKLOADS[args.workload]
+    interp = args.workload.startswith("interp")
+    L = 64
+    N = size * L if interp else size
+    x = activations(N, d, dev)
+    lds = baseline_dicts(d, x, dev)
+    if interp:
+        ms, res = timed(lambda: MT.top_activating_fragments(lds, x, arith=args.arith), K, W)
+        del res
+    else:
+        ms, res = timed(lambda: MT.evaluate_dicts(lds, x, segment=1000, arith=args.arith), K, W)
+        del res
+    torch_lds = lds[1:]
+
+    def stock_eval(ld):
+        D = ld.get_learned_dict().to(dev)
+        times, mean, m2, m3, m4 = (torch.zeros(ld.n_feats, device=dev) for _ in range(5))
+        seen = 0
+        for i in range(0, N, 1000):
+            c = ld.encode(x[i:i + 1000].float())
+            bm = c.mean(dim=0)
+            times += (bm != 0).float()
+            mean = (seen * mean + 1000 * bm) / (seen + 1000)
+            m2 = (seen * m2 + 1000 * (c ** 2).mean(dim=0)) / (seen + 1000)
+            m3 = (seen * m3 + 1000 * (c ** 3).mean(dim=0)) / (seen + 1000)
+            m4 = (seen * m4 + 1000 * (c ** 4).mean(dim=0)) / (seen + 1000)
+            seen += 1000
+        sq = torch.zeros((), dtype=torch.float64, device=dev)
+        nz = torch.zeros(ld.n_feats, device=dev)
+        for i in range(0, N, 8192):
+            b = x[i:i + 8192].float()
+            c = ld.encode(b)
+            sq += (b - c @ D).pow(2).sum().double()
+            nz += (c != 0).float().sum(dim=0)
+        return sq, mean
+
+    def stock_interp(ld):
+        n = ld.n_feats
+        fmax = torch.empty(size, n, device=dev)
+        for g0 in range(0, size, 128):
+            g1 = min(size, g0 + 128)
+            fmax[g0:g1] = ld.encode(x[g0 * L:g1 * L].float()).reshape(g1 - g0, L, n).amax(1)
+        return torch.topk(fmax, 20, dim=0).indices
+
+    stock = stock_interp if interp else stock_eval
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    ref = {}
+    try:
+        for name, allow in (("fp32", False), ("tf32", True)):
+            torch.backends.cuda.matmul.allow_tf32 = allow
+            ref[name] = {type(ld).__name__: timed(lambda: stock(ld), 1, 1)[0] for ld in torch_lds}
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+    ica_ms = sklearn_ica_encode_ms(x, N)
+    ref_total = {k: sum(v.values()) + (ica_ms or 0.0) for k, v in ref.items()}
+    gpu, limit = card_info(0)
+    print(json.dumps({
+        "metric": "ms per pass over the three baselines (" + ("top_activating_fragments" if interp else "evaluate_dicts")
+                  + ")", "workload": args.workload, "desc": desc, "value": ms, "unit": "ms", "d": d, "rows": N,
+        "rows_per_s": N / (ms * 1e-3), "arith": args.arith, "steps": K, "warmup": W,
+        "reference": {"torch_gpu_ms": ref, "ica_sklearn_host_ms": ica_ms,
+                      "ica_sklearn": {"scaled": True, "timed_rows": SKLEARN_ROWS,
+                                      "what": "encode only: rows to host fp64, StandardScaler.transform, FastICA.transform, "
+                                              "code to the device"} if ica_ms is not None else "sklearn not installed",
+                      "total_ms": ref_total},
+        "speedup_vs_reference_fp32": ref_total["fp32"] / ms, "speedup_vs_reference_tf32": ref_total["tf32"] / ms,
+        "gpu": gpu, "power_limit_w": limit,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="mmcs_cfg2",
-                    choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS) + sorted(INTERP_WORKLOADS))
+                    choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS) + sorted(INTERP_WORKLOADS) +
+                    sorted(BASELINE_WORKLOADS))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
     args = ap.parse_args()
-    if args.workload in INTERP_WORKLOADS:
+    if args.workload in BASELINE_WORKLOADS:
+        run_baselines(args)
+    elif args.workload in INTERP_WORKLOADS:
         run_interp(args)
     else:
         (run_eval if args.workload in EVAL_WORKLOADS else run_mmcs)(args)

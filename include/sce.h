@@ -39,7 +39,9 @@ extern "C" {
  * never sees sce_step_tracked launches exactly the kernels it did before.
  * 201 also covers the forward-only modifiers SCE_CODE_LINEAR and SCE_DECODER_RAW, or'ed into desc.variant of an SCE_UNTIED
  * plan (ICAEncoder, RandomDict). They live in bits the variant word never used, so the descriptor keeps its layout and a
- * caller built against the earlier 201 header keeps working unchanged. */
+ * caller built against the earlier 201 header keeps working unchanged.
+ * 201 also covers the additive entry points sce_forward_split_workspace_bytes / sce_forward_split (the top- and
+ * rest-feature FVU) and the constant SCE_SPLIT_MAX_TOP. Every other entry point is unchanged. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -318,6 +320,34 @@ int sce_forward_fragments(sce_plan* plan, const float* x, int B, int L, long lon
                           unsigned long long seed, float* top_val, long long* top_frag, float* top_act,
                           long long* rnd_key, long long* rnd_frag, float* rnd_act, int* n_active, void* workspace,
                           size_t workspace_bytes, void* stream);
+
+/* The top- and rest-feature reconstruction errors (standard_metrics.py:316-342 fraction_variance_unexplained_top_activating):
+ * sce_forward on B rows, then, per model m, with T_m = top_cols[m] (n_top chosen features), t = the decode of the code
+ * restricted to T_m (sum over s of c[m, r, T_m[s]] times dictionary row T_m[s], normalised as the plan normalises it:
+ * tied and untied with the norm floor, TOPK without, SCE_DECODER_RAW as given) and x_hat the plan's reconstruction:
+ *   sq_top[m]   device fp64 [M], ACCUMULATED: += sum over the B rows and d columns of (x - t)^2
+ *   sq_rest[m]  device fp64 [M], ACCUMULATED: += sum of (x - (x_hat - t))^2, the decode of the code without T_m
+ * with x the batch as the plan reads it ([B,d], or [M,B,d] with x_per_model). Both are fp32 partials per 32 rows, added
+ * in a fixed order in fp64: bitwise repeatable. The dense code is never formed.
+ *   n_top       1 .. SCE_SPLIT_MAX_TOP
+ *   top_cols    device int32 [M, n_top]: distinct columns in [0, n) per model. They are copied to the host and checked
+ *               before any launch, so the call synchronises `stream` once.
+ *   x_hat       optional device fp32 [M,B,d]: sce_forward's reconstruction (else it is kept in the workspace)
+ *   x_hat_top   optional device fp32 [M,B,d]: t
+ * Centred plans (desc.centering != 0) reconstruct the centred batch, so the sums above are not the reference's (which
+ * compares center(t) and center(x_hat - t) with the raw batch): they need x_hat and x_hat_top and leave sq_top / sq_rest
+ * untouched (they may be NULL), and the caller forms the residuals. Every other plan needs sq_top and sq_rest.
+ *   workspace   >= sce_forward_split_workspace_bytes(desc, B, n_top), 1024-byte aligned: x_hat, the chosen code columns
+ *               and dictionary rows, and the partials, M (B d + B n_top + n_top d + 2 ceil(B/32)) fp32 (config 2, M = 16,
+ *               d = 512, B = 8192, n_top = 2: 257 MiB). Host-only; returns 0 for an invalid desc, B outside [1, batch_max],
+ *               n_top outside [1, SCE_SPLIT_MAX_TOP] or n_top > n.
+ * Not available for SCE_TIED_LEARNED_CENTER, nor with desc.encoder_nonneg or desc.input_shift, as sce_forward_stats.
+ * Asynchronous on `stream` after the check of top_cols. */
+#define SCE_SPLIT_MAX_TOP 64
+size_t sce_forward_split_workspace_bytes(const sce_desc* desc, int B, int n_top);
+int sce_forward_split(sce_plan* plan, const float* x, int B, int n_top, const int* top_cols, double* sq_top,
+                      double* sq_rest, float* x_hat, float* x_hat_top, void* workspace, size_t workspace_bytes,
+                      void* stream);
 
 /* Dead-feature resampling (experiments/huge_batch_size.py:120-146 WorstIndices, :189-250 process_reinit), per model m,
  * over a WINDOW of tracked steps (the sce_step_tracked calls since the caller emptied the lists, or since sce_resample):

@@ -19,6 +19,7 @@ LIB_PATH = os.environ.get("SCE_LIB") or os.path.join(_HERE, "libsce.so")
 
 SCE_TIED, SCE_UNTIED, SCE_TOPK, SCE_TIED_LEARNED_CENTER = 0, 1, 2, 3
 SCE_CODE_LINEAR, SCE_DECODER_RAW = 1 << 8, 1 << 9     # forward-only modifiers of SCE_UNTIED, or'ed into desc.variant
+SCE_SPLIT_MAX_TOP = 64      # largest n_top of sce_forward_split
 SCE_ADAM_FROZEN_T1, SCE_ADAM_STANDARD = 0, 1
 SCE_LOSS_COLS = 4
 SCE_ARITH_AUTO, SCE_ARITH_BF16X3, SCE_ARITH_F16F8 = 0, 1, 2
@@ -32,7 +33,8 @@ EXPORTS = [
     "sce_last_launch_count", "sce_get_step_count", "sce_set_step_count", "sce_profile_begin", "sce_profile_end",
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
-    "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_synth_rows", "sce_read_center_grad",
+    "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_forward_split_workspace_bytes", "sce_forward_split",
+    "sce_synth_rows", "sce_read_center_grad",
     "sce_second_moments_workspace_bytes", "sce_second_moments", "sce_ica_pass_workspace_bytes", "sce_ica_pass",
     "sce_nmf_project_workspace_bytes", "sce_nmf_project", "sce_nmf_grams_workspace_bytes", "sce_nmf_grams",
     "sce_nmf_cd_sweep_workspace_bytes", "sce_nmf_cd_sweep", "sce_nmf_residual_workspace_bytes", "sce_nmf_residual",
@@ -209,6 +211,9 @@ def load():
     lib.sce_fragments_workspace_bytes.argtypes = [C.POINTER(SceDesc), i, i]
     lib.sce_forward_fragments.argtypes = [vp, vp, i, i, ll, i, i, C.c_ulonglong, vp, vp, vp, vp, vp, vp, vp, vp,
                                           C.c_size_t, vp]
+    lib.sce_forward_split_workspace_bytes.restype = C.c_size_t
+    lib.sce_forward_split_workspace_bytes.argtypes = [C.POINTER(SceDesc), i, i]
+    lib.sce_forward_split.argtypes = [vp, vp, i, i, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
     lib.sce_synth_rows.argtypes = [vp, i, i, vp, i, ll, i, C.c_ulonglong, i, f, vp, i, vp, vp, vp, i, vp]
     lib.sce_second_moments_workspace_bytes.restype = C.c_size_t
     lib.sce_second_moments_workspace_bytes.argtypes = [i, i]

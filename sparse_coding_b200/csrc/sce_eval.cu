@@ -365,6 +365,144 @@ static int launch_fragments(Launcher& launcher, const CodeView<SRC>& c, bool lin
 }
 
 // ------------------------------------------------------------------------------------------------
+// top- and rest-feature reconstruction errors (sce_forward_split; standard_metrics.py:316-342
+// fraction_variance_unexplained_top_activating): with t the decode of the code on the chosen columns alone, the
+// residuals x - t and x - (x^ - t), summed per 32 rows. The decode of the rest is x^ - t, so only the n_top chosen
+// columns of the code and rows of the dictionary are ever read besides x^.
+// ------------------------------------------------------------------------------------------------
+// c_top[m][r][s] = c[m, r, cols[m][s]], the code as the engine holds it. Grid (<= 1024, M).
+template <int SRC>
+__global__ void __launch_bounds__(256) code_columns_kernel(CodeView<SRC> c, int B, int n_top, const int* __restrict__ cols,
+                                                           float* __restrict__ c_top) {
+  const int m = blockIdx.y;
+  const long long cells = (long long)B * n_top;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(i / n_top), s = (int)(i - (long long)r * n_top);
+    c_top[(long long)m * cells + i] = c.at(m, r, __ldg(cols + m * n_top + s));
+  }
+}
+
+// d_top[m][s] = dictionary row cols[m][s] of w [M][n][d], divided by max(||row||, floor) (floor <= 0: by ||row||) where
+// `normalize`, as given otherwise. The norm is summed in dict_rows_kernel's order, so the row is bitwise the fp32 row the
+// plan splits into its planes. One block of 128 threads per (s, m); d % 4 == 0.
+__global__ void __launch_bounds__(128) chosen_rows_kernel(const float* __restrict__ w, const int* __restrict__ cols, int n,
+                                                          int d, int n_top, int normalize, float floor,
+                                                          float* __restrict__ d_top) {
+  __shared__ float red[8];
+  const int s = blockIdx.x, m = blockIdx.y;
+  const float* e = w + ((long long)m * n + __ldg(cols + m * n_top + s)) * d;
+  float* o = d_top + ((long long)m * n_top + s) * d;
+  float sc = 1.f;
+  if (normalize) {
+    float ss = 0.f, unused = 0.f;
+    for (int c = threadIdx.x * 4; c < d; c += 512) {
+      const float4 v = *reinterpret_cast<const float4*>(e + c);
+      ss = __fadd_rn(ss, dot4_rn(v, v));
+    }
+    block_sum2(ss, unused, red);
+    const float nrm = sqrtf(ss);
+    sc = (floor > 0.f && nrm < floor) ? floor : nrm;
+  }
+  for (int c = threadIdx.x * 4; c < d; c += 512) {
+    const float4 v = *reinterpret_cast<const float4*>(e + c);
+    *reinterpret_cast<float4*>(o + c) = make_float4(v.x / sc, v.y / sc, v.z / sc, v.w / sc);
+  }
+}
+
+// Per block of 32 rows and model: t = sum_s c_top[r][s] d_top[s] (fp32, s ascending), x_hat_top = t where given, and
+// with `part` the fp32 sums of (x - t)^2 and (x - (x^ - t))^2 over the block's rows to part[m][rb][0 / 1]. Warp w takes
+// the rows w, w + 8, ..., lane l the columns 4 l + 128 i; the 8 warps' sums are added in warp order: no atomics.
+__global__ void __launch_bounds__(256) split_residual_kernel(const float* __restrict__ x, long long x_model_stride,
+                                                             const float* __restrict__ x_hat,
+                                                             const float* __restrict__ c_top,
+                                                             const float* __restrict__ d_top, int B, int d, int n_top,
+                                                             float* __restrict__ x_hat_top, float* __restrict__ part) {
+  __shared__ float red[2][8];
+  const int rb = blockIdx.x, m = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float* dt = d_top + (long long)m * n_top * d;
+  float a = 0.f, b = 0.f;
+  const int r_end = min(B, rb * 32 + 32);
+  for (int r = rb * 32 + warp; r < r_end; r += 8) {
+    const float* ct = c_top + ((long long)m * B + r) * n_top;
+    const float* xr = x + m * x_model_stride + (long long)r * d;
+    const long long row = ((long long)m * B + r) * d;
+    for (int col = 4 * lane; col < d; col += 128) {
+      float t[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int s = 0; s < n_top; ++s) {
+        const float cs = __ldg(ct + s);
+        const float4 dv = __ldg(reinterpret_cast<const float4*>(dt + (long long)s * d + col));
+        t[0] = fmaf(cs, dv.x, t[0]);
+        t[1] = fmaf(cs, dv.y, t[1]);
+        t[2] = fmaf(cs, dv.z, t[2]);
+        t[3] = fmaf(cs, dv.w, t[3]);
+      }
+      if (x_hat_top) *reinterpret_cast<float4*>(x_hat_top + row + col) = make_float4(t[0], t[1], t[2], t[3]);
+      if (part) {
+        const float4 xv = __ldg(reinterpret_cast<const float4*>(xr + col));
+        const float4 hv = __ldg(reinterpret_cast<const float4*>(x_hat + row + col));
+        const float xs[4] = {xv.x, xv.y, xv.z, xv.w}, hs[4] = {hv.x, hv.y, hv.z, hv.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const float rt = xs[u] - t[u], rr = xs[u] - (hs[u] - t[u]);
+          a = fmaf(rt, rt, a);
+          b = fmaf(rr, rr, b);
+        }
+      }
+    }
+  }
+  if (!part) return;   // (grid-uniform)
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+  }
+  if (lane == 0) {
+    red[0][warp] = a;
+    red[1][warp] = b;
+  }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    float v = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) v += red[threadIdx.x][w];
+    part[((long long)m * gridDim.x + rb) * 2 + threadIdx.x] = v;
+  }
+}
+
+// sq_top[m] += sum over the row blocks, in order, of part[m][rb][0] (fp64); sq_rest likewise from part[m][rb][1]
+__global__ void split_reduce_kernel(const float* __restrict__ part, int row_blocks, int M, double* __restrict__ sq_top,
+                                    double* __restrict__ sq_rest) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  double a = 0.0, b = 0.0;
+  for (int rb = 0; rb < row_blocks; ++rb) {
+    a += (double)part[((long long)m * row_blocks + rb) * 2];
+    b += (double)part[((long long)m * row_blocks + rb) * 2 + 1];
+  }
+  sq_top[m] += a;
+  sq_rest[m] += b;
+}
+
+static bool split_top_ok(const sce_desc& d, int n_top) { return n_top >= 1 && n_top <= SCE_SPLIT_MAX_TOP && n_top <= d.n; }
+
+// The workspace of one split call: x^ [M][B][d], the chosen code columns [M][B][n_top] and dictionary rows
+// [M][n_top][d], and the residual partials [M][ceil(B / 32)][2], fp32. With base == nullptr only measures it.
+struct SplitCarve {
+  float *x_hat, *c_top, *d_top, *part;
+};
+static size_t split_carve(uint8_t* base, const sce_desc& d, int B, int n_top, SplitCarve* out) {
+  const size_t M = d.n_models;
+  Carve c{base, 0};
+  SplitCarve w;
+  w.x_hat = c.take<float>(M * B * d.d);
+  w.c_top = c.take<float>(M * B * n_top);
+  w.d_top = c.take<float>(M * n_top * d.d);
+  w.part = c.take<float>(M * ((B + 31) / 32) * 2);
+  if (out) *out = w;
+  return align_up(c.off, 1024);
+}
+
+// ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
 extern "C" {
@@ -478,6 +616,69 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   CUDA_TRY(cudaMemsetAsync(w.open, 0, (size_t)d.n_models * d.n * sizeof(int), call.st));
   return call.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
                      L, 0, n_active, w.open);
+}
+
+size_t sce_forward_split_workspace_bytes(const sce_desc* desc, int B, int n_top) {
+  if (validate(desc) || B < 1 || B > desc->batch_max || !split_top_ok(*desc, n_top) || !plan_config(*desc).evaluable)
+    return 0;
+  return split_carve(nullptr, *desc, B, n_top, nullptr);
+}
+
+int sce_forward_split(sce_plan* p, const float* x, int B, int n_top, const int* top_cols, double* sq_top, double* sq_rest,
+                      float* x_hat, float* x_hat_top, void* workspace, size_t workspace_bytes, void* stream) {
+  TRY(check_forward_only(p, x, B, "forward_split: "));
+  const sce_desc& d = p->d;
+  if (!split_top_ok(d, n_top))
+    return fail(SCE_ERR_INVALID, "forward_split: n_top = %d must lie in [1, min(n = %d, %d)]", n_top, d.n, SCE_SPLIT_MAX_TOP);
+  if (!top_cols) return fail(SCE_ERR_INVALID, "forward_split: top_cols is NULL");
+  const bool centred = d.centering != 0;
+  if (centred && (!x_hat || !x_hat_top))
+    return fail(SCE_ERR_INVALID, "forward_split: a centred plan needs x_hat and x_hat_top (the caller forms its residuals)");
+  if (!centred && (!sq_top || !sq_rest)) return fail(SCE_ERR_INVALID, "forward_split: sq_top and sq_rest are required");
+  SplitCarve w;
+  const size_t need = split_carve(static_cast<uint8_t*>(workspace), d, B, n_top, &w);
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_split: ")) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the columns are checked on the host before anything is launched
+  const int M = d.n_models;
+  int* cols = static_cast<int*>(std::malloc(sizeof(int) * M * n_top));
+  if (!cols) return fail(SCE_ERR_INVALID, "forward_split: out of host memory");
+  cudaError_t e = cudaMemcpyAsync(cols, top_cols, sizeof(int) * M * n_top, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  int bad = e == cudaSuccess ? SCE_OK : fail(SCE_ERR_CUDA, "forward_split: reading top_cols: %s", cudaGetErrorString(e));
+  for (int m = 0; m < M && !bad; ++m)
+    for (int s = 0; s < n_top && !bad; ++s) {
+      const int j = cols[m * n_top + s];
+      if (j < 0 || j >= d.n)
+        bad = fail(SCE_ERR_INVALID, "forward_split: top_cols[%d][%d] = %d outside [0, n = %d)", m, s, j, d.n);
+      for (int s2 = 0; s2 < s && !bad; ++s2)
+        if (cols[m * n_top + s2] == j)
+          bad = fail(SCE_ERR_INVALID, "forward_split: column %d appears twice in top_cols[%d]", j, m);
+    }
+  std::free(cols);
+  if (bad) return bad;
+  PlanCall c;
+  float* xh = x_hat ? x_hat : w.x_hat;
+  TRY(run_pipeline(c, p, x, B, st, xh, false, nullptr, nullptr));
+  p->last_launches = c.count;   // the pipeline's: the split kernels below are not counted
+  const PlanConfig& cfg = p->cfg;
+  // the decoding dictionary, normalised as the plan's planes are (SCE_DECODER_RAW: as given)
+  const float* dict = cfg.untied ? p->b.decoder : p->b.encoder;
+  TRY(c.launch(chosen_rows_kernel, dim3(n_top, M), 128, 0, dict, top_cols, d.n, d.d, n_top, cfg.raw_decoder ? 0 : 1,
+               d.norm_floor, w.d_top));
+  const long long blocks = ((long long)B * n_top + 255) / 256;
+  auto columns = [&](auto src) {
+    constexpr int SRC = decltype(src)::value;
+    return c.launch(code_columns_kernel<SRC>, dim3((unsigned)(blocks < 1024 ? blocks : 1024), M), 256, 0, code_view<SRC>(p),
+                    B, n_top, top_cols, w.c_top);
+  };
+  // (a forward pass leaves the code planes row-major)
+  TRY(cfg.topk ? columns(std::integral_constant<int, kCodeScores>{}) : with_arith(cfg.arith, columns));
+  const int row_blocks = (B + 31) / 32;
+  TRY(c.launch(split_residual_kernel, dim3(row_blocks, M), 256, 0, x, cfg.x_models ? (long long)B * d.d : 0LL, xh, w.c_top,
+               w.d_top, B, d.d, n_top, x_hat_top, centred ? nullptr : w.part));
+  if (centred) return SCE_OK;
+  return c.launch(split_reduce_kernel, dim3((M + 127) / 128), 128, 0, w.part, row_blocks, M, sq_top, sq_rest);
 }
 
 }  // extern "C"

@@ -473,6 +473,7 @@ class _StatsPlan(_DictPlan):
         self.l0 = torch.zeros(M, dtype=torch.float64, device=dev)
         self.losses = torch.empty(M, _lib.SCE_LOSS_COLS, dtype=torch.float32, device=dev)
         self.nnz = torch.empty(M, dtype=torch.float32, device=dev)
+        self.batch_max = batch_max
 
     def run(self, x, seg, phase):
         lib = _lib.load()
@@ -489,6 +490,56 @@ class _StatsPlan(_DictPlan):
             r = (x[None] - self.trans[:, None]) - torch.bmm(x_hat / self.scale[:, None], self.rot)
             self.sq += r.double().pow(2).sum(dim=(1, 2))
         self.l0 += self.nnz.double() * B
+
+    def start_split(self, top):
+        """Ready the pass of the top- and rest-feature errors: ``top`` [M, n_top] int64, the chosen features per model.
+        The statistics pass is over, so its workspace gives way to this one."""
+        M, n_top = top.shape
+        self.n_top, self.top = n_top, top
+        self.top_cols = top.to(torch.int32).contiguous()
+        self._pass_ws = None
+        self.split_bytes = _lib.load().sce_forward_split_workspace_bytes(C.byref(self.desc), self.batch_max, n_top)
+        self._split_ws, self.split_ptr = _lib.workspace(self.split_bytes, self.dev, "sce_forward_split_workspace_bytes")
+        self.sq_top = torch.zeros(M, dtype=torch.float64, device=self.dev)
+        self.sq_rest = torch.zeros(M, dtype=torch.float64, device=self.dev)
+
+    def run_split(self, x):
+        B, d = x.shape
+        x_hat = x_hat_top = None
+        if self.centred:
+            x_hat = torch.empty(self.M, B, d, dtype=torch.float32, device=self.dev)
+            x_hat_top = torch.empty_like(x_hat)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        _lib.check(_lib.load().sce_forward_split(
+            self.plan, self.batch(x).data_ptr(), B, self.n_top, self.top_cols.data_ptr(), self.sq_top.data_ptr(),
+            self.sq_rest.data_ptr(), ptr(x_hat), ptr(x_hat_top), self.split_ptr, self.split_bytes, self.stream),
+            "sce_forward_split")
+        if self.centred:
+            # the reference applies center (not uncenter) to both partial reconstructions, then compares them with the
+            # raw batch (standard_metrics.py:335-339; SURVEY Q14)
+            cen = lambda v: torch.bmm(v - self.trans[:, None], self.rot.transpose(1, 2)) * self.scale[:, None]
+            self.sq_top += (x[None] - cen(x_hat_top)).double().pow(2).sum(dim=(1, 2))
+            self.sq_rest += (x[None] - cen(x_hat - x_hat_top)).double().pow(2).sum(dim=(1, 2))
+
+
+def _top_features(sums, n):
+    """The ``n_top`` features of largest mean code among the first ``n``, from the fp64 code sums [n_pad]: descending,
+    equal sums ordered by the lower feature index."""
+    return torch.sort(sums[:n], descending=True, stable=True).indices
+
+
+def _check_n_top(n_top, lds):
+    if n_top is None:
+        return None
+    if isinstance(n_top, bool) or not isinstance(n_top, (int, np.integer)):
+        raise ValueError(f"n_top must be an integer, got {n_top!r}")
+    n_top = int(n_top)
+    if not 1 <= n_top <= _lib.SCE_SPLIT_MAX_TOP:
+        raise ValueError(f"n_top must lie in [1, {_lib.SCE_SPLIT_MAX_TOP}], got {n_top}")
+    for i, ld in enumerate(lds):
+        if n_top > int(ld.n_feats):
+            raise ValueError(f"n_top = {n_top} exceeds dictionary {i}'s {int(ld.n_feats)} features")
+    return n_top
 
 
 def _dict_inputs(learned_dicts, activations, arith, centre):
@@ -553,11 +604,12 @@ def _eval_rows(activations, dev, cuts):
         yield xb.float().contiguous()
 
 
-def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
+def _evaluate(learned_dicts, activations, segment, threshold, arith, centre, n_top=None):
     if int(segment) < 1:
         raise ValueError(f"batch_size / segment must be >= 1, got {segment}")
     segment = int(segment)
     lds, groups, ar = _dict_inputs(learned_dicts, activations, arith, centre)
+    n_top = _check_n_top(n_top, lds)
     dev = _cuda_device(activations, "dictionary evaluation")
     N, d = activations.shape
     # engine calls: a multiple of the segment where one fits, and a cut where the last segment starts (its sums are
@@ -581,6 +633,19 @@ def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
             s1 += xd.sum(0)
             s2 += xd.pow(2).sum(0)
         _check_f16f8_range(plans, ar)
+        if n_top is not None:
+            # the second pass: each dictionary's top features from the first pass's code sums, then the two errors
+            for p, idx in plans:
+                top = torch.stack([_top_features(p.sums[k, :, 0], int(lds[i].n_feats))[:n_top] for k, i in enumerate(idx)])
+                if p.kind == "ica":     # (no second pass: the reference's decode of its code raises, as for ``fvu``)
+                    p.top = top
+                else:
+                    p.start_split(top)
+            split = [p for p, _ in plans if p.kind != "ica"]
+            if split:
+                for x in _eval_rows(activations, dev, cuts):
+                    for p in split:
+                        p.run_split(x)
         total = (s2 - s1 * s1 / N).sum()
         r_last = N - last
         for (p, idx), sn in zip(plans, snap):
@@ -603,12 +668,17 @@ def _evaluate(learned_dicts, activations, segment, threshold, arith, centre):
                        "m3": m3.float(), "m4": m4.float(), "var": var.float(),
                        "skew": (m3 / var.pow(1.5).clamp(min=1e-8)).float(),
                        "kurtosis": (m4 / var.pow(2).clamp(min=1e-8)).float()}
+                if n_top is not None:
+                    nan = torch.full((), float("nan"), device=dev)
+                    out["top_features"] = p.top[k].clone()
+                    out["fvu_top"] = (p.sq_top[k] / total).float() if p.kind != "ica" else nan
+                    out["fvu_rest"] = (p.sq_rest[k] / total).float() if p.kind != "ica" else nan.clone()
                 results[i] = _to_device(out, activations.device)
     return results
 
 
 def evaluate_dicts(learned_dicts, activations: torch.Tensor, segment: int = 1000,
-                   threshold: int = EVER_ACTIVE_THRESHOLD, arith: str = "auto"):
+                   threshold: int = EVER_ACTIVE_THRESHOLD, arith: str = "auto", n_top: Optional[int] = None):
     """Scores of exported dictionaries on a set of activations, in one pass for all of them.
 
     ``learned_dicts``: LearnedDicts or ``(LearnedDict, hparams)`` pairs (what ``torch.load("learned_dicts.pt")``
@@ -624,14 +694,32 @@ def evaluate_dicts(learned_dicts, activations: torch.Tensor, segment: int = 1000
       ``frac_dead``, ``rows`` as :func:`evaluate_batches` (FVU with the residual in the raw space, as the reference's
       ``fraction_variance_unexplained``), and ``times_active``, ``mean``, ``m2``, ``m3``, ``m4``, ``var``, ``skew``,
       ``kurtosis`` as ``calc_moments_streaming`` with ``batch_size = segment`` defines them (standard_metrics.py:482-511:
-      ``times_active`` counts segments, the last partial segment is weighted like a full one)."""
-    return _evaluate(learned_dicts, activations, segment, threshold, arith, centre=True)
+      ``times_active`` counts segments, the last partial segment is weighted like a full one).
+
+    With an integer ``n_top`` (1 .. 64, at most every dictionary's ``n_feats``; the reference has no such bound), a
+    second pass over the activations adds the scores of ``fraction_variance_unexplained_top_activating``
+    (standard_metrics.py:316-342):
+      ``top_features`` [n_top] int64: the features of largest mean code over all N rows, descending, equal means
+                       ordered by the lower feature index (the reference's argsort leaves their order open)
+      ``fvu_top``      mean((x - x^_top)^2) / the total variance of ``fvu``, with x^_top the decode of the code on
+                       ``top_features`` alone, and ``fvu_rest`` the same for the code on every other feature. As the
+                       reference, a centred TiedSAE passes both decodes through ``center`` (not ``uncenter``) before
+                       comparing them with the raw batch (SURVEY Q14). NaN for ICAEncoder, as ``fvu``.
+    The other entries are bitwise those of a call without ``n_top``."""
+    return _evaluate(learned_dicts, activations, segment, threshold, arith, centre=True, n_top=n_top)
 
 
 # drop-ins with the reference's names, argument order and results (standard_metrics.py:305-314, 344-345, 446-454,
 # 482-511), on the device of the activations
 def fraction_variance_unexplained(model, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:
     return _evaluate([model], batch, 1000, EVER_ACTIVE_THRESHOLD, arith, centre=True)[0]["fvu"]
+
+
+def fraction_variance_unexplained_top_activating(model, batch: torch.Tensor, n_top: int = 2, arith: str = "auto"):
+    """(FVU of the decode of the ``n_top`` features of largest mean code, FVU of the decode of the others), 0-dim
+    tensors; see :func:`evaluate_dicts`."""
+    r = _evaluate([model], batch, 1000, EVER_ACTIVE_THRESHOLD, arith, centre=True, n_top=n_top)[0]
+    return r["fvu_top"], r["fvu_rest"]
 
 
 def r_squared(model, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:

@@ -7,11 +7,14 @@
   interp_*: record selection for reading features (interpret.py make_feature_activation_dataset + interpret's choice of
           top and random records). One pass = metrics.top_activating_fragments of every dictionary over 50 000 fragments
           of 64 fp16 rows, 20 + 20 records per feature with their per-token values.
+  topfvu_cfg2: the top- and rest-feature FVU (fraction_variance_unexplained_top_activating, n_top = 2) of the config-2
+          dictionaries. One pass = metrics.evaluate_dicts(n_top=2), whose second pass is timed as the difference to the
+          call without n_top.
   *_baselines: the same two passes on the baselines of sweep_baselines.py: one ICAEncoder, RandomDict(512) and
           IdentityReLU(512) at d = 512, in one pass (2^20 rows / 50 000 fragments of 64 rows).
 
     python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5|interp_cfg2|interp_cfg5|
-                                             eval_baselines|interp_baselines [--steps K --warmup W --arith ...]
+                                             eval_baselines|interp_baselines|topfvu_cfg2 [--steps K --warmup W --arith ...]
 
 Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
 computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
@@ -452,16 +455,86 @@ def run_baselines(args):
     }), flush=True)
 
 
+TOPFVU_WORKLOADS = {
+    # name: (M, n, d, rows, n_top, description)
+    "topfvu_cfg2": (16, 4096, 512, 1 << 20, 2, "16 seeded config-2 TiedSAE dictionaries (4096 x 512) over 2^20 fp16 rows, "
+                                               "n_top = 2"),
+}
+TOPFVU_REF_ROWS = 1 << 16     # rows the reference's function is timed on per call (its three [rows, n] fp32 tensors)
+
+
+def run_topfvu(args):
+    """The top- and rest-feature FVU (standard_metrics.py:316-342): evaluate_dicts(n_top) over all rows and dictionaries,
+    the same call without n_top (the difference is the cost of the second pass), and the reference's function per
+    dictionary in fp32 and TF32 on the same GPU, timed on TOPFVU_REF_ROWS rows and scaled to the workload's rows."""
+    import sparse_coding_b200 as S
+    from oracle import top_fvu_oracle as TO
+    from sparse_coding_b200 import metrics as MT
+
+    dev, K, W = setup(args)
+    M, n, d, N, k, desc = TOPFVU_WORKLOADS[args.workload]
+    lds = [S.FunctionalTiedSAE.to_learned_dict(p, b) for p, b in make_models(S.FunctionalTiedSAE, M, d, n, seed=0)]
+    for ld in lds:
+        ld.to_device(dev)
+    x = activations(N, d, dev)
+    ms_split, r = timed(lambda: MT.evaluate_dicts(lds, x, arith=args.arith, n_top=k), K, W)
+    ms_plain, _ = timed(lambda: MT.evaluate_dicts(lds, x, arith=args.arith), K, W)
+
+    def stock(ld, xs):
+        """the reference's function, written out (standard_metrics.py:316-342)"""
+        c = ld.encode(ld.center(xs))
+        idxs = torch.argsort(c.mean(dim=0), descending=True)
+        c_top = torch.zeros_like(c)
+        c_top[:, idxs[:k]] = c[:, idxs[:k]]
+        c_rest = torch.zeros_like(c)
+        c_rest[:, idxs[k:]] = c[:, idxs[k:]]
+        x_top, x_rest = ld.center(ld.decode(c_top)), ld.center(ld.decode(c_rest))
+        var = (xs - xs.mean(dim=0)).pow(2).mean()
+        return (xs - x_top).pow(2).mean() / var, (xs - x_rest).pow(2).mean() / var
+
+    sub = x[:TOPFVU_REF_ROWS].float()
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    try:
+        torch.backends.cuda.matmul.allow_tf32 = False
+        ms_fp32, _ = timed(lambda: stock(lds[0], sub), 3, 1)
+        torch.backends.cuda.matmul.allow_tf32 = True
+        ms_tf32, _ = timed(lambda: stock(lds[0], sub), 3, 1)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+    # deviation of the engine from fp64 on a subsample, dictionary 0
+    small = x[:16384 + 500]
+    m64 = {"kind": "tied", "encoder": lds[0].encoder.double(), "encoder_bias": lds[0].encoder_bias.double()}
+    t64, r64, _ = TO.fraction_variance_unexplained_top_activating(m64, small.double(), k)
+    e = MT.evaluate_dicts(lds[:1], small, arith=args.arith, n_top=k)[0]
+    scale = N / TOPFVU_REF_ROWS
+    name, limit = card_info(0)
+    print(json.dumps({
+        "metric": "ms per evaluation pass with the top- and rest-feature FVU (evaluate_dicts(n_top))",
+        "workload": args.workload, "desc": desc, "value": ms_split, "unit": "ms", "dictionaries": M, "n": n, "d": d,
+        "rows": N, "n_top": k, "arith": args.arith, "steps": K, "warmup": W,
+        "without_n_top_ms": ms_plain, "second_pass_ms": ms_split - ms_plain,
+        "fvu_top_rest_dict0": [float(r[0]["fvu_top"]), float(r[0]["fvu_rest"])],
+        "deviation_from_fp64": {"fvu_top_rel": abs(float(e["fvu_top"]) / float(t64) - 1),
+                                "fvu_rest_rel": abs(float(e["fvu_rest"]) / float(r64) - 1)},
+        "stock_torch_gpu_per_dictionary": {"rows_timed": TOPFVU_REF_ROWS, "fp32_ms": ms_fp32 * scale,
+                                           "tf32_ms": ms_tf32 * scale, "scaled_by": scale},
+        "speedup_vs_stock_fp32": ms_fp32 * scale * M / ms_split, "speedup_vs_stock_tf32": ms_tf32 * scale * M / ms_split,
+        "gpu": name, "power_limit_w": limit,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="mmcs_cfg2",
                     choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS) + sorted(INTERP_WORKLOADS) +
-                    sorted(BASELINE_WORKLOADS))
+                    sorted(BASELINE_WORKLOADS) + sorted(TOPFVU_WORKLOADS))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
     args = ap.parse_args()
-    if args.workload in BASELINE_WORKLOADS:
+    if args.workload in TOPFVU_WORKLOADS:
+        run_topfvu(args)
+    elif args.workload in BASELINE_WORKLOADS:
         run_baselines(args)
     elif args.workload in INTERP_WORKLOADS:
         run_interp(args)

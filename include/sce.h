@@ -41,7 +41,9 @@ extern "C" {
  * plan (ICAEncoder, RandomDict). They live in bits the variant word never used, so the descriptor keeps its layout and a
  * caller built against the earlier 201 header keeps working unchanged.
  * 201 also covers the additive entry points sce_forward_split_workspace_bytes / sce_forward_split (the top- and
- * rest-feature FVU) and the constant SCE_SPLIT_MAX_TOP. Every other entry point is unchanged. */
+ * rest-feature FVU) and the constant SCE_SPLIT_MAX_TOP. Every other entry point is unchanged.
+ * 201 also covers the additive entry points sce_interference_workspace_bytes / sce_code_interference and
+ * sce_expected_interference_workspace_bytes / sce_expected_interference (the expected interference). */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -348,6 +350,33 @@ size_t sce_forward_split_workspace_bytes(const sce_desc* desc, int B, int n_top)
 int sce_forward_split(sce_plan* plan, const float* x, int B, int n_top, const int* top_cols, double* sq_top,
                       double* sq_rest, float* x_hat, float* x_hat_top, void* workspace, size_t workspace_bytes,
                       void* stream);
+
+/* Expected interference (big_sweep.py:43-57 calc_expected_interference), per model m, of the code c [B, n] of the plan's
+ * LAST sce_forward / sce_forward_stats call (its B rows) and the dictionary the plan decodes with (tied and top-k: the
+ * encoder, untied: the decoder), as stored. With W_i = row i / max(||row i||, 1e-8) for every kind (whatever the plan's
+ * own decode normalises; SURVEY Q15) and A_r = {j : c[r, j] != 0}:
+ *   totals[r, i] = sum over j in A_r of (W_i . W_j)^2 c[r, j]      (fp32 FMA dot products)
+ *   cap[r, i]    = c[r, i] / max(totals[r, i], 1e-8)                 (i in A_r; 0 elsewhere)
+ *   cap_sums[m]  device fp64 [M, n], ACCUMULATED: += sum over the B rows of cap[r, j]
+ *   nz_counts[m] device int64 [M, n], ACCUMULATED: += number of rows with c[r, j] != 0
+ * The reference's result is cap_sums / max(nz_counts, 1) over all rows. Only the Gram of each row's active dictionary
+ * rows is formed (O(|A_r|^2 d) per row, the active set tiled 64 at a time, any size up to n); the [n, n] cosine matrix
+ * never is. Per-feature partials of 32 rows are added in a fixed order in fp64: bitwise repeatable.
+ *   workspace   >= sce_interference_workspace_bytes(desc, B), 1024-byte aligned: the normalised dictionary and the
+ *               partials, M (n ceil(d / 32) 32 + 2 n ceil(B / 32)) fp32 (config 2, M = 16, n = 4096, d = 512, B = 8192:
+ *               256 MiB). Host-only; returns 0 for an invalid desc or B outside [1, batch_max].
+ * Not available for SCE_TIED_LEARNED_CENTER, nor with desc.encoder_nonneg or desc.input_shift, as sce_forward_stats.
+ * Asynchronous on `stream`. */
+size_t sce_interference_workspace_bytes(const sce_desc* desc, int B);
+int sce_code_interference(sce_plan* plan, int B, double* cap_sums, long long* nz_counts, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
+/* The same for a caller-held code, without a plan: dict device fp32 [n, d], code device fp32 [B, n] (any n, d >= 1),
+ * cap_sums device fp64 [n] and nz_counts device int64 [n], ACCUMULATED. The workspace (>= the query's bytes, 1024-byte
+ * aligned) grows with B; call once per slice of rows to bound it. The query returns 0 for n, d or B < 1. */
+size_t sce_expected_interference_workspace_bytes(int n, int d, int B);
+int sce_expected_interference(const float* dict, int n, int d, const float* code, int B, double* cap_sums,
+                              long long* nz_counts, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Dead-feature resampling (experiments/huge_batch_size.py:120-146 WorstIndices, :189-250 process_reinit), per model m,
  * over a WINDOW of tracked steps (the sce_step_tracked calls since the caller emptied the lists, or since sce_resample):

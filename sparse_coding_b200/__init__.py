@@ -7,7 +7,8 @@ LearnedDict / TiedSAE / UntiedSAE (learned_dict.py), plus the driver loop pieces
 on-device metrics (metrics.py) and the synthetic datasets of sc_datasets/random_dataset.py generated on the GPU
 (synthetic.py)."""
 from . import metrics
-from .metrics import (batched_calc_feature_n_ever_active, calc_moments_streaming, evaluate_dicts,
+from .metrics import (batched_calc_feature_n_ever_active, calc_expected_interference, calc_moments_streaming,
+                      evaluate_dicts,
                       fraction_variance_unexplained, fraction_variance_unexplained_top_activating,
                       mean_nonzero_activations, r_squared, top_activating_fragments)
 from .ensemble import CodeProxy, FunctionalEnsemble, optim_str_to_func, stack_dict, unstack_dict
@@ -25,7 +26,8 @@ __all__ = [
     "AdamConfig", "CodeProxy", "DictSignature", "FunctionalEnsemble", "FunctionalMaskedSAE", "FunctionalMaskedTiedSAE",
     "FunctionalPositiveTiedSAE", "FunctionalSAE", "FunctionalTiedCenteredSAE", "FunctionalTiedSAE", "LearnedDict",
     "TiedSAE", "TopKEncoder", "TopKLearnedDict", "UntiedSAE",
-    "adam", "batched_calc_feature_n_ever_active", "calc_moments_streaming", "evaluate_dicts",
+    "adam", "batched_calc_feature_n_ever_active", "calc_expected_interference", "calc_moments_streaming",
+    "evaluate_dicts",
     "fraction_variance_unexplained", "fraction_variance_unexplained_top_activating", "mean_nonzero_activations", "optim_str_to_func", "r_squared", "stack_dict",
     "top_activating_fragments", "unstack_dict",
     "RandomDatasetGenerator", "SparseMixDataset", "SyntheticChunks", "generate_corr_matrix",

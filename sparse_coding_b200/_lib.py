@@ -34,6 +34,8 @@ EXPORTS = [
     "sce_plan_arith", "sce_input_absmax", "sce_health", "sce_clear_health", "sce_active_counts",
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
     "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_forward_split_workspace_bytes", "sce_forward_split",
+    "sce_interference_workspace_bytes", "sce_code_interference", "sce_expected_interference_workspace_bytes",
+    "sce_expected_interference",
     "sce_synth_rows", "sce_read_center_grad",
     "sce_second_moments_workspace_bytes", "sce_second_moments", "sce_ica_pass_workspace_bytes", "sce_ica_pass",
     "sce_nmf_project_workspace_bytes", "sce_nmf_project", "sce_nmf_grams_workspace_bytes", "sce_nmf_grams",
@@ -214,6 +216,12 @@ def load():
     lib.sce_forward_split_workspace_bytes.restype = C.c_size_t
     lib.sce_forward_split_workspace_bytes.argtypes = [C.POINTER(SceDesc), i, i]
     lib.sce_forward_split.argtypes = [vp, vp, i, i, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_interference_workspace_bytes.restype = C.c_size_t
+    lib.sce_interference_workspace_bytes.argtypes = [C.POINTER(SceDesc), i]
+    lib.sce_code_interference.argtypes = [vp, i, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_expected_interference_workspace_bytes.restype = C.c_size_t
+    lib.sce_expected_interference_workspace_bytes.argtypes = [i, i, i]
+    lib.sce_expected_interference.argtypes = [vp, i, i, vp, i, vp, vp, vp, C.c_size_t, vp]
     lib.sce_synth_rows.argtypes = [vp, i, i, vp, i, ll, i, C.c_ulonglong, i, f, vp, i, vp, vp, vp, i, vp]
     lib.sce_second_moments_workspace_bytes.restype = C.c_size_t
     lib.sce_second_moments_workspace_bytes.argtypes = [i, i]

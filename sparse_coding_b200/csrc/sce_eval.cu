@@ -1,6 +1,7 @@
 // sce_eval.cu — the entry points that read a plan's call back: the dense code (sce_read_code), activation counts
-// (sce_active_counts), the evaluation statistics of a forward pass (sce_forward_stats) and its top-activating and
-// random activating fragments (sce_forward_fragments).
+// (sce_active_counts), the evaluation statistics of a forward pass (sce_forward_stats), its top-activating and
+// random activating fragments (sce_forward_fragments), the top- and rest-feature errors (sce_forward_split) and the
+// expected interference of its code (sce_code_interference; sce_expected_interference for a caller-held code).
 #include "sce_plan.cuh"
 
 namespace sce {
@@ -503,6 +504,235 @@ static size_t split_carve(uint8_t* base, const sce_desc& d, int B, int n_top, Sp
 }
 
 // ------------------------------------------------------------------------------------------------
+// expected interference (sce_code_interference, sce_expected_interference; big_sweep.py:43-57
+// calc_expected_interference): with W the dictionary rows divided by max(||row||, 1e-8) and A_r the features with
+// c[r, j] != 0, totals[r, i] = sum over j in A_r of (W_i . W_j)^2 c[r, j] and cap[r, i] = c[r, i] / max(totals, 1e-8)
+// for i in A_r (0 elsewhere). Only the Gram of each row's active dictionary rows is formed, O(|A_r|^2 d) per row,
+// tiled by kIfTile features, so the active set may be any size.
+// ------------------------------------------------------------------------------------------------
+constexpr int kCodeDense = kCodeScores + 1;   // a caller-held fp32 code [B][n] (sce_expected_interference)
+constexpr int kIfTile = 64;                   // active features per Gram tile
+constexpr int kIfK = 32;                      // dictionary columns per staged chunk
+constexpr int kIfRows = 32;                   // rows per block, added in order into the block's partials
+constexpr int kIfLd = kIfTile + 4;            // (16-byte aligned rows of the staged chunks)
+
+// wn[m][j][0 .. dp) = w[m][j] / max(||w[m][j]||, 1e-8), zero from d on. One block of 128 threads per (j, m).
+__global__ void __launch_bounds__(128) clamp_rows_kernel(const float* __restrict__ w, int n, int d, int dp,
+                                                         float* __restrict__ wn) {
+  __shared__ float red[8];
+  const int j = blockIdx.x, m = blockIdx.y;
+  const float* e = w + ((long long)m * n + j) * d;
+  float* o = wn + ((long long)m * n + j) * dp;
+  float ss = 0.f, unused = 0.f;
+  for (int c = threadIdx.x; c < d; c += 128) ss = fmaf(e[c], e[c], ss);
+  block_sum2(ss, unused, red);
+  const float nrm = sqrtf(ss), sc = nrm < 1e-8f ? 1e-8f : nrm;
+  for (int c = threadIdx.x; c < dp; c += 128) o[c] = c < d ? e[c] / sc : 0.f;
+}
+
+// c[m, r, j]: the plan's code through its CodeView, or the dense code
+template <int SRC>
+__device__ __forceinline__ float if_code(const CodeView<SRC>& c, const float* dense, int m, int r, int j) {
+  if constexpr (SRC == kCodeDense) return __ldg(dense + (long long)r * c.n + j);
+  else return c.at(m, r, j);
+}
+
+// The column of the k-th candidate of a row (k < the row's count): mask[w] bit l is column 32 w + l, before[w] the
+// candidates in the words below w
+__device__ __forceinline__ int if_column(const uint32_t* mask, const int* before, int n_chunks, int k) {
+  int lo = 0, hi = n_chunks - 1;   // the last word w with before[w] <= k
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (before[mid] <= k) lo = mid;
+    else hi = mid - 1;
+  }
+  return 32 * lo + (int)__fns(mask[lo], 0, k - before[lo] + 1);
+}
+
+// Per block of kIfRows rows and model, rows in order: part[m][rb][0][j] = sum of cap[r, j], part[m][rb][1][j] = number of
+// rows with c[r, j] != 0. The candidates of a row are its activity-mask bits (plan code; exactly its c != 0 set) or its
+// non-zero entries (dense code); a candidate whose value reads 0 adds nothing. The I and J tiles of kIfTile candidates
+// are staged kIfK dictionary columns at a time; thread (ty, tx) forms the Gram entries (4 ty + u, 4 tx + v) in fp32 FMA,
+// then totals[i] gets sum over v of g^2 c_j, added over the 16 tx lanes and the J tiles in a fixed order.
+// Dynamic shared memory: 2 ceil(n / 32) + 1 words (the row's mask and the ranks before each word).
+template <int SRC>
+__global__ void __launch_bounds__(256, 2) interference_kernel(CodeView<SRC> c, const float* __restrict__ dense,
+                                                           const float* __restrict__ wn, int dp, int B,
+                                                           float* __restrict__ part) {
+  extern __shared__ uint32_t if_words[];
+  __shared__ __align__(16) float sa[kIfK][kIfLd];
+  __shared__ __align__(16) float sb[kIfK][kIfLd];
+  __shared__ int col_i[kIfTile], col_j[kIfTile];
+  __shared__ float val_i[kIfTile], val_j[kIfTile], tot[kIfTile];
+  const int n = c.n, n_chunks = (n + 31) / 32;
+  uint32_t* mask = if_words;
+  int* before = reinterpret_cast<int*>(if_words + n_chunks);
+  const int rb = blockIdx.x, m = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tx = tid & 15, ty = tid >> 4;
+  float* pc = part + ((long long)m * gridDim.x + rb) * 2 * n;
+  for (int j = tid; j < 2 * n; j += 256) pc[j] = 0.f;
+  const float* wm = wn + (long long)m * n * dp;
+  const int r_end = min(B, rb * kIfRows + kIfRows);
+  // the k-th candidate of the row and its code value, or (-1, 0) past the last
+  auto candidate = [&](int r, int k, int L, int* col, float* val) {
+    int j = -1;
+    float v = 0.f;
+    if (k < L) {
+      j = if_column(mask, before, n_chunks, k);
+      v = if_code(c, dense, m, r, j);
+    }
+    *col = j;
+    *val = v;
+  };
+  for (int r = rb * kIfRows; r < r_end; ++r) {
+    __syncthreads();   // the previous row (and the zeroing of pc) is done
+    if constexpr (SRC == kCodeDense) {
+      for (int w = warp; w < n_chunks; w += 8) {
+        const int j = 32 * w + lane;
+        const uint32_t bits = __ballot_sync(0xffffffffu, j < n && __ldg(dense + (long long)r * n + j) != 0.f);
+        if (lane == 0) mask[w] = bits;
+      }
+    } else {
+      for (int w = tid; w < n_chunks; w += 256) {
+        uint32_t bits = __brev(__ldg(c.pos + ((long long)m * n_chunks + w) * c.batch_max + r));
+        if (32 * w + 32 > n) bits &= (1u << (n - 32 * w)) - 1u;
+        mask[w] = bits;
+      }
+    }
+    __syncthreads();
+    if (warp == 0) {   // exclusive ranks of the words, 32 at a time
+      int carry = 0;
+      for (int w0 = 0; w0 < n_chunks; w0 += 32) {
+        const int w = w0 + lane, v = w < n_chunks ? __popc(mask[w]) : 0;
+        int s = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int t = __shfl_up_sync(0xffffffffu, s, o);
+          if (lane >= o) s += t;
+        }
+        if (w < n_chunks) before[w] = carry + s - v;
+        carry += __shfl_sync(0xffffffffu, s, 31);
+      }
+      if (lane == 0) before[n_chunks] = carry;
+    }
+    __syncthreads();
+    const int L = before[n_chunks];
+    for (int i0 = 0; i0 < L; i0 += kIfTile) {
+      if (tid < kIfTile) {
+        candidate(r, i0 + tid, L, &col_i[tid], &val_i[tid]);
+        tot[tid] = 0.f;
+      }
+      for (int j0 = 0; j0 < L; j0 += kIfTile) {
+        const bool same = j0 == i0;
+        if (!same && tid < kIfTile) candidate(r, j0 + tid, L, &col_j[tid], &val_j[tid]);
+        __syncthreads();
+        const int* cj = same ? col_i : col_j;
+        const float* vj = same ? val_i : val_j;
+        float acc[4][4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+#pragma unroll
+          for (int v = 0; v < 4; ++v) acc[u][v] = 0.f;
+        for (int k0 = 0; k0 < dp; k0 += kIfK) {
+          for (int q = tid; q < kIfTile * kIfK / 4; q += 256) {
+            const int t = q >> 3, k = (q & 7) * 4;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (col_i[t] >= 0) v = __ldg(reinterpret_cast<const float4*>(wm + (long long)col_i[t] * dp + k0 + k));
+            sa[k][t] = v.x;
+            sa[k + 1][t] = v.y;
+            sa[k + 2][t] = v.z;
+            sa[k + 3][t] = v.w;
+            if (!same) {
+              v = make_float4(0.f, 0.f, 0.f, 0.f);
+              if (cj[t] >= 0) v = __ldg(reinterpret_cast<const float4*>(wm + (long long)cj[t] * dp + k0 + k));
+              sb[k][t] = v.x;
+              sb[k + 1][t] = v.y;
+              sb[k + 2][t] = v.z;
+              sb[k + 3][t] = v.w;
+            }
+          }
+          __syncthreads();
+          const float(*bt)[kIfLd] = same ? sa : sb;
+#pragma unroll 8
+          for (int k = 0; k < kIfK; ++k) {
+            const float4 a = *reinterpret_cast<const float4*>(&sa[k][4 * ty]);
+            const float4 b = *reinterpret_cast<const float4*>(&bt[k][4 * tx]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+#pragma unroll
+              for (int v = 0; v < 4; ++v) acc[u][v] = fmaf(av[u], bv[v], acc[u][v]);
+          }
+          __syncthreads();
+        }
+        float s[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          s[u] = 0.f;
+#pragma unroll
+          for (int v = 0; v < 4; ++v) s[u] = fmaf(acc[u][v] * acc[u][v], vj[4 * tx + v], s[u]);
+#pragma unroll
+          for (int o = 8; o > 0; o >>= 1) s[u] += __shfl_xor_sync(0xffffffffu, s[u], o);
+        }
+        if (tx == 0)
+#pragma unroll
+          for (int u = 0; u < 4; ++u) tot[4 * ty + u] += s[u];
+        __syncthreads();   // tot is complete; col_j / val_j may be replaced
+      }
+      if (tid < kIfTile && col_i[tid] >= 0 && val_i[tid] != 0.f) {
+        const float t = tot[tid];
+        pc[col_i[tid]] += val_i[tid] / (t < 1e-8f ? 1e-8f : t);   // (a NaN total stays NaN, as torch.clamp keeps it)
+        pc[n + col_i[tid]] += 1.f;
+      }
+      __syncthreads();   // before the next I tile replaces col_i / val_i / tot
+    }
+  }
+}
+
+// cap_sums[m][j] += sum over the row blocks, in order, of part[m][rb][0][j] (fp64); nz_counts[m][j] += those of [1][j]
+__global__ void interference_reduce_kernel(const float* __restrict__ part, int row_blocks, int n,
+                                           double* __restrict__ cap_sums, long long* __restrict__ nz_counts) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, m = blockIdx.y;
+  if (j >= n) return;
+  double a = 0.0;
+  long long k = 0;
+  for (int rb = 0; rb < row_blocks; ++rb) {
+    const float* o = part + ((long long)m * row_blocks + rb) * 2 * n + j;
+    a += (double)__ldg(o);
+    k += (long long)__ldg(o + n);
+  }
+  cap_sums[(long long)m * n + j] += a;
+  nz_counts[(long long)m * n + j] += k;
+}
+
+// The workspace of one interference call: the clamp-normalised dictionary [M][n][dp] (dp = d rounded up to kIfK) and the
+// row-block partials [M][ceil(B / kIfRows)][2][n], fp32. With base == nullptr only measures it.
+struct IfCarve {
+  float *wn, *part;
+};
+static int if_width(int d) { return (d + kIfK - 1) / kIfK * kIfK; }
+static size_t if_carve(uint8_t* base, size_t M, size_t n, int d, int B, IfCarve* out) {
+  Carve c{base, 0};
+  IfCarve w;
+  w.wn = c.take<float>(M * n * if_width(d));
+  w.part = c.take<float>(M * ((B + kIfRows - 1) / kIfRows) * 2 * n);
+  if (out) *out = w;
+  return align_up(c.off, 1024);
+}
+
+// clamp_rows_kernel, interference_kernel<SRC> and the reduction on `dict` [M][n][d] and the code of view `c`
+template <int SRC>
+static int launch_interference(Launcher& L, const CodeView<SRC>& c, const float* dense, const float* dict, int M, int d,
+                               int B, const IfCarve& w, double* cap_sums, long long* nz_counts) {
+  const int n = c.n, dp = if_width(d), row_blocks = (B + kIfRows - 1) / kIfRows;
+  TRY(L.launch(clamp_rows_kernel, dim3(n, M), 128, 0, dict, n, d, dp, w.wn));
+  const size_t smem = sizeof(uint32_t) * (2 * ((n + 31) / 32) + 1);
+  CUDA_TRY(cudaFuncSetAttribute(interference_kernel<SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  TRY(L.launch(interference_kernel<SRC>, dim3(row_blocks, M), 256, smem, c, dense, w.wn, dp, B, w.part));
+  return L.launch(interference_reduce_kernel, dim3((n + 255) / 256, M), 256, 0, w.part, row_blocks, n, cap_sums, nz_counts);
+}
+
+// ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
 extern "C" {
@@ -679,6 +909,54 @@ int sce_forward_split(sce_plan* p, const float* x, int B, int n_top, const int* 
                w.d_top, B, d.d, n_top, x_hat_top, centred ? nullptr : w.part));
   if (centred) return SCE_OK;
   return c.launch(split_reduce_kernel, dim3((M + 127) / 128), 128, 0, w.part, row_blocks, M, sq_top, sq_rest);
+}
+
+size_t sce_interference_workspace_bytes(const sce_desc* desc, int B) {
+  if (validate(desc) || B < 1 || B > desc->batch_max || !plan_config(*desc).evaluable) return 0;
+  return if_carve(nullptr, desc->n_models, desc->n, desc->d, B, nullptr);
+}
+
+int sce_code_interference(sce_plan* p, int B, double* cap_sums, long long* nz_counts, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  if (!p) return fail(SCE_ERR_INVALID, "code_interference: plan is NULL");
+  if (!p->cfg.evaluable)
+    return fail(SCE_ERR_INVALID, "code_interference: not available for the learned-centre variant or with encoder_nonneg / "
+                                 "input_shift; evaluate the exported dictionaries (TiedSAE)");
+  TRY(check_rows(p, B, "code_interference: "));
+  if (!cap_sums || !nz_counts) return fail(SCE_ERR_INVALID, "code_interference: cap_sums and nz_counts are required");
+  const sce_desc& d = p->d;
+  IfCarve w;
+  const size_t need = if_carve(static_cast<uint8_t*>(workspace), d.n_models, d.n, d.d, B, &w);
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "code_interference: ")) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  // the dictionary the plan decodes with, as stored: every kind is normalised here with the clamp alone
+  const float* dict = p->cfg.untied ? p->b.decoder : p->b.encoder;
+  auto run = [&](auto src) {
+    constexpr int SRC = decltype(src)::value;
+    return launch_interference<SRC>(L, code_view<SRC>(p), nullptr, dict, d.n_models, d.d, B, w, cap_sums, nz_counts);
+  };
+  if (p->cfg.topk) return run(std::integral_constant<int, kCodeScores>{});
+  if (p->code_batch_major) return run(std::integral_constant<int, kCodeBatchMajor>{});
+  return with_arith(p->cfg.arith, run);
+}
+
+size_t sce_expected_interference_workspace_bytes(int n, int d, int B) {
+  if (n < 1 || d < 1 || B < 1) return 0;
+  return if_carve(nullptr, 1, n, d, B, nullptr);
+}
+
+int sce_expected_interference(const float* dict, int n, int d, const float* code, int B, double* cap_sums,
+                              long long* nz_counts, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!dict || !code) return fail(SCE_ERR_INVALID, "expected_interference: dict / code is NULL");
+  if (n < 1 || d < 1 || B < 1)
+    return fail(SCE_ERR_INVALID, "expected_interference: n = %d, d = %d and B = %d must be >= 1", n, d, B);
+  if (!cap_sums || !nz_counts) return fail(SCE_ERR_INVALID, "expected_interference: cap_sums and nz_counts are required");
+  IfCarve w;
+  const size_t need = if_carve(static_cast<uint8_t*>(workspace), 1, n, d, B, &w);
+  if (int rc = check_workspace(workspace, workspace_bytes, need, "expected_interference: ")) return rc;
+  Launcher L{static_cast<cudaStream_t>(stream)};
+  const CodeView<kCodeDense> c{nullptr, nullptr, nullptr, nullptr, nullptr, (n + 31) / 32, B, n, 0};
+  return launch_interference<kCodeDense>(L, c, code, dict, 1, d, B, w, cap_sums, nz_counts);
 }
 
 }  // extern "C"

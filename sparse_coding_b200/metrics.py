@@ -461,7 +461,7 @@ class _DictPlan:
 class _StatsPlan(_DictPlan):
     """A dictionary plan with the statistics accumulators of :func:`evaluate_dicts`."""
 
-    def __init__(self, key, lds, batch_max, arith, dev):
+    def __init__(self, key, lds, batch_max, arith, dev, interference=False):
         super().__init__(key, lds, batch_max, arith, dev)
         M, n = self.M, self.n
         self.ws_bytes = _lib.load().sce_forward_stats_workspace_bytes(C.byref(self.desc), batch_max)
@@ -474,6 +474,12 @@ class _StatsPlan(_DictPlan):
         self.losses = torch.empty(M, _lib.SCE_LOSS_COLS, dtype=torch.float32, device=dev)
         self.nnz = torch.empty(M, dtype=torch.float32, device=dev)
         self.batch_max = batch_max
+        self.cap_sums = self.nz_counts = None
+        if interference:     # the expected interference of each call's code (sce_code_interference)
+            self.if_bytes = _lib.load().sce_interference_workspace_bytes(C.byref(self.desc), batch_max)
+            self._if_ws, self.if_ptr = _lib.workspace(self.if_bytes, dev, "sce_interference_workspace_bytes")
+            self.cap_sums = torch.zeros(M, n, dtype=torch.float64, device=dev)
+            self.nz_counts = torch.zeros(M, n, dtype=torch.int64, device=dev)
 
     def run(self, x, seg, phase):
         lib = _lib.load()
@@ -484,6 +490,9 @@ class _StatsPlan(_DictPlan):
             self.losses.data_ptr(), self.nnz.data_ptr(), self.sums.data_ptr(), self.seg_counts.data_ptr(),
             self.seg_open.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream), "sce_forward_stats")
         _lib.check(lib.sce_active_counts(self.plan, B, self.counts.data_ptr(), self.stream), "sce_active_counts")
+        if self.cap_sums is not None:
+            _lib.check(lib.sce_code_interference(self.plan, B, self.cap_sums.data_ptr(), self.nz_counts.data_ptr(),
+                                                 self.if_ptr, self.if_bytes, self.stream), "sce_code_interference")
         if x_hat is None:
             self.sq += self.losses[:, 1].double() * (B * d)
         else:       # the reference's residual x - uncenter(x^_c), in the raw space (standard_metrics.py:310-314)
@@ -604,10 +613,12 @@ def _eval_rows(activations, dev, cuts):
         yield xb.float().contiguous()
 
 
-def _evaluate(learned_dicts, activations, segment, threshold, arith, centre, n_top=None):
+def _evaluate(learned_dicts, activations, segment, threshold, arith, centre, n_top=None, interference=False):
     if int(segment) < 1:
         raise ValueError(f"batch_size / segment must be >= 1, got {segment}")
     segment = int(segment)
+    if not isinstance(interference, (bool, np.bool_)):
+        raise ValueError(f"interference must be True or False, got {interference!r}")
     lds, groups, ar = _dict_inputs(learned_dicts, activations, arith, centre)
     n_top = _check_n_top(n_top, lds)
     dev = _cuda_device(activations, "dictionary evaluation")
@@ -620,7 +631,8 @@ def _evaluate(learned_dicts, activations, segment, threshold, arith, centre, n_t
     cuts = [(s, min(s + rows, last)) for s in range(0, last, rows)] + [(s, min(s + rows, N)) for s in range(last, N, rows)]
     batch_max = max(e - s for s, e in cuts)
     results = [None] * len(lds)
-    with _plans(groups, lds, dev, lambda key, g: _StatsPlan(key, g, batch_max, ar, dev)) as plans:
+    make = lambda key, g: _StatsPlan(key, g, batch_max, ar, dev, interference=bool(interference))
+    with _plans(groups, lds, dev, make) as plans:
         s1 = torch.zeros(d, dtype=torch.float64, device=dev)
         s2 = torch.zeros(d, dtype=torch.float64, device=dev)
         snap = [torch.zeros_like(p.sums) for p, _ in plans]
@@ -673,12 +685,15 @@ def _evaluate(learned_dicts, activations, segment, threshold, arith, centre, n_t
                     out["top_features"] = p.top[k].clone()
                     out["fvu_top"] = (p.sq_top[k] / total).float() if p.kind != "ica" else nan
                     out["fvu_rest"] = (p.sq_rest[k] / total).float() if p.kind != "ica" else nan.clone()
+                if interference:
+                    out["expected_interference"] = (p.cap_sums[k, :n] / p.nz_counts[k, :n].clamp(min=1)).float()
                 results[i] = _to_device(out, activations.device)
     return results
 
 
 def evaluate_dicts(learned_dicts, activations: torch.Tensor, segment: int = 1000,
-                   threshold: int = EVER_ACTIVE_THRESHOLD, arith: str = "auto", n_top: Optional[int] = None):
+                   threshold: int = EVER_ACTIVE_THRESHOLD, arith: str = "auto", n_top: Optional[int] = None,
+                   interference: bool = False):
     """Scores of exported dictionaries on a set of activations, in one pass for all of them.
 
     ``learned_dicts``: LearnedDicts or ``(LearnedDict, hparams)`` pairs (what ``torch.load("learned_dicts.pt")``
@@ -705,8 +720,15 @@ def evaluate_dicts(learned_dicts, activations: torch.Tensor, segment: int = 1000
                        ``top_features`` alone, and ``fvu_rest`` the same for the code on every other feature. As the
                        reference, a centred TiedSAE passes both decodes through ``center`` (not ``uncenter``) before
                        comparing them with the raw batch (SURVEY Q14). NaN for ICAEncoder, as ``fvu``.
-    The other entries are bitwise those of a call without ``n_top``."""
-    return _evaluate(learned_dicts, activations, segment, threshold, arith, centre=True, n_top=n_top)
+    The other entries are bitwise those of a call without ``n_top``.
+
+    With ``interference=True`` the statistics pass also adds ``expected_interference`` [n] fp32: the reference's
+    ``calc_expected_interference(ld.get_learned_dict(), code)`` (big_sweep.py:43-57) over all N rows of the code the
+    engine computes, on every kind (ICAEncoder's signed code included). Only each row's active features are compared,
+    so the [n, n] cosine matrix is never formed (libsce ``sce_code_interference``; SURVEY Q15). The other entries are
+    bitwise those of a call without it."""
+    return _evaluate(learned_dicts, activations, segment, threshold, arith, centre=True, n_top=n_top,
+                     interference=interference)
 
 
 # drop-ins with the reference's names, argument order and results (standard_metrics.py:305-314, 344-345, 446-454,
@@ -720,6 +742,48 @@ def fraction_variance_unexplained_top_activating(model, batch: torch.Tensor, n_t
     tensors; see :func:`evaluate_dicts`."""
     r = _evaluate([model], batch, 1000, EVER_ACTIVE_THRESHOLD, arith, centre=True, n_top=n_top)[0]
     return r["fvu_top"], r["fvu_rest"]
+
+
+_INTERFERENCE_ROWS = 8192   # code rows per sce_expected_interference call (its workspace grows with them)
+
+
+def calc_expected_interference(dictionary: torch.Tensor, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:
+    """big_sweep.py:43-57 on the GPU: ``dictionary`` [n, d] (its rows are normalised here with the 1e-8 clamp) and
+    ``batch`` the CODE [B, n] (not the activations), both on one CUDA device. Returns [n] fp32 on that device: for
+    each feature, the sum over the rows where its code is non-zero of c / max(sum_j cos^2 c_j, 1e-8), over that row
+    count (at least 1). The code is used as given in fp32, so ``arith`` (checked, for the drop-ins' common signature)
+    changes nothing: the cosines are fp32 FMA dot products either way."""
+    _lib.arith_code(arith)
+    if not torch.is_tensor(dictionary) or not torch.is_tensor(batch):
+        raise TypeError("dictionary and batch must be tensors")
+    if dictionary.dim() != 2 or batch.dim() != 2:
+        raise ValueError(f"dictionary must be [n, d] and batch [B, n], got {tuple(dictionary.shape)} and "
+                         f"{tuple(batch.shape)}")
+    n, d = dictionary.shape
+    if batch.shape[1] != n:
+        raise ValueError(f"batch has {batch.shape[1]} features, the dictionary {n}")
+    if n == 0 or d == 0 or batch.shape[0] == 0:
+        raise ValueError(f"empty dictionary [{n}, {d}] or batch [{batch.shape[0]}, {n}]")
+    if batch.device.type != "cuda" or dictionary.device != batch.device:
+        raise ValueError("calc_expected_interference runs in the sm_90a CUDA engine: dictionary and batch must be on "
+                         f"one CUDA device, got {dictionary.device} and {batch.device}")
+    if not (dictionary.is_floating_point() and batch.is_floating_point()):
+        raise ValueError(f"dictionary and batch must be floating point, got {dictionary.dtype} and {batch.dtype}")
+    dev = batch.device
+    lib = _lib.load()
+    w = dictionary.detach().float().contiguous()
+    rows = min(batch.shape[0], _INTERFERENCE_ROWS)
+    need = lib.sce_expected_interference_workspace_bytes(n, d, rows)
+    cap = torch.zeros(n, dtype=torch.float64, device=dev)
+    nz = torch.zeros(n, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        ws, ws_ptr = _lib.workspace(need, dev, "sce_expected_interference_workspace_bytes")
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        for s in range(0, batch.shape[0], rows):
+            c = batch[s:s + rows].detach().float().contiguous()
+            _lib.check(lib.sce_expected_interference(w.data_ptr(), n, d, c.data_ptr(), c.shape[0], cap.data_ptr(),
+                                                     nz.data_ptr(), ws_ptr, need, stream), "sce_expected_interference")
+    return (cap / nz.clamp(min=1)).float()
 
 
 def r_squared(model, batch: torch.Tensor, arith: str = "auto") -> torch.Tensor:

@@ -10,11 +10,15 @@
   topfvu_cfg2: the top- and rest-feature FVU (fraction_variance_unexplained_top_activating, n_top = 2) of the config-2
           dictionaries. One pass = metrics.evaluate_dicts(n_top=2), whose second pass is timed as the difference to the
           call without n_top.
+  interference_cfg2: the expected interference (big_sweep.py calc_expected_interference) of the config-2 dictionaries.
+          One pass = metrics.evaluate_dicts(interference=True); the difference to the call without it is the cost of the
+          interference kernels.
   *_baselines: the same two passes on the baselines of sweep_baselines.py: one ICAEncoder, RandomDict(512) and
           IdentityReLU(512) at d = 512, in one pass (2^20 rows / 50 000 fragments of 64 rows).
 
     python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5|interp_cfg2|interp_cfg5|
-                                             eval_baselines|interp_baselines|topfvu_cfg2 [--steps K --warmup W --arith ...]
+                                             eval_baselines|interp_baselines|topfvu_cfg2|
+                                             interference_cfg2 [--steps K --warmup W --arith ...]
 
 Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
 computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
@@ -523,16 +527,97 @@ def run_topfvu(args):
     }), flush=True)
 
 
+INTERFERENCE_WORKLOADS = {
+    # name: (M, n, d, rows, description)
+    "interference_cfg2": (16, 4096, 512, 1 << 20, "16 seeded config-2 TiedSAE dictionaries (4096 x 512) over 2^20 fp16 "
+                                                  "rows"),
+}
+SPARSE_FRAC = 50 / 4096
+INTERFERENCE_REF_ROWS = (2000, 1 << 14)   # the sample log_standard_metrics takes, and a larger one to scale from
+
+
+def run_interference(args):
+    """The expected interference (big_sweep.py:43-57): evaluate_dicts(interference=True) over all rows and dictionaries,
+    the same call without it, and the reference's function per dictionary in fp32 and TF32 on the same GPU (code from
+    the dictionary's own encode), on each of INTERFERENCE_REF_ROWS rows; the larger is also scaled to the workload's."""
+    import sparse_coding_b200 as S
+    from oracle import interference_oracle as IO
+    from sparse_coding_b200 import metrics as MT
+
+    dev, K, W = setup(args)
+    M, n, d, N, desc = INTERFERENCE_WORKLOADS[args.workload]
+    lds = [S.FunctionalTiedSAE.to_learned_dict(p, b) for p, b in make_models(S.FunctionalTiedSAE, M, d, n, seed=0)]
+    x = activations(N, d, dev)
+    for ld in lds:
+        # untrained dictionaries fire on about half the features: set each bias so that its feature fires on SPARSE_FRAC
+        # of a sample's rows (L0 about 50, as trained config-2 dictionaries), where the per-row work is what it will be
+        ld.to_device(dev)
+        pre = x[:8192].float() @ ld.get_learned_dict().T
+        ld.encoder_bias = -pre.kthvalue(int(pre.shape[0] * (1.0 - SPARSE_FRAC)), dim=0).values
+    print(f"interference_cfg2: dictionaries ready, mean L0 of dictionary 0 on the sample "
+          f"{float((lds[0].encode(x[:8192].float()) != 0).sum(1).float().mean()):.1f}", file=sys.stderr, flush=True)
+    ms_with, r = timed(lambda: MT.evaluate_dicts(lds, x, arith=args.arith, interference=True), K, W)
+    print(f"interference_cfg2: {ms_with:.0f} ms per pass with interference", file=sys.stderr, flush=True)
+    ms_plain, _ = timed(lambda: MT.evaluate_dicts(lds, x, arith=args.arith), K, W)
+
+    def stock(dictionary, batch):
+        """the reference's function, written out (big_sweep.py:43-57)"""
+        norms = torch.norm(dictionary, 2, dim=-1)
+        normed_weights = dictionary / torch.clamp(norms, 1e-8)[:, None]
+        cosines = torch.einsum("ij,kj->ik", normed_weights, normed_weights)
+        totals = torch.einsum("ij,bj->bi", cosines**2, batch)
+        capacities = batch / torch.clamp(totals, min=1e-8)
+        nonzero_count = batch.count_nonzero(dim=0).float()
+        return capacities.sum(dim=0) / torch.clamp(nonzero_count, min=1.0)
+
+    w0 = lds[0].get_learned_dict()
+    ref = {}
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    try:
+        for rows in INTERFERENCE_REF_ROWS:
+            c = lds[0].encode(x[:rows].float())
+            for mode in ("fp32", "tf32"):
+                torch.backends.cuda.matmul.allow_tf32 = mode == "tf32"
+                ms, _ = timed(lambda: stock(w0, c), 5, 2)
+                ref[f"{mode}_ms_{rows}_rows"] = ms
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+    big = INTERFERENCE_REF_ROWS[-1]
+    scale = N / big
+    # deviation of the engine from fp64 on a subsample, dictionary 0 (the drop-in on the same code)
+    c = lds[0].encode(x[:big].float())
+    want = IO.expected_interference(w0, c)
+    got = S.calc_expected_interference(w0, c)
+    live = want != 0
+    l0 = float((c != 0).sum(1).float().mean())
+    name, limit = card_info(0)
+    print(json.dumps({
+        "metric": "ms per evaluation pass with the expected interference (evaluate_dicts(interference=True))",
+        "workload": args.workload, "desc": desc, "value": ms_with, "unit": "ms", "dictionaries": M, "n": n, "d": d,
+        "rows": N, "arith": args.arith, "steps": K, "warmup": W, "mean_l0_dict0": l0,
+        "without_interference_ms": ms_plain, "interference_ms": ms_with - ms_plain,
+        "mean_interference_dict0": float(r[0]["expected_interference"].mean()),
+        "dropin_deviation_from_fp64_rel": float(((got.double() - want) / want)[live].abs().max()),
+        "stock_torch_gpu_per_dictionary": dict(ref, scaled_fp32_ms=ref[f"fp32_ms_{big}_rows"] * scale,
+                                               scaled_tf32_ms=ref[f"tf32_ms_{big}_rows"] * scale, scaled_by=scale),
+        "speedup_vs_stock_fp32": ref[f"fp32_ms_{big}_rows"] * scale * M / ms_with,
+        "speedup_vs_stock_tf32": ref[f"tf32_ms_{big}_rows"] * scale * M / ms_with,
+        "gpu": name, "power_limit_w": limit,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="mmcs_cfg2",
                     choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS) + sorted(INTERP_WORKLOADS) +
-                    sorted(BASELINE_WORKLOADS) + sorted(TOPFVU_WORKLOADS))
+                    sorted(BASELINE_WORKLOADS) + sorted(TOPFVU_WORKLOADS) + sorted(INTERFERENCE_WORKLOADS))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
     args = ap.parse_args()
-    if args.workload in TOPFVU_WORKLOADS:
+    if args.workload in INTERFERENCE_WORKLOADS:
+        run_interference(args)
+    elif args.workload in TOPFVU_WORKLOADS:
         run_topfvu(args)
     elif args.workload in BASELINE_WORKLOADS:
         run_baselines(args)

@@ -5,7 +5,7 @@ NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v
 CSRC := sparse_coding_b200/csrc
 LIB := sparse_coding_b200/libsce.so
 # one object per family of entry points (make -j compiles them side by side)
-LIB_OBJS := $(patsubst %,build/%.o,sce_abi sce_plan sce_eval sce_track sce_similarity sce_rowpass)
+LIB_OBJS := $(patsubst %,build/%.o,sce_abi sce_plan sce_eval sce_track sce_similarity sce_rowpass sce_correlation)
 
 all: $(LIB)
 

@@ -43,7 +43,9 @@ extern "C" {
  * 201 also covers the additive entry points sce_forward_split_workspace_bytes / sce_forward_split (the top- and
  * rest-feature FVU) and the constant SCE_SPLIT_MAX_TOP. Every other entry point is unchanged.
  * 201 also covers the additive entry points sce_interference_workspace_bytes / sce_code_interference and
- * sce_expected_interference_workspace_bytes / sce_expected_interference (the expected interference). */
+ * sce_expected_interference_workspace_bytes / sce_expected_interference (the expected interference).
+ * 201 also covers the additive entry points sce_cross_moments_workspace_bytes / sce_cross_moments and
+ * sce_correlation_finish (the correlation of two dictionaries' codes). Every other entry point is unchanged. */
 #define SCE_VERSION 201 /* major*10000 + minor*100 + patch */
 
 typedef enum sce_status {
@@ -377,6 +379,38 @@ int sce_code_interference(sce_plan* plan, int B, double* cap_sums, long long* nz
 size_t sce_expected_interference_workspace_bytes(int n, int d, int B);
 int sce_expected_interference(const float* dict, int n, int d, const float* code, int B, double* cap_sums,
                               long long* nz_counts, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Cross-code moments of two plans (inter_dict_connections.ipynb's covariance cell): after a sce_forward_stats call of
+ * each plan on the same B paired rows (row r of plan_a's batch paired with row r of plan_b's), for every model pair
+ * (i, j), with C_a[i] [B, n_a] and C_b[j] [B, n_b] the codes those calls left in the plans,
+ *   acc[i][j][p][q]  device fp64 [M_a][M_b][n_a][n_b], ACCUMULATED: += sum over the B rows of C_a[i][r, p] C_b[j][r, q]
+ * The operands are the code planes the plans hold (the dense code never reaches memory); the product runs on the weight
+ * gradient's GEMM over slices of at most 2048 rows, each summed in fp32 on the tensor cores and added in fp64 in slice
+ * order: bitwise repeatable. Padding columns of a plan (coef_mask) hold 0 and add 0. The per-feature sums and sums of
+ * squares are the moment sums sce_forward_stats already made. plan_a may be plan_b.
+ *   B            in [1, min(batch_max)]: the rows of both plans' last calls
+ *   workspace    >= sce_cross_moments_workspace_bytes(plan_a, plan_b, B), 1024-byte aligned: one fp32 partial
+ *                n_a n_b 4 bytes (n = 4096: 64 MiB). Host-only; returns 0 unless both plans are evaluable, resolved to the
+ *                same arithmetic on the same device, and B fits both.
+ * Not available for SCE_TIED_LEARNED_CENTER, nor with desc.encoder_nonneg or desc.input_shift, as sce_forward_stats;
+ * nor after a training step (the call must follow sce_forward_stats). Asynchronous on `stream`. */
+size_t sce_cross_moments_workspace_bytes(const sce_plan* plan_a, const sce_plan* plan_b, int B);
+int sce_cross_moments(sce_plan* plan_a, sce_plan* plan_b, int B, double* acc, void* workspace, size_t workspace_bytes,
+                      void* stream);
+
+/* The correlation of one model pair from its fp64 sums over N = rows rows, without a plan: with mean = s1 / N,
+ * var = s2 / N - mean^2 per feature and cov[p][q] = acc[p * lda + q] / N - mean_a[p] mean_b[q] (fp64),
+ *   corr[p][q] = cov[p][q] / sqrt(var_a[p] var_b[q]), NaN unless both variances are > 0
+ *   corr, cov      device fp32 [n_a][n_b], each optional (NULL: not written)
+ *   max_ab[p], arg_ab[p]  device fp32 / int64 [n_a]: the largest corr[p][:] and its column; NaN entries are skipped, equal
+ *                  values go to the lower index, and a row with no defined entry gets NaN and -1
+ *   max_ba, arg_ba device fp32 / int64 [n_b]: the same over the columns corr[:][q]
+ *   sums_a, sums_b device fp64 [n_a][4] / [n_b][4]: sce_forward_stats' moment sums of one model (s1, s2 read)
+ *   lda            >= n_b: the row pitch of acc (a plan's padded n_b; only the first n_b columns are read)
+ * The maxima are taken in fp64 over the values corr holds before rounding. Deterministic; asynchronous on `stream`. */
+int sce_correlation_finish(const double* acc, int n_a, int n_b, int lda, const double* sums_a, const double* sums_b,
+                           long long rows, float* corr, float* cov, float* max_ab, long long* arg_ab, float* max_ba,
+                           long long* arg_ba, void* stream);
 
 /* Dead-feature resampling (experiments/huge_batch_size.py:120-146 WorstIndices, :189-250 process_reinit), per model m,
  * over a WINDOW of tracked steps (the sce_step_tracked calls since the caller emptied the lists, or since sce_resample):

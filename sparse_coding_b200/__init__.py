@@ -8,7 +8,7 @@ on-device metrics (metrics.py) and the synthetic datasets of sc_datasets/random_
 (synthetic.py)."""
 from . import metrics
 from .metrics import (batched_calc_feature_n_ever_active, calc_expected_interference, calc_moments_streaming,
-                      evaluate_dicts,
+                      code_correlation, evaluate_dicts,
                       fraction_variance_unexplained, fraction_variance_unexplained_top_activating,
                       mean_nonzero_activations, r_squared, top_activating_fragments)
 from .ensemble import CodeProxy, FunctionalEnsemble, optim_str_to_func, stack_dict, unstack_dict
@@ -27,7 +27,7 @@ __all__ = [
     "FunctionalPositiveTiedSAE", "FunctionalSAE", "FunctionalTiedCenteredSAE", "FunctionalTiedSAE", "LearnedDict",
     "TiedSAE", "TopKEncoder", "TopKLearnedDict", "UntiedSAE",
     "adam", "batched_calc_feature_n_ever_active", "calc_expected_interference", "calc_moments_streaming",
-    "evaluate_dicts",
+    "code_correlation", "evaluate_dicts",
     "fraction_variance_unexplained", "fraction_variance_unexplained_top_activating", "mean_nonzero_activations", "optim_str_to_func", "r_squared", "stack_dict",
     "top_activating_fragments", "unstack_dict",
     "RandomDatasetGenerator", "SparseMixDataset", "SyntheticChunks", "generate_corr_matrix",

@@ -35,7 +35,7 @@ EXPORTS = [
     "sce_similarity_workspace_bytes", "sce_similarity", "sce_forward_stats_workspace_bytes", "sce_forward_stats",
     "sce_fragments_workspace_bytes", "sce_forward_fragments", "sce_forward_split_workspace_bytes", "sce_forward_split",
     "sce_interference_workspace_bytes", "sce_code_interference", "sce_expected_interference_workspace_bytes",
-    "sce_expected_interference",
+    "sce_expected_interference", "sce_cross_moments_workspace_bytes", "sce_cross_moments", "sce_correlation_finish",
     "sce_synth_rows", "sce_read_center_grad",
     "sce_second_moments_workspace_bytes", "sce_second_moments", "sce_ica_pass_workspace_bytes", "sce_ica_pass",
     "sce_nmf_project_workspace_bytes", "sce_nmf_project", "sce_nmf_grams_workspace_bytes", "sce_nmf_grams",
@@ -222,6 +222,10 @@ def load():
     lib.sce_expected_interference_workspace_bytes.restype = C.c_size_t
     lib.sce_expected_interference_workspace_bytes.argtypes = [i, i, i]
     lib.sce_expected_interference.argtypes = [vp, i, i, vp, i, vp, vp, vp, C.c_size_t, vp]
+    lib.sce_cross_moments_workspace_bytes.restype = C.c_size_t
+    lib.sce_cross_moments_workspace_bytes.argtypes = [vp, vp, i]
+    lib.sce_cross_moments.argtypes = [vp, vp, i, vp, vp, C.c_size_t, vp]
+    lib.sce_correlation_finish.argtypes = [vp, i, i, i, vp, vp, ll, vp, vp, vp, vp, vp, vp, vp]
     lib.sce_synth_rows.argtypes = [vp, i, i, vp, i, ll, i, C.c_ulonglong, i, f, vp, i, vp, vp, vp, i, vp]
     lib.sce_second_moments_workspace_bytes.restype = C.c_size_t
     lib.sce_second_moments_workspace_bytes.argtypes = [i, i]

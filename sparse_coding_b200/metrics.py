@@ -807,6 +807,152 @@ def calc_moments_streaming(learned_dict, activations: torch.Tensor, batch_size: 
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# Correlation of two dictionaries' features over paired activations (inter_dict_connections.ipynb, the cell that
+# "iteratively build[s] covariance matrixes for encodings"): per pair of dictionaries, the fp64 cross sums C_a^T C_b of
+# their codes, summed from the code planes each forward-only plan holds (libsce ``sce_cross_moments``), with the
+# per-feature sums of the statistics pass; correlation, covariance and best matches are formed on the device
+# (``sce_correlation_finish``). The dense [N, n] code is never formed.
+# ---------------------------------------------------------------------------------------------------------------------
+class _CodePlan(_DictPlan):
+    """A dictionary plan whose calls leave their code for ``sce_cross_moments`` and add to its moment sums."""
+
+    def __init__(self, key, lds, batch_max, arith, dev):
+        super().__init__(key, lds, batch_max, arith, dev)
+        M, n = self.M, self.n
+        self.ws_bytes = _lib.load().sce_forward_stats_workspace_bytes(C.byref(self.desc), batch_max)
+        self._pass_ws, self.ws_ptr = _lib.workspace(self.ws_bytes, dev, "sce_forward_stats_workspace_bytes")
+        self.sums = torch.zeros(M, n, 4, dtype=torch.float64, device=dev)
+        self.seg_counts = torch.zeros(M, n, dtype=torch.int32, device=dev)
+        self.losses = torch.empty(M, _lib.SCE_LOSS_COLS, dtype=torch.float32, device=dev)
+        self.nnz = torch.empty(M, dtype=torch.float32, device=dev)
+
+    def run(self, x):
+        _lib.check(_lib.load().sce_forward_stats(
+            self.plan, self.batch(x).data_ptr(), x.shape[0], 1, 0, None, self.losses.data_ptr(), self.nnz.data_ptr(),
+            self.sums.data_ptr(), self.seg_counts.data_ptr(), None, self.ws_ptr, self.ws_bytes, self.stream),
+            "sce_forward_stats")
+
+
+def _dict_list(x):
+    """A LearnedDict, a ``(LearnedDict, hparams)`` pair, or a list of either -> a list."""
+    if isinstance(x, tuple) and len(x) == 2 and isinstance(x[1], dict):
+        return [x]
+    return list(x) if isinstance(x, (list, tuple)) else [x]
+
+
+def _cross_moment_bytes(shapes_a, shapes_b, full):
+    """(accumulator bytes, workspace bytes, output bytes) of every pair of the plan shapes ``(M, n_pad)`` of the two
+    sides: fp64 [M_a, M_b, n_a, n_b] per plan pair, one fp32 [n_a, n_b] partial for the largest pair, and with ``full``
+    the fp32 correlation and covariance of every dictionary pair."""
+    acc = sum(8 * Ma * Mb * na * nb for Ma, na in shapes_a for Mb, nb in shapes_b)
+    ws = max(-(-4 * na * nb // 1024) * 1024 + 1024 for _, na in shapes_a for _, nb in shapes_b)
+    out = sum(2 * 4 * Ma * Mb * na * nb for Ma, na in shapes_a for Mb, nb in shapes_b) if full else 0
+    return acc, ws, out
+
+
+def _check_cross_memory(need: int, free: int):
+    if need > free:
+        raise ValueError(f"code_correlation: the cross-moment accumulators, workspace and outputs need {need} bytes, "
+                         f"more than the {free} bytes free on the device: pass fewer dictionaries per call, or "
+                         "full=False")
+
+
+def code_correlation(a, x_a: torch.Tensor, b, x_b: Optional[torch.Tensor] = None, *, full: bool = True,
+                     arith: str = "auto"):
+    """The correlation of the features of dictionaries ``a`` with those of ``b`` over paired activations, for every pair
+    of ``a × b`` in one pass over the rows (inter_dict_connections.ipynb's covariance cell, as its text intends: the
+    population Pearson correlation over all N rows; SURVEY Q16).
+
+    ``a``, ``b``: a LearnedDict, a ``(LearnedDict, hparams)`` pair, or a list of either, of every kind
+    :func:`evaluate_dicts` runs. ``x_a`` [N, d_a] and ``x_b`` [N, d_b] (fp32 or fp16, on the CPU or a CUDA device, both
+    on one device): row r of one is paired with row r of the other; ``x_b=None``: ``b`` encodes ``x_a``. The codes are
+    ``ld.encode(x)`` of the rows as given (no ``center``). ``arith``: the engine's operand arithmetic; "auto" runs bf16x3.
+
+    Returns a nested list ``[i][j]`` of dicts, with tensors on the device of ``x_a``:
+      ``mean_a``, ``var_a`` [n_a] and ``mean_b``, ``var_b`` [n_b] fp64: population moments over the N rows
+      ``correlation`` and ``covariance`` [n_a, n_b] fp32 (population form, sums over N), only with ``full=True``
+      ``max_corr_ab`` [n_a] fp32 and ``argmax_ab`` [n_a] int64: each feature of a's most correlated feature of b;
+      ``max_corr_ba`` / ``argmax_ba`` the same the other way round
+      ``rows``: N
+    A correlation is NaN where either variance is 0. The maxima skip NaN entries and give equal values to the lower
+    index; a feature with no defined entry gets NaN and index -1. The cross sums are fp64 sums of fp32 slice products
+    of at most 2048 rows on the tensor cores: bitwise repeatable. The accumulators take 8 n_a n_b bytes per pair on the
+    device; a call whose accumulators, workspace and outputs exceed the free device memory raises ``ValueError``."""
+    lds_a, lds_b = _dict_list(a), _dict_list(b)
+    xs = [x_a] + ([] if x_b is None else [x_b])
+    for name, x in zip(("x_a", "x_b"), xs):
+        if not torch.is_tensor(x):
+            raise TypeError(f"{name} must be a tensor")
+    if x_b is not None:
+        if x_b.dim() == 2 and x_a.dim() == 2 and x_b.shape[0] != x_a.shape[0]:
+            raise ValueError(f"x_a and x_b must hold the same number of paired rows, got {x_a.shape[0]} and "
+                             f"{x_b.shape[0]}")
+        if x_b.device != x_a.device:
+            raise ValueError(f"x_a and x_b must be on one device, got {x_a.device} and {x_b.device}")
+    if not isinstance(full, (bool, np.bool_)):
+        raise ValueError(f"full must be True or False, got {full!r}")
+    lds_a, groups_a, ar = _dict_inputs(lds_a, x_a, arith, centre=False)
+    lds_b, groups_b, _ = _dict_inputs(lds_b, x_a if x_b is None else x_b, arith, centre=False)
+    dev = _cuda_device(x_a, "code correlation")
+    N = x_a.shape[0]
+    share = x_b is None and len(lds_a) == len(lds_b) and all(p is q for p, q in zip(lds_a, lds_b))
+    cuts = [(s, min(s + _EVAL_ROWS, N)) for s in range(0, N, _EVAL_ROWS)]
+    batch_max = max(e - s for s, e in cuts)
+    shapes = lambda groups: [(len(idx), key[1]) for key, idx in groups.items()]
+    need = sum(_cross_moment_bytes(shapes(groups_a), shapes(groups_b), bool(full)))
+    with torch.cuda.device(dev):
+        _check_cross_memory(need, torch.cuda.mem_get_info(dev)[0])
+    make = lambda key, g: _CodePlan(key, g, batch_max, ar, dev)
+    lib = _lib.load()
+    with contextlib.ExitStack() as stack:
+        plans_a = stack.enter_context(_plans(groups_a, lds_a, dev, make))
+        plans_b = plans_a if share else stack.enter_context(_plans(groups_b, lds_b, dev, make))
+        pairs = [(pa, pb) for pa, _ in plans_a for pb, _ in plans_b]
+        acc = [torch.zeros(pa.M, pb.M, pa.n, pb.n, dtype=torch.float64, device=dev) for pa, pb in pairs]
+        ws_bytes = max(lib.sce_cross_moments_workspace_bytes(pa.plan, pb.plan, batch_max) for pa, pb in pairs)
+        cross_ws, ws_ptr = _lib.workspace(ws_bytes, dev, "sce_cross_moments_workspace_bytes")
+        stream = plans_a[0][0].stream
+        rows_b = _eval_rows(x_b, dev, cuts) if x_b is not None else None
+        for xa in _eval_rows(x_a, dev, cuts):
+            for p, _ in plans_a:
+                p.run(xa)
+            if not share:
+                xb = xa if x_b is None else next(rows_b)
+                for p, _ in plans_b:
+                    p.run(xb)
+            for (pa, pb), s in zip(pairs, acc):
+                _lib.check(lib.sce_cross_moments(pa.plan, pb.plan, xa.shape[0], s.data_ptr(), ws_ptr, ws_bytes, stream),
+                           "sce_cross_moments")
+        _check_f16f8_range(plans_a + ([] if share else plans_b), ar)
+        del cross_ws
+        results = [[None] * len(lds_b) for _ in lds_a]
+        moments = lambda s: (s[:, 0] / N, s[:, 1] / N - (s[:, 0] / N) ** 2)
+        for (pa, pb), s in zip(pairs, acc):
+            ia, ib = next(i for p, i in plans_a if p is pa), next(i for p, i in plans_b if p is pb)
+            for k, i in enumerate(ia):
+                na = int(lds_a[i].n_feats)
+                for m, j in enumerate(ib):
+                    nb = int(lds_b[j].n_feats)
+                    out = {"rows": N}
+                    out["mean_a"], out["var_a"] = moments(pa.sums[k, :na])
+                    out["mean_b"], out["var_b"] = moments(pb.sums[m, :nb])
+                    corr = torch.empty(na, nb, dtype=torch.float32, device=dev) if full else None
+                    cov = torch.empty(na, nb, dtype=torch.float32, device=dev) if full else None
+                    mx_ab, mx_ba = (torch.empty(c, dtype=torch.float32, device=dev) for c in (na, nb))
+                    ag_ab, ag_ba = (torch.empty(c, dtype=torch.int64, device=dev) for c in (na, nb))
+                    ptr = lambda t: t.data_ptr() if t is not None else None
+                    _lib.check(lib.sce_correlation_finish(
+                        s[k, m].data_ptr(), na, nb, pb.n, pa.sums[k].data_ptr(), pb.sums[m].data_ptr(), N, ptr(corr),
+                        ptr(cov), mx_ab.data_ptr(), ag_ab.data_ptr(), mx_ba.data_ptr(), ag_ba.data_ptr(), stream),
+                        "sce_correlation_finish")
+                    if full:
+                        out["correlation"], out["covariance"] = corr, cov
+                    out.update(max_corr_ab=mx_ab, argmax_ab=ag_ab, max_corr_ba=mx_ba, argmax_ba=ag_ba)
+                    results[i][j] = _to_device(out, x_a.device)
+    return results
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # Record selection for reading what features mean (interpret.py:82-212 make_feature_activation_dataset, :265-321
 # interpret): per feature, the fragments with the largest maximum and a random sample of the fragments in which it fires,
 # with their per-token code values (libsce ``sce_forward_fragments``). The [N, n] code and the reference's F·L·N fp16

@@ -13,12 +13,14 @@
   interference_cfg2: the expected interference (big_sweep.py calc_expected_interference) of the config-2 dictionaries.
           One pass = metrics.evaluate_dicts(interference=True); the difference to the call without it is the cost of the
           interference kernels.
+  corr_*: the correlation of two dictionaries' features over paired rows (inter_dict_connections.ipynb's covariance
+          cell). One pass = metrics.code_correlation of every pair over every row.
   *_baselines: the same two passes on the baselines of sweep_baselines.py: one ICAEncoder, RandomDict(512) and
           IdentityReLU(512) at d = 512, in one pass (2^20 rows / 50 000 fragments of 64 rows).
 
     python tools/bench_metrics.py --workload mmcs_cfg2|mmcs_cfg5|eval_cfg2|eval_cfg5|interp_cfg2|interp_cfg5|
                                              eval_baselines|interp_baselines|topfvu_cfg2|
-                                             interference_cfg2 [--steps K --warmup W --arith ...]
+                                             interference_cfg2|corr_nb|corr_cfg2 [--steps K --warmup W --arith ...]
 
 Prints one JSON line: CUDA-event ms per pass, algorithmic TFLOP/s (2 n_a n_b d per pair and per capacity), the same
 computation as fp32 einsums + maxima and again with TF32 allowed, the maximum deviation of each from an fp64 result, and
@@ -606,16 +608,114 @@ def run_interference(args):
     }), flush=True)
 
 
+CORR_WORKLOADS = {
+    # name: (n_up, n_base, n_down, d, rows, description)
+    "corr_nb": (2048, 512, 2048, 512, 1 << 20, "the notebook's case: an upstream TiedSAE (2048 x 512) and a RandomDict(512) "
+                                                "against a downstream TiedSAE (2048 x 512), 2^20 paired fp16 rows"),
+    "corr_cfg2": (4096, 0, 4096, 512, 1 << 20, "two seeded config-2 TiedSAE dictionaries (4096 x 512), 2^20 paired fp16 "
+                                                "rows"),
+}
+CORR_REF_ROWS = 1 << 17     # rows the cell's op sequence is timed on, scaled to the workload's
+CORR_CHECK_ROWS = 1 << 14   # subsample of the fp64 comparison
+
+
+def run_corr(args):
+    """code_correlation of every pair against the cell's op sequence on the same GPU (three fp32 encodes per batch of
+    8192 rows, the per-feature sums and squares, and two dense [n, B] x [B, n] cross products, then the correlation),
+    in fp32 and in TF32, timed on CORR_REF_ROWS rows and scaled. The deviation of each from fp64 is measured on
+    CORR_CHECK_ROWS rows, where the engine runs on the same subsample."""
+    import sparse_coding_b200 as S
+    from sparse_coding_b200 import metrics as MT
+    from sparse_coding_b200.learned_dict import RandomDict
+
+    dev, K, W = setup(args)
+    n_up, n_base, n_down, d, N, desc = CORR_WORKLOADS[args.workload]
+    up = S.FunctionalTiedSAE.to_learned_dict(*make_models(S.FunctionalTiedSAE, 1, d, n_up, seed=0)[0])
+    down = S.FunctionalTiedSAE.to_learned_dict(*make_models(S.FunctionalTiedSAE, 1, d, n_down, seed=1)[0])
+    torch.manual_seed(2)
+    a = [up] + ([RandomDict(d, n_base)] if n_base else [])
+    for ld in a + [down]:
+        ld.to_device(dev)
+    x_a = activations(N, d, dev)
+    mix = torch.randn(d, d, generator=torch.Generator(device=dev).manual_seed(3), device=dev) / d ** 0.5
+    x_b = torch.empty_like(x_a)
+    for i in range(0, N, 1 << 16):          # the next layer: a fixed mixing of this one, plus noise
+        x_b[i:i + (1 << 16)] = (x_a[i:i + (1 << 16)].float() @ mix + 0.05 * torch.randn(min(1 << 16, N - i), d,
+                                                                                         device=dev)).half()
+    ms, _ = timed(lambda: MT.code_correlation(a, x_a, [down], x_b, arith=args.arith), K, W)
+
+    def stock(xa, xb):
+        """the cell's sequence, with the moments centred as it intends"""
+        sums = [None] * len(a)
+        cross = [None] * len(a)
+        sd = None
+        for i in range(0, xa.shape[0], 8192):
+            cd = down.encode(xb[i:i + 8192].float())
+            sd = torch.stack([cd.sum(0), (cd * cd).sum(0)]) + (0 if sd is None else sd)
+            for k, ld in enumerate(a):
+                c = ld.encode(xa[i:i + 8192].float())
+                s = torch.stack([c.sum(0), (c * c).sum(0)])
+                sums[k] = s if sums[k] is None else sums[k] + s
+                cross[k] = c.T @ cd if cross[k] is None else cross[k] + c.T @ cd
+        rows = xa.shape[0]
+        out = []
+        for k in range(len(a)):
+            ma, mb = sums[k][0] / rows, sd[0] / rows
+            va, vb = sums[k][1] / rows - ma * ma, sd[1] / rows - mb * mb
+            out.append((cross[k] / rows - ma[:, None] * mb[None, :]) / torch.sqrt(torch.outer(va, vb)))
+        return out
+
+    ref, dev_corr = {}, {}
+    tf32 = torch.backends.cuda.matmul.allow_tf32
+    xs_a, xs_b = x_a[:CORR_CHECK_ROWS], x_b[:CORR_CHECK_ROWS]
+    def fp64(ca, cb):     # the population correlation in fp64 on the device (oracle/correlation_oracle.py's formula)
+        ca, cb = ca.double(), cb.double()
+        ma, mb = ca.mean(0), cb.mean(0)
+        va, vb = (ca * ca).mean(0) - ma * ma, (cb * cb).mean(0) - mb * mb
+        return ((ca.T @ cb / ca.shape[0] - ma[:, None] * mb[None, :]) / torch.sqrt(torch.outer(va, vb))).cpu()
+
+    want = [fp64(ld.encode(xs_a.float()), down.encode(xs_b.float())) for ld in a]
+    defined = lambda t: t.nan_to_num(0.0).abs()
+    try:
+        for mode in ("fp32", "tf32"):
+            torch.backends.cuda.matmul.allow_tf32 = mode == "tf32"
+            ref[f"{mode}_ms_{CORR_REF_ROWS}_rows"], _ = timed(lambda: stock(x_a[:CORR_REF_ROWS], x_b[:CORR_REF_ROWS]), 2, 1)
+            got = stock(xs_a, xs_b)
+            dev_corr[mode] = max(float(defined(g.double().cpu() - w).max()) for g, w in zip(got, want))
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = tf32
+    eng = MT.code_correlation(a, xs_a, [down], xs_b, arith=args.arith)
+    dev_corr["engine"] = max(float(defined(eng[k][0]["correlation"].double().cpu() - w).max()) for k, w in enumerate(want))
+    scale = N / CORR_REF_ROWS
+    name, limit = card_info(0)
+    clock = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=clocks.max.sm,clocks.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True).stdout.strip()
+    print(json.dumps({
+        "metric": "ms per correlation pass (code_correlation of every pair over every row)", "workload": args.workload,
+        "desc": desc, "value": ms, "unit": "ms", "n_a": [ld.n_feats for ld in a], "n_b": n_down, "d": d, "rows": N,
+        "arith": args.arith, "steps": K, "warmup": W,
+        "stock_torch_gpu": dict(ref, scaled_fp32_ms=ref[f"fp32_ms_{CORR_REF_ROWS}_rows"] * scale,
+                                scaled_tf32_ms=ref[f"tf32_ms_{CORR_REF_ROWS}_rows"] * scale, scaled_by=scale),
+        "speedup_vs_stock_fp32": ref[f"fp32_ms_{CORR_REF_ROWS}_rows"] * scale / ms,
+        "speedup_vs_stock_tf32": ref[f"tf32_ms_{CORR_REF_ROWS}_rows"] * scale / ms,
+        "max_abs_corr_deviation_from_fp64": dev_corr, "check_rows": CORR_CHECK_ROWS,
+        "gpu": name, "power_limit_w": limit, "sm_clock_max_and_current_mhz": clock,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="mmcs_cfg2",
                     choices=sorted(MMCS_WORKLOADS) + sorted(EVAL_WORKLOADS) + sorted(INTERP_WORKLOADS) +
-                    sorted(BASELINE_WORKLOADS) + sorted(TOPFVU_WORKLOADS) + sorted(INTERFERENCE_WORKLOADS))
+                    sorted(BASELINE_WORKLOADS) + sorted(TOPFVU_WORKLOADS) + sorted(INTERFERENCE_WORKLOADS) +
+                    sorted(CORR_WORKLOADS))
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--arith", default="auto", choices=["auto", "bf16x3", "f16f8"])
     args = ap.parse_args()
-    if args.workload in INTERFERENCE_WORKLOADS:
+    if args.workload in CORR_WORKLOADS:
+        run_corr(args)
+    elif args.workload in INTERFERENCE_WORKLOADS:
         run_interference(args)
     elif args.workload in TOPFVU_WORKLOADS:
         run_topfvu(args)

@@ -368,6 +368,7 @@ int sce_forward_split(sce_plan* plan, const float* x, int B, int n_top, const in
  *               partials, M (n ceil(d / 32) 32 + 2 n ceil(B / 32)) fp32 (config 2, M = 16, n = 4096, d = 512, B = 8192:
  *               256 MiB). Host-only; returns 0 for an invalid desc or B outside [1, batch_max].
  * Not available for SCE_TIED_LEARNED_CENTER, nor with desc.encoder_nonneg or desc.input_shift, as sce_forward_stats.
+ * Refuses a plan whose last call was a training step, as sce_cross_moments does.
  * Asynchronous on `stream`. */
 size_t sce_interference_workspace_bytes(const sce_desc* desc, int B);
 int sce_code_interference(sce_plan* plan, int B, double* cap_sums, long long* nz_counts, void* workspace,

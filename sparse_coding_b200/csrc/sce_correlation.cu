@@ -31,8 +31,14 @@ __global__ void __launch_bounds__(256) cross_add_kernel(const float* __restrict_
   }
 }
 
-static bool cross_plans_ok(const sce_plan* a, const sce_plan* b) {
-  return a && b && a->cfg.evaluable && b->cfg.evaluable && a->cfg.arith == b->cfg.arith && a->device == b->device;
+// The two plans of a cross-moments call and of its workspace query: each evaluable, one arithmetic, one device
+static int check_cross_plans(const sce_plan* a, const sce_plan* b) {
+  TRY(check_evaluable(a, "cross_moments: plan_a: "));
+  TRY(check_evaluable(b, "cross_moments: plan_b: "));
+  if (a->cfg.arith != b->cfg.arith)
+    return fail(SCE_ERR_INVALID, "cross_moments: the two plans resolved to different arithmetics");
+  if (a->device != b->device) return fail(SCE_ERR_INVALID, "cross_moments: the two plans live on different devices");
+  return SCE_OK;
 }
 
 template <int AR>
@@ -161,7 +167,7 @@ __global__ void __launch_bounds__(256) corr_cols_kernel(CorrArgs a, float* __res
 extern "C" {
 
 size_t sce_cross_moments_workspace_bytes(const sce_plan* a, const sce_plan* b, int B) {
-  if (!cross_plans_ok(a, b) || B < 1 || B > a->d.batch_max || B > b->d.batch_max) return 0;
+  if (!a || !b || check_cross_plans(a, b) || B < 1 || B > a->d.batch_max || B > b->d.batch_max) return 0;
   return align_up((size_t)a->d.n * b->d.n * sizeof(float), 1024);
 }
 
@@ -169,15 +175,11 @@ int sce_cross_moments(sce_plan* a, sce_plan* b, int B, double* acc, void* worksp
                       void* stream) {
   // ---- arguments (all checked before any CUDA call)
   if (!a || !b || !acc) return fail(SCE_ERR_INVALID, "cross_moments: plan_a, plan_b and acc are required");
-  if (!a->cfg.evaluable || !b->cfg.evaluable)
-    return fail(SCE_ERR_INVALID, "cross_moments: not available for learned-centre, encoder_nonneg or input_shift plans");
-  if (a->cfg.arith != b->cfg.arith)
-    return fail(SCE_ERR_INVALID, "cross_moments: the two plans resolved to different arithmetics");
-  if (a->device != b->device) return fail(SCE_ERR_INVALID, "cross_moments: the two plans live on different devices");
+  TRY(check_cross_plans(a, b));
   TRY(check_rows(a, B, "cross_moments: plan_a: "));
   TRY(check_rows(b, B, "cross_moments: plan_b: "));
-  if (a->code_batch_major || b->code_batch_major)
-    return fail(SCE_ERR_INVALID, "cross_moments: a plan's last call was a training step; follow sce_forward_stats");
+  TRY(check_forward_code(a, "cross_moments: plan_a: "));
+  TRY(check_forward_code(b, "cross_moments: plan_b: "));
   if (reinterpret_cast<uintptr_t>(acc) % 8) return fail(SCE_ERR_INVALID, "cross_moments: acc must be 8-byte aligned");
   TRY(check_workspace(workspace, workspace_bytes, sce_cross_moments_workspace_bytes(a, b, B), "cross_moments: "));
 

@@ -2,6 +2,8 @@
 // (sce_active_counts), the evaluation statistics of a forward pass (sce_forward_stats), its top-activating and
 // random activating fragments (sce_forward_fragments), the top- and rest-feature errors (sce_forward_split) and the
 // expected interference of its code (sce_code_interference; sce_expected_interference for a caller-held code).
+#include <vector>
+
 #include "sce_plan.cuh"
 
 namespace sce {
@@ -189,6 +191,14 @@ template <int SRC>
 static CodeView<SRC> code_view(const sce_plan* p) {
   return {p->c.hi, p->c.lo, SRC == kCodeBatchMajor ? p->ct.x8 : p->c.x8, p->scores, p->act_pos, (p->d.n + 31) / 32,
           p->d.batch_max, p->d.n, p->cfg.bpad};
+}
+
+// Calls f(std::integral_constant<int, SRC>) with the source of the code a forward call leaves: top-k plans' scores, the
+// arithmetic's row-major planes otherwise (a forward pass leaves them row-major, check_forward_code)
+template <class F>
+static int with_forward_code(const sce_plan* p, F&& f) {
+  if (p->cfg.topk) return f(std::integral_constant<int, kCodeScores>{});
+  return with_arith(p->cfg.arith, f);
 }
 
 // out [M][B][n] fp32 = the code of the B rows of the last call. Grid (<= 1024, M), two adjacent columns per thread.
@@ -747,7 +757,8 @@ int sce_read_code(sce_plan* p, int B, float* out_code, void* stream) {
     return L.launch(read_code_kernel<SRC>, dim3((unsigned)(blocks < 1024 ? blocks : 1024), p->d.n_models), 256, 0,
                     code_view<SRC>(p), B, out_code);
   };
-  // (top-k plans too: the selection writes their code planes)
+  // Not with_forward_code: this call also serves the code of a training step (FunctionalEnsemble's aux["c"]), whose
+  // dw_native backward leaves the residual plane batch-major only; top-k plans read the planes their selection wrote.
   if (p->code_batch_major) return read(std::integral_constant<int, kCodeBatchMajor>{});
   return with_arith(p->cfg.arith, read);
 }
@@ -764,16 +775,19 @@ int sce_active_counts(sce_plan* plan, int B, int* counts, void* stream) {
 // The checks that open sce_forward_stats and sce_forward_fragments; `prefix` names the entry point in the messages
 static int check_forward_only(const sce_plan* p, const float* x, int B, const char* prefix) {
   if (!p) return fail(SCE_ERR_INVALID, "%splan is NULL", prefix);
-  if (!p->cfg.evaluable)
-    return fail(SCE_ERR_INVALID, "%snot available for the learned-centre variant or with encoder_nonneg / input_shift; "
-                                 "evaluate the exported dictionaries (TiedSAE)", prefix);
+  TRY(check_evaluable(p, prefix));
   TRY(check_rows(p, B, prefix));
   if (!x) return fail(SCE_ERR_INVALID, "%sx is NULL", prefix);
   return SCE_OK;
 }
 
+// What every forward-only workspace query asks of its descriptor and rows: valid, evaluable, B in [1, batch_max]
+static bool forward_only_query_ok(const sce_desc* desc, int B) {
+  return !validate(desc) && B >= 1 && B <= desc->batch_max && plan_config(*desc).evaluable;
+}
+
 size_t sce_forward_stats_workspace_bytes(const sce_desc* desc, int B) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !plan_config(*desc).evaluable) return 0;
+  if (!forward_only_query_ok(desc, B)) return 0;
   return stats_carve(nullptr, *desc, B, nullptr);
 }
 
@@ -808,7 +822,7 @@ int sce_forward_stats(sce_plan* p, const float* x, int B, int seg, int seg_phase
 }
 
 size_t sce_fragments_workspace_bytes(const sce_desc* desc, int B, int L) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !frag_len_ok(L) || B % L || !plan_config(*desc).evaluable) return 0;
+  if (!forward_only_query_ok(desc, B) || !frag_len_ok(L) || B % L) return 0;
   return frag_carve(nullptr, *desc, B, L, nullptr);
 }
 
@@ -835,13 +849,11 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
   TRY(run_pipeline(call, p, x, B, static_cast<cudaStream_t>(stream), nullptr, false, nullptr, nullptr));
   p->last_launches = call.count;   // the pipeline's: the fragment kernels below are not counted
   const int n_chunks = (d.n + 31) / 32, G = B / L;
-  auto fragments = [&](auto src) {
+  TRY(with_forward_code(p, [&](auto src) {
     constexpr int SRC = decltype(src)::value;
     return launch_fragments<SRC>(call, code_view<SRC>(p), p->cfg.linear, d.n_models, L, G, frag0, w.fmax, w.active, n_top, n_random,
                                  seed, top_val, top_frag, top_act, rnd_key, rnd_frag, rnd_act);
-  };
-  // (a forward pass leaves the code planes row-major)
-  TRY(p->cfg.topk ? fragments(std::integral_constant<int, kCodeScores>{}) : with_arith(p->cfg.arith, fragments));
+  }));
   // active fragments: segments of L rows, cut at fragment boundaries (phase 0, no segment stays open)
   CUDA_TRY(cudaMemsetAsync(w.open, 0, (size_t)d.n_models * d.n * sizeof(int), call.st));
   return call.launch(segment_count_kernel, dim3(n_chunks, d.n_models), 256, 0, p->act_pos, n_chunks, d.batch_max, B, d.n,
@@ -849,8 +861,7 @@ int sce_forward_fragments(sce_plan* p, const float* x, int B, int L, long long f
 }
 
 size_t sce_forward_split_workspace_bytes(const sce_desc* desc, int B, int n_top) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !split_top_ok(*desc, n_top) || !plan_config(*desc).evaluable)
-    return 0;
+  if (!forward_only_query_ok(desc, B) || !split_top_ok(*desc, n_top)) return 0;
   return split_carve(nullptr, *desc, B, n_top, nullptr);
 }
 
@@ -869,24 +880,21 @@ int sce_forward_split(sce_plan* p, const float* x, int B, int n_top, const int* 
   const size_t need = split_carve(static_cast<uint8_t*>(workspace), d, B, n_top, &w);
   if (int rc = check_workspace(workspace, workspace_bytes, need, "forward_split: ")) return rc;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the columns are checked on the host before anything is launched
+  // the columns are checked on the host before anything is launched: each in [0, n), none twice in a model's list
   const int M = d.n_models;
-  int* cols = static_cast<int*>(std::malloc(sizeof(int) * M * n_top));
-  if (!cols) return fail(SCE_ERR_INVALID, "forward_split: out of host memory");
-  cudaError_t e = cudaMemcpyAsync(cols, top_cols, sizeof(int) * M * n_top, cudaMemcpyDeviceToHost, st);
+  std::vector<int> cols((size_t)M * n_top);
+  cudaError_t e = cudaMemcpyAsync(cols.data(), top_cols, sizeof(int) * cols.size(), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  int bad = e == cudaSuccess ? SCE_OK : fail(SCE_ERR_CUDA, "forward_split: reading top_cols: %s", cudaGetErrorString(e));
-  for (int m = 0; m < M && !bad; ++m)
-    for (int s = 0; s < n_top && !bad; ++s) {
+  if (e != cudaSuccess) return fail(SCE_ERR_CUDA, "forward_split: reading top_cols: %s", cudaGetErrorString(e));
+  for (int m = 0; m < M; ++m)
+    for (int s = 0; s < n_top; ++s) {
       const int j = cols[m * n_top + s];
       if (j < 0 || j >= d.n)
-        bad = fail(SCE_ERR_INVALID, "forward_split: top_cols[%d][%d] = %d outside [0, n = %d)", m, s, j, d.n);
-      for (int s2 = 0; s2 < s && !bad; ++s2)
+        return fail(SCE_ERR_INVALID, "forward_split: top_cols[%d][%d] = %d outside [0, n = %d)", m, s, j, d.n);
+      for (int s2 = 0; s2 < s; ++s2)
         if (cols[m * n_top + s2] == j)
-          bad = fail(SCE_ERR_INVALID, "forward_split: column %d appears twice in top_cols[%d]", j, m);
+          return fail(SCE_ERR_INVALID, "forward_split: column %d appears twice in top_cols[%d]", j, m);
     }
-  std::free(cols);
-  if (bad) return bad;
   PlanCall c;
   float* xh = x_hat ? x_hat : w.x_hat;
   TRY(run_pipeline(c, p, x, B, st, xh, false, nullptr, nullptr));
@@ -897,13 +905,11 @@ int sce_forward_split(sce_plan* p, const float* x, int B, int n_top, const int* 
   TRY(c.launch(chosen_rows_kernel, dim3(n_top, M), 128, 0, dict, top_cols, d.n, d.d, n_top, cfg.raw_decoder ? 0 : 1,
                d.norm_floor, w.d_top));
   const long long blocks = ((long long)B * n_top + 255) / 256;
-  auto columns = [&](auto src) {
+  TRY(with_forward_code(p, [&](auto src) {
     constexpr int SRC = decltype(src)::value;
     return c.launch(code_columns_kernel<SRC>, dim3((unsigned)(blocks < 1024 ? blocks : 1024), M), 256, 0, code_view<SRC>(p),
                     B, n_top, top_cols, w.c_top);
-  };
-  // (a forward pass leaves the code planes row-major)
-  TRY(cfg.topk ? columns(std::integral_constant<int, kCodeScores>{}) : with_arith(cfg.arith, columns));
+  }));
   const int row_blocks = (B + 31) / 32;
   TRY(c.launch(split_residual_kernel, dim3(row_blocks, M), 256, 0, x, cfg.x_models ? (long long)B * d.d : 0LL, xh, w.c_top,
                w.d_top, B, d.d, n_top, x_hat_top, centred ? nullptr : w.part));
@@ -912,17 +918,16 @@ int sce_forward_split(sce_plan* p, const float* x, int B, int n_top, const int* 
 }
 
 size_t sce_interference_workspace_bytes(const sce_desc* desc, int B) {
-  if (validate(desc) || B < 1 || B > desc->batch_max || !plan_config(*desc).evaluable) return 0;
+  if (!forward_only_query_ok(desc, B)) return 0;
   return if_carve(nullptr, desc->n_models, desc->n, desc->d, B, nullptr);
 }
 
 int sce_code_interference(sce_plan* p, int B, double* cap_sums, long long* nz_counts, void* workspace,
                           size_t workspace_bytes, void* stream) {
   if (!p) return fail(SCE_ERR_INVALID, "code_interference: plan is NULL");
-  if (!p->cfg.evaluable)
-    return fail(SCE_ERR_INVALID, "code_interference: not available for the learned-centre variant or with encoder_nonneg / "
-                                 "input_shift; evaluate the exported dictionaries (TiedSAE)");
+  TRY(check_evaluable(p, "code_interference: "));
   TRY(check_rows(p, B, "code_interference: "));
+  TRY(check_forward_code(p, "code_interference: "));
   if (!cap_sums || !nz_counts) return fail(SCE_ERR_INVALID, "code_interference: cap_sums and nz_counts are required");
   const sce_desc& d = p->d;
   IfCarve w;
@@ -931,13 +936,10 @@ int sce_code_interference(sce_plan* p, int B, double* cap_sums, long long* nz_co
   Launcher L{static_cast<cudaStream_t>(stream)};
   // the dictionary the plan decodes with, as stored: every kind is normalised here with the clamp alone
   const float* dict = p->cfg.untied ? p->b.decoder : p->b.encoder;
-  auto run = [&](auto src) {
+  return with_forward_code(p, [&](auto src) {
     constexpr int SRC = decltype(src)::value;
     return launch_interference<SRC>(L, code_view<SRC>(p), nullptr, dict, d.n_models, d.d, B, w, cap_sums, nz_counts);
-  };
-  if (p->cfg.topk) return run(std::integral_constant<int, kCodeScores>{});
-  if (p->code_batch_major) return run(std::integral_constant<int, kCodeBatchMajor>{});
-  return with_arith(p->cfg.arith, run);
+  });
 }
 
 size_t sce_expected_interference_workspace_bytes(int n, int d, int B) {

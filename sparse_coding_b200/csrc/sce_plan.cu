@@ -303,6 +303,22 @@ int check_rows(const sce_plan* p, int B, const char* prefix) {
   return SCE_OK;
 }
 
+// the forward-only passes: plans whose forward is that of their export (a TiedSAE)
+int check_evaluable(const sce_plan* p, const char* prefix) {
+  if (!p->cfg.evaluable)
+    return fail(SCE_ERR_INVALID, "%snot available for the learned-centre variant or with encoder_nonneg / input_shift; "
+                                 "evaluate the exported dictionaries (TiedSAE)", prefix);
+  return SCE_OK;
+}
+
+// the passes that read the code of the plan's last forward call: a dw_native training step leaves its residual plane
+// batch-major only (code_batch_major)
+int check_forward_code(const sce_plan* p, const char* prefix) {
+  if (p->code_batch_major)
+    return fail(SCE_ERR_INVALID, "%sa plan's last call was a training step; follow sce_forward_stats", prefix);
+  return SCE_OK;
+}
+
 // the training entry points (sce_step, sce_step_host, sce_grads, sce_step_tracked, sce_resample), before any device call
 int check_trainable(const sce_plan* p, const char* prefix) {
   if (p->cfg.forward_only)

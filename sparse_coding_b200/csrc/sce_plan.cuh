@@ -161,6 +161,8 @@ struct PlanCall : Launcher {
 __attribute__((visibility("hidden"))) int validate(const sce_desc* d);
 __attribute__((visibility("hidden"))) PlanConfig plan_config(const sce_desc& d);
 __attribute__((visibility("hidden"))) int check_rows(const sce_plan* p, int B, const char* prefix);
+__attribute__((visibility("hidden"))) int check_evaluable(const sce_plan* p, const char* prefix);
+__attribute__((visibility("hidden"))) int check_forward_code(const sce_plan* p, const char* prefix);
 __attribute__((visibility("hidden"))) int check_trainable(const sce_plan* p, const char* prefix);
 __attribute__((visibility("hidden"))) int run_pipeline(PlanCall& c, sce_plan* p, const float* x, int B, cudaStream_t st,
                                                        float* x_hat, bool backward, float* out_losses, float* out_nnz,

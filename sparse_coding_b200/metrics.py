@@ -481,14 +481,19 @@ class _StatsPlan(_DictPlan):
             self.cap_sums = torch.zeros(M, n, dtype=torch.float64, device=dev)
             self.nz_counts = torch.zeros(M, n, dtype=torch.int64, device=dev)
 
+    def stats(self, x, seg, phase, x_hat=None):
+        """The forward pass of ``x`` [B, d] with its moment sums and segment counts; the plan keeps the code of these
+        rows, which the calls that follow read."""
+        _lib.check(_lib.load().sce_forward_stats(
+            self.plan, self.batch(x).data_ptr(), x.shape[0], seg, phase, x_hat.data_ptr() if x_hat is not None else None,
+            self.losses.data_ptr(), self.nnz.data_ptr(), self.sums.data_ptr(), self.seg_counts.data_ptr(),
+            self.seg_open.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream), "sce_forward_stats")
+
     def run(self, x, seg, phase):
         lib = _lib.load()
         B, d = x.shape
         x_hat = torch.empty(self.M, B, d, dtype=torch.float32, device=self.dev) if self.centred else None
-        _lib.check(lib.sce_forward_stats(
-            self.plan, self.batch(x).data_ptr(), B, seg, phase, x_hat.data_ptr() if x_hat is not None else None,
-            self.losses.data_ptr(), self.nnz.data_ptr(), self.sums.data_ptr(), self.seg_counts.data_ptr(),
-            self.seg_open.data_ptr(), self.ws_ptr, self.ws_bytes, self.stream), "sce_forward_stats")
+        self.stats(x, seg, phase, x_hat)
         _lib.check(lib.sce_active_counts(self.plan, B, self.counts.data_ptr(), self.stream), "sce_active_counts")
         if self.cap_sums is not None:
             _lib.check(lib.sce_code_interference(self.plan, B, self.cap_sums.data_ptr(), self.nz_counts.data_ptr(),
@@ -813,24 +818,12 @@ def calc_moments_streaming(learned_dict, activations: torch.Tensor, batch_size: 
 # per-feature sums of the statistics pass; correlation, covariance and best matches are formed on the device
 # (``sce_correlation_finish``). The dense [N, n] code is never formed.
 # ---------------------------------------------------------------------------------------------------------------------
-class _CodePlan(_DictPlan):
-    """A dictionary plan whose calls leave their code for ``sce_cross_moments`` and add to its moment sums."""
-
-    def __init__(self, key, lds, batch_max, arith, dev):
-        super().__init__(key, lds, batch_max, arith, dev)
-        M, n = self.M, self.n
-        self.ws_bytes = _lib.load().sce_forward_stats_workspace_bytes(C.byref(self.desc), batch_max)
-        self._pass_ws, self.ws_ptr = _lib.workspace(self.ws_bytes, dev, "sce_forward_stats_workspace_bytes")
-        self.sums = torch.zeros(M, n, 4, dtype=torch.float64, device=dev)
-        self.seg_counts = torch.zeros(M, n, dtype=torch.int32, device=dev)
-        self.losses = torch.empty(M, _lib.SCE_LOSS_COLS, dtype=torch.float32, device=dev)
-        self.nnz = torch.empty(M, dtype=torch.float32, device=dev)
+class _CodePlan(_StatsPlan):
+    """A statistics plan whose calls run the forward pass and its moment sums alone (no activity counts, loss or
+    interference): ``sce_cross_moments`` reads the code they leave."""
 
     def run(self, x):
-        _lib.check(_lib.load().sce_forward_stats(
-            self.plan, self.batch(x).data_ptr(), x.shape[0], 1, 0, None, self.losses.data_ptr(), self.nnz.data_ptr(),
-            self.sums.data_ptr(), self.seg_counts.data_ptr(), None, self.ws_ptr, self.ws_bytes, self.stream),
-            "sce_forward_stats")
+        self.stats(x, 1, 0)
 
 
 def _dict_list(x):
